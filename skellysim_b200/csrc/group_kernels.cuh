@@ -20,9 +20,10 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include "skb_internal.hpp" // kMaxGroup
+
 namespace skb {
 
-constexpr int kMaxGroup = 16;
 constexpr int kGroupPhases = 4;
 
 struct GroupPushArgs {

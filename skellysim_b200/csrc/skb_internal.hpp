@@ -62,6 +62,19 @@ struct EvalOpts {
                                // d_u_out + 3 n_src (group mode: the leading rows are partial sums that live elsewhere)
 };
 
+constexpr int kMaxGroup = 16; // members of a multi-GPU group (group_kernels.cuh, skb_mflow)
+
+// forces_torques [6 x n_bodies] (body_container.cpp:134) -> forces and torques, 3 x n_bodies each
+void split_forces_torques(const double *ft, int n_bodies, std::vector<double> &f, std::vector<double> &t);
+
+} // namespace skb
+
+// ---- flow internals that skb_mflow.cu needs (skb_matvec.cu) ----
+struct skb_flow;
+namespace skb {
+cudaStream_t flow_stream(const skb_flow *fl); // the stream of the flow's own calls
+// sizes the buffers of the background streamer (skb_flow_set_overlap) for n_rows own periphery rows, if it is on
+int flow_size_overlap(skb_flow *fl, long long n_rows);
 } // namespace skb
 
 // ---- context internals (shared by skb_runtime.cu and skb_matvec.cu) ----

@@ -68,7 +68,14 @@ struct skb_flow {
     TargetCache tc_fib, tc_shell, tc_body;
     bool mv_dirty = true;
     int cross_mode = -1;    // fiber <-> periphery cross kernel in the matvec: -1 auto, 0 off, 1 on whenever applicable
-    bool use_cross = false; // decided by prepare_matvec_targets
+    // how matvec_core evaluates, decided by prepare_matvec_targets
+    struct MatvecPlan {
+        bool grouped = false; // group member: the strengths come packed from the group window (push), not the caller
+        // producer of the fiber rows: the plain kernel; the symmetric kernel's complete rows (whole system on this
+        // device, cross kernel); or this member's symmetric partial sums, pulled together from all members' windows
+        enum FiberRows { kPlain, kSymComplete, kSymPartial } fib_rows = kPlain;
+        bool cross = false;   // fiber <-> periphery pairs through the cross kernel
+    } plan;
     CrossState cross;
     bool self_excl = false; // matvec: skip intra-fiber pairs in the kernels instead of compute-then-subtract (N3, opt-in)
     long long win_begin = 0, win_end = -1; // target window of the matvec in [fibers|shell|bodies] rows; -1 = all
@@ -127,7 +134,6 @@ struct skb_flow {
         long long n_fib = 0, n_shell = 0, n_pad_fib = 0, n_pad_shell = 0; // geometry the window was laid out for
         unsigned long long epoch = 0;
         bool dry = false;             // warm-up pass: no flags, own window only (skb_flow_group_warmup)
-        bool use_sym = false;         // fiber rows: symmetric block rows + pull-reduce (else own rows with the plain kernel)
         bool connected() const {
             for (int m = 0; m < size; ++m)
                 if (!peer[m])
@@ -144,7 +150,6 @@ struct skb_flow {
         cudaEvent_t fork = nullptr, join = nullptr;
         DevBuf y;                  // A x of the own periphery rows
         skb_dense *dn = nullptr;   // pending background product of the call in flight (nullptr: none)
-        const double *d_x = nullptr;
         bool launched = false;
     } bg;
     DevBuf scratch_u; // group mode: landing zone of eval_on_device's default output (never read)
@@ -163,10 +168,33 @@ static int ensure_ctx(skb_flow *fl, skb_ctx **slot) {
     return skb_ctx_create_on(&fl->dev, 1, slot);
 }
 
+// every kernel launch of this file: check it, count it globally and in the statistics of the call in flight
+static int launched(skb_flow *fl, int n) {
+    CUDA_TRY(cudaGetLastError());
+    count_launch(n);
+    fl->launches += n;
+    return SKB_OK;
+}
+
+// self term of the fibers (fcfd.cpp:203-210): d_vel rows [0, node_end - node_begin) are the fiber nodes
+// [node_begin, node_end), the packed strengths are those of ctx's last Stokeslet evaluation
+static int fiber_self_term(skb_flow *fl, skb_ctx *ctx, double eta, double *d_vel, long long node_begin,
+                           long long node_end) {
+    const SourceSet &s = ctx->devs[0].src[SKB_STOKESLET];
+    if (node_end <= node_begin || s.excl) // fused form: the pair kernels skipped every intra-fiber pair
+        return SKB_OK;
+    const size_t smem = (size_t)fl->max_fiber_nodes * 6 * sizeof(double);
+    fiber_self_subtract_kernel<<<fl->n_fibers, 128, smem, fl->cur>>>(
+        (const double *)fl->r_fib.ptr, s.f_cur, (const long long *)fl->fiber_offset.ptr, 1.0 / (8.0 * M_PI * eta),
+        kReg * kReg, kEps, d_vel, node_begin, node_end);
+    return launched(fl, 1);
+}
+
 // ---- device-side flows: ctx already has its targets and sources ------------------------------------------------
+// mode / d_forces: the caller's forces (kRaw) or already packed strengths (kPacked).
 // subtract_self: the first (node_end - node_begin) targets are the fiber nodes [node_begin, node_end)
-static int fibers_dev(skb_flow *fl, skb_ctx *ctx, const double *d_forces, double eta, int subtract_self,
-                      double *d_vel, int accumulate, long long node_begin, long long node_end) {
+static int fibers_dev(skb_flow *fl, skb_ctx *ctx, StrengthMode mode, const double *d_forces, double eta,
+                      int subtract_self, double *d_vel, int accumulate, long long node_begin, long long node_end) {
     DeviceState &d = ctx->devs[0];
     if (d.n_trg == 0)
         return SKB_OK;
@@ -176,29 +204,20 @@ static int fibers_dev(skb_flow *fl, skb_ctx *ctx, const double *d_forces, double
         return SKB_OK;
     }
     // weighted forces -> Stokeslet all-to-all, / eta  (fcfd.cpp:185-199, kernels.cpp:365)
-    SKB_TRY(eval_on_device(ctx, d, SKB_STOKESLET, kRaw, d_forces, 0.0, d_vel, accumulate, fl->cur, false,
+    SKB_TRY(eval_on_device(ctx, d, SKB_STOKESLET, mode, d_forces, 0.0, d_vel, accumulate, fl->cur, false,
                            &fl->launches, nullptr, 1.0 / eta));
     fl->pairs += fl->n_fib * d.n_trg;
-    if (subtract_self && ctx->devs[0].src[SKB_STOKESLET].excl) {
-        // opt-in fused form: the pair kernels already skipped every intra-fiber pair (skb_flow_set_self_exclusion)
-    } else if (subtract_self) { // fcfd.cpp:203-210; the first N_f targets are the fiber nodes themselves
-        if (d.n_trg < node_end - node_begin)
-            return set_error(SKB_ERR_INVALID, "fiber flow with subtract_self needs the fiber nodes as the first "
-                                              "%lld targets (n_trg = %lld)", node_end - node_begin, d.n_trg);
-        const size_t smem = (size_t)fl->max_fiber_nodes * 6 * sizeof(double);
-        fiber_self_subtract_kernel<<<fl->n_fibers, 128, smem, fl->cur>>>(
-            (const double *)fl->r_fib.ptr, d.src[SKB_STOKESLET].f_cur,
-            (const long long *)fl->fiber_offset.ptr, 1.0 / (8.0 * M_PI * eta), kReg * kReg, kEps, d_vel, node_begin,
-            node_end);
-        CUDA_TRY(cudaGetLastError());
-        count_launch(1);
-        fl->launches += 1;
-    }
-    return SKB_OK;
+    if (!subtract_self)
+        return SKB_OK;
+    if (!d.src[SKB_STOKESLET].excl && d.n_trg < node_end - node_begin)
+        return set_error(SKB_ERR_INVALID, "fiber flow with subtract_self needs the fiber nodes as the first "
+                                          "%lld targets (n_trg = %lld)", node_end - node_begin, d.n_trg);
+    return fiber_self_term(fl, ctx, eta, d_vel, node_begin, node_end);
 }
 
-static int periphery_dev(skb_flow *fl, skb_ctx *ctx, const double *d_density, double eta, double *d_vel,
-                         int accumulate) {
+// mode / d_density: the caller's densities (kNormalDensity) or already packed sym6 strengths (kPacked)
+static int periphery_dev(skb_flow *fl, skb_ctx *ctx, StrengthMode mode, const double *d_density, double eta,
+                         double *d_vel, int accumulate) {
     DeviceState &d = ctx->devs[0];
     if (d.n_trg == 0)
         return SKB_OK;
@@ -208,8 +227,8 @@ static int periphery_dev(skb_flow *fl, skb_ctx *ctx, const double *d_density, do
         return SKB_OK;
     }
     // f_dl = 2 eta n (x) rho formed on the device, stresslet, / eta  (periphery.cpp:68-74, kernels.cpp:358)
-    SKB_TRY(eval_on_device(ctx, d, SKB_STRESSLET, kNormalDensity, d_density, 2.0 * eta, d_vel, accumulate, fl->cur,
-                           false, &fl->launches, nullptr, 1.0 / eta));
+    SKB_TRY(eval_on_device(ctx, d, SKB_STRESSLET, mode, d_density, 2.0 * eta, d_vel, accumulate, fl->cur, false,
+                           &fl->launches, nullptr, 1.0 / eta));
     fl->pairs += fl->n_shell * d.n_trg;
     return SKB_OK;
 }
@@ -235,11 +254,8 @@ static int bodies_dev(skb_flow *fl, skb_ctx *ctx, const double *d_density, const
     rotlet_add_kernel<<<(unsigned)((d.n_trg + bs - 1) / bs), bs, 0, fl->cur>>>(
         (const double *)fl->centers.ptr, d_torque, fl->n_bodies, (const double *)d.r_trg.ptr, d.n_trg,
         1.0 / (8.0 * M_PI * eta), kReg * kReg, kEps * kEps, d_vel);
-    CUDA_TRY(cudaGetLastError());
-    count_launch(1);
-    fl->launches += 1;
     fl->pairs += (fl->n_body + 2 * (long long)fl->n_bodies) * d.n_trg;
-    return SKB_OK;
+    return launched(fl, 1);
 }
 
 static int upload(skb_flow *fl, DevBuf &buf, const double *h, size_t n_doubles) {
@@ -247,6 +263,11 @@ static int upload(skb_flow *fl, DevBuf &buf, const double *h, size_t n_doubles) 
         return SKB_OK;
     SKB_TRY(buf.ensure(n_doubles * 8));
     CUDA_TRY(cudaMemcpyAsync(buf.ptr, h, n_doubles * 8, cudaMemcpyHostToDevice, fl->stream));
+    return SKB_OK;
+}
+static int download(skb_flow *fl, double *h, const DevBuf &buf, size_t n_doubles) {
+    if (n_doubles > 0)
+        CUDA_TRY(cudaMemcpyAsync(h, buf.ptr, n_doubles * 8, cudaMemcpyDeviceToHost, fl->stream));
     return SKB_OK;
 }
 
@@ -258,7 +279,7 @@ static int set_targets_cached(skb_ctx *ctx, TargetCache &tc, const double *r_trg
     return SKB_OK;
 }
 
-static void split_forces_torques(const double *ft, int n_bodies, std::vector<double> &f, std::vector<double> &t) {
+void skb::split_forces_torques(const double *ft, int n_bodies, std::vector<double> &f, std::vector<double> &t) {
     f.resize(3 * (size_t)n_bodies);
     t.resize(3 * (size_t)n_bodies);
     for (int b = 0; b < n_bodies; ++b)
@@ -313,6 +334,33 @@ static unsigned long long buffer_key(const skb_flow *fl, int which) {
         }
     }
     return h;
+}
+
+// Inputs and output of a call: the caller's arrays, or (pinned == true) copies in the pinned staging
+// [fiber forces | periphery densities | body densities | body forces | body torques | output] when the call is small
+// enough to be replayed as one CUDA graph, whose memcpy nodes need fixed host addresses
+struct Staged {
+    const double *ff, *sd, *bd, *f, *t;
+    double *v;
+    bool pinned;
+};
+static int stage_inputs(skb_flow *fl, const double *ff, const double *sd, const double *bd,
+                        const std::vector<double> &f, const std::vector<double> &t, double *v, size_t n_out,
+                        Staged &s) {
+    const long long nf = fl->n_fib, ns = fl->n_shell, nb = fl->n_body;
+    const size_t n_in = (size_t)(nf + ns + nb) * 3 + f.size() + t.size();
+    s = Staged{ff, sd, bd, f.data(), t.data(), v, false};
+    if (!fl->graphs_enabled || (n_in + n_out) * 8 > kGraphMaxBytes)
+        return SKB_OK;
+    SKB_TRY(ensure_stage(fl, n_in + n_out));
+    double *h_ff = fl->h_stage, *h_sd = h_ff + 3 * nf, *h_bd = h_sd + 3 * ns, *h_f = h_bd + 3 * nb, *h_t = h_f + f.size();
+    if (nf) std::memcpy(h_ff, ff, (size_t)nf * 24);
+    if (ns) std::memcpy(h_sd, sd, (size_t)ns * 24);
+    if (nb) std::memcpy(h_bd, bd, (size_t)nb * 24);
+    if (!f.empty()) std::memcpy(h_f, f.data(), f.size() * 8);
+    if (!t.empty()) std::memcpy(h_t, t.data(), t.size() * 8);
+    s = Staged{h_ff, h_sd, h_bd, h_f, h_t, h_t + t.size(), true};
+    return SKB_OK;
 }
 
 // Run `body` (asynchronous work on fl->stream, fixed addresses only) either directly, as a capture followed by a
@@ -370,6 +418,29 @@ static int finish_stats(skb_flow *fl) {
     cudaEventElapsedTime(&b, fl->evt0, fl->evt1);
     fl->stats.device_ms = a;
     fl->stats.total_ms = b;
+    fl->stats.n_pairs = fl->pairs;
+    fl->stats.launches = fl->launches;
+    return SKB_OK;
+}
+
+// frame of the host-pointer entry points on fl->stream: device_ms spans the device work, total_ms also the uploads
+// before it and the downloads after it; returns once the downloads have landed
+template <class Up, class Work, class Down> static int host_frame(skb_flow *fl, Up up, Work work, Down down) {
+    fl->cur = fl->stream;
+    CUDA_TRY(cudaEventRecord(fl->evt0, fl->stream));
+    SKB_TRY(up());
+    CUDA_TRY(cudaEventRecord(fl->ev0, fl->stream));
+    SKB_TRY(work());
+    CUDA_TRY(cudaEventRecord(fl->ev1, fl->stream));
+    SKB_TRY(down());
+    CUDA_TRY(cudaEventRecord(fl->evt1, fl->stream));
+    return finish_stats(fl);
+}
+static int nothing() { return SKB_OK; }
+
+// the device-pointer entry points run asynchronously on the caller's stream: no timings
+static int device_stats(skb_flow *fl) {
+    fl->stats.device_ms = fl->stats.total_ms = 0;
     fl->stats.n_pairs = fl->pairs;
     fl->stats.launches = fl->launches;
     return SKB_OK;
@@ -494,8 +565,7 @@ int skb_flow_set_fibers(skb_flow *fl, const double *r_fib, const int *n_nodes, c
         fiber_weights_kernel<<<n_fibers, 64, 0, fl->stream>>>((const long long *)fl->fiber_offset.ptr,
                                                               (const double *)fl->fiber_length.ptr, n_fibers,
                                                               (double *)s.weights.ptr);
-        CUDA_TRY(cudaGetLastError());
-        count_launch(1);
+        SKB_TRY(launched(fl, 1));
         s.has_weights = true;
     }
     CUDA_TRY(cudaStreamSynchronize(fl->stream));
@@ -549,17 +619,17 @@ int skb_flow_fibers(skb_flow *fl, const double *r_trg, int64_t n_trg, const doub
     SKB_TRY(set_targets_cached(fl->fib[0], fl->tc_fib, r_trg, n_trg));
     if (n_trg == 0)
         return SKB_OK;
-    CUDA_TRY(cudaEventRecord(fl->evt0, fl->stream));
-    SKB_TRY(upload(fl, fl->in_fib, fib_forces, (size_t)fl->n_fib * 3));
-    SKB_TRY(fl->vel.ensure((size_t)n_trg * 24));
-    CUDA_TRY(cudaEventRecord(fl->ev0, fl->stream));
-    fl->cur = fl->stream;
-    SKB_TRY(fibers_dev(fl, fl->fib[0], (const double *)fl->in_fib.ptr, eta, subtract_self, (double *)fl->vel.ptr, 0, 0,
-                       fl->n_fib));
-    CUDA_TRY(cudaEventRecord(fl->ev1, fl->stream));
-    CUDA_TRY(cudaMemcpyAsync(vel, fl->vel.ptr, (size_t)n_trg * 24, cudaMemcpyDeviceToHost, fl->stream));
-    CUDA_TRY(cudaEventRecord(fl->evt1, fl->stream));
-    return finish_stats(fl);
+    return host_frame(
+        fl,
+        [&]() -> int {
+            SKB_TRY(upload(fl, fl->in_fib, fib_forces, (size_t)fl->n_fib * 3));
+            return fl->vel.ensure((size_t)n_trg * 24);
+        },
+        [&] {
+            return fibers_dev(fl, fl->fib[0], kRaw, (const double *)fl->in_fib.ptr, eta, subtract_self,
+                              (double *)fl->vel.ptr, 0, 0, fl->n_fib);
+        },
+        [&] { return download(fl, vel, fl->vel, (size_t)n_trg * 3); });
 }
 
 int skb_flow_periphery(skb_flow *fl, const double *r_trg, int64_t n_trg, const double *density, double eta,
@@ -571,16 +641,17 @@ int skb_flow_periphery(skb_flow *fl, const double *r_trg, int64_t n_trg, const d
     SKB_TRY(set_targets_cached(fl->shell[0], fl->tc_shell, r_trg, n_trg));
     if (n_trg == 0)
         return SKB_OK;
-    CUDA_TRY(cudaEventRecord(fl->evt0, fl->stream));
-    SKB_TRY(upload(fl, fl->in_shell, density, (size_t)fl->n_shell * 3));
-    SKB_TRY(fl->vel.ensure((size_t)n_trg * 24));
-    CUDA_TRY(cudaEventRecord(fl->ev0, fl->stream));
-    fl->cur = fl->stream;
-    SKB_TRY(periphery_dev(fl, fl->shell[0], (const double *)fl->in_shell.ptr, eta, (double *)fl->vel.ptr, 0));
-    CUDA_TRY(cudaEventRecord(fl->ev1, fl->stream));
-    CUDA_TRY(cudaMemcpyAsync(vel, fl->vel.ptr, (size_t)n_trg * 24, cudaMemcpyDeviceToHost, fl->stream));
-    CUDA_TRY(cudaEventRecord(fl->evt1, fl->stream));
-    return finish_stats(fl);
+    return host_frame(
+        fl,
+        [&]() -> int {
+            SKB_TRY(upload(fl, fl->in_shell, density, (size_t)fl->n_shell * 3));
+            return fl->vel.ensure((size_t)n_trg * 24);
+        },
+        [&] {
+            return periphery_dev(fl, fl->shell[0], kNormalDensity, (const double *)fl->in_shell.ptr, eta,
+                                 (double *)fl->vel.ptr, 0);
+        },
+        [&] { return download(fl, vel, fl->vel, (size_t)n_trg * 3); });
 }
 
 int skb_flow_bodies(skb_flow *fl, const double *r_trg, int64_t n_trg, const double *densities,
@@ -595,20 +666,19 @@ int skb_flow_bodies(skb_flow *fl, const double *r_trg, int64_t n_trg, const doub
         return SKB_OK;
     std::vector<double> f, t;
     split_forces_torques(forces_torques, fl->n_bodies, f, t);
-    CUDA_TRY(cudaEventRecord(fl->evt0, fl->stream));
-    SKB_TRY(upload(fl, fl->in_body, densities, (size_t)fl->n_body * 3));
-    SKB_TRY(upload(fl, fl->in_force, f.data(), f.size()));
-    SKB_TRY(upload(fl, fl->in_torque, t.data(), t.size()));
-    SKB_TRY(fl->vel.ensure((size_t)n_trg * 24));
-    CUDA_TRY(cudaEventRecord(fl->ev0, fl->stream));
-    fl->cur = fl->stream;
-    SKB_TRY(bodies_dev(fl, fl->body[0], (const double *)fl->in_body.ptr, (const double *)fl->in_force.ptr,
-                       (const double *)fl->in_torque.ptr, eta, (double *)fl->vel.ptr, 0));
-    CUDA_TRY(cudaEventRecord(fl->ev1, fl->stream));
-    CUDA_TRY(cudaMemcpyAsync(vel, fl->vel.ptr, (size_t)n_trg * 24, cudaMemcpyDeviceToHost, fl->stream));
-    CUDA_TRY(cudaEventRecord(fl->evt1, fl->stream));
-    CUDA_TRY(cudaStreamSynchronize(fl->stream)); // f, t are stack-owned staging
-    return finish_stats(fl);
+    return host_frame(
+        fl,
+        [&]() -> int {
+            SKB_TRY(upload(fl, fl->in_body, densities, (size_t)fl->n_body * 3));
+            SKB_TRY(upload(fl, fl->in_force, f.data(), f.size()));
+            SKB_TRY(upload(fl, fl->in_torque, t.data(), t.size()));
+            return fl->vel.ensure((size_t)n_trg * 24);
+        },
+        [&] {
+            return bodies_dev(fl, fl->body[0], (const double *)fl->in_body.ptr, (const double *)fl->in_force.ptr,
+                              (const double *)fl->in_torque.ptr, eta, (double *)fl->vel.ptr, 0);
+        },
+        [&] { return download(fl, vel, fl->vel, (size_t)n_trg * 3); });
 }
 
 int skb_flow_set_point_sources(skb_flow *fl, const double *positions, const double *forces, const double *torques,
@@ -668,23 +738,22 @@ int skb_flow_velocity_at_targets(skb_flow *fl, const double *r_trg, int64_t n_tr
     std::vector<double> f, t;
     if (fl->n_bodies > 0)
         split_forces_torques(body_forces_torques, fl->n_bodies, f, t);
-    fl->cur = fl->stream;
-    const long long nf = fl->n_fib, ns = fl->n_shell, nb = fl->n_body;
     SKB_TRY(fl->vel.ensure((size_t)n_trg * 24));
     double *d_v = (double *)fl->vel.ptr;
-    // device-side sequence with the strengths at (ff, sd, bd, fo, to) and the velocities going to v_host
-    auto body = [&](const double *ff, const double *sd, const double *bd, const double *fo, const double *to,
-                    double *v_host) -> int {
-        SKB_TRY(upload(fl, fl->in_fib, ff, (size_t)nf * 3));
-        SKB_TRY(upload(fl, fl->in_shell, sd, (size_t)ns * 3));
-        SKB_TRY(upload(fl, fl->in_body, bd, (size_t)nb * 3));
-        SKB_TRY(upload(fl, fl->in_force, fo, f.size()));
-        SKB_TRY(upload(fl, fl->in_torque, to, t.size()));
+    Staged s;
+    SKB_TRY(stage_inputs(fl, fib_forces, shell_density, body_densities, f, t, vel, (size_t)n_trg * 3, s));
+    // device-side sequence from the (staged) strengths to the (staged) velocities
+    auto body = [&]() -> int {
+        SKB_TRY(upload(fl, fl->in_fib, s.ff, (size_t)fl->n_fib * 3));
+        SKB_TRY(upload(fl, fl->in_shell, s.sd, (size_t)fl->n_shell * 3));
+        SKB_TRY(upload(fl, fl->in_body, s.bd, (size_t)fl->n_body * 3));
+        SKB_TRY(upload(fl, fl->in_force, s.f, f.size()));
+        SKB_TRY(upload(fl, fl->in_torque, s.t, t.size()));
         // fc_->flow(r_trg, f_on_fibers, eta, /*subtract_self=*/false) + bc_.flow + shell_->flow   system.cpp:355-359
-        SKB_TRY(fibers_dev(fl, fl->fib[0], (const double *)fl->in_fib.ptr, eta, 0, d_v, 0, 0, 0));
+        SKB_TRY(fibers_dev(fl, fl->fib[0], kRaw, (const double *)fl->in_fib.ptr, eta, 0, d_v, 0, 0, 0));
         SKB_TRY(bodies_dev(fl, fl->body[0], (const double *)fl->in_body.ptr, (const double *)fl->in_force.ptr,
                            (const double *)fl->in_torque.ptr, eta, d_v, 1));
-        SKB_TRY(periphery_dev(fl, fl->shell[0], (const double *)fl->in_shell.ptr, eta, d_v, 1));
+        SKB_TRY(periphery_dev(fl, fl->shell[0], kNormalDensity, (const double *)fl->in_shell.ptr, eta, d_v, 1));
         // + psc_.flow(r_trg, eta, time) + bs_.flow(r_trg, eta)                                  system.cpp:358-359
         const double *d_trg = (const double *)fl->fib[0]->devs[0].r_trg.ptr;
         const int bs = 128;
@@ -698,54 +767,30 @@ int skb_flow_velocity_at_targets(skb_flow *fl, const double *r_trg, int64_t n_tr
                                                            (const double *)fl->pt_torque.ptr, fl->n_points, d_trg,
                                                            n_trg, 1.0 / (8.0 * M_PI * eta), kReg * kReg, kEps * kEps,
                                                            d_v);
-            CUDA_TRY(cudaGetLastError());
-            count_launch(2);
-            fl->launches += 2;
+            SKB_TRY(launched(fl, 2));
         }
         if (fl->has_background) {
             background_add_kernel<<<nblk, bs, 0, fl->stream>>>(d_trg, n_trg, fl->bg_comp[0], fl->bg_comp[1],
                                                                fl->bg_comp[2], fl->bg_scale[0], fl->bg_scale[1],
                                                                fl->bg_scale[2], fl->bg_uniform[0], fl->bg_uniform[1],
                                                                fl->bg_uniform[2], d_v);
-            CUDA_TRY(cudaGetLastError());
-            count_launch(1);
-            fl->launches += 1;
+            SKB_TRY(launched(fl, 1));
         }
-        CUDA_TRY(cudaMemcpyAsync(v_host, d_v, (size_t)n_trg * 24, cudaMemcpyDeviceToHost, fl->stream));
-        return SKB_OK;
+        return download(fl, s.v, fl->vel, (size_t)n_trg * 3);
     };
-    const size_t n_in = (size_t)(nf + ns + nb) * 3 + f.size() + t.size(), n_out = (size_t)n_trg * 3;
-    CUDA_TRY(cudaEventRecord(fl->evt0, fl->stream));
-    CUDA_TRY(cudaEventRecord(fl->ev0, fl->stream));
-    if (fl->graphs_enabled && (n_in + n_out) * 8 <= kGraphMaxBytes) {
-        // the listener / streamline integrator asks for 1-6 targets per call (streamline.cpp:11-35): launch-bound
-        SKB_TRY(ensure_stage(fl, n_in + n_out));
-        double *h = fl->h_stage;
-        double *h_ff = h, *h_sd = h_ff + 3 * nf, *h_bd = h_sd + 3 * ns, *h_f = h_bd + 3 * nb, *h_t = h_f + f.size();
-        double *h_v = h_t + t.size();
-        if (nf) std::memcpy(h_ff, fib_forces, (size_t)nf * 24);
-        if (ns) std::memcpy(h_sd, shell_density, (size_t)ns * 24);
-        if (nb) std::memcpy(h_bd, body_densities, (size_t)nb * 24);
-        if (!f.empty()) std::memcpy(h_f, f.data(), f.size() * 8);
-        if (!t.empty()) std::memcpy(h_t, t.data(), t.size() * 8);
-        unsigned long long key = mix_key(fl->geom_version, (unsigned long long)n_trg);
-        key = mix_key(key, dbl_bits(eta));
-        key = mix_key(key, buffer_key(fl, 0));
-        // same count but different targets: the captured sequence assumed the old targets' relation to the sources
-        key = mix_key(key, fl->tc_fib.version);
-        key = mix_key(key, fl->tc_shell.version);
-        key = mix_key(key, fl->tc_body.version);
-        SKB_TRY(run_graphed(fl, fl->g_vat, key, [&]() { return body(h_ff, h_sd, h_bd, h_f, h_t, h_v); }));
-        CUDA_TRY(cudaEventRecord(fl->ev1, fl->stream));
-        CUDA_TRY(cudaEventRecord(fl->evt1, fl->stream));
-        SKB_TRY(finish_stats(fl));
-        std::memcpy(vel, h_v, (size_t)n_trg * 24);
-        return SKB_OK;
-    }
-    SKB_TRY(body(fib_forces, shell_density, body_densities, f.data(), t.data(), vel));
-    CUDA_TRY(cudaEventRecord(fl->ev1, fl->stream));
-    CUDA_TRY(cudaEventRecord(fl->evt1, fl->stream));
-    return finish_stats(fl);
+    if (!s.pinned)
+        return host_frame(fl, nothing, body, nothing);
+    // the listener / streamline integrator asks for 1-6 targets per call (streamline.cpp:11-35): launch-bound
+    unsigned long long key = mix_key(fl->geom_version, (unsigned long long)n_trg);
+    key = mix_key(key, dbl_bits(eta));
+    key = mix_key(key, buffer_key(fl, 0));
+    // same count but different targets: the captured sequence assumed the old targets' relation to the sources
+    key = mix_key(key, fl->tc_fib.version);
+    key = mix_key(key, fl->tc_shell.version);
+    key = mix_key(key, fl->tc_body.version);
+    SKB_TRY(host_frame(fl, nothing, [&] { return run_graphed(fl, fl->g_vat, key, body); }, nothing));
+    std::memcpy(vel, s.v, (size_t)n_trg * 24);
+    return SKB_OK;
 }
 
 // resolve the target window / ranges into fiber, shell and body pieces and (re)build the matvec target lists
@@ -784,10 +829,10 @@ static int prepare_matvec_targets(skb_flow *fl) {
             return set_error(SKB_ERR_STATE, "group member: the geometry changed size since skb_flow_group_init "
                                             "(%lld/%lld fiber, %lld/%lld periphery nodes); re-initialise the group",
                              nf, fl->grp.n_fib, ns, fl->grp.n_shell);
-        // fiber rows through the symmetric block rows of this member (partial sums, pulled together afterwards) when
-        // the self-interaction is big enough for that kernel; otherwise the member's own rows with the plain kernel
-        fl->grp.use_sym = nf >= 2LL * sym_block_nodes();
     }
+    // group: fiber rows through the symmetric block rows of this member (partial sums, pulled together afterwards)
+    // when the self-interaction is big enough for that kernel; otherwise the member's own rows with the plain kernel
+    const bool sym_partial = grouped && nf >= 2LL * sym_block_nodes();
     // fiber <-> periphery pairs in one pass (cross_kernels.cuh) when both classes are big enough to matter and the
     // symmetric kernel carries the fiber rows (so that the fiber evaluator's remaining targets are the body rows only)
     static const int cross_env = [] {
@@ -795,10 +840,15 @@ static int prepare_matvec_targets(skb_flow *fl) {
         return e ? atoi(e) : -1;
     }();
     const int cmode = fl->cross_mode >= 0 ? fl->cross_mode : cross_env;
-    const bool sym_rows = grouped ? fl->grp.use_sym
+    const bool sym_rows = grouped ? sym_partial
                                   : (fl->fa == 0 && fl->fb == nf && fl->sa == 0 && fl->sb == ns &&
                                      nf >= (cmode == 1 ? 2LL * sym_block_nodes() : 4096));
-    fl->use_cross = cmode != 0 && sym_rows && n_fw > 0 && ns >= (cmode == 1 ? 1 : 256);
+    const bool use_cross = cmode != 0 && sym_rows && n_fw > 0 && ns >= (cmode == 1 ? 1 : 256);
+    fl->plan.grouped = grouped;
+    fl->plan.cross = use_cross;
+    fl->plan.fib_rows = sym_partial ? skb_flow::MatvecPlan::kSymPartial
+                        : use_cross ? skb_flow::MatvecPlan::kSymComplete
+                                    : skb_flow::MatvecPlan::kPlain;
     // target lists of apply_matvec: r_all = [fibers | shell | bodies] (system.cpp:284-291),
     // r_fibbody = [fibers | bodies] (system.cpp:301-303), both restricted to this rank's pieces
     std::vector<double> r_win, r_fb;
@@ -806,22 +856,22 @@ static int prepare_matvec_targets(skb_flow *fl) {
     r_win.insert(r_win.end(), fl->h_r_fib.begin() + 3 * fl->fa, fl->h_r_fib.begin() + 3 * fl->fb);
     r_win.insert(r_win.end(), fl->h_r_shell.begin() + 3 * fl->sa, fl->h_r_shell.begin() + 3 * fl->sb);
     r_win.insert(r_win.end(), fl->h_r_body.begin() + 3 * fl->ba, fl->h_r_body.begin() + 3 * fl->bb);
-    if (!fl->use_cross)
+    if (!use_cross)
         r_fb.insert(r_fb.end(), fl->h_r_fib.begin() + 3 * fl->fa, fl->h_r_fib.begin() + 3 * fl->fb);
     r_fb.insert(r_fb.end(), fl->h_r_body.begin() + 3 * fl->ba, fl->h_r_body.begin() + 3 * fl->bb);
-    if (grouped && fl->grp.use_sym) {
+    if (sym_partial) {
         // fiber sources meet [ALL fiber nodes | own shell rows | own body rows]; with the cross kernel the periphery
         // rows are not targets of this evaluator
         std::vector<double> r_sym;
         r_sym.reserve((size_t)(nf + n_sw + n_bw) * 3);
         r_sym.insert(r_sym.end(), fl->h_r_fib.begin(), fl->h_r_fib.end());
-        if (!fl->use_cross)
+        if (!use_cross)
             r_sym.insert(r_sym.end(), fl->h_r_shell.begin() + 3 * fl->sa, fl->h_r_shell.begin() + 3 * fl->sb);
         r_sym.insert(r_sym.end(), fl->h_r_body.begin() + 3 * fl->ba, fl->h_r_body.begin() + 3 * fl->bb);
         SKB_TRY(skb_ctx_set_symmetric(fl->fib[1], 1));
         SKB_TRY(skb_ctx_set_sym_partition(fl->fib[1], fl->grp.rank, fl->grp.size));
         SKB_TRY(skb_set_targets(fl->fib[1], r_sym.data(), (long long)r_sym.size() / 3));
-    } else if (fl->use_cross) {
+    } else if (use_cross) {
         std::vector<double> r_fibbody(fl->h_r_fib.begin() + 3 * fl->fa, fl->h_r_fib.begin() + 3 * fl->fb);
         r_fibbody.insert(r_fibbody.end(), fl->h_r_body.begin() + 3 * fl->ba, fl->h_r_body.begin() + 3 * fl->bb);
         SKB_TRY(skb_ctx_set_sym_partition(fl->fib[1], 0, 1));
@@ -832,7 +882,7 @@ static int prepare_matvec_targets(skb_flow *fl) {
     }
     SKB_TRY(skb_set_targets(fl->body[1], r_win.data(), fl->n_win));
     SKB_TRY(skb_set_targets(fl->shell[1], r_fb.data(), (long long)r_fb.size() / 3));
-    const bool all_fibers_lead = (fl->fa == 0 && fl->fb == nf) || (grouped && fl->grp.use_sym);
+    const bool all_fibers_lead = (fl->fa == 0 && fl->fb == nf) || sym_partial;
     if (fl->self_excl && fl->n_fib > 0) {
         if (!all_fibers_lead)
             return set_error(SKB_ERR_INVALID, "skb_flow_set_self_exclusion needs all fiber nodes as the leading matvec "
@@ -849,7 +899,7 @@ static int prepare_matvec_targets(skb_flow *fl) {
     return SKB_OK;
 }
 
-// ---- group exchange steps (group_kernels.cuh) on fl->cur ---------------------------------------------------------
+// ---- matvec_core and its steps, on fl->cur -----------------------------------------------------------------------
 // The pending dense product of apply_matvec_core goes out on the side stream, ordered after everything on fl->cur so far
 // (its input is complete), and runs beside whatever fl->cur launches next.  The side stream has the highest priority:
 // its one-warp CTAs (one per SM) are placed before the pair kernel's CTAs fill the SMs.
@@ -869,14 +919,22 @@ static int overlap_buffers(skb_flow *fl, long long n_rows) {
     SKB_TRY(B.y.ensure((size_t)n_rows * 8 + 8));
     return SKB_OK;
 }
-static int overlap_launch(skb_flow *fl) {
+
+// the complete x_shell on this device, input of the periphery's dense operator: the caller's vector without a group;
+// with one, the gathered copy in the window half (epoch parity) of the group matvec in flight
+static const double *full_x_shell(const skb_flow *fl, const double *d_xs) {
+    const skb_flow::Group &G = fl->grp;
+    return G.size > 1 ? G.at<double>(G.rank, G.off_xshell[G.epoch & 1]) : d_xs;
+}
+
+static int overlap_launch(skb_flow *fl, const double *d_xs) {
     skb_flow::Overlap &B = fl->bg;
     if (!B.dn || B.launched)
         return SKB_OK;
     CUDA_TRY(cudaEventRecord(B.fork, fl->cur));
     CUDA_TRY(cudaStreamWaitEvent(B.stream, B.fork, 0));
-    SKB_TRY(skb_dense_apply_background_device(B.dn, SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY, B.d_x, (double *)B.y.ptr,
-                                              B.stream));
+    SKB_TRY(skb_dense_apply_background_device(B.dn, SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY, full_x_shell(fl, d_xs),
+                                              (double *)B.y.ptr, B.stream));
     CUDA_TRY(cudaEventRecord(B.join, B.stream));
     B.launched = true;
     fl->launches += 1;
@@ -898,285 +956,194 @@ static int group_flag(skb_flow *fl, int phase, bool do_signal, bool do_wait) {
     a.do_wait = do_wait;
     a.timeout_cycles = 20ULL * 1000 * 1000 * 1000; // ~10 s at 2 GHz
     group_flag_kernel<<<1, 32, 0, fl->cur>>>(a);
-    CUDA_TRY(cudaGetLastError());
-    count_launch(1);
-    fl->launches += 1;
-    return SKB_OK;
+    return launched(fl, 1);
 }
 
-// device-side matvec flow of a group member on fl->cur: d_ff / d_sd are the strengths of the OWN fibers / periphery
-// rows, body inputs are complete on every member; d_v = [own fiber rows | own shell rows | own body rows] of v_all
-static int matvec_core_group(skb_flow *fl, const double *d_ff, const double *d_sd, const double *d_bd, const double *d_f,
-                             const double *d_t, double eta, double *d_v) {
+// PUSH: pack the own strengths once and store them into every member's window (pack + all-gather in one kernel)
+static int group_push(skb_flow *fl, const double *d_ff, const double *d_sd, double eta) {
     skb_flow::Group &G = fl->grp;
-    if (!G.dry && !G.connected())
-        return set_error(SKB_ERR_STATE, "group member %d: not all peers are connected (skb_flow_group_import / _connect)",
-                         G.rank);
-    const long long ns = fl->n_shell, nf = fl->n_fib;
-    const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa, n_bw = fl->bb - fl->ba;
-    G.epoch += 1;
+    const DeviceState &df = fl->fib[1]->devs[0];
     const int par = (int)(G.epoch & 1);
-    DeviceState &df = fl->fib[1]->devs[0];
-    // 1. PUSH: pack own strengths once, store them into every member's window (pack + all-gather in one kernel)
-    {
-        GroupPushArgs a;
-        a.fw = d_ff;
-        a.weight = df.src[SKB_STOKESLET].has_weights ? (const double *)df.src[SKB_STOKESLET].weights.ptr : nullptr;
-        a.fa = fl->fa;
-        a.n_f = n_fw;
-        a.density = d_sd;
-        a.normal = ns ? (const double *)fl->shell[1]->devs[0].src[SKB_STRESSLET].normals.ptr : nullptr;
-        a.sa = fl->sa;
-        a.n_s = n_sw;
-        a.two_eta = 2.0 * eta;
-        a.size = G.dry ? 1 : G.size;
-        for (int m = 0; m < a.size; ++m) {
-            const int who = G.dry ? G.rank : m;
-            a.f_sl[m] = G.at<double>(who, G.off_fsl[par]);
-            a.f_shell[m] = G.at<double>(who, G.off_fshell[par]);
-            a.x_shell[m] = G.at<double>(who, G.off_xshell[par]);
-        }
-        const long long work = 3 * n_fw + n_sw;
-        if (work > 0) {
-            const unsigned nblk = (unsigned)std::min<long long>((work + 255) / 256, 4LL * df.info.num_sms);
-            group_push_kernel<<<nblk, 256, 0, fl->cur>>>(a);
-            CUDA_TRY(cudaGetLastError());
-            count_launch(1);
-            fl->launches += 1;
-        }
+    const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
+    GroupPushArgs a;
+    a.fw = d_ff;
+    a.weight = df.src[SKB_STOKESLET].has_weights ? (const double *)df.src[SKB_STOKESLET].weights.ptr : nullptr;
+    a.fa = fl->fa;
+    a.n_f = n_fw;
+    a.density = d_sd;
+    a.normal = fl->n_shell ? (const double *)fl->shell[1]->devs[0].src[SKB_STRESSLET].normals.ptr : nullptr;
+    a.sa = fl->sa;
+    a.n_s = n_sw;
+    a.two_eta = 2.0 * eta;
+    a.size = G.dry ? 1 : G.size;
+    for (int m = 0; m < a.size; ++m) {
+        const int who = G.dry ? G.rank : m;
+        a.f_sl[m] = G.at<double>(who, G.off_fsl[par]);
+        a.f_shell[m] = G.at<double>(who, G.off_fshell[par]);
+        a.x_shell[m] = G.at<double>(who, G.off_xshell[par]);
     }
-    // 2. every member's strengths have landed here
-    SKB_TRY(group_flag(fl, 0, true, true));
-    SKB_TRY(overlap_launch(fl)); // (x_shell is complete in the window from here on)
-    const double *f_sl = G.at<double>(G.rank, G.off_fsl[par]);
-    const double *f_shell = G.at<double>(G.rank, G.off_fshell[par]);
-    double *u_part = G.at<double>(G.rank, G.off_upart);
-    // 3. v = fc.flow(r_all, fw, eta)  (system.cpp:299): own block rows of the symmetric fiber-fiber interaction
-    //    (partial sums for ALL fiber nodes -> u_part) + own shell / body rows (complete -> d_v)
-    if (fl->n_fibers > 0 && df.n_trg > 0) {
-        if (G.use_sym) {
-            SKB_TRY(fl->scratch_u.ensure((size_t)df.n_trg * 24));
-            EvalOpts o;
-            o.d_u_sym = u_part;
-            o.sym_accumulate = 0;
-            o.d_u_rem = fl->use_cross ? d_v + 3 * (n_fw + n_sw) : d_v + 3 * n_fw; // cross: body rows only
-            SKB_TRY(eval_on_device(fl->fib[1], df, SKB_STOKESLET, kPacked, f_sl, 0.0, (double *)fl->scratch_u.ptr, 0,
-                                   fl->cur, false, &fl->launches, nullptr, 1.0 / eta, o));
-            if (!fl->fib[1]->last_was_sym)
-                return set_error(SKB_ERR_STATE, "group member %d: the symmetric kernel declined (memory for the reverse "
-                                                "partials?); lower SKB_SYM_MAX_BYTES pressure or use fewer nodes per GPU",
-                                 G.rank);
-            fl->pairs += nf * nf / G.size + nf * ((fl->use_cross ? 0 : n_sw) + n_bw);
-            if (fl->use_cross && ns > 0) {
-                // own fibers x ALL periphery nodes in one pass: stresslet sums at the own fiber rows (complete) and
-                // this member's partial Stokeslet sums at every periphery row (pulled together after flag B)
-                DeviceState &dsh = fl->shell[1]->devs[0];
-                const SourceSet &sf = df.src[SKB_STOKESLET], &ss = dsh.src[SKB_STRESSLET];
-                SKB_TRY(cross_eval(fl->cross, df.info, (const double *)sf.r.ptr, f_sl, fl->fa, n_fw,
-                                   (const double *)ss.r.ptr, f_shell, ns, ss.n_pad, -3.0 / (8.0 * M_PI * eta),
-                                   1.0 / (8.0 * M_PI * eta), d_v, 0, G.at<double>(G.rank, G.off_upart_shell), 0, fl->cur,
-                                   &fl->launches));
-                fl->pairs += 2 * n_fw * ns;
-            }
-            SKB_TRY(group_flag(fl, 1, true, false)); // my partial sums are complete
-        } else {
-            SKB_TRY(eval_on_device(fl->fib[1], df, SKB_STOKESLET, kPacked, f_sl, 0.0, d_v, 0, fl->cur, false,
-                                   &fl->launches, nullptr, 1.0 / eta));
-            fl->pairs += nf * df.n_trg;
-        }
-    } else if (fl->n_win > 0) {
-        CUDA_TRY(cudaMemsetAsync(d_v, 0, (size_t)fl->n_win * 24, fl->cur));
-    }
-    const bool fib_rows_pending = G.use_sym && fl->n_fibers > 0; // d_v's fiber rows are not complete yet
-    const bool crossed = fl->use_cross && G.use_sym && fl->n_fibers > 0 && ns > 0;
-    // 4. v_fibers, v_bodies += shell.flow(r_fibbody, x_shell, eta)   (system.cpp:304,313-315)
-    bool fib_rows_set = !fib_rows_pending || (crossed && n_fw > 0); // (the cross kernel wrote the own fiber rows)
-    if (crossed) {
-        if (n_sw > 0) // own periphery rows: body flow accumulates first, the members' Stokeslet partials are pulled in below
-            CUDA_TRY(cudaMemsetAsync(d_v + 3 * n_fw, 0, (size_t)n_sw * 24, fl->cur));
-        if (n_bw > 0) { // periphery -> own body rows
-            DeviceState &dsh = fl->shell[1]->devs[0];
-            SKB_TRY(fl->tmp.ensure((size_t)n_bw * 24 + 8));
-            SKB_TRY(eval_on_device(fl->shell[1], dsh, SKB_STRESSLET, kPacked, f_shell, 2.0 * eta, (double *)fl->tmp.ptr, 0,
-                                   fl->cur, false, &fl->launches, nullptr, 1.0 / eta));
-            add_inplace_kernel<<<(unsigned)((3 * n_bw + 255) / 256), 256, 0, fl->cur>>>(
-                d_v + 3 * (n_fw + n_sw), (const double *)fl->tmp.ptr, 3 * n_bw);
-            CUDA_TRY(cudaGetLastError());
-            count_launch(1);
-            fl->launches += 1;
-            fl->pairs += ns * n_bw;
-        }
-    } else if (ns > 0 && n_fw + n_bw > 0) {
-        DeviceState &dsh = fl->shell[1]->devs[0];
-        SKB_TRY(fl->tmp.ensure((size_t)(n_fw + n_bw) * 24 + 8));
-        double *d_tmp = (double *)fl->tmp.ptr;
-        SKB_TRY(eval_on_device(fl->shell[1], dsh, SKB_STRESSLET, kPacked, f_shell, 2.0 * eta, d_tmp, 0, fl->cur, false,
-                               &fl->launches, nullptr, 1.0 / eta));
-        fl->pairs += ns * dsh.n_trg;
-        const int bs = 256;
-        if (n_fw > 0) {
-            if (fib_rows_pending) {
-                CUDA_TRY(cudaMemcpyAsync(d_v, d_tmp, (size_t)n_fw * 24, cudaMemcpyDeviceToDevice, fl->cur));
-                fib_rows_set = true;
-            } else {
-                add_inplace_kernel<<<(unsigned)((3 * n_fw + bs - 1) / bs), bs, 0, fl->cur>>>(d_v, d_tmp, 3 * n_fw);
-                count_launch(1);
-                fl->launches += 1;
-            }
-        }
-        if (n_bw > 0) {
-            add_inplace_kernel<<<(unsigned)((3 * n_bw + bs - 1) / bs), bs, 0, fl->cur>>>(
-                d_v + 3 * (n_fw + n_sw), d_tmp + 3 * n_fw, 3 * n_bw);
-            count_launch(1);
-            fl->launches += 1;
-        }
-        CUDA_TRY(cudaGetLastError());
-    }
-    if (!fib_rows_set && n_fw > 0)
-        CUDA_TRY(cudaMemsetAsync(d_v, 0, (size_t)n_fw * 24, fl->cur));
-    // 5. v_all += bc.flow(r_all, x_bodies, body_link_conditions, eta)     (system.cpp:316)
-    SKB_TRY(bodies_dev(fl, fl->body[1], d_bd, d_f, d_t, eta, d_v, 1));
-    // 6. PULL: own fiber rows += sum over the members' partial sums (reduce-scatter fused with the accumulation)
-    if (fib_rows_pending) {
-        SKB_TRY(group_flag(fl, 1, false, true));
-        if (n_fw > 0) {
-            GroupPullArgs a;
-            a.size = G.dry ? 1 : G.size;
-            for (int m = 0; m < a.size; ++m)
-                a.u_part[m] = G.at<double>(G.dry ? G.rank : m, G.off_upart);
-            a.fa = fl->fa;
-            a.n_f = n_fw;
-            a.v = d_v;
-            a.accumulate = 1;
-            group_pull_kernel<<<(unsigned)((3 * n_fw + 255) / 256), 256, 0, fl->cur>>>(a);
-            CUDA_TRY(cudaGetLastError());
-            count_launch(1);
-            fl->launches += 1;
-        }
-        if (crossed && n_sw > 0) { // own periphery rows += the members' Stokeslet partials
-            GroupPullArgs a;
-            a.size = G.dry ? 1 : G.size;
-            for (int m = 0; m < a.size; ++m)
-                a.u_part[m] = G.at<double>(G.dry ? G.rank : m, G.off_upart_shell);
-            a.fa = fl->sa;
-            a.n_f = n_sw;
-            a.v = d_v + 3 * n_fw;
-            a.accumulate = 1;
-            group_pull_kernel<<<(unsigned)((3 * n_sw + 255) / 256), 256, 0, fl->cur>>>(a);
-            CUDA_TRY(cudaGetLastError());
-            count_launch(1);
-            fl->launches += 1;
-        }
-    }
-    // 7. self term of the own fibers (fcfd.cpp:203-210), unless the kernels already skipped intra-fiber pairs
-    if (n_fw > 0 && !df.src[SKB_STOKESLET].excl) {
-        const size_t smem = (size_t)fl->max_fiber_nodes * 6 * sizeof(double);
-        fiber_self_subtract_kernel<<<fl->n_fibers, 128, smem, fl->cur>>>(
-            (const double *)fl->r_fib.ptr, f_sl, (const long long *)fl->fiber_offset.ptr, 1.0 / (8.0 * M_PI * eta),
-            kReg * kReg, kEps, d_v, fl->fa, fl->fb);
-        CUDA_TRY(cudaGetLastError());
-        count_launch(1);
-        fl->launches += 1;
-    }
-    return SKB_OK;
+    const long long work = 3 * n_fw + n_sw;
+    if (work == 0)
+        return SKB_OK;
+    const unsigned nblk = (unsigned)std::min<long long>((work + 255) / 256, 4LL * df.info.num_sms);
+    group_push_kernel<<<nblk, 256, 0, fl->cur>>>(a);
+    return launched(fl, 1);
 }
 
-// The same with the fiber <-> periphery pairs in one geometry pass (cross_kernels.cuh): whole system on this device.
-//   fiber evaluator targets  = [fibers | bodies]   (symmetric fiber-fiber block + the body rows)
-//   cross kernel             : stresslet of every periphery node at the fiber nodes, Stokeslet of every fiber node at
-//                              the periphery nodes (system.cpp:299 and :304,313-315 from one pass over the pairs)
-//   periphery evaluator      = [bodies] only
-static int matvec_core_cross(skb_flow *fl, const double *d_ff, const double *d_sd, const double *d_bd, const double *d_f,
-                             const double *d_t, double eta, double *d_v) {
-    const long long ns = fl->n_shell, nf = fl->n_fib;
-    const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa, n_bw = fl->bb - fl->ba; // == nf, ns, nb here
+// PULL: d_v rows [0, n_rows) += the sum of every member's partial rows [row0, row0 + n_rows) at window offset `off`
+// (reduce-scatter fused with the accumulation)
+static int group_pull(skb_flow *fl, size_t off, long long row0, long long n_rows, double *d_v) {
+    if (n_rows == 0)
+        return SKB_OK;
+    const skb_flow::Group &G = fl->grp;
+    GroupPullArgs a;
+    a.size = G.dry ? 1 : G.size;
+    for (int m = 0; m < a.size; ++m)
+        a.u_part[m] = G.at<double>(G.dry ? G.rank : m, off);
+    a.fa = row0;
+    a.n_f = n_rows;
+    a.v = d_v;
+    a.accumulate = 1;
+    group_pull_kernel<<<(unsigned)((3 * n_rows + 255) / 256), 256, 0, fl->cur>>>(a);
+    return launched(fl, 1);
+}
+
+// v = fc.flow(r_all, fw, eta)  (system.cpp:299) at the fiber evaluator's targets.  Symmetric producers: the symmetric
+// kernel writes the fiber rows -- complete, or in a group this member's partial sums for ALL fiber rows into its
+// window -- and the plain kernel the rest: [own periphery rows (not with the cross kernel) | own body rows]
+static int fiber_rows(skb_flow *fl, StrengthMode mode, const double *ff, double eta, double *d_v) {
+    const skb_flow::MatvecPlan &P = fl->plan;
+    if (P.fib_rows == skb_flow::MatvecPlan::kPlain)
+        return fibers_dev(fl, fl->fib[1], mode, ff, eta, 0, d_v, 0, fl->fa, fl->fb);
+    const skb_flow::Group &G = fl->grp;
+    const long long nf = fl->n_fib, n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa, n_bw = fl->bb - fl->ba;
     DeviceState &df = fl->fib[1]->devs[0];
-    DeviceState &dsh = fl->shell[1]->devs[0];
-    double *d_v_body = d_v + 3 * (n_fw + n_sw);
-    // fc.flow at [fibers | bodies]: the symmetric kernel writes the fiber rows, the plain kernel the body rows.  Should the
-    // symmetric path decline (memory), everything lands contiguously in the scratch buffer and is moved into place.
     SKB_TRY(fl->scratch_u.ensure((size_t)df.n_trg * 24 + 8));
     EvalOpts o;
-    o.d_u_sym = d_v;
-    o.d_u_rem = d_v_body;
-    SKB_TRY(eval_on_device(fl->fib[1], df, SKB_STOKESLET, kRaw, d_ff, 0.0, (double *)fl->scratch_u.ptr, 0, fl->cur, false,
-                           &fl->launches, nullptr, 1.0 / eta, o));
-    if (!fl->fib[1]->last_was_sym) {
-        CUDA_TRY(cudaMemcpyAsync(d_v, fl->scratch_u.ptr, (size_t)n_fw * 24, cudaMemcpyDeviceToDevice, fl->cur));
-        if (n_bw > 0)
-            CUDA_TRY(cudaMemcpyAsync(d_v_body, (const double *)fl->scratch_u.ptr + 3 * n_fw, (size_t)n_bw * 24,
-                                     cudaMemcpyDeviceToDevice, fl->cur));
-    }
-    fl->pairs += nf * (n_fw + n_bw);
-    if (!df.src[SKB_STOKESLET].excl) { // fcfd.cpp:203-210
-        const size_t smem = (size_t)fl->max_fiber_nodes * 6 * sizeof(double);
-        fiber_self_subtract_kernel<<<fl->n_fibers, 128, smem, fl->cur>>>(
-            (const double *)fl->r_fib.ptr, df.src[SKB_STOKESLET].f_cur, (const long long *)fl->fiber_offset.ptr,
-            1.0 / (8.0 * M_PI * eta), kReg * kReg, kEps, d_v, fl->fa, fl->fb);
-        CUDA_TRY(cudaGetLastError());
-        count_launch(1);
-        fl->launches += 1;
-    }
-    // periphery strengths 2 eta n (x) rho -> sym6 (periphery.cpp:68-71), once for both uses
-    SKB_TRY(pack_on_device(dsh, SKB_STRESSLET, kNormalDensity, d_sd, 2.0 * eta, fl->cur, &fl->launches));
-    const SourceSet &sf = df.src[SKB_STOKESLET], &ss = dsh.src[SKB_STRESSLET];
-    SKB_TRY(cross_eval(fl->cross, df.info, (const double *)sf.r.ptr, sf.f_cur, fl->fa, n_fw, (const double *)ss.r.ptr,
-                       ss.f_cur, ns, ss.n_pad, -3.0 / (8.0 * M_PI * eta), 1.0 / (8.0 * M_PI * eta), d_v, 1,
-                       d_v + 3 * n_fw, 0, fl->cur, &fl->launches));
-    fl->pairs += 2 * n_fw * ns;
-    // periphery -> body rows (system.cpp:313-315)
-    if (n_bw > 0) {
-        SKB_TRY(fl->tmp.ensure((size_t)n_bw * 24 + 8));
-        SKB_TRY(eval_on_device(fl->shell[1], dsh, SKB_STRESSLET, kPacked, ss.f_cur, 2.0 * eta, (double *)fl->tmp.ptr, 0,
-                               fl->cur, false, &fl->launches, nullptr, 1.0 / eta));
-        add_inplace_kernel<<<(unsigned)((3 * n_bw + 255) / 256), 256, 0, fl->cur>>>(d_v_body, (const double *)fl->tmp.ptr,
-                                                                                  3 * n_bw);
-        CUDA_TRY(cudaGetLastError());
-        count_launch(1);
-        fl->launches += 1;
-        fl->pairs += ns * n_bw;
-    }
-    // v_all += bc.flow(r_all, x_bodies, body_link_conditions, eta)     system.cpp:316
-    SKB_TRY(bodies_dev(fl, fl->body[1], d_bd, d_f, d_t, eta, d_v, 1));
+    o.d_u_sym = P.grouped ? G.at<double>(G.rank, G.off_upart) : d_v;
+    o.d_u_rem = d_v + 3 * (n_fw + (P.cross ? n_sw : 0));
+    SKB_TRY(eval_on_device(fl->fib[1], df, SKB_STOKESLET, mode, ff, 0.0, (double *)fl->scratch_u.ptr, 0, fl->cur,
+                           false, &fl->launches, nullptr, 1.0 / eta, o));
+    fl->pairs += nf * nf / (P.grouped ? G.size : 1) + nf * ((P.cross ? 0 : n_sw) + n_bw);
+    if (fl->fib[1]->last_was_sym)
+        return SKB_OK;
+    if (P.grouped)
+        return set_error(SKB_ERR_STATE, "group member %d: the symmetric kernel declined (memory for the reverse "
+                                        "partials?); lower SKB_SYM_MAX_BYTES pressure or use fewer nodes per GPU",
+                         G.rank);
+    // the symmetric path declined (memory): everything landed contiguously in the scratch buffer
+    CUDA_TRY(cudaMemcpyAsync(d_v, fl->scratch_u.ptr, (size_t)n_fw * 24, cudaMemcpyDeviceToDevice, fl->cur));
+    if (n_bw > 0)
+        CUDA_TRY(cudaMemcpyAsync(o.d_u_rem, (const double *)fl->scratch_u.ptr + 3 * n_fw, (size_t)n_bw * 24,
+                                 cudaMemcpyDeviceToDevice, fl->cur));
     return SKB_OK;
 }
 
-// device-side matvec flow on fl->cur: all strengths resident, d_v = window rows of v_all
+// fiber <-> periphery pairs in one geometry pass (cross_kernels.cuh): stresslet sums of every periphery node (packed
+// strengths s6) at the own fiber rows, Stokeslet sums of the own fibers at every periphery row.  Without a group both
+// are complete: the fiber rows add onto the fiber-fiber sums, the periphery rows are written.  In a group the fiber rows
+// are written (the fiber-fiber sums come with the pull), the Stokeslet sums are this member's partials in its window,
+// and the own periphery rows start from zero until the members' partials are pulled in.
+static int cross_rows(skb_flow *fl, const double *s6, double eta, double *d_v) {
+    const bool grouped = fl->plan.grouped;
+    const skb_flow::Group &G = fl->grp;
+    const long long ns = fl->n_shell, n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
+    DeviceState &df = fl->fib[1]->devs[0];
+    const SourceSet &sf = df.src[SKB_STOKESLET], &ss = fl->shell[1]->devs[0].src[SKB_STRESSLET];
+    double *u_shell = grouped ? G.at<double>(G.rank, G.off_upart_shell) : d_v + 3 * n_fw;
+    SKB_TRY(cross_eval(fl->cross, df.info, (const double *)sf.r.ptr, sf.f_cur, fl->fa, n_fw, (const double *)ss.r.ptr,
+                       s6, ns, ss.n_pad, -3.0 / (8.0 * M_PI * eta), 1.0 / (8.0 * M_PI * eta), d_v, grouped ? 0 : 1,
+                       u_shell, 0, fl->cur, &fl->launches));
+    fl->pairs += 2 * n_fw * ns;
+    if (grouped && n_sw > 0)
+        CUDA_TRY(cudaMemsetAsync(d_v + 3 * n_fw, 0, (size_t)n_sw * 24, fl->cur));
+    return SKB_OK;
+}
+
+// v_fibers, v_bodies += shell.flow(r_fibbody, x_shell, eta)  (system.cpp:304,313-315) through tmp.  The periphery
+// evaluator's targets are [own fiber rows | own body rows], the body rows only when the cross kernel covers the fiber
+// rows.  A group member's symmetric path has not written its fiber rows yet: they are set here (copied, or zeroed
+// without periphery) and the pull adds the fiber-fiber sums.
+static int periphery_rows(skb_flow *fl, StrengthMode mode, const double *sd, double eta, double *d_v) {
+    const long long ns = fl->n_shell, n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa, n_bw = fl->bb - fl->ba;
+    const long long n_fr = fl->plan.cross ? 0 : n_fw; // fiber rows among the periphery evaluator's targets
+    const bool set_fib = fl->plan.fib_rows == skb_flow::MatvecPlan::kSymPartial;
+    if (ns == 0 || n_fr + n_bw == 0) {
+        if (set_fib && n_fr > 0)
+            CUDA_TRY(cudaMemsetAsync(d_v, 0, (size_t)n_fr * 24, fl->cur));
+        return SKB_OK;
+    }
+    SKB_TRY(fl->tmp.ensure((size_t)(n_fr + n_bw) * 24 + 8));
+    double *d_tmp = (double *)fl->tmp.ptr;
+    SKB_TRY(periphery_dev(fl, fl->shell[1], mode, sd, eta, d_tmp, 0));
+    const int bs = 256;
+    if (n_fr > 0 && set_fib) {
+        CUDA_TRY(cudaMemcpyAsync(d_v, d_tmp, (size_t)n_fr * 24, cudaMemcpyDeviceToDevice, fl->cur));
+    } else if (n_fr > 0) {
+        add_inplace_kernel<<<(unsigned)((3 * n_fr + bs - 1) / bs), bs, 0, fl->cur>>>(d_v, d_tmp, 3 * n_fr);
+        SKB_TRY(launched(fl, 1));
+    }
+    if (n_bw > 0) {
+        add_inplace_kernel<<<(unsigned)((3 * n_bw + bs - 1) / bs), bs, 0, fl->cur>>>(d_v + 3 * (n_fw + n_sw),
+                                                                                  d_tmp + 3 * n_fr, 3 * n_bw);
+        SKB_TRY(launched(fl, 1));
+    }
+    return SKB_OK;
+}
+
+// device-side matvec flow on fl->cur, as fl->plan says: d_ff / d_sd are the strengths of the own fibers / periphery
+// rows (all of them without a group), body inputs are complete; d_v = [own fiber rows | own shell rows | own body rows]
+// of v_all
 static int matvec_core(skb_flow *fl, const double *d_ff, const double *d_sd, const double *d_bd, const double *d_f,
                        const double *d_t, double eta, double *d_v) {
-    if (fl->grp.size > 1)
-        return matvec_core_group(fl, d_ff, d_sd, d_bd, d_f, d_t, eta, d_v);
-    const long long ns = fl->n_shell;
-    const long long n_win = fl->n_win, n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa, n_bw = fl->bb - fl->ba;
-    if (n_win == 0)
+    const skb_flow::MatvecPlan &P = fl->plan;
+    skb_flow::Group &G = fl->grp;
+    const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
+    // strengths as the caller ships them (packed by the evaluations), or packed by the push into the group window
+    StrengthMode fmode = kRaw, smode = kNormalDensity;
+    const double *ff = d_ff, *sd = d_sd;
+    if (P.grouped) {
+        if (!G.dry && !G.connected())
+            return set_error(SKB_ERR_STATE, "group member %d: not all peers are connected (skb_flow_group_import / "
+                                            "_connect)", G.rank);
+        G.epoch += 1; // the only place it advances: its parity picks the window half of this matvec
+        SKB_TRY(group_push(fl, d_ff, d_sd, eta));
+        SKB_TRY(group_flag(fl, 0, true, true)); // every member's strengths have landed here
+        fmode = smode = kPacked;
+        ff = G.at<double>(G.rank, G.off_fsl[G.epoch & 1]);
+        sd = G.at<double>(G.rank, G.off_fshell[G.epoch & 1]);
+    } else if (fl->n_win == 0) {
         return SKB_OK;
-    SKB_TRY(overlap_launch(fl));
-    if (fl->use_cross)
-        return matvec_core_cross(fl, d_ff, d_sd, d_bd, d_f, d_t, eta, d_v);
-    // v_all = fc.flow(r_all, fw, eta)                                  system.cpp:299
-    // (this rank's fiber rows come first, so the self term applies to targets [0, n_fw) of its list)
-    SKB_TRY(fibers_dev(fl, fl->fib[1], d_ff, eta, n_fw > 0, d_v, 0, fl->fa, fl->fb));
-    // v_fibers, v_bodies += shell.flow(r_fibbody, x_shell, eta)         system.cpp:304,313-315
-    if (ns > 0 && n_fw + n_bw > 0) {
-        SKB_TRY(fl->tmp.ensure((size_t)(n_fw + n_bw) * 24 + 8));
-        double *d_tmp = (double *)fl->tmp.ptr;
-        SKB_TRY(periphery_dev(fl, fl->shell[1], d_sd, eta, d_tmp, 0));
-        const int bs = 256;
-        if (n_fw > 0) {
-            add_inplace_kernel<<<(unsigned)((3 * n_fw + bs - 1) / bs), bs, 0, fl->cur>>>(d_v, d_tmp, 3 * n_fw);
-            count_launch(1);
-            fl->launches += 1;
-        }
-        if (n_bw > 0) {
-            add_inplace_kernel<<<(unsigned)((3 * n_bw + bs - 1) / bs), bs, 0, fl->cur>>>(
-                d_v + 3 * (n_fw + n_sw), d_tmp + 3 * n_fw, 3 * n_bw);
-            count_launch(1);
-            fl->launches += 1;
-        }
-        CUDA_TRY(cudaGetLastError());
     }
-    // v_all += bc.flow(r_all, x_bodies, body_link_conditions, eta)     system.cpp:316
+    SKB_TRY(overlap_launch(fl, d_sd)); // (x_shell is complete on this device from here on)
+    SKB_TRY(fiber_rows(fl, fmode, ff, eta, d_v));
+    // The self term subtracts from the fiber rows: without a group right after the fiber flow; a group member
+    // subtracts it last, once the pull has completed its fiber rows (the plain-kernel member keeps that order too).
+    if (!P.grouped)
+        SKB_TRY(fiber_self_term(fl, fl->fib[1], eta, d_v, fl->fa, fl->fb));
+    if (P.cross) {
+        if (!P.grouped) { // periphery strengths 2 eta n (x) rho -> sym6 (periphery.cpp:68-71), once for both uses
+            DeviceState &dsh = fl->shell[1]->devs[0];
+            SKB_TRY(pack_on_device(dsh, SKB_STRESSLET, kNormalDensity, d_sd, 2.0 * eta, fl->cur, &fl->launches));
+            smode = kPacked;
+            sd = dsh.src[SKB_STRESSLET].f_cur;
+        }
+        SKB_TRY(cross_rows(fl, sd, eta, d_v));
+    }
+    const bool partial = P.fib_rows == skb_flow::MatvecPlan::kSymPartial;
+    if (partial)
+        SKB_TRY(group_flag(fl, 1, true, false)); // my partial sums are complete
+    SKB_TRY(periphery_rows(fl, smode, sd, eta, d_v));
+    // v_all += bc.flow(r_all, x_bodies, body_link_conditions, eta)     (system.cpp:316)
     SKB_TRY(bodies_dev(fl, fl->body[1], d_bd, d_f, d_t, eta, d_v, 1));
+    if (partial) {
+        SKB_TRY(group_flag(fl, 1, false, true));
+        SKB_TRY(group_pull(fl, G.off_upart, fl->fa, n_fw, d_v));
+        if (P.cross) // own periphery rows += the members' Stokeslet partials
+            SKB_TRY(group_pull(fl, G.off_upart_shell, fl->sa, n_sw, d_v + 3 * n_fw));
+    }
+    if (P.grouped)
+        SKB_TRY(fiber_self_term(fl, fl->fib[1], eta, d_v, fl->fa, fl->fb));
     return SKB_OK;
 }
 
@@ -1302,12 +1269,12 @@ int skb_flow_group_warmup(skb_flow *fl) {
     CUDA_TRY(cudaMemsetAsync(z.ptr, 0, n_z * 8, fl->stream));
     SKB_TRY(fl->vel.ensure((size_t)fl->n_win * 24 + 8));
     SKB_TRY(fl->in_fib.ensure((size_t)n_fw * 24 + 8));
-    if (n_sw > 0 && fl->bg.enabled)
-        SKB_TRY(overlap_buffers(fl, 3 * n_sw));
+    if (n_sw > 0)
+        SKB_TRY(flow_size_overlap(fl, 3 * n_sw));
     fl->cur = fl->stream;
     fl->grp.dry = true;
     const double *zp = (const double *)z.ptr;
-    int rc = matvec_core_group(fl, zp, zp, zp, zp, zp, 1.0, (double *)fl->vel.ptr);
+    int rc = matvec_core(fl, zp, zp, zp, zp, zp, 1.0, (double *)fl->vel.ptr);
     fl->grp.dry = false;
     cudaError_t e = cudaStreamSynchronize(fl->stream);
     fl->grp.epoch = 0;
@@ -1418,61 +1385,39 @@ int skb_flow_matvec(skb_flow *fl, const double *fib_forces, const double *shell_
     std::vector<double> f, t;
     if (fl->n_bodies > 0)
         split_forces_torques(body_forces_torques, fl->n_bodies, f, t);
-    fl->cur = fl->stream;
-    const size_t n_in = (size_t)(nf + ns + nb) * 3 + f.size() + t.size(), n_out = (size_t)n_win * 3;
-    if (fl->graphs_enabled && (n_in + n_out) * 8 <= kGraphMaxBytes) {
-        // launch-bound size: stage through pinned memory and replay the whole sequence as one CUDA graph
-        SKB_TRY(ensure_stage(fl, n_in + n_out));
-        double *h = fl->h_stage;
-        double *h_ff = h, *h_sd = h_ff + 3 * nf, *h_bd = h_sd + 3 * ns, *h_f = h_bd + 3 * nb, *h_t = h_f + f.size();
-        double *h_v = h_t + t.size();
-        if (nf) std::memcpy(h_ff, fib_forces, (size_t)nf * 24);
-        if (ns) std::memcpy(h_sd, shell_density, (size_t)ns * 24);
-        if (nb) std::memcpy(h_bd, body_densities, (size_t)nb * 24);
-        if (!f.empty()) std::memcpy(h_f, f.data(), f.size() * 8);
-        if (!t.empty()) std::memcpy(h_t, t.data(), t.size() * 8);
-        SKB_TRY(fl->vel.ensure((size_t)n_win * 24));
-        unsigned long long key = mix_key(fl->geom_version, (unsigned long long)fl->fa);
-        key = mix_key(key, (unsigned long long)fl->n_win);
-        key = mix_key(key, dbl_bits(eta));
-        key = mix_key(key, buffer_key(fl, 1));
-        const size_t nfs = f.size();
-        auto body = [&]() -> int {
-            SKB_TRY(upload(fl, fl->in_fib, h_ff, (size_t)nf * 3));
-            SKB_TRY(upload(fl, fl->in_shell, h_sd, (size_t)ns * 3));
-            SKB_TRY(upload(fl, fl->in_body, h_bd, (size_t)nb * 3));
-            SKB_TRY(upload(fl, fl->in_force, h_f, nfs));
-            SKB_TRY(upload(fl, fl->in_torque, h_t, nfs));
-            SKB_TRY(matvec_core(fl, (const double *)fl->in_fib.ptr, (const double *)fl->in_shell.ptr,
-                                (const double *)fl->in_body.ptr, (const double *)fl->in_force.ptr,
-                                (const double *)fl->in_torque.ptr, eta, (double *)fl->vel.ptr));
-            CUDA_TRY(cudaMemcpyAsync(h_v, fl->vel.ptr, (size_t)n_win * 24, cudaMemcpyDeviceToHost, fl->stream));
-            return SKB_OK;
-        };
-        CUDA_TRY(cudaEventRecord(fl->evt0, fl->stream));
-        CUDA_TRY(cudaEventRecord(fl->ev0, fl->stream));
-        SKB_TRY(run_graphed(fl, fl->g_matvec, key, body));
-        CUDA_TRY(cudaEventRecord(fl->ev1, fl->stream));
-        CUDA_TRY(cudaEventRecord(fl->evt1, fl->stream));
-        SKB_TRY(finish_stats(fl));
-        std::memcpy(v_all, h_v, (size_t)n_win * 24);
-        return SKB_OK;
-    }
-    CUDA_TRY(cudaEventRecord(fl->evt0, fl->stream));
-    SKB_TRY(upload(fl, fl->in_fib, fib_forces, (size_t)nf * 3));
-    SKB_TRY(upload(fl, fl->in_shell, shell_density, (size_t)ns * 3));
-    SKB_TRY(upload(fl, fl->in_body, body_densities, (size_t)nb * 3));
-    SKB_TRY(upload(fl, fl->in_force, f.data(), f.size()));
-    SKB_TRY(upload(fl, fl->in_torque, t.data(), t.size()));
     SKB_TRY(fl->vel.ensure((size_t)n_win * 24));
-    CUDA_TRY(cudaEventRecord(fl->ev0, fl->stream));
-    SKB_TRY(matvec_core(fl, (const double *)fl->in_fib.ptr, (const double *)fl->in_shell.ptr,
-                        (const double *)fl->in_body.ptr, (const double *)fl->in_force.ptr,
-                        (const double *)fl->in_torque.ptr, eta, (double *)fl->vel.ptr));
-    CUDA_TRY(cudaEventRecord(fl->ev1, fl->stream));
-    CUDA_TRY(cudaMemcpyAsync(v_all, fl->vel.ptr, (size_t)n_win * 24, cudaMemcpyDeviceToHost, fl->stream));
-    CUDA_TRY(cudaEventRecord(fl->evt1, fl->stream));
-    return finish_stats(fl);
+    Staged s;
+    SKB_TRY(stage_inputs(fl, fib_forces, shell_density, body_densities, f, t, v_all, (size_t)n_win * 3, s));
+    auto up = [&]() -> int {
+        SKB_TRY(upload(fl, fl->in_fib, s.ff, (size_t)nf * 3));
+        SKB_TRY(upload(fl, fl->in_shell, s.sd, (size_t)ns * 3));
+        SKB_TRY(upload(fl, fl->in_body, s.bd, (size_t)nb * 3));
+        SKB_TRY(upload(fl, fl->in_force, s.f, f.size()));
+        return upload(fl, fl->in_torque, s.t, t.size());
+    };
+    auto work = [&] {
+        return matvec_core(fl, (const double *)fl->in_fib.ptr, (const double *)fl->in_shell.ptr,
+                           (const double *)fl->in_body.ptr, (const double *)fl->in_force.ptr,
+                           (const double *)fl->in_torque.ptr, eta, (double *)fl->vel.ptr);
+    };
+    auto down = [&] { return download(fl, s.v, fl->vel, (size_t)n_win * 3); };
+    if (!s.pinned)
+        return host_frame(fl, up, work, down);
+    // launch-bound size: replay the whole sequence, copies included, as one CUDA graph
+    unsigned long long key = mix_key(fl->geom_version, (unsigned long long)fl->fa);
+    key = mix_key(key, (unsigned long long)fl->n_win);
+    key = mix_key(key, dbl_bits(eta));
+    key = mix_key(key, buffer_key(fl, 1));
+    auto graphed = [&] {
+        return run_graphed(fl, fl->g_matvec, key, [&]() -> int {
+            SKB_TRY(up());
+            SKB_TRY(work());
+            return down();
+        });
+    };
+    SKB_TRY(host_frame(fl, nothing, graphed, nothing));
+    std::memcpy(v_all, s.v, (size_t)n_win * 24);
+    return SKB_OK;
 }
 
 int skb_flow_matvec_device(skb_flow *fl, const double *d_fib_forces, const double *d_shell_density,
@@ -1494,11 +1439,7 @@ int skb_flow_matvec_device(skb_flow *fl, const double *d_fib_forces, const doubl
     fl->cur = (cudaStream_t)stream;
     SKB_TRY(matvec_core(fl, d_fib_forces, d_shell_density, d_body_densities, d_body_forces, d_body_torques, eta,
                         d_v_window));
-    fl->stats.device_ms = 0;
-    fl->stats.total_ms = 0;
-    fl->stats.n_pairs = fl->pairs;
-    fl->stats.launches = fl->launches;
-    return SKB_OK;
+    return device_stats(fl);
 }
 
 // ---- per-fiber dense operators (SURVEY.md §8f N2) ---------------------------------------------------------------
@@ -1676,10 +1617,7 @@ static int fiber_force_dev(skb_flow *fl, const double *d_x, double *d_fw) {
         return SKB_OK;
     fiber_gemv_kernel<1><<<fl->n_items_F, kFiberGemvThreads, fl->gemv_smem, fl->cur>>>(
         (const FiberGemvItem *)fl->items_F.ptr, (const double *)fl->op_F.ptr, d_x, d_fw, FiberVelArgs{});
-    CUDA_TRY(cudaGetLastError());
-    count_launch(1);
-    fl->launches += 1;
-    return SKB_OK;
+    return launched(fl, 1);
 }
 
 // res = A_ x - P_downsample_bc vT(v) + xs_vT + y_BC per fiber (ffd.cpp:276-312), one launch; on fl->cur
@@ -1699,10 +1637,7 @@ static int fiber_matvec_dev(skb_flow *fl, const double *d_x, const double *d_v, 
     va.v_boundary = d_vb;
     fiber_gemv_kernel<2><<<fl->n_items_A, kFiberGemvThreads, fl->gemv_smem, fl->cur>>>(
         (const FiberGemvItem *)fl->items_A.ptr, (const double *)fl->op_A.ptr, d_x, d_res, va);
-    CUDA_TRY(cudaGetLastError());
-    count_launch(1);
-    fl->launches += 1;
-    return SKB_OK;
+    return launched(fl, 1);
 }
 
 // y = A_^-1 x per fiber: FiberContainerFiniteDifference::apply_preconditioner (fcfd.cpp:331-339) with the LU solve
@@ -1712,10 +1647,7 @@ static int fiber_precond_dev(skb_flow *fl, const double *d_x, double *d_y) {
         return SKB_OK;
     fiber_gemv_kernel<0><<<fl->n_items_A, kFiberGemvThreads, fl->gemv_smem, fl->cur>>>(
         (const FiberGemvItem *)fl->items_A.ptr, (const double *)fl->op_Ainv.ptr, d_x, d_y, FiberVelArgs{});
-    CUDA_TRY(cudaGetLastError());
-    count_launch(1);
-    fl->launches += 1;
-    return SKB_OK;
+    return launched(fl, 1);
 }
 
 static int need_precond(const skb_flow *fl, const char *who) {
@@ -1739,15 +1671,10 @@ int skb_flow_apply_fiber_preconditioner(skb_flow *fl, const double *x_fibers, do
     if (!x_fibers || !y)
         return set_error(SKB_ERR_INVALID, "skb_flow_apply_fiber_preconditioner: NULL argument");
     CUDA_TRY(cudaSetDevice(fl->dev));
-    fl->cur = fl->stream;
-    CUDA_TRY(cudaEventRecord(fl->evt0, fl->stream));
-    CUDA_TRY(cudaMemcpyAsync(fl->x_fib.ptr, x_fibers, (size_t)nf * 32, cudaMemcpyHostToDevice, fl->stream));
-    CUDA_TRY(cudaEventRecord(fl->ev0, fl->stream));
-    SKB_TRY(fiber_precond_dev(fl, (const double *)fl->x_fib.ptr, (double *)fl->res_fib.ptr));
-    CUDA_TRY(cudaEventRecord(fl->ev1, fl->stream));
-    CUDA_TRY(cudaMemcpyAsync(y, fl->res_fib.ptr, (size_t)nf * 32, cudaMemcpyDeviceToHost, fl->stream));
-    CUDA_TRY(cudaEventRecord(fl->evt1, fl->stream));
-    return finish_stats(fl);
+    return host_frame(
+        fl, [&] { return upload(fl, fl->x_fib, x_fibers, (size_t)nf * 4); },
+        [&] { return fiber_precond_dev(fl, (const double *)fl->x_fib.ptr, (double *)fl->res_fib.ptr); },
+        [&] { return download(fl, y, fl->res_fib, (size_t)nf * 4); });
 }
 
 int skb_flow_apply_fiber_preconditioner_device(skb_flow *fl, const double *d_x_fibers, double *d_y, void *stream) {
@@ -1762,10 +1689,7 @@ int skb_flow_apply_fiber_preconditioner_device(skb_flow *fl, const double *d_x_f
     CUDA_TRY(cudaSetDevice(fl->dev));
     fl->cur = (cudaStream_t)stream;
     SKB_TRY(fiber_precond_dev(fl, d_x_fibers, d_y));
-    fl->stats.device_ms = fl->stats.total_ms = 0;
-    fl->stats.n_pairs = 0;
-    fl->stats.launches = fl->launches;
-    return SKB_OK;
+    return device_stats(fl);
 }
 
 int skb_flow_apply_fiber_force(skb_flow *fl, const double *x_fibers, double *fw) {
@@ -1779,16 +1703,14 @@ int skb_flow_apply_fiber_force(skb_flow *fl, const double *x_fibers, double *fw)
     if (!x_fibers || !fw)
         return set_error(SKB_ERR_INVALID, "skb_flow_apply_fiber_force: NULL argument");
     CUDA_TRY(cudaSetDevice(fl->dev));
-    fl->cur = fl->stream;
-    CUDA_TRY(cudaEventRecord(fl->evt0, fl->stream));
-    CUDA_TRY(cudaMemcpyAsync(fl->x_fib.ptr, x_fibers, (size_t)nf * 32, cudaMemcpyHostToDevice, fl->stream));
-    SKB_TRY(fl->in_fib.ensure((size_t)nf * 24));
-    CUDA_TRY(cudaEventRecord(fl->ev0, fl->stream));
-    SKB_TRY(fiber_force_dev(fl, (const double *)fl->x_fib.ptr, (double *)fl->in_fib.ptr));
-    CUDA_TRY(cudaEventRecord(fl->ev1, fl->stream));
-    CUDA_TRY(cudaMemcpyAsync(fw, fl->in_fib.ptr, (size_t)nf * 24, cudaMemcpyDeviceToHost, fl->stream));
-    CUDA_TRY(cudaEventRecord(fl->evt1, fl->stream));
-    return finish_stats(fl);
+    return host_frame(
+        fl,
+        [&]() -> int {
+            SKB_TRY(upload(fl, fl->x_fib, x_fibers, (size_t)nf * 4));
+            return fl->in_fib.ensure((size_t)nf * 24);
+        },
+        [&] { return fiber_force_dev(fl, (const double *)fl->x_fib.ptr, (double *)fl->in_fib.ptr); },
+        [&] { return download(fl, fw, fl->in_fib, (size_t)nf * 3); });
 }
 
 int skb_flow_fiber_matvec(skb_flow *fl, const double *x_fibers, const double *v_fibers, const double *v_fib_boundary,
@@ -1803,21 +1725,18 @@ int skb_flow_fiber_matvec(skb_flow *fl, const double *x_fibers, const double *v_
     if (!x_fibers || !v_fibers || !res)
         return set_error(SKB_ERR_INVALID, "skb_flow_fiber_matvec: NULL argument");
     CUDA_TRY(cudaSetDevice(fl->dev));
-    fl->cur = fl->stream;
-    CUDA_TRY(cudaEventRecord(fl->evt0, fl->stream));
-    CUDA_TRY(cudaMemcpyAsync(fl->x_fib.ptr, x_fibers, (size_t)nf * 32, cudaMemcpyHostToDevice, fl->stream));
-    SKB_TRY(fl->vel.ensure((size_t)nf * 24));
-    CUDA_TRY(cudaMemcpyAsync(fl->vel.ptr, v_fibers, (size_t)nf * 24, cudaMemcpyHostToDevice, fl->stream));
-    if (v_fib_boundary)
-        CUDA_TRY(cudaMemcpyAsync(fl->vb.ptr, v_fib_boundary, (size_t)(fl->op_f1 - fl->op_f0) * 56, cudaMemcpyHostToDevice,
-                                 fl->stream));
-    CUDA_TRY(cudaEventRecord(fl->ev0, fl->stream));
-    SKB_TRY(fiber_matvec_dev(fl, (const double *)fl->x_fib.ptr, (const double *)fl->vel.ptr,
-                             v_fib_boundary ? (const double *)fl->vb.ptr : nullptr, (double *)fl->res_fib.ptr));
-    CUDA_TRY(cudaEventRecord(fl->ev1, fl->stream));
-    CUDA_TRY(cudaMemcpyAsync(res, fl->res_fib.ptr, (size_t)nf * 32, cudaMemcpyDeviceToHost, fl->stream));
-    CUDA_TRY(cudaEventRecord(fl->evt1, fl->stream));
-    return finish_stats(fl);
+    return host_frame(
+        fl,
+        [&]() -> int {
+            SKB_TRY(upload(fl, fl->x_fib, x_fibers, (size_t)nf * 4));
+            SKB_TRY(upload(fl, fl->vel, v_fibers, (size_t)nf * 3));
+            return v_fib_boundary ? upload(fl, fl->vb, v_fib_boundary, (size_t)(fl->op_f1 - fl->op_f0) * 7) : SKB_OK;
+        },
+        [&] {
+            return fiber_matvec_dev(fl, (const double *)fl->x_fib.ptr, (const double *)fl->vel.ptr,
+                                    v_fib_boundary ? (const double *)fl->vb.ptr : nullptr, (double *)fl->res_fib.ptr);
+        },
+        [&] { return download(fl, res, fl->res_fib, (size_t)nf * 4); });
 }
 
 int skb_flow_apply_fiber_force_device(skb_flow *fl, const double *d_x_fibers, double *d_fw, void *stream) {
@@ -1832,10 +1751,7 @@ int skb_flow_apply_fiber_force_device(skb_flow *fl, const double *d_x_fibers, do
     CUDA_TRY(cudaSetDevice(fl->dev));
     fl->cur = (cudaStream_t)stream;
     SKB_TRY(fiber_force_dev(fl, d_x_fibers, d_fw));
-    fl->stats.device_ms = fl->stats.total_ms = 0;
-    fl->stats.n_pairs = 0;
-    fl->stats.launches = fl->launches;
-    return SKB_OK;
+    return device_stats(fl);
 }
 
 int skb_flow_fiber_matvec_device(skb_flow *fl, const double *d_x_fibers, const double *d_v_fibers,
@@ -1851,10 +1767,7 @@ int skb_flow_fiber_matvec_device(skb_flow *fl, const double *d_x_fibers, const d
     CUDA_TRY(cudaSetDevice(fl->dev));
     fl->cur = (cudaStream_t)stream;
     SKB_TRY(fiber_matvec_dev(fl, d_x_fibers, d_v_fibers, d_v_fib_boundary, d_res));
-    fl->stats.device_ms = fl->stats.total_ms = 0;
-    fl->stats.n_pairs = 0;
-    fl->stats.launches = fl->launches;
-    return SKB_OK;
+    return device_stats(fl);
 }
 
 } // extern "C"
@@ -1871,7 +1784,7 @@ static int apply_matvec_core(skb_flow *fl, skb_dense *dn, const double *d_x, con
     SKB_TRY(fl->vel.ensure((size_t)fl->n_win * 24 + 8));
     // res_shell's dense part, stresslet_plus_complementary_ * x_shell (system.cpp:319, periphery.cpp:38-47), depends on
     // x_shell only: it is handed to the background streamer, which matvec_core launches as soon as x_shell is complete
-    // on this device -- the caller's vector without a group, the gathered copy in the window with one
+    // on this device (full_x_shell)
     skb_flow::Overlap &B = fl->bg;
     B.dn = nullptr;
     B.launched = false;
@@ -1879,7 +1792,6 @@ static int apply_matvec_core(skb_flow *fl, skb_dense *dn, const double *d_x, con
     if (dense_rows && B.enabled) {
         SKB_TRY(overlap_buffers(fl, 3 * n_sw));
         B.dn = dn;
-        B.d_x = fl->grp.size > 1 ? fl->grp.at<double>(fl->grp.rank, fl->grp.off_xshell[(fl->grp.epoch + 1) & 1]) : d_xs;
     }
     // MatrixXd fw = fc.apply_fiber_force(x_fibers)                       system.cpp:298
     SKB_TRY(fiber_force_dev(fl, d_x, (double *)fl->in_fib.ptr));
@@ -1894,17 +1806,12 @@ static int apply_matvec_core(skb_flow *fl, skb_dense *dn, const double *d_x, con
             CUDA_TRY(cudaStreamWaitEvent(fl->cur, B.join, 0));
             add_out_kernel<<<(unsigned)((3 * n_sw + 255) / 256), 256, 0, fl->cur>>>(d_out_shell, (const double *)B.y.ptr,
                                                                                    d_v_shell, 3 * n_sw);
-            CUDA_TRY(cudaGetLastError());
-            count_launch(1);
-            fl->launches += 1;
+            SKB_TRY(launched(fl, 1));
         } else if (dn) {
             // res_shell = shell.matvec(x_shell, v_shell) = stresslet_plus_complementary_ * x_shell + v_shell in one
             // kernel at the end of the stream (skb_flow_set_overlap(fl, 0))
-            const double *d_x_full = d_xs;
-            if (fl->grp.size > 1)
-                d_x_full = fl->grp.at<double>(fl->grp.rank, fl->grp.off_xshell[fl->grp.epoch & 1]);
-            SKB_TRY(skb_dense_apply_device(dn, SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY, d_x_full, d_v_shell, d_out_shell,
-                                           fl->cur));
+            SKB_TRY(skb_dense_apply_device(dn, SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY, full_x_shell(fl, d_xs), d_v_shell,
+                                           d_out_shell, fl->cur));
             fl->launches += 1;
         } else {
             CUDA_TRY(cudaMemcpyAsync(d_out_shell, d_v_shell, (size_t)n_sw * 24, cudaMemcpyDeviceToDevice, fl->cur));
@@ -1957,34 +1864,32 @@ static int apply_matvec_impl(skb_flow *fl, skb_dense *dn, const double *x_fibers
     std::vector<double> f, t;
     if (fl->n_bodies > 0)
         split_forces_torques(body_forces_torques, fl->n_bodies, f, t);
-    fl->cur = fl->stream;
-    CUDA_TRY(cudaEventRecord(fl->evt0, fl->stream));
-    if (nf)
-        CUDA_TRY(cudaMemcpyAsync(fl->x_fib.ptr, x_fibers, (size_t)nf * 32, cudaMemcpyHostToDevice, fl->stream));
-    if (nf && fiber_link_conditions)
-        CUDA_TRY(cudaMemcpyAsync(fl->vb.ptr, fiber_link_conditions, (size_t)(fl->op_f1 - fl->op_f0) * 56,
-                                 cudaMemcpyHostToDevice, fl->stream));
-    SKB_TRY(upload(fl, fl->in_shell, shell_density, (size_t)ns * 3));
-    SKB_TRY(upload(fl, fl->in_body, body_densities, (size_t)nb * 3));
-    SKB_TRY(upload(fl, fl->in_force, f.data(), f.size()));
-    SKB_TRY(upload(fl, fl->in_torque, t.data(), t.size()));
-    SKB_TRY(fl->res_shell.ensure((size_t)ns * 24 + 8));
-    SKB_TRY(fl->tmp_b.ensure((size_t)nb * 24 + 8));
-    CUDA_TRY(cudaEventRecord(fl->ev0, fl->stream));
-    SKB_TRY(apply_matvec_core(fl, dn, (const double *)fl->x_fib.ptr, (const double *)fl->in_shell.ptr,
-                              (const double *)fl->in_body.ptr, (const double *)fl->in_force.ptr,
-                              (const double *)fl->in_torque.ptr,
-                              (nf && fiber_link_conditions) ? (const double *)fl->vb.ptr : nullptr, eta,
-                              (double *)fl->res_fib.ptr, (double *)fl->res_shell.ptr, (double *)fl->tmp_b.ptr));
-    CUDA_TRY(cudaEventRecord(fl->ev1, fl->stream));
-    if (nf)
-        CUDA_TRY(cudaMemcpyAsync(res_fibers, fl->res_fib.ptr, (size_t)nf * 32, cudaMemcpyDeviceToHost, fl->stream));
-    if (ns)
-        CUDA_TRY(cudaMemcpyAsync(v_shell, fl->res_shell.ptr, (size_t)ns * 24, cudaMemcpyDeviceToHost, fl->stream));
-    if (nb)
-        CUDA_TRY(cudaMemcpyAsync(v_bodies, fl->tmp_b.ptr, (size_t)nb * 24, cudaMemcpyDeviceToHost, fl->stream));
-    CUDA_TRY(cudaEventRecord(fl->evt1, fl->stream));
-    return finish_stats(fl);
+    const bool link = nf && fiber_link_conditions;
+    return host_frame(
+        fl,
+        [&]() -> int {
+            SKB_TRY(upload(fl, fl->x_fib, x_fibers, (size_t)nf * 4));
+            if (link)
+                SKB_TRY(upload(fl, fl->vb, fiber_link_conditions, (size_t)(fl->op_f1 - fl->op_f0) * 7));
+            SKB_TRY(upload(fl, fl->in_shell, shell_density, (size_t)ns * 3));
+            SKB_TRY(upload(fl, fl->in_body, body_densities, (size_t)nb * 3));
+            SKB_TRY(upload(fl, fl->in_force, f.data(), f.size()));
+            SKB_TRY(upload(fl, fl->in_torque, t.data(), t.size()));
+            SKB_TRY(fl->res_shell.ensure((size_t)ns * 24 + 8));
+            return fl->tmp_b.ensure((size_t)nb * 24 + 8);
+        },
+        [&] {
+            return apply_matvec_core(fl, dn, (const double *)fl->x_fib.ptr, (const double *)fl->in_shell.ptr,
+                                     (const double *)fl->in_body.ptr, (const double *)fl->in_force.ptr,
+                                     (const double *)fl->in_torque.ptr, link ? (const double *)fl->vb.ptr : nullptr,
+                                     eta, (double *)fl->res_fib.ptr, (double *)fl->res_shell.ptr,
+                                     (double *)fl->tmp_b.ptr);
+        },
+        [&]() -> int {
+            SKB_TRY(download(fl, res_fibers, fl->res_fib, (size_t)nf * 4));
+            SKB_TRY(download(fl, v_shell, fl->res_shell, (size_t)ns * 3));
+            return download(fl, v_bodies, fl->tmp_b, (size_t)nb * 3);
+        });
 }
 
 extern "C" {
@@ -2034,10 +1939,7 @@ int skb_flow_apply_matvec_device(skb_flow *fl, skb_dense *dn, const double *d_x_
     fl->cur = (cudaStream_t)stream;
     SKB_TRY(apply_matvec_core(fl, dn, d_x_fibers, d_x_shell, d_body_densities, d_body_forces, d_body_torques,
                               d_fiber_link_conditions, eta, d_res_fibers, d_out_shell, d_v_bodies));
-    fl->stats.device_ms = fl->stats.total_ms = 0;
-    fl->stats.n_pairs = fl->pairs;
-    fl->stats.launches = fl->launches;
-    return SKB_OK;
+    return device_stats(fl);
 }
 
 int skb_flow_last_sym_kernel(const skb_flow *fl, double *ms, int64_t *pairs) {
@@ -2055,596 +1957,7 @@ int skb_flow_last_stats(const skb_flow *fl, skb_flow_stats *out) {
 
 } // extern "C"
 
-// =====================================================================================================================
-// skb_mflow -- ONE process, n GPUs (include/skelly_b200_flow.h): the multi-device shape the reference's "direct
-// evaluators need a single rank" rule admits (src/core/system.cpp:618-623).  One group member (skb_flow) per device,
-// connected through peer memory; whole fibers, periphery rows and body rows are block-partitioned over the members.
-// Every member is driven by its own host thread, so the n launch sequences are issued concurrently.
-// =====================================================================================================================
-#include <condition_variable>
-#include <functional>
-#include <mutex>
-#include <string>
-#include <thread>
-
-namespace {
-class Workers {
-  public:
-    explicit Workers(int n) : n_(n), task_(n), state_(n, 0), rc_(n, 0), msg_(n) {
-        for (int g = 0; g < n; ++g)
-            th_.emplace_back([this, g] { loop(g); });
-    }
-    ~Workers() {
-        {
-            std::lock_guard<std::mutex> lk(mu_);
-            stop_ = true;
-        }
-        cv_.notify_all();
-        for (auto &t : th_)
-            t.join();
-    }
-    // run fn(g) on every worker; returns the first non-zero status (its message becomes this thread's last error)
-    int run(const std::function<int(int)> &fn) {
-        {
-            std::lock_guard<std::mutex> lk(mu_);
-            for (int g = 0; g < n_; ++g) {
-                task_[g] = fn;
-                state_[g] = 1;
-            }
-        }
-        cv_.notify_all();
-        std::unique_lock<std::mutex> lk(mu_);
-        done_.wait(lk, [this] {
-            for (int g = 0; g < n_; ++g)
-                if (state_[g] != 0)
-                    return false;
-            return true;
-        });
-        for (int g = 0; g < n_; ++g)
-            if (rc_[g] != SKB_OK)
-                return set_error(rc_[g], "device member %d: %s", g, msg_[g].c_str());
-        return SKB_OK;
-    }
-
-  private:
-    void loop(int g) {
-        for (;;) {
-            std::function<int(int)> fn;
-            {
-                std::unique_lock<std::mutex> lk(mu_);
-                cv_.wait(lk, [this, g] { return stop_ || state_[g] == 1; });
-                if (stop_)
-                    return;
-                fn = task_[g];
-            }
-            const int rc = fn(g);
-            {
-                std::lock_guard<std::mutex> lk(mu_);
-                rc_[g] = rc;
-                msg_[g] = rc == SKB_OK ? "" : last_error();
-                state_[g] = 0;
-            }
-            done_.notify_all();
-        }
-    }
-    int n_;
-    std::vector<std::function<int(int)>> task_;
-    std::vector<int> state_, rc_;
-    std::vector<std::string> msg_;
-    std::vector<std::thread> th_;
-    std::mutex mu_;
-    std::condition_variable cv_, done_;
-    bool stop_ = false;
-};
-} // namespace
-
-struct skb_mflow {
-    int n = 0;
-    std::vector<int> devs;
-    std::vector<skb_flow *> m;
-    std::vector<skb_dense *> dn;
-    std::unique_ptr<Workers> workers;
-    // geometry (host copies of what the partition needs)
-    long long n_fib = 0, n_shell = 0, n_body = 0;
-    int n_fibers = 0, n_bodies = 0;
-    std::vector<int> fiber_n;
-    std::vector<long long> fiber_off;
-    // partition: member g owns fibers [f0[g], f1[g]), periphery rows [s0, s1), body rows [b0, b1)
-    std::vector<int> f0, f1;
-    std::vector<long long> s0, s1, b0, b1;
-    bool part_dirty = true;
-    bool has_dense = false;
-    bool ops_ready = false;
-    struct IO { // per-member device buffers of the host-pointer calls
-        DevBuf x, xs, bd, f, t, link, res, outs, vb, ff, v;
-        cudaEvent_t e0 = nullptr, e1 = nullptr;
-    };
-    std::vector<IO> io;
-    skb_flow_stats stats{};
-};
-
-// member g of n owns whole fibers [f0, f1) -- cut where the running node count passes g/n of the total
-// (fcfd.cpp:102-120 splits by fiber count; by node count balances ragged suspensions as well) -- and equal blocks of
-// the periphery and body rows
-static void partition_rows(const std::vector<long long> &fiber_off, long long n_shell, long long n_body, int n,
-                           std::vector<int> &f0, std::vector<int> &f1, std::vector<long long> &s0,
-                           std::vector<long long> &s1, std::vector<long long> &b0, std::vector<long long> &b1) {
-    const int n_fibers = (int)fiber_off.size() - 1;
-    const long long n_fib = n_fibers > 0 ? fiber_off[(size_t)n_fibers] : 0;
-    f0.assign(n, 0), f1.assign(n, 0);
-    s0.assign(n, 0), s1.assign(n, 0), b0.assign(n, 0), b1.assign(n, 0);
-    int f = 0;
-    for (int g = 0; g < n; ++g) {
-        f0[g] = f;
-        const long long want = n_fib * (g + 1) / n;
-        while (f < n_fibers && fiber_off[(size_t)f + 1] <= want)
-            ++f;
-        if (g == n - 1)
-            f = std::max(n_fibers, 0);
-        f1[g] = f;
-    }
-    const long long cs = (n_shell + n - 1) / n, cb = (n_body + n - 1) / n;
-    for (int g = 0; g < n; ++g) {
-        s0[g] = std::min(n_shell, g * cs);
-        s1[g] = std::min(n_shell, (g + 1) * cs);
-        b0[g] = std::min(n_body, g * cb);
-        b1[g] = std::min(n_body, (g + 1) * cb);
-    }
+cudaStream_t skb::flow_stream(const skb_flow *fl) { return fl->stream; }
+int skb::flow_size_overlap(skb_flow *fl, long long n_rows) {
+    return fl->bg.enabled ? overlap_buffers(fl, n_rows) : SKB_OK;
 }
-
-static void mflow_partition(skb_mflow *mf) {
-    std::vector<long long> off = mf->fiber_off;
-    if (off.empty())
-        off.push_back(0);
-    partition_rows(off, mf->n_shell, mf->n_body, mf->n, mf->f0, mf->f1, mf->s0, mf->s1, mf->b0, mf->b1);
-}
-
-// ranges + group wiring, after any change of the geometry's sizes
-static int mflow_prepare(skb_mflow *mf) {
-    if (!mf->part_dirty)
-        return SKB_OK;
-    mflow_partition(mf);
-    for (int g = 0; g < mf->n; ++g) {
-        SKB_TRY(skb_flow_set_target_ranges(mf->m[g], mf->f0[g], mf->f1[g], mf->s0[g], mf->s1[g], mf->b0[g], mf->b1[g]));
-        SKB_TRY(skb_flow_group_init(mf->m[g], g, mf->n));
-    }
-    for (int g = 0; g < mf->n; ++g)
-        for (int h = 0; h < mf->n; ++h)
-            if (g != h)
-                SKB_TRY(skb_flow_group_connect(mf->m[g], h, mf->m[h]));
-    for (int g = 0; g < mf->n; ++g) // all allocations up front: members may share a device (see skb_flow_group_warmup)
-        SKB_TRY(skb_flow_group_warmup(mf->m[g]));
-    mf->part_dirty = false;
-    mf->ops_ready = false;
-    return SKB_OK;
-}
-
-extern "C" {
-
-int skb_mflow_create(const int *devices, int n, skb_mflow **out) {
-    if (!out || n < 1 || n > kMaxGroup)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_create: need 1 <= n <= %d devices", kMaxGroup);
-    *out = nullptr;
-    std::unique_ptr<skb_mflow> mf(new skb_mflow);
-    mf->n = n;
-    mf->m.assign(n, nullptr);
-    mf->dn.assign(n, nullptr);
-    mf->io.resize(n);
-    for (int g = 0; g < n; ++g) {
-        mf->devs.push_back(devices ? devices[g] : g);
-        int rc = skb_flow_create(mf->devs[g], &mf->m[g]);
-        if (rc == SKB_OK) {
-            cudaSetDevice(mf->devs[g]);
-            if (cudaEventCreate(&mf->io[g].e0) != cudaSuccess || cudaEventCreate(&mf->io[g].e1) != cudaSuccess)
-                rc = set_error(SKB_ERR_CUDA, "cudaEventCreate failed");
-        }
-        if (rc != SKB_OK) {
-            for (int h = 0; h <= g; ++h)
-                skb_flow_destroy(mf->m[h]);
-            return rc;
-        }
-    }
-    mf->workers.reset(new Workers(n));
-    *out = mf.release();
-    return SKB_OK;
-}
-
-int skb_mflow_destroy(skb_mflow *mf) {
-    if (!mf)
-        return SKB_OK;
-    mf->workers.reset();
-    for (int g = 0; g < mf->n; ++g) {
-        cudaSetDevice(mf->devs[g]);
-        cudaDeviceSynchronize();
-    }
-    for (int g = 0; g < mf->n; ++g) {
-        cudaSetDevice(mf->devs[g]);
-        skb_mflow::IO &io = mf->io[g];
-        DevBuf *bufs[] = {&io.x, &io.xs, &io.bd, &io.f, &io.t, &io.link, &io.res, &io.outs, &io.vb, &io.ff, &io.v};
-        for (DevBuf *b : bufs)
-            b->release();
-        if (io.e0) cudaEventDestroy(io.e0);
-        if (io.e1) cudaEventDestroy(io.e1);
-        skb_dense_destroy(mf->dn[g]);
-        skb_flow_destroy(mf->m[g]);
-    }
-    delete mf;
-    return SKB_OK;
-}
-
-int skb_mflow_n_devices(const skb_mflow *mf, int *n) {
-    if (!mf || !n)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_n_devices: NULL");
-    *n = mf->n;
-    return SKB_OK;
-}
-
-int skb_mflow_set_fibers(skb_mflow *mf, const double *r_fib, const int *n_nodes, const double *length, int n_fibers) {
-    if (!mf || n_fibers < 0)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_set_fibers: bad arguments");
-    std::vector<long long> off((size_t)n_fibers + 1, 0);
-    for (int f = 0; f < n_fibers; ++f)
-        off[(size_t)f + 1] = off[(size_t)f] + (n_nodes ? n_nodes[f] : 0);
-    const bool resized = off != mf->fiber_off;
-    SKB_TRY(mf->workers->run([&](int g) -> int { return skb_flow_set_fibers(mf->m[g], r_fib, n_nodes, length, n_fibers); }));
-    mf->n_fibers = n_fibers;
-    mf->n_fib = off[(size_t)n_fibers];
-    mf->fiber_off = off;
-    mf->fiber_n.assign(n_nodes, n_nodes + n_fibers);
-    mf->ops_ready = false;
-    if (resized)
-        mf->part_dirty = true;
-    return SKB_OK;
-}
-
-int skb_mflow_set_periphery(skb_mflow *mf, const double *node_pos, const double *node_normal, int64_t n_nodes) {
-    if (!mf || n_nodes < 0)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_set_periphery: bad arguments");
-    SKB_TRY(mf->workers->run([&](int g) -> int { return skb_flow_set_periphery(mf->m[g], node_pos, node_normal, n_nodes); }));
-    if (mf->n_shell != n_nodes)
-        mf->part_dirty = true;
-    mf->n_shell = n_nodes;
-    return SKB_OK;
-}
-
-int skb_mflow_set_bodies(skb_mflow *mf, const double *node_pos, const double *node_normal, int64_t n_nodes,
-                         const double *centers, int n_bodies) {
-    if (!mf || n_nodes < 0 || n_bodies < 0)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_set_bodies: bad arguments");
-    SKB_TRY(mf->workers->run(
-        [&](int g) { return skb_flow_set_bodies(mf->m[g], node_pos, node_normal, n_nodes, centers, n_bodies); }));
-    if (mf->n_body != n_nodes)
-        mf->part_dirty = true;
-    mf->n_body = n_nodes;
-    mf->n_bodies = n_bodies;
-    return SKB_OK;
-}
-
-int skb_mflow_set_cross(skb_mflow *mf, int mode) {
-    if (!mf)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_set_cross: NULL");
-    for (int g = 0; g < mf->n; ++g)
-        SKB_TRY(skb_flow_set_cross(mf->m[g], mode));
-    mf->part_dirty = true; // the members' target lists change: re-run the warm-up
-    return SKB_OK;
-}
-
-int skb_mflow_set_overlap(skb_mflow *mf, int on) {
-    if (!mf)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_set_overlap: NULL");
-    for (int g = 0; g < mf->n; ++g)
-        SKB_TRY(skb_flow_set_overlap(mf->m[g], on));
-    return SKB_OK;
-}
-
-int skb_mflow_set_self_exclusion(skb_mflow *mf, int fused) {
-    if (!mf)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_set_self_exclusion: NULL");
-    for (int g = 0; g < mf->n; ++g)
-        SKB_TRY(skb_flow_set_self_exclusion(mf->m[g], fused));
-    return SKB_OK;
-}
-
-int skb_mflow_partition(skb_mflow *mf, int member, int *fiber_begin, int *fiber_end, int64_t *shell_begin,
-                        int64_t *shell_end, int64_t *body_begin, int64_t *body_end) {
-    if (!mf || member < 0 || member >= mf->n)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_partition: bad member");
-    SKB_TRY(mflow_prepare(mf));
-    if (fiber_begin) *fiber_begin = mf->f0[member];
-    if (fiber_end) *fiber_end = mf->f1[member];
-    if (shell_begin) *shell_begin = mf->s0[member];
-    if (shell_end) *shell_end = mf->s1[member];
-    if (body_begin) *body_begin = mf->b0[member];
-    if (body_end) *body_end = mf->b1[member];
-    return SKB_OK;
-}
-
-// host-only (no GPU needed): the partition skb_mflow uses, for rank-per-GPU hosts that want the same one
-int skb_partition_query(const int *n_nodes, int n_fibers, int64_t n_shell, int64_t n_body, int n_members, int member,
-                        int64_t *out6) {
-    if (n_fibers < 0 || (n_fibers > 0 && !n_nodes) || n_shell < 0 || n_body < 0 || n_members < 1 || member < 0 ||
-        member >= n_members || !out6)
-        return set_error(SKB_ERR_INVALID, "skb_partition_query: bad arguments");
-    std::vector<long long> off((size_t)n_fibers + 1, 0);
-    for (int f = 0; f < n_fibers; ++f)
-        off[(size_t)f + 1] = off[(size_t)f] + n_nodes[f];
-    std::vector<int> f0, f1;
-    std::vector<long long> s0, s1, b0, b1;
-    partition_rows(off, n_shell, n_body, n_members, f0, f1, s0, s1, b0, b1);
-    out6[0] = f0[member], out6[1] = f1[member], out6[2] = s0[member], out6[3] = s1[member], out6[4] = b0[member],
-    out6[5] = b1[member];
-    return SKB_OK;
-}
-
-int skb_mflow_set_fiber_class(skb_mflow *mf, int n_nodes, const double *D_1_0, const double *P_downsample_bc) {
-    if (!mf)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_set_fiber_class: NULL");
-    for (int g = 0; g < mf->n; ++g)
-        SKB_TRY(skb_flow_set_fiber_class(mf->m[g], n_nodes, D_1_0, P_downsample_bc));
-    mf->ops_ready = false;
-    return SKB_OK;
-}
-
-// element offset of fiber f's block in a concatenation of per-fiber (k n) x (4 n) matrices
-static long long op_offset(const skb_mflow *mf, int f, int k) {
-    long long o = 0;
-    for (int i = 0; i < f; ++i)
-        o += (long long)k * 4 * mf->fiber_n[(size_t)i] * mf->fiber_n[(size_t)i];
-    return o;
-}
-
-int skb_mflow_set_fiber_operators(skb_mflow *mf, const double *A, const double *force_operator, const double *xs,
-                                  const double *length_prev, const int *plus_bc_velocity) {
-    if (!mf)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_set_fiber_operators: NULL");
-    SKB_TRY(mflow_prepare(mf));
-    if (mf->n_fibers > 0 && (!A || !force_operator || !xs || !length_prev || !plus_bc_velocity))
-        return set_error(SKB_ERR_INVALID, "skb_mflow_set_fiber_operators: NULL argument");
-    SKB_TRY(mf->workers->run([&](int g) -> int {
-        const int f0 = mf->f0[g];
-        if (mf->f1[g] == f0)
-            return skb_flow_set_fiber_operators(mf->m[g], nullptr, nullptr, nullptr, nullptr, nullptr);
-        return skb_flow_set_fiber_operators(mf->m[g], A + op_offset(mf, f0, 4), force_operator + op_offset(mf, f0, 3),
-                                            xs + 3 * mf->fiber_off[(size_t)f0], length_prev + f0, plus_bc_velocity + f0);
-    }));
-    mf->ops_ready = true;
-    return SKB_OK;
-}
-
-int skb_mflow_set_fiber_preconditioner(skb_mflow *mf, const double *A_inv) {
-    if (!mf || !mf->ops_ready)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_set_fiber_preconditioner: call skb_mflow_set_fiber_operators first");
-    return mf->workers->run([&](int g) -> int {
-        const int f0 = mf->f0[g];
-        return skb_flow_set_fiber_preconditioner(mf->m[g], mf->f1[g] == f0 ? nullptr : A_inv + op_offset(mf, f0, 4));
-    });
-}
-
-// the periphery's dense operator, rows block-partitioned like the periphery rows (periphery.cpp:387-417)
-int skb_mflow_set_dense(skb_mflow *mf, int op, const double *A_rowmajor, int64_t n_rows, int64_t n_cols) {
-    if (!mf || !A_rowmajor || n_rows != 3 * mf->n_shell || n_cols != 3 * mf->n_shell)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_set_dense: need the (3 N_s) x (3 N_s) operator of the %lld periphery "
-                                          "nodes set before", mf ? mf->n_shell : 0LL);
-    SKB_TRY(mflow_prepare(mf));
-    SKB_TRY(mf->workers->run([&](int g) -> int {
-        if (!mf->dn[g])
-            SKB_TRY(skb_dense_create_on(&mf->devs[g], 1, &mf->dn[g]));
-        return skb_dense_set_matrix(mf->dn[g], op, A_rowmajor + (size_t)(3 * mf->s0[g]) * (size_t)n_cols,
-                                    3 * (mf->s1[g] - mf->s0[g]), n_cols);
-    }));
-    if (op == SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY)
-        mf->has_dense = true;
-    return SKB_OK;
-}
-
-static int mflow_collect_stats(skb_mflow *mf) {
-    double dev_ms = 0;
-    long long pairs = 0;
-    int launches = 0;
-    for (int g = 0; g < mf->n; ++g) {
-        float ms = 0;
-        cudaSetDevice(mf->devs[g]);
-        if (cudaEventElapsedTime(&ms, mf->io[g].e0, mf->io[g].e1) == cudaSuccess)
-            dev_ms = std::max(dev_ms, (double)ms);
-        else
-            (void)cudaGetLastError();
-        skb_flow_stats st{};
-        skb_flow_last_stats(mf->m[g], &st);
-        pairs += st.n_pairs;
-        launches += st.launches;
-        int missing = -1;
-        SKB_TRY(skb_flow_group_error(mf->m[g], &missing));
-        if (missing >= 0)
-            return set_error(SKB_ERR_STATE, "device member %d timed out waiting for member %d (a peer failed or never "
-                                            "issued the matching call)", g, missing);
-    }
-    mf->stats.device_ms = dev_ms;
-    mf->stats.total_ms = dev_ms;
-    mf->stats.n_pairs = pairs;
-    mf->stats.launches = launches;
-    return SKB_OK;
-}
-
-// Size every member's transfer buffers on the CALLING thread, before any member starts launching: cudaMalloc /
-// cudaFree may synchronise the whole device and must not run while a peer on the same device sits in a flag wait.
-static int mflow_size_io(skb_mflow *mf, size_t n_ft) {
-    for (int g = 0; g < mf->n; ++g) {
-        CUDA_TRY(cudaSetDevice(mf->devs[g]));
-        skb_mflow::IO &io = mf->io[g];
-        const long long a = mf->fiber_off.empty() ? 0 : mf->fiber_off[(size_t)mf->f0[g]],
-                        b = mf->fiber_off.empty() ? 0 : mf->fiber_off[(size_t)mf->f1[g]];
-        const size_t n_fw = (size_t)(b - a), n_sw = (size_t)(mf->s1[g] - mf->s0[g]), n_bw = (size_t)(mf->b1[g] - mf->b0[g]);
-        const size_t n_fibers = (size_t)(mf->f1[g] - mf->f0[g]);
-        SKB_TRY(io.x.ensure(n_fw * 32 + 8));
-        SKB_TRY(io.ff.ensure(n_fw * 24 + 8));
-        SKB_TRY(io.xs.ensure(n_sw * 24 + 8));
-        SKB_TRY(io.bd.ensure((size_t)mf->n_body * 24 + 8));
-        SKB_TRY(io.f.ensure(n_ft * 8 + 8));
-        SKB_TRY(io.t.ensure(n_ft * 8 + 8));
-        SKB_TRY(io.link.ensure(n_fibers * 56 + 8));
-        SKB_TRY(io.res.ensure(n_fw * 32 + 8));
-        SKB_TRY(io.outs.ensure(n_sw * 24 + 8));
-        SKB_TRY(io.vb.ensure(n_bw * 24 + 8));
-        SKB_TRY(io.v.ensure((n_fw + n_sw + n_bw) * 24 + 8));
-        if (mf->has_dense && n_sw > 0 && mf->m[g]->bg.enabled)
-            SKB_TRY(overlap_buffers(mf->m[g], 3 * (long long)n_sw));
-    }
-    return SKB_OK;
-}
-
-// v_all over [fibers | periphery | bodies] like skb_flow_matvec; complete host arrays in and out
-int skb_mflow_matvec(skb_mflow *mf, const double *fib_forces, const double *shell_density, const double *body_densities,
-                     const double *body_forces_torques, double eta, double *v_all) {
-    if (!mf || !(eta > 0))
-        return set_error(SKB_ERR_INVALID, "skb_mflow_matvec: bad arguments");
-    const long long nf = mf->n_fib, ns = mf->n_shell, nb = mf->n_body;
-    if ((nf > 0 && !fib_forces) || (ns > 0 && !shell_density) || (nb > 0 && !body_densities) ||
-        (mf->n_bodies > 0 && !body_forces_torques) || (nf + ns + nb > 0 && !v_all))
-        return set_error(SKB_ERR_INVALID, "skb_mflow_matvec: NULL input for a non-empty class");
-    SKB_TRY(mflow_prepare(mf));
-    std::vector<double> f, t;
-    if (mf->n_bodies > 0)
-        split_forces_torques(body_forces_torques, mf->n_bodies, f, t);
-    SKB_TRY(mflow_size_io(mf, f.size()));
-    SKB_TRY(mf->workers->run([&](int g) -> int {
-        skb_flow *fl = mf->m[g];
-        skb_mflow::IO &io = mf->io[g];
-        CUDA_TRY(cudaSetDevice(mf->devs[g]));
-        const long long a = mf->fiber_off.empty() ? 0 : mf->fiber_off[(size_t)mf->f0[g]],
-                        b = mf->fiber_off.empty() ? 0 : mf->fiber_off[(size_t)mf->f1[g]];
-        const long long n_fw = b - a, n_sw = mf->s1[g] - mf->s0[g], n_bw = mf->b1[g] - mf->b0[g];
-        cudaStream_t st = fl->stream;
-        auto put = [&](DevBuf &buf, const double *h, size_t n_dbl) -> int {
-            SKB_TRY(buf.ensure(n_dbl * 8 + 8));
-            if (n_dbl)
-                CUDA_TRY(cudaMemcpyAsync(buf.ptr, h, n_dbl * 8, cudaMemcpyHostToDevice, st));
-            return SKB_OK;
-        };
-        SKB_TRY(put(io.ff, fib_forces ? fib_forces + 3 * a : nullptr, (size_t)n_fw * 3));
-        SKB_TRY(put(io.xs, shell_density ? shell_density + 3 * mf->s0[g] : nullptr, (size_t)n_sw * 3));
-        SKB_TRY(put(io.bd, body_densities, (size_t)nb * 3));
-        SKB_TRY(put(io.f, f.data(), f.size()));
-        SKB_TRY(put(io.t, t.data(), t.size()));
-        SKB_TRY(io.v.ensure((size_t)(n_fw + n_sw + n_bw) * 24 + 8));
-        CUDA_TRY(cudaEventRecord(io.e0, st));
-        SKB_TRY(skb_flow_matvec_device(fl, (const double *)io.ff.ptr, (const double *)io.xs.ptr,
-                                       (const double *)io.bd.ptr, (const double *)io.f.ptr, (const double *)io.t.ptr, eta,
-                                       (double *)io.v.ptr, st));
-        CUDA_TRY(cudaEventRecord(io.e1, st));
-        double *d_v = (double *)io.v.ptr;
-        if (n_fw)
-            CUDA_TRY(cudaMemcpyAsync(v_all + 3 * a, d_v, (size_t)n_fw * 24, cudaMemcpyDeviceToHost, st));
-        if (n_sw)
-            CUDA_TRY(cudaMemcpyAsync(v_all + 3 * (nf + mf->s0[g]), d_v + 3 * n_fw, (size_t)n_sw * 24,
-                                     cudaMemcpyDeviceToHost, st));
-        if (n_bw)
-            CUDA_TRY(cudaMemcpyAsync(v_all + 3 * (nf + ns + mf->b0[g]), d_v + 3 * (n_fw + n_sw), (size_t)n_bw * 24,
-                                     cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-        return SKB_OK;
-    }));
-    return mflow_collect_stats(mf);
-}
-
-// System::apply_matvec (system.cpp:269-324) over n devices: complete host arrays in and out.  out_shell = res_shell
-// when skb_mflow_set_dense(SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY) was called, else v_shell.
-int skb_mflow_apply_matvec(skb_mflow *mf, const double *x_fibers, const double *x_shell, const double *body_densities,
-                           const double *body_forces_torques, const double *fiber_link_conditions, double eta,
-                           double *res_fibers, double *out_shell, double *v_bodies) {
-    if (!mf || !(eta > 0))
-        return set_error(SKB_ERR_INVALID, "skb_mflow_apply_matvec: bad arguments");
-    if (!mf->ops_ready)
-        return set_error(SKB_ERR_STATE, "skb_mflow_apply_matvec: call skb_mflow_set_fiber_operators first");
-    const long long nf = mf->n_fib, ns = mf->n_shell, nb = mf->n_body;
-    if ((nf > 0 && (!x_fibers || !res_fibers)) || (ns > 0 && (!x_shell || !out_shell)) ||
-        (nb > 0 && (!body_densities || !v_bodies)) || (mf->n_bodies > 0 && !body_forces_torques))
-        return set_error(SKB_ERR_INVALID, "skb_mflow_apply_matvec: NULL argument for a non-empty class");
-    SKB_TRY(mflow_prepare(mf));
-    std::vector<double> f, t;
-    if (mf->n_bodies > 0)
-        split_forces_torques(body_forces_torques, mf->n_bodies, f, t);
-    SKB_TRY(mflow_size_io(mf, f.size()));
-    SKB_TRY(mf->workers->run([&](int g) -> int {
-        skb_flow *fl = mf->m[g];
-        skb_mflow::IO &io = mf->io[g];
-        CUDA_TRY(cudaSetDevice(mf->devs[g]));
-        const int f0 = mf->f0[g], f1 = mf->f1[g];
-        const long long a = mf->fiber_off.empty() ? 0 : mf->fiber_off[(size_t)f0],
-                        b = mf->fiber_off.empty() ? 0 : mf->fiber_off[(size_t)f1];
-        const long long n_fw = b - a, n_sw = mf->s1[g] - mf->s0[g], n_bw = mf->b1[g] - mf->b0[g];
-        cudaStream_t st = fl->stream;
-        auto put = [&](DevBuf &buf, const double *h, size_t n_dbl) -> int {
-            SKB_TRY(buf.ensure(n_dbl * 8 + 8));
-            if (n_dbl && h)
-                CUDA_TRY(cudaMemcpyAsync(buf.ptr, h, n_dbl * 8, cudaMemcpyHostToDevice, st));
-            return SKB_OK;
-        };
-        SKB_TRY(put(io.x, x_fibers ? x_fibers + 4 * a : nullptr, (size_t)n_fw * 4));
-        SKB_TRY(put(io.xs, x_shell ? x_shell + 3 * mf->s0[g] : nullptr, (size_t)n_sw * 3));
-        SKB_TRY(put(io.bd, body_densities, (size_t)nb * 3));
-        SKB_TRY(put(io.f, f.data(), f.size()));
-        SKB_TRY(put(io.t, t.data(), t.size()));
-        SKB_TRY(put(io.link, fiber_link_conditions ? fiber_link_conditions + 7 * (long long)f0 : nullptr,
-                    (size_t)(f1 - f0) * 7));
-        SKB_TRY(io.res.ensure((size_t)n_fw * 32 + 8));
-        SKB_TRY(io.outs.ensure((size_t)n_sw * 24 + 8));
-        SKB_TRY(io.vb.ensure((size_t)n_bw * 24 + 8));
-        CUDA_TRY(cudaEventRecord(io.e0, st));
-        SKB_TRY(skb_flow_apply_matvec_device(
-            fl, mf->has_dense ? mf->dn[g] : nullptr, (const double *)io.x.ptr, (const double *)io.xs.ptr,
-            (const double *)io.bd.ptr, (const double *)io.f.ptr, (const double *)io.t.ptr,
-            (fiber_link_conditions && f1 > f0) ? (const double *)io.link.ptr : nullptr, eta, (double *)io.res.ptr,
-            (double *)io.outs.ptr, (double *)io.vb.ptr, st));
-        CUDA_TRY(cudaEventRecord(io.e1, st));
-        if (n_fw)
-            CUDA_TRY(cudaMemcpyAsync(res_fibers + 4 * a, io.res.ptr, (size_t)n_fw * 32, cudaMemcpyDeviceToHost, st));
-        if (n_sw)
-            CUDA_TRY(cudaMemcpyAsync(out_shell + 3 * mf->s0[g], io.outs.ptr, (size_t)n_sw * 24, cudaMemcpyDeviceToHost,
-                                     st));
-        if (n_bw)
-            CUDA_TRY(cudaMemcpyAsync(v_bodies + 3 * mf->b0[g], io.vb.ptr, (size_t)n_bw * 24, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-        return SKB_OK;
-    }));
-    return mflow_collect_stats(mf);
-}
-
-// System::velocity_at_targets (system.cpp:330-384) over n devices: the targets are block-partitioned, every device
-// holds all sources
-int skb_mflow_velocity_at_targets(skb_mflow *mf, const double *r_trg, int64_t n_trg, const double *fib_forces,
-                                  const double *shell_density, const double *body_densities,
-                                  const double *body_forces_torques, double eta, double *vel) {
-    if (!mf || n_trg < 0 || (n_trg > 0 && (!r_trg || !vel)) || !(eta > 0))
-        return set_error(SKB_ERR_INVALID, "skb_mflow_velocity_at_targets: bad arguments");
-    const long long chunk = (n_trg + mf->n - 1) / mf->n;
-    SKB_TRY(mf->workers->run([&](int g) -> int {
-        const long long b = std::min<long long>(n_trg, g * chunk), e = std::min<long long>(n_trg, (g + 1) * chunk);
-        if (e <= b)
-            return (int)SKB_OK;
-        return skb_flow_velocity_at_targets(mf->m[g], r_trg + 3 * b, e - b, fib_forces, shell_density, body_densities,
-                                            body_forces_torques, eta, vel + 3 * b);
-    }));
-    double dev_ms = 0;
-    long long pairs = 0;
-    int launches = 0;
-    for (int g = 0; g < mf->n; ++g) {
-        skb_flow_stats st{};
-        skb_flow_last_stats(mf->m[g], &st);
-        dev_ms = std::max(dev_ms, st.device_ms);
-        pairs += st.n_pairs;
-        launches += st.launches;
-    }
-    mf->stats.device_ms = mf->stats.total_ms = dev_ms;
-    mf->stats.n_pairs = pairs;
-    mf->stats.launches = launches;
-    return SKB_OK;
-}
-
-int skb_mflow_last_stats(const skb_mflow *mf, skb_flow_stats *out) {
-    if (!mf || !out)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_last_stats: NULL");
-    *out = mf->stats;
-    return SKB_OK;
-}
-
-} // extern "C"

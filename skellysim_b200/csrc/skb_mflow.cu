@@ -1,0 +1,618 @@
+// skb_mflow.cu -- ONE process, n GPUs (include/skelly_b200_flow.h): the multi-device shape the reference's "direct
+// evaluators need a single rank" rule admits (src/core/system.cpp:618-623).  One group member (skb_flow) per device,
+// connected through peer memory; whole fibers, periphery rows and body rows are block-partitioned over the members.
+// Every member is driven by its own host thread, so the n launch sequences are issued concurrently.  A client of the
+// skb_flow_* API plus the few internals declared in skb_internal.hpp.
+#include "skb_internal.hpp"
+#include "../../include/skelly_b200_flow.h"
+#include "../../include/skelly_b200_dense.h"
+
+#include <algorithm>
+#include <condition_variable>
+#include <functional>
+#include <memory>
+#include <mutex>
+#include <string>
+#include <thread>
+#include <vector>
+
+using namespace skb;
+
+#define CUDA_TRY(expr)                                                                                                \
+    do {                                                                                                              \
+        cudaError_t _e = (expr);                                                                                      \
+        if (_e != cudaSuccess)                                                                                        \
+            return set_error(SKB_ERR_CUDA, "%s failed at %s:%d: %s", #expr, __FILE__, __LINE__,                      \
+                             cudaGetErrorString(_e));                                                                 \
+    } while (0)
+#define SKB_TRY(expr)                                                                                                 \
+    do {                                                                                                              \
+        int _rc = (expr);                                                                                             \
+        if (_rc != SKB_OK)                                                                                            \
+            return _rc;                                                                                               \
+    } while (0)
+
+namespace {
+class Workers {
+  public:
+    explicit Workers(int n) : n_(n), task_(n), state_(n, 0), rc_(n, 0), msg_(n) {
+        for (int g = 0; g < n; ++g)
+            th_.emplace_back([this, g] { loop(g); });
+    }
+    ~Workers() {
+        {
+            std::lock_guard<std::mutex> lk(mu_);
+            stop_ = true;
+        }
+        cv_.notify_all();
+        for (auto &t : th_)
+            t.join();
+    }
+    // run fn(g) on every worker; returns the first non-zero status (its message becomes this thread's last error)
+    int run(const std::function<int(int)> &fn) {
+        {
+            std::lock_guard<std::mutex> lk(mu_);
+            for (int g = 0; g < n_; ++g) {
+                task_[g] = fn;
+                state_[g] = 1;
+            }
+        }
+        cv_.notify_all();
+        std::unique_lock<std::mutex> lk(mu_);
+        done_.wait(lk, [this] {
+            for (int g = 0; g < n_; ++g)
+                if (state_[g] != 0)
+                    return false;
+            return true;
+        });
+        for (int g = 0; g < n_; ++g)
+            if (rc_[g] != SKB_OK)
+                return set_error(rc_[g], "device member %d: %s", g, msg_[g].c_str());
+        return SKB_OK;
+    }
+
+  private:
+    void loop(int g) {
+        for (;;) {
+            std::function<int(int)> fn;
+            {
+                std::unique_lock<std::mutex> lk(mu_);
+                cv_.wait(lk, [this, g] { return stop_ || state_[g] == 1; });
+                if (stop_)
+                    return;
+                fn = task_[g];
+            }
+            const int rc = fn(g);
+            {
+                std::lock_guard<std::mutex> lk(mu_);
+                rc_[g] = rc;
+                msg_[g] = rc == SKB_OK ? "" : last_error();
+                state_[g] = 0;
+            }
+            done_.notify_all();
+        }
+    }
+    int n_;
+    std::vector<std::function<int(int)>> task_;
+    std::vector<int> state_, rc_;
+    std::vector<std::string> msg_;
+    std::vector<std::thread> th_;
+    std::mutex mu_;
+    std::condition_variable cv_, done_;
+    bool stop_ = false;
+};
+} // namespace
+
+struct skb_mflow {
+    int n = 0;
+    std::vector<int> devs;
+    std::vector<skb_flow *> m;
+    std::vector<skb_dense *> dn;
+    std::unique_ptr<Workers> workers;
+    // geometry (host copies of what the partition needs)
+    long long n_fib = 0, n_shell = 0, n_body = 0;
+    int n_fibers = 0, n_bodies = 0;
+    std::vector<int> fiber_n;
+    std::vector<long long> fiber_off;
+    // partition: member g owns fibers [f0[g], f1[g]), periphery rows [s0, s1), body rows [b0, b1)
+    std::vector<int> f0, f1;
+    std::vector<long long> s0, s1, b0, b1;
+    bool part_dirty = true;
+    bool has_dense = false;
+    bool ops_ready = false;
+    struct IO { // per-member device buffers of the host-pointer calls
+        DevBuf x, xs, bd, f, t, link, res, outs, vb, ff, v;
+        cudaEvent_t e0 = nullptr, e1 = nullptr;
+    };
+    std::vector<IO> io;
+    skb_flow_stats stats{};
+};
+
+// member g of n owns whole fibers [f0, f1) -- cut where the running node count passes g/n of the total
+// (fcfd.cpp:102-120 splits by fiber count; by node count balances ragged suspensions as well) -- and equal blocks of
+// the periphery and body rows
+static void partition_rows(const std::vector<long long> &fiber_off, long long n_shell, long long n_body, int n,
+                           std::vector<int> &f0, std::vector<int> &f1, std::vector<long long> &s0,
+                           std::vector<long long> &s1, std::vector<long long> &b0, std::vector<long long> &b1) {
+    const int n_fibers = (int)fiber_off.size() - 1;
+    const long long n_fib = n_fibers > 0 ? fiber_off[(size_t)n_fibers] : 0;
+    f0.assign(n, 0), f1.assign(n, 0);
+    s0.assign(n, 0), s1.assign(n, 0), b0.assign(n, 0), b1.assign(n, 0);
+    int f = 0;
+    for (int g = 0; g < n; ++g) {
+        f0[g] = f;
+        const long long want = n_fib * (g + 1) / n;
+        while (f < n_fibers && fiber_off[(size_t)f + 1] <= want)
+            ++f;
+        if (g == n - 1)
+            f = std::max(n_fibers, 0);
+        f1[g] = f;
+    }
+    const long long cs = (n_shell + n - 1) / n, cb = (n_body + n - 1) / n;
+    for (int g = 0; g < n; ++g) {
+        s0[g] = std::min(n_shell, g * cs);
+        s1[g] = std::min(n_shell, (g + 1) * cs);
+        b0[g] = std::min(n_body, g * cb);
+        b1[g] = std::min(n_body, (g + 1) * cb);
+    }
+}
+
+static void mflow_partition(skb_mflow *mf) {
+    std::vector<long long> off = mf->fiber_off;
+    if (off.empty())
+        off.push_back(0);
+    partition_rows(off, mf->n_shell, mf->n_body, mf->n, mf->f0, mf->f1, mf->s0, mf->s1, mf->b0, mf->b1);
+}
+
+// ranges + group wiring, after any change of the geometry's sizes
+static int mflow_prepare(skb_mflow *mf) {
+    if (!mf->part_dirty)
+        return SKB_OK;
+    mflow_partition(mf);
+    for (int g = 0; g < mf->n; ++g) {
+        SKB_TRY(skb_flow_set_target_ranges(mf->m[g], mf->f0[g], mf->f1[g], mf->s0[g], mf->s1[g], mf->b0[g], mf->b1[g]));
+        SKB_TRY(skb_flow_group_init(mf->m[g], g, mf->n));
+    }
+    for (int g = 0; g < mf->n; ++g)
+        for (int h = 0; h < mf->n; ++h)
+            if (g != h)
+                SKB_TRY(skb_flow_group_connect(mf->m[g], h, mf->m[h]));
+    for (int g = 0; g < mf->n; ++g) // all allocations up front: members may share a device (see skb_flow_group_warmup)
+        SKB_TRY(skb_flow_group_warmup(mf->m[g]));
+    mf->part_dirty = false;
+    mf->ops_ready = false;
+    return SKB_OK;
+}
+
+extern "C" {
+
+int skb_mflow_create(const int *devices, int n, skb_mflow **out) {
+    if (!out || n < 1 || n > kMaxGroup)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_create: need 1 <= n <= %d devices", kMaxGroup);
+    *out = nullptr;
+    std::unique_ptr<skb_mflow> mf(new skb_mflow);
+    mf->n = n;
+    mf->m.assign(n, nullptr);
+    mf->dn.assign(n, nullptr);
+    mf->io.resize(n);
+    for (int g = 0; g < n; ++g) {
+        mf->devs.push_back(devices ? devices[g] : g);
+        int rc = skb_flow_create(mf->devs[g], &mf->m[g]);
+        if (rc == SKB_OK) {
+            cudaSetDevice(mf->devs[g]);
+            if (cudaEventCreate(&mf->io[g].e0) != cudaSuccess || cudaEventCreate(&mf->io[g].e1) != cudaSuccess)
+                rc = set_error(SKB_ERR_CUDA, "cudaEventCreate failed");
+        }
+        if (rc != SKB_OK) {
+            for (int h = 0; h <= g; ++h)
+                skb_flow_destroy(mf->m[h]);
+            return rc;
+        }
+    }
+    mf->workers.reset(new Workers(n));
+    *out = mf.release();
+    return SKB_OK;
+}
+
+int skb_mflow_destroy(skb_mflow *mf) {
+    if (!mf)
+        return SKB_OK;
+    mf->workers.reset();
+    for (int g = 0; g < mf->n; ++g) {
+        cudaSetDevice(mf->devs[g]);
+        cudaDeviceSynchronize();
+    }
+    for (int g = 0; g < mf->n; ++g) {
+        cudaSetDevice(mf->devs[g]);
+        skb_mflow::IO &io = mf->io[g];
+        DevBuf *bufs[] = {&io.x, &io.xs, &io.bd, &io.f, &io.t, &io.link, &io.res, &io.outs, &io.vb, &io.ff, &io.v};
+        for (DevBuf *b : bufs)
+            b->release();
+        if (io.e0) cudaEventDestroy(io.e0);
+        if (io.e1) cudaEventDestroy(io.e1);
+        skb_dense_destroy(mf->dn[g]);
+        skb_flow_destroy(mf->m[g]);
+    }
+    delete mf;
+    return SKB_OK;
+}
+
+int skb_mflow_n_devices(const skb_mflow *mf, int *n) {
+    if (!mf || !n)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_n_devices: NULL");
+    *n = mf->n;
+    return SKB_OK;
+}
+
+int skb_mflow_set_fibers(skb_mflow *mf, const double *r_fib, const int *n_nodes, const double *length, int n_fibers) {
+    if (!mf || n_fibers < 0)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_set_fibers: bad arguments");
+    std::vector<long long> off((size_t)n_fibers + 1, 0);
+    for (int f = 0; f < n_fibers; ++f)
+        off[(size_t)f + 1] = off[(size_t)f] + (n_nodes ? n_nodes[f] : 0);
+    const bool resized = off != mf->fiber_off;
+    SKB_TRY(mf->workers->run([&](int g) -> int { return skb_flow_set_fibers(mf->m[g], r_fib, n_nodes, length, n_fibers); }));
+    mf->n_fibers = n_fibers;
+    mf->n_fib = off[(size_t)n_fibers];
+    mf->fiber_off = off;
+    mf->fiber_n.assign(n_nodes, n_nodes + n_fibers);
+    mf->ops_ready = false;
+    if (resized)
+        mf->part_dirty = true;
+    return SKB_OK;
+}
+
+int skb_mflow_set_periphery(skb_mflow *mf, const double *node_pos, const double *node_normal, int64_t n_nodes) {
+    if (!mf || n_nodes < 0)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_set_periphery: bad arguments");
+    SKB_TRY(mf->workers->run([&](int g) -> int { return skb_flow_set_periphery(mf->m[g], node_pos, node_normal, n_nodes); }));
+    if (mf->n_shell != n_nodes)
+        mf->part_dirty = true;
+    mf->n_shell = n_nodes;
+    return SKB_OK;
+}
+
+int skb_mflow_set_bodies(skb_mflow *mf, const double *node_pos, const double *node_normal, int64_t n_nodes,
+                         const double *centers, int n_bodies) {
+    if (!mf || n_nodes < 0 || n_bodies < 0)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_set_bodies: bad arguments");
+    SKB_TRY(mf->workers->run(
+        [&](int g) { return skb_flow_set_bodies(mf->m[g], node_pos, node_normal, n_nodes, centers, n_bodies); }));
+    if (mf->n_body != n_nodes)
+        mf->part_dirty = true;
+    mf->n_body = n_nodes;
+    mf->n_bodies = n_bodies;
+    return SKB_OK;
+}
+
+int skb_mflow_set_cross(skb_mflow *mf, int mode) {
+    if (!mf)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_set_cross: NULL");
+    for (int g = 0; g < mf->n; ++g)
+        SKB_TRY(skb_flow_set_cross(mf->m[g], mode));
+    mf->part_dirty = true; // the members' target lists change: re-run the warm-up
+    return SKB_OK;
+}
+
+int skb_mflow_set_overlap(skb_mflow *mf, int on) {
+    if (!mf)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_set_overlap: NULL");
+    for (int g = 0; g < mf->n; ++g)
+        SKB_TRY(skb_flow_set_overlap(mf->m[g], on));
+    return SKB_OK;
+}
+
+int skb_mflow_set_self_exclusion(skb_mflow *mf, int fused) {
+    if (!mf)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_set_self_exclusion: NULL");
+    for (int g = 0; g < mf->n; ++g)
+        SKB_TRY(skb_flow_set_self_exclusion(mf->m[g], fused));
+    return SKB_OK;
+}
+
+int skb_mflow_partition(skb_mflow *mf, int member, int *fiber_begin, int *fiber_end, int64_t *shell_begin,
+                        int64_t *shell_end, int64_t *body_begin, int64_t *body_end) {
+    if (!mf || member < 0 || member >= mf->n)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_partition: bad member");
+    SKB_TRY(mflow_prepare(mf));
+    if (fiber_begin) *fiber_begin = mf->f0[member];
+    if (fiber_end) *fiber_end = mf->f1[member];
+    if (shell_begin) *shell_begin = mf->s0[member];
+    if (shell_end) *shell_end = mf->s1[member];
+    if (body_begin) *body_begin = mf->b0[member];
+    if (body_end) *body_end = mf->b1[member];
+    return SKB_OK;
+}
+
+// host-only (no GPU needed): the partition skb_mflow uses, for rank-per-GPU hosts that want the same one
+int skb_partition_query(const int *n_nodes, int n_fibers, int64_t n_shell, int64_t n_body, int n_members, int member,
+                        int64_t *out6) {
+    if (n_fibers < 0 || (n_fibers > 0 && !n_nodes) || n_shell < 0 || n_body < 0 || n_members < 1 || member < 0 ||
+        member >= n_members || !out6)
+        return set_error(SKB_ERR_INVALID, "skb_partition_query: bad arguments");
+    std::vector<long long> off((size_t)n_fibers + 1, 0);
+    for (int f = 0; f < n_fibers; ++f)
+        off[(size_t)f + 1] = off[(size_t)f] + n_nodes[f];
+    std::vector<int> f0, f1;
+    std::vector<long long> s0, s1, b0, b1;
+    partition_rows(off, n_shell, n_body, n_members, f0, f1, s0, s1, b0, b1);
+    out6[0] = f0[member], out6[1] = f1[member], out6[2] = s0[member], out6[3] = s1[member], out6[4] = b0[member],
+    out6[5] = b1[member];
+    return SKB_OK;
+}
+
+int skb_mflow_set_fiber_class(skb_mflow *mf, int n_nodes, const double *D_1_0, const double *P_downsample_bc) {
+    if (!mf)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_set_fiber_class: NULL");
+    for (int g = 0; g < mf->n; ++g)
+        SKB_TRY(skb_flow_set_fiber_class(mf->m[g], n_nodes, D_1_0, P_downsample_bc));
+    mf->ops_ready = false;
+    return SKB_OK;
+}
+
+// element offset of fiber f's block in a concatenation of per-fiber (k n) x (4 n) matrices
+static long long op_offset(const skb_mflow *mf, int f, int k) {
+    long long o = 0;
+    for (int i = 0; i < f; ++i)
+        o += (long long)k * 4 * mf->fiber_n[(size_t)i] * mf->fiber_n[(size_t)i];
+    return o;
+}
+
+int skb_mflow_set_fiber_operators(skb_mflow *mf, const double *A, const double *force_operator, const double *xs,
+                                  const double *length_prev, const int *plus_bc_velocity) {
+    if (!mf)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_set_fiber_operators: NULL");
+    SKB_TRY(mflow_prepare(mf));
+    if (mf->n_fibers > 0 && (!A || !force_operator || !xs || !length_prev || !plus_bc_velocity))
+        return set_error(SKB_ERR_INVALID, "skb_mflow_set_fiber_operators: NULL argument");
+    SKB_TRY(mf->workers->run([&](int g) -> int {
+        const int f0 = mf->f0[g];
+        if (mf->f1[g] == f0)
+            return skb_flow_set_fiber_operators(mf->m[g], nullptr, nullptr, nullptr, nullptr, nullptr);
+        return skb_flow_set_fiber_operators(mf->m[g], A + op_offset(mf, f0, 4), force_operator + op_offset(mf, f0, 3),
+                                            xs + 3 * mf->fiber_off[(size_t)f0], length_prev + f0, plus_bc_velocity + f0);
+    }));
+    mf->ops_ready = true;
+    return SKB_OK;
+}
+
+int skb_mflow_set_fiber_preconditioner(skb_mflow *mf, const double *A_inv) {
+    if (!mf || !mf->ops_ready)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_set_fiber_preconditioner: call skb_mflow_set_fiber_operators first");
+    return mf->workers->run([&](int g) -> int {
+        const int f0 = mf->f0[g];
+        return skb_flow_set_fiber_preconditioner(mf->m[g], mf->f1[g] == f0 ? nullptr : A_inv + op_offset(mf, f0, 4));
+    });
+}
+
+// the periphery's dense operator, rows block-partitioned like the periphery rows (periphery.cpp:387-417)
+int skb_mflow_set_dense(skb_mflow *mf, int op, const double *A_rowmajor, int64_t n_rows, int64_t n_cols) {
+    if (!mf || !A_rowmajor || n_rows != 3 * mf->n_shell || n_cols != 3 * mf->n_shell)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_set_dense: need the (3 N_s) x (3 N_s) operator of the %lld periphery "
+                                          "nodes set before", mf ? mf->n_shell : 0LL);
+    SKB_TRY(mflow_prepare(mf));
+    SKB_TRY(mf->workers->run([&](int g) -> int {
+        if (!mf->dn[g])
+            SKB_TRY(skb_dense_create_on(&mf->devs[g], 1, &mf->dn[g]));
+        return skb_dense_set_matrix(mf->dn[g], op, A_rowmajor + (size_t)(3 * mf->s0[g]) * (size_t)n_cols,
+                                    3 * (mf->s1[g] - mf->s0[g]), n_cols);
+    }));
+    if (op == SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY)
+        mf->has_dense = true;
+    return SKB_OK;
+}
+
+static int mflow_collect_stats(skb_mflow *mf) {
+    double dev_ms = 0;
+    long long pairs = 0;
+    int launches = 0;
+    for (int g = 0; g < mf->n; ++g) {
+        float ms = 0;
+        cudaSetDevice(mf->devs[g]);
+        if (cudaEventElapsedTime(&ms, mf->io[g].e0, mf->io[g].e1) == cudaSuccess)
+            dev_ms = std::max(dev_ms, (double)ms);
+        else
+            (void)cudaGetLastError();
+        skb_flow_stats st{};
+        skb_flow_last_stats(mf->m[g], &st);
+        pairs += st.n_pairs;
+        launches += st.launches;
+        int missing = -1;
+        SKB_TRY(skb_flow_group_error(mf->m[g], &missing));
+        if (missing >= 0)
+            return set_error(SKB_ERR_STATE, "device member %d timed out waiting for member %d (a peer failed or never "
+                                            "issued the matching call)", g, missing);
+    }
+    mf->stats.device_ms = dev_ms;
+    mf->stats.total_ms = dev_ms;
+    mf->stats.n_pairs = pairs;
+    mf->stats.launches = launches;
+    return SKB_OK;
+}
+
+// rows of member g: fiber nodes [a, a + n_fw), n_fibers whole fibers, n_sw periphery rows, n_bw body rows
+struct MemberRows {
+    long long a, n_fw, n_sw, n_bw;
+    int n_fibers;
+};
+static MemberRows member_rows(const skb_mflow *mf, int g) {
+    const long long a = mf->fiber_off.empty() ? 0 : mf->fiber_off[(size_t)mf->f0[g]],
+                    b = mf->fiber_off.empty() ? 0 : mf->fiber_off[(size_t)mf->f1[g]];
+    return MemberRows{a, b - a, mf->s1[g] - mf->s0[g], mf->b1[g] - mf->b0[g], mf->f1[g] - mf->f0[g]};
+}
+
+// buf (n_dbl doubles, at least 8 bytes) <- h on st; h == NULL leaves it unset
+static int put(DevBuf &buf, const double *h, size_t n_dbl, cudaStream_t st) {
+    SKB_TRY(buf.ensure(n_dbl * 8 + 8));
+    if (n_dbl && h)
+        CUDA_TRY(cudaMemcpyAsync(buf.ptr, h, n_dbl * 8, cudaMemcpyHostToDevice, st));
+    return SKB_OK;
+}
+
+// Size every member's transfer buffers on the CALLING thread, before any member starts launching: cudaMalloc /
+// cudaFree may synchronise the whole device and must not run while a peer on the same device sits in a flag wait.
+static int mflow_size_io(skb_mflow *mf, size_t n_ft) {
+    for (int g = 0; g < mf->n; ++g) {
+        CUDA_TRY(cudaSetDevice(mf->devs[g]));
+        skb_mflow::IO &io = mf->io[g];
+        const MemberRows r = member_rows(mf, g);
+        const size_t n_fw = (size_t)r.n_fw, n_sw = (size_t)r.n_sw, n_bw = (size_t)r.n_bw, n_fibers = (size_t)r.n_fibers;
+        SKB_TRY(io.x.ensure(n_fw * 32 + 8));
+        SKB_TRY(io.ff.ensure(n_fw * 24 + 8));
+        SKB_TRY(io.xs.ensure(n_sw * 24 + 8));
+        SKB_TRY(io.bd.ensure((size_t)mf->n_body * 24 + 8));
+        SKB_TRY(io.f.ensure(n_ft * 8 + 8));
+        SKB_TRY(io.t.ensure(n_ft * 8 + 8));
+        SKB_TRY(io.link.ensure(n_fibers * 56 + 8));
+        SKB_TRY(io.res.ensure(n_fw * 32 + 8));
+        SKB_TRY(io.outs.ensure(n_sw * 24 + 8));
+        SKB_TRY(io.vb.ensure(n_bw * 24 + 8));
+        SKB_TRY(io.v.ensure((n_fw + n_sw + n_bw) * 24 + 8));
+        if (mf->has_dense && n_sw > 0)
+            SKB_TRY(flow_size_overlap(mf->m[g], 3 * (long long)n_sw));
+    }
+    return SKB_OK;
+}
+
+// v_all over [fibers | periphery | bodies] like skb_flow_matvec; complete host arrays in and out
+int skb_mflow_matvec(skb_mflow *mf, const double *fib_forces, const double *shell_density, const double *body_densities,
+                     const double *body_forces_torques, double eta, double *v_all) {
+    if (!mf || !(eta > 0))
+        return set_error(SKB_ERR_INVALID, "skb_mflow_matvec: bad arguments");
+    const long long nf = mf->n_fib, ns = mf->n_shell, nb = mf->n_body;
+    if ((nf > 0 && !fib_forces) || (ns > 0 && !shell_density) || (nb > 0 && !body_densities) ||
+        (mf->n_bodies > 0 && !body_forces_torques) || (nf + ns + nb > 0 && !v_all))
+        return set_error(SKB_ERR_INVALID, "skb_mflow_matvec: NULL input for a non-empty class");
+    SKB_TRY(mflow_prepare(mf));
+    std::vector<double> f, t;
+    if (mf->n_bodies > 0)
+        split_forces_torques(body_forces_torques, mf->n_bodies, f, t);
+    SKB_TRY(mflow_size_io(mf, f.size()));
+    SKB_TRY(mf->workers->run([&](int g) -> int {
+        skb_flow *fl = mf->m[g];
+        skb_mflow::IO &io = mf->io[g];
+        CUDA_TRY(cudaSetDevice(mf->devs[g]));
+        const MemberRows r = member_rows(mf, g);
+        const long long a = r.a, n_fw = r.n_fw, n_sw = r.n_sw, n_bw = r.n_bw;
+        cudaStream_t st = flow_stream(fl);
+        SKB_TRY(put(io.ff, fib_forces ? fib_forces + 3 * a : nullptr, (size_t)n_fw * 3, st));
+        SKB_TRY(put(io.xs, shell_density ? shell_density + 3 * mf->s0[g] : nullptr, (size_t)n_sw * 3, st));
+        SKB_TRY(put(io.bd, body_densities, (size_t)nb * 3, st));
+        SKB_TRY(put(io.f, f.data(), f.size(), st));
+        SKB_TRY(put(io.t, t.data(), t.size(), st));
+        SKB_TRY(io.v.ensure((size_t)(n_fw + n_sw + n_bw) * 24 + 8));
+        CUDA_TRY(cudaEventRecord(io.e0, st));
+        SKB_TRY(skb_flow_matvec_device(fl, (const double *)io.ff.ptr, (const double *)io.xs.ptr,
+                                       (const double *)io.bd.ptr, (const double *)io.f.ptr, (const double *)io.t.ptr, eta,
+                                       (double *)io.v.ptr, st));
+        CUDA_TRY(cudaEventRecord(io.e1, st));
+        double *d_v = (double *)io.v.ptr;
+        if (n_fw)
+            CUDA_TRY(cudaMemcpyAsync(v_all + 3 * a, d_v, (size_t)n_fw * 24, cudaMemcpyDeviceToHost, st));
+        if (n_sw)
+            CUDA_TRY(cudaMemcpyAsync(v_all + 3 * (nf + mf->s0[g]), d_v + 3 * n_fw, (size_t)n_sw * 24,
+                                     cudaMemcpyDeviceToHost, st));
+        if (n_bw)
+            CUDA_TRY(cudaMemcpyAsync(v_all + 3 * (nf + ns + mf->b0[g]), d_v + 3 * (n_fw + n_sw), (size_t)n_bw * 24,
+                                     cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        return SKB_OK;
+    }));
+    return mflow_collect_stats(mf);
+}
+
+// System::apply_matvec (system.cpp:269-324) over n devices: complete host arrays in and out.  out_shell = res_shell
+// when skb_mflow_set_dense(SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY) was called, else v_shell.
+int skb_mflow_apply_matvec(skb_mflow *mf, const double *x_fibers, const double *x_shell, const double *body_densities,
+                           const double *body_forces_torques, const double *fiber_link_conditions, double eta,
+                           double *res_fibers, double *out_shell, double *v_bodies) {
+    if (!mf || !(eta > 0))
+        return set_error(SKB_ERR_INVALID, "skb_mflow_apply_matvec: bad arguments");
+    if (!mf->ops_ready)
+        return set_error(SKB_ERR_STATE, "skb_mflow_apply_matvec: call skb_mflow_set_fiber_operators first");
+    const long long nf = mf->n_fib, ns = mf->n_shell, nb = mf->n_body;
+    if ((nf > 0 && (!x_fibers || !res_fibers)) || (ns > 0 && (!x_shell || !out_shell)) ||
+        (nb > 0 && (!body_densities || !v_bodies)) || (mf->n_bodies > 0 && !body_forces_torques))
+        return set_error(SKB_ERR_INVALID, "skb_mflow_apply_matvec: NULL argument for a non-empty class");
+    SKB_TRY(mflow_prepare(mf));
+    std::vector<double> f, t;
+    if (mf->n_bodies > 0)
+        split_forces_torques(body_forces_torques, mf->n_bodies, f, t);
+    SKB_TRY(mflow_size_io(mf, f.size()));
+    SKB_TRY(mf->workers->run([&](int g) -> int {
+        skb_flow *fl = mf->m[g];
+        skb_mflow::IO &io = mf->io[g];
+        CUDA_TRY(cudaSetDevice(mf->devs[g]));
+        const int f0 = mf->f0[g], f1 = mf->f1[g];
+        const MemberRows r = member_rows(mf, g);
+        const long long a = r.a, n_fw = r.n_fw, n_sw = r.n_sw, n_bw = r.n_bw;
+        cudaStream_t st = flow_stream(fl);
+        SKB_TRY(put(io.x, x_fibers ? x_fibers + 4 * a : nullptr, (size_t)n_fw * 4, st));
+        SKB_TRY(put(io.xs, x_shell ? x_shell + 3 * mf->s0[g] : nullptr, (size_t)n_sw * 3, st));
+        SKB_TRY(put(io.bd, body_densities, (size_t)nb * 3, st));
+        SKB_TRY(put(io.f, f.data(), f.size(), st));
+        SKB_TRY(put(io.t, t.data(), t.size(), st));
+        SKB_TRY(put(io.link, fiber_link_conditions ? fiber_link_conditions + 7 * (long long)f0 : nullptr,
+                    (size_t)(f1 - f0) * 7, st));
+        SKB_TRY(io.res.ensure((size_t)n_fw * 32 + 8));
+        SKB_TRY(io.outs.ensure((size_t)n_sw * 24 + 8));
+        SKB_TRY(io.vb.ensure((size_t)n_bw * 24 + 8));
+        CUDA_TRY(cudaEventRecord(io.e0, st));
+        SKB_TRY(skb_flow_apply_matvec_device(
+            fl, mf->has_dense ? mf->dn[g] : nullptr, (const double *)io.x.ptr, (const double *)io.xs.ptr,
+            (const double *)io.bd.ptr, (const double *)io.f.ptr, (const double *)io.t.ptr,
+            (fiber_link_conditions && f1 > f0) ? (const double *)io.link.ptr : nullptr, eta, (double *)io.res.ptr,
+            (double *)io.outs.ptr, (double *)io.vb.ptr, st));
+        CUDA_TRY(cudaEventRecord(io.e1, st));
+        if (n_fw)
+            CUDA_TRY(cudaMemcpyAsync(res_fibers + 4 * a, io.res.ptr, (size_t)n_fw * 32, cudaMemcpyDeviceToHost, st));
+        if (n_sw)
+            CUDA_TRY(cudaMemcpyAsync(out_shell + 3 * mf->s0[g], io.outs.ptr, (size_t)n_sw * 24, cudaMemcpyDeviceToHost,
+                                     st));
+        if (n_bw)
+            CUDA_TRY(cudaMemcpyAsync(v_bodies + 3 * mf->b0[g], io.vb.ptr, (size_t)n_bw * 24, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        return SKB_OK;
+    }));
+    return mflow_collect_stats(mf);
+}
+
+// System::velocity_at_targets (system.cpp:330-384) over n devices: the targets are block-partitioned, every device
+// holds all sources
+int skb_mflow_velocity_at_targets(skb_mflow *mf, const double *r_trg, int64_t n_trg, const double *fib_forces,
+                                  const double *shell_density, const double *body_densities,
+                                  const double *body_forces_torques, double eta, double *vel) {
+    if (!mf || n_trg < 0 || (n_trg > 0 && (!r_trg || !vel)) || !(eta > 0))
+        return set_error(SKB_ERR_INVALID, "skb_mflow_velocity_at_targets: bad arguments");
+    const long long chunk = (n_trg + mf->n - 1) / mf->n;
+    SKB_TRY(mf->workers->run([&](int g) -> int {
+        const long long b = std::min<long long>(n_trg, g * chunk), e = std::min<long long>(n_trg, (g + 1) * chunk);
+        if (e <= b)
+            return (int)SKB_OK;
+        return skb_flow_velocity_at_targets(mf->m[g], r_trg + 3 * b, e - b, fib_forces, shell_density, body_densities,
+                                            body_forces_torques, eta, vel + 3 * b);
+    }));
+    double dev_ms = 0;
+    long long pairs = 0;
+    int launches = 0;
+    for (int g = 0; g < mf->n; ++g) {
+        skb_flow_stats st{};
+        skb_flow_last_stats(mf->m[g], &st);
+        dev_ms = std::max(dev_ms, st.device_ms);
+        pairs += st.n_pairs;
+        launches += st.launches;
+    }
+    mf->stats.device_ms = mf->stats.total_ms = dev_ms;
+    mf->stats.n_pairs = pairs;
+    mf->stats.launches = launches;
+    return SKB_OK;
+}
+
+int skb_mflow_last_stats(const skb_mflow *mf, skb_flow_stats *out) {
+    if (!mf || !out)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_last_stats: NULL");
+    *out = mf->stats;
+    return SKB_OK;
+}
+
+} // extern "C"
