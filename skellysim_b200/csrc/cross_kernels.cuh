@@ -19,14 +19,8 @@
 
 namespace skb {
 
-#ifndef SKB_CROSS_T
-#define SKB_CROSS_T 4 // fiber nodes per thread
-#endif
-#ifndef SKB_CROSS_MINB
-#define SKB_CROSS_MINB 3
-#endif
-constexpr int kCrossT = SKB_CROSS_T;
-constexpr int kCrossMinB = SKB_CROSS_MINB;
+constexpr int kCrossT = 4;    // fiber nodes per thread
+constexpr int kCrossMinB = 3; // resident CTAs per SM
 constexpr int kCrossBlock = kSymThreads * kCrossT;
 
 struct CrossArgs {

@@ -21,16 +21,6 @@ namespace skb {
 constexpr int kFiberGemvRows = 32;   // rows per CTA
 constexpr int kFiberGemvSlices = 8;  // column slices per row
 constexpr int kFiberGemvThreads = kFiberGemvRows * kFiberGemvSlices;
-// Are the first eight columns of a thread's row fetched into registers ahead of the x load (and of the MODE 2 preamble)?
-// MODE 0/1: yes.  MODE 2: NO -- the eight live values pushed it to 62 registers = 4 CTAs per SM; without them it fits
-// 32 registers = 8 CTAs per SM, and the other CTAs' loads cover this CTA's preamble better than its own early loads do
-// (a cp.async prefetch into shared memory was slower than both).
-#ifndef SKB_FIBER_PRE
-#define SKB_FIBER_PRE 1
-#endif
-#ifndef SKB_FIBER_PRE2
-#define SKB_FIBER_PRE2 0
-#endif
 
 struct FiberGemvItem {
     long long mat_off; // element offset of M_f in the concatenated operator buffer
@@ -59,11 +49,8 @@ struct FiberVelArgs {
 
 // CTAs per SM the register budget must allow: the kernels are latency x bandwidth bound (8 loads in flight per thread),
 // so resident CTAs are what counts (8 x 256 threads x 32 registers fill the register file).
-#ifndef SKB_FIBER_MINB2
-#define SKB_FIBER_MINB2 8
-#endif
 template <int MODE>
-__global__ void __launch_bounds__(kFiberGemvThreads, MODE == 2 ? SKB_FIBER_MINB2 : 8)
+__global__ void __launch_bounds__(kFiberGemvThreads, 8)
     fiber_gemv_kernel(const FiberGemvItem *__restrict__ items, const double *__restrict__ mats,
                       const double *__restrict__ x, double *__restrict__ out, const FiberVelArgs va) {
     extern __shared__ double fg_smem[];
@@ -76,13 +63,16 @@ __global__ void __launch_bounds__(kFiberGemvThreads, MODE == 2 ? SKB_FIBER_MINB2
     for (int j = threadIdx.x; j < it.cols; j += kFiberGemvThreads)
         xs_sh[j] = x[it.x_off + j];
     const int n = it.n_nodes;
-    // MODE 0/1: the first columns of this thread's row go out to HBM NOW, ahead of the x load
-    constexpr int kPre = MODE == 2 ? SKB_FIBER_PRE2 : SKB_FIBER_PRE;
+    // MODE 0/1: the first eight columns of this thread's row go out to HBM NOW, ahead of the x load.  MODE 2 does not
+    // prefetch them ahead of its preamble: the eight live values pushed it to 62 registers = 4 CTAs per SM; without them
+    // it fits 32 registers = 8 CTAs per SM, and the other CTAs' loads cover this CTA's preamble better than its own early
+    // loads do (a cp.async prefetch into shared memory was slower than both).
+    constexpr bool kPre = MODE != 2;
     const int lr0 = threadIdx.x & (kFiberGemvRows - 1), q0 = threadIdx.x / kFiberGemvRows;
     const bool row_ok = it.row0 + lr0 < it.rows;
-    const bool first_ok = kPre == 1 && row_ok && q0 + 7 * kFiberGemvSlices < it.cols;
+    const bool first_ok = kPre && row_ok && q0 + 7 * kFiberGemvSlices < it.cols;
     double v0[8];
-    if (kPre == 1 && first_ok) {
+    if (kPre && first_ok) {
         const double *m0 = mats + it.mat_off + it.row0 + lr0;
 #pragma unroll
         for (int u = 0; u < 8; ++u)
@@ -144,7 +134,7 @@ __global__ void __launch_bounds__(kFiberGemvThreads, MODE == 2 ? SKB_FIBER_MINB2
         const double *m = mats + it.mat_off + row;
         const long long ld = it.rows;
         int j = q;
-        if (kPre == 1 && first_ok) { // (loaded before the preamble)
+        if (kPre && first_ok) { // (loaded before the preamble)
 #pragma unroll
             for (int u = 0; u < 8; ++u)
                 acc = fma(v0[u], xs_sh[j + u * kFiberGemvSlices], acc);

@@ -29,17 +29,9 @@
 
 #include "tma_ptx.cuh"
 
-#ifndef SKB_SRC_UNROLL
-#define SKB_SRC_UNROLL 1 // source-pair iterations unrolled in the hot loop (tuning knob)
-#endif
-
 namespace skb {
 
-constexpr int kSrcUnroll = SKB_SRC_UNROLL;
-#ifndef SKB_CHAIN_GROUP
-#define SKB_CHAIN_GROUP 4 // independent pair chains evaluated stage-wise together when T >= 4 (tuning knob)
-#endif
-constexpr int kChainGroup = SKB_CHAIN_GROUP;
+constexpr int kChainGroup = 4;      // independent pair chains evaluated stage-wise together when T >= 4
 constexpr int kSrcTile = 128;       // sources per shared-memory stage
 constexpr int kStages = 4;          // TMA ring depth
 constexpr int kPrefetch = 2;        // tiles in flight ahead of the one being consumed (< kStages - 1)
@@ -289,7 +281,7 @@ __device__ __forceinline__ void stokeslet_two_sources(const double (&tx)[T], con
             uz[t] = fma(y[c], vz[c], uz[t]);
         }
     } else {
-        constexpr int G = (T % kChainGroup == 0) ? kChainGroup : 4;
+        constexpr int G = kChainGroup;
 #pragma unroll
         for (int src = 0; src < 2; ++src) {
 #pragma unroll
@@ -343,7 +335,7 @@ __device__ __forceinline__ void stresslet_two_sources(const double (&tx)[T], con
             uz[t] = fma(dz[c], co[c], uz[t]);
         }
     } else {
-        constexpr int G = (T % kChainGroup == 0) ? kChainGroup : 4;
+        constexpr int G = kChainGroup;
 #pragma unroll
         for (int src = 0; src < 2; ++src) {
 #pragma unroll
@@ -480,7 +472,7 @@ __global__ void __launch_bounds__(kCtaThreads, MINB) pair_sum_kernel(const PairA
         long long left = a.n_src - (long long)(first_tile + k) * kSrcTile;
         const int jmax = left >= kSrcTile ? kSrcTile / 2 : (int)((left + 1) >> 1);
         // the stresslet's longer body gains from exposing the next sources' LDS early
-        constexpr int kUnroll = (KIND == kStresslet && T <= 4) ? 2 * kSrcUnroll : kSrcUnroll;
+        constexpr int kUnroll = (KIND == kStresslet && T <= 4) ? 2 : 1;
 #pragma unroll kUnroll
         for (int j = 0; j < jmax; ++j) {
             // two sources per iteration: 48 B of positions = 3 x LDS.128 (warp-wide broadcast)

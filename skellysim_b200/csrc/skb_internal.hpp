@@ -12,7 +12,6 @@ namespace skb {
 struct DeviceInfo {
     int dev = 0;
     int num_sms = 0;
-    int cc_major = 0, cc_minor = 0;
     int occupancy[2][4] = {{1, 1, 1, 1}, {1, 1, 1, 1}}; // [kind][T index: 1,2,4,8] resident CTAs / SM
 };
 
@@ -41,7 +40,10 @@ long long launch_count();
 // side is ordered on `st`.
 int upload_pageable(void *d_dst, const void *h_src, size_t bytes, cudaStream_t st);
 
-DeviceInfo query_device(int dev);
+// Takes device `dev` into use, once per device and process: rejects anything but compute capability 9.0 and loads the
+// kernels that need launch attributes, with those attributes set.  Makes `dev` current.
+int prepare_device(int dev);
+DeviceInfo query_device(int dev); // (of a prepared device)
 LaunchPlan plan_launch(const DeviceInfo &di, int kind, long long n_trg, int n_src_tiles, int force_T, int force_S);
 int launch_pair_sum(const DeviceInfo &di, int kind, const double *d_r_src, const double *d_f_packed, long long n_src,
                     long long n_src_pad, const double *d_r_trg, long long n_trg, double *d_partial,
@@ -98,7 +100,7 @@ struct SourceSet {
     // symmetric (Newton's third law) path of the Stokeslet self-interaction, sym_kernels.cuh
     int self_state = -1;       // -1 unknown, 0 targets do not start with these sources, 1 they do
     bool sym_plan_valid = false;
-    int sym_T = 0, sym_nb = 0, sym_items = 0, sym_part = 0, sym_parts = 1, sym_owned = 0;
+    int sym_nb = 0, sym_items = 0, sym_part = 0, sym_parts = 1, sym_owned = 0;
     skb::DevBuf sym_item_buf, sym_row_begin, sym_P, sym_F, sym_row_ids /* block row I of every row of sym_P */, sym_flag;
     long long sym_pairs = 0; // ordered (target, source) pairs one launch of the symmetric kernel covers (both directions)
 };
@@ -168,9 +170,6 @@ int cross_eval(CrossState &cs, const DeviceInfo &di, const double *d_r_fib, cons
                long long n_rows, const double *d_r_sh, const double *d_s6, long long n_sh, long long n_sh_pad,
                double scale_dl, double scale_sl, double *d_u_fib, int acc_fib, double *d_u_shell, int acc_shell,
                cudaStream_t st, int *launches);
-
-// background row streamer (skb_dense.cu, stream_kernels.cuh): load the kernel and fix its attributes on `dev`
-int dense_stream_preload(int dev);
 
 struct SymItem;
 long long sym_block_nodes(); // nodes per block of the symmetric kernel (its I side)

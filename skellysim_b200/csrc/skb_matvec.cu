@@ -911,8 +911,8 @@ static int overlap_buffers(skb_flow *fl, long long n_rows) {
         CUDA_TRY(cudaStreamCreateWithPriority(&B.stream, cudaStreamNonBlocking, hi));
         CUDA_TRY(cudaEventCreateWithFlags(&B.fork, cudaEventDisableTiming));
         CUDA_TRY(cudaEventCreateWithFlags(&B.join, cudaEventDisableTiming));
-        // nothing may be loaded lazily later, while a group member on this device spins on a flag
-        SKB_TRY(dense_stream_preload(fl->dev));
+        // nothing may be loaded lazily later, while a group member on this device spins on a flag (the streamer itself
+        // was loaded when the device was prepared, prepare_device)
         cudaFuncAttributes fa;
         CUDA_TRY(cudaFuncGetAttributes(&fa, add_out_kernel));
     }

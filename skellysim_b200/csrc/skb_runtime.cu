@@ -7,11 +7,8 @@
 #include "pair_kernels.cuh"
 #include "sym_kernels.cuh"
 #include "cross_kernels.cuh"
+#include "stream_kernels.cuh"
 #include "skb_internal.hpp"
-
-#ifndef SKB_CARVEOUT_MAX
-#define SKB_CARVEOUT_MAX 1
-#endif
 
 #include <algorithm>
 #include <atomic>
@@ -52,27 +49,20 @@ long long launch_count() { return g_launches.load(std::memory_order_relaxed); }
 // ------------------------------------------------------------------------------------------------
 template <int KIND, int T, int MINB, bool EXCL = false>
 static cudaError_t launch_variant(const PairArgs &a, dim3 grid, cudaStream_t st) {
-    using L = SmemLayout<KIND, T, EXCL>;
-    auto kern = pair_sum_kernel<KIND, T, MINB, EXCL>;
-    static bool attr_set[64] = {false};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 64 && !attr_set[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::total_bytes);
-        if (e != cudaSuccess)
-            return e;
-        attr_set[dev] = true;
-    }
-    kern<<<grid, kCtaThreads, L::total_bytes, st>>>(a);
+    pair_sum_kernel<KIND, T, MINB, EXCL><<<grid, kCtaThreads, SmemLayout<KIND, T, EXCL>::total_bytes, st>>>(a);
     return cudaGetLastError();
+}
+
+template <int KIND, int T, int MINB, bool EXCL = false> static cudaError_t set_smem_variant() {
+    return cudaFuncSetAttribute(pair_sum_kernel<KIND, T, MINB, EXCL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                SmemLayout<KIND, T, EXCL>::total_bytes);
 }
 
 template <int KIND, int T, int MINB> static int occupancy_variant() {
     using L = SmemLayout<KIND, T>;
-    auto kern = pair_sum_kernel<KIND, T, MINB>;
-    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::total_bytes);
     int nb = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kCtaThreads, L::total_bytes) != cudaSuccess)
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, pair_sum_kernel<KIND, T, MINB>, kCtaThreads, L::total_bytes) !=
+        cudaSuccess)
         nb = 1;
     return nb < 1 ? 1 : nb;
 }
@@ -93,8 +83,6 @@ DeviceInfo query_device(int dev) {
     cudaSetDevice(dev);
     cudaGetDeviceProperties(&p, dev);
     di.num_sms = p.multiProcessorCount;
-    di.cc_major = p.major;
-    di.cc_minor = p.minor;
     const int Ts[4] = {1, 2, 4, 8};
     for (int k = 0; k < 2; ++k)
         for (int ti = 0; ti < 4; ++ti) {
@@ -352,6 +340,51 @@ using namespace skb;
             return _rc;                                                                                               \
     } while (0)
 
+// The launch attributes of every kernel that has them: the dynamic shared memory of the kernels that use more than the
+// default 48 KB, and the max-shared carve-out of pair_sym_kernel, pair_cross_kernel and the background row streamer
+// that runs beside them (an SM switches its shared-memory configuration only when idle, so a different preference would
+// keep them from sharing it).  Setting an attribute also loads the kernel.  This runs where a device is first taken into
+// use (skb_ctx and skb_dense creation), so that no kernel is loaded lazily in the middle of a matvec -- for instance
+// while a group member on the same device spins on a flag.
+int skb::prepare_device(int dev) {
+    static std::mutex mu;
+    static std::vector<bool> done;
+    std::lock_guard<std::mutex> lock(mu);
+    CUDA_TRY(cudaSetDevice(dev));
+    if (dev < (int)done.size() && done[dev])
+        return SKB_OK;
+    int major = 0, minor = 0;
+    CUDA_TRY(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
+    CUDA_TRY(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
+    // sm_90a code runs on compute capability 9.0 only (arch-specific targets are not forward compatible)
+    if (major != 9 || minor != 0)
+        return set_error(SKB_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", dev, major,
+                         minor);
+    for (int T : {1, 2, 4, 8}) {
+#define SMEM_CALL(KIND, T, MINB) CUDA_TRY((set_smem_variant<KIND, T, MINB>()))
+#define SMEM_CALL_EXCL(KIND, T, MINB) CUDA_TRY((set_smem_variant<KIND, T, MINB, true>()))
+        SKB_DISPATCH_T(kStokeslet, T, SMEM_CALL)
+        SKB_DISPATCH_T(kStokeslet, T, SMEM_CALL_EXCL)
+        SKB_DISPATCH_T(kStresslet, T, SMEM_CALL)
+#undef SMEM_CALL
+#undef SMEM_CALL_EXCL
+    }
+    auto set_shared = [](auto kern, int bytes) {
+        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+        return e == cudaSuccess ? cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                                       cudaSharedmemCarveoutMaxShared)
+                                : e;
+    };
+    CUDA_TRY(set_shared(pair_sym_kernel<kSymT, kSymMinB, false>, SymSmem<kSymT>::total_bytes));
+    CUDA_TRY(set_shared(pair_sym_kernel<kSymT, kSymMinB, true>, SymSmem<kSymT>::total_bytes));
+    CUDA_TRY(set_shared(pair_cross_kernel<kCrossT, kCrossMinB>, CrossSmem<kCrossT>::total_bytes));
+    CUDA_TRY(set_shared(dense_stream_kernel, kStreamSmemBytes));
+    if (dev >= (int)done.size())
+        done.resize(dev + 1);
+    done[dev] = true;
+    return SKB_OK;
+}
+
 // ------------------------------------------------------------------------------------------------
 // context
 // ------------------------------------------------------------------------------------------------
@@ -381,12 +414,8 @@ static int ctx_create_impl(const int *ids, int n, skb_ctx **out) {
         const int dev = ids ? ids[g] : g;
         if (dev < 0 || dev >= n_dev)
             return set_error(SKB_ERR_INVALID, "device id %d out of range", dev);
-        CUDA_TRY(cudaSetDevice(dev));
+        SKB_TRY(prepare_device(dev));
         d.info = query_device(dev);
-        // sm_90a code runs on compute capability 9.0 only (arch-specific targets are not forward compatible)
-        if (d.info.cc_major != 9 || d.info.cc_minor != 0)
-            return set_error(SKB_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", dev,
-                             d.info.cc_major, d.info.cc_minor);
         CUDA_TRY(cudaStreamCreateWithFlags(&d.stream, cudaStreamNonBlocking));
         // (d.aux_stream is created on first use by the symmetric path: most contexts of a flow never need one, and a
         // device has a finite number of hardware queues for independent streams)
@@ -801,27 +830,8 @@ __global__ void self_check_kernel(const double *__restrict__ a, const double *__
         *differs = 1;
 }
 
-template <int T, int MINB, bool EXCL>
-static cudaError_t launch_sym(const SymArgs &a, int n_items, cudaStream_t st) {
-    using L = SymSmem<T>;
-    auto kern = pair_sym_kernel<T, MINB, EXCL>;
-    static bool attr_set[64] = {false};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 64 && !attr_set[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::total_bytes);
-        if (e != cudaSuccess)
-            return e;
-#if SKB_CARVEOUT_MAX
-        // one shared-memory configuration for this kernel and the background row streamer (stream_kernels.cuh): an SM
-        // switches configuration only when idle, so a different preference would keep the two from sharing it
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-        if (e != cudaSuccess)
-            return e;
-#endif
-        attr_set[dev] = true;
-    }
-    kern<<<n_items, kSymThreads, L::total_bytes, st>>>(a);
+template <bool EXCL> static cudaError_t launch_sym(const SymArgs &a, int n_items, cudaStream_t st) {
+    pair_sym_kernel<kSymT, kSymMinB, EXCL><<<n_items, kSymThreads, SymSmem<kSymT>::total_bytes, st>>>(a);
     return cudaGetLastError();
 }
 
@@ -847,48 +857,39 @@ static int sym_owned_rows(int nb, int part, int parts) {
     return n;
 }
 
-// Work items of the symmetric kernel: (I, groups [g0, g1)) over the upper triangle of nb blocks INCLUDING the block
-// diagonal (row I starts at its own first group), restricted to the block rows owned by `part`.  Units are 32-node groups (kSymGroupsPerBlock per block).  Guided sizes: most of the
-// work goes out in large items (about a quarter of a CTA slot's share each), the last ~30 % in items a quarter of that
-// size and the last ~8 % in single stages (4 groups = 17 us of one CTA slot), so that all CTA slots drain together: the
-// hardware hands the next item to whichever slot frees up first, in `order` (large items first).  item.slot is the
-// item's row-major position, row_begin[b]..row_begin[b+1] the slots of row b (their forward partials are summed in
-// that order by sym_reduce_kernel).
-void build_sym_items(int nb, int part, int parts, int num_sms, std::vector<SymItem> &order,
-                     std::vector<int> &row_begin) {
-    const int gpb = kSymGroupsPerBlock, sg = kSymStageGroups;
-    const int occ = kSymMinB;
-    auto env_int = [](const char *name, int dflt) {
-        const char *e = getenv(name);
-        return e && atoi(e) > 0 ? atoi(e) : dflt;
-    };
-    static const int waves = env_int("SKB_SYM_WAVES", 4);      // large items per CTA slot (if all work were large items)
-    static const int pct_mid = env_int("SKB_SYM_PCT_MID", 30);  // last x % of the work: quarter-size items
-    static const int pct_fine = env_int("SKB_SYM_PCT_FINE", 8); // last x % of the work: single stages
-    long long work = 0; // groups x blocks owned by this part
-    for (int I = 0; I < nb; ++I)
-        if (sym_row_owner(I, parts) == part)
-            work += (long long)gpb * (nb - I);
-    const long long slots = (long long)num_sms * occ;
-    long long big = work / std::max<long long>(1, slots * waves);
+// One row of work items: block I of the I side meets the J groups [g0, g0 + n_groups); its items write row prow of P.
+struct ItemRow {
+    int I, g0, n_groups, prow;
+};
+
+// The work items of one launch of the symmetric or the cross kernel: `rows` (in increasing I) cut into items (I, groups
+// [g0, g1)), in units of 32-node groups.  Guided sizes: most of the work goes out in large items (about a quarter of a
+// CTA slot's share each), the last ~30 % in items a quarter of that size and the last ~8 % in single stages (4 groups =
+// 17 us of one CTA slot), so that all `slots` CTA slots drain together: the hardware hands the next item to whichever
+// slot frees up first, in `order` (large items first).  item.slot is the item's row-major position,
+// row_begin[b]..row_begin[b+1] the slots of block row b < n_blocks (their forward partials are summed in that order by
+// the reduction kernel).
+static void cut_items(const std::vector<ItemRow> &rows, int n_blocks, long long slots, std::vector<SymItem> &order,
+                      std::vector<int> &row_begin) {
+    const int sg = kSymStageGroups;
+    long long work = 0;
+    for (const ItemRow &r : rows)
+        work += r.n_groups;
+    long long big = work / std::max<long long>(1, slots * 4); // 4 large items per CTA slot (if all work were large items)
     big = std::max<long long>(sg, std::min<long long>(big / sg * sg, 1024LL * sg));
     const long long mid = std::max<long long>(sg, big / 4 / sg * sg);
     struct Piece {
         int I, g0, g1, prow;
     };
     std::vector<Piece> pieces;
-    int prow = 0;
-    for (int I = 0; I < nb; ++I) {
-        if (sym_row_owner(I, parts) != part)
-            continue;
-        const int my_prow = prow++; // every owned row has a P row, in increasing I (sym_reduce_kernel counts the same way)
-        const int first = gpb * I, len = gpb * (nb - I); // from the block's own groups (the block diagonal) onwards
+    for (const ItemRow &r : rows) {
+        const int len = r.n_groups;
         const int n_chunks = (int)((len + big - 1) / big);
         for (int c = 0; c < n_chunks; ++c) { // near-equal chunks, cut at stage boundaries
             const int a = (int)((long long)(len / sg) * c / n_chunks) * sg;
             const int b = c + 1 == n_chunks ? len : (int)((long long)(len / sg) * (c + 1) / n_chunks) * sg;
             if (b > a)
-                pieces.push_back(Piece{I, first + a, first + b, my_prow});
+                pieces.push_back(Piece{r.I, r.g0 + a, r.g0 + b, r.prow});
         }
     }
     // the tail of the launch order is cut finer
@@ -897,8 +898,8 @@ void build_sym_items(int nb, int part, int parts, int num_sms, std::vector<SymIt
     std::vector<Piece> fine;
     long long done = 0;
     // (at most ~6 items of a tier per CTA slot: more would only add forward-partial slabs)
-    const long long fine_work = std::min<long long>(work * pct_fine / 100, slots * 6 * sg);
-    const long long mid_work = std::min<long long>(work * pct_mid / 100, fine_work + slots * 6 * mid);
+    const long long fine_work = std::min<long long>(work * 8 / 100, slots * 6 * sg);
+    const long long mid_work = std::min<long long>(work * 30 / 100, fine_work + slots * 6 * mid);
     for (const Piece &pc : pieces) {
         const long long len = pc.g1 - pc.g0;
         const long long left = work - done;
@@ -911,16 +912,42 @@ void build_sym_items(int nb, int part, int parts, int num_sms, std::vector<SymIt
     std::sort(fine.begin(), fine.end(),
               [](const Piece &x, const Piece &y) { return x.I != y.I ? x.I < y.I : x.g0 < y.g0; });
     std::vector<SymItem> items(fine.size());
-    row_begin.assign(nb + 1, 0);
+    row_begin.assign(n_blocks + 1, 0);
     for (size_t i = 0; i < fine.size(); ++i) {
         items[i] = SymItem{fine[i].I, fine[i].g0, fine[i].g1, (int)i, fine[i].prow, 0};
         row_begin[fine[i].I + 1] = (int)i + 1;
     }
-    for (int b = 0; b < nb; ++b) // rows without items inherit the running count
+    for (int b = 0; b < n_blocks; ++b) // rows without items inherit the running count
         row_begin[b + 1] = std::max(row_begin[b + 1], row_begin[b]);
     order = items;
     std::stable_sort(order.begin(), order.end(),
                      [](const SymItem &x, const SymItem &y) { return (x.g1 - x.g0) > (y.g1 - y.g0); });
+}
+
+// Work items of the symmetric kernel: the upper triangle of nb blocks INCLUDING the block diagonal (row I starts at its
+// own first group), restricted to the block rows owned by `part`.
+void build_sym_items(int nb, int part, int parts, int num_sms, std::vector<SymItem> &order,
+                     std::vector<int> &row_begin) {
+    const int gpb = kSymGroupsPerBlock;
+    std::vector<ItemRow> rows;
+    for (int I = 0; I < nb; ++I) // every owned row has a P row, in increasing I (sym_reduce_kernel counts the same way)
+        if (sym_row_owner(I, parts) == part)
+            rows.push_back(ItemRow{I, gpb * I, gpb * (nb - I), (int)rows.size()});
+    cut_items(rows, nb, (long long)num_sms * kSymMinB, order, row_begin);
+}
+
+// Puts a plan on the device: the items in launch order, row_begin, and one forward-partial slab (block x 3 doubles) per
+// item.  Waits for the copies: the host vectors may go out of scope on return.
+static int upload_plan(const std::vector<SymItem> &order, const std::vector<int> &row_begin, long long block,
+                       DevBuf &items, DevBuf &d_row_begin, DevBuf &F, cudaStream_t st) {
+    SKB_TRY(items.ensure(order.size() * sizeof(SymItem) + 16));
+    SKB_TRY(d_row_begin.ensure(row_begin.size() * sizeof(int)));
+    SKB_TRY(F.ensure(order.size() * (size_t)block * 24 + 16));
+    CUDA_TRY(cudaMemcpyAsync(items.ptr, order.data(), order.size() * sizeof(SymItem), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_row_begin.ptr, row_begin.data(), row_begin.size() * sizeof(int), cudaMemcpyHostToDevice,
+                             st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return SKB_OK;
 }
 
 // Are the first n_src targets bit-identical to the Stokeslet sources?  (decided once per set of positions)
@@ -949,8 +976,7 @@ static int ensure_self_state(DeviceState &d, SourceSet &s, cudaStream_t st) {
 static int sym_prepare(skb_ctx *ctx, DeviceState &d, cudaStream_t st, int *use) {
     *use = 0;
     SourceSet &s = d.src[SKB_STOKESLET];
-    const int T = kSymT;
-    const long long block = (long long)kSymThreads * T;
+    const long long block = sym_block_nodes();
     if (s.n < 4096 && ctx->sym_mode != 1)
         return SKB_OK; // too small to matter
     if (s.n < 2 * block || d.n_trg < s.n)
@@ -961,37 +987,30 @@ static int sym_prepare(skb_ctx *ctx, DeviceState &d, cudaStream_t st, int *use) 
     SKB_TRY(ensure_self_state(d, s, st));
     if (s.self_state != 1)
         return SKB_OK;
-    if (!s.sym_plan_valid || s.sym_T != T || s.sym_nb != (int)nb || s.sym_part != d.sym_part ||
-        s.sym_parts != d.sym_parts) {
-        std::vector<SymItem> order;
-        std::vector<int> row_begin;
-        build_sym_items((int)nb, d.sym_part, d.sym_parts, d.info.num_sms, order, row_begin);
-        SKB_TRY(s.sym_item_buf.ensure(order.size() * sizeof(SymItem) + 16));
-        SKB_TRY(s.sym_row_begin.ensure(row_begin.size() * sizeof(int)));
-        if (s.sym_P.ensure((size_t)sym_owned_rows((int)nb, d.sym_part, d.sym_parts) * (size_t)s.n_pad * 24) !=
-            SKB_OK) { // not enough free memory for the reverse partials: the plain kernel serves this geometry
+    if (!s.sym_plan_valid || s.sym_nb != (int)nb || s.sym_part != d.sym_part || s.sym_parts != d.sym_parts) {
+        std::vector<int> owned; // block rows of P's rows, for sym_reduce_kernel
+        for (int I = 0; I < (int)nb; ++I)
+            if (sym_row_owner(I, d.sym_parts) == d.sym_part)
+                owned.push_back(I);
+        const size_t p_bytes = owned.size() * (size_t)s.n_pad * 24;
+        if (s.sym_P.ensure(p_bytes) != SKB_OK) { // not enough free memory for the reverse partials: the plain kernel
+                                                 // serves this geometry
             (void)cudaGetLastError();
             if (ctx->sym_layout) // every device holds ALL leading targets there and the caller reduce-scatters the
                                  // partial sums: a silent switch to the plain kernel would count them P times
                 return set_error(SKB_ERR_ALLOC, "symmetric multi-device layout: no memory for the reverse partials "
                                                 "(%zu bytes); free memory or skb_ctx_set_symmetric(ctx, 0)",
-                                 (size_t)sym_owned_rows((int)nb, d.sym_part, d.sym_parts) * (size_t)s.n_pad * 24);
+                                 p_bytes);
             s.self_state = 0;
             return SKB_OK;
         }
-        SKB_TRY(s.sym_F.ensure(order.size() * (size_t)block * 24 + 16));
-        std::vector<int> owned;
-        for (int I = 0; I < (int)nb; ++I)
-            if (sym_row_owner(I, d.sym_parts) == d.sym_part)
-                owned.push_back(I);
-        SKB_TRY(s.sym_row_ids.ensure(owned.size() * sizeof(int) + 16)); // (block rows of P's rows, for sym_reduce_kernel)
+        SKB_TRY(s.sym_row_ids.ensure(owned.size() * sizeof(int) + 16));
         CUDA_TRY(cudaMemcpyAsync(s.sym_row_ids.ptr, owned.data(), owned.size() * sizeof(int), cudaMemcpyHostToDevice, st));
         s.sym_owned = (int)owned.size();
-        CUDA_TRY(cudaMemcpyAsync(s.sym_item_buf.ptr, order.data(), order.size() * sizeof(SymItem),
-                                 cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaMemcpyAsync(s.sym_row_begin.ptr, row_begin.data(), row_begin.size() * sizeof(int),
-                                 cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaStreamSynchronize(st)); // host vectors go out of scope
+        std::vector<SymItem> order;
+        std::vector<int> row_begin;
+        build_sym_items((int)nb, d.sym_part, d.sym_parts, d.info.num_sms, order, row_begin);
+        SKB_TRY(upload_plan(order, row_begin, block, s.sym_item_buf, s.sym_row_begin, s.sym_F, st));
         // pairs of one launch: every ordered pair of real nodes in (owned row I, any block J > I), both directions
         long long pairs = 0;
         for (long long I = 0; I < nb; ++I) {
@@ -1002,7 +1021,6 @@ static int sym_prepare(skb_ctx *ctx, DeviceState &d, cudaStream_t st, int *use) 
             pairs += 2 * nI * after + nI * nI; // both directions beyond the block + the block diagonal
         }
         s.sym_pairs = pairs;
-        s.sym_T = T;
         s.sym_nb = (int)nb;
         s.sym_items = (int)order.size();
         s.sym_part = d.sym_part;
@@ -1020,8 +1038,7 @@ static int sym_eval(skb_ctx *ctx, DeviceState &d, double *d_u_out, int accumulat
     const double *f_packed = s.f_cur;
     if (!d.aux_stream)
         CUDA_TRY(cudaStreamCreateWithFlags(&d.aux_stream, cudaStreamNonBlocking));
-    const int T = s.sym_T;
-    const long long block = (long long)kSymThreads * T;
+    const long long block = sym_block_nodes();
     SymArgs a;
     a.r = (const double *)s.r.ptr;
     a.f = f_packed;
@@ -1034,8 +1051,7 @@ static int sym_eval(skb_ctx *ctx, DeviceState &d, double *d_u_out, int accumulat
     if (s.sym_items > 0) {
         a.fid = s.excl ? (const int *)s.excl_ids.ptr : nullptr;
         CUDA_TRY(cudaEventRecord(d.ev_s0, st));
-        e = s.excl ? launch_sym<kSymT, kSymMinB, true>(a, s.sym_items, st)
-                   : launch_sym<kSymT, kSymMinB, false>(a, s.sym_items, st);
+        e = s.excl ? launch_sym<true>(a, s.sym_items, st) : launch_sym<false>(a, s.sym_items, st);
         if (e == cudaSuccess)
             CUDA_TRY(cudaEventRecord(d.ev_s1, st));
         d.sym_timed = true;
@@ -1064,57 +1080,6 @@ namespace skb {
 
 long long cross_block_nodes() { return kCrossBlock; }
 
-// Work items of the cross kernel: rectangles (fiber block I, periphery groups [g0, g1)), every block meets every group;
-// guided sizes as for the symmetric kernel (large items first, a fine tail).
-static void build_cross_items(int n_blocks, int n_groups, int num_sms, std::vector<SymItem> &order,
-                              std::vector<int> &row_begin) {
-    const int sg = kSymStageGroups;
-    const long long work = (long long)n_blocks * n_groups;
-    const long long slots = (long long)num_sms * kCrossMinB;
-    long long big = work / std::max<long long>(1, slots * 4);
-    big = std::max<long long>(sg, std::min<long long>(big / sg * sg, 1024LL * sg));
-    const long long mid = std::max<long long>(sg, big / 4 / sg * sg);
-    struct Piece {
-        int I, g0, g1;
-    };
-    std::vector<Piece> pieces;
-    for (int I = 0; I < n_blocks; ++I) {
-        const int n_chunks = (int)((n_groups + big - 1) / big);
-        for (int c = 0; c < n_chunks; ++c) {
-            const int a = (int)((long long)(n_groups / sg) * c / n_chunks) * sg;
-            const int b = c + 1 == n_chunks ? n_groups : (int)((long long)(n_groups / sg) * (c + 1) / n_chunks) * sg;
-            if (b > a)
-                pieces.push_back(Piece{I, a, b});
-        }
-    }
-    std::stable_sort(pieces.begin(), pieces.end(),
-                     [](const Piece &x, const Piece &y) { return (x.g1 - x.g0) > (y.g1 - y.g0); });
-    std::vector<Piece> fine;
-    long long done = 0;
-    const long long fine_work = std::min<long long>(work * 8 / 100, slots * 6 * sg);
-    const long long mid_work = std::min<long long>(work * 30 / 100, fine_work + slots * 6 * mid);
-    for (const Piece &pc : pieces) {
-        const long long len = pc.g1 - pc.g0, left = work - done;
-        const long long unit = left <= fine_work ? sg : left <= mid_work ? mid : len;
-        for (long long g = pc.g0; g < pc.g1; g += unit)
-            fine.push_back(Piece{pc.I, (int)g, (int)std::min<long long>(pc.g1, g + unit)});
-        done += len;
-    }
-    std::sort(fine.begin(), fine.end(),
-              [](const Piece &x, const Piece &y) { return x.I != y.I ? x.I < y.I : x.g0 < y.g0; });
-    std::vector<SymItem> items(fine.size());
-    row_begin.assign(n_blocks + 1, 0);
-    for (size_t i = 0; i < fine.size(); ++i) {
-        items[i] = SymItem{fine[i].I, fine[i].g0, fine[i].g1, (int)i, fine[i].I, 0};
-        row_begin[fine[i].I + 1] = (int)i + 1;
-    }
-    for (int b = 0; b < n_blocks; ++b)
-        row_begin[b + 1] = std::max(row_begin[b + 1], row_begin[b]);
-    order = items;
-    std::stable_sort(order.begin(), order.end(),
-                     [](const SymItem &x, const SymItem &y) { return (x.g1 - x.g0) > (y.g1 - y.g0); });
-}
-
 int cross_eval(CrossState &cs, const DeviceInfo &di, const double *d_r_fib, const double *d_h, long long node0,
                long long n_rows, const double *d_r_sh, const double *d_s6, long long n_sh, long long n_sh_pad,
                double scale_dl, double scale_sl, double *d_u_fib, int acc_fib, double *d_u_shell, int acc_shell,
@@ -1126,17 +1091,15 @@ int cross_eval(CrossState &cs, const DeviceInfo &di, const double *d_r_fib, cons
     const int n_groups = (int)((n_sh + kSymGroup - 1) / kSymGroup);
     if (!cs.valid || cs.node0 != node0 || cs.n_rows != n_rows || cs.n_sh != n_sh || cs.n_sh_pad != n_sh_pad ||
         cs.num_sms != di.num_sms) {
+        // items: rectangles (fiber block I, periphery groups [g0, g1)), every block meets every group
+        std::vector<ItemRow> rows;
+        for (int I = 0; I < n_blocks; ++I)
+            rows.push_back(ItemRow{I, 0, n_groups, I});
         std::vector<SymItem> order;
         std::vector<int> row_begin;
-        build_cross_items(n_blocks, n_groups, di.num_sms, order, row_begin);
-        SKB_TRY(cs.items.ensure(order.size() * sizeof(SymItem) + 16));
-        SKB_TRY(cs.row_begin.ensure(row_begin.size() * sizeof(int)));
+        cut_items(rows, n_blocks, (long long)di.num_sms * kCrossMinB, order, row_begin);
         SKB_TRY(cs.P.ensure((size_t)n_blocks * (size_t)n_sh_pad * 24));
-        SKB_TRY(cs.F.ensure(order.size() * (size_t)block * 24 + 16));
-        CUDA_TRY(cudaMemcpyAsync(cs.items.ptr, order.data(), order.size() * sizeof(SymItem), cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaMemcpyAsync(cs.row_begin.ptr, row_begin.data(), row_begin.size() * sizeof(int),
-                                 cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaStreamSynchronize(st)); // host vectors go out of scope
+        SKB_TRY(upload_plan(order, row_begin, block, cs.items, cs.row_begin, cs.F, st));
         cs.node0 = node0, cs.n_rows = n_rows, cs.n_sh = n_sh, cs.n_sh_pad = n_sh_pad;
         cs.n_blocks = n_blocks, cs.n_items = (int)order.size(), cs.num_sms = di.num_sms;
         cs.valid = true;
@@ -1152,20 +1115,7 @@ int cross_eval(CrossState &cs, const DeviceInfo &di, const double *d_r_fib, cons
     a.n_sh_pad = n_sh_pad;
     a.node0 = node0;
     a.n_rows = n_rows;
-    using L = CrossSmem<kCrossT>;
-    auto kern = pair_cross_kernel<kCrossT, kCrossMinB>;
-    static bool attr_set[64] = {false};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 64 && !attr_set[dev]) {
-        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::total_bytes));
-#if SKB_CARVEOUT_MAX
-        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                      cudaSharedmemCarveoutMaxShared));
-#endif
-        attr_set[dev] = true;
-    }
-    kern<<<cs.n_items, kSymThreads, L::total_bytes, st>>>(a);
+    pair_cross_kernel<kCrossT, kCrossMinB><<<cs.n_items, kSymThreads, CrossSmem<kCrossT>::total_bytes, st>>>(a);
     CUDA_TRY(cudaGetLastError());
     const long long nr3 = 3 * n_rows, ns3 = 3 * n_sh;
     cross_reduce_fib_kernel<<<(unsigned)((nr3 + 255) / 256), 256, 0, st>>>(
@@ -1300,7 +1250,7 @@ int eval_on_device(skb_ctx *ctx, DeviceState &d, int kind, StrengthMode mode, co
             CUDA_TRY(cudaEventRecord(d.ev_join, d.aux_stream));
             CUDA_TRY(cudaStreamWaitEvent(st, d.ev_join, 0));
         }
-        plan.T = s.sym_T;
+        plan.T = kSymT;
         plan.n_splits = 1;
         plan.grid_x = (unsigned)s.sym_items;
         plan.tiles_per_split = 0;

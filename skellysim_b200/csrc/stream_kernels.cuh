@@ -31,17 +31,9 @@ namespace skb {
 constexpr int kStreamConsumers = 64;                 // two consumer warps
 constexpr int kStreamThreads = kStreamConsumers + 32; // + the producer warp (five lanes active)
 constexpr int kStreamRows = 4;     // rows per group (x is re-used 4 times per load)
-#ifndef SKB_STREAM_COLS
-#define SKB_STREAM_COLS 512
-#endif
-#ifndef SKB_STREAM_HINT
-#define SKB_STREAM_HINT 1
-#endif
-constexpr int kStreamCols = SKB_STREAM_COLS; // columns per stage (a multiple of 128)
-#ifndef SKB_STREAM_STAGES
-#define SKB_STREAM_STAGES 5
-#endif
-constexpr int kStreamStages = SKB_STREAM_STAGES;
+constexpr int kStreamCols = 512;   // columns per stage (a multiple of 128)
+constexpr int kStreamStages = 5;
+constexpr int kStreamMaxNReg = 32; // registers per thread: fits beside pair_sym_kernel (see above)
 constexpr int kStreamRowBytes = kStreamCols * 8;
 constexpr int kStreamStageBytes = (kStreamRows + 1) * kStreamRowBytes; // rows of A, then the segment of x
 // ring | full + empty barriers | (group, chunk) of every stage | cross-warp sums
@@ -58,135 +50,8 @@ struct StreamArgs {
     unsigned long long *next_group; // ticket counter, zero at launch
 };
 
-#ifndef SKB_STREAM_MAXNREG
-#define SKB_STREAM_MAXNREG 32
-#endif
-__global__ void __maxnreg__(SKB_STREAM_MAXNREG) dense_stream_kernel(const StreamArgs a) {
-    extern __shared__ __align__(128) unsigned char st_smem[];
-    uint64_t *full_bar = reinterpret_cast<uint64_t *>(st_smem + kStreamBarOffset);
-    uint64_t *empty_bar = full_bar + kStreamStages;
-    int2 *meta = reinterpret_cast<int2 *>(st_smem + kStreamMetaOffset);
-    double *red = reinterpret_cast<double *>(st_smem + kStreamRedOffset);
-    const int t = threadIdx.x;
-    const int n_chunks = (int)((a.n_cols + kStreamCols - 1) / kStreamCols);
-    if (t == 0) {
-        for (int s = 0; s < kStreamStages; ++s) {
-            mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], kStreamConsumers / 32);
-        }
-        mbar_fence_init();
-    }
-    __syncthreads();
-
-    if (t >= kStreamConsumers) {
-        // ---- producer: lanes 0..3 own one row of the group each, lane 4 the segment of x; every lane keeps its own source
-        // pointer, so a stage costs one short instruction sequence per lane, not five address computations in one lane
-        // (that first version spent ~150 cycles per copy and was bound by it whatever the ring depth) ----
-        const int lane = t - kStreamConsumers;
-        if (lane > kStreamRows)
-            return;
-        constexpr unsigned kMask = (2u << kStreamRows) - 1u;
-        const long long n_groups = (a.n_rows + kStreamRows - 1) / kStreamRows;
-        const uint64_t policy = l2_policy_evict_first();
-        long long group = blockIdx.x;
-        int s = 0;
-        uint32_t empty_parity = 1; // parity of the phase BEFORE the first use: the wait falls through on a fresh barrier
-        for (;;) {
-            if (group >= n_groups) { // end marker: completes on the arrive alone
-                if (lane == 0) {
-                    mbar_wait(&empty_bar[s], empty_parity);
-                    meta[s] = make_int2(-1, 0);
-                    mbar_arrive(&full_bar[s]);
-                }
-                return;
-            }
-            // the ticket of the FOLLOWING group is drawn a whole group ahead of its use
-            unsigned long long ticket = 0;
-            if (lane == 0)
-                ticket = atomicAdd(a.next_group, 1ULL);
-            const long long row0 = group * kStreamRows;
-            const int rows = (int)min((long long)kStreamRows, a.n_rows - row0);
-            const double *src = lane < kStreamRows ? a.A + (row0 + lane) * a.n_cols : a.x;
-            const bool active = lane == kStreamRows || lane < rows;
-            long long left = a.n_cols;
-            for (int c = 0; c < n_chunks; ++c) {
-                mbar_wait(&empty_bar[s], empty_parity); // the consumers are done with the stage's previous use
-                const uint32_t bytes = (uint32_t)(min((long long)kStreamCols, left) * 8);
-                unsigned char *dst = st_smem + s * kStreamStageBytes + lane * kStreamRowBytes;
-                if (lane == 0) {
-                    meta[s] = make_int2((int)group, c);
-                    mbar_arrive_expect_tx(&full_bar[s], bytes * (rows + 1));
-                }
-                if (active) {
-#if SKB_STREAM_HINT
-                    if (lane < kStreamRows)
-                        tma_bulk_g2s_hint(dst, src, bytes, &full_bar[s], policy);
-                    else
-#endif
-                        tma_bulk_g2s(dst, src, bytes, &full_bar[s]);
-                }
-                src += kStreamCols;
-                left -= kStreamCols;
-                if (++s == kStreamStages) {
-                    s = 0;
-                    empty_parity ^= 1u;
-                }
-            }
-            group = (long long)gridDim.x + (long long)__shfl_sync(kMask, ticket, 0);
-        }
-    }
-
-    // ---- consumers ----
-    double acc[kStreamRows];
-#pragma unroll
-    for (int i = 0; i < kStreamRows; ++i)
-        acc[i] = 0.0;
-    const int n_pairs_last = (int)((a.n_cols - (long long)(n_chunks - 1) * kStreamCols) >> 1); // pairs of the last chunk
-    int s = 0;
-    uint32_t full_parity = 0;
-    for (;; s = (s + 1 == kStreamStages) ? 0 : s + 1, full_parity ^= (s == 0)) {
-        mbar_wait(&full_bar[s], full_parity);
-        const int2 m = meta[s];
-        if (m.x < 0)
-            break;
-        const int n_pairs = m.y == n_chunks - 1 ? n_pairs_last : kStreamCols / 2;
-        const unsigned char *stage = st_smem + s * kStreamStageBytes;
-        // thread t owns the column pairs t and 64 + t of the chunk: consecutive lanes read consecutive 16-byte words
-#pragma unroll
-        for (int h = 0; h < kStreamCols / 2 / kStreamConsumers; ++h) {
-            const int p = h * kStreamConsumers + t;
-            if (p < n_pairs) {
-                const double2 xv = *reinterpret_cast<const double2 *>(stage + kStreamRows * kStreamRowBytes + p * 16);
-#pragma unroll
-                for (int i = 0; i < kStreamRows; ++i) {
-                    // (rows beyond n_rows of the last group hold stale ring data: their sums are never stored)
-                    const double2 av = *reinterpret_cast<const double2 *>(stage + i * kStreamRowBytes + p * 16);
-                    acc[i] = fma(av.x, xv.x, acc[i]);
-                    acc[i] = fma(av.y, xv.y, acc[i]);
-                }
-            }
-        }
-        __syncwarp();
-        if ((t & 31) == 0)
-            mbar_arrive(&empty_bar[s]); // this warp is done with the stage
-        if (m.y == n_chunks - 1) { // the group is complete: fixed tree over the 64 consumer threads
-#pragma unroll
-            for (int i = 0; i < kStreamRows; ++i) {
-                double v = acc[i];
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1)
-                    v += __shfl_xor_sync(0xffffffffu, v, o);
-                if ((t & 31) == 0)
-                    red[(t >> 5) * kStreamRows + i] = v;
-                acc[i] = 0.0;
-            }
-            asm volatile("bar.sync 1, %0;" ::"n"(kStreamConsumers) : "memory");
-            const long long row = (long long)m.x * kStreamRows + t;
-            if (t < kStreamRows && row < a.n_rows)
-                a.y[row] = red[t] + red[kStreamRows + t];
-            asm volatile("bar.sync 1, %0;" ::"n"(kStreamConsumers) : "memory"); // red is free again
-        }
-    }
-}
+// defined in skb_dense.cu, the one translation unit that launches it (prepare_device in skb_runtime.cu sets its
+// attributes)
+__global__ void __maxnreg__(kStreamMaxNReg) dense_stream_kernel(const StreamArgs a);
 
 } // namespace skb

@@ -25,26 +25,10 @@
 
 namespace skb {
 
-#ifndef SKB_SYM_T
-#define SKB_SYM_T 8 // nodes of the I block per thread (tuning knob)
-#endif
-#ifndef SKB_SYM_MINB
-#define SKB_SYM_MINB 2 // resident CTAs per SM asked of ptxas (register cap 65536 / (128 * MINB))
-#endif
-#ifndef SKB_SYM_UNROLL
-#define SKB_SYM_UNROLL 1 // ring steps unrolled
-#endif
-#ifndef SKB_SYM_PREFETCH
-#define SKB_SYM_PREFETCH 1 // 1: the next step's record is loaded from shared memory before this step's chain
-#endif
 constexpr int kSymThreads = 128;
-constexpr int kSymT = SKB_SYM_T;
-constexpr int kSymMinB = SKB_SYM_MINB;
-constexpr int kSymUnroll = SKB_SYM_UNROLL;
-#ifndef SKB_SYM_STAGES
-#define SKB_SYM_STAGES 4 // TMA ring depth (a stage is 6 KB)
-#endif
-constexpr int kSymStages = SKB_SYM_STAGES;
+constexpr int kSymT = 8;            // nodes of the I block per thread
+constexpr int kSymMinB = 2;         // resident CTAs per SM
+constexpr int kSymStages = 4;       // TMA ring depth (a stage is 6 KB)
 constexpr int kSymPrefetch = kSymStages > 2 ? 2 : 1; // stages in flight ahead of the one being consumed
 constexpr int kSymGroup = 32;       // nodes per J group (one ring)
 constexpr int kSymStageGroups = 4;  // groups per stage
@@ -177,18 +161,13 @@ __device__ __forceinline__ void stokeslet_pairpairs(const double (&tx)[T], const
     }
 }
 
-// SKB_SYM_MAXNREG caps the registers per thread below what (kSymThreads, MINB) allows: at 240 the two resident CTAs
-// leave 4 096 registers of the SM free -- room for the 64-thread CTA of the background row streamer (stream_kernels.cuh).
-#ifndef SKB_SYM_MAXNREG
-#define SKB_SYM_MAXNREG 240
-#endif
-#if SKB_SYM_MAXNREG > 0
-#define SKB_SYM_BOUNDS __maxnreg__(SKB_SYM_MAXNREG)
-#else
-#define SKB_SYM_BOUNDS __launch_bounds__(kSymThreads, MINB)
-#endif
+// The register cap is below the 256 that (kSymThreads, kSymMinB) allows: at 240 the two resident CTAs leave 1 024
+// registers free in each of the SM's four sub-partitions -- room for the CTA of the background row streamer
+// (stream_kernels.cuh), three warps of 32 registers.  (MINB, the residency the cap is chosen for, is not read here.)
+constexpr int kSymMaxNReg = 240;
 template <int T, int MINB, bool EXCL = false>
-__global__ void SKB_SYM_BOUNDS pair_sym_kernel(const SymArgs a) {
+__global__ void __maxnreg__(kSymMaxNReg) pair_sym_kernel(const SymArgs a) {
+    static_assert(T % 4 == 0, "the pair chains run in groups of 4");
     using L = SymSmem<T>;
     constexpr int kBlock = L::block;
     constexpr int kWarps = kSymThreads / 32;
@@ -261,7 +240,8 @@ __global__ void SKB_SYM_BOUNDS pair_sym_kernel(const SymArgs a) {
             constexpr bool REV = decltype(rev_tag)::value;
             const int base = gi * kSymGroup;
             double urx = 0.0, ury = 0.0, urz = 0.0;
-#if SKB_SYM_PREFETCH
+            // the next step's record is loaded from shared memory before this step's chain (24 B stride: bank-conflict
+            // free for 64-bit loads)
             double nrx, nry, nrz, ngx, ngy, ngz;
             int nid = 0;
             {
@@ -271,10 +251,8 @@ __global__ void SKB_SYM_BOUNDS pair_sym_kernel(const SymArgs a) {
                 if constexpr (EXCL)
                     nid = ids[idx];
             }
-#endif
-            _Pragma("unroll kSymUnroll")
+#pragma unroll 1
             for (int st = 0; st < 32; ++st) {
-#if SKB_SYM_PREFETCH
                 const double rx = nrx, ry = nry, rz = nrz, gx = ngx, gy = ngy, gz = ngz;
                 const int rid = nid;
                 {
@@ -284,34 +262,23 @@ __global__ void SKB_SYM_BOUNDS pair_sym_kernel(const SymArgs a) {
                     if constexpr (EXCL)
                         nid = ids[idx];
                 }
-#else
-                const int idx = base + ((lane + st) & 31);
-                // per-lane record from shared memory: 24 B stride is bank-conflict free for 64-bit loads
-                const double rx = ps[3 * idx + 0], ry = ps[3 * idx + 1], rz = ps[3 * idx + 2];
-                const double gx = fs[3 * idx + 0], gy = fs[3 * idx + 1], gz = fs[3 * idx + 2];
-                const int rid = EXCL ? ids[idx] : 0;
-#endif
-                if constexpr (T <= 4) {
-                    stokeslet_pairpairs<T, EXCL, REV>(tx, ty, tz, hx, hy, hz, rx, ry, rz, gx, gy, gz, ufx, ufy, ufz, urx,
-                                                      ury, urz, tfid, rid);
-                } else { // chains in groups of 4: bounds the live temporaries
+                // chains in groups of 4: bounds the live temporaries
 #pragma unroll
-                    for (int g0 = 0; g0 < T; g0 += 4) {
-                        double ax[4], ay[4], az[4], bx[4], by[4], bz[4], cx[4], cy[4], cz[4];
-                        int ti[4];
+                for (int g0 = 0; g0 < T; g0 += 4) {
+                    double ax[4], ay[4], az[4], bx[4], by[4], bz[4], cx[4], cy[4], cz[4];
+                    int ti[4];
 #pragma unroll
-                        for (int c = 0; c < 4; ++c) {
-                            ti[c] = tfid[g0 + c];
-                            ax[c] = tx[g0 + c], ay[c] = ty[g0 + c], az[c] = tz[g0 + c];
-                            bx[c] = hx[g0 + c], by[c] = hy[g0 + c], bz[c] = hz[g0 + c];
-                            cx[c] = ufx[g0 + c], cy[c] = ufy[g0 + c], cz[c] = ufz[g0 + c];
-                        }
-                        stokeslet_pairpairs<4, EXCL, REV>(ax, ay, az, bx, by, bz, rx, ry, rz, gx, gy, gz, cx, cy, cz, urx,
-                                                          ury, urz, ti, rid);
-#pragma unroll
-                        for (int c = 0; c < 4; ++c)
-                            ufx[g0 + c] = cx[c], ufy[g0 + c] = cy[c], ufz[g0 + c] = cz[c];
+                    for (int c = 0; c < 4; ++c) {
+                        ti[c] = tfid[g0 + c];
+                        ax[c] = tx[g0 + c], ay[c] = ty[g0 + c], az[c] = tz[g0 + c];
+                        bx[c] = hx[g0 + c], by[c] = hy[g0 + c], bz[c] = hz[g0 + c];
+                        cx[c] = ufx[g0 + c], cy[c] = ufy[g0 + c], cz[c] = ufz[g0 + c];
                     }
+                    stokeslet_pairpairs<4, EXCL, REV>(ax, ay, az, bx, by, bz, rx, ry, rz, gx, gy, gz, cx, cy, cz, urx, ury,
+                                                      urz, ti, rid);
+#pragma unroll
+                    for (int c = 0; c < 4; ++c)
+                        ufx[g0 + c] = cx[c], ufy[g0 + c] = cy[c], ufz[g0 + c] = cz[c];
                 }
                 if constexpr (REV) {
                     // the record moves to lane - 1 for the next step; its accumulator goes with it
