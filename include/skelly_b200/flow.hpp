@@ -140,6 +140,35 @@ template <class M> class FlowEngineT {
         }
         check(skb_flow_set_fiber_preconditioner(st_->fl, a.data()), "skb_flow_set_fiber_preconditioner");
     }
+    /// FiberFiniteDifference::matrices_.at(n_nodes): D_2_0, D_3_0, D_4_0 (n x n each, pre-transposed like D_1_0,
+    /// ffd.cpp:537-540); build_fiber_operators needs them, and set_fiber_class, for every node count in use
+    void set_fiber_class_derivatives(int n_nodes, const M &D_2_0, const M &D_3_0, const M &D_4_0) {
+        check(skb_flow_set_fiber_class_derivatives(st_->fl, n_nodes, D_2_0.data(), D_3_0.data(), D_4_0.data()),
+              "skb_flow_set_fiber_class_derivatives");
+    }
+    /// Once per timestep after set_fibers, instead of set_fiber_operators + set_fiber_preconditioner: A_,
+    /// force_operator_, xs_ and A_^-1 of every fiber built on the device from the positions and lengths of set_fibers
+    /// (update_derivatives, update_linear_operator, update_force_operator, apply_bc_rectangular's operator half,
+    /// update_preconditioner); one skb_fiber_params per fiber
+    void build_fiber_operators(const std::vector<skb_fiber_params> &params, double dt, double eta) {
+        if (params.size() != st_->n_nodes.size())
+            throw std::runtime_error("skelly_b200: build_fiber_operators needs one entry per fiber of set_fibers");
+        check(skb_flow_build_fiber_operators(st_->fl, params.data(), dt, eta), "skb_flow_build_fiber_operators");
+    }
+    /// The resident operators back, in set_fiber_operators' layouts: A / A_inv the concatenated column-major 4n x 4n
+    /// matrices, force_operator the 3n x 4n ones, xs 3 x N_f
+    void get_fiber_operators(std::vector<double> &A, std::vector<double> &force_operator, M &xs,
+                             std::vector<double> &A_inv) const {
+        size_t na = 0;
+        for (int n : st_->n_nodes)
+            na += (size_t)16 * n * n;
+        A.assign(na, 0.0);
+        force_operator.assign(na / 4 * 3, 0.0);
+        A_inv.assign(na, 0.0);
+        xs = M::Zero(3, st_->n_fib);
+        check(skb_flow_get_fiber_operators(st_->fl, A.data(), force_operator.data(), xs.data(), A_inv.data()),
+              "skb_flow_get_fiber_operators");
+    }
     /// FiberContainerFiniteDifference::apply_preconditioner (fcfd.cpp:331-339): y = A_^-1 x per fiber
     M apply_fiber_preconditioner(const M &x_fibers) const {
         M y = M::Zero(4 * st_->n_fib, 1);

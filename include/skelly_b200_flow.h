@@ -197,6 +197,49 @@ SKB_API int skb_flow_apply_fiber_preconditioner(skb_flow *fl, const double *x_fi
 SKB_API int skb_flow_apply_fiber_preconditioner_device(skb_flow *fl, const double *d_x_fibers, double *d_y,
                                                        void *stream);
 
+/* ---- the per-fiber operators built on the device ------------------------------------------------------------
+ * What FiberContainerFiniteDifference::update_cache_variables and ::apply_bc_rectangular (fcfd.cpp:147-157,
+ * 261-269) do per fiber on the host before every solve -- update_derivatives (fiber_finite_difference.cpp:62-68),
+ * update_linear_operator (:97-187), update_force_operator (:317-335), the operator half of apply_bc_rectangular
+ * (`A_ = P_downsample_bc * A_` plus the 14 boundary rows, :347-512) and update_preconditioner (`A_LU_.compute(A_)`,
+ * :340) -- from the positions and lengths of the last skb_flow_set_fibers and a few scalars per fiber, instead of
+ * uploading A_, force_operator_ and A_^-1 (about 1 GB per timestep at 3000 fibers x 32 nodes).  The RHS (update_RHS
+ * and the RHS half of apply_bc_rectangular) stays with the caller.
+ *
+ * skb_flow_set_fiber_class_derivatives: the higher derivative matrices of FiberFiniteDifference::matrices_.at(n)
+ *   (:537-540), stored pre-transposed exactly like the reference (column-major n x n each).  The build needs them,
+ *   and skb_flow_set_fiber_class, for every node count in use. */
+SKB_API int skb_flow_set_fiber_class_derivatives(skb_flow *fl, int n_nodes, const double *D_2_0,
+                                                 const double *D_3_0, const double *D_4_0);
+
+typedef struct skb_fiber_params {   /* one per fiber, 48 bytes */
+    double length_prev;             /* length_prev_  (derivatives and fc.matvec)              */
+    double bending_rigidity;        /* bending_rigidity_                                      */
+    double radius;                  /* radius_ -> epsilon_ = radius_/length_ (hpp:140-144)    */
+    double penalty_param;           /* penalty_param_                                         */
+    double beta_tstep;              /* beta_tstep_                                            */
+    int32_t minus_clamped;          /* bc_minus_ = (Velocity, AngularVelocity), else (Force, Torque) */
+    int32_t plus_hinged;            /* bc_plus_  = (Velocity, Torque),          else (Force, Torque) */
+} skb_fiber_params;
+
+/* update_derivatives + update_linear_operator + update_force_operator + the operator part of apply_bc_rectangular +
+ * update_preconditioner, for every fiber of this flow, on the device, from the positions and lengths of the last
+ * skb_flow_set_fibers.  Leaves exactly the state skb_flow_set_fiber_operators followed by
+ * skb_flow_set_fiber_preconditioner leaves (A_, force_operator_, xs_, length_prev, plus flag, A_^-1); either call
+ * replaces what the other left.  Under skb_flow_set_target_ranges (or a window that cuts no fiber) it builds the own
+ * fibers only and `params` holds the own fibers.  Refused (SKB_ERR_INVALID, before any launch): a node count without
+ * skb_flow_set_fiber_class or skb_flow_set_fiber_class_derivatives, n < 8 (the D_4 stencil has 8 points) or n > 128,
+ * a flag outside {0, 1}, a non-positive length_prev, radius, dt or eta.
+ * The inverse is Gauss-Jordan elimination with partial pivoting (Eigen's PartialPivLU does not detect a singular A_
+ * either, and neither does this): a STRAIGHT fiber that is both clamped at the minus end and hinged at the plus end has
+ * a singular A_ (condition number ~1e18 for every n), and its inverse is meaningless.
+ * skb_flow_last_stats afterwards: device_ms = the build's kernels, total_ms = with the upload of its per-fiber tables. */
+SKB_API int skb_flow_build_fiber_operators(skb_flow *fl, const skb_fiber_params *params, double dt, double eta);
+
+/* read the resident operators back, same layouts as skb_flow_set_fiber_operators / _preconditioner (own fibers);
+ * NULL skips an array */
+SKB_API int skb_flow_get_fiber_operators(skb_flow *fl, double *A, double *force_operator, double *xs, double *A_inv);
+
 /* System::apply_matvec (system.cpp:269-324) with the fiber operators on the device:
  *   fw = apply_fiber_force(x_fibers); v_all = the fused flow of skb_flow_matvec;
  *   res_fibers = fc.matvec(x_fibers, v_fibers, fiber_link_conditions)
@@ -271,6 +314,10 @@ SKB_API int skb_mflow_set_fiber_class(skb_mflow *mf, int n_nodes, const double *
 SKB_API int skb_mflow_set_fiber_operators(skb_mflow *mf, const double *A, const double *force_operator,
                                           const double *xs, const double *length_prev, const int *plus_bc_velocity);
 SKB_API int skb_mflow_set_fiber_preconditioner(skb_mflow *mf, const double *A_inv);
+SKB_API int skb_mflow_set_fiber_class_derivatives(skb_mflow *mf, int n_nodes, const double *D_2_0,
+                                                  const double *D_3_0, const double *D_4_0);
+/* params of ALL fibers; every member builds its own slice on its own device, in parallel */
+SKB_API int skb_mflow_build_fiber_operators(skb_mflow *mf, const skb_fiber_params *params, double dt, double eta);
 /* op = skb_dense_op (skelly_b200_dense.h); A row-major (3 N_s) x (3 N_s) */
 SKB_API int skb_mflow_set_dense(skb_mflow *mf, int op, const double *A_rowmajor, int64_t n_rows, int64_t n_cols);
 SKB_API int skb_mflow_matvec(skb_mflow *mf, const double *fib_forces, const double *shell_density,

@@ -39,6 +39,17 @@ class DenseStats(C.Structure):
     _fields_ = [("kernel_ms", C.c_double), ("total_ms", C.c_double), ("bytes", C.c_int64)]
 
 
+class FiberParams(C.Structure):
+    """skb_fiber_params (include/skelly_b200_flow.h): the per-fiber scalars of skb_flow_build_fiber_operators."""
+    _fields_ = [("length_prev", C.c_double), ("bending_rigidity", C.c_double), ("radius", C.c_double),
+                ("penalty_param", C.c_double), ("beta_tstep", C.c_double), ("minus_clamped", C.c_int32),
+                ("plus_hinged", C.c_int32)]
+
+
+# the same record as a numpy dtype: a whole container's parameters are filled column by column
+FIBER_PARAMS_DTYPE = np.dtype([(name, np.float64 if ct is C.c_double else np.int32) for name, ct in FiberParams._fields_])
+
+
 def library_path() -> str:
     return _LIB
 
@@ -142,6 +153,8 @@ def library() -> C.CDLL:
         "skb_mflow_set_fiber_class": ([ctxp, C.c_int, _dp, _dp], C.c_int),
         "skb_mflow_set_fiber_operators": ([ctxp, _dp, _dp, _dp, _dp, C.POINTER(C.c_int)], C.c_int),
         "skb_mflow_set_fiber_preconditioner": ([ctxp, _dp], C.c_int),
+        "skb_mflow_set_fiber_class_derivatives": ([ctxp, C.c_int, _dp, _dp, _dp], C.c_int),
+        "skb_mflow_build_fiber_operators": ([ctxp, C.POINTER(FiberParams), C.c_double, C.c_double], C.c_int),
         "skb_mflow_set_dense": ([ctxp, C.c_int, _dp, C.c_int64, C.c_int64], C.c_int),
         "skb_mflow_matvec": ([ctxp, _dp, _dp, _dp, _dp, C.c_double, _dp], C.c_int),
         "skb_mflow_apply_matvec": ([ctxp, _dp, _dp, _dp, _dp, _dp, C.c_double, _dp, _dp, _dp], C.c_int),
@@ -157,6 +170,9 @@ def library() -> C.CDLL:
         "skb_flow_apply_fiber_preconditioner": ([ctxp, _dp, _dp], C.c_int),
         "skb_flow_apply_fiber_preconditioner_device": ([ctxp, C.c_void_p, C.c_void_p, C.c_void_p], C.c_int),
         "skb_flow_fiber_matvec": ([ctxp, _dp, _dp, _dp, _dp], C.c_int),
+        "skb_flow_set_fiber_class_derivatives": ([ctxp, C.c_int, _dp, _dp, _dp], C.c_int),
+        "skb_flow_build_fiber_operators": ([ctxp, C.POINTER(FiberParams), C.c_double, C.c_double], C.c_int),
+        "skb_flow_get_fiber_operators": ([ctxp, _dp, _dp, _dp, _dp], C.c_int),
         "skb_flow_apply_matvec": ([ctxp, _dp, _dp, _dp, _dp, _dp, C.c_double, _dp, _dp, _dp], C.c_int),
         "skb_flow_apply_matvec_dense": ([ctxp, ctxp, _dp, _dp, _dp, _dp, _dp, C.c_double, _dp, _dp, _dp], C.c_int),
         "skb_dense_apply_device": ([ctxp, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p], C.c_int),
@@ -197,6 +213,31 @@ def _arr(x, cols):
 
 def _p(x):
     return x.ctypes.data_as(_dp)
+
+
+def _class_derivatives(n_nodes, D_2_0, D_3_0, D_4_0):
+    n = int(n_nodes)
+    Ds = [np.asfortranarray(D, dtype=np.float64) for D in (D_2_0, D_3_0, D_4_0)]
+    if any(D.shape != (n, n) for D in Ds):
+        raise ValueError(f"derivative matrices for n={n}: got {[D.shape for D in Ds]}")
+    return n, Ds
+
+
+def fiber_params(n_fibers, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
+                 plus_hinged):
+    """skb_fiber_params of n_fibers fibers; every argument is a per-fiber array or a scalar for all of them."""
+    p = np.zeros(int(n_fibers), dtype=FIBER_PARAMS_DTYPE)
+    for name, v in zip(FIBER_PARAMS_DTYPE.names, (length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
+                                                   minus_clamped, plus_hinged)):
+        v = np.asarray(v)
+        if v.ndim and v.shape != (int(n_fibers),):
+            raise ValueError(f"{name}: expected a scalar or {int(n_fibers)} values, got shape {v.shape}")
+        p[name] = v
+    return p
+
+
+def _params_ptr(p):
+    return p.ctypes.data_as(C.POINTER(FiberParams)) if p.size else None
 
 
 def device_count() -> int:
@@ -557,6 +598,54 @@ class Flow:
         Ai = self._colmajor_concat(A_inv_list)
         _check(library().skb_flow_set_fiber_preconditioner(self._h, _p(Ai)))
 
+    def set_fiber_class_derivatives(self, n_nodes: int, D_2_0, D_3_0, D_4_0):
+        """The higher derivative matrices of FiberFiniteDifference::matrices_.at(n) (pre-transposed like D_1_0), needed
+        by build_fiber_operators for every node count in use."""
+        n, (D2, D3, D4) = _class_derivatives(n_nodes, D_2_0, D_3_0, D_4_0)
+        _check(library().skb_flow_set_fiber_class_derivatives(self._h, n, _p(D2), _p(D3), _p(D4)))
+
+    def _own_fibers(self):
+        """(first, end) fiber of the current window / ranges (all fibers without either)."""
+        off = getattr(self, "_fiber_off", np.zeros(1, dtype=np.int64))
+        nfib = len(off) - 1
+        if getattr(self, "_ranges", None):
+            f0 = min(max(self._ranges[0], 0), nfib)
+            return f0, min(max(self._ranges[1], f0), nfib)
+        w0, w1 = getattr(self, "_window", None) or (0, -1)
+        nf = int(off[-1])
+        w0 = min(max(w0, 0), nf)
+        w1 = nf if w1 < 0 else min(max(w1, w0), nf)
+        return int(np.searchsorted(off, w0)), int(np.searchsorted(off, w1))
+
+    def build_fiber_operators(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
+                              plus_hinged, dt, eta):
+        """A_, force_operator_, xs_ and A_^-1 of the (own) fibers built on the device from the positions and lengths of
+        set_fibers (update_derivatives, update_linear_operator, update_force_operator, the operator half of
+        apply_bc_rectangular, update_preconditioner).  Per-fiber arrays or scalars; the flags are 0 / 1."""
+        f0, f1 = self._own_fibers()
+        p = fiber_params(f1 - f0, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
+                         plus_hinged)
+        _check(library().skb_flow_build_fiber_operators(self._h, _params_ptr(p), float(dt), float(eta)))
+
+    def get_fiber_operators(self, inverse=True):
+        """The resident operators of the (own) fibers: dict(A=[(4n,4n)], force=[(3n,4n)], xs=(N_own,3),
+        A_inv=[(4n,4n)] or None)."""
+        f0, f1 = self._own_fibers()
+        n_nodes = np.diff(getattr(self, "_fiber_off", np.zeros(1, dtype=np.int64)))[f0:f1].astype(int)
+        A = np.empty(int(np.sum(16 * n_nodes ** 2)))
+        F = np.empty(int(np.sum(12 * n_nodes ** 2)))
+        Ai = np.empty_like(A) if inverse else None
+        xs = np.empty((int(np.sum(n_nodes)), 3))
+        _check(library().skb_flow_get_fiber_operators(self._h, _p(A), _p(F), _p(xs), _p(Ai) if inverse else None))
+
+        def split(buf, rows):
+            out, o = [], 0
+            for n in n_nodes:
+                out.append(buf[o:o + rows * n * 4 * n].reshape(4 * n, rows * n).T)
+                o += rows * n * 4 * n
+            return out
+        return dict(A=split(A, 4), force=split(F, 3), xs=xs, A_inv=split(Ai, 4) if inverse else None)
+
     def apply_fiber_preconditioner(self, x_fibers):
         """fc.apply_preconditioner (fcfd.cpp:331-339): y = A_^-1 x per (own) fiber."""
         x = np.ascontiguousarray(x_fibers, dtype=np.float64).reshape(-1)
@@ -766,6 +855,17 @@ class MultiFlow:
     def set_fiber_preconditioner(self, A_inv_list):
         Ai = Flow._colmajor_concat(A_inv_list)
         _check(library().skb_mflow_set_fiber_preconditioner(self._h, _p(Ai)))
+
+    def set_fiber_class_derivatives(self, n_nodes: int, D_2_0, D_3_0, D_4_0):
+        n, (D2, D3, D4) = _class_derivatives(n_nodes, D_2_0, D_3_0, D_4_0)
+        _check(library().skb_mflow_set_fiber_class_derivatives(self._h, n, _p(D2), _p(D3), _p(D4)))
+
+    def build_fiber_operators(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
+                              plus_hinged, dt, eta):
+        """Flow.build_fiber_operators for ALL fibers; every device builds its own slice."""
+        p = fiber_params(self.n_fibers, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
+                         plus_hinged)
+        _check(library().skb_mflow_build_fiber_operators(self._h, _params_ptr(p), float(dt), float(eta)))
 
     def set_dense(self, op: int, A):
         A = np.ascontiguousarray(A, dtype=np.float64)

@@ -43,6 +43,8 @@ int upload_pageable(void *d_dst, const void *h_src, size_t bytes, cudaStream_t s
 // Takes device `dev` into use, once per device and process: rejects anything but compute capability 9.0 and loads the
 // kernels that need launch attributes, with those attributes set.  Makes `dev` current.
 int prepare_device(int dev);
+// the launch attributes of the kernels of fiber_build.cuh (skb_matvec.cu); called by prepare_device
+int prepare_fiber_build_kernels();
 DeviceInfo query_device(int dev); // (of a prepared device)
 LaunchPlan plan_launch(const DeviceInfo &di, int kind, long long n_trg, int n_src_tiles, int force_T, int force_S);
 int launch_pair_sum(const DeviceInfo &di, int kind, const double *d_r_src, const double *d_f_packed, long long n_src,

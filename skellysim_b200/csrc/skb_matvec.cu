@@ -3,6 +3,7 @@
 // (src/core/system.cpp:284-316).  Built on the pair-kernel contexts of skb_runtime.cu; everything between the
 // upload of the strengths and the download of the velocities stays on the device.
 #include "aux_kernels.cuh"
+#include "fiber_build.cuh"
 #include "fiber_ops.cuh"
 #include "group_kernels.cuh"
 #include "skb_internal.hpp"
@@ -113,6 +114,7 @@ struct skb_flow {
     std::vector<long long> h_fiber_off;
     struct FiberClass {
         std::vector<double> D, P; // D_1_0 (n x n), P_downsample_bc ((4n-14) x 4n), column-major
+        std::vector<double> D234; // D_2_0 | D_3_0 | D_4_0 (n x n each): skb_flow_set_fiber_class_derivatives
     };
     std::map<int, FiberClass> fiber_classes;
     bool ops_ready = false;
@@ -120,7 +122,9 @@ struct skb_flow {
     size_t gemv_smem = 0;
     DevBuf op_A, op_F, op_xs, op_len, op_plus, op_class, op_classD, op_classP, op_classR, op_ranges, items_A, items_F;
     DevBuf x_fib, res_fib, vb, res_shell, op_Ainv, tmp_b;
+    DevBuf bld_params, bld_items, bld_tiles, bld_inv; // skb_flow_build_fiber_operators (fiber_build.cuh)
     long long op_A_elems = 0;               // elements of the concatenated A_ (and of A_^-1)
+    long long op_F_elems = 0;               // ... of force_operator_
     unsigned long long ops_gen = 0, precond_gen = 0; // the preconditioner belongs to one set of operators
     // multi-GPU group (group_kernels.cuh): one member per GPU, exchange through peer memory
     struct Group {
@@ -499,7 +503,8 @@ int skb_flow_destroy(skb_flow *fl) {
     DevBuf *bufs[] = {&fl->fiber_offset, &fl->fiber_length, &fl->r_fib, &fl->r_shell, &fl->r_body, &fl->centers,
                       &fl->pt_pos, &fl->pt_force, &fl->pt_torque, &fl->in_fib, &fl->in_shell, &fl->in_body, &fl->in_force, &fl->in_torque, &fl->vel, &fl->tmp,
                       &fl->op_A, &fl->op_F, &fl->op_xs, &fl->op_len, &fl->op_plus, &fl->op_class, &fl->op_classD,
-                      &fl->op_classP, &fl->op_classR, &fl->op_ranges, &fl->items_A, &fl->items_F, &fl->x_fib, &fl->res_fib, &fl->vb, &fl->res_shell, &fl->op_Ainv, &fl->tmp_b};
+                      &fl->op_classP, &fl->op_classR, &fl->op_ranges, &fl->items_A, &fl->items_F, &fl->x_fib, &fl->res_fib, &fl->vb, &fl->res_shell, &fl->op_Ainv, &fl->tmp_b,
+                      &fl->bld_params, &fl->bld_items, &fl->bld_tiles, &fl->bld_inv};
     for (DevBuf *b : bufs)
         b->release();
     fl->g_matvec.reset();
@@ -1457,14 +1462,26 @@ int skb_flow_set_fiber_class(skb_flow *fl, int n_nodes, const double *D_1_0, con
     return SKB_OK;
 }
 
-int skb_flow_set_fiber_operators(skb_flow *fl, const double *A, const double *force_operator, const double *xs,
-                                 const double *length_prev, const int *plus_bc_velocity) {
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_operators: NULL flow");
-    fl->ops_ready = false;
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    // the resident operators are those of the fibers whose rows are in this flow's target list: all of them, or the
-    // rank's own fibers under skb_flow_set_target_ranges / an aligned skb_flow_set_target_window
+int skb_flow_set_fiber_class_derivatives(skb_flow *fl, int n_nodes, const double *D_2_0, const double *D_3_0,
+                                         const double *D_4_0) {
+    if (!fl || !D_2_0 || !D_3_0 || !D_4_0)
+        return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_class_derivatives: NULL argument");
+    if (n_nodes < kBuildMinNodes || n_nodes > kBuildMaxNodes)
+        return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_class_derivatives: n_nodes = %d (the device build takes "
+                                          "%d <= n <= %d)", n_nodes, kBuildMinNodes, kBuildMaxNodes);
+    const size_t nn = (size_t)n_nodes * n_nodes;
+    std::vector<double> &d = fl->fiber_classes[n_nodes].D234;
+    d.assign(D_2_0, D_2_0 + nn);
+    d.insert(d.end(), D_3_0, D_3_0 + nn);
+    d.insert(d.end(), D_4_0, D_4_0 + nn);
+    return SKB_OK;
+}
+
+} // extern "C"
+
+// The fibers whose operators are resident: those whose rows are in this flow's target list -- all of them, or the
+// rank's own fibers under skb_flow_set_target_ranges / an aligned skb_flow_set_target_window.
+static int own_fibers(skb_flow *fl, const char *who) {
     SKB_TRY(prepare_matvec_targets(fl));
     int f0 = 0, f1 = 0;
     if (fl->n_fibers > 0) {
@@ -1472,31 +1489,43 @@ int skb_flow_set_fiber_operators(skb_flow *fl, const double *A, const double *fo
         f0 = (int)(std::lower_bound(off.begin(), off.end(), fl->fa) - off.begin());
         f1 = (int)(std::lower_bound(off.begin(), off.end(), fl->fb) - off.begin());
         if (off[(size_t)f0] != fl->fa || off[(size_t)f1] != fl->fb)
-            return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_operators: the target window [%lld, %lld) cuts a "
-                                              "fiber; use skb_flow_set_target_ranges (whole fibers)", fl->fa, fl->fb);
+            return set_error(SKB_ERR_INVALID, "%s: the target window [%lld, %lld) cuts a fiber; use "
+                                              "skb_flow_set_target_ranges (whole fibers)", who, fl->fa, fl->fb);
     }
     fl->op_f0 = f0;
     fl->op_f1 = f1;
-    const int nfib = f1 - f0;
-    if (nfib == 0) {
-        fl->n_items_A = fl->n_items_F = 0;
-        fl->ops_ready = true;
-        return SKB_OK;
-    }
-    if (!A || !force_operator || !xs || !length_prev || !plus_bc_velocity)
-        return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_operators: NULL argument");
-    // class matrices -> one device buffer, per-fiber offsets into it; per class also the non-zero column range of every
-    // row of P_downsample_bc (block diagonal in the reference, ffd.cpp:551-555: the kernel walks the range only)
-    std::vector<double> h_class;
+    return SKB_OK;
+}
+
+// Where the resident operators of the own fibers live, shared by skb_flow_set_fiber_operators and
+// skb_flow_build_fiber_operators: the class matrices in one buffer, the non-zero column range of every row of
+// P_downsample_bc, the GEMV work items, and every fiber's offsets into A_ / force_operator_.
+struct FiberOpsPlan {
+    std::vector<double> h_class;              // per class: D_1_0 | P_downsample_bc [| D_2_0 | D_3_0 | D_4_0]
     std::vector<int2> h_ranges;
+    std::vector<long long> cD, cP, cR;        // per own fiber: its class's D_1_0, P, ranges
+    std::vector<long long> offA_f, offF_f;    // per own fiber: its A_ / force_operator_
+    std::vector<FiberGemvItem> itA, itF;
+    long long offA = 0, offF = 0;
+};
+
+// build: the operators are made on the device (class derivatives needed, n within the build's range);
+// length_prev: checked per fiber when given
+static int plan_fiber_operators(skb_flow *fl, bool build, const double *length_prev, FiberOpsPlan &pl) {
+    const int f0 = fl->op_f0, nfib = fl->op_f1 - fl->op_f0;
+    // class matrices -> one device buffer, per-fiber offsets into it; per class also the non-zero column range of every
+    // row of P_downsample_bc (block diagonal in the reference, ffd.cpp:551-555: the kernels walk the range only)
     std::map<int, std::pair<long long, long long>> class_off;
     std::map<int, long long> range_off;
     for (const auto &kv : fl->fiber_classes) {
-        class_off[kv.first] = {(long long)h_class.size(), (long long)(h_class.size() + kv.second.D.size())};
-        h_class.insert(h_class.end(), kv.second.D.begin(), kv.second.D.end());
-        h_class.insert(h_class.end(), kv.second.P.begin(), kv.second.P.end());
+        if (kv.second.D.empty()) // only skb_flow_set_fiber_class_derivatives was called for this n
+            continue;
+        class_off[kv.first] = {(long long)pl.h_class.size(), (long long)(pl.h_class.size() + kv.second.D.size())};
+        pl.h_class.insert(pl.h_class.end(), kv.second.D.begin(), kv.second.D.end());
+        pl.h_class.insert(pl.h_class.end(), kv.second.P.begin(), kv.second.P.end());
+        pl.h_class.insert(pl.h_class.end(), kv.second.D234.begin(), kv.second.D234.end());
         const int nn = kv.first, bc = 4 * nn - 14;
-        range_off[nn] = (long long)h_ranges.size();
+        range_off[nn] = (long long)pl.h_ranges.size();
         for (int r = 0; r < bc; ++r) {
             int c0 = 4 * nn, c1 = 0;
             for (int c = 0; c < 4 * nn; ++c)
@@ -1504,7 +1533,7 @@ int skb_flow_set_fiber_operators(skb_flow *fl, const double *A, const double *fo
                     c0 = std::min(c0, c);
                     c1 = c + 1;
                 }
-            h_ranges.push_back(c1 > c0 ? make_int2(c0, c1) : make_int2(0, 0));
+            pl.h_ranges.push_back(c1 > c0 ? make_int2(c0, c1) : make_int2(0, 0));
         }
         for (int j = 0; j < nn; ++j) { // D_1_0 (n x n, column-major): non-zero row range of every column (banded)
             int i0 = nn, i1 = 0;
@@ -1513,12 +1542,11 @@ int skb_flow_set_fiber_operators(skb_flow *fl, const double *A, const double *fo
                     i0 = std::min(i0, i);
                     i1 = i + 1;
                 }
-            h_ranges.push_back(i1 > i0 ? make_int2(i0, i1) : make_int2(0, 0));
+            pl.h_ranges.push_back(i1 > i0 ? make_int2(i0, i1) : make_int2(0, 0));
         }
     }
-    std::vector<long long> cD((size_t)nfib), cP((size_t)nfib), cR((size_t)nfib);
-    std::vector<FiberGemvItem> itA, itF;
-    long long offA = 0, offF = 0;
+    pl.cD.resize((size_t)nfib), pl.cP.resize((size_t)nfib), pl.cR.resize((size_t)nfib);
+    pl.offA_f.resize((size_t)nfib), pl.offF_f.resize((size_t)nfib);
     int max_n = 0;
     const long long node0 = fl->h_fiber_off[(size_t)f0]; // x / fw / v / res of the own fibers are indexed from here
     for (int f = 0; f < nfib; ++f) {
@@ -1527,19 +1555,27 @@ int skb_flow_set_fiber_operators(skb_flow *fl, const double *A, const double *fo
         if (it == class_off.end())
             return set_error(SKB_ERR_INVALID, "fiber %d has %d nodes but skb_flow_set_fiber_class(%d, ...) was never "
                                               "called", f0 + f, n, n);
-        if (!(length_prev[f] > 0))
+        if (build && (n < kBuildMinNodes || n > kBuildMaxNodes))
+            return set_error(SKB_ERR_INVALID, "fiber %d has %d nodes: the device build takes %d <= n <= %d", f0 + f, n,
+                             kBuildMinNodes, kBuildMaxNodes);
+        if (build && fl->fiber_classes[n].D234.empty())
+            return set_error(SKB_ERR_INVALID, "fiber %d has %d nodes but skb_flow_set_fiber_class_derivatives(%d, ...) "
+                                              "was never called", f0 + f, n, n);
+        if (length_prev && !(length_prev[f] > 0))
             return set_error(SKB_ERR_INVALID, "fiber %d: length_prev = %g", f0 + f, length_prev[f]);
-        cD[f] = it->second.first;
-        cP[f] = it->second.second;
-        cR[f] = range_off[n];
+        pl.cD[f] = it->second.first;
+        pl.cP[f] = it->second.second;
+        pl.cR[f] = range_off[n];
+        pl.offA_f[f] = pl.offA;
+        pl.offF_f[f] = pl.offF;
         max_n = std::max(max_n, n);
         const long long node_off = fl->h_fiber_off[(size_t)(f0 + f)] - node0;
         for (int r0 = 0; r0 < 4 * n; r0 += kFiberGemvRows)
-            itA.push_back(FiberGemvItem{offA, 4 * node_off, 4 * node_off, 4 * n, 4 * n, r0, n, f, 0});
+            pl.itA.push_back(FiberGemvItem{pl.offA, 4 * node_off, 4 * node_off, 4 * n, 4 * n, r0, n, f, 0});
         for (int r0 = 0; r0 < 3 * n; r0 += kFiberGemvRows)
-            itF.push_back(FiberGemvItem{offF, 4 * node_off, node_off, 3 * n, 4 * n, r0, n, f, 0});
-        offA += 16LL * n * n;
-        offF += 12LL * n * n;
+            pl.itF.push_back(FiberGemvItem{pl.offF, 4 * node_off, node_off, 3 * n, 4 * n, r0, n, f, 0});
+        pl.offA += 16LL * n * n;
+        pl.offF += 12LL * n * n;
     }
     // x (4n) + slice partials + vT (4n) + s (n)
     fl->gemv_smem = ((size_t)2 * ((4 * max_n + 1) & ~1) + kFiberGemvThreads + (size_t)max_n) * sizeof(double);
@@ -1553,35 +1589,73 @@ int skb_flow_set_fiber_operators(skb_flow *fl, const double *A, const double *fo
         CUDA_TRY(cudaFuncSetAttribute(fiber_gemv_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       (int)fl->gemv_smem));
     }
+    return SKB_OK;
+}
+
+static int put_async(skb_flow *fl, DevBuf &b, const void *h, size_t bytes) {
+    SKB_TRY(b.ensure(bytes));
+    CUDA_TRY(cudaMemcpyAsync(b.ptr, h, bytes, cudaMemcpyHostToDevice, fl->stream));
+    return SKB_OK;
+}
+
+// the plan's buffers on the device and room for the operators and the per-call vectors (on fl->stream; the caller
+// synchronises before `pl` goes out of scope)
+static int upload_fiber_plan(skb_flow *fl, const FiberOpsPlan &pl) {
     const long long nf = fl->fb - fl->fa; // nodes of the own fibers
-    auto put = [&](DevBuf &b, const void *h, size_t bytes) -> int {
-        SKB_TRY(b.ensure(bytes));
-        CUDA_TRY(cudaMemcpyAsync(b.ptr, h, bytes, cudaMemcpyHostToDevice, fl->stream));
-        return SKB_OK;
-    };
-    SKB_TRY(fl->op_A.ensure((size_t)offA * 8));
-    SKB_TRY(fl->op_F.ensure((size_t)offF * 8));
-    SKB_TRY(upload_pageable(fl->op_A.ptr, A, (size_t)offA * 8, fl->stream));
-    SKB_TRY(upload_pageable(fl->op_F.ptr, force_operator, (size_t)offF * 8, fl->stream));
-    SKB_TRY(put(fl->op_xs, xs, (size_t)nf * 24));
-    SKB_TRY(put(fl->op_len, length_prev, (size_t)nfib * 8));
-    SKB_TRY(put(fl->op_plus, plus_bc_velocity, (size_t)nfib * sizeof(int)));
-    SKB_TRY(put(fl->op_class, h_class.data(), h_class.size() * 8));
-    SKB_TRY(put(fl->op_classD, cD.data(), cD.size() * 8));
-    SKB_TRY(put(fl->op_classP, cP.data(), cP.size() * 8));
-    SKB_TRY(put(fl->op_classR, cR.data(), cR.size() * 8));
-    SKB_TRY(put(fl->op_ranges, h_ranges.data(), h_ranges.size() * sizeof(int2)));
-    SKB_TRY(put(fl->items_A, itA.data(), itA.size() * sizeof(FiberGemvItem)));
-    SKB_TRY(put(fl->items_F, itF.data(), itF.size() * sizeof(FiberGemvItem)));
+    const int nfib = fl->op_f1 - fl->op_f0;
+    SKB_TRY(fl->op_A.ensure((size_t)pl.offA * 8));
+    SKB_TRY(fl->op_F.ensure((size_t)pl.offF * 8));
+    SKB_TRY(fl->op_xs.ensure((size_t)nf * 24));
+    SKB_TRY(put_async(fl, fl->op_class, pl.h_class.data(), pl.h_class.size() * 8));
+    SKB_TRY(put_async(fl, fl->op_classD, pl.cD.data(), pl.cD.size() * 8));
+    SKB_TRY(put_async(fl, fl->op_classP, pl.cP.data(), pl.cP.size() * 8));
+    SKB_TRY(put_async(fl, fl->op_classR, pl.cR.data(), pl.cR.size() * 8));
+    SKB_TRY(put_async(fl, fl->op_ranges, pl.h_ranges.data(), pl.h_ranges.size() * sizeof(int2)));
+    SKB_TRY(put_async(fl, fl->items_A, pl.itA.data(), pl.itA.size() * sizeof(FiberGemvItem)));
+    SKB_TRY(put_async(fl, fl->items_F, pl.itF.data(), pl.itF.size() * sizeof(FiberGemvItem)));
     SKB_TRY(fl->x_fib.ensure((size_t)nf * 32));
     SKB_TRY(fl->res_fib.ensure((size_t)nf * 32));
     SKB_TRY(fl->vb.ensure((size_t)nfib * 56));
-    CUDA_TRY(cudaStreamSynchronize(fl->stream)); // the host vectors above go out of scope
-    fl->n_items_A = (int)itA.size();
-    fl->n_items_F = (int)itF.size();
-    fl->op_A_elems = offA;
+    return SKB_OK;
+}
+
+static void commit_fiber_plan(skb_flow *fl, const FiberOpsPlan &pl) {
+    fl->n_items_A = (int)pl.itA.size();
+    fl->n_items_F = (int)pl.itF.size();
+    fl->op_A_elems = pl.offA;
+    fl->op_F_elems = pl.offF;
     fl->ops_gen++;
     fl->ops_ready = true;
+}
+
+extern "C" {
+
+int skb_flow_set_fiber_operators(skb_flow *fl, const double *A, const double *force_operator, const double *xs,
+                                 const double *length_prev, const int *plus_bc_velocity) {
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_operators: NULL flow");
+    fl->ops_ready = false;
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    SKB_TRY(own_fibers(fl, "skb_flow_set_fiber_operators"));
+    const int nfib = fl->op_f1 - fl->op_f0;
+    if (nfib == 0) {
+        fl->n_items_A = fl->n_items_F = 0;
+        fl->ops_ready = true;
+        return SKB_OK;
+    }
+    if (!A || !force_operator || !xs || !length_prev || !plus_bc_velocity)
+        return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_operators: NULL argument");
+    FiberOpsPlan pl;
+    SKB_TRY(plan_fiber_operators(fl, false, length_prev, pl));
+    SKB_TRY(upload_fiber_plan(fl, pl));
+    const long long nf = fl->fb - fl->fa;
+    SKB_TRY(upload_pageable(fl->op_A.ptr, A, (size_t)pl.offA * 8, fl->stream));
+    SKB_TRY(upload_pageable(fl->op_F.ptr, force_operator, (size_t)pl.offF * 8, fl->stream));
+    CUDA_TRY(cudaMemcpyAsync(fl->op_xs.ptr, xs, (size_t)nf * 24, cudaMemcpyHostToDevice, fl->stream));
+    SKB_TRY(put_async(fl, fl->op_len, length_prev, (size_t)nfib * 8));
+    SKB_TRY(put_async(fl, fl->op_plus, plus_bc_velocity, (size_t)nfib * sizeof(int)));
+    CUDA_TRY(cudaStreamSynchronize(fl->stream)); // the host vectors above go out of scope
+    commit_fiber_plan(fl, pl);
     return SKB_OK;
 }
 
@@ -1602,7 +1676,131 @@ int skb_flow_set_fiber_preconditioner(skb_flow *fl, const double *A_inv) {
     return SKB_OK;
 }
 
+int skb_flow_build_fiber_operators(skb_flow *fl, const skb_fiber_params *params, double dt, double eta) {
+    static_assert(sizeof(skb_fiber_params) == 48 && sizeof(FiberParamsDev) == 48, "skb_fiber_params layout");
+    const char *who = "skb_flow_build_fiber_operators";
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    fl->ops_ready = false;
+    if (!(dt > 0) || !(eta > 0))
+        return set_error(SKB_ERR_INVALID, "%s: dt = %g, eta = %g (both must be > 0)", who, dt, eta);
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    SKB_TRY(own_fibers(fl, who));
+    const int f0 = fl->op_f0, nfib = fl->op_f1 - fl->op_f0;
+    if (nfib > 0 && !params)
+        return set_error(SKB_ERR_INVALID, "%s: NULL params", who);
+    for (int f = 0; f < nfib; ++f) {
+        const skb_fiber_params &p = params[f];
+        if (!(p.length_prev > 0) || !(p.radius > 0))
+            return set_error(SKB_ERR_INVALID, "fiber %d: length_prev = %g, radius = %g (both must be > 0)", f0 + f,
+                             p.length_prev, p.radius);
+        if ((p.minus_clamped != 0 && p.minus_clamped != 1) || (p.plus_hinged != 0 && p.plus_hinged != 1))
+            return set_error(SKB_ERR_INVALID, "fiber %d: minus_clamped = %d, plus_hinged = %d (each must be 0 or 1)",
+                             f0 + f, p.minus_clamped, p.plus_hinged);
+    }
+    FiberOpsPlan pl;
+    if (nfib == 0) {
+        commit_fiber_plan(fl, pl);
+        fl->precond_gen = fl->ops_gen;
+        return SKB_OK;
+    }
+    SKB_TRY(plan_fiber_operators(fl, true, nullptr, pl));
+    // per fiber: where its operators, nodes and class matrices are; per tile of columns: one assembly CTA; per node
+    // count: the matrices the inverse kernel takes in one launch
+    std::vector<FiberBuildItem> items((size_t)nfib);
+    std::vector<FiberTileItem> tiles;
+    std::vector<double> lp((size_t)nfib);
+    std::vector<int> plus((size_t)nfib);
+    std::map<int, std::vector<long long>> inv_by_n;
+    size_t smem = 0;
+    const long long node0 = fl->h_fiber_off[(size_t)f0];
+    for (int f = 0; f < nfib; ++f) {
+        const int n = fl->h_fiber_n[(size_t)(f0 + f)];
+        const long long node = fl->h_fiber_off[(size_t)(f0 + f)];
+        items[f] = FiberBuildItem{pl.offA_f[f], pl.offF_f[f], node, node - node0, pl.cD[f], pl.cR[f], n, f0 + f};
+        for (int c = 0; c < 4 * n; c += build_tile_cols(n))
+            tiles.push_back(FiberTileItem{f, c});
+        smem = std::max(smem, build_smem_bytes(n));
+        inv_by_n[n].push_back(pl.offA_f[f]);
+        lp[f] = params[f].length_prev;
+        plus[f] = params[f].plus_hinged;
+    }
+    std::vector<long long> inv_off;
+    for (const auto &kv : inv_by_n)
+        inv_off.insert(inv_off.end(), kv.second.begin(), kv.second.end());
+    begin_stats(fl);
+    CUDA_TRY(cudaEventRecord(fl->evt0, fl->stream));
+    SKB_TRY(upload_fiber_plan(fl, pl));
+    SKB_TRY(fl->op_Ainv.ensure((size_t)pl.offA * 8));
+    SKB_TRY(put_async(fl, fl->op_len, lp.data(), lp.size() * 8));
+    SKB_TRY(put_async(fl, fl->op_plus, plus.data(), plus.size() * sizeof(int)));
+    SKB_TRY(put_async(fl, fl->bld_params, params, (size_t)nfib * sizeof(skb_fiber_params)));
+    SKB_TRY(put_async(fl, fl->bld_items, items.data(), items.size() * sizeof(FiberBuildItem)));
+    SKB_TRY(put_async(fl, fl->bld_tiles, tiles.data(), tiles.size() * sizeof(FiberTileItem)));
+    SKB_TRY(put_async(fl, fl->bld_inv, inv_off.data(), inv_off.size() * sizeof(long long)));
+
+    BuildArgs ba;
+    ba.items = (const FiberBuildItem *)fl->bld_items.ptr;
+    ba.tiles = (const FiberTileItem *)fl->bld_tiles.ptr;
+    ba.params = (const FiberParamsDev *)fl->bld_params.ptr;
+    ba.class_mats = (const double *)fl->op_class.ptr;
+    ba.row_range = (const int2 *)fl->op_ranges.ptr;
+    ba.r_fib = (const double *)fl->r_fib.ptr;
+    ba.length = (const double *)fl->fiber_length.ptr;
+    ba.dt = dt;
+    ba.eta = eta;
+    ba.A = (double *)fl->op_A.ptr;
+    ba.F = (double *)fl->op_F.ptr;
+    ba.xs = (double *)fl->op_xs.ptr;
+    CUDA_TRY(cudaEventRecord(fl->ev0, fl->stream));
+    fiber_assemble_kernel<<<(unsigned)tiles.size(), kBuildThreads, smem, fl->stream>>>(ba);
+    SKB_TRY(launched(fl, 1));
+    size_t first = 0;
+    for (const auto &kv : inv_by_n) {
+        const int m = 4 * kv.first, cs = inverse_cluster_size(m);
+        cudaLaunchConfig_t cfg = {};
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeClusterDimension;
+        attr[0].val.clusterDim.x = (unsigned)cs;
+        attr[0].val.clusterDim.y = attr[0].val.clusterDim.z = 1;
+        cfg.gridDim = dim3((unsigned)(kv.second.size() * cs));
+        cfg.blockDim = dim3(kInverseThreads);
+        cfg.dynamicSmemBytes = inverse_smem_bytes(m, cs);
+        cfg.stream = fl->stream;
+        cfg.attrs = attr;
+        cfg.numAttrs = 1;
+        void (*kern)(const long long *, const double *, double *, int) =
+            m <= 128 ? fiber_inverse_kernel<4> : fiber_inverse_kernel<16>;
+        if (cs > 1) {
+            int n_clusters = 0;
+            CUDA_TRY(cudaOccupancyMaxActiveClusters(&n_clusters, kern, &cfg));
+            if (n_clusters < 1)
+                return set_error(SKB_ERR_CUDA, "%s: a cluster of %d CTAs x %zu bytes of shared memory (n = %d) does not "
+                                               "fit on device %d", who, cs, cfg.dynamicSmemBytes, kv.first, fl->dev);
+        }
+        CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, (const long long *)fl->bld_inv.ptr + first,
+                                    (const double *)fl->op_A.ptr, (double *)fl->op_Ainv.ptr, m));
+        SKB_TRY(launched(fl, 1));
+        first += kv.second.size();
+    }
+    CUDA_TRY(cudaEventRecord(fl->ev1, fl->stream));
+    CUDA_TRY(cudaEventRecord(fl->evt1, fl->stream));
+    SKB_TRY(finish_stats(fl)); // (synchronises: the host vectors above go out of scope)
+    commit_fiber_plan(fl, pl);
+    fl->precond_gen = fl->ops_gen; // the inverse belongs to these operators
+    return SKB_OK;
+}
+
 } // extern "C"
+
+// (prepare_device, skb_runtime.cu: this is the translation unit that holds the build kernels)
+int skb::prepare_fiber_build_kernels() {
+    for (auto kern : {fiber_inverse_kernel<4>, fiber_inverse_kernel<16>}) {
+        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kInverseSmemMax));
+        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    }
+    return SKB_OK;
+}
 
 static int need_ops(const skb_flow *fl, const char *who) {
     if (!fl->ops_ready)
@@ -1659,6 +1857,27 @@ static int need_precond(const skb_flow *fl, const char *who) {
 }
 
 extern "C" {
+
+int skb_flow_get_fiber_operators(skb_flow *fl, double *A, double *force_operator, double *xs, double *A_inv) {
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "skb_flow_get_fiber_operators: NULL flow");
+    SKB_TRY(need_ops(fl, "skb_flow_get_fiber_operators"));
+    if (A_inv)
+        SKB_TRY(need_precond(fl, "skb_flow_get_fiber_operators"));
+    if (fl->n_items_A == 0)
+        return SKB_OK;
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    CUDA_TRY(cudaStreamSynchronize(fl->stream));
+    if (A)
+        CUDA_TRY(cudaMemcpy(A, fl->op_A.ptr, (size_t)fl->op_A_elems * 8, cudaMemcpyDeviceToHost));
+    if (force_operator)
+        CUDA_TRY(cudaMemcpy(force_operator, fl->op_F.ptr, (size_t)fl->op_F_elems * 8, cudaMemcpyDeviceToHost));
+    if (xs)
+        CUDA_TRY(cudaMemcpy(xs, fl->op_xs.ptr, (size_t)(fl->fb - fl->fa) * 24, cudaMemcpyDeviceToHost));
+    if (A_inv)
+        CUDA_TRY(cudaMemcpy(A_inv, fl->op_Ainv.ptr, (size_t)fl->op_A_elems * 8, cudaMemcpyDeviceToHost));
+    return SKB_OK;
+}
 
 int skb_flow_apply_fiber_preconditioner(skb_flow *fl, const double *x_fibers, double *y) {
     if (!fl)

@@ -385,6 +385,28 @@ int skb_mflow_set_fiber_preconditioner(skb_mflow *mf, const double *A_inv) {
     });
 }
 
+int skb_mflow_set_fiber_class_derivatives(skb_mflow *mf, int n_nodes, const double *D_2_0, const double *D_3_0,
+                                          const double *D_4_0) {
+    if (!mf)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_set_fiber_class_derivatives: NULL");
+    for (int g = 0; g < mf->n; ++g)
+        SKB_TRY(skb_flow_set_fiber_class_derivatives(mf->m[g], n_nodes, D_2_0, D_3_0, D_4_0));
+    return SKB_OK;
+}
+
+int skb_mflow_build_fiber_operators(skb_mflow *mf, const skb_fiber_params *params, double dt, double eta) {
+    if (!mf)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_build_fiber_operators: NULL");
+    SKB_TRY(mflow_prepare(mf));
+    if (mf->n_fibers > 0 && !params)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_build_fiber_operators: NULL params");
+    SKB_TRY(mf->workers->run([&](int g) -> int {
+        return skb_flow_build_fiber_operators(mf->m[g], mf->f1[g] == mf->f0[g] ? nullptr : params + mf->f0[g], dt, eta);
+    }));
+    mf->ops_ready = true;
+    return SKB_OK;
+}
+
 // the periphery's dense operator, rows block-partitioned like the periphery rows (periphery.cpp:387-417)
 int skb_mflow_set_dense(skb_mflow *mf, int op, const double *A_rowmajor, int64_t n_rows, int64_t n_cols) {
     if (!mf || !A_rowmajor || n_rows != 3 * mf->n_shell || n_cols != 3 * mf->n_shell)

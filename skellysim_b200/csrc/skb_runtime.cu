@@ -379,6 +379,7 @@ int skb::prepare_device(int dev) {
     CUDA_TRY(set_shared(pair_sym_kernel<kSymT, kSymMinB, true>, SymSmem<kSymT>::total_bytes));
     CUDA_TRY(set_shared(pair_cross_kernel<kCrossT, kCrossMinB>, CrossSmem<kCrossT>::total_bytes));
     CUDA_TRY(set_shared(dense_stream_kernel, kStreamSmemBytes));
+    SKB_TRY(prepare_fiber_build_kernels());
     if (dev >= (int)done.size())
         done.resize(dev + 1);
     done[dev] = true;
