@@ -105,8 +105,8 @@ __global__ void __launch_bounds__(256) dense_gemv_kernel(const double *__restric
 
 struct DenseDev {
     int dev = 0, num_sms = 0;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t e0 = nullptr, e1 = nullptr, t0 = nullptr, t1 = nullptr;
+    Stream stream;
+    Event e0, e1, t0, t1;
     long long row_begin[2] = {0, 0}, n_rows[2] = {0, 0};
     DevBuf A[2], x, v, y, ticket, ticket_bg;
 };
@@ -245,6 +245,13 @@ __global__ void __maxnreg__(kStreamMaxNReg) dense_stream_kernel(const StreamArgs
 } // namespace skb
 
 struct skb_dense {
+    ~skb_dense() {
+        while (!devs.empty()) { // each device's buffers are freed with that device current
+            if (devs.back().stream) // (an entry a failed create never reached owns nothing)
+                cudaSetDevice(devs.back().dev);
+            devs.pop_back();
+        }
+    }
     std::vector<DenseDev> devs;
     long long rows[2] = {-1, -1}, cols[2] = {0, 0};
     skb_dense_stats stats{};
@@ -273,11 +280,11 @@ static int dense_create_impl(const int *ids, int n_gpus, skb_dense **out) {
         cudaDeviceProp p;
         CUDA_TRY(cudaGetDeviceProperties(&p, d.dev));
         d.num_sms = p.multiProcessorCount;
-        CUDA_TRY(cudaStreamCreateWithFlags(&d.stream, cudaStreamNonBlocking));
-        CUDA_TRY(cudaEventCreate(&d.e0));
-        CUDA_TRY(cudaEventCreate(&d.e1));
-        CUDA_TRY(cudaEventCreate(&d.t0));
-        CUDA_TRY(cudaEventCreate(&d.t1));
+        CUDA_TRY(cudaStreamCreateWithFlags(d.stream.out(), cudaStreamNonBlocking));
+        CUDA_TRY(cudaEventCreate(d.e0.out()));
+        CUDA_TRY(cudaEventCreate(d.e1.out()));
+        CUDA_TRY(cudaEventCreate(d.t0.out()));
+        CUDA_TRY(cudaEventCreate(d.t1.out()));
     }
     *out = dn.release();
     return SKB_OK;
@@ -299,23 +306,9 @@ int skb_dense_device(const skb_dense *dn, int index, int *device) {
 int skb_dense_destroy(skb_dense *dn) {
     if (!dn)
         return SKB_OK;
-    for (auto &d : dn->devs) {
-        cudaSetDevice(d.dev);
+    for (auto &d : dn->devs)
         if (d.stream)
             cudaStreamSynchronize(d.stream);
-        d.A[0].release();
-        d.A[1].release();
-        d.x.release();
-        d.v.release();
-        d.y.release();
-        d.ticket.release();
-        d.ticket_bg.release();
-        if (d.e0) cudaEventDestroy(d.e0);
-        if (d.e1) cudaEventDestroy(d.e1);
-        if (d.t0) cudaEventDestroy(d.t0);
-        if (d.t1) cudaEventDestroy(d.t1);
-        if (d.stream) cudaStreamDestroy(d.stream);
-    }
     delete dn;
     return SKB_OK;
 }

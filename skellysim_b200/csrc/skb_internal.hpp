@@ -5,6 +5,8 @@
 #include <cuda_runtime.h>
 #include <functional>
 #include <stddef.h>
+#include <type_traits>
+#include <utility>
 #include <vector>
 
 namespace skb {
@@ -22,11 +24,61 @@ struct LaunchPlan {
     unsigned grid_x = 1;     // target tiles
 };
 
+// Device memory with one owner.  The destructor frees it; the device it lives on must be current then.
 struct DevBuf {
     void *ptr = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(DevBuf &&o) noexcept { *this = std::move(o); }
+    DevBuf &operator=(DevBuf &&o) noexcept { // o takes the old buffer and frees it
+        std::swap(ptr, o.ptr);
+        std::swap(cap, o.cap);
+        return *this;
+    }
+    ~DevBuf() {
+        if (ptr)
+            cudaFree(ptr);
+    }
     int ensure(size_t bytes); // grow-only; contents are NOT preserved
-    void release();
+};
+static_assert(!std::is_copy_constructible<DevBuf>::value && !std::is_copy_assignable<DevBuf>::value,
+              "a copy would free the buffer twice");
+
+// One CUDA handle (stream, event, graph exec, pinned or IPC-mapped pointer) and the call that releases it.  Converts to
+// the raw handle, so launches and API calls take it unchanged; out() hands its address to the call that creates it.
+template <class H, auto Release> class Owned {
+    H h_ = nullptr;
+
+  public:
+    Owned() = default;
+    Owned(Owned &&o) noexcept : h_(o.h_) { o.h_ = nullptr; }
+    Owned &operator=(Owned &&o) noexcept {
+        std::swap(h_, o.h_);
+        return *this;
+    }
+    ~Owned() { reset(); }
+    operator H() const { return h_; }
+    H get() const { return h_; }
+    H *out() {
+        reset();
+        return &h_;
+    }
+    void reset() {
+        if (h_)
+            Release(h_);
+        h_ = nullptr;
+    }
+};
+using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
+using Event = Owned<cudaEvent_t, cudaEventDestroy>;
+using GraphExec = Owned<cudaGraphExec_t, cudaGraphExecDestroy>;
+using PinnedHost = Owned<double *, cudaFreeHost>;
+using DevPtr = Owned<void *, cudaFree>;              // exact-size allocation (DevBuf rounds up)
+using IpcPtr = Owned<void *, cudaIpcCloseMemHandle>; // a peer's memory mapped into this process
+
+// unique_ptr deleter of a library object: its C API destroy function
+template <auto Destroy> struct Destroyer {
+    template <class T> void operator()(T *p) const { Destroy(p); }
 };
 
 int set_error(int code, const char *fmt, ...) __attribute__((format(printf, 2, 3)));
@@ -109,11 +161,11 @@ struct SourceSet {
 
 struct DeviceState {
     skb::DeviceInfo info;
-    cudaStream_t stream = nullptr;
-    cudaStream_t aux_stream = nullptr;              // remainder targets run beside the symmetric kernel
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_fork2 = nullptr, ev_join2 = nullptr;
-    cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr, ev_k0 = nullptr, ev_k1 = nullptr;
-    cudaEvent_t ev_s0 = nullptr, ev_s1 = nullptr; // around the symmetric kernel's launch (its live duration inside a step)
+    skb::Stream stream;
+    skb::Stream aux_stream;              // remainder targets run beside the symmetric kernel
+    skb::Event ev_fork, ev_join;
+    skb::Event ev_t0, ev_t1, ev_k0, ev_k1;
+    skb::Event ev_s0, ev_s1; // around the symmetric kernel's launch (its live duration inside a step)
     bool sym_timed = false;
     long long trg_begin = 0, n_trg = 0; // this device's block of the global target list
     // symmetric multi-device layout: targets = [all n_self leading targets | remainder rows [rem_begin, +rem_count)]
@@ -125,6 +177,7 @@ struct DeviceState {
 };
 
 struct skb_ctx {
+    ~skb_ctx(); // releases each device's state with that device current
     std::vector<DeviceState> devs;
     long long n_trg = -1;
     int force_T = 0, force_S = 0;
@@ -159,10 +212,6 @@ struct CrossState {
     long long node0 = -1, n_rows = -1, n_sh = -1, n_sh_pad = -1;
     int n_blocks = 0, n_items = 0, num_sms = 0;
     DevBuf items, row_begin, P, F;
-    void release() {
-        items.release(), row_begin.release(), P.release(), F.release();
-        valid = false;
-    }
 };
 long long cross_block_nodes();
 // u_fib[n_rows x 3] (=|+=) scale_dl * (stresslet sums of ALL periphery nodes at fiber nodes [node0, node0 + n_rows));

@@ -53,19 +53,20 @@ struct TargetCache {
         ++version;
     }
 };
+using CtxPtr = std::unique_ptr<skb_ctx, Destroyer<skb_ctx_destroy>>;
 } // namespace
 
 struct skb_flow {
     int dev = 0;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr, evt0 = nullptr, evt1 = nullptr;
+    Stream stream;
+    Event ev0, ev1, evt0, evt1;
     // geometry
     long long n_fib = 0, n_shell = 0, n_body = 0;
     int n_fibers = 0, n_bodies = 0, max_fiber_nodes = 0;
     DevBuf fiber_offset, fiber_length, r_fib, r_shell, r_body, centers;
     std::vector<double> h_r_fib, h_r_shell, h_r_body; // host copies to assemble the matvec target lists
     // evaluators: [0] arbitrary targets, [1] matvec target lists
-    skb_ctx *fib[2] = {nullptr, nullptr}, *shell[2] = {nullptr, nullptr}, *body[2] = {nullptr, nullptr};
+    CtxPtr fib[2], shell[2], body[2];
     TargetCache tc_fib, tc_shell, tc_body;
     bool mv_dirty = true;
     int cross_mode = -1;    // fiber <-> periphery cross kernel in the matvec: -1 auto, 0 off, 1 on whenever applicable
@@ -92,20 +93,18 @@ struct skb_flow {
     bool has_background = false;
     // CUDA-graph replay of the launch-bound small-size calls (BASELINE C1, listener / streamline path)
     struct GraphSlot {
-        cudaGraphExec_t exec = nullptr;
+        GraphExec exec;
         unsigned long long key = 0, seen = 0;
         int launches = 0;
         long long pairs = 0;
         void reset() {
-            if (exec)
-                cudaGraphExecDestroy(exec);
-            exec = nullptr;
+            exec.reset();
             key = seen = 0;
         }
     } g_matvec, g_vat;
     unsigned long long geom_version = 1;
     bool graphs_enabled = true;
-    double *h_stage = nullptr; // pinned staging: the graph's memcpy nodes need fixed host addresses
+    PinnedHost h_stage; // pinned staging: the graph's memcpy nodes need fixed host addresses
     size_t h_stage_cap = 0;
     int bg_comp[3] = {0, 1, 2};
     double bg_scale[3] = {0, 0, 0}, bg_uniform[3] = {0, 0, 0};
@@ -129,10 +128,10 @@ struct skb_flow {
     // multi-GPU group (group_kernels.cuh): one member per GPU, exchange through peer memory
     struct Group {
         int rank = 0, size = 1;
-        void *window = nullptr;       // this member's window (cudaMalloc: exportable through CUDA IPC)
+        DevPtr window;                // this member's window (cudaMalloc: exportable through CUDA IPC)
         size_t window_bytes = 0;
         void *peer[kMaxGroup] = {};   // base address of every member's window as mapped here (peer[rank] == window)
-        bool peer_ipc[kMaxGroup] = {};
+        IpcPtr ipc[kMaxGroup];        // the windows of other processes' members that this one has mapped
         size_t off_flags = 0, off_fsl[2] = {0, 0}, off_fshell[2] = {0, 0}, off_xshell[2] = {0, 0}, off_upart = 0;
         size_t off_upart_shell = 0;   // partial periphery velocities (cross kernel: own fibers -> ALL periphery rows)
         long long n_fib = 0, n_shell = 0, n_pad_fib = 0, n_pad_shell = 0; // geometry the window was laid out for
@@ -150,8 +149,8 @@ struct skb_flow {
     // input (the complete x_shell) is there, joined before res_shell is assembled
     struct Overlap {
         bool enabled = true;       // skb_flow_set_overlap
-        cudaStream_t stream = nullptr;
-        cudaEvent_t fork = nullptr, join = nullptr;
+        Stream stream;
+        Event fork, join;
         DevBuf y;                  // A x of the own periphery rows
         skb_dense *dn = nullptr;   // pending background product of the call in flight (nullptr: none)
         bool launched = false;
@@ -164,12 +163,11 @@ struct skb_flow {
     long long pairs = 0;
 };
 
-static void group_release(skb_flow *fl);
-
-static int ensure_ctx(skb_flow *fl, skb_ctx **slot) {
-    if (*slot)
-        return SKB_OK;
-    return skb_ctx_create_on(&fl->dev, 1, slot);
+static int create_ctx(int dev, CtxPtr &slot) {
+    skb_ctx *ctx = nullptr;
+    const int rc = skb_ctx_create_on(&dev, 1, &ctx);
+    slot.reset(ctx);
+    return rc;
 }
 
 // every kernel launch of this file: check it, count it globally and in the statistics of the call in flight
@@ -309,13 +307,10 @@ static unsigned long long dbl_bits(double x) {
 static int ensure_stage(skb_flow *fl, size_t n_doubles) {
     if (n_doubles <= fl->h_stage_cap)
         return SKB_OK;
-    if (fl->h_stage)
-        cudaFreeHost(fl->h_stage);
-    fl->h_stage = nullptr;
     fl->h_stage_cap = 0;
     fl->g_matvec.reset(); // graphs hold the old staging addresses
     fl->g_vat.reset();
-    CUDA_TRY(cudaMallocHost((void **)&fl->h_stage, (n_doubles + 64) * 8));
+    CUDA_TRY(cudaMallocHost((void **)fl->h_stage.out(), (n_doubles + 64) * 8));
     fl->h_stage_cap = n_doubles + 64;
     return SKB_OK;
 }
@@ -327,7 +322,7 @@ static unsigned long long buffer_key(const skb_flow *fl, int which) {
                             &fl->tmp,    &fl->pt_pos,   &fl->pt_force, &fl->pt_torque, &fl->centers, &fl->r_fib};
     for (const DevBuf *b : bufs)
         h = mix_key(h, (unsigned long long)(uintptr_t)b->ptr);
-    const skb_ctx *ctxs[] = {fl->fib[which], fl->shell[which], fl->body[which]};
+    const skb_ctx *ctxs[] = {fl->fib[which].get(), fl->shell[which].get(), fl->body[which].get()};
     for (const skb_ctx *c : ctxs) {
         const DeviceState &d = c->devs[0];
         h = mix_key(h, (unsigned long long)(uintptr_t)d.r_trg.ptr);
@@ -379,18 +374,17 @@ template <class Body> static int run_graphed(skb_flow *fl, skb_flow::GraphSlot &
         return SKB_OK;
     }
     if (slot.seen == key && fl->graphs_enabled) {
-        if (slot.exec) {
-            cudaGraphExecDestroy(slot.exec);
-            slot.exec = nullptr;
-        }
+        slot.reset();
         cudaGraph_t graph = nullptr;
+        cudaGraphExec_t exec = nullptr;
         const long long before = launch_count();
         CUDA_TRY(cudaStreamBeginCapture(fl->stream, cudaStreamCaptureModeThreadLocal));
         const int rc = body();
         cudaError_t e = cudaStreamEndCapture(fl->stream, &graph);
         count_launch((int)(before - launch_count())); // nothing was launched while capturing
         if (rc == SKB_OK && e == cudaSuccess && graph &&
-            cudaGraphInstantiate(&slot.exec, graph, nullptr, nullptr, 0) == cudaSuccess) {
+            cudaGraphInstantiate(&exec, graph, nullptr, nullptr, 0) == cudaSuccess) {
+            *slot.exec.out() = exec; // the slot takes only a successfully instantiated graph
             cudaGraphDestroy(graph);
             slot.key = key;
             slot.launches = fl->launches;
@@ -402,7 +396,6 @@ template <class Body> static int run_graphed(skb_flow *fl, skb_flow::GraphSlot &
         if (graph)
             cudaGraphDestroy(graph);
         (void)cudaGetLastError();
-        slot.exec = nullptr;
         fl->graphs_enabled = false; // capture is not possible in this process: stay on the direct path
         fl->launches = 0;
         fl->pairs = 0;
@@ -464,26 +457,26 @@ int skb_flow_create(int device, skb_flow **out) {
     std::unique_ptr<skb_flow> fl(new skb_flow);
     fl->dev = device;
     CUDA_TRY(cudaSetDevice(device));
-    CUDA_TRY(cudaStreamCreateWithFlags(&fl->stream, cudaStreamNonBlocking));
-    CUDA_TRY(cudaEventCreate(&fl->ev0));
-    CUDA_TRY(cudaEventCreate(&fl->ev1));
-    CUDA_TRY(cudaEventCreate(&fl->evt0));
-    CUDA_TRY(cudaEventCreate(&fl->evt1));
+    CUDA_TRY(cudaStreamCreateWithFlags(fl->stream.out(), cudaStreamNonBlocking));
+    CUDA_TRY(cudaEventCreate(fl->ev0.out()));
+    CUDA_TRY(cudaEventCreate(fl->ev1.out()));
+    CUDA_TRY(cudaEventCreate(fl->evt0.out()));
+    CUDA_TRY(cudaEventCreate(fl->evt1.out()));
     if (const char *e = getenv("SKB_GRAPHS"))
         fl->graphs_enabled = atoi(e) != 0;
     if (const char *e = getenv("SKB_OVERLAP")) // A/B switch of skb_flow_set_overlap's default
         fl->bg.enabled = atoi(e) != 0;
     for (int k = 0; k < 2; ++k) {
-        SKB_TRY(ensure_ctx(fl.get(), &fl->fib[k]));
-        SKB_TRY(ensure_ctx(fl.get(), &fl->shell[k]));
-        SKB_TRY(ensure_ctx(fl.get(), &fl->body[k]));
+        SKB_TRY(create_ctx(device, fl->fib[k]));
+        SKB_TRY(create_ctx(device, fl->shell[k]));
+        SKB_TRY(create_ctx(device, fl->body[k]));
     }
     // empty classes until set_* is called
     for (int k = 0; k < 2; ++k) {
-        SKB_TRY(skb_set_sources(fl->fib[k], SKB_STOKESLET, nullptr, 0));
-        SKB_TRY(skb_set_sources(fl->shell[k], SKB_STRESSLET, nullptr, 0));
-        SKB_TRY(skb_set_sources(fl->body[k], SKB_STRESSLET, nullptr, 0));
-        SKB_TRY(skb_set_sources(fl->body[k], SKB_STOKESLET, nullptr, 0));
+        SKB_TRY(skb_set_sources(fl->fib[k].get(), SKB_STOKESLET, nullptr, 0));
+        SKB_TRY(skb_set_sources(fl->shell[k].get(), SKB_STRESSLET, nullptr, 0));
+        SKB_TRY(skb_set_sources(fl->body[k].get(), SKB_STRESSLET, nullptr, 0));
+        SKB_TRY(skb_set_sources(fl->body[k].get(), SKB_STOKESLET, nullptr, 0));
     }
     *out = fl.release();
     return SKB_OK;
@@ -493,36 +486,7 @@ int skb_flow_destroy(skb_flow *fl) {
     if (!fl)
         return SKB_OK;
     cudaSetDevice(fl->dev);
-    if (fl->stream)
-        cudaStreamSynchronize(fl->stream);
-    for (int k = 0; k < 2; ++k) {
-        skb_ctx_destroy(fl->fib[k]);
-        skb_ctx_destroy(fl->shell[k]);
-        skb_ctx_destroy(fl->body[k]);
-    }
-    DevBuf *bufs[] = {&fl->fiber_offset, &fl->fiber_length, &fl->r_fib, &fl->r_shell, &fl->r_body, &fl->centers,
-                      &fl->pt_pos, &fl->pt_force, &fl->pt_torque, &fl->in_fib, &fl->in_shell, &fl->in_body, &fl->in_force, &fl->in_torque, &fl->vel, &fl->tmp,
-                      &fl->op_A, &fl->op_F, &fl->op_xs, &fl->op_len, &fl->op_plus, &fl->op_class, &fl->op_classD,
-                      &fl->op_classP, &fl->op_classR, &fl->op_ranges, &fl->items_A, &fl->items_F, &fl->x_fib, &fl->res_fib, &fl->vb, &fl->res_shell, &fl->op_Ainv, &fl->tmp_b,
-                      &fl->bld_params, &fl->bld_items, &fl->bld_tiles, &fl->bld_inv};
-    for (DevBuf *b : bufs)
-        b->release();
-    fl->g_matvec.reset();
-    fl->g_vat.reset();
-    group_release(fl);
-    fl->scratch_u.release();
-    fl->cross.release();
-    fl->bg.y.release();
-    if (fl->bg.fork) cudaEventDestroy(fl->bg.fork);
-    if (fl->bg.join) cudaEventDestroy(fl->bg.join);
-    if (fl->bg.stream) cudaStreamDestroy(fl->bg.stream);
-    if (fl->h_stage)
-        cudaFreeHost(fl->h_stage);
-    if (fl->ev0) cudaEventDestroy(fl->ev0);
-    if (fl->ev1) cudaEventDestroy(fl->ev1);
-    if (fl->evt0) cudaEventDestroy(fl->evt0);
-    if (fl->evt1) cudaEventDestroy(fl->evt1);
-    if (fl->stream) cudaStreamDestroy(fl->stream);
+    cudaStreamSynchronize(fl->stream);
     delete fl;
     return SKB_OK;
 }
@@ -551,7 +515,7 @@ int skb_flow_set_fibers(skb_flow *fl, const double *r_fib, const int *n_nodes, c
     fl->geom_version++;
     CUDA_TRY(cudaSetDevice(fl->dev));
     for (int k = 0; k < 2; ++k)
-        SKB_TRY(skb_set_sources(fl->fib[k], SKB_STOKESLET, r_fib, fl->n_fib));
+        SKB_TRY(skb_set_sources(fl->fib[k].get(), SKB_STOKESLET, r_fib, fl->n_fib));
     if (n_fibers == 0)
         return SKB_OK;
     SKB_TRY(fl->fiber_offset.ensure(off.size() * 8));
@@ -585,8 +549,8 @@ int skb_flow_set_periphery(skb_flow *fl, const double *node_pos, const double *n
     fl->mv_dirty = true;
     fl->geom_version++;
     for (int k = 0; k < 2; ++k) {
-        SKB_TRY(skb_set_sources(fl->shell[k], SKB_STRESSLET, node_pos, n_nodes));
-        SKB_TRY(skb_set_source_normals(fl->shell[k], node_normal, n_nodes));
+        SKB_TRY(skb_set_sources(fl->shell[k].get(), SKB_STRESSLET, node_pos, n_nodes));
+        SKB_TRY(skb_set_source_normals(fl->shell[k].get(), node_normal, n_nodes));
     }
     return SKB_OK;
 }
@@ -602,9 +566,9 @@ int skb_flow_set_bodies(skb_flow *fl, const double *node_pos, const double *node
     fl->mv_dirty = true;
     fl->geom_version++;
     for (int k = 0; k < 2; ++k) {
-        SKB_TRY(skb_set_sources(fl->body[k], SKB_STRESSLET, node_pos, n_nodes));
-        SKB_TRY(skb_set_source_normals(fl->body[k], node_normal, n_nodes));
-        SKB_TRY(skb_set_sources(fl->body[k], SKB_STOKESLET, centers, n_bodies));
+        SKB_TRY(skb_set_sources(fl->body[k].get(), SKB_STRESSLET, node_pos, n_nodes));
+        SKB_TRY(skb_set_source_normals(fl->body[k].get(), node_normal, n_nodes));
+        SKB_TRY(skb_set_sources(fl->body[k].get(), SKB_STOKESLET, centers, n_bodies));
     }
     if (n_bodies > 0) {
         CUDA_TRY(cudaSetDevice(fl->dev));
@@ -621,7 +585,7 @@ int skb_flow_fibers(skb_flow *fl, const double *r_trg, int64_t n_trg, const doub
         return set_error(SKB_ERR_INVALID, "skb_flow_fibers: bad arguments");
     CUDA_TRY(cudaSetDevice(fl->dev));
     begin_stats(fl);
-    SKB_TRY(set_targets_cached(fl->fib[0], fl->tc_fib, r_trg, n_trg));
+    SKB_TRY(set_targets_cached(fl->fib[0].get(), fl->tc_fib, r_trg, n_trg));
     if (n_trg == 0)
         return SKB_OK;
     return host_frame(
@@ -631,7 +595,7 @@ int skb_flow_fibers(skb_flow *fl, const double *r_trg, int64_t n_trg, const doub
             return fl->vel.ensure((size_t)n_trg * 24);
         },
         [&] {
-            return fibers_dev(fl, fl->fib[0], kRaw, (const double *)fl->in_fib.ptr, eta, subtract_self,
+            return fibers_dev(fl, fl->fib[0].get(), kRaw, (const double *)fl->in_fib.ptr, eta, subtract_self,
                               (double *)fl->vel.ptr, 0, 0, fl->n_fib);
         },
         [&] { return download(fl, vel, fl->vel, (size_t)n_trg * 3); });
@@ -643,7 +607,7 @@ int skb_flow_periphery(skb_flow *fl, const double *r_trg, int64_t n_trg, const d
         return set_error(SKB_ERR_INVALID, "skb_flow_periphery: bad arguments");
     CUDA_TRY(cudaSetDevice(fl->dev));
     begin_stats(fl);
-    SKB_TRY(set_targets_cached(fl->shell[0], fl->tc_shell, r_trg, n_trg));
+    SKB_TRY(set_targets_cached(fl->shell[0].get(), fl->tc_shell, r_trg, n_trg));
     if (n_trg == 0)
         return SKB_OK;
     return host_frame(
@@ -653,7 +617,7 @@ int skb_flow_periphery(skb_flow *fl, const double *r_trg, int64_t n_trg, const d
             return fl->vel.ensure((size_t)n_trg * 24);
         },
         [&] {
-            return periphery_dev(fl, fl->shell[0], kNormalDensity, (const double *)fl->in_shell.ptr, eta,
+            return periphery_dev(fl, fl->shell[0].get(), kNormalDensity, (const double *)fl->in_shell.ptr, eta,
                                  (double *)fl->vel.ptr, 0);
         },
         [&] { return download(fl, vel, fl->vel, (size_t)n_trg * 3); });
@@ -666,7 +630,7 @@ int skb_flow_bodies(skb_flow *fl, const double *r_trg, int64_t n_trg, const doub
         return set_error(SKB_ERR_INVALID, "skb_flow_bodies: bad arguments");
     CUDA_TRY(cudaSetDevice(fl->dev));
     begin_stats(fl);
-    SKB_TRY(set_targets_cached(fl->body[0], fl->tc_body, r_trg, n_trg));
+    SKB_TRY(set_targets_cached(fl->body[0].get(), fl->tc_body, r_trg, n_trg));
     if (n_trg == 0)
         return SKB_OK;
     std::vector<double> f, t;
@@ -680,7 +644,7 @@ int skb_flow_bodies(skb_flow *fl, const double *r_trg, int64_t n_trg, const doub
             return fl->vel.ensure((size_t)n_trg * 24);
         },
         [&] {
-            return bodies_dev(fl, fl->body[0], (const double *)fl->in_body.ptr, (const double *)fl->in_force.ptr,
+            return bodies_dev(fl, fl->body[0].get(), (const double *)fl->in_body.ptr, (const double *)fl->in_force.ptr,
                               (const double *)fl->in_torque.ptr, eta, (double *)fl->vel.ptr, 0);
         },
         [&] { return download(fl, vel, fl->vel, (size_t)n_trg * 3); });
@@ -735,9 +699,9 @@ int skb_flow_velocity_at_targets(skb_flow *fl, const double *r_trg, int64_t n_tr
     CUDA_TRY(cudaSetDevice(fl->dev));
     begin_stats(fl);
     // the three "arbitrary target" evaluators share one cached target list
-    SKB_TRY(set_targets_cached(fl->fib[0], fl->tc_fib, r_trg, n_trg));
-    SKB_TRY(set_targets_cached(fl->shell[0], fl->tc_shell, r_trg, n_trg));
-    SKB_TRY(set_targets_cached(fl->body[0], fl->tc_body, r_trg, n_trg));
+    SKB_TRY(set_targets_cached(fl->fib[0].get(), fl->tc_fib, r_trg, n_trg));
+    SKB_TRY(set_targets_cached(fl->shell[0].get(), fl->tc_shell, r_trg, n_trg));
+    SKB_TRY(set_targets_cached(fl->body[0].get(), fl->tc_body, r_trg, n_trg));
     if (n_trg == 0)
         return SKB_OK;
     std::vector<double> f, t;
@@ -755,10 +719,10 @@ int skb_flow_velocity_at_targets(skb_flow *fl, const double *r_trg, int64_t n_tr
         SKB_TRY(upload(fl, fl->in_force, s.f, f.size()));
         SKB_TRY(upload(fl, fl->in_torque, s.t, t.size()));
         // fc_->flow(r_trg, f_on_fibers, eta, /*subtract_self=*/false) + bc_.flow + shell_->flow   system.cpp:355-359
-        SKB_TRY(fibers_dev(fl, fl->fib[0], kRaw, (const double *)fl->in_fib.ptr, eta, 0, d_v, 0, 0, 0));
-        SKB_TRY(bodies_dev(fl, fl->body[0], (const double *)fl->in_body.ptr, (const double *)fl->in_force.ptr,
+        SKB_TRY(fibers_dev(fl, fl->fib[0].get(), kRaw, (const double *)fl->in_fib.ptr, eta, 0, d_v, 0, 0, 0));
+        SKB_TRY(bodies_dev(fl, fl->body[0].get(), (const double *)fl->in_body.ptr, (const double *)fl->in_force.ptr,
                            (const double *)fl->in_torque.ptr, eta, d_v, 1));
-        SKB_TRY(periphery_dev(fl, fl->shell[0], kNormalDensity, (const double *)fl->in_shell.ptr, eta, d_v, 1));
+        SKB_TRY(periphery_dev(fl, fl->shell[0].get(), kNormalDensity, (const double *)fl->in_shell.ptr, eta, d_v, 1));
         // + psc_.flow(r_trg, eta, time) + bs_.flow(r_trg, eta)                                  system.cpp:358-359
         const double *d_trg = (const double *)fl->fib[0]->devs[0].r_trg.ptr;
         const int bs = 128;
@@ -873,20 +837,20 @@ static int prepare_matvec_targets(skb_flow *fl) {
         if (!use_cross)
             r_sym.insert(r_sym.end(), fl->h_r_shell.begin() + 3 * fl->sa, fl->h_r_shell.begin() + 3 * fl->sb);
         r_sym.insert(r_sym.end(), fl->h_r_body.begin() + 3 * fl->ba, fl->h_r_body.begin() + 3 * fl->bb);
-        SKB_TRY(skb_ctx_set_symmetric(fl->fib[1], 1));
-        SKB_TRY(skb_ctx_set_sym_partition(fl->fib[1], fl->grp.rank, fl->grp.size));
-        SKB_TRY(skb_set_targets(fl->fib[1], r_sym.data(), (long long)r_sym.size() / 3));
+        SKB_TRY(skb_ctx_set_symmetric(fl->fib[1].get(), 1));
+        SKB_TRY(skb_ctx_set_sym_partition(fl->fib[1].get(), fl->grp.rank, fl->grp.size));
+        SKB_TRY(skb_set_targets(fl->fib[1].get(), r_sym.data(), (long long)r_sym.size() / 3));
     } else if (use_cross) {
         std::vector<double> r_fibbody(fl->h_r_fib.begin() + 3 * fl->fa, fl->h_r_fib.begin() + 3 * fl->fb);
         r_fibbody.insert(r_fibbody.end(), fl->h_r_body.begin() + 3 * fl->ba, fl->h_r_body.begin() + 3 * fl->bb);
-        SKB_TRY(skb_ctx_set_sym_partition(fl->fib[1], 0, 1));
-        SKB_TRY(skb_set_targets(fl->fib[1], r_fibbody.data(), (long long)r_fibbody.size() / 3));
+        SKB_TRY(skb_ctx_set_sym_partition(fl->fib[1].get(), 0, 1));
+        SKB_TRY(skb_set_targets(fl->fib[1].get(), r_fibbody.data(), (long long)r_fibbody.size() / 3));
     } else {
-        SKB_TRY(skb_ctx_set_sym_partition(fl->fib[1], 0, 1));
-        SKB_TRY(skb_set_targets(fl->fib[1], r_win.data(), fl->n_win));
+        SKB_TRY(skb_ctx_set_sym_partition(fl->fib[1].get(), 0, 1));
+        SKB_TRY(skb_set_targets(fl->fib[1].get(), r_win.data(), fl->n_win));
     }
-    SKB_TRY(skb_set_targets(fl->body[1], r_win.data(), fl->n_win));
-    SKB_TRY(skb_set_targets(fl->shell[1], r_fb.data(), (long long)r_fb.size() / 3));
+    SKB_TRY(skb_set_targets(fl->body[1].get(), r_win.data(), fl->n_win));
+    SKB_TRY(skb_set_targets(fl->shell[1].get(), r_fb.data(), (long long)r_fb.size() / 3));
     const bool all_fibers_lead = (fl->fa == 0 && fl->fb == nf) || sym_partial;
     if (fl->self_excl && fl->n_fib > 0) {
         if (!all_fibers_lead)
@@ -896,9 +860,9 @@ static int prepare_matvec_targets(skb_flow *fl) {
         for (int f = 0; f < fl->n_fibers; ++f)
             for (long long i = fl->h_fiber_off[(size_t)f]; i < fl->h_fiber_off[(size_t)f + 1]; ++i)
                 ids[(size_t)i] = f;
-        SKB_TRY(skb_set_source_exclusion_ids(fl->fib[1], ids.data(), nf));
+        SKB_TRY(skb_set_source_exclusion_ids(fl->fib[1].get(), ids.data(), nf));
     } else {
-        SKB_TRY(skb_set_source_exclusion_ids(fl->fib[1], nullptr, 0));
+        SKB_TRY(skb_set_source_exclusion_ids(fl->fib[1].get(), nullptr, 0));
     }
     fl->mv_dirty = false;
     return SKB_OK;
@@ -913,9 +877,9 @@ static int overlap_buffers(skb_flow *fl, long long n_rows) {
     if (!B.stream) {
         int lo = 0, hi = 0;
         CUDA_TRY(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-        CUDA_TRY(cudaStreamCreateWithPriority(&B.stream, cudaStreamNonBlocking, hi));
-        CUDA_TRY(cudaEventCreateWithFlags(&B.fork, cudaEventDisableTiming));
-        CUDA_TRY(cudaEventCreateWithFlags(&B.join, cudaEventDisableTiming));
+        CUDA_TRY(cudaStreamCreateWithPriority(B.stream.out(), cudaStreamNonBlocking, hi));
+        CUDA_TRY(cudaEventCreateWithFlags(B.fork.out(), cudaEventDisableTiming));
+        CUDA_TRY(cudaEventCreateWithFlags(B.join.out(), cudaEventDisableTiming));
         // nothing may be loaded lazily later, while a group member on this device spins on a flag (the streamer itself
         // was loaded when the device was prepared, prepare_device)
         cudaFuncAttributes fa;
@@ -1019,7 +983,7 @@ static int group_pull(skb_flow *fl, size_t off, long long row0, long long n_rows
 static int fiber_rows(skb_flow *fl, StrengthMode mode, const double *ff, double eta, double *d_v) {
     const skb_flow::MatvecPlan &P = fl->plan;
     if (P.fib_rows == skb_flow::MatvecPlan::kPlain)
-        return fibers_dev(fl, fl->fib[1], mode, ff, eta, 0, d_v, 0, fl->fa, fl->fb);
+        return fibers_dev(fl, fl->fib[1].get(), mode, ff, eta, 0, d_v, 0, fl->fa, fl->fb);
     const skb_flow::Group &G = fl->grp;
     const long long nf = fl->n_fib, n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa, n_bw = fl->bb - fl->ba;
     DeviceState &df = fl->fib[1]->devs[0];
@@ -1027,7 +991,7 @@ static int fiber_rows(skb_flow *fl, StrengthMode mode, const double *ff, double 
     EvalOpts o;
     o.d_u_sym = P.grouped ? G.at<double>(G.rank, G.off_upart) : d_v;
     o.d_u_rem = d_v + 3 * (n_fw + (P.cross ? n_sw : 0));
-    SKB_TRY(eval_on_device(fl->fib[1], df, SKB_STOKESLET, mode, ff, 0.0, (double *)fl->scratch_u.ptr, 0, fl->cur,
+    SKB_TRY(eval_on_device(fl->fib[1].get(), df, SKB_STOKESLET, mode, ff, 0.0, (double *)fl->scratch_u.ptr, 0, fl->cur,
                            false, &fl->launches, nullptr, 1.0 / eta, o));
     fl->pairs += nf * nf / (P.grouped ? G.size : 1) + nf * ((P.cross ? 0 : n_sw) + n_bw);
     if (fl->fib[1]->last_was_sym)
@@ -1080,7 +1044,7 @@ static int periphery_rows(skb_flow *fl, StrengthMode mode, const double *sd, dou
     }
     SKB_TRY(fl->tmp.ensure((size_t)(n_fr + n_bw) * 24 + 8));
     double *d_tmp = (double *)fl->tmp.ptr;
-    SKB_TRY(periphery_dev(fl, fl->shell[1], mode, sd, eta, d_tmp, 0));
+    SKB_TRY(periphery_dev(fl, fl->shell[1].get(), mode, sd, eta, d_tmp, 0));
     const int bs = 256;
     if (n_fr > 0 && set_fib) {
         CUDA_TRY(cudaMemcpyAsync(d_v, d_tmp, (size_t)n_fr * 24, cudaMemcpyDeviceToDevice, fl->cur));
@@ -1125,7 +1089,7 @@ static int matvec_core(skb_flow *fl, const double *d_ff, const double *d_sd, con
     // The self term subtracts from the fiber rows: without a group right after the fiber flow; a group member
     // subtracts it last, once the pull has completed its fiber rows (the plain-kernel member keeps that order too).
     if (!P.grouped)
-        SKB_TRY(fiber_self_term(fl, fl->fib[1], eta, d_v, fl->fa, fl->fb));
+        SKB_TRY(fiber_self_term(fl, fl->fib[1].get(), eta, d_v, fl->fa, fl->fb));
     if (P.cross) {
         if (!P.grouped) { // periphery strengths 2 eta n (x) rho -> sym6 (periphery.cpp:68-71), once for both uses
             DeviceState &dsh = fl->shell[1]->devs[0];
@@ -1140,7 +1104,7 @@ static int matvec_core(skb_flow *fl, const double *d_ff, const double *d_sd, con
         SKB_TRY(group_flag(fl, 1, true, false)); // my partial sums are complete
     SKB_TRY(periphery_rows(fl, smode, sd, eta, d_v));
     // v_all += bc.flow(r_all, x_bodies, body_link_conditions, eta)     (system.cpp:316)
-    SKB_TRY(bodies_dev(fl, fl->body[1], d_bd, d_f, d_t, eta, d_v, 1));
+    SKB_TRY(bodies_dev(fl, fl->body[1].get(), d_bd, d_f, d_t, eta, d_v, 1));
     if (partial) {
         SKB_TRY(group_flag(fl, 1, false, true));
         SKB_TRY(group_pull(fl, G.off_upart, fl->fa, n_fw, d_v));
@@ -1148,32 +1112,17 @@ static int matvec_core(skb_flow *fl, const double *d_ff, const double *d_sd, con
             SKB_TRY(group_pull(fl, G.off_upart_shell, fl->sa, n_sw, d_v + 3 * n_fw));
     }
     if (P.grouped)
-        SKB_TRY(fiber_self_term(fl, fl->fib[1], eta, d_v, fl->fa, fl->fb));
+        SKB_TRY(fiber_self_term(fl, fl->fib[1].get(), eta, d_v, fl->fa, fl->fb));
     return SKB_OK;
 }
 
 // ---- group membership (multi-GPU through peer memory, group_kernels.cuh) ------------------------------------------
-} // extern "C"
-
-static void group_release(skb_flow *fl) {
-    skb_flow::Group &G = fl->grp;
-    cudaSetDevice(fl->dev);
-    for (int m = 0; m < G.size; ++m)
-        if (m != G.rank && G.peer[m] && G.peer_ipc[m])
-            cudaIpcCloseMemHandle(G.peer[m]);
-    if (G.window)
-        cudaFree(G.window);
-    G = skb_flow::Group();
-}
-
-extern "C" {
-
 int skb_flow_group_init(skb_flow *fl, int rank, int size) {
     if (!fl || size < 1 || size > kMaxGroup || rank < 0 || rank >= size)
         return set_error(SKB_ERR_INVALID, "skb_flow_group_init: need 0 <= rank < size <= %d", kMaxGroup);
     CUDA_TRY(cudaSetDevice(fl->dev));
     CUDA_TRY(cudaStreamSynchronize(fl->stream));
-    group_release(fl);
+    fl->grp = skb_flow::Group();
     fl->mv_dirty = true;
     fl->ops_ready = false;
     fl->geom_version++;
@@ -1202,7 +1151,7 @@ int skb_flow_group_init(skb_flow *fl, int rank, int size) {
     G.off_upart = take((size_t)G.n_fib * 24 + 16);
     G.off_upart_shell = take((size_t)G.n_shell * 24 + 16);
     G.window_bytes = off;
-    CUDA_TRY(cudaMalloc(&G.window, G.window_bytes));
+    CUDA_TRY(cudaMalloc(G.window.out(), G.window_bytes));
     CUDA_TRY(cudaMemset(G.window, 0, G.window_bytes)); // flags at epoch 0, strength pads zero for good
     G.peer[rank] = G.window;
     return SKB_OK;
@@ -1225,10 +1174,8 @@ int skb_flow_group_import(skb_flow *fl, int peer_rank, const void *handle) {
     CUDA_TRY(cudaSetDevice(fl->dev));
     cudaIpcMemHandle_t h;
     std::memcpy(&h, handle, sizeof(h));
-    void *p = nullptr;
-    CUDA_TRY(cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
-    fl->grp.peer[peer_rank] = p;
-    fl->grp.peer_ipc[peer_rank] = true;
+    CUDA_TRY(cudaIpcOpenMemHandle(fl->grp.ipc[peer_rank].out(), h, cudaIpcMemLazyEnablePeerAccess));
+    fl->grp.peer[peer_rank] = fl->grp.ipc[peer_rank];
     return SKB_OK;
 }
 
@@ -1253,7 +1200,6 @@ int skb_flow_group_connect(skb_flow *fl, int peer_rank, skb_flow *peer) {
                              cudaGetErrorString(e));
     }
     fl->grp.peer[peer_rank] = peer->grp.window;
-    fl->grp.peer_ipc[peer_rank] = false;
     return SKB_OK;
 }
 
@@ -1283,7 +1229,6 @@ int skb_flow_group_warmup(skb_flow *fl) {
     fl->grp.dry = false;
     cudaError_t e = cudaStreamSynchronize(fl->stream);
     fl->grp.epoch = 0;
-    z.release();
     if (rc != SKB_OK)
         return rc;
     if (e != cudaSuccess)
@@ -1308,7 +1253,7 @@ int skb_flow_group_error(skb_flow *fl, int *missing_peer) {
         return SKB_OK;
     unsigned long long w = 0;
     CUDA_TRY(cudaSetDevice(fl->dev));
-    CUDA_TRY(cudaMemcpy(&w, (char *)fl->grp.window + fl->grp.off_flags + (size_t)kGroupPhases * kMaxGroup * 8, 8,
+    CUDA_TRY(cudaMemcpy(&w, (char *)fl->grp.window.get() + fl->grp.off_flags + (size_t)kGroupPhases * kMaxGroup * 8, 8,
                         cudaMemcpyDeviceToHost));
     if (w)
         *missing_peer = (int)(w - 1);
@@ -2164,7 +2109,7 @@ int skb_flow_apply_matvec_device(skb_flow *fl, skb_dense *dn, const double *d_x_
 int skb_flow_last_sym_kernel(const skb_flow *fl, double *ms, int64_t *pairs) {
     if (!fl)
         return set_error(SKB_ERR_INVALID, "skb_flow_last_sym_kernel: NULL");
-    return skb_ctx_last_sym_kernel(fl->fib[1], ms, pairs);
+    return skb_ctx_last_sym_kernel(fl->fib[1].get(), ms, pairs);
 }
 
 int skb_flow_last_stats(const skb_flow *fl, skb_flow_stats *out) {

@@ -104,11 +104,12 @@ class Workers {
 } // namespace
 
 struct skb_mflow {
+    ~skb_mflow();
     int n = 0;
     std::vector<int> devs;
-    std::vector<skb_flow *> m;
-    std::vector<skb_dense *> dn;
-    std::unique_ptr<Workers> workers;
+    std::vector<std::unique_ptr<skb_flow, Destroyer<skb_flow_destroy>>> m;
+    std::vector<std::unique_ptr<skb_dense, Destroyer<skb_dense_destroy>>> dn;
+    std::unique_ptr<Workers> workers; // declared after m and dn: its threads are joined before any member goes
     // geometry (host copies of what the partition needs)
     long long n_fib = 0, n_shell = 0, n_body = 0;
     int n_fibers = 0, n_bodies = 0;
@@ -122,7 +123,7 @@ struct skb_mflow {
     bool ops_ready = false;
     struct IO { // per-member device buffers of the host-pointer calls
         DevBuf x, xs, bd, f, t, link, res, outs, vb, ff, v;
-        cudaEvent_t e0 = nullptr, e1 = nullptr;
+        Event e0, e1;
     };
     std::vector<IO> io;
     skb_flow_stats stats{};
@@ -170,18 +171,25 @@ static int mflow_prepare(skb_mflow *mf) {
         return SKB_OK;
     mflow_partition(mf);
     for (int g = 0; g < mf->n; ++g) {
-        SKB_TRY(skb_flow_set_target_ranges(mf->m[g], mf->f0[g], mf->f1[g], mf->s0[g], mf->s1[g], mf->b0[g], mf->b1[g]));
-        SKB_TRY(skb_flow_group_init(mf->m[g], g, mf->n));
+        SKB_TRY(skb_flow_set_target_ranges(mf->m[g].get(), mf->f0[g], mf->f1[g], mf->s0[g], mf->s1[g], mf->b0[g], mf->b1[g]));
+        SKB_TRY(skb_flow_group_init(mf->m[g].get(), g, mf->n));
     }
     for (int g = 0; g < mf->n; ++g)
         for (int h = 0; h < mf->n; ++h)
             if (g != h)
-                SKB_TRY(skb_flow_group_connect(mf->m[g], h, mf->m[h]));
+                SKB_TRY(skb_flow_group_connect(mf->m[g].get(), h, mf->m[h].get()));
     for (int g = 0; g < mf->n; ++g) // all allocations up front: members may share a device (see skb_flow_group_warmup)
-        SKB_TRY(skb_flow_group_warmup(mf->m[g]));
+        SKB_TRY(skb_flow_group_warmup(mf->m[g].get()));
     mf->part_dirty = false;
     mf->ops_ready = false;
     return SKB_OK;
+}
+
+skb_mflow::~skb_mflow() {
+    while (!io.empty()) { // each member's buffers are freed with its device current
+        cudaSetDevice(devs[io.size() - 1]);
+        io.pop_back();
+    }
 }
 
 extern "C" {
@@ -192,22 +200,17 @@ int skb_mflow_create(const int *devices, int n, skb_mflow **out) {
     *out = nullptr;
     std::unique_ptr<skb_mflow> mf(new skb_mflow);
     mf->n = n;
-    mf->m.assign(n, nullptr);
-    mf->dn.assign(n, nullptr);
-    mf->io.resize(n);
+    mf->dn.resize(n);
     for (int g = 0; g < n; ++g) {
         mf->devs.push_back(devices ? devices[g] : g);
-        int rc = skb_flow_create(mf->devs[g], &mf->m[g]);
-        if (rc == SKB_OK) {
-            cudaSetDevice(mf->devs[g]);
-            if (cudaEventCreate(&mf->io[g].e0) != cudaSuccess || cudaEventCreate(&mf->io[g].e1) != cudaSuccess)
-                rc = set_error(SKB_ERR_CUDA, "cudaEventCreate failed");
-        }
-        if (rc != SKB_OK) {
-            for (int h = 0; h <= g; ++h)
-                skb_flow_destroy(mf->m[h]);
-            return rc;
-        }
+        skb_flow *fl = nullptr;
+        const int rc = skb_flow_create(mf->devs[g], &fl);
+        mf->m.emplace_back(fl);
+        SKB_TRY(rc);
+        CUDA_TRY(cudaSetDevice(mf->devs[g]));
+        mf->io.emplace_back(); // io[g] only once member g exists: ~skb_mflow makes devs[g] current for it
+        CUDA_TRY(cudaEventCreate(mf->io[g].e0.out()));
+        CUDA_TRY(cudaEventCreate(mf->io[g].e1.out()));
     }
     mf->workers.reset(new Workers(n));
     *out = mf.release();
@@ -221,17 +224,6 @@ int skb_mflow_destroy(skb_mflow *mf) {
     for (int g = 0; g < mf->n; ++g) {
         cudaSetDevice(mf->devs[g]);
         cudaDeviceSynchronize();
-    }
-    for (int g = 0; g < mf->n; ++g) {
-        cudaSetDevice(mf->devs[g]);
-        skb_mflow::IO &io = mf->io[g];
-        DevBuf *bufs[] = {&io.x, &io.xs, &io.bd, &io.f, &io.t, &io.link, &io.res, &io.outs, &io.vb, &io.ff, &io.v};
-        for (DevBuf *b : bufs)
-            b->release();
-        if (io.e0) cudaEventDestroy(io.e0);
-        if (io.e1) cudaEventDestroy(io.e1);
-        skb_dense_destroy(mf->dn[g]);
-        skb_flow_destroy(mf->m[g]);
     }
     delete mf;
     return SKB_OK;
@@ -251,7 +243,7 @@ int skb_mflow_set_fibers(skb_mflow *mf, const double *r_fib, const int *n_nodes,
     for (int f = 0; f < n_fibers; ++f)
         off[(size_t)f + 1] = off[(size_t)f] + (n_nodes ? n_nodes[f] : 0);
     const bool resized = off != mf->fiber_off;
-    SKB_TRY(mf->workers->run([&](int g) -> int { return skb_flow_set_fibers(mf->m[g], r_fib, n_nodes, length, n_fibers); }));
+    SKB_TRY(mf->workers->run([&](int g) -> int { return skb_flow_set_fibers(mf->m[g].get(), r_fib, n_nodes, length, n_fibers); }));
     mf->n_fibers = n_fibers;
     mf->n_fib = off[(size_t)n_fibers];
     mf->fiber_off = off;
@@ -265,7 +257,7 @@ int skb_mflow_set_fibers(skb_mflow *mf, const double *r_fib, const int *n_nodes,
 int skb_mflow_set_periphery(skb_mflow *mf, const double *node_pos, const double *node_normal, int64_t n_nodes) {
     if (!mf || n_nodes < 0)
         return set_error(SKB_ERR_INVALID, "skb_mflow_set_periphery: bad arguments");
-    SKB_TRY(mf->workers->run([&](int g) -> int { return skb_flow_set_periphery(mf->m[g], node_pos, node_normal, n_nodes); }));
+    SKB_TRY(mf->workers->run([&](int g) -> int { return skb_flow_set_periphery(mf->m[g].get(), node_pos, node_normal, n_nodes); }));
     if (mf->n_shell != n_nodes)
         mf->part_dirty = true;
     mf->n_shell = n_nodes;
@@ -277,7 +269,7 @@ int skb_mflow_set_bodies(skb_mflow *mf, const double *node_pos, const double *no
     if (!mf || n_nodes < 0 || n_bodies < 0)
         return set_error(SKB_ERR_INVALID, "skb_mflow_set_bodies: bad arguments");
     SKB_TRY(mf->workers->run(
-        [&](int g) { return skb_flow_set_bodies(mf->m[g], node_pos, node_normal, n_nodes, centers, n_bodies); }));
+        [&](int g) { return skb_flow_set_bodies(mf->m[g].get(), node_pos, node_normal, n_nodes, centers, n_bodies); }));
     if (mf->n_body != n_nodes)
         mf->part_dirty = true;
     mf->n_body = n_nodes;
@@ -289,7 +281,7 @@ int skb_mflow_set_cross(skb_mflow *mf, int mode) {
     if (!mf)
         return set_error(SKB_ERR_INVALID, "skb_mflow_set_cross: NULL");
     for (int g = 0; g < mf->n; ++g)
-        SKB_TRY(skb_flow_set_cross(mf->m[g], mode));
+        SKB_TRY(skb_flow_set_cross(mf->m[g].get(), mode));
     mf->part_dirty = true; // the members' target lists change: re-run the warm-up
     return SKB_OK;
 }
@@ -298,7 +290,7 @@ int skb_mflow_set_overlap(skb_mflow *mf, int on) {
     if (!mf)
         return set_error(SKB_ERR_INVALID, "skb_mflow_set_overlap: NULL");
     for (int g = 0; g < mf->n; ++g)
-        SKB_TRY(skb_flow_set_overlap(mf->m[g], on));
+        SKB_TRY(skb_flow_set_overlap(mf->m[g].get(), on));
     return SKB_OK;
 }
 
@@ -306,7 +298,7 @@ int skb_mflow_set_self_exclusion(skb_mflow *mf, int fused) {
     if (!mf)
         return set_error(SKB_ERR_INVALID, "skb_mflow_set_self_exclusion: NULL");
     for (int g = 0; g < mf->n; ++g)
-        SKB_TRY(skb_flow_set_self_exclusion(mf->m[g], fused));
+        SKB_TRY(skb_flow_set_self_exclusion(mf->m[g].get(), fused));
     return SKB_OK;
 }
 
@@ -345,7 +337,7 @@ int skb_mflow_set_fiber_class(skb_mflow *mf, int n_nodes, const double *D_1_0, c
     if (!mf)
         return set_error(SKB_ERR_INVALID, "skb_mflow_set_fiber_class: NULL");
     for (int g = 0; g < mf->n; ++g)
-        SKB_TRY(skb_flow_set_fiber_class(mf->m[g], n_nodes, D_1_0, P_downsample_bc));
+        SKB_TRY(skb_flow_set_fiber_class(mf->m[g].get(), n_nodes, D_1_0, P_downsample_bc));
     mf->ops_ready = false;
     return SKB_OK;
 }
@@ -368,8 +360,8 @@ int skb_mflow_set_fiber_operators(skb_mflow *mf, const double *A, const double *
     SKB_TRY(mf->workers->run([&](int g) -> int {
         const int f0 = mf->f0[g];
         if (mf->f1[g] == f0)
-            return skb_flow_set_fiber_operators(mf->m[g], nullptr, nullptr, nullptr, nullptr, nullptr);
-        return skb_flow_set_fiber_operators(mf->m[g], A + op_offset(mf, f0, 4), force_operator + op_offset(mf, f0, 3),
+            return skb_flow_set_fiber_operators(mf->m[g].get(), nullptr, nullptr, nullptr, nullptr, nullptr);
+        return skb_flow_set_fiber_operators(mf->m[g].get(), A + op_offset(mf, f0, 4), force_operator + op_offset(mf, f0, 3),
                                             xs + 3 * mf->fiber_off[(size_t)f0], length_prev + f0, plus_bc_velocity + f0);
     }));
     mf->ops_ready = true;
@@ -381,7 +373,7 @@ int skb_mflow_set_fiber_preconditioner(skb_mflow *mf, const double *A_inv) {
         return set_error(SKB_ERR_INVALID, "skb_mflow_set_fiber_preconditioner: call skb_mflow_set_fiber_operators first");
     return mf->workers->run([&](int g) -> int {
         const int f0 = mf->f0[g];
-        return skb_flow_set_fiber_preconditioner(mf->m[g], mf->f1[g] == f0 ? nullptr : A_inv + op_offset(mf, f0, 4));
+        return skb_flow_set_fiber_preconditioner(mf->m[g].get(), mf->f1[g] == f0 ? nullptr : A_inv + op_offset(mf, f0, 4));
     });
 }
 
@@ -390,7 +382,7 @@ int skb_mflow_set_fiber_class_derivatives(skb_mflow *mf, int n_nodes, const doub
     if (!mf)
         return set_error(SKB_ERR_INVALID, "skb_mflow_set_fiber_class_derivatives: NULL");
     for (int g = 0; g < mf->n; ++g)
-        SKB_TRY(skb_flow_set_fiber_class_derivatives(mf->m[g], n_nodes, D_2_0, D_3_0, D_4_0));
+        SKB_TRY(skb_flow_set_fiber_class_derivatives(mf->m[g].get(), n_nodes, D_2_0, D_3_0, D_4_0));
     return SKB_OK;
 }
 
@@ -401,7 +393,7 @@ int skb_mflow_build_fiber_operators(skb_mflow *mf, const skb_fiber_params *param
     if (mf->n_fibers > 0 && !params)
         return set_error(SKB_ERR_INVALID, "skb_mflow_build_fiber_operators: NULL params");
     SKB_TRY(mf->workers->run([&](int g) -> int {
-        return skb_flow_build_fiber_operators(mf->m[g], mf->f1[g] == mf->f0[g] ? nullptr : params + mf->f0[g], dt, eta);
+        return skb_flow_build_fiber_operators(mf->m[g].get(), mf->f1[g] == mf->f0[g] ? nullptr : params + mf->f0[g], dt, eta);
     }));
     mf->ops_ready = true;
     return SKB_OK;
@@ -414,9 +406,12 @@ int skb_mflow_set_dense(skb_mflow *mf, int op, const double *A_rowmajor, int64_t
                                           "nodes set before", mf ? mf->n_shell : 0LL);
     SKB_TRY(mflow_prepare(mf));
     SKB_TRY(mf->workers->run([&](int g) -> int {
-        if (!mf->dn[g])
-            SKB_TRY(skb_dense_create_on(&mf->devs[g], 1, &mf->dn[g]));
-        return skb_dense_set_matrix(mf->dn[g], op, A_rowmajor + (size_t)(3 * mf->s0[g]) * (size_t)n_cols,
+        if (!mf->dn[g]) {
+            skb_dense *dn = nullptr;
+            SKB_TRY(skb_dense_create_on(&mf->devs[g], 1, &dn));
+            mf->dn[g].reset(dn);
+        }
+        return skb_dense_set_matrix(mf->dn[g].get(), op, A_rowmajor + (size_t)(3 * mf->s0[g]) * (size_t)n_cols,
                                     3 * (mf->s1[g] - mf->s0[g]), n_cols);
     }));
     if (op == SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY)
@@ -436,11 +431,11 @@ static int mflow_collect_stats(skb_mflow *mf) {
         else
             (void)cudaGetLastError();
         skb_flow_stats st{};
-        skb_flow_last_stats(mf->m[g], &st);
+        skb_flow_last_stats(mf->m[g].get(), &st);
         pairs += st.n_pairs;
         launches += st.launches;
         int missing = -1;
-        SKB_TRY(skb_flow_group_error(mf->m[g], &missing));
+        SKB_TRY(skb_flow_group_error(mf->m[g].get(), &missing));
         if (missing >= 0)
             return set_error(SKB_ERR_STATE, "device member %d timed out waiting for member %d (a peer failed or never "
                                             "issued the matching call)", g, missing);
@@ -491,7 +486,7 @@ static int mflow_size_io(skb_mflow *mf, size_t n_ft) {
         SKB_TRY(io.vb.ensure(n_bw * 24 + 8));
         SKB_TRY(io.v.ensure((n_fw + n_sw + n_bw) * 24 + 8));
         if (mf->has_dense && n_sw > 0)
-            SKB_TRY(flow_size_overlap(mf->m[g], 3 * (long long)n_sw));
+            SKB_TRY(flow_size_overlap(mf->m[g].get(), 3 * (long long)n_sw));
     }
     return SKB_OK;
 }
@@ -511,7 +506,7 @@ int skb_mflow_matvec(skb_mflow *mf, const double *fib_forces, const double *shel
         split_forces_torques(body_forces_torques, mf->n_bodies, f, t);
     SKB_TRY(mflow_size_io(mf, f.size()));
     SKB_TRY(mf->workers->run([&](int g) -> int {
-        skb_flow *fl = mf->m[g];
+        skb_flow *fl = mf->m[g].get();
         skb_mflow::IO &io = mf->io[g];
         CUDA_TRY(cudaSetDevice(mf->devs[g]));
         const MemberRows r = member_rows(mf, g);
@@ -562,7 +557,7 @@ int skb_mflow_apply_matvec(skb_mflow *mf, const double *x_fibers, const double *
         split_forces_torques(body_forces_torques, mf->n_bodies, f, t);
     SKB_TRY(mflow_size_io(mf, f.size()));
     SKB_TRY(mf->workers->run([&](int g) -> int {
-        skb_flow *fl = mf->m[g];
+        skb_flow *fl = mf->m[g].get();
         skb_mflow::IO &io = mf->io[g];
         CUDA_TRY(cudaSetDevice(mf->devs[g]));
         const int f0 = mf->f0[g], f1 = mf->f1[g];
@@ -581,7 +576,7 @@ int skb_mflow_apply_matvec(skb_mflow *mf, const double *x_fibers, const double *
         SKB_TRY(io.vb.ensure((size_t)n_bw * 24 + 8));
         CUDA_TRY(cudaEventRecord(io.e0, st));
         SKB_TRY(skb_flow_apply_matvec_device(
-            fl, mf->has_dense ? mf->dn[g] : nullptr, (const double *)io.x.ptr, (const double *)io.xs.ptr,
+            fl, mf->has_dense ? mf->dn[g].get() : nullptr, (const double *)io.x.ptr, (const double *)io.xs.ptr,
             (const double *)io.bd.ptr, (const double *)io.f.ptr, (const double *)io.t.ptr,
             (fiber_link_conditions && f1 > f0) ? (const double *)io.link.ptr : nullptr, eta, (double *)io.res.ptr,
             (double *)io.outs.ptr, (double *)io.vb.ptr, st));
@@ -611,7 +606,7 @@ int skb_mflow_velocity_at_targets(skb_mflow *mf, const double *r_trg, int64_t n_
         const long long b = std::min<long long>(n_trg, g * chunk), e = std::min<long long>(n_trg, (g + 1) * chunk);
         if (e <= b)
             return (int)SKB_OK;
-        return skb_flow_velocity_at_targets(mf->m[g], r_trg + 3 * b, e - b, fib_forces, shell_density, body_densities,
+        return skb_flow_velocity_at_targets(mf->m[g].get(), r_trg + 3 * b, e - b, fib_forces, shell_density, body_densities,
                                             body_forces_torques, eta, vel + 3 * b);
     }));
     double dev_ms = 0;
@@ -619,7 +614,7 @@ int skb_mflow_velocity_at_targets(skb_mflow *mf, const double *r_trg, int64_t n_
     int launches = 0;
     for (int g = 0; g < mf->n; ++g) {
         skb_flow_stats st{};
-        skb_flow_last_stats(mf->m[g], &st);
+        skb_flow_last_stats(mf->m[g].get(), &st);
         dev_ms = std::max(dev_ms, st.device_ms);
         pairs += st.n_pairs;
         launches += st.launches;

@@ -214,10 +214,7 @@ int launch_reduce(const double *d_partial, double *d_u, long long n_trg, int n_s
 int DevBuf::ensure(size_t bytes) {
     if (bytes <= cap)
         return SKB_OK;
-    if (ptr)
-        cudaFree(ptr);
-    ptr = nullptr;
-    cap = 0;
+    *this = DevBuf(); // the old buffer goes before the new one is allocated
     size_t want = bytes + bytes / 8 + 256;
     cudaError_t e = cudaMalloc(&ptr, want);
     if (e != cudaSuccess) {
@@ -226,12 +223,6 @@ int DevBuf::ensure(size_t bytes) {
     }
     cap = want;
     return SKB_OK;
-}
-void DevBuf::release() {
-    if (ptr)
-        cudaFree(ptr);
-    ptr = nullptr;
-    cap = 0;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -395,6 +386,16 @@ static int check_kind(int kind) {
     return SKB_OK;
 }
 
+skb_ctx::~skb_ctx() {
+    while (!devs.empty()) { // each device's buffers are freed with that device current
+        if (devs.back().stream) // (an entry a failed create never reached owns nothing)
+            cudaSetDevice(devs.back().info.dev);
+        devs.pop_back();
+    }
+    if (nccl)
+        nccl_group_destroy(nccl);
+}
+
 static int ctx_create_impl(const int *ids, int n, skb_ctx **out) {
     if (!out)
         return set_error(SKB_ERR_INVALID, "skb_ctx_create: out == NULL");
@@ -417,19 +418,17 @@ static int ctx_create_impl(const int *ids, int n, skb_ctx **out) {
             return set_error(SKB_ERR_INVALID, "device id %d out of range", dev);
         SKB_TRY(prepare_device(dev));
         d.info = query_device(dev);
-        CUDA_TRY(cudaStreamCreateWithFlags(&d.stream, cudaStreamNonBlocking));
+        CUDA_TRY(cudaStreamCreateWithFlags(d.stream.out(), cudaStreamNonBlocking));
         // (d.aux_stream is created on first use by the symmetric path: most contexts of a flow never need one, and a
         // device has a finite number of hardware queues for independent streams)
-        CUDA_TRY(cudaEventCreateWithFlags(&d.ev_fork, cudaEventDisableTiming));
-        CUDA_TRY(cudaEventCreateWithFlags(&d.ev_join, cudaEventDisableTiming));
-        CUDA_TRY(cudaEventCreateWithFlags(&d.ev_fork2, cudaEventDisableTiming));
-        CUDA_TRY(cudaEventCreateWithFlags(&d.ev_join2, cudaEventDisableTiming));
-        CUDA_TRY(cudaEventCreate(&d.ev_t0));
-        CUDA_TRY(cudaEventCreate(&d.ev_t1));
-        CUDA_TRY(cudaEventCreate(&d.ev_k0));
-        CUDA_TRY(cudaEventCreate(&d.ev_k1));
-        CUDA_TRY(cudaEventCreate(&d.ev_s0));
-        CUDA_TRY(cudaEventCreate(&d.ev_s1));
+        CUDA_TRY(cudaEventCreateWithFlags(d.ev_fork.out(), cudaEventDisableTiming));
+        CUDA_TRY(cudaEventCreateWithFlags(d.ev_join.out(), cudaEventDisableTiming));
+        CUDA_TRY(cudaEventCreate(d.ev_t0.out()));
+        CUDA_TRY(cudaEventCreate(d.ev_t1.out()));
+        CUDA_TRY(cudaEventCreate(d.ev_k0.out()));
+        CUDA_TRY(cudaEventCreate(d.ev_k1.out()));
+        CUDA_TRY(cudaEventCreate(d.ev_s0.out()));
+        CUDA_TRY(cudaEventCreate(d.ev_s1.out()));
     }
     if (n > 1)
         SKB_TRY(nccl_group_create(ctx->devs.size(), [&](int g) { return ctx->devs[g].info.dev; }, &ctx->nccl));
@@ -466,45 +465,9 @@ int skb_ctx_create_on(const int *device_ids, int n_gpus, skb_ctx **out) {
 int skb_ctx_destroy(skb_ctx *ctx) {
     if (!ctx)
         return SKB_OK;
-    for (auto &d : ctx->devs) {
-        cudaSetDevice(d.info.dev);
+    for (auto &d : ctx->devs)
         if (d.stream)
             cudaStreamSynchronize(d.stream);
-        d.r_trg.release();
-        d.u.release();
-        d.partial.release();
-        d.scratch.release();
-        d.u_rs.release();
-        for (auto &s : d.src) {
-            s.r.release();
-            s.normals.release();
-            s.weights.release();
-            s.sym_item_buf.release();
-            s.sym_row_begin.release();
-            s.sym_P.release();
-            s.sym_F.release();
-            s.sym_row_ids.release();
-            s.sym_flag.release();
-            s.f_raw.release();
-            s.f_packed.release();
-            s.excl_ids.release();
-            s.excl_trg.release();
-        }
-        if (d.ev_t0) cudaEventDestroy(d.ev_t0);
-        if (d.ev_t1) cudaEventDestroy(d.ev_t1);
-        if (d.ev_k0) cudaEventDestroy(d.ev_k0);
-        if (d.ev_k1) cudaEventDestroy(d.ev_k1);
-        if (d.ev_s0) cudaEventDestroy(d.ev_s0);
-        if (d.ev_s1) cudaEventDestroy(d.ev_s1);
-        if (d.ev_fork) cudaEventDestroy(d.ev_fork);
-        if (d.ev_join) cudaEventDestroy(d.ev_join);
-        if (d.ev_fork2) cudaEventDestroy(d.ev_fork2);
-        if (d.ev_join2) cudaEventDestroy(d.ev_join2);
-        if (d.aux_stream) cudaStreamDestroy(d.aux_stream);
-        if (d.stream) cudaStreamDestroy(d.stream);
-    }
-    if (ctx->nccl)
-        nccl_group_destroy(ctx->nccl);
     delete ctx;
     return SKB_OK;
 }
@@ -1038,7 +1001,7 @@ static int sym_eval(skb_ctx *ctx, DeviceState &d, double *d_u_out, int accumulat
     SourceSet &s = d.src[SKB_STOKESLET];
     const double *f_packed = s.f_cur;
     if (!d.aux_stream)
-        CUDA_TRY(cudaStreamCreateWithFlags(&d.aux_stream, cudaStreamNonBlocking));
+        CUDA_TRY(cudaStreamCreateWithFlags(d.aux_stream.out(), cudaStreamNonBlocking));
     const long long block = sym_block_nodes();
     SymArgs a;
     a.r = (const double *)s.r.ptr;
@@ -1209,7 +1172,7 @@ int eval_on_device(skb_ctx *ctx, DeviceState &d, int kind, StrengthMode mode, co
     const double scale = scale_mul * (kind == SKB_STOKESLET ? 1.0 : -3.0) / (8.0 * M_PI);
     cudaStream_t st_std = st;
     if (n_sym > 0 && !d.aux_stream)
-        CUDA_TRY(cudaStreamCreateWithFlags(&d.aux_stream, cudaStreamNonBlocking));
+        CUDA_TRY(cudaStreamCreateWithFlags(d.aux_stream.out(), cudaStreamNonBlocking));
     if (n_sym > 0 && n_trg_std > 0) { // fork: the remainder fills the SMs the symmetric kernel's tail leaves idle
         CUDA_TRY(cudaEventRecord(d.ev_fork, st));
         CUDA_TRY(cudaStreamWaitEvent(d.aux_stream, d.ev_fork, 0));

@@ -69,6 +69,28 @@ def test_product_never_imports_oracle():
     assert not bad, bad
 
 
+def test_device_resources_are_released_only_by_their_owners():
+    # every stream, event, graph exec, device or pinned allocation and IPC mapping of the library is held by an owner
+    # type of skb_internal.hpp (DevBuf, Owned) that releases it; a release call anywhere else is a hand-written teardown
+    # list that can fall out of step with the structs.  (The process-lifetime objects -- the pinned upload ring, the
+    # default context, prepare_device's table -- are never released: static destructors would run after the CUDA
+    # runtime's own teardown at exit.)
+    release = re.compile(r"\b(cudaFree|cudaFreeHost|cudaEventDestroy|cudaStreamDestroy|cudaGraphExecDestroy|"
+                         r"cudaIpcCloseMemHandle)\b")
+    bad = []
+    for base in ("skellysim_b200", "include"):
+        for dirpath, _, files in os.walk(os.path.join(ROOT, base)):
+            for f in files:
+                if f == "skb_internal.hpp" or not f.endswith((".cu", ".cuh", ".cpp", ".hpp", ".h")):
+                    continue
+                txt = open(os.path.join(dirpath, f), errors="ignore").read()
+                txt = re.sub(r"/\*.*?\*/", lambda m: "\n" * m.group().count("\n"), txt, flags=re.S)
+                for i, line in enumerate(txt.splitlines(), 1):
+                    if release.search(line.split("//")[0]):
+                        bad.append(f"{f}:{i}: {line.strip()}")
+    assert not bad, bad
+
+
 def test_null_handles_are_refused_before_any_cuda_call():
     # argument errors come back as codes with a message (never a crash), GPU or not
     L = capi.library()
