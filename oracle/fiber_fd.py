@@ -139,20 +139,35 @@ class FiberOperators:
     fiber_finite_difference.cpp:74-95); minus_clamped / plus_pinned select the other branches."""
 
     def __init__(self, x, length, bending_rigidity=2.5e-3, radius=0.0125, eta=1.0, dt=1e-2, length_prev=None,
-                 minus_clamped=False, plus_pinned=False, penalty_param=500.0, beta_tstep=1.0):
-        x = np.asarray(x, dtype=np.float64)
+                 minus_clamped=False, plus_pinned=False, penalty_param=500.0, beta_tstep=1.0, dtype=np.float64,
+                 absolute=False):
+        """dtype: the arithmetic.  The inputs (positions, scalars, the class matrices of compute_matrices) are float64
+        values either way, so np.longdouble evaluates exactly the function of them that a float64 evaluation rounds.
+
+        absolute=True evaluates the error scale S of every output instead: the same computation with every input
+        replaced by |.| and every subtraction turned into an addition (c_0 = -log(e eps^2) / (8 pi eta) enters as
+        (|log(e eps^2)| + 4) / (8 pi eta): the log's absolute error is u times that).  Any float64 evaluation order of
+        an output y then satisfies |fl(y) - y| <= gamma_k S(y), k the operations on its longest path."""
+        f = np.dtype(dtype).type
+        x = np.asarray(x, dtype=np.float64).astype(f)
         self.n = n = x.shape[0]
-        self.x = x
-        self.length = float(length)
-        self.length_prev = float(length if length_prev is None else length_prev)
-        self.E = float(bending_rigidity)
-        eps = radius / self.length                                        # fiber_finite_difference.hpp:141
-        self.c_0 = -np.log(np.e * eps ** 2) / (8 * np.pi * eta)           # :142
-        self.c_1 = 2.0 / (8.0 * np.pi * eta)                              # :143
-        self.penalty, self.beta, self.dt = float(penalty_param), float(beta_tstep), float(dt)
+        self.x = np.abs(x) if absolute else x
+        self.sg = f(1.0 if absolute else -1.0)                            # the sign of every subtraction
+        self.dtype = f
+        self.length = f(np.float64(length))
+        self.length_prev = f(np.float64(length if length_prev is None else length_prev))
+        self.E = f(np.float64(bending_rigidity))
+        eta = f(np.float64(eta))
+        eps = f(np.float64(radius)) / self.length                         # fiber_finite_difference.hpp:141
+        lg = np.log(f(np.e) * eps ** 2)
+        self.c_0 = (np.abs(lg) + 4) / (8 * f(np.pi) * eta) if absolute else -lg / (8 * f(np.pi) * eta)   # :142
+        self.c_1 = 2.0 / (8.0 * f(np.pi) * eta)                           # :143
+        self.penalty, self.beta, self.dt = (f(np.float64(v)) for v in (penalty_param, beta_tstep, dt))
         self.bc_minus = (BC_VELOCITY, BC_ANGULAR_VELOCITY) if minus_clamped else (BC_FORCE, BC_TORQUE)   # :75-78
         self.bc_plus = (BC_VELOCITY, BC_TORQUE) if plus_pinned else (BC_FORCE, BC_TORQUE)               # :84-88
         self.mats = compute_matrices(n)
+        self._m = {k: (np.abs(v) if absolute else v).astype(f) for k, v in self.mats.items()
+                   if k.startswith("D_") or k == "P_downsample_bc"}
         self._update_derivatives()
         self._update_linear_operator()
         self._apply_bc_rectangular()
@@ -160,39 +175,39 @@ class FiberOperators:
 
     # xs_ = (2/L_prev)^k * x_ * D_k_0 with x_ 3 x n  ==  (n,3): D_k_0^T-free form x^T-consistent: (x_ D)^T = D^T x
     def _update_derivatives(self):                                        # fiber_finite_difference.cpp:62-72
-        m, x, lp = self.mats, self.x, self.length_prev
+        m, x, lp = self._m, self.x, self.length_prev
         self.xs = (2.0 / lp) ** 1 * (m["D_1_0"].T @ x)
         self.xss = (2.0 / lp) ** 2 * (m["D_2_0"].T @ x)
         self.xsss = (2.0 / lp) ** 3 * (m["D_3_0"].T @ x)
         self.xssss = (2.0 / lp) ** 4 * (m["D_4_0"].T @ x)
 
     def _update_linear_operator(self):                                    # :97-187
-        n, m, L = self.n, self.mats, self.length
+        n, m, L, sg = self.n, self._m, self.length, self.sg
         D_1 = m["D_1_0"].T * (2.0 / L) ** 1                               # :101-104
         D_2 = m["D_2_0"].T * (2.0 / L) ** 2
         D_3 = m["D_3_0"].T * (2.0 / L) ** 3
         D_4 = m["D_4_0"].T * (2.0 / L) ** 4
         E, c0, c1 = self.E, self.c_0, self.c_1
         xs, xss, xsss = self.xs, self.xss, self.xsss
-        I = np.eye(n)
+        I = np.eye(n, dtype=self.dtype)
         cw = lambda D, v: D * v[:, None]                                  # (D.colwise() * v): row i scaled by v_i
-        A = np.zeros((4 * n, 4 * n))
+        A = np.zeros((4 * n, 4 * n), dtype=self.dtype)
         blk = lambda r, c: (slice(r * n, (r + 1) * n), slice(c * n, (c + 1) * n))
         for a in range(3):                                                # :146-159
             for b in range(3):
                 if a == b:
                     A[blk(a, a)] = (self.beta / self.dt * I + E * c0 * cw(D_4, 1.0 + xs[:, a] ** 2)
-                                    + E * c1 * cw(D_4, 1.0 - xs[:, a] ** 2))
+                                    + E * c1 * cw(D_4, 1.0 + sg * xs[:, a] ** 2))
                 else:
-                    A[blk(a, b)] = E * (c0 - c1) * cw(D_4, xs[:, a] * xs[:, b])
-            A[blk(a, 3)] = -(c0 * 2.0) * cw(D_1, xs[:, a]) - (c0 + c1) * np.diag(xss[:, a])            # :161-168
-            A[blk(3, a)] = (-(c1 + 7.0 * c0) * E * cw(D_4, xss[:, a]) - 6.0 * c0 * E * cw(D_3, xsss[:, a])
-                            - self.penalty * cw(D_1, xs[:, a]))                                        # :173-183
-        A[blk(3, 3)] = -2.0 * c0 * D_2 + (c0 + c1) * np.diag(np.sum(xss ** 2, axis=1))                 # :185-186
+                    A[blk(a, b)] = E * (c0 + sg * c1) * cw(D_4, xs[:, a] * xs[:, b])
+            A[blk(a, 3)] = sg * (c0 * 2.0) * cw(D_1, xs[:, a]) + sg * (c0 + c1) * np.diag(xss[:, a])      # :161-168
+            A[blk(3, a)] = (sg * (c1 + 7.0 * c0) * E * cw(D_4, xss[:, a]) + sg * 6.0 * c0 * E * cw(D_3, xsss[:, a])
+                            + sg * self.penalty * cw(D_1, xs[:, a]))                                   # :173-183
+        A[blk(3, 3)] = sg * 2.0 * c0 * D_2 + (c0 + c1) * np.diag(np.sum(xss ** 2, axis=1))             # :185-186
         self.A = A
 
     def _apply_bc_rectangular(self):                                      # :347-516 (operator part; RHS not needed)
-        n, m, L = self.n, self.mats, self.length
+        n, m, L, sg = self.n, self._m, self.length, self.sg
         D_1 = m["D_1_0"].T * (2.0 / L) ** 1
         D_2 = m["D_2_0"].T * (2.0 / L) ** 2
         D_3 = m["D_3_0"].T * (2.0 / L) ** 3
@@ -200,7 +215,7 @@ class FiberOperators:
         xs, xss = self.xs, self.xss
         A = self.A
         A[:4 * n - 14] = m["P_downsample_bc"] @ A                         # :356
-        B = np.zeros((14, 4 * n))                                         # :362-363
+        B = np.zeros((14, 4 * n), dtype=self.dtype)                                       # :362-363
         bdt = self.beta / self.dt
         if self.bc_minus[0] == BC_VELOCITY:                               # :366-384
             B[0, 0 * n] = B[1, 1 * n] = B[2, 2 * n] = bdt
@@ -210,9 +225,9 @@ class FiberOperators:
         else:                                                             # Force :386-405
             for k in range(3):
                 B[k, k * n:(k + 1) * n] = E * D_3[0]
-                B[k, 3 * n] = -xs[0, k]
-                B[3, k * n:(k + 1) * n] = -E * D_2[0] * xss[0, k]
-            B[3, 3 * n] = -1
+                B[k, 3 * n] = sg * xs[0, k]
+                B[3, k * n:(k + 1) * n] = sg * E * D_2[0] * xss[0, k]
+            B[3, 3 * n] = sg
         if self.bc_minus[1] == BC_ANGULAR_VELOCITY:                       # :415-424
             for k in range(3):
                 B[4 + k, k * n:(k + 1) * n] = bdt * D_1[0]
@@ -227,7 +242,7 @@ class FiberOperators:
             B[10, 3 * n:4 * n] = (2.0 * c0) * D_1[e]
         else:                                                             # Force :466-487
             for k in range(3):
-                B[7 + k, k * n:(k + 1) * n] = -E * D_3[e]
+                B[7 + k, k * n:(k + 1) * n] = sg * E * D_3[e]
                 B[7 + k, 4 * n - 1] = xs[e, k]
                 B[10, k * n:(k + 1) * n] = E * D_2[e] * xss[e, k]
             B[10, 4 * n - 1] = 1.0
@@ -237,12 +252,12 @@ class FiberOperators:
         self.A = A
 
     def _update_force_operator(self):                                     # :317-335
-        n, m, L = self.n, self.mats, self.length
+        n, m, L, sg = self.n, self._m, self.length, self.sg
         D_1 = m["D_1_0"] * (2.0 / L) ** 1
         D_4 = m["D_4_0"] * (2.0 / L) ** 4
-        F = np.zeros((3 * n, 4 * n))
+        F = np.zeros((3 * n, 4 * n), dtype=self.dtype)
         for i in range(3):
-            F[i * n:(i + 1) * n, i * n:(i + 1) * n] = -self.E * D_4.T                                   # :328
+            F[i * n:(i + 1) * n, i * n:(i + 1) * n] = self.sg * self.E * D_4.T                                  # :328
             blk = np.diag(self.xss[:, i])                                                               # :330
             blk = blk + (D_1 * self.xs[:, i][None, :]).T                                                # :332-333
             F[i * n:(i + 1) * n, 3 * n:4 * n] = blk
@@ -274,3 +289,56 @@ def suspension_operators(r_fib, n_nodes, lengths, eta=1.0, dt=1e-2, seed=0, clam
         off += n
     ops["xs"] = np.concatenate(xs) if xs else np.zeros((0, 3))
     return ops
+
+
+def gauss_jordan_inverse(A, dtype=np.float64, pivot_window=None, pivoting=True, recip_rel_err=0.0):
+    """Host restatement of fiber_build.cuh's fiber_inverse_kernel in `dtype`: in-place Gauss-Jordan elimination with
+    partial pivoting (the first row of largest magnitude in rows [k, m)), the pivot row scaled by the reciprocal of the
+    pivot, column k eliminated from every other row with the pivot column as it was before the step, and the column
+    interchanges that undo the pivoting applied at the end as one permutation.  The kernel fuses the elimination's
+    multiply-add; numpy rounds the product first.  np.longdouble gives the extended-precision inverse of the same
+    float64 matrix.
+
+    The keyword arguments plant defects that a test of the kernel must catch: a pivot search over rows [k, k +
+    pivot_window) only, no pivoting at all, a pivot reciprocal off by the relative error recip_rel_err."""
+    M = np.array(A, dtype=np.float64).astype(dtype)
+    m = M.shape[0]
+    piv = np.empty(m, dtype=np.int64)
+    for k in range(m):
+        p = k
+        if pivoting:
+            hi = m if pivot_window is None else min(m, k + pivot_window)
+            p = k + int(np.argmax(np.abs(M[k:hi, k])))
+        piv[k] = p
+        rc = M[:, k].copy()                              # the published pivot column, row-swapped
+        rc[k], rc[p] = rc[p], rc[k]
+        if p != k:
+            M[[k, p]] = M[[p, k]]
+        inv = 1 / rc[k]
+        if recip_rel_err:
+            inv = inv * (1 + recip_rel_err)
+        r = M[k] * inv
+        r[k] = inv
+        M[k] = r
+        M[:k, k] = 0
+        M[k + 1:, k] = 0
+        M[:k] -= np.outer(rc[:k], r)
+        M[k + 1:] -= np.outer(rc[k + 1:], r)
+    perm = np.arange(m)
+    for k in range(m - 1, -1, -1):
+        perm[k], perm[piv[k]] = perm[piv[k]], perm[k]
+    return M[:, perm]
+
+
+def extended_inverse(A):
+    """A^-1 of the float64 matrix A in np.longdouble: Gauss-Jordan with partial pivoting and one step of iterative
+    refinement with a long-double residual, X <- X + X (I - A X).  Also returns the correction a second step would
+    apply, an independent estimate of the extended inverse's own error."""
+    if np.finfo(np.longdouble).nmant < 63:
+        raise RuntimeError(f"np.longdouble has {np.finfo(np.longdouble).nmant + 1} mantissa bits here; an extended-"
+                           "precision reference needs at least 64")
+    A_ext = np.asarray(A, dtype=np.float64).astype(np.longdouble)
+    I = np.eye(A_ext.shape[0], dtype=np.longdouble)
+    X = gauss_jordan_inverse(A, np.longdouble)
+    X = X + X @ (I - A_ext @ X)
+    return X, X @ (I - A_ext @ X)
