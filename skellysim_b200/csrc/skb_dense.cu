@@ -11,20 +11,6 @@
 
 using namespace skb;
 
-#define CUDA_TRY(expr)                                                                                                \
-    do {                                                                                                              \
-        cudaError_t _e = (expr);                                                                                      \
-        if (_e != cudaSuccess)                                                                                        \
-            return set_error(SKB_ERR_CUDA, "%s failed at %s:%d: %s", #expr, __FILE__, __LINE__,                      \
-                             cudaGetErrorString(_e));                                                                 \
-    } while (0)
-#define SKB_TRY(expr)                                                                                                 \
-    do {                                                                                                              \
-        int _rc = (expr);                                                                                             \
-        if (_rc != SKB_OK)                                                                                            \
-            return _rc;                                                                                               \
-    } while (0)
-
 namespace {
 
 // 128-bit streaming load of the matrix (read once, keep it out of L1)

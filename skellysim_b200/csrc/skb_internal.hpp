@@ -4,10 +4,13 @@
 
 #include <cuda_runtime.h>
 #include <functional>
+#include <map>
 #include <stddef.h>
 #include <type_traits>
 #include <utility>
 #include <vector>
+
+struct skb_fiber_params;
 
 namespace skb {
 
@@ -82,6 +85,20 @@ template <auto Destroy> struct Destroyer {
 };
 
 int set_error(int code, const char *fmt, ...) __attribute__((format(printf, 2, 3)));
+// return from the enclosing function with the error of a failed CUDA call / library call
+#define CUDA_TRY(expr)                                                                                                \
+    do {                                                                                                              \
+        cudaError_t _e = (expr);                                                                                      \
+        if (_e != cudaSuccess)                                                                                        \
+            return ::skb::set_error(SKB_ERR_CUDA, "%s failed at %s:%d: %s", #expr, __FILE__, __LINE__,                \
+                                    cudaGetErrorString(_e));                                                          \
+    } while (0)
+#define SKB_TRY(expr)                                                                                                 \
+    do {                                                                                                              \
+        int _rc = (expr);                                                                                             \
+        if (_rc != SKB_OK)                                                                                            \
+            return _rc;                                                                                               \
+    } while (0)
 const char *last_error();
 void count_launch(int n);
 long long launch_count();
@@ -95,8 +112,8 @@ int upload_pageable(void *d_dst, const void *h_src, size_t bytes, cudaStream_t s
 // Takes device `dev` into use, once per device and process: rejects anything but compute capability 9.0 and loads the
 // kernels that need launch attributes, with those attributes set.  Makes `dev` current.
 int prepare_device(int dev);
-// the launch attributes of the kernels of fiber_build.cuh (skb_matvec.cu); called by prepare_device
-int prepare_fiber_build_kernels();
+// the launch attributes of the kernels of fiber_ops.cuh and fiber_build.cuh (skb_fiber.cu); called by prepare_device
+int prepare_fiber_kernels();
 DeviceInfo query_device(int dev); // (of a prepared device)
 LaunchPlan plan_launch(const DeviceInfo &di, int kind, long long n_trg, int n_src_tiles, int force_T, int force_S);
 int launch_pair_sum(const DeviceInfo &di, int kind, const double *d_r_src, const double *d_f_packed, long long n_src,
@@ -122,6 +139,68 @@ constexpr int kMaxGroup = 16; // members of a multi-GPU group (group_kernels.cuh
 
 // forces_torques [6 x n_bodies] (body_container.cpp:134) -> forces and torques, 3 x n_bodies each
 void split_forces_torques(const double *ft, int n_bodies, std::vector<double> &f, std::vector<double> &t);
+
+// ---- per-fiber dense operators of a flow (SURVEY.md §8f N2; skb_fiber.cu) ----
+// The fibers whose operators are resident (the fiber rows of the flow's target list) and what the build reads
+struct OwnFibers {
+    int f0 = 0, f1 = 0;             // fibers [f0, f1)
+    const int *n = nullptr;         // node count of every fiber of the flow
+    const long long *off = nullptr; // first node of every fiber of the flow (n_fibers + 1 entries)
+    const double *r_fib = nullptr;  // device: positions of all fiber nodes
+    const double *length = nullptr; // device: length of every fiber
+    cudaStream_t stream = nullptr;  // uploads, the build and the read-back are ordered on it
+    int count() const { return f1 - f0; }
+    long long nodes() const { return f1 > f0 ? off[f1] - off[f0] : 0; }
+};
+
+// A_, force_operator_, xs_ and A_^-1 of one set of own fibers, resident for the timestep, and the GEMVs over them.
+// The caller has checked its pointers for NULL and made the flow's device current.
+class FiberOps {
+  public:
+    int set_class(int n_nodes, const double *D_1_0, const double *P_downsample_bc); // drops the operators
+    int set_class_derivatives(int n_nodes, const double *D_2_0, const double *D_3_0, const double *D_4_0);
+    int upload(const OwnFibers &own, const double *A, const double *force_operator, const double *xs,
+               const double *length_prev, const int *plus_bc_velocity);
+    int upload_inverse(const double *A_inv, cudaStream_t st);
+    // the device build, checked and planned on the host first; `frame` runs stage (the table uploads), then launch
+    // (assembly and inverse kernels, adding to *launches) and returns once own.stream has drained.  No own fibers:
+    // the empty set, without a frame
+    using Step = std::function<int()>;
+    int build(const OwnFibers &own, const ::skb_fiber_params *params, double dt, double eta, int *launches,
+              const std::function<int(const Step &stage, const Step &launch)> &frame);
+    // on st, each adding its launches to *launches: fw = force_operator_ x; res = fc.matvec(x, v, vb); y = A_^-1 x
+    int force(const double *d_x, double *d_fw, cudaStream_t st, int *launches) const;
+    int matvec(const double *d_x, const double *d_v, const double *d_vb, double *d_res, cudaStream_t st,
+               int *launches) const;
+    int precondition(const double *d_x, double *d_y, cudaStream_t st, int *launches) const;
+    int read(double *A, double *force_operator, double *xs, double *A_inv, cudaStream_t st) const; // any may be NULL
+    int ready(const char *who, bool with_inverse = false) const; // an error naming `who` unless they are resident
+    bool empty() const { return n_items_A == 0; }
+    int n_fibers() const { return f1 - f0; }
+    void invalidate() { ready_ = false; }
+
+  private:
+    struct Plan;
+    int plan(const OwnFibers &own, const double *length_prev, const ::skb_fiber_params *build, Plan &pl);
+    int upload_plan(const OwnFibers &own, const Plan &pl);
+    void commit(const OwnFibers &own, const Plan &pl);
+
+    struct FiberClass {
+        std::vector<double> D, P; // D_1_0 (n x n), P_downsample_bc ((4n-14) x 4n), column-major
+        std::vector<double> D234; // D_2_0 | D_3_0 | D_4_0 (n x n each): set_class_derivatives
+    };
+    std::map<int, FiberClass> classes;
+    bool ready_ = false;
+    int f0 = 0, f1 = 0;    // the fibers of the resident operators
+    long long n_nodes = 0; // ... and their nodes
+    int n_items_A = 0, n_items_F = 0;
+    size_t gemv_smem = 0;
+    DevBuf op_A, op_F, op_xs, op_Ainv, op_len, op_plus, op_class, op_classD, op_classP, op_classR, op_ranges, items_A,
+        items_F, bld_params, bld_items, bld_tiles, bld_inv;
+    long long op_A_elems = 0;                        // elements of the concatenated A_ (and of A_^-1)
+    long long op_F_elems = 0;                        // ... of force_operator_
+    unsigned long long ops_gen = 0, precond_gen = 0; // the inverse belongs to one set of operators
+};
 
 } // namespace skb
 

@@ -3,8 +3,6 @@
 // (src/core/system.cpp:284-316).  Built on the pair-kernel contexts of skb_runtime.cu; everything between the
 // upload of the strengths and the download of the velocities stays on the device.
 #include "aux_kernels.cuh"
-#include "fiber_build.cuh"
-#include "fiber_ops.cuh"
 #include "group_kernels.cuh"
 #include "skb_internal.hpp"
 #include "../../include/skelly_b200_flow.h"
@@ -14,25 +12,10 @@
 #include <cstdint>
 #include <cstdlib>
 #include <cstring>
-#include <map>
 #include <memory>
 #include <vector>
 
 using namespace skb;
-
-#define CUDA_TRY(expr)                                                                                                \
-    do {                                                                                                              \
-        cudaError_t _e = (expr);                                                                                      \
-        if (_e != cudaSuccess)                                                                                        \
-            return set_error(SKB_ERR_CUDA, "%s failed at %s:%d: %s", #expr, __FILE__, __LINE__,                      \
-                             cudaGetErrorString(_e));                                                                 \
-    } while (0)
-#define SKB_TRY(expr)                                                                                                 \
-    do {                                                                                                              \
-        int _rc = (expr);                                                                                             \
-        if (_rc != SKB_OK)                                                                                            \
-            return _rc;                                                                                               \
-    } while (0)
 
 namespace {
 // reference defaults of the regularised helpers (include/kernels.hpp:38-46): reg = 5e-3, eps = 1e-5
@@ -86,7 +69,6 @@ struct skb_flow {
     // resolved pieces of the matvec target list: fiber rows [fa,fb), shell rows [sa,sb), body rows [ba,bb);
     // the output has n_win = (fb-fa)+(sb-sa)+(bb-ba) rows in that order
     long long fa = 0, fb = 0, sa = 0, sb = 0, ba = 0, bb = 0, n_win = 0;
-    int op_f0 = 0, op_f1 = 0; // fibers [op_f0, op_f1) whose operators are resident (the fiber rows of the target list)
     cudaStream_t cur = nullptr;            // stream of the call in flight (own stream or the caller's)
     int n_points = 0;
     DevBuf pt_pos, pt_force, pt_torque;
@@ -108,23 +90,9 @@ struct skb_flow {
     size_t h_stage_cap = 0;
     int bg_comp[3] = {0, 1, 2};
     double bg_scale[3] = {0, 0, 0}, bg_uniform[3] = {0, 0, 0};
-    // per-fiber dense operators (SURVEY.md §8f N2): A_, force_operator_, xs_ resident for the timestep
-    std::vector<int> h_fiber_n;
-    std::vector<long long> h_fiber_off;
-    struct FiberClass {
-        std::vector<double> D, P; // D_1_0 (n x n), P_downsample_bc ((4n-14) x 4n), column-major
-        std::vector<double> D234; // D_2_0 | D_3_0 | D_4_0 (n x n each): skb_flow_set_fiber_class_derivatives
-    };
-    std::map<int, FiberClass> fiber_classes;
-    bool ops_ready = false;
-    int n_items_A = 0, n_items_F = 0;
-    size_t gemv_smem = 0;
-    DevBuf op_A, op_F, op_xs, op_len, op_plus, op_class, op_classD, op_classP, op_classR, op_ranges, items_A, items_F;
-    DevBuf x_fib, res_fib, vb, res_shell, op_Ainv, tmp_b;
-    DevBuf bld_params, bld_items, bld_tiles, bld_inv; // skb_flow_build_fiber_operators (fiber_build.cuh)
-    long long op_A_elems = 0;               // elements of the concatenated A_ (and of A_^-1)
-    long long op_F_elems = 0;               // ... of force_operator_
-    unsigned long long ops_gen = 0, precond_gen = 0; // the preconditioner belongs to one set of operators
+    std::vector<int> h_fiber_n;         // nodes of every fiber
+    std::vector<long long> h_fiber_off; // first node of every fiber (n_fibers + 1)
+    FiberOps ops; // per-fiber dense operators of the fibers whose rows are in the target list (skb_fiber.cu)
     // multi-GPU group (group_kernels.cuh): one member per GPU, exchange through peer memory
     struct Group {
         int rank = 0, size = 1;
@@ -157,7 +125,7 @@ struct skb_flow {
     } bg;
     DevBuf scratch_u; // group mode: landing zone of eval_on_device's default output (never read)
     // staging
-    DevBuf in_fib, in_shell, in_body, in_force, in_torque, vel, tmp;
+    DevBuf in_fib, in_shell, in_body, in_force, in_torque, vel, tmp, x_fib, res_fib, vb, res_shell, tmp_b;
     skb_flow_stats stats{};
     int launches = 0;
     long long pairs = 0;
@@ -443,6 +411,21 @@ static int device_stats(skb_flow *fl) {
     return SKB_OK;
 }
 
+// frame of the fiber operators' GEMV entry points: the operators' check (`inverse`: with their inverse), nothing to do
+// without own fibers, the arguments, then call(nodes of the own fibers) on the flow's device
+template <class Call> static int fiber_ops_call(skb_flow *fl, const char *who, bool inverse, bool args, Call call) {
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    SKB_TRY(fl->ops.ready(who, inverse));
+    begin_stats(fl);
+    if (fl->ops.empty())
+        return SKB_OK;
+    if (!args)
+        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    return call((size_t)(fl->fb - fl->fa));
+}
+
 extern "C" {
 
 int skb_flow_create(int device, skb_flow **out) {
@@ -510,7 +493,7 @@ int skb_flow_set_fibers(skb_flow *fl, const double *r_fib, const int *n_nodes, c
     fl->h_r_fib.assign(r_fib, r_fib + 3 * fl->n_fib);
     fl->h_fiber_n.assign(n_nodes, n_nodes + n_fibers);
     fl->h_fiber_off = off;
-    fl->ops_ready = false; // operators belong to one set of fibers
+    fl->ops.invalidate(); // operators belong to one set of fibers
     fl->mv_dirty = true;
     fl->geom_version++;
     CUDA_TRY(cudaSetDevice(fl->dev));
@@ -1124,7 +1107,7 @@ int skb_flow_group_init(skb_flow *fl, int rank, int size) {
     CUDA_TRY(cudaStreamSynchronize(fl->stream));
     fl->grp = skb_flow::Group();
     fl->mv_dirty = true;
-    fl->ops_ready = false;
+    fl->ops.invalidate();
     fl->geom_version++;
     if (size == 1)
         return SKB_OK;
@@ -1293,7 +1276,7 @@ int skb_flow_set_target_window(skb_flow *fl, int64_t begin, int64_t end) {
     fl->win_end = end;
     fl->use_ranges = false;
     fl->mv_dirty = true;
-    fl->ops_ready = false; // resident fiber operators belong to one set of fiber rows
+    fl->ops.invalidate(); // resident fiber operators belong to one set of fiber rows
     fl->geom_version++;
     return SKB_OK;
 }
@@ -1311,7 +1294,7 @@ int skb_flow_set_target_ranges(skb_flow *fl, int fiber_begin, int fiber_end, int
     fl->rq_b1 = body_end;
     fl->use_ranges = true;
     fl->mv_dirty = true;
-    fl->ops_ready = false;
+    fl->ops.invalidate();
     fl->geom_version++;
     return SKB_OK;
 }
@@ -1392,41 +1375,24 @@ int skb_flow_matvec_device(skb_flow *fl, const double *d_fib_forces, const doubl
     return device_stats(fl);
 }
 
-// ---- per-fiber dense operators (SURVEY.md §8f N2) ---------------------------------------------------------------
+// ---- per-fiber dense operators (SURVEY.md §8f N2, skb_fiber.cu) ------------------------------------------------
 
 int skb_flow_set_fiber_class(skb_flow *fl, int n_nodes, const double *D_1_0, const double *P_downsample_bc) {
     if (!fl || !D_1_0 || !P_downsample_bc)
         return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_class: NULL argument");
-    if (n_nodes < 4) // bc_start_i = 4n - 14 must leave room for the 14 boundary rows (ffd.cpp:279)
-        return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_class: n_nodes = %d (need >= 4)", n_nodes);
-    const size_t n = (size_t)n_nodes;
-    skb_flow::FiberClass &c = fl->fiber_classes[n_nodes];
-    c.D.assign(D_1_0, D_1_0 + n * n);
-    c.P.assign(P_downsample_bc, P_downsample_bc + (4 * n - 14) * 4 * n);
-    fl->ops_ready = false;
-    return SKB_OK;
+    return fl->ops.set_class(n_nodes, D_1_0, P_downsample_bc);
 }
 
 int skb_flow_set_fiber_class_derivatives(skb_flow *fl, int n_nodes, const double *D_2_0, const double *D_3_0,
                                          const double *D_4_0) {
     if (!fl || !D_2_0 || !D_3_0 || !D_4_0)
         return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_class_derivatives: NULL argument");
-    if (n_nodes < kBuildMinNodes || n_nodes > kBuildMaxNodes)
-        return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_class_derivatives: n_nodes = %d (the device build takes "
-                                          "%d <= n <= %d)", n_nodes, kBuildMinNodes, kBuildMaxNodes);
-    const size_t nn = (size_t)n_nodes * n_nodes;
-    std::vector<double> &d = fl->fiber_classes[n_nodes].D234;
-    d.assign(D_2_0, D_2_0 + nn);
-    d.insert(d.end(), D_3_0, D_3_0 + nn);
-    d.insert(d.end(), D_4_0, D_4_0 + nn);
-    return SKB_OK;
+    return fl->ops.set_class_derivatives(n_nodes, D_2_0, D_3_0, D_4_0);
 }
-
-} // extern "C"
 
 // The fibers whose operators are resident: those whose rows are in this flow's target list -- all of them, or the
 // rank's own fibers under skb_flow_set_target_ranges / an aligned skb_flow_set_target_window.
-static int own_fibers(skb_flow *fl, const char *who) {
+static int own_fibers(skb_flow *fl, const char *who, OwnFibers &own) {
     SKB_TRY(prepare_matvec_targets(fl));
     int f0 = 0, f1 = 0;
     if (fl->n_fibers > 0) {
@@ -1437,501 +1403,132 @@ static int own_fibers(skb_flow *fl, const char *who) {
             return set_error(SKB_ERR_INVALID, "%s: the target window [%lld, %lld) cuts a fiber; use "
                                               "skb_flow_set_target_ranges (whole fibers)", who, fl->fa, fl->fb);
     }
-    fl->op_f0 = f0;
-    fl->op_f1 = f1;
+    own = OwnFibers{f0, f1, fl->h_fiber_n.data(), fl->h_fiber_off.data(), (const double *)fl->r_fib.ptr,
+                    (const double *)fl->fiber_length.ptr, fl->stream};
     return SKB_OK;
 }
-
-// Where the resident operators of the own fibers live, shared by skb_flow_set_fiber_operators and
-// skb_flow_build_fiber_operators: the class matrices in one buffer, the non-zero column range of every row of
-// P_downsample_bc, the GEMV work items, and every fiber's offsets into A_ / force_operator_.
-struct FiberOpsPlan {
-    std::vector<double> h_class;              // per class: D_1_0 | P_downsample_bc [| D_2_0 | D_3_0 | D_4_0]
-    std::vector<int2> h_ranges;
-    std::vector<long long> cD, cP, cR;        // per own fiber: its class's D_1_0, P, ranges
-    std::vector<long long> offA_f, offF_f;    // per own fiber: its A_ / force_operator_
-    std::vector<FiberGemvItem> itA, itF;
-    long long offA = 0, offF = 0;
-};
-
-// build: the operators are made on the device (class derivatives needed, n within the build's range);
-// length_prev: checked per fiber when given
-static int plan_fiber_operators(skb_flow *fl, bool build, const double *length_prev, FiberOpsPlan &pl) {
-    const int f0 = fl->op_f0, nfib = fl->op_f1 - fl->op_f0;
-    // class matrices -> one device buffer, per-fiber offsets into it; per class also the non-zero column range of every
-    // row of P_downsample_bc (block diagonal in the reference, ffd.cpp:551-555: the kernels walk the range only)
-    std::map<int, std::pair<long long, long long>> class_off;
-    std::map<int, long long> range_off;
-    for (const auto &kv : fl->fiber_classes) {
-        if (kv.second.D.empty()) // only skb_flow_set_fiber_class_derivatives was called for this n
-            continue;
-        class_off[kv.first] = {(long long)pl.h_class.size(), (long long)(pl.h_class.size() + kv.second.D.size())};
-        pl.h_class.insert(pl.h_class.end(), kv.second.D.begin(), kv.second.D.end());
-        pl.h_class.insert(pl.h_class.end(), kv.second.P.begin(), kv.second.P.end());
-        pl.h_class.insert(pl.h_class.end(), kv.second.D234.begin(), kv.second.D234.end());
-        const int nn = kv.first, bc = 4 * nn - 14;
-        range_off[nn] = (long long)pl.h_ranges.size();
-        for (int r = 0; r < bc; ++r) {
-            int c0 = 4 * nn, c1 = 0;
-            for (int c = 0; c < 4 * nn; ++c)
-                if (kv.second.P[(size_t)c * bc + r] != 0.0) {
-                    c0 = std::min(c0, c);
-                    c1 = c + 1;
-                }
-            pl.h_ranges.push_back(c1 > c0 ? make_int2(c0, c1) : make_int2(0, 0));
-        }
-        for (int j = 0; j < nn; ++j) { // D_1_0 (n x n, column-major): non-zero row range of every column (banded)
-            int i0 = nn, i1 = 0;
-            for (int i = 0; i < nn; ++i)
-                if (kv.second.D[(size_t)j * nn + i] != 0.0) {
-                    i0 = std::min(i0, i);
-                    i1 = i + 1;
-                }
-            pl.h_ranges.push_back(i1 > i0 ? make_int2(i0, i1) : make_int2(0, 0));
-        }
-    }
-    pl.cD.resize((size_t)nfib), pl.cP.resize((size_t)nfib), pl.cR.resize((size_t)nfib);
-    pl.offA_f.resize((size_t)nfib), pl.offF_f.resize((size_t)nfib);
-    int max_n = 0;
-    const long long node0 = fl->h_fiber_off[(size_t)f0]; // x / fw / v / res of the own fibers are indexed from here
-    for (int f = 0; f < nfib; ++f) {
-        const int n = fl->h_fiber_n[(size_t)(f0 + f)];
-        auto it = class_off.find(n);
-        if (it == class_off.end())
-            return set_error(SKB_ERR_INVALID, "fiber %d has %d nodes but skb_flow_set_fiber_class(%d, ...) was never "
-                                              "called", f0 + f, n, n);
-        if (build && (n < kBuildMinNodes || n > kBuildMaxNodes))
-            return set_error(SKB_ERR_INVALID, "fiber %d has %d nodes: the device build takes %d <= n <= %d", f0 + f, n,
-                             kBuildMinNodes, kBuildMaxNodes);
-        if (build && fl->fiber_classes[n].D234.empty())
-            return set_error(SKB_ERR_INVALID, "fiber %d has %d nodes but skb_flow_set_fiber_class_derivatives(%d, ...) "
-                                              "was never called", f0 + f, n, n);
-        if (length_prev && !(length_prev[f] > 0))
-            return set_error(SKB_ERR_INVALID, "fiber %d: length_prev = %g", f0 + f, length_prev[f]);
-        pl.cD[f] = it->second.first;
-        pl.cP[f] = it->second.second;
-        pl.cR[f] = range_off[n];
-        pl.offA_f[f] = pl.offA;
-        pl.offF_f[f] = pl.offF;
-        max_n = std::max(max_n, n);
-        const long long node_off = fl->h_fiber_off[(size_t)(f0 + f)] - node0;
-        for (int r0 = 0; r0 < 4 * n; r0 += kFiberGemvRows)
-            pl.itA.push_back(FiberGemvItem{pl.offA, 4 * node_off, 4 * node_off, 4 * n, 4 * n, r0, n, f, 0});
-        for (int r0 = 0; r0 < 3 * n; r0 += kFiberGemvRows)
-            pl.itF.push_back(FiberGemvItem{pl.offF, 4 * node_off, node_off, 3 * n, 4 * n, r0, n, f, 0});
-        pl.offA += 16LL * n * n;
-        pl.offF += 12LL * n * n;
-    }
-    // x (4n) + slice partials + vT (4n) + s (n)
-    fl->gemv_smem = ((size_t)2 * ((4 * max_n + 1) & ~1) + kFiberGemvThreads + (size_t)max_n) * sizeof(double);
-    if (fl->gemv_smem > 200 * 1024)
-        return set_error(SKB_ERR_INVALID, "fiber with %d nodes exceeds the shared-memory fiber operator kernels", max_n);
-    if (fl->gemv_smem > 48 * 1024) {
-        CUDA_TRY(cudaFuncSetAttribute(fiber_gemv_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)fl->gemv_smem));
-        CUDA_TRY(cudaFuncSetAttribute(fiber_gemv_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)fl->gemv_smem));
-        CUDA_TRY(cudaFuncSetAttribute(fiber_gemv_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)fl->gemv_smem));
-    }
-    return SKB_OK;
-}
-
-static int put_async(skb_flow *fl, DevBuf &b, const void *h, size_t bytes) {
-    SKB_TRY(b.ensure(bytes));
-    CUDA_TRY(cudaMemcpyAsync(b.ptr, h, bytes, cudaMemcpyHostToDevice, fl->stream));
-    return SKB_OK;
-}
-
-// the plan's buffers on the device and room for the operators and the per-call vectors (on fl->stream; the caller
-// synchronises before `pl` goes out of scope)
-static int upload_fiber_plan(skb_flow *fl, const FiberOpsPlan &pl) {
-    const long long nf = fl->fb - fl->fa; // nodes of the own fibers
-    const int nfib = fl->op_f1 - fl->op_f0;
-    SKB_TRY(fl->op_A.ensure((size_t)pl.offA * 8));
-    SKB_TRY(fl->op_F.ensure((size_t)pl.offF * 8));
-    SKB_TRY(fl->op_xs.ensure((size_t)nf * 24));
-    SKB_TRY(put_async(fl, fl->op_class, pl.h_class.data(), pl.h_class.size() * 8));
-    SKB_TRY(put_async(fl, fl->op_classD, pl.cD.data(), pl.cD.size() * 8));
-    SKB_TRY(put_async(fl, fl->op_classP, pl.cP.data(), pl.cP.size() * 8));
-    SKB_TRY(put_async(fl, fl->op_classR, pl.cR.data(), pl.cR.size() * 8));
-    SKB_TRY(put_async(fl, fl->op_ranges, pl.h_ranges.data(), pl.h_ranges.size() * sizeof(int2)));
-    SKB_TRY(put_async(fl, fl->items_A, pl.itA.data(), pl.itA.size() * sizeof(FiberGemvItem)));
-    SKB_TRY(put_async(fl, fl->items_F, pl.itF.data(), pl.itF.size() * sizeof(FiberGemvItem)));
-    SKB_TRY(fl->x_fib.ensure((size_t)nf * 32));
-    SKB_TRY(fl->res_fib.ensure((size_t)nf * 32));
-    SKB_TRY(fl->vb.ensure((size_t)nfib * 56));
-    return SKB_OK;
-}
-
-static void commit_fiber_plan(skb_flow *fl, const FiberOpsPlan &pl) {
-    fl->n_items_A = (int)pl.itA.size();
-    fl->n_items_F = (int)pl.itF.size();
-    fl->op_A_elems = pl.offA;
-    fl->op_F_elems = pl.offF;
-    fl->ops_gen++;
-    fl->ops_ready = true;
-}
-
-extern "C" {
 
 int skb_flow_set_fiber_operators(skb_flow *fl, const double *A, const double *force_operator, const double *xs,
                                  const double *length_prev, const int *plus_bc_velocity) {
     if (!fl)
         return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_operators: NULL flow");
-    fl->ops_ready = false;
+    fl->ops.invalidate();
     CUDA_TRY(cudaSetDevice(fl->dev));
-    SKB_TRY(own_fibers(fl, "skb_flow_set_fiber_operators"));
-    const int nfib = fl->op_f1 - fl->op_f0;
-    if (nfib == 0) {
-        fl->n_items_A = fl->n_items_F = 0;
-        fl->ops_ready = true;
-        return SKB_OK;
-    }
-    if (!A || !force_operator || !xs || !length_prev || !plus_bc_velocity)
+    OwnFibers own;
+    SKB_TRY(own_fibers(fl, "skb_flow_set_fiber_operators", own));
+    if (own.count() > 0 && (!A || !force_operator || !xs || !length_prev || !plus_bc_velocity))
         return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_operators: NULL argument");
-    FiberOpsPlan pl;
-    SKB_TRY(plan_fiber_operators(fl, false, length_prev, pl));
-    SKB_TRY(upload_fiber_plan(fl, pl));
-    const long long nf = fl->fb - fl->fa;
-    SKB_TRY(upload_pageable(fl->op_A.ptr, A, (size_t)pl.offA * 8, fl->stream));
-    SKB_TRY(upload_pageable(fl->op_F.ptr, force_operator, (size_t)pl.offF * 8, fl->stream));
-    CUDA_TRY(cudaMemcpyAsync(fl->op_xs.ptr, xs, (size_t)nf * 24, cudaMemcpyHostToDevice, fl->stream));
-    SKB_TRY(put_async(fl, fl->op_len, length_prev, (size_t)nfib * 8));
-    SKB_TRY(put_async(fl, fl->op_plus, plus_bc_velocity, (size_t)nfib * sizeof(int)));
-    CUDA_TRY(cudaStreamSynchronize(fl->stream)); // the host vectors above go out of scope
-    commit_fiber_plan(fl, pl);
-    return SKB_OK;
+    return fl->ops.upload(own, A, force_operator, xs, length_prev, plus_bc_velocity);
 }
 
 int skb_flow_set_fiber_preconditioner(skb_flow *fl, const double *A_inv) {
     if (!fl)
         return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_preconditioner: NULL flow");
-    if (!fl->ops_ready)
-        return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_preconditioner: call skb_flow_set_fiber_operators "
-                                          "first (it defines the fibers and their order)");
-    if (fl->op_A_elems > 0) {
-        if (!A_inv)
-            return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_preconditioner: NULL argument");
-        CUDA_TRY(cudaSetDevice(fl->dev));
-        SKB_TRY(fl->op_Ainv.ensure((size_t)fl->op_A_elems * 8));
-        SKB_TRY(upload_pageable(fl->op_Ainv.ptr, A_inv, (size_t)fl->op_A_elems * 8, fl->stream));
-    }
-    fl->precond_gen = fl->ops_gen;
-    return SKB_OK;
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    return fl->ops.upload_inverse(A_inv, fl->stream);
 }
 
 int skb_flow_build_fiber_operators(skb_flow *fl, const skb_fiber_params *params, double dt, double eta) {
-    static_assert(sizeof(skb_fiber_params) == 48 && sizeof(FiberParamsDev) == 48, "skb_fiber_params layout");
     const char *who = "skb_flow_build_fiber_operators";
     if (!fl)
         return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    fl->ops_ready = false;
+    fl->ops.invalidate();
     if (!(dt > 0) || !(eta > 0))
         return set_error(SKB_ERR_INVALID, "%s: dt = %g, eta = %g (both must be > 0)", who, dt, eta);
     CUDA_TRY(cudaSetDevice(fl->dev));
-    SKB_TRY(own_fibers(fl, who));
-    const int f0 = fl->op_f0, nfib = fl->op_f1 - fl->op_f0;
-    if (nfib > 0 && !params)
+    OwnFibers own;
+    SKB_TRY(own_fibers(fl, who, own));
+    if (own.count() > 0 && !params)
         return set_error(SKB_ERR_INVALID, "%s: NULL params", who);
-    for (int f = 0; f < nfib; ++f) {
-        const skb_fiber_params &p = params[f];
-        if (!(p.length_prev > 0) || !(p.radius > 0))
-            return set_error(SKB_ERR_INVALID, "fiber %d: length_prev = %g, radius = %g (both must be > 0)", f0 + f,
-                             p.length_prev, p.radius);
-        if ((p.minus_clamped != 0 && p.minus_clamped != 1) || (p.plus_hinged != 0 && p.plus_hinged != 1))
-            return set_error(SKB_ERR_INVALID, "fiber %d: minus_clamped = %d, plus_hinged = %d (each must be 0 or 1)",
-                             f0 + f, p.minus_clamped, p.plus_hinged);
-    }
-    FiberOpsPlan pl;
-    if (nfib == 0) {
-        commit_fiber_plan(fl, pl);
-        fl->precond_gen = fl->ops_gen;
-        return SKB_OK;
-    }
-    SKB_TRY(plan_fiber_operators(fl, true, nullptr, pl));
-    // per fiber: where its operators, nodes and class matrices are; per tile of columns: one assembly CTA; per node
-    // count: the matrices the inverse kernel takes in one launch
-    std::vector<FiberBuildItem> items((size_t)nfib);
-    std::vector<FiberTileItem> tiles;
-    std::vector<double> lp((size_t)nfib);
-    std::vector<int> plus((size_t)nfib);
-    std::map<int, std::vector<long long>> inv_by_n;
-    size_t smem = 0;
-    const long long node0 = fl->h_fiber_off[(size_t)f0];
-    for (int f = 0; f < nfib; ++f) {
-        const int n = fl->h_fiber_n[(size_t)(f0 + f)];
-        const long long node = fl->h_fiber_off[(size_t)(f0 + f)];
-        items[f] = FiberBuildItem{pl.offA_f[f], pl.offF_f[f], node, node - node0, pl.cD[f], pl.cR[f], n, f0 + f};
-        for (int c = 0; c < 4 * n; c += build_tile_cols(n))
-            tiles.push_back(FiberTileItem{f, c});
-        smem = std::max(smem, build_smem_bytes(n));
-        inv_by_n[n].push_back(pl.offA_f[f]);
-        lp[f] = params[f].length_prev;
-        plus[f] = params[f].plus_hinged;
-    }
-    std::vector<long long> inv_off;
-    for (const auto &kv : inv_by_n)
-        inv_off.insert(inv_off.end(), kv.second.begin(), kv.second.end());
-    begin_stats(fl);
-    CUDA_TRY(cudaEventRecord(fl->evt0, fl->stream));
-    SKB_TRY(upload_fiber_plan(fl, pl));
-    SKB_TRY(fl->op_Ainv.ensure((size_t)pl.offA * 8));
-    SKB_TRY(put_async(fl, fl->op_len, lp.data(), lp.size() * 8));
-    SKB_TRY(put_async(fl, fl->op_plus, plus.data(), plus.size() * sizeof(int)));
-    SKB_TRY(put_async(fl, fl->bld_params, params, (size_t)nfib * sizeof(skb_fiber_params)));
-    SKB_TRY(put_async(fl, fl->bld_items, items.data(), items.size() * sizeof(FiberBuildItem)));
-    SKB_TRY(put_async(fl, fl->bld_tiles, tiles.data(), tiles.size() * sizeof(FiberTileItem)));
-    SKB_TRY(put_async(fl, fl->bld_inv, inv_off.data(), inv_off.size() * sizeof(long long)));
-
-    BuildArgs ba;
-    ba.items = (const FiberBuildItem *)fl->bld_items.ptr;
-    ba.tiles = (const FiberTileItem *)fl->bld_tiles.ptr;
-    ba.params = (const FiberParamsDev *)fl->bld_params.ptr;
-    ba.class_mats = (const double *)fl->op_class.ptr;
-    ba.row_range = (const int2 *)fl->op_ranges.ptr;
-    ba.r_fib = (const double *)fl->r_fib.ptr;
-    ba.length = (const double *)fl->fiber_length.ptr;
-    ba.dt = dt;
-    ba.eta = eta;
-    ba.A = (double *)fl->op_A.ptr;
-    ba.F = (double *)fl->op_F.ptr;
-    ba.xs = (double *)fl->op_xs.ptr;
-    CUDA_TRY(cudaEventRecord(fl->ev0, fl->stream));
-    fiber_assemble_kernel<<<(unsigned)tiles.size(), kBuildThreads, smem, fl->stream>>>(ba);
-    SKB_TRY(launched(fl, 1));
-    size_t first = 0;
-    for (const auto &kv : inv_by_n) {
-        const int m = 4 * kv.first, cs = inverse_cluster_size(m);
-        cudaLaunchConfig_t cfg = {};
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = (unsigned)cs;
-        attr[0].val.clusterDim.y = attr[0].val.clusterDim.z = 1;
-        cfg.gridDim = dim3((unsigned)(kv.second.size() * cs));
-        cfg.blockDim = dim3(kInverseThreads);
-        cfg.dynamicSmemBytes = inverse_smem_bytes(m, cs);
-        cfg.stream = fl->stream;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
-        void (*kern)(const long long *, const double *, double *, int) =
-            m <= 128 ? fiber_inverse_kernel<4> : fiber_inverse_kernel<16>;
-        if (cs > 1) {
-            int n_clusters = 0;
-            CUDA_TRY(cudaOccupancyMaxActiveClusters(&n_clusters, kern, &cfg));
-            if (n_clusters < 1)
-                return set_error(SKB_ERR_CUDA, "%s: a cluster of %d CTAs x %zu bytes of shared memory (n = %d) does not "
-                                               "fit on device %d", who, cs, cfg.dynamicSmemBytes, kv.first, fl->dev);
-        }
-        CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, (const long long *)fl->bld_inv.ptr + first,
-                                    (const double *)fl->op_A.ptr, (double *)fl->op_Ainv.ptr, m));
-        SKB_TRY(launched(fl, 1));
-        first += kv.second.size();
-    }
-    CUDA_TRY(cudaEventRecord(fl->ev1, fl->stream));
-    CUDA_TRY(cudaEventRecord(fl->evt1, fl->stream));
-    SKB_TRY(finish_stats(fl)); // (synchronises: the host vectors above go out of scope)
-    commit_fiber_plan(fl, pl);
-    fl->precond_gen = fl->ops_gen; // the inverse belongs to these operators
-    return SKB_OK;
+    // device_ms spans the assembly and inverse kernels, total_ms also the table uploads before them
+    return fl->ops.build(own, params, dt, eta, &fl->launches,
+                         [&](const FiberOps::Step &stage, const FiberOps::Step &launch) {
+                             begin_stats(fl);
+                             return host_frame(fl, stage, launch, nothing);
+                         });
 }
-
-} // extern "C"
-
-// (prepare_device, skb_runtime.cu: this is the translation unit that holds the build kernels)
-int skb::prepare_fiber_build_kernels() {
-    for (auto kern : {fiber_inverse_kernel<4>, fiber_inverse_kernel<16>}) {
-        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kInverseSmemMax));
-        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-    }
-    return SKB_OK;
-}
-
-static int need_ops(const skb_flow *fl, const char *who) {
-    if (!fl->ops_ready)
-        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_fiber_operators after skb_flow_set_fibers / "
-                                          "skb_flow_set_fiber_class first", who);
-    return SKB_OK;
-}
-
-// fw = force_operator_ * x per fiber, scattered to 3 x N_f (fcfd.cpp:272-287); on fl->cur
-static int fiber_force_dev(skb_flow *fl, const double *d_x, double *d_fw) {
-    if (fl->n_items_F == 0)
-        return SKB_OK;
-    fiber_gemv_kernel<1><<<fl->n_items_F, kFiberGemvThreads, fl->gemv_smem, fl->cur>>>(
-        (const FiberGemvItem *)fl->items_F.ptr, (const double *)fl->op_F.ptr, d_x, d_fw, FiberVelArgs{});
-    return launched(fl, 1);
-}
-
-// res = A_ x - P_downsample_bc vT(v) + xs_vT + y_BC per fiber (ffd.cpp:276-312), one launch; on fl->cur
-static int fiber_matvec_dev(skb_flow *fl, const double *d_x, const double *d_v, const double *d_vb, double *d_res) {
-    if (fl->n_items_A == 0)
-        return SKB_OK;
-    FiberVelArgs va;
-    va.xs = (const double *)fl->op_xs.ptr;
-    va.v = d_v;
-    va.length_prev = (const double *)fl->op_len.ptr;
-    va.plus_velocity = (const int *)fl->op_plus.ptr;
-    va.class_mats = (const double *)fl->op_class.ptr;
-    va.class_D = (const long long *)fl->op_classD.ptr;
-    va.class_P = (const long long *)fl->op_classP.ptr;
-    va.row_range = (const int2 *)fl->op_ranges.ptr;
-    va.class_R = (const long long *)fl->op_classR.ptr;
-    va.v_boundary = d_vb;
-    fiber_gemv_kernel<2><<<fl->n_items_A, kFiberGemvThreads, fl->gemv_smem, fl->cur>>>(
-        (const FiberGemvItem *)fl->items_A.ptr, (const double *)fl->op_A.ptr, d_x, d_res, va);
-    return launched(fl, 1);
-}
-
-// y = A_^-1 x per fiber: FiberContainerFiniteDifference::apply_preconditioner (fcfd.cpp:331-339) with the LU solve
-// replaced by a GEMV over the explicit inverse (same shapes and item list as A_); on fl->cur
-static int fiber_precond_dev(skb_flow *fl, const double *d_x, double *d_y) {
-    if (fl->n_items_A == 0)
-        return SKB_OK;
-    fiber_gemv_kernel<0><<<fl->n_items_A, kFiberGemvThreads, fl->gemv_smem, fl->cur>>>(
-        (const FiberGemvItem *)fl->items_A.ptr, (const double *)fl->op_Ainv.ptr, d_x, d_y, FiberVelArgs{});
-    return launched(fl, 1);
-}
-
-static int need_precond(const skb_flow *fl, const char *who) {
-    SKB_TRY(need_ops(fl, who));
-    if (fl->precond_gen != fl->ops_gen)
-        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_fiber_preconditioner after "
-                                          "skb_flow_set_fiber_operators first", who);
-    return SKB_OK;
-}
-
-extern "C" {
 
 int skb_flow_get_fiber_operators(skb_flow *fl, double *A, double *force_operator, double *xs, double *A_inv) {
+    const char *who = "skb_flow_get_fiber_operators";
     if (!fl)
-        return set_error(SKB_ERR_INVALID, "skb_flow_get_fiber_operators: NULL flow");
-    SKB_TRY(need_ops(fl, "skb_flow_get_fiber_operators"));
-    if (A_inv)
-        SKB_TRY(need_precond(fl, "skb_flow_get_fiber_operators"));
-    if (fl->n_items_A == 0)
-        return SKB_OK;
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    SKB_TRY(fl->ops.ready(who, A_inv != nullptr));
     CUDA_TRY(cudaSetDevice(fl->dev));
-    CUDA_TRY(cudaStreamSynchronize(fl->stream));
-    if (A)
-        CUDA_TRY(cudaMemcpy(A, fl->op_A.ptr, (size_t)fl->op_A_elems * 8, cudaMemcpyDeviceToHost));
-    if (force_operator)
-        CUDA_TRY(cudaMemcpy(force_operator, fl->op_F.ptr, (size_t)fl->op_F_elems * 8, cudaMemcpyDeviceToHost));
-    if (xs)
-        CUDA_TRY(cudaMemcpy(xs, fl->op_xs.ptr, (size_t)(fl->fb - fl->fa) * 24, cudaMemcpyDeviceToHost));
-    if (A_inv)
-        CUDA_TRY(cudaMemcpy(A_inv, fl->op_Ainv.ptr, (size_t)fl->op_A_elems * 8, cudaMemcpyDeviceToHost));
-    return SKB_OK;
+    return fl->ops.read(A, force_operator, xs, A_inv, fl->stream);
 }
 
+// host pointers: through host_frame on the flow's stream; device pointers: asynchronously on the caller's stream
 int skb_flow_apply_fiber_preconditioner(skb_flow *fl, const double *x_fibers, double *y) {
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "skb_flow_apply_fiber_preconditioner: NULL flow");
-    SKB_TRY(need_precond(fl, "skb_flow_apply_fiber_preconditioner"));
-    const long long nf = fl->fb - fl->fa;
-    begin_stats(fl);
-    if (nf == 0)
-        return SKB_OK;
-    if (!x_fibers || !y)
-        return set_error(SKB_ERR_INVALID, "skb_flow_apply_fiber_preconditioner: NULL argument");
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    return host_frame(
-        fl, [&] { return upload(fl, fl->x_fib, x_fibers, (size_t)nf * 4); },
-        [&] { return fiber_precond_dev(fl, (const double *)fl->x_fib.ptr, (double *)fl->res_fib.ptr); },
-        [&] { return download(fl, y, fl->res_fib, (size_t)nf * 4); });
+    return fiber_ops_call(fl, "skb_flow_apply_fiber_preconditioner", true, x_fibers && y, [&](size_t nf) {
+        SKB_TRY(fl->res_fib.ensure(nf * 32));
+        return host_frame(
+            fl, [&] { return upload(fl, fl->x_fib, x_fibers, nf * 4); },
+            [&] {
+                return fl->ops.precondition((const double *)fl->x_fib.ptr, (double *)fl->res_fib.ptr, fl->cur,
+                                            &fl->launches);
+            },
+            [&] { return download(fl, y, fl->res_fib, nf * 4); });
+    });
 }
 
 int skb_flow_apply_fiber_preconditioner_device(skb_flow *fl, const double *d_x_fibers, double *d_y, void *stream) {
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "skb_flow_apply_fiber_preconditioner_device: NULL flow");
-    SKB_TRY(need_precond(fl, "skb_flow_apply_fiber_preconditioner_device"));
-    begin_stats(fl);
-    if (fl->n_items_A == 0)
-        return SKB_OK;
-    if (!d_x_fibers || !d_y)
-        return set_error(SKB_ERR_INVALID, "skb_flow_apply_fiber_preconditioner_device: NULL argument");
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    fl->cur = (cudaStream_t)stream;
-    SKB_TRY(fiber_precond_dev(fl, d_x_fibers, d_y));
-    return device_stats(fl);
+    return fiber_ops_call(fl, "skb_flow_apply_fiber_preconditioner_device", true, d_x_fibers && d_y, [&](size_t) {
+        fl->cur = (cudaStream_t)stream;
+        SKB_TRY(fl->ops.precondition(d_x_fibers, d_y, fl->cur, &fl->launches));
+        return device_stats(fl);
+    });
 }
 
 int skb_flow_apply_fiber_force(skb_flow *fl, const double *x_fibers, double *fw) {
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "skb_flow_apply_fiber_force: NULL flow");
-    SKB_TRY(need_ops(fl, "skb_flow_apply_fiber_force"));
-    const long long nf = fl->fb - fl->fa; // nodes of the own fibers (all of them without a window)
-    begin_stats(fl);
-    if (nf == 0)
-        return SKB_OK;
-    if (!x_fibers || !fw)
-        return set_error(SKB_ERR_INVALID, "skb_flow_apply_fiber_force: NULL argument");
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    return host_frame(
-        fl,
-        [&]() -> int {
-            SKB_TRY(upload(fl, fl->x_fib, x_fibers, (size_t)nf * 4));
-            return fl->in_fib.ensure((size_t)nf * 24);
-        },
-        [&] { return fiber_force_dev(fl, (const double *)fl->x_fib.ptr, (double *)fl->in_fib.ptr); },
-        [&] { return download(fl, fw, fl->in_fib, (size_t)nf * 3); });
+    return fiber_ops_call(fl, "skb_flow_apply_fiber_force", false, x_fibers && fw, [&](size_t nf) {
+        return host_frame(
+            fl,
+            [&]() -> int {
+                SKB_TRY(upload(fl, fl->x_fib, x_fibers, nf * 4));
+                return fl->in_fib.ensure(nf * 24);
+            },
+            [&] {
+                return fl->ops.force((const double *)fl->x_fib.ptr, (double *)fl->in_fib.ptr, fl->cur, &fl->launches);
+            },
+            [&] { return download(fl, fw, fl->in_fib, nf * 3); });
+    });
 }
 
 int skb_flow_fiber_matvec(skb_flow *fl, const double *x_fibers, const double *v_fibers, const double *v_fib_boundary,
                           double *res) {
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "skb_flow_fiber_matvec: NULL flow");
-    SKB_TRY(need_ops(fl, "skb_flow_fiber_matvec"));
-    const long long nf = fl->fb - fl->fa;
-    begin_stats(fl);
-    if (nf == 0)
-        return SKB_OK;
-    if (!x_fibers || !v_fibers || !res)
-        return set_error(SKB_ERR_INVALID, "skb_flow_fiber_matvec: NULL argument");
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    return host_frame(
-        fl,
-        [&]() -> int {
-            SKB_TRY(upload(fl, fl->x_fib, x_fibers, (size_t)nf * 4));
-            SKB_TRY(upload(fl, fl->vel, v_fibers, (size_t)nf * 3));
-            return v_fib_boundary ? upload(fl, fl->vb, v_fib_boundary, (size_t)(fl->op_f1 - fl->op_f0) * 7) : SKB_OK;
-        },
-        [&] {
-            return fiber_matvec_dev(fl, (const double *)fl->x_fib.ptr, (const double *)fl->vel.ptr,
-                                    v_fib_boundary ? (const double *)fl->vb.ptr : nullptr, (double *)fl->res_fib.ptr);
-        },
-        [&] { return download(fl, res, fl->res_fib, (size_t)nf * 4); });
+    return fiber_ops_call(fl, "skb_flow_fiber_matvec", false, x_fibers && v_fibers && res, [&](size_t nf) {
+        SKB_TRY(fl->res_fib.ensure(nf * 32));
+        return host_frame(
+            fl,
+            [&]() -> int {
+                SKB_TRY(upload(fl, fl->x_fib, x_fibers, nf * 4));
+                SKB_TRY(upload(fl, fl->vel, v_fibers, nf * 3));
+                return v_fib_boundary ? upload(fl, fl->vb, v_fib_boundary, (size_t)fl->ops.n_fibers() * 7) : SKB_OK;
+            },
+            [&] {
+                return fl->ops.matvec((const double *)fl->x_fib.ptr, (const double *)fl->vel.ptr,
+                                      v_fib_boundary ? (const double *)fl->vb.ptr : nullptr,
+                                      (double *)fl->res_fib.ptr, fl->cur, &fl->launches);
+            },
+            [&] { return download(fl, res, fl->res_fib, nf * 4); });
+    });
 }
 
 int skb_flow_apply_fiber_force_device(skb_flow *fl, const double *d_x_fibers, double *d_fw, void *stream) {
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "skb_flow_apply_fiber_force_device: NULL flow");
-    SKB_TRY(need_ops(fl, "skb_flow_apply_fiber_force_device"));
-    begin_stats(fl);
-    if (fl->n_items_F == 0)
-        return SKB_OK;
-    if (!d_x_fibers || !d_fw)
-        return set_error(SKB_ERR_INVALID, "skb_flow_apply_fiber_force_device: NULL argument");
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    fl->cur = (cudaStream_t)stream;
-    SKB_TRY(fiber_force_dev(fl, d_x_fibers, d_fw));
-    return device_stats(fl);
+    return fiber_ops_call(fl, "skb_flow_apply_fiber_force_device", false, d_x_fibers && d_fw, [&](size_t) {
+        fl->cur = (cudaStream_t)stream;
+        SKB_TRY(fl->ops.force(d_x_fibers, d_fw, fl->cur, &fl->launches));
+        return device_stats(fl);
+    });
 }
 
 int skb_flow_fiber_matvec_device(skb_flow *fl, const double *d_x_fibers, const double *d_v_fibers,
                                  const double *d_v_fib_boundary, double *d_res, void *stream) {
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "skb_flow_fiber_matvec_device: NULL flow");
-    SKB_TRY(need_ops(fl, "skb_flow_fiber_matvec_device"));
-    begin_stats(fl);
-    if (fl->n_items_A == 0)
-        return SKB_OK;
-    if (!d_x_fibers || !d_v_fibers || !d_res)
-        return set_error(SKB_ERR_INVALID, "skb_flow_fiber_matvec_device: NULL argument");
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    fl->cur = (cudaStream_t)stream;
-    SKB_TRY(fiber_matvec_dev(fl, d_x_fibers, d_v_fibers, d_v_fib_boundary, d_res));
-    return device_stats(fl);
+    return fiber_ops_call(fl, "skb_flow_fiber_matvec_device", false, d_x_fibers && d_v_fibers && d_res, [&](size_t) {
+        fl->cur = (cudaStream_t)stream;
+        SKB_TRY(fl->ops.matvec(d_x_fibers, d_v_fibers, d_v_fib_boundary, d_res, fl->cur, &fl->launches));
+        return device_stats(fl);
+    });
 }
 
 } // extern "C"
@@ -1958,11 +1555,11 @@ static int apply_matvec_core(skb_flow *fl, skb_dense *dn, const double *d_x, con
         B.dn = dn;
     }
     // MatrixXd fw = fc.apply_fiber_force(x_fibers)                       system.cpp:298
-    SKB_TRY(fiber_force_dev(fl, d_x, (double *)fl->in_fib.ptr));
+    SKB_TRY(fl->ops.force(d_x, (double *)fl->in_fib.ptr, fl->cur, &fl->launches));
     // v_all of system.cpp:299-316 (own rows)
     SKB_TRY(matvec_core(fl, (const double *)fl->in_fib.ptr, d_xs, d_bd, d_f, d_t, eta, (double *)fl->vel.ptr));
     // res_fibers = fc.matvec(x_fibers, v_fibers, fiber_link_conditions)   system.cpp:318
-    SKB_TRY(fiber_matvec_dev(fl, d_x, (const double *)fl->vel.ptr, d_link, d_res_fib));
+    SKB_TRY(fl->ops.matvec(d_x, (const double *)fl->vel.ptr, d_link, d_res_fib, fl->cur, &fl->launches));
     const double *d_v_shell = (const double *)fl->vel.ptr + 3 * n_fw;
     if (n_sw > 0 && d_out_shell) {
         if (dense_rows && B.launched) {
@@ -2011,7 +1608,7 @@ static int apply_matvec_impl(skb_flow *fl, skb_dense *dn, const double *x_fibers
                              double *v_bodies) {
     if (!fl || !(eta > 0))
         return set_error(SKB_ERR_INVALID, "skb_flow_apply_matvec: bad arguments");
-    SKB_TRY(need_ops(fl, "skb_flow_apply_matvec"));
+    SKB_TRY(fl->ops.ready("skb_flow_apply_matvec"));
     const long long nf = fl->n_fib, ns = fl->n_shell, nb = fl->n_body, n_all = nf + ns + nb;
     if ((nf > 0 && (!x_fibers || !res_fibers)) || (ns > 0 && (!shell_density || !v_shell)) ||
         (nb > 0 && (!body_densities || !v_bodies)) || (fl->n_bodies > 0 && !body_forces_torques))
@@ -2034,11 +1631,12 @@ static int apply_matvec_impl(skb_flow *fl, skb_dense *dn, const double *x_fibers
         [&]() -> int {
             SKB_TRY(upload(fl, fl->x_fib, x_fibers, (size_t)nf * 4));
             if (link)
-                SKB_TRY(upload(fl, fl->vb, fiber_link_conditions, (size_t)(fl->op_f1 - fl->op_f0) * 7));
+                SKB_TRY(upload(fl, fl->vb, fiber_link_conditions, (size_t)fl->ops.n_fibers() * 7));
             SKB_TRY(upload(fl, fl->in_shell, shell_density, (size_t)ns * 3));
             SKB_TRY(upload(fl, fl->in_body, body_densities, (size_t)nb * 3));
             SKB_TRY(upload(fl, fl->in_force, f.data(), f.size()));
             SKB_TRY(upload(fl, fl->in_torque, t.data(), t.size()));
+            SKB_TRY(fl->res_fib.ensure((size_t)nf * 32));
             SKB_TRY(fl->res_shell.ensure((size_t)ns * 24 + 8));
             return fl->tmp_b.ensure((size_t)nb * 24 + 8);
         },
@@ -2083,7 +1681,7 @@ int skb_flow_apply_matvec_device(skb_flow *fl, skb_dense *dn, const double *d_x_
                                  double *d_res_fibers, double *d_out_shell, double *d_v_bodies, void *stream) {
     if (!fl || !(eta > 0))
         return set_error(SKB_ERR_INVALID, "skb_flow_apply_matvec_device: bad arguments");
-    SKB_TRY(need_ops(fl, "skb_flow_apply_matvec_device"));
+    SKB_TRY(fl->ops.ready("skb_flow_apply_matvec_device"));
     CUDA_TRY(cudaSetDevice(fl->dev));
     begin_stats(fl);
     SKB_TRY(prepare_matvec_targets(fl));

@@ -317,20 +317,6 @@ int upload_pageable(void *d_dst, const void *h_src, size_t bytes, cudaStream_t s
 
 using namespace skb;
 
-#define CUDA_TRY(expr)                                                                                                \
-    do {                                                                                                              \
-        cudaError_t _e = (expr);                                                                                      \
-        if (_e != cudaSuccess)                                                                                        \
-            return set_error(SKB_ERR_CUDA, "%s failed at %s:%d: %s", #expr, __FILE__, __LINE__,                      \
-                             cudaGetErrorString(_e));                                                                 \
-    } while (0)
-#define SKB_TRY(expr)                                                                                                 \
-    do {                                                                                                              \
-        int _rc = (expr);                                                                                             \
-        if (_rc != SKB_OK)                                                                                            \
-            return _rc;                                                                                               \
-    } while (0)
-
 // The launch attributes of every kernel that has them: the dynamic shared memory of the kernels that use more than the
 // default 48 KB, and the max-shared carve-out of pair_sym_kernel, pair_cross_kernel and the background row streamer
 // that runs beside them (an SM switches its shared-memory configuration only when idle, so a different preference would
@@ -370,7 +356,7 @@ int skb::prepare_device(int dev) {
     CUDA_TRY(set_shared(pair_sym_kernel<kSymT, kSymMinB, true>, SymSmem<kSymT>::total_bytes));
     CUDA_TRY(set_shared(pair_cross_kernel<kCrossT, kCrossMinB>, CrossSmem<kCrossT>::total_bytes));
     CUDA_TRY(set_shared(dense_stream_kernel, kStreamSmemBytes));
-    SKB_TRY(prepare_fiber_build_kernels());
+    SKB_TRY(prepare_fiber_kernels());
     if (dev >= (int)done.size())
         done.resize(dev + 1);
     done[dev] = true;
