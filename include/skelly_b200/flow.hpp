@@ -155,6 +155,25 @@ template <class M> class FlowEngineT {
             throw std::runtime_error("skelly_b200: build_fiber_operators needs one entry per fiber of set_fibers");
         check(skb_flow_build_fiber_operators(st_->fl, params.data(), dt, eta), "skb_flow_build_fiber_operators");
     }
+    /// The fiber block of System::get_rhs (4 N_f) as System::prep_state_for_solver leaves it: fc.update_rhs(dt,
+    /// v_on_fibers, motor + f_external), then fc.apply_bcs(dt, v_on_fibers, f_external), formed on the device.
+    /// v_growth / force_scale per fiber (empty: zero growth / no motors); v_on_fibers / f_external 3 x N_f (size 0: the
+    /// reference's empty matrix).  Needs set_fiber_class and set_fiber_class_derivatives, not the operators.
+    M build_fiber_rhs(const std::vector<skb_fiber_params> &params, const std::vector<double> &v_growth,
+                      const std::vector<double> &force_scale, const M &v_on_fibers, const M &f_external, double dt,
+                      double eta) const {
+        const size_t nfib = st_->n_nodes.size();
+        if (params.size() != nfib || (!v_growth.empty() && v_growth.size() != nfib) ||
+            (!force_scale.empty() && force_scale.size() != nfib))
+            throw std::runtime_error("skelly_b200: build_fiber_rhs needs one entry per fiber of set_fibers");
+        M rhs = M::Zero(4 * st_->n_fib, 1);
+        check(skb_flow_build_fiber_rhs(st_->fl, params.data(), v_growth.empty() ? nullptr : v_growth.data(),
+                                       force_scale.empty() ? nullptr : force_scale.data(),
+                                       v_on_fibers.size() > 0 ? v_on_fibers.data() : nullptr,
+                                       f_external.size() > 0 ? f_external.data() : nullptr, dt, eta, rhs.data()),
+              "skb_flow_build_fiber_rhs");
+        return rhs;
+    }
     /// The resident operators back, in set_fiber_operators' layouts: A / A_inv the concatenated column-major 4n x 4n
     /// matrices, force_operator the 3n x 4n ones, xs 3 x N_f
     void get_fiber_operators(std::vector<double> &A, std::vector<double> &force_operator, M &xs,

@@ -203,8 +203,8 @@ SKB_API int skb_flow_apply_fiber_preconditioner_device(skb_flow *fl, const doubl
  * update_linear_operator (:97-187), update_force_operator (:317-335), the operator half of apply_bc_rectangular
  * (`A_ = P_downsample_bc * A_` plus the 14 boundary rows, :347-512) and update_preconditioner (`A_LU_.compute(A_)`,
  * :340) -- from the positions and lengths of the last skb_flow_set_fibers and a few scalars per fiber, instead of
- * uploading A_, force_operator_ and A_^-1 (about 1 GB per timestep at 3000 fibers x 32 nodes).  The RHS (update_RHS
- * and the RHS half of apply_bc_rectangular) stays with the caller.
+ * uploading A_, force_operator_ and A_^-1 (about 1 GB per timestep at 3000 fibers x 32 nodes).  The fiber block of the
+ * RHS (update_RHS and the RHS half of apply_bc_rectangular) is formed on the device too: skb_flow_build_fiber_rhs.
  *
  * skb_flow_set_fiber_class_derivatives: the higher derivative matrices of FiberFiniteDifference::matrices_.at(n)
  *   (:537-540), stored pre-transposed exactly like the reference (column-major n x n each).  The build needs them,
@@ -235,6 +235,36 @@ typedef struct skb_fiber_params {   /* one per fiber, 48 bytes */
  * a singular A_ (condition number ~1e18 for every n), and its inverse is meaningless.
  * skb_flow_last_stats afterwards: device_ms = the build's kernels, total_ms = with the upload of its per-fiber tables. */
 SKB_API int skb_flow_build_fiber_operators(skb_flow *fl, const skb_fiber_params *params, double dt, double eta);
+
+/* The fiber block of System::get_rhs (fcfd.cpp:319-328) as System::prep_state_for_solver leaves it (system.cpp:416-453):
+ * RHS_ of every fiber after fc.update_rhs(dt, v_on_fibers, motor + f_external) and fc.apply_bcs(dt, v_on_fibers,
+ * f_external) -- update_derivatives, FiberFiniteDifference::update_RHS (fiber_finite_difference.cpp:198-274) and the RHS
+ * half of apply_bc_rectangular (:358-504) -- from the positions and lengths of the last skb_flow_set_fibers.
+ *   rhs: 4 per own node, [x; y; z; T] per fiber in container order.  Rows [0, 4n-14) of a fiber are
+ *        P_downsample_bc * RHS_ of update_RHS, rows [4n-14, 4n) the 14 boundary entries of the branches the flags of
+ *        `params` select (the same flags as skb_flow_build_fiber_operators).
+ *   params: as for skb_flow_build_fiber_operators (length_prev for xs_ / xss_, radius -> c_0 with length_).
+ *   v_growth: v_growth_ per own fiber (s_dot = (1 + alpha) v_growth / 2); NULL: all zero.
+ *   force_scale: force_scale_ per own fiber: the motor force force_scale_ xs_ (generate_constant_force,
+ *        fcfd.cpp:160-169) is added to f_external in update_RHS only; NULL: no motors.
+ *   v_on_fibers, f_external: 3 x N_own, the flow at the fiber nodes and the external force; NULL: the reference's empty
+ *        matrix (`flow.size() == 0`).  The boundary entries see f_external alone.
+ * Needs skb_flow_set_fiber_class and skb_flow_set_fiber_class_derivatives for every node count in use, not the
+ * operators: it works whether they were uploaded, built or never set, and leaves them and their inverse untouched.
+ * Under skb_flow_set_target_ranges (or a window that cuts no fiber) every array holds the own fibers only.  Refused
+ * (SKB_ERR_INVALID, before any launch): what skb_flow_build_fiber_operators refuses, a non-finite v_growth or
+ * force_scale, NULL params or rhs.  skb_flow_last_stats afterwards: device_ms = the kernel, total_ms = with the uploads
+ * of the inputs and the per-fiber tables and the download of rhs.
+ * The _device form takes d_v_on_fibers, d_f_external and d_rhs on this flow's device and works on `stream`.  Its small
+ * per-fiber tables come from host memory: it returns once they are staged, without waiting for the kernel (not
+ * capturable into a CUDA graph).  Its stats count the launch, with no timings. */
+SKB_API int skb_flow_build_fiber_rhs(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
+                                     const double *force_scale, const double *v_on_fibers, const double *f_external,
+                                     double dt, double eta, double *rhs);
+SKB_API int skb_flow_build_fiber_rhs_device(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
+                                            const double *force_scale, const double *d_v_on_fibers,
+                                            const double *d_f_external, double dt, double eta, double *d_rhs,
+                                            void *stream);
 
 /* read the resident operators back, same layouts as skb_flow_set_fiber_operators / _preconditioner (own fibers);
  * NULL skips an array */
@@ -318,6 +348,10 @@ SKB_API int skb_mflow_set_fiber_class_derivatives(skb_mflow *mf, int n_nodes, co
                                                   const double *D_3_0, const double *D_4_0);
 /* params of ALL fibers; every member builds its own slice on its own device, in parallel */
 SKB_API int skb_mflow_build_fiber_operators(skb_mflow *mf, const skb_fiber_params *params, double dt, double eta);
+/* skb_flow_build_fiber_rhs with the complete arrays of ALL fibers; every member forms its own slice of rhs */
+SKB_API int skb_mflow_build_fiber_rhs(skb_mflow *mf, const skb_fiber_params *params, const double *v_growth,
+                                      const double *force_scale, const double *v_on_fibers, const double *f_external,
+                                      double dt, double eta, double *rhs);
 /* op = skb_dense_op (skelly_b200_dense.h); A row-major (3 N_s) x (3 N_s) */
 SKB_API int skb_mflow_set_dense(skb_mflow *mf, int op, const double *A_rowmajor, int64_t n_rows, int64_t n_cols);
 SKB_API int skb_mflow_matvec(skb_mflow *mf, const double *fib_forces, const double *shell_density,

@@ -173,6 +173,12 @@ def library() -> C.CDLL:
         "skb_flow_set_fiber_class_derivatives": ([ctxp, C.c_int, _dp, _dp, _dp], C.c_int),
         "skb_flow_build_fiber_operators": ([ctxp, C.POINTER(FiberParams), C.c_double, C.c_double], C.c_int),
         "skb_flow_get_fiber_operators": ([ctxp, _dp, _dp, _dp, _dp], C.c_int),
+        "skb_flow_build_fiber_rhs": ([ctxp, C.POINTER(FiberParams), _dp, _dp, _dp, _dp, C.c_double, C.c_double, _dp],
+                                     C.c_int),
+        "skb_flow_build_fiber_rhs_device": ([ctxp, C.POINTER(FiberParams), _dp, _dp, C.c_void_p, C.c_void_p,
+                                             C.c_double, C.c_double, C.c_void_p, C.c_void_p], C.c_int),
+        "skb_mflow_build_fiber_rhs": ([ctxp, C.POINTER(FiberParams), _dp, _dp, _dp, _dp, C.c_double, C.c_double, _dp],
+                                      C.c_int),
         "skb_flow_apply_matvec": ([ctxp, _dp, _dp, _dp, _dp, _dp, C.c_double, _dp, _dp, _dp], C.c_int),
         "skb_flow_apply_matvec_dense": ([ctxp, ctxp, _dp, _dp, _dp, _dp, _dp, C.c_double, _dp, _dp, _dp], C.c_int),
         "skb_dense_apply_device": ([ctxp, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p], C.c_int),
@@ -238,6 +244,30 @@ def fiber_params(n_fibers, length_prev, bending_rigidity, radius, penalty_param,
 
 def _params_ptr(p):
     return p.ctypes.data_as(C.POINTER(FiberParams)) if p.size else None
+
+
+def _per_fiber(v, n_fibers):
+    """None (the C ABI's NULL) or a per-fiber array / scalar as n_fibers contiguous doubles"""
+    if v is None:
+        return None
+    v = np.asarray(v, dtype=np.float64)
+    if v.ndim and v.shape != (int(n_fibers),):
+        raise ValueError(f"expected a scalar or {int(n_fibers)} values, got shape {v.shape}")
+    return np.ascontiguousarray(np.broadcast_to(v, (int(n_fibers),)))
+
+
+def _opt_p(x):
+    return None if x is None else _p(x)
+
+
+def _fiber_rhs_args(n_fibers, n_nodes, params, v_growth, force_scale, v_on_fibers, f_external):
+    """skb_fiber_params, v_growth, force_scale and the (n_nodes, 3) inputs of a fiber RHS call, each None where absent"""
+    p = fiber_params(n_fibers, *params)
+    v, f = (None if a is None else _arr(a, 3) for a in (v_on_fibers, f_external))
+    for a in (v, f):
+        if a is not None and a.shape[0] != n_nodes:
+            raise ValueError(f"expected ({n_nodes}, 3) node values, got {a.shape}")
+    return p, _per_fiber(v_growth, n_fibers), _per_fiber(force_scale, n_fibers), v, f
 
 
 def device_count() -> int:
@@ -627,6 +657,36 @@ class Flow:
                          plus_hinged)
         _check(library().skb_flow_build_fiber_operators(self._h, _params_ptr(p), float(dt), float(eta)))
 
+    def build_fiber_rhs(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
+                        plus_hinged, dt, eta, v_on_fibers=None, f_external=None, v_growth=None, force_scale=None):
+        """The fiber block of the RHS (4 N_own,) as System::prep_state_for_solver leaves it: update_RHS with f_external
+        + force_scale xs_, then the RHS half of apply_bc_rectangular with f_external.  Parameters as for
+        build_fiber_operators; v_on_fibers / f_external (N_own, 3) and v_growth / force_scale (per-fiber arrays or
+        scalars) may be None: no flow / force, zero growth, no motors."""
+        f0, f1 = self._own_fibers()
+        n_own = self._pieces()[0]
+        p, vg, fs, v, f = _fiber_rhs_args(f1 - f0, n_own, (length_prev, bending_rigidity, radius, penalty_param,
+                                                           beta_tstep, minus_clamped, plus_hinged),
+                                          v_growth, force_scale, v_on_fibers, f_external)
+        rhs = np.empty(4 * n_own)
+        _check(library().skb_flow_build_fiber_rhs(self._h, _params_ptr(p), _opt_p(vg), _opt_p(fs), _opt_p(v), _opt_p(f),
+                                                  float(dt), float(eta), _p(rhs)))
+        return rhs
+
+    def build_fiber_rhs_device(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
+                               plus_hinged, dt, eta, d_v_on_fibers: int, d_f_external: int, d_rhs: int, v_growth=None,
+                               force_scale=None, stream: int = 0):
+        """build_fiber_rhs on device pointers (0: none for the inputs), asynchronous on `stream`; returns once the
+        per-fiber tables are staged."""
+        f0, f1 = self._own_fibers()
+        p, vg, fs, _, _ = _fiber_rhs_args(f1 - f0, 0, (length_prev, bending_rigidity, radius, penalty_param,
+                                                       beta_tstep, minus_clamped, plus_hinged),
+                                          v_growth, force_scale, None, None)
+        _check(library().skb_flow_build_fiber_rhs_device(
+            self._h, _params_ptr(p), _opt_p(vg), _opt_p(fs), C.c_void_p(d_v_on_fibers) if d_v_on_fibers else None,
+            C.c_void_p(d_f_external) if d_f_external else None, float(dt), float(eta), C.c_void_p(d_rhs),
+            C.c_void_p(stream)))
+
     def get_fiber_operators(self, inverse=True):
         """The resident operators of the (own) fibers: dict(A=[(4n,4n)], force=[(3n,4n)], xs=(N_own,3),
         A_inv=[(4n,4n)] or None)."""
@@ -866,6 +926,18 @@ class MultiFlow:
         p = fiber_params(self.n_fibers, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
                          plus_hinged)
         _check(library().skb_mflow_build_fiber_operators(self._h, _params_ptr(p), float(dt), float(eta)))
+
+    def build_fiber_rhs(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
+                        plus_hinged, dt, eta, v_on_fibers=None, f_external=None, v_growth=None, force_scale=None):
+        """Flow.build_fiber_rhs for ALL fibers; every device forms its own slice."""
+        p, vg, fs, v, f = _fiber_rhs_args(self.n_fibers, self.n_fib, (length_prev, bending_rigidity, radius,
+                                                                      penalty_param, beta_tstep, minus_clamped,
+                                                                      plus_hinged),
+                                          v_growth, force_scale, v_on_fibers, f_external)
+        rhs = np.empty(4 * self.n_fib)
+        _check(library().skb_mflow_build_fiber_rhs(self._h, _params_ptr(p), _opt_p(vg), _opt_p(fs), _opt_p(v),
+                                                   _opt_p(f), float(dt), float(eta), _p(rhs)))
+        return rhs
 
     def set_dense(self, op: int, A):
         A = np.ascontiguousarray(A, dtype=np.float64)

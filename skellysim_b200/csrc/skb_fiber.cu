@@ -1,12 +1,15 @@
 // skb_fiber.cu -- the per-fiber dense operators of a flow (FiberOps, skb_internal.hpp): class matrices, the plan of the
-// own fibers, the caller's operators and inverse or their device build (fiber_build.cuh), and the launches of
-// fiber_gemv_kernel (fiber_ops.cuh).  Knows nothing of skb_flow: skb_matvec.cu hands it the own fibers.
+// own fibers, the caller's operators and inverse or their device build (fiber_build.cuh), the launches of
+// fiber_gemv_kernel (fiber_ops.cuh), and the fiber block of the RHS (fiber_rhs.cuh) with tables of its own.  Knows
+// nothing of skb_flow: skb_matvec.cu hands it the own fibers.
 #include "fiber_build.cuh"
 #include "fiber_ops.cuh"
+#include "fiber_rhs.cuh"
 #include "skb_internal.hpp"
 #include "../../include/skelly_b200_flow.h"
 
 #include <algorithm>
+#include <cmath>
 
 using namespace skb;
 
@@ -64,6 +67,7 @@ int FiberOps::set_class(int n_nodes, const double *D_1_0, const double *P_downsa
     c.D.assign(D_1_0, D_1_0 + n * n);
     c.P.assign(P_downsample_bc, P_downsample_bc + (4 * n - 14) * 4 * n);
     ready_ = false;
+    class_gen++;
     return SKB_OK;
 }
 
@@ -76,6 +80,40 @@ int FiberOps::set_class_derivatives(int n_nodes, const double *D_2_0, const doub
     d.assign(D_2_0, D_2_0 + nn);
     d.insert(d.end(), D_3_0, D_3_0 + nn);
     d.insert(d.end(), D_4_0, D_4_0 + nn);
+    class_gen++;
+    return SKB_OK;
+}
+
+// class matrices -> one device buffer [D_1_0 | P_downsample_bc | D_2_0 | D_3_0 | D_4_0] per class; per class also the
+// non-zero column range of every row of P_downsample_bc (block diagonal in the reference, ffd.cpp:551-555: the kernels
+// walk the range only) and the non-zero row range of every column of D_1_0
+void FiberOps::pack_classes(ClassPack &cp) const {
+    for (const auto &kv : classes) {
+        if (kv.second.D.empty()) // only set_class_derivatives was called for this n
+            continue;
+        const int nn = kv.first, bc = 4 * nn - 14;
+        cp.off[nn] = {(long long)cp.mats.size(), (long long)cp.ranges.size()};
+        cp.mats.insert(cp.mats.end(), kv.second.D.begin(), kv.second.D.end());
+        cp.mats.insert(cp.mats.end(), kv.second.P.begin(), kv.second.P.end());
+        cp.mats.insert(cp.mats.end(), kv.second.D234.begin(), kv.second.D234.end());
+        nonzero_ranges(kv.second.P.data(), bc, 1, 4 * nn, bc, cp.ranges);
+        // D_1_0 (n x n, column-major): non-zero row range of every column (banded)
+        nonzero_ranges(kv.second.D.data(), nn, nn, nn, 1, cp.ranges);
+    }
+}
+
+// derivatives: the device build's and the RHS's needs (class derivatives, n within the build's range)
+int FiberOps::check_class(int f, int n, bool derivatives) const {
+    auto it = classes.find(n);
+    if (it == classes.end() || it->second.D.empty())
+        return set_error(SKB_ERR_INVALID, "fiber %d has %d nodes but skb_flow_set_fiber_class(%d, ...) was never "
+                                          "called", f, n, n);
+    if (derivatives && (n < kBuildMinNodes || n > kBuildMaxNodes))
+        return set_error(SKB_ERR_INVALID, "fiber %d has %d nodes: the device build takes %d <= n <= %d", f, n,
+                         kBuildMinNodes, kBuildMaxNodes);
+    if (derivatives && it->second.D234.empty())
+        return set_error(SKB_ERR_INVALID, "fiber %d has %d nodes but skb_flow_set_fiber_class_derivatives(%d, ...) "
+                                          "was never called", f, n, n);
     return SKB_OK;
 }
 
@@ -83,43 +121,22 @@ int FiberOps::set_class_derivatives(int n_nodes, const double *D_2_0, const doub
 // within the build's range), whose tables are planned too
 int FiberOps::plan(const OwnFibers &own, const double *length_prev, const skb_fiber_params *build, Plan &pl) {
     const int f0 = own.f0, nfib = own.count();
-    // class matrices -> one device buffer, per-fiber offsets into it; per class also the non-zero column range of every
-    // row of P_downsample_bc (block diagonal in the reference, ffd.cpp:551-555: the kernels walk the range only)
-    std::map<int, std::pair<long long, long long>> class_off;
-    std::map<int, long long> range_off;
-    for (const auto &kv : classes) {
-        if (kv.second.D.empty()) // only set_class_derivatives was called for this n
-            continue;
-        class_off[kv.first] = {(long long)pl.h_class.size(), (long long)(pl.h_class.size() + kv.second.D.size())};
-        pl.h_class.insert(pl.h_class.end(), kv.second.D.begin(), kv.second.D.end());
-        pl.h_class.insert(pl.h_class.end(), kv.second.P.begin(), kv.second.P.end());
-        pl.h_class.insert(pl.h_class.end(), kv.second.D234.begin(), kv.second.D234.end());
-        const int nn = kv.first, bc = 4 * nn - 14;
-        range_off[nn] = (long long)pl.h_ranges.size();
-        nonzero_ranges(kv.second.P.data(), bc, 1, 4 * nn, bc, pl.h_ranges);
-        // D_1_0 (n x n, column-major): non-zero row range of every column (banded)
-        nonzero_ranges(kv.second.D.data(), nn, nn, nn, 1, pl.h_ranges);
-    }
+    ClassPack cp;
+    pack_classes(cp);
+    pl.h_class = std::move(cp.mats);
+    pl.h_ranges = std::move(cp.ranges);
     pl.cD.resize((size_t)nfib), pl.cP.resize((size_t)nfib), pl.cR.resize((size_t)nfib);
     int max_n = 0;
     const long long node0 = own.off[f0]; // x / fw / v / res of the own fibers are indexed from here
     for (int f = 0; f < nfib; ++f) {
         const int n = own.n[f0 + f];
-        auto it = class_off.find(n);
-        if (it == class_off.end())
-            return set_error(SKB_ERR_INVALID, "fiber %d has %d nodes but skb_flow_set_fiber_class(%d, ...) was never "
-                                              "called", f0 + f, n, n);
-        if (build && (n < kBuildMinNodes || n > kBuildMaxNodes))
-            return set_error(SKB_ERR_INVALID, "fiber %d has %d nodes: the device build takes %d <= n <= %d", f0 + f, n,
-                             kBuildMinNodes, kBuildMaxNodes);
-        if (build && classes[n].D234.empty())
-            return set_error(SKB_ERR_INVALID, "fiber %d has %d nodes but skb_flow_set_fiber_class_derivatives(%d, ...) "
-                                              "was never called", f0 + f, n, n);
+        SKB_TRY(check_class(f0 + f, n, build != nullptr));
         if (length_prev && !(length_prev[f] > 0))
             return set_error(SKB_ERR_INVALID, "fiber %d: length_prev = %g", f0 + f, length_prev[f]);
-        pl.cD[f] = it->second.first;
-        pl.cP[f] = it->second.second;
-        pl.cR[f] = range_off[n];
+        const auto &co = cp.off[n];
+        pl.cD[f] = co.first;
+        pl.cP[f] = co.first + (long long)n * n;
+        pl.cR[f] = co.second;
         max_n = std::max(max_n, n);
         const long long node_off = own.off[f0 + f] - node0;
         if (build) {
@@ -215,12 +232,9 @@ int FiberOps::upload_inverse(const double *A_inv, cudaStream_t st) {
     return SKB_OK;
 }
 
-int FiberOps::build(const OwnFibers &own, const skb_fiber_params *params, double dt, double eta, int *launches,
-                    const std::function<int(const Step &stage, const Step &launch)> &frame) {
+static int check_params(const OwnFibers &own, const skb_fiber_params *params) {
     static_assert(sizeof(skb_fiber_params) == 48 && sizeof(FiberParamsDev) == 48, "skb_fiber_params layout");
-    ready_ = false;
-    const int nfib = own.count();
-    for (int f = 0; f < nfib; ++f) {
+    for (int f = 0; f < own.count(); ++f) {
         const skb_fiber_params &p = params[f];
         if (!(p.length_prev > 0) || !(p.radius > 0))
             return set_error(SKB_ERR_INVALID, "fiber %d: length_prev = %g, radius = %g (both must be > 0)",
@@ -229,6 +243,14 @@ int FiberOps::build(const OwnFibers &own, const skb_fiber_params *params, double
             return set_error(SKB_ERR_INVALID, "fiber %d: minus_clamped = %d, plus_hinged = %d (each must be 0 or 1)",
                              own.f0 + f, p.minus_clamped, p.plus_hinged);
     }
+    return SKB_OK;
+}
+
+int FiberOps::build(const OwnFibers &own, const skb_fiber_params *params, double dt, double eta, int *launches,
+                    const std::function<int(const Step &stage, const Step &launch)> &frame) {
+    ready_ = false;
+    const int nfib = own.count();
+    SKB_TRY(check_params(own, params));
     Plan b;
     if (nfib > 0)
         SKB_TRY(plan(own, nullptr, params, b));
@@ -288,6 +310,69 @@ int FiberOps::build(const OwnFibers &own, const skb_fiber_params *params, double
     commit(own, b);
     precond_gen = ops_gen; // the inverse belongs to these operators
     return SKB_OK;
+}
+
+// The tables go up from pageable host memory: cudaMemcpyAsync returns once they are staged, so `frame` need not wait
+// for the kernel.  The class matrices are uploaded again only when a set_class* call changed them.
+int FiberOps::rhs(const OwnFibers &own, const skb_fiber_params *params, const double *v_growth,
+                  const double *force_scale, const double *d_v, const double *d_f, double dt, double eta,
+                  double *d_rhs, int *launches, const std::function<int(const Step &stage, const Step &launch)> &frame) {
+    const int nfib = own.count();
+    if (nfib == 0)
+        return SKB_OK;
+    SKB_TRY(check_params(own, params));
+    const bool repack = rhs_class_gen != class_gen;
+    ClassPack fresh;
+    if (repack)
+        pack_classes(fresh);
+    const ClassPack &cp = repack ? fresh : rhs_pack;
+    std::vector<FiberRhsItem> items((size_t)nfib);
+    std::vector<double2> growth((size_t)nfib);
+    const long long node0 = own.off[own.f0];
+    int max_n = 0;
+    for (int f = 0; f < nfib; ++f) {
+        const int n = own.n[own.f0 + f];
+        SKB_TRY(check_class(own.f0 + f, n, true));
+        const double vg = v_growth ? v_growth[f] : 0.0, fs = force_scale ? force_scale[f] : 0.0;
+        if (!std::isfinite(vg) || !std::isfinite(fs))
+            return set_error(SKB_ERR_INVALID, "fiber %d: v_growth = %g, force_scale = %g (both must be finite)",
+                             own.f0 + f, vg, fs);
+        const auto &co = cp.off.at(n);
+        items[(size_t)f] = FiberRhsItem{own.off[own.f0 + f], own.off[own.f0 + f] - node0, co.first, co.second, n,
+                                        own.f0 + f};
+        growth[(size_t)f] = make_double2(vg, fs);
+        max_n = std::max(max_n, n);
+    }
+    if (repack) {
+        rhs_pack = std::move(fresh);
+        rhs_class_gen = ~0ULL; // current once uploaded
+    }
+    const cudaStream_t st = own.stream;
+    auto stage = [&]() -> int {
+        if (rhs_pending) // the previous call's kernel, on whichever stream, still reads these tables
+            CUDA_TRY(cudaStreamWaitEvent(st, rhs_done, 0));
+        if (rhs_class_gen != class_gen) {
+            SKB_TRY(put_async(rhs_class, rhs_pack.mats.data(), rhs_pack.mats.size() * 8, st));
+            SKB_TRY(put_async(rhs_ranges, rhs_pack.ranges.data(), rhs_pack.ranges.size() * sizeof(int2), st));
+            rhs_class_gen = class_gen;
+        }
+        SKB_TRY(put_async(rhs_items, items.data(), items.size() * sizeof(FiberRhsItem), st));
+        SKB_TRY(put_async(rhs_params, params, (size_t)nfib * sizeof(skb_fiber_params), st));
+        return put_async(rhs_growth, growth.data(), growth.size() * sizeof(double2), st);
+    };
+    auto launch = [&]() -> int {
+        const RhsArgs ra{(const FiberRhsItem *)rhs_items.ptr, (const FiberParamsDev *)rhs_params.ptr,
+                         (const double2 *)rhs_growth.ptr, (const double *)rhs_class.ptr, (const int2 *)rhs_ranges.ptr,
+                         own.r_fib, own.length, d_v, d_f, force_scale != nullptr, dt, eta, d_rhs};
+        fiber_rhs_kernel<<<(unsigned)nfib, kRhsThreads, rhs_smem_bytes(max_n), st>>>(ra);
+        SKB_TRY(launched(launches));
+        if (!rhs_done)
+            CUDA_TRY(cudaEventCreateWithFlags(rhs_done.out(), cudaEventDisableTiming));
+        CUDA_TRY(cudaEventRecord(rhs_done, st));
+        rhs_pending = true;
+        return SKB_OK;
+    };
+    return frame(stage, launch);
 }
 
 int FiberOps::ready(const char *who, bool with_inverse) const {

@@ -168,6 +168,13 @@ class FiberOps {
     using Step = std::function<int()>;
     int build(const OwnFibers &own, const ::skb_fiber_params *params, double dt, double eta, int *launches,
               const std::function<int(const Step &stage, const Step &launch)> &frame);
+    // the fiber block of the RHS into d_rhs (4 per own node) from d_v / d_f (3 per own node, either may be NULL),
+    // checked on the host first; `frame` runs stage (the table uploads on own.stream), then launch.  Needs the class
+    // matrices and derivatives, not the operators: its tables are its own, and the resident operators, their inverse
+    // and the GEMV launches stay as they are.  v_growth / force_scale per own fiber, may be NULL
+    int rhs(const OwnFibers &own, const ::skb_fiber_params *params, const double *v_growth, const double *force_scale,
+            const double *d_v, const double *d_f, double dt, double eta, double *d_rhs, int *launches,
+            const std::function<int(const Step &stage, const Step &launch)> &frame);
     // on st, each adding its launches to *launches: fw = force_operator_ x; res = fc.matvec(x, v, vb); y = A_^-1 x
     int force(const double *d_x, double *d_fw, cudaStream_t st, int *launches) const;
     int matvec(const double *d_x, const double *d_v, const double *d_vb, double *d_res, cudaStream_t st,
@@ -189,7 +196,16 @@ class FiberOps {
         std::vector<double> D, P; // D_1_0 (n x n), P_downsample_bc ((4n-14) x 4n), column-major
         std::vector<double> D234; // D_2_0 | D_3_0 | D_4_0 (n x n each): set_class_derivatives
     };
+    // the class matrices packed into one buffer: per n the offsets of its block and of its row ranges
+    struct ClassPack {
+        std::vector<double> mats;
+        std::vector<int2> ranges;
+        std::map<int, std::pair<long long, long long>> off;
+    };
+    void pack_classes(ClassPack &cp) const;
+    int check_class(int f, int n, bool derivatives) const; // fiber f has n nodes: its class is set
     std::map<int, FiberClass> classes;
+    unsigned long long class_gen = 0; // bumped by set_class / set_class_derivatives
     bool ready_ = false;
     int f0 = 0, f1 = 0;    // the fibers of the resident operators
     long long n_nodes = 0; // ... and their nodes
@@ -200,6 +216,13 @@ class FiberOps {
     long long op_A_elems = 0;                        // elements of the concatenated A_ (and of A_^-1)
     long long op_F_elems = 0;                        // ... of force_operator_
     unsigned long long ops_gen = 0, precond_gen = 0; // the inverse belongs to one set of operators
+    // the RHS's own tables: the class matrices as of rhs_class_gen (kept on the host while the device copy is current),
+    // the per-fiber tables of the last call, and the event after its kernel (the next call's uploads wait for it)
+    ClassPack rhs_pack;
+    unsigned long long rhs_class_gen = ~0ULL;
+    DevBuf rhs_class, rhs_ranges, rhs_items, rhs_params, rhs_growth;
+    Event rhs_done;
+    bool rhs_pending = false;
 };
 
 } // namespace skb

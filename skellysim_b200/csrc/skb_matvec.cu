@@ -1448,6 +1448,60 @@ int skb_flow_build_fiber_operators(skb_flow *fl, const skb_fiber_params *params,
                          });
 }
 
+// checks shared by the two forms of the fiber RHS, then the own fibers on the flow's device; stats of no launch
+static int fiber_rhs_args(skb_flow *fl, const char *who, const skb_fiber_params *params, const double *rhs, double dt,
+                          double eta, OwnFibers &own) {
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    if (!(dt > 0) || !(eta > 0))
+        return set_error(SKB_ERR_INVALID, "%s: dt = %g, eta = %g (both must be > 0)", who, dt, eta);
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    SKB_TRY(own_fibers(fl, who, own));
+    if (own.count() > 0 && (!params || !rhs))
+        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
+    begin_stats(fl);
+    return device_stats(fl);
+}
+
+int skb_flow_build_fiber_rhs(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
+                             const double *force_scale, const double *v_on_fibers, const double *f_external, double dt,
+                             double eta, double *rhs) {
+    OwnFibers own;
+    SKB_TRY(fiber_rhs_args(fl, "skb_flow_build_fiber_rhs", params, rhs, dt, eta, own));
+    const size_t nf = (size_t)own.nodes();
+    SKB_TRY(fl->vel.ensure(nf * 24));
+    SKB_TRY(fl->in_fib.ensure(nf * 24));
+    SKB_TRY(fl->res_fib.ensure(nf * 32));
+    // device_ms spans the kernel, total_ms also the uploads before it and the download after it
+    return fl->ops.rhs(own, params, v_growth, force_scale, v_on_fibers ? (const double *)fl->vel.ptr : nullptr,
+                       f_external ? (const double *)fl->in_fib.ptr : nullptr, dt, eta, (double *)fl->res_fib.ptr,
+                       &fl->launches, [&](const FiberOps::Step &stage, const FiberOps::Step &launch) {
+                           auto up = [&]() -> int {
+                               if (v_on_fibers)
+                                   SKB_TRY(upload(fl, fl->vel, v_on_fibers, nf * 3));
+                               if (f_external)
+                                   SKB_TRY(upload(fl, fl->in_fib, f_external, nf * 3));
+                               return stage();
+                           };
+                           return host_frame(fl, up, launch, [&] { return download(fl, rhs, fl->res_fib, nf * 4); });
+                       });
+}
+
+int skb_flow_build_fiber_rhs_device(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
+                                    const double *force_scale, const double *d_v_on_fibers, const double *d_f_external,
+                                    double dt, double eta, double *d_rhs, void *stream) {
+    OwnFibers own;
+    SKB_TRY(fiber_rhs_args(fl, "skb_flow_build_fiber_rhs_device", params, d_rhs, dt, eta, own));
+    own.stream = (cudaStream_t)stream;
+    return fl->ops.rhs(own, params, v_growth, force_scale, d_v_on_fibers, d_f_external, dt, eta, d_rhs, &fl->launches,
+                       [&](const FiberOps::Step &stage, const FiberOps::Step &launch) {
+                           fl->cur = own.stream;
+                           SKB_TRY(stage());
+                           SKB_TRY(launch());
+                           return device_stats(fl);
+                       });
+}
+
 int skb_flow_get_fiber_operators(skb_flow *fl, double *A, double *force_operator, double *xs, double *A_inv) {
     const char *who = "skb_flow_get_fiber_operators";
     if (!fl)

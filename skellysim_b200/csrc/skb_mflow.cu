@@ -385,6 +385,27 @@ int skb_mflow_build_fiber_operators(skb_mflow *mf, const skb_fiber_params *param
     return SKB_OK;
 }
 
+int skb_mflow_build_fiber_rhs(skb_mflow *mf, const skb_fiber_params *params, const double *v_growth,
+                              const double *force_scale, const double *v_on_fibers, const double *f_external, double dt,
+                              double eta, double *rhs) {
+    if (!mf)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_build_fiber_rhs: NULL");
+    SKB_TRY(mflow_prepare(mf));
+    if (mf->n_fibers > 0 && (!params || !rhs))
+        return set_error(SKB_ERR_INVALID, "skb_mflow_build_fiber_rhs: NULL argument");
+    return mf->workers->run([&](int g) -> int {
+        const int f0 = mf->f0[g];
+        skb_flow *fl = mf->m[g].get();
+        if (mf->f1[g] == f0)
+            return skb_flow_build_fiber_rhs(fl, nullptr, nullptr, nullptr, nullptr, nullptr, dt, eta, nullptr);
+        const long long node = mf->fiber_off[(size_t)f0];
+        return skb_flow_build_fiber_rhs(fl, params + f0, v_growth ? v_growth + f0 : nullptr,
+                                        force_scale ? force_scale + f0 : nullptr,
+                                        v_on_fibers ? v_on_fibers + 3 * node : nullptr,
+                                        f_external ? f_external + 3 * node : nullptr, dt, eta, rhs + 4 * node);
+    });
+}
+
 // the periphery's dense operator, rows block-partitioned like the periphery rows (periphery.cpp:387-417)
 int skb_mflow_set_dense(skb_mflow *mf, int op, const double *A_rowmajor, int64_t n_rows, int64_t n_cols) {
     if (!mf || !A_rowmajor || n_rows != 3 * mf->n_shell || n_cols != 3 * mf->n_shell)
