@@ -162,7 +162,9 @@ SKB_API int skb_flow_group_error(skb_flow *fl, int *missing_peer);
  *
  * skb_flow_set_fiber_class: the per-node-count constants FiberFiniteDifference::matrices_.at(n)
  *   (fiber_finite_difference.cpp:537-555): D_1_0 (n x n) and P_downsample_bc ((4n-14) x 4n).  Call once per
- *   distinct n (n >= 4), any time before skb_flow_set_fiber_operators.
+ *   distinct n (n >= 4), any time before skb_flow_set_fiber_operators.  The matrices are uploaded at once,
+ *   after the work in flight on the flow's device has finished (the fiber kernels may still read the previous ones),
+ *   so the call can also return SKB_ERR_CUDA.
  * skb_flow_set_fiber_operators: once per timestep, after skb_flow_set_fibers (which defines the fibers and their
  *   node counts): A = concatenated A_ (4n x 4n each), force_operator = concatenated force_operator_ (3n x 4n
  *   each), xs = 3 x N_f tangents xs_, length_prev[f] = length_prev_, plus_bc_velocity[f] = (bc_plus_.first ==
@@ -208,7 +210,8 @@ SKB_API int skb_flow_apply_fiber_preconditioner_device(skb_flow *fl, const doubl
  *
  * skb_flow_set_fiber_class_derivatives: the higher derivative matrices of FiberFiniteDifference::matrices_.at(n)
  *   (:537-540), stored pre-transposed exactly like the reference (column-major n x n each).  The build needs them,
- *   and skb_flow_set_fiber_class, for every node count in use. */
+ *   and skb_flow_set_fiber_class, for every node count in use.  Uploaded like skb_flow_set_fiber_class's matrices;
+ *   the operators stay. */
 SKB_API int skb_flow_set_fiber_class_derivatives(skb_flow *fl, int n_nodes, const double *D_2_0,
                                                  const double *D_3_0, const double *D_4_0);
 

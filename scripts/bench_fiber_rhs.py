@@ -26,7 +26,7 @@ def fiber_rhs_leg(local_rank=0, reps=20, n_checked=6):
     """skb_flow_build_fiber_rhs, warm, median of `reps`: device_ms (CUDA events around the kernel, skb_flow_last_stats),
     total_ms (with the uploads of v_on_fibers, f_external and the per-fiber tables and the download of the RHS), the
     host clock around the call, and the kernel alone from torch.profiler.  Bytes from shapes: host -> device (two
-    3 x N_f inputs and 104 bytes of tables per fiber), device -> host (4 N_f), and the kernel's compulsory global
+    3 x N_f inputs and 120 bytes of tables per fiber), device -> host (4 N_f), and the kernel's compulsory global
     traffic (positions, the two inputs, the output; the class matrices stay in L2).  A sample of fibers is held to the
     long-double reference (tests/fiber_rhs_reference.py): max |dev - ext| / (u S)."""
     from fiber_rhs_reference import fiber_rhs  # the sample check
@@ -81,8 +81,8 @@ def fiber_rhs_leg(local_rank=0, reps=20, n_checked=6):
         out[f"{n_fibers}x{n}"] = {
             "device_ms": float(np.median(dev_ms)), "total_ms": float(np.median(tot_ms)),
             "wall_ms": float(np.median(wall)), "kernel_ms_profiler": k_ms,
-            "h2d_bytes": int(2 * nf * 24 + n_fibers * 104), "d2h_bytes": int(nf * 32),
-            "kernel_global_bytes": int(nf * (3 * 24 + 32) + n_fibers * 104),
+            "h2d_bytes": int(2 * nf * 24 + n_fibers * 120), "d2h_bytes": int(nf * 32),
+            "kernel_global_bytes": int(nf * (3 * 24 + 32) + n_fibers * 120),
             "sample_max_err_over_uS": worst, "n_checked": int(n_checked)}
     out["note"] = ("device_ms: CUDA events around the RHS kernel (skb_flow_last_stats); total_ms: with the uploads of "
                    "the inputs and per-fiber tables and the download of the RHS (pageable host memory); wall_ms: host "

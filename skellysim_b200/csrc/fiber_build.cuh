@@ -35,17 +35,17 @@ struct FiberParamsDev {
     int minus_clamped, plus_hinged;
 };
 
-struct FiberBuildItem {
-    long long a_off, f_off; // element offsets of A_ / force_operator_ in op_A / op_F
+struct FiberItem {
+    long long a_off, f_off; // element offsets of A_ / force_operator_ in op_A / op_F (the build only)
     long long node;         // first node of the fiber in r_fib (all fibers)
-    long long own_node;     // first node among the resident fibers (op_xs)
+    long long own_node;     // first node among the own fibers (op_xs; the RHS's v, f and, times 4, its output)
     long long cls;          // element offset of the class block [D_1_0 | P_downsample_bc | D_2_0 | D_3_0 | D_4_0]
     long long rng;          // element offset of the class's P row ranges in the range buffer
     int n, fiber;           // nodes; index of the fiber in the container (fiber_length)
 };
 
 struct FiberTileItem {
-    int item; // FiberBuildItem index == params index
+    int item; // FiberItem index == params index
     int col0; // first column of the tile
 };
 
@@ -73,8 +73,32 @@ inline int inverse_cluster_size(int m) {
     return 0;
 }
 
+// update_derivatives, K = 2 or 3: x_^{(k)} = (2 / length_prev_)^k x_ D_k_0 into d1 + 3n (k-1), [n x 3] each, k = 1 .. K
+// (D_3_0 follows D_2_0).  Thread t forms the entries e = t (mod blockDim.x); the caller synchronises.  (ffd.cpp:62-68)
+template <int K>
+__device__ __forceinline__ void update_derivatives(const double *xv, const double *D1, const double *D2, int n,
+                                                   double sp, double *d1) {
+    const double *D3 = D2 + (size_t)n * n;
+    double *d2 = d1 + 3 * n, *d3 = d2 + 3 * n;
+    for (int e = threadIdx.x; e < 3 * n; e += blockDim.x) {
+        const int i = e / 3, c = e - 3 * i;
+        double s1 = 0.0, s2 = 0.0, s3 = 0.0;
+        for (int j = 0; j < n; ++j) {
+            const double xj = xv[3 * j + c];
+            s1 = fma(D1[i * n + j], xj, s1);
+            s2 = fma(D2[i * n + j], xj, s2);
+            if (K == 3)
+                s3 = fma(D3[i * n + j], xj, s3);
+        }
+        d1[e] = sp * s1;
+        d2[e] = (sp * sp) * s2;
+        if (K == 3)
+            d3[e] = (sp * sp * sp) * s3;
+    }
+}
+
 struct BuildArgs {
-    const FiberBuildItem *items;
+    const FiberItem *items;
     const FiberTileItem *tiles;
     const FiberParamsDev *params;
     const double *class_mats;
@@ -88,7 +112,7 @@ struct BuildArgs {
 __global__ void __launch_bounds__(kBuildThreads) fiber_assemble_kernel(const BuildArgs a) {
     extern __shared__ double fb_smem[];
     const FiberTileItem tile = a.tiles[blockIdx.x];
-    const FiberBuildItem it = a.items[tile.item];
+    const FiberItem it = a.items[tile.item];
     const FiberParamsDev prm = a.params[tile.item];
     const int n = it.n, m = 4 * n, bc = m - 14, T = build_tile_cols(n);
     const int ncols = min(T, m - tile.col0);
@@ -102,21 +126,7 @@ __global__ void __launch_bounds__(kBuildThreads) fiber_assemble_kernel(const Bui
     for (int e = threadIdx.x; e < 3 * n; e += blockDim.x)
         xv[e] = a.r_fib[3 * it.node + e];
     __syncthreads();
-    // update_derivatives: x_^{(k)} = (2 / length_prev_)^k x_ D_k_0                                  (ffd.cpp:62-68)
-    const double sp = 2.0 / prm.length_prev;
-    for (int e = threadIdx.x; e < 3 * n; e += blockDim.x) {
-        const int i = e / 3, c = e - 3 * i;
-        double s1 = 0.0, s2 = 0.0, s3 = 0.0;
-        for (int j = 0; j < n; ++j) {
-            const double xj = xv[3 * j + c];
-            s1 = fma(D1[i * n + j], xj, s1);
-            s2 = fma(D2[i * n + j], xj, s2);
-            s3 = fma(D3[i * n + j], xj, s3);
-        }
-        d1[e] = sp * s1;
-        d2[e] = (sp * sp) * s2;
-        d3[e] = (sp * sp * sp) * s3;
-    }
+    update_derivatives<3>(xv, D1, D2, n, 2.0 / prm.length_prev, d1);
     __syncthreads();
     if (tile.col0 == 0)
         for (int e = threadIdx.x; e < 3 * n; e += blockDim.x)

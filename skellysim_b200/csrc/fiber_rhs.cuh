@@ -4,9 +4,9 @@
 // boundary-condition branch, :377-383, 399-404, 422-423, 432-433, 455-463, 481-486, 502-504).
 //
 //   fiber_rhs_kernel  One CTA per fiber.  Positions, velocities and forces are staged in shared memory; xs_ and xss_
-//       are formed as update_derivatives does (the loop of fiber_assemble_kernel, k = 1, 2), then v D_1 and f_tot D_1
-//       with D_1 scaled by length_, the raw 4n vector of update_RHS, rows [0, 4n-14) = P_downsample_bc * raw over each
-//       row's non-zero column range (as the assembly does for A_), and the 14 boundary entries.
+//       are formed by update_derivatives (fiber_build.cuh, K = 2), then v D_1 and f_tot D_1 with D_1 scaled by
+//       length_, the raw 4n vector of update_RHS, rows [0, 4n-14) = P_downsample_bc * raw over each row's non-zero
+//       column range (as the assembly does for A_), and the 14 boundary entries.
 //
 // f_tot = f_external + force_scale_ xs_ (System::prep_state_for_solver, system.cpp:416-451; the motor force of
 // generate_constant_force, fcfd.cpp:160-169) feeds update_RHS; the boundary entries see f_external alone (system.cpp:453).
@@ -17,18 +17,10 @@ namespace skb {
 
 constexpr int kRhsThreads = 128; // fiber_rhs_kernel
 
-struct FiberRhsItem {
-    long long node;     // first node of the fiber in r_fib (all fibers)
-    long long own_node; // first node among the own fibers (v, f and, times 4, the output)
-    long long cls;      // element offset of the class block [D_1_0 | P_downsample_bc | D_2_0 | ...]
-    long long rng;      // element offset of the class's P row ranges in the range buffer
-    int n, fiber;       // nodes; index of the fiber in the container (fiber_length)
-};
-
 __host__ __device__ inline size_t rhs_smem_bytes(int n) { return (size_t)28 * n * sizeof(double); }
 
 struct RhsArgs {
-    const FiberRhsItem *items;
+    const FiberItem *items;
     const FiberParamsDev *params;
     const double2 *growth; // per fiber: (v_growth_, force_scale_)
     const double *class_mats;
@@ -43,7 +35,7 @@ struct RhsArgs {
 
 __global__ void __launch_bounds__(kRhsThreads) fiber_rhs_kernel(const RhsArgs a) {
     extern __shared__ double fr_smem[];
-    const FiberRhsItem it = a.items[blockIdx.x];
+    const FiberItem it = a.items[blockIdx.x];
     const FiberParamsDev prm = a.params[blockIdx.x];
     const double2 gr = a.growth[blockIdx.x];
     const int n = it.n, m = 4 * n, bc = m - 14;
@@ -65,20 +57,9 @@ __global__ void __launch_bounds__(kRhsThreads) fiber_rhs_kernel(const RhsArgs a)
         fe[e] = has_f ? a.f[3 * it.own_node + e] : 0.0;
     }
     __syncthreads();
-    // update_derivatives with length_prev_ (ffd.cpp:62-68), the loop of fiber_assemble_kernel for k = 1, 2
-    const double sp = 2.0 / prm.length_prev;
-    for (int e = threadIdx.x; e < 3 * n; e += blockDim.x) {
-        const int i = e / 3, c = e - 3 * i;
-        double s1 = 0.0, s2 = 0.0;
-        for (int j = 0; j < n; ++j) {
-            const double xj = xv[3 * j + c];
-            s1 = fma(D1[i * n + j], xj, s1);
-            s2 = fma(D2[i * n + j], xj, s2);
-        }
-        d1[e] = sp * s1;
-        d2[e] = (sp * sp) * s2;
+    update_derivatives<2>(xv, D1, D2, n, 2.0 / prm.length_prev, d1);
+    for (int e = threadIdx.x; e < 3 * n; e += blockDim.x) // (d1[e] was formed by this thread)
         ft[e] = a.motor ? fe[e] + gr.y * d1[e] : fe[e];
-    }
     __syncthreads();
 
     // update_RHS takes D_1 with length_ (ffd.cpp:201): (v D_1)_i = sum_j v_j D_1_0(j, i) 2 / length_

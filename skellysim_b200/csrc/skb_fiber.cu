@@ -1,7 +1,7 @@
-// skb_fiber.cu -- the per-fiber dense operators of a flow (FiberOps, skb_internal.hpp): class matrices, the plan of the
-// own fibers, the caller's operators and inverse or their device build (fiber_build.cuh), the launches of
-// fiber_gemv_kernel (fiber_ops.cuh), and the fiber block of the RHS (fiber_rhs.cuh) with tables of its own.  Knows
-// nothing of skb_flow: skb_matvec.cu hands it the own fibers.
+// skb_fiber.cu -- the per-fiber dense operators of a flow (FiberOps, skb_internal.hpp): the class matrices and their one
+// device table, the plan of the own fibers, the caller's operators and inverse or their device build (fiber_build.cuh),
+// the launches of fiber_gemv_kernel (fiber_ops.cuh), and the fiber block of the RHS (fiber_rhs.cuh) with per-fiber
+// tables of its own.  Knows nothing of skb_flow: skb_matvec.cu hands it the own fibers.
 #include "fiber_build.cuh"
 #include "fiber_ops.cuh"
 #include "fiber_rhs.cuh"
@@ -16,15 +16,13 @@ using namespace skb;
 // fiber_gemv_kernel's dynamic shared memory: the plan refuses more, prepare_fiber_kernels allows this much
 static constexpr size_t kGemvSmemMax = 200 * 1024;
 
-// Where the operators of the own fibers live (class matrices, non-zero ranges, GEMV items, offsets into A_ and
-// force_operator_) and a build's tables: per fiber, per assembly CTA (a tile of columns), per inverse launch (node count)
+// Where the operators of the own fibers live (GEMV items, offsets into A_, force_operator_ and the class table) and a
+// build's tables: per fiber, per assembly CTA (a tile of columns), per inverse launch (node count)
 struct FiberOps::Plan {
-    std::vector<double> h_class;              // per class: D_1_0 | P_downsample_bc [| D_2_0 | D_3_0 | D_4_0]
-    std::vector<int2> h_ranges;
     std::vector<long long> cD, cP, cR;        // per own fiber: its class's D_1_0, P, ranges
     std::vector<FiberGemvItem> itA, itF;
     long long offA = 0, offF = 0;
-    std::vector<FiberBuildItem> items;
+    std::vector<FiberItem> items;
     std::vector<FiberTileItem> tiles;
     std::vector<double> lp;
     std::vector<int> plus;
@@ -59,47 +57,57 @@ static int put_async(DevBuf &b, const void *h, size_t bytes, cudaStream_t st) {
     return SKB_OK;
 }
 
-int FiberOps::set_class(int n_nodes, const double *D_1_0, const double *P_downsample_bc) {
+int FiberOps::set_class(int n_nodes, const double *D_1_0, const double *P_downsample_bc, cudaStream_t st) {
     if (n_nodes < 4) // bc_start_i = 4n - 14 must leave room for the 14 boundary rows (ffd.cpp:279)
         return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_class: n_nodes = %d (need >= 4)", n_nodes);
     const size_t n = (size_t)n_nodes;
     FiberClass &c = classes[n_nodes];
     c.D.assign(D_1_0, D_1_0 + n * n);
     c.P.assign(P_downsample_bc, P_downsample_bc + (4 * n - 14) * 4 * n);
-    ready_ = false;
-    class_gen++;
-    return SKB_OK;
+    ready_ = false; // the offsets of the other classes may have moved
+    return upload_classes(st);
 }
 
-int FiberOps::set_class_derivatives(int n_nodes, const double *D_2_0, const double *D_3_0, const double *D_4_0) {
+int FiberOps::set_class_derivatives(int n_nodes, const double *D_2_0, const double *D_3_0, const double *D_4_0,
+                                    cudaStream_t st) {
     if (n_nodes < kBuildMinNodes || n_nodes > kBuildMaxNodes)
         return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_class_derivatives: n_nodes = %d (the device build takes "
                                           "%d <= n <= %d)", n_nodes, kBuildMinNodes, kBuildMaxNodes);
     const size_t nn = (size_t)n_nodes * n_nodes;
-    std::vector<double> &d = classes[n_nodes].D234;
-    d.assign(D_2_0, D_2_0 + nn);
-    d.insert(d.end(), D_3_0, D_3_0 + nn);
-    d.insert(d.end(), D_4_0, D_4_0 + nn);
-    class_gen++;
-    return SKB_OK;
+    FiberClass &c = classes[n_nodes];
+    c.D234.assign(D_2_0, D_2_0 + nn);
+    c.D234.insert(c.D234.end(), D_3_0, D_3_0 + nn);
+    c.D234.insert(c.D234.end(), D_4_0, D_4_0 + nn);
+    return c.D.empty() ? SKB_OK : upload_classes(st); // without set_class(n) yet: its block is written then
 }
 
-// class matrices -> one device buffer [D_1_0 | P_downsample_bc | D_2_0 | D_3_0 | D_4_0] per class; per class also the
-// non-zero column range of every row of P_downsample_bc (block diagonal in the reference, ffd.cpp:551-555: the kernels
-// walk the range only) and the non-zero row range of every column of D_1_0
-void FiberOps::pack_classes(ClassPack &cp) const {
+// classes -> class_mats / class_ranges / class_off, in order of n.  Per class also the non-zero column range of every
+// row of P_downsample_bc (block diagonal in the reference, ffd.cpp:551-555: the kernels walk the range only) and the
+// non-zero row range of every column of D_1_0.
+int FiberOps::upload_classes(cudaStream_t st) {
+    std::vector<double> mats;
+    std::vector<int2> ranges;
+    class_off.clear();
     for (const auto &kv : classes) {
         if (kv.second.D.empty()) // only set_class_derivatives was called for this n
             continue;
         const int nn = kv.first, bc = 4 * nn - 14;
-        cp.off[nn] = {(long long)cp.mats.size(), (long long)cp.ranges.size()};
-        cp.mats.insert(cp.mats.end(), kv.second.D.begin(), kv.second.D.end());
-        cp.mats.insert(cp.mats.end(), kv.second.P.begin(), kv.second.P.end());
-        cp.mats.insert(cp.mats.end(), kv.second.D234.begin(), kv.second.D234.end());
-        nonzero_ranges(kv.second.P.data(), bc, 1, 4 * nn, bc, cp.ranges);
+        class_off[nn] = {(long long)mats.size(), (long long)ranges.size()};
+        mats.insert(mats.end(), kv.second.D.begin(), kv.second.D.end());
+        mats.insert(mats.end(), kv.second.P.begin(), kv.second.P.end());
+        if (kv.second.D234.empty())
+            mats.resize(mats.size() + 3 * (size_t)nn * nn, 0.0);
+        else
+            mats.insert(mats.end(), kv.second.D234.begin(), kv.second.D234.end());
+        nonzero_ranges(kv.second.P.data(), bc, 1, 4 * nn, bc, ranges);
         // D_1_0 (n x n, column-major): non-zero row range of every column (banded)
-        nonzero_ranges(kv.second.D.data(), nn, nn, nn, 1, cp.ranges);
+        nonzero_ranges(kv.second.D.data(), nn, nn, nn, 1, ranges);
     }
+    CUDA_TRY(cudaDeviceSynchronize()); // the GEMVs, the build and the RHS may still read the table, on any stream
+    SKB_TRY(put_async(class_mats, mats.data(), mats.size() * 8, st));
+    SKB_TRY(put_async(class_ranges, ranges.data(), ranges.size() * sizeof(int2), st));
+    CUDA_TRY(cudaStreamSynchronize(st)); // complete before any later launch, on any stream
+    return SKB_OK;
 }
 
 // derivatives: the device build's and the RHS's needs (class derivatives, n within the build's range)
@@ -117,31 +125,36 @@ int FiberOps::check_class(int f, int n, bool derivatives) const {
     return SKB_OK;
 }
 
+// a_off / f_off are the build's
+int FiberOps::item(const OwnFibers &own, int f, bool derivatives, FiberItem &it) const {
+    const int n = own.n[f];
+    SKB_TRY(check_class(f, n, derivatives));
+    const auto &co = class_off.at(n);
+    it = FiberItem{0, 0, own.off[f], own.off[f] - own.off[own.f0], co.first, co.second, n, f};
+    return SKB_OK;
+}
+
 // length_prev: checked per fiber when given; build: the parameters of a device build (class derivatives needed, n
 // within the build's range), whose tables are planned too
 int FiberOps::plan(const OwnFibers &own, const double *length_prev, const skb_fiber_params *build, Plan &pl) {
     const int f0 = own.f0, nfib = own.count();
-    ClassPack cp;
-    pack_classes(cp);
-    pl.h_class = std::move(cp.mats);
-    pl.h_ranges = std::move(cp.ranges);
     pl.cD.resize((size_t)nfib), pl.cP.resize((size_t)nfib), pl.cR.resize((size_t)nfib);
     int max_n = 0;
-    const long long node0 = own.off[f0]; // x / fw / v / res of the own fibers are indexed from here
     for (int f = 0; f < nfib; ++f) {
-        const int n = own.n[f0 + f];
-        SKB_TRY(check_class(f0 + f, n, build != nullptr));
+        FiberItem it;
+        SKB_TRY(item(own, f0 + f, build != nullptr, it));
         if (length_prev && !(length_prev[f] > 0))
             return set_error(SKB_ERR_INVALID, "fiber %d: length_prev = %g", f0 + f, length_prev[f]);
-        const auto &co = cp.off[n];
-        pl.cD[f] = co.first;
-        pl.cP[f] = co.first + (long long)n * n;
-        pl.cR[f] = co.second;
+        const int n = it.n;
+        const long long node_off = it.own_node; // x / fw / v / res of the own fibers are indexed from their first node
+        pl.cD[f] = it.cls;
+        pl.cP[f] = it.cls + (long long)n * n;
+        pl.cR[f] = it.rng;
         max_n = std::max(max_n, n);
-        const long long node_off = own.off[f0 + f] - node0;
         if (build) {
-            pl.items.push_back(FiberBuildItem{pl.offA, pl.offF, own.off[f0 + f], node_off, pl.cD[f], pl.cR[f], n,
-                                              f0 + f});
+            it.a_off = pl.offA;
+            it.f_off = pl.offF;
+            pl.items.push_back(it);
             for (int c = 0; c < 4 * n; c += build_tile_cols(n))
                 pl.tiles.push_back(FiberTileItem{f, c});
             pl.smem = std::max(pl.smem, build_smem_bytes(n));
@@ -172,11 +185,9 @@ int FiberOps::upload_plan(const OwnFibers &own, const Plan &pl) {
     SKB_TRY(op_A.ensure((size_t)pl.offA * 8));
     SKB_TRY(op_F.ensure((size_t)pl.offF * 8));
     SKB_TRY(op_xs.ensure((size_t)own.nodes() * 24));
-    SKB_TRY(put_async(op_class, pl.h_class.data(), pl.h_class.size() * 8, st));
     SKB_TRY(put_async(op_classD, pl.cD.data(), pl.cD.size() * 8, st));
     SKB_TRY(put_async(op_classP, pl.cP.data(), pl.cP.size() * 8, st));
     SKB_TRY(put_async(op_classR, pl.cR.data(), pl.cR.size() * 8, st));
-    SKB_TRY(put_async(op_ranges, pl.h_ranges.data(), pl.h_ranges.size() * sizeof(int2), st));
     SKB_TRY(put_async(items_A, pl.itA.data(), pl.itA.size() * sizeof(FiberGemvItem), st));
     SKB_TRY(put_async(items_F, pl.itF.data(), pl.itF.size() * sizeof(FiberGemvItem), st));
     return SKB_OK;
@@ -261,14 +272,14 @@ int FiberOps::build(const OwnFibers &own, const skb_fiber_params *params, double
         SKB_TRY(put_async(op_len, b.lp.data(), b.lp.size() * 8, st));
         SKB_TRY(put_async(op_plus, b.plus.data(), b.plus.size() * sizeof(int), st));
         SKB_TRY(put_async(bld_params, params, (size_t)nfib * sizeof(skb_fiber_params), st));
-        SKB_TRY(put_async(bld_items, b.items.data(), b.items.size() * sizeof(FiberBuildItem), st));
+        SKB_TRY(put_async(bld_items, b.items.data(), b.items.size() * sizeof(FiberItem), st));
         SKB_TRY(put_async(bld_tiles, b.tiles.data(), b.tiles.size() * sizeof(FiberTileItem), st));
         return put_async(bld_inv, b.inv_off.data(), b.inv_off.size() * sizeof(long long), st);
     };
     auto launch = [&]() -> int {
-        const BuildArgs ba{(const FiberBuildItem *)bld_items.ptr, (const FiberTileItem *)bld_tiles.ptr,
-                           (const FiberParamsDev *)bld_params.ptr, (const double *)op_class.ptr,
-                           (const int2 *)op_ranges.ptr, own.r_fib, own.length, dt, eta, (double *)op_A.ptr,
+        const BuildArgs ba{(const FiberItem *)bld_items.ptr, (const FiberTileItem *)bld_tiles.ptr,
+                           (const FiberParamsDev *)bld_params.ptr, (const double *)class_mats.ptr,
+                           (const int2 *)class_ranges.ptr, own.r_fib, own.length, dt, eta, (double *)op_A.ptr,
                            (double *)op_F.ptr, (double *)op_xs.ptr};
         fiber_assemble_kernel<<<(unsigned)b.tiles.size(), kBuildThreads, b.smem, st>>>(ba);
         SKB_TRY(launched(launches));
@@ -313,7 +324,7 @@ int FiberOps::build(const OwnFibers &own, const skb_fiber_params *params, double
 }
 
 // The tables go up from pageable host memory: cudaMemcpyAsync returns once they are staged, so `frame` need not wait
-// for the kernel.  The class matrices are uploaded again only when a set_class* call changed them.
+// for the kernel.
 int FiberOps::rhs(const OwnFibers &own, const skb_fiber_params *params, const double *v_growth,
                   const double *force_scale, const double *d_v, const double *d_f, double dt, double eta,
                   double *d_rhs, int *launches, const std::function<int(const Step &stage, const Step &launch)> &frame) {
@@ -321,49 +332,30 @@ int FiberOps::rhs(const OwnFibers &own, const skb_fiber_params *params, const do
     if (nfib == 0)
         return SKB_OK;
     SKB_TRY(check_params(own, params));
-    const bool repack = rhs_class_gen != class_gen;
-    ClassPack fresh;
-    if (repack)
-        pack_classes(fresh);
-    const ClassPack &cp = repack ? fresh : rhs_pack;
-    std::vector<FiberRhsItem> items((size_t)nfib);
+    std::vector<FiberItem> items((size_t)nfib);
     std::vector<double2> growth((size_t)nfib);
-    const long long node0 = own.off[own.f0];
     int max_n = 0;
     for (int f = 0; f < nfib; ++f) {
-        const int n = own.n[own.f0 + f];
-        SKB_TRY(check_class(own.f0 + f, n, true));
+        SKB_TRY(item(own, own.f0 + f, true, items[(size_t)f]));
         const double vg = v_growth ? v_growth[f] : 0.0, fs = force_scale ? force_scale[f] : 0.0;
         if (!std::isfinite(vg) || !std::isfinite(fs))
             return set_error(SKB_ERR_INVALID, "fiber %d: v_growth = %g, force_scale = %g (both must be finite)",
                              own.f0 + f, vg, fs);
-        const auto &co = cp.off.at(n);
-        items[(size_t)f] = FiberRhsItem{own.off[own.f0 + f], own.off[own.f0 + f] - node0, co.first, co.second, n,
-                                        own.f0 + f};
         growth[(size_t)f] = make_double2(vg, fs);
-        max_n = std::max(max_n, n);
-    }
-    if (repack) {
-        rhs_pack = std::move(fresh);
-        rhs_class_gen = ~0ULL; // current once uploaded
+        max_n = std::max(max_n, items[(size_t)f].n);
     }
     const cudaStream_t st = own.stream;
     auto stage = [&]() -> int {
         if (rhs_pending) // the previous call's kernel, on whichever stream, still reads these tables
             CUDA_TRY(cudaStreamWaitEvent(st, rhs_done, 0));
-        if (rhs_class_gen != class_gen) {
-            SKB_TRY(put_async(rhs_class, rhs_pack.mats.data(), rhs_pack.mats.size() * 8, st));
-            SKB_TRY(put_async(rhs_ranges, rhs_pack.ranges.data(), rhs_pack.ranges.size() * sizeof(int2), st));
-            rhs_class_gen = class_gen;
-        }
-        SKB_TRY(put_async(rhs_items, items.data(), items.size() * sizeof(FiberRhsItem), st));
+        SKB_TRY(put_async(rhs_items, items.data(), items.size() * sizeof(FiberItem), st));
         SKB_TRY(put_async(rhs_params, params, (size_t)nfib * sizeof(skb_fiber_params), st));
         return put_async(rhs_growth, growth.data(), growth.size() * sizeof(double2), st);
     };
     auto launch = [&]() -> int {
-        const RhsArgs ra{(const FiberRhsItem *)rhs_items.ptr, (const FiberParamsDev *)rhs_params.ptr,
-                         (const double2 *)rhs_growth.ptr, (const double *)rhs_class.ptr, (const int2 *)rhs_ranges.ptr,
-                         own.r_fib, own.length, d_v, d_f, force_scale != nullptr, dt, eta, d_rhs};
+        const RhsArgs ra{(const FiberItem *)rhs_items.ptr, (const FiberParamsDev *)rhs_params.ptr,
+                         (const double2 *)rhs_growth.ptr, (const double *)class_mats.ptr,
+                         (const int2 *)class_ranges.ptr, own.r_fib, own.length, d_v, d_f, force_scale != nullptr, dt, eta, d_rhs};
         fiber_rhs_kernel<<<(unsigned)nfib, kRhsThreads, rhs_smem_bytes(max_n), st>>>(ra);
         SKB_TRY(launched(launches));
         if (!rhs_done)
@@ -400,8 +392,8 @@ int FiberOps::matvec(const double *d_x, const double *d_v, const double *d_vb, d
     if (n_items_A == 0)
         return SKB_OK;
     const FiberVelArgs va{(const double *)op_xs.ptr, d_v, (const double *)op_len.ptr, (const int *)op_plus.ptr,
-                          (const double *)op_class.ptr, (const long long *)op_classD.ptr,
-                          (const long long *)op_classP.ptr, (const int2 *)op_ranges.ptr,
+                          (const double *)class_mats.ptr, (const long long *)op_classD.ptr,
+                          (const long long *)op_classP.ptr, (const int2 *)class_ranges.ptr,
                           (const long long *)op_classR.ptr, d_vb};
     fiber_gemv_kernel<2><<<n_items_A, kFiberGemvThreads, gemv_smem, st>>>(
         (const FiberGemvItem *)items_A.ptr, (const double *)op_A.ptr, d_x, d_res, va);

@@ -153,12 +153,17 @@ struct OwnFibers {
     long long nodes() const { return f1 > f0 ? off[f1] - off[f0] : 0; }
 };
 
+struct FiberItem; // fiber_build.cuh
+
 // A_, force_operator_, xs_ and A_^-1 of one set of own fibers, resident for the timestep, and the GEMVs over them.
 // The caller has checked its pointers for NULL and made the flow's device current.
 class FiberOps {
   public:
-    int set_class(int n_nodes, const double *D_1_0, const double *P_downsample_bc); // drops the operators
-    int set_class_derivatives(int n_nodes, const double *D_2_0, const double *D_3_0, const double *D_4_0);
+    // the class matrices of n_nodes, uploaded at once on st after the device has drained (the GEMVs, the build and the
+    // RHS read them on any stream); set_class drops the operators
+    int set_class(int n_nodes, const double *D_1_0, const double *P_downsample_bc, cudaStream_t st);
+    int set_class_derivatives(int n_nodes, const double *D_2_0, const double *D_3_0, const double *D_4_0,
+                              cudaStream_t st);
     int upload(const OwnFibers &own, const double *A, const double *force_operator, const double *xs,
                const double *length_prev, const int *plus_bc_velocity);
     int upload_inverse(const double *A_inv, cudaStream_t st);
@@ -170,8 +175,8 @@ class FiberOps {
               const std::function<int(const Step &stage, const Step &launch)> &frame);
     // the fiber block of the RHS into d_rhs (4 per own node) from d_v / d_f (3 per own node, either may be NULL),
     // checked on the host first; `frame` runs stage (the table uploads on own.stream), then launch.  Needs the class
-    // matrices and derivatives, not the operators: its tables are its own, and the resident operators, their inverse
-    // and the GEMV launches stay as they are.  v_growth / force_scale per own fiber, may be NULL
+    // matrices and derivatives, not the operators: its per-fiber tables are its own, and the resident operators, their
+    // inverse and the GEMV launches stay as they are.  v_growth / force_scale per own fiber, may be NULL
     int rhs(const OwnFibers &own, const ::skb_fiber_params *params, const double *v_growth, const double *force_scale,
             const double *d_v, const double *d_f, double dt, double eta, double *d_rhs, int *launches,
             const std::function<int(const Step &stage, const Step &launch)> &frame);
@@ -196,31 +201,27 @@ class FiberOps {
         std::vector<double> D, P; // D_1_0 (n x n), P_downsample_bc ((4n-14) x 4n), column-major
         std::vector<double> D234; // D_2_0 | D_3_0 | D_4_0 (n x n each): set_class_derivatives
     };
-    // the class matrices packed into one buffer: per n the offsets of its block and of its row ranges
-    struct ClassPack {
-        std::vector<double> mats;
-        std::vector<int2> ranges;
-        std::map<int, std::pair<long long, long long>> off;
-    };
-    void pack_classes(ClassPack &cp) const;
+    int upload_classes(cudaStream_t st);
     int check_class(int f, int n, bool derivatives) const; // fiber f has n nodes: its class is set
+    int item(const OwnFibers &own, int f, bool derivatives, FiberItem &it) const; // own fiber f, check_class first
     std::map<int, FiberClass> classes;
-    unsigned long long class_gen = 0; // bumped by set_class / set_class_derivatives
+    // the device copy of `classes` (upload_classes): per n with set_class a block [D_1_0 | P_downsample_bc | D_2_0 |
+    // D_3_0 | D_4_0], the last three zero until set_class_derivatives, so that a block's offset depends only on which
+    // n have set_class; and the non-zero ranges of P's rows and D_1_0's columns.  class_off[n]: offsets of both
+    std::map<int, std::pair<long long, long long>> class_off;
+    DevBuf class_mats, class_ranges;
     bool ready_ = false;
     int f0 = 0, f1 = 0;    // the fibers of the resident operators
     long long n_nodes = 0; // ... and their nodes
     int n_items_A = 0, n_items_F = 0;
     size_t gemv_smem = 0;
-    DevBuf op_A, op_F, op_xs, op_Ainv, op_len, op_plus, op_class, op_classD, op_classP, op_classR, op_ranges, items_A,
-        items_F, bld_params, bld_items, bld_tiles, bld_inv;
+    DevBuf op_A, op_F, op_xs, op_Ainv, op_len, op_plus, op_classD, op_classP, op_classR, items_A, items_F, bld_params,
+        bld_items, bld_tiles, bld_inv;
     long long op_A_elems = 0;                        // elements of the concatenated A_ (and of A_^-1)
     long long op_F_elems = 0;                        // ... of force_operator_
     unsigned long long ops_gen = 0, precond_gen = 0; // the inverse belongs to one set of operators
-    // the RHS's own tables: the class matrices as of rhs_class_gen (kept on the host while the device copy is current),
-    // the per-fiber tables of the last call, and the event after its kernel (the next call's uploads wait for it)
-    ClassPack rhs_pack;
-    unsigned long long rhs_class_gen = ~0ULL;
-    DevBuf rhs_class, rhs_ranges, rhs_items, rhs_params, rhs_growth;
+    // the RHS's per-fiber tables of the last call, and the event after its kernel (the next call's uploads wait for it)
+    DevBuf rhs_items, rhs_params, rhs_growth;
     Event rhs_done;
     bool rhs_pending = false;
 };

@@ -1380,14 +1380,16 @@ int skb_flow_matvec_device(skb_flow *fl, const double *d_fib_forces, const doubl
 int skb_flow_set_fiber_class(skb_flow *fl, int n_nodes, const double *D_1_0, const double *P_downsample_bc) {
     if (!fl || !D_1_0 || !P_downsample_bc)
         return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_class: NULL argument");
-    return fl->ops.set_class(n_nodes, D_1_0, P_downsample_bc);
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    return fl->ops.set_class(n_nodes, D_1_0, P_downsample_bc, fl->stream);
 }
 
 int skb_flow_set_fiber_class_derivatives(skb_flow *fl, int n_nodes, const double *D_2_0, const double *D_3_0,
                                          const double *D_4_0) {
     if (!fl || !D_2_0 || !D_3_0 || !D_4_0)
         return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_class_derivatives: NULL argument");
-    return fl->ops.set_class_derivatives(n_nodes, D_2_0, D_3_0, D_4_0);
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    return fl->ops.set_class_derivatives(n_nodes, D_2_0, D_3_0, D_4_0, fl->stream);
 }
 
 // The fibers whose operators are resident: those whose rows are in this flow's target list -- all of them, or the

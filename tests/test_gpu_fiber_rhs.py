@@ -6,7 +6,9 @@ with n = 8 .. 128 mixed in
 one container, all four boundary-condition combinations, with and without each optional input, in the host form and
 the device form on a non-default stream.  Also: a straight free fiber in a uniform flow is advected through the device
 operators and their inverse; target ranges and MultiFlow tile the single-flow result bitwise; an RHS call leaves the
-resident operators, their inverse and the matvec bitwise unchanged; every rejection comes before any launch."""
+resident operators, their inverse and the matvec bitwise unchanged; class matrices replaced after use, or set in
+another order of n, leave the build, the RHS and the matvec bitwise as a flow that only saw the final ones; every
+rejection comes before any launch."""
 import os
 import shutil
 import subprocess
@@ -223,7 +225,8 @@ def test_rhs_leaves_the_operators_untouched(system):
                 fl.set_fiber_preconditioner(ops["A_inv"])
             before, ops0 = matvec(fl), fl.get_fiber_operators()
             first = rhs_host(fl, prm, inp)
-            # class derivatives set again (same values, the operators stay): the RHS uploads its class tables anew
+            # class derivatives set again (same values, the operators stay): the class table is uploaded anew under
+            # the resident operators, whose GEMV reads it at the same offsets
             n = fib["n_nodes"][0]
             m = fiber_fd_matrices(n)
             fl.set_fiber_class_derivatives(n, m["D_2_0"], m["D_3_0"], m["D_4_0"])
@@ -234,6 +237,77 @@ def test_rhs_leaves_the_operators_untouched(system):
             for k in ("A", "force", "A_inv"):
                 assert all(np.array_equal(a, b) for a, b in zip(ops0[k], ops1[k])), (how, k)
             assert np.array_equal(ops0["xs"], ops1["xs"]), how
+
+
+def set_class_matrices(fl, n_values, scale=1.0, derivatives_first=False):
+    for n in n_values:
+        m = {k: v * scale for k, v in fiber_fd_matrices(n).items() if k.startswith(("D_", "P_downsample"))}
+        calls = [lambda: fl.set_fiber_class(n, m["D_1_0"], m["P_downsample_bc"]),
+                 lambda: fl.set_fiber_class_derivatives(n, m["D_2_0"], m["D_3_0"], m["D_4_0"])]
+        for call in calls[::-1] if derivatives_first else calls:
+            call()
+
+
+def class_table_outputs(fl, fib, prm, inp, shell, body):
+    """what the class table feeds: the build's operators and inverse, the RHS, the matvec and the preconditioner"""
+    rng = np.random.default_rng(5)
+    x = rng.normal(size=4 * fib["pos"].shape[0])
+    link = rng.normal(size=(len(fib["n_nodes"]), 7))
+    return (fl.get_fiber_operators(), rhs_host(fl, prm, inp),
+            fl.apply_matvec(x, shell["density"], body["density"], ft_of(body), ETA, link) +
+            (fl.apply_fiber_preconditioner(x),))
+
+
+def assert_same_outputs(got, want, label):
+    ops, rhs, mv = got
+    for k in ("A", "force", "A_inv"):
+        assert all(np.array_equal(a, b) for a, b in zip(ops[k], want[0][k])), (label, k)
+    assert np.array_equal(ops["xs"], want[0]["xs"]), label
+    assert np.array_equal(rhs, want[1]), label
+    for a, b in zip(mv, want[2]):
+        assert np.array_equal(a, b), label
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("derivatives_first", [False, True])
+def test_class_matrices_replaced(system, derivatives_first):
+    """perturbed class matrices in use (a build, an RHS, uploaded operators), then the real ones again: every output
+    equals a flow's that only ever saw the real ones"""
+    fib, prm, inp, _ = system
+    shell, body = empty_shell_body(3, 200, 60)
+    n_values = sorted(set(fib["n_nodes"]))
+    with skb.Flow(0) as fl:
+        load(fl, fib, shell, body)
+        set_class_matrices(fl, n_values)
+        build(fl, prm)
+        want = class_table_outputs(fl, fib, prm, inp, shell, body)
+    with skb.Flow(0) as fl:
+        load(fl, fib, shell, body)
+        set_class_matrices(fl, n_values, scale=1.0 + 1e-3)
+        build(fl, prm)
+        perturbed = rhs_host(fl, prm, inp)
+        assert not np.array_equal(perturbed, want[1])
+        ops = fl.get_fiber_operators()
+        fl.set_fiber_operators(ops["A"], ops["force"], ops["xs"], prm["length_prev"], prm["plus_hinged"])
+        fl.set_fiber_preconditioner(ops["A_inv"])
+        set_class_matrices(fl, n_values, derivatives_first=derivatives_first)
+        build(fl, prm)
+        assert_same_outputs(class_table_outputs(fl, fib, prm, inp, shell, body), want, derivatives_first)
+
+
+@pytest.mark.gpu
+def test_class_order_does_not_matter(system):
+    """the classes set in ascending and in descending n give the same operators, RHS and matvec"""
+    fib, prm, inp, _ = system
+    shell, body = empty_shell_body(3, 200, 60)
+    out = []
+    for n_values in (sorted(set(fib["n_nodes"])), sorted(set(fib["n_nodes"]), reverse=True)):
+        with skb.Flow(0) as fl:
+            load(fl, fib, shell, body)
+            set_class_matrices(fl, n_values)
+            build(fl, prm)
+            out.append(class_table_outputs(fl, fib, prm, inp, shell, body))
+    assert_same_outputs(out[1], out[0], "descending")
 
 
 @pytest.mark.gpu
