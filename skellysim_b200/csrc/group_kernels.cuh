@@ -3,20 +3,14 @@
 //
 // A group is one skb_flow per GPU -- all in one process (skb_mflow: the shape the reference's "direct evaluators need
 // a single rank" rule admits, src/core/system.cpp:618-623) or one per process (CUDA IPC, rank-per-GPU hosts).  Every
-// member owns a WINDOW of device memory that all members can address:
-//
-//   flags    [4][kMaxGroup]  epoch counters, one slot per (phase, writer)                  -- written by peers
-//   f_sl     [2][n_pad_fib*3]   packed (trapezoid-weighted) Stokeslet strengths of ALL fiber nodes   -- by peers
-//   f_shell  [2][n_pad_shell*6] packed sym6 stresslet strengths of ALL periphery nodes                -- by peers
-//   x_shell  [2][n_shell*3]     periphery density of ALL nodes (input of the dense operator)          -- by peers
-//   u_part   [n_fib*3]          this member's partial fiber velocities (its rows of the symmetric block) -- by itself
+// member owns a WINDOW of device memory that all members can address; its layout is described at the declaration of
+// skb::Group (skb_internal.hpp), whose steps (skb_group.cu, the only includer of this file) launch these kernels.
 //
 // One matvec = (1) PUSH: every member packs the strengths of ITS fibers / periphery rows once and stores them into
 // all windows (the pack kernel and the all-gather are one kernel; 2.3 MB per member at 1e5 nodes); (2) flag barrier;
 // (3) pair kernels on local memory only (TMA sources come from the member's own window); (4) flag barrier;
-// (5) PULL: every member adds up the partial velocities of its own fiber rows from all windows (the reduce-scatter,
-// fused with the accumulation into the velocity vector).  [2] = double buffering by epoch parity: a peer may already
-// push the next matvec's strengths while this member still reads the current ones.
+// (5) PULL: every member adds up the partial velocities of its own fiber rows (and, with the cross kernel, of its own
+// periphery rows) from all windows (the reduce-scatter, fused with the accumulation into the velocity vector).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -114,7 +108,7 @@ __global__ void group_flag_kernel(const GroupFlagArgs a) {
 }
 
 struct GroupPullArgs {
-    const double *u_part[kMaxGroup]; // every member's partial fiber velocities [n_fib*3]
+    const double *u_part[kMaxGroup]; // every member's partial velocities (u_part [n_fib*3] or u_part_shell [n_shell*3])
     int size;
     long long fa, n_f; // own fiber rows
     double *v;         // [n_f*3] (+)= sum over members, fixed order

@@ -135,7 +135,7 @@ struct EvalOpts {
                                // d_u_out + 3 n_src (group mode: the leading rows are partial sums that live elsewhere)
 };
 
-constexpr int kMaxGroup = 16; // members of a multi-GPU group (group_kernels.cuh, skb_mflow)
+constexpr int kMaxGroup = 16; // members of a multi-GPU group (Group, group_kernels.cuh, skb_mflow)
 
 // forces_torques [6 x n_bodies] (body_container.cpp:134) -> forces and torques, 3 x n_bodies each
 void split_forces_torques(const double *ft, int n_bodies, std::vector<double> &f, std::vector<double> &t);
@@ -224,6 +224,78 @@ class FiberOps {
     DevBuf rhs_items, rhs_params, rhs_growth;
     Event rhs_done;
     bool rhs_pending = false;
+};
+
+// ---- one member of a multi-GPU group of flows (DESIGN.md §4; skb_group.cu, group_kernels.cuh) ----
+// A group is one flow per GPU exchanging strengths and partial velocities through peer memory.  Every member owns a
+// WINDOW of device memory that all members can address, laid out by init (each piece 256-byte aligned):
+//
+//   flags        [4][kMaxGroup] + 8  epoch counters, one slot per (phase, writer); then the error word (0, or
+//                                    1 + the rank a flag wait gave up on)                        -- written by peers
+//   f_sl         [2][n_pad_fib*3]    packed (trapezoid-weighted) Stokeslet strengths of ALL fiber nodes   -- by peers
+//   f_shell      [2][n_pad_shell*6]  packed sym6 stresslet strengths of ALL periphery nodes                -- by peers
+//   x_shell      [2][n_shell*3]      periphery density of ALL nodes (input of the dense operator)          -- by peers
+//   u_part       [n_fib*3]           this member's partial velocities of ALL fiber rows                  -- by itself
+//   u_part_shell [n_shell*3]         its partial velocities of ALL periphery rows (cross kernel)        -- by itself
+//
+// [2]: double buffering by epoch parity -- a peer may already push the next matvec's strengths while this member still
+// reads the current ones.  A default-constructed Group is no member (size 1).  Knows nothing of skb_flow: the caller
+// has made the flow's device current, and every step runs on the stream it passes, adding its launches to *launches.
+class Group {
+  public:
+    // allocates and zeroes the window of member `rank` of `size` for that many fiber / periphery nodes; n_pad_*: the
+    // padded source counts of the flow's evaluators (the window replaces their packed strengths).  Size 1: no member
+    int init(int rank, int size, long long n_fib, long long n_pad_fib, long long n_shell, long long n_pad_shell);
+    int export_handle(void *handle) const;                     // the window's CUDA-IPC handle
+    int import_handle(int peer_rank, const void *handle);      // maps another process's member's window
+    int connect(int peer_rank, const Group &peer, int dev, int peer_dev); // a member in this process, on peer_dev
+    int missing_peer(int *missing) const; // -1, or the rank a flag wait gave up on (no window: -1)
+
+    bool member() const { return size_ > 1; }
+    bool has_window() const { return window_.get() != nullptr; }
+    int rank() const { return rank_; }
+    int size() const { return size_; }
+    int check_layout(long long n_fib, long long n_shell) const; // an error unless the window was laid out for these
+    // solo (warm-up, profiling): no flags, push and pull over this member's own window only, no connectedness check
+    void set_solo(bool solo) { solo_ = solo; }
+    void restart() { epoch_ = 0; } // the next matvec is the group's first
+
+    // ---- one matvec: begin, push, barrier(0), pair kernels, barrier(1), pull ----
+    int begin(); // refuses a member whose peers are not all connected; advances the epoch (its parity picks the half)
+    // pack the own strengths once and store them into every window: fiber forces d_fw [n_f*3] of nodes [fa, fa + n_f)
+    // (weighted by d_weight of ALL fiber nodes, NULL: 1), periphery densities d_density [n_s*3] of rows [sa, sa + n_s)
+    // (sym6 with two_eta and d_normal of ALL periphery nodes, and raw into x_shell)
+    int push(const double *d_fw, const double *d_weight, long long fa, long long n_f, const double *d_density,
+             const double *d_normal, long long sa, long long n_s, double two_eta, int num_sms, cudaStream_t st,
+             int *launches) const;
+    int barrier(int phase, bool signal, bool wait, cudaStream_t st, int *launches) const;
+    // d_v rows [0, n_rows) += the sum of every member's partial rows [row0, row0 + n_rows), in rank order
+    enum Partials { kFiberRows, kShellRows };
+    int pull(Partials which, long long row0, long long n_rows, double *d_v, cudaStream_t st, int *launches) const;
+
+    // this member's window, in the half of the matvec in flight
+    double *f_sl() const { return own(lay_.f_sl[epoch_ & 1]); }
+    double *f_shell() const { return own(lay_.f_shell[epoch_ & 1]); }
+    double *x_shell() const { return own(lay_.x_shell[epoch_ & 1]); }
+    double *u_part() const { return own(lay_.u_part); }
+    double *u_part_shell() const { return own(lay_.u_part_shell); }
+
+  private:
+    struct Layout { // byte offsets of the window's pieces
+        size_t flags = 0, f_sl[2] = {0, 0}, f_shell[2] = {0, 0}, x_shell[2] = {0, 0}, u_part = 0, u_part_shell = 0;
+        size_t bytes = 0;
+    };
+    double *own(size_t off) const { return reinterpret_cast<double *>((char *)window_.get() + off); }
+    int windows(char **w) const; // the windows push and pull reach (solo: the own one only); returns their count
+
+    int rank_ = 0, size_ = 1;
+    DevPtr window_;              // this member's window (cudaMalloc: exportable through CUDA IPC)
+    Layout lay_;
+    void *peer_[kMaxGroup] = {}; // every member's window as mapped here (peer_[rank_] == window_)
+    IpcPtr ipc_[kMaxGroup];      // the windows of other processes' members that this one has mapped
+    long long n_fib_ = 0, n_shell_ = 0; // geometry the window was laid out for
+    unsigned long long epoch_ = 0;
+    bool solo_ = false;
 };
 
 } // namespace skb

@@ -3,7 +3,6 @@
 // (src/core/system.cpp:284-316).  Built on the pair-kernel contexts of skb_runtime.cu; everything between the
 // upload of the strengths and the download of the velocities stays on the device.
 #include "aux_kernels.cuh"
-#include "group_kernels.cuh"
 #include "skb_internal.hpp"
 #include "../../include/skelly_b200_flow.h"
 #include "../../include/skelly_b200_dense.h"
@@ -93,26 +92,7 @@ struct skb_flow {
     std::vector<int> h_fiber_n;         // nodes of every fiber
     std::vector<long long> h_fiber_off; // first node of every fiber (n_fibers + 1)
     FiberOps ops; // per-fiber dense operators of the fibers whose rows are in the target list (skb_fiber.cu)
-    // multi-GPU group (group_kernels.cuh): one member per GPU, exchange through peer memory
-    struct Group {
-        int rank = 0, size = 1;
-        DevPtr window;                // this member's window (cudaMalloc: exportable through CUDA IPC)
-        size_t window_bytes = 0;
-        void *peer[kMaxGroup] = {};   // base address of every member's window as mapped here (peer[rank] == window)
-        IpcPtr ipc[kMaxGroup];        // the windows of other processes' members that this one has mapped
-        size_t off_flags = 0, off_fsl[2] = {0, 0}, off_fshell[2] = {0, 0}, off_xshell[2] = {0, 0}, off_upart = 0;
-        size_t off_upart_shell = 0;   // partial periphery velocities (cross kernel: own fibers -> ALL periphery rows)
-        long long n_fib = 0, n_shell = 0, n_pad_fib = 0, n_pad_shell = 0; // geometry the window was laid out for
-        unsigned long long epoch = 0;
-        bool dry = false;             // warm-up pass: no flags, own window only (skb_flow_group_warmup)
-        bool connected() const {
-            for (int m = 0; m < size; ++m)
-                if (!peer[m])
-                    return false;
-            return true;
-        }
-        template <class T> T *at(int member, size_t off) const { return reinterpret_cast<T *>((char *)peer[member] + off); }
-    } grp;
+    Group grp; // multi-GPU group membership: one member per GPU, exchange through peer memory (skb_group.cu)
     // Periphery::matvec's dense operator beside the pair kernels (stream_kernels.cuh): forked onto bg_stream once its
     // input (the complete x_shell) is there, joined before res_shell is assembled
     struct Overlap {
@@ -772,15 +752,12 @@ static int prepare_matvec_targets(skb_flow *fl) {
     }
     const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa, n_bw = fl->bb - fl->ba;
     fl->n_win = n_fw + n_sw + n_bw;
-    const bool grouped = fl->grp.size > 1;
+    const bool grouped = fl->grp.member();
     if (grouped) {
         if (!fl->use_ranges)
             return set_error(SKB_ERR_STATE, "group member: call skb_flow_set_target_ranges (own fibers / periphery rows / "
                                             "body rows) before the first matvec");
-        if (fl->grp.n_fib != nf || fl->grp.n_shell != ns)
-            return set_error(SKB_ERR_STATE, "group member: the geometry changed size since skb_flow_group_init "
-                                            "(%lld/%lld fiber, %lld/%lld periphery nodes); re-initialise the group",
-                             nf, fl->grp.n_fib, ns, fl->grp.n_shell);
+        SKB_TRY(fl->grp.check_layout(nf, ns));
     }
     // group: fiber rows through the symmetric block rows of this member (partial sums, pulled together afterwards)
     // when the self-interaction is big enough for that kernel; otherwise the member's own rows with the plain kernel
@@ -821,7 +798,7 @@ static int prepare_matvec_targets(skb_flow *fl) {
             r_sym.insert(r_sym.end(), fl->h_r_shell.begin() + 3 * fl->sa, fl->h_r_shell.begin() + 3 * fl->sb);
         r_sym.insert(r_sym.end(), fl->h_r_body.begin() + 3 * fl->ba, fl->h_r_body.begin() + 3 * fl->bb);
         SKB_TRY(skb_ctx_set_symmetric(fl->fib[1].get(), 1));
-        SKB_TRY(skb_ctx_set_sym_partition(fl->fib[1].get(), fl->grp.rank, fl->grp.size));
+        SKB_TRY(skb_ctx_set_sym_partition(fl->fib[1].get(), fl->grp.rank(), fl->grp.size()));
         SKB_TRY(skb_set_targets(fl->fib[1].get(), r_sym.data(), (long long)r_sym.size() / 3));
     } else if (use_cross) {
         std::vector<double> r_fibbody(fl->h_r_fib.begin() + 3 * fl->fa, fl->h_r_fib.begin() + 3 * fl->fb);
@@ -875,8 +852,7 @@ static int overlap_buffers(skb_flow *fl, long long n_rows) {
 // the complete x_shell on this device, input of the periphery's dense operator: the caller's vector without a group;
 // with one, the gathered copy in the window half (epoch parity) of the group matvec in flight
 static const double *full_x_shell(const skb_flow *fl, const double *d_xs) {
-    const skb_flow::Group &G = fl->grp;
-    return G.size > 1 ? G.at<double>(G.rank, G.off_xshell[G.epoch & 1]) : d_xs;
+    return fl->grp.member() ? fl->grp.x_shell() : d_xs;
 }
 
 static int overlap_launch(skb_flow *fl, const double *d_xs) {
@@ -893,73 +869,6 @@ static int overlap_launch(skb_flow *fl, const double *d_xs) {
     return SKB_OK;
 }
 
-static int group_flag(skb_flow *fl, int phase, bool do_signal, bool do_wait) {
-    skb_flow::Group &G = fl->grp;
-    if (G.dry)
-        return SKB_OK;
-    GroupFlagArgs a;
-    for (int m = 0; m < G.size; ++m)
-        a.flags[m] = G.at<unsigned long long>(m, G.off_flags);
-    a.rank = G.rank;
-    a.size = G.size;
-    a.phase = phase;
-    a.epoch = G.epoch;
-    a.do_signal = do_signal;
-    a.do_wait = do_wait;
-    a.timeout_cycles = 20ULL * 1000 * 1000 * 1000; // ~10 s at 2 GHz
-    group_flag_kernel<<<1, 32, 0, fl->cur>>>(a);
-    return launched(fl, 1);
-}
-
-// PUSH: pack the own strengths once and store them into every member's window (pack + all-gather in one kernel)
-static int group_push(skb_flow *fl, const double *d_ff, const double *d_sd, double eta) {
-    skb_flow::Group &G = fl->grp;
-    const DeviceState &df = fl->fib[1]->devs[0];
-    const int par = (int)(G.epoch & 1);
-    const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
-    GroupPushArgs a;
-    a.fw = d_ff;
-    a.weight = df.src[SKB_STOKESLET].has_weights ? (const double *)df.src[SKB_STOKESLET].weights.ptr : nullptr;
-    a.fa = fl->fa;
-    a.n_f = n_fw;
-    a.density = d_sd;
-    a.normal = fl->n_shell ? (const double *)fl->shell[1]->devs[0].src[SKB_STRESSLET].normals.ptr : nullptr;
-    a.sa = fl->sa;
-    a.n_s = n_sw;
-    a.two_eta = 2.0 * eta;
-    a.size = G.dry ? 1 : G.size;
-    for (int m = 0; m < a.size; ++m) {
-        const int who = G.dry ? G.rank : m;
-        a.f_sl[m] = G.at<double>(who, G.off_fsl[par]);
-        a.f_shell[m] = G.at<double>(who, G.off_fshell[par]);
-        a.x_shell[m] = G.at<double>(who, G.off_xshell[par]);
-    }
-    const long long work = 3 * n_fw + n_sw;
-    if (work == 0)
-        return SKB_OK;
-    const unsigned nblk = (unsigned)std::min<long long>((work + 255) / 256, 4LL * df.info.num_sms);
-    group_push_kernel<<<nblk, 256, 0, fl->cur>>>(a);
-    return launched(fl, 1);
-}
-
-// PULL: d_v rows [0, n_rows) += the sum of every member's partial rows [row0, row0 + n_rows) at window offset `off`
-// (reduce-scatter fused with the accumulation)
-static int group_pull(skb_flow *fl, size_t off, long long row0, long long n_rows, double *d_v) {
-    if (n_rows == 0)
-        return SKB_OK;
-    const skb_flow::Group &G = fl->grp;
-    GroupPullArgs a;
-    a.size = G.dry ? 1 : G.size;
-    for (int m = 0; m < a.size; ++m)
-        a.u_part[m] = G.at<double>(G.dry ? G.rank : m, off);
-    a.fa = row0;
-    a.n_f = n_rows;
-    a.v = d_v;
-    a.accumulate = 1;
-    group_pull_kernel<<<(unsigned)((3 * n_rows + 255) / 256), 256, 0, fl->cur>>>(a);
-    return launched(fl, 1);
-}
-
 // v = fc.flow(r_all, fw, eta)  (system.cpp:299) at the fiber evaluator's targets.  Symmetric producers: the symmetric
 // kernel writes the fiber rows -- complete, or in a group this member's partial sums for ALL fiber rows into its
 // window -- and the plain kernel the rest: [own periphery rows (not with the cross kernel) | own body rows]
@@ -967,22 +876,22 @@ static int fiber_rows(skb_flow *fl, StrengthMode mode, const double *ff, double 
     const skb_flow::MatvecPlan &P = fl->plan;
     if (P.fib_rows == skb_flow::MatvecPlan::kPlain)
         return fibers_dev(fl, fl->fib[1].get(), mode, ff, eta, 0, d_v, 0, fl->fa, fl->fb);
-    const skb_flow::Group &G = fl->grp;
+    const Group &G = fl->grp;
     const long long nf = fl->n_fib, n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa, n_bw = fl->bb - fl->ba;
     DeviceState &df = fl->fib[1]->devs[0];
     SKB_TRY(fl->scratch_u.ensure((size_t)df.n_trg * 24 + 8));
     EvalOpts o;
-    o.d_u_sym = P.grouped ? G.at<double>(G.rank, G.off_upart) : d_v;
+    o.d_u_sym = P.grouped ? G.u_part() : d_v;
     o.d_u_rem = d_v + 3 * (n_fw + (P.cross ? n_sw : 0));
     SKB_TRY(eval_on_device(fl->fib[1].get(), df, SKB_STOKESLET, mode, ff, 0.0, (double *)fl->scratch_u.ptr, 0, fl->cur,
                            false, &fl->launches, nullptr, 1.0 / eta, o));
-    fl->pairs += nf * nf / (P.grouped ? G.size : 1) + nf * ((P.cross ? 0 : n_sw) + n_bw);
+    fl->pairs += nf * nf / (P.grouped ? G.size() : 1) + nf * ((P.cross ? 0 : n_sw) + n_bw);
     if (fl->fib[1]->last_was_sym)
         return SKB_OK;
     if (P.grouped)
         return set_error(SKB_ERR_STATE, "group member %d: the symmetric kernel declined (memory for the reverse "
                                         "partials?); lower SKB_SYM_MAX_BYTES pressure or use fewer nodes per GPU",
-                         G.rank);
+                         G.rank());
     // the symmetric path declined (memory): everything landed contiguously in the scratch buffer
     CUDA_TRY(cudaMemcpyAsync(d_v, fl->scratch_u.ptr, (size_t)n_fw * 24, cudaMemcpyDeviceToDevice, fl->cur));
     if (n_bw > 0)
@@ -998,11 +907,10 @@ static int fiber_rows(skb_flow *fl, StrengthMode mode, const double *ff, double 
 // and the own periphery rows start from zero until the members' partials are pulled in.
 static int cross_rows(skb_flow *fl, const double *s6, double eta, double *d_v) {
     const bool grouped = fl->plan.grouped;
-    const skb_flow::Group &G = fl->grp;
     const long long ns = fl->n_shell, n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
     DeviceState &df = fl->fib[1]->devs[0];
     const SourceSet &sf = df.src[SKB_STOKESLET], &ss = fl->shell[1]->devs[0].src[SKB_STRESSLET];
-    double *u_shell = grouped ? G.at<double>(G.rank, G.off_upart_shell) : d_v + 3 * n_fw;
+    double *u_shell = grouped ? fl->grp.u_part_shell() : d_v + 3 * n_fw;
     SKB_TRY(cross_eval(fl->cross, df.info, (const double *)sf.r.ptr, sf.f_cur, fl->fa, n_fw, (const double *)ss.r.ptr,
                        s6, ns, ss.n_pad, -3.0 / (8.0 * M_PI * eta), 1.0 / (8.0 * M_PI * eta), d_v, grouped ? 0 : 1,
                        u_shell, 0, fl->cur, &fl->launches));
@@ -1049,21 +957,22 @@ static int periphery_rows(skb_flow *fl, StrengthMode mode, const double *sd, dou
 static int matvec_core(skb_flow *fl, const double *d_ff, const double *d_sd, const double *d_bd, const double *d_f,
                        const double *d_t, double eta, double *d_v) {
     const skb_flow::MatvecPlan &P = fl->plan;
-    skb_flow::Group &G = fl->grp;
+    Group &G = fl->grp;
     const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
     // strengths as the caller ships them (packed by the evaluations), or packed by the push into the group window
     StrengthMode fmode = kRaw, smode = kNormalDensity;
     const double *ff = d_ff, *sd = d_sd;
     if (P.grouped) {
-        if (!G.dry && !G.connected())
-            return set_error(SKB_ERR_STATE, "group member %d: not all peers are connected (skb_flow_group_import / "
-                                            "_connect)", G.rank);
-        G.epoch += 1; // the only place it advances: its parity picks the window half of this matvec
-        SKB_TRY(group_push(fl, d_ff, d_sd, eta));
-        SKB_TRY(group_flag(fl, 0, true, true)); // every member's strengths have landed here
+        SKB_TRY(G.begin());
+        const DeviceState &df = fl->fib[1]->devs[0];
+        const SourceSet &sf = df.src[SKB_STOKESLET];
+        SKB_TRY(G.push(d_ff, sf.has_weights ? (const double *)sf.weights.ptr : nullptr, fl->fa, n_fw, d_sd,
+                       fl->n_shell ? (const double *)fl->shell[1]->devs[0].src[SKB_STRESSLET].normals.ptr : nullptr,
+                       fl->sa, n_sw, 2.0 * eta, df.info.num_sms, fl->cur, &fl->launches));
+        SKB_TRY(G.barrier(0, true, true, fl->cur, &fl->launches)); // every member's strengths have landed here
         fmode = smode = kPacked;
-        ff = G.at<double>(G.rank, G.off_fsl[G.epoch & 1]);
-        sd = G.at<double>(G.rank, G.off_fshell[G.epoch & 1]);
+        ff = G.f_sl();
+        sd = G.f_shell();
     } else if (fl->n_win == 0) {
         return SKB_OK;
     }
@@ -1084,106 +993,58 @@ static int matvec_core(skb_flow *fl, const double *d_ff, const double *d_sd, con
     }
     const bool partial = P.fib_rows == skb_flow::MatvecPlan::kSymPartial;
     if (partial)
-        SKB_TRY(group_flag(fl, 1, true, false)); // my partial sums are complete
+        SKB_TRY(G.barrier(1, true, false, fl->cur, &fl->launches)); // my partial sums are complete
     SKB_TRY(periphery_rows(fl, smode, sd, eta, d_v));
     // v_all += bc.flow(r_all, x_bodies, body_link_conditions, eta)     (system.cpp:316)
     SKB_TRY(bodies_dev(fl, fl->body[1].get(), d_bd, d_f, d_t, eta, d_v, 1));
     if (partial) {
-        SKB_TRY(group_flag(fl, 1, false, true));
-        SKB_TRY(group_pull(fl, G.off_upart, fl->fa, n_fw, d_v));
+        SKB_TRY(G.barrier(1, false, true, fl->cur, &fl->launches));
+        SKB_TRY(G.pull(Group::kFiberRows, fl->fa, n_fw, d_v, fl->cur, &fl->launches));
         if (P.cross) // own periphery rows += the members' Stokeslet partials
-            SKB_TRY(group_pull(fl, G.off_upart_shell, fl->sa, n_sw, d_v + 3 * n_fw));
+            SKB_TRY(G.pull(Group::kShellRows, fl->sa, n_sw, d_v + 3 * n_fw, fl->cur, &fl->launches));
     }
     if (P.grouped)
         SKB_TRY(fiber_self_term(fl, fl->fib[1].get(), eta, d_v, fl->fa, fl->fb));
     return SKB_OK;
 }
 
-// ---- group membership (multi-GPU through peer memory, group_kernels.cuh) ------------------------------------------
+// ---- group membership (multi-GPU through peer memory, skb_group.cu) ----------------------------------------------
 int skb_flow_group_init(skb_flow *fl, int rank, int size) {
     if (!fl || size < 1 || size > kMaxGroup || rank < 0 || rank >= size)
         return set_error(SKB_ERR_INVALID, "skb_flow_group_init: need 0 <= rank < size <= %d", kMaxGroup);
     CUDA_TRY(cudaSetDevice(fl->dev));
     CUDA_TRY(cudaStreamSynchronize(fl->stream));
-    fl->grp = skb_flow::Group();
     fl->mv_dirty = true;
     fl->ops.invalidate();
     fl->geom_version++;
-    if (size == 1)
-        return SKB_OK;
-    skb_flow::Group &G = fl->grp;
-    G.rank = rank;
-    G.size = size;
-    G.n_fib = fl->n_fib;
-    G.n_shell = fl->n_shell;
     // the same padded sizes the evaluator contexts use (set_sources_impl): the window replaces their f_packed
-    G.n_pad_fib = fl->n_fib > 0 ? fl->fib[1]->devs[0].src[SKB_STOKESLET].n_pad : 0;
-    G.n_pad_shell = fl->n_shell > 0 ? fl->shell[1]->devs[0].src[SKB_STRESSLET].n_pad : 0;
-    size_t off = 0;
-    auto take = [&](size_t bytes) {
-        const size_t at = off;
-        off += (bytes + 255) & ~(size_t)255;
-        return at;
-    };
-    G.off_flags = take((size_t)(kGroupPhases * kMaxGroup + 8) * 8);
-    for (int b = 0; b < 2; ++b) {
-        G.off_fsl[b] = take((size_t)G.n_pad_fib * 24 + 16);
-        G.off_fshell[b] = take((size_t)G.n_pad_shell * 48 + 16);
-        G.off_xshell[b] = take((size_t)G.n_shell * 24 + 16);
-    }
-    G.off_upart = take((size_t)G.n_fib * 24 + 16);
-    G.off_upart_shell = take((size_t)G.n_shell * 24 + 16);
-    G.window_bytes = off;
-    CUDA_TRY(cudaMalloc(G.window.out(), G.window_bytes));
-    CUDA_TRY(cudaMemset(G.window, 0, G.window_bytes)); // flags at epoch 0, strength pads zero for good
-    G.peer[rank] = G.window;
-    return SKB_OK;
+    const long long n_pad_fib = fl->n_fib > 0 ? fl->fib[1]->devs[0].src[SKB_STOKESLET].n_pad : 0;
+    const long long n_pad_shell = fl->n_shell > 0 ? fl->shell[1]->devs[0].src[SKB_STRESSLET].n_pad : 0;
+    return fl->grp.init(rank, size, fl->n_fib, n_pad_fib, fl->n_shell, n_pad_shell);
 }
 
 int skb_flow_group_export(skb_flow *fl, void *handle) {
-    if (!fl || !handle || !fl->grp.window)
+    if (!fl || !handle || !fl->grp.has_window())
         return set_error(SKB_ERR_INVALID, "skb_flow_group_export: no group window (skb_flow_group_init with size > 1 first)");
-    static_assert(sizeof(cudaIpcMemHandle_t) == SKB_FLOW_IPC_HANDLE_BYTES, "handle size");
     CUDA_TRY(cudaSetDevice(fl->dev));
-    cudaIpcMemHandle_t h;
-    CUDA_TRY(cudaIpcGetMemHandle(&h, fl->grp.window));
-    std::memcpy(handle, &h, sizeof(h));
-    return SKB_OK;
+    return fl->grp.export_handle(handle);
 }
 
 int skb_flow_group_import(skb_flow *fl, int peer_rank, const void *handle) {
-    if (!fl || !handle || !fl->grp.window || peer_rank < 0 || peer_rank >= fl->grp.size || peer_rank == fl->grp.rank)
+    if (!fl || !handle || !fl->grp.has_window() || peer_rank < 0 || peer_rank >= fl->grp.size() ||
+        peer_rank == fl->grp.rank())
         return set_error(SKB_ERR_INVALID, "skb_flow_group_import: bad arguments");
     CUDA_TRY(cudaSetDevice(fl->dev));
-    cudaIpcMemHandle_t h;
-    std::memcpy(&h, handle, sizeof(h));
-    CUDA_TRY(cudaIpcOpenMemHandle(fl->grp.ipc[peer_rank].out(), h, cudaIpcMemLazyEnablePeerAccess));
-    fl->grp.peer[peer_rank] = fl->grp.ipc[peer_rank];
-    return SKB_OK;
+    return fl->grp.import_handle(peer_rank, handle);
 }
 
 int skb_flow_group_connect(skb_flow *fl, int peer_rank, skb_flow *peer) {
-    if (!fl || !peer || !fl->grp.window || !peer->grp.window || peer_rank < 0 || peer_rank >= fl->grp.size ||
-        peer_rank == fl->grp.rank || peer->grp.rank != peer_rank || peer->grp.size != fl->grp.size)
+    if (!fl || !peer || !fl->grp.has_window() || !peer->grp.has_window() || peer_rank < 0 ||
+        peer_rank >= fl->grp.size() || peer_rank == fl->grp.rank() || peer->grp.rank() != peer_rank ||
+        peer->grp.size() != fl->grp.size())
         return set_error(SKB_ERR_INVALID, "skb_flow_group_connect: bad arguments");
-    if (peer->grp.window_bytes != fl->grp.window_bytes || peer->grp.n_fib != fl->grp.n_fib ||
-        peer->grp.n_shell != fl->grp.n_shell)
-        return set_error(SKB_ERR_INVALID, "skb_flow_group_connect: the two members were laid out for different geometries");
     CUDA_TRY(cudaSetDevice(fl->dev));
-    if (peer->dev != fl->dev) {
-        int can = 0;
-        CUDA_TRY(cudaDeviceCanAccessPeer(&can, fl->dev, peer->dev));
-        if (!can)
-            return set_error(SKB_ERR_CUDA, "device %d cannot address device %d (no NVLink / P2P path)", fl->dev, peer->dev);
-        cudaError_t e = cudaDeviceEnablePeerAccess(peer->dev, 0);
-        if (e == cudaErrorPeerAccessAlreadyEnabled)
-            (void)cudaGetLastError();
-        else if (e != cudaSuccess)
-            return set_error(SKB_ERR_CUDA, "cudaDeviceEnablePeerAccess(%d -> %d): %s", fl->dev, peer->dev,
-                             cudaGetErrorString(e));
-    }
-    fl->grp.peer[peer_rank] = peer->grp.window;
-    return SKB_OK;
+    return fl->grp.connect(peer_rank, peer->grp, fl->dev, peer->dev);
 }
 
 // One matvec of this member alone (no flags, own window only, zero strengths): every buffer of the path reaches its
@@ -1192,7 +1053,7 @@ int skb_flow_group_connect(skb_flow *fl, int peer_rank, skb_flow *peer) {
 int skb_flow_group_warmup(skb_flow *fl) {
     if (!fl)
         return set_error(SKB_ERR_INVALID, "skb_flow_group_warmup: NULL flow");
-    if (fl->grp.size <= 1)
+    if (!fl->grp.member())
         return SKB_OK;
     CUDA_TRY(cudaSetDevice(fl->dev));
     SKB_TRY(prepare_matvec_targets(fl));
@@ -1206,12 +1067,12 @@ int skb_flow_group_warmup(skb_flow *fl) {
     if (n_sw > 0)
         SKB_TRY(flow_size_overlap(fl, 3 * n_sw));
     fl->cur = fl->stream;
-    fl->grp.dry = true;
+    fl->grp.set_solo(true);
     const double *zp = (const double *)z.ptr;
     int rc = matvec_core(fl, zp, zp, zp, zp, zp, 1.0, (double *)fl->vel.ptr);
-    fl->grp.dry = false;
+    fl->grp.set_solo(false);
     cudaError_t e = cudaStreamSynchronize(fl->stream);
-    fl->grp.epoch = 0;
+    fl->grp.restart();
     if (rc != SKB_OK)
         return rc;
     if (e != cudaSuccess)
@@ -1222,25 +1083,17 @@ int skb_flow_group_warmup(skb_flow *fl) {
 // Profiling aid: evaluate this member's share ALONE from now on (no flags, own window only) -- the per-rank device time
 // of an n-way group on one GPU.  Results are the member's partial view, not the group's.
 int skb_flow_group_set_solo(skb_flow *fl, int solo) {
-    if (!fl || fl->grp.size <= 1)
+    if (!fl || !fl->grp.member())
         return set_error(SKB_ERR_INVALID, "skb_flow_group_set_solo: not a group member");
-    fl->grp.dry = solo != 0;
+    fl->grp.set_solo(solo != 0);
     return SKB_OK;
 }
 
 int skb_flow_group_error(skb_flow *fl, int *missing_peer) {
     if (!fl || !missing_peer)
         return set_error(SKB_ERR_INVALID, "skb_flow_group_error: NULL");
-    *missing_peer = -1;
-    if (!fl->grp.window)
-        return SKB_OK;
-    unsigned long long w = 0;
     CUDA_TRY(cudaSetDevice(fl->dev));
-    CUDA_TRY(cudaMemcpy(&w, (char *)fl->grp.window.get() + fl->grp.off_flags + (size_t)kGroupPhases * kMaxGroup * 8, 8,
-                        cudaMemcpyDeviceToHost));
-    if (w)
-        *missing_peer = (int)(w - 1);
-    return SKB_OK;
+    return fl->grp.missing_peer(missing_peer);
 }
 
 int skb_flow_set_cross(skb_flow *fl, int mode) {
@@ -1674,7 +1527,7 @@ static int apply_matvec_impl(skb_flow *fl, skb_dense *dn, const double *x_fibers
     if (n_all == 0)
         return SKB_OK;
     SKB_TRY(prepare_matvec_targets(fl));
-    if (fl->n_win != n_all || fl->grp.size > 1)
+    if (fl->n_win != n_all || fl->grp.member())
         return set_error(SKB_ERR_INVALID, "skb_flow_apply_matvec needs the full target window (have %lld of %lld "
                                           "rows); group members use skb_flow_apply_matvec_device / skb_mflow_*",
                          fl->n_win, n_all);
@@ -1748,9 +1601,9 @@ int skb_flow_apply_matvec_device(skb_flow *fl, skb_dense *dn, const double *d_x_
         (fl->n_body > 0 && !d_body_densities) || (n_bw > 0 && !d_v_bodies) ||
         (fl->n_bodies > 0 && (!d_body_forces || !d_body_torques)))
         return set_error(SKB_ERR_INVALID, "skb_flow_apply_matvec_device: NULL argument for a non-empty class");
-    if (fl->grp.size == 1 && fl->n_win == 0)
+    if (!fl->grp.member() && fl->n_win == 0)
         return SKB_OK;
-    if (fl->grp.size == 1 && fl->n_win != fl->n_fib + fl->n_shell + fl->n_body)
+    if (!fl->grp.member() && fl->n_win != fl->n_fib + fl->n_shell + fl->n_body)
         return set_error(SKB_ERR_INVALID, "skb_flow_apply_matvec_device: a flow that owns only part of the rows must be a "
                                           "group member (skb_flow_group_init): the fiber forces of the other rows' "
                                           "fibers have to come from somewhere");

@@ -307,7 +307,7 @@ def test_rank_apply_matvec_sequencing_and_collectives(tmp_path, world):
     assert np.array_equal(np.concatenate([p["v_b"] for p in parts]), ref_v[nf + ns:])
 
 
-# ---- the peer-memory group protocol (group_kernels.cuh / matvec_core_group), emulated on CPU with gloo ----------------
+# ---- the peer-memory group protocol (skb_group.cu / matvec_core), emulated on CPU with gloo ---------------------------
 def _group_worker(rank, world, port, n_fibers, n_shell, block, out_dir):
     """One group member: push (all-gather of the own strengths), partial fiber velocities from the member's serpentine
     block rows of the symmetric fiber-fiber interaction (both directions of every block pair + own diagonal blocks),
