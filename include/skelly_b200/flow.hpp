@@ -238,6 +238,38 @@ template <class M> class FlowEngineT {
               "skb_flow_apply_matvec_dense");
         return res;
     }
+    // ---- the whole solution vector [fibers | shell | bodies] with the bodies on the device (one GPU) ----
+    /// Once per timestep after set_bodies, per body in the order of the solution vector: n_nodes, node_weights_ (N_b),
+    /// ex_ / ey_ / ez_ (3 x N_b each, body_spherical.cpp:168-181) and A_inv = the column-major (3n+6)^2 inverses of A_,
+    /// concatenated (empty: the system preconditioner refuses bodies)
+    void set_body_operators(const std::vector<int> &n_nodes, const std::vector<double> &node_weights, const M &ex,
+                            const M &ey, const M &ez, const std::vector<double> &A_inv) {
+        check(skb_flow_set_body_operators(st_->fl, n_nodes.data(), (int)n_nodes.size(), node_weights.data(), ex.data(),
+                                          ey.data(), ez.data(), A_inv.empty() ? nullptr : A_inv.data()),
+              "skb_flow_set_body_operators");
+    }
+    /// Once per timestep after set_fibers / set_bodies, per fiber: body index (binding_site_.first, -1 = free), lab-frame
+    /// nucleation site (3 x n_fibers), bending_rigidity_; an empty `body`: no fiber is bound
+    void set_fiber_links(const std::vector<int> &body, const M &site, const std::vector<double> &bending_rigidity) {
+        if (!body.empty() && (body.size() != st_->n_nodes.size() || bending_rigidity.size() != body.size()))
+            throw std::runtime_error("skelly_b200: set_fiber_links needs one entry per fiber of set_fibers");
+        check(skb_flow_set_fiber_links(st_->fl, body.empty() ? nullptr : body.data(), site.data(),
+                                       bending_rigidity.data()),
+              "skb_flow_set_fiber_links");
+    }
+    /// System::apply_matvec (system.cpp:269-324) on the whole solution vector; dn holds stresslet_plus_complementary_
+    M apply_system_matvec(skb_dense *dn, const M &x, double eta) const {
+        M res = M::Zero(x.size(), 1);
+        check(skb_flow_apply_system_matvec(st_->fl, dn, x.data(), eta, res.data()), "skb_flow_apply_system_matvec");
+        return res;
+    }
+    /// System::apply_preconditioner (system.cpp:248-262) on the whole solution vector; dn holds M_inv_
+    M apply_system_preconditioner(skb_dense *dn, const M &x) const {
+        M y = M::Zero(x.size(), 1);
+        check(skb_flow_apply_system_preconditioner(st_->fl, dn, x.data(), y.data()),
+              "skb_flow_apply_system_preconditioner");
+        return y;
+    }
     // ---- switches of the matvec (all optional; defaults are the fast paths with the reference's semantics) ----
     /// fibers <-> periphery pairs in one geometry pass: -1 auto (default), 0 never, 1 whenever applicable
     void set_cross(int mode) { check(skb_flow_set_cross(st_->fl, mode), "skb_flow_set_cross"); }

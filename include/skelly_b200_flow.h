@@ -305,6 +305,63 @@ SKB_API int skb_flow_apply_matvec_device(skb_flow *fl, struct skb_dense *dn, con
                                          const double *d_fiber_link_conditions, double eta, double *d_res_fibers,
                                          double *d_out_shell, double *d_v_bodies, void *stream);
 
+/* ---- the whole solution vector: the body block and the fiber-body links on the device ------------------------
+ * System::apply_matvec (system.cpp:269-324) and System::apply_preconditioner (system.cpp:248-262) on the reference's
+ * whole solution vector [fibers | shell | bodies] (get_solution_maps, system.cpp:69-92): x_fibers 4 per fiber node
+ * ([x; y; z; T] per fiber), x_shell 3 per periphery node, x_bodies (3 n_b + 6) per body ([densities (3 x n_b) ; U ;
+ * omega], body_spherical.cpp:42-43).  What a caller computed on the host per GMRES iteration before --
+ * BodyContainer::calculate_link_conditions (body_container.cpp:171-267), ::matvec (:487-504 -> body_spherical.cpp:39-63)
+ * and ::apply_preconditioner (:510-521) -- runs on the device: this is A_fiber_hydro::apply / P_inv_hydro::apply
+ * (solver_hydro.cpp:23-48) on a whole vector.  Spherical and ellipsoidal bodies have the same matvec and
+ * preconditioner (body_ellipsoidal.cpp:37-63), so no body type is passed; deformable bodies do not exist here (the
+ * reference throws for them, body_container.cpp:453).  K_ is never uploaded: K U = u + omega x (x_i - c) and
+ * K^T lambda = [sum lambda_i ; sum (x_i - c) x lambda_i] follow from the node positions and centres of
+ * skb_flow_set_bodies (body_spherical.cpp:74-86).
+ *
+ * Bodies are in ONE order, that of skb_flow_set_bodies, which must be the order of the bodies in the solution vector
+ * (the reference's flow orders them spherical..., ellipsoidal..., body_container.cpp:278-290, the solution vector and
+ * the link forces by `bodies`, :532-546; a caller with both kinds passes them to skb_flow_set_bodies in `bodies`
+ * order).  Each bound fiber reads its own slice of x_fibers and writes its own column of the link conditions: the
+ * reference's loop skips `i_fib++` and `xt_offset += 4 n` for a free fiber (:202-204, 262-263), which agrees with this
+ * whenever the bound fibers precede the free ones.
+ *
+ * skb_flow_set_body_operators: once per timestep, after skb_flow_set_bodies (which drops them).  n_nodes[b] per body
+ *   (summing to the node count of skb_flow_set_bodies, same order), node_weights (N_b, node_weights_), ex / ey / ez
+ *   (3 x N_b each, AoS like the positions: ex_, ey_, ez_ of update_singularity_subtraction_vecs, body_spherical.cpp:
+ *   168-181), A_inv: per body the column-major (3 n_b + 6)^2 inverse of A_ (update_preconditioner, :104-126),
+ *   concatenated, or NULL (then the system preconditioner refuses bodies).  Refused: node counts that do not sum to
+ *   skb_flow_set_bodies' count, a node weight <= 0, n_bodies other than skb_flow_set_bodies', a body too large for the
+ *   preconditioner's GEMV (3 n_b + 6 > ~25000).
+ * skb_flow_set_fiber_links: once per timestep, after skb_flow_set_fibers / _bodies / _fiber_class (each drops the links).
+ *   Per fiber of the flow: body[f] (binding_site_.first, -1 = free), site (3 x n_fibers, the lab-frame nucleation site
+ *   get_nucleation_site, unused for a free fiber), bending_rigidity[f] (bending_rigidity_; the table carries its own, so
+ *   the links work whether the fiber operators were uploaded or built).  body == NULL: no fiber is bound.  Refused: a
+ *   body index outside [-1, n_bodies), a bound fiber whose node count lacks skb_flow_set_fiber_class_derivatives (the
+ *   link needs D_2_0 and D_3_0), a nucleation site at the body centre (site_pos.normalized(), :256, would divide by 0).
+ *   xs_.col(0) comes from the resident fiber operators and length_ from skb_flow_set_fibers at every apply.
+ *
+ * skb_flow_apply_system_matvec(_device): res = A x, both of size 4 N_f + 3 N_s + sum(3 n_b + 6); dn holds
+ *   SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY (3 N_s x 3 N_s, on the flow's device; may be NULL only if N_s == 0).
+ * skb_flow_apply_system_preconditioner(_device): y = P^-1 x -- the fibers' A_^-1 (skb_flow_set_fiber_preconditioner or
+ *   the build), the periphery's M_inv (dn holds SKB_DENSE_M_INV), the bodies' A_^-1 (a GEMV over the explicit inverse,
+ *   like the fibers').
+ * The host forms ship x once and res / y once; the _device forms are asynchronous on `stream`.  All four refuse
+ * (SKB_ERR_INVALID, before any launch, earlier state untouched): a group member or a flow whose target window / ranges
+ * do not cover every row (multi-GPU is not supported: a body's K^T lambda needs all of its nodes, and the reference
+ * keeps the bodies on rank 0), fiber operators not resident (with their inverse for the preconditioner), bodies without
+ * skb_flow_set_body_operators, fibers and bodies without skb_flow_set_fiber_links (matvec), no A_inv (preconditioner),
+ * dn == NULL or of the wrong shape with periphery nodes present.  The results are bitwise reproducible run to run: the
+ * bodies' link forces are added per body in container order, without atomics. */
+SKB_API int skb_flow_set_body_operators(skb_flow *fl, const int *n_nodes, int n_bodies, const double *node_weights,
+                                        const double *ex, const double *ey, const double *ez, const double *A_inv);
+SKB_API int skb_flow_set_fiber_links(skb_flow *fl, const int *body, const double *site, const double *bending_rigidity);
+SKB_API int skb_flow_apply_system_matvec(skb_flow *fl, struct skb_dense *dn, const double *x, double eta, double *res);
+SKB_API int skb_flow_apply_system_matvec_device(skb_flow *fl, struct skb_dense *dn, const double *d_x, double eta,
+                                                double *d_res, void *stream);
+SKB_API int skb_flow_apply_system_preconditioner(skb_flow *fl, struct skb_dense *dn, const double *x, double *y);
+SKB_API int skb_flow_apply_system_preconditioner_device(skb_flow *fl, struct skb_dense *dn, const double *d_x,
+                                                        double *d_y, void *stream);
+
 typedef struct skb_flow_stats {
     double device_ms;   /* CUDA-event time of the last call, first launch to last kernel (copies excluded) */
     double total_ms;    /* including H2D / D2H */

@@ -192,6 +192,12 @@ def library() -> C.CDLL:
         "skb_dense_apply": ([ctxp, C.c_int, _dp, _dp, _dp], C.c_int),
         "skb_dense_last_stats": ([ctxp, C.POINTER(DenseStats)], C.c_int),
         "skb_flow_matvec_device": ([ctxp] + [C.c_void_p] * 5 + [C.c_double, C.c_void_p, C.c_void_p], C.c_int),
+        "skb_flow_set_body_operators": ([ctxp, C.POINTER(C.c_int), C.c_int, _dp, _dp, _dp, _dp, _dp], C.c_int),
+        "skb_flow_set_fiber_links": ([ctxp, C.POINTER(C.c_int), _dp, _dp], C.c_int),
+        "skb_flow_apply_system_matvec": ([ctxp, ctxp, _dp, C.c_double, _dp], C.c_int),
+        "skb_flow_apply_system_matvec_device": ([ctxp, ctxp, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p], C.c_int),
+        "skb_flow_apply_system_preconditioner": ([ctxp, ctxp, _dp, _dp], C.c_int),
+        "skb_flow_apply_system_preconditioner_device": ([ctxp, ctxp, C.c_void_p, C.c_void_p, C.c_void_p], C.c_int),
     }
     global BOUND_FUNCTIONS
     BOUND_FUNCTIONS = tuple(sorted(sig))
@@ -785,6 +791,62 @@ class Flow:
                                                       vp(d_x_shell), vp(d_body_densities), vp(d_body_forces),
                                                       vp(d_body_torques), vp(d_fiber_link_conditions), float(eta),
                                                       vp(d_res_fibers), vp(d_out_shell), vp(d_v_bodies), vp(stream)))
+
+    # ---- the whole solution vector [fibers | shell | bodies] with the bodies on the device ----
+    def set_body_operators(self, n_nodes, node_weights, ex, ey, ez, A_inv_list=None):
+        """Per body (order of set_bodies = order in the solution vector): node count, node_weights_ (N_b,), ex_ / ey_ /
+        ez_ (N_b, 3) each, and A_^-1 ((3n+6, 3n+6) per body, a list) or None (no system preconditioner for bodies)."""
+        n = np.ascontiguousarray(n_nodes, dtype=np.int32)
+        w = np.ascontiguousarray(node_weights, dtype=np.float64).reshape(-1)
+        ex, ey, ez = _arr(ex, 3), _arr(ey, 3), _arr(ez, 3)
+        Ai = None if A_inv_list is None else self._colmajor_concat(A_inv_list)
+        _check(library().skb_flow_set_body_operators(self._h, n.ctypes.data_as(C.POINTER(C.c_int)), int(n.shape[0]),
+                                                     _p(w), _p(ex), _p(ey), _p(ez), None if Ai is None else _p(Ai)))
+        self._body_sol = int(np.sum(3 * n + 6))
+
+    def set_fiber_links(self, body=None, site=None, bending_rigidity=None):
+        """Per fiber: body index (-1 free), lab-frame nucleation site (n_fibers, 3), bending_rigidity_; body=None: no
+        fiber is bound."""
+        if body is None:
+            _check(library().skb_flow_set_fiber_links(self._h, None, None, None))
+            return
+        b = np.ascontiguousarray(body, dtype=np.int32)
+        st = _arr(site, 3)
+        E = np.ascontiguousarray(np.broadcast_to(np.asarray(bending_rigidity, dtype=np.float64), b.shape))
+        assert st.shape[0] == b.shape[0]
+        _check(library().skb_flow_set_fiber_links(self._h, b.ctypes.data_as(C.POINTER(C.c_int)), _p(st), _p(E)))
+
+    def solution_size(self) -> int:
+        """4 N_f + 3 N_s + sum(3 n_b + 6) (the bodies' part as set_body_operators was last given)"""
+        return 4 * self.n_fib + 3 * self.n_shell + (getattr(self, "_body_sol", 0) if self.n_bodies else 0)
+
+    def apply_system_matvec(self, x, eta, dense=None):
+        """System::apply_matvec (system.cpp:269-324) on the whole solution vector x: returns res = A x."""
+        x = np.ascontiguousarray(x, dtype=np.float64).reshape(-1)
+        assert x.shape[0] == self.solution_size()
+        res = np.empty_like(x)
+        _check(library().skb_flow_apply_system_matvec(self._h, dense._h if dense is not None else None, _p(x),
+                                                      float(eta), _p(res)))
+        return res
+
+    def apply_system_matvec_device(self, dense, d_x: int, eta: float, d_res: int, stream: int = 0):
+        _check(library().skb_flow_apply_system_matvec_device(self._h, dense._h if dense is not None else None,
+                                                             C.c_void_p(d_x), float(eta), C.c_void_p(d_res),
+                                                             C.c_void_p(stream)))
+
+    def apply_system_preconditioner(self, x, dense=None):
+        """System::apply_preconditioner (system.cpp:248-262) on the whole solution vector x: returns y = P^-1 x."""
+        x = np.ascontiguousarray(x, dtype=np.float64).reshape(-1)
+        assert x.shape[0] == self.solution_size()
+        y = np.empty_like(x)
+        _check(library().skb_flow_apply_system_preconditioner(self._h, dense._h if dense is not None else None, _p(x),
+                                                              _p(y)))
+        return y
+
+    def apply_system_preconditioner_device(self, dense, d_x: int, d_y: int, stream: int = 0):
+        _check(library().skb_flow_apply_system_preconditioner_device(self._h, dense._h if dense is not None else None,
+                                                                     C.c_void_p(d_x), C.c_void_p(d_y),
+                                                                     C.c_void_p(stream)))
 
     # ---- multi-GPU groups (peer memory) ----
     def last_sym_kernel(self):

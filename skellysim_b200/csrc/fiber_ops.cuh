@@ -21,6 +21,7 @@ namespace skb {
 constexpr int kFiberGemvRows = 32;   // rows per CTA
 constexpr int kFiberGemvSlices = 8;  // column slices per row
 constexpr int kFiberGemvThreads = kFiberGemvRows * kFiberGemvSlices;
+constexpr size_t kFiberGemvSmemMax = 200 * 1024; // dynamic shared memory the kernels are allowed (prepare_fiber_kernels)
 
 struct FiberGemvItem {
     long long mat_off; // element offset of M_f in the concatenated operator buffer

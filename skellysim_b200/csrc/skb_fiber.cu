@@ -14,7 +14,7 @@
 using namespace skb;
 
 // fiber_gemv_kernel's dynamic shared memory: the plan refuses more, prepare_fiber_kernels allows this much
-static constexpr size_t kGemvSmemMax = 200 * 1024;
+static constexpr size_t kGemvSmemMax = kFiberGemvSmemMax;
 
 // Where the operators of the own fibers live (GEMV items, offsets into A_, force_operator_ and the class table) and a
 // build's tables: per fiber, per assembly CTA (a tile of columns), per inverse launch (node count)
@@ -122,6 +122,12 @@ int FiberOps::check_class(int f, int n, bool derivatives) const {
     if (derivatives && it->second.D234.empty())
         return set_error(SKB_ERR_INVALID, "fiber %d has %d nodes but skb_flow_set_fiber_class_derivatives(%d, ...) "
                                           "was never called", f, n, n);
+    return SKB_OK;
+}
+
+int FiberOps::derivative_offset(int f, int n, long long *off) const {
+    SKB_TRY(check_class(f, n, true));
+    *off = class_off.at(n).first + (long long)n * n + (4LL * n - 14) * 4 * n; // past D_1_0 and P_downsample_bc
     return SKB_OK;
 }
 
@@ -407,6 +413,17 @@ int FiberOps::precondition(const double *d_x, double *d_y, cudaStream_t st, int 
         return SKB_OK;
     fiber_gemv_kernel<0><<<n_items_A, kFiberGemvThreads, gemv_smem, st>>>(
         (const FiberGemvItem *)items_A.ptr, (const double *)op_Ainv.ptr, d_x, d_y, FiberVelArgs{});
+    return launched(launches);
+}
+
+int skb::launch_gemv(const FiberGemvItem *d_items, int n_items, const double *mats, const double *x, double *y,
+                     size_t smem, cudaStream_t st, int *launches) {
+    if (n_items == 0)
+        return SKB_OK;
+    if (smem > kGemvSmemMax)
+        return set_error(SKB_ERR_INVALID, "a GEMV of %zu bytes of shared memory exceeds the limit of %zu", smem,
+                         kGemvSmemMax);
+    fiber_gemv_kernel<0><<<n_items, kFiberGemvThreads, smem, st>>>(d_items, mats, x, y, FiberVelArgs{});
     return launched(launches);
 }
 

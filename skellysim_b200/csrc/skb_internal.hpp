@@ -190,6 +190,12 @@ class FiberOps {
     bool empty() const { return n_items_A == 0; }
     int n_fibers() const { return f1 - f0; }
     void invalidate() { ready_ = false; }
+    // what the fiber-body links read (BodyOps): the element offset of D_2_0 of fiber f's class (n nodes) in the class
+    // table, D_3_0 following -- an error unless skb_flow_set_fiber_class_derivatives(n) was called; offsets move when
+    // set_class adds a node count.  The table and the resident tangents xs_ (3 per own node) on the device
+    int derivative_offset(int f, int n, long long *off) const;
+    const double *class_table() const { return (const double *)class_mats.ptr; }
+    const double *tangents() const { return (const double *)op_xs.ptr; }
 
   private:
     struct Plan;
@@ -224,6 +230,58 @@ class FiberOps {
     DevBuf rhs_items, rhs_params, rhs_growth;
     Event rhs_done;
     bool rhs_pending = false;
+};
+
+struct FiberGemvItem; // fiber_ops.cuh
+// y = M x per item with fiber_gemv_kernel<0> (launched from skb_fiber.cu, which sets its shared-memory limit), adding
+// one launch to *launches; smem = fiber_gemv_kernel's dynamic shared memory for the widest item
+int launch_gemv(const FiberGemvItem *d_items, int n_items, const double *mats, const double *x, double *y, size_t smem,
+                cudaStream_t st, int *launches);
+
+// ---- the bodies' per-timestep operators and the fiber-body links of a single-device flow (skb_body.cu) ----
+// The body block of System::apply_matvec / ::apply_preconditioner (BodyContainer::matvec / ::apply_preconditioner,
+// body_container.cpp:487-521) and BodyContainer::calculate_link_conditions (:171-267), on the device.  Bodies are in
+// the order of skb_flow_set_bodies, which is the order of the solution vector.  The caller has checked its pointers
+// for NULL and made the flow's device current; every step runs on the stream it passes.
+class BodyOps {
+  public:
+    // per body: n_nodes (summing to n_body_nodes), node_weights_, ex_ / ey_ / ez_ (3 per node), A_^-1 (column-major
+    // (3n+6)^2, concatenated; may be NULL); r_body / centers: the flow's geometry (host).  Checked first: a refusal
+    // leaves the earlier operators
+    int set_operators(const int *n_nodes, int n_bodies, long long n_body_nodes, const double *r_body,
+                      const double *centers, const double *node_weights, const double *ex, const double *ey,
+                      const double *ez, const double *A_inv, cudaStream_t st);
+    // per fiber of `own` (all fibers of the flow): body index (-1 free; body == NULL: none bound), lab-frame nucleation
+    // site, bending_rigidity_.  Checked first: a refusal leaves the earlier links
+    int set_links(const OwnFibers &own, const FiberOps &ops, int n_bodies, const double *centers, const int *body,
+                  const double *site, const double *rigidity, cudaStream_t st);
+    void drop_operators() { ops_set_ = false; }
+    void drop_links() { links_set_ = false; }
+    bool has_operators() const { return ops_set_; }
+    bool has_inverse() const { return ops_set_ && inv_set_; }
+    bool has_links() const { return links_set_; }
+    long long solution_size() const { return sol_size_; }
+
+    // one matvec: the link conditions (*d_link: 7 per fiber, NULL when no fiber is bound), the bodies' link forces /
+    // torques and their densities gathered from x_bodies (forces(), torques(), densities()).  length: length_ per fiber
+    int links(const FiberOps &ops, const double *d_length, const double *d_x_fib, const double *d_x_bodies,
+              const double **d_link, cudaStream_t st, int *launches);
+    const double *densities() const { return (const double *)dens_.ptr; }
+    const double *forces() const { return (const double *)force_.ptr; }
+    const double *torques() const { return (const double *)torque_.ptr; }
+    // res_bodies = bc.matvec(v_bodies, x_bodies); y = A_^-1 x per body
+    int matvec(const double *d_x_bodies, const double *d_v_bodies, double *d_res, cudaStream_t st,
+               int *launches) const;
+    int precondition(const double *d_x, double *d_y, cudaStream_t st, int *launches) const;
+
+  private:
+    bool ops_set_ = false, inv_set_ = false, links_set_ = false, any_bound_ = false;
+    int n_bodies_ = 0, n_fibers_ = 0, n_gemv_ = 0;
+    long long sol_size_ = 0;
+    size_t gemv_smem_ = 0;
+    DevBuf items_, r_, centers_, weights_, ex_, ey_, ez_, a_inv_, gemv_items_; // set_operators
+    DevBuf link_fibers_, csr_begin_, csr_fib_, link_, contrib_;                 // set_links
+    DevBuf dens_, force_, torque_;                                              // per matvec
 };
 
 // ---- one member of a multi-GPU group of flows (DESIGN.md §4; skb_group.cu, group_kernels.cuh) ----

@@ -92,6 +92,8 @@ struct skb_flow {
     std::vector<int> h_fiber_n;         // nodes of every fiber
     std::vector<long long> h_fiber_off; // first node of every fiber (n_fibers + 1)
     FiberOps ops; // per-fiber dense operators of the fibers whose rows are in the target list (skb_fiber.cu)
+    BodyOps bodies; // the bodies' operators and the fiber-body links of the whole-vector operator (skb_body.cu)
+    std::vector<double> h_centers; // body centres (set_fiber_links measures the nucleation sites from them)
     Group grp; // multi-GPU group membership: one member per GPU, exchange through peer memory (skb_group.cu)
     // Periphery::matvec's dense operator beside the pair kernels (stream_kernels.cuh): forked onto bg_stream once its
     // input (the complete x_shell) is there, joined before res_shell is assembled
@@ -106,6 +108,7 @@ struct skb_flow {
     DevBuf scratch_u; // group mode: landing zone of eval_on_device's default output (never read)
     // staging
     DevBuf in_fib, in_shell, in_body, in_force, in_torque, vel, tmp, x_fib, res_fib, vb, res_shell, tmp_b;
+    DevBuf sys_x, sys_y; // the whole solution vector in and out of the host forms of the system operator
     skb_flow_stats stats{};
     int launches = 0;
     long long pairs = 0;
@@ -474,6 +477,7 @@ int skb_flow_set_fibers(skb_flow *fl, const double *r_fib, const int *n_nodes, c
     fl->h_fiber_n.assign(n_nodes, n_nodes + n_fibers);
     fl->h_fiber_off = off;
     fl->ops.invalidate(); // operators belong to one set of fibers
+    fl->bodies.drop_links(); // ... and so do the links
     fl->mv_dirty = true;
     fl->geom_version++;
     CUDA_TRY(cudaSetDevice(fl->dev));
@@ -526,6 +530,9 @@ int skb_flow_set_bodies(skb_flow *fl, const double *node_pos, const double *node
     fl->n_body = n_nodes;
     fl->n_bodies = n_bodies;
     fl->h_r_body.assign(node_pos, node_pos + 3 * n_nodes);
+    fl->h_centers.assign(centers, centers + 3 * (size_t)n_bodies);
+    fl->bodies.drop_operators(); // the bodies' operators and the nucleation sites belong to one placement
+    fl->bodies.drop_links();
     fl->mv_dirty = true;
     fl->geom_version++;
     for (int k = 0; k < 2; ++k) {
@@ -1234,6 +1241,7 @@ int skb_flow_set_fiber_class(skb_flow *fl, int n_nodes, const double *D_1_0, con
     if (!fl || !D_1_0 || !P_downsample_bc)
         return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_class: NULL argument");
     CUDA_TRY(cudaSetDevice(fl->dev));
+    fl->bodies.drop_links(); // a new node count moves the class table's offsets the links hold
     return fl->ops.set_class(n_nodes, D_1_0, P_downsample_bc, fl->stream);
 }
 
@@ -1624,6 +1632,185 @@ int skb_flow_last_stats(const skb_flow *fl, skb_flow_stats *out) {
         return set_error(SKB_ERR_INVALID, "skb_flow_last_stats: NULL");
     *out = fl->stats;
     return SKB_OK;
+}
+
+} // extern "C"
+
+// ---- the whole-vector operator and preconditioner with the bodies on the device (skb_body.cu) -------------------
+// The solution vector is [fibers (4 per node) | shell (3 per node) | bodies (3 n_b + 6 each)] (get_solution_maps,
+// system.cpp:69-92); single device, whole target list.
+
+extern "C" {
+
+int skb_flow_set_body_operators(skb_flow *fl, const int *n_nodes, int n_bodies, const double *node_weights,
+                                const double *ex, const double *ey, const double *ez, const double *A_inv) {
+    const char *who = "skb_flow_set_body_operators";
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    if (fl->grp.member())
+        return set_error(SKB_ERR_INVALID, "%s: the body block runs on a single device, not in a group", who);
+    if (n_bodies != fl->n_bodies)
+        return set_error(SKB_ERR_INVALID, "%s: %d bodies, skb_flow_set_bodies has %d", who, n_bodies, fl->n_bodies);
+    if (n_bodies > 0 && (!n_nodes || !node_weights || !ex || !ey || !ez))
+        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    return fl->bodies.set_operators(n_nodes, n_bodies, fl->n_body, fl->h_r_body.data(), fl->h_centers.data(),
+                                    node_weights, ex, ey, ez, A_inv, fl->stream);
+}
+
+int skb_flow_set_fiber_links(skb_flow *fl, const int *body, const double *site, const double *bending_rigidity) {
+    const char *who = "skb_flow_set_fiber_links";
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    if (fl->grp.member())
+        return set_error(SKB_ERR_INVALID, "%s: the body block runs on a single device, not in a group", who);
+    if (body && fl->n_fibers > 0 && (!site || !bending_rigidity))
+        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    const OwnFibers all{0, fl->n_fibers, fl->h_fiber_n.data(), fl->h_fiber_off.data(), (const double *)fl->r_fib.ptr,
+                        (const double *)fl->fiber_length.ptr, fl->stream};
+    return fl->bodies.set_links(all, fl->ops, fl->n_bodies, fl->h_centers.data(), body, site, bending_rigidity,
+                                fl->stream);
+}
+
+} // extern "C"
+
+// The checks of the system operator (matvec: stresslet_plus_complementary in dn; precondition: M_inv and the
+// inverses), all before any launch; then the flow's device is current and its target list resolved.
+static int system_args(skb_flow *fl, skb_dense *dn, const char *who, bool precondition, bool args) {
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    if (fl->grp.member())
+        return set_error(SKB_ERR_INVALID, "%s: multi-GPU is not supported: a body's K^T lambda needs all of its nodes "
+                                          "(the reference keeps the bodies on rank 0); use a single-device flow", who);
+    SKB_TRY(fl->ops.ready(who, precondition));
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    SKB_TRY(prepare_matvec_targets(fl));
+    const long long n_all = fl->n_fib + fl->n_shell + fl->n_body;
+    if (fl->n_win != n_all)
+        return set_error(SKB_ERR_INVALID, "%s: needs the whole target list (%lld of %lld rows are set by a target window "
+                                          "or ranges); multi-GPU is not supported", who, fl->n_win, n_all);
+    if (fl->n_shell > 0) {
+        if (!dn)
+            return set_error(SKB_ERR_INVALID, "%s: the periphery needs its dense operator (dn == NULL)", who);
+        const int op = precondition ? SKB_DENSE_M_INV : SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY;
+        int dn_dev = -1;
+        int64_t rows = 0, cols = 0;
+        SKB_TRY(skb_dense_device(dn, 0, &dn_dev));
+        SKB_TRY(skb_dense_shape(dn, op, &rows, &cols));
+        if (dn_dev != fl->dev || rows != 3 * fl->n_shell || cols != 3 * fl->n_shell)
+            return set_error(SKB_ERR_INVALID, "%s: the dense handle holds a %lld x %lld %s on device %d, need %lld x %lld "
+                                              "on device %d", who, (long long)rows, (long long)cols,
+                             precondition ? "M_inv" : "stresslet_plus_complementary", dn_dev, 3 * fl->n_shell,
+                             3 * fl->n_shell, fl->dev);
+    }
+    if (fl->n_bodies > 0) {
+        if (!fl->bodies.has_operators())
+            return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_body_operators after skb_flow_set_bodies", who);
+        if (precondition && !fl->bodies.has_inverse())
+            return set_error(SKB_ERR_INVALID, "%s: skb_flow_set_body_operators was given no A_inv", who);
+        if (!precondition && fl->n_fibers > 0 && !fl->bodies.has_links())
+            return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_fiber_links after skb_flow_set_fibers / "
+                                              "skb_flow_set_bodies (NULL body: no fiber is bound)", who);
+    }
+    if (!args)
+        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
+    begin_stats(fl);
+    return SKB_OK;
+}
+
+static long long solution_size(const skb_flow *fl) {
+    return 4 * fl->n_fib + 3 * fl->n_shell + (fl->n_bodies > 0 ? fl->bodies.solution_size() : 0);
+}
+
+// System::apply_matvec (system.cpp:269-324) on fl->cur: the links, forces / torques and densities of the bodies from
+// x, then apply_matvec_core unchanged, then bc.matvec on its v_bodies rows
+static int system_matvec_core(skb_flow *fl, skb_dense *dn, const double *d_x, double eta, double *d_res) {
+    const long long nf = fl->n_fib, ns = fl->n_shell;
+    const double *x_fib = d_x, *x_shell = d_x + 4 * nf, *x_bodies = x_shell + 3 * ns;
+    double *res_fib = d_res, *res_shell = d_res + 4 * nf, *res_bodies = res_shell + 3 * ns;
+    const double *link = nullptr, *bd = nullptr, *f = nullptr, *t = nullptr;
+    if (fl->n_bodies > 0) { // fc.calculate_link_conditions (system.cpp:311), the densities out of x_bodies
+        SKB_TRY(fl->bodies.links(fl->ops, (const double *)fl->fiber_length.ptr, x_fib, x_bodies, &link, fl->cur,
+                                 &fl->launches));
+        bd = fl->bodies.densities();
+        f = fl->bodies.forces();
+        t = fl->bodies.torques();
+    }
+    SKB_TRY(fl->tmp_b.ensure((size_t)fl->n_body * 24 + 8));
+    double *v_bodies = (double *)fl->tmp_b.ptr;
+    SKB_TRY(apply_matvec_core(fl, dn, x_fib, x_shell, bd, f, t, link, eta, res_fib, res_shell, v_bodies));
+    // res_bodies = bc.matvec(v_bodies, x_bodies)                          system.cpp:320
+    return fl->n_bodies > 0 ? fl->bodies.matvec(x_bodies, v_bodies, res_bodies, fl->cur, &fl->launches) : SKB_OK;
+}
+
+// System::apply_preconditioner (system.cpp:248-262) on fl->cur
+static int system_precondition_core(skb_flow *fl, skb_dense *dn, const double *d_x, double *d_y) {
+    const long long nf = fl->n_fib, ns = fl->n_shell;
+    SKB_TRY(fl->ops.precondition(d_x, d_y, fl->cur, &fl->launches));
+    if (ns > 0) {
+        SKB_TRY(skb_dense_apply_device(dn, SKB_DENSE_M_INV, d_x + 4 * nf, nullptr, d_y + 4 * nf, fl->cur));
+        fl->launches += 1;
+    }
+    return fl->n_bodies > 0
+               ? fl->bodies.precondition(d_x + 4 * nf + 3 * ns, d_y + 4 * nf + 3 * ns, fl->cur, &fl->launches)
+               : SKB_OK;
+}
+
+extern "C" {
+
+int skb_flow_apply_system_matvec(skb_flow *fl, skb_dense *dn, const double *x, double eta, double *res) {
+    const char *who = "skb_flow_apply_system_matvec";
+    SKB_TRY(system_args(fl, dn, who, false, (x && res) || solution_size(fl) == 0));
+    if (!(eta > 0))
+        return set_error(SKB_ERR_INVALID, "%s: eta = %g", who, eta);
+    const size_t n = (size_t)solution_size(fl);
+    if (n == 0)
+        return SKB_OK;
+    SKB_TRY(fl->sys_x.ensure(n * 8));
+    SKB_TRY(fl->sys_y.ensure(n * 8));
+    return host_frame(
+        fl, [&] { return upload(fl, fl->sys_x, x, n); },
+        [&] { return system_matvec_core(fl, dn, (const double *)fl->sys_x.ptr, eta, (double *)fl->sys_y.ptr); },
+        [&] { return download(fl, res, fl->sys_y, n); });
+}
+
+int skb_flow_apply_system_matvec_device(skb_flow *fl, skb_dense *dn, const double *d_x, double eta, double *d_res,
+                                        void *stream) {
+    const char *who = "skb_flow_apply_system_matvec_device";
+    SKB_TRY(system_args(fl, dn, who, false, (d_x && d_res) || solution_size(fl) == 0));
+    if (!(eta > 0))
+        return set_error(SKB_ERR_INVALID, "%s: eta = %g", who, eta);
+    if (solution_size(fl) == 0)
+        return SKB_OK;
+    fl->cur = (cudaStream_t)stream;
+    SKB_TRY(system_matvec_core(fl, dn, d_x, eta, d_res));
+    return device_stats(fl);
+}
+
+int skb_flow_apply_system_preconditioner(skb_flow *fl, skb_dense *dn, const double *x, double *y) {
+    const char *who = "skb_flow_apply_system_preconditioner";
+    SKB_TRY(system_args(fl, dn, who, true, (x && y) || solution_size(fl) == 0));
+    const size_t n = (size_t)solution_size(fl);
+    if (n == 0)
+        return SKB_OK;
+    SKB_TRY(fl->sys_x.ensure(n * 8));
+    SKB_TRY(fl->sys_y.ensure(n * 8));
+    return host_frame(
+        fl, [&] { return upload(fl, fl->sys_x, x, n); },
+        [&] { return system_precondition_core(fl, dn, (const double *)fl->sys_x.ptr, (double *)fl->sys_y.ptr); },
+        [&] { return download(fl, y, fl->sys_y, n); });
+}
+
+int skb_flow_apply_system_preconditioner_device(skb_flow *fl, skb_dense *dn, const double *d_x, double *d_y,
+                                                void *stream) {
+    const char *who = "skb_flow_apply_system_preconditioner_device";
+    SKB_TRY(system_args(fl, dn, who, true, (d_x && d_y) || solution_size(fl) == 0));
+    if (solution_size(fl) == 0)
+        return SKB_OK;
+    fl->cur = (cudaStream_t)stream;
+    SKB_TRY(system_precondition_core(fl, dn, d_x, d_y));
+    return device_stats(fl);
 }
 
 } // extern "C"

@@ -11,9 +11,10 @@ One GMRES iteration of the reference is `P_inv_hydro::apply` followed by `A_fibe
 preconditioning, solver_hydro.cpp:79-81).  Both are evaluated here with every vector resident on the device: the fiber
 block of the preconditioner is a batched GEMV over explicit inverses (skb_flow_apply_fiber_preconditioner_device), the
 periphery block a row-block GEMV with M_inv (skb_dense_apply_device), the operator apply is
-skb_flow_apply_matvec_device.  Only the body block -- a few hundred unknowns per body, host glue in the reference too
-(BodyContainer::matvec / apply_preconditioner, body_container.cpp) -- is left to the caller: `apply` hands back the
-velocities at the body nodes and takes the body densities / link forces as (small) device tensors.
+skb_flow_apply_matvec_device.  HydroOperator leaves the body block to the caller: `apply` hands back the velocities at
+the body nodes and takes the body densities / link forces as (small) device tensors.  SystemOperator does not: it
+applies A and P^-1 to whole solution vectors [fibers | shell | bodies] with the body block and the fiber-body links on
+the device as well (skb_flow_apply_system_matvec_device / _preconditioner_device).
 
 This module sequences calls and owns work vectors; it computes nothing itself.  torch is used for device memory only.
 """
@@ -83,3 +84,42 @@ def iterate(op: HydroOperator, x_f, x_s, body_density, body_forces, body_torques
         x_f = r_f / scale
         x_s = r_s / scale
     return x_f, x_s
+
+
+class SystemOperator:
+    """A and P^-1 of the whole mobility system on whole solution vectors [fibers | shell | bodies] (get_solution_maps,
+    system.cpp:69-92) for ONE single-device flow: A_fiber_hydro::apply / P_inv_hydro::apply with nothing left to the
+    caller.  flow: capi.Flow with geometry, fiber operators and preconditioner, body operators and fiber links set;
+    dense: capi.Dense holding stresslet_plus_complementary and M_inv, or None without a periphery."""
+
+    def __init__(self, flow, dense, eta: float, device):
+        import torch
+        self.torch = torch
+        self.flow, self.dense, self.eta = flow, dense, float(eta)
+        self.n = flow.solution_size()
+        kw = dict(dtype=torch.float64, device=device)
+        self.res = torch.zeros(max(self.n, 1), **kw)
+        self.y = torch.zeros(max(self.n, 1), **kw)
+        self.launches = 0
+
+    def _stream(self):
+        return self.torch.cuda.current_stream().cuda_stream
+
+    def apply(self, x):
+        """System::apply_matvec (system.cpp:269-324): A x -- a view valid until the next call."""
+        self.flow.apply_system_matvec_device(self.dense, x.data_ptr(), self.eta, self.res.data_ptr(), self._stream())
+        self.launches = self.flow.stats()["launches"]
+        return self.res[:self.n]
+
+    def apply_preconditioner(self, x):
+        """System::apply_preconditioner (system.cpp:248-262): P^-1 x -- a view valid until the next call."""
+        self.flow.apply_system_preconditioner_device(self.dense, x.data_ptr(), self.y.data_ptr(), self._stream())
+        return self.y[:self.n]
+
+
+def iterate_system(op: SystemOperator, x, n_iter: int):
+    """iterate() for whole solution vectors: `n_iter` times x <- A P^-1 x, rescaled to unit max-norm on the device."""
+    for _ in range(n_iter):
+        r = op.apply(op.apply_preconditioner(x))
+        x = r / r.abs().max()
+    return x
