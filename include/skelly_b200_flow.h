@@ -134,8 +134,10 @@ SKB_API int skb_flow_matvec_device(skb_flow *fl, const double *d_fib_forces, con
  *     skb_mflow_* below, which does all of that;
  *   one process per GPU: skb_flow_group_init, skb_flow_group_export -> exchange the 64-byte handles by any means
  *     (MPI_Allgather, torch.distributed) -> skb_flow_group_import for every peer.
- * skb_flow_group_init must follow the geometry calls (the window is laid out for their node counts; positions may
- * change later, counts may not).  In a group, the *_device entry points take the OWN slices: fiber forces / x_fibers of
+ * skb_flow_group_init must follow the geometry calls (the window is laid out for their fiber and periphery node counts
+ * and for the number of bodies, whose link forces it carries; positions may change later, counts may not: a member
+ * whose counts changed refuses its matvec until the group is initialised again -- skb_mflow does that itself, and then
+ * wants its fiber operators set again).  In a group, the *_device entry points take the OWN slices: fiber forces / x_fibers of
  * the own fibers, periphery density of the own rows; body inputs are complete on every member.  All members must issue
  * the same sequence of matvec calls (like any collective). */
 #define SKB_FLOW_IPC_HANDLE_BYTES 64
@@ -347,8 +349,7 @@ SKB_API int skb_flow_apply_matvec_device(skb_flow *fl, struct skb_dense *dn, con
  *   like the fibers').
  * The host forms ship x once and res / y once; the _device forms are asynchronous on `stream`.  All four refuse
  * (SKB_ERR_INVALID, before any launch, earlier state untouched): a group member or a flow whose target window / ranges
- * do not cover every row (multi-GPU is not supported: a body's K^T lambda needs all of its nodes, and the reference
- * keeps the bodies on rank 0), fiber operators not resident (with their inverse for the preconditioner), bodies without
+ * do not cover every row (over several devices use skb_mflow_set_body_operators and its siblings below), fiber operators not resident (with their inverse for the preconditioner), bodies without
  * skb_flow_set_body_operators, fibers and bodies without skb_flow_set_fiber_links (matvec), no A_inv (preconditioner),
  * dn == NULL or of the wrong shape with periphery nodes present.  The results are bitwise reproducible run to run: the
  * bodies' link forces are added per body in container order, without atomics. */
@@ -422,6 +423,31 @@ SKB_API int skb_mflow_apply_matvec(skb_mflow *mf, const double *x_fibers, const 
                                    const double *body_densities, const double *body_forces_torques,
                                    const double *fiber_link_conditions, double eta, double *res_fibers,
                                    double *out_shell, double *v_bodies);
+/* The whole-vector operator and preconditioner over n devices: the skb_flow_set_body_operators / _set_fiber_links /
+ * _apply_system_matvec / _apply_system_preconditioner twins, with the same arguments (complete host arrays of all
+ * bodies and all fibers, the whole solution vector in and out), the same refusals (before any launch, earlier state
+ * untouched; the body checks cover every body and fiber, not just a member's) and the same drop rules
+ * (skb_mflow_set_bodies drops the body operators and the links, skb_mflow_set_fibers / _set_fiber_class the links).
+ * The periphery's operators come from skb_mflow_set_dense: SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY for the matvec,
+ * SKB_DENSE_M_INV for the preconditioner; each member's row block must fit the current periphery (after
+ * skb_mflow_set_periphery changed the node count, a block set before is refused until skb_mflow_set_dense is called
+ * again).  A change of the number of bodies re-initialises the group (its window carries the link forces): the fiber
+ * operators must then be set again, as after any change of the node counts.
+ *   Rows: member g owns, besides its fibers' and periphery rows (skb_mflow_partition), the 3 rows of each body node in
+ * its body rows [b0, b1) and the six rows [U; w] of every body whose FIRST node lies in [b0, b1); it keeps the
+ * inverses of the bodies it owns rows of.  x_bodies is complete on every member (system.cpp:306-311), so a body's
+ * K^T lambda sums over all of its nodes wherever its six rows are.
+ *   Link forces: every member computes the link conditions of its own fibers and, per body, the sum of its own bound
+ * fibers' forces and torques in container order; the members' partials are exchanged through the group window and
+ * added in member (rank) order, 0 first (the MPI_Allreduce of body_container.cpp:128-135).  Every member thus holds
+ * bitwise the same totals, and the result is bitwise reproducible run to run for a given device list; it differs from
+ * the single-device order by rounding only.  With one device it is the skb_flow path. */
+SKB_API int skb_mflow_set_body_operators(skb_mflow *mf, const int *n_nodes, int n_bodies, const double *node_weights,
+                                         const double *ex, const double *ey, const double *ez, const double *A_inv);
+SKB_API int skb_mflow_set_fiber_links(skb_mflow *mf, const int *body, const double *site,
+                                      const double *bending_rigidity);
+SKB_API int skb_mflow_apply_system_matvec(skb_mflow *mf, const double *x, double eta, double *res);
+SKB_API int skb_mflow_apply_system_preconditioner(skb_mflow *mf, const double *x, double *y);
 /* System::velocity_at_targets (system.cpp:330-384): targets block-partitioned over the devices */
 SKB_API int skb_mflow_velocity_at_targets(skb_mflow *mf, const double *r_trg, int64_t n_trg, const double *fib_forces,
                                           const double *shell_density, const double *body_densities,

@@ -158,6 +158,10 @@ def library() -> C.CDLL:
         "skb_mflow_set_dense": ([ctxp, C.c_int, _dp, C.c_int64, C.c_int64], C.c_int),
         "skb_mflow_matvec": ([ctxp, _dp, _dp, _dp, _dp, C.c_double, _dp], C.c_int),
         "skb_mflow_apply_matvec": ([ctxp, _dp, _dp, _dp, _dp, _dp, C.c_double, _dp, _dp, _dp], C.c_int),
+        "skb_mflow_set_body_operators": ([ctxp, C.POINTER(C.c_int), C.c_int, _dp, _dp, _dp, _dp, _dp], C.c_int),
+        "skb_mflow_set_fiber_links": ([ctxp, C.POINTER(C.c_int), _dp, _dp], C.c_int),
+        "skb_mflow_apply_system_matvec": ([ctxp, _dp, C.c_double, _dp], C.c_int),
+        "skb_mflow_apply_system_preconditioner": ([ctxp, _dp, _dp], C.c_int),
         "skb_mflow_velocity_at_targets": ([ctxp, _dp, C.c_int64, _dp, _dp, _dp, _dp, C.c_double, _dp], C.c_int),
         "skb_mflow_last_stats": ([ctxp, C.POINTER(FlowStats)], C.c_int),
         "skb_flow_set_target_ranges": ([ctxp, C.c_int, C.c_int] + [C.c_int64] * 4, C.c_int),
@@ -1026,6 +1030,50 @@ class MultiFlow:
         _check(library().skb_mflow_apply_matvec(self._h, _p(x), _p(b), _p(c), _p(ft), None if vb is None else _p(vb),
                                                 float(eta), _p(res), _p(o_s), _p(v_b)))
         return res, o_s, v_b
+
+    # ---- the whole solution vector [fibers | shell | bodies] over the devices (the Flow twins' conventions) ----
+    def set_body_operators(self, n_nodes, node_weights, ex, ey, ez, A_inv_list=None):
+        """As Flow.set_body_operators, for all bodies; every device keeps the bodies it owns rows of."""
+        n = np.ascontiguousarray(n_nodes, dtype=np.int32)
+        w = np.ascontiguousarray(node_weights, dtype=np.float64).reshape(-1)
+        ex, ey, ez = _arr(ex, 3), _arr(ey, 3), _arr(ez, 3)
+        Ai = None if A_inv_list is None else Flow._colmajor_concat(A_inv_list)
+        _check(library().skb_mflow_set_body_operators(self._h, n.ctypes.data_as(C.POINTER(C.c_int)), int(n.shape[0]),
+                                                      _p(w), _p(ex), _p(ey), _p(ez), None if Ai is None else _p(Ai)))
+        self._body_sol = int(np.sum(3 * n + 6))
+
+    def set_fiber_links(self, body=None, site=None, bending_rigidity=None):
+        """As Flow.set_fiber_links, for all fibers; body=None: no fiber is bound."""
+        if body is None:
+            _check(library().skb_mflow_set_fiber_links(self._h, None, None, None))
+            return
+        b = np.ascontiguousarray(body, dtype=np.int32)
+        st = _arr(site, 3)
+        E = np.ascontiguousarray(np.broadcast_to(np.asarray(bending_rigidity, dtype=np.float64), b.shape))
+        assert st.shape[0] == b.shape[0]
+        _check(library().skb_mflow_set_fiber_links(self._h, b.ctypes.data_as(C.POINTER(C.c_int)), _p(st), _p(E)))
+
+    def solution_size(self) -> int:
+        """4 N_f + 3 N_s + sum(3 n_b + 6) (the bodies' part as set_body_operators was last given)"""
+        return 4 * self.n_fib + 3 * self.n_shell + (getattr(self, "_body_sol", 0) if self.n_bodies else 0)
+
+    def apply_system_matvec(self, x, eta):
+        """System::apply_matvec on the whole solution vector x over the devices: returns res = A x.  The periphery's
+        operator is set_dense(DENSE_STRESSLET_PLUS_COMPLEMENTARY, ...)."""
+        x = np.ascontiguousarray(x, dtype=np.float64).reshape(-1)
+        assert x.shape[0] == self.solution_size()
+        res = np.empty_like(x)
+        _check(library().skb_mflow_apply_system_matvec(self._h, _p(x), float(eta), _p(res)))
+        return res
+
+    def apply_system_preconditioner(self, x):
+        """System::apply_preconditioner on the whole solution vector x over the devices: returns y = P^-1 x.  The
+        periphery's operator is set_dense(DENSE_M_INV, ...)."""
+        x = np.ascontiguousarray(x, dtype=np.float64).reshape(-1)
+        assert x.shape[0] == self.solution_size()
+        y = np.empty_like(x)
+        _check(library().skb_mflow_apply_system_preconditioner(self._h, _p(x), _p(y)))
+        return y
 
     def velocity_at_targets(self, r_trg, fib_forces, shell_density, body_densities, body_forces_torques, eta):
         r_trg = _arr(r_trg, 3)

@@ -9,6 +9,7 @@
 //                        densities gathered out of x_bodies into the 3 x N_b layout of the body flow (:286-289).
 //   body_matvec_kernel   SphericalBody::matvec (body_spherical.cpp:39-63; EllipsoidalBody::matvec is the same code) per
 //                        body: the node rows and the 6 rows -K^T lambda + U with a fixed-order reduction tree.
+//                        <true>: the rows a group member of skb_mflow owns (BodyOps, skb_internal.hpp).
 // K_ is never stored: K U = u + w x (x_i - c) and K^T lambda = [sum lambda_i ; sum (x_i - c) x lambda_i]
 // (update_K_matrix, body_spherical.cpp:74-86).
 #pragma once
@@ -143,14 +144,19 @@ __global__ void __launch_bounds__(kBodyThreads)
 }
 
 // res (x_bodies layout) of every body.  r: body node positions (3 per node), centers (3 per body), w: node_weights_,
-// ex / ey / ez: the singularity-subtraction vectors (3 per node), v: v_bodies (3 per node)
+// ex / ey / ez: the singularity-subtraction vectors (3 per node), v: v_bodies (3 per node).
+// kWindow (a group member, BodyOps): bodies b_first + blockIdx.x; only the node rows of nodes in [lo, hi) and the six
+// rows of a body whose first node is in [lo, hi) are written, v holds the nodes [lo, hi) only.  K^T lambda still sums
+// over all of the body's nodes (x_bodies and the geometry are complete), in the same order as without the window.
+template <bool kWindow>
 __global__ void __launch_bounds__(kBodyThreads)
     body_matvec_kernel(const BodyItem *__restrict__ bodies, const double *__restrict__ r,
                        const double *__restrict__ centers, const double *__restrict__ wgt,
                        const double *__restrict__ ex, const double *__restrict__ ey, const double *__restrict__ ez,
-                       const double *__restrict__ x_bodies, const double *__restrict__ v, double *__restrict__ res) {
+                       const double *__restrict__ x_bodies, const double *__restrict__ v, double *__restrict__ res,
+                       int b_first, long long lo, long long hi) {
     __shared__ double red[6][kBodyThreads];
-    const int b = blockIdx.x;
+    const int b = kWindow ? b_first + (int)blockIdx.x : (int)blockIdx.x;
     const BodyItem it = bodies[b];
     const int n = it.n_nodes;
     const double *x = x_bodies + it.sol_off;
@@ -168,8 +174,10 @@ __global__ void __launch_bounds__(kBodyThreads)
         cross3(rr, d, r_d);
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
-            const double cxyz = dx * ex[3 * g + k] + dy * ey[3 * g + k] + dz * ez[3 * g + k];
-            out[3 * i + k] = -cxyz - (u[k] + om_r[k]) + v[3 * g + k]; // :60
+            if (!kWindow || (g >= lo && g < hi)) {
+                const double cxyz = dx * ex[3 * g + k] + dy * ey[3 * g + k] + dz * ez[3 * g + k];
+                out[3 * i + k] = -cxyz - (u[k] + om_r[k]) + v[3 * (g - (kWindow ? lo : 0)) + k]; // :60
+            }
             acc[k] += d[k];
             acc[3 + k] += r_d[k];
         }
@@ -185,7 +193,7 @@ __global__ void __launch_bounds__(kBodyThreads)
                 red[k][threadIdx.x] += red[k][threadIdx.x + h];
         __syncthreads();
     }
-    if (threadIdx.x < 6)
+    if (threadIdx.x < 6 && (!kWindow || (it.node_off >= lo && it.node_off < hi)))
         out[3 * n + threadIdx.x] = -red[threadIdx.x][0] + x[3 * n + threadIdx.x]; // res_com = -K^T lambda + U  :61
 }
 

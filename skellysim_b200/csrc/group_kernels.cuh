@@ -11,6 +11,8 @@
 // (3) pair kernels on local memory only (TMA sources come from the member's own window); (4) flag barrier;
 // (5) PULL: every member adds up the partial velocities of its own fiber rows (and, with the cross kernel, of its own
 // periphery rows) from all windows (the reduce-scatter, fused with the accumulation into the velocity vector).
+// The whole-vector operator adds one store of the member's partial link forces into every window before (2) and one
+// rank-order sum of them after it.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -125,6 +127,47 @@ __global__ void group_pull_kernel(const GroupPullArgs a) {
     for (int m = 0; m < a.size; ++m)
         acc += __ldcv(a.u_part[m] + 3 * a.fa + i); // peer memory: never from a stale cache line
     a.v[i] = acc;
+}
+
+// ---- the bodies' link forces and torques of the whole-vector operator (BodyContainer, body_container.cpp:128-135) ----
+// Every member sums the links of ITS bound fibers per body (body_sum_kernel); the partials [F (3 n_b) | L (3 n_b)] go
+// into the member's slot of every window before flag barrier A, and after it every member adds up the slots of its own
+// window in rank order -- the MPI_Allreduce of the reference, bitwise the same total on every member and run to run.
+struct GroupFtStoreArgs {
+    const double *f, *t; // [n_bodies*3] each: this member's partial forces / torques
+    int n3;              // 3 n_bodies
+    int size;
+    double *slot[kMaxGroup]; // this member's slot [6 n_bodies] in every window
+};
+
+__global__ void group_ft_store_kernel(const GroupFtStoreArgs a) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= 2 * a.n3)
+        return;
+    const double v = i < a.n3 ? a.f[i] : a.t[i - a.n3];
+    for (int m = 0; m < a.size; ++m)
+        a.slot[m][i] = v;
+}
+
+struct GroupFtReduceArgs {
+    const double *slots; // this member's window: slot m at slots + m * stride
+    long long stride;    // 6 n_bodies
+    int first, count;    // the slots to add, in this order
+    int n3;
+    double *f, *t; // [n_bodies*3] each: the totals
+};
+
+__global__ void group_ft_reduce_kernel(const GroupFtReduceArgs a) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= 2 * a.n3)
+        return;
+    double acc = 0.0;
+    for (int m = a.first; m < a.first + a.count; ++m)
+        acc += __ldcv(a.slots + m * a.stride + i); // stored by peers: never from a stale cache line
+    if (i < a.n3)
+        a.f[i] = acc;
+    else
+        a.t[i - a.n3] = acc;
 }
 
 } // namespace skb

@@ -28,25 +28,45 @@ static int put(DevBuf &b, const void *h, size_t bytes, cudaStream_t st) {
 
 int BodyOps::set_operators(const int *n_nodes, int n_bodies, long long n_body_nodes, const double *r_body,
                            const double *centers, const double *node_weights, const double *ex, const double *ey,
-                           const double *ez, const double *A_inv, cudaStream_t st) {
+                           const double *ez, const double *A_inv, cudaStream_t st, long long lo, long long hi) {
     const char *who = "skb_flow_set_body_operators";
+    const bool windowed = hi >= 0;
     std::vector<BodyItem> items((size_t)n_bodies);
     std::vector<FiberGemvItem> gemv;
     long long nodes = 0, sol = 0, inv = 0;
-    int max_cols = 0;
+    long long inv_first = 0, inv_own = 0; // windowed: the owned bodies' inverses, contiguous in A_inv
+    int max_cols = 0, b0 = n_bodies, b1 = 0;
     for (int b = 0; b < n_bodies; ++b) {
         const int n = n_nodes[b];
         if (n < 1)
             return set_error(SKB_ERR_INVALID, "%s: body %d has %d nodes", who, b, n);
         items[(size_t)b] = BodyItem{nodes, sol, n, 0};
         const int m = 3 * n + 6;
-        for (int r0 = 0; r0 < m; r0 += kFiberGemvRows)
-            gemv.push_back(FiberGemvItem{inv, sol, sol, m, m, r0, n, b, 0});
+        if (!windowed) {
+            for (int r0 = 0; r0 < m; r0 += kFiberGemvRows)
+                gemv.push_back(FiberGemvItem{inv, sol, sol, m, m, r0, n, b, 0});
+        } else if (nodes < hi && nodes + n > lo) {
+            // the owned rows of this body: node rows [r_lo, r_hi), and [3n, 3n + 6) if its first node is owned; a
+            // 32-row block that reaches any of them is evaluated (the other rows of the block are never read)
+            if (b0 > b)
+                b0 = b, inv_first = inv;
+            b1 = b + 1;
+            const int r_lo = 3 * (int)(std::max(lo, nodes) - nodes), r_hi = 3 * (int)(std::min(hi, nodes + n) - nodes);
+            const bool six = nodes >= lo;
+            for (int r0 = 0; r0 < m; r0 += kFiberGemvRows) {
+                const int r1 = r0 + kFiberGemvRows;
+                if ((r0 < r_hi && r1 > r_lo) || (six && r1 > 3 * n))
+                    gemv.push_back(FiberGemvItem{inv - inv_first, sol, sol, m, m, r0, n, b, 0});
+            }
+            inv_own = inv + (long long)m * m - inv_first;
+        }
         max_cols = std::max(max_cols, m);
         nodes += n;
         sol += m;
         inv += (long long)m * m;
     }
+    if (!windowed)
+        inv_own = inv;
     if (nodes != n_body_nodes)
         return set_error(SKB_ERR_INVALID, "%s: the bodies' node counts sum to %lld, skb_flow_set_bodies has %lld nodes",
                          who, nodes, n_body_nodes);
@@ -70,13 +90,25 @@ int BodyOps::set_operators(const int *n_nodes, int n_bodies, long long n_body_no
     SKB_TRY(dens_.ensure((size_t)nodes * 24 + 8));
     SKB_TRY(force_.ensure((size_t)n_bodies * 24 + 8));
     SKB_TRY(torque_.ensure((size_t)n_bodies * 24 + 8));
-    if (A_inv && inv > 0) {
-        SKB_TRY(a_inv_.ensure((size_t)inv * 8));
-        SKB_TRY(upload_pageable(a_inv_.ptr, A_inv, (size_t)inv * 8, st));
+    if (A_inv && inv_own > 0) {
+        SKB_TRY(a_inv_.ensure((size_t)inv_own * 8));
+        SKB_TRY(upload_pageable(a_inv_.ptr, A_inv + inv_first, (size_t)inv_own * 8, st));
     }
     CUDA_TRY(cudaStreamSynchronize(st)); // the host tables above go out of scope
+    if (windowed) { // a group member's kernels are loaded now: a lazy load at the first launch would wait behind a
+                    // peer on the same device spinning on a flag
+        cudaFuncAttributes fa;
+        CUDA_TRY(cudaFuncGetAttributes(&fa, fiber_link_kernel));
+        CUDA_TRY(cudaFuncGetAttributes(&fa, body_sum_kernel));
+        CUDA_TRY(cudaFuncGetAttributes(&fa, body_matvec_kernel<true>));
+    }
     n_bodies_ = n_bodies;
     sol_size_ = sol;
+    windowed_ = windowed;
+    win_b0_ = std::min(b0, b1);
+    win_b1_ = b1;
+    win_lo_ = lo;
+    win_hi_ = hi;
     n_gemv_ = (int)gemv.size();
     gemv_smem_ = smem;
     inv_set_ = A_inv != nullptr || n_bodies == 0;
@@ -85,7 +117,8 @@ int BodyOps::set_operators(const int *n_nodes, int n_bodies, long long n_body_no
 }
 
 int BodyOps::set_links(const OwnFibers &own, const FiberOps &ops, int n_bodies, const double *centers,
-                       const int *body, const double *site, const double *rigidity, cudaStream_t st) {
+                       const int *body, const double *site, const double *rigidity, cudaStream_t st,
+                       bool check_only) {
     const char *who = "skb_flow_set_fiber_links";
     const int nfib = own.count();
     std::vector<LinkFiber> lf((size_t)nfib);
@@ -110,6 +143,8 @@ int BodyOps::set_links(const OwnFibers &own, const FiberOps &ops, int n_bodies, 
         count[(size_t)b + 1]++;
         any = true;
     }
+    if (check_only)
+        return SKB_OK;
     // bound fibers per body, in container order
     for (int b = 0; b < n_bodies; ++b)
         count[(size_t)b + 1] += count[(size_t)b];
@@ -157,10 +192,18 @@ int BodyOps::matvec(const double *d_x_bodies, const double *d_v_bodies, double *
                     int *launches) const {
     if (n_bodies_ == 0)
         return SKB_OK;
-    body_matvec_kernel<<<(unsigned)n_bodies_, kBodyThreads, 0, st>>>(
-        (const BodyItem *)items_.ptr, (const double *)r_.ptr, (const double *)centers_.ptr,
-        (const double *)weights_.ptr, (const double *)ex_.ptr, (const double *)ey_.ptr, (const double *)ez_.ptr,
-        d_x_bodies, d_v_bodies, d_res);
+    const BodyItem *items = (const BodyItem *)items_.ptr;
+    const double *r = (const double *)r_.ptr, *c = (const double *)centers_.ptr, *w = (const double *)weights_.ptr,
+                 *ex = (const double *)ex_.ptr, *ey = (const double *)ey_.ptr, *ez = (const double *)ez_.ptr;
+    if (!windowed_) {
+        body_matvec_kernel<false><<<(unsigned)n_bodies_, kBodyThreads, 0, st>>>(items, r, c, w, ex, ey, ez, d_x_bodies,
+                                                                                d_v_bodies, d_res, 0, 0, 0);
+        return launched(launches);
+    }
+    if (win_b1_ == win_b0_) // no body row is this member's
+        return SKB_OK;
+    body_matvec_kernel<true><<<(unsigned)(win_b1_ - win_b0_), kBodyThreads, 0, st>>>(
+        items, r, c, w, ex, ey, ez, d_x_bodies, d_v_bodies, d_res, win_b0_, win_lo_, win_hi_);
     return launched(launches);
 }
 

@@ -20,7 +20,8 @@ static int launched(int *launches) {
     return SKB_OK;
 }
 
-int Group::init(int rank, int size, long long n_fib, long long n_pad_fib, long long n_shell, long long n_pad_shell) {
+int Group::init(int rank, int size, long long n_fib, long long n_pad_fib, long long n_shell, long long n_pad_shell,
+                int n_bodies) {
     *this = Group(); // the old window and mappings are released here
     if (size == 1)
         return SKB_OK;
@@ -28,6 +29,7 @@ int Group::init(int rank, int size, long long n_fib, long long n_pad_fib, long l
     size_ = size;
     n_fib_ = n_fib;
     n_shell_ = n_shell;
+    n_bodies_ = n_bodies;
     size_t off = 0;
     auto take = [&](size_t bytes) {
         const size_t at = off;
@@ -39,12 +41,18 @@ int Group::init(int rank, int size, long long n_fib, long long n_pad_fib, long l
         lay_.f_sl[b] = take((size_t)n_pad_fib * 24 + 16);
         lay_.f_shell[b] = take((size_t)n_pad_shell * 48 + 16);
         lay_.x_shell[b] = take((size_t)n_shell * 24 + 16);
+        lay_.ft_part[b] = take((size_t)kMaxGroup * n_bodies * 48 + 16);
     }
     lay_.u_part = take((size_t)n_fib * 24 + 16);
     lay_.u_part_shell = take((size_t)n_shell * 24 + 16);
     lay_.bytes = off;
     CUDA_TRY(cudaMalloc(window_.out(), lay_.bytes));
     CUDA_TRY(cudaMemset(window_, 0, lay_.bytes)); // flags at epoch 0, strength pads zero for good
+    // loaded now, not lazily at their first launch, which would wait behind a peer on this device spinning on a flag
+    // (the warm-up's solo matvec does not run them)
+    cudaFuncAttributes fa;
+    CUDA_TRY(cudaFuncGetAttributes(&fa, group_ft_store_kernel));
+    CUDA_TRY(cudaFuncGetAttributes(&fa, group_ft_reduce_kernel));
     peer_[rank] = window_;
     return SKB_OK;
 }
@@ -66,7 +74,8 @@ int Group::import_handle(int peer_rank, const void *handle) {
 }
 
 int Group::connect(int peer_rank, const Group &peer, int dev, int peer_dev) {
-    if (peer.lay_.bytes != lay_.bytes || peer.n_fib_ != n_fib_ || peer.n_shell_ != n_shell_)
+    if (peer.lay_.bytes != lay_.bytes || peer.n_fib_ != n_fib_ || peer.n_shell_ != n_shell_ ||
+        peer.n_bodies_ != n_bodies_)
         return set_error(SKB_ERR_INVALID, "skb_flow_group_connect: the two members were laid out for different geometries");
     if (peer_dev != dev) {
         int can = 0;
@@ -96,11 +105,11 @@ int Group::missing_peer(int *missing) const {
     return SKB_OK;
 }
 
-int Group::check_layout(long long n_fib, long long n_shell) const {
-    if (n_fib_ != n_fib || n_shell_ != n_shell)
+int Group::check_layout(long long n_fib, long long n_shell, int n_bodies) const {
+    if (n_fib_ != n_fib || n_shell_ != n_shell || n_bodies_ != n_bodies)
         return set_error(SKB_ERR_STATE, "group member: the geometry changed size since skb_flow_group_init "
-                                        "(%lld/%lld fiber, %lld/%lld periphery nodes); re-initialise the group",
-                         n_fib, n_fib_, n_shell, n_shell_);
+                                        "(%lld/%lld fiber, %lld/%lld periphery nodes, %d/%d bodies); re-initialise the "
+                                        "group", n_fib, n_fib_, n_shell, n_shell_, n_bodies, n_bodies_);
     return SKB_OK;
 }
 
@@ -166,6 +175,39 @@ int Group::barrier(int phase, bool signal, bool wait, cudaStream_t st, int *laun
     a.do_wait = wait;
     a.timeout_cycles = kFlagTimeoutCycles;
     group_flag_kernel<<<1, 32, 0, st>>>(a);
+    return launched(launches);
+}
+
+// this member's partial forces / torques into its slot of every window (before barrier 0)
+int Group::push_forces(const double *d_f, const double *d_t, cudaStream_t st, int *launches) const {
+    if (n_bodies_ == 0)
+        return SKB_OK;
+    const size_t off = lay_.ft_part[epoch_ & 1] + (size_t)rank_ * n_bodies_ * 48;
+    GroupFtStoreArgs a;
+    a.f = d_f;
+    a.t = d_t;
+    a.n3 = 3 * n_bodies_;
+    char *w[kMaxGroup];
+    a.size = windows(w);
+    for (int m = 0; m < a.size; ++m)
+        a.slot[m] = (double *)(w[m] + off);
+    group_ft_store_kernel<<<(unsigned)((2 * a.n3 + 255) / 256), 256, 0, st>>>(a);
+    return launched(launches);
+}
+
+// the totals out of this member's window, slots in rank order (after barrier 0); solo: the own partial only
+int Group::reduce_forces(double *d_f, double *d_t, cudaStream_t st, int *launches) const {
+    if (n_bodies_ == 0)
+        return SKB_OK;
+    GroupFtReduceArgs a;
+    a.slots = own(lay_.ft_part[epoch_ & 1]);
+    a.stride = 6LL * n_bodies_;
+    a.first = solo_ ? rank_ : 0;
+    a.count = solo_ ? 1 : size_;
+    a.n3 = 3 * n_bodies_;
+    a.f = d_f;
+    a.t = d_t;
+    group_ft_reduce_kernel<<<(unsigned)((2 * a.n3 + 255) / 256), 256, 0, st>>>(a);
     return launched(launches);
 }
 

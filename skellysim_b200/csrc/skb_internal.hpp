@@ -243,18 +243,23 @@ int launch_gemv(const FiberGemvItem *d_items, int n_items, const double *mats, c
 // body_container.cpp:487-521) and BodyContainer::calculate_link_conditions (:171-267), on the device.  Bodies are in
 // the order of skb_flow_set_bodies, which is the order of the solution vector.  The caller has checked its pointers
 // for NULL and made the flow's device current; every step runs on the stream it passes.
+//
+// A group member (skb_mflow) owns the body node rows [lo, hi) of the solution vector -- 3 rows each -- and the six rows
+// [U; w] of every body whose FIRST node lies in [lo, hi); it keeps the inverses of the bodies it owns rows of, and
+// matvec / precondition write those rows only (of an output in the complete body layout).
 class BodyOps {
   public:
     // per body: n_nodes (summing to n_body_nodes), node_weights_, ex_ / ey_ / ez_ (3 per node), A_^-1 (column-major
-    // (3n+6)^2, concatenated; may be NULL); r_body / centers: the flow's geometry (host).  Checked first: a refusal
-    // leaves the earlier operators
+    // (3n+6)^2, concatenated; may be NULL); r_body / centers: the flow's geometry (host).  hi >= 0: a member's body
+    // node rows [lo, hi).  Checked first: a refusal leaves the earlier operators
     int set_operators(const int *n_nodes, int n_bodies, long long n_body_nodes, const double *r_body,
                       const double *centers, const double *node_weights, const double *ex, const double *ey,
-                      const double *ez, const double *A_inv, cudaStream_t st);
-    // per fiber of `own` (all fibers of the flow): body index (-1 free; body == NULL: none bound), lab-frame nucleation
-    // site, bending_rigidity_.  Checked first: a refusal leaves the earlier links
+                      const double *ez, const double *A_inv, cudaStream_t st, long long lo = 0, long long hi = -1);
+    // per fiber of `own` (all fibers of the flow, or a member's own fibers): body index (-1 free; body == NULL: none
+    // bound), lab-frame nucleation site, bending_rigidity_.  Checked first: a refusal leaves the earlier links;
+    // check_only: the checks and nothing else
     int set_links(const OwnFibers &own, const FiberOps &ops, int n_bodies, const double *centers, const int *body,
-                  const double *site, const double *rigidity, cudaStream_t st);
+                  const double *site, const double *rigidity, cudaStream_t st, bool check_only = false);
     void drop_operators() { ops_set_ = false; }
     void drop_links() { links_set_ = false; }
     bool has_operators() const { return ops_set_; }
@@ -263,13 +268,16 @@ class BodyOps {
     long long solution_size() const { return sol_size_; }
 
     // one matvec: the link conditions (*d_link: 7 per fiber, NULL when no fiber is bound), the bodies' link forces /
-    // torques and their densities gathered from x_bodies (forces(), torques(), densities()).  length: length_ per fiber
+    // torques and their densities gathered from x_bodies (forces(), torques(), densities()).  length: length_ per fiber.
+    // Over a member's own fibers the forces and torques are its partial sums
     int links(const FiberOps &ops, const double *d_length, const double *d_x_fib, const double *d_x_bodies,
               const double **d_link, cudaStream_t st, int *launches);
     const double *densities() const { return (const double *)dens_.ptr; }
     const double *forces() const { return (const double *)force_.ptr; }
     const double *torques() const { return (const double *)torque_.ptr; }
-    // res_bodies = bc.matvec(v_bodies, x_bodies); y = A_^-1 x per body
+    // res_bodies = bc.matvec(v_bodies, x_bodies); y = A_^-1 x per body.  A member's precondition evaluates every
+    // 32-row block of a body's GEMV that reaches one of its rows: the other rows of such a block are written to d_y as
+    // well and are scratch -- only the member's own rows of d_y are results
     int matvec(const double *d_x_bodies, const double *d_v_bodies, double *d_res, cudaStream_t st,
                int *launches) const;
     int precondition(const double *d_x, double *d_y, cudaStream_t st, int *launches) const;
@@ -278,6 +286,9 @@ class BodyOps {
     bool ops_set_ = false, inv_set_ = false, links_set_ = false, any_bound_ = false;
     int n_bodies_ = 0, n_fibers_ = 0, n_gemv_ = 0;
     long long sol_size_ = 0;
+    bool windowed_ = false; // a member's rows: bodies [win_b0_, win_b1_) have nodes in [win_lo_, win_hi_)
+    int win_b0_ = 0, win_b1_ = 0;
+    long long win_lo_ = 0, win_hi_ = 0;
     size_t gemv_smem_ = 0;
     DevBuf items_, r_, centers_, weights_, ex_, ey_, ez_, a_inv_, gemv_items_; // set_operators
     DevBuf link_fibers_, csr_begin_, csr_fib_, link_, contrib_;                 // set_links
@@ -293,6 +304,8 @@ class BodyOps {
 //   f_sl         [2][n_pad_fib*3]    packed (trapezoid-weighted) Stokeslet strengths of ALL fiber nodes   -- by peers
 //   f_shell      [2][n_pad_shell*6]  packed sym6 stresslet strengths of ALL periphery nodes                -- by peers
 //   x_shell      [2][n_shell*3]      periphery density of ALL nodes (input of the dense operator)          -- by peers
+//   ft_part      [2][kMaxGroup][n_bodies*6]  per member its partial link forces / torques of ALL bodies
+//                                    ([F | L]; the whole-vector operator, skb_mflow_apply_system_matvec) -- by peers
 //   u_part       [n_fib*3]           this member's partial velocities of ALL fiber rows                  -- by itself
 //   u_part_shell [n_shell*3]         its partial velocities of ALL periphery rows (cross kernel)        -- by itself
 //
@@ -303,7 +316,8 @@ class Group {
   public:
     // allocates and zeroes the window of member `rank` of `size` for that many fiber / periphery nodes; n_pad_*: the
     // padded source counts of the flow's evaluators (the window replaces their packed strengths).  Size 1: no member
-    int init(int rank, int size, long long n_fib, long long n_pad_fib, long long n_shell, long long n_pad_shell);
+    int init(int rank, int size, long long n_fib, long long n_pad_fib, long long n_shell, long long n_pad_shell,
+             int n_bodies);
     int export_handle(void *handle) const;                     // the window's CUDA-IPC handle
     int import_handle(int peer_rank, const void *handle);      // maps another process's member's window
     int connect(int peer_rank, const Group &peer, int dev, int peer_dev); // a member in this process, on peer_dev
@@ -313,7 +327,7 @@ class Group {
     bool has_window() const { return window_.get() != nullptr; }
     int rank() const { return rank_; }
     int size() const { return size_; }
-    int check_layout(long long n_fib, long long n_shell) const; // an error unless the window was laid out for these
+    int check_layout(long long n_fib, long long n_shell, int n_bodies) const; // an error unless laid out for these
     // solo (warm-up, profiling): no flags, push and pull over this member's own window only, no connectedness check
     void set_solo(bool solo) { solo_ = solo; }
     void restart() { epoch_ = 0; } // the next matvec is the group's first
@@ -327,6 +341,11 @@ class Group {
              const double *d_normal, long long sa, long long n_s, double two_eta, int num_sms, cudaStream_t st,
              int *launches) const;
     int barrier(int phase, bool signal, bool wait, cudaStream_t st, int *launches) const;
+    // the bodies' link forces of the whole-vector operator: push_forces stores this member's partials d_f / d_t
+    // [n_bodies*3 each] into its slot of every window (before barrier 0); reduce_forces (after it) writes the sum of
+    // every member's slot, in rank order, to d_f / d_t
+    int push_forces(const double *d_f, const double *d_t, cudaStream_t st, int *launches) const;
+    int reduce_forces(double *d_f, double *d_t, cudaStream_t st, int *launches) const;
     // d_v rows [0, n_rows) += the sum of every member's partial rows [row0, row0 + n_rows), in rank order
     enum Partials { kFiberRows, kShellRows };
     int pull(Partials which, long long row0, long long n_rows, double *d_v, cudaStream_t st, int *launches) const;
@@ -340,7 +359,8 @@ class Group {
 
   private:
     struct Layout { // byte offsets of the window's pieces
-        size_t flags = 0, f_sl[2] = {0, 0}, f_shell[2] = {0, 0}, x_shell[2] = {0, 0}, u_part = 0, u_part_shell = 0;
+        size_t flags = 0, f_sl[2] = {0, 0}, f_shell[2] = {0, 0}, x_shell[2] = {0, 0}, ft_part[2] = {0, 0}, u_part = 0,
+               u_part_shell = 0;
         size_t bytes = 0;
     };
     double *own(size_t off) const { return reinterpret_cast<double *>((char *)window_.get() + off); }
@@ -352,6 +372,7 @@ class Group {
     void *peer_[kMaxGroup] = {}; // every member's window as mapped here (peer_[rank_] == window_)
     IpcPtr ipc_[kMaxGroup];      // the windows of other processes' members that this one has mapped
     long long n_fib_ = 0, n_shell_ = 0; // geometry the window was laid out for
+    int n_bodies_ = 0;
     unsigned long long epoch_ = 0;
     bool solo_ = false;
 };
@@ -360,10 +381,33 @@ class Group {
 
 // ---- flow internals that skb_mflow.cu needs (skb_matvec.cu) ----
 struct skb_flow;
+struct skb_dense;
 namespace skb {
 cudaStream_t flow_stream(const skb_flow *fl); // the stream of the flow's own calls
 // sizes the buffers of the background streamer (skb_flow_set_overlap) for n_rows own periphery rows, if it is on
 int flow_size_overlap(skb_flow *fl, long long n_rows);
+
+// The whole-vector operator on one member of skb_mflow (the members of a group, or the single flow of a one-device
+// skb_mflow), after its target ranges are set.  The arguments are those of skb_flow_set_body_operators /
+// _set_fiber_links for ALL bodies / fibers; a member keeps the part its ranges own (BodyOps).  check_only: check the
+// links of every fiber and keep the earlier ones
+int flow_member_body_operators(skb_flow *fl, const int *n_nodes, int n_bodies, const double *node_weights,
+                               const double *ex, const double *ey, const double *ez, const double *A_inv);
+int flow_member_fiber_links(skb_flow *fl, const int *body, const double *site, const double *rigidity,
+                            bool check_only);
+// the state the system calls need (system_args without the dense operator): an error naming `who` unless it is there
+int flow_member_system_ready(skb_flow *fl, const char *who, bool precondition);
+int flow_size_system(skb_flow *fl); // sizes the buffers the two calls below use (before any member launches)
+// on st: x_fib 4 per own fiber node, x_shell 3 per own periphery row, x_bodies complete; res_fib / res_shell own rows,
+// res_bodies in the complete body layout, the owned rows written.  dn: the member's rows of
+// stresslet_plus_complementary (NULL without periphery rows)
+int flow_member_system_matvec(skb_flow *fl, skb_dense *dn, const double *d_x_fib, const double *d_x_shell,
+                              const double *d_x_bodies, double eta, double *d_res_fib, double *d_res_shell,
+                              double *d_res_bodies, cudaStream_t st);
+// the same layout, x_shell complete (3 per periphery node); dn: the member's rows of M_inv
+int flow_member_system_precondition(skb_flow *fl, skb_dense *dn, const double *d_x_fib, const double *d_x_shell,
+                                    const double *d_x_bodies, double *d_y_fib, double *d_y_shell, double *d_y_bodies,
+                                    cudaStream_t st);
 } // namespace skb
 
 // ---- context internals (shared by skb_runtime.cu and skb_matvec.cu) ----

@@ -95,6 +95,10 @@ struct skb_flow {
     BodyOps bodies; // the bodies' operators and the fiber-body links of the whole-vector operator (skb_body.cu)
     std::vector<double> h_centers; // body centres (set_fiber_links measures the nucleation sites from them)
     Group grp; // multi-GPU group membership: one member per GPU, exchange through peer memory (skb_group.cu)
+    // a member's whole-vector matvec in flight: matvec_core exchanges the bodies' partial link forces through the
+    // window and the body flow reads their totals from ft_sum ([F | L], 6 per body)
+    bool ft_exchange = false;
+    DevBuf ft_sum;
     // Periphery::matvec's dense operator beside the pair kernels (stream_kernels.cuh): forked onto bg_stream once its
     // input (the complete x_shell) is there, joined before res_shell is assembled
     struct Overlap {
@@ -764,7 +768,7 @@ static int prepare_matvec_targets(skb_flow *fl) {
         if (!fl->use_ranges)
             return set_error(SKB_ERR_STATE, "group member: call skb_flow_set_target_ranges (own fibers / periphery rows / "
                                             "body rows) before the first matvec");
-        SKB_TRY(fl->grp.check_layout(nf, ns));
+        SKB_TRY(fl->grp.check_layout(nf, ns, fl->n_bodies));
     }
     // group: fiber rows through the symmetric block rows of this member (partial sums, pulled together afterwards)
     // when the self-interaction is big enough for that kernel; otherwise the member's own rows with the plain kernel
@@ -976,7 +980,16 @@ static int matvec_core(skb_flow *fl, const double *d_ff, const double *d_sd, con
         SKB_TRY(G.push(d_ff, sf.has_weights ? (const double *)sf.weights.ptr : nullptr, fl->fa, n_fw, d_sd,
                        fl->n_shell ? (const double *)fl->shell[1]->devs[0].src[SKB_STRESSLET].normals.ptr : nullptr,
                        fl->sa, n_sw, 2.0 * eta, df.info.num_sms, fl->cur, &fl->launches));
+        const bool ft = fl->ft_exchange && fl->n_bodies > 0; // d_f / d_t: this member's partial link forces
+        if (ft)
+            SKB_TRY(G.push_forces(d_f, d_t, fl->cur, &fl->launches));
         SKB_TRY(G.barrier(0, true, true, fl->cur, &fl->launches)); // every member's strengths have landed here
+        if (ft) { // the bodies' link forces and torques: the members' partials in rank order (body_container.cpp:134)
+            double *sum = (double *)fl->ft_sum.ptr;
+            SKB_TRY(G.reduce_forces(sum, sum + 3 * fl->n_bodies, fl->cur, &fl->launches));
+            d_f = sum;
+            d_t = sum + 3 * fl->n_bodies;
+        }
         fmode = smode = kPacked;
         ff = G.f_sl();
         sd = G.f_shell();
@@ -1027,7 +1040,7 @@ int skb_flow_group_init(skb_flow *fl, int rank, int size) {
     // the same padded sizes the evaluator contexts use (set_sources_impl): the window replaces their f_packed
     const long long n_pad_fib = fl->n_fib > 0 ? fl->fib[1]->devs[0].src[SKB_STOKESLET].n_pad : 0;
     const long long n_pad_shell = fl->n_shell > 0 ? fl->shell[1]->devs[0].src[SKB_STRESSLET].n_pad : 0;
-    return fl->grp.init(rank, size, fl->n_fib, n_pad_fib, fl->n_shell, n_pad_shell);
+    return fl->grp.init(rank, size, fl->n_fib, n_pad_fib, fl->n_shell, n_pad_shell, fl->n_bodies);
 }
 
 int skb_flow_group_export(skb_flow *fl, void *handle) {
@@ -1814,6 +1827,100 @@ int skb_flow_apply_system_preconditioner_device(skb_flow *fl, skb_dense *dn, con
 }
 
 } // extern "C"
+
+// ---- the whole-vector operator on a member of skb_mflow (skb_internal.hpp) ---------------------------------------
+// A member holds its own fibers' links and its body rows' operators (BodyOps); x_bodies is complete on every member.
+// The bodies' link forces are exchanged inside matvec_core (ft_exchange); a single flow (a one-device skb_mflow) takes
+// the path of skb_flow_apply_system_matvec.
+
+int skb::flow_member_body_operators(skb_flow *fl, const int *n_nodes, int n_bodies, const double *node_weights,
+                                    const double *ex, const double *ey, const double *ez, const double *A_inv) {
+    if (n_bodies != fl->n_bodies)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_set_body_operators: %d bodies, skb_mflow_set_bodies has %d",
+                         n_bodies, fl->n_bodies);
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    SKB_TRY(prepare_matvec_targets(fl));
+    const bool member = fl->grp.member();
+    return fl->bodies.set_operators(n_nodes, n_bodies, fl->n_body, fl->h_r_body.data(), fl->h_centers.data(),
+                                    node_weights, ex, ey, ez, A_inv, fl->stream, member ? fl->ba : 0,
+                                    member ? fl->bb : -1);
+}
+
+int skb::flow_member_fiber_links(skb_flow *fl, const int *body, const double *site, const double *rigidity,
+                                 bool check_only) {
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    OwnFibers own{0, fl->n_fibers, fl->h_fiber_n.data(), fl->h_fiber_off.data(), (const double *)fl->r_fib.ptr,
+                  (const double *)fl->fiber_length.ptr, fl->stream};
+    if (!check_only)
+        SKB_TRY(own_fibers(fl, "skb_mflow_set_fiber_links", own));
+    const int f0 = own.f0;
+    return fl->bodies.set_links(own, fl->ops, fl->n_bodies, fl->h_centers.data(), body ? body + f0 : nullptr,
+                                body ? site + 3 * (size_t)f0 : nullptr, body ? rigidity + f0 : nullptr, fl->stream,
+                                check_only);
+}
+
+int skb::flow_member_system_ready(skb_flow *fl, const char *who, bool precondition) {
+    SKB_TRY(fl->ops.ready(who, precondition));
+    if (fl->n_bodies > 0) {
+        if (!fl->bodies.has_operators())
+            return set_error(SKB_ERR_INVALID, "%s: call skb_mflow_set_body_operators after skb_mflow_set_bodies", who);
+        if (precondition && !fl->bodies.has_inverse())
+            return set_error(SKB_ERR_INVALID, "%s: skb_mflow_set_body_operators was given no A_inv", who);
+        if (!precondition && fl->n_fibers > 0 && !fl->bodies.has_links())
+            return set_error(SKB_ERR_INVALID, "%s: call skb_mflow_set_fiber_links after skb_mflow_set_fibers / "
+                                              "skb_mflow_set_bodies (NULL body: no fiber is bound)", who);
+    }
+    return SKB_OK;
+}
+
+int skb::flow_size_system(skb_flow *fl) {
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    SKB_TRY(prepare_matvec_targets(fl));
+    SKB_TRY(fl->tmp_b.ensure((size_t)(fl->bb - fl->ba) * 24 + 8));
+    return fl->ft_sum.ensure((size_t)fl->n_bodies * 48 + 8);
+}
+
+int skb::flow_member_system_matvec(skb_flow *fl, skb_dense *dn, const double *d_x_fib, const double *d_x_shell,
+                                   const double *d_x_bodies, double eta, double *d_res_fib, double *d_res_shell,
+                                   double *d_res_bodies, cudaStream_t st) {
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    begin_stats(fl);
+    fl->cur = st;
+    const double *link = nullptr, *bd = nullptr, *f = nullptr, *t = nullptr;
+    if (fl->n_bodies > 0) { // the links of the own fibers; their partial forces / torques on every body
+        const auto &off = fl->h_fiber_off;
+        const long long f0 = fl->n_fibers ? std::lower_bound(off.begin(), off.end(), fl->fa) - off.begin() : 0;
+        SKB_TRY(fl->bodies.links(fl->ops, (const double *)fl->fiber_length.ptr + f0, d_x_fib, d_x_bodies, &link,
+                                 fl->cur, &fl->launches));
+        bd = fl->bodies.densities();
+        f = fl->bodies.forces();
+        t = fl->bodies.torques();
+    }
+    double *v_bodies = (double *)fl->tmp_b.ptr; // own body rows
+    fl->ft_exchange = fl->grp.member();
+    const int rc = apply_matvec_core(fl, dn, d_x_fib, d_x_shell, bd, f, t, link, eta, d_res_fib, d_res_shell, v_bodies);
+    fl->ft_exchange = false;
+    SKB_TRY(rc);
+    if (fl->n_bodies > 0)
+        SKB_TRY(fl->bodies.matvec(d_x_bodies, v_bodies, d_res_bodies, fl->cur, &fl->launches));
+    return device_stats(fl);
+}
+
+int skb::flow_member_system_precondition(skb_flow *fl, skb_dense *dn, const double *d_x_fib, const double *d_x_shell,
+                                         const double *d_x_bodies, double *d_y_fib, double *d_y_shell,
+                                         double *d_y_bodies, cudaStream_t st) {
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    begin_stats(fl);
+    fl->cur = st;
+    SKB_TRY(fl->ops.precondition(d_x_fib, d_y_fib, st, &fl->launches));
+    if (fl->sb > fl->sa) { // the member's rows of M_inv times the complete x_shell
+        SKB_TRY(skb_dense_apply_device(dn, SKB_DENSE_M_INV, d_x_shell, nullptr, d_y_shell, st));
+        fl->launches += 1;
+    }
+    if (fl->n_bodies > 0)
+        SKB_TRY(fl->bodies.precondition(d_x_bodies, d_y_bodies, st, &fl->launches));
+    return device_stats(fl);
+}
 
 cudaStream_t skb::flow_stream(const skb_flow *fl) { return fl->stream; }
 int skb::flow_size_overlap(skb_flow *fl, long long n_rows) {

@@ -105,10 +105,14 @@ struct skb_mflow {
     std::vector<int> f0, f1;
     std::vector<long long> s0, s1, b0, b1;
     bool part_dirty = true;
-    bool has_dense = false;
+    bool has_dense = false, has_minv = false; // skb_mflow_set_dense: stresslet_plus_complementary, M_inv
     bool ops_ready = false;
+    std::vector<int> body_n; // node counts of skb_mflow_set_body_operators (the body part of the solution vector)
+    long long body_sol = 0;  // ... its size, sum(3 n + 6)
     struct IO { // per-member device buffers of the host-pointer calls
         DevBuf x, xs, bd, f, t, link, res, outs, vb, ff, v;
+        DevBuf xsa, xb, rb; // the system calls: complete x_shell, complete x_bodies, body rows in the complete layout
+                            // (only the member's own rows of rb are results: BodyOps::precondition)
         Event e0, e1;
     };
     std::vector<IO> io;
@@ -256,7 +260,7 @@ int skb_mflow_set_bodies(skb_mflow *mf, const double *node_pos, const double *no
         return set_error(SKB_ERR_INVALID, "skb_mflow_set_bodies: bad arguments");
     SKB_TRY(mf->workers->run(
         [&](int g) { return skb_flow_set_bodies(mf->m[g].get(), node_pos, node_normal, n_nodes, centers, n_bodies); }));
-    if (mf->n_body != n_nodes)
+    if (mf->n_body != n_nodes || mf->n_bodies != n_bodies) // (the window holds 6 partials per body)
         mf->part_dirty = true;
     mf->n_body = n_nodes;
     mf->n_bodies = n_bodies;
@@ -423,6 +427,8 @@ int skb_mflow_set_dense(skb_mflow *mf, int op, const double *A_rowmajor, int64_t
     }));
     if (op == SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY)
         mf->has_dense = true;
+    if (op == SKB_DENSE_M_INV)
+        mf->has_minv = true;
     return SKB_OK;
 }
 
@@ -475,7 +481,8 @@ static int put(DevBuf &buf, const double *h, size_t n_dbl, cudaStream_t st) {
 
 // Size every member's transfer buffers on the CALLING thread, before any member starts launching: cudaMalloc /
 // cudaFree may synchronise the whole device and must not run while a peer on the same device sits in a flag wait.
-static int mflow_size_io(skb_mflow *mf, size_t n_ft) {
+// system: also the buffers of the whole-vector calls
+static int mflow_size_io(skb_mflow *mf, size_t n_ft, bool system = false) {
     for (int g = 0; g < mf->n; ++g) {
         CUDA_TRY(cudaSetDevice(mf->devs[g]));
         skb_mflow::IO &io = mf->io[g];
@@ -494,6 +501,12 @@ static int mflow_size_io(skb_mflow *mf, size_t n_ft) {
         SKB_TRY(io.v.ensure((n_fw + n_sw + n_bw) * 24 + 8));
         if (mf->has_dense && n_sw > 0)
             SKB_TRY(flow_size_overlap(mf->m[g].get(), 3 * (long long)n_sw));
+        if (system) {
+            SKB_TRY(io.xsa.ensure((size_t)mf->n_shell * 24 + 8));
+            SKB_TRY(io.xb.ensure((size_t)mf->body_sol * 8 + 8));
+            SKB_TRY(io.rb.ensure((size_t)mf->body_sol * 8 + 8));
+            SKB_TRY(flow_size_system(mf->m[g].get()));
+        }
     }
     return SKB_OK;
 }
@@ -595,6 +608,176 @@ int skb_mflow_apply_matvec(skb_mflow *mf, const double *x_fibers, const double *
                                      st));
         if (n_bw)
             CUDA_TRY(cudaMemcpyAsync(v_bodies + 3 * mf->b0[g], io.vb.ptr, (size_t)n_bw * 24, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        return SKB_OK;
+    }));
+    return mflow_collect_stats(mf);
+}
+
+// ---- the whole-vector operator [fibers | shell | bodies] over n devices ----------------------------------------------
+// Row ownership: member g owns its fibers' rows, its periphery rows and, of the body part, the 3 rows of each body node
+// in [b0, b1) and the six rows [U; w] of every body whose first node lies in [b0, b1) (skellysim_b200.distributed
+// .system_rows).  Its owned rows of the body part, as [begin, end) offsets into it, adjacent pieces merged
+static std::vector<std::pair<long long, long long>> body_rows(const std::vector<int> &body_n, long long b0,
+                                                              long long b1) {
+    std::vector<std::pair<long long, long long>> out;
+    auto add = [&](long long a, long long e) {
+        if (e <= a)
+            return;
+        if (!out.empty() && out.back().second == a)
+            out.back().second = e;
+        else
+            out.emplace_back(a, e);
+    };
+    long long node = 0, sol = 0;
+    for (int n : body_n) {
+        add(sol + 3 * (std::max(b0, node) - node), sol + 3 * (std::min(b1, node + n) - node));
+        if (node >= b0 && node < b1)
+            add(sol + 3LL * n, sol + 3LL * n + 6);
+        node += n;
+        sol += 3LL * n + 6;
+    }
+    return out;
+}
+
+int skb_mflow_set_body_operators(skb_mflow *mf, const int *n_nodes, int n_bodies, const double *node_weights,
+                                 const double *ex, const double *ey, const double *ez, const double *A_inv) {
+    const char *who = "skb_mflow_set_body_operators";
+    if (!mf)
+        return set_error(SKB_ERR_INVALID, "%s: NULL", who);
+    if (n_bodies != mf->n_bodies)
+        return set_error(SKB_ERR_INVALID, "%s: %d bodies, skb_mflow_set_bodies has %d", who, n_bodies, mf->n_bodies);
+    if (n_bodies > 0 && (!n_nodes || !node_weights || !ex || !ey || !ez))
+        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
+    SKB_TRY(mflow_prepare(mf));
+    // every member checks the same complete arrays first, so all of them refuse or none does
+    SKB_TRY(mf->workers->run([&](int g) -> int {
+        return flow_member_body_operators(mf->m[g].get(), n_nodes, n_bodies, node_weights, ex, ey, ez, A_inv);
+    }));
+    mf->body_n.assign(n_nodes, n_nodes + n_bodies);
+    mf->body_sol = 0;
+    for (int n : mf->body_n)
+        mf->body_sol += 3LL * n + 6;
+    return SKB_OK;
+}
+
+int skb_mflow_set_fiber_links(skb_mflow *mf, const int *body, const double *site, const double *bending_rigidity) {
+    const char *who = "skb_mflow_set_fiber_links";
+    if (!mf)
+        return set_error(SKB_ERR_INVALID, "%s: NULL", who);
+    if (body && mf->n_fibers > 0 && (!site || !bending_rigidity))
+        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
+    SKB_TRY(mflow_prepare(mf));
+    // the checks of every fiber before any member replaces its links (a member checks its own fibers only)
+    SKB_TRY(flow_member_fiber_links(mf->m[0].get(), body, site, bending_rigidity, true));
+    return mf->workers->run(
+        [&](int g) -> int { return flow_member_fiber_links(mf->m[g].get(), body, site, bending_rigidity, false); });
+}
+
+// the refusals of both system calls, before any launch; then every buffer they use is sized
+static int mflow_system_args(skb_mflow *mf, const char *who, bool precondition, bool args) {
+    if (!mf)
+        return set_error(SKB_ERR_INVALID, "%s: NULL", who);
+    SKB_TRY(mflow_prepare(mf)); // (a new partition drops the fiber operators)
+    if (!mf->ops_ready)
+        return set_error(SKB_ERR_STATE, "%s: call skb_mflow_set_fiber_operators first", who);
+    for (int g = 0; g < mf->n; ++g)
+        SKB_TRY(flow_member_system_ready(mf->m[g].get(), who, precondition));
+    const int op = precondition ? SKB_DENSE_M_INV : SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY;
+    const char *op_name = precondition ? "SKB_DENSE_M_INV" : "SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY";
+    if (mf->n_shell > 0 && !(precondition ? mf->has_minv : mf->has_dense))
+        return set_error(SKB_ERR_INVALID, "%s: the periphery needs its dense operator (skb_mflow_set_dense with %s)",
+                         who, op_name);
+    // each member's row block must fit the periphery as it is now (skb_mflow_set_periphery may have changed its size)
+    for (int g = 0; g < mf->n && mf->n_shell > 0; ++g) {
+        const long long n_sw = mf->s1[g] - mf->s0[g];
+        int64_t rows = -1, cols = -1;
+        if (n_sw > 0 && mf->dn[g])
+            SKB_TRY(skb_dense_shape(mf->dn[g].get(), op, &rows, &cols));
+        if (n_sw > 0 && (rows != 3 * n_sw || cols != 3 * mf->n_shell))
+            return set_error(SKB_ERR_INVALID, "%s: device member %d holds a %lld x %lld block of %s, need its %lld rows "
+                                              "x %lld of the %lld periphery nodes (call skb_mflow_set_dense again after "
+                                              "skb_mflow_set_periphery)", who, g, (long long)rows, (long long)cols,
+                             op_name, 3 * n_sw, 3 * mf->n_shell, mf->n_shell);
+    }
+    if (!args)
+        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
+    return mflow_size_io(mf, 0, true);
+}
+
+static long long mflow_solution_size(const skb_mflow *mf) {
+    return 4 * mf->n_fib + 3 * mf->n_shell + (mf->n_bodies > 0 ? mf->body_sol : 0);
+}
+
+// member g's owned rows of the device results into the complete host vector out
+static int mflow_download_rows(skb_mflow *mf, int g, double *out, cudaStream_t st) {
+    skb_mflow::IO &io = mf->io[g];
+    const MemberRows r = member_rows(mf, g);
+    const long long nf = mf->n_fib, ns = mf->n_shell;
+    if (r.n_fw)
+        CUDA_TRY(cudaMemcpyAsync(out + 4 * r.a, io.res.ptr, (size_t)r.n_fw * 32, cudaMemcpyDeviceToHost, st));
+    if (r.n_sw)
+        CUDA_TRY(cudaMemcpyAsync(out + 4 * nf + 3 * mf->s0[g], io.outs.ptr, (size_t)r.n_sw * 24,
+                                 cudaMemcpyDeviceToHost, st));
+    if (mf->n_bodies > 0)
+        for (const auto &p : body_rows(mf->body_n, mf->b0[g], mf->b1[g]))
+            CUDA_TRY(cudaMemcpyAsync(out + 4 * nf + 3 * ns + p.first, (const double *)io.rb.ptr + p.first,
+                                     (size_t)(p.second - p.first) * 8, cudaMemcpyDeviceToHost, st));
+    return SKB_OK;
+}
+
+// System::apply_matvec (system.cpp:269-324) over n devices on the whole solution vector
+int skb_mflow_apply_system_matvec(skb_mflow *mf, const double *x, double eta, double *res) {
+    const char *who = "skb_mflow_apply_system_matvec";
+    SKB_TRY(mflow_system_args(mf, who, false, (x && res) || (mf && mflow_solution_size(mf) == 0)));
+    if (!(eta > 0))
+        return set_error(SKB_ERR_INVALID, "%s: eta = %g", who, eta);
+    if (mflow_solution_size(mf) == 0)
+        return SKB_OK;
+    const long long nf = mf->n_fib, ns = mf->n_shell, nbs = mflow_solution_size(mf) - 4 * nf - 3 * ns;
+    SKB_TRY(mf->workers->run([&](int g) -> int {
+        skb_flow *fl = mf->m[g].get();
+        skb_mflow::IO &io = mf->io[g];
+        CUDA_TRY(cudaSetDevice(mf->devs[g]));
+        const MemberRows r = member_rows(mf, g);
+        cudaStream_t st = flow_stream(fl);
+        SKB_TRY(put(io.x, x + 4 * r.a, (size_t)r.n_fw * 4, st));
+        SKB_TRY(put(io.xs, x + 4 * nf + 3 * mf->s0[g], (size_t)r.n_sw * 3, st));
+        SKB_TRY(put(io.xb, x + 4 * nf + 3 * ns, (size_t)nbs, st)); // complete, as system.cpp:306-311 has it
+        CUDA_TRY(cudaEventRecord(io.e0, st));
+        SKB_TRY(flow_member_system_matvec(fl, mf->has_dense ? mf->dn[g].get() : nullptr, (const double *)io.x.ptr,
+                                          (const double *)io.xs.ptr, (const double *)io.xb.ptr, eta,
+                                          (double *)io.res.ptr, (double *)io.outs.ptr, (double *)io.rb.ptr, st));
+        CUDA_TRY(cudaEventRecord(io.e1, st));
+        SKB_TRY(mflow_download_rows(mf, g, res, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        return SKB_OK;
+    }));
+    return mflow_collect_stats(mf);
+}
+
+// System::apply_preconditioner (system.cpp:248-262) over n devices: block diagonal, no exchange
+int skb_mflow_apply_system_preconditioner(skb_mflow *mf, const double *x, double *y) {
+    const char *who = "skb_mflow_apply_system_preconditioner";
+    SKB_TRY(mflow_system_args(mf, who, true, (x && y) || (mf && mflow_solution_size(mf) == 0)));
+    if (mflow_solution_size(mf) == 0)
+        return SKB_OK;
+    const long long nf = mf->n_fib, ns = mf->n_shell, nbs = mflow_solution_size(mf) - 4 * nf - 3 * ns;
+    SKB_TRY(mf->workers->run([&](int g) -> int {
+        skb_flow *fl = mf->m[g].get();
+        skb_mflow::IO &io = mf->io[g];
+        CUDA_TRY(cudaSetDevice(mf->devs[g]));
+        const MemberRows r = member_rows(mf, g);
+        cudaStream_t st = flow_stream(fl);
+        SKB_TRY(put(io.x, x + 4 * r.a, (size_t)r.n_fw * 4, st));
+        SKB_TRY(put(io.xsa, r.n_sw ? x + 4 * nf : nullptr, (size_t)ns * 3, st));
+        SKB_TRY(put(io.xb, x + 4 * nf + 3 * ns, (size_t)nbs, st));
+        CUDA_TRY(cudaEventRecord(io.e0, st));
+        SKB_TRY(flow_member_system_precondition(fl, mf->dn[g].get(), (const double *)io.x.ptr,
+                                                (const double *)io.xsa.ptr, (const double *)io.xb.ptr,
+                                                (double *)io.res.ptr, (double *)io.outs.ptr, (double *)io.rb.ptr, st));
+        CUDA_TRY(cudaEventRecord(io.e1, st));
+        SKB_TRY(mflow_download_rows(mf, g, y, st));
         CUDA_TRY(cudaStreamSynchronize(st));
         return SKB_OK;
     }));

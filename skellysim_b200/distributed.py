@@ -88,6 +88,30 @@ def reference_rank_ranges(n_fibers: int, n_shell_nodes: int, n_body_nodes: int, 
     return f0, f1, s0, s1, b0, b1
 
 
+def system_rows(partition, fiber_n_nodes, n_shell: int, body_n_nodes):
+    """The indices of the whole solution vector [fibers (4 per node) | shell (3 per node) | bodies (3 n + 6 each)] one
+    member owns, ascending.  partition: its six target ranges (f0, f1, s0, s1, b0, b1), as skb_mflow_partition /
+    capi.partition_query give them.  Besides its fibers' and periphery rows, the member owns the 3 rows of each body node
+    in [b0, b1) and the six rows [U; w] of every body whose first node lies in [b0, b1) -- the rule of
+    skb_mflow_apply_system_matvec."""
+    import numpy as np
+    f0, f1, s0, s1, b0, b1 = (int(v) for v in partition)
+    fn = np.asarray(fiber_n_nodes, dtype=np.int64)
+    node_off = np.concatenate([[0], np.cumsum(fn)])
+    n_fib = int(node_off[-1])
+    pieces = [np.arange(4 * node_off[f0], 4 * node_off[f1]), 4 * n_fib + np.arange(3 * s0, 3 * s1)]
+    base, node = 4 * n_fib + 3 * int(n_shell), 0
+    for n in (int(v) for v in body_n_nodes):
+        lo, hi = max(b0, node), min(b1, node + n)
+        if lo < hi:
+            pieces.append(base + np.arange(3 * (lo - node), 3 * (hi - node)))
+        if b0 <= node < b1:
+            pieces.append(base + 3 * n + np.arange(6))
+        node += n
+        base += 3 * n + 6
+    return np.concatenate(pieces).astype(np.int64)
+
+
 def connect_group(flow, rank: int, world: int, group=None):
     """One rank per GPU: make `flow` (geometry and target ranges already set) a member of a peer-memory group.  Every
     rank exports the CUDA-IPC handle of its window, the 64-byte handles travel through torch.distributed once, every
