@@ -62,9 +62,9 @@ SKB_API int skb_flow_velocity_at_targets(skb_flow *fl, const double *r_trg, int6
                                          const double *shell_density, const double *body_densities,
                                          const double *body_forces_torques, double eta, double *vel);
 
-/* Optional analytic add-ons of velocity_at_targets (system.cpp:358-359): point forces/torques
- * (PointSourceContainer::flow, point_source.cpp:16-54: regularised Oseen contraction + rotlet; the caller passes
- * the points that are alive at the current time) and the linear background flow (BackgroundSource::flow,
+/* Optional analytic add-ons of velocity_at_targets (system.cpp:358-359) and of skb_flow_build_system_rhs: point
+ * forces/torques (PointSourceContainer::flow, point_source.cpp:16-54: regularised Oseen contraction + rotlet; the caller
+ * passes the points that are alive at the current time) and the linear background flow (BackgroundSource::flow,
  * background_source.cpp:15-24: u_j = uniform_j + r[components_j] * scale_factor_j).  n_points == 0 / NULL clears. */
 SKB_API int skb_flow_set_point_sources(skb_flow *fl, const double *positions, const double *forces,
                                        const double *torques, int n_points);
@@ -363,6 +363,37 @@ SKB_API int skb_flow_apply_system_preconditioner(skb_flow *fl, struct skb_dense 
 SKB_API int skb_flow_apply_system_preconditioner_device(skb_flow *fl, struct skb_dense *dn, const double *d_x,
                                                         double *d_y, void *stream);
 
+/* ---- the right-hand side of the whole system --------------------------------------------------------------------
+ * System::prep_state_for_solver's RHS (system.cpp:398-458) as Solver::set_RHS lays it out (solver_hydro.cpp:51-61):
+ * rhs has 4 N_f + 3 N_s + sum(3 n_b + 6) entries, the layout of the system calls above.  In the reference's order:
+ *   v_all  = fc.flow(r_all, f_external, eta), the fiber self term subtracted (system.cpp:425; motor forces are not in
+ *            this flow), + bc.flow(r_all, 0, F_T, eta): the bodies' centre Stokeslets and rotlets (:431-443)
+ *   v_all += the point sources and the background flow of skb_flow_set_point_sources / _set_background (:445-446)
+ *   fibers: skb_flow_build_fiber_rhs on the fiber rows of v_all (update_rhs with motor + f_external, apply_bcs with
+ *           f_external, :451-453); shell: -v_shell (periphery.cpp:86); body b: [-v of its nodes ; 0 0 0 0 0 0]
+ *           (body_spherical.cpp:134-138).  The periphery's densities and the link conditions do not enter.
+ * The flow is skb_flow_matvec's (f_external, zero periphery and body densities, F_T): its symmetric and cross kernels
+ * and skb_flow_set_self_exclusion apply, and its rows are bitwise those of that call.  params / v_growth / force_scale as
+ * skb_flow_build_fiber_rhs; f_external 3 x N_f or NULL (no external fiber force: no fiber flow);
+ * body_forces_torques 6 x n_bodies (as skb_flow_matvec) or NULL (all zero, the reference's `.any()` false).
+ * Needs skb_flow_set_fiber_class and _class_derivatives for every node count in use and, with bodies,
+ * skb_flow_set_body_operators (its node counts place each body's six rows); not the fiber operators, their inverse or
+ * the links, and it leaves them and the body operators untouched.  Refused (SKB_ERR_INVALID, before any launch,
+ * earlier state untouched): what skb_flow_build_fiber_rhs refuses, NULL params or rhs where there are fibers or
+ * entries, a non-finite external force or torque (host forms: the _device form does not read its inputs on the host),
+ * bodies without body operators, a group member, a target window or ranges that do not cover every row (over several
+ * devices use skb_mflow_build_system_rhs).
+ * The _device form follows skb_flow_build_fiber_rhs_device: everything on this flow's device, asynchronous on `stream`,
+ * the per-fiber tables from host memory; d_body_forces / d_body_torques 3 x n_bodies each (as skb_flow_matvec_device),
+ * either NULL for zero. */
+SKB_API int skb_flow_build_system_rhs(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
+                                      const double *force_scale, const double *f_external,
+                                      const double *body_forces_torques, double dt, double eta, double *rhs);
+SKB_API int skb_flow_build_system_rhs_device(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
+                                             const double *force_scale, const double *d_f_external,
+                                             const double *d_body_forces, const double *d_body_torques, double dt,
+                                             double eta, double *d_rhs, void *stream);
+
 typedef struct skb_flow_stats {
     double device_ms;   /* CUDA-event time of the last call, first launch to last kernel (copies excluded) */
     double total_ms;    /* including H2D / D2H */
@@ -448,6 +479,19 @@ SKB_API int skb_mflow_set_fiber_links(skb_mflow *mf, const int *body, const doub
                                       const double *bending_rigidity);
 SKB_API int skb_mflow_apply_system_matvec(skb_mflow *mf, const double *x, double eta, double *res);
 SKB_API int skb_mflow_apply_system_preconditioner(skb_mflow *mf, const double *x, double *y);
+/* skb_flow_build_system_rhs over n devices, the same arguments (complete host arrays of all fibers and bodies, the whole
+ * vector out) and refusals, every member's checked before any device starts.  Each member forms its own rows (those of
+ * skb_mflow_apply_system_matvec); the flow is the group's matvec flow, and the complete F_T enter every member's body
+ * flow as they are.  With one device it is the skb_flow path. */
+SKB_API int skb_mflow_build_system_rhs(skb_mflow *mf, const skb_fiber_params *params, const double *v_growth,
+                                       const double *force_scale, const double *f_external,
+                                       const double *body_forces_torques, double dt, double eta, double *rhs);
+/* skb_flow_set_point_sources / _set_background on every device: skb_mflow_velocity_at_targets and
+ * skb_mflow_build_system_rhs include them */
+SKB_API int skb_mflow_set_point_sources(skb_mflow *mf, const double *positions, const double *forces,
+                                        const double *torques, int n_points);
+SKB_API int skb_mflow_set_background(skb_mflow *mf, const int *components, const double *scale_factor,
+                                     const double *uniform);
 /* System::velocity_at_targets (system.cpp:330-384): targets block-partitioned over the devices */
 SKB_API int skb_mflow_velocity_at_targets(skb_mflow *mf, const double *r_trg, int64_t n_trg, const double *fib_forces,
                                           const double *shell_density, const double *body_densities,

@@ -202,6 +202,14 @@ def library() -> C.CDLL:
         "skb_flow_apply_system_matvec_device": ([ctxp, ctxp, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p], C.c_int),
         "skb_flow_apply_system_preconditioner": ([ctxp, ctxp, _dp, _dp], C.c_int),
         "skb_flow_apply_system_preconditioner_device": ([ctxp, ctxp, C.c_void_p, C.c_void_p, C.c_void_p], C.c_int),
+        "skb_flow_build_system_rhs": ([ctxp, C.POINTER(FiberParams), _dp, _dp, _dp, _dp, C.c_double, C.c_double, _dp],
+                                      C.c_int),
+        "skb_flow_build_system_rhs_device": ([ctxp, C.POINTER(FiberParams), _dp, _dp] + [C.c_void_p] * 3
+                                             + [C.c_double, C.c_double, C.c_void_p, C.c_void_p], C.c_int),
+        "skb_mflow_build_system_rhs": ([ctxp, C.POINTER(FiberParams), _dp, _dp, _dp, _dp, C.c_double, C.c_double, _dp],
+                                       C.c_int),
+        "skb_mflow_set_point_sources": ([ctxp, _dp, _dp, _dp, C.c_int], C.c_int),
+        "skb_mflow_set_background": ([ctxp, C.POINTER(C.c_int), _dp, _dp], C.c_int),
     }
     global BOUND_FUNCTIONS
     BOUND_FUNCTIONS = tuple(sorted(sig))
@@ -278,6 +286,16 @@ def _fiber_rhs_args(n_fibers, n_nodes, params, v_growth, force_scale, v_on_fiber
         if a is not None and a.shape[0] != n_nodes:
             raise ValueError(f"expected ({n_nodes}, 3) node values, got {a.shape}")
     return p, _per_fiber(v_growth, n_fibers), _per_fiber(force_scale, n_fibers), v, f
+
+
+def _system_rhs_args(n_fibers, n_nodes, n_bodies, params, v_growth, force_scale, f_external, body_forces_torques):
+    """_fiber_rhs_args of a system RHS call (f_external in place of the flow) and its (n_bodies, 6) external F_T, each
+    None where absent"""
+    p, vg, fs, _, f = _fiber_rhs_args(n_fibers, n_nodes, params, v_growth, force_scale, None, f_external)
+    ft = None if body_forces_torques is None else _arr(body_forces_torques, 6)
+    if ft is not None and ft.shape[0] != n_bodies:
+        raise ValueError(f"expected ({n_bodies}, 6) body forces and torques, got {ft.shape}")
+    return p, vg, fs, f, ft
 
 
 def device_count() -> int:
@@ -852,6 +870,37 @@ class Flow:
                                                                      C.c_void_p(d_x), C.c_void_p(d_y),
                                                                      C.c_void_p(stream)))
 
+    def build_system_rhs(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
+                         plus_hinged, dt, eta, f_external=None, body_forces_torques=None, v_growth=None,
+                         force_scale=None):
+        """System::prep_state_for_solver's RHS (system.cpp:398-458) as a whole solution vector (solution_size(),):
+        the flow of f_external (N_f, 3) and of the bodies' external forces / torques (n_bodies, 6), plus the point
+        sources and the background flow, into the fiber block (build_fiber_rhs's parameters), -v_shell and
+        [-v_body ; 0] per body.  f_external / body_forces_torques None: zero."""
+        f0, f1 = self._own_fibers()
+        p, vg, fs, f, ft = _system_rhs_args(f1 - f0, self.n_fib, self.n_bodies,
+                                            (length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
+                                             minus_clamped, plus_hinged), v_growth, force_scale, f_external,
+                                            body_forces_torques)
+        rhs = np.empty(self.solution_size())
+        _check(library().skb_flow_build_system_rhs(self._h, _params_ptr(p), _opt_p(vg), _opt_p(fs), _opt_p(f),
+                                                   _opt_p(ft), float(dt), float(eta), _p(rhs)))
+        return rhs
+
+    def build_system_rhs_device(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
+                                minus_clamped, plus_hinged, dt, eta, d_f_external: int, d_body_forces: int,
+                                d_body_torques: int, d_rhs: int, v_growth=None, force_scale=None, stream: int = 0):
+        """build_system_rhs on device pointers (0: none for the inputs; forces and torques (n_bodies, 3) each),
+        asynchronous on `stream`; returns once the per-fiber tables are staged."""
+        f0, f1 = self._own_fibers()
+        p, vg, fs, _, _ = _system_rhs_args(f1 - f0, 0, self.n_bodies,
+                                           (length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
+                                            minus_clamped, plus_hinged), v_growth, force_scale, None, None)
+        vp = lambda a: C.c_void_p(a) if a else None
+        _check(library().skb_flow_build_system_rhs_device(self._h, _params_ptr(p), _opt_p(vg), _opt_p(fs),
+                                                          vp(d_f_external), vp(d_body_forces), vp(d_body_torques),
+                                                          float(dt), float(eta), vp(d_rhs), vp(stream)))
+
     # ---- multi-GPU groups (peer memory) ----
     def last_sym_kernel(self):
         """(ms, ordered pairs) of the last launch of the symmetric fiber-fiber kernel inside matvec()."""
@@ -1074,6 +1123,33 @@ class MultiFlow:
         y = np.empty_like(x)
         _check(library().skb_mflow_apply_system_preconditioner(self._h, _p(x), _p(y)))
         return y
+
+    def build_system_rhs(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
+                         plus_hinged, dt, eta, f_external=None, body_forces_torques=None, v_growth=None,
+                         force_scale=None):
+        """Flow.build_system_rhs over the devices, every device forming its own rows: the whole vector
+        (solution_size(),)."""
+        p, vg, fs, f, ft = _system_rhs_args(self.n_fibers, self.n_fib, self.n_bodies,
+                                            (length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
+                                             minus_clamped, plus_hinged), v_growth, force_scale, f_external,
+                                            body_forces_torques)
+        rhs = np.empty(self.solution_size())
+        _check(library().skb_mflow_build_system_rhs(self._h, _params_ptr(p), _opt_p(vg), _opt_p(fs), _opt_p(f),
+                                                    _opt_p(ft), float(dt), float(eta), _p(rhs)))
+        return rhs
+
+    def set_point_sources(self, positions, forces, torques):
+        """Flow.set_point_sources on every device (velocity_at_targets and build_system_rhs include them)."""
+        positions, forces, torques = _arr(positions, 3), _arr(forces, 3), _arr(torques, 3)
+        _check(library().skb_mflow_set_point_sources(self._h, _p(positions), _p(forces), _p(torques),
+                                                     positions.shape[0]))
+
+    def set_background(self, components, scale_factor, uniform):
+        """Flow.set_background on every device."""
+        comp = (C.c_int * 3)(*[int(c) for c in components])
+        sc = np.ascontiguousarray(scale_factor, dtype=np.float64)
+        un = np.ascontiguousarray(uniform, dtype=np.float64)
+        _check(library().skb_mflow_set_background(self._h, comp, _p(sc), _p(un)))
 
     def velocity_at_targets(self, r_trg, fib_forces, shell_density, body_densities, body_forces_torques, eta):
         r_trg = _arr(r_trg, 3)

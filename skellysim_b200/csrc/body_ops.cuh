@@ -10,6 +10,7 @@
 //   body_matvec_kernel   SphericalBody::matvec (body_spherical.cpp:39-63; EllipsoidalBody::matvec is the same code) per
 //                        body: the node rows and the 6 rows -K^T lambda + U with a fixed-order reduction tree.
 //                        <true>: the rows a group member of skb_mflow owns (BodyOps, skb_internal.hpp).
+//   system_rhs_rows_kernel  the shell and body rows of System::prep_state_for_solver's RHS: -v, and six zeros per body.
 // K_ is never stored: K U = u + w x (x_i - c) and K^T lambda = [sum lambda_i ; sum (x_i - c) x lambda_i]
 // (update_K_matrix, body_spherical.cpp:74-86).
 #pragma once
@@ -195,6 +196,30 @@ __global__ void __launch_bounds__(kBodyThreads)
     }
     if (threadIdx.x < 6 && (!kWindow || (it.node_off >= lo && it.node_off < hi)))
         out[3 * n + threadIdx.x] = -red[threadIdx.x][0] + x[3 * n + threadIdx.x]; // res_com = -K^T lambda + U  :61
+}
+
+// The shell and body rows of System::prep_state_for_solver's RHS (system.cpp:448,455): Periphery::update_RHS
+// (periphery.cpp:86) rhs_shell = -v_shell, and per body update_RHS (body_spherical.cpp:134-138) [-v of its nodes ; six
+// zeros].  CTAs [0, n_body_ctas) take the bodies b_first + blockIdx.x: the node rows of nodes in [lo, hi) (v holds the
+// nodes [lo, hi)) and the six rows of a body whose first node is in [lo, hi), of rhs_bodies in the x_bodies layout --
+// the rows a group member owns, or every row with lo = 0, hi = N_b.  The other CTAs negate the n_shell3 shell entries.
+__global__ void __launch_bounds__(kBodyThreads)
+    system_rhs_rows_kernel(const BodyItem *__restrict__ bodies, int b_first, int n_body_ctas, long long lo,
+                           long long hi, const double *__restrict__ v, double *__restrict__ rhs_bodies,
+                           const double *__restrict__ v_shell, long long n_shell3, double *__restrict__ rhs_shell) {
+    if ((int)blockIdx.x >= n_body_ctas) {
+        const long long stride = (long long)(gridDim.x - n_body_ctas) * kBodyThreads;
+        for (long long i = (long long)(blockIdx.x - n_body_ctas) * kBodyThreads + threadIdx.x; i < n_shell3; i += stride)
+            rhs_shell[i] = -v_shell[i];
+        return;
+    }
+    const BodyItem it = bodies[b_first + (int)blockIdx.x];
+    double *out = rhs_bodies + it.sol_off;
+    const long long a = max(lo, it.node_off), e = min(hi, it.node_off + it.n_nodes);
+    for (long long k = 3 * a + threadIdx.x; k < 3 * e; k += kBodyThreads)
+        out[k - 3 * it.node_off] = -v[k - 3 * lo];
+    if (threadIdx.x < 6 && it.node_off >= lo && it.node_off < hi)
+        out[3 * it.n_nodes + threadIdx.x] = 0.0;
 }
 
 } // namespace skb

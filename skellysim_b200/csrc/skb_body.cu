@@ -6,6 +6,7 @@
 #include "skb_internal.hpp"
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <vector>
 
@@ -204,6 +205,31 @@ int BodyOps::matvec(const double *d_x_bodies, const double *d_v_bodies, double *
         return SKB_OK;
     body_matvec_kernel<true><<<(unsigned)(win_b1_ - win_b0_), kBodyThreads, 0, st>>>(
         items, r, c, w, ex, ey, ez, d_x_bodies, d_v_bodies, d_res, win_b0_, win_lo_, win_hi_);
+    return launched(launches);
+}
+
+int skb::load_rhs_rows_kernel() {
+    cudaFuncAttributes fa;
+    CUDA_TRY(cudaFuncGetAttributes(&fa, system_rhs_rows_kernel));
+    return SKB_OK;
+}
+
+int BodyOps::rhs_rows(bool bodies, const double *d_v_bodies, double *d_rhs_bodies, const double *d_v_shell,
+                      long long n_shell_rows, double *d_rhs_shell, cudaStream_t st, int *launches) const {
+    int b0 = 0, nb = 0;
+    long long lo = 0, hi = 0;
+    if (bodies && n_bodies_ > 0) {
+        b0 = windowed_ ? win_b0_ : 0;
+        nb = windowed_ ? win_b1_ - win_b0_ : n_bodies_;
+        lo = windowed_ ? win_lo_ : 0;
+        hi = windowed_ ? win_hi_ : LLONG_MAX;
+    }
+    const long long n3 = 3 * n_shell_rows;
+    const int shell_ctas = (int)std::min<long long>((n3 + kBodyThreads - 1) / kBodyThreads, 1024);
+    if (nb + shell_ctas == 0)
+        return SKB_OK;
+    system_rhs_rows_kernel<<<(unsigned)(nb + shell_ctas), kBodyThreads, 0, st>>>(
+        (const BodyItem *)items_.ptr, b0, nb, lo, hi, d_v_bodies, d_rhs_bodies, d_v_shell, n3, d_rhs_shell);
     return launched(launches);
 }
 

@@ -451,5 +451,9 @@ int skb::prepare_fiber_kernels() {
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kInverseSmemMax));
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     }
+    // loaded now: a group member's system RHS launches it, and a lazy load then could wait behind a peer on the same
+    // device spinning on a flag
+    cudaFuncAttributes fa;
+    CUDA_TRY(cudaFuncGetAttributes(&fa, fiber_rhs_kernel));
     return SKB_OK;
 }

@@ -281,6 +281,11 @@ class BodyOps {
     int matvec(const double *d_x_bodies, const double *d_v_bodies, double *d_res, cudaStream_t st,
                int *launches) const;
     int precondition(const double *d_x, double *d_y, cudaStream_t st, int *launches) const;
+    // the shell and body rows of the RHS in one launch: d_rhs_shell = -d_v_shell (n_shell_rows rows) and, with
+    // `bodies`, per body [-v of its nodes ; 0 x 6] into d_rhs_bodies (x_bodies layout, the rows matvec writes) from
+    // d_v_bodies (the body rows matvec reads)
+    int rhs_rows(bool bodies, const double *d_v_bodies, double *d_rhs_bodies, const double *d_v_shell,
+                 long long n_shell_rows, double *d_rhs_shell, cudaStream_t st, int *launches) const;
 
   private:
     bool ops_set_ = false, inv_set_ = false, links_set_ = false, any_bound_ = false;
@@ -294,6 +299,8 @@ class BodyOps {
     DevBuf link_fibers_, csr_begin_, csr_fib_, link_, contrib_;                 // set_links
     DevBuf dens_, force_, torque_;                                              // per matvec
 };
+// loads the kernel of BodyOps::rhs_rows (a group member's first launch must not load it lazily)
+int load_rhs_rows_kernel();
 
 // ---- one member of a multi-GPU group of flows (DESIGN.md §4; skb_group.cu, group_kernels.cuh) ----
 // A group is one flow per GPU exchanging strengths and partial velocities through peer memory.  Every member owns a
@@ -408,6 +415,17 @@ int flow_member_system_matvec(skb_flow *fl, skb_dense *dn, const double *d_x_fib
 int flow_member_system_precondition(skb_flow *fl, skb_dense *dn, const double *d_x_fib, const double *d_x_shell,
                                     const double *d_x_bodies, double *d_y_fib, double *d_y_shell, double *d_y_bodies,
                                     cudaStream_t st);
+// The system RHS (skb_flow_build_system_rhs) on a member; params / v_growth / force_scale of ALL fibers.
+// flow_member_rhs_prepare, on the calling thread before any member launches: the refusals (the member's fibers and
+// bodies), the upload of the fiber block's per-fiber tables, and every buffer and kernel the call uses.
+// flow_member_system_rhs on st: d_fext 3 per own fiber node or NULL, d_f / d_t 3 per body (complete) or NULL; the
+// outputs as flow_member_system_matvec's
+int flow_member_rhs_prepare(skb_flow *fl, const ::skb_fiber_params *params, const double *v_growth,
+                            const double *force_scale, double dt, double eta);
+int flow_member_system_rhs(skb_flow *fl, const ::skb_fiber_params *params, const double *v_growth,
+                           const double *force_scale, const double *d_fext, const double *d_f, const double *d_t,
+                           double dt, double eta, double *d_rhs_fib, double *d_rhs_shell, double *d_rhs_bodies,
+                           cudaStream_t st);
 } // namespace skb
 
 // ---- context internals (shared by skb_runtime.cu and skb_matvec.cu) ----

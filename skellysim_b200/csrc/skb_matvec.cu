@@ -113,6 +113,8 @@ struct skb_flow {
     // staging
     DevBuf in_fib, in_shell, in_body, in_force, in_torque, vel, tmp, x_fib, res_fib, vb, res_shell, tmp_b;
     DevBuf sys_x, sys_y; // the whole solution vector in and out of the host forms of the system operator
+    DevBuf zeros;        // the system RHS: the zero densities (and absent forces) its flow takes, n_zeros doubles
+    long long n_zeros = 0;
     skb_flow_stats stats{};
     int launches = 0;
     long long pairs = 0;
@@ -213,6 +215,32 @@ static int bodies_dev(skb_flow *fl, skb_ctx *ctx, const double *d_density, const
         1.0 / (8.0 * M_PI * eta), kReg * kReg, kEps * kEps, d_vel);
     fl->pairs += (fl->n_body + 2 * (long long)fl->n_bodies) * d.n_trg;
     return launched(fl, 1);
+}
+
+// + psc.flow(r_trg, eta, time) + bs.flow(r_trg, eta) (system.cpp:358-359, 445-446) on st: the point sources of
+// skb_flow_set_point_sources and the background flow of skb_flow_set_background at the n_trg targets d_trg, added to
+// the rows of d_v in this order: Oseen contraction, rotlet, background
+static int add_sources(skb_flow *fl, const double *d_trg, long long n_trg, double eta, double *d_v, cudaStream_t st) {
+    const int bs = 128;
+    const unsigned nblk = (unsigned)((n_trg + bs - 1) / bs);
+    if (n_trg == 0)
+        return SKB_OK;
+    if (fl->n_points > 0) {
+        oseen_contract_add_kernel<<<nblk, bs, 0, st>>>((const double *)fl->pt_pos.ptr, (const double *)fl->pt_force.ptr,
+                                                       fl->n_points, d_trg, n_trg, 1.0 / (8.0 * M_PI * eta),
+                                                       kReg * kReg, kEps, d_v);
+        rotlet_add_kernel<<<nblk, bs, 0, st>>>((const double *)fl->pt_pos.ptr, (const double *)fl->pt_torque.ptr,
+                                               fl->n_points, d_trg, n_trg, 1.0 / (8.0 * M_PI * eta), kReg * kReg,
+                                               kEps * kEps, d_v);
+        SKB_TRY(launched(fl, 2));
+    }
+    if (fl->has_background) {
+        background_add_kernel<<<nblk, bs, 0, st>>>(d_trg, n_trg, fl->bg_comp[0], fl->bg_comp[1], fl->bg_comp[2],
+                                                   fl->bg_scale[0], fl->bg_scale[1], fl->bg_scale[2],
+                                                   fl->bg_uniform[0], fl->bg_uniform[1], fl->bg_uniform[2], d_v);
+        SKB_TRY(launched(fl, 1));
+    }
+    return SKB_OK;
 }
 
 static int upload(skb_flow *fl, DevBuf &buf, const double *h, size_t n_doubles) {
@@ -698,27 +726,7 @@ int skb_flow_velocity_at_targets(skb_flow *fl, const double *r_trg, int64_t n_tr
                            (const double *)fl->in_torque.ptr, eta, d_v, 1));
         SKB_TRY(periphery_dev(fl, fl->shell[0].get(), kNormalDensity, (const double *)fl->in_shell.ptr, eta, d_v, 1));
         // + psc_.flow(r_trg, eta, time) + bs_.flow(r_trg, eta)                                  system.cpp:358-359
-        const double *d_trg = (const double *)fl->fib[0]->devs[0].r_trg.ptr;
-        const int bs = 128;
-        const unsigned nblk = (unsigned)((n_trg + bs - 1) / bs);
-        if (fl->n_points > 0) {
-            oseen_contract_add_kernel<<<nblk, bs, 0, fl->stream>>>((const double *)fl->pt_pos.ptr,
-                                                                   (const double *)fl->pt_force.ptr, fl->n_points,
-                                                                   d_trg, n_trg, 1.0 / (8.0 * M_PI * eta),
-                                                                   kReg * kReg, kEps, d_v);
-            rotlet_add_kernel<<<nblk, bs, 0, fl->stream>>>((const double *)fl->pt_pos.ptr,
-                                                           (const double *)fl->pt_torque.ptr, fl->n_points, d_trg,
-                                                           n_trg, 1.0 / (8.0 * M_PI * eta), kReg * kReg, kEps * kEps,
-                                                           d_v);
-            SKB_TRY(launched(fl, 2));
-        }
-        if (fl->has_background) {
-            background_add_kernel<<<nblk, bs, 0, fl->stream>>>(d_trg, n_trg, fl->bg_comp[0], fl->bg_comp[1],
-                                                               fl->bg_comp[2], fl->bg_scale[0], fl->bg_scale[1],
-                                                               fl->bg_scale[2], fl->bg_uniform[0], fl->bg_uniform[1],
-                                                               fl->bg_uniform[2], d_v);
-            SKB_TRY(launched(fl, 1));
-        }
+        SKB_TRY(add_sources(fl, (const double *)fl->fib[0]->devs[0].r_trg.ptr, n_trg, eta, d_v, fl->stream));
         return download(fl, s.v, fl->vel, (size_t)n_trg * 3);
     };
     if (!s.pinned)
@@ -1828,6 +1836,156 @@ int skb_flow_apply_system_preconditioner_device(skb_flow *fl, skb_dense *dn, con
 
 } // extern "C"
 
+// ---- the right-hand side of the whole system (System::prep_state_for_solver, system.cpp:398-458) --------------------
+// One device call from the external forces to the RHS vector [fibers | shell | bodies], laid out as Solver::set_RHS
+// copies it (solver_hydro.cpp:51-61).  Its flow is matvec_core unchanged -- f_ext as the fiber strengths, zero periphery
+// and body densities, the bodies' external F_T -- so that the symmetric and cross kernels, the self term and, in a
+// group, the exchange through the window serve it as they serve the matvec.
+
+// the zero densities of the RHS flow (and the zero forces it takes for an absent f_external or F_T), the velocities,
+// and the kernels the call launches besides matvec_core's, loaded now (the first launch of a group member must not load
+// a kernel lazily while a peer on the same device spins on a flag)
+static int rhs_buffers(skb_flow *fl) {
+    const long long n = std::max<long long>({3 * (fl->fb - fl->fa), 3 * (fl->sb - fl->sa), 3 * fl->n_body,
+                                             3LL * fl->n_bodies, 1LL});
+    SKB_TRY(fl->zeros.ensure((size_t)n * 8));
+    fl->n_zeros = n;
+    SKB_TRY(fl->vel.ensure((size_t)fl->n_win * 24 + 8));
+    cudaFuncAttributes fa;
+    CUDA_TRY(cudaFuncGetAttributes(&fa, oseen_contract_add_kernel));
+    CUDA_TRY(cudaFuncGetAttributes(&fa, rotlet_add_kernel));
+    CUDA_TRY(cudaFuncGetAttributes(&fa, background_add_kernel));
+    return load_rhs_rows_kernel();
+}
+
+// System::prep_state_for_solver's RHS (system.cpp:421-455) on fl->cur, the rows of this flow's target list: d_fext 3 per
+// own fiber node or NULL (no external fiber force), d_f / d_t 3 per body, complete, or NULL (zero); d_rhs_fib 4 per own
+// fiber node, d_rhs_shell 3 per own periphery row, d_rhs_bodies in the x_bodies layout (the rows BodyOps owns written).
+// params / v_growth / force_scale per own fiber.  Every check, the fiber block's included, precedes the first launch.
+static int system_rhs_core(skb_flow *fl, OwnFibers own, const skb_fiber_params *params, const double *v_growth,
+                           const double *force_scale, const double *d_fext, const double *d_f, const double *d_t,
+                           double dt, double eta, double *d_rhs_fib, double *d_rhs_shell, double *d_rhs_bodies) {
+    const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
+    double *d_v = (double *)fl->vel.ptr;
+    const double *zero = (const double *)fl->zeros.ptr;
+    own.stream = fl->cur;
+    fl->bg.dn = nullptr; // no dense operator: nothing goes to the background streamer
+    fl->bg.launched = false;
+    auto run = [&](const FiberOps::Step *stage, const FiberOps::Step *launch) -> int {
+        if (stage) // the fiber block's per-fiber tables
+            SKB_TRY((*stage)());
+        CUDA_TRY(cudaMemsetAsync(fl->zeros.ptr, 0, (size_t)fl->n_zeros * 8, fl->cur));
+        // v_all = fc.flow(r_all, f_ext, eta), self term subtracted (system.cpp:425), + bc.flow(r_all, 0, F_T, eta)
+        // (:442).  F_T are complete on every member and go straight to the body flow (no ft_exchange): each counts once
+        SKB_TRY(matvec_core(fl, d_fext ? d_fext : zero, zero, zero, d_f ? d_f : zero, d_t ? d_t : zero, eta, d_v));
+        // v_all += psc.flow + bs.flow (:445-446).  The body evaluator's matvec targets are the rows of d_v, in its order
+        SKB_TRY(add_sources(fl, (const double *)fl->body[1]->devs[0].r_trg.ptr, fl->n_win, eta, d_v, fl->cur));
+        // fc.update_rhs(dt, v_fibers, motor + f_ext) + fc.apply_bcs(dt, v_fibers, f_ext) (:451-453)
+        if (launch)
+            SKB_TRY((*launch)());
+        // bc.update_RHS(v_bodies), shell.update_RHS(v_shell) (:448, 455)
+        return fl->bodies.rhs_rows(fl->n_bodies > 0, d_v + 3 * (n_fw + n_sw), d_rhs_bodies, d_v + 3 * n_fw, n_sw,
+                                   d_rhs_shell, fl->cur, &fl->launches);
+    };
+    bool framed = false; // FiberOps::rhs calls the frame only when there are own fibers
+    SKB_TRY(fl->ops.rhs(own, params, v_growth, force_scale, d_v, d_fext, dt, eta, d_rhs_fib, &fl->launches,
+                        [&](const FiberOps::Step &stage, const FiberOps::Step &launch) {
+                            framed = true;
+                            return run(&stage, &launch);
+                        }));
+    return framed ? SKB_OK : run(nullptr, nullptr);
+}
+
+static int finite(const double *a, size_t n) {
+    for (size_t i = 0; i < n; ++i)
+        if (!std::isfinite(a[i]))
+            return 0;
+    return 1;
+}
+
+// the refusals of the two skb_flow forms, before any launch; then the own fibers, the flow's device current, the
+// buffers sized
+static int system_rhs_args(skb_flow *fl, const char *who, const skb_fiber_params *params, bool out, double dt,
+                           double eta, OwnFibers &own) {
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    if (fl->grp.member())
+        return set_error(SKB_ERR_INVALID, "%s: a group member's rows need the others' fiber forces; over several devices "
+                                          "use skb_mflow_build_system_rhs", who);
+    if (!(dt > 0) || !(eta > 0))
+        return set_error(SKB_ERR_INVALID, "%s: dt = %g, eta = %g (both must be > 0)", who, dt, eta);
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    SKB_TRY(own_fibers(fl, who, own));
+    const long long n_all = fl->n_fib + fl->n_shell + fl->n_body;
+    if (fl->n_win != n_all)
+        return set_error(SKB_ERR_INVALID, "%s: needs the whole target list (%lld of %lld rows are set by a target window "
+                                          "or ranges); over several devices use skb_mflow_build_system_rhs", who,
+                         fl->n_win, n_all);
+    if (fl->n_bodies > 0 && !fl->bodies.has_operators())
+        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_body_operators after skb_flow_set_bodies (the body rows "
+                                          "are laid out by its node counts)", who);
+    if ((own.count() > 0 && !params) || (solution_size(fl) > 0 && !out))
+        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
+    begin_stats(fl);
+    return rhs_buffers(fl);
+}
+
+extern "C" {
+
+int skb_flow_build_system_rhs(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
+                              const double *force_scale, const double *f_external, const double *body_forces_torques,
+                              double dt, double eta, double *rhs) {
+    const char *who = "skb_flow_build_system_rhs";
+    OwnFibers own;
+    SKB_TRY(system_rhs_args(fl, who, params, rhs != nullptr, dt, eta, own));
+    const long long nf = fl->n_fib, ns = fl->n_shell;
+    if ((f_external && !finite(f_external, (size_t)nf * 3)) ||
+        (body_forces_torques && !finite(body_forces_torques, (size_t)fl->n_bodies * 6)))
+        return set_error(SKB_ERR_INVALID, "%s: a non-finite external force or torque", who);
+    const size_t n = (size_t)solution_size(fl);
+    if (n == 0)
+        return SKB_OK;
+    std::vector<double> f, t;
+    if (body_forces_torques && fl->n_bodies > 0)
+        split_forces_torques(body_forces_torques, fl->n_bodies, f, t);
+    SKB_TRY(fl->sys_y.ensure(n * 8));
+    double *d_rhs = (double *)fl->sys_y.ptr;
+    return host_frame(
+        fl,
+        [&]() -> int {
+            if (f_external)
+                SKB_TRY(upload(fl, fl->in_fib, f_external, (size_t)nf * 3));
+            SKB_TRY(upload(fl, fl->in_force, f.data(), f.size()));
+            return upload(fl, fl->in_torque, t.data(), t.size());
+        },
+        [&] {
+            return system_rhs_core(fl, own, params, v_growth, force_scale,
+                                   f_external && nf ? (const double *)fl->in_fib.ptr : nullptr,
+                                   f.empty() ? nullptr : (const double *)fl->in_force.ptr,
+                                   t.empty() ? nullptr : (const double *)fl->in_torque.ptr, dt, eta, d_rhs,
+                                   d_rhs + 4 * nf, d_rhs + 4 * nf + 3 * ns);
+        },
+        [&] { return download(fl, rhs, fl->sys_y, n); });
+}
+
+int skb_flow_build_system_rhs_device(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
+                                     const double *force_scale, const double *d_f_external,
+                                     const double *d_body_forces, const double *d_body_torques, double dt, double eta,
+                                     double *d_rhs, void *stream) {
+    OwnFibers own;
+    SKB_TRY(system_rhs_args(fl, "skb_flow_build_system_rhs_device", params, d_rhs != nullptr, dt, eta, own));
+    if (solution_size(fl) == 0)
+        return SKB_OK;
+    const long long nf = fl->n_fib, ns = fl->n_shell;
+    fl->cur = (cudaStream_t)stream;
+    SKB_TRY(system_rhs_core(fl, own, params, v_growth, force_scale, nf ? d_f_external : nullptr,
+                            fl->n_bodies ? d_body_forces : nullptr, fl->n_bodies ? d_body_torques : nullptr, dt, eta,
+                            d_rhs, d_rhs + 4 * nf, d_rhs + 4 * nf + 3 * ns));
+    return device_stats(fl);
+}
+
+} // extern "C"
+
 // ---- the whole-vector operator on a member of skb_mflow (skb_internal.hpp) ---------------------------------------
 // A member holds its own fibers' links and its body rows' operators (BodyOps); x_bodies is complete on every member.
 // The bodies' link forces are exchanged inside matvec_core (ft_exchange); a single flow (a one-device skb_mflow) takes
@@ -1919,6 +2077,45 @@ int skb::flow_member_system_precondition(skb_flow *fl, skb_dense *dn, const doub
     }
     if (fl->n_bodies > 0)
         SKB_TRY(fl->bodies.precondition(d_x_bodies, d_y_bodies, st, &fl->launches));
+    return device_stats(fl);
+}
+
+// a member's slice of a per-fiber array of ALL fibers (NULL stays NULL, and so does the slice of no fibers)
+template <class T> static const T *own_slice(const T *all, const OwnFibers &own) {
+    return all && own.count() > 0 ? all + own.f0 : nullptr;
+}
+
+int skb::flow_member_rhs_prepare(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
+                                 const double *force_scale, double dt, double eta) {
+    const char *who = "skb_mflow_build_system_rhs";
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    OwnFibers own;
+    SKB_TRY(own_fibers(fl, who, own));
+    if (fl->n_bodies > 0 && !fl->bodies.has_operators())
+        return set_error(SKB_ERR_INVALID, "%s: call skb_mflow_set_body_operators after skb_mflow_set_bodies", who);
+    SKB_TRY(rhs_buffers(fl));
+    // the fiber block's checks, and its tables uploaded once so that their buffers have their size before any launch
+    return fl->ops.rhs(own, own_slice(params, own), own_slice(v_growth, own), own_slice(force_scale, own), nullptr,
+                       nullptr, dt, eta, nullptr, &fl->launches,
+                       [&](const FiberOps::Step &stage, const FiberOps::Step &) -> int {
+                           SKB_TRY(stage());
+                           CUDA_TRY(cudaStreamSynchronize(own.stream));
+                           return SKB_OK;
+                       });
+}
+
+int skb::flow_member_system_rhs(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
+                                const double *force_scale, const double *d_fext, const double *d_f, const double *d_t,
+                                double dt, double eta, double *d_rhs_fib, double *d_rhs_shell, double *d_rhs_bodies,
+                                cudaStream_t st) {
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    begin_stats(fl);
+    fl->cur = st;
+    OwnFibers own;
+    SKB_TRY(own_fibers(fl, "skb_mflow_build_system_rhs", own));
+    SKB_TRY(system_rhs_core(fl, own, own_slice(params, own), own_slice(v_growth, own), own_slice(force_scale, own),
+                            fl->fb > fl->fa ? d_fext : nullptr, d_f, d_t, dt, eta, d_rhs_fib, d_rhs_shell,
+                            d_rhs_bodies));
     return device_stats(fl);
 }
 

@@ -8,6 +8,7 @@
 #include "../../include/skelly_b200_dense.h"
 
 #include <algorithm>
+#include <cmath>
 #include <condition_variable>
 #include <functional>
 #include <memory>
@@ -782,6 +783,84 @@ int skb_mflow_apply_system_preconditioner(skb_mflow *mf, const double *x, double
         return SKB_OK;
     }));
     return mflow_collect_stats(mf);
+}
+
+// System::prep_state_for_solver's RHS (system.cpp:398-458) over n devices: every member forms its own rows of the
+// whole vector.  The flow is the group's matvec flow (strengths pushed to every window, the members' partial sums pulled
+// together); the bodies' external F_T are complete on every member and enter the body flow as they are.
+int skb_mflow_build_system_rhs(skb_mflow *mf, const skb_fiber_params *params, const double *v_growth,
+                               const double *force_scale, const double *f_external, const double *body_forces_torques,
+                               double dt, double eta, double *rhs) {
+    const char *who = "skb_mflow_build_system_rhs";
+    if (!mf)
+        return set_error(SKB_ERR_INVALID, "%s: NULL", who);
+    if (!(dt > 0) || !(eta > 0))
+        return set_error(SKB_ERR_INVALID, "%s: dt = %g, eta = %g (both must be > 0)", who, dt, eta);
+    SKB_TRY(mflow_prepare(mf));
+    auto finite = [](const double *a, size_t n) {
+        for (size_t i = 0; i < n; ++i)
+            if (!std::isfinite(a[i]))
+                return false;
+        return true;
+    };
+    if ((f_external && !finite(f_external, (size_t)mf->n_fib * 3)) ||
+        (body_forces_torques && !finite(body_forces_torques, (size_t)mf->n_bodies * 6)))
+        return set_error(SKB_ERR_INVALID, "%s: a non-finite external force or torque", who);
+    if (mf->n_fibers > 0 && !params)
+        return set_error(SKB_ERR_INVALID, "%s: NULL params", who);
+    // every member's checks and buffers, on this thread, before any member launches (a refusal after a peer had pushed
+    // its strengths would leave that peer waiting on a flag)
+    for (int g = 0; g < mf->n; ++g)
+        SKB_TRY(flow_member_rhs_prepare(mf->m[g].get(), params, v_growth, force_scale, dt, eta));
+    const long long n = mflow_solution_size(mf);
+    if (n > 0 && !rhs)
+        return set_error(SKB_ERR_INVALID, "%s: NULL rhs", who);
+    if (n == 0)
+        return SKB_OK;
+    std::vector<double> f, t;
+    if (body_forces_torques && mf->n_bodies > 0)
+        split_forces_torques(body_forces_torques, mf->n_bodies, f, t);
+    SKB_TRY(mflow_size_io(mf, f.size(), true));
+    SKB_TRY(mf->workers->run([&](int g) -> int {
+        skb_flow *fl = mf->m[g].get();
+        skb_mflow::IO &io = mf->io[g];
+        CUDA_TRY(cudaSetDevice(mf->devs[g]));
+        const MemberRows r = member_rows(mf, g);
+        cudaStream_t st = flow_stream(fl);
+        SKB_TRY(put(io.ff, f_external ? f_external + 3 * r.a : nullptr, (size_t)r.n_fw * 3, st));
+        SKB_TRY(put(io.f, f.data(), f.size(), st));
+        SKB_TRY(put(io.t, t.data(), t.size(), st));
+        CUDA_TRY(cudaEventRecord(io.e0, st));
+        SKB_TRY(flow_member_system_rhs(fl, params, v_growth, force_scale,
+                                       f_external ? (const double *)io.ff.ptr : nullptr,
+                                       f.empty() ? nullptr : (const double *)io.f.ptr,
+                                       t.empty() ? nullptr : (const double *)io.t.ptr, dt, eta, (double *)io.res.ptr,
+                                       (double *)io.outs.ptr, (double *)io.rb.ptr, st));
+        CUDA_TRY(cudaEventRecord(io.e1, st));
+        SKB_TRY(mflow_download_rows(mf, g, rhs, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        return SKB_OK;
+    }));
+    return mflow_collect_stats(mf);
+}
+
+// the analytic sources of velocity_at_targets and of the system RHS, on every member
+int skb_mflow_set_point_sources(skb_mflow *mf, const double *positions, const double *forces, const double *torques,
+                                int n_points) {
+    if (!mf)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_set_point_sources: NULL");
+    for (int g = 0; g < mf->n; ++g)
+        SKB_TRY(skb_flow_set_point_sources(mf->m[g].get(), positions, forces, torques, n_points));
+    return SKB_OK;
+}
+
+int skb_mflow_set_background(skb_mflow *mf, const int *components, const double *scale_factor,
+                             const double *uniform) {
+    if (!mf)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_set_background: NULL");
+    for (int g = 0; g < mf->n; ++g)
+        SKB_TRY(skb_flow_set_background(mf->m[g].get(), components, scale_factor, uniform));
+    return SKB_OK;
 }
 
 // System::velocity_at_targets (system.cpp:330-384) over n devices: the targets are block-partitioned, every device

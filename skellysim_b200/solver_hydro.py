@@ -14,7 +14,8 @@ periphery block a row-block GEMV with M_inv (skb_dense_apply_device), the operat
 skb_flow_apply_matvec_device.  HydroOperator leaves the body block to the caller: `apply` hands back the velocities at
 the body nodes and takes the body densities / link forces as (small) device tensors.  SystemOperator does not: it
 applies A and P^-1 to whole solution vectors [fibers | shell | bodies] with the body block and the fiber-body links on
-the device as well (skb_flow_apply_system_matvec_device / _preconditioner_device).
+the device as well (skb_flow_apply_system_matvec_device / _preconditioner_device), and builds the right-hand side of
+the solve there too (skb_flow_build_system_rhs_device).
 
 This module sequences calls and owns work vectors; it computes nothing itself.  torch is used for device memory only.
 """
@@ -115,6 +116,21 @@ class SystemOperator:
         """System::apply_preconditioner (system.cpp:248-262): P^-1 x -- a view valid until the next call."""
         self.flow.apply_system_preconditioner_device(self.dense, x.data_ptr(), self.y.data_ptr(), self._stream())
         return self.y[:self.n]
+
+    def rhs(self, fiber_params, dt: float, f_external=None, body_forces=None, body_torques=None, v_growth=None,
+            force_scale=None):
+        """System::prep_state_for_solver's RHS (system.cpp:398-458), Solver::set_RHS's vector (solver_hydro.cpp:51-61):
+        a new device tensor of solution_size().  fiber_params: the 7 per-fiber parameters of
+        capi.Flow.build_fiber_operators (length_prev ... plus_hinged); f_external (N_f, 3), body_forces / body_torques
+        (n_bodies, 3): device tensors or None (zero)."""
+        torch = self.torch
+        out = torch.empty(max(self.n, 1), dtype=torch.float64, device=self.res.device)
+        p = lambda t: t.data_ptr() if t is not None and t.numel() else 0
+        self.flow.build_system_rhs_device(*fiber_params, dt, self.eta, p(f_external), p(body_forces), p(body_torques),
+                                          out.data_ptr(), v_growth=v_growth, force_scale=force_scale,
+                                          stream=self._stream())
+        self.launches = self.flow.stats()["launches"]
+        return out[:self.n]
 
 
 def iterate_system(op: SystemOperator, x, n_iter: int):
