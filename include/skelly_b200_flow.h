@@ -349,7 +349,8 @@ SKB_API int skb_flow_apply_matvec_device(skb_flow *fl, struct skb_dense *dn, con
  *   like the fibers').
  * The host forms ship x once and res / y once; the _device forms are asynchronous on `stream`.  All four refuse
  * (SKB_ERR_INVALID, before any launch, earlier state untouched): a group member or a flow whose target window / ranges
- * do not cover every row (over several devices use skb_mflow_set_body_operators and its siblings below), fiber operators not resident (with their inverse for the preconditioner), bodies without
+ * do not cover every row (over several devices use skb_mflow_set_body_operators and its siblings below, or on one process
+ * per GPU the skb_flow_group_* calls above), fiber operators not resident (with their inverse for the preconditioner), bodies without
  * skb_flow_set_body_operators, fibers and bodies without skb_flow_set_fiber_links (matvec), no A_inv (preconditioner),
  * dn == NULL or of the wrong shape with periphery nodes present.  The results are bitwise reproducible run to run: the
  * bodies' link forces are added per body in container order, without atomics. */
@@ -382,7 +383,7 @@ SKB_API int skb_flow_apply_system_preconditioner_device(skb_flow *fl, struct skb
  * earlier state untouched): what skb_flow_build_fiber_rhs refuses, NULL params or rhs where there are fibers or
  * entries, a non-finite external force or torque (host forms: the _device form does not read its inputs on the host),
  * bodies without body operators, a group member, a target window or ranges that do not cover every row (over several
- * devices use skb_mflow_build_system_rhs).
+ * devices use skb_mflow_build_system_rhs, or on one process per GPU skb_flow_group_build_system_rhs_device).
  * The _device form follows skb_flow_build_fiber_rhs_device: everything on this flow's device, asynchronous on `stream`,
  * the per-fiber tables from host memory; d_body_forces / d_body_torques 3 x n_bodies each (as skb_flow_matvec_device),
  * either NULL for zero. */
@@ -393,6 +394,63 @@ SKB_API int skb_flow_build_system_rhs_device(skb_flow *fl, const skb_fiber_param
                                              const double *force_scale, const double *d_f_external,
                                              const double *d_body_forces, const double *d_body_torques, double dt,
                                              double eta, double *d_rhs, void *stream);
+
+/* ---- the whole-vector calls on one rank per GPU ---------------------------------------------------------------------
+ * A group member (skb_flow_group_init ... skb_flow_group_warmup above) applies A, P^-1 and builds the RHS on its LOCAL
+ * vector: its own rows of the whole vector [fibers | shell | bodies], in ascending global order --
+ *   x_local = [4 per own fiber node | 3 per own periphery row | own body rows],
+ * the own body rows being the 3 rows of each body node in its body rows [b0, b1) (skb_flow_set_target_ranges) and the
+ * six rows [U; w] of every body whose FIRST node lies in [b0, b1) (the rows of skb_mflow_apply_system_matvec,
+ * distributed.system_rows; skb_group_body_pieces gives their places).  The members' local vectors tile the whole vector
+ * once; no rank needs a full-length vector.  Every member stores its own body rows (for the preconditioner also its own
+ * periphery rows) into all windows and meets its peers at a flag before it reads the complete x_bodies / x_shell from
+ * its own window; the rest is the protocol of skb_mflow, and the results are bitwise those of skb_mflow on the same
+ * device list.
+ *   skb_flow_group_set_body_operators: the arrays of ALL bodies, as skb_flow_set_body_operators (bodies are complete on
+ *     every member); the member keeps the inverses of the bodies it owns rows of, lays out its body rows, and sizes every
+ *     buffer the three calls below use, for the member's current target ranges (all six of them).  After
+ *     skb_flow_group_init and the target ranges; a change of the ranges wants the group set up again (init, the
+ *     handle exchange, the warm-up) and then this call, or the three calls below refuse.
+ *   skb_flow_group_set_fiber_links: body / site / bending_rigidity of the OWN fibers (as every per-fiber array under
+ *     target ranges), otherwise as skb_flow_set_fiber_links.
+ *   skb_flow_group_apply_system_matvec_device: d_res_local = the own rows of A x; dn holds the member's rows of
+ *     SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY (3 n_own_shell x 3 N_s, skb_dense_create_on this flow's device; may be
+ *     NULL without own periphery rows).
+ *   skb_flow_group_apply_system_preconditioner_device: d_y_local = the own rows of P^-1 x; dn holds the member's rows of
+ *     SKB_DENSE_M_INV.
+ *   skb_flow_group_build_system_rhs_device: d_rhs_local = the own rows of the RHS; params / v_growth / force_scale of
+ *     the OWN fibers, d_f_external 3 per own fiber node or NULL, d_body_forces / d_body_torques complete (3 x n_bodies
+ *     each, as skb_flow_build_system_rhs_device) or NULL: they enter the body flow as they are, once.
+ * All three are asynchronous on `stream`; consecutive calls of a member must be ordered (one stream, or the caller's
+ * events).  Every member must make the same sequence of calls, as with any collective.  A refusal (SKB_ERR_INVALID /
+ * SKB_ERR_STATE, before any launch, earlier state untouched) is LOCAL to the rank that refused: the refusals of the
+ * single-device twins, a dense block that does not fit the member's rows and the current periphery, no
+ * skb_flow_group_set_body_operators for the member's current target ranges (fiber, periphery AND body rows), a member whose peers are not all
+ * connected.  A rank that goes on after a peer refused waits on a flag until the time-out (skb_flow_group_error), so a
+ * caller agrees on the set-up calls' return codes (e.g. an all-reduce) before the first apply.  None of the three
+ * allocates device memory: the set-up calls and the warm-up sized everything, so no cudaMalloc / cudaFree meets a
+ * peer's flag wait on the same device.  On a flow that is not a group member the five calls are the single-device
+ * calls (whole vector, bitwise). */
+SKB_API int skb_flow_group_set_body_operators(skb_flow *fl, const int *n_nodes, int n_bodies,
+                                              const double *node_weights, const double *ex, const double *ey,
+                                              const double *ez, const double *A_inv);
+SKB_API int skb_flow_group_set_fiber_links(skb_flow *fl, const int *body, const double *site,
+                                           const double *bending_rigidity);
+SKB_API int skb_flow_group_apply_system_matvec_device(skb_flow *fl, struct skb_dense *dn, const double *d_x_local,
+                                                      double eta, double *d_res_local, void *stream);
+SKB_API int skb_flow_group_apply_system_preconditioner_device(skb_flow *fl, struct skb_dense *dn,
+                                                              const double *d_x_local, double *d_y_local,
+                                                              void *stream);
+SKB_API int skb_flow_group_build_system_rhs_device(skb_flow *fl, const skb_fiber_params *params,
+                                                   const double *v_growth, const double *force_scale,
+                                                   const double *d_f_external, const double *d_body_forces,
+                                                   const double *d_body_torques, double dt, double eta,
+                                                   double *d_rhs_local, void *stream);
+/* host-only (no GPU needed): the places of a member's own body rows [body_begin, body_end) -- as runs of consecutive
+ * entries, 3 int64 per run: offset in the local vector's body part, offset in the whole vector's body part, length.
+ * *n_pieces = the number of runs (at most 3); refused if it exceeds max_pieces. */
+SKB_API int skb_group_body_pieces(const int *n_nodes, int n_bodies, int64_t body_begin, int64_t body_end,
+                                  int64_t *pieces, int max_pieces, int *n_pieces);
 
 typedef struct skb_flow_stats {
     double device_ms;   /* CUDA-event time of the last call, first launch to last kernel (copies excluded) */

@@ -208,6 +208,16 @@ def library() -> C.CDLL:
                                              + [C.c_double, C.c_double, C.c_void_p, C.c_void_p], C.c_int),
         "skb_mflow_build_system_rhs": ([ctxp, C.POINTER(FiberParams), _dp, _dp, _dp, _dp, C.c_double, C.c_double, _dp],
                                        C.c_int),
+        "skb_flow_group_set_body_operators": ([ctxp, C.POINTER(C.c_int), C.c_int, _dp, _dp, _dp, _dp, _dp], C.c_int),
+        "skb_flow_group_set_fiber_links": ([ctxp, C.POINTER(C.c_int), _dp, _dp], C.c_int),
+        "skb_flow_group_apply_system_matvec_device": ([ctxp, ctxp, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p],
+                                                      C.c_int),
+        "skb_flow_group_apply_system_preconditioner_device": ([ctxp, ctxp, C.c_void_p, C.c_void_p, C.c_void_p],
+                                                              C.c_int),
+        "skb_flow_group_build_system_rhs_device": ([ctxp, C.POINTER(FiberParams), _dp, _dp] + [C.c_void_p] * 3
+                                                   + [C.c_double, C.c_double, C.c_void_p, C.c_void_p], C.c_int),
+        "skb_group_body_pieces": ([C.POINTER(C.c_int), C.c_int, C.c_int64, C.c_int64, C.POINTER(C.c_int64), C.c_int,
+                                   C.POINTER(C.c_int)], C.c_int),
         "skb_mflow_set_point_sources": ([ctxp, _dp, _dp, _dp, C.c_int], C.c_int),
         "skb_mflow_set_background": ([ctxp, C.POINTER(C.c_int), _dp, _dp], C.c_int),
     }
@@ -935,6 +945,60 @@ class Flow:
         _check(library().skb_flow_group_error(self._h, C.byref(m)))
         return m.value
 
+    # ---- the whole-vector calls of one rank per GPU, on the member's local vector ----
+    def group_set_body_operators(self, n_nodes, node_weights, ex, ey, ez, A_inv_list=None):
+        """set_body_operators on a group member (arrays of ALL bodies): it keeps what its body rows need, lays out its
+        local vector's body rows and sizes the buffers of the group_* system calls.  Not a member: set_body_operators."""
+        n = np.ascontiguousarray(n_nodes, dtype=np.int32)
+        w = np.ascontiguousarray(node_weights, dtype=np.float64).reshape(-1)
+        ex, ey, ez = _arr(ex, 3), _arr(ey, 3), _arr(ez, 3)
+        Ai = None if A_inv_list is None else self._colmajor_concat(A_inv_list)
+        _check(library().skb_flow_group_set_body_operators(self._h, n.ctypes.data_as(C.POINTER(C.c_int)),
+                                                           int(n.shape[0]), _p(w), _p(ex), _p(ey), _p(ez),
+                                                           None if Ai is None else _p(Ai)))
+        self._body_sol = int(np.sum(3 * n + 6))
+
+    def group_set_fiber_links(self, body=None, site=None, bending_rigidity=None):
+        """set_fiber_links on a group member: body index, nucleation site (n, 3) and bending_rigidity_ of the OWN
+        fibers; body=None: none of them is bound."""
+        if body is None:
+            _check(library().skb_flow_group_set_fiber_links(self._h, None, None, None))
+            return
+        b = np.ascontiguousarray(body, dtype=np.int32)
+        st = _arr(site, 3)
+        E = np.ascontiguousarray(np.broadcast_to(np.asarray(bending_rigidity, dtype=np.float64), b.shape))
+        assert st.shape[0] == b.shape[0]
+        _check(library().skb_flow_group_set_fiber_links(self._h, b.ctypes.data_as(C.POINTER(C.c_int)), _p(st), _p(E)))
+
+    def group_apply_system_matvec_device(self, dense, d_x_local: int, eta: float, d_res_local: int, stream: int = 0):
+        """the member's rows of A x from its rows of x (distributed.system_rows), asynchronous on `stream`"""
+        vp = lambda a: C.c_void_p(a) if a else None
+        _check(library().skb_flow_group_apply_system_matvec_device(self._h, dense._h if dense is not None else None,
+                                                                   vp(d_x_local), float(eta), vp(d_res_local),
+                                                                   vp(stream)))
+
+    def group_apply_system_preconditioner_device(self, dense, d_x_local: int, d_y_local: int, stream: int = 0):
+        """the member's rows of P^-1 x from its rows of x, asynchronous on `stream`"""
+        vp = lambda a: C.c_void_p(a) if a else None
+        _check(library().skb_flow_group_apply_system_preconditioner_device(
+            self._h, dense._h if dense is not None else None, vp(d_x_local), vp(d_y_local), vp(stream)))
+
+    def group_build_system_rhs_device(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
+                                      minus_clamped, plus_hinged, dt, eta, d_f_external: int, d_body_forces: int,
+                                      d_body_torques: int, d_rhs_local: int, v_growth=None, force_scale=None,
+                                      stream: int = 0):
+        """build_system_rhs_device on a group member: per-fiber arrays of the OWN fibers, f_external of their nodes,
+        forces and torques of ALL bodies ((n_bodies, 3) each; 0: none); the member's rows of the RHS."""
+        f0, f1 = self._own_fibers()
+        p, vg, fs, _, _ = _system_rhs_args(f1 - f0, 0, self.n_bodies,
+                                           (length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
+                                            minus_clamped, plus_hinged), v_growth, force_scale, None, None)
+        vp = lambda a: C.c_void_p(a) if a else None
+        _check(library().skb_flow_group_build_system_rhs_device(self._h, _params_ptr(p), _opt_p(vg), _opt_p(fs),
+                                                                vp(d_f_external), vp(d_body_forces),
+                                                                vp(d_body_torques), float(dt), float(eta),
+                                                                vp(d_rhs_local), vp(stream)))
+
     def stats(self) -> dict:
         s = FlowStats()
         _check(library().skb_flow_last_stats(self._h, C.byref(s)))
@@ -1252,6 +1316,18 @@ def partition_query(fiber_n_nodes, n_shell, n_body, n_members, member):
     _check(library().skb_partition_query(nn.ctypes.data_as(C.POINTER(C.c_int)), int(nn.shape[0]), int(n_shell),
                                          int(n_body), int(n_members), int(member), out))
     return tuple(int(v) for v in out)
+
+
+def group_body_pieces(body_n_nodes, body_begin, body_end):
+    """The places of a group member's own body rows [body_begin, body_end) (no GPU needed): an (n, 3) int64 array of
+    runs (offset in the local vector's body part, offset in the whole vector's body part, length), ascending."""
+    nn = np.ascontiguousarray(body_n_nodes, dtype=np.int32)
+    out = np.zeros((8, 3), dtype=np.int64)
+    k = C.c_int(0)
+    _check(library().skb_group_body_pieces(nn.ctypes.data_as(C.POINTER(C.c_int)), int(nn.shape[0]), int(body_begin),
+                                           int(body_end), out.ctypes.data_as(C.POINTER(C.c_int64)), out.shape[0],
+                                           C.byref(k)))
+    return out[:k.value].copy()
 
 
 def sym_groups_per_block() -> int:

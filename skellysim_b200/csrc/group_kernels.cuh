@@ -12,15 +12,18 @@
 // (5) PULL: every member adds up the partial velocities of its own fiber rows (and, with the cross kernel, of its own
 // periphery rows) from all windows (the reduce-scatter, fused with the accumulation into the velocity vector).
 // The whole-vector operator adds one store of the member's partial link forces into every window before (2) and one
-// rank-order sum of them after it.
+// rank-order sum of them after it.  A rank-per-GPU member's whole-vector calls (skb_flow_group_*) first store its own
+// rows of the solution vector -- body rows, and for the preconditioner periphery rows -- into every window and meet at
+// the rows phase, so that every member reads the complete x_bodies / x_shell from its own window.
 #pragma once
 #include <cuda_runtime.h>
 
-#include "skb_internal.hpp" // kMaxGroup
+#include "skb_internal.hpp" // kMaxGroup, kMaxRowPieces
 
 namespace skb {
 
-constexpr int kGroupPhases = 4;
+constexpr int kGroupPhases = 5;
+constexpr int kRowsPhase = 4; // the exchange of a member's own solution rows (skb_flow_group_* whole-vector calls)
 
 struct GroupPushArgs {
     // own fibers: raw forces -> weighted, into rows [fa, fa + n_f) of every member's f_sl
@@ -168,6 +171,67 @@ __global__ void group_ft_reduce_kernel(const GroupFtReduceArgs a) {
         a.f[i] = acc;
     else
         a.t[i - a.n3] = acc;
+}
+
+// ---- a member's own rows of the solution vector (skb_flow_group_* whole-vector calls) ----
+// The member's body rows are its local vector's body part, compacted in ascending global order; the piece table maps
+// them onto the body part of the whole vector: piece p covers local entries [local, local + len) and body-part entries
+// [body, body + len) (RowPieces, skb_internal.hpp: at most kMaxRowPieces, built when the body operators are set).
+struct RowPiecesDev {
+    long long local[kMaxRowPieces], body[kMaxRowPieces], len[kMaxRowPieces];
+    int n;
+    long long total; // sum of len
+};
+
+// the body-part offset of local entry i (the pieces ascend; unrolled over the table, so it stays in registers)
+__device__ __forceinline__ long long row_piece_offset(const RowPiecesDev &p, long long i) {
+    long long lo = p.local[0], bo = p.body[0];
+#pragma unroll
+    for (int k = 1; k < kMaxRowPieces; ++k)
+        if (k < p.n && p.local[k] <= i)
+            lo = p.local[k], bo = p.body[k];
+    return bo + (i - lo);
+}
+
+struct GroupRowsStoreArgs {
+    RowPiecesDev pieces;
+    const double *body;  // [pieces.total] the own body rows of the local vector
+    const double *shell; // [n_shell3] the own periphery rows (3 per row), NULL: none stored
+    long long shell_off, n_shell3; // -> x_shell entries [shell_off, shell_off + n_shell3)
+    int size;
+    double *x_body[kMaxGroup];
+    double *x_shell[kMaxGroup];
+};
+
+// the own rows into every window: body rows scattered to their place in x_body, periphery rows into x_shell
+__global__ void group_rows_store_kernel(const GroupRowsStoreArgs a) {
+    const long long nb = a.pieces.total, n = nb + a.n_shell3;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        if (i < nb) {
+            const double v = a.body[i];
+            const long long o = row_piece_offset(a.pieces, i);
+            for (int m = 0; m < a.size; ++m)
+                a.x_body[m][o] = v;
+        } else {
+            const long long s = i - nb;
+            const double v = a.shell[s];
+            for (int m = 0; m < a.size; ++m)
+                a.x_shell[m][a.shell_off + s] = v;
+        }
+    }
+}
+
+struct GroupRowsCompactArgs {
+    RowPiecesDev pieces;
+    const double *full; // a body output in the whole body layout
+    double *local;      // [pieces.total] the member's own rows of it
+};
+
+__global__ void group_rows_compact_kernel(const GroupRowsCompactArgs a) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < a.pieces.total)
+        a.local[i] = a.full[row_piece_offset(a.pieces, i)];
 }
 
 } // namespace skb

@@ -474,3 +474,9 @@ int skb_dense_last_stats(const skb_dense *dn, skb_dense_stats *out) {
 }
 
 } // extern "C"
+
+int skb::load_dense_kernels() {
+    cudaFuncAttributes fa;
+    CUDA_TRY(cudaFuncGetAttributes(&fa, dense_gemv_kernel));
+    return SKB_OK;
+}

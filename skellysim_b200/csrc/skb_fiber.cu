@@ -373,6 +373,16 @@ int FiberOps::rhs(const OwnFibers &own, const skb_fiber_params *params, const do
     return frame(stage, launch);
 }
 
+int FiberOps::size_rhs(int n_fibers) {
+    const size_t n = (size_t)std::max(n_fibers, 0);
+    SKB_TRY(rhs_items.ensure(n * sizeof(FiberItem)));
+    SKB_TRY(rhs_params.ensure(n * sizeof(skb_fiber_params)));
+    SKB_TRY(rhs_growth.ensure(n * sizeof(double2)));
+    if (!rhs_done)
+        CUDA_TRY(cudaEventCreateWithFlags(rhs_done.out(), cudaEventDisableTiming));
+    return SKB_OK;
+}
+
 int FiberOps::ready(const char *who, bool with_inverse) const {
     if (!ready_)
         return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_fiber_operators after skb_flow_set_fibers / "

@@ -21,7 +21,7 @@ static int launched(int *launches) {
 }
 
 int Group::init(int rank, int size, long long n_fib, long long n_pad_fib, long long n_shell, long long n_pad_shell,
-                int n_bodies) {
+                long long n_body, int n_bodies) {
     *this = Group(); // the old window and mappings are released here
     if (size == 1)
         return SKB_OK;
@@ -29,6 +29,7 @@ int Group::init(int rank, int size, long long n_fib, long long n_pad_fib, long l
     size_ = size;
     n_fib_ = n_fib;
     n_shell_ = n_shell;
+    n_body_ = n_body;
     n_bodies_ = n_bodies;
     size_t off = 0;
     auto take = [&](size_t bytes) {
@@ -42,6 +43,7 @@ int Group::init(int rank, int size, long long n_fib, long long n_pad_fib, long l
         lay_.f_shell[b] = take((size_t)n_pad_shell * 48 + 16);
         lay_.x_shell[b] = take((size_t)n_shell * 24 + 16);
         lay_.ft_part[b] = take((size_t)kMaxGroup * n_bodies * 48 + 16);
+        lay_.x_body[b] = take((size_t)n_body * 24 + (size_t)n_bodies * 48 + 16);
     }
     lay_.u_part = take((size_t)n_fib * 24 + 16);
     lay_.u_part_shell = take((size_t)n_shell * 24 + 16);
@@ -51,8 +53,13 @@ int Group::init(int rank, int size, long long n_fib, long long n_pad_fib, long l
     // loaded now, not lazily at their first launch, which would wait behind a peer on this device spinning on a flag
     // (the warm-up's solo matvec does not run them)
     cudaFuncAttributes fa;
+    CUDA_TRY(cudaFuncGetAttributes(&fa, group_flag_kernel));
+    CUDA_TRY(cudaFuncGetAttributes(&fa, group_push_kernel));
+    CUDA_TRY(cudaFuncGetAttributes(&fa, group_pull_kernel));
     CUDA_TRY(cudaFuncGetAttributes(&fa, group_ft_store_kernel));
     CUDA_TRY(cudaFuncGetAttributes(&fa, group_ft_reduce_kernel));
+    CUDA_TRY(cudaFuncGetAttributes(&fa, group_rows_store_kernel));
+    CUDA_TRY(cudaFuncGetAttributes(&fa, group_rows_compact_kernel));
     peer_[rank] = window_;
     return SKB_OK;
 }
@@ -75,7 +82,7 @@ int Group::import_handle(int peer_rank, const void *handle) {
 
 int Group::connect(int peer_rank, const Group &peer, int dev, int peer_dev) {
     if (peer.lay_.bytes != lay_.bytes || peer.n_fib_ != n_fib_ || peer.n_shell_ != n_shell_ ||
-        peer.n_bodies_ != n_bodies_)
+        peer.n_body_ != n_body_ || peer.n_bodies_ != n_bodies_)
         return set_error(SKB_ERR_INVALID, "skb_flow_group_connect: the two members were laid out for different geometries");
     if (peer_dev != dev) {
         int can = 0;
@@ -105,11 +112,12 @@ int Group::missing_peer(int *missing) const {
     return SKB_OK;
 }
 
-int Group::check_layout(long long n_fib, long long n_shell, int n_bodies) const {
-    if (n_fib_ != n_fib || n_shell_ != n_shell || n_bodies_ != n_bodies)
+int Group::check_layout(long long n_fib, long long n_shell, long long n_body, int n_bodies) const {
+    if (n_fib_ != n_fib || n_shell_ != n_shell || n_body_ != n_body || n_bodies_ != n_bodies)
         return set_error(SKB_ERR_STATE, "group member: the geometry changed size since skb_flow_group_init "
-                                        "(%lld/%lld fiber, %lld/%lld periphery nodes, %d/%d bodies); re-initialise the "
-                                        "group", n_fib, n_fib_, n_shell, n_shell_, n_bodies, n_bodies_);
+                                        "(%lld/%lld fiber, %lld/%lld periphery, %lld/%lld body nodes, %d/%d bodies); "
+                                        "re-initialise the group", n_fib, n_fib_, n_shell, n_shell_, n_body, n_body_,
+                         n_bodies, n_bodies_);
     return SKB_OK;
 }
 
@@ -120,12 +128,17 @@ int Group::windows(char **w) const {
     return n;
 }
 
-int Group::begin() {
+int Group::connected() const {
     if (!solo_)
         for (int m = 0; m < size_; ++m)
             if (!peer_[m])
                 return set_error(SKB_ERR_STATE, "group member %d: not all peers are connected (skb_flow_group_import / "
                                                 "_connect)", rank_);
+    return SKB_OK;
+}
+
+int Group::begin() {
+    SKB_TRY(connected());
     epoch_ += 1; // the only place it advances
     return SKB_OK;
 }
@@ -227,4 +240,117 @@ int Group::pull(Partials which, long long row0, long long n_rows, double *d_v, c
     a.accumulate = 1;
     group_pull_kernel<<<(unsigned)((3 * n_rows + 255) / 256), 256, 0, st>>>(a);
     return launched(launches);
+}
+
+// ---- a rank-per-GPU member's own rows of the solution vector ----
+
+bool skb::body_row_pieces(const int *n_nodes, int n_bodies, long long b0, long long b1, std::vector<RowPiece> &out) {
+    out.clear();
+    long long local = 0;
+    auto add = [&](long long a, long long e) { // body-part entries [a, e)
+        if (e <= a)
+            return;
+        if (!out.empty() && out.back().body + out.back().len == a)
+            out.back().len += e - a;
+        else
+            out.push_back(RowPiece{local, a, e - a});
+        local += e - a;
+    };
+    long long node = 0, sol = 0;
+    for (int b = 0; b < n_bodies; ++b) {
+        const long long n = n_nodes[b];
+        add(sol + 3 * (std::max(b0, node) - node), sol + 3 * (std::min(b1, node + n) - node));
+        if (node >= b0 && node < b1)
+            add(sol + 3 * n, sol + 3 * n + 6);
+        node += n;
+        sol += 3 * n + 6;
+    }
+    return out.size() <= (size_t)kMaxRowPieces;
+}
+
+void Group::set_body_rows(const std::vector<RowPiece> &pieces, const Ranges &ranges) {
+    rows_ = Rows();
+    for (const RowPiece &p : pieces) {
+        rows_.local[rows_.n] = p.local;
+        rows_.body[rows_.n] = p.body;
+        rows_.len[rows_.n] = p.len;
+        rows_.n += 1;
+        rows_.total += p.len;
+    }
+    rows_set_ = true;
+    rows_ranges_ = ranges;
+}
+
+static RowPiecesDev pieces_dev(const long long *local, const long long *body, const long long *len, int n,
+                               long long total) {
+    RowPiecesDev p;
+    for (int k = 0; k < kMaxRowPieces; ++k) {
+        p.local[k] = k < n ? local[k] : 0;
+        p.body[k] = k < n ? body[k] : 0;
+        p.len[k] = k < n ? len[k] : 0;
+    }
+    p.n = n;
+    p.total = total;
+    return p;
+}
+
+// the own rows into every window (before the rows phase's barrier)
+int Group::store_rows(const double *d_body, const double *d_shell, long long sa, long long n_s, int num_sms,
+                      cudaStream_t st, int *launches) const {
+    const int par = (int)(epoch_ & 1);
+    GroupRowsStoreArgs a;
+    a.pieces = pieces_dev(rows_.local, rows_.body, rows_.len, rows_.n, rows_.total);
+    a.body = d_body;
+    a.shell = d_shell;
+    a.shell_off = 3 * sa;
+    a.n_shell3 = d_shell ? 3 * n_s : 0;
+    char *w[kMaxGroup];
+    a.size = windows(w);
+    for (int m = 0; m < a.size; ++m) {
+        a.x_body[m] = (double *)(w[m] + lay_.x_body[par]);
+        a.x_shell[m] = (double *)(w[m] + lay_.x_shell[par]);
+    }
+    const long long work = a.pieces.total + a.n_shell3;
+    if (work == 0)
+        return SKB_OK;
+    const unsigned nblk = (unsigned)std::min<long long>((work + 255) / 256, 4LL * num_sms);
+    group_rows_store_kernel<<<nblk, 256, 0, st>>>(a);
+    return launched(launches);
+}
+
+int Group::rows_barrier(bool signal, bool wait, cudaStream_t st, int *launches) const {
+    return barrier(kRowsPhase, signal, wait, st, launches);
+}
+
+int Group::compact_rows(const double *d_full, double *d_local, cudaStream_t st, int *launches) const {
+    if (rows_.total == 0)
+        return SKB_OK;
+    GroupRowsCompactArgs a;
+    a.pieces = pieces_dev(rows_.local, rows_.body, rows_.len, rows_.n, rows_.total);
+    a.full = d_full;
+    a.local = d_local;
+    group_rows_compact_kernel<<<(unsigned)((rows_.total + 255) / 256), 256, 0, st>>>(a);
+    return launched(launches);
+}
+
+// host-only: the pieces a rank-per-GPU member's local vector is laid out by
+extern "C" int skb_group_body_pieces(const int *n_nodes, int n_bodies, int64_t body_begin, int64_t body_end,
+                                     int64_t *pieces, int max_pieces, int *n_pieces) {
+    if (n_bodies < 0 || (n_bodies > 0 && !n_nodes) || body_begin < 0 || body_end < body_begin || !n_pieces ||
+        max_pieces < 0 || (max_pieces > 0 && !pieces))
+        return set_error(SKB_ERR_INVALID, "skb_group_body_pieces: bad arguments");
+    for (int b = 0; b < n_bodies; ++b)
+        if (n_nodes[b] < 1)
+            return set_error(SKB_ERR_INVALID, "skb_group_body_pieces: body %d has %d nodes", b, n_nodes[b]);
+    std::vector<RowPiece> out;
+    body_row_pieces(n_nodes, n_bodies, body_begin, body_end, out);
+    *n_pieces = (int)out.size();
+    if ((int)out.size() > max_pieces)
+        return set_error(SKB_ERR_INVALID, "skb_group_body_pieces: %d pieces, room for %d", (int)out.size(), max_pieces);
+    for (size_t k = 0; k < out.size(); ++k) {
+        pieces[3 * k + 0] = out[k].local;
+        pieces[3 * k + 1] = out[k].body;
+        pieces[3 * k + 2] = out[k].len;
+    }
+    return SKB_OK;
 }

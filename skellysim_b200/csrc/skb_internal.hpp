@@ -2,6 +2,7 @@
 #pragma once
 #include "../../include/skelly_b200.h"
 
+#include <array>
 #include <cuda_runtime.h>
 #include <functional>
 #include <map>
@@ -137,6 +138,17 @@ struct EvalOpts {
 
 constexpr int kMaxGroup = 16; // members of a multi-GPU group (Group, group_kernels.cuh, skb_mflow)
 
+// A member's owned rows of the body part of the solution vector (distributed.system_rows): body node rows [b0, b1)
+// (3 each) and the six rows [U; w] of every body whose first node lies in [b0, b1), as runs of consecutive entries in
+// ascending order, adjacent runs merged.  At most three: the tail of a body cut at b0 (its six rows belong to the member
+// that holds its first node), the bodies that follow up to the one cut at b1, and that body's six rows.
+constexpr int kMaxRowPieces = 3;
+struct RowPiece {
+    long long local, body, len; // local-vector offset (within the body part), body-part offset, length
+};
+// the pieces of body rows [b0, b1) over bodies of n_nodes[0..n_bodies) nodes; false if they do not fit kMaxRowPieces
+bool body_row_pieces(const int *n_nodes, int n_bodies, long long b0, long long b1, std::vector<RowPiece> &out);
+
 // forces_torques [6 x n_bodies] (body_container.cpp:134) -> forces and torques, 3 x n_bodies each
 void split_forces_torques(const double *ft, int n_bodies, std::vector<double> &f, std::vector<double> &t);
 
@@ -186,6 +198,9 @@ class FiberOps {
                int *launches) const;
     int precondition(const double *d_x, double *d_y, cudaStream_t st, int *launches) const;
     int read(double *A, double *force_operator, double *xs, double *A_inv, cudaStream_t st) const; // any may be NULL
+    // the per-fiber tables and the event of rhs() for n_fibers own fibers, at their final size (a group member's RHS
+    // must not allocate once its peers may wait on a flag)
+    int size_rhs(int n_fibers);
     int ready(const char *who, bool with_inverse = false) const; // an error naming `who` unless they are resident
     bool empty() const { return n_items_A == 0; }
     int n_fibers() const { return f1 - f0; }
@@ -301,30 +316,38 @@ class BodyOps {
 };
 // loads the kernel of BodyOps::rhs_rows (a group member's first launch must not load it lazily)
 int load_rhs_rows_kernel();
+// loads the kernel of skb_dense_apply_device (skb_dense.cu), for the same reason: a kernel loaded lazily while a peer on
+// the same device spins on a flag waits for that peer, which waits for this member
+int load_dense_kernels();
 
 // ---- one member of a multi-GPU group of flows (DESIGN.md §4; skb_group.cu, group_kernels.cuh) ----
 // A group is one flow per GPU exchanging strengths and partial velocities through peer memory.  Every member owns a
 // WINDOW of device memory that all members can address, laid out by init (each piece 256-byte aligned):
 //
-//   flags        [4][kMaxGroup] + 8  epoch counters, one slot per (phase, writer); then the error word (0, or
+//   flags        [5][kMaxGroup] + 8  epoch counters, one slot per (phase, writer); then the error word (0, or
 //                                    1 + the rank a flag wait gave up on)                        -- written by peers
 //   f_sl         [2][n_pad_fib*3]    packed (trapezoid-weighted) Stokeslet strengths of ALL fiber nodes   -- by peers
 //   f_shell      [2][n_pad_shell*6]  packed sym6 stresslet strengths of ALL periphery nodes                -- by peers
-//   x_shell      [2][n_shell*3]      periphery density of ALL nodes (input of the dense operator)          -- by peers
+//   x_shell      [2][n_shell*3]      periphery density of ALL nodes (input of the dense operator; the matvec's push
+//                                    and the rank-per-GPU preconditioner's row store write it)    -- by peers
 //   ft_part      [2][kMaxGroup][n_bodies*6]  per member its partial link forces / torques of ALL bodies
 //                                    ([F | L]; the whole-vector operator, skb_mflow_apply_system_matvec) -- by peers
+//   x_body       [2][n_body*3 + n_bodies*6]  the body part of the solution vector, complete (every member stores
+//                                    its own rows; skb_flow_group_apply_system_*)                   -- by peers
 //   u_part       [n_fib*3]           this member's partial velocities of ALL fiber rows                  -- by itself
 //   u_part_shell [n_shell*3]         its partial velocities of ALL periphery rows (cross kernel)        -- by itself
 //
-// [2]: double buffering by epoch parity -- a peer may already push the next matvec's strengths while this member still
-// reads the current ones.  A default-constructed Group is no member (size 1).  Knows nothing of skb_flow: the caller
-// has made the flow's device current, and every step runs on the stream it passes, adding its launches to *launches.
+// [2]: double buffering by epoch parity -- a peer may already push the next call's strengths or rows while this member
+// still reads the current ones (DESIGN.md §4 argues why the other half is never still being read).  A
+// default-constructed Group is no member (size 1).  Knows nothing of skb_flow: the caller has made the flow's device
+// current, and every step runs on the stream it passes, adding its launches to *launches.
 class Group {
   public:
-    // allocates and zeroes the window of member `rank` of `size` for that many fiber / periphery nodes; n_pad_*: the
-    // padded source counts of the flow's evaluators (the window replaces their packed strengths).  Size 1: no member
+    // allocates and zeroes the window of member `rank` of `size` for that many fiber / periphery / body nodes and
+    // bodies; n_pad_*: the padded source counts of the flow's evaluators (the window replaces their packed strengths).
+    // Size 1: no member
     int init(int rank, int size, long long n_fib, long long n_pad_fib, long long n_shell, long long n_pad_shell,
-             int n_bodies);
+             long long n_body, int n_bodies);
     int export_handle(void *handle) const;                     // the window's CUDA-IPC handle
     int import_handle(int peer_rank, const void *handle);      // maps another process's member's window
     int connect(int peer_rank, const Group &peer, int dev, int peer_dev); // a member in this process, on peer_dev
@@ -334,12 +357,14 @@ class Group {
     bool has_window() const { return window_.get() != nullptr; }
     int rank() const { return rank_; }
     int size() const { return size_; }
-    int check_layout(long long n_fib, long long n_shell, int n_bodies) const; // an error unless laid out for these
+    // an error unless laid out for these
+    int check_layout(long long n_fib, long long n_shell, long long n_body, int n_bodies) const;
     // solo (warm-up, profiling): no flags, push and pull over this member's own window only, no connectedness check
     void set_solo(bool solo) { solo_ = solo; }
     void restart() { epoch_ = 0; } // the next matvec is the group's first
 
     // ---- one matvec: begin, push, barrier(0), pair kernels, barrier(1), pull ----
+    int connected() const; // an error unless every peer's window is mapped (solo: always)
     int begin(); // refuses a member whose peers are not all connected; advances the epoch (its parity picks the half)
     // pack the own strengths once and store them into every window: fiber forces d_fw [n_f*3] of nodes [fa, fa + n_f)
     // (weighted by d_weight of ALL fiber nodes, NULL: 1), periphery densities d_density [n_s*3] of rows [sa, sa + n_s)
@@ -357,18 +382,40 @@ class Group {
     enum Partials { kFiberRows, kShellRows };
     int pull(Partials which, long long row0, long long n_rows, double *d_v, cudaStream_t st, int *launches) const;
 
+    // ---- a rank-per-GPU member's own rows of the solution vector (skb_flow_group_* whole-vector calls) ----
+    // the member's resolved target ranges: fiber nodes [fa, fb), periphery rows [sa, sb), body nodes [ba, bb)
+    using Ranges = std::array<long long, 6>;
+    // the pieces of its body rows [ba, bb) (body_row_pieces), kept until init, and the ranges the caller sized its
+    // buffers for; rows_for: they were set for exactly these ranges (any other split of the rows wants the set-up again)
+    void set_body_rows(const std::vector<RowPiece> &pieces, const Ranges &ranges);
+    bool rows_for(const Ranges &ranges) const { return rows_set_ && rows_ranges_ == ranges; }
+    long long body_rows() const { return rows_.total; } // own body rows of the local vector
+    // d_body [body_rows()] into x_body of every window at the pieces' places, and (d_shell != NULL) the own periphery
+    // rows d_shell [n_s*3] of rows [sa, sa + n_s) into x_shell, in one kernel (before the rows phase's barrier)
+    int store_rows(const double *d_body, const double *d_shell, long long sa, long long n_s, int num_sms,
+                   cudaStream_t st, int *launches) const;
+    int rows_barrier(bool signal, bool wait, cudaStream_t st, int *launches) const; // barrier of the rows phase
+    // d_local [body_rows()] = the own rows of d_full (the whole body layout)
+    int compact_rows(const double *d_full, double *d_local, cudaStream_t st, int *launches) const;
+
     // this member's window, in the half of the matvec in flight
     double *f_sl() const { return own(lay_.f_sl[epoch_ & 1]); }
     double *f_shell() const { return own(lay_.f_shell[epoch_ & 1]); }
     double *x_shell() const { return own(lay_.x_shell[epoch_ & 1]); }
+    double *x_body() const { return own(lay_.x_body[epoch_ & 1]); }
     double *u_part() const { return own(lay_.u_part); }
     double *u_part_shell() const { return own(lay_.u_part_shell); }
 
   private:
     struct Layout { // byte offsets of the window's pieces
-        size_t flags = 0, f_sl[2] = {0, 0}, f_shell[2] = {0, 0}, x_shell[2] = {0, 0}, ft_part[2] = {0, 0}, u_part = 0,
-               u_part_shell = 0;
+        size_t flags = 0, f_sl[2] = {0, 0}, f_shell[2] = {0, 0}, x_shell[2] = {0, 0}, ft_part[2] = {0, 0},
+               x_body[2] = {0, 0}, u_part = 0, u_part_shell = 0;
         size_t bytes = 0;
+    };
+    struct Rows { // the piece table of set_body_rows, as the kernels take it (RowPiecesDev, group_kernels.cuh)
+        long long local[kMaxRowPieces] = {}, body[kMaxRowPieces] = {}, len[kMaxRowPieces] = {};
+        int n = 0;
+        long long total = 0;
     };
     double *own(size_t off) const { return reinterpret_cast<double *>((char *)window_.get() + off); }
     int windows(char **w) const; // the windows push and pull reach (solo: the own one only); returns their count
@@ -378,10 +425,13 @@ class Group {
     Layout lay_;
     void *peer_[kMaxGroup] = {}; // every member's window as mapped here (peer_[rank_] == window_)
     IpcPtr ipc_[kMaxGroup];      // the windows of other processes' members that this one has mapped
-    long long n_fib_ = 0, n_shell_ = 0; // geometry the window was laid out for
+    long long n_fib_ = 0, n_shell_ = 0, n_body_ = 0; // geometry the window was laid out for
     int n_bodies_ = 0;
     unsigned long long epoch_ = 0;
     bool solo_ = false;
+    Rows rows_;
+    bool rows_set_ = false;
+    Ranges rows_ranges_ = {};
 };
 
 } // namespace skb

@@ -99,6 +99,10 @@ struct skb_flow {
     // window and the body flow reads their totals from ft_sum ([F | L], 6 per body)
     bool ft_exchange = false;
     DevBuf ft_sum;
+    // a rank-per-GPU member's whole-vector matvec has begun the epoch (and exchanged its body rows in it): matvec_core
+    // runs its protocol in that epoch instead of beginning one
+    bool grp_open = false;
+    DevBuf sys_rb; // a member's body output in the whole body layout (skb_flow_group_*), compacted to its own rows
     // Periphery::matvec's dense operator beside the pair kernels (stream_kernels.cuh): forked onto bg_stream once its
     // input (the complete x_shell) is there, joined before res_shell is assembled
     struct Overlap {
@@ -776,7 +780,7 @@ static int prepare_matvec_targets(skb_flow *fl) {
         if (!fl->use_ranges)
             return set_error(SKB_ERR_STATE, "group member: call skb_flow_set_target_ranges (own fibers / periphery rows / "
                                             "body rows) before the first matvec");
-        SKB_TRY(fl->grp.check_layout(nf, ns, fl->n_bodies));
+        SKB_TRY(fl->grp.check_layout(nf, ns, nb, fl->n_bodies));
     }
     // group: fiber rows through the symmetric block rows of this member (partial sums, pulled together afterwards)
     // when the self-interaction is big enough for that kernel; otherwise the member's own rows with the plain kernel
@@ -982,7 +986,8 @@ static int matvec_core(skb_flow *fl, const double *d_ff, const double *d_sd, con
     StrengthMode fmode = kRaw, smode = kNormalDensity;
     const double *ff = d_ff, *sd = d_sd;
     if (P.grouped) {
-        SKB_TRY(G.begin());
+        if (!fl->grp_open)
+            SKB_TRY(G.begin());
         const DeviceState &df = fl->fib[1]->devs[0];
         const SourceSet &sf = df.src[SKB_STOKESLET];
         SKB_TRY(G.push(d_ff, sf.has_weights ? (const double *)sf.weights.ptr : nullptr, fl->fa, n_fw, d_sd,
@@ -1048,7 +1053,7 @@ int skb_flow_group_init(skb_flow *fl, int rank, int size) {
     // the same padded sizes the evaluator contexts use (set_sources_impl): the window replaces their f_packed
     const long long n_pad_fib = fl->n_fib > 0 ? fl->fib[1]->devs[0].src[SKB_STOKESLET].n_pad : 0;
     const long long n_pad_shell = fl->n_shell > 0 ? fl->shell[1]->devs[0].src[SKB_STRESSLET].n_pad : 0;
-    return fl->grp.init(rank, size, fl->n_fib, n_pad_fib, fl->n_shell, n_pad_shell, fl->n_bodies);
+    return fl->grp.init(rank, size, fl->n_fib, n_pad_fib, fl->n_shell, n_pad_shell, fl->n_body, fl->n_bodies);
 }
 
 int skb_flow_group_export(skb_flow *fl, void *handle) {
@@ -2038,12 +2043,11 @@ int skb::flow_size_system(skb_flow *fl) {
     return fl->ft_sum.ensure((size_t)fl->n_bodies * 48 + 8);
 }
 
-int skb::flow_member_system_matvec(skb_flow *fl, skb_dense *dn, const double *d_x_fib, const double *d_x_shell,
-                                   const double *d_x_bodies, double eta, double *d_res_fib, double *d_res_shell,
-                                   double *d_res_bodies, cudaStream_t st) {
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    begin_stats(fl);
-    fl->cur = st;
+// the links of the own fibers, apply_matvec_core with the exchange of their partial forces, the owned body rows; on
+// fl->cur
+static int member_system_matvec_core(skb_flow *fl, skb_dense *dn, const double *d_x_fib, const double *d_x_shell,
+                                     const double *d_x_bodies, double eta, double *d_res_fib, double *d_res_shell,
+                                     double *d_res_bodies) {
     const double *link = nullptr, *bd = nullptr, *f = nullptr, *t = nullptr;
     if (fl->n_bodies > 0) { // the links of the own fibers; their partial forces / torques on every body
         const auto &off = fl->h_fiber_off;
@@ -2059,8 +2063,17 @@ int skb::flow_member_system_matvec(skb_flow *fl, skb_dense *dn, const double *d_
     const int rc = apply_matvec_core(fl, dn, d_x_fib, d_x_shell, bd, f, t, link, eta, d_res_fib, d_res_shell, v_bodies);
     fl->ft_exchange = false;
     SKB_TRY(rc);
-    if (fl->n_bodies > 0)
-        SKB_TRY(fl->bodies.matvec(d_x_bodies, v_bodies, d_res_bodies, fl->cur, &fl->launches));
+    return fl->n_bodies > 0 ? fl->bodies.matvec(d_x_bodies, v_bodies, d_res_bodies, fl->cur, &fl->launches) : SKB_OK;
+}
+
+int skb::flow_member_system_matvec(skb_flow *fl, skb_dense *dn, const double *d_x_fib, const double *d_x_shell,
+                                   const double *d_x_bodies, double eta, double *d_res_fib, double *d_res_shell,
+                                   double *d_res_bodies, cudaStream_t st) {
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    begin_stats(fl);
+    fl->cur = st;
+    SKB_TRY(member_system_matvec_core(fl, dn, d_x_fib, d_x_shell, d_x_bodies, eta, d_res_fib, d_res_shell,
+                                      d_res_bodies));
     return device_stats(fl);
 }
 
@@ -2118,6 +2131,218 @@ int skb::flow_member_system_rhs(skb_flow *fl, const skb_fiber_params *params, co
                             d_rhs_bodies));
     return device_stats(fl);
 }
+
+// ---- the whole-vector calls of a rank-per-GPU group member (skb_flow_group_*, include/skelly_b200_flow.h) ----------
+// A member holds only its own rows of the solution vector, in ascending global order (distributed.system_rows):
+// x_local = [4 per own fiber node | 3 per own periphery row | own body rows].  Before a matvec or a preconditioner it
+// stores its own body rows (and, for the preconditioner, its own periphery rows) into every window and meets its peers
+// at the rows phase; from there on the complete x_bodies / x_shell are in its own window, and the member path of
+// skb_mflow runs on them unchanged.  Body outputs land in the whole body layout (sys_rb) and are compacted to the own
+// rows in one launch.
+
+// the resolved target ranges the set-up sized the member's buffers for (prepare_matvec_targets has run)
+static Group::Ranges group_ranges(const skb_flow *fl) { return {fl->fa, fl->fb, fl->sa, fl->sb, fl->ba, fl->bb}; }
+
+static long long group_local_size(const skb_flow *fl) {
+    return 4 * (fl->fb - fl->fa) + 3 * (fl->sb - fl->sa) + fl->grp.body_rows();
+}
+
+// the refusals of the group matvec (stresslet_plus_complementary in dn) and preconditioner (M_inv in dn, the inverses),
+// all before any launch; then the flow's device is current and its target ranges resolved
+static int group_system_args(skb_flow *fl, skb_dense *dn, const char *who, bool precondition) {
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    SKB_TRY(fl->grp.connected());
+    SKB_TRY(prepare_matvec_targets(fl));
+    if (!fl->grp.rows_for(group_ranges(fl)))
+        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_group_set_body_operators after skb_flow_group_init and after "
+                                          "every change of the target ranges", who);
+    SKB_TRY(fl->ops.ready(who, precondition));
+    if (fl->n_bodies > 0) {
+        if (!fl->bodies.has_operators())
+            return set_error(SKB_ERR_INVALID, "%s: call skb_flow_group_set_body_operators after skb_flow_set_bodies", who);
+        if (precondition && !fl->bodies.has_inverse())
+            return set_error(SKB_ERR_INVALID, "%s: skb_flow_group_set_body_operators was given no A_inv", who);
+        if (!precondition && fl->n_fibers > 0 && !fl->bodies.has_links())
+            return set_error(SKB_ERR_INVALID, "%s: call skb_flow_group_set_fiber_links after skb_flow_set_fibers / "
+                                              "skb_flow_set_bodies (NULL body: no fiber is bound)", who);
+    }
+    const long long n_sw = fl->sb - fl->sa;
+    if (n_sw > 0) {
+        const int op = precondition ? SKB_DENSE_M_INV : SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY;
+        const char *op_name = precondition ? "M_inv" : "stresslet_plus_complementary";
+        if (!dn)
+            return set_error(SKB_ERR_INVALID, "%s: the member's periphery rows need their block of %s (dn == NULL)", who,
+                             op_name);
+        int dn_dev = -1;
+        int64_t rows = -1, cols = -1;
+        SKB_TRY(skb_dense_device(dn, 0, &dn_dev));
+        SKB_TRY(skb_dense_shape(dn, op, &rows, &cols));
+        if (dn_dev != fl->dev || rows != 3 * n_sw || cols != 3 * fl->n_shell)
+            return set_error(SKB_ERR_INVALID, "%s: the dense handle holds a %lld x %lld block of %s on device %d, need the "
+                                              "member's %lld rows x %lld of the %lld periphery nodes on device %d", who,
+                             (long long)rows, (long long)cols, op_name, dn_dev, 3 * n_sw, 3 * fl->n_shell, fl->n_shell,
+                             fl->dev);
+    }
+    return SKB_OK;
+}
+
+extern "C" {
+
+int skb_flow_group_set_body_operators(skb_flow *fl, const int *n_nodes, int n_bodies, const double *node_weights,
+                                      const double *ex, const double *ey, const double *ez, const double *A_inv) {
+    const char *who = "skb_flow_group_set_body_operators";
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    if (!fl->grp.member())
+        return skb_flow_set_body_operators(fl, n_nodes, n_bodies, node_weights, ex, ey, ez, A_inv);
+    if (n_bodies != fl->n_bodies)
+        return set_error(SKB_ERR_INVALID, "%s: %d bodies, skb_flow_set_bodies has %d", who, n_bodies, fl->n_bodies);
+    if (n_bodies > 0 && (!n_nodes || !node_weights || !ex || !ey || !ez))
+        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    OwnFibers own;
+    SKB_TRY(own_fibers(fl, who, own)); // the target ranges resolved, the window's layout checked
+    SKB_TRY(fl->bodies.set_operators(n_nodes, n_bodies, fl->n_body, fl->h_r_body.data(), fl->h_centers.data(),
+                                     node_weights, ex, ey, ez, A_inv, fl->stream, fl->ba, fl->bb));
+    std::vector<RowPiece> pieces;
+    if (!body_row_pieces(n_nodes, n_bodies, fl->ba, fl->bb, pieces))
+        return set_error(SKB_ERR_STATE, "%s: the body rows [%lld, %lld) make %d pieces (at most %d)", who, fl->ba,
+                         fl->bb, (int)pieces.size(), kMaxRowPieces);
+    // every buffer the three whole-vector calls use, at its final size now: none of them allocates while a peer on
+    // this device may wait on a flag (the warm-up sized the matvec flow's own)
+    SKB_TRY(fl->sys_rb.ensure((size_t)fl->bodies.solution_size() * 8 + 8));
+    SKB_TRY(flow_size_system(fl));
+    SKB_TRY(rhs_buffers(fl));
+    SKB_TRY(fl->ops.size_rhs(own.count()));
+    SKB_TRY(load_dense_kernels()); // the preconditioner's M_inv rows (and the matvec's without the streamer)
+    fl->grp.set_body_rows(pieces, group_ranges(fl));
+    return SKB_OK;
+}
+
+int skb_flow_group_set_fiber_links(skb_flow *fl, const int *body, const double *site, const double *bending_rigidity) {
+    const char *who = "skb_flow_group_set_fiber_links";
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    if (!fl->grp.member())
+        return skb_flow_set_fiber_links(fl, body, site, bending_rigidity);
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    OwnFibers own;
+    SKB_TRY(own_fibers(fl, who, own));
+    if (body && own.count() > 0 && (!site || !bending_rigidity))
+        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
+    return fl->bodies.set_links(own, fl->ops, fl->n_bodies, fl->h_centers.data(), body, site, bending_rigidity,
+                                fl->stream);
+}
+
+int skb_flow_group_apply_system_matvec_device(skb_flow *fl, skb_dense *dn, const double *d_x_local, double eta,
+                                              double *d_res_local, void *stream) {
+    const char *who = "skb_flow_group_apply_system_matvec_device";
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    if (!fl->grp.member())
+        return skb_flow_apply_system_matvec_device(fl, dn, d_x_local, eta, d_res_local, stream);
+    SKB_TRY(group_system_args(fl, dn, who, false));
+    if (!(eta > 0))
+        return set_error(SKB_ERR_INVALID, "%s: eta = %g", who, eta);
+    if (group_local_size(fl) > 0 && (!d_x_local || !d_res_local))
+        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
+    begin_stats(fl);
+    fl->cur = (cudaStream_t)stream;
+    Group &G = fl->grp;
+    const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
+    const double *x_fib = d_x_local, *x_shell = x_fib + 4 * n_fw, *x_body = x_shell + 3 * n_sw;
+    double *res_fib = d_res_local, *res_shell = res_fib + 4 * n_fw, *res_body = res_shell + 3 * n_sw;
+    double *full = (double *)fl->sys_rb.ptr;
+    const bool bodies = fl->n_bodies > 0;
+    SKB_TRY(G.begin());
+    if (bodies) { // the complete x_bodies in every window first: the links read the bodies' U, w before barrier A
+        SKB_TRY(G.store_rows(x_body, nullptr, 0, 0, fl->fib[1]->devs[0].info.num_sms, fl->cur, &fl->launches));
+        SKB_TRY(G.rows_barrier(true, true, fl->cur, &fl->launches));
+    }
+    fl->grp_open = true; // matvec_core's push, barriers and pull run in this epoch
+    const int rc = member_system_matvec_core(fl, dn, x_fib, x_shell, bodies ? G.x_body() : nullptr, eta, res_fib,
+                                             res_shell, full);
+    fl->grp_open = false;
+    SKB_TRY(rc);
+    if (bodies)
+        SKB_TRY(G.compact_rows(full, res_body, fl->cur, &fl->launches));
+    return device_stats(fl);
+}
+
+int skb_flow_group_apply_system_preconditioner_device(skb_flow *fl, skb_dense *dn, const double *d_x_local,
+                                                      double *d_y_local, void *stream) {
+    const char *who = "skb_flow_group_apply_system_preconditioner_device";
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    if (!fl->grp.member())
+        return skb_flow_apply_system_preconditioner_device(fl, dn, d_x_local, d_y_local, stream);
+    SKB_TRY(group_system_args(fl, dn, who, true));
+    if (group_local_size(fl) > 0 && (!d_x_local || !d_y_local))
+        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
+    begin_stats(fl);
+    fl->cur = (cudaStream_t)stream;
+    Group &G = fl->grp;
+    const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
+    const double *x_fib = d_x_local, *x_shell = x_fib + 4 * n_fw, *x_body = x_shell + 3 * n_sw;
+    double *y_fib = d_y_local, *y_shell = y_fib + 4 * n_fw, *y_body = y_shell + 3 * n_sw;
+    double *full = (double *)fl->sys_rb.ptr;
+    // the complete x_shell and x_bodies in every window; the fibers' A_^-1 runs while the peers' rows arrive
+    SKB_TRY(G.begin());
+    SKB_TRY(G.store_rows(x_body, n_sw > 0 ? x_shell : nullptr, fl->sa, n_sw, fl->fib[1]->devs[0].info.num_sms, fl->cur,
+                         &fl->launches));
+    SKB_TRY(G.rows_barrier(true, false, fl->cur, &fl->launches));
+    SKB_TRY(fl->ops.precondition(x_fib, y_fib, fl->cur, &fl->launches));
+    SKB_TRY(G.rows_barrier(false, true, fl->cur, &fl->launches));
+    if (n_sw > 0) { // the member's rows of M_inv times the complete x_shell
+        SKB_TRY(skb_dense_apply_device(dn, SKB_DENSE_M_INV, G.x_shell(), nullptr, y_shell, fl->cur));
+        fl->launches += 1;
+    }
+    if (fl->n_bodies > 0) {
+        SKB_TRY(fl->bodies.precondition(G.x_body(), full, fl->cur, &fl->launches));
+        SKB_TRY(G.compact_rows(full, y_body, fl->cur, &fl->launches));
+    }
+    return device_stats(fl);
+}
+
+int skb_flow_group_build_system_rhs_device(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
+                                           const double *force_scale, const double *d_f_external,
+                                           const double *d_body_forces, const double *d_body_torques, double dt,
+                                           double eta, double *d_rhs_local, void *stream) {
+    const char *who = "skb_flow_group_build_system_rhs_device";
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    if (!fl->grp.member())
+        return skb_flow_build_system_rhs_device(fl, params, v_growth, force_scale, d_f_external, d_body_forces,
+                                                d_body_torques, dt, eta, d_rhs_local, stream);
+    if (!(dt > 0) || !(eta > 0))
+        return set_error(SKB_ERR_INVALID, "%s: dt = %g, eta = %g (both must be > 0)", who, dt, eta);
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    SKB_TRY(fl->grp.connected());
+    OwnFibers own;
+    SKB_TRY(own_fibers(fl, who, own));
+    if (!fl->grp.rows_for(group_ranges(fl)))
+        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_group_set_body_operators after skb_flow_group_init and after "
+                                          "every change of the target ranges", who);
+    if (fl->n_bodies > 0 && !fl->bodies.has_operators())
+        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_group_set_body_operators after skb_flow_set_bodies (the "
+                                          "body rows are laid out by its node counts)", who);
+    if ((own.count() > 0 && !params) || (group_local_size(fl) > 0 && !d_rhs_local))
+        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
+    begin_stats(fl);
+    fl->cur = (cudaStream_t)stream;
+    const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
+    double *rhs_fib = d_rhs_local, *rhs_shell = rhs_fib + 4 * n_fw, *rhs_body = rhs_shell + 3 * n_sw;
+    double *full = (double *)fl->sys_rb.ptr;
+    // the fiber block's checks come first inside system_rhs_core, before its first launch; F_T complete, as they are
+    SKB_TRY(system_rhs_core(fl, own, params, v_growth, force_scale, own.count() > 0 ? d_f_external : nullptr,
+                            fl->n_bodies ? d_body_forces : nullptr, fl->n_bodies ? d_body_torques : nullptr, dt, eta,
+                            rhs_fib, rhs_shell, full));
+    if (fl->n_bodies > 0)
+        SKB_TRY(fl->grp.compact_rows(full, rhs_body, fl->cur, &fl->launches));
+    return device_stats(fl);
+}
+
+} // extern "C"
 
 cudaStream_t skb::flow_stream(const skb_flow *fl) { return fl->stream; }
 int skb::flow_size_overlap(skb_flow *fl, long long n_rows) {

@@ -231,3 +231,60 @@ class RankApplyMatvec:
                                    link_own.data_ptr() if link_own is not None else 0, self._res.data_ptr(), st)
         a, b = self.n_fib_own, self.n_fib_own + self.n_shell_own
         return self._res[:4 * a], self._v[a:b], self._v[b:b + self.n_body_own]
+
+
+class RankSystemOperator:
+    """A and P^-1 of the whole mobility system, and its right-hand side, on ONE rank's local vector: the rank-per-GPU
+    twin of solver_hydro.SystemOperator (A_fiber_hydro::apply / P_inv_hydro::apply / Solver::set_RHS of one MPI rank on
+    its Tpetra local view).
+
+    flow: a capi.Flow that is a connected group member (target ranges = `partition`, connect_group, fiber operators,
+    group_set_body_operators, group_set_fiber_links); dense_matvec / dense_minv: capi.Dense on the flow's device holding
+    the member's rows of stresslet_plus_complementary / M_inv (None without own periphery rows).  The local vector is
+    x[local_rows] of the whole vector, local_rows = system_rows(partition, fiber_n_nodes, n_shell, body_n_nodes): the
+    union over the ranks is the whole vector, each row once.  Every rank must make the same calls in the same order.
+    This class sequences the calls and owns the work vectors; it computes nothing itself."""
+
+    def __init__(self, flow, dense_matvec, dense_minv, partition, fiber_n_nodes, n_shell, body_n_nodes, eta, device):
+        import torch
+        self.torch = torch
+        self.flow, self.dense_matvec, self.dense_minv, self.eta = flow, dense_matvec, dense_minv, float(eta)
+        self.local_rows = system_rows(partition, fiber_n_nodes, n_shell, body_n_nodes)
+        self.n = int(self.local_rows.size)
+        kw = dict(dtype=torch.float64, device=device)
+        self.res = torch.zeros(max(self.n, 1), **kw)
+        self.y = torch.zeros(max(self.n, 1), **kw)
+        self.b = torch.zeros(max(self.n, 1), **kw)  # owned: no call allocates while a peer may wait on a flag
+        self.launches = 0
+
+    def _stream(self):
+        return self.torch.cuda.current_stream().cuda_stream
+
+    @staticmethod
+    def _ptr(t):
+        return t.data_ptr() if t is not None and t.numel() else 0
+
+    def apply(self, x_local):
+        """the rank's rows of A x (System::apply_matvec) -- a view valid until the next call"""
+        self.flow.group_apply_system_matvec_device(self.dense_matvec, self._ptr(x_local), self.eta, self.res.data_ptr(),
+                                                   self._stream())
+        self.launches = self.flow.stats()["launches"]
+        return self.res[:self.n]
+
+    def apply_preconditioner(self, x_local):
+        """the rank's rows of P^-1 x (System::apply_preconditioner) -- a view valid until the next call"""
+        self.flow.group_apply_system_preconditioner_device(self.dense_minv, self._ptr(x_local), self.y.data_ptr(),
+                                                           self._stream())
+        self.launches = self.flow.stats()["launches"]
+        return self.y[:self.n]
+
+    def rhs(self, fiber_params, dt: float, f_external=None, body_forces=None, body_torques=None, v_growth=None,
+            force_scale=None):
+        """the rank's rows of the RHS (System::prep_state_for_solver) -- a view valid until the next call.  fiber_params
+        and v_growth / force_scale: of the OWN fibers; f_external (own fiber nodes, 3); body_forces / body_torques
+        (n_bodies, 3) of ALL bodies, the same on every rank; None: zero."""
+        self.flow.group_build_system_rhs_device(*fiber_params, dt, self.eta, self._ptr(f_external),
+                                                self._ptr(body_forces), self._ptr(body_torques), self.b.data_ptr(),
+                                                v_growth=v_growth, force_scale=force_scale, stream=self._stream())
+        self.launches = self.flow.stats()["launches"]
+        return self.b[:self.n]
