@@ -353,7 +353,15 @@ SKB_API int skb_flow_apply_matvec_device(skb_flow *fl, struct skb_dense *dn, con
  * per GPU the skb_flow_group_* calls above), fiber operators not resident (with their inverse for the preconditioner), bodies without
  * skb_flow_set_body_operators, fibers and bodies without skb_flow_set_fiber_links (matvec), no A_inv (preconditioner),
  * dn == NULL or of the wrong shape with periphery nodes present.  The results are bitwise reproducible run to run: the
- * bodies' link forces are added per body in container order, without atomics. */
+ * bodies' link forces are added per body in container order, without atomics.
+ * An empty block needs none of its set-up, here, in skb_flow_build_system_rhs, in the skb_mflow_* system calls and in
+ * the partial operator (skb_flow_apply_matvec(_device), skb_mflow_apply_matvec):
+ * without fibers no fiber class, operators, preconditioner or links (a flow whose fibers all went away needs no new
+ * upload: skb_flow_set_fibers drops the old operators); without periphery no dense handle (dn may be NULL); without
+ * bodies no skb_flow_set_body_operators.  A group member (skb_flow_group_*) still calls
+ * skb_flow_group_set_body_operators, which lays out its rows, and uploads the operators of its own fibers, none or
+ * not.  The empty upload of an empty block is accepted and changes no result.  A solution vector of length 0 makes
+ * every call return SKB_OK without a launch; its vectors may be NULL. */
 SKB_API int skb_flow_set_body_operators(skb_flow *fl, const int *n_nodes, int n_bodies, const double *node_weights,
                                         const double *ex, const double *ey, const double *ez, const double *A_inv);
 SKB_API int skb_flow_set_fiber_links(skb_flow *fl, const int *body, const double *site, const double *bending_rigidity);

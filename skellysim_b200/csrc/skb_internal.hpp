@@ -204,7 +204,11 @@ class FiberOps {
     int ready(const char *who, bool with_inverse = false) const; // an error naming `who` unless they are resident
     bool empty() const { return n_items_A == 0; }
     int n_fibers() const { return f1 - f0; }
-    void invalidate() { ready_ = false; }
+    // drops the resident operators: no GEMV runs on them again (a flow left with no fibers has the empty set)
+    void invalidate() {
+        ready_ = false;
+        n_items_A = n_items_F = 0;
+    }
     // what the fiber-body links read (BodyOps): the element offset of D_2_0 of fiber f's class (n nodes) in the class
     // table, D_3_0 following -- an error unless skb_flow_set_fiber_class_derivatives(n) was called; offsets move when
     // set_class adds a node count.  The table and the resident tangents xs_ (3 per own node) on the device

@@ -1551,7 +1551,8 @@ static int apply_matvec_impl(skb_flow *fl, skb_dense *dn, const double *x_fibers
                              double *v_bodies) {
     if (!fl || !(eta > 0))
         return set_error(SKB_ERR_INVALID, "skb_flow_apply_matvec: bad arguments");
-    SKB_TRY(fl->ops.ready("skb_flow_apply_matvec"));
+    if (fl->n_fibers > 0) // no fibers: the empty operator set, uploaded or not
+        SKB_TRY(fl->ops.ready("skb_flow_apply_matvec"));
     const long long nf = fl->n_fib, ns = fl->n_shell, nb = fl->n_body, n_all = nf + ns + nb;
     if ((nf > 0 && (!x_fibers || !res_fibers)) || (ns > 0 && (!shell_density || !v_shell)) ||
         (nb > 0 && (!body_densities || !v_bodies)) || (fl->n_bodies > 0 && !body_forces_torques))
@@ -1624,7 +1625,8 @@ int skb_flow_apply_matvec_device(skb_flow *fl, skb_dense *dn, const double *d_x_
                                  double *d_res_fibers, double *d_out_shell, double *d_v_bodies, void *stream) {
     if (!fl || !(eta > 0))
         return set_error(SKB_ERR_INVALID, "skb_flow_apply_matvec_device: bad arguments");
-    SKB_TRY(fl->ops.ready("skb_flow_apply_matvec_device"));
+    if (fl->n_fibers > 0)
+        SKB_TRY(fl->ops.ready("skb_flow_apply_matvec_device"));
     CUDA_TRY(cudaSetDevice(fl->dev));
     begin_stats(fl);
     SKB_TRY(prepare_matvec_targets(fl));
@@ -1709,7 +1711,8 @@ static int system_args(skb_flow *fl, skb_dense *dn, const char *who, bool precon
     if (fl->grp.member())
         return set_error(SKB_ERR_INVALID, "%s: multi-GPU is not supported: a body's K^T lambda needs all of its nodes "
                                           "(the reference keeps the bodies on rank 0); use a single-device flow", who);
-    SKB_TRY(fl->ops.ready(who, precondition));
+    if (fl->n_fibers > 0) // no fibers: the empty operator set, uploaded or not
+        SKB_TRY(fl->ops.ready(who, precondition));
     CUDA_TRY(cudaSetDevice(fl->dev));
     SKB_TRY(prepare_matvec_targets(fl));
     const long long n_all = fl->n_fib + fl->n_shell + fl->n_body;
@@ -2023,7 +2026,8 @@ int skb::flow_member_fiber_links(skb_flow *fl, const int *body, const double *si
 }
 
 int skb::flow_member_system_ready(skb_flow *fl, const char *who, bool precondition) {
-    SKB_TRY(fl->ops.ready(who, precondition));
+    if (fl->n_fibers > 0)
+        SKB_TRY(fl->ops.ready(who, precondition));
     if (fl->n_bodies > 0) {
         if (!fl->bodies.has_operators())
             return set_error(SKB_ERR_INVALID, "%s: call skb_mflow_set_body_operators after skb_mflow_set_bodies", who);
@@ -2156,7 +2160,8 @@ static int group_system_args(skb_flow *fl, skb_dense *dn, const char *who, bool 
     if (!fl->grp.rows_for(group_ranges(fl)))
         return set_error(SKB_ERR_INVALID, "%s: call skb_flow_group_set_body_operators after skb_flow_group_init and after "
                                           "every change of the target ranges", who);
-    SKB_TRY(fl->ops.ready(who, precondition));
+    if (fl->n_fibers > 0)
+        SKB_TRY(fl->ops.ready(who, precondition));
     if (fl->n_bodies > 0) {
         if (!fl->bodies.has_operators())
             return set_error(SKB_ERR_INVALID, "%s: call skb_flow_group_set_body_operators after skb_flow_set_bodies", who);

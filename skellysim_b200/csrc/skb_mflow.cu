@@ -566,7 +566,7 @@ int skb_mflow_apply_matvec(skb_mflow *mf, const double *x_fibers, const double *
                            double *res_fibers, double *out_shell, double *v_bodies) {
     if (!mf || !(eta > 0))
         return set_error(SKB_ERR_INVALID, "skb_mflow_apply_matvec: bad arguments");
-    if (!mf->ops_ready)
+    if (!mf->ops_ready && mf->n_fibers > 0) // no fibers: the empty operator set, uploaded or not
         return set_error(SKB_ERR_STATE, "skb_mflow_apply_matvec: call skb_mflow_set_fiber_operators first");
     const long long nf = mf->n_fib, ns = mf->n_shell, nb = mf->n_body;
     if ((nf > 0 && (!x_fibers || !res_fibers)) || (ns > 0 && (!x_shell || !out_shell)) ||
@@ -680,7 +680,7 @@ static int mflow_system_args(skb_mflow *mf, const char *who, bool precondition, 
     if (!mf)
         return set_error(SKB_ERR_INVALID, "%s: NULL", who);
     SKB_TRY(mflow_prepare(mf)); // (a new partition drops the fiber operators)
-    if (!mf->ops_ready)
+    if (!mf->ops_ready && mf->n_fibers > 0) // no fibers: the empty operator set, uploaded or not
         return set_error(SKB_ERR_STATE, "%s: call skb_mflow_set_fiber_operators first", who);
     for (int g = 0; g < mf->n; ++g)
         SKB_TRY(flow_member_system_ready(mf->m[g].get(), who, precondition));

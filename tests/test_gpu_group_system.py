@@ -102,10 +102,12 @@ class Members:
             f0, f1, s0, s1 = self.parts[g][:4]
             for k in ops["D_1_0"]:
                 fl.set_fiber_class(k, ops["D_1_0"][k], ops["P"][k])
-                fl.set_fiber_class_derivatives(k, ops["D_2_0"][k], ops["D_3_0"][k], ops["D_4_0"][k])
+                if k in ops["D_2_0"]:  # (a class beyond the device build's node counts has none)
+                    fl.set_fiber_class_derivatives(k, ops["D_2_0"][k], ops["D_3_0"][k], ops["D_4_0"][k])
             fl.set_fiber_operators(ops["A"][f0:f1], ops["force"][f0:f1], ops["xs"][off[f0]:off[f1]],
                                    ops["length_prev"][f0:f1], ops["plus"][f0:f1])
-            fl.set_fiber_preconditioner([np.linalg.inv(A) for A in ops["A"][f0:f1]])
+            fl.set_fiber_preconditioner(ops["A_inv"][f0:f1] if "A_inv" in ops else
+                                        [np.linalg.inv(A) for A in ops["A"][f0:f1]])
             fl.group_set_body_operators(bodies["n_nodes"], bodies["weights"], bodies["ex"], bodies["ey"], bodies["ez"],
                                         [np.linalg.inv(A) for A in bodies["A"]] if body_inverse else None)
             fl.group_set_fiber_links(links["body"][f0:f1], links["site"][f0:f1], links["rigidity"][f0:f1])

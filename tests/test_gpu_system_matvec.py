@@ -57,10 +57,11 @@ def setup_flow(fl, dn, fib, shell, bodies, ops, links, build=None):
     load(fl, fib, shell, dict(pos=bodies["pos"], normals=bodies["normals"], centers=bodies["centers"]))
     for n in ops["D_1_0"]:
         fl.set_fiber_class(n, ops["D_1_0"][n], ops["P"][n])
-        fl.set_fiber_class_derivatives(n, ops["D_2_0"][n], ops["D_3_0"][n], ops["D_4_0"][n])
+        if n in ops["D_2_0"]:  # (a class beyond the device build's node counts has none)
+            fl.set_fiber_class_derivatives(n, ops["D_2_0"][n], ops["D_3_0"][n], ops["D_4_0"][n])
     if build is None:
         fl.set_fiber_operators(ops["A"], ops["force"], ops["xs"], ops["length_prev"], ops["plus"])
-        fl.set_fiber_preconditioner([np.linalg.inv(A) for A in ops["A"]])
+        fl.set_fiber_preconditioner(ops["A_inv"] if "A_inv" in ops else [np.linalg.inv(A) for A in ops["A"]])
     else:
         fl.build_fiber_operators(*build)
     if bodies["n_nodes"]:
