@@ -365,6 +365,37 @@ SKB_API int skb_flow_apply_matvec_device(skb_flow *fl, struct skb_dense *dn, con
 SKB_API int skb_flow_set_body_operators(skb_flow *fl, const int *n_nodes, int n_bodies, const double *node_weights,
                                         const double *ex, const double *ey, const double *ez, const double *A_inv);
 SKB_API int skb_flow_set_fiber_links(skb_flow *fl, const int *body, const double *site, const double *bending_rigidity);
+
+/* ---- rigid bodies placed on the device (DESIGN.md §3.6) ---------------------------------------------------------
+ * A rigid body's operators only move with it: placed at centre c and rotation R (x_i = c + R r_i, n_i = R n_i,ref,
+ * body_spherical.cpp:146-159), its A_ is Q A_0 Q^T with Q = blockdiag(R, ..., R) (one R per node and two for [U; w]),
+ * so A_^-1 = Q A_0^-1 Q^T, and per node E_i = [ex_i ey_i ez_i] = R E_i,0 R^T -- for spherical and ellipsoidal bodies
+ * alike.  The flow keeps the body-frame operators resident and forms the placed ones from them on the device, always
+ * from the body frame (never from the previous placement, so no rounding accumulates over the steps).
+ *   skb_flow_set_body_frames: once per run, after skb_flow_set_bodies (n_bodies and the node total must be its).  Per
+ *     body n_nodes[b]; per node the body-frame position node_pos_ref (node_positions_ref_, relative to the centre),
+ *     normal node_normal_ref (node_normals_ref_) and node_weights (node_weights_), 3 / 3 / 1 per node; ex0 / ey0 / ez0
+ *     and A_inv0 as skb_flow_set_body_operators takes them, of each body placed at identity orientation (any centre):
+ *     place(anything, identity) then update_cache_variables.  A_inv0 may be NULL (then the system preconditioner
+ *     refuses bodies).  Drops the resident body operators and links; keeps the body-frame E and inverses next to the
+ *     placed ones (twice the inverses' memory).  Refused as skb_flow_set_body_operators.
+ *   skb_flow_place_bodies: once per timestep.  centers 3 per body, orientations 4 per body, the unit quaternion
+ *     (w, x, y, z) of orientation_.  R is Eigen's toRotationMatrix formula of it, the same R for the nodes and the
+ *     operators.  Leaves the flow exactly as skb_flow_set_bodies(c + R r_ref, R n_ref, centers) followed by
+ *     skb_flow_set_body_operators with the placed operators would: the fiber links are dropped (set them again with
+ *     the new nucleation sites).  Refused (SKB_ERR_INVALID, before any launch, earlier state untouched): no frames, a
+ *     body count or node total of skb_flow_set_bodies other than the frames', an orientation that is not finite or
+ *     not unit within SKB_UNIT_QUATERNION_TOL (| w^2 + x^2 + y^2 + z^2 - 1 | above it: not a rotation), a group member
+ *     (skb_flow_group_place_bodies).
+ *   skb_flow_get_body_operators: the resident ex_ / ey_ / ez_ (3 x N_b each) and the resident inverses (concatenated,
+ *     column-major; a group member's: those of the bodies it owns rows of), as skb_flow_set_body_operators took them.
+ *     NULL skips an array.  Refused without resident operators (A_inv: without an inverse). */
+#define SKB_UNIT_QUATERNION_TOL 1e-12
+SKB_API int skb_flow_set_body_frames(skb_flow *fl, const int *n_nodes, int n_bodies, const double *node_pos_ref,
+                                     const double *node_normal_ref, const double *node_weights, const double *ex0,
+                                     const double *ey0, const double *ez0, const double *A_inv0);
+SKB_API int skb_flow_place_bodies(skb_flow *fl, const double *centers, const double *orientations);
+SKB_API int skb_flow_get_body_operators(skb_flow *fl, double *ex, double *ey, double *ez, double *A_inv);
 SKB_API int skb_flow_apply_system_matvec(skb_flow *fl, struct skb_dense *dn, const double *x, double eta, double *res);
 SKB_API int skb_flow_apply_system_matvec_device(skb_flow *fl, struct skb_dense *dn, const double *d_x, double eta,
                                                 double *d_res, void *stream);
@@ -444,6 +475,16 @@ SKB_API int skb_flow_group_set_body_operators(skb_flow *fl, const int *n_nodes, 
                                               const double *ez, const double *A_inv);
 SKB_API int skb_flow_group_set_fiber_links(skb_flow *fl, const int *body, const double *site,
                                            const double *bending_rigidity);
+/* skb_flow_set_body_frames / _place_bodies on a group member (arrays of ALL bodies).  The frames call also does what
+ * skb_flow_group_set_body_operators does: the member keeps the body-frame inverses of the bodies it owns rows of,
+ * lays out its body rows and sizes every buffer, the placement's included.  The place call then allocates no device
+ * memory and loads no kernel, so it may run while a peer on the same device waits on a flag; it refuses, locally, what
+ * skb_flow_place_bodies refuses and body rows other than the frames'.  Not a member: the single-device calls. */
+SKB_API int skb_flow_group_set_body_frames(skb_flow *fl, const int *n_nodes, int n_bodies, const double *node_pos_ref,
+                                           const double *node_normal_ref, const double *node_weights,
+                                           const double *ex0, const double *ey0, const double *ez0,
+                                           const double *A_inv0);
+SKB_API int skb_flow_group_place_bodies(skb_flow *fl, const double *centers, const double *orientations);
 SKB_API int skb_flow_group_apply_system_matvec_device(skb_flow *fl, struct skb_dense *dn, const double *d_x_local,
                                                       double eta, double *d_res_local, void *stream);
 SKB_API int skb_flow_group_apply_system_preconditioner_device(skb_flow *fl, struct skb_dense *dn,
@@ -543,6 +584,13 @@ SKB_API int skb_mflow_set_body_operators(skb_mflow *mf, const int *n_nodes, int 
                                          const double *ex, const double *ey, const double *ez, const double *A_inv);
 SKB_API int skb_mflow_set_fiber_links(skb_mflow *mf, const int *body, const double *site,
                                       const double *bending_rigidity);
+/* skb_flow_set_body_frames / _place_bodies over n devices, forwarded to every member (each keeps the body-frame
+ * inverses of the bodies it owns rows of); every member's refusals are checked before any member changes.  A new
+ * partition (a change of the node counts) wants the frames set again. */
+SKB_API int skb_mflow_set_body_frames(skb_mflow *mf, const int *n_nodes, int n_bodies, const double *node_pos_ref,
+                                      const double *node_normal_ref, const double *node_weights, const double *ex0,
+                                      const double *ey0, const double *ez0, const double *A_inv0);
+SKB_API int skb_mflow_place_bodies(skb_mflow *mf, const double *centers, const double *orientations);
 SKB_API int skb_mflow_apply_system_matvec(skb_mflow *mf, const double *x, double eta, double *res);
 SKB_API int skb_mflow_apply_system_preconditioner(skb_mflow *mf, const double *x, double *y);
 /* skb_flow_build_system_rhs over n devices, the same arguments (complete host arrays of all fibers and bodies, the whole

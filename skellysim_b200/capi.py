@@ -218,6 +218,13 @@ def library() -> C.CDLL:
                                                    + [C.c_double, C.c_double, C.c_void_p, C.c_void_p], C.c_int),
         "skb_group_body_pieces": ([C.POINTER(C.c_int), C.c_int, C.c_int64, C.c_int64, C.POINTER(C.c_int64), C.c_int,
                                    C.POINTER(C.c_int)], C.c_int),
+        "skb_flow_set_body_frames": ([ctxp, C.POINTER(C.c_int), C.c_int] + [_dp] * 7, C.c_int),
+        "skb_flow_place_bodies": ([ctxp, _dp, _dp], C.c_int),
+        "skb_flow_get_body_operators": ([ctxp, _dp, _dp, _dp, _dp], C.c_int),
+        "skb_flow_group_set_body_frames": ([ctxp, C.POINTER(C.c_int), C.c_int] + [_dp] * 7, C.c_int),
+        "skb_flow_group_place_bodies": ([ctxp, _dp, _dp], C.c_int),
+        "skb_mflow_set_body_frames": ([ctxp, C.POINTER(C.c_int), C.c_int] + [_dp] * 7, C.c_int),
+        "skb_mflow_place_bodies": ([ctxp, _dp, _dp], C.c_int),
         "skb_mflow_set_point_sources": ([ctxp, _dp, _dp, _dp, C.c_int], C.c_int),
         "skb_mflow_set_background": ([ctxp, C.POINTER(C.c_int), _dp, _dp], C.c_int),
     }
@@ -286,6 +293,25 @@ def _per_fiber(v, n_fibers):
 
 def _opt_p(x):
     return None if x is None else _p(x)
+
+
+def _frame_arrays(n_nodes, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0, A_inv0_list):
+    """the arrays of skb_flow_set_body_frames (A_inv0 column-major and concatenated, or None)"""
+    n = np.ascontiguousarray(n_nodes, dtype=np.int32)
+    w = np.ascontiguousarray(node_weights, dtype=np.float64).reshape(-1)
+    Ai = None if A_inv0_list is None else Flow._colmajor_concat(A_inv0_list)
+    return (n, _arr(node_pos_ref, 3), _arr(node_normal_ref, 3), w, _arr(ex0, 3), _arr(ey0, 3), _arr(ez0, 3), Ai)
+
+
+def _frame_call(fn, h, arrays):
+    n, *rest, Ai = arrays
+    _check(fn(h, n.ctypes.data_as(C.POINTER(C.c_int)), int(n.shape[0]), *(_p(a) for a in rest), _opt_p(Ai)))
+
+
+def _place_call(fn, h, centers, orientations):
+    c, q = _arr(centers, 3), _arr(orientations, 4)
+    assert c.shape[0] == q.shape[0]
+    _check(fn(h, _p(c), _p(q)))
 
 
 def _fiber_rhs_args(n_fibers, n_nodes, params, v_growth, force_scale, v_on_fibers, f_external):
@@ -835,6 +861,45 @@ class Flow:
         _check(library().skb_flow_set_body_operators(self._h, n.ctypes.data_as(C.POINTER(C.c_int)), int(n.shape[0]),
                                                      _p(w), _p(ex), _p(ey), _p(ez), None if Ai is None else _p(Ai)))
         self._body_sol = int(np.sum(3 * n + 6))
+        self._body_n = n
+
+    def set_body_frames(self, n_nodes, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0, A_inv0_list=None):
+        """The bodies' operators in their body frame, once per run after set_bodies: per body its node count, per node
+        node_positions_ref_ / node_normals_ref_ (N_b, 3) and node_weights_ (N_b,), ex_ / ey_ / ez_ (N_b, 3) and
+        A_^-1 ((3n+6, 3n+6) per body, a list, or None) of the body at identity orientation.  place_bodies then forms
+        the placed operators on the device."""
+        a = _frame_arrays(n_nodes, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0, A_inv0_list)
+        _frame_call(library().skb_flow_set_body_frames, self._h, a)
+        self._body_sol, self._body_n = int(np.sum(3 * a[0] + 6)), a[0]
+
+    def place_bodies(self, centers, orientations):
+        """Once per timestep: the bodies at centres (n_bodies, 3) and unit quaternions (w, x, y, z) (n_bodies, 4) --
+        their nodes, normals and operators, as set_bodies + set_body_operators with the placed ones would leave them.
+        The fiber links are dropped."""
+        _place_call(library().skb_flow_place_bodies, self._h, centers, orientations)
+
+    def get_body_operators(self, inverse=True):
+        """The resident body operators: dict(ex, ey, ez (N_b, 3) each, A_inv = per body its (3n+6, 3n+6) inverse, None
+        for a body whose inverse a group member does not keep; A_inv None with inverse=False)."""
+        n = np.asarray(getattr(self, "_body_n", np.zeros(0, dtype=np.int32)), dtype=np.int64)
+        nb = int(n.sum())
+        ex, ey, ez = (np.empty((nb, 3)) for _ in range(3))
+        node0 = np.concatenate([[0], np.cumsum(n)])
+        kept = np.ones(len(n), dtype=bool)
+        if getattr(self, "_member", False):  # the bodies with a node in the member's body rows
+            b0, b1 = self._ranges[4], self._ranges[5]
+            kept = (node0[:-1] < b1) & (node0[1:] > b0)
+        m = 3 * n + 6
+        Ai = np.empty(int(np.sum(m[kept] ** 2))) if inverse else None
+        _check(library().skb_flow_get_body_operators(self._h, _p(ex), _p(ey), _p(ez), _opt_p(Ai)))
+        out, o = [], 0
+        for k, mk in zip(kept, m):
+            if inverse and k:
+                out.append(Ai[o:o + mk * mk].reshape(mk, mk).T)
+                o += mk * mk
+            else:
+                out.append(None)
+        return dict(ex=ex, ey=ey, ez=ez, A_inv=out if inverse else None)
 
     def set_fiber_links(self, body=None, site=None, bending_rigidity=None):
         """Per fiber: body index (-1 free), lab-frame nucleation site (n_fibers, 3), bending_rigidity_; body=None: no
@@ -920,6 +985,7 @@ class Flow:
 
     def group_init(self, rank: int, size: int):
         _check(library().skb_flow_group_init(self._h, int(rank), int(size)))
+        self._member = int(size) > 1
 
     def group_export(self) -> bytes:
         buf = C.create_string_buffer(64)
@@ -957,6 +1023,19 @@ class Flow:
                                                            int(n.shape[0]), _p(w), _p(ex), _p(ey), _p(ez),
                                                            None if Ai is None else _p(Ai)))
         self._body_sol = int(np.sum(3 * n + 6))
+        self._body_n = n
+
+    def group_set_body_frames(self, n_nodes, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0,
+                              A_inv0_list=None):
+        """set_body_frames on a group member (arrays of ALL bodies): it keeps the body-frame inverses of the bodies it
+        owns rows of, lays out its body rows and sizes every buffer, as group_set_body_operators does."""
+        a = _frame_arrays(n_nodes, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0, A_inv0_list)
+        _frame_call(library().skb_flow_group_set_body_frames, self._h, a)
+        self._body_sol, self._body_n = int(np.sum(3 * a[0] + 6)), a[0]
+
+    def group_place_bodies(self, centers, orientations):
+        """place_bodies on a group member; allocates no device memory"""
+        _place_call(library().skb_flow_group_place_bodies, self._h, centers, orientations)
 
     def group_set_fiber_links(self, body=None, site=None, bending_rigidity=None):
         """set_fiber_links on a group member: body index, nucleation site (n, 3) and bending_rigidity_ of the OWN
@@ -1154,6 +1233,16 @@ class MultiFlow:
         _check(library().skb_mflow_set_body_operators(self._h, n.ctypes.data_as(C.POINTER(C.c_int)), int(n.shape[0]),
                                                       _p(w), _p(ex), _p(ey), _p(ez), None if Ai is None else _p(Ai)))
         self._body_sol = int(np.sum(3 * n + 6))
+
+    def set_body_frames(self, n_nodes, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0, A_inv0_list=None):
+        """As Flow.set_body_frames, for all bodies; every device keeps the body-frame inverses it owns rows of."""
+        a = _frame_arrays(n_nodes, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0, A_inv0_list)
+        _frame_call(library().skb_mflow_set_body_frames, self._h, a)
+        self._body_sol = int(np.sum(3 * a[0] + 6))
+
+    def place_bodies(self, centers, orientations):
+        """As Flow.place_bodies, on every device."""
+        _place_call(library().skb_mflow_place_bodies, self._h, centers, orientations)
 
     def set_fiber_links(self, body=None, site=None, bending_rigidity=None):
         """As Flow.set_fiber_links, for all fibers; body=None: no fiber is bound."""

@@ -11,6 +11,9 @@
 //                        body: the node rows and the 6 rows -K^T lambda + U with a fixed-order reduction tree.
 //                        <true>: the rows a group member of skb_mflow owns (BodyOps, skb_internal.hpp).
 //   system_rhs_rows_kernel  the shell and body rows of System::prep_state_for_solver's RHS: -v, and six zeros per body.
+//   body_place_kernel    a rigid body's operators at rotation R from those of its body frame (skb_flow_place_bodies,
+//                        DESIGN.md §3.6): A_^-1 = Q A_0^-1 Q^T, Q = blockdiag(R, ..., R), one 3 x 3 tile at a time,
+//                        and per node E_i = R E_i,0 R^T, E_i = [ex_i ey_i ez_i].
 // K_ is never stored: K U = u + w x (x_i - c) and K^T lambda = [sum lambda_i ; sum (x_i - c) x lambda_i]
 // (update_K_matrix, body_spherical.cpp:74-86).
 #pragma once
@@ -220,6 +223,121 @@ __global__ void __launch_bounds__(kBodyThreads)
         out[k - 3 * it.node_off] = -v[k - 3 * lo];
     if (threadIdx.x < 6 && it.node_off >= lo && it.node_off < hi)
         out[3 * it.n_nodes + threadIdx.x] = 0.0;
+}
+
+// ---- placement of a rigid body (body_place_kernel) ----
+// Every entry of A_ and of ex_ / ey_ / ez_ depends on the nodes only through differences of positions, their norms and
+// dot products with the normals, and K_ through x_i - c: placing the body at (c, R) maps A_0 to Q A_0 Q^T, so its
+// inverse to Q A_0^-1 Q^T, and E_i,0 to R E_i,0 R^T.  (3n + 6 is a multiple of 3: the [U; w] rows and columns form two
+// more tiles that R rotates like the node tiles.)
+struct PlaceBody {       // one body whose inverse is kept
+    long long inv_off;   // element offset of its (3n+6)^2 column-major inverse in the kept inverses
+    int m;               // 3n + 6
+    int body;            // index of its rotation
+    int cta0;            // first CTA of its column tiles (one CTA per 3 columns)
+    int pad;
+};
+
+constexpr int kPlaceThreads = 256;
+constexpr int kPlaceRows = 3 * kPlaceThreads; // rows of a column tile staged per pass
+
+// Y = R X R^T of one 3 x 3 tile, x[q][p] = X(p, q): Z = X R^T, then Y = R Z, each entry a three-term FMA chain
+__device__ __forceinline__ void rotate_tile(const double (&R)[9], const double (&x)[3][3], double (&y)[3][3]) {
+    double z[3][3];
+#pragma unroll
+    for (int p = 0; p < 3; ++p)
+#pragma unroll
+        for (int b = 0; b < 3; ++b)
+            z[b][p] = fma(x[2][p], R[3 * b + 2], fma(x[1][p], R[3 * b + 1], x[0][p] * R[3 * b]));
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+#pragma unroll
+        for (int b = 0; b < 3; ++b)
+            y[b][a] = fma(R[3 * a + 2], z[b][2], fma(R[3 * a + 1], z[b][1], R[3 * a] * z[b][0]));
+}
+
+// CTAs [0, n_inv_ctas): one column tile (3 consecutive columns, contiguous in the column-major inverse) of a kept
+// inverse each, streamed through shared memory in passes of kPlaceRows rows -- coalesced loads of X0, each thread
+// rotates one 3 x 3 tile in place, coalesced stores of X.  CTAs n_inv_ctas + b: body b's nodes, E_i = R E_i,0 R^T.
+// R: 9 per body, row-major.
+__global__ void __launch_bounds__(kPlaceThreads)
+    body_place_kernel(const PlaceBody *__restrict__ place, int n_place, int n_inv_ctas, const BodyItem *__restrict__ bodies,
+                      const double *__restrict__ R, const double *__restrict__ X0, double *__restrict__ X,
+                      const double *__restrict__ ex0, const double *__restrict__ ey0, const double *__restrict__ ez0,
+                      double *__restrict__ ex, double *__restrict__ ey, double *__restrict__ ez) {
+    __shared__ double tile[3][kPlaceRows];
+    const int t = threadIdx.x;
+    if ((int)blockIdx.x >= n_inv_ctas) {
+        const int b = (int)blockIdx.x - n_inv_ctas;
+        const BodyItem it = bodies[b];
+        double Rb[9];
+#pragma unroll
+        for (int k = 0; k < 9; ++k)
+            Rb[k] = R[9 * b + k];
+        for (int i = t; i < it.n_nodes; i += kPlaceThreads) {
+            const long long g = 3 * (it.node_off + i);
+            double e[3][3], y[3][3];
+#pragma unroll
+            for (int p = 0; p < 3; ++p) {
+                e[0][p] = ex0[g + p];
+                e[1][p] = ey0[g + p];
+                e[2][p] = ez0[g + p];
+            }
+            rotate_tile(Rb, e, y);
+#pragma unroll
+            for (int a = 0; a < 3; ++a) {
+                ex[g + a] = y[0][a];
+                ey[g + a] = y[1][a];
+                ez[g + a] = y[2][a];
+            }
+        }
+        return;
+    }
+    int lo = 0, hi = n_place - 1; // the last body whose cta0 <= blockIdx.x
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (place[mid].cta0 <= (int)blockIdx.x)
+            lo = mid;
+        else
+            hi = mid - 1;
+    }
+    const PlaceBody pb = place[lo];
+    const int m = pb.m;
+    const long long col = 3LL * ((int)blockIdx.x - pb.cta0);
+    const double *src = X0 + pb.inv_off + col * m;
+    double *dst = X + pb.inv_off + col * m;
+    double Rb[9];
+#pragma unroll
+    for (int k = 0; k < 9; ++k)
+        Rb[k] = R[9 * pb.body + k];
+    for (int r0 = 0; r0 < m; r0 += kPlaceRows) {
+        const int rows = min(kPlaceRows, m - r0);
+#pragma unroll
+        for (int q = 0; q < 3; ++q)
+            for (int i = t; i < rows; i += kPlaceThreads)
+                tile[q][i] = src[(long long)q * m + r0 + i];
+        __syncthreads();
+        if (3 * t < rows) { // rows is a multiple of 3: the thread's tile is whole
+            double x[3][3], y[3][3];
+#pragma unroll
+            for (int q = 0; q < 3; ++q)
+#pragma unroll
+                for (int p = 0; p < 3; ++p)
+                    x[q][p] = tile[q][3 * t + p];
+            rotate_tile(Rb, x, y);
+#pragma unroll
+            for (int q = 0; q < 3; ++q)
+#pragma unroll
+                for (int p = 0; p < 3; ++p)
+                    tile[q][3 * t + p] = y[q][p];
+        }
+        __syncthreads();
+#pragma unroll
+        for (int q = 0; q < 3; ++q)
+            for (int i = t; i < rows; i += kPlaceThreads)
+                dst[(long long)q * m + r0 + i] = tile[q][i];
+        __syncthreads();
+    }
 }
 
 } // namespace skb

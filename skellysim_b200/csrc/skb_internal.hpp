@@ -279,6 +279,30 @@ class BodyOps {
     // check_only: the checks and nothing else
     int set_links(const OwnFibers &own, const FiberOps &ops, int n_bodies, const double *centers, const int *body,
                   const double *site, const double *rigidity, cudaStream_t st, bool check_only = false);
+    // The body frame of rigid bodies (skb_flow_set_body_frames): per body n_nodes (summing to n_body_nodes), the
+    // reference nodes, normals and weights (3, 3, 1 per node), ex_ / ey_ / ez_ and A_^-1 (may be NULL) at identity
+    // orientation.  Kept resident next to the placed operators, the inverses of the bodies a member owns rows of only;
+    // sizes every buffer set_operators and place use and loads the placement kernel, and drops the placed operators.
+    // Checked first: a refusal leaves the earlier frames and operators
+    int set_frames(const int *n_nodes, int n_bodies, long long n_body_nodes, const double *pos_ref,
+                   const double *normal_ref, const double *node_weights, const double *ex0, const double *ey0,
+                   const double *ez0, const double *A_inv0, cudaStream_t st, long long lo = 0, long long hi = -1);
+    bool has_frames() const { return frames_set_; }
+    int frame_bodies() const { return (int)frame_n_.size(); }
+    long long frame_nodes() const { return (long long)frame_w_.size(); }
+    const int *frame_node_counts() const { return frame_n_.data(); }
+    bool frame_window(long long lo, long long hi) const { return frame_lo_ == lo && frame_hi_ == hi; }
+    // the nodes and normals at rotations R (9 per body, row-major) and centres: x_i = c + R r_i, n_i = R n_i,ref
+    void placed_geometry(const double *R, const double *centers, std::vector<double> &pos,
+                         std::vector<double> &normals) const;
+    // the operators of the frames at rotations R, with r_body / centers the flow's geometry (placed_geometry): the
+    // state set_operators would leave with the placed operators; allocates nothing.  The caller has checked that
+    // the frames match the flow's bodies
+    int place(const double *R, const double *r_body, const double *centers, cudaStream_t st);
+    // the resident ex_ / ey_ / ez_ (3 per node) and the kept inverses (concatenated, column-major); NULL skips one
+    int read(double *ex, double *ey, double *ez, double *A_inv, cudaStream_t st) const;
+    long long kept_inverse_elements() const { return inv_own_; }
+
     void drop_operators() { ops_set_ = false; }
     void drop_links() { links_set_ = false; }
     bool has_operators() const { return ops_set_; }
@@ -307,9 +331,23 @@ class BodyOps {
                  long long n_shell_rows, double *d_rhs_shell, cudaStream_t st, int *launches) const;
 
   private:
+    struct Plan; // the layout of one set of node counts and row window (skb_body.cu)
+    int plan(const char *who, const int *n_nodes, int n_bodies, long long n_body_nodes, const double *node_weights,
+             bool with_inverse, long long lo, long long hi, Plan &pl) const;
+    int upload_layout(const Plan &pl, const double *r_body, const double *centers, const double *node_weights,
+                      cudaStream_t st);
+    void commit(const Plan &pl, bool with_inverse);
+
     bool ops_set_ = false, inv_set_ = false, links_set_ = false, any_bound_ = false;
     int n_bodies_ = 0, n_fibers_ = 0, n_gemv_ = 0;
-    long long sol_size_ = 0;
+    long long sol_size_ = 0, inv_own_ = 0;
+    // the frames: host copies of what place needs, the placement table of the kept inverses
+    bool frames_set_ = false, frame_inv_ = false;
+    std::vector<int> frame_n_;
+    std::vector<double> frame_r_, frame_nrm_, frame_w_;
+    long long frame_lo_ = 0, frame_hi_ = -1;
+    int n_place_ = 0, place_ctas_ = 0;
+    DevBuf ex0_, ey0_, ez0_, a_inv0_, place_items_, rot_;
     bool windowed_ = false; // a member's rows: bodies [win_b0_, win_b1_) have nodes in [win_lo_, win_hi_)
     int win_b0_ = 0, win_b1_ = 0;
     long long win_lo_ = 0, win_hi_ = 0;
@@ -456,6 +494,13 @@ int flow_member_body_operators(skb_flow *fl, const int *n_nodes, int n_bodies, c
                                const double *ex, const double *ey, const double *ez, const double *A_inv);
 int flow_member_fiber_links(skb_flow *fl, const int *body, const double *site, const double *rigidity,
                             bool check_only);
+// skb_mflow_set_body_frames / _place_bodies on a member (arguments of ALL bodies): the frames; the refusals of a
+// placement, with the rotations R (9 per body) it places at; the placement itself, after every member's refusals
+int flow_member_body_frames(skb_flow *fl, const int *n_nodes, int n_bodies, const double *pos_ref,
+                            const double *normal_ref, const double *node_weights, const double *ex0, const double *ey0,
+                            const double *ez0, const double *A_inv0);
+int flow_member_place_args(skb_flow *fl, const double *centers, const double *orientations, std::vector<double> &R);
+int flow_member_place(skb_flow *fl, const double *centers, const std::vector<double> &R);
 // the state the system calls need (system_args without the dense operator): an error naming `who` unless it is there
 int flow_member_system_ready(skb_flow *fl, const char *who, bool precondition);
 int flow_size_system(skb_flow *fl); // sizes the buffers the two calls below use (before any member launches)

@@ -1703,6 +1703,137 @@ int skb_flow_set_fiber_links(skb_flow *fl, const int *body, const double *site, 
 
 } // extern "C"
 
+// ---- rigid bodies placed from their body frame (BodyOps::set_frames / ::place, DESIGN.md §3.6) --------------------
+
+// R (row-major) of a unit quaternion (w, x, y, z): the formula of Eigen's QuaternionBase::toRotationMatrix
+static void quaternion_rotation(const double *q, double *R) {
+    const double w = q[0], x = q[1], y = q[2], z = q[3];
+    const double tx = 2.0 * x, ty = 2.0 * y, tz = 2.0 * z;
+    const double twx = tx * w, twy = ty * w, twz = tz * w;
+    const double txx = tx * x, txy = ty * x, txz = tz * x;
+    const double tyy = ty * y, tyz = tz * y, tzz = tz * z;
+    R[0] = 1.0 - (tyy + tzz), R[1] = txy - twz, R[2] = txz + twy;
+    R[3] = txy + twz, R[4] = 1.0 - (txx + tzz), R[5] = tyz - twx;
+    R[6] = txz - twy, R[7] = tyz + twx, R[8] = 1.0 - (txx + tyy);
+}
+
+// the frames of the flow's bodies, for its body rows [lo, hi) (hi < 0: every row)
+static int body_frames(skb_flow *fl, const char *who, const int *n_nodes, int n_bodies, const double *pos_ref,
+                       const double *normal_ref, const double *node_weights, const double *ex0, const double *ey0,
+                       const double *ez0, const double *A_inv0, long long lo, long long hi) {
+    if (n_bodies != fl->n_bodies)
+        return set_error(SKB_ERR_INVALID, "%s: %d bodies, skb_flow_set_bodies has %d", who, n_bodies, fl->n_bodies);
+    if (n_bodies > 0 && (!n_nodes || !pos_ref || !normal_ref || !node_weights || !ex0 || !ey0 || !ez0))
+        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    return fl->bodies.set_frames(n_nodes, n_bodies, fl->n_body, pos_ref, normal_ref, node_weights, ex0, ey0, ez0,
+                                 A_inv0, fl->stream, lo, hi);
+}
+
+// the refusals of a placement, before any state changes: frames that match the flow's bodies and its body rows
+// [lo, hi), finite unit quaternions.  R: the rotations, 9 per body
+static int placement_args(skb_flow *fl, const char *who, const double *centers, const double *orientations,
+                          long long lo, long long hi, std::vector<double> &R) {
+    const BodyOps &b = fl->bodies;
+    if (!b.has_frames())
+        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_body_frames first", who);
+    if (b.frame_bodies() != fl->n_bodies || b.frame_nodes() != fl->n_body)
+        return set_error(SKB_ERR_INVALID, "%s: the flow has %d bodies of %lld nodes, the frames %d bodies of %lld nodes "
+                                          "(set the frames again after skb_flow_set_bodies changes them)", who,
+                         fl->n_bodies, fl->n_body, b.frame_bodies(), b.frame_nodes());
+    if (!b.frame_window(lo, hi))
+        return set_error(SKB_ERR_INVALID, "%s: the body rows changed since the frames were set (set them again)", who);
+    const int nb = fl->n_bodies;
+    if (nb > 0 && (!centers || !orientations))
+        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
+    R.resize((size_t)nb * 9);
+    for (int i = 0; i < nb; ++i) {
+        const double *q = orientations + 4 * (size_t)i;
+        const double n2 = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
+        if (!(std::fabs(n2 - 1.0) <= SKB_UNIT_QUATERNION_TOL))
+            return set_error(SKB_ERR_INVALID, "%s: orientation %d = (%g, %g, %g, %g) is not a finite unit quaternion "
+                                              "(|q|^2 - 1 = %g, tolerance %g)", who, i, q[0], q[1], q[2], q[3],
+                             n2 - 1.0, SKB_UNIT_QUATERNION_TOL);
+        quaternion_rotation(q, &R[9 * (size_t)i]);
+    }
+    return SKB_OK;
+}
+
+// after placement_args: the nodes and normals through skb_flow_set_bodies (which drops the operators and the links),
+// then the operators from the frames
+static int place_bodies(skb_flow *fl, const double *centers, const std::vector<double> &R) {
+    std::vector<double> pos, nrm;
+    fl->bodies.placed_geometry(R.data(), centers, pos, nrm);
+    SKB_TRY(skb_flow_set_bodies(fl, pos.data(), nrm.data(), fl->n_body, centers, fl->n_bodies));
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    return fl->bodies.place(R.data(), fl->h_r_body.data(), fl->h_centers.data(), fl->stream);
+}
+
+int skb::flow_member_body_frames(skb_flow *fl, const int *n_nodes, int n_bodies, const double *pos_ref,
+                                 const double *normal_ref, const double *node_weights, const double *ex0,
+                                 const double *ey0, const double *ez0, const double *A_inv0) {
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    SKB_TRY(prepare_matvec_targets(fl));
+    const bool member = fl->grp.member();
+    return body_frames(fl, "skb_mflow_set_body_frames", n_nodes, n_bodies, pos_ref, normal_ref, node_weights, ex0,
+                       ey0, ez0, A_inv0, member ? fl->ba : 0, member ? fl->bb : -1);
+}
+
+int skb::flow_member_place_args(skb_flow *fl, const double *centers, const double *orientations,
+                                std::vector<double> &R) {
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    SKB_TRY(prepare_matvec_targets(fl));
+    const bool member = fl->grp.member();
+    return placement_args(fl, "skb_mflow_place_bodies", centers, orientations, member ? fl->ba : 0,
+                          member ? fl->bb : -1, R);
+}
+
+int skb::flow_member_place(skb_flow *fl, const double *centers, const std::vector<double> &R) {
+    return place_bodies(fl, centers, R);
+}
+
+extern "C" {
+
+int skb_flow_set_body_frames(skb_flow *fl, const int *n_nodes, int n_bodies, const double *node_pos_ref,
+                             const double *node_normal_ref, const double *node_weights, const double *ex0,
+                             const double *ey0, const double *ez0, const double *A_inv0) {
+    const char *who = "skb_flow_set_body_frames";
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    if (fl->grp.member())
+        return set_error(SKB_ERR_INVALID, "%s: a group member sets its frames with skb_flow_group_set_body_frames", who);
+    return body_frames(fl, who, n_nodes, n_bodies, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0, A_inv0,
+                       0, -1);
+}
+
+int skb_flow_place_bodies(skb_flow *fl, const double *centers, const double *orientations) {
+    const char *who = "skb_flow_place_bodies";
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    if (fl->grp.member())
+        return set_error(SKB_ERR_INVALID, "%s: a group member places its bodies with skb_flow_group_place_bodies", who);
+    std::vector<double> R;
+    SKB_TRY(placement_args(fl, who, centers, orientations, 0, -1, R));
+    return place_bodies(fl, centers, R);
+}
+
+int skb_flow_get_body_operators(skb_flow *fl, double *ex, double *ey, double *ez, double *A_inv) {
+    const char *who = "skb_flow_get_body_operators";
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    if (fl->n_bodies > 0 && !fl->bodies.has_operators())
+        return set_error(SKB_ERR_INVALID, "%s: no body operators are resident (skb_flow_set_body_operators or "
+                                          "skb_flow_place_bodies after skb_flow_set_bodies)", who);
+    if (fl->n_bodies > 0 && A_inv && !fl->bodies.has_inverse())
+        return set_error(SKB_ERR_INVALID, "%s: the resident body operators have no A_inv", who);
+    if (fl->n_bodies == 0)
+        return SKB_OK;
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    return fl->bodies.read(ex, ey, ez, A_inv, fl->stream);
+}
+
+} // extern "C"
+
 // The checks of the system operator (matvec: stresslet_plus_complementary in dn; precondition: M_inv and the
 // inverses), all before any launch; then the flow's device is current and its target list resolved.
 static int system_args(skb_flow *fl, skb_dense *dn, const char *who, bool precondition, bool args) {
@@ -2222,6 +2353,51 @@ int skb_flow_group_set_body_operators(skb_flow *fl, const int *n_nodes, int n_bo
     SKB_TRY(load_dense_kernels()); // the preconditioner's M_inv rows (and the matvec's without the streamer)
     fl->grp.set_body_rows(pieces, group_ranges(fl));
     return SKB_OK;
+}
+
+int skb_flow_group_set_body_frames(skb_flow *fl, const int *n_nodes, int n_bodies, const double *node_pos_ref,
+                                   const double *node_normal_ref, const double *node_weights, const double *ex0,
+                                   const double *ey0, const double *ez0, const double *A_inv0) {
+    const char *who = "skb_flow_group_set_body_frames";
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    if (!fl->grp.member())
+        return skb_flow_set_body_frames(fl, n_nodes, n_bodies, node_pos_ref, node_normal_ref, node_weights, ex0, ey0,
+                                        ez0, A_inv0);
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    OwnFibers own;
+    SKB_TRY(own_fibers(fl, who, own)); // the target ranges resolved, the window's layout checked
+    SKB_TRY(body_frames(fl, who, n_nodes, n_bodies, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0, A_inv0,
+                        fl->ba, fl->bb));
+    std::vector<RowPiece> pieces;
+    if (!body_row_pieces(n_nodes, n_bodies, fl->ba, fl->bb, pieces))
+        return set_error(SKB_ERR_STATE, "%s: the body rows [%lld, %lld) make %d pieces (at most %d)", who, fl->ba,
+                         fl->bb, (int)pieces.size(), kMaxRowPieces);
+    long long sol = 0;
+    for (int b = 0; b < n_bodies; ++b)
+        sol += 3LL * n_nodes[b] + 6;
+    // every buffer of the three whole-vector calls at its final size, as skb_flow_group_set_body_operators does
+    SKB_TRY(fl->sys_rb.ensure((size_t)sol * 8 + 8));
+    SKB_TRY(flow_size_system(fl));
+    SKB_TRY(rhs_buffers(fl));
+    SKB_TRY(fl->ops.size_rhs(own.count()));
+    SKB_TRY(load_dense_kernels());
+    fl->grp.set_body_rows(pieces, group_ranges(fl));
+    return SKB_OK;
+}
+
+int skb_flow_group_place_bodies(skb_flow *fl, const double *centers, const double *orientations) {
+    const char *who = "skb_flow_group_place_bodies";
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    if (!fl->grp.member())
+        return skb_flow_place_bodies(fl, centers, orientations);
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    SKB_TRY(prepare_matvec_targets(fl));
+    std::vector<double> R;
+    SKB_TRY(placement_args(fl, who, centers, orientations, fl->ba, fl->bb, R));
+    SKB_TRY(place_bodies(fl, centers, R));
+    return prepare_matvec_targets(fl); // the new body rows' targets now, not at the first matvec
 }
 
 int skb_flow_group_set_fiber_links(skb_flow *fl, const int *body, const double *site, const double *bending_rigidity) {

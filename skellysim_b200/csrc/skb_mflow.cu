@@ -662,6 +662,39 @@ int skb_mflow_set_body_operators(skb_mflow *mf, const int *n_nodes, int n_bodies
     return SKB_OK;
 }
 
+int skb_mflow_set_body_frames(skb_mflow *mf, const int *n_nodes, int n_bodies, const double *node_pos_ref,
+                              const double *node_normal_ref, const double *node_weights, const double *ex0,
+                              const double *ey0, const double *ez0, const double *A_inv0) {
+    const char *who = "skb_mflow_set_body_frames";
+    if (!mf)
+        return set_error(SKB_ERR_INVALID, "%s: NULL", who);
+    if (n_bodies != mf->n_bodies)
+        return set_error(SKB_ERR_INVALID, "%s: %d bodies, skb_mflow_set_bodies has %d", who, n_bodies, mf->n_bodies);
+    if (n_bodies > 0 && (!n_nodes || !node_pos_ref || !node_normal_ref || !node_weights || !ex0 || !ey0 || !ez0))
+        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
+    SKB_TRY(mflow_prepare(mf));
+    // every member checks the same complete arrays first, so all of them refuse or none does
+    SKB_TRY(mf->workers->run([&](int g) -> int {
+        return flow_member_body_frames(mf->m[g].get(), n_nodes, n_bodies, node_pos_ref, node_normal_ref, node_weights,
+                                       ex0, ey0, ez0, A_inv0);
+    }));
+    mf->body_n.assign(n_nodes, n_nodes + n_bodies); // the layout every placement keeps
+    mf->body_sol = 0;
+    for (int n : mf->body_n)
+        mf->body_sol += 3LL * n + 6;
+    return SKB_OK;
+}
+
+int skb_mflow_place_bodies(skb_mflow *mf, const double *centers, const double *orientations) {
+    if (!mf)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_place_bodies: NULL");
+    SKB_TRY(mflow_prepare(mf));
+    std::vector<std::vector<double>> R((size_t)mf->n);
+    for (int g = 0; g < mf->n; ++g) // every member's refusals before any member places
+        SKB_TRY(flow_member_place_args(mf->m[g].get(), centers, orientations, R[(size_t)g]));
+    return mf->workers->run([&](int g) -> int { return flow_member_place(mf->m[g].get(), centers, R[(size_t)g]); });
+}
+
 int skb_mflow_set_fiber_links(skb_mflow *mf, const int *body, const double *site, const double *bending_rigidity) {
     const char *who = "skb_mflow_set_fiber_links";
     if (!mf)
