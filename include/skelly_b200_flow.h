@@ -434,6 +434,70 @@ SKB_API int skb_flow_build_system_rhs_device(skb_flow *fl, const skb_fiber_param
                                              const double *d_body_forces, const double *d_body_torques, double dt,
                                              double eta, double *d_rhs, void *stream);
 
+/* ---- the solve of the whole system ----------------------------------------------------------------------------------
+ * Solver::solve (solver_hydro.cpp:64-95) as the reference configures Belos: restarted GMRES with right preconditioning
+ * (each Arnoldi step is z = P^-1 v_k, then w = A z, with the two system calls above), x0 = 0 (Solver's X_ is a fresh zero
+ * vector at every System::solve), ICGS orthogonalization (two classical Gram-Schmidt passes, then the normalization), the
+ * Hessenberg least-squares problem by Givens rotations on the host.  The implicit residual estimate |g_{k+1}| ends a cycle
+ * once it is <= tol ||b||_2; then x += P^-1 V y and the explicit ||b - A x||_2 decides: <= tol ||b||_2 is convergence,
+ * anything else restarts from x (never convergence on the implicit estimate alone).  A cycle also ends after num_blocks
+ * steps (a restart from x) and at max_iters Arnoldi steps in all (converged = 0 unless the explicit residual then meets
+ * tol; the current iterate is returned, SKB_OK).  A new vector whose norm after the two passes is 0 or at most
+ * 16 u (u = 2^-53) of its norm before them spans nothing new ("happy breakdown"): the Krylov space is invariant, the
+ * step is taken as an exact solve in it, and the explicit check follows.  ||b|| = 0: x = 0, converged, 0 iterations.
+ * Belos's defaults, which the reference keeps: Num Blocks 300, Maximum Iterations 1000; gmres_tol defaults to 1e-10.
+ *
+ * The basis V stays on the device (column-major, num_blocks + 1 columns); one Arnoldi step is three passes over it
+ * (DESIGN.md §3.8), every dot summed in a fixed order without atomics, so a solve is bitwise reproducible run to run.
+ * After each step the Hessenberg column goes to pinned host memory with one event wait: the call is asynchronous on
+ * `stream` except for that wait per step and one per cycle end.
+ *
+ * skb_flow_set_gmres: sizes the workspace for the flow's current solution size and up to num_blocks basis vectors per
+ *   cycle ((num_blocks + 1) x n doubles for V: 971 MB at n = 403 206 and 300 blocks).  Call it after the set-up that
+ *   fixes the solution size (skb_flow_set_fibers / _periphery / _bodies / skb_flow_set_body_operators), and again when it
+ *   changes.  Refused: num_blocks outside [1, SKB_GMRES_MAX_BLOCKS].
+ * skb_flow_solve_system(_device): x = A^-1 rhs on whole solution vectors (the layout of skb_flow_apply_system_matvec);
+ *   dn holds SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY and SKB_DENSE_M_INV (NULL only without periphery).  info is filled
+ *   on SKB_OK; history, if not NULL, holds max_iters + 1 doubles and receives the implicit relative residual after each
+ *   of the info->iterations steps (history[0] = 1, the start x0 = 0).  The host form ships rhs once and x once; the
+ *   _device form takes both on the flow's device.  Refused (SKB_ERR_INVALID, before any launch, x and earlier state
+ *   untouched): everything skb_flow_apply_system_matvec and _preconditioner refuse, eta <= 0, tol <= 0 or not finite,
+ *   num_blocks outside [1, the num_blocks of skb_flow_set_gmres], max_iters < 0, NULL info, no skb_flow_set_gmres for
+ *   the current solution size.  A solution vector of length 0 returns SKB_OK (converged, 0 iterations) without a
+ *   launch or a workspace. */
+#define SKB_GMRES_MAX_BLOCKS 1024
+typedef struct skb_solve_info {
+    int32_t converged;        /* 1: ||b - A x||_2 <= tol ||b||_2 */
+    int32_t iterations;       /* Arnoldi steps in all */
+    int32_t restarts;         /* cycles after the first */
+    int32_t reserved;
+    double implicit_residual; /* the last implicit estimate |g_{k+1}| / ||b||_2 */
+    double explicit_residual; /* ||b - A x||_2 / ||b||_2 of the returned x (0 when ||b|| = 0) */
+    double residual;          /* ||b - A x||_2, what Solver::get_residual logs */
+} skb_solve_info;
+SKB_API int skb_flow_set_gmres(skb_flow *fl, int num_blocks);
+SKB_API int skb_flow_solve_system(skb_flow *fl, struct skb_dense *dn, const double *rhs, double eta, double tol,
+                                  int num_blocks, int max_iters, double *x, skb_solve_info *info, double *history);
+SKB_API int skb_flow_solve_system_device(skb_flow *fl, struct skb_dense *dn, const double *d_rhs, double eta,
+                                         double tol, int num_blocks, int max_iters, double *d_x, skb_solve_info *info,
+                                         double *history, void *stream);
+/* One rank per GPU (the local-vector calls below): skb_flow_set_gmres on a group member sizes the workspace for its
+ * LOCAL rows (after skb_flow_group_set_body_operators, which lays them out); skb_flow_group_solve_system_device solves
+ * on the local vectors d_rhs_local / d_x_local, with A and P^-1 the member's skb_flow_group_apply_system_matvec_device
+ * (dn_spc: its rows of SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY) and _preconditioner_device (dn_minv: its rows of
+ * SKB_DENSE_M_INV).  Every dot product is an all-reduce over the members through the group window (DESIGN.md §4): each
+ * member adds every member's partial sums in rank order, so all of them hold bitwise the same Hessenberg column, take
+ * the same decisions and stop at the same step, and return bitwise the same info and history.  A member that owns no
+ * row takes part all the same (its vectors may be NULL).  Every member must call it with the same tol, num_blocks and
+ * max_iters; a refusal is local to the rank (as for the other group calls: agree on the set-up's return codes first).
+ * Refused besides what skb_flow_solve_system refuses: what the two local-vector calls refuse, a workspace set up for
+ * other target ranges.  On a flow that is no member: skb_flow_solve_system_device (dn_spc and dn_minv may be one handle
+ * holding both). */
+SKB_API int skb_flow_group_solve_system_device(skb_flow *fl, struct skb_dense *dn_spc, struct skb_dense *dn_minv,
+                                               const double *d_rhs_local, double eta, double tol, int num_blocks,
+                                               int max_iters, double *d_x_local, skb_solve_info *info,
+                                               double *history, void *stream);
+
 /* ---- the whole-vector calls on one rank per GPU ---------------------------------------------------------------------
  * A group member (skb_flow_group_init ... skb_flow_group_warmup above) applies A, P^-1 and builds the RHS on its LOCAL
  * vector: its own rows of the whole vector [fibers | shell | bodies], in ascending global order --
@@ -600,6 +664,16 @@ SKB_API int skb_mflow_apply_system_preconditioner(skb_mflow *mf, const double *x
 SKB_API int skb_mflow_build_system_rhs(skb_mflow *mf, const skb_fiber_params *params, const double *v_growth,
                                        const double *force_scale, const double *f_external,
                                        const double *body_forces_torques, double dt, double eta, double *rhs);
+/* skb_flow_solve_system over n devices: complete host rhs in, complete host x out.  skb_mflow_set_gmres lays out every
+ * member's local rows (as skb_flow_group_set_body_operators does, after skb_mflow_set_body_operators or
+ * _set_body_frames) and sizes its workspace; each member thread then runs skb_flow_group_solve_system_device on its
+ * rows, so every member reports bitwise the same info and history.  Refusals as skb_flow_solve_system's and
+ * skb_mflow_apply_system_matvec's / _preconditioner's, every member's checked before any device starts; no
+ * skb_mflow_set_gmres since the partition or the bodies' node counts changed.  With one device it is the skb_flow path,
+ * bitwise. */
+SKB_API int skb_mflow_set_gmres(skb_mflow *mf, int num_blocks);
+SKB_API int skb_mflow_solve_system(skb_mflow *mf, const double *rhs, double eta, double tol, int num_blocks,
+                                   int max_iters, double *x, skb_solve_info *info, double *history);
 /* skb_flow_set_point_sources / _set_background on every device: skb_mflow_velocity_at_targets and
  * skb_mflow_build_system_rhs include them */
 SKB_API int skb_mflow_set_point_sources(skb_mflow *mf, const double *positions, const double *forces,

@@ -35,6 +35,18 @@ class FlowStats(C.Structure):
     _fields_ = [("device_ms", C.c_double), ("total_ms", C.c_double), ("n_pairs", C.c_int64), ("launches", C.c_int32)]
 
 
+class SolveInfo(C.Structure):
+    """skb_solve_info (include/skelly_b200_flow.h): the outcome of skb_flow_solve_system."""
+    _fields_ = [("converged", C.c_int32), ("iterations", C.c_int32), ("restarts", C.c_int32), ("reserved", C.c_int32),
+                ("implicit_residual", C.c_double), ("explicit_residual", C.c_double), ("residual", C.c_double)]
+
+    def as_dict(self):
+        return {name: getattr(self, name) for name, _ in self._fields_ if name != "reserved"}
+
+
+GMRES_MAX_BLOCKS = 1024  # SKB_GMRES_MAX_BLOCKS
+
+
 class DenseStats(C.Structure):
     _fields_ = [("kernel_ms", C.c_double), ("total_ms", C.c_double), ("bytes", C.c_int64)]
 
@@ -227,6 +239,16 @@ def library() -> C.CDLL:
         "skb_mflow_place_bodies": ([ctxp, _dp, _dp], C.c_int),
         "skb_mflow_set_point_sources": ([ctxp, _dp, _dp, _dp, C.c_int], C.c_int),
         "skb_mflow_set_background": ([ctxp, C.POINTER(C.c_int), _dp, _dp], C.c_int),
+        "skb_flow_set_gmres": ([ctxp, C.c_int], C.c_int),
+        "skb_flow_solve_system": ([ctxp, ctxp, _dp, C.c_double, C.c_double, C.c_int, C.c_int, _dp,
+                                   C.POINTER(SolveInfo), _dp], C.c_int),
+        "skb_flow_solve_system_device": ([ctxp, ctxp, C.c_void_p, C.c_double, C.c_double, C.c_int, C.c_int,
+                                          C.c_void_p, C.POINTER(SolveInfo), _dp, C.c_void_p], C.c_int),
+        "skb_flow_group_solve_system_device": ([ctxp, ctxp, ctxp, C.c_void_p, C.c_double, C.c_double, C.c_int, C.c_int,
+                                                C.c_void_p, C.POINTER(SolveInfo), _dp, C.c_void_p], C.c_int),
+        "skb_mflow_set_gmres": ([ctxp, C.c_int], C.c_int),
+        "skb_mflow_solve_system": ([ctxp, _dp, C.c_double, C.c_double, C.c_int, C.c_int, _dp, C.POINTER(SolveInfo),
+                                    _dp], C.c_int),
     }
     global BOUND_FUNCTIONS
     BOUND_FUNCTIONS = tuple(sorted(sig))
@@ -976,6 +998,36 @@ class Flow:
                                                           vp(d_f_external), vp(d_body_forces), vp(d_body_torques),
                                                           float(dt), float(eta), vp(d_rhs), vp(stream)))
 
+    def set_gmres(self, num_blocks: int = 300):
+        """Size the workspace of solve_system for the current solution size and up to num_blocks basis vectors."""
+        _check(library().skb_flow_set_gmres(self._h, int(num_blocks)))
+
+    def solve_system(self, rhs, eta, dense=None, tol=1e-10, num_blocks=300, max_iters=1000):
+        """Solver::solve (solver_hydro.cpp:64-95): x = A^-1 rhs by restarted right-preconditioned GMRES on the device.
+        Returns (x, info, history): info a dict of skb_solve_info, history the implicit relative residual after each
+        Arnoldi step (history[0] = 1)."""
+        b = np.ascontiguousarray(rhs, dtype=np.float64).reshape(-1)
+        assert b.shape[0] == self.solution_size()
+        x = np.empty_like(b)
+        info = SolveInfo()
+        hist = np.full(max(int(max_iters), 0) + 1, np.nan)
+        _check(library().skb_flow_solve_system(self._h, dense._h if dense is not None else None, _p(b), float(eta),
+                                               float(tol), int(num_blocks), int(max_iters), _p(x), C.byref(info),
+                                               _p(hist)))
+        return x, info.as_dict(), hist[:info.iterations + 1]
+
+    def solve_system_device(self, dense, d_rhs: int, eta: float, d_x: int, tol=1e-10, num_blocks=300,
+                            max_iters=1000, stream: int = 0):
+        """solve_system on device pointers, asynchronous on `stream` except for one host wait per Arnoldi step.
+        Returns (info, history) as solve_system."""
+        info = SolveInfo()
+        hist = np.full(max(int(max_iters), 0) + 1, np.nan)
+        _check(library().skb_flow_solve_system_device(self._h, dense._h if dense is not None else None,
+                                                      C.c_void_p(d_rhs), float(eta), float(tol), int(num_blocks),
+                                                      int(max_iters), C.c_void_p(d_x), C.byref(info), _p(hist),
+                                                      C.c_void_p(stream)))
+        return info.as_dict(), hist[:info.iterations + 1]
+
     # ---- multi-GPU groups (peer memory) ----
     def last_sym_kernel(self):
         """(ms, ordered pairs) of the last launch of the symmetric fiber-fiber kernel inside matvec()."""
@@ -1061,6 +1113,19 @@ class Flow:
         vp = lambda a: C.c_void_p(a) if a else None
         _check(library().skb_flow_group_apply_system_preconditioner_device(
             self._h, dense._h if dense is not None else None, vp(d_x_local), vp(d_y_local), vp(stream)))
+
+    def group_solve_system_device(self, dense_matvec, dense_minv, d_rhs_local: int, eta: float, d_x_local: int,
+                                  tol=1e-10, num_blocks=300, max_iters=1000, stream: int = 0):
+        """solve_system_device on the member's local rows (set_gmres after group_set_body_operators); every member
+        calls it alike.  Returns (info, history), bitwise the same on every member."""
+        info = SolveInfo()
+        hist = np.full(max(int(max_iters), 0) + 1, np.nan)
+        vp = lambda a: C.c_void_p(a) if a else None
+        h = lambda d: d._h if d is not None else None
+        _check(library().skb_flow_group_solve_system_device(self._h, h(dense_matvec), h(dense_minv), vp(d_rhs_local),
+                                                            float(eta), float(tol), int(num_blocks), int(max_iters),
+                                                            vp(d_x_local), C.byref(info), _p(hist), vp(stream)))
+        return info.as_dict(), hist[:info.iterations + 1]
 
     def group_build_system_rhs_device(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
                                       minus_clamped, plus_hinged, dt, eta, d_f_external: int, d_body_forces: int,
@@ -1276,6 +1341,21 @@ class MultiFlow:
         y = np.empty_like(x)
         _check(library().skb_mflow_apply_system_preconditioner(self._h, _p(x), _p(y)))
         return y
+
+    def set_gmres(self, num_blocks: int = 300):
+        """Lay out every member's local rows and size its solve workspace (after set_body_operators)."""
+        _check(library().skb_mflow_set_gmres(self._h, int(num_blocks)))
+
+    def solve_system(self, rhs, eta, tol=1e-10, num_blocks=300, max_iters=1000):
+        """Flow.solve_system over the devices, every member solving its own rows: returns (x, info, history)."""
+        b = np.ascontiguousarray(rhs, dtype=np.float64).reshape(-1)
+        assert b.shape[0] == self.solution_size()
+        x = np.empty_like(b)
+        info = SolveInfo()
+        hist = np.full(max(int(max_iters), 0) + 1, np.nan)
+        _check(library().skb_mflow_solve_system(self._h, _p(b), float(eta), float(tol), int(num_blocks),
+                                                int(max_iters), _p(x), C.byref(info), _p(hist)))
+        return x, info.as_dict(), hist[:info.iterations + 1]
 
     def build_system_rhs(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
                          plus_hinged, dt, eta, f_external=None, body_forces_torques=None, v_growth=None,

@@ -22,8 +22,9 @@
 
 namespace skb {
 
-constexpr int kGroupPhases = 5;
+constexpr int kGroupPhases = 6;
 constexpr int kRowsPhase = 4; // the exchange of a member's own solution rows (skb_flow_group_* whole-vector calls)
+constexpr int kDotsPhase = 5; // the all-reduce of a solve's dot products (Group::reduce_dots)
 
 struct GroupPushArgs {
     // own fibers: raw forces -> weighted, into rows [fa, fa + n_f) of every member's f_sl
@@ -171,6 +172,35 @@ __global__ void group_ft_reduce_kernel(const GroupFtReduceArgs a) {
         a.f[i] = acc;
     else
         a.t[i - a.n3] = acc;
+}
+
+// ---- the all-reduce of a solve's dot products (skb_flow_group_solve_system_device) ----
+// The ft_part pattern: every member stores its m partial dots into its slot of every window, meets its peers at the dots
+// phase, and adds the slots of its own window in rank order, so every member holds bitwise the same sums.
+struct GroupDotsStoreArgs {
+    const double *v; // [m] this member's partials
+    int m, size;
+    double *slot[kMaxGroup]; // this member's slot in every window
+};
+
+__global__ void group_dots_store_kernel(const GroupDotsStoreArgs a) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= a.m)
+        return;
+    const double v = a.v[i];
+    for (int k = 0; k < a.size; ++k)
+        a.slot[k][i] = v;
+}
+
+__global__ void group_dots_reduce_kernel(const double *slots, long long stride, int first, int count, int m,
+                                         double *out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m)
+        return;
+    double acc = 0.0;
+    for (int k = first; k < first + count; ++k)
+        acc += __ldcv(slots + k * stride + i); // stored by peers: never from a stale cache line
+    out[i] = acc;
 }
 
 // ---- a member's own rows of the solution vector (skb_flow_group_* whole-vector calls) ----

@@ -44,6 +44,7 @@ int Group::init(int rank, int size, long long n_fib, long long n_pad_fib, long l
         lay_.x_shell[b] = take((size_t)n_shell * 24 + 16);
         lay_.ft_part[b] = take((size_t)kMaxGroup * n_bodies * 48 + 16);
         lay_.x_body[b] = take((size_t)n_body * 24 + (size_t)n_bodies * 48 + 16);
+        lay_.dots[b] = take((size_t)kMaxGroup * kDotsSlot * 8);
     }
     lay_.u_part = take((size_t)n_fib * 24 + 16);
     lay_.u_part_shell = take((size_t)n_shell * 24 + 16);
@@ -60,6 +61,8 @@ int Group::init(int rank, int size, long long n_fib, long long n_pad_fib, long l
     CUDA_TRY(cudaFuncGetAttributes(&fa, group_ft_reduce_kernel));
     CUDA_TRY(cudaFuncGetAttributes(&fa, group_rows_store_kernel));
     CUDA_TRY(cudaFuncGetAttributes(&fa, group_rows_compact_kernel));
+    CUDA_TRY(cudaFuncGetAttributes(&fa, group_dots_store_kernel));
+    CUDA_TRY(cudaFuncGetAttributes(&fa, group_dots_reduce_kernel));
     peer_[rank] = window_;
     return SKB_OK;
 }
@@ -221,6 +224,28 @@ int Group::reduce_forces(double *d_f, double *d_t, cudaStream_t st, int *launche
     a.f = d_f;
     a.t = d_t;
     group_ft_reduce_kernel<<<(unsigned)((2 * a.n3 + 255) / 256), 256, 0, st>>>(a);
+    return launched(launches);
+}
+
+// one epoch of its own: begin, the store into this member's slot of every window, the dots phase, the rank-order sum
+int Group::reduce_dots(double *d_v, int m, cudaStream_t st, int *launches) {
+    if (m > kDotsSlot)
+        return set_error(SKB_ERR_INVALID, "group member %d: %d dots exceed the window's slot of %d", rank_, m, kDotsSlot);
+    SKB_TRY(begin());
+    const int par = (int)(epoch_ & 1);
+    GroupDotsStoreArgs a;
+    a.v = d_v;
+    a.m = m;
+    char *w[kMaxGroup];
+    a.size = windows(w);
+    for (int k = 0; k < a.size; ++k)
+        a.slot[k] = (double *)(w[k] + lay_.dots[par]) + (size_t)rank_ * kDotsSlot;
+    const unsigned blocks = (unsigned)((m + 255) / 256);
+    group_dots_store_kernel<<<blocks, 256, 0, st>>>(a);
+    SKB_TRY(launched(launches));
+    SKB_TRY(barrier(kDotsPhase, true, true, st, launches));
+    group_dots_reduce_kernel<<<blocks, 256, 0, st>>>(own(lay_.dots[par]), kDotsSlot, solo_ ? rank_ : 0,
+                                                     solo_ ? 1 : size_, m, d_v);
     return launched(launches);
 }
 

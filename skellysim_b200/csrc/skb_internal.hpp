@@ -12,6 +12,7 @@
 #include <vector>
 
 struct skb_fiber_params;
+struct skb_solve_info;
 
 namespace skb {
 
@@ -137,6 +138,8 @@ struct EvalOpts {
 };
 
 constexpr int kMaxGroup = 16; // members of a multi-GPU group (Group, group_kernels.cuh, skb_mflow)
+constexpr int kMaxKrylov = 1024; // the largest num_blocks of a solve (SKB_GMRES_MAX_BLOCKS)
+constexpr int kDotsSlot = kMaxKrylov + 2; // dots one reduction carries: k + 1 basis columns and a norm
 
 // A member's owned rows of the body part of the solution vector (distributed.system_rows): body node rows [b0, b1)
 // (3 each) and the six rows [U; w] of every body whose first node lies in [b0, b1), as runs of consecutive entries in
@@ -376,6 +379,8 @@ int load_dense_kernels();
 //                                    ([F | L]; the whole-vector operator, skb_mflow_apply_system_matvec) -- by peers
 //   x_body       [2][n_body*3 + n_bodies*6]  the body part of the solution vector, complete (every member stores
 //                                    its own rows; skb_flow_group_apply_system_*)                   -- by peers
+//   dots         [2][kMaxGroup][kDotsSlot]  per member its partial dot products of a solve step (reduce_dots)
+//                                    -- by peers
 //   u_part       [n_fib*3]           this member's partial velocities of ALL fiber rows                  -- by itself
 //   u_part_shell [n_shell*3]         its partial velocities of ALL periphery rows (cross kernel)        -- by itself
 //
@@ -439,6 +444,9 @@ class Group {
     int rows_barrier(bool signal, bool wait, cudaStream_t st, int *launches) const; // barrier of the rows phase
     // d_local [body_rows()] = the own rows of d_full (the whole body layout)
     int compact_rows(const double *d_full, double *d_local, cudaStream_t st, int *launches) const;
+    // the all-reduce of a solve's dot products, one epoch of its own (begin, the dots phase's full barrier): d_v[0, m) =
+    // the sum over every member's d_v in rank order, bitwise the same on every member.  Not a member: nothing to do
+    int reduce_dots(double *d_v, int m, cudaStream_t st, int *launches);
 
     // this member's window, in the half of the matvec in flight
     double *f_sl() const { return own(lay_.f_sl[epoch_ & 1]); }
@@ -451,7 +459,7 @@ class Group {
   private:
     struct Layout { // byte offsets of the window's pieces
         size_t flags = 0, f_sl[2] = {0, 0}, f_shell[2] = {0, 0}, x_shell[2] = {0, 0}, ft_part[2] = {0, 0},
-               x_body[2] = {0, 0}, u_part = 0, u_part_shell = 0;
+               x_body[2] = {0, 0}, dots[2] = {0, 0}, u_part = 0, u_part_shell = 0;
         size_t bytes = 0;
     };
     struct Rows { // the piece table of set_body_rows, as the kernels take it (RowPiecesDev, group_kernels.cuh)
@@ -476,12 +484,75 @@ class Group {
     Ranges rows_ranges_ = {};
 };
 
+// ---- right-preconditioned restarted GMRES on the device (skb_solve.cu, krylov_kernels.cuh) ----
+// The workspace of one solution size -- the basis V of (num_blocks + 1) columns, the per-CTA dot partials, the
+// Hessenberg scalars and the pinned words the host reads once per Arnoldi step -- and the iteration over two operators
+// given as calls on the solve's stream.  Givens rotations, the triangular solve and every stopping decision run on the
+// host from the words the device reduced in a fixed order.
+class Krylov {
+  public:
+    // sizes everything for n rows (0 allowed: a group member that owns none still takes part in every reduction) and
+    // up to num_blocks basis vectors per cycle on the current device (num_sms: its SMs, which fix the reduction grid),
+    // and loads the kernels; key: what else the size belongs to (a member's target ranges).  A set-up call: allocates
+    int setup(long long n, int num_blocks, int num_sms, const std::array<long long, 6> &key);
+    bool sized_for(long long n, const std::array<long long, 6> &key) const { return set_ && n_ == n && key_ == key; }
+    int blocks() const { return m_cap_; }
+    // the host forms' copies of b and x (n doubles each), sized by setup
+    double *stage_b() const { return (double *)b_.ptr; }
+    double *stage_x() const { return (double *)x_.ptr; }
+    // out = A in / P^-1 in, enqueued on the solve's stream
+    using Apply = std::function<int(const double *d_in, double *d_out)>;
+    // d_v[0, m) (device, on the solve's stream) = the sum of every member's d_v: the all-reduce of a group member
+    // (Group::reduce_dots); empty for a single flow
+    using Reduce = std::function<int(double *d_v, int m)>;
+    // x = the GMRES solution of A x = b (x0 = 0, right preconditioning, ICGS); d_x is written, d_b only read.  info
+    // (skb_solve_info) and history (iterations + 1 implicit relative residuals, may be NULL) as skb_flow_solve_system
+    // documents them.  Each launch adds to *launches.  The host waits for one event per Arnoldi step and per cycle end
+    int solve(const Apply &A, const Apply &P_inv, const Reduce &reduce, const double *d_b, double *d_x, double tol,
+              int num_blocks, int max_iters, cudaStream_t st, ::skb_solve_info *info, double *history, int *launches);
+
+  private:
+    int pass(int which, int k, double *d_w, const double *d_coef, double *d_out, const Reduce &reduce,
+             cudaStream_t st, int *launches);
+    // V col 0 = b - ax, its norm^2 -> nrm[1]
+    int residual(const double *d_b, const double *d_ax, const Reduce &reduce, cudaStream_t st, int *launches);
+    int wait(cudaStream_t st); // the device words -> host_, then one event wait
+
+    bool set_ = false;
+    long long n_ = 0, ld_ = 0, rows_per_ = 0;
+    std::array<long long, 6> key_ = {};
+    int m_cap_ = 0, ctas_ = 0, ldp_ = 0;
+    DevBuf V_, z_, u_, part_, small_, b_, x_;
+    PinnedHost host_;
+    Event done_;
+    std::vector<double> H_, cs_, sn_, g_, y_; // the Hessenberg matrix ((m + 1) x m, column-major) and its rotations
+};
+
 } // namespace skb
 
 // ---- flow internals that skb_mflow.cu needs (skb_matvec.cu) ----
 struct skb_flow;
 struct skb_dense;
 namespace skb {
+// ---- and that skb_solve.cu needs: the flow's GMRES workspace, the checks of both system calls (dn holds both
+// operators) with *n = the solution size, one apply on st of a single-device flow whose checks have passed, and its
+// launch counter and SM count
+Krylov &flow_krylov(skb_flow *fl);
+Group &flow_group(skb_flow *fl);
+// the refusals of the two system calls the solve makes (a group member's local-vector calls, else the single-device
+// ones): dn_spc holds stresslet_plus_complementary, dn_minv M_inv; *n = the (local) solution size, *key its ranges
+int flow_solve_args(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const char *who, long long *n,
+                    std::array<long long, 6> *key);
+// the size and key skb_flow_set_gmres sizes for (a member: its local rows, which need its rows laid out)
+int flow_gmres_size(skb_flow *fl, const char *who, long long *n, std::array<long long, 6> *key);
+// a member of skb_mflow: lays out its local rows (what skb_flow_group_set_body_operators does besides the operators)
+// for the node counts of the bodies' operators it holds
+int flow_member_lay_out_rows(skb_flow *fl, const int *n_nodes, int n_bodies);
+int *flow_launches(skb_flow *fl);
+int flow_finish_device_stats(skb_flow *fl, int launches); // the stats of a _device call that made `launches`
+long long flow_whole_size(skb_flow *fl); // the whole solution vector's size (of every member alike)
+int flow_num_sms(const skb_flow *fl);
+int flow_device(const skb_flow *fl);
 cudaStream_t flow_stream(const skb_flow *fl); // the stream of the flow's own calls
 // sizes the buffers of the background streamer (skb_flow_set_overlap) for n_rows own periphery rows, if it is on
 int flow_size_overlap(skb_flow *fl, long long n_rows);

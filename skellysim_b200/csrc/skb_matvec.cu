@@ -119,6 +119,7 @@ struct skb_flow {
     DevBuf sys_x, sys_y; // the whole solution vector in and out of the host forms of the system operator
     DevBuf zeros;        // the system RHS: the zero densities (and absent forces) its flow takes, n_zeros doubles
     long long n_zeros = 0;
+    Krylov kry; // the workspace of skb_flow_solve_system (skb_solve.cu)
     skb_flow_stats stats{};
     int launches = 0;
     long long pairs = 0;
@@ -2524,6 +2525,73 @@ int skb_flow_group_build_system_rhs_device(skb_flow *fl, const skb_fiber_params 
 }
 
 } // extern "C"
+
+Krylov &skb::flow_krylov(skb_flow *fl) { return fl->kry; }
+Group &skb::flow_group(skb_flow *fl) { return fl->grp; }
+long long skb::flow_whole_size(skb_flow *fl) { return solution_size(fl); }
+int *skb::flow_launches(skb_flow *fl) { return &fl->launches; }
+int skb::flow_num_sms(const skb_flow *fl) { return fl->fib[1]->devs[0].info.num_sms; }
+int skb::flow_device(const skb_flow *fl) { return fl->dev; }
+
+int skb::flow_finish_device_stats(skb_flow *fl, int launches) {
+    fl->pairs = 0;
+    fl->launches = launches;
+    return device_stats(fl);
+}
+
+int skb::flow_solve_args(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const char *who, long long *n,
+                         std::array<long long, 6> *key) {
+    if (fl->grp.member()) {
+        SKB_TRY(group_system_args(fl, dn_spc, who, false));
+        SKB_TRY(group_system_args(fl, dn_minv, who, true));
+        *n = group_local_size(fl);
+        *key = group_ranges(fl);
+        return SKB_OK;
+    }
+    SKB_TRY(system_args(fl, dn_spc, who, false, true));
+    SKB_TRY(system_args(fl, dn_minv, who, true, true));
+    *n = solution_size(fl);
+    *key = {};
+    return SKB_OK;
+}
+
+int skb::flow_gmres_size(skb_flow *fl, const char *who, long long *n, std::array<long long, 6> *key) {
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    if (!fl->grp.member()) {
+        *n = solution_size(fl);
+        *key = {};
+        return SKB_OK;
+    }
+    SKB_TRY(prepare_matvec_targets(fl));
+    if (!fl->grp.rows_for(group_ranges(fl)))
+        return set_error(SKB_ERR_INVALID, "%s: a group member's rows are laid out by skb_flow_group_set_body_operators "
+                                          "(after skb_flow_group_init and every change of the target ranges)", who);
+    *n = group_local_size(fl);
+    *key = group_ranges(fl);
+    return SKB_OK;
+}
+
+int skb::flow_member_lay_out_rows(skb_flow *fl, const int *n_nodes, int n_bodies) {
+    const char *who = "skb_mflow_set_gmres";
+    if (!fl->grp.member())
+        return SKB_OK;
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    OwnFibers own;
+    SKB_TRY(own_fibers(fl, who, own));
+    std::vector<RowPiece> pieces;
+    if (!body_row_pieces(n_nodes, n_bodies, fl->ba, fl->bb, pieces))
+        return set_error(SKB_ERR_STATE, "%s: the body rows [%lld, %lld) make %d pieces (at most %d)", who, fl->ba,
+                         fl->bb, (int)pieces.size(), kMaxRowPieces);
+    long long sol = 0;
+    for (int b = 0; b < n_bodies; ++b)
+        sol += 3LL * n_nodes[b] + 6;
+    // every buffer of the local-vector calls at its final size, as skb_flow_group_set_body_operators does
+    SKB_TRY(fl->sys_rb.ensure((size_t)sol * 8 + 8));
+    SKB_TRY(flow_size_system(fl));
+    SKB_TRY(load_dense_kernels());
+    fl->grp.set_body_rows(pieces, group_ranges(fl));
+    return SKB_OK;
+}
 
 cudaStream_t skb::flow_stream(const skb_flow *fl) { return fl->stream; }
 int skb::flow_size_overlap(skb_flow *fl, long long n_rows) {

@@ -15,6 +15,7 @@
 #include <mutex>
 #include <string>
 #include <thread>
+#include <cstring>
 #include <vector>
 
 using namespace skb;
@@ -117,6 +118,9 @@ struct skb_mflow {
         Event e0, e1;
     };
     std::vector<IO> io;
+    // skb_mflow_set_gmres: the partition and body node counts it laid the members' local rows out for
+    bool gmres_set = false;
+    std::vector<long long> gmres_layout;
     skb_flow_stats stats{};
 };
 
@@ -932,6 +936,124 @@ int skb_mflow_last_stats(const skb_mflow *mf, skb_flow_stats *out) {
         return set_error(SKB_ERR_INVALID, "skb_mflow_last_stats: NULL");
     *out = mf->stats;
     return SKB_OK;
+}
+
+} // extern "C"
+
+// ---- the solve (skb_mflow_set_gmres / _solve_system): every member runs skb_flow_group_solve_system_device ----------
+static std::vector<long long> gmres_layout(const skb_mflow *mf) {
+    std::vector<long long> v;
+    for (int g = 0; g < mf->n; ++g)
+        v.insert(v.end(), {(long long)mf->f0[g], (long long)mf->f1[g], mf->s0[g], mf->s1[g], mf->b0[g], mf->b1[g]});
+    v.insert(v.end(), mf->body_n.begin(), mf->body_n.end());
+    return v;
+}
+
+// member g's rows of a whole vector in its local order [fiber rows | shell rows | body pieces]: copy(whole offset,
+// local offset, length) per run
+template <class Copy> static void member_local(const skb_mflow *mf, int g, Copy copy) {
+    const MemberRows r = member_rows(mf, g);
+    const long long nf = mf->n_fib, ns = mf->n_shell;
+    long long at = 0;
+    copy(4 * r.a, at, 4 * r.n_fw);
+    at += 4 * r.n_fw;
+    copy(4 * nf + 3 * mf->s0[g], at, 3 * r.n_sw);
+    at += 3 * r.n_sw;
+    if (mf->n_bodies > 0)
+        for (const auto &p : body_rows(mf->body_n, mf->b0[g], mf->b1[g])) {
+            copy(4 * nf + 3 * ns + p.first, at, p.second - p.first);
+            at += p.second - p.first;
+        }
+}
+
+extern "C" {
+
+int skb_mflow_set_gmres(skb_mflow *mf, int num_blocks) {
+    const char *who = "skb_mflow_set_gmres";
+    if (!mf)
+        return set_error(SKB_ERR_INVALID, "%s: NULL", who);
+    if (num_blocks < 1 || num_blocks > kMaxKrylov)
+        return set_error(SKB_ERR_INVALID, "%s: num_blocks = %d (must be in [1, %d])", who, num_blocks, kMaxKrylov);
+    SKB_TRY(mflow_prepare(mf));
+    if (mf->n_bodies > 0 && (int)mf->body_n.size() != mf->n_bodies)
+        return set_error(SKB_ERR_INVALID, "%s: call skb_mflow_set_body_operators first", who);
+    mf->gmres_set = false;
+    SKB_TRY(mf->workers->run([&](int g) -> int {
+        skb_flow *fl = mf->m[(size_t)g].get();
+        SKB_TRY(flow_member_lay_out_rows(fl, mf->body_n.data(), mf->n_bodies));
+        return skb_flow_set_gmres(fl, num_blocks);
+    }));
+    mf->gmres_layout = gmres_layout(mf);
+    mf->gmres_set = true;
+    return SKB_OK;
+}
+
+int skb_mflow_solve_system(skb_mflow *mf, const double *rhs, double eta, double tol, int num_blocks, int max_iters,
+                           double *x, skb_solve_info *info, double *history) {
+    const char *who = "skb_mflow_solve_system";
+    const bool empty = mf && mflow_solution_size(mf) == 0;
+    // every member's refusals before any device starts: a member that went on alone would wait on its peers' flags
+    SKB_TRY(mflow_system_args(mf, who, false, (rhs && x) || empty));
+    SKB_TRY(mflow_system_args(mf, who, true, (rhs && x) || empty));
+    if (!(eta > 0))
+        return set_error(SKB_ERR_INVALID, "%s: eta = %g", who, eta);
+    if (!(tol > 0) || !std::isfinite(tol))
+        return set_error(SKB_ERR_INVALID, "%s: tol = %g (must be finite and > 0)", who, tol);
+    if (num_blocks < 1 || num_blocks > kMaxKrylov)
+        return set_error(SKB_ERR_INVALID, "%s: num_blocks = %d (must be in [1, %d])", who, num_blocks, kMaxKrylov);
+    if (max_iters < 0)
+        return set_error(SKB_ERR_INVALID, "%s: max_iters = %d", who, max_iters);
+    if (!info)
+        return set_error(SKB_ERR_INVALID, "%s: NULL info", who);
+    if (empty) {
+        std::memset(info, 0, sizeof(*info));
+        info->converged = 1;
+        return SKB_OK;
+    }
+    if (!mf->gmres_set || mf->gmres_layout != gmres_layout(mf))
+        return set_error(SKB_ERR_INVALID, "%s: call skb_mflow_set_gmres after the partition or the bodies' node counts "
+                                          "changed", who);
+    for (int g = 0; g < mf->n; ++g) {
+        skb_flow *fl = mf->m[(size_t)g].get();
+        long long n = 0;
+        std::array<long long, 6> key;
+        SKB_TRY(flow_gmres_size(fl, who, &n, &key));
+        if (!flow_krylov(fl).sized_for(n, key) || num_blocks > flow_krylov(fl).blocks())
+            return set_error(SKB_ERR_INVALID, "%s: num_blocks = %d, skb_mflow_set_gmres sized device member %d for %d",
+                             who, num_blocks, g, flow_krylov(fl).blocks());
+    }
+    std::vector<skb_solve_info> infos((size_t)mf->n);
+    std::vector<std::vector<double>> hist((size_t)mf->n, std::vector<double>(history ? (size_t)max_iters + 1 : 0));
+    SKB_TRY(mf->workers->run([&](int g) -> int {
+        skb_flow *fl = mf->m[(size_t)g].get();
+        CUDA_TRY(cudaSetDevice(mf->devs[(size_t)g]));
+        const Krylov &kry = flow_krylov(fl);
+        cudaStream_t st = flow_stream(fl);
+        std::vector<double> loc;
+        member_local(mf, g, [&](long long whole, long long, long long len) {
+            loc.insert(loc.end(), rhs + whole, rhs + whole + len);
+        });
+        if (!loc.empty())
+            CUDA_TRY(cudaMemcpyAsync(kry.stage_b(), loc.data(), loc.size() * 8, cudaMemcpyHostToDevice, st));
+        skb_dense *dn = mf->dn[(size_t)g].get();
+        SKB_TRY(skb_flow_group_solve_system_device(fl, dn, dn, kry.stage_b(), eta, tol, num_blocks, max_iters,
+                                                   kry.stage_x(), &infos[(size_t)g],
+                                                   history ? hist[(size_t)g].data() : nullptr, st));
+        if (!loc.empty())
+            CUDA_TRY(cudaMemcpyAsync(loc.data(), kry.stage_x(), loc.size() * 8, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        member_local(mf, g, [&](long long whole, long long at, long long len) {
+            std::memcpy(x + whole, loc.data() + at, (size_t)len * 8);
+        });
+        return SKB_OK;
+    }));
+    for (int g = 1; g < mf->n; ++g) // the all-reduce leaves every member the same scalars
+        if (std::memcmp(&infos[(size_t)g], &infos[0], sizeof(skb_solve_info)) != 0 || hist[(size_t)g] != hist[0])
+            return set_error(SKB_ERR_STATE, "%s: device member %d ended its solve unlike member 0", who, g);
+    *info = infos[0];
+    if (history)
+        std::memcpy(history, hist[0].data(), (size_t)(info->iterations + 1) * 8);
+    return mflow_collect_stats(mf);
 }
 
 } // extern "C"

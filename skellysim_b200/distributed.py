@@ -288,3 +288,23 @@ class RankSystemOperator:
                                                 v_growth=v_growth, force_scale=force_scale, stream=self._stream())
         self.launches = self.flow.stats()["launches"]
         return self.b[:self.n]
+
+    def set_gmres(self, num_blocks: int = 300):
+        """Size the rank's solve workspace (skb_flow_set_gmres on its local rows) and the solution it returns.  A set-up
+        call: it allocates, so every rank makes it before any rank's first solve (a peer on the same device may spin on
+        a flag while another allocates)."""
+        self.flow.set_gmres(num_blocks)
+        self.x = self.torch.zeros_like(self.res)
+        self._gmres_blocks = int(num_blocks)
+
+    def solve(self, b_local, tol: float = 1e-10, num_blocks: int = 300, max_iters: int = 1000):
+        """Solver::solve on the rank's local rows (skb_flow_group_solve_system_device): every rank calls it alike with
+        its rows of b and gets its rows of x (a view valid until the next call) and info -- bitwise the same on every
+        rank, history included.  Needs set_gmres(num_blocks or more) first."""
+        if getattr(self, "_gmres_blocks", 0) < num_blocks:
+            raise RuntimeError("RankSystemOperator.solve: call set_gmres(num_blocks) on every rank first")
+        info, hist = self.flow.group_solve_system_device(self.dense_matvec, self.dense_minv, self._ptr(b_local),
+                                                         self.eta, self.x.data_ptr(), tol=tol, num_blocks=num_blocks,
+                                                         max_iters=max_iters, stream=self._stream())
+        self.launches = self.flow.stats()["launches"]
+        return self.x[:self.n], dict(info, history=hist)

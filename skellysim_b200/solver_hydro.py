@@ -132,6 +132,24 @@ class SystemOperator:
         self.launches = self.flow.stats()["launches"]
         return out[:self.n]
 
+    def set_gmres(self, num_blocks: int = 300):
+        """Size the solve's workspace (skb_flow_set_gmres) for up to num_blocks basis vectors per cycle."""
+        self.flow.set_gmres(num_blocks)
+        self._gmres_blocks = int(num_blocks)
+
+    def solve(self, b, tol: float = 1e-10, num_blocks: int = 300, max_iters: int = 1000):
+        """Solver::solve (solver_hydro.cpp:64-95): x = A^-1 b by restarted right-preconditioned GMRES on the device
+        (skb_flow_solve_system_device), from x0 = 0.  b: a device tensor of solution_size().  Returns (x, info): x a new
+        device tensor, info skb_solve_info as a dict plus "history", the implicit relative residual after each Arnoldi
+        step.  The workspace is set up on first use, or again when num_blocks exceeds the one set up."""
+        if getattr(self, "_gmres_blocks", 0) < num_blocks or self.flow.solution_size() != self.n:
+            self.set_gmres(num_blocks)
+        x = self.torch.empty(max(self.n, 1), dtype=self.torch.float64, device=self.res.device)
+        info, hist = self.flow.solve_system_device(self.dense, b.data_ptr(), self.eta, x.data_ptr(), tol=tol,
+                                                   num_blocks=num_blocks, max_iters=max_iters, stream=self._stream())
+        self.launches = self.flow.stats()["launches"]
+        return x[:self.n], dict(info, history=hist)
+
 
 def iterate_system(op: SystemOperator, x, n_iter: int):
     """iterate() for whole solution vectors: `n_iter` times x <- A P^-1 x, rescaled to unit max-norm on the device."""
