@@ -498,6 +498,56 @@ SKB_API int skb_flow_group_solve_system_device(skb_flow *fl, struct skb_dense *d
                                                int max_iters, double *d_x_local, skb_solve_info *info,
                                                double *history, void *stream);
 
+/* ---- one timestep of the whole system ----------------------------------------------------------------------------
+ * System::step (system.cpp:482-492) on a single-device flow, in the reference's order (DESIGN.md §3.9):
+ *   1. skb_flow_set_fiber_links from the current placement: site = c + R(q) site_ref of each bound fiber, its bending
+ *      rigidity from params;
+ *   2. skb_flow_build_fiber_operators(params, dt, eta);
+ *   3. skb_flow_build_system_rhs_device (params, v_growth, force_scale, f_external, body_forces_torques);
+ *   4. skb_flow_solve_system_device from x0 = 0 into the workspace of skb_flow_set_gmres;
+ *   5. the fiber step kernel: FiberContainerFiniteDifference::step (fcfd.cpp:292-302), ::repin_to_bodies (:308-316) to
+ *      the nucleation sites at the bodies' new placement, and ::fiber_error_local (:79-89) on the repinned nodes;
+ *   6. the bodies' step on the host from their rows [U; w] (48 bytes per body): c_new = c + dt U, phi = dt w and, if
+ *      |phi| > 0, q_new = (cos |phi|/2, sin(|phi|/2) phi/|phi|) * q (Eigen's product order), normalised;
+ *   7. the new geometry installed: the fiber positions through skb_flow_set_fibers (node counts and lengths unchanged),
+ *      the bodies through skb_flow_place_bodies(c_new, q_new), the links at the new sites.
+ * The step is not refused for a solve that did not converge: it advances from whatever the solve returned, as the
+ * reference does, and info->solve reports it.  x (the solution, NULL ok) and tension (N_f, NULL ok) receive the step's
+ * solution.  info->fiber_error is the max over fibers and nodes of | ||xs_i|| - 1 | after the step (0 without fibers),
+ * info->worst_fiber the first fiber attaining it (-1 without fibers).
+ *   fiber_body: per fiber its body (binding_site_.first, -1 free; NULL: all free); site_ref: 3 per fiber, the body-frame
+ *   nucleation site (nucleation_sites_ref_ of the binding site; NULL without bound fibers).  Bodies must be placed by
+ *   skb_flow_set_body_frames (with A_inv0) and a first skb_flow_place_bodies: the step places from the frames.
+ * Two deviations from the reference (DESIGN.md §5): a body always moves to c + dt U (the reference translates only
+ * inside place(), which it calls only when |phi| != 0), and q_new is normalised (placement refuses a quaternion that
+ * drifted off unit norm).  A solution whose new fiber positions or body rows are not finite is not installed: geometry
+ * and placement stay, info->fiber_error is NaN and the call returns SKB_ERR_STATE.
+ * Refused (SKB_ERR_INVALID, before any launch, earlier state untouched): everything the four composed calls refuse,
+ * dt <= 0 or not finite, bodies without frames and a first placement, a fiber_body index outside [-1, n_bodies), a
+ * group member, a target window or ranges that do not cover every row, no skb_flow_set_gmres for the current solution
+ * size (which also sizes the step's own buffers; the composed calls size theirs on their first use, as they do when
+ * called alone).  An empty block needs none of its
+ * set-up; an empty system returns SKB_OK (converged, nothing moves) without a launch.
+ * skb_flow_fiber_error: the step kernel's error on the current geometry: *max_error over every fiber, per_fiber (NULL
+ *   ok) per fiber.  Needs skb_flow_set_fiber_class of every node count, n <= 128.
+ * skb_flow_get_placement: the centres (3 per body) and quaternions (4 per body) of the last skb_flow_place_bodies (or
+ *   step); NULL skips an array.  Refused when the bodies were not placed since skb_flow_set_bodies.
+ * skb_flow_get_fibers: the fiber positions (3 x N_f) of the last skb_flow_set_fibers (or step), from the host copy the
+ *   flow keeps. */
+typedef struct skb_step_info {
+    skb_solve_info solve; /* as skb_flow_solve_system */
+    double fiber_error;   /* max over fibers and nodes after the step; 0 without fibers; NaN: not installed */
+    int32_t worst_fiber;  /* the fiber attaining it, -1 without fibers */
+    int32_t reserved;
+} skb_step_info;
+SKB_API int skb_flow_step(skb_flow *fl, struct skb_dense *dn, const skb_fiber_params *params, const double *v_growth,
+                          const double *force_scale, const double *f_external, const double *body_forces_torques,
+                          const int *fiber_body, const double *site_ref, double dt, double eta, double tol,
+                          int num_blocks, int max_iters, double *x, double *tension, skb_step_info *info);
+SKB_API int skb_flow_fiber_error(skb_flow *fl, double *max_error, double *per_fiber);
+SKB_API int skb_flow_get_placement(skb_flow *fl, double *centers, double *orientations);
+SKB_API int skb_flow_get_fibers(skb_flow *fl, double *r_fib);
+
 /* ---- the whole-vector calls on one rank per GPU ---------------------------------------------------------------------
  * A group member (skb_flow_group_init ... skb_flow_group_warmup above) applies A, P^-1 and builds the RHS on its LOCAL
  * vector: its own rows of the whole vector [fibers | shell | bodies], in ascending global order --
@@ -676,6 +726,21 @@ SKB_API int skb_mflow_solve_system(skb_mflow *mf, const double *rhs, double eta,
                                    int max_iters, double *x, skb_solve_info *info, double *history);
 /* skb_flow_set_point_sources / _set_background on every device: skb_mflow_velocity_at_targets and
  * skb_mflow_build_system_rhs include them */
+/* skb_flow_step over n devices: the same arguments as complete host arrays of all fibers and bodies, the same refusals
+ * (every member's before any member launches) and the same deviations.  The links, the build, the RHS and the solve are
+ * the skb_mflow calls; each member then runs the fiber step kernel on its own fibers, reading its rows of the solution
+ * on its device, and downloads their new positions into one host array; the bodies' step is done once on the host from
+ * the complete solution; every member installs the same complete geometry and is placed at the same (c, q).
+ * info->fiber_error is the max over all members' fibers.  skb_mflow_set_gmres sizes the step's buffers.  The RHS and
+ * the solution cross the host once each, as skb_mflow_build_system_rhs and skb_mflow_solve_system take them.  With one
+ * device it is bitwise skb_flow_step. */
+SKB_API int skb_mflow_step(skb_mflow *mf, const skb_fiber_params *params, const double *v_growth,
+                           const double *force_scale, const double *f_external, const double *body_forces_torques,
+                           const int *fiber_body, const double *site_ref, double dt, double eta, double tol,
+                           int num_blocks, int max_iters, double *x, double *tension, skb_step_info *info);
+/* skb_flow_get_fibers / _get_placement of the geometry every member holds */
+SKB_API int skb_mflow_get_fibers(skb_mflow *mf, double *r_fib);
+SKB_API int skb_mflow_get_placement(skb_mflow *mf, double *centers, double *orientations);
 SKB_API int skb_mflow_set_point_sources(skb_mflow *mf, const double *positions, const double *forces,
                                         const double *torques, int n_points);
 SKB_API int skb_mflow_set_background(skb_mflow *mf, const int *components, const double *scale_factor,

@@ -45,6 +45,15 @@ class SolveInfo(C.Structure):
 
 
 GMRES_MAX_BLOCKS = 1024  # SKB_GMRES_MAX_BLOCKS
+ERR_STATE = 4  # SKB_ERR_STATE
+
+
+class StepInfo(C.Structure):
+    """skb_step_info (include/skelly_b200_flow.h): the outcome of skb_flow_step."""
+    _fields_ = [("solve", SolveInfo), ("fiber_error", C.c_double), ("worst_fiber", C.c_int32), ("reserved", C.c_int32)]
+
+    def as_dict(self):
+        return dict(self.solve.as_dict(), fiber_error=self.fiber_error, worst_fiber=self.worst_fiber)
 
 
 class DenseStats(C.Structure):
@@ -247,6 +256,15 @@ def library() -> C.CDLL:
         "skb_flow_group_solve_system_device": ([ctxp, ctxp, ctxp, C.c_void_p, C.c_double, C.c_double, C.c_int, C.c_int,
                                                 C.c_void_p, C.POINTER(SolveInfo), _dp, C.c_void_p], C.c_int),
         "skb_mflow_set_gmres": ([ctxp, C.c_int], C.c_int),
+        "skb_flow_step": ([ctxp, ctxp, C.POINTER(FiberParams), _dp, _dp, _dp, _dp, C.POINTER(C.c_int), _dp, C.c_double,
+                           C.c_double, C.c_double, C.c_int, C.c_int, _dp, _dp, C.POINTER(StepInfo)], C.c_int),
+        "skb_flow_fiber_error": ([ctxp, _dp, _dp], C.c_int),
+        "skb_flow_get_placement": ([ctxp, _dp, _dp], C.c_int),
+        "skb_flow_get_fibers": ([ctxp, _dp], C.c_int),
+        "skb_mflow_step": ([ctxp, C.POINTER(FiberParams), _dp, _dp, _dp, _dp, C.POINTER(C.c_int), _dp, C.c_double,
+                            C.c_double, C.c_double, C.c_int, C.c_int, _dp, _dp, C.POINTER(StepInfo)], C.c_int),
+        "skb_mflow_get_fibers": ([ctxp, _dp], C.c_int),
+        "skb_mflow_get_placement": ([ctxp, _dp, _dp], C.c_int),
         "skb_mflow_solve_system": ([ctxp, _dp, C.c_double, C.c_double, C.c_int, C.c_int, _dp, C.POINTER(SolveInfo),
                                     _dp], C.c_int),
     }
@@ -354,6 +372,27 @@ def _system_rhs_args(n_fibers, n_nodes, n_bodies, params, v_growth, force_scale,
     if ft is not None and ft.shape[0] != n_bodies:
         raise ValueError(f"expected ({n_bodies}, 6) body forces and torques, got {ft.shape}")
     return p, vg, fs, f, ft
+
+
+def _step_call(fl, call, n_fibers, params, dt, eta, f_external, body_forces_torques, fiber_body, site_ref, v_growth,
+               force_scale, tol, num_blocks, max_iters):
+    """the arguments of skb_flow_step / skb_mflow_step after the handles; returns (x, tension, info dict).  SKB_ERR_STATE
+    with a NaN fiber_error is the step that was not installed; anything else non-zero raises"""
+    p, vg, fs, f, ft = _system_rhs_args(n_fibers, fl.n_fib, fl.n_bodies, params, v_growth, force_scale, f_external,
+                                        body_forces_torques)
+    fb = None if fiber_body is None else np.ascontiguousarray(fiber_body, dtype=np.int32).reshape(-1)
+    if fb is not None and fb.shape[0] != n_fibers:
+        raise ValueError(f"expected {n_fibers} fiber_body entries, got {fb.shape[0]}")
+    sr = None if site_ref is None else _arr(site_ref, 3)
+    x = np.empty(fl.solution_size())
+    tension = np.empty(fl.n_fib)
+    info = StepInfo()
+    rc = call(_params_ptr(p), _opt_p(vg), _opt_p(fs), _opt_p(f), _opt_p(ft),
+              None if fb is None else fb.ctypes.data_as(C.POINTER(C.c_int)), _opt_p(sr), float(dt), float(eta),
+              float(tol), int(num_blocks), int(max_iters), _p(x), _p(tension), C.byref(info))
+    if not (rc == ERR_STATE and np.isnan(info.fiber_error)):
+        _check(rc)
+    return x, tension, info.as_dict()
 
 
 def device_count() -> int:
@@ -559,6 +598,7 @@ class Flow:
                                              _p(lengths), int(n_nodes.shape[0])))
         self.n_fib = r_fib.shape[0]
         self._fiber_off = np.concatenate([[0], np.cumsum(n_nodes, dtype=np.int64)])
+        self._lengths = lengths.copy()
 
     def set_periphery(self, node_pos, node_normal):
         node_pos, node_normal = _arr(node_pos, 3), _arr(node_normal, 3)
@@ -1028,6 +1068,41 @@ class Flow:
                                                       C.c_void_p(stream)))
         return info.as_dict(), hist[:info.iterations + 1]
 
+    def step(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped, plus_hinged, dt,
+             eta, dense=None, f_external=None, body_forces_torques=None, fiber_body=None, site_ref=None,
+             v_growth=None, force_scale=None, tol=1e-10, num_blocks=300, max_iters=1000):
+        """System::step (system.cpp:482-492) on the device: links, fiber operators, RHS and solve at the current
+        geometry, then the fibers' and bodies' step and the new geometry installed.  fiber_body (N_fibers,) ints, -1
+        free, or None; site_ref (N_fibers, 3) body-frame nucleation sites, or None.  Returns (x, tension, info): info
+        a dict of skb_step_info (the solve's fields, fiber_error, worst_fiber).  A solution with non-finite new
+        positions installs nothing and returns fiber_error NaN."""
+        return _step_call(self, lambda *a: library().skb_flow_step(self._h, dense._h if dense is not None else None, *a),
+                          self._n_fibers(), (length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
+                                             minus_clamped, plus_hinged), dt, eta, f_external, body_forces_torques,
+                          fiber_body, site_ref, v_growth, force_scale, tol, num_blocks, max_iters)
+
+    def _n_fibers(self):
+        return len(getattr(self, "_fiber_off", [0])) - 1
+
+    def fiber_error(self):
+        """fiber_error_local (fcfd.cpp:79-89) of the current geometry on the device: (max, per-fiber maxima)"""
+        m = C.c_double(0)
+        per = np.empty(self._n_fibers())
+        _check(library().skb_flow_fiber_error(self._h, C.byref(m), _p(per)))
+        return m.value, per
+
+    def fibers(self):
+        """the fiber positions (N_f, 3) of the last set_fibers or step"""
+        r = np.empty((self.n_fib, 3))
+        _check(library().skb_flow_get_fibers(self._h, _p(r)))
+        return r
+
+    def placement(self):
+        """(centres (n_bodies, 3), quaternions (n_bodies, 4)) of the last place_bodies or step"""
+        c, q = np.empty((self.n_bodies, 3)), np.empty((self.n_bodies, 4))
+        _check(library().skb_flow_get_placement(self._h, _p(c), _p(q)))
+        return c, q
+
     # ---- multi-GPU groups (peer memory) ----
     def last_sym_kernel(self):
         """(ms, ordered pairs) of the last launch of the symmetric fiber-fiber kernel inside matvec()."""
@@ -1187,6 +1262,8 @@ class MultiFlow:
         _check(library().skb_mflow_set_fibers(self._h, _p(r_fib), n_nodes.ctypes.data_as(C.POINTER(C.c_int)),
                                               _p(lengths), int(n_nodes.shape[0])))
         self.n_fib, self.n_fibers = r_fib.shape[0], int(n_nodes.shape[0])
+        self._fiber_off = np.concatenate([[0], np.cumsum(n_nodes, dtype=np.int64)])
+        self._lengths = lengths.copy()
 
     def set_periphery(self, node_pos, node_normal):
         node_pos, node_normal = _arr(node_pos, 3), _arr(node_normal, 3)
@@ -1319,6 +1396,27 @@ class MultiFlow:
         E = np.ascontiguousarray(np.broadcast_to(np.asarray(bending_rigidity, dtype=np.float64), b.shape))
         assert st.shape[0] == b.shape[0]
         _check(library().skb_mflow_set_fiber_links(self._h, b.ctypes.data_as(C.POINTER(C.c_int)), _p(st), _p(E)))
+
+    def step(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped, plus_hinged, dt,
+             eta, dense=None, f_external=None, body_forces_torques=None, fiber_body=None, site_ref=None,
+             v_growth=None, force_scale=None, tol=1e-10, num_blocks=300, max_iters=1000):
+        """Flow.step over the devices (dense: unused, the periphery's operators come from set_dense)"""
+        return _step_call(self, lambda *a: library().skb_mflow_step(self._h, *a), self.n_fibers,
+                          (length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
+                           plus_hinged), dt, eta, f_external, body_forces_torques, fiber_body, site_ref, v_growth,
+                          force_scale, tol, num_blocks, max_iters)
+
+    def fibers(self):
+        """the fiber positions (N_f, 3) every device holds"""
+        r = np.empty((self.n_fib, 3))
+        _check(library().skb_mflow_get_fibers(self._h, _p(r)))
+        return r
+
+    def placement(self):
+        """(centres (n_bodies, 3), quaternions (n_bodies, 4)) of the last place_bodies or step"""
+        c, q = np.empty((self.n_bodies, 3)), np.empty((self.n_bodies, 4))
+        _check(library().skb_mflow_get_placement(self._h, _p(c), _p(q)))
+        return c, q
 
     def solution_size(self) -> int:
         """4 N_f + 3 N_s + sum(3 n_b + 6) (the bodies' part as set_body_operators was last given)"""

@@ -5,6 +5,7 @@
 #include "fiber_build.cuh"
 #include "fiber_ops.cuh"
 #include "fiber_rhs.cuh"
+#include "step_kernels.cuh"
 #include "skb_internal.hpp"
 #include "../../include/skelly_b200_flow.h"
 
@@ -371,6 +372,37 @@ int FiberOps::rhs(const OwnFibers &own, const skb_fiber_params *params, const do
         return SKB_OK;
     };
     return frame(stage, launch);
+}
+
+int FiberOps::check_step(const OwnFibers &own, const skb_fiber_params *params, const double *v_growth,
+                         const double *force_scale) const {
+    SKB_TRY(check_params(own, params));
+    for (int f = 0; f < own.count(); ++f) {
+        SKB_TRY(check_class(own.f0 + f, own.n[own.f0 + f], true));
+        const double vg = v_growth ? v_growth[f] : 0.0, fs = force_scale ? force_scale[f] : 0.0;
+        if (!std::isfinite(vg) || !std::isfinite(fs))
+            return set_error(SKB_ERR_INVALID, "fiber %d: v_growth = %g, force_scale = %g (both must be finite)",
+                             own.f0 + f, vg, fs);
+    }
+    return SKB_OK;
+}
+
+int FiberOps::step_items(const OwnFibers &own, std::vector<StepItem> &items) const {
+    items.assign((size_t)own.count(), StepItem{});
+    for (int f = 0; f < own.count(); ++f) {
+        const int g = own.f0 + f, n = own.n[g];
+        SKB_TRY(check_class(g, n, false));
+        if (n > kStepMaxNodes)
+            return set_error(SKB_ERR_INVALID, "fiber %d has %d nodes: the fiber step takes at most %d", g, n,
+                             kStepMaxNodes);
+        const auto &co = class_off.at(n);
+        StepItem &it = items[(size_t)f];
+        it.node = own.off[g] - own.off[own.f0];
+        it.d1 = co.first;
+        it.rng = co.second + 4LL * n - 14; // past P_downsample_bc's row ranges
+        it.n = n;
+    }
+    return SKB_OK;
 }
 
 int FiberOps::size_rhs(int n_fibers) {

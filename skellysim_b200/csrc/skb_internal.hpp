@@ -169,6 +169,7 @@ struct OwnFibers {
 };
 
 struct FiberItem; // fiber_build.cuh
+struct StepItem;  // step_kernels.cuh
 
 // A_, force_operator_, xs_ and A_^-1 of one set of own fibers, resident for the timestep, and the GEMVs over them.
 // The caller has checked its pointers for NULL and made the flow's device current.
@@ -217,6 +218,14 @@ class FiberOps {
     // set_class adds a node count.  The table and the resident tangents xs_ (3 per own node) on the device
     int derivative_offset(int f, int n, long long *off) const;
     const double *class_table() const { return (const double *)class_mats.ptr; }
+    const int2 *class_range_table() const { return (const int2 *)class_ranges.ptr; }
+    // the fiber step's item of every own fiber (step_kernels.cuh: its D_1_0 and their column ranges; node offsets from
+    // the first own node, free); an error unless each node count has skb_flow_set_fiber_class and at most
+    // kStepMaxNodes nodes
+    int step_items(const OwnFibers &own, std::vector<StepItem> &items) const;
+    // the refusals of build() and rhs() for these arguments, without a launch or a change of state
+    int check_step(const OwnFibers &own, const ::skb_fiber_params *params, const double *v_growth,
+                   const double *force_scale) const;
     const double *tangents() const { return (const double *)op_xs.ptr; }
 
   private:
@@ -557,6 +566,55 @@ cudaStream_t flow_stream(const skb_flow *fl); // the stream of the flow's own ca
 // sizes the buffers of the background streamer (skb_flow_set_overlap) for n_rows own periphery rows, if it is on
 int flow_size_overlap(skb_flow *fl, long long n_rows);
 
+// ---- and that the time step of a single-device flow needs (skb_step.cu) ----
+// the step's device buffers: per fiber its item and error, per fiber node its new position and tension, the external
+// forces and torques of the RHS.  Sized by skb_flow_set_gmres (the step itself allocates none of them)
+struct StepBuffers {
+    DevBuf items, r_new, tension, err, fext, force, torque;
+    int size(int n_fibers, long long n_fib, int n_bodies);
+    bool sized_for(int n_fibers, long long n_fib, int n_bodies) const {
+        return n_fibers_ == n_fibers && n_fib_ == n_fib && n_bodies_ == n_bodies;
+    }
+
+  private:
+    int n_fibers_ = -1, n_bodies_ = -1;
+    long long n_fib_ = -1;
+};
+struct FlowState {
+    OwnFibers fibers;               // every fiber of the flow
+    const double *length = nullptr; // host: length_ of every fiber (skb_flow_set_fibers)
+    const double *positions = nullptr; // host: the positions of every fiber node
+    long long n_shell = 0;
+    int n_bodies = 0;
+    const double *centers = nullptr, *orientations = nullptr; // host: where skb_flow_place_bodies last placed them
+    bool placed = false; // the bodies were placed since skb_flow_set_bodies last changed them (or there are none)
+    FiberOps *ops = nullptr;
+    BodyOps *bodies = nullptr;
+    StepBuffers *buf = nullptr;
+};
+FlowState flow_state(skb_flow *fl); // (its device current)
+// the refusals of the whole-vector system calls that do not depend on what the step itself sets (fiber operators and
+// links): no group member, the whole target list, dn holding both periphery operators, bodies placed with an inverse
+int flow_step_checks(skb_flow *fl, skb_dense *dn, const char *who);
+// R (row-major) of a unit quaternion (w, x, y, z): the formula of Eigen's QuaternionBase::toRotationMatrix
+void quaternion_rotation(const double *q, double *R);
+// the pieces of the step shared by skb_flow_step and skb_mflow_step (skb_step.cu).  launch_fiber_step: fiber_step_kernel
+// over the fibers `own` of the flow of s on st (items from FiberOps::step_items; from_solution: d_in is their block of a
+// solution, 4 per own node, new positions and tensions to s.buf; else d_in holds positions), errors to s.buf->err
+int launch_fiber_step(const FlowState &s, const OwnFibers &own, const std::vector<StepItem> &items, const double *d_in,
+                      bool from_solution, cudaStream_t st);
+// BodyContainer::step of one body from its rows U, w (DESIGN.md §5: always translated, q normalised)
+void body_step(const double *c, const double *q, const double *U, const double *w, double dt, double *c_new,
+               double *q_new);
+// per fiber c + R(q) site_ref of its body (0 for a free fiber)
+void nucleation_sites(int n_fibers, const int *body, const double *site_ref, const double *centers,
+                      const double *orientations, std::vector<double> &sites);
+// uw = the rows [U; w] (6 per body) of the body part x_bodies of a solution, bodies of n_nodes nodes
+void body_rows(const int *n_nodes, int n_bodies, const double *x_bodies, std::vector<double> &uw);
+bool all_finite(const std::vector<double> &a);
+// the max of per-fiber errors and the first fiber attaining it (NaN wins; none: 0 and -1)
+void reduce_errors(const std::vector<double> &err, double *max_error, int *worst);
+
 // The whole-vector operator on one member of skb_mflow (the members of a group, or the single flow of a one-device
 // skb_mflow), after its target ranges are set.  The arguments are those of skb_flow_set_body_operators /
 // _set_fiber_links for ALL bodies / fibers; a member keeps the part its ranges own (BodyOps).  check_only: check the
@@ -571,7 +629,7 @@ int flow_member_body_frames(skb_flow *fl, const int *n_nodes, int n_bodies, cons
                             const double *normal_ref, const double *node_weights, const double *ex0, const double *ey0,
                             const double *ez0, const double *A_inv0);
 int flow_member_place_args(skb_flow *fl, const double *centers, const double *orientations, std::vector<double> &R);
-int flow_member_place(skb_flow *fl, const double *centers, const std::vector<double> &R);
+int flow_member_place(skb_flow *fl, const double *centers, const double *orientations, const std::vector<double> &R);
 // the state the system calls need (system_args without the dense operator): an error naming `who` unless it is there
 int flow_member_system_ready(skb_flow *fl, const char *who, bool precondition);
 int flow_size_system(skb_flow *fl); // sizes the buffers the two calls below use (before any member launches)

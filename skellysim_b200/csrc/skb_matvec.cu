@@ -94,6 +94,10 @@ struct skb_flow {
     FiberOps ops; // per-fiber dense operators of the fibers whose rows are in the target list (skb_fiber.cu)
     BodyOps bodies; // the bodies' operators and the fiber-body links of the whole-vector operator (skb_body.cu)
     std::vector<double> h_centers; // body centres (set_fiber_links measures the nucleation sites from them)
+    std::vector<double> h_fiber_len; // length_ of every fiber (the time step installs its new positions with them)
+    std::vector<double> h_orient;    // the quaternions of the last skb_flow_place_bodies (4 per body) ...
+    bool placed = false;             // ... valid until skb_flow_set_bodies changes the bodies otherwise
+    StepBuffers stepbuf;             // the buffers of skb_flow_step (skb_step.cu)
     Group grp; // multi-GPU group membership: one member per GPU, exchange through peer memory (skb_group.cu)
     // a member's whole-vector matvec in flight: matvec_core exchanges the bodies' partial link forces through the
     // window and the body flow reads their totals from ft_sum ([F | L], 6 per body)
@@ -512,6 +516,7 @@ int skb_flow_set_fibers(skb_flow *fl, const double *r_fib, const int *n_nodes, c
     fl->max_fiber_nodes = max_n;
     fl->h_r_fib.assign(r_fib, r_fib + 3 * fl->n_fib);
     fl->h_fiber_n.assign(n_nodes, n_nodes + n_fibers);
+    fl->h_fiber_len.assign(length, length + n_fibers);
     fl->h_fiber_off = off;
     fl->ops.invalidate(); // operators belong to one set of fibers
     fl->bodies.drop_links(); // ... and so do the links
@@ -568,6 +573,7 @@ int skb_flow_set_bodies(skb_flow *fl, const double *node_pos, const double *node
     fl->n_bodies = n_bodies;
     fl->h_r_body.assign(node_pos, node_pos + 3 * n_nodes);
     fl->h_centers.assign(centers, centers + 3 * (size_t)n_bodies);
+    fl->placed = false; // skb_flow_place_bodies sets it again after this call
     fl->bodies.drop_operators(); // the bodies' operators and the nucleation sites belong to one placement
     fl->bodies.drop_links();
     fl->mv_dirty = true;
@@ -1706,8 +1712,7 @@ int skb_flow_set_fiber_links(skb_flow *fl, const int *body, const double *site, 
 
 // ---- rigid bodies placed from their body frame (BodyOps::set_frames / ::place, DESIGN.md §3.6) --------------------
 
-// R (row-major) of a unit quaternion (w, x, y, z): the formula of Eigen's QuaternionBase::toRotationMatrix
-static void quaternion_rotation(const double *q, double *R) {
+void skb::quaternion_rotation(const double *q, double *R) {
     const double w = q[0], x = q[1], y = q[2], z = q[3];
     const double tx = 2.0 * x, ty = 2.0 * y, tz = 2.0 * z;
     const double twx = tx * w, twy = ty * w, twz = tz * w;
@@ -1762,12 +1767,15 @@ static int placement_args(skb_flow *fl, const char *who, const double *centers, 
 
 // after placement_args: the nodes and normals through skb_flow_set_bodies (which drops the operators and the links),
 // then the operators from the frames
-static int place_bodies(skb_flow *fl, const double *centers, const std::vector<double> &R) {
+static int place_bodies(skb_flow *fl, const double *centers, const double *orientations, const std::vector<double> &R) {
     std::vector<double> pos, nrm;
     fl->bodies.placed_geometry(R.data(), centers, pos, nrm);
     SKB_TRY(skb_flow_set_bodies(fl, pos.data(), nrm.data(), fl->n_body, centers, fl->n_bodies));
     CUDA_TRY(cudaSetDevice(fl->dev));
-    return fl->bodies.place(R.data(), fl->h_r_body.data(), fl->h_centers.data(), fl->stream);
+    SKB_TRY(fl->bodies.place(R.data(), fl->h_r_body.data(), fl->h_centers.data(), fl->stream));
+    fl->h_orient.assign(orientations, orientations + 4 * (size_t)fl->n_bodies);
+    fl->placed = true;
+    return SKB_OK;
 }
 
 int skb::flow_member_body_frames(skb_flow *fl, const int *n_nodes, int n_bodies, const double *pos_ref,
@@ -1789,8 +1797,9 @@ int skb::flow_member_place_args(skb_flow *fl, const double *centers, const doubl
                           member ? fl->bb : -1, R);
 }
 
-int skb::flow_member_place(skb_flow *fl, const double *centers, const std::vector<double> &R) {
-    return place_bodies(fl, centers, R);
+int skb::flow_member_place(skb_flow *fl, const double *centers, const double *orientations,
+                           const std::vector<double> &R) {
+    return place_bodies(fl, centers, orientations, R);
 }
 
 extern "C" {
@@ -1815,7 +1824,7 @@ int skb_flow_place_bodies(skb_flow *fl, const double *centers, const double *ori
         return set_error(SKB_ERR_INVALID, "%s: a group member places its bodies with skb_flow_group_place_bodies", who);
     std::vector<double> R;
     SKB_TRY(placement_args(fl, who, centers, orientations, 0, -1, R));
-    return place_bodies(fl, centers, R);
+    return place_bodies(fl, centers, orientations, R);
 }
 
 int skb_flow_get_body_operators(skb_flow *fl, double *ex, double *ey, double *ez, double *A_inv) {
@@ -1835,6 +1844,23 @@ int skb_flow_get_body_operators(skb_flow *fl, double *ex, double *ey, double *ez
 
 } // extern "C"
 
+// dn holds the periphery's operator of the system call (matvec: stresslet_plus_complementary; precondition: M_inv)
+static int dense_args(skb_flow *fl, skb_dense *dn, const char *who, bool precondition) {
+    if (!dn)
+        return set_error(SKB_ERR_INVALID, "%s: the periphery needs its dense operator (dn == NULL)", who);
+    const int op = precondition ? SKB_DENSE_M_INV : SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY;
+    int dn_dev = -1;
+    int64_t rows = 0, cols = 0;
+    SKB_TRY(skb_dense_device(dn, 0, &dn_dev));
+    SKB_TRY(skb_dense_shape(dn, op, &rows, &cols));
+    if (dn_dev != fl->dev || rows != 3 * fl->n_shell || cols != 3 * fl->n_shell)
+        return set_error(SKB_ERR_INVALID, "%s: the dense handle holds a %lld x %lld %s on device %d, need %lld x %lld "
+                                          "on device %d", who, (long long)rows, (long long)cols,
+                         precondition ? "M_inv" : "stresslet_plus_complementary", dn_dev, 3 * fl->n_shell,
+                         3 * fl->n_shell, fl->dev);
+    return SKB_OK;
+}
+
 // The checks of the system operator (matvec: stresslet_plus_complementary in dn; precondition: M_inv and the
 // inverses), all before any launch; then the flow's device is current and its target list resolved.
 static int system_args(skb_flow *fl, skb_dense *dn, const char *who, bool precondition, bool args) {
@@ -1851,20 +1877,8 @@ static int system_args(skb_flow *fl, skb_dense *dn, const char *who, bool precon
     if (fl->n_win != n_all)
         return set_error(SKB_ERR_INVALID, "%s: needs the whole target list (%lld of %lld rows are set by a target window "
                                           "or ranges); multi-GPU is not supported", who, fl->n_win, n_all);
-    if (fl->n_shell > 0) {
-        if (!dn)
-            return set_error(SKB_ERR_INVALID, "%s: the periphery needs its dense operator (dn == NULL)", who);
-        const int op = precondition ? SKB_DENSE_M_INV : SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY;
-        int dn_dev = -1;
-        int64_t rows = 0, cols = 0;
-        SKB_TRY(skb_dense_device(dn, 0, &dn_dev));
-        SKB_TRY(skb_dense_shape(dn, op, &rows, &cols));
-        if (dn_dev != fl->dev || rows != 3 * fl->n_shell || cols != 3 * fl->n_shell)
-            return set_error(SKB_ERR_INVALID, "%s: the dense handle holds a %lld x %lld %s on device %d, need %lld x %lld "
-                                              "on device %d", who, (long long)rows, (long long)cols,
-                             precondition ? "M_inv" : "stresslet_plus_complementary", dn_dev, 3 * fl->n_shell,
-                             3 * fl->n_shell, fl->dev);
-    }
+    if (fl->n_shell > 0)
+        SKB_TRY(dense_args(fl, dn, who, precondition));
     if (fl->n_bodies > 0) {
         if (!fl->bodies.has_operators())
             return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_body_operators after skb_flow_set_bodies", who);
@@ -2397,7 +2411,7 @@ int skb_flow_group_place_bodies(skb_flow *fl, const double *centers, const doubl
     SKB_TRY(prepare_matvec_targets(fl));
     std::vector<double> R;
     SKB_TRY(placement_args(fl, who, centers, orientations, fl->ba, fl->bb, R));
-    SKB_TRY(place_bodies(fl, centers, R));
+    SKB_TRY(place_bodies(fl, centers, orientations, R));
     return prepare_matvec_targets(fl); // the new body rows' targets now, not at the first matvec
 }
 
@@ -2596,4 +2610,45 @@ int skb::flow_member_lay_out_rows(skb_flow *fl, const int *n_nodes, int n_bodies
 cudaStream_t skb::flow_stream(const skb_flow *fl) { return fl->stream; }
 int skb::flow_size_overlap(skb_flow *fl, long long n_rows) {
     return fl->bg.enabled ? overlap_buffers(fl, n_rows) : SKB_OK;
+}
+
+FlowState skb::flow_state(skb_flow *fl) {
+    FlowState s;
+    s.fibers = OwnFibers{0, fl->n_fibers, fl->h_fiber_n.data(), fl->h_fiber_off.data(), (const double *)fl->r_fib.ptr,
+                         (const double *)fl->fiber_length.ptr, fl->stream};
+    s.length = fl->h_fiber_len.data();
+    s.positions = fl->h_r_fib.data();
+    s.n_shell = fl->n_shell;
+    s.n_bodies = fl->n_bodies;
+    s.centers = fl->h_centers.data();
+    s.orientations = fl->h_orient.data();
+    s.placed = fl->n_bodies == 0 || fl->placed;
+    s.ops = &fl->ops;
+    s.bodies = &fl->bodies;
+    s.buf = &fl->stepbuf;
+    return s;
+}
+
+int skb::flow_step_checks(skb_flow *fl, skb_dense *dn, const char *who) {
+    if (fl->grp.member())
+        return set_error(SKB_ERR_INVALID, "%s: a group member does not step (every member would need the others' new "
+                                          "fiber positions); over several devices use skb_mflow", who);
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    SKB_TRY(prepare_matvec_targets(fl));
+    const long long n_all = fl->n_fib + fl->n_shell + fl->n_body;
+    if (fl->n_win != n_all)
+        return set_error(SKB_ERR_INVALID, "%s: needs the whole target list (%lld of %lld rows are set by a target window "
+                                          "or ranges)", who, fl->n_win, n_all);
+    if (fl->n_shell > 0) {
+        SKB_TRY(dense_args(fl, dn, who, false));
+        SKB_TRY(dense_args(fl, dn, who, true));
+    }
+    if (fl->n_bodies > 0) {
+        if (!fl->bodies.has_frames() || !fl->placed || !fl->bodies.has_operators())
+            return set_error(SKB_ERR_INVALID, "%s: the step places the bodies from their frames: call "
+                                              "skb_flow_set_body_frames and a first skb_flow_place_bodies", who);
+        if (!fl->bodies.has_inverse())
+            return set_error(SKB_ERR_INVALID, "%s: skb_flow_set_body_frames was given no A_inv", who);
+    }
+    return SKB_OK;
 }
