@@ -138,6 +138,9 @@ typedef struct skb_eval_stats {
 SKB_API int skb_last_eval_stats(const skb_ctx *ctx, skb_eval_stats *out);
 /* total number of kernels this library has launched in this process */
 SKB_API int64_t skb_launch_count(void);
+/* total number of times this library's grow-only device buffers have allocated (cudaMalloc) in this process: a call
+ * documented to allocate nothing leaves it unchanged */
+SKB_API int64_t skb_buffer_alloc_count(void);
 /* tuning overrides (0 = automatic): targets per thread in {1,2,4,8}, source splits >= 1 */
 SKB_API int skb_ctx_set_tuning(skb_ctx *ctx, int targets_per_thread, int source_splits);
 

@@ -545,6 +545,39 @@ SKB_API int skb_flow_step(skb_flow *fl, struct skb_dense *dn, const skb_fiber_pa
                           const int *fiber_body, const double *site_ref, double dt, double eta, double tol,
                           int num_blocks, int max_iters, double *x, double *tension, skb_step_info *info);
 SKB_API int skb_flow_fiber_error(skb_flow *fl, double *max_error, double *per_fiber);
+/* skb_flow_step on one rank per GPU, on a connected group member (the local-vector calls below).  params, v_growth,
+ * force_scale, fiber_body and site_ref cover the OWN fibers (as skb_flow_group_set_fiber_links); d_f_external holds 3
+ * values per own fiber node, d_body_forces / d_body_torques 3 per body of ALL bodies (each NULL ok), all on the device;
+ * dn_spc / dn_minv are the member's row blocks of the two periphery operators.  In order:
+ *   1. skb_flow_group_set_fiber_links from the current placement, skb_flow_build_fiber_operators,
+ *      skb_flow_group_build_system_rhs_device and skb_flow_group_solve_system_device: the solution is bitwise what a
+ *      caller composing those calls gets;
+ *   2. the body rows all-gathered through the group window (an epoch of its own): every member reads [U; w] of every
+ *      body from its own window and steps the bodies on the host, so all hold the same placement and sites;
+ *   3. the step kernel over the own fibers, its new positions and per-fiber errors stored straight into every member's
+ *      window (an epoch of its own); every member reads the complete positions and errors from its own window;
+ *   4. the non-finite checks and the error's max over the COMPLETE arrays: every member returns the same code,
+ *      fiber_error and worst_fiber (a fiber index among ALL fibers); a non-finite solution is installed by no member
+ *      (SKB_ERR_STATE, NaN fiber_error);
+ *   5. the install: skb_flow_set_fibers with the complete positions, skb_flow_group_place_bodies, and
+ *      skb_flow_group_set_fiber_links at the new sites.
+ * d_x_local (NULL ok) receives the member's local rows of the solution, d_tension (NULL ok) the tension of its own
+ * fiber nodes.  The call runs on `stream` (the links, the build and the install on the flow's own stream, drained
+ * before it returns).  It allocates no device memory and loads no kernel: skb_flow_set_gmres on the member, called
+ * after the fiber classes and their derivatives are set, sizes and loads what it uses -- the step's buffers, the fiber
+ * build's and the fiber-body links' for the own fibers, and a pinned host copy through which the device inputs' finiteness
+ * is checked (DESIGN.md §3.9).  Every member must call it alike.  Refused, locally and before any launch: what
+ * skb_flow_step refuses (but for membership and the whole target list; f_external and the body forces and torques are
+ * read back for their check), what the local-vector calls refuse, no skb_flow_set_gmres for the member's current target
+ * ranges or none since the fiber classes were set, a fiber_body index outside [-1, n_bodies) among the own fibers.  On a flow that is no group member: skb_flow_step, its x and tension on the device (dn_spc holds both
+ * operators; dn_minv is not read). */
+SKB_API int skb_flow_group_step_device(skb_flow *fl, struct skb_dense *dn_spc, struct skb_dense *dn_minv,
+                                       const skb_fiber_params *params, const double *v_growth,
+                                       const double *force_scale, const double *d_f_external,
+                                       const double *d_body_forces, const double *d_body_torques,
+                                       const int *fiber_body, const double *site_ref, double dt, double eta,
+                                       double tol, int num_blocks, int max_iters, double *d_x_local,
+                                       double *d_tension, skb_step_info *info, void *stream);
 SKB_API int skb_flow_get_placement(skb_flow *fl, double *centers, double *orientations);
 SKB_API int skb_flow_get_fibers(skb_flow *fl, double *r_fib);
 

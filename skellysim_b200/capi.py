@@ -119,6 +119,7 @@ def library() -> C.CDLL:
         "skb_sync": ([ctxp], C.c_int),
         "skb_last_eval_stats": ([ctxp, C.POINTER(EvalStats)], C.c_int),
         "skb_launch_count": ([], C.c_int64),
+        "skb_buffer_alloc_count": ([], C.c_int64),
         "skb_ctx_set_tuning": ([ctxp, C.c_int, C.c_int], C.c_int),
         "skb_measure_fp64_peak": ([ctxp, C.POINTER(C.c_double)], C.c_int),
         "skb_ctx_set_symmetric": ([ctxp, C.c_int], C.c_int),
@@ -263,6 +264,9 @@ def library() -> C.CDLL:
         "skb_flow_get_fibers": ([ctxp, _dp], C.c_int),
         "skb_mflow_step": ([ctxp, C.POINTER(FiberParams), _dp, _dp, _dp, _dp, C.POINTER(C.c_int), _dp, C.c_double,
                             C.c_double, C.c_double, C.c_int, C.c_int, _dp, _dp, C.POINTER(StepInfo)], C.c_int),
+        "skb_flow_group_step_device": ([ctxp, ctxp, ctxp, C.POINTER(FiberParams), _dp, _dp] + [C.c_void_p] * 3
+                                       + [C.POINTER(C.c_int), _dp, C.c_double, C.c_double, C.c_double, C.c_int,
+                                          C.c_int, C.c_void_p, C.c_void_p, C.POINTER(StepInfo), C.c_void_p], C.c_int),
         "skb_mflow_get_fibers": ([ctxp, _dp], C.c_int),
         "skb_mflow_get_placement": ([ctxp, _dp, _dp], C.c_int),
         "skb_mflow_solve_system": ([ctxp, _dp, C.c_double, C.c_double, C.c_int, C.c_int, _dp, C.POINTER(SolveInfo),
@@ -403,6 +407,11 @@ def device_count() -> int:
 
 def launch_count() -> int:
     return int(library().skb_launch_count())
+
+
+def buffer_alloc_count() -> int:
+    """device allocations of the library's grow-only buffers in this process (skb_buffer_alloc_count)"""
+    return int(library().skb_buffer_alloc_count())
 
 
 def stokeslet_direct(r_src, f_src, r_trg):
@@ -1217,6 +1226,36 @@ class Flow:
                                                                 vp(d_f_external), vp(d_body_forces),
                                                                 vp(d_body_torques), float(dt), float(eta),
                                                                 vp(d_rhs_local), vp(stream)))
+
+    def group_step_device(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
+                          plus_hinged, dt, eta, dense_matvec=None, dense_minv=None, d_f_external: int = 0,
+                          d_body_forces: int = 0, d_body_torques: int = 0, fiber_body=None, site_ref=None,
+                          v_growth=None, force_scale=None, tol=1e-10, num_blocks=300, max_iters=1000,
+                          d_x_local: int = 0, d_tension: int = 0, stream: int = 0):
+        """step on a group member (skb_flow_group_step_device): the fibers' parameters, fiber_body and site_ref of the
+        OWN fibers, f_external of their nodes and the forces / torques ((n_bodies, 3) each) of ALL bodies as device
+        pointers (0: none); d_x_local / d_tension (0: not wanted) receive the member's local rows of the solution and
+        its own fibers' tensions.  Every member calls it alike and gets the same info dict; a solution with non-finite
+        new positions installs nothing on any member and returns fiber_error NaN.  Not a member: step()."""
+        f0, f1 = self._own_fibers()
+        p, vg, fs, _, _ = _system_rhs_args(f1 - f0, 0, self.n_bodies,
+                                           (length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
+                                            minus_clamped, plus_hinged), v_growth, force_scale, None, None)
+        fb = None if fiber_body is None else np.ascontiguousarray(fiber_body, dtype=np.int32).reshape(-1)
+        if fb is not None and fb.shape[0] != f1 - f0:
+            raise ValueError(f"expected {f1 - f0} fiber_body entries (the own fibers), got {fb.shape[0]}")
+        sr = None if site_ref is None else _arr(site_ref, 3)
+        vp = lambda a: C.c_void_p(a) if a else None
+        h = lambda d: d._h if d is not None else None
+        info = StepInfo()
+        rc = library().skb_flow_group_step_device(
+            self._h, h(dense_matvec), h(dense_minv), _params_ptr(p), _opt_p(vg), _opt_p(fs), vp(d_f_external),
+            vp(d_body_forces), vp(d_body_torques), None if fb is None else fb.ctypes.data_as(C.POINTER(C.c_int)),
+            _opt_p(sr), float(dt), float(eta), float(tol), int(num_blocks), int(max_iters), vp(d_x_local),
+            vp(d_tension), C.byref(info), vp(stream))
+        if not (rc == ERR_STATE and np.isnan(info.fiber_error)):
+            _check(rc)
+        return info.as_dict()
 
     def stats(self) -> dict:
         s = FlowStats()

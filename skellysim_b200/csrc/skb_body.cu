@@ -313,6 +313,15 @@ int BodyOps::set_links(const OwnFibers &own, const FiberOps &ops, int n_bodies, 
     return SKB_OK;
 }
 
+int BodyOps::size_links(int n_fibers, int n_bodies) {
+    const size_t nf = (size_t)std::max(n_fibers, 0);
+    SKB_TRY(link_fibers_.ensure(nf * sizeof(LinkFiber)));
+    SKB_TRY(csr_begin_.ensure(((size_t)std::max(n_bodies, 0) + 1) * sizeof(int)));
+    SKB_TRY(csr_fib_.ensure(nf * sizeof(int)));
+    SKB_TRY(link_.ensure(nf * 56));
+    return contrib_.ensure(nf * 48);
+}
+
 int BodyOps::links(const FiberOps &ops, const double *d_length, const double *d_x_fib, const double *d_x_bodies,
                    const double **d_link, cudaStream_t st, int *launches) {
     *d_link = nullptr;

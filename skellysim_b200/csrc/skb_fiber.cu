@@ -405,6 +405,40 @@ int FiberOps::step_items(const OwnFibers &own, std::vector<StepItem> &items) con
     return SKB_OK;
 }
 
+int FiberOps::size_build(const OwnFibers &own) {
+    cudaFuncAttributes fa;
+    CUDA_TRY(cudaFuncGetAttributes(&fa, fiber_assemble_kernel));
+    const int nfib = own.count();
+    for (int f = own.f0; f < own.f1; ++f) { // a class the build lacks: nothing to size, the build refuses later
+        const auto it = classes.find(own.n[f]);
+        if (it == classes.end() || it->second.D.empty() || it->second.D234.empty() || own.n[f] < kBuildMinNodes ||
+            own.n[f] > kBuildMaxNodes)
+            return SKB_OK;
+    }
+    const std::array<long long, 4> key = build_key(own);
+    if (nfib == 0) {
+        build_key_ = key;
+        return SKB_OK;
+    }
+    const std::vector<skb_fiber_params> params((size_t)nfib, skb_fiber_params{});
+    Plan b;
+    const size_t smem = gemv_smem; // (the plan's GEMV bound belongs to the resident operators until the build)
+    const int rc = plan(own, nullptr, params.data(), b);
+    gemv_smem = smem;
+    SKB_TRY(rc);
+    for (auto [buf, bytes] : std::initializer_list<std::pair<DevBuf *, size_t>>{
+             {&op_A, (size_t)b.offA * 8}, {&op_F, (size_t)b.offF * 8}, {&op_xs, (size_t)own.nodes() * 24},
+             {&op_Ainv, (size_t)b.offA * 8}, {&op_classD, b.cD.size() * 8}, {&op_classP, b.cP.size() * 8},
+             {&op_classR, b.cR.size() * 8}, {&items_A, b.itA.size() * sizeof(FiberGemvItem)},
+             {&items_F, b.itF.size() * sizeof(FiberGemvItem)}, {&op_len, b.lp.size() * 8},
+             {&op_plus, b.plus.size() * sizeof(int)}, {&bld_params, (size_t)nfib * sizeof(skb_fiber_params)},
+             {&bld_items, b.items.size() * sizeof(FiberItem)}, {&bld_tiles, b.tiles.size() * sizeof(FiberTileItem)},
+             {&bld_inv, b.inv_off.size() * sizeof(long long)}})
+        SKB_TRY(buf->ensure(bytes));
+    build_key_ = key;
+    return SKB_OK;
+}
+
 int FiberOps::size_rhs(int n_fibers) {
     const size_t n = (size_t)std::max(n_fibers, 0);
     SKB_TRY(rhs_items.ensure(n * sizeof(FiberItem)));

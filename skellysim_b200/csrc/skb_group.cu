@@ -21,7 +21,7 @@ static int launched(int *launches) {
 }
 
 int Group::init(int rank, int size, long long n_fib, long long n_pad_fib, long long n_shell, long long n_pad_shell,
-                long long n_body, int n_bodies) {
+                long long n_body, int n_bodies, int n_fibers) {
     *this = Group(); // the old window and mappings are released here
     if (size == 1)
         return SKB_OK;
@@ -31,6 +31,7 @@ int Group::init(int rank, int size, long long n_fib, long long n_pad_fib, long l
     n_shell_ = n_shell;
     n_body_ = n_body;
     n_bodies_ = n_bodies;
+    n_fibers_ = n_fibers;
     size_t off = 0;
     auto take = [&](size_t bytes) {
         const size_t at = off;
@@ -45,6 +46,7 @@ int Group::init(int rank, int size, long long n_fib, long long n_pad_fib, long l
         lay_.ft_part[b] = take((size_t)kMaxGroup * n_bodies * 48 + 16);
         lay_.x_body[b] = take((size_t)n_body * 24 + (size_t)n_bodies * 48 + 16);
         lay_.dots[b] = take((size_t)kMaxGroup * kDotsSlot * 8);
+        lay_.r_step[b] = take((size_t)n_fib * 24 + (size_t)n_fibers * 8 + 16);
     }
     lay_.u_part = take((size_t)n_fib * 24 + 16);
     lay_.u_part_shell = take((size_t)n_shell * 24 + 16);
@@ -85,7 +87,7 @@ int Group::import_handle(int peer_rank, const void *handle) {
 
 int Group::connect(int peer_rank, const Group &peer, int dev, int peer_dev) {
     if (peer.lay_.bytes != lay_.bytes || peer.n_fib_ != n_fib_ || peer.n_shell_ != n_shell_ ||
-        peer.n_body_ != n_body_ || peer.n_bodies_ != n_bodies_)
+        peer.n_body_ != n_body_ || peer.n_bodies_ != n_bodies_ || peer.n_fibers_ != n_fibers_)
         return set_error(SKB_ERR_INVALID, "skb_flow_group_connect: the two members were laid out for different geometries");
     if (peer_dev != dev) {
         int can = 0;
@@ -115,12 +117,12 @@ int Group::missing_peer(int *missing) const {
     return SKB_OK;
 }
 
-int Group::check_layout(long long n_fib, long long n_shell, long long n_body, int n_bodies) const {
-    if (n_fib_ != n_fib || n_shell_ != n_shell || n_body_ != n_body || n_bodies_ != n_bodies)
+int Group::check_layout(long long n_fib, long long n_shell, long long n_body, int n_bodies, int n_fibers) const {
+    if (n_fib_ != n_fib || n_shell_ != n_shell || n_body_ != n_body || n_bodies_ != n_bodies || n_fibers_ != n_fibers)
         return set_error(SKB_ERR_STATE, "group member: the geometry changed size since skb_flow_group_init "
-                                        "(%lld/%lld fiber, %lld/%lld periphery, %lld/%lld body nodes, %d/%d bodies); "
-                                        "re-initialise the group", n_fib, n_fib_, n_shell, n_shell_, n_body, n_body_,
-                         n_bodies, n_bodies_);
+                                        "(%lld/%lld fiber, %lld/%lld periphery, %lld/%lld body nodes, %d/%d bodies, "
+                                        "%d/%d fibers); re-initialise the group", n_fib, n_fib_, n_shell, n_shell_,
+                         n_body, n_body_, n_bodies, n_bodies_, n_fibers, n_fibers_);
     return SKB_OK;
 }
 
@@ -265,6 +267,14 @@ int Group::pull(Partials which, long long row0, long long n_rows, double *d_v, c
     a.accumulate = 1;
     group_pull_kernel<<<(unsigned)((3 * n_rows + 255) / 256), 256, 0, st>>>(a);
     return launched(launches);
+}
+
+int Group::step_windows(double **r_step) const {
+    char *w[kMaxGroup];
+    const int n = windows(w);
+    for (int m = 0; m < n; ++m)
+        r_step[m] = (double *)(w[m] + lay_.r_step[epoch_ & 1]);
+    return n;
 }
 
 // ---- a rank-per-GPU member's own rows of the solution vector ----

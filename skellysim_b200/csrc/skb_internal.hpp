@@ -205,6 +205,11 @@ class FiberOps {
     // the per-fiber tables and the event of rhs() for n_fibers own fibers, at their final size (a group member's RHS
     // must not allocate once its peers may wait on a flag)
     int size_rhs(int n_fibers);
+    // every buffer build() fills for the fibers `own` at its final size, and the assembly kernel loaded (a group step
+    // builds while its peers may wait on a flag); nothing is sized while a class the build needs is missing, and then
+    // build_sized_for(own) stays false
+    int size_build(const OwnFibers &own);
+    bool build_sized_for(const OwnFibers &own) const { return build_key_ == build_key(own); }
     int ready(const char *who, bool with_inverse = false) const; // an error naming `who` unless they are resident
     bool empty() const { return n_items_A == 0; }
     int n_fibers() const { return f1 - f0; }
@@ -261,6 +266,11 @@ class FiberOps {
     DevBuf rhs_items, rhs_params, rhs_growth;
     Event rhs_done;
     bool rhs_pending = false;
+    // the fibers and nodes size_build sized for
+    static std::array<long long, 4> build_key(const OwnFibers &own) {
+        return {own.f0, own.f1, own.count() > 0 ? own.off[own.f0] : 0, own.nodes()};
+    }
+    std::array<long long, 4> build_key_ = {-1, -1, -1, -1};
 };
 
 struct FiberGemvItem; // fiber_ops.cuh
@@ -291,6 +301,9 @@ class BodyOps {
     // check_only: the checks and nothing else
     int set_links(const OwnFibers &own, const FiberOps &ops, int n_bodies, const double *centers, const int *body,
                   const double *site, const double *rigidity, cudaStream_t st, bool check_only = false);
+    // every buffer set_links fills, at its size for n_fibers fibers (all of them bound) and n_bodies bodies: a later
+    // set_links of as many fibers allocates nothing (a group step sets the links while its peers may wait on a flag)
+    int size_links(int n_fibers, int n_bodies);
     // The body frame of rigid bodies (skb_flow_set_body_frames): per body n_nodes (summing to n_body_nodes), the
     // reference nodes, normals and weights (3, 3, 1 per node), ex_ / ey_ / ez_ and A_^-1 (may be NULL) at identity
     // orientation.  Kept resident next to the placed operators, the inverses of the bodies a member owns rows of only;
@@ -390,6 +403,8 @@ int load_dense_kernels();
 //                                    its own rows; skb_flow_group_apply_system_*)                   -- by peers
 //   dots         [2][kMaxGroup][kDotsSlot]  per member its partial dot products of a solve step (reduce_dots)
 //                                    -- by peers
+//   r_step       [2][n_fib*3 + n_fibers]  the new positions of ALL fiber nodes and the errors of ALL fibers after a
+//                                    group step (skb_flow_group_step_device; group_fiber_step_kernel)  -- by peers
 //   u_part       [n_fib*3]           this member's partial velocities of ALL fiber rows                  -- by itself
 //   u_part_shell [n_shell*3]         its partial velocities of ALL periphery rows (cross kernel)        -- by itself
 //
@@ -399,11 +414,11 @@ int load_dense_kernels();
 // current, and every step runs on the stream it passes, adding its launches to *launches.
 class Group {
   public:
-    // allocates and zeroes the window of member `rank` of `size` for that many fiber / periphery / body nodes and
-    // bodies; n_pad_*: the padded source counts of the flow's evaluators (the window replaces their packed strengths).
-    // Size 1: no member
+    // allocates and zeroes the window of member `rank` of `size` for that many fiber / periphery / body nodes, bodies
+    // and fibers; n_pad_*: the padded source counts of the flow's evaluators (the window replaces their packed
+    // strengths).  Size 1: no member
     int init(int rank, int size, long long n_fib, long long n_pad_fib, long long n_shell, long long n_pad_shell,
-             long long n_body, int n_bodies);
+             long long n_body, int n_bodies, int n_fibers);
     int export_handle(void *handle) const;                     // the window's CUDA-IPC handle
     int import_handle(int peer_rank, const void *handle);      // maps another process's member's window
     int connect(int peer_rank, const Group &peer, int dev, int peer_dev); // a member in this process, on peer_dev
@@ -414,7 +429,7 @@ class Group {
     int rank() const { return rank_; }
     int size() const { return size_; }
     // an error unless laid out for these
-    int check_layout(long long n_fib, long long n_shell, long long n_body, int n_bodies) const;
+    int check_layout(long long n_fib, long long n_shell, long long n_body, int n_bodies, int n_fibers) const;
     // solo (warm-up, profiling): no flags, push and pull over this member's own window only, no connectedness check
     void set_solo(bool solo) { solo_ = solo; }
     void restart() { epoch_ = 0; } // the next matvec is the group's first
@@ -457,18 +472,24 @@ class Group {
     // the sum over every member's d_v in rank order, bitwise the same on every member.  Not a member: nothing to do
     int reduce_dots(double *d_v, int m, cudaStream_t st, int *launches);
 
+    // ---- the all-gather of a group step's new fiber positions and errors (skb_flow_group_step_device) ----
+    // r_step of every window the step's store reaches, in the current epoch's half (solo: the own one only); returns
+    // their count.  The store is group_fiber_step_kernel itself; then the rows phase's barrier, in the step's epoch
+    int step_windows(double **r_step) const;
+
     // this member's window, in the half of the matvec in flight
     double *f_sl() const { return own(lay_.f_sl[epoch_ & 1]); }
     double *f_shell() const { return own(lay_.f_shell[epoch_ & 1]); }
     double *x_shell() const { return own(lay_.x_shell[epoch_ & 1]); }
     double *x_body() const { return own(lay_.x_body[epoch_ & 1]); }
+    double *r_step() const { return own(lay_.r_step[epoch_ & 1]); }
     double *u_part() const { return own(lay_.u_part); }
     double *u_part_shell() const { return own(lay_.u_part_shell); }
 
   private:
     struct Layout { // byte offsets of the window's pieces
         size_t flags = 0, f_sl[2] = {0, 0}, f_shell[2] = {0, 0}, x_shell[2] = {0, 0}, ft_part[2] = {0, 0},
-               x_body[2] = {0, 0}, dots[2] = {0, 0}, u_part = 0, u_part_shell = 0;
+               x_body[2] = {0, 0}, dots[2] = {0, 0}, r_step[2] = {0, 0}, u_part = 0, u_part_shell = 0;
         size_t bytes = 0;
     };
     struct Rows { // the piece table of set_body_rows, as the kernels take it (RowPiecesDev, group_kernels.cuh)
@@ -485,7 +506,7 @@ class Group {
     void *peer_[kMaxGroup] = {}; // every member's window as mapped here (peer_[rank_] == window_)
     IpcPtr ipc_[kMaxGroup];      // the windows of other processes' members that this one has mapped
     long long n_fib_ = 0, n_shell_ = 0, n_body_ = 0; // geometry the window was laid out for
-    int n_bodies_ = 0;
+    int n_bodies_ = 0, n_fibers_ = 0;
     unsigned long long epoch_ = 0;
     bool solo_ = false;
     Rows rows_;
@@ -568,9 +589,11 @@ int flow_size_overlap(skb_flow *fl, long long n_rows);
 
 // ---- and that the time step of a single-device flow needs (skb_step.cu) ----
 // the step's device buffers: per fiber its item and error, per fiber node its new position and tension, the external
-// forces and torques of the RHS.  Sized by skb_flow_set_gmres (the step itself allocates none of them)
+// forces and torques of the RHS; and a pinned host copy of a group step's device inputs (3 per fiber node + 6 per body)
+// for their finiteness check.  Sized by skb_flow_set_gmres (the step itself allocates none of them)
 struct StepBuffers {
     DevBuf items, r_new, tension, err, fext, force, torque;
+    PinnedHost check;
     int size(int n_fibers, long long n_fib, int n_bodies);
     bool sized_for(int n_fibers, long long n_fib, int n_bodies) const {
         return n_fibers_ == n_fibers && n_fib_ == n_fib && n_bodies_ == n_bodies;
@@ -579,6 +602,7 @@ struct StepBuffers {
   private:
     int n_fibers_ = -1, n_bodies_ = -1;
     long long n_fib_ = -1;
+    size_t check_cap_ = 0; // doubles of `check`
 };
 struct FlowState {
     OwnFibers fibers;               // every fiber of the flow
@@ -596,6 +620,14 @@ FlowState flow_state(skb_flow *fl); // (its device current)
 // the refusals of the whole-vector system calls that do not depend on what the step itself sets (fiber operators and
 // links): no group member, the whole target list, dn holding both periphery operators, bodies placed with an inverse
 int flow_step_checks(skb_flow *fl, skb_dense *dn, const char *who);
+// a group member (skb_flow_set_gmres): the fiber build's and the links' buffers for its own fibers at their final size
+// (FiberOps::size_build, BodyOps::size_links); else nothing
+int flow_size_group_step(skb_flow *fl);
+// the same for a group member's step (skb_flow_group_step_device): its peers connected, its rows laid out for its
+// target ranges, dn_spc / dn_minv its row blocks of the two periphery operators, bodies placed with an inverse; then
+// own = its fibers, *n its local solution size and *key its ranges (what skb_flow_set_gmres sized for)
+int flow_group_step_checks(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const char *who, OwnFibers &own,
+                           long long *n, std::array<long long, 6> *key);
 // R (row-major) of a unit quaternion (w, x, y, z): the formula of Eigen's QuaternionBase::toRotationMatrix
 void quaternion_rotation(const double *q, double *R);
 // the pieces of the step shared by skb_flow_step and skb_mflow_step (skb_step.cu).  launch_fiber_step: fiber_step_kernel

@@ -787,7 +787,7 @@ static int prepare_matvec_targets(skb_flow *fl) {
         if (!fl->use_ranges)
             return set_error(SKB_ERR_STATE, "group member: call skb_flow_set_target_ranges (own fibers / periphery rows / "
                                             "body rows) before the first matvec");
-        SKB_TRY(fl->grp.check_layout(nf, ns, nb, fl->n_bodies));
+        SKB_TRY(fl->grp.check_layout(nf, ns, nb, fl->n_bodies, fl->n_fibers));
     }
     // group: fiber rows through the symmetric block rows of this member (partial sums, pulled together afterwards)
     // when the self-interaction is big enough for that kernel; otherwise the member's own rows with the plain kernel
@@ -1060,7 +1060,8 @@ int skb_flow_group_init(skb_flow *fl, int rank, int size) {
     // the same padded sizes the evaluator contexts use (set_sources_impl): the window replaces their f_packed
     const long long n_pad_fib = fl->n_fib > 0 ? fl->fib[1]->devs[0].src[SKB_STOKESLET].n_pad : 0;
     const long long n_pad_shell = fl->n_shell > 0 ? fl->shell[1]->devs[0].src[SKB_STRESSLET].n_pad : 0;
-    return fl->grp.init(rank, size, fl->n_fib, n_pad_fib, fl->n_shell, n_pad_shell, fl->n_body, fl->n_bodies);
+    return fl->grp.init(rank, size, fl->n_fib, n_pad_fib, fl->n_shell, n_pad_shell, fl->n_body, fl->n_bodies,
+                        fl->n_fibers);
 }
 
 int skb_flow_group_export(skb_flow *fl, void *handle) {
@@ -2297,6 +2298,8 @@ static long long group_local_size(const skb_flow *fl) {
     return 4 * (fl->fb - fl->fa) + 3 * (fl->sb - fl->sa) + fl->grp.body_rows();
 }
 
+static int group_dense_args(skb_flow *fl, skb_dense *dn, const char *who, bool precondition);
+
 // the refusals of the group matvec (stresslet_plus_complementary in dn) and preconditioner (M_inv in dn, the inverses),
 // all before any launch; then the flow's device is current and its target ranges resolved
 static int group_system_args(skb_flow *fl, skb_dense *dn, const char *who, bool precondition) {
@@ -2317,6 +2320,11 @@ static int group_system_args(skb_flow *fl, skb_dense *dn, const char *who, bool 
             return set_error(SKB_ERR_INVALID, "%s: call skb_flow_group_set_fiber_links after skb_flow_set_fibers / "
                                               "skb_flow_set_bodies (NULL body: no fiber is bound)", who);
     }
+    return group_dense_args(fl, dn, who, precondition);
+}
+
+// dn: the member's row block of M_inv (precondition) or stresslet_plus_complementary, if it owns periphery rows
+static int group_dense_args(skb_flow *fl, skb_dense *dn, const char *who, bool precondition) {
     const long long n_sw = fl->sb - fl->sa;
     if (n_sw > 0) {
         const int op = precondition ? SKB_DENSE_M_INV : SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY;
@@ -2605,6 +2613,39 @@ int skb::flow_member_lay_out_rows(skb_flow *fl, const int *n_nodes, int n_bodies
     SKB_TRY(load_dense_kernels());
     fl->grp.set_body_rows(pieces, group_ranges(fl));
     return SKB_OK;
+}
+
+int skb::flow_group_step_checks(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const char *who, OwnFibers &own,
+                                long long *n, std::array<long long, 6> *key) {
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    SKB_TRY(fl->grp.connected());
+    SKB_TRY(own_fibers(fl, who, own)); // the target ranges resolved, whole fibers, the window's layout checked
+    if (!fl->grp.rows_for(group_ranges(fl)))
+        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_group_set_body_frames / _set_body_operators after "
+                                          "skb_flow_group_init and after every change of the target ranges", who);
+    SKB_TRY(group_dense_args(fl, dn_spc, who, false));
+    SKB_TRY(group_dense_args(fl, dn_minv, who, true));
+    if (fl->n_bodies > 0) {
+        if (!fl->bodies.has_frames() || !fl->placed || !fl->bodies.has_operators())
+            return set_error(SKB_ERR_INVALID, "%s: the step places the bodies from their frames: call "
+                                              "skb_flow_group_set_body_frames and a first skb_flow_group_place_bodies",
+                             who);
+        if (!fl->bodies.has_inverse())
+            return set_error(SKB_ERR_INVALID, "%s: skb_flow_group_set_body_frames was given no A_inv", who);
+    }
+    *n = group_local_size(fl);
+    *key = group_ranges(fl);
+    return SKB_OK;
+}
+
+int skb::flow_size_group_step(skb_flow *fl) {
+    if (!fl->grp.member())
+        return SKB_OK;
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    OwnFibers own;
+    SKB_TRY(own_fibers(fl, "skb_flow_set_gmres", own));
+    SKB_TRY(fl->ops.size_build(own));
+    return fl->bodies.size_links(own.count(), fl->n_bodies);
 }
 
 cudaStream_t skb::flow_stream(const skb_flow *fl) { return fl->stream; }

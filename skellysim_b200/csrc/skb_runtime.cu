@@ -30,6 +30,7 @@ namespace skb {
 // ------------------------------------------------------------------------------------------------
 static thread_local std::string g_last_error = "";
 static std::atomic<long long> g_launches{0};
+static std::atomic<long long> g_buffer_allocs{0};
 
 int set_error(int code, const char *fmt, ...) {
     char buf[1024];
@@ -222,6 +223,7 @@ int DevBuf::ensure(size_t bytes) {
         return set_error(SKB_ERR_ALLOC, "cudaMalloc(%zu) failed: %s", want, cudaGetErrorString(e));
     }
     cap = want;
+    g_buffer_allocs.fetch_add(1, std::memory_order_relaxed);
     return SKB_OK;
 }
 
@@ -427,6 +429,7 @@ extern "C" {
 const char *skb_version(void) { return "skelly_b200 0.1.0 (sm_90a)"; }
 const char *skb_last_error_string(void) { return last_error(); }
 int64_t skb_launch_count(void) { return launch_count(); }
+int64_t skb_buffer_alloc_count(void) { return g_buffer_allocs.load(std::memory_order_relaxed); }
 
 int skb_device_count(int *n) {
     if (!n)

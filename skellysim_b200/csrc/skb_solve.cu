@@ -292,8 +292,10 @@ int skb_flow_set_gmres(skb_flow *fl, int num_blocks) {
     std::array<long long, 6> key;
     SKB_TRY(flow_gmres_size(fl, who, &n, &key));
     SKB_TRY(flow_krylov(fl).setup(n, num_blocks, flow_num_sms(fl), key));
-    const FlowState s = flow_state(fl); // the buffers of skb_flow_step / skb_mflow_step beside the solve's
-    return s.buf->size(s.fibers.count(), s.fibers.nodes(), s.n_bodies);
+    // the buffers of skb_flow_step / skb_mflow_step / skb_flow_group_step_device beside the solve's
+    const FlowState s = flow_state(fl);
+    SKB_TRY(s.buf->size(s.fibers.count(), s.fibers.nodes(), s.n_bodies));
+    return flow_size_group_step(fl);
 }
 
 int skb_flow_solve_system(skb_flow *fl, skb_dense *dn, const double *rhs, double eta, double tol, int num_blocks,

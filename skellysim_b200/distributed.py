@@ -308,3 +308,108 @@ class RankSystemOperator:
                                                          max_iters=max_iters, stream=self._stream())
         self.launches = self.flow.stats()["launches"]
         return self.x[:self.n], dict(info, history=hist)
+
+
+class RankStepper:
+    """System::step on one rank per GPU: the twin of timestep.Stepper for a capi.Flow that is a connected group member,
+    with the same methods (positions, placement, step, backup, restore), so that timestep.run drives it unchanged.
+
+    flow: the member (target ranges = `partition`, connect_group, fiber classes, group_set_body_frames or
+    group_set_body_operators, a first group_place_bodies); dense: a capi.Dense on its device holding its row blocks of
+    both periphery operators (None without own periphery rows).  params (the seven of Flow.build_fiber_operators),
+    fiber_body, site_ref, v_growth and force_scale are given for ALL fibers, as to Stepper; the stepper keeps the own
+    fibers' slices.  step's f_external is of ALL fiber nodes too.  Every member holds the whole geometry, so positions()
+    and placement() are complete on every rank.  Every rank must make the same calls in the same order.
+
+    The device buffers the step reads and writes are allocated here, once: no step or restore allocates through torch's
+    allocator while a peer may wait on a flag (device: the flow's torch device).  After the step, x (the member's local rows of the solution,
+    system_rows order) and tension (its own fiber nodes) hold the step's outputs."""
+
+    def __init__(self, flow, dense, params, eta, partition, fiber_body=None, site_ref=None, v_growth=None,
+                 force_scale=None, tol=1e-10, num_blocks=300, max_iters=1000, body_n_nodes=None, device="cuda"):
+        import numpy as np
+        import torch
+        self.torch = torch
+        self.flow, self.dense, self.eta = flow, dense, float(eta)
+        self.tol, self.num_blocks, self.max_iters = tol, num_blocks, max_iters
+        off = np.asarray(flow._fiber_off, dtype=np.int64)
+        self.partition = tuple(int(v) for v in partition)
+        f0, f1 = self.partition[:2]
+        self.nodes = (int(off[f0]), int(off[f1]))  # the own fiber nodes [a, b)
+        own = lambda v: v[f0:f1] if np.ndim(v) else v
+        self.params = tuple(own(p) for p in params)
+        self.fiber_body = None if fiber_body is None else np.asarray(fiber_body, dtype=np.int32).reshape(-1)[f0:f1]
+        self.site_ref = None if site_ref is None else np.asarray(site_ref, dtype=np.float64).reshape(-1, 3)[f0:f1]
+        self.v_growth, self.force_scale = own(v_growth), own(force_scale)
+        body_n = getattr(flow, "_body_n", []) if body_n_nodes is None else body_n_nodes
+        self.local_rows = system_rows(self.partition, np.diff(off), getattr(flow, "n_shell", 0), body_n)
+        kw = dict(dtype=torch.float64, device=device)
+        nb, m = int(flow.n_bodies), self.nodes[1] - self.nodes[0]
+        self._fext = torch.zeros((max(m, 1), 3), **kw)
+        self._force = torch.zeros((max(nb, 1), 3), **kw)
+        self._torque = torch.zeros((max(nb, 1), 3), **kw)
+        self._x = torch.zeros(max(int(self.local_rows.size), 1), **kw)
+        self._tension = torch.zeros(max(m, 1), **kw)
+        self._backup = None
+
+    @property
+    def x(self):
+        return self._x[:self.local_rows.size]
+
+    @property
+    def tension(self):
+        return self._tension[:self.nodes[1] - self.nodes[0]]
+
+    def set_gmres(self, num_blocks=None):
+        """skb_flow_set_gmres on the member's local rows: sizes the solve's workspace and everything the step uses.  A
+        set-up call: every rank makes it before any rank's first step."""
+        self.flow.set_gmres(int(self.num_blocks if num_blocks is None else num_blocks))
+
+    def positions(self):
+        return self.flow.fibers()
+
+    def placement(self):
+        import numpy as np
+        if self.flow.n_bodies == 0:
+            return np.zeros((0, 3)), np.zeros((0, 4))
+        return self.flow.placement()
+
+    def _stream(self):
+        return self.torch.cuda.current_stream(self._x.device).cuda_stream if self._x.is_cuda else 0
+
+    def _upload(self, dst, host):
+        """host rows into the preallocated device buffer dst (no allocation on the device); returns its pointer"""
+        import numpy as np
+        if host is None or len(host) == 0:
+            return 0
+        dst[:len(host)].copy_(self.torch.from_numpy(np.ascontiguousarray(host, dtype=np.float64)))
+        return dst.data_ptr()
+
+    def step(self, dt, f_external=None, body_forces_torques=None):
+        """one System::step on every member alike; returns the step's info, the same on every member (a NaN
+        fiber_error: the solution was not finite and no member installed anything)"""
+        import numpy as np
+        a, b = self.nodes
+        fe = None if f_external is None else np.asarray(f_external, dtype=np.float64).reshape(-1, 3)[a:b]
+        ft = None if body_forces_torques is None else np.asarray(body_forces_torques, dtype=np.float64).reshape(-1, 6)
+        p_fe = self._upload(self._fext, fe)
+        p_f = self._upload(self._force, None if ft is None else ft[:, :3])
+        p_t = self._upload(self._torque, None if ft is None else ft[:, 3:])
+        return self.flow.group_step_device(*self.params, dt, self.eta, dense_matvec=self.dense, dense_minv=self.dense,
+                                           d_f_external=p_fe, d_body_forces=p_f, d_body_torques=p_t,
+                                           fiber_body=self.fiber_body, site_ref=self.site_ref,
+                                           v_growth=self.v_growth, force_scale=self.force_scale, tol=self.tol,
+                                           num_blocks=self.num_blocks, max_iters=self.max_iters,
+                                           d_x_local=self._x.data_ptr() if self.local_rows.size else 0,
+                                           d_tension=self._tension.data_ptr() if b > a else 0, stream=self._stream())
+
+    def backup(self):
+        self._backup = (self.positions(), *self.placement())
+
+    def restore(self):
+        """the backed-up geometry on this member: set_fibers and group_place_bodies, no group protocol"""
+        import numpy as np
+        r, c, q = self._backup
+        self.flow.set_fibers(r, np.diff(self.flow._fiber_off), self.flow._lengths)
+        if self.flow.n_bodies:
+            self.flow.group_place_bodies(c, q)
