@@ -760,13 +760,12 @@ SKB_API int skb_mflow_solve_system(skb_mflow *mf, const double *rhs, double eta,
 /* skb_flow_set_point_sources / _set_background on every device: skb_mflow_velocity_at_targets and
  * skb_mflow_build_system_rhs include them */
 /* skb_flow_step over n devices: the same arguments as complete host arrays of all fibers and bodies, the same refusals
- * (every member's before any member launches) and the same deviations.  The links, the build, the RHS and the solve are
- * the skb_mflow calls; each member then runs the fiber step kernel on its own fibers, reading its rows of the solution
- * on its device, and downloads their new positions into one host array; the bodies' step is done once on the host from
- * the complete solution; every member installs the same complete geometry and is placed at the same (c, q).
- * info->fiber_error is the max over all members' fibers.  skb_mflow_set_gmres sizes the step's buffers.  The RHS and
- * the solution cross the host once each, as skb_mflow_build_system_rhs and skb_mflow_solve_system take them.  With one
- * device it is bitwise skb_flow_step. */
+ * (every member's before any member launches) and the same deviations.  Every member runs skb_flow_group_step_device on
+ * its own slice of the arguments, on its own host thread: the inputs go up once (each member's own f_external, the
+ * complete body forces and torques), the body rows and the new fiber geometry are all-gathered through the members'
+ * group windows, and every member takes the same decision and installs the same complete geometry and placement.
+ * info->fiber_error is the max over all fibers.  x and tension come down once, each member's own rows.
+ * skb_mflow_set_gmres sizes the step's buffers.  With one device it is bitwise skb_flow_step. */
 SKB_API int skb_mflow_step(skb_mflow *mf, const skb_fiber_params *params, const double *v_growth,
                            const double *force_scale, const double *f_external, const double *body_forces_torques,
                            const int *fiber_body, const double *site_ref, double dt, double eta, double tol,

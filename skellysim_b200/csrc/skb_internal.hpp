@@ -13,6 +13,7 @@
 
 struct skb_fiber_params;
 struct skb_solve_info;
+struct skb_step_info;
 
 namespace skb {
 
@@ -169,7 +170,15 @@ struct OwnFibers {
 };
 
 struct FiberItem; // fiber_build.cuh
-struct StepItem;  // step_kernels.cuh
+// a fiber of the fiber step (step_kernels.cuh), as FiberOps::step_items fills it and the step places it
+struct StepItem {
+    long long node;  // first node of the fiber among the launch's nodes (positions 3 per node, solution 4 per node)
+    long long d1;    // element offset of its class's D_1_0 (n x n, column-major) in the class table
+    long long rng;   // offset of its class's D_1_0 column ranges (int2 per column) in the class ranges
+    double site[3];  // the lab-frame nucleation site a bound fiber is repinned to
+    int n;           // nodes
+    int bound;       // 1: repin to site
+};
 
 // A_, force_operator_, xs_ and A_^-1 of one set of own fibers, resident for the timestep, and the GEMVs over them.
 // The caller has checked its pointers for NULL and made the flow's device current.
@@ -589,7 +598,8 @@ int flow_size_overlap(skb_flow *fl, long long n_rows);
 
 // ---- and that the time step of a single-device flow needs (skb_step.cu) ----
 // the step's device buffers: per fiber its item and error, per fiber node its new position and tension, the external
-// forces and torques of the RHS; and a pinned host copy of a group step's device inputs (3 per fiber node + 6 per body)
+// forces and torques of the RHS; and a pinned host copy of skb_flow_group_step_device's device inputs (3 per fiber
+// node + 6 per body)
 // for their finiteness check.  Sized by skb_flow_set_gmres (the step itself allocates none of them)
 struct StepBuffers {
     DevBuf items, r_new, tension, err, fext, force, torque;
@@ -630,22 +640,45 @@ int flow_group_step_checks(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, 
                            long long *n, std::array<long long, 6> *key);
 // R (row-major) of a unit quaternion (w, x, y, z): the formula of Eigen's QuaternionBase::toRotationMatrix
 void quaternion_rotation(const double *q, double *R);
-// the pieces of the step shared by skb_flow_step and skb_mflow_step (skb_step.cu).  launch_fiber_step: fiber_step_kernel
-// over the fibers `own` of the flow of s on st (items from FiberOps::step_items; from_solution: d_in is their block of a
-// solution, 4 per own node, new positions and tensions to s.buf; else d_in holds positions), errors to s.buf->err
-int launch_fiber_step(const FlowState &s, const OwnFibers &own, const std::vector<StepItem> &items, const double *d_in,
-                      bool from_solution, cudaStream_t st);
-// BodyContainer::step of one body from its rows U, w (DESIGN.md §5: always translated, q normalised)
-void body_step(const double *c, const double *q, const double *U, const double *w, double dt, double *c_new,
-               double *q_new);
-// per fiber c + R(q) site_ref of its body (0 for a free fiber)
-void nucleation_sites(int n_fibers, const int *body, const double *site_ref, const double *centers,
-                      const double *orientations, std::vector<double> &sites);
-// uw = the rows [U; w] (6 per body) of the body part x_bodies of a solution, bodies of n_nodes nodes
-void body_rows(const int *n_nodes, int n_bodies, const double *x_bodies, std::vector<double> &uw);
-bool all_finite(const std::vector<double> &a);
-// the max of per-fiber errors and the first fiber attaining it (NaN wins; none: 0 and -1)
-void reduce_errors(const std::vector<double> &err, double *max_error, int *worst);
+// the refusals of a solve's tol, num_blocks and max_iters (each caller checks its own eta)
+int solve_scalar_args(const char *who, double tol, int num_blocks, int max_iters);
+// ---- the time step (skb_step.cu), which skb_mflow_step drives on every member ----
+// the per-fiber arguments of a step (of the fibers it steps: a group member's own) and its scalars
+struct StepArgs {
+    const ::skb_fiber_params *params;
+    const double *v_growth, *force_scale;
+    const int *fiber_body;
+    const double *site_ref;
+    double dt, eta, tol;
+    int num_blocks, max_iters;
+};
+// what a step's refusals leave for its run: the fibers it steps, their items, bending rigidity and current nucleation
+// sites, and the (local) solution size
+struct StepCall {
+    OwnFibers own;
+    std::vector<StepItem> items;
+    std::vector<double> rigidity, sites;
+    long long n = 0;
+};
+// the refusals of the step's host arguments: the scalars; params, fiber_body and site_ref of nf fibers (the first is
+// fiber f0) against nb bodies; the external forces of n_fib fiber nodes and the forces and torques of nb bodies finite
+int step_scalar_args(const char *who, const ::skb_step_info *info, double dt, double eta, double tol, int num_blocks,
+                     int max_iters);
+int step_fiber_args(const char *who, const ::skb_fiber_params *params, const int *fiber_body, const double *site_ref,
+                    int f0, int nf, int nb);
+int step_host_inputs(const char *who, const double *f_external, long long n_fib, const double *body_forces_torques,
+                     int nb);
+// skb_flow_group_step_device in two halves (on a flow that is no member, such as a one-device skb_mflow's, those of
+// skb_flow_step).  group_step_checks: every refusal except the device inputs' finiteness, before any launch, with the
+// arguments of the member's own fibers.  group_step_run: the step itself, which meets the member's peers at flag
+// waits -- every member's checks must have passed first.  Inputs on the device as the
+// public call takes them; x_local / tension (host or device memory, NULL: not wanted) receive the member's local rows
+// of the solution and its own fibers' tensions, also when the step is not installed (SKB_ERR_STATE)
+int group_step_checks(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const StepArgs &a, ::skb_step_info *info,
+                      const char *who, StepCall &c);
+int group_step_run(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const StepArgs &a, StepCall &c,
+                   const double *d_f_external, const double *d_body_forces, const double *d_body_torques,
+                   double *x_local, double *tension, ::skb_step_info *info, const char *who, cudaStream_t st);
 
 // The whole-vector operator on one member of skb_mflow (the members of a group, or the single flow of a one-device
 // skb_mflow), after its target ranges are set.  The arguments are those of skb_flow_set_body_operators /

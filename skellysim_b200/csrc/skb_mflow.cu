@@ -4,7 +4,6 @@
 // Every member is driven by its own host thread, so the n launch sequences are issued concurrently.  A client of the
 // skb_flow_* API plus the few internals declared in skb_internal.hpp.
 #include "skb_internal.hpp"
-#include "step_kernels.cuh"
 #include "../../include/skelly_b200_flow.h"
 #include "../../include/skelly_b200_dense.h"
 
@@ -12,7 +11,6 @@
 #include <cmath>
 #include <condition_variable>
 #include <functional>
-#include <limits>
 #include <memory>
 #include <mutex>
 #include <string>
@@ -999,12 +997,7 @@ int skb_mflow_solve_system(skb_mflow *mf, const double *rhs, double eta, double 
     SKB_TRY(mflow_system_args(mf, who, true, (rhs && x) || empty));
     if (!(eta > 0))
         return set_error(SKB_ERR_INVALID, "%s: eta = %g", who, eta);
-    if (!(tol > 0) || !std::isfinite(tol))
-        return set_error(SKB_ERR_INVALID, "%s: tol = %g (must be finite and > 0)", who, tol);
-    if (num_blocks < 1 || num_blocks > kMaxKrylov)
-        return set_error(SKB_ERR_INVALID, "%s: num_blocks = %d (must be in [1, %d])", who, num_blocks, kMaxKrylov);
-    if (max_iters < 0)
-        return set_error(SKB_ERR_INVALID, "%s: max_iters = %d", who, max_iters);
+    SKB_TRY(solve_scalar_args(who, tol, num_blocks, max_iters));
     if (!info)
         return set_error(SKB_ERR_INVALID, "%s: NULL info", who);
     if (empty) {
@@ -1058,161 +1051,91 @@ int skb_mflow_solve_system(skb_mflow *mf, const double *rhs, double eta, double 
     return mflow_collect_stats(mf);
 }
 
-// System::step over the devices (skb_flow_step's order): the links, the build, the RHS and the solve of the skb_mflow
-// calls, then on every member's thread fiber_step_kernel over its own fibers, reading its rows of the solution where the
-// solve left them on its device; the bodies' step once on the host; the same complete geometry installed on every member
+// System::step over the devices: skb_flow_group_step_device's run on every member's thread, after every member's
+// refusals on this one.  The members all-gather the body rows and the new fiber geometry through their group windows,
+// so every member takes the same decision and installs the same complete geometry
 int skb_mflow_step(skb_mflow *mf, const skb_fiber_params *params, const double *v_growth, const double *force_scale,
                    const double *f_external, const double *body_forces_torques, const int *fiber_body,
                    const double *site_ref, double dt, double eta, double tol, int num_blocks, int max_iters, double *x,
                    double *tension, skb_step_info *info) {
     const char *who = "skb_mflow_step";
-    // ---- every member's refusals, before any member launches ----
+    // ---- every member's refusals, before any member launches: a member that refused on its own thread would leave
+    // its peers waiting on a flag ----
     if (!mf)
         return set_error(SKB_ERR_INVALID, "%s: NULL", who);
-    if (!info)
-        return set_error(SKB_ERR_INVALID, "%s: NULL info", who);
-    if (!(dt > 0) || !std::isfinite(dt))
-        return set_error(SKB_ERR_INVALID, "%s: dt = %g (must be finite and > 0)", who, dt);
-    if (!(eta > 0) || !std::isfinite(eta))
-        return set_error(SKB_ERR_INVALID, "%s: eta = %g (must be finite and > 0)", who, eta);
-    if (!(tol > 0) || !std::isfinite(tol))
-        return set_error(SKB_ERR_INVALID, "%s: tol = %g (must be finite and > 0)", who, tol);
-    if (num_blocks < 1 || num_blocks > kMaxKrylov)
-        return set_error(SKB_ERR_INVALID, "%s: num_blocks = %d (must be in [1, %d])", who, num_blocks, kMaxKrylov);
-    if (max_iters < 0)
-        return set_error(SKB_ERR_INVALID, "%s: max_iters = %d", who, max_iters);
+    const int nb = mf->n_bodies;
+    SKB_TRY(step_scalar_args(who, info, dt, eta, tol, num_blocks, max_iters));
+    SKB_TRY(step_fiber_args(who, params, fiber_body, site_ref, 0, mf->n_fibers, nb));
+    SKB_TRY(step_host_inputs(who, f_external, mf->n_fib, body_forces_torques, nb));
     SKB_TRY(mflow_prepare(mf));
-    const int nf = mf->n_fibers, nb = mf->n_bodies;
-    const long long n_fib = mf->n_fib;
-    if (nf > 0 && !params)
-        return set_error(SKB_ERR_INVALID, "%s: NULL params", who);
-    bool any_bound = false;
-    for (int f = 0; f < nf; ++f) {
-        const int b = fiber_body ? fiber_body[f] : -1;
-        if (b < -1 || b >= nb)
-            return set_error(SKB_ERR_INVALID, "%s: fiber %d is bound to body %d (the flow has %d bodies; -1 = free)",
-                             who, f, b, nb);
-        any_bound = any_bound || b >= 0;
-    }
-    if (any_bound && !site_ref)
-        return set_error(SKB_ERR_INVALID, "%s: NULL site_ref with bound fibers", who);
-    for (long long i = 0; f_external && i < 3 * n_fib; ++i)
-        if (!std::isfinite(f_external[i]))
-            return set_error(SKB_ERR_INVALID, "%s: a non-finite external force", who);
-    for (int i = 0; body_forces_torques && i < 6 * nb; ++i)
-        if (!std::isfinite(body_forces_torques[i]))
-            return set_error(SKB_ERR_INVALID, "%s: a non-finite external body force or torque", who);
     if (mf->n_shell > 0 && (!mf->has_dense || !mf->has_minv))
         return set_error(SKB_ERR_INVALID, "%s: the periphery needs both dense operators (skb_mflow_set_dense)", who);
-    std::vector<FlowState> st_g((size_t)mf->n);
-    std::vector<OwnFibers> own((size_t)mf->n);
-    std::vector<std::vector<StepItem>> items((size_t)mf->n);
-    for (int g = 0; g < mf->n; ++g) {
-        skb_flow *fl = mf->m[(size_t)g].get();
-        CUDA_TRY(cudaSetDevice(mf->devs[(size_t)g]));
-        st_g[(size_t)g] = flow_state(fl);
-        const FlowState &s = st_g[(size_t)g];
-        own[(size_t)g] = s.fibers;
-        own[(size_t)g].f0 = mf->f0[(size_t)g];
-        own[(size_t)g].f1 = mf->f1[(size_t)g];
-        if (nb > 0 && (!s.placed || !s.bodies->has_frames() || !s.bodies->has_operators() || !s.bodies->has_inverse()))
-            return set_error(SKB_ERR_INVALID, "%s: the step places the bodies from their frames: call "
-                                              "skb_mflow_set_body_frames (with A_inv0) and a first skb_mflow_place_bodies",
-                             who);
-        SKB_TRY(flow_member_rhs_prepare(fl, params, v_growth, force_scale, dt, eta)); // the build's and RHS's refusals
-        SKB_TRY(s.ops->step_items(own[(size_t)g], items[(size_t)g]));
-    }
-    const FlowState &s0 = st_g[0];
-    std::vector<double> sites, rigidity((size_t)nf);
-    for (int f = 0; f < nf; ++f)
-        rigidity[(size_t)f] = params[f].bending_rigidity;
-    nucleation_sites(nf, fiber_body, site_ref, s0.centers, s0.orientations, sites);
-    SKB_TRY(flow_member_fiber_links(mf->m[0].get(), fiber_body, sites.data(), rigidity.data(), true));
-    const long long n = mflow_solution_size(mf);
-    std::memset(info, 0, sizeof(*info));
-    info->worst_fiber = -1;
-    if (n == 0) {
+    if (mflow_solution_size(mf) == 0) { // the empty system: nothing moves
+        std::memset(info, 0, sizeof(*info));
+        info->worst_fiber = -1;
         info->solve.converged = 1;
         return SKB_OK;
     }
     if (!mf->gmres_set || mf->gmres_layout != gmres_layout(mf))
         return set_error(SKB_ERR_INVALID, "%s: call skb_mflow_set_gmres after the partition or the bodies' node counts "
                                           "changed", who);
+    std::vector<StepArgs> args((size_t)mf->n);
+    std::vector<StepCall> calls((size_t)mf->n);
     for (int g = 0; g < mf->n; ++g) {
         skb_flow *fl = mf->m[(size_t)g].get();
-        long long nl = 0;
-        std::array<long long, 6> key;
-        SKB_TRY(flow_gmres_size(fl, who, &nl, &key));
-        if (!flow_krylov(fl).sized_for(nl, key) || num_blocks > flow_krylov(fl).blocks() ||
-            !st_g[(size_t)g].buf->sized_for(nf, n_fib, nb))
-            return set_error(SKB_ERR_INVALID, "%s: num_blocks = %d, skb_mflow_set_gmres sized device member %d for %d",
-                             who, num_blocks, g, flow_krylov(fl).blocks());
+        const int f0 = mf->f0[(size_t)g];
+        auto own = [&](auto *all, int k) { // the member's slice, k per fiber (NULL stays NULL, and so does no fiber's)
+            return all && mf->f1[(size_t)g] > f0 ? all + (size_t)k * f0 : nullptr;
+        };
+        args[(size_t)g] = StepArgs{own(params, 1), own(v_growth, 1), own(force_scale, 1), own(fiber_body, 1),
+                                   own(site_ref, 3), dt, eta, tol, num_blocks, max_iters};
+        skb_dense *dn = mf->dn[(size_t)g].get();
+        SKB_TRY(group_step_checks(fl, dn, dn, args[(size_t)g], info, who, calls[(size_t)g]));
+        // (also the RHS's buffers at their size and its tables uploaded, as every skb_mflow RHS does first)
+        SKB_TRY(flow_member_rhs_prepare(fl, params, v_growth, force_scale, dt, eta));
     }
+    std::vector<double> f, t;
+    if (body_forces_torques && nb > 0)
+        split_forces_torques(body_forces_torques, nb, f, t);
+    SKB_TRY(mflow_size_io(mf, f.size()));
 
-    // ---- the links, the operators, the RHS and the solve from the current placement ----
-    SKB_TRY(skb_mflow_set_fiber_links(mf, fiber_body, sites.data(), rigidity.data()));
-    SKB_TRY(skb_mflow_build_fiber_operators(mf, params, dt, eta));
-    std::vector<double> rhs((size_t)n), xs((size_t)n);
-    SKB_TRY(skb_mflow_build_system_rhs(mf, params, v_growth, force_scale, f_external, body_forces_torques, dt, eta,
-                                       rhs.data()));
-    SKB_TRY(skb_mflow_solve_system(mf, rhs.data(), eta, tol, num_blocks, max_iters, xs.data(), &info->solve, nullptr));
-
-    // ---- the bodies' step once, on the host, from the complete solution ----
-    std::vector<double> uw, c_new(3 * (size_t)nb), q_new(4 * (size_t)nb), sites_new;
-    const long long body0 = 4 * n_fib + 3 * mf->n_shell;
-    body_rows(mf->body_n.data(), nb, xs.data() + body0, uw);
-    for (int b = 0; b < nb; ++b)
-        body_step(s0.centers + 3 * (size_t)b, s0.orientations + 4 * (size_t)b, &uw[6 * (size_t)b],
-                  &uw[6 * (size_t)b + 3], dt, &c_new[3 * (size_t)b], &q_new[4 * (size_t)b]);
-    const bool bodies_finite = all_finite(uw);
-    if (bodies_finite)
-        nucleation_sites(nf, fiber_body, site_ref, c_new.data(), q_new.data(), sites_new);
-    else
-        sites_new.assign(3 * (size_t)nf, 0.0);
-
-    // ---- every member's own fibers on its device, from its rows of the solution; one download each ----
-    std::vector<double> r_new(3 * (size_t)n_fib), ten((size_t)n_fib), err((size_t)nf);
-    SKB_TRY(mf->workers->run([&](int g) -> int {
+    // ---- every member's step; its local rows of the solution and its own tensions into the complete host arrays ----
+    std::vector<skb_step_info> infos((size_t)mf->n);
+    const int rc = mf->workers->run([&](int g) -> int {
         skb_flow *fl = mf->m[(size_t)g].get();
+        skb_mflow::IO &io = mf->io[(size_t)g];
         CUDA_TRY(cudaSetDevice(mf->devs[(size_t)g]));
-        const OwnFibers &o = own[(size_t)g];
-        const FlowState &s = st_g[(size_t)g];
-        std::vector<StepItem> &it = items[(size_t)g];
-        for (int k = 0; k < o.count(); ++k) {
-            const int f = o.f0 + k;
-            it[(size_t)k].bound = fiber_body && fiber_body[f] >= 0;
-            std::memcpy(it[(size_t)k].site, &sites_new[3 * (size_t)f], sizeof(it[(size_t)k].site));
-        }
-        if (o.count() == 0)
-            return SKB_OK;
+        const MemberRows r = member_rows(mf, g);
         const cudaStream_t st = flow_stream(fl);
-        SKB_TRY(launch_fiber_step(s, o, it, flow_krylov(fl).stage_x(), true, st)); // the local vector starts with them
-        const long long a = o.off[o.f0], m = o.nodes();
-        CUDA_TRY(cudaMemcpyAsync(&r_new[3 * (size_t)a], s.buf->r_new.ptr, (size_t)m * 24, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaMemcpyAsync(&ten[(size_t)a], s.buf->tension.ptr, (size_t)m * 8, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaMemcpyAsync(&err[(size_t)o.f0], s.buf->err.ptr, (size_t)o.count() * 8, cudaMemcpyDeviceToHost,
-                                 st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-        return SKB_OK;
-    }));
-    if (x)
-        std::memcpy(x, xs.data(), (size_t)n * 8);
-    if (tension && n_fib > 0)
-        std::memcpy(tension, ten.data(), (size_t)n_fib * 8);
-    if (!bodies_finite || !all_finite(r_new)) {
-        info->fiber_error = std::numeric_limits<double>::quiet_NaN();
-        return set_error(SKB_ERR_STATE, "%s: the solution holds non-finite %s; the geometry is unchanged", who,
-                         bodies_finite ? "fiber positions" : "body velocities");
-    }
-    reduce_errors(err, &info->fiber_error, &info->worst_fiber);
-
-    // ---- the same complete geometry installed on every member ----
-    const std::vector<int> n_nodes(mf->fiber_n);
-    const std::vector<double> length(s0.length, s0.length + nf);
-    SKB_TRY(skb_mflow_set_fibers(mf, r_new.data(), n_nodes.data(), length.data(), nf));
-    if (nb > 0)
-        SKB_TRY(skb_mflow_place_bodies(mf, c_new.data(), q_new.data()));
-    return skb_mflow_set_fiber_links(mf, fiber_body, sites_new.data(), rigidity.data());
+        SKB_TRY(put(io.ff, f_external ? f_external + 3 * r.a : nullptr, (size_t)r.n_fw * 3, st));
+        SKB_TRY(put(io.f, f.data(), f.size(), st));
+        SKB_TRY(put(io.t, t.data(), t.size(), st));
+        std::vector<double> loc(x ? (size_t)calls[(size_t)g].n : 0);
+        skb_dense *dn = mf->dn[(size_t)g].get();
+        CUDA_TRY(cudaEventRecord(io.e0, st));
+        const int rc_g = group_step_run(fl, dn, dn, args[(size_t)g], calls[(size_t)g],
+                                        f_external ? (const double *)io.ff.ptr : nullptr,
+                                        f.empty() ? nullptr : (const double *)io.f.ptr,
+                                        t.empty() ? nullptr : (const double *)io.t.ptr, x ? loc.data() : nullptr,
+                                        tension ? tension + r.a : nullptr, &infos[(size_t)g], who, st);
+        if (rc_g != SKB_OK && rc_g != SKB_ERR_STATE) // (SKB_ERR_STATE: not installed, the outputs are there)
+            return rc_g;
+        CUDA_TRY(cudaEventRecord(io.e1, st));
+        if (x)
+            member_local(mf, g, [&](long long whole, long long at, long long len) {
+                std::memcpy(x + whole, loc.data() + at, (size_t)len * 8);
+            });
+        return rc_g;
+    });
+    mf->ops_ready = rc == SKB_ERR_STATE; // built by the step; an installed step set new fibers, which drops them
+    if (rc != SKB_OK && rc != SKB_ERR_STATE)
+        return rc;
+    for (int g = 1; g < mf->n; ++g) // the members decided from the same complete arrays
+        if (std::memcmp(&infos[(size_t)g], &infos[0], sizeof(skb_step_info)) != 0)
+            return set_error(SKB_ERR_STATE, "%s: device member %d ended its step unlike member 0", who, g);
+    *info = infos[0];
+    SKB_TRY(mflow_collect_stats(mf));
+    return rc; // (SKB_ERR_STATE keeps the message of the member that reported it)
 }
 
 // every member holds the same geometry: member 0's

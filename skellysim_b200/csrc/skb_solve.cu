@@ -215,6 +215,16 @@ int Krylov::solve(const Apply &A, const Apply &P_inv, const Reduce &reduce, cons
     return SKB_OK;
 }
 
+int skb::solve_scalar_args(const char *who, double tol, int num_blocks, int max_iters) {
+    if (!(tol > 0) || !std::isfinite(tol))
+        return set_error(SKB_ERR_INVALID, "%s: tol = %g (must be finite and > 0)", who, tol);
+    if (num_blocks < 1 || num_blocks > kMaxKrylov)
+        return set_error(SKB_ERR_INVALID, "%s: num_blocks = %d (must be in [1, %d])", who, num_blocks, kMaxKrylov);
+    if (max_iters < 0)
+        return set_error(SKB_ERR_INVALID, "%s: max_iters = %d", who, max_iters);
+    return SKB_OK;
+}
+
 // the refusals of every form, before any launch; *n = the (local) solution size, 0 with an empty system: nothing to
 // do (info filled).  group: the local-vector call of a group member (dn_spc / dn_minv its rows of the two operators)
 static int solve_args(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const char *who, bool group, double eta,
@@ -228,12 +238,7 @@ static int solve_args(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const
     SKB_TRY(flow_solve_args(fl, dn_spc, dn_minv, who, n, &key));
     if (!(eta > 0))
         return set_error(SKB_ERR_INVALID, "%s: eta = %g", who, eta);
-    if (!(tol > 0) || !std::isfinite(tol))
-        return set_error(SKB_ERR_INVALID, "%s: tol = %g (must be finite and > 0)", who, tol);
-    if (num_blocks < 1 || num_blocks > kMaxKrylov)
-        return set_error(SKB_ERR_INVALID, "%s: num_blocks = %d (must be in [1, %d])", who, num_blocks, kMaxKrylov);
-    if (max_iters < 0)
-        return set_error(SKB_ERR_INVALID, "%s: max_iters = %d", who, max_iters);
+    SKB_TRY(solve_scalar_args(who, tol, num_blocks, max_iters));
     if (!info)
         return set_error(SKB_ERR_INVALID, "%s: NULL info", who);
     if (flow_whole_size(fl) == 0) { // every member of an empty system returns here alike

@@ -1,7 +1,7 @@
 // skb_step.cu -- System::step (system.cpp:482-492) of a single-device flow (include/skelly_b200_flow.h, skb_flow_step)
-// and of a rank-per-GPU group member (skb_flow_group_step_device): the links, the fiber operators, the RHS and the
-// solve of the existing calls, then the fiber step kernel (step_kernels.cuh), the bodies' step on the host and the
-// installation of the new geometry.
+// and of a rank-per-GPU group member (skb_flow_group_step_device, which skb_mflow_step runs on every member): the
+// links, the fiber operators, the RHS and the solve of the existing calls, then the fiber step kernel
+// (step_kernels.cuh), the bodies' step on the host and the installation of the new geometry.
 #include "step_kernels.cuh"
 #include "skb_internal.hpp"
 #include "../../include/skelly_b200_flow.h"
@@ -49,8 +49,11 @@ int StepBuffers::size(int n_fibers, long long n_fib, int n_bodies) {
     return SKB_OK;
 }
 
-int skb::launch_fiber_step(const FlowState &s, const OwnFibers &own, const std::vector<StepItem> &items,
-                           const double *d_in, bool from_solution, cudaStream_t st) {
+// fiber_step_kernel over the fibers `own` of the flow of s on st (items from FiberOps::step_items; from_solution: d_in is
+// their block of a solution, 4 per own node, new positions and tensions to s.buf; else d_in holds positions), errors to
+// s.buf->err
+static int launch_fiber_step(const FlowState &s, const OwnFibers &own, const std::vector<StepItem> &items,
+                             const double *d_in, bool from_solution, cudaStream_t st) {
     const int nf = own.count();
     if (nf == 0)
         return SKB_OK;
@@ -74,8 +77,8 @@ int skb::launch_fiber_step(const FlowState &s, const OwnFibers &own, const std::
 // BodyContainer::step / SphericalBody::step (body_container.cpp:48-61, body_spherical.cpp:13-35) of one body from its
 // rows U, w, with two deviations (DESIGN.md §5): the body always moves to c + dt U, and the new quaternion is
 // normalised.  phi = dt w; |phi| > 0: q_new = (cos |phi|/2, sin(|phi|/2) phi / |phi|) * q in Eigen's product order
-void skb::body_step(const double *c, const double *q, const double *U, const double *w, double dt, double *c_new,
-               double *q_new) {
+static void body_step(const double *c, const double *q, const double *U, const double *w, double dt, double *c_new,
+                      double *q_new) {
     for (int k = 0; k < 3; ++k)
         c_new[k] = c[k] + U[k] * dt;
     const double phi[3] = {w[0] * dt, w[1] * dt, w[2] * dt};
@@ -95,8 +98,8 @@ void skb::body_step(const double *c, const double *q, const double *U, const dou
 
 // the lab-frame nucleation site of every bound fiber (get_nucleation_site): c + R site_ref, R of the body's quaternion;
 // 0 for a free fiber
-void skb::nucleation_sites(int n_fibers, const int *body, const double *site_ref, const double *centers,
-                      const double *orientations, std::vector<double> &sites) {
+static void nucleation_sites(int n_fibers, const int *body, const double *site_ref, const double *centers,
+                             const double *orientations, std::vector<double> &sites) {
     sites.assign(3 * (size_t)n_fibers, 0.0);
     for (int f = 0; f < n_fibers; ++f) {
         const int b = body ? body[f] : -1;
@@ -110,17 +113,7 @@ void skb::nucleation_sites(int n_fibers, const int *body, const double *site_ref
     }
 }
 
-void skb::body_rows(const int *n_nodes, int n_bodies, const double *x_bodies, std::vector<double> &uw) {
-    uw.resize(6 * (size_t)n_bodies);
-    long long off = 0;
-    for (int b = 0; b < n_bodies; ++b) {
-        off += 3LL * n_nodes[b];
-        std::memcpy(&uw[6 * (size_t)b], x_bodies + off, 48);
-        off += 6;
-    }
-}
-
-bool skb::all_finite(const std::vector<double> &a) {
+static bool all_finite(const std::vector<double> &a) {
     for (double v : a)
         if (!std::isfinite(v))
             return false;
@@ -128,7 +121,7 @@ bool skb::all_finite(const std::vector<double> &a) {
 }
 
 // the flow's fiber error from the per-fiber maxima: their max and the first fiber attaining it (NaN wins)
-void skb::reduce_errors(const std::vector<double> &err, double *max_error, int *worst) {
+static void reduce_errors(const std::vector<double> &err, double *max_error, int *worst) {
     *max_error = 0.0;
     *worst = -1;
     for (size_t f = 0; f < err.size(); ++f)
@@ -138,21 +131,323 @@ void skb::reduce_errors(const std::vector<double> &err, double *max_error, int *
         }
 }
 
-// the refusals of the step's scalar arguments, shared by skb_flow_step and skb_flow_group_step_device
-static int step_scalar_args(const char *who, const skb_step_info *info, double dt, double eta, double tol,
-                            int num_blocks, int max_iters) {
+// ---- the refusals ----------------------------------------------------------------------------------------------------
+int skb::step_scalar_args(const char *who, const skb_step_info *info, double dt, double eta, double tol,
+                          int num_blocks, int max_iters) {
     if (!info)
         return set_error(SKB_ERR_INVALID, "%s: NULL info", who);
     if (!(dt > 0) || !std::isfinite(dt))
         return set_error(SKB_ERR_INVALID, "%s: dt = %g (must be finite and > 0)", who, dt);
     if (!(eta > 0) || !std::isfinite(eta))
         return set_error(SKB_ERR_INVALID, "%s: eta = %g (must be finite and > 0)", who, eta);
-    if (!(tol > 0) || !std::isfinite(tol))
-        return set_error(SKB_ERR_INVALID, "%s: tol = %g (must be finite and > 0)", who, tol);
-    if (num_blocks < 1 || num_blocks > kMaxKrylov)
-        return set_error(SKB_ERR_INVALID, "%s: num_blocks = %d (must be in [1, %d])", who, num_blocks, kMaxKrylov);
-    if (max_iters < 0)
-        return set_error(SKB_ERR_INVALID, "%s: max_iters = %d", who, max_iters);
+    return solve_scalar_args(who, tol, num_blocks, max_iters);
+}
+
+int skb::step_fiber_args(const char *who, const skb_fiber_params *params, const int *fiber_body,
+                         const double *site_ref, int f0, int nf, int nb) {
+    if (nf > 0 && !params)
+        return set_error(SKB_ERR_INVALID, "%s: NULL params", who);
+    bool any_bound = false;
+    for (int f = 0; f < nf; ++f) {
+        const int b = fiber_body ? fiber_body[f] : -1;
+        if (b < -1 || b >= nb)
+            return set_error(SKB_ERR_INVALID, "%s: fiber %d is bound to body %d (the flow has %d bodies; -1 = free)",
+                             who, f0 + f, b, nb);
+        any_bound = any_bound || b >= 0;
+    }
+    if (any_bound && !site_ref)
+        return set_error(SKB_ERR_INVALID, "%s: NULL site_ref with bound fibers", who);
+    return SKB_OK;
+}
+
+int skb::step_host_inputs(const char *who, const double *f_external, long long n_fib,
+                          const double *body_forces_torques, int nb) {
+    for (long long i = 0; f_external && i < 3 * n_fib; ++i)
+        if (!std::isfinite(f_external[i]))
+            return set_error(SKB_ERR_INVALID, "%s: a non-finite external force", who);
+    for (int i = 0; body_forces_torques && i < 6 * nb; ++i)
+        if (!std::isfinite(body_forces_torques[i]))
+            return set_error(SKB_ERR_INVALID, "%s: a non-finite external body force or torque", who);
+    return SKB_OK;
+}
+
+// step_host_inputs for device inputs: the external forces of m fiber nodes and the forces and torques of the flow's
+// bodies, read back into the pinned copy skb_flow_set_gmres sized (24 B per fiber node, 48 B per body) and scanned
+// there.  Copies, not launches, so a refusal still comes before any launch
+static int step_device_inputs(const char *who, const FlowState &s, const double *d_f_external, long long m,
+                              const double *d_body_forces, const double *d_body_torques, cudaStream_t st) {
+    const size_t nb3 = s.n_bodies > 0 ? 3 * (size_t)s.n_bodies : 0;
+    const double *d[3] = {d_f_external, d_body_forces, d_body_torques};
+    const size_t count[3] = {3 * (size_t)m, nb3, nb3};
+    double *h = s.buf->check.get();
+    bool finite[3] = {true, true, true};
+    for (int k = 0; k < 3; ++k) {
+        if (!d[k] || count[k] == 0)
+            continue;
+        CUDA_TRY(cudaMemcpyAsync(h, d[k], count[k] * 8, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        for (size_t i = 0; i < count[k] && finite[k]; ++i)
+            finite[k] = std::isfinite(h[i]);
+    }
+    if (!finite[0])
+        return set_error(SKB_ERR_INVALID, "%s: a non-finite external force", who);
+    if (!finite[1] || !finite[2])
+        return set_error(SKB_ERR_INVALID, "%s: a non-finite external body force or torque", who);
+    return SKB_OK;
+}
+
+// the refusals that concern the fibers the step advances (c.own): their arguments, their links at the current placement
+// and their classes; c is left with their rigidity, current nucleation sites and items
+static int own_fiber_checks(skb_flow *fl, const FlowState &s, const StepArgs &a, const char *who, StepCall &c) {
+    const int nf = c.own.count();
+    SKB_TRY(step_fiber_args(who, a.params, a.fiber_body, a.site_ref, c.own.f0, nf, s.n_bodies));
+    c.rigidity.resize((size_t)nf);
+    for (int f = 0; f < nf; ++f)
+        c.rigidity[(size_t)f] = a.params[f].bending_rigidity;
+    nucleation_sites(nf, a.fiber_body, a.site_ref, s.centers, s.orientations, c.sites);
+    SKB_TRY(s.bodies->set_links(c.own, *s.ops, s.n_bodies, s.centers, a.fiber_body, c.sites.data(),
+                                c.rigidity.data(), flow_stream(fl), true));
+    SKB_TRY(s.ops->check_step(c.own, a.params, a.v_growth, a.force_scale));
+    return s.ops->step_items(c.own, c.items);
+}
+
+// every refusal of skb_flow_step but its inputs' finiteness (they are on the host or on the device)
+static int step_checks(skb_flow *fl, skb_dense *dn, const StepArgs &a, skb_step_info *info, const char *who,
+                       StepCall &c) {
+    SKB_TRY(step_scalar_args(who, info, a.dt, a.eta, a.tol, a.num_blocks, a.max_iters));
+    SKB_TRY(flow_step_checks(fl, dn, who));
+    const FlowState s = flow_state(fl);
+    c.own = s.fibers;
+    SKB_TRY(own_fiber_checks(fl, s, a, who, c));
+    std::array<long long, 6> key;
+    SKB_TRY(flow_gmres_size(fl, who, &c.n, &key));
+    Krylov &kry = flow_krylov(fl);
+    if (c.n > 0 && (!kry.sized_for(c.n, key) || !s.buf->sized_for(s.fibers.count(), s.fibers.nodes(), s.n_bodies)))
+        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_gmres for the current solution size (%lld)", who, c.n);
+    if (c.n > 0 && a.num_blocks > kry.blocks())
+        return set_error(SKB_ERR_INVALID, "%s: num_blocks = %d, skb_flow_set_gmres sized the workspace for %d", who,
+                         a.num_blocks, kry.blocks());
+    return SKB_OK;
+}
+
+int skb::group_step_checks(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const StepArgs &a,
+                           skb_step_info *info, const char *who, StepCall &c) {
+    if (!flow_group(fl).member())
+        return step_checks(fl, dn_spc, a, info, who, c);
+    SKB_TRY(step_scalar_args(who, info, a.dt, a.eta, a.tol, a.num_blocks, a.max_iters));
+    std::array<long long, 6> key;
+    SKB_TRY(flow_group_step_checks(fl, dn_spc, dn_minv, who, c.own, &c.n, &key));
+    const FlowState s = flow_state(fl);
+    SKB_TRY(own_fiber_checks(fl, s, a, who, c));
+    Krylov &kry = flow_krylov(fl);
+    if (!kry.sized_for(c.n, key) || !s.buf->sized_for(s.fibers.count(), s.fibers.nodes(), s.n_bodies))
+        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_gmres for the member's current target ranges", who);
+    if (!s.ops->build_sized_for(c.own)) // (the build's buffers are sized only once every class it needs is set)
+        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_gmres after the fiber classes and their derivatives "
+                                          "are set (it sizes the fiber build's buffers)", who);
+    if (a.num_blocks > kry.blocks())
+        return set_error(SKB_ERR_INVALID, "%s: num_blocks = %d, skb_flow_set_gmres sized the workspace for %d", who,
+                         a.num_blocks, kry.blocks());
+    return SKB_OK;
+}
+
+// ---- the pieces both runs share --------------------------------------------------------------------------------------
+// uw = the rows [U; w] of every body (6 per body) from the body part of a solution on the device, 48 bytes per body
+static int body_rows(const FlowState &s, const double *d_x_bodies, std::vector<double> &uw, cudaStream_t st) {
+    uw.resize(6 * (size_t)s.n_bodies);
+    if (s.n_bodies == 0)
+        return SKB_OK;
+    const int *nodes = s.bodies->frame_node_counts();
+    long long off = 0;
+    for (int b = 0; b < s.n_bodies; ++b) {
+        off += 3LL * nodes[b];
+        CUDA_TRY(cudaMemcpyAsync(&uw[6 * (size_t)b], d_x_bodies + off, 48, cudaMemcpyDeviceToHost, st));
+        off += 6;
+    }
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return SKB_OK;
+}
+
+// the bodies' step from their rows uw, the new nucleation sites of the step's fibers (0 where a row is not finite: such
+// a step is not installed) and their items' repin at them; false: a row is not finite
+static bool advance_bodies(const FlowState &s, const StepArgs &a, const std::vector<double> &uw, StepCall &c,
+                           std::vector<double> &c_new, std::vector<double> &q_new, std::vector<double> &sites_new) {
+    c_new.resize(3 * (size_t)s.n_bodies);
+    q_new.resize(4 * (size_t)s.n_bodies);
+    for (int b = 0; b < s.n_bodies; ++b)
+        body_step(s.centers + 3 * (size_t)b, s.orientations + 4 * (size_t)b, &uw[6 * (size_t)b],
+                  &uw[6 * (size_t)b + 3], a.dt, &c_new[3 * (size_t)b], &q_new[4 * (size_t)b]);
+    const bool finite = all_finite(uw);
+    if (finite)
+        nucleation_sites(c.own.count(), a.fiber_body, a.site_ref, c_new.data(), q_new.data(), sites_new);
+    else
+        sites_new.assign(3 * (size_t)c.own.count(), 0.0);
+    for (size_t f = 0; f < c.items.size(); ++f) {
+        c.items[f].bound = a.fiber_body && a.fiber_body[f] >= 0;
+        std::memcpy(c.items[f].site, &sites_new[3 * f], sizeof(c.items[f].site));
+    }
+    return finite;
+}
+
+// one decision from the complete new positions and the bodies' rows: a non-finite solution is installed nowhere (the
+// caller's restore has nothing to undo); else the fiber error
+static int decide(const char *who, bool bodies_finite, const std::vector<double> &r_new,
+                  const std::vector<double> &err, skb_step_info *info) {
+    if (!bodies_finite || !all_finite(r_new)) {
+        info->fiber_error = std::numeric_limits<double>::quiet_NaN();
+        return set_error(SKB_ERR_STATE, "%s: the solution holds non-finite %s; the geometry is unchanged", who,
+                         bodies_finite ? "fiber positions" : "body velocities");
+    }
+    reduce_errors(err, &info->fiber_error, &info->worst_fiber);
+    return SKB_OK;
+}
+
+// ---- the two runs ----------------------------------------------------------------------------------------------------
+// System::step of a single-device flow whose refusals have passed, on the flow's stream: d_f_external 3 per fiber node,
+// d_body_forces / d_body_torques 3 per body (NULL: none); x / tension host or device memory (NULL: not wanted)
+static int step_run(skb_flow *fl, skb_dense *dn, const StepArgs &a, StepCall &c, const double *d_f_external,
+                    const double *d_body_forces, const double *d_body_torques, double *x, double *tension,
+                    skb_step_info *info, const char *who) {
+    std::memset(info, 0, sizeof(*info));
+    info->worst_fiber = -1;
+    if (c.n == 0) { // the empty system: nothing moves
+        info->solve.converged = 1;
+        return SKB_OK;
+    }
+
+    // ---- System::step: the links, the operators, the RHS and the solve from the current placement ----
+    const FlowState s = flow_state(fl);
+    const int nf = s.fibers.count(), nb = s.n_bodies;
+    const long long n_fib = s.fibers.nodes();
+    const cudaStream_t st = flow_stream(fl);
+    Krylov &kry = flow_krylov(fl);
+    SKB_TRY(skb_flow_set_fiber_links(fl, a.fiber_body, c.sites.data(), c.rigidity.data()));
+    SKB_TRY(skb_flow_build_fiber_operators(fl, a.params, a.dt, a.eta));
+    SKB_TRY(skb_flow_build_system_rhs_device(fl, a.params, a.v_growth, a.force_scale,
+                                             n_fib > 0 ? d_f_external : nullptr, nb > 0 ? d_body_forces : nullptr,
+                                             nb > 0 ? d_body_torques : nullptr, a.dt, a.eta, kry.stage_b(), st));
+    SKB_TRY(skb_flow_solve_system_device(fl, dn, kry.stage_b(), a.eta, a.tol, a.num_blocks, a.max_iters,
+                                         kry.stage_x(), &info->solve, nullptr, st));
+    const double *d_x = kry.stage_x();
+
+    // ---- the bodies' step from their rows [U; w], on the host ----
+    std::vector<double> uw, c_new, q_new, sites_new;
+    SKB_TRY(body_rows(s, d_x + 4 * n_fib + 3 * s.n_shell, uw, st));
+    const bool bodies_finite = advance_bodies(s, a, uw, c, c_new, q_new, sites_new);
+
+    // ---- the fibers' step, repin and error on the device; one download of the new positions ----
+    SKB_TRY(launch_fiber_step(s, s.fibers, c.items, d_x, true, st));
+    const StepBuffers &buf = *s.buf;
+    std::vector<double> r_new(3 * (size_t)n_fib), err((size_t)nf);
+    if (nf > 0) {
+        CUDA_TRY(cudaMemcpyAsync(r_new.data(), buf.r_new.ptr, r_new.size() * 8, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(err.data(), buf.err.ptr, err.size() * 8, cudaMemcpyDeviceToHost, st));
+        if (tension)
+            CUDA_TRY(cudaMemcpyAsync(tension, buf.tension.ptr, (size_t)n_fib * 8, cudaMemcpyDefault, st));
+    }
+    if (x)
+        CUDA_TRY(cudaMemcpyAsync(x, d_x, (size_t)c.n * 8, cudaMemcpyDefault, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    SKB_TRY(decide(who, bodies_finite, r_new, err, info));
+
+    // ---- install: the new positions through skb_flow_set_fibers (same node counts and lengths, so the partition and
+    // the class table stay), the placement, the links at the new sites ----
+    const std::vector<int> n_nodes(s.fibers.n, s.fibers.n + nf);
+    const std::vector<double> length(s.length, s.length + nf);
+    // (every argument below has passed its call's checks already: only a CUDA error can stop the install half-way)
+    SKB_TRY(skb_flow_set_fibers(fl, r_new.data(), n_nodes.data(), length.data(), nf));
+    if (nb > 0)
+        SKB_TRY(skb_flow_place_bodies(fl, c_new.data(), q_new.data()));
+    return skb_flow_set_fiber_links(fl, a.fiber_body, sites_new.data(), c.rigidity.data());
+}
+
+// System::step on one rank per GPU: the composed local-vector calls, then two epochs of the group's own protocol --
+// the body rows all-gathered through x_body, the fiber step fused with the all-gather of its results through r_step --
+// and the same decision and the same complete geometry on every member
+int skb::group_step_run(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const StepArgs &a, StepCall &c,
+                        const double *d_f_external, const double *d_body_forces, const double *d_body_torques,
+                        double *x_local, double *tension, skb_step_info *info, const char *who, cudaStream_t st) {
+    if (!flow_group(fl).member()) { // skb_flow_step's run, on the flow's stream once the caller's work on st is done
+        CUDA_TRY(cudaStreamSynchronize(st));
+        return step_run(fl, dn_spc, a, c, d_f_external, d_body_forces, d_body_torques, x_local, tension, info, who);
+    }
+    std::memset(info, 0, sizeof(*info));
+    info->worst_fiber = -1;
+    if (flow_whole_size(fl) == 0) { // the empty system, on every member alike: nothing moves
+        info->solve.converged = 1;
+        return SKB_OK;
+    }
+
+    // ---- System::step: the links, the operators (on the flow's stream, drained), the RHS and the solve on st ----
+    const FlowState s = flow_state(fl);
+    Group &G = flow_group(fl);
+    Krylov &kry = flow_krylov(fl);
+    const StepBuffers &buf = *s.buf;
+    const int nf = s.fibers.count(), nfo = c.own.count(), nb = s.n_bodies;
+    const long long n_fib = s.fibers.nodes(), m = c.own.nodes();
+    SKB_TRY(skb_flow_group_set_fiber_links(fl, a.fiber_body, c.sites.data(), c.rigidity.data()));
+    SKB_TRY(skb_flow_build_fiber_operators(fl, a.params, a.dt, a.eta));
+    CUDA_TRY(cudaStreamSynchronize(flow_stream(fl)));
+    SKB_TRY(skb_flow_group_build_system_rhs_device(fl, a.params, a.v_growth, a.force_scale, d_f_external,
+                                                   d_body_forces, d_body_torques, a.dt, a.eta, kry.stage_b(), st));
+    SKB_TRY(skb_flow_group_solve_system_device(fl, dn_spc, dn_minv, kry.stage_b(), a.eta, a.tol, a.num_blocks,
+                                               a.max_iters, kry.stage_x(), &info->solve, nullptr, st));
+    const double *d_x = kry.stage_x(); // [4 per own fiber node | 3 per own periphery row | own body rows]
+    int *launches = flow_launches(fl); // the protocol's launches join the flow's count, as in the other member calls
+
+    // ---- the body rows all-gathered (an epoch of its own: the rows phase), [U; w] of every body from the own window,
+    // the bodies' step on the host: every member from the same bits ----
+    std::vector<double> uw, c_new, q_new, sites_new;
+    if (nb > 0) {
+        SKB_TRY(G.begin());
+        SKB_TRY(G.store_rows(d_x + c.n - G.body_rows(), nullptr, 0, 0, flow_num_sms(fl), st, launches));
+        SKB_TRY(G.rows_barrier(true, true, st, launches));
+        SKB_TRY(body_rows(s, G.x_body(), uw, st));
+    }
+    const bool bodies_finite = advance_bodies(s, a, uw, c, c_new, q_new, sites_new);
+
+    // ---- the own fibers' step, repin and error fused with the all-gather of the results into r_step of every window
+    // (an epoch of its own, the rows phase again), then the complete positions and errors from the own window ----
+    std::vector<double> r_new(3 * (size_t)n_fib), err((size_t)nf);
+    if (nf > 0) {
+        SKB_TRY(G.begin());
+        if (nfo > 0) {
+            CUDA_TRY(cudaMemcpyAsync(buf.items.ptr, c.items.data(), (size_t)nfo * sizeof(StepItem),
+                                     cudaMemcpyHostToDevice, st));
+            StepGather g;
+            g.size = G.step_windows(g.r_step);
+            g.n_fib = n_fib;
+            g.node0 = c.own.off[c.own.f0];
+            g.fiber0 = c.own.f0;
+            group_fiber_step_kernel<<<nfo, kStepThreads, 0, st>>>((const StepItem *)buf.items.ptr, d_x,
+                                                                  s.ops->class_table(), s.ops->class_range_table(),
+                                                                  c.own.length + c.own.f0, (double *)buf.tension.ptr,
+                                                                  g);
+            CUDA_TRY(cudaGetLastError());
+            count_launch(1);
+            *launches += 1;
+        }
+        SKB_TRY(G.rows_barrier(true, true, st, launches));
+        CUDA_TRY(cudaMemcpyAsync(r_new.data(), G.r_step(), r_new.size() * 8, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(err.data(), G.r_step() + 3 * n_fib, err.size() * 8, cudaMemcpyDeviceToHost, st));
+        if (tension && m > 0)
+            CUDA_TRY(cudaMemcpyAsync(tension, buf.tension.ptr, (size_t)m * 8, cudaMemcpyDefault, st));
+    }
+    if (x_local && c.n > 0)
+        CUDA_TRY(cudaMemcpyAsync(x_local, d_x, (size_t)c.n * 8, cudaMemcpyDefault, st));
+    CUDA_TRY(cudaStreamSynchronize(st)); // the downloads land before this member's next signal
+
+    // ---- one decision, from the complete arrays every member holds alike ----
+    SKB_TRY(decide(who, bodies_finite, r_new, err, info));
+
+    // ---- install the complete geometry (same counts: the window, the partition and every buffer stay) ----
+    const std::vector<int> n_nodes(s.fibers.n, s.fibers.n + nf);
+    const std::vector<double> length(s.length, s.length + nf);
+    SKB_TRY(skb_flow_set_fibers(fl, r_new.data(), n_nodes.data(), length.data(), nf));
+    if (nb > 0)
+        SKB_TRY(skb_flow_group_place_bodies(fl, c_new.data(), q_new.data()));
+    SKB_TRY(skb_flow_group_set_fiber_links(fl, a.fiber_body, sites_new.data(), c.rigidity.data()));
+    CUDA_TRY(cudaStreamSynchronize(flow_stream(fl)));
     return SKB_OK;
 }
 
@@ -163,191 +458,32 @@ int skb_flow_step(skb_flow *fl, skb_dense *dn, const skb_fiber_params *params, c
                   const int *fiber_body, const double *site_ref, double dt, double eta, double tol, int num_blocks,
                   int max_iters, double *x, double *tension, skb_step_info *info) {
     const char *who = "skb_flow_step";
-    // ---- every refusal, before any launch ----
     if (!fl)
         return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    SKB_TRY(step_scalar_args(who, info, dt, eta, tol, num_blocks, max_iters));
-    SKB_TRY(flow_step_checks(fl, dn, who));
-    const FlowState s = flow_state(fl);
-    const int nf = s.fibers.count(), nb = s.n_bodies;
-    const long long n_fib = s.fibers.nodes();
-    if (nf > 0 && !params)
-        return set_error(SKB_ERR_INVALID, "%s: NULL params", who);
-    bool any_bound = false;
-    for (int f = 0; f < nf; ++f) {
-        const int b = fiber_body ? fiber_body[f] : -1;
-        if (b < -1 || b >= nb)
-            return set_error(SKB_ERR_INVALID, "%s: fiber %d is bound to body %d (the flow has %d bodies; -1 = free)",
-                             who, f, b, nb);
-        any_bound = any_bound || b >= 0;
-    }
-    if (any_bound && !site_ref)
-        return set_error(SKB_ERR_INVALID, "%s: NULL site_ref with bound fibers", who);
-    std::vector<double> sites, rigidity((size_t)nf);
-    for (int f = 0; f < nf; ++f)
-        rigidity[(size_t)f] = params[f].bending_rigidity;
-    nucleation_sites(nf, fiber_body, site_ref, s.centers, s.orientations, sites);
-    const cudaStream_t st = flow_stream(fl);
-    SKB_TRY(s.bodies->set_links(s.fibers, *s.ops, nb, s.centers, fiber_body, sites.data(), rigidity.data(), st, true));
-    SKB_TRY(s.ops->check_step(s.fibers, params, v_growth, force_scale));
-    std::vector<StepItem> items;
-    SKB_TRY(s.ops->step_items(s.fibers, items));
-    for (long long i = 0; f_external && i < 3 * n_fib; ++i)
-        if (!std::isfinite(f_external[i]))
-            return set_error(SKB_ERR_INVALID, "%s: a non-finite external force", who);
-    for (int i = 0; body_forces_torques && i < 6 * nb; ++i)
-        if (!std::isfinite(body_forces_torques[i]))
-            return set_error(SKB_ERR_INVALID, "%s: a non-finite external body force or torque", who);
-    long long n = 0;
-    std::array<long long, 6> key;
-    SKB_TRY(flow_gmres_size(fl, who, &n, &key));
-    Krylov &kry = flow_krylov(fl);
-    if (n > 0 && (!kry.sized_for(n, key) || !s.buf->sized_for(nf, n_fib, nb)))
-        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_gmres for the current solution size (%lld)", who, n);
-    if (n > 0 && num_blocks > kry.blocks())
-        return set_error(SKB_ERR_INVALID, "%s: num_blocks = %d, skb_flow_set_gmres sized the workspace for %d", who,
-                         num_blocks, kry.blocks());
-    std::memset(info, 0, sizeof(*info));
-    info->worst_fiber = -1;
-    if (n == 0) { // the empty system: nothing moves
-        info->solve.converged = 1;
-        return SKB_OK;
-    }
-
-    // ---- System::step: the links, the operators, the RHS and the solve from the current placement ----
-    StepBuffers &buf = *s.buf;
-    SKB_TRY(skb_flow_set_fiber_links(fl, fiber_body, sites.data(), rigidity.data()));
-    SKB_TRY(skb_flow_build_fiber_operators(fl, params, dt, eta));
-    std::vector<double> F, T;
-    if (body_forces_torques && nb > 0)
-        split_forces_torques(body_forces_torques, nb, F, T);
-    const bool fext = f_external && n_fib > 0;
-    if (fext)
-        CUDA_TRY(cudaMemcpyAsync(buf.fext.ptr, f_external, (size_t)n_fib * 24, cudaMemcpyHostToDevice, st));
-    if (!F.empty()) {
-        CUDA_TRY(cudaMemcpyAsync(buf.force.ptr, F.data(), F.size() * 8, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaMemcpyAsync(buf.torque.ptr, T.data(), T.size() * 8, cudaMemcpyHostToDevice, st));
-    }
-    SKB_TRY(skb_flow_build_system_rhs_device(fl, params, v_growth, force_scale,
-                                             fext ? (const double *)buf.fext.ptr : nullptr,
-                                             F.empty() ? nullptr : (const double *)buf.force.ptr,
-                                             F.empty() ? nullptr : (const double *)buf.torque.ptr, dt, eta,
-                                             kry.stage_b(), st));
-    SKB_TRY(skb_flow_solve_system_device(fl, dn, kry.stage_b(), eta, tol, num_blocks, max_iters, kry.stage_x(),
-                                         &info->solve, nullptr, st));
-    const double *d_x = kry.stage_x();
-
-    // ---- the bodies' step from their rows [U; w], on the host: one copy of the body part, the rows picked here ----
-    const long long body0 = 4 * n_fib + 3 * s.n_shell;
-    std::vector<double> xb((size_t)(n - body0));
-    if (nb > 0)
-        CUDA_TRY(cudaMemcpyAsync(xb.data(), d_x + body0, xb.size() * 8, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    std::vector<double> uw, c_new(3 * (size_t)nb), q_new(4 * (size_t)nb);
-    body_rows(s.bodies->frame_node_counts(), nb, xb.data(), uw);
-    for (int b = 0; b < nb; ++b)
-        body_step(s.centers + 3 * (size_t)b, s.orientations + 4 * (size_t)b, &uw[6 * (size_t)b],
-                  &uw[6 * (size_t)b + 3], dt, &c_new[3 * (size_t)b], &q_new[4 * (size_t)b]);
-    const bool bodies_finite = all_finite(uw);
-    std::vector<double> sites_new;
-    if (bodies_finite)
-        nucleation_sites(nf, fiber_body, site_ref, c_new.data(), q_new.data(), sites_new);
-    else
-        sites_new.assign(3 * (size_t)nf, 0.0);
-
-    // ---- the fibers' step, repin and error on the device; one download of the new positions ----
-    for (int f = 0; f < nf; ++f) {
-        StepItem &it = items[(size_t)f];
-        it.bound = fiber_body && fiber_body[f] >= 0;
-        std::memcpy(it.site, &sites_new[3 * (size_t)f], sizeof(it.site));
-    }
-    SKB_TRY(launch_fiber_step(s, s.fibers, items, d_x, true, st));
-    std::vector<double> r_new(3 * (size_t)n_fib), err((size_t)nf);
-    if (nf > 0) {
-        CUDA_TRY(cudaMemcpyAsync(r_new.data(), buf.r_new.ptr, r_new.size() * 8, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaMemcpyAsync(err.data(), buf.err.ptr, err.size() * 8, cudaMemcpyDeviceToHost, st));
-        if (tension)
-            CUDA_TRY(cudaMemcpyAsync(tension, buf.tension.ptr, (size_t)n_fib * 8, cudaMemcpyDeviceToHost, st));
-    }
-    if (x)
-        CUDA_TRY(cudaMemcpyAsync(x, d_x, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    if (!bodies_finite || !all_finite(r_new)) { // not installed: the caller's restore has nothing to undo
-        info->fiber_error = std::numeric_limits<double>::quiet_NaN();
-        return set_error(SKB_ERR_STATE, "%s: the solution holds non-finite %s; the geometry is unchanged", who,
-                         bodies_finite ? "fiber positions" : "body velocities");
-    }
-    reduce_errors(err, &info->fiber_error, &info->worst_fiber);
-
-    // ---- install: the new positions through skb_flow_set_fibers (same node counts and lengths, so the partition and
-    // the class table stay), the placement, the links at the new sites ----
-    const std::vector<int> n_nodes(s.fibers.n, s.fibers.n + nf);
-    const std::vector<double> length(s.length, s.length + nf);
-    // (every argument below has passed its call's checks already: only a CUDA error can stop the install half-way)
-    SKB_TRY(skb_flow_set_fibers(fl, r_new.data(), n_nodes.data(), length.data(), nf));
-    if (nb > 0)
-        SKB_TRY(skb_flow_place_bodies(fl, c_new.data(), q_new.data()));
-    return skb_flow_set_fiber_links(fl, fiber_body, sites_new.data(), rigidity.data());
-}
-
-// skb_flow_step on a flow that is no group member, its device arguments through the host
-static int step_not_member(skb_flow *fl, skb_dense *dn, const skb_fiber_params *params, const double *v_growth,
-                           const double *force_scale, const double *d_f_external, const double *d_body_forces,
-                           const double *d_body_torques, const int *fiber_body, const double *site_ref, double dt,
-                           double eta, double tol, int num_blocks, int max_iters, double *d_x, double *d_tension,
-                           skb_step_info *info, cudaStream_t st) {
-    CUDA_TRY(cudaSetDevice(flow_device(fl)));
+    const StepArgs a{params, v_growth, force_scale, fiber_body, site_ref, dt, eta, tol, num_blocks, max_iters};
+    StepCall c;
+    SKB_TRY(step_checks(fl, dn, a, info, who, c));
     const FlowState s = flow_state(fl);
     const long long n_fib = s.fibers.nodes();
     const int nb = s.n_bodies;
-    std::vector<double> fext(d_f_external ? 3 * (size_t)n_fib : 0), F(3 * (size_t)nb, 0.0), T(3 * (size_t)nb, 0.0),
-        ft;
-    if (!fext.empty())
-        CUDA_TRY(cudaMemcpyAsync(fext.data(), d_f_external, fext.size() * 8, cudaMemcpyDeviceToHost, st));
-    if (nb > 0 && d_body_forces)
-        CUDA_TRY(cudaMemcpyAsync(F.data(), d_body_forces, F.size() * 8, cudaMemcpyDeviceToHost, st));
-    if (nb > 0 && d_body_torques)
-        CUDA_TRY(cudaMemcpyAsync(T.data(), d_body_torques, T.size() * 8, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    if (nb > 0 && (d_body_forces || d_body_torques)) {
-        ft.resize(6 * (size_t)nb);
-        for (int b = 0; b < nb; ++b)
-            for (int k = 0; k < 3; ++k) {
-                ft[6 * (size_t)b + k] = F[3 * (size_t)b + k];
-                ft[6 * (size_t)b + 3 + k] = T[3 * (size_t)b + k];
-            }
+    SKB_TRY(step_host_inputs(who, f_external, n_fib, body_forces_torques, nb));
+    // the inputs into the step's own buffers, on the stream the step runs on
+    StepBuffers &buf = *s.buf;
+    const cudaStream_t st = flow_stream(fl);
+    const bool fext = f_external && n_fib > 0, ft = body_forces_torques && nb > 0;
+    if (fext)
+        CUDA_TRY(cudaMemcpyAsync(buf.fext.ptr, f_external, (size_t)n_fib * 24, cudaMemcpyHostToDevice, st));
+    std::vector<double> F, T;
+    if (ft) {
+        split_forces_torques(body_forces_torques, nb, F, T);
+        CUDA_TRY(cudaMemcpyAsync(buf.force.ptr, F.data(), F.size() * 8, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(buf.torque.ptr, T.data(), T.size() * 8, cudaMemcpyHostToDevice, st));
     }
-    const long long n = flow_whole_size(fl);
-    std::vector<double> x(d_x ? (size_t)n : 0), tension(d_tension ? (size_t)n_fib : 0);
-    const int rc = skb_flow_step(fl, dn, params, v_growth, force_scale, fext.empty() ? nullptr : fext.data(),
-                                 ft.empty() ? nullptr : ft.data(), fiber_body, site_ref, dt, eta, tol, num_blocks,
-                                 max_iters, d_x ? x.data() : nullptr, d_tension ? tension.data() : nullptr, info);
-    if (rc != SKB_OK && rc != SKB_ERR_STATE)
-        return rc;
-    if (d_x && n > 0)
-        CUDA_TRY(cudaMemcpyAsync(d_x, x.data(), (size_t)n * 8, cudaMemcpyHostToDevice, st));
-    if (d_tension && n_fib > 0)
-        CUDA_TRY(cudaMemcpyAsync(d_tension, tension.data(), (size_t)n_fib * 8, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    return rc;
+    return step_run(fl, dn, a, c, fext ? (const double *)buf.fext.ptr : nullptr,
+                    ft ? (const double *)buf.force.ptr : nullptr, ft ? (const double *)buf.torque.ptr : nullptr, x,
+                    tension, info, who);
 }
 
-// count doubles of d (device, NULL: nothing to check) through the pinned host copy `h` on st: all finite?  A copy, not a
-// launch, so a refusal on its result still comes before any launch
-static int device_finite(const double *d, size_t count, double *h, cudaStream_t st, bool *finite) {
-    *finite = true;
-    if (count == 0 || !d)
-        return SKB_OK;
-    CUDA_TRY(cudaMemcpyAsync(h, d, count * 8, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    for (size_t i = 0; i < count && *finite; ++i)
-        *finite = std::isfinite(h[i]);
-    return SKB_OK;
-}
-
-// System::step on one rank per GPU: the composed local-vector calls, then two epochs of the group's own protocol --
-// the body rows all-gathered through x_body, the fiber step fused with the all-gather of its results through r_step --
-// and the same decision and the same complete geometry on every member
 int skb_flow_group_step_device(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const skb_fiber_params *params,
                                const double *v_growth, const double *force_scale, const double *d_f_external,
                                const double *d_body_forces, const double *d_body_torques, const int *fiber_body,
@@ -356,161 +492,14 @@ int skb_flow_group_step_device(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_mi
                                void *stream) {
     const char *who = "skb_flow_group_step_device";
     const cudaStream_t st = (cudaStream_t)stream;
-    // ---- every refusal, before any launch ----
     if (!fl)
         return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    if (!flow_group(fl).member())
-        return step_not_member(fl, dn_spc, params, v_growth, force_scale, d_f_external, d_body_forces, d_body_torques,
-                               fiber_body, site_ref, dt, eta, tol, num_blocks, max_iters, d_x_local, d_tension, info,
-                               st);
-    SKB_TRY(step_scalar_args(who, info, dt, eta, tol, num_blocks, max_iters));
-    OwnFibers own;
-    long long n = 0;
-    std::array<long long, 6> key;
-    SKB_TRY(flow_group_step_checks(fl, dn_spc, dn_minv, who, own, &n, &key));
-    const FlowState s = flow_state(fl);
-    Group &G = flow_group(fl);
-    const int nf = s.fibers.count(), nfo = own.count(), nb = s.n_bodies;
-    const long long n_fib = s.fibers.nodes(), m = own.nodes(), n_sw = key[3] - key[2];
-    if (nfo > 0 && !params)
-        return set_error(SKB_ERR_INVALID, "%s: NULL params", who);
-    bool any_bound = false;
-    for (int f = 0; f < nfo; ++f) {
-        const int b = fiber_body ? fiber_body[f] : -1;
-        if (b < -1 || b >= nb)
-            return set_error(SKB_ERR_INVALID, "%s: own fiber %d (fiber %d) is bound to body %d (the flow has %d "
-                                              "bodies; -1 = free)", who, f, own.f0 + f, b, nb);
-        any_bound = any_bound || b >= 0;
-    }
-    if (any_bound && !site_ref)
-        return set_error(SKB_ERR_INVALID, "%s: NULL site_ref with bound fibers", who);
-    std::vector<double> sites, rigidity((size_t)nfo);
-    for (int f = 0; f < nfo; ++f)
-        rigidity[(size_t)f] = params[f].bending_rigidity;
-    nucleation_sites(nfo, fiber_body, site_ref, s.centers, s.orientations, sites);
-    SKB_TRY(s.bodies->set_links(own, *s.ops, nb, s.centers, fiber_body, sites.data(), rigidity.data(), flow_stream(fl),
-                                true));
-    SKB_TRY(s.ops->check_step(own, params, v_growth, force_scale));
-    std::vector<StepItem> items;
-    SKB_TRY(s.ops->step_items(own, items));
-    Krylov &kry = flow_krylov(fl);
-    if (!kry.sized_for(n, key) || !s.buf->sized_for(nf, n_fib, nb))
-        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_gmres for the member's current target ranges", who);
-    if (!s.ops->build_sized_for(own)) // (the build's buffers are sized only once every class it needs is set)
-        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_gmres after the fiber classes and their derivatives "
-                                          "are set (it sizes the fiber build's buffers)", who);
-    // the device inputs through the pinned copy skb_flow_set_gmres sized: 24 B per own node, 48 B per body
-    double *h = s.buf->check.get();
-    bool fin_f = true, fin_b = true, fin_t = true;
-    SKB_TRY(device_finite(d_f_external, 3 * (size_t)m, h, st, &fin_f));
-    if (!fin_f)
-        return set_error(SKB_ERR_INVALID, "%s: a non-finite external force", who);
-    if (nb > 0) {
-        SKB_TRY(device_finite(d_body_forces, 3 * (size_t)nb, h, st, &fin_b));
-        SKB_TRY(device_finite(d_body_torques, 3 * (size_t)nb, h, st, &fin_t));
-    }
-    if (!fin_b || !fin_t)
-        return set_error(SKB_ERR_INVALID, "%s: a non-finite external body force or torque", who);
-    if (num_blocks > kry.blocks())
-        return set_error(SKB_ERR_INVALID, "%s: num_blocks = %d, skb_flow_set_gmres sized the workspace for %d", who,
-                         num_blocks, kry.blocks());
-    std::memset(info, 0, sizeof(*info));
-    info->worst_fiber = -1;
-    if (flow_whole_size(fl) == 0) { // the empty system, on every member alike: nothing moves
-        info->solve.converged = 1;
-        return SKB_OK;
-    }
-
-    // ---- System::step: the links, the operators (on the flow's stream, drained), the RHS and the solve on st ----
-    StepBuffers &buf = *s.buf;
-    SKB_TRY(skb_flow_group_set_fiber_links(fl, fiber_body, sites.data(), rigidity.data()));
-    SKB_TRY(skb_flow_build_fiber_operators(fl, params, dt, eta));
-    CUDA_TRY(cudaStreamSynchronize(flow_stream(fl)));
-    SKB_TRY(skb_flow_group_build_system_rhs_device(fl, params, v_growth, force_scale, d_f_external, d_body_forces,
-                                                   d_body_torques, dt, eta, kry.stage_b(), st));
-    SKB_TRY(skb_flow_group_solve_system_device(fl, dn_spc, dn_minv, kry.stage_b(), eta, tol, num_blocks, max_iters,
-                                               kry.stage_x(), &info->solve, nullptr, st));
-    const double *d_x = kry.stage_x(); // [4 per own fiber node | 3 per own periphery row | own body rows]
-    int *launches = flow_launches(fl); // the protocol's launches join the flow's count, as in the other member calls
-
-    // ---- the body rows all-gathered (an epoch of its own: the rows phase), [U; w] of every body from the own window
-    // (48 bytes per body), the bodies' step on the host: every member from the same bits ----
-    std::vector<double> uw(6 * (size_t)nb), c_new(3 * (size_t)nb), q_new(4 * (size_t)nb);
-    if (nb > 0) {
-        SKB_TRY(G.begin());
-        SKB_TRY(G.store_rows(d_x + 4 * m + 3 * n_sw, nullptr, 0, 0, flow_num_sms(fl), st, launches));
-        SKB_TRY(G.rows_barrier(true, true, st, launches));
-        const int *nodes = s.bodies->frame_node_counts();
-        long long off = 0;
-        for (int b = 0; b < nb; ++b) {
-            off += 3LL * nodes[b];
-            CUDA_TRY(cudaMemcpyAsync(&uw[6 * (size_t)b], G.x_body() + off, 48, cudaMemcpyDeviceToHost, st));
-            off += 6;
-        }
-        CUDA_TRY(cudaStreamSynchronize(st));
-    }
-    for (int b = 0; b < nb; ++b)
-        body_step(s.centers + 3 * (size_t)b, s.orientations + 4 * (size_t)b, &uw[6 * (size_t)b],
-                  &uw[6 * (size_t)b + 3], dt, &c_new[3 * (size_t)b], &q_new[4 * (size_t)b]);
-    const bool bodies_finite = all_finite(uw);
-    std::vector<double> sites_new;
-    if (bodies_finite)
-        nucleation_sites(nfo, fiber_body, site_ref, c_new.data(), q_new.data(), sites_new);
-    else
-        sites_new.assign(3 * (size_t)nfo, 0.0);
-
-    // ---- the own fibers' step, repin and error fused with the all-gather of the results into r_step of every window
-    // (an epoch of its own, the rows phase again), then the complete positions and errors from the own window ----
-    std::vector<double> r_new(3 * (size_t)n_fib), err((size_t)nf);
-    if (nf > 0) {
-        SKB_TRY(G.begin());
-        if (nfo > 0) {
-            for (int f = 0; f < nfo; ++f) {
-                StepItem &it = items[(size_t)f];
-                it.bound = fiber_body && fiber_body[f] >= 0;
-                std::memcpy(it.site, &sites_new[3 * (size_t)f], sizeof(it.site));
-            }
-            CUDA_TRY(cudaMemcpyAsync(buf.items.ptr, items.data(), (size_t)nfo * sizeof(StepItem),
-                                     cudaMemcpyHostToDevice, st));
-            StepGather g;
-            g.size = G.step_windows(g.r_step);
-            g.n_fib = n_fib;
-            g.node0 = own.off[own.f0];
-            g.fiber0 = own.f0;
-            group_fiber_step_kernel<<<nfo, kStepThreads, 0, st>>>((const StepItem *)buf.items.ptr, d_x,
-                                                                  s.ops->class_table(), s.ops->class_range_table(),
-                                                                  own.length + own.f0, (double *)buf.tension.ptr, g);
-            CUDA_TRY(cudaGetLastError());
-            count_launch(1);
-            *launches += 1;
-        }
-        SKB_TRY(G.rows_barrier(true, true, st, launches));
-        CUDA_TRY(cudaMemcpyAsync(r_new.data(), G.r_step(), r_new.size() * 8, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaMemcpyAsync(err.data(), G.r_step() + 3 * n_fib, err.size() * 8, cudaMemcpyDeviceToHost, st));
-        if (d_tension && m > 0)
-            CUDA_TRY(cudaMemcpyAsync(d_tension, buf.tension.ptr, (size_t)m * 8, cudaMemcpyDeviceToDevice, st));
-    }
-    if (d_x_local && n > 0)
-        CUDA_TRY(cudaMemcpyAsync(d_x_local, d_x, (size_t)n * 8, cudaMemcpyDeviceToDevice, st));
-    CUDA_TRY(cudaStreamSynchronize(st)); // the downloads land before this member's next signal
-
-    // ---- one decision, from the complete arrays every member holds alike ----
-    if (!bodies_finite || !all_finite(r_new)) {
-        info->fiber_error = std::numeric_limits<double>::quiet_NaN();
-        return set_error(SKB_ERR_STATE, "%s: the solution holds non-finite %s; the geometry is unchanged", who,
-                         bodies_finite ? "fiber positions" : "body velocities");
-    }
-    reduce_errors(err, &info->fiber_error, &info->worst_fiber);
-
-    // ---- install the complete geometry (same counts: the window, the partition and every buffer stay) ----
-    const std::vector<int> n_nodes(s.fibers.n, s.fibers.n + nf);
-    const std::vector<double> length(s.length, s.length + nf);
-    SKB_TRY(skb_flow_set_fibers(fl, r_new.data(), n_nodes.data(), length.data(), nf));
-    if (nb > 0)
-        SKB_TRY(skb_flow_group_place_bodies(fl, c_new.data(), q_new.data()));
-    SKB_TRY(skb_flow_group_set_fiber_links(fl, fiber_body, sites_new.data(), rigidity.data()));
-    CUDA_TRY(cudaStreamSynchronize(flow_stream(fl)));
-    return SKB_OK;
+    const StepArgs a{params, v_growth, force_scale, fiber_body, site_ref, dt, eta, tol, num_blocks, max_iters};
+    StepCall c;
+    SKB_TRY(group_step_checks(fl, dn_spc, dn_minv, a, info, who, c));
+    SKB_TRY(step_device_inputs(who, flow_state(fl), d_f_external, c.own.nodes(), d_body_forces, d_body_torques, st));
+    return group_step_run(fl, dn_spc, dn_minv, a, c, d_f_external, d_body_forces, d_body_torques, d_x_local, d_tension,
+                          info, who, st);
 }
 
 int skb_flow_fiber_error(skb_flow *fl, double *max_error, double *per_fiber) {

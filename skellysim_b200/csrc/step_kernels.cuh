@@ -16,21 +16,12 @@
 // window (DESIGN.md §4), at its place among ALL fibers.  The values are those fiber_step_kernel writes, bit for bit:
 // both kernels run one body (fiber_step) and differ only in where its outputs go.
 #pragma once
-#include <cuda_runtime.h>
+#include "skb_internal.hpp" // StepItem
 
 namespace skb {
 
 constexpr int kStepThreads = 128;
 constexpr int kStepMaxNodes = 128; // the device build's largest fiber (kBuildMaxNodes): 3n doubles of shared memory
-
-struct StepItem {
-    long long node;  // first node of the fiber among the launch's nodes (positions 3 per node, solution 4 per node)
-    long long d1;    // element offset of its class's D_1_0 (n x n, column-major) in the class table
-    long long rng;   // offset of its class's D_1_0 column ranges (int2 per column) in the class ranges
-    double site[3];  // the lab-frame nucleation site a bound fiber is repinned to
-    int n;           // nodes
-    int bound;       // 1: repin to site
-};
 
 // NaN wins: a fiber with a non-finite node reports a NaN error instead of hiding it
 __device__ __forceinline__ double step_max(double a, double b) { return (a > b || a != a) ? a : b; }

@@ -3,10 +3,12 @@ distributed.RankStepper): every member steps its own fibers and reads the others
 from its own group window, so that all members hold the same geometry and take the same decision.
 
 The members live in one process, connected by skb_flow_group_connect, each driven by its own Python thread on its own
-stream, on device lists [0, 0] and [0, 0, 0] and on the real lists when more GPUs are present.  Each member's info, its
+stream, on device lists [0, 0] and [0, 0, 0] and on the real lists when more GPUs are present.  skb_mflow_step runs the
+same member step from the library's own threads, on host arrays it slices and uploads itself; each member's info, its
 local rows of the solution (scattered through local_rows), its own tensions and the geometry it holds afterwards are
-held bitwise to skb_mflow_step on the same device list, step after step; each group step runs before the skb_mflow
-step it is compared with, the first one straight after set_gmres.  The step must allocate nothing and load no kernel
+held bitwise to it on the same device list, step after step, so that the Python driver (RankStepper's slices, uploads
+and device inputs) is held to the library's.  Each group step runs before the skb_mflow step it is compared with, the
+first one straight after set_gmres.  The step must allocate nothing and load no kernel
 while a peer on the same device may spin on a flag: every group step here is held to leave the library's buffer
 allocation count (skb_buffer_alloc_count) and torch's allocation count unchanged.  A lazy kernel load cannot be seen in
 a process where earlier tests already ran the kernels, so one test runs a first group step in a fresh process, before

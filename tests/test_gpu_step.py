@@ -477,11 +477,32 @@ def test_a_non_finite_solution_with_a_body_installs_nothing():
 
 
 def test_refusals_with_a_body_leave_fibers_and_placement_untouched():
+    refusals_with_a_body(None)
+
+
+def test_refusals_with_a_body_over_three_members_leave_fibers_and_placement_untouched():
+    """the members own one fiber each, so that fiber_body=[0, 1, -1] is a refusal only member 1's fiber shows"""
+    refusals_with_a_body([0, 0, 0])
+
+
+def refusals_with_a_body(devs):
+    """on a Flow (devs None) or over skb_mflow on devs: a refused step launches nothing and changes nothing, and the
+    next step is bitwise the step of a twin that saw no refusal (over skb_mflow that step also fails if any member's
+    flag wait timed out)"""
     case = step_case("FPB")
-    with contextlib.ExitStack() as stack:
-        fl = stack.enter_context(skb.Flow(0))
-        dn = stack.enter_context(skb.Dense(device_ids=[0]))
+
+    def stepping(stack):
+        if devs is None:
+            fl, dn = stack.enter_context(skb.Flow(0)), stack.enter_context(skb.Dense(device_ids=[0]))
+        else:
+            fl, dn = stack.enter_context(skb.MultiFlow(devs)), None
         set_up(fl, dn, case)
+        return fl, dn
+
+    with contextlib.ExitStack() as stack:
+        fl, dn = stepping(stack)
+        if devs is not None:
+            assert [fl.partition(g)[:2] for g in range(3)] == [(0, 1), (1, 2), (2, 3)]
         r0, (c0, q0) = fl.fibers(), fl.placement()
         bad = [dict(dt=0.0), dict(fiber_body=[0, 1, -1]), dict(site_ref=None), dict(num_blocks=301),
                dict(body_forces_torques=np.full((1, 6), np.inf))]
@@ -495,8 +516,13 @@ def test_refusals_with_a_body_leave_fibers_and_placement_untouched():
             c1, q1 = fl.placement()
             assert np.array_equal(fl.fibers(), r0) and np.array_equal(c0, c1) and np.array_equal(q0, q1), kw
         # and the links stay: a step after the refusals is the step from the untouched state
-        _, _, info = step_of(fl, dn, case)
+        x, tension, info = step_of(fl, dn, case)
         assert np.isfinite(info["fiber_error"])
+        twin, dn2 = stepping(stack)
+        x2, tension2, info2 = step_of(twin, dn2, case)
+        assert np.array_equal(x, x2) and np.array_equal(tension, tension2) and info == info2
+        assert np.array_equal(fl.fibers(), twin.fibers())
+        assert all(np.array_equal(u, v) for u, v in zip(fl.placement(), twin.placement()))
 
 
 def test_stepper_backs_up_and_restores_a_multiflow():
