@@ -1,0 +1,314 @@
+// skb_flow.hpp -- the flow (include/skelly_b200_flow.h) and what the translation units built on it share:
+// skb_matvec.cu (its lifetime, geometry, flows and matvec orchestration), skb_system.cu (the whole-system calls),
+// skb_solve.cu, skb_step.cu and skb_mflow.cu.  Free functions in namespace skb that take the flow.
+#pragma once
+#include "skb_internal.hpp"
+#include "../../include/skelly_b200_flow.h"
+#include "../../include/skelly_b200_dense.h"
+
+#include <array>
+#include <cstring>
+#include <memory>
+#include <vector>
+
+namespace skb {
+struct TargetCache {
+    std::vector<double> host;
+    bool valid = false;
+    unsigned long long version = 0; // bumped by every upload: part of the CUDA-graph key (a replay bakes in whether
+                                    // the symmetric path -- targets start with the sources -- was taken)
+    bool same(const double *r, long long n) const {
+        return valid && (long long)host.size() == 3 * n && (n == 0 || std::memcmp(host.data(), r, (size_t)n * 24) == 0);
+    }
+    void store(const double *r, long long n) {
+        host.assign(r, r + 3 * n);
+        valid = true;
+        ++version;
+    }
+};
+using CtxPtr = std::unique_ptr<skb_ctx, Destroyer<skb_ctx_destroy>>;
+
+// the step's device buffers: per fiber its item and error, per fiber node its new position and tension, the external
+// forces and torques of the RHS; and a pinned host copy of skb_flow_group_step_device's device inputs (3 per fiber
+// node + 6 per body)
+// for their finiteness check.  Sized by skb_flow_set_gmres (the step itself allocates none of them)
+struct StepBuffers {
+    DevBuf items, r_new, tension, err, fext, force, torque;
+    PinnedHost check;
+    int size(int n_fibers, long long n_fib, int n_bodies);
+    bool sized_for(int n_fibers, long long n_fib, int n_bodies) const {
+        return n_fibers_ == n_fibers && n_fib_ == n_fib && n_bodies_ == n_bodies;
+    }
+
+  private:
+    int n_fibers_ = -1, n_bodies_ = -1;
+    long long n_fib_ = -1;
+    size_t check_cap_ = 0; // doubles of `check`
+};
+} // namespace skb
+
+struct skb_flow {
+    int dev = 0;
+    skb::Stream stream;
+    skb::Event ev0, ev1, evt0, evt1;
+    // geometry
+    long long n_fib = 0, n_shell = 0, n_body = 0;
+    int n_fibers = 0, n_bodies = 0, max_fiber_nodes = 0;
+    skb::DevBuf fiber_offset, fiber_length, r_fib, r_shell, r_body, centers;
+    std::vector<double> h_r_fib, h_r_shell, h_r_body; // host copies to assemble the matvec target lists
+    // evaluators: [0] arbitrary targets, [1] matvec target lists
+    skb::CtxPtr fib[2], shell[2], body[2];
+    skb::TargetCache tc_fib, tc_shell, tc_body;
+    bool mv_dirty = true;
+    int cross_mode = -1;    // fiber <-> periphery cross kernel in the matvec: -1 auto, 0 off, 1 on whenever applicable
+    // how matvec_core evaluates, decided by prepare_matvec_targets
+    struct MatvecPlan {
+        bool grouped = false; // group member: the strengths come packed from the group window (push), not the caller
+        // producer of the fiber rows: the plain kernel; the symmetric kernel's complete rows (whole system on this
+        // device, cross kernel); or this member's symmetric partial sums, pulled together from all members' windows
+        enum FiberRows { kPlain, kSymComplete, kSymPartial } fib_rows = kPlain;
+        bool cross = false;   // fiber <-> periphery pairs through the cross kernel
+    } plan;
+    skb::CrossState cross;
+    bool self_excl = false; // matvec: skip intra-fiber pairs in the kernels instead of compute-then-subtract (N3, opt-in)
+    long long win_begin = 0, win_end = -1; // target window of the matvec in [fibers|shell|bodies] rows; -1 = all
+    bool use_ranges = false;               // skb_flow_set_target_ranges instead of a contiguous window
+    long long rq_f0 = 0, rq_f1 = 0, rq_s0 = 0, rq_s1 = 0, rq_b0 = 0, rq_b1 = 0; // requested (fiber indices, rows)
+    // resolved pieces of the matvec target list: fiber rows [fa,fb), shell rows [sa,sb), body rows [ba,bb);
+    // the output has n_win = (fb-fa)+(sb-sa)+(bb-ba) rows in that order
+    long long fa = 0, fb = 0, sa = 0, sb = 0, ba = 0, bb = 0, n_win = 0;
+    cudaStream_t cur = nullptr;            // stream of the call in flight (own stream or the caller's)
+    int n_points = 0;
+    skb::DevBuf pt_pos, pt_force, pt_torque;
+    bool has_background = false;
+    // CUDA-graph replay of the launch-bound small-size calls (BASELINE C1, listener / streamline path)
+    struct GraphSlot {
+        skb::GraphExec exec;
+        unsigned long long key = 0, seen = 0;
+        int launches = 0;
+        long long pairs = 0;
+        void reset() {
+            exec.reset();
+            key = seen = 0;
+        }
+    } g_matvec, g_vat;
+    unsigned long long geom_version = 1;
+    bool graphs_enabled = true;
+    skb::PinnedHost h_stage; // pinned staging: the graph's memcpy nodes need fixed host addresses
+    size_t h_stage_cap = 0;
+    int bg_comp[3] = {0, 1, 2};
+    double bg_scale[3] = {0, 0, 0}, bg_uniform[3] = {0, 0, 0};
+    std::vector<int> h_fiber_n;         // nodes of every fiber
+    std::vector<long long> h_fiber_off; // first node of every fiber (n_fibers + 1)
+    skb::FiberOps ops; // per-fiber dense operators of the fibers whose rows are in the target list (skb_fiber.cu)
+    skb::BodyOps bodies; // the bodies' operators and the fiber-body links of the whole-vector operator (skb_body.cu)
+    std::vector<double> h_centers; // body centres (set_fiber_links measures the nucleation sites from them)
+    std::vector<double> h_fiber_len; // length_ of every fiber (the time step installs its new positions with them)
+    std::vector<double> h_orient;    // the quaternions of the last skb_flow_place_bodies (4 per body) ...
+    bool placed = false;             // ... valid until skb_flow_set_bodies changes the bodies otherwise
+    skb::StepBuffers stepbuf;             // the buffers of skb_flow_step (skb_step.cu)
+    skb::Group grp; // multi-GPU group membership: one member per GPU, exchange through peer memory (skb_group.cu)
+    // a member's whole-vector matvec in flight: matvec_core exchanges the bodies' partial link forces through the
+    // window and the body flow reads their totals from ft_sum ([F | L], 6 per body)
+    bool ft_exchange = false;
+    skb::DevBuf ft_sum;
+    // a rank-per-GPU member's whole-vector matvec has begun the epoch (and exchanged its body rows in it): matvec_core
+    // runs its protocol in that epoch instead of beginning one
+    bool grp_open = false;
+    skb::DevBuf sys_rb; // a member's body output in the whole body layout (skb_flow_group_*), compacted to its own rows
+    // Periphery::matvec's dense operator beside the pair kernels (stream_kernels.cuh): forked onto bg_stream once its
+    // input (the complete x_shell) is there, joined before res_shell is assembled
+    struct Overlap {
+        bool enabled = true;       // skb_flow_set_overlap
+        skb::Stream stream;
+        skb::Event fork, join;
+        skb::DevBuf y;                  // A x of the own periphery rows
+        skb_dense *dn = nullptr;   // pending background product of the call in flight (nullptr: none)
+        bool launched = false;
+    } bg;
+    skb::DevBuf scratch_u; // group mode: landing zone of eval_on_device's default output (never read)
+    // staging
+    skb::DevBuf in_fib, in_shell, in_body, in_force, in_torque, vel, tmp, x_fib, res_fib, vb, res_shell, tmp_b;
+    skb::DevBuf sys_x, sys_y; // the whole solution vector in and out of the host forms of the system operator
+    skb::DevBuf zeros;        // the system RHS: the zero densities (and absent forces) its flow takes, n_zeros doubles
+    long long n_zeros = 0;
+    skb::Krylov kry; // the workspace of skb_flow_solve_system (skb_solve.cu)
+    skb_flow_stats stats{};
+    int launches = 0;
+    long long pairs = 0;
+};
+
+namespace skb {
+// every fiber of the flow
+inline OwnFibers all_fibers(const skb_flow *fl) {
+    return OwnFibers{0, fl->n_fibers, fl->h_fiber_n.data(), fl->h_fiber_off.data(), (const double *)fl->r_fib.ptr,
+                     (const double *)fl->fiber_length.ptr, fl->stream};
+}
+
+// ---- skb_matvec.cu ----
+// resolve the target window / ranges into fiber, shell and body pieces and (re)build the matvec target lists
+int prepare_matvec_targets(skb_flow *fl);
+// The fibers whose operators are resident: those whose rows are in this flow's target list -- all of them, or the
+// rank's own fibers under skb_flow_set_target_ranges / an aligned skb_flow_set_target_window.
+int own_fibers(skb_flow *fl, const char *who, OwnFibers &own);
+// the background streamer's buffers for n_rows own periphery rows
+int overlap_buffers(skb_flow *fl, long long n_rows);
+// device-side matvec flow on fl->cur, as fl->plan says: d_ff / d_sd are the strengths of the own fibers / periphery
+// rows (all of them without a group), body inputs are complete; d_v = [own fiber rows | own shell rows | own body rows]
+// of v_all
+int matvec_core(skb_flow *fl, const double *d_ff, const double *d_sd, const double *d_bd, const double *d_f,
+                const double *d_t, double eta, double *d_v);
+// System::apply_matvec (system.cpp:298-319) on fl->cur, everything device resident.  Inputs are the OWN slices of a
+// group member (all of them without a group): d_x 4 per own fiber node, d_xs 3 per own periphery row, body inputs
+// complete, d_link 7 per own fiber or NULL.  Outputs: d_res_fib 4 per own node, d_out_shell 3 per own periphery row
+// (res_shell when dn != NULL, else v_shell), d_v_bodies 3 per own body row; any of them may be NULL when empty.
+int apply_matvec_core(skb_flow *fl, skb_dense *dn, const double *d_x, const double *d_xs, const double *d_bd,
+                      const double *d_f, const double *d_t, const double *d_link, double eta, double *d_res_fib,
+                      double *d_out_shell, double *d_v_bodies);
+// + psc.flow(r_trg, eta, time) + bs.flow(r_trg, eta) (system.cpp:358-359, 445-446) on st: the point sources of
+// skb_flow_set_point_sources and the background flow of skb_flow_set_background at the n_trg targets d_trg, added to
+// the rows of d_v in this order: Oseen contraction, rotlet, background
+int add_sources(skb_flow *fl, const double *d_trg, long long n_trg, double eta, double *d_v, cudaStream_t st);
+int load_source_kernels(); // the kernels of add_sources, loaded now
+int upload(skb_flow *fl, DevBuf &buf, const double *h, size_t n_doubles);
+int download(skb_flow *fl, double *h, const DevBuf &buf, size_t n_doubles);
+void begin_stats(skb_flow *fl);
+int finish_stats(skb_flow *fl);
+// the device-pointer entry points run asynchronously on the caller's stream: no timings
+int device_stats(skb_flow *fl);
+
+// frame of the host-pointer entry points on fl->stream: device_ms spans the device work, total_ms also the uploads
+// before it and the downloads after it; returns once the downloads have landed
+template <class Up, class Work, class Down> int host_frame(skb_flow *fl, Up up, Work work, Down down) {
+    fl->cur = fl->stream;
+    CUDA_TRY(cudaEventRecord(fl->evt0, fl->stream));
+    SKB_TRY(up());
+    CUDA_TRY(cudaEventRecord(fl->ev0, fl->stream));
+    SKB_TRY(work());
+    CUDA_TRY(cudaEventRecord(fl->ev1, fl->stream));
+    SKB_TRY(down());
+    CUDA_TRY(cudaEventRecord(fl->evt1, fl->stream));
+    return finish_stats(fl);
+}
+
+// ---- skb_system.cu: the whole-system calls ----
+// the whole solution vector's size (of every member alike)
+long long solution_size(const skb_flow *fl);
+// a rank-per-GPU member: the resolved target ranges its set-up sized its buffers for (prepare_matvec_targets has run),
+// and the size of its local vector
+Group::Ranges group_ranges(const skb_flow *fl);
+long long group_local_size(const skb_flow *fl);
+
+// The family of calls whose set-up calls a refusal names: `setup` prefixes the calls that set the bodies' operators,
+// frames and links, `geometry` those that set the fibers and bodies
+struct Calls {
+    const char *setup, *geometry;
+};
+constexpr Calls kFlowCalls{"skb_flow_", "skb_flow_"}, kMflowCalls{"skb_mflow_", "skb_mflow_"},
+    kGroupCalls{"skb_flow_group_", "skb_flow_"};
+// What the system calls need besides the dense operator: an error naming `who` unless it is there.  The fiber
+// operators (with their inverse for the preconditioner), the body operators (with their inverse for the preconditioner)
+// and, for the matvec, the fiber links.  step: the step, which builds the fiber operators and sets the links itself but
+// places the bodies from their frames (precondition: the frames' inverse)
+int system_ready(skb_flow *fl, const char *who, const Calls &calls, bool precondition, bool step = false);
+// dn holds this flow's rows of the periphery operator of a system call (matvec: stresslet_plus_complementary;
+// precondition: M_inv): on the flow's device, 3 (sb - sa) rows x 3 n_shell
+int dense_rows(skb_flow *fl, skb_dense *dn, const char *who, bool precondition);
+// an error naming `who` unless the flow's target list is the whole system; `hint` ends the message
+int whole_targets(skb_flow *fl, const char *who, const char *hint);
+// The checks of the system operator of a single-device flow (matvec: stresslet_plus_complementary in dn; precondition:
+// M_inv and the inverses), all before any launch; then the flow's device is current and its target list resolved.
+int system_args(skb_flow *fl, skb_dense *dn, const char *who, bool precondition, bool args);
+// the same for a group member's local-vector calls
+int group_system_args(skb_flow *fl, skb_dense *dn, const char *who, bool precondition);
+
+// the size and key skb_flow_set_gmres sizes for (a member: its local rows, which need its rows laid out)
+int flow_gmres_size(skb_flow *fl, const char *who, long long *n, std::array<long long, 6> *key);
+// a group member (else nothing): lays out its own body rows for bodies of n_nodes and sizes every buffer its
+// local-vector calls use (what skb_flow_group_set_body_operators / _set_body_frames do besides the operators)
+int flow_member_lay_out_rows(skb_flow *fl, const char *who, const int *n_nodes, int n_bodies);
+
+// R (row-major) of a unit quaternion (w, x, y, z): the formula of Eigen's QuaternionBase::toRotationMatrix
+void quaternion_rotation(const double *q, double *R);
+// The frames of the flow's bodies (a member: for its body rows); the refusals of a placement, before any state
+// changes, with the rotations R (9 per body) it places at; the placement itself, after placement_args
+int body_frames(skb_flow *fl, const char *who, const int *n_nodes, int n_bodies, const double *pos_ref,
+                const double *normal_ref, const double *node_weights, const double *ex0, const double *ey0,
+                const double *ez0, const double *A_inv0);
+int placement_args(skb_flow *fl, const char *who, const double *centers, const double *orientations,
+                   std::vector<double> &R);
+int place_bodies(skb_flow *fl, const double *centers, const double *orientations, const std::vector<double> &R);
+
+// The whole-vector operator on one member of skb_mflow (the members of a group, or the single flow of a one-device
+// skb_mflow), after its target ranges are set.  The arguments are those of skb_flow_set_body_operators /
+// _set_fiber_links for ALL bodies / fibers; a member keeps the part its ranges own (BodyOps).  check_only: check the
+// links of every fiber and keep the earlier ones
+int flow_member_body_operators(skb_flow *fl, const int *n_nodes, int n_bodies, const double *node_weights,
+                               const double *ex, const double *ey, const double *ez, const double *A_inv);
+int flow_member_fiber_links(skb_flow *fl, const int *body, const double *site, const double *rigidity,
+                            bool check_only);
+int flow_size_system(skb_flow *fl); // sizes the buffers the two calls below use (before any member launches)
+// on st: x_fib 4 per own fiber node, x_shell 3 per own periphery row, x_bodies complete; res_fib / res_shell own rows,
+// res_bodies in the complete body layout, the owned rows written.  dn: the member's rows of
+// stresslet_plus_complementary (NULL without periphery rows)
+int flow_member_system_matvec(skb_flow *fl, skb_dense *dn, const double *d_x_fib, const double *d_x_shell,
+                              const double *d_x_bodies, double eta, double *d_res_fib, double *d_res_shell,
+                              double *d_res_bodies, cudaStream_t st);
+// the same layout, x_shell complete (3 per periphery node); dn: the member's rows of M_inv
+int flow_member_system_precondition(skb_flow *fl, skb_dense *dn, const double *d_x_fib, const double *d_x_shell,
+                                    const double *d_x_bodies, double *d_y_fib, double *d_y_shell, double *d_y_bodies,
+                                    cudaStream_t st);
+// The system RHS (skb_flow_build_system_rhs) on a member; params / v_growth / force_scale of ALL fibers.
+// flow_member_rhs_prepare, on the calling thread before any member launches: the refusals (the member's fibers and
+// bodies), the upload of the fiber block's per-fiber tables, and every buffer and kernel the call uses.
+// flow_member_system_rhs on st: d_fext 3 per own fiber node or NULL, d_f / d_t 3 per body (complete) or NULL; the
+// outputs as flow_member_system_matvec's
+int flow_member_rhs_prepare(skb_flow *fl, const ::skb_fiber_params *params, const double *v_growth,
+                            const double *force_scale, double dt, double eta);
+int flow_member_system_rhs(skb_flow *fl, const ::skb_fiber_params *params, const double *v_growth,
+                           const double *force_scale, const double *d_fext, const double *d_f, const double *d_t,
+                           double dt, double eta, double *d_rhs_fib, double *d_rhs_shell, double *d_rhs_bodies,
+                           cudaStream_t st);
+
+// ---- skb_solve.cu ----
+// the refusals of a solve's tol, num_blocks and max_iters (each caller checks its own eta)
+int solve_scalar_args(const char *who, double tol, int num_blocks, int max_iters);
+
+// ---- the time step (skb_step.cu), which skb_mflow_step drives on every member ----
+// the per-fiber arguments of a step (of the fibers it steps: a group member's own) and its scalars
+struct StepArgs {
+    const ::skb_fiber_params *params;
+    const double *v_growth, *force_scale;
+    const int *fiber_body;
+    const double *site_ref;
+    double dt, eta, tol;
+    int num_blocks, max_iters;
+};
+// what a step's refusals leave for its run: the fibers it steps, their items, bending rigidity and current nucleation
+// sites, and the (local) solution size
+struct StepCall {
+    OwnFibers own;
+    std::vector<StepItem> items;
+    std::vector<double> rigidity, sites;
+    long long n = 0;
+};
+// the refusals of the step's host arguments: the scalars; params, fiber_body and site_ref of nf fibers (the first is
+// fiber f0) against nb bodies; the external forces of n_fib fiber nodes and the forces and torques of nb bodies finite
+int step_scalar_args(const char *who, const ::skb_step_info *info, double dt, double eta, double tol, int num_blocks,
+                     int max_iters);
+int step_fiber_args(const char *who, const ::skb_fiber_params *params, const int *fiber_body, const double *site_ref,
+                    int f0, int nf, int nb);
+int step_host_inputs(const char *who, const double *f_external, long long n_fib, const double *body_forces_torques,
+                     int nb);
+// skb_flow_group_step_device in two halves (on a flow that is no member, such as a one-device skb_mflow's, those of
+// skb_flow_step).  group_step_checks: every refusal except the device inputs' finiteness, before any launch, with the
+// arguments of the member's own fibers.  group_step_run: the step itself, which meets the member's peers at flag
+// waits -- every member's checks must have passed first.  Inputs on the device as the
+// public call takes them; x_local / tension (host or device memory, NULL: not wanted) receive the member's local rows
+// of the solution and its own fibers' tensions, also when the step is not installed (SKB_ERR_STATE)
+int group_step_checks(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const StepArgs &a, ::skb_step_info *info,
+                      const char *who, StepCall &c);
+int group_step_run(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const StepArgs &a, StepCall &c,
+                   const double *d_f_external, const double *d_body_forces, const double *d_body_torques,
+                   double *x_local, double *tension, ::skb_step_info *info, const char *who, cudaStream_t st);
+} // namespace skb

@@ -13,7 +13,6 @@
 
 struct skb_fiber_params;
 struct skb_solve_info;
-struct skb_step_info;
 
 namespace skb {
 
@@ -419,7 +418,7 @@ int load_dense_kernels();
 //
 // [2]: double buffering by epoch parity -- a peer may already push the next call's strengths or rows while this member
 // still reads the current ones (DESIGN.md §4 argues why the other half is never still being read).  A
-// default-constructed Group is no member (size 1).  Knows nothing of skb_flow: the caller has made the flow's device
+// default-constructed Group is no member (size 1).  Knows nothing of the flow: the caller has made the flow's device
 // current, and every step runs on the stream it passes, adding its launches to *launches.
 class Group {
   public:
@@ -567,158 +566,6 @@ class Krylov {
     std::vector<double> H_, cs_, sn_, g_, y_; // the Hessenberg matrix ((m + 1) x m, column-major) and its rotations
 };
 
-} // namespace skb
-
-// ---- flow internals that skb_mflow.cu needs (skb_matvec.cu) ----
-struct skb_flow;
-struct skb_dense;
-namespace skb {
-// ---- and that skb_solve.cu needs: the flow's GMRES workspace, the checks of both system calls (dn holds both
-// operators) with *n = the solution size, one apply on st of a single-device flow whose checks have passed, and its
-// launch counter and SM count
-Krylov &flow_krylov(skb_flow *fl);
-Group &flow_group(skb_flow *fl);
-// the refusals of the two system calls the solve makes (a group member's local-vector calls, else the single-device
-// ones): dn_spc holds stresslet_plus_complementary, dn_minv M_inv; *n = the (local) solution size, *key its ranges
-int flow_solve_args(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const char *who, long long *n,
-                    std::array<long long, 6> *key);
-// the size and key skb_flow_set_gmres sizes for (a member: its local rows, which need its rows laid out)
-int flow_gmres_size(skb_flow *fl, const char *who, long long *n, std::array<long long, 6> *key);
-// a member of skb_mflow: lays out its local rows (what skb_flow_group_set_body_operators does besides the operators)
-// for the node counts of the bodies' operators it holds
-int flow_member_lay_out_rows(skb_flow *fl, const int *n_nodes, int n_bodies);
-int *flow_launches(skb_flow *fl);
-int flow_finish_device_stats(skb_flow *fl, int launches); // the stats of a _device call that made `launches`
-long long flow_whole_size(skb_flow *fl); // the whole solution vector's size (of every member alike)
-int flow_num_sms(const skb_flow *fl);
-int flow_device(const skb_flow *fl);
-cudaStream_t flow_stream(const skb_flow *fl); // the stream of the flow's own calls
-// sizes the buffers of the background streamer (skb_flow_set_overlap) for n_rows own periphery rows, if it is on
-int flow_size_overlap(skb_flow *fl, long long n_rows);
-
-// ---- and that the time step of a single-device flow needs (skb_step.cu) ----
-// the step's device buffers: per fiber its item and error, per fiber node its new position and tension, the external
-// forces and torques of the RHS; and a pinned host copy of skb_flow_group_step_device's device inputs (3 per fiber
-// node + 6 per body)
-// for their finiteness check.  Sized by skb_flow_set_gmres (the step itself allocates none of them)
-struct StepBuffers {
-    DevBuf items, r_new, tension, err, fext, force, torque;
-    PinnedHost check;
-    int size(int n_fibers, long long n_fib, int n_bodies);
-    bool sized_for(int n_fibers, long long n_fib, int n_bodies) const {
-        return n_fibers_ == n_fibers && n_fib_ == n_fib && n_bodies_ == n_bodies;
-    }
-
-  private:
-    int n_fibers_ = -1, n_bodies_ = -1;
-    long long n_fib_ = -1;
-    size_t check_cap_ = 0; // doubles of `check`
-};
-struct FlowState {
-    OwnFibers fibers;               // every fiber of the flow
-    const double *length = nullptr; // host: length_ of every fiber (skb_flow_set_fibers)
-    const double *positions = nullptr; // host: the positions of every fiber node
-    long long n_shell = 0;
-    int n_bodies = 0;
-    const double *centers = nullptr, *orientations = nullptr; // host: where skb_flow_place_bodies last placed them
-    bool placed = false; // the bodies were placed since skb_flow_set_bodies last changed them (or there are none)
-    FiberOps *ops = nullptr;
-    BodyOps *bodies = nullptr;
-    StepBuffers *buf = nullptr;
-};
-FlowState flow_state(skb_flow *fl); // (its device current)
-// the refusals of the whole-vector system calls that do not depend on what the step itself sets (fiber operators and
-// links): no group member, the whole target list, dn holding both periphery operators, bodies placed with an inverse
-int flow_step_checks(skb_flow *fl, skb_dense *dn, const char *who);
-// a group member (skb_flow_set_gmres): the fiber build's and the links' buffers for its own fibers at their final size
-// (FiberOps::size_build, BodyOps::size_links); else nothing
-int flow_size_group_step(skb_flow *fl);
-// the same for a group member's step (skb_flow_group_step_device): its peers connected, its rows laid out for its
-// target ranges, dn_spc / dn_minv its row blocks of the two periphery operators, bodies placed with an inverse; then
-// own = its fibers, *n its local solution size and *key its ranges (what skb_flow_set_gmres sized for)
-int flow_group_step_checks(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const char *who, OwnFibers &own,
-                           long long *n, std::array<long long, 6> *key);
-// R (row-major) of a unit quaternion (w, x, y, z): the formula of Eigen's QuaternionBase::toRotationMatrix
-void quaternion_rotation(const double *q, double *R);
-// the refusals of a solve's tol, num_blocks and max_iters (each caller checks its own eta)
-int solve_scalar_args(const char *who, double tol, int num_blocks, int max_iters);
-// ---- the time step (skb_step.cu), which skb_mflow_step drives on every member ----
-// the per-fiber arguments of a step (of the fibers it steps: a group member's own) and its scalars
-struct StepArgs {
-    const ::skb_fiber_params *params;
-    const double *v_growth, *force_scale;
-    const int *fiber_body;
-    const double *site_ref;
-    double dt, eta, tol;
-    int num_blocks, max_iters;
-};
-// what a step's refusals leave for its run: the fibers it steps, their items, bending rigidity and current nucleation
-// sites, and the (local) solution size
-struct StepCall {
-    OwnFibers own;
-    std::vector<StepItem> items;
-    std::vector<double> rigidity, sites;
-    long long n = 0;
-};
-// the refusals of the step's host arguments: the scalars; params, fiber_body and site_ref of nf fibers (the first is
-// fiber f0) against nb bodies; the external forces of n_fib fiber nodes and the forces and torques of nb bodies finite
-int step_scalar_args(const char *who, const ::skb_step_info *info, double dt, double eta, double tol, int num_blocks,
-                     int max_iters);
-int step_fiber_args(const char *who, const ::skb_fiber_params *params, const int *fiber_body, const double *site_ref,
-                    int f0, int nf, int nb);
-int step_host_inputs(const char *who, const double *f_external, long long n_fib, const double *body_forces_torques,
-                     int nb);
-// skb_flow_group_step_device in two halves (on a flow that is no member, such as a one-device skb_mflow's, those of
-// skb_flow_step).  group_step_checks: every refusal except the device inputs' finiteness, before any launch, with the
-// arguments of the member's own fibers.  group_step_run: the step itself, which meets the member's peers at flag
-// waits -- every member's checks must have passed first.  Inputs on the device as the
-// public call takes them; x_local / tension (host or device memory, NULL: not wanted) receive the member's local rows
-// of the solution and its own fibers' tensions, also when the step is not installed (SKB_ERR_STATE)
-int group_step_checks(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const StepArgs &a, ::skb_step_info *info,
-                      const char *who, StepCall &c);
-int group_step_run(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const StepArgs &a, StepCall &c,
-                   const double *d_f_external, const double *d_body_forces, const double *d_body_torques,
-                   double *x_local, double *tension, ::skb_step_info *info, const char *who, cudaStream_t st);
-
-// The whole-vector operator on one member of skb_mflow (the members of a group, or the single flow of a one-device
-// skb_mflow), after its target ranges are set.  The arguments are those of skb_flow_set_body_operators /
-// _set_fiber_links for ALL bodies / fibers; a member keeps the part its ranges own (BodyOps).  check_only: check the
-// links of every fiber and keep the earlier ones
-int flow_member_body_operators(skb_flow *fl, const int *n_nodes, int n_bodies, const double *node_weights,
-                               const double *ex, const double *ey, const double *ez, const double *A_inv);
-int flow_member_fiber_links(skb_flow *fl, const int *body, const double *site, const double *rigidity,
-                            bool check_only);
-// skb_mflow_set_body_frames / _place_bodies on a member (arguments of ALL bodies): the frames; the refusals of a
-// placement, with the rotations R (9 per body) it places at; the placement itself, after every member's refusals
-int flow_member_body_frames(skb_flow *fl, const int *n_nodes, int n_bodies, const double *pos_ref,
-                            const double *normal_ref, const double *node_weights, const double *ex0, const double *ey0,
-                            const double *ez0, const double *A_inv0);
-int flow_member_place_args(skb_flow *fl, const double *centers, const double *orientations, std::vector<double> &R);
-int flow_member_place(skb_flow *fl, const double *centers, const double *orientations, const std::vector<double> &R);
-// the state the system calls need (system_args without the dense operator): an error naming `who` unless it is there
-int flow_member_system_ready(skb_flow *fl, const char *who, bool precondition);
-int flow_size_system(skb_flow *fl); // sizes the buffers the two calls below use (before any member launches)
-// on st: x_fib 4 per own fiber node, x_shell 3 per own periphery row, x_bodies complete; res_fib / res_shell own rows,
-// res_bodies in the complete body layout, the owned rows written.  dn: the member's rows of
-// stresslet_plus_complementary (NULL without periphery rows)
-int flow_member_system_matvec(skb_flow *fl, skb_dense *dn, const double *d_x_fib, const double *d_x_shell,
-                              const double *d_x_bodies, double eta, double *d_res_fib, double *d_res_shell,
-                              double *d_res_bodies, cudaStream_t st);
-// the same layout, x_shell complete (3 per periphery node); dn: the member's rows of M_inv
-int flow_member_system_precondition(skb_flow *fl, skb_dense *dn, const double *d_x_fib, const double *d_x_shell,
-                                    const double *d_x_bodies, double *d_y_fib, double *d_y_shell, double *d_y_bodies,
-                                    cudaStream_t st);
-// The system RHS (skb_flow_build_system_rhs) on a member; params / v_growth / force_scale of ALL fibers.
-// flow_member_rhs_prepare, on the calling thread before any member launches: the refusals (the member's fibers and
-// bodies), the upload of the fiber block's per-fiber tables, and every buffer and kernel the call uses.
-// flow_member_system_rhs on st: d_fext 3 per own fiber node or NULL, d_f / d_t 3 per body (complete) or NULL; the
-// outputs as flow_member_system_matvec's
-int flow_member_rhs_prepare(skb_flow *fl, const ::skb_fiber_params *params, const double *v_growth,
-                            const double *force_scale, double dt, double eta);
-int flow_member_system_rhs(skb_flow *fl, const ::skb_fiber_params *params, const double *v_growth,
-                           const double *force_scale, const double *d_fext, const double *d_f, const double *d_t,
-                           double dt, double eta, double *d_rhs_fib, double *d_rhs_shell, double *d_rhs_bodies,
-                           cudaStream_t st);
 } // namespace skb
 
 // ---- context internals (shared by skb_runtime.cu and skb_matvec.cu) ----

@@ -3,9 +3,7 @@
 // (src/core/system.cpp:284-316).  Built on the pair-kernel contexts of skb_runtime.cu; everything between the
 // upload of the strengths and the download of the velocities stays on the device.
 #include "aux_kernels.cuh"
-#include "skb_internal.hpp"
-#include "../../include/skelly_b200_flow.h"
-#include "../../include/skelly_b200_dense.h"
+#include "skb_flow.hpp"
 
 #include <cmath>
 #include <cstdint>
@@ -20,114 +18,7 @@ namespace {
 // reference defaults of the regularised helpers (include/kernels.hpp:38-46): reg = 5e-3, eps = 1e-5
 constexpr double kReg = 5e-3;
 constexpr double kEps = 1e-5;
-
-struct TargetCache {
-    std::vector<double> host;
-    bool valid = false;
-    unsigned long long version = 0; // bumped by every upload: part of the CUDA-graph key (a replay bakes in whether
-                                    // the symmetric path -- targets start with the sources -- was taken)
-    bool same(const double *r, long long n) const {
-        return valid && (long long)host.size() == 3 * n && (n == 0 || std::memcmp(host.data(), r, (size_t)n * 24) == 0);
-    }
-    void store(const double *r, long long n) {
-        host.assign(r, r + 3 * n);
-        valid = true;
-        ++version;
-    }
-};
-using CtxPtr = std::unique_ptr<skb_ctx, Destroyer<skb_ctx_destroy>>;
 } // namespace
-
-struct skb_flow {
-    int dev = 0;
-    Stream stream;
-    Event ev0, ev1, evt0, evt1;
-    // geometry
-    long long n_fib = 0, n_shell = 0, n_body = 0;
-    int n_fibers = 0, n_bodies = 0, max_fiber_nodes = 0;
-    DevBuf fiber_offset, fiber_length, r_fib, r_shell, r_body, centers;
-    std::vector<double> h_r_fib, h_r_shell, h_r_body; // host copies to assemble the matvec target lists
-    // evaluators: [0] arbitrary targets, [1] matvec target lists
-    CtxPtr fib[2], shell[2], body[2];
-    TargetCache tc_fib, tc_shell, tc_body;
-    bool mv_dirty = true;
-    int cross_mode = -1;    // fiber <-> periphery cross kernel in the matvec: -1 auto, 0 off, 1 on whenever applicable
-    // how matvec_core evaluates, decided by prepare_matvec_targets
-    struct MatvecPlan {
-        bool grouped = false; // group member: the strengths come packed from the group window (push), not the caller
-        // producer of the fiber rows: the plain kernel; the symmetric kernel's complete rows (whole system on this
-        // device, cross kernel); or this member's symmetric partial sums, pulled together from all members' windows
-        enum FiberRows { kPlain, kSymComplete, kSymPartial } fib_rows = kPlain;
-        bool cross = false;   // fiber <-> periphery pairs through the cross kernel
-    } plan;
-    CrossState cross;
-    bool self_excl = false; // matvec: skip intra-fiber pairs in the kernels instead of compute-then-subtract (N3, opt-in)
-    long long win_begin = 0, win_end = -1; // target window of the matvec in [fibers|shell|bodies] rows; -1 = all
-    bool use_ranges = false;               // skb_flow_set_target_ranges instead of a contiguous window
-    long long rq_f0 = 0, rq_f1 = 0, rq_s0 = 0, rq_s1 = 0, rq_b0 = 0, rq_b1 = 0; // requested (fiber indices, rows)
-    // resolved pieces of the matvec target list: fiber rows [fa,fb), shell rows [sa,sb), body rows [ba,bb);
-    // the output has n_win = (fb-fa)+(sb-sa)+(bb-ba) rows in that order
-    long long fa = 0, fb = 0, sa = 0, sb = 0, ba = 0, bb = 0, n_win = 0;
-    cudaStream_t cur = nullptr;            // stream of the call in flight (own stream or the caller's)
-    int n_points = 0;
-    DevBuf pt_pos, pt_force, pt_torque;
-    bool has_background = false;
-    // CUDA-graph replay of the launch-bound small-size calls (BASELINE C1, listener / streamline path)
-    struct GraphSlot {
-        GraphExec exec;
-        unsigned long long key = 0, seen = 0;
-        int launches = 0;
-        long long pairs = 0;
-        void reset() {
-            exec.reset();
-            key = seen = 0;
-        }
-    } g_matvec, g_vat;
-    unsigned long long geom_version = 1;
-    bool graphs_enabled = true;
-    PinnedHost h_stage; // pinned staging: the graph's memcpy nodes need fixed host addresses
-    size_t h_stage_cap = 0;
-    int bg_comp[3] = {0, 1, 2};
-    double bg_scale[3] = {0, 0, 0}, bg_uniform[3] = {0, 0, 0};
-    std::vector<int> h_fiber_n;         // nodes of every fiber
-    std::vector<long long> h_fiber_off; // first node of every fiber (n_fibers + 1)
-    FiberOps ops; // per-fiber dense operators of the fibers whose rows are in the target list (skb_fiber.cu)
-    BodyOps bodies; // the bodies' operators and the fiber-body links of the whole-vector operator (skb_body.cu)
-    std::vector<double> h_centers; // body centres (set_fiber_links measures the nucleation sites from them)
-    std::vector<double> h_fiber_len; // length_ of every fiber (the time step installs its new positions with them)
-    std::vector<double> h_orient;    // the quaternions of the last skb_flow_place_bodies (4 per body) ...
-    bool placed = false;             // ... valid until skb_flow_set_bodies changes the bodies otherwise
-    StepBuffers stepbuf;             // the buffers of skb_flow_step (skb_step.cu)
-    Group grp; // multi-GPU group membership: one member per GPU, exchange through peer memory (skb_group.cu)
-    // a member's whole-vector matvec in flight: matvec_core exchanges the bodies' partial link forces through the
-    // window and the body flow reads their totals from ft_sum ([F | L], 6 per body)
-    bool ft_exchange = false;
-    DevBuf ft_sum;
-    // a rank-per-GPU member's whole-vector matvec has begun the epoch (and exchanged its body rows in it): matvec_core
-    // runs its protocol in that epoch instead of beginning one
-    bool grp_open = false;
-    DevBuf sys_rb; // a member's body output in the whole body layout (skb_flow_group_*), compacted to its own rows
-    // Periphery::matvec's dense operator beside the pair kernels (stream_kernels.cuh): forked onto bg_stream once its
-    // input (the complete x_shell) is there, joined before res_shell is assembled
-    struct Overlap {
-        bool enabled = true;       // skb_flow_set_overlap
-        Stream stream;
-        Event fork, join;
-        DevBuf y;                  // A x of the own periphery rows
-        skb_dense *dn = nullptr;   // pending background product of the call in flight (nullptr: none)
-        bool launched = false;
-    } bg;
-    DevBuf scratch_u; // group mode: landing zone of eval_on_device's default output (never read)
-    // staging
-    DevBuf in_fib, in_shell, in_body, in_force, in_torque, vel, tmp, x_fib, res_fib, vb, res_shell, tmp_b;
-    DevBuf sys_x, sys_y; // the whole solution vector in and out of the host forms of the system operator
-    DevBuf zeros;        // the system RHS: the zero densities (and absent forces) its flow takes, n_zeros doubles
-    long long n_zeros = 0;
-    Krylov kry; // the workspace of skb_flow_solve_system (skb_solve.cu)
-    skb_flow_stats stats{};
-    int launches = 0;
-    long long pairs = 0;
-};
 
 static int create_ctx(int dev, CtxPtr &slot) {
     skb_ctx *ctx = nullptr;
@@ -226,10 +117,7 @@ static int bodies_dev(skb_flow *fl, skb_ctx *ctx, const double *d_density, const
     return launched(fl, 1);
 }
 
-// + psc.flow(r_trg, eta, time) + bs.flow(r_trg, eta) (system.cpp:358-359, 445-446) on st: the point sources of
-// skb_flow_set_point_sources and the background flow of skb_flow_set_background at the n_trg targets d_trg, added to
-// the rows of d_v in this order: Oseen contraction, rotlet, background
-static int add_sources(skb_flow *fl, const double *d_trg, long long n_trg, double eta, double *d_v, cudaStream_t st) {
+int skb::add_sources(skb_flow *fl, const double *d_trg, long long n_trg, double eta, double *d_v, cudaStream_t st) {
     const int bs = 128;
     const unsigned nblk = (unsigned)((n_trg + bs - 1) / bs);
     if (n_trg == 0)
@@ -252,14 +140,22 @@ static int add_sources(skb_flow *fl, const double *d_trg, long long n_trg, doubl
     return SKB_OK;
 }
 
-static int upload(skb_flow *fl, DevBuf &buf, const double *h, size_t n_doubles) {
+int skb::load_source_kernels() {
+    cudaFuncAttributes fa;
+    CUDA_TRY(cudaFuncGetAttributes(&fa, oseen_contract_add_kernel));
+    CUDA_TRY(cudaFuncGetAttributes(&fa, rotlet_add_kernel));
+    CUDA_TRY(cudaFuncGetAttributes(&fa, background_add_kernel));
+    return SKB_OK;
+}
+
+int skb::upload(skb_flow *fl, DevBuf &buf, const double *h, size_t n_doubles) {
     if (n_doubles == 0)
         return SKB_OK;
     SKB_TRY(buf.ensure(n_doubles * 8));
     CUDA_TRY(cudaMemcpyAsync(buf.ptr, h, n_doubles * 8, cudaMemcpyHostToDevice, fl->stream));
     return SKB_OK;
 }
-static int download(skb_flow *fl, double *h, const DevBuf &buf, size_t n_doubles) {
+int skb::download(skb_flow *fl, double *h, const DevBuf &buf, size_t n_doubles) {
     if (n_doubles > 0)
         CUDA_TRY(cudaMemcpyAsync(h, buf.ptr, n_doubles * 8, cudaMemcpyDeviceToHost, fl->stream));
     return SKB_OK;
@@ -271,16 +167,6 @@ static int set_targets_cached(skb_ctx *ctx, TargetCache &tc, const double *r_trg
     SKB_TRY(skb_set_targets(ctx, r_trg, n_trg));
     tc.store(r_trg, n_trg);
     return SKB_OK;
-}
-
-void skb::split_forces_torques(const double *ft, int n_bodies, std::vector<double> &f, std::vector<double> &t) {
-    f.resize(3 * (size_t)n_bodies);
-    t.resize(3 * (size_t)n_bodies);
-    for (int b = 0; b < n_bodies; ++b)
-        for (int k = 0; k < 3; ++k) {
-            f[3 * b + k] = ft[6 * b + k];     // forces_torques.block(0,0,3,n)  body_container.cpp:134
-            t[3 * b + k] = ft[6 * b + 3 + k]; // forces_torques.block(3,0,3,n)
-        }
 }
 
 
@@ -396,11 +282,11 @@ template <class Body> static int run_graphed(skb_flow *fl, skb_flow::GraphSlot &
     return body();
 }
 
-static void begin_stats(skb_flow *fl) {
+void skb::begin_stats(skb_flow *fl) {
     fl->launches = 0;
     fl->pairs = 0;
 }
-static int finish_stats(skb_flow *fl) {
+int skb::finish_stats(skb_flow *fl) {
     CUDA_TRY(cudaStreamSynchronize(fl->stream));
     float a = 0, b = 0;
     cudaEventElapsedTime(&a, fl->ev0, fl->ev1);
@@ -412,23 +298,9 @@ static int finish_stats(skb_flow *fl) {
     return SKB_OK;
 }
 
-// frame of the host-pointer entry points on fl->stream: device_ms spans the device work, total_ms also the uploads
-// before it and the downloads after it; returns once the downloads have landed
-template <class Up, class Work, class Down> static int host_frame(skb_flow *fl, Up up, Work work, Down down) {
-    fl->cur = fl->stream;
-    CUDA_TRY(cudaEventRecord(fl->evt0, fl->stream));
-    SKB_TRY(up());
-    CUDA_TRY(cudaEventRecord(fl->ev0, fl->stream));
-    SKB_TRY(work());
-    CUDA_TRY(cudaEventRecord(fl->ev1, fl->stream));
-    SKB_TRY(down());
-    CUDA_TRY(cudaEventRecord(fl->evt1, fl->stream));
-    return finish_stats(fl);
-}
 static int nothing() { return SKB_OK; }
 
-// the device-pointer entry points run asynchronously on the caller's stream: no timings
-static int device_stats(skb_flow *fl) {
+int skb::device_stats(skb_flow *fl) {
     fl->stats.device_ms = fl->stats.total_ms = 0;
     fl->stats.n_pairs = fl->pairs;
     fl->stats.launches = fl->launches;
@@ -755,8 +627,9 @@ int skb_flow_velocity_at_targets(skb_flow *fl, const double *r_trg, int64_t n_tr
     return SKB_OK;
 }
 
-// resolve the target window / ranges into fiber, shell and body pieces and (re)build the matvec target lists
-static int prepare_matvec_targets(skb_flow *fl) {
+} // extern "C"
+
+int skb::prepare_matvec_targets(skb_flow *fl) {
     const long long nf = fl->n_fib, ns = fl->n_shell, nb = fl->n_body, n_all = nf + ns + nb;
     if (!fl->mv_dirty)
         return SKB_OK;
@@ -862,7 +735,7 @@ static int prepare_matvec_targets(skb_flow *fl) {
 // The pending dense product of apply_matvec_core goes out on the side stream, ordered after everything on fl->cur so far
 // (its input is complete), and runs beside whatever fl->cur launches next.  The side stream has the highest priority:
 // its one-warp CTAs (one per SM) are placed before the pair kernel's CTAs fill the SMs.
-static int overlap_buffers(skb_flow *fl, long long n_rows) {
+int skb::overlap_buffers(skb_flow *fl, long long n_rows) {
     skb_flow::Overlap &B = fl->bg;
     if (!B.stream) {
         int lo = 0, hi = 0;
@@ -981,11 +854,8 @@ static int periphery_rows(skb_flow *fl, StrengthMode mode, const double *sd, dou
     return SKB_OK;
 }
 
-// device-side matvec flow on fl->cur, as fl->plan says: d_ff / d_sd are the strengths of the own fibers / periphery
-// rows (all of them without a group), body inputs are complete; d_v = [own fiber rows | own shell rows | own body rows]
-// of v_all
-static int matvec_core(skb_flow *fl, const double *d_ff, const double *d_sd, const double *d_bd, const double *d_f,
-                       const double *d_t, double eta, double *d_v) {
+int skb::matvec_core(skb_flow *fl, const double *d_ff, const double *d_sd, const double *d_bd, const double *d_f,
+                     const double *d_t, double eta, double *d_v) {
     const skb_flow::MatvecPlan &P = fl->plan;
     Group &G = fl->grp;
     const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
@@ -1048,6 +918,8 @@ static int matvec_core(skb_flow *fl, const double *d_ff, const double *d_sd, con
     return SKB_OK;
 }
 
+extern "C" {
+
 // ---- group membership (multi-GPU through peer memory, skb_group.cu) ----------------------------------------------
 int skb_flow_group_init(skb_flow *fl, int rank, int size) {
     if (!fl || size < 1 || size > kMaxGroup || rank < 0 || rank >= size)
@@ -1105,8 +977,8 @@ int skb_flow_group_warmup(skb_flow *fl) {
     CUDA_TRY(cudaMemsetAsync(z.ptr, 0, n_z * 8, fl->stream));
     SKB_TRY(fl->vel.ensure((size_t)fl->n_win * 24 + 8));
     SKB_TRY(fl->in_fib.ensure((size_t)n_fw * 24 + 8));
-    if (n_sw > 0)
-        SKB_TRY(flow_size_overlap(fl, 3 * n_sw));
+    if (n_sw > 0 && fl->bg.enabled)
+        SKB_TRY(overlap_buffers(fl, 3 * n_sw));
     fl->cur = fl->stream;
     fl->grp.set_solo(true);
     const double *zp = (const double *)z.ptr;
@@ -1287,9 +1159,9 @@ int skb_flow_set_fiber_class_derivatives(skb_flow *fl, int n_nodes, const double
     return fl->ops.set_class_derivatives(n_nodes, D_2_0, D_3_0, D_4_0, fl->stream);
 }
 
-// The fibers whose operators are resident: those whose rows are in this flow's target list -- all of them, or the
-// rank's own fibers under skb_flow_set_target_ranges / an aligned skb_flow_set_target_window.
-static int own_fibers(skb_flow *fl, const char *who, OwnFibers &own) {
+} // extern "C"
+
+int skb::own_fibers(skb_flow *fl, const char *who, OwnFibers &own) {
     SKB_TRY(prepare_matvec_targets(fl));
     int f0 = 0, f1 = 0;
     if (fl->n_fibers > 0) {
@@ -1304,6 +1176,8 @@ static int own_fibers(skb_flow *fl, const char *who, OwnFibers &own) {
                     (const double *)fl->fiber_length.ptr, fl->stream};
     return SKB_OK;
 }
+
+extern "C" {
 
 int skb_flow_set_fiber_operators(skb_flow *fl, const double *A, const double *force_operator, const double *xs,
                                  const double *length_prev, const int *plus_bc_velocity) {
@@ -1484,13 +1358,9 @@ int skb_flow_fiber_matvec_device(skb_flow *fl, const double *d_x_fibers, const d
 
 } // extern "C"
 
-// System::apply_matvec (system.cpp:298-319) on fl->cur, everything device resident.  Inputs are the OWN slices of a
-// group member (all of them without a group): d_x 4 per own fiber node, d_xs 3 per own periphery row, body inputs
-// complete, d_link 7 per own fiber or NULL.  Outputs: d_res_fib 4 per own node, d_out_shell 3 per own periphery row
-// (res_shell when dn != NULL, else v_shell), d_v_bodies 3 per own body row; any of them may be NULL when empty.
-static int apply_matvec_core(skb_flow *fl, skb_dense *dn, const double *d_x, const double *d_xs, const double *d_bd,
-                             const double *d_f, const double *d_t, const double *d_link, double eta, double *d_res_fib,
-                             double *d_out_shell, double *d_v_bodies) {
+int skb::apply_matvec_core(skb_flow *fl, skb_dense *dn, const double *d_x, const double *d_xs, const double *d_bd,
+                           const double *d_f, const double *d_t, const double *d_link, double eta, double *d_res_fib,
+                           double *d_out_shell, double *d_v_bodies) {
     const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa, n_bw = fl->bb - fl->ba;
     SKB_TRY(fl->in_fib.ensure((size_t)n_fw * 24 + 8));
     SKB_TRY(fl->vel.ensure((size_t)fl->n_win * 24 + 8));
@@ -1533,22 +1403,6 @@ static int apply_matvec_core(skb_flow *fl, skb_dense *dn, const double *d_x, con
     if (n_bw > 0 && d_v_bodies)
         CUDA_TRY(cudaMemcpyAsync(d_v_bodies, (const double *)fl->vel.ptr + 3 * (n_fw + n_sw), (size_t)n_bw * 24,
                                  cudaMemcpyDeviceToDevice, fl->cur));
-    return SKB_OK;
-}
-
-static int check_dense_handle(skb_flow *fl, skb_dense *dn, const char *who) {
-    int dn_dev = -1;
-    SKB_TRY(skb_dense_device(dn, 0, &dn_dev));
-    if (fl->dev != dn_dev)
-        return set_error(SKB_ERR_INVALID, "%s: the flow is on device %d, the dense handle on device %d", who, fl->dev,
-                         dn_dev);
-    SKB_TRY(prepare_matvec_targets(fl));
-    int64_t rows = 0, cols = 0;
-    SKB_TRY(skb_dense_shape(dn, SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY, &rows, &cols));
-    const long long want_rows = 3 * (fl->sb - fl->sa);
-    if (rows != want_rows || cols != 3 * fl->n_shell)
-        return set_error(SKB_ERR_INVALID, "%s: stresslet_plus_complementary is %lld x %lld, need the %lld own rows x %lld",
-                         who, (long long)rows, (long long)cols, want_rows, 3 * fl->n_shell);
     return SKB_OK;
 }
 
@@ -1622,7 +1476,7 @@ int skb_flow_apply_matvec_dense(skb_flow *fl, skb_dense *dn, const double *x_fib
                                 double *res_shell, double *v_bodies) {
     if (!fl || !dn)
         return set_error(SKB_ERR_INVALID, "skb_flow_apply_matvec_dense: NULL handle");
-    SKB_TRY(check_dense_handle(fl, dn, "skb_flow_apply_matvec_dense"));
+    SKB_TRY(dense_rows(fl, dn, "skb_flow_apply_matvec_dense", false));
     return apply_matvec_impl(fl, dn, x_fibers, x_shell, body_densities, body_forces_torques, fiber_link_conditions,
                              eta, res_fibers, res_shell, v_bodies);
 }
@@ -1639,7 +1493,7 @@ int skb_flow_apply_matvec_device(skb_flow *fl, skb_dense *dn, const double *d_x_
     begin_stats(fl);
     SKB_TRY(prepare_matvec_targets(fl));
     if (dn)
-        SKB_TRY(check_dense_handle(fl, dn, "skb_flow_apply_matvec_device"));
+        SKB_TRY(dense_rows(fl, dn, "skb_flow_apply_matvec_device", false));
     const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa, n_bw = fl->bb - fl->ba;
     if ((n_fw > 0 && (!d_x_fibers || !d_res_fibers)) || (n_sw > 0 && (!d_x_shell || !d_out_shell)) ||
         (fl->n_body > 0 && !d_body_densities) || (n_bw > 0 && !d_v_bodies) ||
@@ -1671,1025 +1525,3 @@ int skb_flow_last_stats(const skb_flow *fl, skb_flow_stats *out) {
 }
 
 } // extern "C"
-
-// ---- the whole-vector operator and preconditioner with the bodies on the device (skb_body.cu) -------------------
-// The solution vector is [fibers (4 per node) | shell (3 per node) | bodies (3 n_b + 6 each)] (get_solution_maps,
-// system.cpp:69-92); single device, whole target list.
-
-extern "C" {
-
-int skb_flow_set_body_operators(skb_flow *fl, const int *n_nodes, int n_bodies, const double *node_weights,
-                                const double *ex, const double *ey, const double *ez, const double *A_inv) {
-    const char *who = "skb_flow_set_body_operators";
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    if (fl->grp.member())
-        return set_error(SKB_ERR_INVALID, "%s: the body block runs on a single device, not in a group", who);
-    if (n_bodies != fl->n_bodies)
-        return set_error(SKB_ERR_INVALID, "%s: %d bodies, skb_flow_set_bodies has %d", who, n_bodies, fl->n_bodies);
-    if (n_bodies > 0 && (!n_nodes || !node_weights || !ex || !ey || !ez))
-        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    return fl->bodies.set_operators(n_nodes, n_bodies, fl->n_body, fl->h_r_body.data(), fl->h_centers.data(),
-                                    node_weights, ex, ey, ez, A_inv, fl->stream);
-}
-
-int skb_flow_set_fiber_links(skb_flow *fl, const int *body, const double *site, const double *bending_rigidity) {
-    const char *who = "skb_flow_set_fiber_links";
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    if (fl->grp.member())
-        return set_error(SKB_ERR_INVALID, "%s: the body block runs on a single device, not in a group", who);
-    if (body && fl->n_fibers > 0 && (!site || !bending_rigidity))
-        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    const OwnFibers all{0, fl->n_fibers, fl->h_fiber_n.data(), fl->h_fiber_off.data(), (const double *)fl->r_fib.ptr,
-                        (const double *)fl->fiber_length.ptr, fl->stream};
-    return fl->bodies.set_links(all, fl->ops, fl->n_bodies, fl->h_centers.data(), body, site, bending_rigidity,
-                                fl->stream);
-}
-
-} // extern "C"
-
-// ---- rigid bodies placed from their body frame (BodyOps::set_frames / ::place, DESIGN.md §3.6) --------------------
-
-void skb::quaternion_rotation(const double *q, double *R) {
-    const double w = q[0], x = q[1], y = q[2], z = q[3];
-    const double tx = 2.0 * x, ty = 2.0 * y, tz = 2.0 * z;
-    const double twx = tx * w, twy = ty * w, twz = tz * w;
-    const double txx = tx * x, txy = ty * x, txz = tz * x;
-    const double tyy = ty * y, tyz = tz * y, tzz = tz * z;
-    R[0] = 1.0 - (tyy + tzz), R[1] = txy - twz, R[2] = txz + twy;
-    R[3] = txy + twz, R[4] = 1.0 - (txx + tzz), R[5] = tyz - twx;
-    R[6] = txz - twy, R[7] = tyz + twx, R[8] = 1.0 - (txx + tyy);
-}
-
-// the frames of the flow's bodies, for its body rows [lo, hi) (hi < 0: every row)
-static int body_frames(skb_flow *fl, const char *who, const int *n_nodes, int n_bodies, const double *pos_ref,
-                       const double *normal_ref, const double *node_weights, const double *ex0, const double *ey0,
-                       const double *ez0, const double *A_inv0, long long lo, long long hi) {
-    if (n_bodies != fl->n_bodies)
-        return set_error(SKB_ERR_INVALID, "%s: %d bodies, skb_flow_set_bodies has %d", who, n_bodies, fl->n_bodies);
-    if (n_bodies > 0 && (!n_nodes || !pos_ref || !normal_ref || !node_weights || !ex0 || !ey0 || !ez0))
-        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    return fl->bodies.set_frames(n_nodes, n_bodies, fl->n_body, pos_ref, normal_ref, node_weights, ex0, ey0, ez0,
-                                 A_inv0, fl->stream, lo, hi);
-}
-
-// the refusals of a placement, before any state changes: frames that match the flow's bodies and its body rows
-// [lo, hi), finite unit quaternions.  R: the rotations, 9 per body
-static int placement_args(skb_flow *fl, const char *who, const double *centers, const double *orientations,
-                          long long lo, long long hi, std::vector<double> &R) {
-    const BodyOps &b = fl->bodies;
-    if (!b.has_frames())
-        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_body_frames first", who);
-    if (b.frame_bodies() != fl->n_bodies || b.frame_nodes() != fl->n_body)
-        return set_error(SKB_ERR_INVALID, "%s: the flow has %d bodies of %lld nodes, the frames %d bodies of %lld nodes "
-                                          "(set the frames again after skb_flow_set_bodies changes them)", who,
-                         fl->n_bodies, fl->n_body, b.frame_bodies(), b.frame_nodes());
-    if (!b.frame_window(lo, hi))
-        return set_error(SKB_ERR_INVALID, "%s: the body rows changed since the frames were set (set them again)", who);
-    const int nb = fl->n_bodies;
-    if (nb > 0 && (!centers || !orientations))
-        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
-    R.resize((size_t)nb * 9);
-    for (int i = 0; i < nb; ++i) {
-        const double *q = orientations + 4 * (size_t)i;
-        const double n2 = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
-        if (!(std::fabs(n2 - 1.0) <= SKB_UNIT_QUATERNION_TOL))
-            return set_error(SKB_ERR_INVALID, "%s: orientation %d = (%g, %g, %g, %g) is not a finite unit quaternion "
-                                              "(|q|^2 - 1 = %g, tolerance %g)", who, i, q[0], q[1], q[2], q[3],
-                             n2 - 1.0, SKB_UNIT_QUATERNION_TOL);
-        quaternion_rotation(q, &R[9 * (size_t)i]);
-    }
-    return SKB_OK;
-}
-
-// after placement_args: the nodes and normals through skb_flow_set_bodies (which drops the operators and the links),
-// then the operators from the frames
-static int place_bodies(skb_flow *fl, const double *centers, const double *orientations, const std::vector<double> &R) {
-    std::vector<double> pos, nrm;
-    fl->bodies.placed_geometry(R.data(), centers, pos, nrm);
-    SKB_TRY(skb_flow_set_bodies(fl, pos.data(), nrm.data(), fl->n_body, centers, fl->n_bodies));
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    SKB_TRY(fl->bodies.place(R.data(), fl->h_r_body.data(), fl->h_centers.data(), fl->stream));
-    fl->h_orient.assign(orientations, orientations + 4 * (size_t)fl->n_bodies);
-    fl->placed = true;
-    return SKB_OK;
-}
-
-int skb::flow_member_body_frames(skb_flow *fl, const int *n_nodes, int n_bodies, const double *pos_ref,
-                                 const double *normal_ref, const double *node_weights, const double *ex0,
-                                 const double *ey0, const double *ez0, const double *A_inv0) {
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    SKB_TRY(prepare_matvec_targets(fl));
-    const bool member = fl->grp.member();
-    return body_frames(fl, "skb_mflow_set_body_frames", n_nodes, n_bodies, pos_ref, normal_ref, node_weights, ex0,
-                       ey0, ez0, A_inv0, member ? fl->ba : 0, member ? fl->bb : -1);
-}
-
-int skb::flow_member_place_args(skb_flow *fl, const double *centers, const double *orientations,
-                                std::vector<double> &R) {
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    SKB_TRY(prepare_matvec_targets(fl));
-    const bool member = fl->grp.member();
-    return placement_args(fl, "skb_mflow_place_bodies", centers, orientations, member ? fl->ba : 0,
-                          member ? fl->bb : -1, R);
-}
-
-int skb::flow_member_place(skb_flow *fl, const double *centers, const double *orientations,
-                           const std::vector<double> &R) {
-    return place_bodies(fl, centers, orientations, R);
-}
-
-extern "C" {
-
-int skb_flow_set_body_frames(skb_flow *fl, const int *n_nodes, int n_bodies, const double *node_pos_ref,
-                             const double *node_normal_ref, const double *node_weights, const double *ex0,
-                             const double *ey0, const double *ez0, const double *A_inv0) {
-    const char *who = "skb_flow_set_body_frames";
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    if (fl->grp.member())
-        return set_error(SKB_ERR_INVALID, "%s: a group member sets its frames with skb_flow_group_set_body_frames", who);
-    return body_frames(fl, who, n_nodes, n_bodies, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0, A_inv0,
-                       0, -1);
-}
-
-int skb_flow_place_bodies(skb_flow *fl, const double *centers, const double *orientations) {
-    const char *who = "skb_flow_place_bodies";
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    if (fl->grp.member())
-        return set_error(SKB_ERR_INVALID, "%s: a group member places its bodies with skb_flow_group_place_bodies", who);
-    std::vector<double> R;
-    SKB_TRY(placement_args(fl, who, centers, orientations, 0, -1, R));
-    return place_bodies(fl, centers, orientations, R);
-}
-
-int skb_flow_get_body_operators(skb_flow *fl, double *ex, double *ey, double *ez, double *A_inv) {
-    const char *who = "skb_flow_get_body_operators";
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    if (fl->n_bodies > 0 && !fl->bodies.has_operators())
-        return set_error(SKB_ERR_INVALID, "%s: no body operators are resident (skb_flow_set_body_operators or "
-                                          "skb_flow_place_bodies after skb_flow_set_bodies)", who);
-    if (fl->n_bodies > 0 && A_inv && !fl->bodies.has_inverse())
-        return set_error(SKB_ERR_INVALID, "%s: the resident body operators have no A_inv", who);
-    if (fl->n_bodies == 0)
-        return SKB_OK;
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    return fl->bodies.read(ex, ey, ez, A_inv, fl->stream);
-}
-
-} // extern "C"
-
-// dn holds the periphery's operator of the system call (matvec: stresslet_plus_complementary; precondition: M_inv)
-static int dense_args(skb_flow *fl, skb_dense *dn, const char *who, bool precondition) {
-    if (!dn)
-        return set_error(SKB_ERR_INVALID, "%s: the periphery needs its dense operator (dn == NULL)", who);
-    const int op = precondition ? SKB_DENSE_M_INV : SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY;
-    int dn_dev = -1;
-    int64_t rows = 0, cols = 0;
-    SKB_TRY(skb_dense_device(dn, 0, &dn_dev));
-    SKB_TRY(skb_dense_shape(dn, op, &rows, &cols));
-    if (dn_dev != fl->dev || rows != 3 * fl->n_shell || cols != 3 * fl->n_shell)
-        return set_error(SKB_ERR_INVALID, "%s: the dense handle holds a %lld x %lld %s on device %d, need %lld x %lld "
-                                          "on device %d", who, (long long)rows, (long long)cols,
-                         precondition ? "M_inv" : "stresslet_plus_complementary", dn_dev, 3 * fl->n_shell,
-                         3 * fl->n_shell, fl->dev);
-    return SKB_OK;
-}
-
-// The checks of the system operator (matvec: stresslet_plus_complementary in dn; precondition: M_inv and the
-// inverses), all before any launch; then the flow's device is current and its target list resolved.
-static int system_args(skb_flow *fl, skb_dense *dn, const char *who, bool precondition, bool args) {
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    if (fl->grp.member())
-        return set_error(SKB_ERR_INVALID, "%s: multi-GPU is not supported: a body's K^T lambda needs all of its nodes "
-                                          "(the reference keeps the bodies on rank 0); use a single-device flow", who);
-    if (fl->n_fibers > 0) // no fibers: the empty operator set, uploaded or not
-        SKB_TRY(fl->ops.ready(who, precondition));
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    SKB_TRY(prepare_matvec_targets(fl));
-    const long long n_all = fl->n_fib + fl->n_shell + fl->n_body;
-    if (fl->n_win != n_all)
-        return set_error(SKB_ERR_INVALID, "%s: needs the whole target list (%lld of %lld rows are set by a target window "
-                                          "or ranges); multi-GPU is not supported", who, fl->n_win, n_all);
-    if (fl->n_shell > 0)
-        SKB_TRY(dense_args(fl, dn, who, precondition));
-    if (fl->n_bodies > 0) {
-        if (!fl->bodies.has_operators())
-            return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_body_operators after skb_flow_set_bodies", who);
-        if (precondition && !fl->bodies.has_inverse())
-            return set_error(SKB_ERR_INVALID, "%s: skb_flow_set_body_operators was given no A_inv", who);
-        if (!precondition && fl->n_fibers > 0 && !fl->bodies.has_links())
-            return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_fiber_links after skb_flow_set_fibers / "
-                                              "skb_flow_set_bodies (NULL body: no fiber is bound)", who);
-    }
-    if (!args)
-        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
-    begin_stats(fl);
-    return SKB_OK;
-}
-
-static long long solution_size(const skb_flow *fl) {
-    return 4 * fl->n_fib + 3 * fl->n_shell + (fl->n_bodies > 0 ? fl->bodies.solution_size() : 0);
-}
-
-// System::apply_matvec (system.cpp:269-324) on fl->cur: the links, forces / torques and densities of the bodies from
-// x, then apply_matvec_core unchanged, then bc.matvec on its v_bodies rows
-static int system_matvec_core(skb_flow *fl, skb_dense *dn, const double *d_x, double eta, double *d_res) {
-    const long long nf = fl->n_fib, ns = fl->n_shell;
-    const double *x_fib = d_x, *x_shell = d_x + 4 * nf, *x_bodies = x_shell + 3 * ns;
-    double *res_fib = d_res, *res_shell = d_res + 4 * nf, *res_bodies = res_shell + 3 * ns;
-    const double *link = nullptr, *bd = nullptr, *f = nullptr, *t = nullptr;
-    if (fl->n_bodies > 0) { // fc.calculate_link_conditions (system.cpp:311), the densities out of x_bodies
-        SKB_TRY(fl->bodies.links(fl->ops, (const double *)fl->fiber_length.ptr, x_fib, x_bodies, &link, fl->cur,
-                                 &fl->launches));
-        bd = fl->bodies.densities();
-        f = fl->bodies.forces();
-        t = fl->bodies.torques();
-    }
-    SKB_TRY(fl->tmp_b.ensure((size_t)fl->n_body * 24 + 8));
-    double *v_bodies = (double *)fl->tmp_b.ptr;
-    SKB_TRY(apply_matvec_core(fl, dn, x_fib, x_shell, bd, f, t, link, eta, res_fib, res_shell, v_bodies));
-    // res_bodies = bc.matvec(v_bodies, x_bodies)                          system.cpp:320
-    return fl->n_bodies > 0 ? fl->bodies.matvec(x_bodies, v_bodies, res_bodies, fl->cur, &fl->launches) : SKB_OK;
-}
-
-// System::apply_preconditioner (system.cpp:248-262) on fl->cur
-static int system_precondition_core(skb_flow *fl, skb_dense *dn, const double *d_x, double *d_y) {
-    const long long nf = fl->n_fib, ns = fl->n_shell;
-    SKB_TRY(fl->ops.precondition(d_x, d_y, fl->cur, &fl->launches));
-    if (ns > 0) {
-        SKB_TRY(skb_dense_apply_device(dn, SKB_DENSE_M_INV, d_x + 4 * nf, nullptr, d_y + 4 * nf, fl->cur));
-        fl->launches += 1;
-    }
-    return fl->n_bodies > 0
-               ? fl->bodies.precondition(d_x + 4 * nf + 3 * ns, d_y + 4 * nf + 3 * ns, fl->cur, &fl->launches)
-               : SKB_OK;
-}
-
-extern "C" {
-
-int skb_flow_apply_system_matvec(skb_flow *fl, skb_dense *dn, const double *x, double eta, double *res) {
-    const char *who = "skb_flow_apply_system_matvec";
-    SKB_TRY(system_args(fl, dn, who, false, (x && res) || solution_size(fl) == 0));
-    if (!(eta > 0))
-        return set_error(SKB_ERR_INVALID, "%s: eta = %g", who, eta);
-    const size_t n = (size_t)solution_size(fl);
-    if (n == 0)
-        return SKB_OK;
-    SKB_TRY(fl->sys_x.ensure(n * 8));
-    SKB_TRY(fl->sys_y.ensure(n * 8));
-    return host_frame(
-        fl, [&] { return upload(fl, fl->sys_x, x, n); },
-        [&] { return system_matvec_core(fl, dn, (const double *)fl->sys_x.ptr, eta, (double *)fl->sys_y.ptr); },
-        [&] { return download(fl, res, fl->sys_y, n); });
-}
-
-int skb_flow_apply_system_matvec_device(skb_flow *fl, skb_dense *dn, const double *d_x, double eta, double *d_res,
-                                        void *stream) {
-    const char *who = "skb_flow_apply_system_matvec_device";
-    SKB_TRY(system_args(fl, dn, who, false, (d_x && d_res) || solution_size(fl) == 0));
-    if (!(eta > 0))
-        return set_error(SKB_ERR_INVALID, "%s: eta = %g", who, eta);
-    if (solution_size(fl) == 0)
-        return SKB_OK;
-    fl->cur = (cudaStream_t)stream;
-    SKB_TRY(system_matvec_core(fl, dn, d_x, eta, d_res));
-    return device_stats(fl);
-}
-
-int skb_flow_apply_system_preconditioner(skb_flow *fl, skb_dense *dn, const double *x, double *y) {
-    const char *who = "skb_flow_apply_system_preconditioner";
-    SKB_TRY(system_args(fl, dn, who, true, (x && y) || solution_size(fl) == 0));
-    const size_t n = (size_t)solution_size(fl);
-    if (n == 0)
-        return SKB_OK;
-    SKB_TRY(fl->sys_x.ensure(n * 8));
-    SKB_TRY(fl->sys_y.ensure(n * 8));
-    return host_frame(
-        fl, [&] { return upload(fl, fl->sys_x, x, n); },
-        [&] { return system_precondition_core(fl, dn, (const double *)fl->sys_x.ptr, (double *)fl->sys_y.ptr); },
-        [&] { return download(fl, y, fl->sys_y, n); });
-}
-
-int skb_flow_apply_system_preconditioner_device(skb_flow *fl, skb_dense *dn, const double *d_x, double *d_y,
-                                                void *stream) {
-    const char *who = "skb_flow_apply_system_preconditioner_device";
-    SKB_TRY(system_args(fl, dn, who, true, (d_x && d_y) || solution_size(fl) == 0));
-    if (solution_size(fl) == 0)
-        return SKB_OK;
-    fl->cur = (cudaStream_t)stream;
-    SKB_TRY(system_precondition_core(fl, dn, d_x, d_y));
-    return device_stats(fl);
-}
-
-} // extern "C"
-
-// ---- the right-hand side of the whole system (System::prep_state_for_solver, system.cpp:398-458) --------------------
-// One device call from the external forces to the RHS vector [fibers | shell | bodies], laid out as Solver::set_RHS
-// copies it (solver_hydro.cpp:51-61).  Its flow is matvec_core unchanged -- f_ext as the fiber strengths, zero periphery
-// and body densities, the bodies' external F_T -- so that the symmetric and cross kernels, the self term and, in a
-// group, the exchange through the window serve it as they serve the matvec.
-
-// the zero densities of the RHS flow (and the zero forces it takes for an absent f_external or F_T), the velocities,
-// and the kernels the call launches besides matvec_core's, loaded now (the first launch of a group member must not load
-// a kernel lazily while a peer on the same device spins on a flag)
-static int rhs_buffers(skb_flow *fl) {
-    const long long n = std::max<long long>({3 * (fl->fb - fl->fa), 3 * (fl->sb - fl->sa), 3 * fl->n_body,
-                                             3LL * fl->n_bodies, 1LL});
-    SKB_TRY(fl->zeros.ensure((size_t)n * 8));
-    fl->n_zeros = n;
-    SKB_TRY(fl->vel.ensure((size_t)fl->n_win * 24 + 8));
-    cudaFuncAttributes fa;
-    CUDA_TRY(cudaFuncGetAttributes(&fa, oseen_contract_add_kernel));
-    CUDA_TRY(cudaFuncGetAttributes(&fa, rotlet_add_kernel));
-    CUDA_TRY(cudaFuncGetAttributes(&fa, background_add_kernel));
-    return load_rhs_rows_kernel();
-}
-
-// System::prep_state_for_solver's RHS (system.cpp:421-455) on fl->cur, the rows of this flow's target list: d_fext 3 per
-// own fiber node or NULL (no external fiber force), d_f / d_t 3 per body, complete, or NULL (zero); d_rhs_fib 4 per own
-// fiber node, d_rhs_shell 3 per own periphery row, d_rhs_bodies in the x_bodies layout (the rows BodyOps owns written).
-// params / v_growth / force_scale per own fiber.  Every check, the fiber block's included, precedes the first launch.
-static int system_rhs_core(skb_flow *fl, OwnFibers own, const skb_fiber_params *params, const double *v_growth,
-                           const double *force_scale, const double *d_fext, const double *d_f, const double *d_t,
-                           double dt, double eta, double *d_rhs_fib, double *d_rhs_shell, double *d_rhs_bodies) {
-    const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
-    double *d_v = (double *)fl->vel.ptr;
-    const double *zero = (const double *)fl->zeros.ptr;
-    own.stream = fl->cur;
-    fl->bg.dn = nullptr; // no dense operator: nothing goes to the background streamer
-    fl->bg.launched = false;
-    auto run = [&](const FiberOps::Step *stage, const FiberOps::Step *launch) -> int {
-        if (stage) // the fiber block's per-fiber tables
-            SKB_TRY((*stage)());
-        CUDA_TRY(cudaMemsetAsync(fl->zeros.ptr, 0, (size_t)fl->n_zeros * 8, fl->cur));
-        // v_all = fc.flow(r_all, f_ext, eta), self term subtracted (system.cpp:425), + bc.flow(r_all, 0, F_T, eta)
-        // (:442).  F_T are complete on every member and go straight to the body flow (no ft_exchange): each counts once
-        SKB_TRY(matvec_core(fl, d_fext ? d_fext : zero, zero, zero, d_f ? d_f : zero, d_t ? d_t : zero, eta, d_v));
-        // v_all += psc.flow + bs.flow (:445-446).  The body evaluator's matvec targets are the rows of d_v, in its order
-        SKB_TRY(add_sources(fl, (const double *)fl->body[1]->devs[0].r_trg.ptr, fl->n_win, eta, d_v, fl->cur));
-        // fc.update_rhs(dt, v_fibers, motor + f_ext) + fc.apply_bcs(dt, v_fibers, f_ext) (:451-453)
-        if (launch)
-            SKB_TRY((*launch)());
-        // bc.update_RHS(v_bodies), shell.update_RHS(v_shell) (:448, 455)
-        return fl->bodies.rhs_rows(fl->n_bodies > 0, d_v + 3 * (n_fw + n_sw), d_rhs_bodies, d_v + 3 * n_fw, n_sw,
-                                   d_rhs_shell, fl->cur, &fl->launches);
-    };
-    bool framed = false; // FiberOps::rhs calls the frame only when there are own fibers
-    SKB_TRY(fl->ops.rhs(own, params, v_growth, force_scale, d_v, d_fext, dt, eta, d_rhs_fib, &fl->launches,
-                        [&](const FiberOps::Step &stage, const FiberOps::Step &launch) {
-                            framed = true;
-                            return run(&stage, &launch);
-                        }));
-    return framed ? SKB_OK : run(nullptr, nullptr);
-}
-
-static int finite(const double *a, size_t n) {
-    for (size_t i = 0; i < n; ++i)
-        if (!std::isfinite(a[i]))
-            return 0;
-    return 1;
-}
-
-// the refusals of the two skb_flow forms, before any launch; then the own fibers, the flow's device current, the
-// buffers sized
-static int system_rhs_args(skb_flow *fl, const char *who, const skb_fiber_params *params, bool out, double dt,
-                           double eta, OwnFibers &own) {
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    if (fl->grp.member())
-        return set_error(SKB_ERR_INVALID, "%s: a group member's rows need the others' fiber forces; over several devices "
-                                          "use skb_mflow_build_system_rhs", who);
-    if (!(dt > 0) || !(eta > 0))
-        return set_error(SKB_ERR_INVALID, "%s: dt = %g, eta = %g (both must be > 0)", who, dt, eta);
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    SKB_TRY(own_fibers(fl, who, own));
-    const long long n_all = fl->n_fib + fl->n_shell + fl->n_body;
-    if (fl->n_win != n_all)
-        return set_error(SKB_ERR_INVALID, "%s: needs the whole target list (%lld of %lld rows are set by a target window "
-                                          "or ranges); over several devices use skb_mflow_build_system_rhs", who,
-                         fl->n_win, n_all);
-    if (fl->n_bodies > 0 && !fl->bodies.has_operators())
-        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_body_operators after skb_flow_set_bodies (the body rows "
-                                          "are laid out by its node counts)", who);
-    if ((own.count() > 0 && !params) || (solution_size(fl) > 0 && !out))
-        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
-    begin_stats(fl);
-    return rhs_buffers(fl);
-}
-
-extern "C" {
-
-int skb_flow_build_system_rhs(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
-                              const double *force_scale, const double *f_external, const double *body_forces_torques,
-                              double dt, double eta, double *rhs) {
-    const char *who = "skb_flow_build_system_rhs";
-    OwnFibers own;
-    SKB_TRY(system_rhs_args(fl, who, params, rhs != nullptr, dt, eta, own));
-    const long long nf = fl->n_fib, ns = fl->n_shell;
-    if ((f_external && !finite(f_external, (size_t)nf * 3)) ||
-        (body_forces_torques && !finite(body_forces_torques, (size_t)fl->n_bodies * 6)))
-        return set_error(SKB_ERR_INVALID, "%s: a non-finite external force or torque", who);
-    const size_t n = (size_t)solution_size(fl);
-    if (n == 0)
-        return SKB_OK;
-    std::vector<double> f, t;
-    if (body_forces_torques && fl->n_bodies > 0)
-        split_forces_torques(body_forces_torques, fl->n_bodies, f, t);
-    SKB_TRY(fl->sys_y.ensure(n * 8));
-    double *d_rhs = (double *)fl->sys_y.ptr;
-    return host_frame(
-        fl,
-        [&]() -> int {
-            if (f_external)
-                SKB_TRY(upload(fl, fl->in_fib, f_external, (size_t)nf * 3));
-            SKB_TRY(upload(fl, fl->in_force, f.data(), f.size()));
-            return upload(fl, fl->in_torque, t.data(), t.size());
-        },
-        [&] {
-            return system_rhs_core(fl, own, params, v_growth, force_scale,
-                                   f_external && nf ? (const double *)fl->in_fib.ptr : nullptr,
-                                   f.empty() ? nullptr : (const double *)fl->in_force.ptr,
-                                   t.empty() ? nullptr : (const double *)fl->in_torque.ptr, dt, eta, d_rhs,
-                                   d_rhs + 4 * nf, d_rhs + 4 * nf + 3 * ns);
-        },
-        [&] { return download(fl, rhs, fl->sys_y, n); });
-}
-
-int skb_flow_build_system_rhs_device(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
-                                     const double *force_scale, const double *d_f_external,
-                                     const double *d_body_forces, const double *d_body_torques, double dt, double eta,
-                                     double *d_rhs, void *stream) {
-    OwnFibers own;
-    SKB_TRY(system_rhs_args(fl, "skb_flow_build_system_rhs_device", params, d_rhs != nullptr, dt, eta, own));
-    if (solution_size(fl) == 0)
-        return SKB_OK;
-    const long long nf = fl->n_fib, ns = fl->n_shell;
-    fl->cur = (cudaStream_t)stream;
-    SKB_TRY(system_rhs_core(fl, own, params, v_growth, force_scale, nf ? d_f_external : nullptr,
-                            fl->n_bodies ? d_body_forces : nullptr, fl->n_bodies ? d_body_torques : nullptr, dt, eta,
-                            d_rhs, d_rhs + 4 * nf, d_rhs + 4 * nf + 3 * ns));
-    return device_stats(fl);
-}
-
-} // extern "C"
-
-// ---- the whole-vector operator on a member of skb_mflow (skb_internal.hpp) ---------------------------------------
-// A member holds its own fibers' links and its body rows' operators (BodyOps); x_bodies is complete on every member.
-// The bodies' link forces are exchanged inside matvec_core (ft_exchange); a single flow (a one-device skb_mflow) takes
-// the path of skb_flow_apply_system_matvec.
-
-int skb::flow_member_body_operators(skb_flow *fl, const int *n_nodes, int n_bodies, const double *node_weights,
-                                    const double *ex, const double *ey, const double *ez, const double *A_inv) {
-    if (n_bodies != fl->n_bodies)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_set_body_operators: %d bodies, skb_mflow_set_bodies has %d",
-                         n_bodies, fl->n_bodies);
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    SKB_TRY(prepare_matvec_targets(fl));
-    const bool member = fl->grp.member();
-    return fl->bodies.set_operators(n_nodes, n_bodies, fl->n_body, fl->h_r_body.data(), fl->h_centers.data(),
-                                    node_weights, ex, ey, ez, A_inv, fl->stream, member ? fl->ba : 0,
-                                    member ? fl->bb : -1);
-}
-
-int skb::flow_member_fiber_links(skb_flow *fl, const int *body, const double *site, const double *rigidity,
-                                 bool check_only) {
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    OwnFibers own{0, fl->n_fibers, fl->h_fiber_n.data(), fl->h_fiber_off.data(), (const double *)fl->r_fib.ptr,
-                  (const double *)fl->fiber_length.ptr, fl->stream};
-    if (!check_only)
-        SKB_TRY(own_fibers(fl, "skb_mflow_set_fiber_links", own));
-    const int f0 = own.f0;
-    return fl->bodies.set_links(own, fl->ops, fl->n_bodies, fl->h_centers.data(), body ? body + f0 : nullptr,
-                                body ? site + 3 * (size_t)f0 : nullptr, body ? rigidity + f0 : nullptr, fl->stream,
-                                check_only);
-}
-
-int skb::flow_member_system_ready(skb_flow *fl, const char *who, bool precondition) {
-    if (fl->n_fibers > 0)
-        SKB_TRY(fl->ops.ready(who, precondition));
-    if (fl->n_bodies > 0) {
-        if (!fl->bodies.has_operators())
-            return set_error(SKB_ERR_INVALID, "%s: call skb_mflow_set_body_operators after skb_mflow_set_bodies", who);
-        if (precondition && !fl->bodies.has_inverse())
-            return set_error(SKB_ERR_INVALID, "%s: skb_mflow_set_body_operators was given no A_inv", who);
-        if (!precondition && fl->n_fibers > 0 && !fl->bodies.has_links())
-            return set_error(SKB_ERR_INVALID, "%s: call skb_mflow_set_fiber_links after skb_mflow_set_fibers / "
-                                              "skb_mflow_set_bodies (NULL body: no fiber is bound)", who);
-    }
-    return SKB_OK;
-}
-
-int skb::flow_size_system(skb_flow *fl) {
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    SKB_TRY(prepare_matvec_targets(fl));
-    SKB_TRY(fl->tmp_b.ensure((size_t)(fl->bb - fl->ba) * 24 + 8));
-    return fl->ft_sum.ensure((size_t)fl->n_bodies * 48 + 8);
-}
-
-// the links of the own fibers, apply_matvec_core with the exchange of their partial forces, the owned body rows; on
-// fl->cur
-static int member_system_matvec_core(skb_flow *fl, skb_dense *dn, const double *d_x_fib, const double *d_x_shell,
-                                     const double *d_x_bodies, double eta, double *d_res_fib, double *d_res_shell,
-                                     double *d_res_bodies) {
-    const double *link = nullptr, *bd = nullptr, *f = nullptr, *t = nullptr;
-    if (fl->n_bodies > 0) { // the links of the own fibers; their partial forces / torques on every body
-        const auto &off = fl->h_fiber_off;
-        const long long f0 = fl->n_fibers ? std::lower_bound(off.begin(), off.end(), fl->fa) - off.begin() : 0;
-        SKB_TRY(fl->bodies.links(fl->ops, (const double *)fl->fiber_length.ptr + f0, d_x_fib, d_x_bodies, &link,
-                                 fl->cur, &fl->launches));
-        bd = fl->bodies.densities();
-        f = fl->bodies.forces();
-        t = fl->bodies.torques();
-    }
-    double *v_bodies = (double *)fl->tmp_b.ptr; // own body rows
-    fl->ft_exchange = fl->grp.member();
-    const int rc = apply_matvec_core(fl, dn, d_x_fib, d_x_shell, bd, f, t, link, eta, d_res_fib, d_res_shell, v_bodies);
-    fl->ft_exchange = false;
-    SKB_TRY(rc);
-    return fl->n_bodies > 0 ? fl->bodies.matvec(d_x_bodies, v_bodies, d_res_bodies, fl->cur, &fl->launches) : SKB_OK;
-}
-
-int skb::flow_member_system_matvec(skb_flow *fl, skb_dense *dn, const double *d_x_fib, const double *d_x_shell,
-                                   const double *d_x_bodies, double eta, double *d_res_fib, double *d_res_shell,
-                                   double *d_res_bodies, cudaStream_t st) {
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    begin_stats(fl);
-    fl->cur = st;
-    SKB_TRY(member_system_matvec_core(fl, dn, d_x_fib, d_x_shell, d_x_bodies, eta, d_res_fib, d_res_shell,
-                                      d_res_bodies));
-    return device_stats(fl);
-}
-
-int skb::flow_member_system_precondition(skb_flow *fl, skb_dense *dn, const double *d_x_fib, const double *d_x_shell,
-                                         const double *d_x_bodies, double *d_y_fib, double *d_y_shell,
-                                         double *d_y_bodies, cudaStream_t st) {
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    begin_stats(fl);
-    fl->cur = st;
-    SKB_TRY(fl->ops.precondition(d_x_fib, d_y_fib, st, &fl->launches));
-    if (fl->sb > fl->sa) { // the member's rows of M_inv times the complete x_shell
-        SKB_TRY(skb_dense_apply_device(dn, SKB_DENSE_M_INV, d_x_shell, nullptr, d_y_shell, st));
-        fl->launches += 1;
-    }
-    if (fl->n_bodies > 0)
-        SKB_TRY(fl->bodies.precondition(d_x_bodies, d_y_bodies, st, &fl->launches));
-    return device_stats(fl);
-}
-
-// a member's slice of a per-fiber array of ALL fibers (NULL stays NULL, and so does the slice of no fibers)
-template <class T> static const T *own_slice(const T *all, const OwnFibers &own) {
-    return all && own.count() > 0 ? all + own.f0 : nullptr;
-}
-
-int skb::flow_member_rhs_prepare(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
-                                 const double *force_scale, double dt, double eta) {
-    const char *who = "skb_mflow_build_system_rhs";
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    OwnFibers own;
-    SKB_TRY(own_fibers(fl, who, own));
-    if (fl->n_bodies > 0 && !fl->bodies.has_operators())
-        return set_error(SKB_ERR_INVALID, "%s: call skb_mflow_set_body_operators after skb_mflow_set_bodies", who);
-    SKB_TRY(rhs_buffers(fl));
-    // the fiber block's checks, and its tables uploaded once so that their buffers have their size before any launch
-    return fl->ops.rhs(own, own_slice(params, own), own_slice(v_growth, own), own_slice(force_scale, own), nullptr,
-                       nullptr, dt, eta, nullptr, &fl->launches,
-                       [&](const FiberOps::Step &stage, const FiberOps::Step &) -> int {
-                           SKB_TRY(stage());
-                           CUDA_TRY(cudaStreamSynchronize(own.stream));
-                           return SKB_OK;
-                       });
-}
-
-int skb::flow_member_system_rhs(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
-                                const double *force_scale, const double *d_fext, const double *d_f, const double *d_t,
-                                double dt, double eta, double *d_rhs_fib, double *d_rhs_shell, double *d_rhs_bodies,
-                                cudaStream_t st) {
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    begin_stats(fl);
-    fl->cur = st;
-    OwnFibers own;
-    SKB_TRY(own_fibers(fl, "skb_mflow_build_system_rhs", own));
-    SKB_TRY(system_rhs_core(fl, own, own_slice(params, own), own_slice(v_growth, own), own_slice(force_scale, own),
-                            fl->fb > fl->fa ? d_fext : nullptr, d_f, d_t, dt, eta, d_rhs_fib, d_rhs_shell,
-                            d_rhs_bodies));
-    return device_stats(fl);
-}
-
-// ---- the whole-vector calls of a rank-per-GPU group member (skb_flow_group_*, include/skelly_b200_flow.h) ----------
-// A member holds only its own rows of the solution vector, in ascending global order (distributed.system_rows):
-// x_local = [4 per own fiber node | 3 per own periphery row | own body rows].  Before a matvec or a preconditioner it
-// stores its own body rows (and, for the preconditioner, its own periphery rows) into every window and meets its peers
-// at the rows phase; from there on the complete x_bodies / x_shell are in its own window, and the member path of
-// skb_mflow runs on them unchanged.  Body outputs land in the whole body layout (sys_rb) and are compacted to the own
-// rows in one launch.
-
-// the resolved target ranges the set-up sized the member's buffers for (prepare_matvec_targets has run)
-static Group::Ranges group_ranges(const skb_flow *fl) { return {fl->fa, fl->fb, fl->sa, fl->sb, fl->ba, fl->bb}; }
-
-static long long group_local_size(const skb_flow *fl) {
-    return 4 * (fl->fb - fl->fa) + 3 * (fl->sb - fl->sa) + fl->grp.body_rows();
-}
-
-static int group_dense_args(skb_flow *fl, skb_dense *dn, const char *who, bool precondition);
-
-// the refusals of the group matvec (stresslet_plus_complementary in dn) and preconditioner (M_inv in dn, the inverses),
-// all before any launch; then the flow's device is current and its target ranges resolved
-static int group_system_args(skb_flow *fl, skb_dense *dn, const char *who, bool precondition) {
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    SKB_TRY(fl->grp.connected());
-    SKB_TRY(prepare_matvec_targets(fl));
-    if (!fl->grp.rows_for(group_ranges(fl)))
-        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_group_set_body_operators after skb_flow_group_init and after "
-                                          "every change of the target ranges", who);
-    if (fl->n_fibers > 0)
-        SKB_TRY(fl->ops.ready(who, precondition));
-    if (fl->n_bodies > 0) {
-        if (!fl->bodies.has_operators())
-            return set_error(SKB_ERR_INVALID, "%s: call skb_flow_group_set_body_operators after skb_flow_set_bodies", who);
-        if (precondition && !fl->bodies.has_inverse())
-            return set_error(SKB_ERR_INVALID, "%s: skb_flow_group_set_body_operators was given no A_inv", who);
-        if (!precondition && fl->n_fibers > 0 && !fl->bodies.has_links())
-            return set_error(SKB_ERR_INVALID, "%s: call skb_flow_group_set_fiber_links after skb_flow_set_fibers / "
-                                              "skb_flow_set_bodies (NULL body: no fiber is bound)", who);
-    }
-    return group_dense_args(fl, dn, who, precondition);
-}
-
-// dn: the member's row block of M_inv (precondition) or stresslet_plus_complementary, if it owns periphery rows
-static int group_dense_args(skb_flow *fl, skb_dense *dn, const char *who, bool precondition) {
-    const long long n_sw = fl->sb - fl->sa;
-    if (n_sw > 0) {
-        const int op = precondition ? SKB_DENSE_M_INV : SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY;
-        const char *op_name = precondition ? "M_inv" : "stresslet_plus_complementary";
-        if (!dn)
-            return set_error(SKB_ERR_INVALID, "%s: the member's periphery rows need their block of %s (dn == NULL)", who,
-                             op_name);
-        int dn_dev = -1;
-        int64_t rows = -1, cols = -1;
-        SKB_TRY(skb_dense_device(dn, 0, &dn_dev));
-        SKB_TRY(skb_dense_shape(dn, op, &rows, &cols));
-        if (dn_dev != fl->dev || rows != 3 * n_sw || cols != 3 * fl->n_shell)
-            return set_error(SKB_ERR_INVALID, "%s: the dense handle holds a %lld x %lld block of %s on device %d, need the "
-                                              "member's %lld rows x %lld of the %lld periphery nodes on device %d", who,
-                             (long long)rows, (long long)cols, op_name, dn_dev, 3 * n_sw, 3 * fl->n_shell, fl->n_shell,
-                             fl->dev);
-    }
-    return SKB_OK;
-}
-
-extern "C" {
-
-int skb_flow_group_set_body_operators(skb_flow *fl, const int *n_nodes, int n_bodies, const double *node_weights,
-                                      const double *ex, const double *ey, const double *ez, const double *A_inv) {
-    const char *who = "skb_flow_group_set_body_operators";
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    if (!fl->grp.member())
-        return skb_flow_set_body_operators(fl, n_nodes, n_bodies, node_weights, ex, ey, ez, A_inv);
-    if (n_bodies != fl->n_bodies)
-        return set_error(SKB_ERR_INVALID, "%s: %d bodies, skb_flow_set_bodies has %d", who, n_bodies, fl->n_bodies);
-    if (n_bodies > 0 && (!n_nodes || !node_weights || !ex || !ey || !ez))
-        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    OwnFibers own;
-    SKB_TRY(own_fibers(fl, who, own)); // the target ranges resolved, the window's layout checked
-    SKB_TRY(fl->bodies.set_operators(n_nodes, n_bodies, fl->n_body, fl->h_r_body.data(), fl->h_centers.data(),
-                                     node_weights, ex, ey, ez, A_inv, fl->stream, fl->ba, fl->bb));
-    std::vector<RowPiece> pieces;
-    if (!body_row_pieces(n_nodes, n_bodies, fl->ba, fl->bb, pieces))
-        return set_error(SKB_ERR_STATE, "%s: the body rows [%lld, %lld) make %d pieces (at most %d)", who, fl->ba,
-                         fl->bb, (int)pieces.size(), kMaxRowPieces);
-    // every buffer the three whole-vector calls use, at its final size now: none of them allocates while a peer on
-    // this device may wait on a flag (the warm-up sized the matvec flow's own)
-    SKB_TRY(fl->sys_rb.ensure((size_t)fl->bodies.solution_size() * 8 + 8));
-    SKB_TRY(flow_size_system(fl));
-    SKB_TRY(rhs_buffers(fl));
-    SKB_TRY(fl->ops.size_rhs(own.count()));
-    SKB_TRY(load_dense_kernels()); // the preconditioner's M_inv rows (and the matvec's without the streamer)
-    fl->grp.set_body_rows(pieces, group_ranges(fl));
-    return SKB_OK;
-}
-
-int skb_flow_group_set_body_frames(skb_flow *fl, const int *n_nodes, int n_bodies, const double *node_pos_ref,
-                                   const double *node_normal_ref, const double *node_weights, const double *ex0,
-                                   const double *ey0, const double *ez0, const double *A_inv0) {
-    const char *who = "skb_flow_group_set_body_frames";
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    if (!fl->grp.member())
-        return skb_flow_set_body_frames(fl, n_nodes, n_bodies, node_pos_ref, node_normal_ref, node_weights, ex0, ey0,
-                                        ez0, A_inv0);
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    OwnFibers own;
-    SKB_TRY(own_fibers(fl, who, own)); // the target ranges resolved, the window's layout checked
-    SKB_TRY(body_frames(fl, who, n_nodes, n_bodies, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0, A_inv0,
-                        fl->ba, fl->bb));
-    std::vector<RowPiece> pieces;
-    if (!body_row_pieces(n_nodes, n_bodies, fl->ba, fl->bb, pieces))
-        return set_error(SKB_ERR_STATE, "%s: the body rows [%lld, %lld) make %d pieces (at most %d)", who, fl->ba,
-                         fl->bb, (int)pieces.size(), kMaxRowPieces);
-    long long sol = 0;
-    for (int b = 0; b < n_bodies; ++b)
-        sol += 3LL * n_nodes[b] + 6;
-    // every buffer of the three whole-vector calls at its final size, as skb_flow_group_set_body_operators does
-    SKB_TRY(fl->sys_rb.ensure((size_t)sol * 8 + 8));
-    SKB_TRY(flow_size_system(fl));
-    SKB_TRY(rhs_buffers(fl));
-    SKB_TRY(fl->ops.size_rhs(own.count()));
-    SKB_TRY(load_dense_kernels());
-    fl->grp.set_body_rows(pieces, group_ranges(fl));
-    return SKB_OK;
-}
-
-int skb_flow_group_place_bodies(skb_flow *fl, const double *centers, const double *orientations) {
-    const char *who = "skb_flow_group_place_bodies";
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    if (!fl->grp.member())
-        return skb_flow_place_bodies(fl, centers, orientations);
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    SKB_TRY(prepare_matvec_targets(fl));
-    std::vector<double> R;
-    SKB_TRY(placement_args(fl, who, centers, orientations, fl->ba, fl->bb, R));
-    SKB_TRY(place_bodies(fl, centers, orientations, R));
-    return prepare_matvec_targets(fl); // the new body rows' targets now, not at the first matvec
-}
-
-int skb_flow_group_set_fiber_links(skb_flow *fl, const int *body, const double *site, const double *bending_rigidity) {
-    const char *who = "skb_flow_group_set_fiber_links";
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    if (!fl->grp.member())
-        return skb_flow_set_fiber_links(fl, body, site, bending_rigidity);
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    OwnFibers own;
-    SKB_TRY(own_fibers(fl, who, own));
-    if (body && own.count() > 0 && (!site || !bending_rigidity))
-        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
-    return fl->bodies.set_links(own, fl->ops, fl->n_bodies, fl->h_centers.data(), body, site, bending_rigidity,
-                                fl->stream);
-}
-
-int skb_flow_group_apply_system_matvec_device(skb_flow *fl, skb_dense *dn, const double *d_x_local, double eta,
-                                              double *d_res_local, void *stream) {
-    const char *who = "skb_flow_group_apply_system_matvec_device";
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    if (!fl->grp.member())
-        return skb_flow_apply_system_matvec_device(fl, dn, d_x_local, eta, d_res_local, stream);
-    SKB_TRY(group_system_args(fl, dn, who, false));
-    if (!(eta > 0))
-        return set_error(SKB_ERR_INVALID, "%s: eta = %g", who, eta);
-    if (group_local_size(fl) > 0 && (!d_x_local || !d_res_local))
-        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
-    begin_stats(fl);
-    fl->cur = (cudaStream_t)stream;
-    Group &G = fl->grp;
-    const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
-    const double *x_fib = d_x_local, *x_shell = x_fib + 4 * n_fw, *x_body = x_shell + 3 * n_sw;
-    double *res_fib = d_res_local, *res_shell = res_fib + 4 * n_fw, *res_body = res_shell + 3 * n_sw;
-    double *full = (double *)fl->sys_rb.ptr;
-    const bool bodies = fl->n_bodies > 0;
-    SKB_TRY(G.begin());
-    if (bodies) { // the complete x_bodies in every window first: the links read the bodies' U, w before barrier A
-        SKB_TRY(G.store_rows(x_body, nullptr, 0, 0, fl->fib[1]->devs[0].info.num_sms, fl->cur, &fl->launches));
-        SKB_TRY(G.rows_barrier(true, true, fl->cur, &fl->launches));
-    }
-    fl->grp_open = true; // matvec_core's push, barriers and pull run in this epoch
-    const int rc = member_system_matvec_core(fl, dn, x_fib, x_shell, bodies ? G.x_body() : nullptr, eta, res_fib,
-                                             res_shell, full);
-    fl->grp_open = false;
-    SKB_TRY(rc);
-    if (bodies)
-        SKB_TRY(G.compact_rows(full, res_body, fl->cur, &fl->launches));
-    return device_stats(fl);
-}
-
-int skb_flow_group_apply_system_preconditioner_device(skb_flow *fl, skb_dense *dn, const double *d_x_local,
-                                                      double *d_y_local, void *stream) {
-    const char *who = "skb_flow_group_apply_system_preconditioner_device";
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    if (!fl->grp.member())
-        return skb_flow_apply_system_preconditioner_device(fl, dn, d_x_local, d_y_local, stream);
-    SKB_TRY(group_system_args(fl, dn, who, true));
-    if (group_local_size(fl) > 0 && (!d_x_local || !d_y_local))
-        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
-    begin_stats(fl);
-    fl->cur = (cudaStream_t)stream;
-    Group &G = fl->grp;
-    const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
-    const double *x_fib = d_x_local, *x_shell = x_fib + 4 * n_fw, *x_body = x_shell + 3 * n_sw;
-    double *y_fib = d_y_local, *y_shell = y_fib + 4 * n_fw, *y_body = y_shell + 3 * n_sw;
-    double *full = (double *)fl->sys_rb.ptr;
-    // the complete x_shell and x_bodies in every window; the fibers' A_^-1 runs while the peers' rows arrive
-    SKB_TRY(G.begin());
-    SKB_TRY(G.store_rows(x_body, n_sw > 0 ? x_shell : nullptr, fl->sa, n_sw, fl->fib[1]->devs[0].info.num_sms, fl->cur,
-                         &fl->launches));
-    SKB_TRY(G.rows_barrier(true, false, fl->cur, &fl->launches));
-    SKB_TRY(fl->ops.precondition(x_fib, y_fib, fl->cur, &fl->launches));
-    SKB_TRY(G.rows_barrier(false, true, fl->cur, &fl->launches));
-    if (n_sw > 0) { // the member's rows of M_inv times the complete x_shell
-        SKB_TRY(skb_dense_apply_device(dn, SKB_DENSE_M_INV, G.x_shell(), nullptr, y_shell, fl->cur));
-        fl->launches += 1;
-    }
-    if (fl->n_bodies > 0) {
-        SKB_TRY(fl->bodies.precondition(G.x_body(), full, fl->cur, &fl->launches));
-        SKB_TRY(G.compact_rows(full, y_body, fl->cur, &fl->launches));
-    }
-    return device_stats(fl);
-}
-
-int skb_flow_group_build_system_rhs_device(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
-                                           const double *force_scale, const double *d_f_external,
-                                           const double *d_body_forces, const double *d_body_torques, double dt,
-                                           double eta, double *d_rhs_local, void *stream) {
-    const char *who = "skb_flow_group_build_system_rhs_device";
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    if (!fl->grp.member())
-        return skb_flow_build_system_rhs_device(fl, params, v_growth, force_scale, d_f_external, d_body_forces,
-                                                d_body_torques, dt, eta, d_rhs_local, stream);
-    if (!(dt > 0) || !(eta > 0))
-        return set_error(SKB_ERR_INVALID, "%s: dt = %g, eta = %g (both must be > 0)", who, dt, eta);
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    SKB_TRY(fl->grp.connected());
-    OwnFibers own;
-    SKB_TRY(own_fibers(fl, who, own));
-    if (!fl->grp.rows_for(group_ranges(fl)))
-        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_group_set_body_operators after skb_flow_group_init and after "
-                                          "every change of the target ranges", who);
-    if (fl->n_bodies > 0 && !fl->bodies.has_operators())
-        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_group_set_body_operators after skb_flow_set_bodies (the "
-                                          "body rows are laid out by its node counts)", who);
-    if ((own.count() > 0 && !params) || (group_local_size(fl) > 0 && !d_rhs_local))
-        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
-    begin_stats(fl);
-    fl->cur = (cudaStream_t)stream;
-    const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
-    double *rhs_fib = d_rhs_local, *rhs_shell = rhs_fib + 4 * n_fw, *rhs_body = rhs_shell + 3 * n_sw;
-    double *full = (double *)fl->sys_rb.ptr;
-    // the fiber block's checks come first inside system_rhs_core, before its first launch; F_T complete, as they are
-    SKB_TRY(system_rhs_core(fl, own, params, v_growth, force_scale, own.count() > 0 ? d_f_external : nullptr,
-                            fl->n_bodies ? d_body_forces : nullptr, fl->n_bodies ? d_body_torques : nullptr, dt, eta,
-                            rhs_fib, rhs_shell, full));
-    if (fl->n_bodies > 0)
-        SKB_TRY(fl->grp.compact_rows(full, rhs_body, fl->cur, &fl->launches));
-    return device_stats(fl);
-}
-
-} // extern "C"
-
-Krylov &skb::flow_krylov(skb_flow *fl) { return fl->kry; }
-Group &skb::flow_group(skb_flow *fl) { return fl->grp; }
-long long skb::flow_whole_size(skb_flow *fl) { return solution_size(fl); }
-int *skb::flow_launches(skb_flow *fl) { return &fl->launches; }
-int skb::flow_num_sms(const skb_flow *fl) { return fl->fib[1]->devs[0].info.num_sms; }
-int skb::flow_device(const skb_flow *fl) { return fl->dev; }
-
-int skb::flow_finish_device_stats(skb_flow *fl, int launches) {
-    fl->pairs = 0;
-    fl->launches = launches;
-    return device_stats(fl);
-}
-
-int skb::flow_solve_args(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const char *who, long long *n,
-                         std::array<long long, 6> *key) {
-    if (fl->grp.member()) {
-        SKB_TRY(group_system_args(fl, dn_spc, who, false));
-        SKB_TRY(group_system_args(fl, dn_minv, who, true));
-        *n = group_local_size(fl);
-        *key = group_ranges(fl);
-        return SKB_OK;
-    }
-    SKB_TRY(system_args(fl, dn_spc, who, false, true));
-    SKB_TRY(system_args(fl, dn_minv, who, true, true));
-    *n = solution_size(fl);
-    *key = {};
-    return SKB_OK;
-}
-
-int skb::flow_gmres_size(skb_flow *fl, const char *who, long long *n, std::array<long long, 6> *key) {
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    if (!fl->grp.member()) {
-        *n = solution_size(fl);
-        *key = {};
-        return SKB_OK;
-    }
-    SKB_TRY(prepare_matvec_targets(fl));
-    if (!fl->grp.rows_for(group_ranges(fl)))
-        return set_error(SKB_ERR_INVALID, "%s: a group member's rows are laid out by skb_flow_group_set_body_operators "
-                                          "(after skb_flow_group_init and every change of the target ranges)", who);
-    *n = group_local_size(fl);
-    *key = group_ranges(fl);
-    return SKB_OK;
-}
-
-int skb::flow_member_lay_out_rows(skb_flow *fl, const int *n_nodes, int n_bodies) {
-    const char *who = "skb_mflow_set_gmres";
-    if (!fl->grp.member())
-        return SKB_OK;
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    OwnFibers own;
-    SKB_TRY(own_fibers(fl, who, own));
-    std::vector<RowPiece> pieces;
-    if (!body_row_pieces(n_nodes, n_bodies, fl->ba, fl->bb, pieces))
-        return set_error(SKB_ERR_STATE, "%s: the body rows [%lld, %lld) make %d pieces (at most %d)", who, fl->ba,
-                         fl->bb, (int)pieces.size(), kMaxRowPieces);
-    long long sol = 0;
-    for (int b = 0; b < n_bodies; ++b)
-        sol += 3LL * n_nodes[b] + 6;
-    // every buffer of the local-vector calls at its final size, as skb_flow_group_set_body_operators does
-    SKB_TRY(fl->sys_rb.ensure((size_t)sol * 8 + 8));
-    SKB_TRY(flow_size_system(fl));
-    SKB_TRY(load_dense_kernels());
-    fl->grp.set_body_rows(pieces, group_ranges(fl));
-    return SKB_OK;
-}
-
-int skb::flow_group_step_checks(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const char *who, OwnFibers &own,
-                                long long *n, std::array<long long, 6> *key) {
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    SKB_TRY(fl->grp.connected());
-    SKB_TRY(own_fibers(fl, who, own)); // the target ranges resolved, whole fibers, the window's layout checked
-    if (!fl->grp.rows_for(group_ranges(fl)))
-        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_group_set_body_frames / _set_body_operators after "
-                                          "skb_flow_group_init and after every change of the target ranges", who);
-    SKB_TRY(group_dense_args(fl, dn_spc, who, false));
-    SKB_TRY(group_dense_args(fl, dn_minv, who, true));
-    if (fl->n_bodies > 0) {
-        if (!fl->bodies.has_frames() || !fl->placed || !fl->bodies.has_operators())
-            return set_error(SKB_ERR_INVALID, "%s: the step places the bodies from their frames: call "
-                                              "skb_flow_group_set_body_frames and a first skb_flow_group_place_bodies",
-                             who);
-        if (!fl->bodies.has_inverse())
-            return set_error(SKB_ERR_INVALID, "%s: skb_flow_group_set_body_frames was given no A_inv", who);
-    }
-    *n = group_local_size(fl);
-    *key = group_ranges(fl);
-    return SKB_OK;
-}
-
-int skb::flow_size_group_step(skb_flow *fl) {
-    if (!fl->grp.member())
-        return SKB_OK;
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    OwnFibers own;
-    SKB_TRY(own_fibers(fl, "skb_flow_set_gmres", own));
-    SKB_TRY(fl->ops.size_build(own));
-    return fl->bodies.size_links(own.count(), fl->n_bodies);
-}
-
-cudaStream_t skb::flow_stream(const skb_flow *fl) { return fl->stream; }
-int skb::flow_size_overlap(skb_flow *fl, long long n_rows) {
-    return fl->bg.enabled ? overlap_buffers(fl, n_rows) : SKB_OK;
-}
-
-FlowState skb::flow_state(skb_flow *fl) {
-    FlowState s;
-    s.fibers = OwnFibers{0, fl->n_fibers, fl->h_fiber_n.data(), fl->h_fiber_off.data(), (const double *)fl->r_fib.ptr,
-                         (const double *)fl->fiber_length.ptr, fl->stream};
-    s.length = fl->h_fiber_len.data();
-    s.positions = fl->h_r_fib.data();
-    s.n_shell = fl->n_shell;
-    s.n_bodies = fl->n_bodies;
-    s.centers = fl->h_centers.data();
-    s.orientations = fl->h_orient.data();
-    s.placed = fl->n_bodies == 0 || fl->placed;
-    s.ops = &fl->ops;
-    s.bodies = &fl->bodies;
-    s.buf = &fl->stepbuf;
-    return s;
-}
-
-int skb::flow_step_checks(skb_flow *fl, skb_dense *dn, const char *who) {
-    if (fl->grp.member())
-        return set_error(SKB_ERR_INVALID, "%s: a group member does not step (every member would need the others' new "
-                                          "fiber positions); over several devices use skb_mflow", who);
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    SKB_TRY(prepare_matvec_targets(fl));
-    const long long n_all = fl->n_fib + fl->n_shell + fl->n_body;
-    if (fl->n_win != n_all)
-        return set_error(SKB_ERR_INVALID, "%s: needs the whole target list (%lld of %lld rows are set by a target window "
-                                          "or ranges)", who, fl->n_win, n_all);
-    if (fl->n_shell > 0) {
-        SKB_TRY(dense_args(fl, dn, who, false));
-        SKB_TRY(dense_args(fl, dn, who, true));
-    }
-    if (fl->n_bodies > 0) {
-        if (!fl->bodies.has_frames() || !fl->placed || !fl->bodies.has_operators())
-            return set_error(SKB_ERR_INVALID, "%s: the step places the bodies from their frames: call "
-                                              "skb_flow_set_body_frames and a first skb_flow_place_bodies", who);
-        if (!fl->bodies.has_inverse())
-            return set_error(SKB_ERR_INVALID, "%s: skb_flow_set_body_frames was given no A_inv", who);
-    }
-    return SKB_OK;
-}

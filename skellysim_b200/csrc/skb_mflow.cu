@@ -2,10 +2,8 @@
 // evaluators need a single rank" rule admits (src/core/system.cpp:618-623).  One group member (skb_flow) per device,
 // connected through peer memory; whole fibers, periphery rows and body rows are block-partitioned over the members.
 // Every member is driven by its own host thread, so the n launch sequences are issued concurrently.  A client of the
-// skb_flow_* API plus the few internals declared in skb_internal.hpp.
-#include "skb_internal.hpp"
-#include "../../include/skelly_b200_flow.h"
-#include "../../include/skelly_b200_dense.h"
+// skb_flow_* API plus the few internals declared in skb_flow.hpp.
+#include "skb_flow.hpp"
 
 #include <algorithm>
 #include <cmath>
@@ -504,8 +502,8 @@ static int mflow_size_io(skb_mflow *mf, size_t n_ft, bool system = false) {
         SKB_TRY(io.outs.ensure(n_sw * 24 + 8));
         SKB_TRY(io.vb.ensure(n_bw * 24 + 8));
         SKB_TRY(io.v.ensure((n_fw + n_sw + n_bw) * 24 + 8));
-        if (mf->has_dense && n_sw > 0)
-            SKB_TRY(flow_size_overlap(mf->m[g].get(), 3 * (long long)n_sw));
+        if (mf->has_dense && n_sw > 0 && mf->m[g]->bg.enabled) // the background streamer's, if it is on
+            SKB_TRY(overlap_buffers(mf->m[g].get(), 3 * (long long)n_sw));
         if (system) {
             SKB_TRY(io.xsa.ensure((size_t)mf->n_shell * 24 + 8));
             SKB_TRY(io.xb.ensure((size_t)mf->body_sol * 8 + 8));
@@ -536,7 +534,7 @@ int skb_mflow_matvec(skb_mflow *mf, const double *fib_forces, const double *shel
         CUDA_TRY(cudaSetDevice(mf->devs[g]));
         const MemberRows r = member_rows(mf, g);
         const long long a = r.a, n_fw = r.n_fw, n_sw = r.n_sw, n_bw = r.n_bw;
-        cudaStream_t st = flow_stream(fl);
+        cudaStream_t st = fl->stream;
         SKB_TRY(put(io.ff, fib_forces ? fib_forces + 3 * a : nullptr, (size_t)n_fw * 3, st));
         SKB_TRY(put(io.xs, shell_density ? shell_density + 3 * mf->s0[g] : nullptr, (size_t)n_sw * 3, st));
         SKB_TRY(put(io.bd, body_densities, (size_t)nb * 3, st));
@@ -588,7 +586,7 @@ int skb_mflow_apply_matvec(skb_mflow *mf, const double *x_fibers, const double *
         const int f0 = mf->f0[g], f1 = mf->f1[g];
         const MemberRows r = member_rows(mf, g);
         const long long a = r.a, n_fw = r.n_fw, n_sw = r.n_sw, n_bw = r.n_bw;
-        cudaStream_t st = flow_stream(fl);
+        cudaStream_t st = fl->stream;
         SKB_TRY(put(io.x, x_fibers ? x_fibers + 4 * a : nullptr, (size_t)n_fw * 4, st));
         SKB_TRY(put(io.xs, x_shell ? x_shell + 3 * mf->s0[g] : nullptr, (size_t)n_sw * 3, st));
         SKB_TRY(put(io.bd, body_densities, (size_t)nb * 3, st));
@@ -679,8 +677,8 @@ int skb_mflow_set_body_frames(skb_mflow *mf, const int *n_nodes, int n_bodies, c
     SKB_TRY(mflow_prepare(mf));
     // every member checks the same complete arrays first, so all of them refuse or none does
     SKB_TRY(mf->workers->run([&](int g) -> int {
-        return flow_member_body_frames(mf->m[g].get(), n_nodes, n_bodies, node_pos_ref, node_normal_ref, node_weights,
-                                       ex0, ey0, ez0, A_inv0);
+        return body_frames(mf->m[g].get(), who, n_nodes, n_bodies, node_pos_ref, node_normal_ref, node_weights, ex0,
+                           ey0, ez0, A_inv0);
     }));
     mf->body_n.assign(n_nodes, n_nodes + n_bodies); // the layout every placement keeps
     mf->body_sol = 0;
@@ -695,8 +693,8 @@ int skb_mflow_place_bodies(skb_mflow *mf, const double *centers, const double *o
     SKB_TRY(mflow_prepare(mf));
     std::vector<std::vector<double>> R((size_t)mf->n);
     for (int g = 0; g < mf->n; ++g) // every member's refusals before any member places
-        SKB_TRY(flow_member_place_args(mf->m[g].get(), centers, orientations, R[(size_t)g]));
-    return mf->workers->run([&](int g) -> int { return flow_member_place(mf->m[g].get(), centers, orientations, R[(size_t)g]); });
+        SKB_TRY(placement_args(mf->m[g].get(), "skb_mflow_place_bodies", centers, orientations, R[(size_t)g]));
+    return mf->workers->run([&](int g) -> int { return place_bodies(mf->m[g].get(), centers, orientations, R[(size_t)g]); });
 }
 
 int skb_mflow_set_fiber_links(skb_mflow *mf, const int *body, const double *site, const double *bending_rigidity) {
@@ -720,7 +718,7 @@ static int mflow_system_args(skb_mflow *mf, const char *who, bool precondition, 
     if (!mf->ops_ready && mf->n_fibers > 0) // no fibers: the empty operator set, uploaded or not
         return set_error(SKB_ERR_STATE, "%s: call skb_mflow_set_fiber_operators first", who);
     for (int g = 0; g < mf->n; ++g)
-        SKB_TRY(flow_member_system_ready(mf->m[g].get(), who, precondition));
+        SKB_TRY(system_ready(mf->m[g].get(), who, kMflowCalls, precondition));
     const int op = precondition ? SKB_DENSE_M_INV : SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY;
     const char *op_name = precondition ? "SKB_DENSE_M_INV" : "SKB_DENSE_STRESSLET_PLUS_COMPLEMENTARY";
     if (mf->n_shell > 0 && !(precondition ? mf->has_minv : mf->has_dense))
@@ -778,7 +776,7 @@ int skb_mflow_apply_system_matvec(skb_mflow *mf, const double *x, double eta, do
         skb_mflow::IO &io = mf->io[g];
         CUDA_TRY(cudaSetDevice(mf->devs[g]));
         const MemberRows r = member_rows(mf, g);
-        cudaStream_t st = flow_stream(fl);
+        cudaStream_t st = fl->stream;
         SKB_TRY(put(io.x, x + 4 * r.a, (size_t)r.n_fw * 4, st));
         SKB_TRY(put(io.xs, x + 4 * nf + 3 * mf->s0[g], (size_t)r.n_sw * 3, st));
         SKB_TRY(put(io.xb, x + 4 * nf + 3 * ns, (size_t)nbs, st)); // complete, as system.cpp:306-311 has it
@@ -806,7 +804,7 @@ int skb_mflow_apply_system_preconditioner(skb_mflow *mf, const double *x, double
         skb_mflow::IO &io = mf->io[g];
         CUDA_TRY(cudaSetDevice(mf->devs[g]));
         const MemberRows r = member_rows(mf, g);
-        cudaStream_t st = flow_stream(fl);
+        cudaStream_t st = fl->stream;
         SKB_TRY(put(io.x, x + 4 * r.a, (size_t)r.n_fw * 4, st));
         SKB_TRY(put(io.xsa, r.n_sw ? x + 4 * nf : nullptr, (size_t)ns * 3, st));
         SKB_TRY(put(io.xb, x + 4 * nf + 3 * ns, (size_t)nbs, st));
@@ -863,7 +861,7 @@ int skb_mflow_build_system_rhs(skb_mflow *mf, const skb_fiber_params *params, co
         skb_mflow::IO &io = mf->io[g];
         CUDA_TRY(cudaSetDevice(mf->devs[g]));
         const MemberRows r = member_rows(mf, g);
-        cudaStream_t st = flow_stream(fl);
+        cudaStream_t st = fl->stream;
         SKB_TRY(put(io.ff, f_external ? f_external + 3 * r.a : nullptr, (size_t)r.n_fw * 3, st));
         SKB_TRY(put(io.f, f.data(), f.size(), st));
         SKB_TRY(put(io.t, t.data(), t.size(), st));
@@ -980,7 +978,7 @@ int skb_mflow_set_gmres(skb_mflow *mf, int num_blocks) {
     mf->gmres_set = false;
     SKB_TRY(mf->workers->run([&](int g) -> int {
         skb_flow *fl = mf->m[(size_t)g].get();
-        SKB_TRY(flow_member_lay_out_rows(fl, mf->body_n.data(), mf->n_bodies));
+        SKB_TRY(flow_member_lay_out_rows(fl, who, mf->body_n.data(), mf->n_bodies));
         return skb_flow_set_gmres(fl, num_blocks);
     }));
     mf->gmres_layout = gmres_layout(mf);
@@ -1013,17 +1011,17 @@ int skb_mflow_solve_system(skb_mflow *mf, const double *rhs, double eta, double 
         long long n = 0;
         std::array<long long, 6> key;
         SKB_TRY(flow_gmres_size(fl, who, &n, &key));
-        if (!flow_krylov(fl).sized_for(n, key) || num_blocks > flow_krylov(fl).blocks())
+        if (!fl->kry.sized_for(n, key) || num_blocks > fl->kry.blocks())
             return set_error(SKB_ERR_INVALID, "%s: num_blocks = %d, skb_mflow_set_gmres sized device member %d for %d",
-                             who, num_blocks, g, flow_krylov(fl).blocks());
+                             who, num_blocks, g, fl->kry.blocks());
     }
     std::vector<skb_solve_info> infos((size_t)mf->n);
     std::vector<std::vector<double>> hist((size_t)mf->n, std::vector<double>(history ? (size_t)max_iters + 1 : 0));
     SKB_TRY(mf->workers->run([&](int g) -> int {
         skb_flow *fl = mf->m[(size_t)g].get();
         CUDA_TRY(cudaSetDevice(mf->devs[(size_t)g]));
-        const Krylov &kry = flow_krylov(fl);
-        cudaStream_t st = flow_stream(fl);
+        const Krylov &kry = fl->kry;
+        cudaStream_t st = fl->stream;
         std::vector<double> loc;
         member_local(mf, g, [&](long long whole, long long, long long len) {
             loc.insert(loc.end(), rhs + whole, rhs + whole + len);
@@ -1106,7 +1104,7 @@ int skb_mflow_step(skb_mflow *mf, const skb_fiber_params *params, const double *
         skb_mflow::IO &io = mf->io[(size_t)g];
         CUDA_TRY(cudaSetDevice(mf->devs[(size_t)g]));
         const MemberRows r = member_rows(mf, g);
-        const cudaStream_t st = flow_stream(fl);
+        const cudaStream_t st = fl->stream;
         SKB_TRY(put(io.ff, f_external ? f_external + 3 * r.a : nullptr, (size_t)r.n_fw * 3, st));
         SKB_TRY(put(io.f, f.data(), f.size(), st));
         SKB_TRY(put(io.t, t.data(), t.size(), st));

@@ -2,8 +2,7 @@
 // whole-system operator and preconditioner of a flow (include/skelly_b200_flow.h, skb_flow_solve_system).  The vector
 // passes are krylov_kernels.cuh; the Hessenberg scalars, the Givens rotations and every decision are on the host.
 #include "krylov_kernels.cuh"
-#include "skb_internal.hpp"
-#include "../../include/skelly_b200_flow.h"
+#include "skb_flow.hpp"
 
 #include <algorithm>
 #include <cmath>
@@ -225,13 +224,31 @@ int skb::solve_scalar_args(const char *who, double tol, int num_blocks, int max_
     return SKB_OK;
 }
 
+// the refusals of the two system calls the solve makes (a group member's local-vector calls, else the single-device
+// ones): dn_spc holds stresslet_plus_complementary, dn_minv M_inv; *n = the (local) solution size, *key its ranges
+static int flow_solve_args(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const char *who, long long *n,
+                           std::array<long long, 6> *key) {
+    if (fl->grp.member()) {
+        SKB_TRY(group_system_args(fl, dn_spc, who, false));
+        SKB_TRY(group_system_args(fl, dn_minv, who, true));
+        *n = group_local_size(fl);
+        *key = group_ranges(fl);
+        return SKB_OK;
+    }
+    SKB_TRY(system_args(fl, dn_spc, who, false, true));
+    SKB_TRY(system_args(fl, dn_minv, who, true, true));
+    *n = solution_size(fl);
+    *key = {};
+    return SKB_OK;
+}
+
 // the refusals of every form, before any launch; *n = the (local) solution size, 0 with an empty system: nothing to
 // do (info filled).  group: the local-vector call of a group member (dn_spc / dn_minv its rows of the two operators)
 static int solve_args(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const char *who, bool group, double eta,
                       double tol, int num_blocks, int max_iters, bool args, skb_solve_info *info, long long *n) {
     if (!fl)
         return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    if (!group && flow_group(fl).member())
+    if (!group && fl->grp.member())
         return set_error(SKB_ERR_INVALID, "%s: a group member solves its local rows with "
                                           "skb_flow_group_solve_system_device", who);
     std::array<long long, 6> key;
@@ -241,13 +258,13 @@ static int solve_args(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const
     SKB_TRY(solve_scalar_args(who, tol, num_blocks, max_iters));
     if (!info)
         return set_error(SKB_ERR_INVALID, "%s: NULL info", who);
-    if (flow_whole_size(fl) == 0) { // every member of an empty system returns here alike
+    if (solution_size(fl) == 0) { // every member of an empty system returns here alike
         std::memset(info, 0, sizeof(*info));
         info->converged = 1;
         *n = 0;
         return SKB_OK;
     }
-    const Krylov &kry = flow_krylov(fl);
+    const Krylov &kry = fl->kry;
     if (!kry.sized_for(*n, key))
         return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_gmres for the current solution size (%lld) and target "
                                           "ranges", who, *n);
@@ -268,21 +285,34 @@ static int run(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const double
     int launches = 0;
     const Krylov::Apply A = [&](const double *in, double *out) -> int {
         SKB_TRY(skb_flow_group_apply_system_matvec_device(fl, dn_spc, in, eta, out, st));
-        launches += *flow_launches(fl);
+        launches += fl->launches;
         return SKB_OK;
     };
     const Krylov::Apply P_inv = [&](const double *in, double *out) -> int {
         SKB_TRY(skb_flow_group_apply_system_preconditioner_device(fl, dn_minv, in, out, st));
-        launches += *flow_launches(fl);
+        launches += fl->launches;
         return SKB_OK;
     };
-    Group &G = flow_group(fl);
+    Group &G = fl->grp;
     Krylov::Reduce reduce;
     if (G.member())
         reduce = [&](double *d_v, int m) -> int { return G.reduce_dots(d_v, m, st, &launches); };
-    SKB_TRY(flow_krylov(fl).solve(A, P_inv, reduce, d_b, d_x, tol, num_blocks, max_iters, st, info, history,
-                                  &launches));
-    return flow_finish_device_stats(fl, launches);
+    SKB_TRY(fl->kry.solve(A, P_inv, reduce, d_b, d_x, tol, num_blocks, max_iters, st, info, history, &launches));
+    fl->pairs = 0;
+    fl->launches = launches;
+    return device_stats(fl);
+}
+
+// a group member (skb_flow_set_gmres): the fiber build's and the links' buffers for its own fibers at their final size
+// (FiberOps::size_build, BodyOps::size_links); else nothing
+static int flow_size_group_step(skb_flow *fl) {
+    if (!fl->grp.member())
+        return SKB_OK;
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    OwnFibers own;
+    SKB_TRY(own_fibers(fl, "skb_flow_set_gmres", own));
+    SKB_TRY(fl->ops.size_build(own));
+    return fl->bodies.size_links(own.count(), fl->n_bodies);
 }
 
 extern "C" {
@@ -296,10 +326,9 @@ int skb_flow_set_gmres(skb_flow *fl, int num_blocks) {
     long long n = 0;
     std::array<long long, 6> key;
     SKB_TRY(flow_gmres_size(fl, who, &n, &key));
-    SKB_TRY(flow_krylov(fl).setup(n, num_blocks, flow_num_sms(fl), key));
+    SKB_TRY(fl->kry.setup(n, num_blocks, fl->fib[1]->devs[0].info.num_sms, key));
     // the buffers of skb_flow_step / skb_mflow_step / skb_flow_group_step_device beside the solve's
-    const FlowState s = flow_state(fl);
-    SKB_TRY(s.buf->size(s.fibers.count(), s.fibers.nodes(), s.n_bodies));
+    SKB_TRY(fl->stepbuf.size(fl->n_fibers, fl->n_fib, fl->n_bodies));
     return flow_size_group_step(fl);
 }
 
@@ -310,8 +339,8 @@ int skb_flow_solve_system(skb_flow *fl, skb_dense *dn, const double *rhs, double
                        &n));
     if (n == 0)
         return SKB_OK;
-    const Krylov &kry = flow_krylov(fl);
-    const cudaStream_t st = flow_stream(fl);
+    const Krylov &kry = fl->kry;
+    const cudaStream_t st = fl->stream;
     CUDA_TRY(cudaMemcpyAsync(kry.stage_b(), rhs, (size_t)n * 8, cudaMemcpyHostToDevice, st));
     SKB_TRY(run(fl, dn, dn, kry.stage_b(), eta, tol, num_blocks, max_iters, kry.stage_x(), info, history, st));
     CUDA_TRY(cudaMemcpyAsync(x, kry.stage_x(), (size_t)n * 8, cudaMemcpyDeviceToHost, st));
@@ -339,7 +368,7 @@ int skb_flow_group_solve_system_device(skb_flow *fl, skb_dense *dn_spc, skb_dens
     if (n == 0)
         return SKB_OK;
     const bool none = n < 0; // owns no row: the workspace's own buffers stand in for the empty vectors
-    const Krylov &kry = flow_krylov(fl);
+    const Krylov &kry = fl->kry;
     return run(fl, dn_spc, dn_minv, none ? kry.stage_b() : d_rhs_local, eta, tol, num_blocks, max_iters,
                none ? kry.stage_x() : d_x_local, info, history, (cudaStream_t)stream);
 }

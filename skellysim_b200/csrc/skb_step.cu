@@ -3,8 +3,7 @@
 // links, the fiber operators, the RHS and the solve of the existing calls, then the fiber step kernel
 // (step_kernels.cuh), the bodies' step on the host and the installation of the new geometry.
 #include "step_kernels.cuh"
-#include "skb_internal.hpp"
-#include "../../include/skelly_b200_flow.h"
+#include "skb_flow.hpp"
 
 #include <cmath>
 #include <cstring>
@@ -49,19 +48,19 @@ int StepBuffers::size(int n_fibers, long long n_fib, int n_bodies) {
     return SKB_OK;
 }
 
-// fiber_step_kernel over the fibers `own` of the flow of s on st (items from FiberOps::step_items; from_solution: d_in is
-// their block of a solution, 4 per own node, new positions and tensions to s.buf; else d_in holds positions), errors to
-// s.buf->err
-static int launch_fiber_step(const FlowState &s, const OwnFibers &own, const std::vector<StepItem> &items,
+// fiber_step_kernel over the fibers `own` of fl on st (items from FiberOps::step_items; from_solution: d_in is their
+// block of a solution, 4 per own node, new positions and tensions to fl->stepbuf; else d_in holds positions), errors to
+// fl->stepbuf.err
+static int launch_fiber_step(skb_flow *fl, const OwnFibers &own, const std::vector<StepItem> &items,
                              const double *d_in, bool from_solution, cudaStream_t st) {
     const int nf = own.count();
     if (nf == 0)
         return SKB_OK;
-    StepBuffers &b = *s.buf;
+    StepBuffers &b = fl->stepbuf;
     CUDA_TRY(cudaMemcpyAsync(b.items.ptr, items.data(), (size_t)nf * sizeof(StepItem), cudaMemcpyHostToDevice, st));
     const StepItem *it = (const StepItem *)b.items.ptr;
-    const double *mats = s.ops->class_table();
-    const int2 *ranges = s.ops->class_range_table();
+    const double *mats = fl->ops.class_table();
+    const int2 *ranges = fl->ops.class_range_table();
     if (from_solution)
         fiber_step_kernel<true><<<nf, kStepThreads, 0, st>>>(it, d_in, mats, ranges, own.length + own.f0,
                                                              (double *)b.r_new.ptr, (double *)b.tension.ptr,
@@ -174,12 +173,12 @@ int skb::step_host_inputs(const char *who, const double *f_external, long long n
 // step_host_inputs for device inputs: the external forces of m fiber nodes and the forces and torques of the flow's
 // bodies, read back into the pinned copy skb_flow_set_gmres sized (24 B per fiber node, 48 B per body) and scanned
 // there.  Copies, not launches, so a refusal still comes before any launch
-static int step_device_inputs(const char *who, const FlowState &s, const double *d_f_external, long long m,
+static int step_device_inputs(const char *who, skb_flow *fl, const double *d_f_external, long long m,
                               const double *d_body_forces, const double *d_body_torques, cudaStream_t st) {
-    const size_t nb3 = s.n_bodies > 0 ? 3 * (size_t)s.n_bodies : 0;
+    const size_t nb3 = fl->n_bodies > 0 ? 3 * (size_t)fl->n_bodies : 0;
     const double *d[3] = {d_f_external, d_body_forces, d_body_torques};
     const size_t count[3] = {3 * (size_t)m, nb3, nb3};
-    double *h = s.buf->check.get();
+    double *h = fl->stepbuf.check.get();
     bool finite[3] = {true, true, true};
     for (int k = 0; k < 3; ++k) {
         if (!d[k] || count[k] == 0)
@@ -198,68 +197,90 @@ static int step_device_inputs(const char *who, const FlowState &s, const double 
 
 // the refusals that concern the fibers the step advances (c.own): their arguments, their links at the current placement
 // and their classes; c is left with their rigidity, current nucleation sites and items
-static int own_fiber_checks(skb_flow *fl, const FlowState &s, const StepArgs &a, const char *who, StepCall &c) {
+static int own_fiber_checks(skb_flow *fl, const StepArgs &a, const char *who, StepCall &c) {
     const int nf = c.own.count();
-    SKB_TRY(step_fiber_args(who, a.params, a.fiber_body, a.site_ref, c.own.f0, nf, s.n_bodies));
+    SKB_TRY(step_fiber_args(who, a.params, a.fiber_body, a.site_ref, c.own.f0, nf, fl->n_bodies));
     c.rigidity.resize((size_t)nf);
     for (int f = 0; f < nf; ++f)
         c.rigidity[(size_t)f] = a.params[f].bending_rigidity;
-    nucleation_sites(nf, a.fiber_body, a.site_ref, s.centers, s.orientations, c.sites);
-    SKB_TRY(s.bodies->set_links(c.own, *s.ops, s.n_bodies, s.centers, a.fiber_body, c.sites.data(),
-                                c.rigidity.data(), flow_stream(fl), true));
-    SKB_TRY(s.ops->check_step(c.own, a.params, a.v_growth, a.force_scale));
-    return s.ops->step_items(c.own, c.items);
+    nucleation_sites(nf, a.fiber_body, a.site_ref, fl->h_centers.data(), fl->h_orient.data(), c.sites);
+    SKB_TRY(fl->bodies.set_links(c.own, fl->ops, fl->n_bodies, fl->h_centers.data(), a.fiber_body, c.sites.data(),
+                                 c.rigidity.data(), fl->stream, true));
+    SKB_TRY(fl->ops.check_step(c.own, a.params, a.v_growth, a.force_scale));
+    return fl->ops.step_items(c.own, c.items);
+}
+
+// the step's buffers were sized for the flow as it is (skb_flow_set_gmres)
+static bool step_sized(const skb_flow *fl) {
+    return fl->stepbuf.sized_for(fl->n_fibers, fl->n_fib, fl->n_bodies);
 }
 
 // every refusal of skb_flow_step but its inputs' finiteness (they are on the host or on the device)
 static int step_checks(skb_flow *fl, skb_dense *dn, const StepArgs &a, skb_step_info *info, const char *who,
                        StepCall &c) {
     SKB_TRY(step_scalar_args(who, info, a.dt, a.eta, a.tol, a.num_blocks, a.max_iters));
-    SKB_TRY(flow_step_checks(fl, dn, who));
-    const FlowState s = flow_state(fl);
-    c.own = s.fibers;
-    SKB_TRY(own_fiber_checks(fl, s, a, who, c));
+    if (fl->grp.member())
+        return set_error(SKB_ERR_INVALID, "%s: a group member does not step (every member would need the others' new "
+                                          "fiber positions); over several devices use skb_mflow", who);
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    SKB_TRY(whole_targets(fl, who, ""));
+    if (fl->n_shell > 0) {
+        SKB_TRY(dense_rows(fl, dn, who, false));
+        SKB_TRY(dense_rows(fl, dn, who, true));
+    }
+    SKB_TRY(system_ready(fl, who, kFlowCalls, true, true));
+    c.own = all_fibers(fl);
+    SKB_TRY(own_fiber_checks(fl, a, who, c));
     std::array<long long, 6> key;
     SKB_TRY(flow_gmres_size(fl, who, &c.n, &key));
-    Krylov &kry = flow_krylov(fl);
-    if (c.n > 0 && (!kry.sized_for(c.n, key) || !s.buf->sized_for(s.fibers.count(), s.fibers.nodes(), s.n_bodies)))
+    if (c.n > 0 && (!fl->kry.sized_for(c.n, key) || !step_sized(fl)))
         return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_gmres for the current solution size (%lld)", who, c.n);
-    if (c.n > 0 && a.num_blocks > kry.blocks())
+    if (c.n > 0 && a.num_blocks > fl->kry.blocks())
         return set_error(SKB_ERR_INVALID, "%s: num_blocks = %d, skb_flow_set_gmres sized the workspace for %d", who,
-                         a.num_blocks, kry.blocks());
+                         a.num_blocks, fl->kry.blocks());
     return SKB_OK;
 }
 
 int skb::group_step_checks(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const StepArgs &a,
                            skb_step_info *info, const char *who, StepCall &c) {
-    if (!flow_group(fl).member())
+    if (!fl->grp.member())
         return step_checks(fl, dn_spc, a, info, who, c);
     SKB_TRY(step_scalar_args(who, info, a.dt, a.eta, a.tol, a.num_blocks, a.max_iters));
-    std::array<long long, 6> key;
-    SKB_TRY(flow_group_step_checks(fl, dn_spc, dn_minv, who, c.own, &c.n, &key));
-    const FlowState s = flow_state(fl);
-    SKB_TRY(own_fiber_checks(fl, s, a, who, c));
-    Krylov &kry = flow_krylov(fl);
-    if (!kry.sized_for(c.n, key) || !s.buf->sized_for(s.fibers.count(), s.fibers.nodes(), s.n_bodies))
+    // its peers connected, its rows laid out for its target ranges, dn_spc / dn_minv its row blocks of the two
+    // periphery operators, bodies placed with an inverse
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    SKB_TRY(fl->grp.connected());
+    SKB_TRY(own_fibers(fl, who, c.own)); // the target ranges resolved, whole fibers, the window's layout checked
+    if (!fl->grp.rows_for(group_ranges(fl)))
+        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_group_set_body_frames / _set_body_operators after "
+                                          "skb_flow_group_init and after every change of the target ranges", who);
+    if (fl->sb > fl->sa) {
+        SKB_TRY(dense_rows(fl, dn_spc, who, false));
+        SKB_TRY(dense_rows(fl, dn_minv, who, true));
+    }
+    SKB_TRY(system_ready(fl, who, kGroupCalls, true, true));
+    c.n = group_local_size(fl);
+    SKB_TRY(own_fiber_checks(fl, a, who, c));
+    if (!fl->kry.sized_for(c.n, group_ranges(fl)) || !step_sized(fl))
         return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_gmres for the member's current target ranges", who);
-    if (!s.ops->build_sized_for(c.own)) // (the build's buffers are sized only once every class it needs is set)
+    if (!fl->ops.build_sized_for(c.own)) // (the build's buffers are sized only once every class it needs is set)
         return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_gmres after the fiber classes and their derivatives "
                                           "are set (it sizes the fiber build's buffers)", who);
-    if (a.num_blocks > kry.blocks())
+    if (a.num_blocks > fl->kry.blocks())
         return set_error(SKB_ERR_INVALID, "%s: num_blocks = %d, skb_flow_set_gmres sized the workspace for %d", who,
-                         a.num_blocks, kry.blocks());
+                         a.num_blocks, fl->kry.blocks());
     return SKB_OK;
 }
 
 // ---- the pieces both runs share --------------------------------------------------------------------------------------
 // uw = the rows [U; w] of every body (6 per body) from the body part of a solution on the device, 48 bytes per body
-static int body_rows(const FlowState &s, const double *d_x_bodies, std::vector<double> &uw, cudaStream_t st) {
-    uw.resize(6 * (size_t)s.n_bodies);
-    if (s.n_bodies == 0)
+static int body_rows(const skb_flow *fl, const double *d_x_bodies, std::vector<double> &uw, cudaStream_t st) {
+    uw.resize(6 * (size_t)fl->n_bodies);
+    if (fl->n_bodies == 0)
         return SKB_OK;
-    const int *nodes = s.bodies->frame_node_counts();
+    const int *nodes = fl->bodies.frame_node_counts();
     long long off = 0;
-    for (int b = 0; b < s.n_bodies; ++b) {
+    for (int b = 0; b < fl->n_bodies; ++b) {
         off += 3LL * nodes[b];
         CUDA_TRY(cudaMemcpyAsync(&uw[6 * (size_t)b], d_x_bodies + off, 48, cudaMemcpyDeviceToHost, st));
         off += 6;
@@ -270,12 +291,12 @@ static int body_rows(const FlowState &s, const double *d_x_bodies, std::vector<d
 
 // the bodies' step from their rows uw, the new nucleation sites of the step's fibers (0 where a row is not finite: such
 // a step is not installed) and their items' repin at them; false: a row is not finite
-static bool advance_bodies(const FlowState &s, const StepArgs &a, const std::vector<double> &uw, StepCall &c,
+static bool advance_bodies(const skb_flow *fl, const StepArgs &a, const std::vector<double> &uw, StepCall &c,
                            std::vector<double> &c_new, std::vector<double> &q_new, std::vector<double> &sites_new) {
-    c_new.resize(3 * (size_t)s.n_bodies);
-    q_new.resize(4 * (size_t)s.n_bodies);
-    for (int b = 0; b < s.n_bodies; ++b)
-        body_step(s.centers + 3 * (size_t)b, s.orientations + 4 * (size_t)b, &uw[6 * (size_t)b],
+    c_new.resize(3 * (size_t)fl->n_bodies);
+    q_new.resize(4 * (size_t)fl->n_bodies);
+    for (int b = 0; b < fl->n_bodies; ++b)
+        body_step(fl->h_centers.data() + 3 * (size_t)b, fl->h_orient.data() + 4 * (size_t)b, &uw[6 * (size_t)b],
                   &uw[6 * (size_t)b + 3], a.dt, &c_new[3 * (size_t)b], &q_new[4 * (size_t)b]);
     const bool finite = all_finite(uw);
     if (finite)
@@ -316,11 +337,10 @@ static int step_run(skb_flow *fl, skb_dense *dn, const StepArgs &a, StepCall &c,
     }
 
     // ---- System::step: the links, the operators, the RHS and the solve from the current placement ----
-    const FlowState s = flow_state(fl);
-    const int nf = s.fibers.count(), nb = s.n_bodies;
-    const long long n_fib = s.fibers.nodes();
-    const cudaStream_t st = flow_stream(fl);
-    Krylov &kry = flow_krylov(fl);
+    const int nf = fl->n_fibers, nb = fl->n_bodies;
+    const long long n_fib = fl->n_fib;
+    const cudaStream_t st = fl->stream;
+    Krylov &kry = fl->kry;
     SKB_TRY(skb_flow_set_fiber_links(fl, a.fiber_body, c.sites.data(), c.rigidity.data()));
     SKB_TRY(skb_flow_build_fiber_operators(fl, a.params, a.dt, a.eta));
     SKB_TRY(skb_flow_build_system_rhs_device(fl, a.params, a.v_growth, a.force_scale,
@@ -332,12 +352,12 @@ static int step_run(skb_flow *fl, skb_dense *dn, const StepArgs &a, StepCall &c,
 
     // ---- the bodies' step from their rows [U; w], on the host ----
     std::vector<double> uw, c_new, q_new, sites_new;
-    SKB_TRY(body_rows(s, d_x + 4 * n_fib + 3 * s.n_shell, uw, st));
-    const bool bodies_finite = advance_bodies(s, a, uw, c, c_new, q_new, sites_new);
+    SKB_TRY(body_rows(fl, d_x + 4 * n_fib + 3 * fl->n_shell, uw, st));
+    const bool bodies_finite = advance_bodies(fl, a, uw, c, c_new, q_new, sites_new);
 
     // ---- the fibers' step, repin and error on the device; one download of the new positions ----
-    SKB_TRY(launch_fiber_step(s, s.fibers, c.items, d_x, true, st));
-    const StepBuffers &buf = *s.buf;
+    SKB_TRY(launch_fiber_step(fl, all_fibers(fl), c.items, d_x, true, st));
+    const StepBuffers &buf = fl->stepbuf;
     std::vector<double> r_new(3 * (size_t)n_fib), err((size_t)nf);
     if (nf > 0) {
         CUDA_TRY(cudaMemcpyAsync(r_new.data(), buf.r_new.ptr, r_new.size() * 8, cudaMemcpyDeviceToHost, st));
@@ -352,8 +372,8 @@ static int step_run(skb_flow *fl, skb_dense *dn, const StepArgs &a, StepCall &c,
 
     // ---- install: the new positions through skb_flow_set_fibers (same node counts and lengths, so the partition and
     // the class table stay), the placement, the links at the new sites ----
-    const std::vector<int> n_nodes(s.fibers.n, s.fibers.n + nf);
-    const std::vector<double> length(s.length, s.length + nf);
+    const std::vector<int> n_nodes(fl->h_fiber_n);
+    const std::vector<double> length(fl->h_fiber_len);
     // (every argument below has passed its call's checks already: only a CUDA error can stop the install half-way)
     SKB_TRY(skb_flow_set_fibers(fl, r_new.data(), n_nodes.data(), length.data(), nf));
     if (nb > 0)
@@ -367,44 +387,44 @@ static int step_run(skb_flow *fl, skb_dense *dn, const StepArgs &a, StepCall &c,
 int skb::group_step_run(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const StepArgs &a, StepCall &c,
                         const double *d_f_external, const double *d_body_forces, const double *d_body_torques,
                         double *x_local, double *tension, skb_step_info *info, const char *who, cudaStream_t st) {
-    if (!flow_group(fl).member()) { // skb_flow_step's run, on the flow's stream once the caller's work on st is done
+    if (!fl->grp.member()) { // skb_flow_step's run, on the flow's stream once the caller's work on st is done
         CUDA_TRY(cudaStreamSynchronize(st));
         return step_run(fl, dn_spc, a, c, d_f_external, d_body_forces, d_body_torques, x_local, tension, info, who);
     }
     std::memset(info, 0, sizeof(*info));
     info->worst_fiber = -1;
-    if (flow_whole_size(fl) == 0) { // the empty system, on every member alike: nothing moves
+    if (solution_size(fl) == 0) { // the empty system, on every member alike: nothing moves
         info->solve.converged = 1;
         return SKB_OK;
     }
 
     // ---- System::step: the links, the operators (on the flow's stream, drained), the RHS and the solve on st ----
-    const FlowState s = flow_state(fl);
-    Group &G = flow_group(fl);
-    Krylov &kry = flow_krylov(fl);
-    const StepBuffers &buf = *s.buf;
-    const int nf = s.fibers.count(), nfo = c.own.count(), nb = s.n_bodies;
-    const long long n_fib = s.fibers.nodes(), m = c.own.nodes();
+    Group &G = fl->grp;
+    Krylov &kry = fl->kry;
+    const StepBuffers &buf = fl->stepbuf;
+    const int nf = fl->n_fibers, nfo = c.own.count(), nb = fl->n_bodies;
+    const long long n_fib = fl->n_fib, m = c.own.nodes();
     SKB_TRY(skb_flow_group_set_fiber_links(fl, a.fiber_body, c.sites.data(), c.rigidity.data()));
     SKB_TRY(skb_flow_build_fiber_operators(fl, a.params, a.dt, a.eta));
-    CUDA_TRY(cudaStreamSynchronize(flow_stream(fl)));
+    CUDA_TRY(cudaStreamSynchronize(fl->stream));
     SKB_TRY(skb_flow_group_build_system_rhs_device(fl, a.params, a.v_growth, a.force_scale, d_f_external,
                                                    d_body_forces, d_body_torques, a.dt, a.eta, kry.stage_b(), st));
     SKB_TRY(skb_flow_group_solve_system_device(fl, dn_spc, dn_minv, kry.stage_b(), a.eta, a.tol, a.num_blocks,
                                                a.max_iters, kry.stage_x(), &info->solve, nullptr, st));
     const double *d_x = kry.stage_x(); // [4 per own fiber node | 3 per own periphery row | own body rows]
-    int *launches = flow_launches(fl); // the protocol's launches join the flow's count, as in the other member calls
+    int *launches = &fl->launches; // the protocol's launches join the flow's count, as in the other member calls
 
     // ---- the body rows all-gathered (an epoch of its own: the rows phase), [U; w] of every body from the own window,
     // the bodies' step on the host: every member from the same bits ----
     std::vector<double> uw, c_new, q_new, sites_new;
     if (nb > 0) {
         SKB_TRY(G.begin());
-        SKB_TRY(G.store_rows(d_x + c.n - G.body_rows(), nullptr, 0, 0, flow_num_sms(fl), st, launches));
+        SKB_TRY(G.store_rows(d_x + c.n - G.body_rows(), nullptr, 0, 0, fl->fib[1]->devs[0].info.num_sms, st,
+                             launches));
         SKB_TRY(G.rows_barrier(true, true, st, launches));
-        SKB_TRY(body_rows(s, G.x_body(), uw, st));
+        SKB_TRY(body_rows(fl, G.x_body(), uw, st));
     }
-    const bool bodies_finite = advance_bodies(s, a, uw, c, c_new, q_new, sites_new);
+    const bool bodies_finite = advance_bodies(fl, a, uw, c, c_new, q_new, sites_new);
 
     // ---- the own fibers' step, repin and error fused with the all-gather of the results into r_step of every window
     // (an epoch of its own, the rows phase again), then the complete positions and errors from the own window ----
@@ -420,7 +440,7 @@ int skb::group_step_run(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, con
             g.node0 = c.own.off[c.own.f0];
             g.fiber0 = c.own.f0;
             group_fiber_step_kernel<<<nfo, kStepThreads, 0, st>>>((const StepItem *)buf.items.ptr, d_x,
-                                                                  s.ops->class_table(), s.ops->class_range_table(),
+                                                                  fl->ops.class_table(), fl->ops.class_range_table(),
                                                                   c.own.length + c.own.f0, (double *)buf.tension.ptr,
                                                                   g);
             CUDA_TRY(cudaGetLastError());
@@ -441,13 +461,13 @@ int skb::group_step_run(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, con
     SKB_TRY(decide(who, bodies_finite, r_new, err, info));
 
     // ---- install the complete geometry (same counts: the window, the partition and every buffer stay) ----
-    const std::vector<int> n_nodes(s.fibers.n, s.fibers.n + nf);
-    const std::vector<double> length(s.length, s.length + nf);
+    const std::vector<int> n_nodes(fl->h_fiber_n);
+    const std::vector<double> length(fl->h_fiber_len);
     SKB_TRY(skb_flow_set_fibers(fl, r_new.data(), n_nodes.data(), length.data(), nf));
     if (nb > 0)
         SKB_TRY(skb_flow_group_place_bodies(fl, c_new.data(), q_new.data()));
     SKB_TRY(skb_flow_group_set_fiber_links(fl, a.fiber_body, sites_new.data(), c.rigidity.data()));
-    CUDA_TRY(cudaStreamSynchronize(flow_stream(fl)));
+    CUDA_TRY(cudaStreamSynchronize(fl->stream));
     return SKB_OK;
 }
 
@@ -463,13 +483,12 @@ int skb_flow_step(skb_flow *fl, skb_dense *dn, const skb_fiber_params *params, c
     const StepArgs a{params, v_growth, force_scale, fiber_body, site_ref, dt, eta, tol, num_blocks, max_iters};
     StepCall c;
     SKB_TRY(step_checks(fl, dn, a, info, who, c));
-    const FlowState s = flow_state(fl);
-    const long long n_fib = s.fibers.nodes();
-    const int nb = s.n_bodies;
+    const long long n_fib = fl->n_fib;
+    const int nb = fl->n_bodies;
     SKB_TRY(step_host_inputs(who, f_external, n_fib, body_forces_torques, nb));
     // the inputs into the step's own buffers, on the stream the step runs on
-    StepBuffers &buf = *s.buf;
-    const cudaStream_t st = flow_stream(fl);
+    StepBuffers &buf = fl->stepbuf;
+    const cudaStream_t st = fl->stream;
     const bool fext = f_external && n_fib > 0, ft = body_forces_torques && nb > 0;
     if (fext)
         CUDA_TRY(cudaMemcpyAsync(buf.fext.ptr, f_external, (size_t)n_fib * 24, cudaMemcpyHostToDevice, st));
@@ -497,7 +516,7 @@ int skb_flow_group_step_device(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_mi
     const StepArgs a{params, v_growth, force_scale, fiber_body, site_ref, dt, eta, tol, num_blocks, max_iters};
     StepCall c;
     SKB_TRY(group_step_checks(fl, dn_spc, dn_minv, a, info, who, c));
-    SKB_TRY(step_device_inputs(who, flow_state(fl), d_f_external, c.own.nodes(), d_body_forces, d_body_torques, st));
+    SKB_TRY(step_device_inputs(who, fl, d_f_external, c.own.nodes(), d_body_forces, d_body_torques, st));
     return group_step_run(fl, dn_spc, dn_minv, a, c, d_f_external, d_body_forces, d_body_torques, d_x_local, d_tension,
                           info, who, st);
 }
@@ -506,18 +525,18 @@ int skb_flow_fiber_error(skb_flow *fl, double *max_error, double *per_fiber) {
     const char *who = "skb_flow_fiber_error";
     if (!fl || !max_error)
         return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
-    CUDA_TRY(cudaSetDevice(flow_device(fl)));
-    const FlowState s = flow_state(fl);
-    const int nf = s.fibers.count();
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    const OwnFibers all = all_fibers(fl);
+    const int nf = all.count();
     std::vector<StepItem> items;
-    SKB_TRY(s.ops->step_items(s.fibers, items));
+    SKB_TRY(fl->ops.step_items(all, items));
     std::vector<double> err((size_t)nf);
     if (nf > 0) {
-        const cudaStream_t st = flow_stream(fl);
-        SKB_TRY(s.buf->items.ensure((size_t)nf * sizeof(StepItem)));
-        SKB_TRY(s.buf->err.ensure((size_t)nf * 8));
-        SKB_TRY(launch_fiber_step(s, s.fibers, items, s.fibers.r_fib, false, st));
-        CUDA_TRY(cudaMemcpyAsync(err.data(), s.buf->err.ptr, (size_t)nf * 8, cudaMemcpyDeviceToHost, st));
+        const cudaStream_t st = fl->stream;
+        SKB_TRY(fl->stepbuf.items.ensure((size_t)nf * sizeof(StepItem)));
+        SKB_TRY(fl->stepbuf.err.ensure((size_t)nf * 8));
+        SKB_TRY(launch_fiber_step(fl, all, items, all.r_fib, false, st));
+        CUDA_TRY(cudaMemcpyAsync(err.data(), fl->stepbuf.err.ptr, (size_t)nf * 8, cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaStreamSynchronize(st));
     }
     int worst = -1;
@@ -531,25 +550,23 @@ int skb_flow_get_placement(skb_flow *fl, double *centers, double *orientations) 
     const char *who = "skb_flow_get_placement";
     if (!fl)
         return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    const FlowState s = flow_state(fl);
-    if (!s.placed)
+    if (fl->n_bodies > 0 && !fl->placed)
         return set_error(SKB_ERR_INVALID, "%s: the bodies were not placed since skb_flow_set_bodies "
                                           "(skb_flow_place_bodies)", who);
     if (centers)
-        std::memcpy(centers, s.centers, 24 * (size_t)s.n_bodies);
+        std::memcpy(centers, fl->h_centers.data(), 24 * (size_t)fl->n_bodies);
     if (orientations)
-        std::memcpy(orientations, s.orientations, 32 * (size_t)s.n_bodies);
+        std::memcpy(orientations, fl->h_orient.data(), 32 * (size_t)fl->n_bodies);
     return SKB_OK;
 }
 
 int skb_flow_get_fibers(skb_flow *fl, double *r_fib) {
     if (!fl)
         return set_error(SKB_ERR_INVALID, "skb_flow_get_fibers: NULL flow");
-    const FlowState s = flow_state(fl);
-    if (s.fibers.nodes() > 0 && !r_fib)
+    if (fl->n_fib > 0 && !r_fib)
         return set_error(SKB_ERR_INVALID, "skb_flow_get_fibers: NULL argument");
-    if (s.fibers.nodes() > 0)
-        std::memcpy(r_fib, s.positions, (size_t)s.fibers.nodes() * 24);
+    if (fl->n_fib > 0)
+        std::memcpy(r_fib, fl->h_r_fib.data(), (size_t)fl->n_fib * 24);
     return SKB_OK;
 }
 
