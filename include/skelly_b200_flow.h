@@ -726,7 +726,12 @@ SKB_API int skb_mflow_apply_matvec(skb_mflow *mf, const double *x_fibers, const 
  * fibers' forces and torques in container order; the members' partials are exchanged through the group window and
  * added in member (rank) order, 0 first (the MPI_Allreduce of body_container.cpp:128-135).  Every member thus holds
  * bitwise the same totals, and the result is bitwise reproducible run to run for a given device list; it differs from
- * the single-device order by rounding only.  With one device it is the skb_flow path. */
+ * the single-device order by rounding only.
+ *   Each member runs the rank-per-GPU calls (skb_flow_group_set_body_operators / _set_fiber_links on its own fibers'
+ * slices, skb_flow_group_apply_system_matvec_device / _preconditioner_device on its local rows, which the driver
+ * gathers from and scatters into the whole host vector).  A member's rows are laid out again before a system call
+ * whenever a new partition re-initialised the group, so no new skb_mflow_set_body_operators is needed after one.
+ * With one device it is the skb_flow path. */
 SKB_API int skb_mflow_set_body_operators(skb_mflow *mf, const int *n_nodes, int n_bodies, const double *node_weights,
                                          const double *ex, const double *ey, const double *ez, const double *A_inv);
 SKB_API int skb_mflow_set_fiber_links(skb_mflow *mf, const int *body, const double *site,
@@ -742,15 +747,15 @@ SKB_API int skb_mflow_apply_system_matvec(skb_mflow *mf, const double *x, double
 SKB_API int skb_mflow_apply_system_preconditioner(skb_mflow *mf, const double *x, double *y);
 /* skb_flow_build_system_rhs over n devices, the same arguments (complete host arrays of all fibers and bodies, the whole
  * vector out) and refusals, every member's checked before any device starts.  Each member forms its own rows (those of
- * skb_mflow_apply_system_matvec); the flow is the group's matvec flow, and the complete F_T enter every member's body
- * flow as they are.  With one device it is the skb_flow path. */
+ * skb_mflow_apply_system_matvec) with skb_flow_group_build_system_rhs_device; the flow is the group's matvec flow, and
+ * the complete F_T enter every member's body flow as they are.  With one device it is the skb_flow path. */
 SKB_API int skb_mflow_build_system_rhs(skb_mflow *mf, const skb_fiber_params *params, const double *v_growth,
                                        const double *force_scale, const double *f_external,
                                        const double *body_forces_torques, double dt, double eta, double *rhs);
-/* skb_flow_solve_system over n devices: complete host rhs in, complete host x out.  skb_mflow_set_gmres lays out every
- * member's local rows (as skb_flow_group_set_body_operators does, after skb_mflow_set_body_operators or
- * _set_body_frames) and sizes its workspace; each member thread then runs skb_flow_group_solve_system_device on its
- * rows, so every member reports bitwise the same info and history.  Refusals as skb_flow_solve_system's and
+/* skb_flow_solve_system over n devices: complete host rhs in, complete host x out.  skb_mflow_set_gmres sizes every
+ * member's workspace for its local rows (laid out again first if a new partition re-initialised the group since
+ * skb_mflow_set_body_operators or _set_body_frames); each member thread then runs skb_flow_group_solve_system_device on
+ * its rows, so every member reports bitwise the same info and history.  Refusals as skb_flow_solve_system's and
  * skb_mflow_apply_system_matvec's / _preconditioner's, every member's checked before any device starts; no
  * skb_mflow_set_gmres since the partition or the bodies' node counts changed.  With one device it is the skb_flow path,
  * bitwise. */

@@ -230,45 +230,15 @@ int flow_member_lay_out_rows(skb_flow *fl, const char *who, const int *n_nodes, 
 
 // R (row-major) of a unit quaternion (w, x, y, z): the formula of Eigen's QuaternionBase::toRotationMatrix
 void quaternion_rotation(const double *q, double *R);
-// The frames of the flow's bodies (a member: for its body rows); the refusals of a placement, before any state
-// changes, with the rotations R (9 per body) it places at; the placement itself, after placement_args
-int body_frames(skb_flow *fl, const char *who, const int *n_nodes, int n_bodies, const double *pos_ref,
-                const double *normal_ref, const double *node_weights, const double *ex0, const double *ey0,
-                const double *ez0, const double *A_inv0);
+// the refusals of a placement, before any state changes, with the rotations R (9 per body) it places at
 int placement_args(skb_flow *fl, const char *who, const double *centers, const double *orientations,
                    std::vector<double> &R);
-int place_bodies(skb_flow *fl, const double *centers, const double *orientations, const std::vector<double> &R);
 
-// The whole-vector operator on one member of skb_mflow (the members of a group, or the single flow of a one-device
-// skb_mflow), after its target ranges are set.  The arguments are those of skb_flow_set_body_operators /
-// _set_fiber_links for ALL bodies / fibers; a member keeps the part its ranges own (BodyOps).  check_only: check the
-// links of every fiber and keep the earlier ones
-int flow_member_body_operators(skb_flow *fl, const int *n_nodes, int n_bodies, const double *node_weights,
-                               const double *ex, const double *ey, const double *ez, const double *A_inv);
-int flow_member_fiber_links(skb_flow *fl, const int *body, const double *site, const double *rigidity,
-                            bool check_only);
-int flow_size_system(skb_flow *fl); // sizes the buffers the two calls below use (before any member launches)
-// on st: x_fib 4 per own fiber node, x_shell 3 per own periphery row, x_bodies complete; res_fib / res_shell own rows,
-// res_bodies in the complete body layout, the owned rows written.  dn: the member's rows of
-// stresslet_plus_complementary (NULL without periphery rows)
-int flow_member_system_matvec(skb_flow *fl, skb_dense *dn, const double *d_x_fib, const double *d_x_shell,
-                              const double *d_x_bodies, double eta, double *d_res_fib, double *d_res_shell,
-                              double *d_res_bodies, cudaStream_t st);
-// the same layout, x_shell complete (3 per periphery node); dn: the member's rows of M_inv
-int flow_member_system_precondition(skb_flow *fl, skb_dense *dn, const double *d_x_fib, const double *d_x_shell,
-                                    const double *d_x_bodies, double *d_y_fib, double *d_y_shell, double *d_y_bodies,
-                                    cudaStream_t st);
-// The system RHS (skb_flow_build_system_rhs) on a member; params / v_growth / force_scale of ALL fibers.
-// flow_member_rhs_prepare, on the calling thread before any member launches: the refusals (the member's fibers and
-// bodies), the upload of the fiber block's per-fiber tables, and every buffer and kernel the call uses.
-// flow_member_system_rhs on st: d_fext 3 per own fiber node or NULL, d_f / d_t 3 per body (complete) or NULL; the
-// outputs as flow_member_system_matvec's
+// skb_mflow_build_system_rhs on one member, on the calling thread before any member launches: the refusals (the
+// member's fibers and bodies; params / v_growth / force_scale of ALL fibers), the upload of the fiber block's per-fiber
+// tables, and every buffer and kernel the RHS uses
 int flow_member_rhs_prepare(skb_flow *fl, const ::skb_fiber_params *params, const double *v_growth,
                             const double *force_scale, double dt, double eta);
-int flow_member_system_rhs(skb_flow *fl, const ::skb_fiber_params *params, const double *v_growth,
-                           const double *force_scale, const double *d_fext, const double *d_f, const double *d_t,
-                           double dt, double eta, double *d_rhs_fib, double *d_rhs_shell, double *d_rhs_bodies,
-                           cudaStream_t st);
 
 // ---- skb_solve.cu ----
 // the refusals of a solve's tol, num_blocks and max_iters (each caller checks its own eta)

@@ -110,9 +110,7 @@ struct skb_mflow {
     std::vector<int> body_n; // node counts of skb_mflow_set_body_operators (the body part of the solution vector)
     long long body_sol = 0;  // ... its size, sum(3 n + 6)
     struct IO { // per-member device buffers of the host-pointer calls
-        DevBuf x, xs, bd, f, t, link, res, outs, vb, ff, v;
-        DevBuf xsa, xb, rb; // the system calls: complete x_shell, complete x_bodies, body rows in the complete layout
-                            // (only the member's own rows of rb are results: BodyOps::precondition)
+        DevBuf x, xs, bd, f, t, link, res, outs, vb, ff, v; // (x / res: also the local vector of the system calls)
         Event e0, e1;
     };
     std::vector<IO> io;
@@ -484,8 +482,7 @@ static int put(DevBuf &buf, const double *h, size_t n_dbl, cudaStream_t st) {
 
 // Size every member's transfer buffers on the CALLING thread, before any member starts launching: cudaMalloc /
 // cudaFree may synchronise the whole device and must not run while a peer on the same device sits in a flag wait.
-// system: also the buffers of the whole-vector calls
-static int mflow_size_io(skb_mflow *mf, size_t n_ft, bool system = false) {
+static int mflow_size_io(skb_mflow *mf, size_t n_ft) {
     for (int g = 0; g < mf->n; ++g) {
         CUDA_TRY(cudaSetDevice(mf->devs[g]));
         skb_mflow::IO &io = mf->io[g];
@@ -504,12 +501,6 @@ static int mflow_size_io(skb_mflow *mf, size_t n_ft, bool system = false) {
         SKB_TRY(io.v.ensure((n_fw + n_sw + n_bw) * 24 + 8));
         if (mf->has_dense && n_sw > 0 && mf->m[g]->bg.enabled) // the background streamer's, if it is on
             SKB_TRY(overlap_buffers(mf->m[g].get(), 3 * (long long)n_sw));
-        if (system) {
-            SKB_TRY(io.xsa.ensure((size_t)mf->n_shell * 24 + 8));
-            SKB_TRY(io.xb.ensure((size_t)mf->body_sol * 8 + 8));
-            SKB_TRY(io.rb.ensure((size_t)mf->body_sol * 8 + 8));
-            SKB_TRY(flow_size_system(mf->m[g].get()));
-        }
     }
     return SKB_OK;
 }
@@ -617,31 +608,108 @@ int skb_mflow_apply_matvec(skb_mflow *mf, const double *x_fibers, const double *
     return mflow_collect_stats(mf);
 }
 
-// ---- the whole-vector operator [fibers | shell | bodies] over n devices ----------------------------------------------
+} // extern "C"
+
+// ---- the whole-vector calls [fibers | shell | bodies] over n devices: every member runs its skb_flow_group_* call ----
 // Row ownership: member g owns its fibers' rows, its periphery rows and, of the body part, the 3 rows of each body node
 // in [b0, b1) and the six rows [U; w] of every body whose first node lies in [b0, b1) (skellysim_b200.distributed
-// .system_rows).  Its owned rows of the body part, as [begin, end) offsets into it, adjacent pieces merged
-static std::vector<std::pair<long long, long long>> body_rows(const std::vector<int> &body_n, long long b0,
-                                                              long long b1) {
-    std::vector<std::pair<long long, long long>> out;
-    auto add = [&](long long a, long long e) {
-        if (e <= a)
-            return;
-        if (!out.empty() && out.back().second == a)
-            out.back().second = e;
-        else
-            out.emplace_back(a, e);
-    };
-    long long node = 0, sol = 0;
-    for (int n : body_n) {
-        add(sol + 3 * (std::max(b0, node) - node), sol + 3 * (std::min(b1, node + n) - node));
-        if (node >= b0 && node < b1)
-            add(sol + 3LL * n, sol + 3LL * n + 6);
-        node += n;
-        sol += 3LL * n + 6;
-    }
-    return out;
+// .system_rows).  A member's local vector holds those rows in ascending order.
+
+static long long mflow_solution_size(const skb_mflow *mf) {
+    return 4 * mf->n_fib + 3 * mf->n_shell + (mf->n_bodies > 0 ? mf->body_sol : 0);
 }
+
+// member g's slice of a per-fiber array of all fibers, k entries per fiber (NULL stays NULL, and so does the slice of a
+// member without fibers)
+template <class T> static T *own_slice(const skb_mflow *mf, int g, T *all, int k = 1) {
+    return all && mf->f1[(size_t)g] > mf->f0[(size_t)g] ? all + (size_t)k * mf->f0[(size_t)g] : nullptr;
+}
+
+// member g's rows of a whole vector in its local order [fiber rows | shell rows | body pieces]: copy(whole offset,
+// local offset, length) per non-empty run, up to the first that fails
+template <class Copy> static int member_local(const skb_mflow *mf, int g, Copy copy) {
+    const MemberRows r = member_rows(mf, g);
+    const long long body = 4 * mf->n_fib + 3 * mf->n_shell, at = 4 * r.n_fw + 3 * r.n_sw;
+    std::vector<RowPiece> pieces;
+    if (mf->n_bodies > 0)
+        body_row_pieces(mf->body_n.data(), (int)mf->body_n.size(), mf->b0[(size_t)g], mf->b1[(size_t)g], pieces);
+    if (r.n_fw)
+        SKB_TRY(copy(4 * r.a, 0, 4 * r.n_fw));
+    if (r.n_sw)
+        SKB_TRY(copy(4 * mf->n_fib + 3 * mf->s0[(size_t)g], 4 * r.n_fw, 3 * r.n_sw));
+    for (const RowPiece &p : pieces)
+        SKB_TRY(copy(body + p.body, at + p.local, p.len));
+    return SKB_OK;
+}
+
+static long long member_local_size(const skb_mflow *mf, int g) {
+    long long n = 0;
+    member_local(mf, g, [&](long long, long long, long long len) {
+        n += len;
+        return SKB_OK;
+    });
+    return n;
+}
+
+// On member g's worker: its rows of the whole host vector `in` (NULL: the call has no input vector) into its local
+// vector d_in, call(stream) between the member's timing events, the local rows of d_out into the whole host vector `out`
+template <class Call>
+static int member_through(skb_mflow *mf, int g, const double *in, double *d_in, const double *d_out, double *out,
+                          Call call) {
+    skb_mflow::IO &io = mf->io[(size_t)g];
+    CUDA_TRY(cudaSetDevice(mf->devs[(size_t)g]));
+    const cudaStream_t st = mf->m[(size_t)g]->stream;
+    if (in)
+        SKB_TRY(member_local(mf, g, [&](long long whole, long long at, long long len) -> int {
+            CUDA_TRY(cudaMemcpyAsync(d_in + at, in + whole, (size_t)len * 8, cudaMemcpyHostToDevice, st));
+            return SKB_OK;
+        }));
+    CUDA_TRY(cudaEventRecord(io.e0, st));
+    SKB_TRY(call(st));
+    CUDA_TRY(cudaEventRecord(io.e1, st));
+    SKB_TRY(member_local(mf, g, [&](long long whole, long long at, long long len) -> int {
+        CUDA_TRY(cudaMemcpyAsync(out + whole, d_out + at, (size_t)len * 8, cudaMemcpyDeviceToHost, st));
+        return SKB_OK;
+    }));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return SKB_OK;
+}
+
+// On the calling thread, before any worker starts: every member whose rows are not laid out for its current ranges (a
+// new partition re-runs skb_flow_group_init) lays them out for the recorded bodies, and its local-vector buffers take
+// their size -- nothing allocates while a peer on the same device waits on a flag
+static int mflow_local_rows(skb_mflow *mf, const char *who) {
+    if (mf->n_bodies > 0 && (int)mf->body_n.size() != mf->n_bodies)
+        return set_error(SKB_ERR_INVALID, "%s: call skb_mflow_set_body_operators first", who);
+    for (int g = 0; g < mf->n; ++g) {
+        skb_flow *fl = mf->m[(size_t)g].get();
+        CUDA_TRY(cudaSetDevice(fl->dev));
+        SKB_TRY(prepare_matvec_targets(fl));
+        if (fl->grp.member() && !fl->grp.rows_for(group_ranges(fl)))
+            SKB_TRY(flow_member_lay_out_rows(fl, who, mf->body_n.data(), mf->n_bodies));
+        const long long n = member_local_size(mf, g);
+        SKB_TRY(mf->io[(size_t)g].x.ensure((size_t)n * 8 + 8));
+        SKB_TRY(mf->io[(size_t)g].res.ensure((size_t)n * 8 + 8));
+    }
+    return SKB_OK;
+}
+
+// the bodies' node counts the members' local rows are laid out by
+static void mflow_set_body_n(skb_mflow *mf, const int *n_nodes, int n_bodies) {
+    mf->body_n.assign(n_nodes, n_nodes + n_bodies);
+    mf->body_sol = 0;
+    for (int n : mf->body_n)
+        mf->body_sol += 3LL * n + 6;
+}
+
+// the link checks of every fiber (a member checks its own fibers only), leaving the links the flow holds as they are
+static int check_fiber_links(skb_flow *fl, const int *body, const double *site, const double *rigidity) {
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    return fl->bodies.set_links(all_fibers(fl), fl->ops, fl->n_bodies, fl->h_centers.data(), body, site, rigidity,
+                                fl->stream, true);
+}
+
+extern "C" {
 
 int skb_mflow_set_body_operators(skb_mflow *mf, const int *n_nodes, int n_bodies, const double *node_weights,
                                  const double *ex, const double *ey, const double *ez, const double *A_inv) {
@@ -655,12 +723,9 @@ int skb_mflow_set_body_operators(skb_mflow *mf, const int *n_nodes, int n_bodies
     SKB_TRY(mflow_prepare(mf));
     // every member checks the same complete arrays first, so all of them refuse or none does
     SKB_TRY(mf->workers->run([&](int g) -> int {
-        return flow_member_body_operators(mf->m[g].get(), n_nodes, n_bodies, node_weights, ex, ey, ez, A_inv);
+        return skb_flow_group_set_body_operators(mf->m[g].get(), n_nodes, n_bodies, node_weights, ex, ey, ez, A_inv);
     }));
-    mf->body_n.assign(n_nodes, n_nodes + n_bodies);
-    mf->body_sol = 0;
-    for (int n : mf->body_n)
-        mf->body_sol += 3LL * n + 6;
+    mflow_set_body_n(mf, n_nodes, n_bodies);
     return SKB_OK;
 }
 
@@ -677,13 +742,10 @@ int skb_mflow_set_body_frames(skb_mflow *mf, const int *n_nodes, int n_bodies, c
     SKB_TRY(mflow_prepare(mf));
     // every member checks the same complete arrays first, so all of them refuse or none does
     SKB_TRY(mf->workers->run([&](int g) -> int {
-        return body_frames(mf->m[g].get(), who, n_nodes, n_bodies, node_pos_ref, node_normal_ref, node_weights, ex0,
-                           ey0, ez0, A_inv0);
+        return skb_flow_group_set_body_frames(mf->m[g].get(), n_nodes, n_bodies, node_pos_ref, node_normal_ref,
+                                              node_weights, ex0, ey0, ez0, A_inv0);
     }));
-    mf->body_n.assign(n_nodes, n_nodes + n_bodies); // the layout every placement keeps
-    mf->body_sol = 0;
-    for (int n : mf->body_n)
-        mf->body_sol += 3LL * n + 6;
+    mflow_set_body_n(mf, n_nodes, n_bodies); // the layout every placement keeps
     return SKB_OK;
 }
 
@@ -691,10 +753,10 @@ int skb_mflow_place_bodies(skb_mflow *mf, const double *centers, const double *o
     if (!mf)
         return set_error(SKB_ERR_INVALID, "skb_mflow_place_bodies: NULL");
     SKB_TRY(mflow_prepare(mf));
-    std::vector<std::vector<double>> R((size_t)mf->n);
+    std::vector<double> R;
     for (int g = 0; g < mf->n; ++g) // every member's refusals before any member places
-        SKB_TRY(placement_args(mf->m[g].get(), "skb_mflow_place_bodies", centers, orientations, R[(size_t)g]));
-    return mf->workers->run([&](int g) -> int { return place_bodies(mf->m[g].get(), centers, orientations, R[(size_t)g]); });
+        SKB_TRY(placement_args(mf->m[g].get(), "skb_mflow_place_bodies", centers, orientations, R));
+    return mf->workers->run([&](int g) -> int { return skb_flow_group_place_bodies(mf->m[g].get(), centers, orientations); });
 }
 
 int skb_mflow_set_fiber_links(skb_mflow *mf, const int *body, const double *site, const double *bending_rigidity) {
@@ -704,13 +766,15 @@ int skb_mflow_set_fiber_links(skb_mflow *mf, const int *body, const double *site
     if (body && mf->n_fibers > 0 && (!site || !bending_rigidity))
         return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
     SKB_TRY(mflow_prepare(mf));
-    // the checks of every fiber before any member replaces its links (a member checks its own fibers only)
-    SKB_TRY(flow_member_fiber_links(mf->m[0].get(), body, site, bending_rigidity, true));
-    return mf->workers->run(
-        [&](int g) -> int { return flow_member_fiber_links(mf->m[g].get(), body, site, bending_rigidity, false); });
+    SKB_TRY(check_fiber_links(mf->m[0].get(), body, site, bending_rigidity)); // before any member replaces its links
+    return mf->workers->run([&](int g) -> int {
+        return skb_flow_group_set_fiber_links(mf->m[g].get(), own_slice(mf, g, body), own_slice(mf, g, site, 3),
+                                              own_slice(mf, g, bending_rigidity));
+    });
 }
 
-// the refusals of both system calls, before any launch; then every buffer they use is sized
+// the refusals of both system calls, before any launch; then every member's rows are laid out and every buffer the
+// calls use is sized
 static int mflow_system_args(skb_mflow *mf, const char *who, bool precondition, bool args) {
     if (!mf)
         return set_error(SKB_ERR_INVALID, "%s: NULL", who);
@@ -738,28 +802,8 @@ static int mflow_system_args(skb_mflow *mf, const char *who, bool precondition, 
     }
     if (!args)
         return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
-    return mflow_size_io(mf, 0, true);
-}
-
-static long long mflow_solution_size(const skb_mflow *mf) {
-    return 4 * mf->n_fib + 3 * mf->n_shell + (mf->n_bodies > 0 ? mf->body_sol : 0);
-}
-
-// member g's owned rows of the device results into the complete host vector out
-static int mflow_download_rows(skb_mflow *mf, int g, double *out, cudaStream_t st) {
-    skb_mflow::IO &io = mf->io[g];
-    const MemberRows r = member_rows(mf, g);
-    const long long nf = mf->n_fib, ns = mf->n_shell;
-    if (r.n_fw)
-        CUDA_TRY(cudaMemcpyAsync(out + 4 * r.a, io.res.ptr, (size_t)r.n_fw * 32, cudaMemcpyDeviceToHost, st));
-    if (r.n_sw)
-        CUDA_TRY(cudaMemcpyAsync(out + 4 * nf + 3 * mf->s0[g], io.outs.ptr, (size_t)r.n_sw * 24,
-                                 cudaMemcpyDeviceToHost, st));
-    if (mf->n_bodies > 0)
-        for (const auto &p : body_rows(mf->body_n, mf->b0[g], mf->b1[g]))
-            CUDA_TRY(cudaMemcpyAsync(out + 4 * nf + 3 * ns + p.first, (const double *)io.rb.ptr + p.first,
-                                     (size_t)(p.second - p.first) * 8, cudaMemcpyDeviceToHost, st));
-    return SKB_OK;
+    SKB_TRY(mflow_local_rows(mf, who));
+    return mflow_size_io(mf, 0);
 }
 
 // System::apply_matvec (system.cpp:269-324) over n devices on the whole solution vector
@@ -770,52 +814,29 @@ int skb_mflow_apply_system_matvec(skb_mflow *mf, const double *x, double eta, do
         return set_error(SKB_ERR_INVALID, "%s: eta = %g", who, eta);
     if (mflow_solution_size(mf) == 0)
         return SKB_OK;
-    const long long nf = mf->n_fib, ns = mf->n_shell, nbs = mflow_solution_size(mf) - 4 * nf - 3 * ns;
     SKB_TRY(mf->workers->run([&](int g) -> int {
-        skb_flow *fl = mf->m[g].get();
         skb_mflow::IO &io = mf->io[g];
-        CUDA_TRY(cudaSetDevice(mf->devs[g]));
-        const MemberRows r = member_rows(mf, g);
-        cudaStream_t st = fl->stream;
-        SKB_TRY(put(io.x, x + 4 * r.a, (size_t)r.n_fw * 4, st));
-        SKB_TRY(put(io.xs, x + 4 * nf + 3 * mf->s0[g], (size_t)r.n_sw * 3, st));
-        SKB_TRY(put(io.xb, x + 4 * nf + 3 * ns, (size_t)nbs, st)); // complete, as system.cpp:306-311 has it
-        CUDA_TRY(cudaEventRecord(io.e0, st));
-        SKB_TRY(flow_member_system_matvec(fl, mf->has_dense ? mf->dn[g].get() : nullptr, (const double *)io.x.ptr,
-                                          (const double *)io.xs.ptr, (const double *)io.xb.ptr, eta,
-                                          (double *)io.res.ptr, (double *)io.outs.ptr, (double *)io.rb.ptr, st));
-        CUDA_TRY(cudaEventRecord(io.e1, st));
-        SKB_TRY(mflow_download_rows(mf, g, res, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-        return SKB_OK;
+        skb_dense *dn = mf->has_dense ? mf->dn[g].get() : nullptr;
+        return member_through(mf, g, x, (double *)io.x.ptr, (const double *)io.res.ptr, res, [&](cudaStream_t st) {
+            return skb_flow_group_apply_system_matvec_device(mf->m[g].get(), dn, (const double *)io.x.ptr, eta,
+                                                             (double *)io.res.ptr, st);
+        });
     }));
     return mflow_collect_stats(mf);
 }
 
-// System::apply_preconditioner (system.cpp:248-262) over n devices: block diagonal, no exchange
+// System::apply_preconditioner (system.cpp:248-262) over n devices
 int skb_mflow_apply_system_preconditioner(skb_mflow *mf, const double *x, double *y) {
     const char *who = "skb_mflow_apply_system_preconditioner";
     SKB_TRY(mflow_system_args(mf, who, true, (x && y) || (mf && mflow_solution_size(mf) == 0)));
     if (mflow_solution_size(mf) == 0)
         return SKB_OK;
-    const long long nf = mf->n_fib, ns = mf->n_shell, nbs = mflow_solution_size(mf) - 4 * nf - 3 * ns;
     SKB_TRY(mf->workers->run([&](int g) -> int {
-        skb_flow *fl = mf->m[g].get();
         skb_mflow::IO &io = mf->io[g];
-        CUDA_TRY(cudaSetDevice(mf->devs[g]));
-        const MemberRows r = member_rows(mf, g);
-        cudaStream_t st = fl->stream;
-        SKB_TRY(put(io.x, x + 4 * r.a, (size_t)r.n_fw * 4, st));
-        SKB_TRY(put(io.xsa, r.n_sw ? x + 4 * nf : nullptr, (size_t)ns * 3, st));
-        SKB_TRY(put(io.xb, x + 4 * nf + 3 * ns, (size_t)nbs, st));
-        CUDA_TRY(cudaEventRecord(io.e0, st));
-        SKB_TRY(flow_member_system_precondition(fl, mf->dn[g].get(), (const double *)io.x.ptr,
-                                                (const double *)io.xsa.ptr, (const double *)io.xb.ptr,
-                                                (double *)io.res.ptr, (double *)io.outs.ptr, (double *)io.rb.ptr, st));
-        CUDA_TRY(cudaEventRecord(io.e1, st));
-        SKB_TRY(mflow_download_rows(mf, g, y, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-        return SKB_OK;
+        return member_through(mf, g, x, (double *)io.x.ptr, (const double *)io.res.ptr, y, [&](cudaStream_t st) {
+            return skb_flow_group_apply_system_preconditioner_device(mf->m[g].get(), mf->dn[g].get(),
+                                                                     (const double *)io.x.ptr, (double *)io.res.ptr, st);
+        });
     }));
     return mflow_collect_stats(mf);
 }
@@ -855,26 +876,22 @@ int skb_mflow_build_system_rhs(skb_mflow *mf, const skb_fiber_params *params, co
     std::vector<double> f, t;
     if (body_forces_torques && mf->n_bodies > 0)
         split_forces_torques(body_forces_torques, mf->n_bodies, f, t);
-    SKB_TRY(mflow_size_io(mf, f.size(), true));
+    SKB_TRY(mflow_local_rows(mf, who));
+    SKB_TRY(mflow_size_io(mf, f.size()));
     SKB_TRY(mf->workers->run([&](int g) -> int {
-        skb_flow *fl = mf->m[g].get();
         skb_mflow::IO &io = mf->io[g];
+        const cudaStream_t st = mf->m[g]->stream;
         CUDA_TRY(cudaSetDevice(mf->devs[g]));
         const MemberRows r = member_rows(mf, g);
-        cudaStream_t st = fl->stream;
         SKB_TRY(put(io.ff, f_external ? f_external + 3 * r.a : nullptr, (size_t)r.n_fw * 3, st));
         SKB_TRY(put(io.f, f.data(), f.size(), st));
         SKB_TRY(put(io.t, t.data(), t.size(), st));
-        CUDA_TRY(cudaEventRecord(io.e0, st));
-        SKB_TRY(flow_member_system_rhs(fl, params, v_growth, force_scale,
-                                       f_external ? (const double *)io.ff.ptr : nullptr,
-                                       f.empty() ? nullptr : (const double *)io.f.ptr,
-                                       t.empty() ? nullptr : (const double *)io.t.ptr, dt, eta, (double *)io.res.ptr,
-                                       (double *)io.outs.ptr, (double *)io.rb.ptr, st));
-        CUDA_TRY(cudaEventRecord(io.e1, st));
-        SKB_TRY(mflow_download_rows(mf, g, rhs, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-        return SKB_OK;
+        return member_through(mf, g, nullptr, nullptr, (const double *)io.res.ptr, rhs, [&](cudaStream_t s) {
+            return skb_flow_group_build_system_rhs_device(
+                mf->m[g].get(), own_slice(mf, g, params), own_slice(mf, g, v_growth), own_slice(mf, g, force_scale),
+                f_external ? (const double *)io.ff.ptr : nullptr, f.empty() ? nullptr : (const double *)io.f.ptr,
+                t.empty() ? nullptr : (const double *)io.t.ptr, dt, eta, (double *)io.res.ptr, s);
+        });
     }));
     return mflow_collect_stats(mf);
 }
@@ -947,23 +964,6 @@ static std::vector<long long> gmres_layout(const skb_mflow *mf) {
     return v;
 }
 
-// member g's rows of a whole vector in its local order [fiber rows | shell rows | body pieces]: copy(whole offset,
-// local offset, length) per run
-template <class Copy> static void member_local(const skb_mflow *mf, int g, Copy copy) {
-    const MemberRows r = member_rows(mf, g);
-    const long long nf = mf->n_fib, ns = mf->n_shell;
-    long long at = 0;
-    copy(4 * r.a, at, 4 * r.n_fw);
-    at += 4 * r.n_fw;
-    copy(4 * nf + 3 * mf->s0[g], at, 3 * r.n_sw);
-    at += 3 * r.n_sw;
-    if (mf->n_bodies > 0)
-        for (const auto &p : body_rows(mf->body_n, mf->b0[g], mf->b1[g])) {
-            copy(4 * nf + 3 * ns + p.first, at, p.second - p.first);
-            at += p.second - p.first;
-        }
-}
-
 extern "C" {
 
 int skb_mflow_set_gmres(skb_mflow *mf, int num_blocks) {
@@ -973,14 +973,9 @@ int skb_mflow_set_gmres(skb_mflow *mf, int num_blocks) {
     if (num_blocks < 1 || num_blocks > kMaxKrylov)
         return set_error(SKB_ERR_INVALID, "%s: num_blocks = %d (must be in [1, %d])", who, num_blocks, kMaxKrylov);
     SKB_TRY(mflow_prepare(mf));
-    if (mf->n_bodies > 0 && (int)mf->body_n.size() != mf->n_bodies)
-        return set_error(SKB_ERR_INVALID, "%s: call skb_mflow_set_body_operators first", who);
+    SKB_TRY(mflow_local_rows(mf, who));
     mf->gmres_set = false;
-    SKB_TRY(mf->workers->run([&](int g) -> int {
-        skb_flow *fl = mf->m[(size_t)g].get();
-        SKB_TRY(flow_member_lay_out_rows(fl, who, mf->body_n.data(), mf->n_bodies));
-        return skb_flow_set_gmres(fl, num_blocks);
-    }));
+    SKB_TRY(mf->workers->run([&](int g) -> int { return skb_flow_set_gmres(mf->m[(size_t)g].get(), num_blocks); }));
     mf->gmres_layout = gmres_layout(mf);
     mf->gmres_set = true;
     return SKB_OK;
@@ -1019,26 +1014,13 @@ int skb_mflow_solve_system(skb_mflow *mf, const double *rhs, double eta, double 
     std::vector<std::vector<double>> hist((size_t)mf->n, std::vector<double>(history ? (size_t)max_iters + 1 : 0));
     SKB_TRY(mf->workers->run([&](int g) -> int {
         skb_flow *fl = mf->m[(size_t)g].get();
-        CUDA_TRY(cudaSetDevice(mf->devs[(size_t)g]));
         const Krylov &kry = fl->kry;
-        cudaStream_t st = fl->stream;
-        std::vector<double> loc;
-        member_local(mf, g, [&](long long whole, long long, long long len) {
-            loc.insert(loc.end(), rhs + whole, rhs + whole + len);
-        });
-        if (!loc.empty())
-            CUDA_TRY(cudaMemcpyAsync(kry.stage_b(), loc.data(), loc.size() * 8, cudaMemcpyHostToDevice, st));
         skb_dense *dn = mf->dn[(size_t)g].get();
-        SKB_TRY(skb_flow_group_solve_system_device(fl, dn, dn, kry.stage_b(), eta, tol, num_blocks, max_iters,
-                                                   kry.stage_x(), &infos[(size_t)g],
-                                                   history ? hist[(size_t)g].data() : nullptr, st));
-        if (!loc.empty())
-            CUDA_TRY(cudaMemcpyAsync(loc.data(), kry.stage_x(), loc.size() * 8, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-        member_local(mf, g, [&](long long whole, long long at, long long len) {
-            std::memcpy(x + whole, loc.data() + at, (size_t)len * 8);
+        return member_through(mf, g, rhs, kry.stage_b(), kry.stage_x(), x, [&](cudaStream_t st) {
+            return skb_flow_group_solve_system_device(fl, dn, dn, kry.stage_b(), eta, tol, num_blocks, max_iters,
+                                                      kry.stage_x(), &infos[(size_t)g],
+                                                      history ? hist[(size_t)g].data() : nullptr, st);
         });
-        return SKB_OK;
     }));
     for (int g = 1; g < mf->n; ++g) // the all-reduce leaves every member the same scalars
         if (std::memcmp(&infos[(size_t)g], &infos[0], sizeof(skb_solve_info)) != 0 || hist[(size_t)g] != hist[0])
@@ -1081,12 +1063,9 @@ int skb_mflow_step(skb_mflow *mf, const skb_fiber_params *params, const double *
     std::vector<StepCall> calls((size_t)mf->n);
     for (int g = 0; g < mf->n; ++g) {
         skb_flow *fl = mf->m[(size_t)g].get();
-        const int f0 = mf->f0[(size_t)g];
-        auto own = [&](auto *all, int k) { // the member's slice, k per fiber (NULL stays NULL, and so does no fiber's)
-            return all && mf->f1[(size_t)g] > f0 ? all + (size_t)k * f0 : nullptr;
-        };
-        args[(size_t)g] = StepArgs{own(params, 1), own(v_growth, 1), own(force_scale, 1), own(fiber_body, 1),
-                                   own(site_ref, 3), dt, eta, tol, num_blocks, max_iters};
+        args[(size_t)g] = StepArgs{own_slice(mf, g, params),     own_slice(mf, g, v_growth),
+                                   own_slice(mf, g, force_scale), own_slice(mf, g, fiber_body),
+                                   own_slice(mf, g, site_ref, 3), dt, eta, tol, num_blocks, max_iters};
         skb_dense *dn = mf->dn[(size_t)g].get();
         SKB_TRY(group_step_checks(fl, dn, dn, args[(size_t)g], info, who, calls[(size_t)g]));
         // (also the RHS's buffers at their size and its tables uploaded, as every skb_mflow RHS does first)
@@ -1122,6 +1101,7 @@ int skb_mflow_step(skb_mflow *mf, const skb_fiber_params *params, const double *
         if (x)
             member_local(mf, g, [&](long long whole, long long at, long long len) {
                 std::memcpy(x + whole, loc.data() + at, (size_t)len * 8);
+                return SKB_OK;
             });
         return rc_g;
     });

@@ -1,7 +1,7 @@
 // skb_system.cu -- the whole-system calls of a flow (include/skelly_b200_flow.h): the bodies' operators, frames,
 // placement and the fiber-body links, System::apply_matvec / ::apply_preconditioner and the RHS of the mobility system
-// on whole solution vectors -- on one device (skb_flow_*), on a member of skb_mflow (flow_member_*) and on one rank per
-// GPU (skb_flow_group_*) -- and the refusals they share.  Built on the matvec orchestration of skb_matvec.cu.
+// on whole solution vectors -- on one device (skb_flow_*) and on a group member (skb_flow_group_*, which skb_mflow
+// drives on its members) -- and the refusals they share.  Built on the matvec orchestration of skb_matvec.cu.
 #include "skb_flow.hpp"
 
 #include <algorithm>
@@ -84,9 +84,10 @@ static int body_window(skb_flow *fl, long long &lo, long long &hi) {
     return SKB_OK;
 }
 
-int skb::body_frames(skb_flow *fl, const char *who, const int *n_nodes, int n_bodies, const double *pos_ref,
-                     const double *normal_ref, const double *node_weights, const double *ex0, const double *ey0,
-                     const double *ez0, const double *A_inv0) {
+// the frames of the flow's bodies (a member: for its body rows)
+static int body_frames(skb_flow *fl, const char *who, const int *n_nodes, int n_bodies, const double *pos_ref,
+                       const double *normal_ref, const double *node_weights, const double *ex0, const double *ey0,
+                       const double *ez0, const double *A_inv0) {
     long long lo, hi;
     SKB_TRY(body_window(fl, lo, hi));
     if (n_bodies != fl->n_bodies)
@@ -129,7 +130,7 @@ int skb::placement_args(skb_flow *fl, const char *who, const double *centers, co
 
 // after placement_args: the nodes and normals through skb_flow_set_bodies (which drops the operators and the links),
 // then the operators from the frames
-int skb::place_bodies(skb_flow *fl, const double *centers, const double *orientations, const std::vector<double> &R) {
+static int place_bodies(skb_flow *fl, const double *centers, const double *orientations, const std::vector<double> &R) {
     std::vector<double> pos, nrm;
     fl->bodies.placed_geometry(R.data(), centers, pos, nrm);
     SKB_TRY(skb_flow_set_bodies(fl, pos.data(), nrm.data(), fl->n_body, centers, fl->n_bodies));
@@ -486,43 +487,8 @@ int skb_flow_build_system_rhs_device(skb_flow *fl, const skb_fiber_params *param
 
 } // extern "C"
 
-// ---- the whole-vector operator on a member of skb_mflow (skb_flow.hpp) -------------------------------------------
-// A member holds its own fibers' links and its body rows' operators (BodyOps); x_bodies is complete on every member.
-// The bodies' link forces are exchanged inside matvec_core (ft_exchange); a single flow (a one-device skb_mflow) takes
-// the path of skb_flow_apply_system_matvec.
-
-int skb::flow_member_body_operators(skb_flow *fl, const int *n_nodes, int n_bodies, const double *node_weights,
-                                    const double *ex, const double *ey, const double *ez, const double *A_inv) {
-    if (n_bodies != fl->n_bodies)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_set_body_operators: %d bodies, skb_mflow_set_bodies has %d",
-                         n_bodies, fl->n_bodies);
-    long long lo, hi;
-    SKB_TRY(body_window(fl, lo, hi));
-    return fl->bodies.set_operators(n_nodes, n_bodies, fl->n_body, fl->h_r_body.data(), fl->h_centers.data(),
-                                    node_weights, ex, ey, ez, A_inv, fl->stream, lo, hi);
-}
-
-int skb::flow_member_fiber_links(skb_flow *fl, const int *body, const double *site, const double *rigidity,
-                                 bool check_only) {
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    OwnFibers own = all_fibers(fl);
-    if (!check_only)
-        SKB_TRY(own_fibers(fl, "skb_mflow_set_fiber_links", own));
-    const int f0 = own.f0;
-    return fl->bodies.set_links(own, fl->ops, fl->n_bodies, fl->h_centers.data(), body ? body + f0 : nullptr,
-                                body ? site + 3 * (size_t)f0 : nullptr, body ? rigidity + f0 : nullptr, fl->stream,
-                                check_only);
-}
-
-int skb::flow_size_system(skb_flow *fl) {
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    SKB_TRY(prepare_matvec_targets(fl));
-    SKB_TRY(fl->tmp_b.ensure((size_t)(fl->bb - fl->ba) * 24 + 8));
-    return fl->ft_sum.ensure((size_t)fl->n_bodies * 48 + 8);
-}
-
-// the links of the own fibers, apply_matvec_core with the exchange of their partial forces, the owned body rows; on
-// fl->cur
+// a group member's: the links of the own fibers, apply_matvec_core with the exchange of their partial forces, the owned
+// body rows; on fl->cur
 static int member_system_matvec_core(skb_flow *fl, skb_dense *dn, const double *d_x_fib, const double *d_x_shell,
                                      const double *d_x_bodies, double eta, double *d_res_fib, double *d_res_shell,
                                      double *d_res_bodies) {
@@ -537,38 +503,11 @@ static int member_system_matvec_core(skb_flow *fl, skb_dense *dn, const double *
         t = fl->bodies.torques();
     }
     double *v_bodies = (double *)fl->tmp_b.ptr; // own body rows
-    fl->ft_exchange = fl->grp.member();
+    fl->ft_exchange = true;
     const int rc = apply_matvec_core(fl, dn, d_x_fib, d_x_shell, bd, f, t, link, eta, d_res_fib, d_res_shell, v_bodies);
     fl->ft_exchange = false;
     SKB_TRY(rc);
     return fl->n_bodies > 0 ? fl->bodies.matvec(d_x_bodies, v_bodies, d_res_bodies, fl->cur, &fl->launches) : SKB_OK;
-}
-
-int skb::flow_member_system_matvec(skb_flow *fl, skb_dense *dn, const double *d_x_fib, const double *d_x_shell,
-                                   const double *d_x_bodies, double eta, double *d_res_fib, double *d_res_shell,
-                                   double *d_res_bodies, cudaStream_t st) {
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    begin_stats(fl);
-    fl->cur = st;
-    SKB_TRY(member_system_matvec_core(fl, dn, d_x_fib, d_x_shell, d_x_bodies, eta, d_res_fib, d_res_shell,
-                                      d_res_bodies));
-    return device_stats(fl);
-}
-
-int skb::flow_member_system_precondition(skb_flow *fl, skb_dense *dn, const double *d_x_fib, const double *d_x_shell,
-                                         const double *d_x_bodies, double *d_y_fib, double *d_y_shell,
-                                         double *d_y_bodies, cudaStream_t st) {
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    begin_stats(fl);
-    fl->cur = st;
-    SKB_TRY(fl->ops.precondition(d_x_fib, d_y_fib, st, &fl->launches));
-    if (fl->sb > fl->sa) { // the member's rows of M_inv times the complete x_shell
-        SKB_TRY(skb_dense_apply_device(dn, SKB_DENSE_M_INV, d_x_shell, nullptr, d_y_shell, st));
-        fl->launches += 1;
-    }
-    if (fl->n_bodies > 0)
-        SKB_TRY(fl->bodies.precondition(d_x_bodies, d_y_bodies, st, &fl->launches));
-    return device_stats(fl);
 }
 
 // a member's slice of a per-fiber array of ALL fibers (NULL stays NULL, and so does the slice of no fibers)
@@ -595,28 +534,13 @@ int skb::flow_member_rhs_prepare(skb_flow *fl, const skb_fiber_params *params, c
                        });
 }
 
-int skb::flow_member_system_rhs(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
-                                const double *force_scale, const double *d_fext, const double *d_f, const double *d_t,
-                                double dt, double eta, double *d_rhs_fib, double *d_rhs_shell, double *d_rhs_bodies,
-                                cudaStream_t st) {
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    begin_stats(fl);
-    fl->cur = st;
-    OwnFibers own;
-    SKB_TRY(own_fibers(fl, "skb_mflow_build_system_rhs", own));
-    SKB_TRY(system_rhs_core(fl, own, own_slice(params, own), own_slice(v_growth, own), own_slice(force_scale, own),
-                            fl->fb > fl->fa ? d_fext : nullptr, d_f, d_t, dt, eta, d_rhs_fib, d_rhs_shell,
-                            d_rhs_bodies));
-    return device_stats(fl);
-}
-
 // ---- the whole-vector calls of a rank-per-GPU group member (skb_flow_group_*, include/skelly_b200_flow.h) ----------
 // A member holds only its own rows of the solution vector, in ascending global order (distributed.system_rows):
 // x_local = [4 per own fiber node | 3 per own periphery row | own body rows].  Before a matvec or a preconditioner it
 // stores its own body rows (and, for the preconditioner, its own periphery rows) into every window and meets its peers
-// at the rows phase; from there on the complete x_bodies / x_shell are in its own window, and the member path of
-// skb_mflow runs on them unchanged.  Body outputs land in the whole body layout (sys_rb) and are compacted to the own
-// rows in one launch.
+// at the rows phase; from there on the complete x_bodies / x_shell are in its own window.  Body outputs land in the
+// whole body layout (sys_rb) and are compacted to the own rows in one launch.  skb_mflow drives these calls on its
+// members (skb_mflow.cu).
 
 Group::Ranges skb::group_ranges(const skb_flow *fl) { return {fl->fa, fl->fb, fl->sa, fl->sb, fl->ba, fl->bb}; }
 
@@ -669,7 +593,8 @@ int skb::flow_member_lay_out_rows(skb_flow *fl, const char *who, const int *n_no
     // every buffer of the local-vector calls at its final size now: none of them allocates while a peer on this device
     // may wait on a flag (the warm-up sized the matvec flow's own)
     SKB_TRY(fl->sys_rb.ensure((size_t)sol * 8 + 8));
-    SKB_TRY(flow_size_system(fl));
+    SKB_TRY(fl->tmp_b.ensure((size_t)(fl->bb - fl->ba) * 24 + 8)); // the matvec's own v_bodies rows
+    SKB_TRY(fl->ft_sum.ensure((size_t)fl->n_bodies * 48 + 8));     // ... and its exchanged link forces
     SKB_TRY(load_dense_kernels()); // the preconditioner's M_inv rows (and the matvec's without the streamer)
     fl->grp.set_body_rows(pieces, group_ranges(fl));
     return SKB_OK;

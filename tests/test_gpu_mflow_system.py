@@ -279,6 +279,44 @@ def test_system_operator_iterations_match_the_reference_loop():
         assert rel_max(got, x) < 1e-11, (devs, rel_max(got, x))
 
 
+def test_a_new_partition_needs_no_new_body_set_up():
+    """set_fibers to another fiber count re-partitions the members and re-runs their group set-up; the whole-vector
+    calls lay the members' rows out again themselves, without a new set_body_operators or set_gmres, and give bitwise
+    what a MultiFlow set up on the new geometry gives.  Both bodies are cut between members."""
+    from test_gpu_system_edges import DT, edge_case, setup_mflow_edges
+    kw = dict(n_fibers=40, nodes=(8, 16, 24, 32), n_shell=300, n_body_nodes=600, n_bodies=2)
+    old = edge_case(kw, 56)
+    # 24 fibers of the same classes, so the classes already set stay valid; the periphery and bodies stay the old ones
+    fib, _, _, ops, links, x, params, _, src = edge_case(dict(kw, n_fibers=24), 57)
+    shell, bodies = old[1], old[2]
+
+    def calls(mf, x, params, src):
+        mf.set_point_sources(*src["points"])
+        mf.set_background(*src["background"])
+        return [mf.apply_system_matvec(x, ETA), mf.apply_system_preconditioner(x),
+                mf.build_system_rhs(*params, DT, ETA, f_external=src["f_ext"], body_forces_torques=src["ft"],
+                                    v_growth=src["v_growth"], force_scale=src["force_scale"])]
+
+    with skb.MultiFlow([0, 0, 0]) as mf:
+        setup_mflow_edges(mf, *old[:5])
+        mf.set_gmres(20)
+        calls(mf, old[5], old[6], old[8])
+        before = [mf.partition(g) for g in range(3)]
+        mf.set_fibers(fib["pos"], fib["n_nodes"], fib["lengths"])
+        mf.set_fiber_operators(ops["A"], ops["force"], ops["xs"], ops["length_prev"], ops["plus"])
+        mf.set_fiber_preconditioner(ops["A_inv"])
+        mf.set_fiber_links(links["body"], links["site"], links["rigidity"])
+        got = calls(mf, x, params, src)
+        parts = [mf.partition(g) for g in range(3)]
+    assert parts != before and all(p[4] % 300 and p[4] < p[5] for p in parts[1:]), (before, parts)
+    with skb.MultiFlow([0, 0, 0]) as mf:
+        setup_mflow_edges(mf, fib, shell, bodies, ops, links)
+        want = calls(mf, x, params, src)
+        assert [mf.partition(g) for g in range(3)] == parts
+    for g, w in zip(got, want):
+        assert np.array_equal(g, w)
+
+
 def _refused(call):
     with pytest.raises(skb.SkbError, match="error [14]:"):  # SKB_ERR_INVALID or SKB_ERR_STATE
         call()
