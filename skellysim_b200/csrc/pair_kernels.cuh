@@ -43,14 +43,6 @@ template <int KIND> struct KindTraits;
 template <> struct KindTraits<kStokeslet> { static constexpr int fdim = 3; };  // packed strengths / source
 template <> struct KindTraits<kStresslet> { static constexpr int fdim = 6; };  // sym6 combinations
 
-// Block row I of the symmetric path's upper triangle belongs to part owner(I): serpentine assignment, so that every
-// part gets the same number of long and short rows (one rank per GPU: each rank evaluates its rows, partial sums are
-// all-reduced).
-__host__ __device__ inline int sym_row_owner(int I, int n_parts) {
-    const int k = I / n_parts, m = I % n_parts;
-    return (k & 1) ? n_parts - 1 - m : m;
-}
-
 struct PairArgs {
     const double *r_src;   // [n_src_pad*3]   padded to a multiple of kSrcTile (pads replicate the last source)
     const double *f_src;   // [n_src_pad*fdim] padded with zeros

@@ -116,6 +116,8 @@ int upload_pageable(void *d_dst, const void *h_src, size_t bytes, cudaStream_t s
 int prepare_device(int dev);
 // the launch attributes of the kernels of fiber_ops.cuh and fiber_build.cuh (skb_fiber.cu); called by prepare_device
 int prepare_fiber_kernels();
+// ... and of the symmetric and cross kernels (skb_sym.cu)
+int prepare_sym_kernels();
 DeviceInfo query_device(int dev); // (of a prepared device)
 LaunchPlan plan_launch(const DeviceInfo &di, int kind, long long n_trg, int n_src_tiles, int force_T, int force_S);
 int launch_pair_sum(const DeviceInfo &di, int kind, const double *d_r_src, const double *d_f_packed, long long n_src,
@@ -566,9 +568,31 @@ class Krylov {
     std::vector<double> H_, cs_, sn_, g_, y_; // the Hessenberg matrix ((m + 1) x m, column-major) and its rotations
 };
 
+// ---- the symmetric and cross pair kernels' host side (skb_sym.cu, sym_kernels.cuh, cross_kernels.cuh) ----
+// One launch of either kernel on the device: its work items in launch order, row_begin (the items of every block row),
+// one forward-partial slab per item (F) and the reverse partials (P)
+struct ItemPlan {
+    DevBuf items, row_begin, F, P;
+    int n_items = 0, n_blocks = 0;
+};
+// The symmetric path of one set of Stokeslet sources: the plan of key (nb, part, parts) and what only it keeps
+struct SymState {
+    int self_state = -1; // -1 unknown, 0 targets do not start with these sources, 1 they do
+    ItemPlan plan;
+    std::array<int, 3> key = {0, 0, 0};
+    DevBuf row_ids, flag; // block row I of every row of P; the answer of the self check
+    int n_owned = 0;      // rows of P
+    long long pairs = 0;  // ordered (target, source) pairs one launch covers (both directions)
+};
+// The cross kernel's plan of key (node0, n_rows, n_sh, n_sh_pad, num_sms): one (fiber rows, periphery) shape
+struct CrossState {
+    ItemPlan plan;
+    std::array<long long, 5> key = {-1, -1, -1, -1, -1};
+};
+
 } // namespace skb
 
-// ---- context internals (shared by skb_runtime.cu and skb_matvec.cu) ----
+// ---- context internals (shared by skb_runtime.cu, skb_sym.cu and skb_matvec.cu) ----
 struct SourceSet {
     long long n = -1; // -1 = never set
     long long n_pad = 0;
@@ -586,12 +610,7 @@ struct SourceSet {
     bool excl = false;
     skb::DevBuf excl_ids, excl_trg;
     long long excl_trg_n = -1;
-    // symmetric (Newton's third law) path of the Stokeslet self-interaction, sym_kernels.cuh
-    int self_state = -1;       // -1 unknown, 0 targets do not start with these sources, 1 they do
-    bool sym_plan_valid = false;
-    int sym_nb = 0, sym_items = 0, sym_part = 0, sym_parts = 1, sym_owned = 0;
-    skb::DevBuf sym_item_buf, sym_row_begin, sym_P, sym_F, sym_row_ids /* block row I of every row of sym_P */, sym_flag;
-    long long sym_pairs = 0; // ordered (target, source) pairs one launch of the symmetric kernel covers (both directions)
+    skb::SymState sym; // symmetric (Newton's third law) path of the Stokeslet self-interaction
 };
 
 struct DeviceState {
@@ -640,15 +659,17 @@ int eval_on_device(skb_ctx *ctx, DeviceState &d, int kind, StrengthMode mode, co
 int pack_on_device(DeviceState &d, int kind, StrengthMode mode, const double *d_f_raw, double two_eta, cudaStream_t st,
                    int *launches);
 
-// fiber <-> periphery in one geometry pass (cross_kernels.cuh): plan and partial buffers of one (fiber rows, periphery)
-// shape
-struct CrossState {
-    bool valid = false;
-    long long node0 = -1, n_rows = -1, n_sh = -1, n_sh_pad = -1;
-    int n_blocks = 0, n_items = 0, num_sms = 0;
-    DevBuf items, row_begin, P, F;
-};
-long long cross_block_nodes();
+// the symmetric and cross kernels (skb_sym.cu)
+long long sym_block_nodes(); // nodes per block of the symmetric kernel (its I side)
+long long sym_mem_budget();  // bytes its reverse partials may occupy on one device
+// are the first n_src targets bit-identical to the Stokeslet sources (s.sym.self_state, decided once per positions)?
+int ensure_self_state(DeviceState &d, SourceSet &s, cudaStream_t st);
+// Decide whether the symmetric path serves d's Stokeslet sources (*use) and make sure its plan and buffers exist
+int sym_prepare(skb_ctx *ctx, DeviceState &d, cudaStream_t st, int *use);
+// u[0 : 3 n_src] (=|+=) scale_mul / (8 pi) * sum over the square block, using the plan above.  Strengths are packed
+int sym_eval(DeviceState &d, double *d_u_out, int accumulate, cudaStream_t st, double scale_mul, int *launches);
+LaunchPlan sym_launch_plan(const SourceSet &s); // the last symmetric launch, as the stats report it
+// fiber <-> periphery in one geometry pass (cross_kernels.cuh), on the plan of cs (made again for a new shape):
 // u_fib[n_rows x 3] (=|+=) scale_dl * (stresslet sums of ALL periphery nodes at fiber nodes [node0, node0 + n_rows));
 // u_shell[n_sh x 3] (=|+=) scale_sl * (Stokeslet sums of those fiber nodes at every periphery node).
 // r_fib / h: positions and packed Stokeslet strengths of all fiber nodes (padded); r_sh / s6: periphery, padded.
@@ -656,11 +677,6 @@ int cross_eval(CrossState &cs, const DeviceInfo &di, const double *d_r_fib, cons
                long long n_rows, const double *d_r_sh, const double *d_s6, long long n_sh, long long n_sh_pad,
                double scale_dl, double scale_sl, double *d_u_fib, int acc_fib, double *d_u_shell, int acc_shell,
                cudaStream_t st, int *launches);
-
-struct SymItem;
-long long sym_block_nodes(); // nodes per block of the symmetric kernel (its I side)
-void build_sym_items(int nb, int part, int parts, int num_sms, std::vector<SymItem> &order,
-                     std::vector<int> &row_begin);
 
 // NCCL is bound at run time (dlopen "libnccl.so.2"): a single-GPU user never needs it, and a host that
 // already loaded NCCL (PyTorch) shares that copy instead of getting a second one.

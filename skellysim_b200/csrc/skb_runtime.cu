@@ -1,12 +1,10 @@
-// skb_runtime.cu -- host side of libskelly_b200.so: evaluator contexts, launch planning, the C ABI
-// declared in include/skelly_b200.h, and the reference-named C++ entry points
-// kernels::stokeslet_direct_gpu_impl / kernels::stresslet_direct_gpu_impl (SkellySim
+// skb_runtime.cu -- host side of libskelly_b200.so: evaluator contexts, the plain kernel's launch planning, the C ABI
+// declared in include/skelly_b200.h (the symmetric and cross kernels' host side: skb_sym.cu), and the reference-named
+// C++ entry points kernels::stokeslet_direct_gpu_impl / kernels::stresslet_direct_gpu_impl (SkellySim
 // include/kernels.hpp:17-20) so the library links in place of src/core/kernels.cu.
 //
 // No CPU fallback exists here: every path ends in a CUDA launch or an error code.
 #include "pair_kernels.cuh"
-#include "sym_kernels.cuh"
-#include "cross_kernels.cuh"
 #include "stream_kernels.cuh"
 #include "skb_internal.hpp"
 
@@ -348,16 +346,10 @@ int skb::prepare_device(int dev) {
 #undef SMEM_CALL
 #undef SMEM_CALL_EXCL
     }
-    auto set_shared = [](auto kern, int bytes) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-        return e == cudaSuccess ? cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                                       cudaSharedmemCarveoutMaxShared)
-                                : e;
-    };
-    CUDA_TRY(set_shared(pair_sym_kernel<kSymT, kSymMinB, false>, SymSmem<kSymT>::total_bytes));
-    CUDA_TRY(set_shared(pair_sym_kernel<kSymT, kSymMinB, true>, SymSmem<kSymT>::total_bytes));
-    CUDA_TRY(set_shared(pair_cross_kernel<kCrossT, kCrossMinB>, CrossSmem<kCrossT>::total_bytes));
-    CUDA_TRY(set_shared(dense_stream_kernel, kStreamSmemBytes));
+    SKB_TRY(prepare_sym_kernels());
+    CUDA_TRY(cudaFuncSetAttribute(dense_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kStreamSmemBytes));
+    CUDA_TRY(cudaFuncSetAttribute(dense_stream_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                  cudaSharedmemCarveoutMaxShared));
     SKB_TRY(prepare_fiber_kernels());
     if (dev >= (int)done.size())
         done.resize(dev + 1);
@@ -502,52 +494,10 @@ int skb_plan_query(int kind, int64_t n_trg, int64_t n_src, int num_sms, const in
     return SKB_OK;
 }
 
-int skb_sym_plan_query(int n_blocks, int part, int n_parts, int num_sms, int max_items, int *items4, int *n_items,
-                       int *row_begin) {
-    if (n_blocks < 1 || n_parts < 1 || part < 0 || part >= n_parts || num_sms < 1 || !n_items)
-        return set_error(SKB_ERR_INVALID, "skb_sym_plan_query: bad arguments");
-    std::vector<SymItem> order;
-    std::vector<int> rb;
-    build_sym_items(n_blocks, part, n_parts, num_sms, order, rb);
-    *n_items = (int)order.size();
-    if (items4)
-        for (int i = 0; i < (int)order.size() && i < max_items; ++i) {
-            items4[4 * i + 0] = order[i].I;
-            items4[4 * i + 1] = order[i].g0;
-            items4[4 * i + 2] = order[i].g1;
-            items4[4 * i + 3] = order[i].slot;
-        }
-    if (row_begin)
-        for (int b = 0; b <= n_blocks; ++b)
-            row_begin[b] = rb[b];
-    return SKB_OK;
-}
-
-int skb_sym_groups_per_block(void) { return kSymGroupsPerBlock; }
-
 int skb_ctx_last_eval_was_symmetric(const skb_ctx *ctx, int *yes) {
     if (!ctx || !yes)
         return set_error(SKB_ERR_INVALID, "skb_ctx_last_eval_was_symmetric: NULL");
     *yes = ctx->last_was_sym ? 1 : 0;
-    return SKB_OK;
-}
-
-int skb_ctx_last_sym_kernel(const skb_ctx *ctx, double *ms, int64_t *pairs) {
-    if (!ctx || !ms || !pairs)
-        return set_error(SKB_ERR_INVALID, "skb_ctx_last_sym_kernel: NULL");
-    *ms = 0;
-    *pairs = 0;
-    const DeviceState &d = ctx->devs[0];
-    if (!d.sym_timed)
-        return SKB_OK;
-    float t = 0;
-    cudaSetDevice(d.info.dev);
-    if (cudaEventElapsedTime(&t, d.ev_s0, d.ev_s1) == cudaSuccess) {
-        *ms = t;
-        *pairs = d.src[SKB_STOKESLET].sym_pairs;
-    } else {
-        (void)cudaGetLastError(); // not finished yet
-    }
     return SKB_OK;
 }
 
@@ -612,8 +562,7 @@ static int set_targets_impl(skb_ctx *ctx, const double *r_trg, long long n_trg, 
     }
     partition_targets(ctx, n_trg);
     for (auto &d : ctx->devs) {
-        d.src[0].self_state = -1;
-        d.src[1].self_state = -1;
+        d.src[0].sym.self_state = -1;
         d.src[0].excl_trg_n = -1;
         if (d.n_trg == 0)
             continue;
@@ -632,11 +581,6 @@ static int set_targets_impl(skb_ctx *ctx, const double *r_trg, long long n_trg, 
     return SKB_OK;
 }
 
-namespace skb {
-static long long sym_mem_budget();
-static int sym_owned_rows(int nb, int part, int parts);
-}
-
 // Multi-device contexts (host-pointer API): put the targets on the devices.  Plain layout: contiguous blocks.
 // Symmetric layout (the targets start with the Stokeslet sources, no stresslet sources in this context): every
 // device holds ALL n_self leading targets -- it evaluates its serpentine share of the self-interaction's block rows
@@ -647,7 +591,7 @@ static int update_layout(skb_ctx *ctx) {
     const long long P = (long long)ctx->devs.size();
     const long long n_trg = ctx->n_trg;
     const long long n_sl = ctx->devs[0].src[SKB_STOKESLET].n, n_dl = ctx->devs[0].src[SKB_STRESSLET].n;
-    const long long block = (long long)kSymThreads * kSymT;
+    const long long block = sym_block_nodes();
     bool want = ctx->sym_mode != 0 && n_dl <= 0 && n_sl >= (ctx->sym_mode == 1 ? 2 * block : 4096) && n_trg >= n_sl &&
                 (long long)ctx->h_src[SKB_STOKESLET].size() == 3 * n_sl &&
                 std::memcmp(ctx->h_trg.data(), ctx->h_src[SKB_STOKESLET].data(), (size_t)n_sl * 24) == 0;
@@ -678,8 +622,7 @@ static int update_layout(skb_ctx *ctx) {
         }
     }
     for (auto &d : ctx->devs) {
-        d.src[0].self_state = want ? 1 : 0; // decided on the host copies
-        d.src[1].self_state = 0;
+        d.src[0].sym.self_state = want ? 1 : 0; // decided on the host copies
         if (d.n_trg == 0)
             continue;
         CUDA_TRY(cudaSetDevice(d.info.dev));
@@ -737,7 +680,7 @@ static int set_sources_impl(skb_ctx *ctx, int kind, const double *r_src, long lo
         s.has_weights = false;
         s.excl = false;    // ids belong to one set of sources
         s.excl_trg_n = -1;
-        s.self_state = -1; // (the symmetric plan depends on the block count only and survives position updates)
+        s.sym.self_state = -1; // (the symmetric plan depends on the block count only and survives position updates)
         if (n_src == 0)
             continue;
         CUDA_TRY(cudaSetDevice(d.info.dev));
@@ -768,323 +711,6 @@ static int set_sources_impl(skb_ctx *ctx, int kind, const double *r_src, long lo
 // ------------------------------------------------------------------------------------------------
 // evaluation
 // ------------------------------------------------------------------------------------------------
-
-// device-side part for one device: pack -> pair kernel -> reduce into d_u_out.  f_raw already resident.
-
-// ------------------------------------------------------------------------------------------------
-// symmetric Stokeslet self-interaction (sym_kernels.cuh)
-// ------------------------------------------------------------------------------------------------
-namespace skb {
-
-__global__ void self_check_kernel(const double *__restrict__ a, const double *__restrict__ b, long long n,
-                                  int *__restrict__ differs) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n && __double_as_longlong(a[i]) != __double_as_longlong(b[i]))
-        *differs = 1;
-}
-
-template <bool EXCL> static cudaError_t launch_sym(const SymArgs &a, int n_items, cudaStream_t st) {
-    pair_sym_kernel<kSymT, kSymMinB, EXCL><<<n_items, kSymThreads, SymSmem<kSymT>::total_bytes, st>>>(a);
-    return cudaGetLastError();
-}
-
-// bytes the reverse partials of the symmetric kernel may occupy: SKB_SYM_MAX_BYTES, else 30 % of the device memory
-// (at least 8 GiB): 24 GB on one 80 GB H100, so a 1e6-node self-interaction (47 GB) takes the plain kernel on one GPU
-// and the symmetric one from 2 GPUs on (1/P of that per rank with the row partition)
-static long long sym_mem_budget() {
-    static long long cached = -1; // all devices of a box are alike; the environment is read once
-    if (cached >= 0)
-        return cached;
-    if (const char *e = getenv("SKB_SYM_MAX_BYTES"))
-        return cached = atoll(e);
-    size_t free_b = 0, total_b = 0;
-    if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess)
-        return cached = 8LL << 30;
-    return cached = std::max<long long>(8LL << 30, (long long)(0.30 * (double)total_b));
-}
-long long sym_block_nodes() { return (long long)kSymThreads * kSymT; }
-static int sym_owned_rows(int nb, int part, int parts) {
-    int n = 0;
-    for (int I = 0; I < nb; ++I)
-        n += sym_row_owner(I, parts) == part;
-    return n;
-}
-
-// One row of work items: block I of the I side meets the J groups [g0, g0 + n_groups); its items write row prow of P.
-struct ItemRow {
-    int I, g0, n_groups, prow;
-};
-
-// The work items of one launch of the symmetric or the cross kernel: `rows` (in increasing I) cut into items (I, groups
-// [g0, g1)), in units of 32-node groups.  Guided sizes: most of the work goes out in large items (about a quarter of a
-// CTA slot's share each), the last ~30 % in items a quarter of that size and the last ~8 % in single stages (4 groups =
-// 17 us of one CTA slot), so that all `slots` CTA slots drain together: the hardware hands the next item to whichever
-// slot frees up first, in `order` (large items first).  item.slot is the item's row-major position,
-// row_begin[b]..row_begin[b+1] the slots of block row b < n_blocks (their forward partials are summed in that order by
-// the reduction kernel).
-static void cut_items(const std::vector<ItemRow> &rows, int n_blocks, long long slots, std::vector<SymItem> &order,
-                      std::vector<int> &row_begin) {
-    const int sg = kSymStageGroups;
-    long long work = 0;
-    for (const ItemRow &r : rows)
-        work += r.n_groups;
-    long long big = work / std::max<long long>(1, slots * 4); // 4 large items per CTA slot (if all work were large items)
-    big = std::max<long long>(sg, std::min<long long>(big / sg * sg, 1024LL * sg));
-    const long long mid = std::max<long long>(sg, big / 4 / sg * sg);
-    struct Piece {
-        int I, g0, g1, prow;
-    };
-    std::vector<Piece> pieces;
-    for (const ItemRow &r : rows) {
-        const int len = r.n_groups;
-        const int n_chunks = (int)((len + big - 1) / big);
-        for (int c = 0; c < n_chunks; ++c) { // near-equal chunks, cut at stage boundaries
-            const int a = (int)((long long)(len / sg) * c / n_chunks) * sg;
-            const int b = c + 1 == n_chunks ? len : (int)((long long)(len / sg) * (c + 1) / n_chunks) * sg;
-            if (b > a)
-                pieces.push_back(Piece{r.I, r.g0 + a, r.g0 + b, r.prow});
-        }
-    }
-    // the tail of the launch order is cut finer
-    std::stable_sort(pieces.begin(), pieces.end(),
-                     [](const Piece &x, const Piece &y) { return (x.g1 - x.g0) > (y.g1 - y.g0); });
-    std::vector<Piece> fine;
-    long long done = 0;
-    // (at most ~6 items of a tier per CTA slot: more would only add forward-partial slabs)
-    const long long fine_work = std::min<long long>(work * 8 / 100, slots * 6 * sg);
-    const long long mid_work = std::min<long long>(work * 30 / 100, fine_work + slots * 6 * mid);
-    for (const Piece &pc : pieces) {
-        const long long len = pc.g1 - pc.g0;
-        const long long left = work - done;
-        const long long unit = left <= fine_work ? sg : left <= mid_work ? mid : len;
-        for (long long g = pc.g0; g < pc.g1; g += unit)
-            fine.push_back(Piece{pc.I, (int)g, (int)std::min<long long>(pc.g1, g + unit), pc.prow});
-        done += len;
-    }
-    // slots: row-major
-    std::sort(fine.begin(), fine.end(),
-              [](const Piece &x, const Piece &y) { return x.I != y.I ? x.I < y.I : x.g0 < y.g0; });
-    std::vector<SymItem> items(fine.size());
-    row_begin.assign(n_blocks + 1, 0);
-    for (size_t i = 0; i < fine.size(); ++i) {
-        items[i] = SymItem{fine[i].I, fine[i].g0, fine[i].g1, (int)i, fine[i].prow, 0};
-        row_begin[fine[i].I + 1] = (int)i + 1;
-    }
-    for (int b = 0; b < n_blocks; ++b) // rows without items inherit the running count
-        row_begin[b + 1] = std::max(row_begin[b + 1], row_begin[b]);
-    order = items;
-    std::stable_sort(order.begin(), order.end(),
-                     [](const SymItem &x, const SymItem &y) { return (x.g1 - x.g0) > (y.g1 - y.g0); });
-}
-
-// Work items of the symmetric kernel: the upper triangle of nb blocks INCLUDING the block diagonal (row I starts at its
-// own first group), restricted to the block rows owned by `part`.
-void build_sym_items(int nb, int part, int parts, int num_sms, std::vector<SymItem> &order,
-                     std::vector<int> &row_begin) {
-    const int gpb = kSymGroupsPerBlock;
-    std::vector<ItemRow> rows;
-    for (int I = 0; I < nb; ++I) // every owned row has a P row, in increasing I (sym_reduce_kernel counts the same way)
-        if (sym_row_owner(I, parts) == part)
-            rows.push_back(ItemRow{I, gpb * I, gpb * (nb - I), (int)rows.size()});
-    cut_items(rows, nb, (long long)num_sms * kSymMinB, order, row_begin);
-}
-
-// Puts a plan on the device: the items in launch order, row_begin, and one forward-partial slab (block x 3 doubles) per
-// item.  Waits for the copies: the host vectors may go out of scope on return.
-static int upload_plan(const std::vector<SymItem> &order, const std::vector<int> &row_begin, long long block,
-                       DevBuf &items, DevBuf &d_row_begin, DevBuf &F, cudaStream_t st) {
-    SKB_TRY(items.ensure(order.size() * sizeof(SymItem) + 16));
-    SKB_TRY(d_row_begin.ensure(row_begin.size() * sizeof(int)));
-    SKB_TRY(F.ensure(order.size() * (size_t)block * 24 + 16));
-    CUDA_TRY(cudaMemcpyAsync(items.ptr, order.data(), order.size() * sizeof(SymItem), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(d_row_begin.ptr, row_begin.data(), row_begin.size() * sizeof(int), cudaMemcpyHostToDevice,
-                             st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    return SKB_OK;
-}
-
-// Are the first n_src targets bit-identical to the Stokeslet sources?  (decided once per set of positions)
-static int ensure_self_state(DeviceState &d, SourceSet &s, cudaStream_t st) {
-    if (s.self_state >= 0)
-        return SKB_OK;
-    if (d.n_trg < s.n || s.n <= 0) {
-        s.self_state = 0;
-        return SKB_OK;
-    }
-    SKB_TRY(s.sym_flag.ensure(sizeof(int)));
-    CUDA_TRY(cudaMemsetAsync(s.sym_flag.ptr, 0, sizeof(int), st));
-    const long long n3 = 3 * s.n;
-    self_check_kernel<<<(unsigned)((n3 + 255) / 256), 256, 0, st>>>((const double *)d.r_trg.ptr, (const double *)s.r.ptr,
-                                                                    n3, (int *)s.sym_flag.ptr);
-    CUDA_TRY(cudaGetLastError());
-    count_launch(1);
-    int differs = 1;
-    CUDA_TRY(cudaMemcpyAsync(&differs, s.sym_flag.ptr, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    s.self_state = differs ? 0 : 1;
-    return SKB_OK;
-}
-
-// Decide whether the symmetric path applies and make sure its plan / buffers exist.
-static int sym_prepare(skb_ctx *ctx, DeviceState &d, cudaStream_t st, int *use) {
-    *use = 0;
-    SourceSet &s = d.src[SKB_STOKESLET];
-    const long long block = sym_block_nodes();
-    if (s.n < 4096 && ctx->sym_mode != 1)
-        return SKB_OK; // too small to matter
-    if (s.n < 2 * block || d.n_trg < s.n)
-        return SKB_OK;
-    const long long nb = s.n_pad / block; // n_pad is a multiple of 1024
-    if ((long long)sym_owned_rows((int)nb, d.sym_part, d.sym_parts) * s.n_pad * 24 > sym_mem_budget())
-        return SKB_OK;
-    SKB_TRY(ensure_self_state(d, s, st));
-    if (s.self_state != 1)
-        return SKB_OK;
-    if (!s.sym_plan_valid || s.sym_nb != (int)nb || s.sym_part != d.sym_part || s.sym_parts != d.sym_parts) {
-        std::vector<int> owned; // block rows of P's rows, for sym_reduce_kernel
-        for (int I = 0; I < (int)nb; ++I)
-            if (sym_row_owner(I, d.sym_parts) == d.sym_part)
-                owned.push_back(I);
-        const size_t p_bytes = owned.size() * (size_t)s.n_pad * 24;
-        if (s.sym_P.ensure(p_bytes) != SKB_OK) { // not enough free memory for the reverse partials: the plain kernel
-                                                 // serves this geometry
-            (void)cudaGetLastError();
-            if (ctx->sym_layout) // every device holds ALL leading targets there and the caller reduce-scatters the
-                                 // partial sums: a silent switch to the plain kernel would count them P times
-                return set_error(SKB_ERR_ALLOC, "symmetric multi-device layout: no memory for the reverse partials "
-                                                "(%zu bytes); free memory or skb_ctx_set_symmetric(ctx, 0)",
-                                 p_bytes);
-            s.self_state = 0;
-            return SKB_OK;
-        }
-        SKB_TRY(s.sym_row_ids.ensure(owned.size() * sizeof(int) + 16));
-        CUDA_TRY(cudaMemcpyAsync(s.sym_row_ids.ptr, owned.data(), owned.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-        s.sym_owned = (int)owned.size();
-        std::vector<SymItem> order;
-        std::vector<int> row_begin;
-        build_sym_items((int)nb, d.sym_part, d.sym_parts, d.info.num_sms, order, row_begin);
-        SKB_TRY(upload_plan(order, row_begin, block, s.sym_item_buf, s.sym_row_begin, s.sym_F, st));
-        // pairs of one launch: every ordered pair of real nodes in (owned row I, any block J > I), both directions
-        long long pairs = 0;
-        for (long long I = 0; I < nb; ++I) {
-            if (sym_row_owner((int)I, d.sym_parts) != d.sym_part)
-                continue;
-            const long long nI = std::max<long long>(0, std::min<long long>(s.n, (I + 1) * block) - I * block);
-            const long long after = std::max<long long>(0, s.n - (I + 1) * block);
-            pairs += 2 * nI * after + nI * nI; // both directions beyond the block + the block diagonal
-        }
-        s.sym_pairs = pairs;
-        s.sym_nb = (int)nb;
-        s.sym_items = (int)order.size();
-        s.sym_part = d.sym_part;
-        s.sym_parts = d.sym_parts;
-        s.sym_plan_valid = true;
-    }
-    *use = 1;
-    return SKB_OK;
-}
-
-// u[0 : 3 n_src] (=|+=) scale * sum over the square block, using the plan above.  Strengths are packed already.
-static int sym_eval(skb_ctx *ctx, DeviceState &d, double *d_u_out, int accumulate, cudaStream_t st, double scale_mul,
-                    int *launches) {
-    SourceSet &s = d.src[SKB_STOKESLET];
-    const double *f_packed = s.f_cur;
-    if (!d.aux_stream)
-        CUDA_TRY(cudaStreamCreateWithFlags(d.aux_stream.out(), cudaStreamNonBlocking));
-    const long long block = sym_block_nodes();
-    SymArgs a;
-    a.r = (const double *)s.r.ptr;
-    a.f = f_packed;
-    a.items = (const SymItem *)s.sym_item_buf.ptr;
-    a.P = (double *)s.sym_P.ptr;
-    a.F = (double *)s.sym_F.ptr;
-    a.n_pad = s.n_pad;
-    a.nb = s.sym_nb;
-    cudaError_t e = cudaSuccess;
-    if (s.sym_items > 0) {
-        a.fid = s.excl ? (const int *)s.excl_ids.ptr : nullptr;
-        CUDA_TRY(cudaEventRecord(d.ev_s0, st));
-        e = s.excl ? launch_sym<true>(a, s.sym_items, st) : launch_sym<false>(a, s.sym_items, st);
-        if (e == cudaSuccess)
-            CUDA_TRY(cudaEventRecord(d.ev_s1, st));
-        d.sym_timed = true;
-        if (e != cudaSuccess)
-            return set_error(SKB_ERR_CUDA, "pair_sym_kernel launch failed: %s", cudaGetErrorString(e));
-        count_launch(1);
-    }
-    const long long n3 = 3 * s.n;
-    const double scale = scale_mul / (8.0 * M_PI);
-    sym_reduce_kernel<<<(unsigned)((n3 + 255) / 256), 256, 0, st>>>(
-        (const double *)s.sym_P.ptr, (const double *)s.sym_F.ptr, (const int *)s.sym_row_begin.ptr,
-        (const int *)s.sym_row_ids.ptr, s.sym_owned, (int)block, s.n_pad, n3, scale, accumulate, d_u_out);
-    e = cudaGetLastError();
-    if (e != cudaSuccess)
-        return set_error(SKB_ERR_CUDA, "sym_reduce_kernel launch failed: %s", cudaGetErrorString(e));
-    count_launch(1);
-    if (launches)
-        *launches += 2;
-    (void)ctx;
-    return SKB_OK;
-}
-
-} // namespace skb
-
-namespace skb {
-
-long long cross_block_nodes() { return kCrossBlock; }
-
-int cross_eval(CrossState &cs, const DeviceInfo &di, const double *d_r_fib, const double *d_h, long long node0,
-               long long n_rows, const double *d_r_sh, const double *d_s6, long long n_sh, long long n_sh_pad,
-               double scale_dl, double scale_sl, double *d_u_fib, int acc_fib, double *d_u_shell, int acc_shell,
-               cudaStream_t st, int *launches) {
-    if (n_rows <= 0 || n_sh <= 0)
-        return SKB_OK;
-    const long long block = kCrossBlock;
-    const int n_blocks = (int)((n_rows + block - 1) / block);
-    const int n_groups = (int)((n_sh + kSymGroup - 1) / kSymGroup);
-    if (!cs.valid || cs.node0 != node0 || cs.n_rows != n_rows || cs.n_sh != n_sh || cs.n_sh_pad != n_sh_pad ||
-        cs.num_sms != di.num_sms) {
-        // items: rectangles (fiber block I, periphery groups [g0, g1)), every block meets every group
-        std::vector<ItemRow> rows;
-        for (int I = 0; I < n_blocks; ++I)
-            rows.push_back(ItemRow{I, 0, n_groups, I});
-        std::vector<SymItem> order;
-        std::vector<int> row_begin;
-        cut_items(rows, n_blocks, (long long)di.num_sms * kCrossMinB, order, row_begin);
-        SKB_TRY(cs.P.ensure((size_t)n_blocks * (size_t)n_sh_pad * 24));
-        SKB_TRY(upload_plan(order, row_begin, block, cs.items, cs.row_begin, cs.F, st));
-        cs.node0 = node0, cs.n_rows = n_rows, cs.n_sh = n_sh, cs.n_sh_pad = n_sh_pad;
-        cs.n_blocks = n_blocks, cs.n_items = (int)order.size(), cs.num_sms = di.num_sms;
-        cs.valid = true;
-    }
-    CrossArgs a;
-    a.r_fib = d_r_fib;
-    a.h = d_h;
-    a.r_sh = d_r_sh;
-    a.s6 = d_s6;
-    a.items = (const SymItem *)cs.items.ptr;
-    a.P = (double *)cs.P.ptr;
-    a.F = (double *)cs.F.ptr;
-    a.n_sh_pad = n_sh_pad;
-    a.node0 = node0;
-    a.n_rows = n_rows;
-    pair_cross_kernel<kCrossT, kCrossMinB><<<cs.n_items, kSymThreads, CrossSmem<kCrossT>::total_bytes, st>>>(a);
-    CUDA_TRY(cudaGetLastError());
-    const long long nr3 = 3 * n_rows, ns3 = 3 * n_sh;
-    cross_reduce_fib_kernel<<<(unsigned)((nr3 + 255) / 256), 256, 0, st>>>(
-        (const double *)cs.F.ptr, (const int *)cs.row_begin.ptr, (int)block, nr3, scale_dl, acc_fib, d_u_fib);
-    cross_reduce_shell_kernel<<<(unsigned)((ns3 + 255) / 256), 256, 0, st>>>((const double *)cs.P.ptr, n_blocks,
-                                                                              n_sh_pad, ns3, scale_sl, acc_shell,
-                                                                              d_u_shell);
-    CUDA_TRY(cudaGetLastError());
-    count_launch(3);
-    if (launches)
-        *launches += 3;
-    return SKB_OK;
-}
-
-} // namespace skb
-
 namespace skb {
 __global__ void excl_target_ids_kernel(const int *__restrict__ src_ids, long long n_src, long long trg_begin,
                                        long long n_trg, int *__restrict__ out) {
@@ -1142,7 +768,7 @@ int eval_on_device(skb_ctx *ctx, DeviceState &d, int kind, StrengthMode mode, co
     const bool excl = kind == SKB_STOKESLET && s.excl;
     if (excl && ctx->devs.size() == 1) { // (multi-device contexts check their host copies of the positions, eval_host)
         SKB_TRY(ensure_self_state(d, s, st));
-        if (s.self_state != 1)
+        if (s.sym.self_state != 1)
             return set_error(SKB_ERR_STATE, "exclusion ids are set, but the targets do not start with the Stokeslet "
                                             "sources (skb_set_source_exclusion_ids)");
     }
@@ -1170,7 +796,7 @@ int eval_on_device(skb_ctx *ctx, DeviceState &d, int kind, StrengthMode mode, co
     LaunchPlan plan{};
     // the long symmetric kernel is launched first so that the remainder's CTAs are dispatched into its tail
     if (n_sym > 0)
-        SKB_TRY(sym_eval(ctx, d, opts.d_u_sym ? opts.d_u_sym : d_u_out,
+        SKB_TRY(sym_eval(d, opts.d_u_sym ? opts.d_u_sym : d_u_out,
                          opts.sym_accumulate >= 0 ? opts.sym_accumulate : accumulate, st, scale_mul, launches));
     if (n_trg_std > 0) {
         const int *d_src_ids = nullptr, *d_trg_ids = nullptr;
@@ -1203,10 +829,7 @@ int eval_on_device(skb_ctx *ctx, DeviceState &d, int kind, StrengthMode mode, co
             CUDA_TRY(cudaEventRecord(d.ev_join, d.aux_stream));
             CUDA_TRY(cudaStreamWaitEvent(st, d.ev_join, 0));
         }
-        plan.T = kSymT;
-        plan.n_splits = 1;
-        plan.grid_x = (unsigned)s.sym_items;
-        plan.tiles_per_split = 0;
+        plan = sym_launch_plan(s);
     }
     if (record_events)
         CUDA_TRY(cudaEventRecord(d.ev_k1, st));

@@ -11,7 +11,7 @@
 // upper triangle (both directions from one geometry pass); the groups of block I itself are the block diagonal, where
 // the forward sums alone already cover every ordered pair (their reverse sums land in a part of P nobody reads).  The
 // non-square remainder (targets beyond the sources) goes through pair_sum_kernel.  Items are as fine as one group (512*T/4 x 32 pairs), so the
-// planner can hand out large items first and small ones last (build_sym_items): the kernel's tail -- and the tail of
+// planner can hand out large items first and small ones last (cut_items, skb_sym.cu): the kernel's tail -- and the tail of
 // every rank's share under multi-GPU sharding -- is a few stages, not one block pair.
 // J groups are staged in shared memory by TMA, up to 4 groups per stage in a 4-stage ring; within a warp the 32 lanes
 // walk a group as a ring: at step s lane l meets node (l + s) mod 32, and that node's reverse accumulator
@@ -20,8 +20,10 @@
 // shared-memory slab; once per stage the four slabs are added in a fixed order (bitwise reproducible) and written to
 // the reverse partial P[row(I)][J nodes].  The final combination (sym_reduce_kernel) is a fixed-order sum.
 #pragma once
-#include "pair_kernels.cuh"
+#include <cstdint>
 #include <type_traits>
+
+#include "tma_ptx.cuh"
 
 namespace skb {
 

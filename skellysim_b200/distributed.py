@@ -52,7 +52,7 @@ def allgather_strengths(gathered, mine, group=None):
 
 def sym_row_owner(block_row: int, n_parts: int) -> int:
     """Owner of block row I of the symmetric kernel's upper triangle (mirror of sym_row_owner in
-    csrc/pair_kernels.cuh): serpentine over rows, so every rank gets the same mix of long and short rows."""
+    csrc/skb_sym.cu): serpentine over rows, so every rank gets the same mix of long and short rows."""
     k, m = divmod(block_row, n_parts)
     return n_parts - 1 - m if (k & 1) else m
 

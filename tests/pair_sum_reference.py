@@ -168,7 +168,7 @@ def k_cross(kind, n_src):
 
 # ---- structure ----------------------------------------------------------------------------------------------------
 def sym_row_owner(I, n_parts):
-    """pair_kernels.cuh sym_row_owner: serpentine"""
+    """skb_sym.cu sym_row_owner: serpentine"""
     k, m = divmod(I, n_parts)
     return n_parts - 1 - m if k & 1 else m
 
