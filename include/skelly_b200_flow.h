@@ -538,7 +538,8 @@ typedef struct skb_step_info {
     skb_solve_info solve; /* as skb_flow_solve_system */
     double fiber_error;   /* max over fibers and nodes after the step; 0 without fibers; NaN: not installed */
     int32_t worst_fiber;  /* the fiber attaining it, -1 without fibers */
-    int32_t reserved;
+    int32_t collided;     /* System::check_collision of the installed geometry (skb_flow_set_periphery_shape); 0
+                             without a shape or when the step was not installed */
 } skb_step_info;
 SKB_API int skb_flow_step(skb_flow *fl, struct skb_dense *dn, const skb_fiber_params *params, const double *v_growth,
                           const double *force_scale, const double *f_external, const double *body_forces_torques,
@@ -580,6 +581,55 @@ SKB_API int skb_flow_group_step_device(skb_flow *fl, struct skb_dense *dn_spc, s
                                        double *d_tension, skb_step_info *info, void *stream);
 SKB_API int skb_flow_get_placement(skb_flow *fl, double *centers, double *orientations);
 SKB_API int skb_flow_get_fibers(skb_flow *fl, double *r_fib);
+
+/* ---- the periphery's shape: repulsion, binding and collision inside the step --------------------------------------
+ * What System::prep_state_for_solver and System::run do with the periphery's shape besides its operators, on the
+ * device (DESIGN.md §3.9): fc_->periphery_force (system.cpp:422; SphericalPeriphery / EllipsoidalPeriphery::
+ * fiber_interaction, periphery.cpp:140-162, 232-263), fc_->update_boundary_conditions (system.cpp:452,
+ * fiber_finite_difference.cpp:74-91) and System::check_collision (system.cpp:576-595).
+ *   repulsion of node i strictly inside the surface (|x| < R, or |x| < |r_cortex| with the reference's 1e-12 guards in
+ *     atan2 and acos): f_0 dr / |dr| exp(-(R - |x|) / l_0), dr = x - (the surface point in the direction of x); 0 on
+ *     or outside the surface and at node 0 of a fiber with fiber_minus_clamped.  A node at the exact centre of a
+ *     sphere divides 0 by 0 as the reference does: its force is NaN (a step refuses it, below).
+ *   plus_hinged of a fiber = binding_active && polar_angle_start <= acos(normalized(x_last).z) <= polar_angle_end &&
+ *     some node within binding_threshold of the surface (normalized() of a zero vector is zero: angle pi/2).
+ *   collided = a fiber node on or beyond the surface (node 0 skipped when the fiber is minus-clamped: params
+ *     minus_clamped of the last step, fiber_minus_clamped before one), a spherical body with |c| + r > R (sphere
+ *     only), or two spherical bodies with |c1 - c2| < r1 + r2.
+ * With a shape set, skb_flow_step, skb_flow_group_step_device and skb_mflow_step (on every member):
+ *   1. before the links and the fiber build, run the pass on the current geometry (own fibers); a non-finite
+ *      repulsion is refused there (SKB_ERR_INVALID, geometry untouched), as a non-finite f_external is;
+ *   2. step with f_external + repulsion (the repulsion alone for a NULL f_external), and with every stepped fiber's
+ *      params plus_hinged replaced by the pass's value -- the reference sets bc_plus_ of every fiber every step, so
+ *      the caller's plus_hinged is ignored then;
+ *   3. after the install, run the pass over ALL fibers and bodies and set info->collided.  Every member of a group
+ *      holds the complete new geometry and returns the same value: each member's own fibers' params minus_clamped
+ *      travel with their new positions in the step's all-gather, so every member skips node 0 of the same fibers.
+ *      A step that is refused or not installed leaves the flags the collision test uses as they were.
+ * skb_flow_set_periphery_shape: the shape, fiber_minus_clamped (per fiber the TOML flag minus_clamped_, not
+ *   is_minus_clamped(); NULL: all 0) and body_radius (per body the radius of a spherical body, 0: not spherical, never
+ *   colliding; NULL: no body takes part).  Sizes the pass's buffers (with a pinned flag buffer) for the flow's fibers
+ *   and loads its kernels; skb_flow_set_gmres sizes them again.  SKB_PERIPHERY_NONE clears the shape (the reference's
+ *   GenericPeriphery: no force, no binding, no collision).  Refused (SKB_ERR_INVALID, before any launch, the earlier
+ *   shape kept): a kind outside the enum, a non-finite parameter, a, b or c <= 0 for the kind in use (a alone for a
+ *   sphere), l_0 <= 0, a flag outside {0, 1}, a negative or non-finite radius, a flow without periphery nodes.  A step
+ *   is refused when the flow's fibers or bodies changed in number since the call (call it again), or when its nodes
+ *   outgrew the buffers (skb_flow_set_gmres sizes them again).
+ *   Every member of a group makes the same call with the complete arrays.
+ * skb_flow_periphery_interaction: the pass on the current geometry: f_periphery 3 per own node, plus_hinged per own
+ *   fiber, *collided over ALL fibers and bodies; each output may be NULL.  Refused without a shape. */
+enum { SKB_PERIPHERY_NONE = 0, SKB_PERIPHERY_SPHERE = 1, SKB_PERIPHERY_ELLIPSOID = 2 };
+typedef struct skb_periphery_shape {
+    int32_t kind;           /* SKB_PERIPHERY_*; NONE also stands for the reference's GenericPeriphery          */
+    int32_t binding_active; /* periphery_binding.active                                                        */
+    double a, b, c;         /* SphericalPeriphery::radius_ (a; b, c ignored) / EllipsoidalPeriphery a_, b_, c_ */
+    double f_0, l_0;        /* fiber_periphery_interaction (params.hpp:45-48)                                  */
+    double polar_angle_start, polar_angle_end, binding_threshold; /* periphery_binding (params.hpp:25-29)    */
+} skb_periphery_shape;
+SKB_API int skb_flow_set_periphery_shape(skb_flow *fl, const skb_periphery_shape *shape,
+                                         const int32_t *fiber_minus_clamped, const double *body_radius);
+SKB_API int skb_flow_periphery_interaction(skb_flow *fl, double *f_periphery, int32_t *plus_hinged,
+                                           int32_t *collided);
 
 /* ---- the whole-vector calls on one rank per GPU ---------------------------------------------------------------------
  * A group member (skb_flow_group_init ... skb_flow_group_warmup above) applies A, P^-1 and builds the RHS on its LOCAL
@@ -775,6 +825,12 @@ SKB_API int skb_mflow_step(skb_mflow *mf, const skb_fiber_params *params, const 
                            const double *force_scale, const double *f_external, const double *body_forces_torques,
                            const int *fiber_body, const double *site_ref, double dt, double eta, double tol,
                            int num_blocks, int max_iters, double *x, double *tension, skb_step_info *info);
+/* skb_flow_set_periphery_shape on every member (the complete arrays); skb_mflow_step applies it on every member */
+SKB_API int skb_mflow_set_periphery_shape(skb_mflow *mf, const skb_periphery_shape *shape,
+                                          const int32_t *fiber_minus_clamped, const double *body_radius);
+/* skb_flow_periphery_interaction over the devices: the complete arrays of all fibers */
+SKB_API int skb_mflow_periphery_interaction(skb_mflow *mf, double *f_periphery, int32_t *plus_hinged,
+                                            int32_t *collided);
 /* skb_flow_get_fibers / _get_placement of the geometry every member holds */
 SKB_API int skb_mflow_get_fibers(skb_mflow *mf, double *r_fib);
 SKB_API int skb_mflow_get_placement(skb_mflow *mf, double *centers, double *orientations);

@@ -50,10 +50,21 @@ ERR_STATE = 4  # SKB_ERR_STATE
 
 class StepInfo(C.Structure):
     """skb_step_info (include/skelly_b200_flow.h): the outcome of skb_flow_step."""
-    _fields_ = [("solve", SolveInfo), ("fiber_error", C.c_double), ("worst_fiber", C.c_int32), ("reserved", C.c_int32)]
+    _fields_ = [("solve", SolveInfo), ("fiber_error", C.c_double), ("worst_fiber", C.c_int32), ("collided", C.c_int32)]
 
     def as_dict(self):
-        return dict(self.solve.as_dict(), fiber_error=self.fiber_error, worst_fiber=self.worst_fiber)
+        return dict(self.solve.as_dict(), fiber_error=self.fiber_error, worst_fiber=self.worst_fiber,
+                    collided=self.collided)
+
+
+PERIPHERY_NONE, PERIPHERY_SPHERE, PERIPHERY_ELLIPSOID = 0, 1, 2  # SKB_PERIPHERY_*
+
+
+class PeripheryShape(C.Structure):
+    """skb_periphery_shape (include/skelly_b200_flow.h)"""
+    _fields_ = [("kind", C.c_int32), ("binding_active", C.c_int32), ("a", C.c_double), ("b", C.c_double),
+                ("c", C.c_double), ("f_0", C.c_double), ("l_0", C.c_double), ("polar_angle_start", C.c_double),
+                ("polar_angle_end", C.c_double), ("binding_threshold", C.c_double)]
 
 
 class DenseStats(C.Structure):
@@ -268,6 +279,10 @@ def library() -> C.CDLL:
                                        + [C.POINTER(C.c_int), _dp, C.c_double, C.c_double, C.c_double, C.c_int,
                                           C.c_int, C.c_void_p, C.c_void_p, C.POINTER(StepInfo), C.c_void_p], C.c_int),
         "skb_mflow_get_fibers": ([ctxp, _dp], C.c_int),
+        "skb_flow_set_periphery_shape": ([ctxp, C.POINTER(PeripheryShape), C.POINTER(C.c_int32), _dp], C.c_int),
+        "skb_flow_periphery_interaction": ([ctxp, _dp, C.POINTER(C.c_int32), C.POINTER(C.c_int32)], C.c_int),
+        "skb_mflow_set_periphery_shape": ([ctxp, C.POINTER(PeripheryShape), C.POINTER(C.c_int32), _dp], C.c_int),
+        "skb_mflow_periphery_interaction": ([ctxp, _dp, C.POINTER(C.c_int32), C.POINTER(C.c_int32)], C.c_int),
         "skb_mflow_get_placement": ([ctxp, _dp, _dp], C.c_int),
         "skb_mflow_solve_system": ([ctxp, _dp, C.c_double, C.c_double, C.c_int, C.c_int, _dp, C.POINTER(SolveInfo),
                                     _dp], C.c_int),
@@ -397,6 +412,34 @@ def _step_call(fl, call, n_fibers, params, dt, eta, f_external, body_forces_torq
     if not (rc == ERR_STATE and np.isnan(info.fiber_error)):
         _check(rc)
     return x, tension, info.as_dict()
+
+
+def _shape_call(fn, h, n_fibers, n_bodies, kind, a, b, c, f_0, l_0, binding_active, polar_angle_start,
+                polar_angle_end, binding_threshold, fiber_minus_clamped, body_radius):
+    s = PeripheryShape(int(kind), int(binding_active), float(a), float(b), float(c), float(f_0), float(l_0),
+                       float(polar_angle_start), float(polar_angle_end), float(binding_threshold))
+    mc = None if fiber_minus_clamped is None else np.ascontiguousarray(fiber_minus_clamped, dtype=np.int32)
+    if mc is not None and mc.shape != (n_fibers,):
+        raise ValueError(f"expected {n_fibers} fiber_minus_clamped flags, got {mc.shape}")
+    br = None if body_radius is None else np.ascontiguousarray(body_radius, dtype=np.float64)
+    if br is not None and br.shape != (n_bodies,):
+        raise ValueError(f"expected {n_bodies} body radii, got {br.shape}")
+    _check(fn(h, C.byref(s), None if mc is None else mc.ctypes.data_as(C.POINTER(C.c_int32)), _opt_p(br)))
+
+
+def _interaction_call(fn, h, n_nodes, n_fibers):
+    f = np.empty((n_nodes, 3))
+    hinged = np.empty(n_fibers, dtype=np.int32)
+    collided = C.c_int32(0)
+    _check(fn(h, _p(f), hinged.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(collided)))
+    return f, hinged, bool(collided.value)
+
+
+_SHAPE_DOC = """The periphery's shape for the step (skb_flow_set_periphery_shape): kind PERIPHERY_SPHERE (radius a),
+        PERIPHERY_ELLIPSOID (semi-axes a, b, c) or PERIPHERY_NONE (clears it); fiber_periphery_interaction f_0, l_0;
+        periphery_binding active, polar angles and threshold; per fiber the TOML flag minus_clamped_ (None: all 0);
+        per body the radius of a spherical body (0: not spherical; None: no body takes part).  The step then adds the
+        repulsion to f_external, takes plus_hinged from the binding and reports the collision test in info["collided"]."""
 
 
 def device_count() -> int:
@@ -1077,14 +1120,31 @@ class Flow:
                                                       C.c_void_p(stream)))
         return info.as_dict(), hist[:info.iterations + 1]
 
+    def set_periphery_shape(self, kind, a, b=0.0, c=0.0, f_0=20.0, l_0=0.05, binding_active=False,
+                            polar_angle_start=0.0, polar_angle_end=np.pi, binding_threshold=0.75,
+                            fiber_minus_clamped=None, body_radius=None):
+        _shape_call(library().skb_flow_set_periphery_shape, self._h, self._n_fibers(), self.n_bodies, kind, a, b, c,
+                    f_0, l_0, binding_active, polar_angle_start, polar_angle_end, binding_threshold,
+                    fiber_minus_clamped, body_radius)
+
+    set_periphery_shape.__doc__ = _SHAPE_DOC
+
+    def periphery_interaction(self, n_own_nodes=None, n_own_fibers=None):
+        """(repulsion (N, 3) of the own nodes, plus_hinged (own fibers,) int32, collided bool over all fibers and
+        bodies) at the current geometry (skb_flow_periphery_interaction); by default all nodes and fibers"""
+        return _interaction_call(library().skb_flow_periphery_interaction, self._h,
+                                 self.n_fib if n_own_nodes is None else int(n_own_nodes),
+                                 self._n_fibers() if n_own_fibers is None else int(n_own_fibers))
+
     def step(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped, plus_hinged, dt,
              eta, dense=None, f_external=None, body_forces_torques=None, fiber_body=None, site_ref=None,
              v_growth=None, force_scale=None, tol=1e-10, num_blocks=300, max_iters=1000):
         """System::step (system.cpp:482-492) on the device: links, fiber operators, RHS and solve at the current
         geometry, then the fibers' and bodies' step and the new geometry installed.  fiber_body (N_fibers,) ints, -1
         free, or None; site_ref (N_fibers, 3) body-frame nucleation sites, or None.  Returns (x, tension, info): info
-        a dict of skb_step_info (the solve's fields, fiber_error, worst_fiber).  A solution with non-finite new
-        positions installs nothing and returns fiber_error NaN."""
+        a dict of skb_step_info (the solve's fields, fiber_error, worst_fiber, collided).  A solution with non-finite
+        new positions installs nothing and returns fiber_error NaN.  With set_periphery_shape, plus_hinged is ignored
+        (the binding sets it) and the repulsion is added to f_external."""
         return _step_call(self, lambda *a: library().skb_flow_step(self._h, dense._h if dense is not None else None, *a),
                           self._n_fibers(), (length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
                                              minus_clamped, plus_hinged), dt, eta, f_external, body_forces_torques,
@@ -1435,6 +1495,19 @@ class MultiFlow:
         E = np.ascontiguousarray(np.broadcast_to(np.asarray(bending_rigidity, dtype=np.float64), b.shape))
         assert st.shape[0] == b.shape[0]
         _check(library().skb_mflow_set_fiber_links(self._h, b.ctypes.data_as(C.POINTER(C.c_int)), _p(st), _p(E)))
+
+    def set_periphery_shape(self, kind, a, b=0.0, c=0.0, f_0=20.0, l_0=0.05, binding_active=False,
+                            polar_angle_start=0.0, polar_angle_end=np.pi, binding_threshold=0.75,
+                            fiber_minus_clamped=None, body_radius=None):
+        _shape_call(library().skb_mflow_set_periphery_shape, self._h, self.n_fibers, self.n_bodies, kind, a, b, c,
+                    f_0, l_0, binding_active, polar_angle_start, polar_angle_end, binding_threshold,
+                    fiber_minus_clamped, body_radius)
+
+    set_periphery_shape.__doc__ = _SHAPE_DOC
+
+    def periphery_interaction(self):
+        """Flow.periphery_interaction over the devices: the complete arrays of all fibers"""
+        return _interaction_call(library().skb_mflow_periphery_interaction, self._h, self.n_fib, self.n_fibers)
 
     def step(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped, plus_hinged, dt,
              eta, dense=None, f_external=None, body_forces_torques=None, fiber_body=None, site_ref=None,

@@ -1,6 +1,6 @@
 // skb_flow.hpp -- the flow (include/skelly_b200_flow.h) and what the translation units built on it share:
 // skb_matvec.cu (its lifetime, geometry, flows and matvec orchestration), skb_system.cu (the whole-system calls),
-// skb_solve.cu, skb_step.cu and skb_mflow.cu.  Free functions in namespace skb that take the flow.
+// skb_solve.cu, skb_step.cu, skb_periphery.cu and skb_mflow.cu.  Free functions in namespace skb that take the flow.
 #pragma once
 #include "skb_internal.hpp"
 #include "../../include/skelly_b200_flow.h"
@@ -44,6 +44,51 @@ struct StepBuffers {
     int n_fibers_ = -1, n_bodies_ = -1;
     long long n_fib_ = -1;
     size_t check_cap_ = 0; // doubles of `check`
+};
+
+// The periphery's shape (skb_flow_set_periphery_shape) and what the step derives from it on the device: the
+// fiber-periphery repulsion, the plus-end binding and the collision test (skb_periphery.cu, periphery_kernels.cuh).
+// Holds the per-fiber and per-body tables of the call, and the buffers of one pass sized for the fibers it was set or
+// sized for (a group step allocates nothing).  The caller has made the flow's device current
+class PeripheryShape {
+  public:
+    // checked first: a refusal leaves the earlier shape.  kind NONE clears it
+    int set(const ::skb_periphery_shape *shape, const int *minus_clamped, const double *body_radius, int n_fibers,
+            long long n_fib, int n_bodies, long long n_shell, cudaStream_t st);
+    bool active() const { return active_; }
+    // the pass's buffers for n_fib nodes (skb_flow_set_gmres); a no-op without a shape
+    int size(long long n_fib);
+    // the per-fiber and per-body tables were set for this many fibers and bodies (only set() changes them)
+    bool counts_fit(int n_fibers, int n_bodies) const { return n_fibers == n_fibers_ && n_bodies == n_bodies_; }
+    // the pass's buffers hold n_fib nodes (set() or size())
+    bool nodes_fit(long long n_fib) const { return n_fib <= cap_nodes_; }
+    // is_minus_clamped() of fibers [f0, f0 + nf) from a step's params: the collision test skips their node 0 then
+    void note_clamped(int f0, int nf, const ::skb_fiber_params *params);
+    // the same flags of ALL fibers as the group step all-gathered them (1.0 / 0.0 per fiber)
+    void note_clamped_all(const std::vector<double> &flags);
+    // minus_clamped of params (fibers [f0, f0 + nf)) uploaded on st into the device table the group step's kernel
+    // reads (clamp_table(), indexed by fiber among ALL fibers), without noting them
+    int upload_clamped(int f0, int nf, const ::skb_fiber_params *params, cudaStream_t st);
+    const int *clamp_table() const { return (const int *)collide_skip_.ptr; }
+    // one launch over the fibers [f0, f1) of offsets d_off and positions d_r_fib (and, with bodies, the n_bodies
+    // centres d_centers): the repulsion of their nodes into force() (with_force), their flags into flags() (host,
+    // f1 - f0 entries, then the bodies' flag); returns once the flags are on the host
+    int run(const double *d_r_fib, const long long *d_off, int f0, int f1, bool with_force, const double *d_centers,
+            int n_bodies, cudaStream_t st, int *launches);
+    const double *force() const { return (const double *)force_.ptr; }
+    const int *flags() const { return (const int *)h_flags_.get(); }
+    // d_out = d_in + force() over n doubles (d_in NULL: force() alone)
+    int add_force(const double *d_in, double *d_out, long long n, cudaStream_t st, int *launches) const;
+
+  private:
+    bool active_ = false;
+    ::skb_periphery_shape s_{};
+    int n_fibers_ = -1, n_bodies_ = -1;
+    long long cap_nodes_ = -1;
+    size_t flag_cap_ = 0; // ints of h_flags_
+    std::vector<int> h_clamped_; // the collision test's node-0 skip per fiber
+    DevBuf force_skip_, collide_skip_, radius_, force_, flags_;
+    PinnedHost h_flags_;
 };
 } // namespace skb
 
@@ -107,6 +152,7 @@ struct skb_flow {
     std::vector<double> h_orient;    // the quaternions of the last skb_flow_place_bodies (4 per body) ...
     bool placed = false;             // ... valid until skb_flow_set_bodies changes the bodies otherwise
     skb::StepBuffers stepbuf;             // the buffers of skb_flow_step (skb_step.cu)
+    skb::PeripheryShape shape;            // skb_flow_set_periphery_shape (skb_periphery.cu)
     skb::Group grp; // multi-GPU group membership: one member per GPU, exchange through peer memory (skb_group.cu)
     // a member's whole-vector matvec in flight: matvec_core exchanges the bodies' partial link forces through the
     // window and the body flow reads their totals from ft_sum ([F | L], 6 per body)
@@ -261,7 +307,21 @@ struct StepCall {
     std::vector<StepItem> items;
     std::vector<double> rigidity, sites;
     long long n = 0;
+    // with a periphery shape: the own fibers' params with plus_hinged from the binding (empty: the caller's params)
+    std::vector<::skb_fiber_params> hinged;
+    const ::skb_fiber_params *params(const StepArgs &a) const { return hinged.empty() ? a.params : hinged.data(); }
 };
+
+// ---- the periphery's shape in the step (skb_periphery.cu) ----
+// with a shape: the pass over the own fibers at the current geometry (the repulsion kept for
+// periphery_add_force, c.hinged filled); refuses a non-finite repulsion and a shape not set or sized for the flow.
+// Changes nothing the step's refusal would have to undo.  Without a shape: nothing
+int periphery_before_step(skb_flow *fl, const char *who, const StepArgs &a, StepCall &c);
+// d_out = d_f_external + the repulsion of the m own nodes of periphery_before_step (d_f_external NULL: the repulsion)
+int periphery_add_force(skb_flow *fl, const double *d_f_external, long long m, double *d_out, cudaStream_t st,
+                        int *launches);
+// System::check_collision of the flow's current geometry, ALL fibers and bodies (0 without a shape)
+int periphery_collided(skb_flow *fl, int *collided, cudaStream_t st, int *launches);
 // the refusals of the step's host arguments: the scalars; params, fiber_body and site_ref of nf fibers (the first is
 // fiber f0) against nb bodies; the external forces of n_fib fiber nodes and the forces and torques of nb bodies finite
 int step_scalar_args(const char *who, const ::skb_step_info *info, double dt, double eta, double tol, int num_blocks,

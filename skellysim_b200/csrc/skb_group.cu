@@ -46,7 +46,7 @@ int Group::init(int rank, int size, long long n_fib, long long n_pad_fib, long l
         lay_.ft_part[b] = take((size_t)kMaxGroup * n_bodies * 48 + 16);
         lay_.x_body[b] = take((size_t)n_body * 24 + (size_t)n_bodies * 48 + 16);
         lay_.dots[b] = take((size_t)kMaxGroup * kDotsSlot * 8);
-        lay_.r_step[b] = take((size_t)n_fib * 24 + (size_t)n_fibers * 8 + 16);
+        lay_.r_step[b] = take((size_t)n_fib * 24 + (size_t)n_fibers * 16 + 16);
     }
     lay_.u_part = take((size_t)n_fib * 24 + 16);
     lay_.u_part_shell = take((size_t)n_shell * 24 + 16);

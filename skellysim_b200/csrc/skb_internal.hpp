@@ -413,8 +413,9 @@ int load_dense_kernels();
 //                                    its own rows; skb_flow_group_apply_system_*)                   -- by peers
 //   dots         [2][kMaxGroup][kDotsSlot]  per member its partial dot products of a solve step (reduce_dots)
 //                                    -- by peers
-//   r_step       [2][n_fib*3 + n_fibers]  the new positions of ALL fiber nodes and the errors of ALL fibers after a
-//                                    group step (skb_flow_group_step_device; group_fiber_step_kernel)  -- by peers
+//   r_step       [2][n_fib*3 + 2*n_fibers]  the new positions of ALL fiber nodes, the errors of ALL fibers and, with a
+//                                    periphery shape, their minus_clamped flags after a group step
+//                                    (skb_flow_group_step_device; group_fiber_step_kernel)             -- by peers
 //   u_part       [n_fib*3]           this member's partial velocities of ALL fiber rows                  -- by itself
 //   u_part_shell [n_shell*3]         its partial velocities of ALL periphery rows (cross kernel)        -- by itself
 //

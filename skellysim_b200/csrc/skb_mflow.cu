@@ -285,6 +285,30 @@ int skb_mflow_set_overlap(skb_mflow *mf, int on) {
     return SKB_OK;
 }
 
+int skb_mflow_set_periphery_shape(skb_mflow *mf, const skb_periphery_shape *shape, const int32_t *fiber_minus_clamped,
+                                  const double *body_radius) {
+    if (!mf)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_set_periphery_shape: NULL");
+    for (int g = 0; g < mf->n; ++g)
+        SKB_TRY(skb_flow_set_periphery_shape(mf->m[g].get(), shape, fiber_minus_clamped, body_radius));
+    return SKB_OK;
+}
+
+// skb_flow_periphery_interaction of every member into the complete arrays: each member's own fibers, member 0's
+// collision test (every member holds the same geometry)
+int skb_mflow_periphery_interaction(skb_mflow *mf, double *f_periphery, int32_t *plus_hinged, int32_t *collided) {
+    if (!mf)
+        return set_error(SKB_ERR_INVALID, "skb_mflow_periphery_interaction: NULL");
+    SKB_TRY(mflow_prepare(mf));
+    for (int g = 0; g < mf->n; ++g) {
+        const int f0 = mf->f0[(size_t)g];
+        const long long a = mf->fiber_off[(size_t)f0];
+        SKB_TRY(skb_flow_periphery_interaction(mf->m[(size_t)g].get(), f_periphery ? f_periphery + 3 * a : nullptr,
+                                               plus_hinged ? plus_hinged + f0 : nullptr, g == 0 ? collided : nullptr));
+    }
+    return SKB_OK;
+}
+
 int skb_mflow_set_self_exclusion(skb_mflow *mf, int fused) {
     if (!mf)
         return set_error(SKB_ERR_INVALID, "skb_mflow_set_self_exclusion: NULL");

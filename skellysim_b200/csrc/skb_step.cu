@@ -238,7 +238,7 @@ static int step_checks(skb_flow *fl, skb_dense *dn, const StepArgs &a, skb_step_
     if (c.n > 0 && a.num_blocks > fl->kry.blocks())
         return set_error(SKB_ERR_INVALID, "%s: num_blocks = %d, skb_flow_set_gmres sized the workspace for %d", who,
                          a.num_blocks, fl->kry.blocks());
-    return SKB_OK;
+    return periphery_before_step(fl, who, a, c);
 }
 
 int skb::group_step_checks(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, const StepArgs &a,
@@ -269,7 +269,7 @@ int skb::group_step_checks(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, 
     if (a.num_blocks > fl->kry.blocks())
         return set_error(SKB_ERR_INVALID, "%s: num_blocks = %d, skb_flow_set_gmres sized the workspace for %d", who,
                          a.num_blocks, fl->kry.blocks());
-    return SKB_OK;
+    return periphery_before_step(fl, who, a, c);
 }
 
 // ---- the pieces both runs share --------------------------------------------------------------------------------------
@@ -341,9 +341,13 @@ static int step_run(skb_flow *fl, skb_dense *dn, const StepArgs &a, StepCall &c,
     const long long n_fib = fl->n_fib;
     const cudaStream_t st = fl->stream;
     Krylov &kry = fl->kry;
+    if (fl->shape.active() && n_fib > 0) { // f_external + the periphery's repulsion, into the step's own buffer
+        SKB_TRY(periphery_add_force(fl, d_f_external, n_fib, (double *)fl->stepbuf.fext.ptr, st, &fl->launches));
+        d_f_external = (const double *)fl->stepbuf.fext.ptr;
+    }
     SKB_TRY(skb_flow_set_fiber_links(fl, a.fiber_body, c.sites.data(), c.rigidity.data()));
-    SKB_TRY(skb_flow_build_fiber_operators(fl, a.params, a.dt, a.eta));
-    SKB_TRY(skb_flow_build_system_rhs_device(fl, a.params, a.v_growth, a.force_scale,
+    SKB_TRY(skb_flow_build_fiber_operators(fl, c.params(a), a.dt, a.eta));
+    SKB_TRY(skb_flow_build_system_rhs_device(fl, c.params(a), a.v_growth, a.force_scale,
                                              n_fib > 0 ? d_f_external : nullptr, nb > 0 ? d_body_forces : nullptr,
                                              nb > 0 ? d_body_torques : nullptr, a.dt, a.eta, kry.stage_b(), st));
     SKB_TRY(skb_flow_solve_system_device(fl, dn, kry.stage_b(), a.eta, a.tol, a.num_blocks, a.max_iters,
@@ -378,7 +382,10 @@ static int step_run(skb_flow *fl, skb_dense *dn, const StepArgs &a, StepCall &c,
     SKB_TRY(skb_flow_set_fibers(fl, r_new.data(), n_nodes.data(), length.data(), nf));
     if (nb > 0)
         SKB_TRY(skb_flow_place_bodies(fl, c_new.data(), q_new.data()));
-    return skb_flow_set_fiber_links(fl, a.fiber_body, sites_new.data(), c.rigidity.data());
+    SKB_TRY(skb_flow_set_fiber_links(fl, a.fiber_body, sites_new.data(), c.rigidity.data()));
+    // System::check_collision of the installed geometry, node 0 skipped on this step's is_minus_clamped()
+    fl->shape.note_clamped(0, nf, c.params(a));
+    return periphery_collided(fl, &info->collided, st, &fl->launches);
 }
 
 // System::step on one rank per GPU: the composed local-vector calls, then two epochs of the group's own protocol --
@@ -404,15 +411,19 @@ int skb::group_step_run(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, con
     const StepBuffers &buf = fl->stepbuf;
     const int nf = fl->n_fibers, nfo = c.own.count(), nb = fl->n_bodies;
     const long long n_fib = fl->n_fib, m = c.own.nodes();
+    int *launches = &fl->launches; // the protocol's launches join the flow's count, as in the other member calls
+    if (fl->shape.active() && m > 0) { // f_external + the periphery's repulsion of the own nodes
+        SKB_TRY(periphery_add_force(fl, d_f_external, m, (double *)buf.fext.ptr, st, launches));
+        d_f_external = (const double *)buf.fext.ptr;
+    }
     SKB_TRY(skb_flow_group_set_fiber_links(fl, a.fiber_body, c.sites.data(), c.rigidity.data()));
-    SKB_TRY(skb_flow_build_fiber_operators(fl, a.params, a.dt, a.eta));
+    SKB_TRY(skb_flow_build_fiber_operators(fl, c.params(a), a.dt, a.eta));
     CUDA_TRY(cudaStreamSynchronize(fl->stream));
-    SKB_TRY(skb_flow_group_build_system_rhs_device(fl, a.params, a.v_growth, a.force_scale, d_f_external,
+    SKB_TRY(skb_flow_group_build_system_rhs_device(fl, c.params(a), a.v_growth, a.force_scale, d_f_external,
                                                    d_body_forces, d_body_torques, a.dt, a.eta, kry.stage_b(), st));
     SKB_TRY(skb_flow_group_solve_system_device(fl, dn_spc, dn_minv, kry.stage_b(), a.eta, a.tol, a.num_blocks,
                                                a.max_iters, kry.stage_x(), &info->solve, nullptr, st));
     const double *d_x = kry.stage_x(); // [4 per own fiber node | 3 per own periphery row | own body rows]
-    int *launches = &fl->launches; // the protocol's launches join the flow's count, as in the other member calls
 
     // ---- the body rows all-gathered (an epoch of its own: the rows phase), [U; w] of every body from the own window,
     // the bodies' step on the host: every member from the same bits ----
@@ -428,17 +439,24 @@ int skb::group_step_run(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, con
 
     // ---- the own fibers' step, repin and error fused with the all-gather of the results into r_step of every window
     // (an epoch of its own, the rows phase again), then the complete positions and errors from the own window ----
-    std::vector<double> r_new(3 * (size_t)n_fib), err((size_t)nf);
+    // with a periphery shape, each own fiber's minus_clamped travels with its error: every member's collision test
+    // then skips node 0 of the same fibers, and all of them return the same `collided` without another exchange
+    const bool shape = fl->shape.active();
+    std::vector<double> r_new(3 * (size_t)n_fib), err((size_t)nf), clamped(shape ? (size_t)nf : 0);
     if (nf > 0) {
         SKB_TRY(G.begin());
         if (nfo > 0) {
             CUDA_TRY(cudaMemcpyAsync(buf.items.ptr, c.items.data(), (size_t)nfo * sizeof(StepItem),
                                      cudaMemcpyHostToDevice, st));
+            if (shape)
+                SKB_TRY(fl->shape.upload_clamped(c.own.f0, nfo, c.params(a), st));
             StepGather g;
             g.size = G.step_windows(g.r_step);
             g.n_fib = n_fib;
             g.node0 = c.own.off[c.own.f0];
             g.fiber0 = c.own.f0;
+            g.n_fibers = nf;
+            g.clamp = shape ? fl->shape.clamp_table() : nullptr;
             group_fiber_step_kernel<<<nfo, kStepThreads, 0, st>>>((const StepItem *)buf.items.ptr, d_x,
                                                                   fl->ops.class_table(), fl->ops.class_range_table(),
                                                                   c.own.length + c.own.f0, (double *)buf.tension.ptr,
@@ -450,6 +468,9 @@ int skb::group_step_run(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, con
         SKB_TRY(G.rows_barrier(true, true, st, launches));
         CUDA_TRY(cudaMemcpyAsync(r_new.data(), G.r_step(), r_new.size() * 8, cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaMemcpyAsync(err.data(), G.r_step() + 3 * n_fib, err.size() * 8, cudaMemcpyDeviceToHost, st));
+        if (shape)
+            CUDA_TRY(cudaMemcpyAsync(clamped.data(), G.r_step() + 3 * n_fib + nf, clamped.size() * 8,
+                                     cudaMemcpyDeviceToHost, st));
         if (tension && m > 0)
             CUDA_TRY(cudaMemcpyAsync(tension, buf.tension.ptr, (size_t)m * 8, cudaMemcpyDefault, st));
     }
@@ -468,7 +489,10 @@ int skb::group_step_run(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, con
         SKB_TRY(skb_flow_group_place_bodies(fl, c_new.data(), q_new.data()));
     SKB_TRY(skb_flow_group_set_fiber_links(fl, a.fiber_body, sites_new.data(), c.rigidity.data()));
     CUDA_TRY(cudaStreamSynchronize(fl->stream));
-    return SKB_OK;
+    // System::check_collision of the complete geometry every member installed, with the all-gathered flags: the same
+    // on every member
+    fl->shape.note_clamped_all(clamped);
+    return periphery_collided(fl, &info->collided, fl->stream, launches);
 }
 
 extern "C" {

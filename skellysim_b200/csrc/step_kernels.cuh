@@ -110,20 +110,28 @@ __global__ void __launch_bounds__(kStepThreads)
 
 constexpr int kStepMaxMembers = 16; // kMaxGroup (skb_internal.hpp), asserted where the group's window is laid out
 
-// the outputs of group_fiber_step_kernel: r_step of every member's window, [3 per node of ALL fibers | 1 per fiber]
+// the outputs of group_fiber_step_kernel: r_step of every member's window, [3 per node of ALL fibers | 1 per fiber |
+// 1 per fiber]: the new positions, the errors and (clamp not NULL) each fiber's minus_clamped flag, which a periphery
+// shape's collision test needs of ALL fibers on every member
 struct StepGather {
     double *r_step[kStepMaxMembers];
     int size;          // windows to store into
     long long n_fib;   // fiber nodes of ALL fibers: the errors start at r_step + 3 n_fib
     long long node0;   // the launch's first node among ALL fiber nodes
     int fiber0;        // the launch's first fiber among ALL fibers
+    int n_fibers;      // ALL fibers: the flags start at r_step + 3 n_fib + n_fibers
+    const int *clamp;  // per fiber among ALL fibers (NULL: no flags)
     __device__ __forceinline__ void pos(long long node, int k, double v) const {
         for (int m = 0; m < size; ++m)
             r_step[m][3 * (node0 + node) + k] = v;
     }
     __device__ __forceinline__ void error(double v) const {
-        for (int m = 0; m < size; ++m)
-            r_step[m][3 * n_fib + fiber0 + blockIdx.x] = v;
+        const int f = fiber0 + (int)blockIdx.x;
+        for (int m = 0; m < size; ++m) {
+            r_step[m][3 * n_fib + f] = v;
+            if (clamp)
+                r_step[m][3 * n_fib + n_fibers + f] = clamp[f] ? 1.0 : 0.0;
+        }
     }
 };
 

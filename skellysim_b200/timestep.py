@@ -1,8 +1,10 @@
 """Time stepping of a whole system: System::step (system.cpp:482-492) through capi.Flow.step, and the acceptance logic
 of System::run (system.cpp:515-568) around it.
 
-The fiber-periphery repulsion, the bodies' force schedule and the collision test stay the caller's host code (DESIGN.md
-§7): `run` takes them as the callables `forces(time, r_fib)` and `collided(r_fib, centers)`.
+The fiber-periphery repulsion, the periphery binding and the collision test run inside the step once the flow has a
+periphery shape (Flow.set_periphery_shape): the step reports the collision test as info["collided"].  The bodies' force
+schedule stays the caller's host code (DESIGN.md §7): `run` takes it as the callable `forces(time, r_fib)`, and a
+caller's own `collided(r_fib, centers)` still replaces the step's test.
 
 One deviation from the reference's loop (DESIGN.md §5): the reference sets dt to the grown dt_new before it advances
 time on an accepted step (system.cpp:554-557), so time advances by a dt no step used.  Here time advances by the dt of
@@ -55,8 +57,9 @@ def run(stepper, t_final, dt, adaptive=True, dt_min=1e-5, dt_max=np.inf, beta_up
     """System::run's loop until time >= t_final.  Each step: backup, forces(time, r_fib) -> (f_external (N_f, 3),
     F_T (n_bodies, 6)), either None (no callable: no external forces), the step, then the acceptance:
       adaptive: accept when converged and fiber_error <= fiber_error_tol, and then grow dt by beta_up (at most dt_max)
-      when fiber_error <= 0.9 fiber_error_tol; otherwise shrink dt by beta_down.  A converged step that collided(r_fib,
-      centers) says True is rejected with dt halved.  A dt below dt_min raises RuntimeError.
+      when fiber_error <= 0.9 fiber_error_tol; otherwise shrink dt by beta_down.  A converged step that collided is
+      rejected with dt halved (system.cpp:542-546): collided(r_fib, centers) decides when given, else the step's
+      info["collided"].  A dt below dt_min raises RuntimeError.
       not adaptive: every step is accepted, dt stays; a step that was not installed (NaN fiber_error) raises.
     A rejected step is restored.  Returns (time, dt, log): log one (time, dt used, accepted, fiber_error) per step."""
     log = []
@@ -73,7 +76,8 @@ def run(stepper, t_final, dt, adaptive=True, dt_min=1e-5, dt_max=np.inf, beta_up
                     dt_new = min(dt_max, dt * beta_up)
             else:
                 dt_new = dt * beta_down
-            if converged and collided is not None and collided(stepper.positions(), stepper.placement()[0]):
+            if converged and (collided(stepper.positions(), stepper.placement()[0]) if collided is not None
+                              else info.get("collided", False)):
                 dt_new, accept = dt * 0.5, False
             if dt_new < dt_min:
                 raise RuntimeError(f"timestep {dt_new:g} smaller than dt_min = {dt_min:g} at time {time:g} "
