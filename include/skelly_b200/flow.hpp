@@ -91,6 +91,50 @@ template <class M> class FlowEngineT {
         return vel;
     }
 
+    // ---- the listener (listener.cpp:86-136) on one frame ----
+    /// body_velocities: 6 x n_bodies [U; omega]; body_kind 0 / 1 (sphere) / 2 (ellipsoid); body_radii 3 x n_bodies
+    void set_listener_frame(const M &fib_forces, const M &shell_density, const M &body_densities,
+                            const M &forces_torques, const M &body_velocities, const std::vector<int32_t> &body_kind,
+                            const M &body_radii, double eta) {
+        check(skb_flow_set_listener_frame(st_->fl, fib_forces.data(), shell_density.data(), body_densities.data(),
+                                          forces_torques.data(), body_velocities.data(), body_kind.data(),
+                                          body_radii.data(), eta),
+              "skb_flow_set_listener_frame");
+    }
+    /// System::velocity_at_targets on the frame, the body-interior replacement included
+    M listener_velocity(const M &r_trg) const {
+        M vel = M::Zero(3, r_trg.cols());
+        check(skb_flow_listener_velocity(st_->fl, r_trg.data(), r_trg.cols(), vel.data()), "skb_flow_listener_velocity");
+        return vel;
+    }
+    /// StreamLine / VortexLine::compute of every seed (3 x n) at once: x and val are 3 x m, time m, per line
+    struct Line {
+        M x, val;
+        std::vector<double> time;
+        int32_t status[2];
+    };
+    std::vector<Line> listener_lines(int kind, const M &x0, const skb_line_request &req) const {
+        const int n = (int)x0.cols();
+        const long row = 2L * req.max_points - 1;
+        std::vector<double> x(3 * n * std::max(row, 1L)), t(n * std::max(row, 1L)), val(x.size());
+        std::vector<int32_t> n_points(n), status(2 * n);
+        check(skb_flow_listener_lines(st_->fl, kind, x0.data(), n, &req, x.data(), t.data(), val.data(),
+                                      n_points.data(), status.data()),
+              "skb_flow_listener_lines");
+        std::vector<Line> out(n);
+        for (int i = 0; i < n; ++i) {
+            const int m = n_points[i];
+            out[i].x = M::Zero(3, m);
+            out[i].val = M::Zero(3, m);
+            std::copy_n(x.data() + 3 * row * i, 3 * m, out[i].x.data());
+            std::copy_n(val.data() + 3 * row * i, 3 * m, out[i].val.data());
+            out[i].time.assign(t.begin() + row * i, t.begin() + row * i + m);
+            out[i].status[0] = status[2 * i];
+            out[i].status[1] = status[2 * i + 1];
+        }
+        return out;
+    }
+
     // ---- per-fiber dense operators on the device (SURVEY.md §8f N2) ----
     /// FiberFiniteDifference::matrices_.at(n_nodes): D_1_0 (n x n), P_downsample_bc ((4n-14) x 4n)  ffd.cpp:537-555
     void set_fiber_class(int n_nodes, const M &D_1_0, const M &P_downsample_bc) {

@@ -71,6 +71,41 @@ SKB_API int skb_flow_set_point_sources(skb_flow *fl, const double *positions, co
 SKB_API int skb_flow_set_background(skb_flow *fl, const int *components, const double *scale_factor,
                                     const double *uniform);
 
+/* ---- the listener: velocity field, streamlines and vortex lines of one frame (listener.cpp:86-136) ----------------
+ * A frame holds the strengths of one solution on the device.  fib_forces, shell_density, body_densities and
+ * body_forces_torques are those of skb_flow_velocity_at_targets (f_on_fibers, the periphery's solution, the body
+ * densities, the link-plus-external forces and torques); body_velocities is [U; omega] per body (6 x n_bodies, the tail
+ * of the body rows of the solution).  body_kind[b] is 0 (no interior test), 1 (sphere: |dx| < body_radii[3b]) or
+ * 2 (ellipsoid: sum dx_i^2 / r_i^2 < 1 on the world-frame dx, the body's orientation ignored as in system.cpp:362-381);
+ * body_radii is 3 per body.  Point sources and the background flow of the flow at the time of the requests are part
+ * of the velocity.  The frame goes stale (the requests refuse with SKB_ERR_STATE) when the geometry, the point sources
+ * or the background flow change after it was set. */
+SKB_API int skb_flow_set_listener_frame(skb_flow *fl, const double *fib_forces, const double *shell_density,
+                                        const double *body_densities, const double *body_forces_torques,
+                                        const double *body_velocities, const int32_t *body_kind,
+                                        const double *body_radii, double eta);
+/* System::velocity_at_targets (system.cpp:330-384) on the frame: skb_flow_velocity_at_targets's velocity, and at a
+ * target inside a body (bodies in the library's order, the last match wins) the body's rigid motion U + omega x dx. */
+SKB_API int skb_flow_listener_velocity(skb_flow *fl, const double *r_trg, int64_t n_trg, double *vel);
+
+/* StreamLine::compute / VortexLine::compute (streamline.cpp) for n_lines seeds x0 (3 each) at once: odeint's
+ * integrate_adaptive with the controlled Cash-Karp 5(4) stepper (default error checker and step adjuster, 500 failed
+ * tries end a line), from t = 0 to +t_final and, with back_integrate, to -t_final.  kind 0 integrates the velocity,
+ * kind 1 the vorticity (central differences at +-1e-7, streamline.cpp:16-35); the integration stops where
+ * |velocity| > 1e3.  Output per line i, left-aligned in rows of 2 max_points - 1 points: the back points reversed
+ * without their copy of x0, then the forward points (join_back_and_forward); x and val are 3 per point (val: the
+ * velocity or the vorticity there), t 1 per point; n_points[i] points.  status[2 i + d] (d = 0 back, 1 forward): 0
+ * reached +-t_final, 1 |velocity| > 1e3, 2 500 failed tries, 3 max_points points in that direction (this library's
+ * cap: the reference has none); the back status is 0 without back_integrate. */
+typedef struct {
+    double dt_init, t_final, abs_err, rel_err;
+    int32_t back_integrate, max_points;
+} skb_line_request;
+enum { SKB_STREAMLINE = 0, SKB_VORTEXLINE = 1 };
+SKB_API int skb_flow_listener_lines(skb_flow *fl, int kind, const double *x0, int32_t n_lines,
+                                    const skb_line_request *req, double *x, double *t, double *val, int32_t *n_points,
+                                    int32_t *status);
+
 /* ---- fused matvec flow -------------------------------------------------------------------------------
  * v_all over targets [fibers | periphery | bodies] (get_node_maps, system.cpp:234-241):
  *   v_all  = fiber flow (all targets, self term subtracted)

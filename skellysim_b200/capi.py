@@ -67,6 +67,11 @@ class PeripheryShape(C.Structure):
                 ("polar_angle_end", C.c_double), ("binding_threshold", C.c_double)]
 
 
+class LineRequest(C.Structure):
+    _fields_ = [("dt_init", C.c_double), ("t_final", C.c_double), ("abs_err", C.c_double), ("rel_err", C.c_double),
+                ("back_integrate", C.c_int32), ("max_points", C.c_int32)]
+
+
 class DenseStats(C.Structure):
     _fields_ = [("kernel_ms", C.c_double), ("total_ms", C.c_double), ("bytes", C.c_int64)]
 
@@ -157,6 +162,11 @@ def library() -> C.CDLL:
         "skb_flow_set_point_sources": ([ctxp, _dp, _dp, _dp, C.c_int], C.c_int),
         "skb_flow_set_background": ([ctxp, C.POINTER(C.c_int), _dp, _dp], C.c_int),
         "skb_flow_velocity_at_targets": ([ctxp, _dp, C.c_int64, _dp, _dp, _dp, _dp, C.c_double, _dp], C.c_int),
+        "skb_flow_set_listener_frame": ([ctxp, _dp, _dp, _dp, _dp, _dp, C.POINTER(C.c_int32), _dp, C.c_double],
+                                        C.c_int),
+        "skb_flow_listener_velocity": ([ctxp, _dp, C.c_int64, _dp], C.c_int),
+        "skb_flow_listener_lines": ([ctxp, C.c_int, _dp, C.c_int32, C.POINTER(LineRequest), _dp, _dp, _dp,
+                                     C.POINTER(C.c_int32), C.POINTER(C.c_int32)], C.c_int),
         "skb_flow_set_target_window": ([ctxp, C.c_int64, C.c_int64], C.c_int),
         "skb_flow_set_self_exclusion": ([ctxp, C.c_int], C.c_int),
         "skb_flow_set_overlap": ([ctxp, C.c_int], C.c_int),
@@ -704,6 +714,53 @@ class Flow:
         _check(library().skb_flow_velocity_at_targets(self._h, _p(r_trg), r_trg.shape[0], _p(a), _p(b), _p(c), _p(ft),
                                                       float(eta), _p(vel)))
         return vel
+
+    def set_listener_frame(self, fib_forces, shell_density, body_densities, body_forces_torques, body_velocities,
+                           body_kind, body_radii, eta):
+        """The listener's frame (listener.cpp): the strengths of velocity_at_targets, and per body [U, omega]
+        (body_velocities, (n_bodies, 6)), the interior test (body_kind: 0 none, 1 sphere, 2 ellipsoid) and its radii
+        ((n_bodies, 3); a sphere reads the first).  Stale once the geometry, point sources or background change."""
+        a, b, c = _arr(fib_forces, 3), _arr(shell_density, 3), _arr(body_densities, 3)
+        ft, uv, radii = _arr(body_forces_torques, 6), _arr(body_velocities, 6), _arr(body_radii, 3)
+        kind = np.ascontiguousarray(body_kind, dtype=np.int32).reshape(-1)
+        _check(library().skb_flow_set_listener_frame(self._h, _p(a), _p(b), _p(c), _p(ft), _p(uv),
+                                                     kind.ctypes.data_as(C.POINTER(C.c_int32)), _p(radii),
+                                                     float(eta)))
+
+    def velocity_field(self, r):
+        """The listener's velocity_field: System::velocity_at_targets on the frame, (n, 3), with the rigid motion
+        U + omega x dx at points inside a body."""
+        r = _arr(r, 3)
+        vel = np.empty((r.shape[0], 3))
+        _check(library().skb_flow_listener_velocity(self._h, _p(r), r.shape[0], _p(vel)))
+        return vel
+
+    def _lines(self, kind, x0, dt_init, t_final, abs_err, rel_err, back_integrate, max_points):
+        x0 = _arr(x0, 3)
+        n, mp = x0.shape[0], int(max_points)
+        req = LineRequest(float(dt_init), float(t_final), float(abs_err), float(rel_err), int(bool(back_integrate)), mp)
+        row = max(2 * mp - 1, 1)
+        x, val, t = np.empty((n, row, 3)), np.empty((n, row, 3)), np.empty((n, row))
+        n_points, status = np.empty(n, dtype=np.int32), np.empty((n, 2), dtype=np.int32)
+        i32 = C.POINTER(C.c_int32)
+        _check(library().skb_flow_listener_lines(self._h, int(kind), _p(x0), n, C.byref(req), _p(x), _p(t), _p(val),
+                                                 n_points.ctypes.data_as(i32), status.ctypes.data_as(i32)))
+        return [{"x": x[i, :k].copy(), "time": t[i, :k].copy(), "val": val[i, :k].copy(),
+                 "status": (int(status[i, 0]), int(status[i, 1]))} for i, k in enumerate(n_points)]
+
+    def streamlines(self, x0, dt_init=0.1, t_final=1.0, abs_err=1e-10, rel_err=1e-6, back_integrate=True,
+                    max_points=1000):
+        """The listener's streamlines (StreamLine::compute) from the seeds x0 (n, 3), all at once on the device.
+        One dict per seed, the reader's keys: "x" (m, 3), "time" (m,), "val" (m, 3) the velocity there, and
+        "status" (back, forward): 0 reached +-t_final, 1 |v| > 1e3, 2 500 failed tries, 3 max_points in that
+        direction."""
+        return self._lines(0, x0, dt_init, t_final, abs_err, rel_err, back_integrate, max_points)
+
+    def vortexlines(self, x0, dt_init=0.1, t_final=1.0, abs_err=1e-10, rel_err=1e-6, back_integrate=True,
+                    max_points=1000):
+        """The listener's vortex lines (VortexLine::compute): streamlines() of the vorticity (central differences at
+        +-1e-7); "val" is the vorticity, the exits still test the velocity."""
+        return self._lines(1, x0, dt_init, t_final, abs_err, rel_err, back_integrate, max_points)
 
     def set_cross(self, mode: int):
         """Fiber <-> periphery pairs of the matvec in one geometry pass: -1 auto (default), 0 never, 1 whenever applicable."""

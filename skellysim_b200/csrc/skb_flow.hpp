@@ -1,5 +1,6 @@
 // skb_flow.hpp -- the flow (include/skelly_b200_flow.h) and what the translation units built on it share:
 // skb_matvec.cu (its lifetime, geometry, flows and matvec orchestration), skb_system.cu (the whole-system calls),
+// skb_listener.cu (the listener's requests),
 // skb_solve.cu, skb_step.cu, skb_periphery.cu and skb_mflow.cu.  Free functions in namespace skb that take the flow.
 #pragma once
 #include "skb_internal.hpp"
@@ -23,6 +24,11 @@ struct TargetCache {
     void store(const double *r, long long n) {
         host.assign(r, r + 3 * n);
         valid = true;
+        ++version;
+    }
+    // another call has put other targets into the evaluator: the next call with host targets uploads them again
+    void invalidate() {
+        valid = false;
         ++version;
     }
 };
@@ -90,6 +96,35 @@ class PeripheryShape {
     DevBuf force_skip_, collide_skip_, radius_, force_, flags_;
     PinnedHost h_flags_;
 };
+
+// The listener's frame (skb_flow_set_listener_frame) and the device state of its requests (skb_listener.cu,
+// listener_kernels.cuh): the strengths and the bodies' rigid motions of one solution, valid while the flow's
+// geom_version is the one they were set at; the lines' state and output, grow-only
+class Listener {
+  public:
+    int set_frame(skb_flow *fl, const double *fib_forces, const double *shell_density, const double *body_densities,
+                  const double *body_forces_torques, const double *body_velocities, const int32_t *body_kind,
+                  const double *body_radii, double eta);
+    int velocity(skb_flow *fl, const double *r_trg, long long n_trg, double *vel);
+    int lines(skb_flow *fl, int kind, const double *x0, int n_lines, const ::skb_line_request *req, double *x,
+              double *t, double *val, int32_t *n_points, int32_t *status);
+
+  private:
+    // the refusal of a request without a current frame
+    int current(const skb_flow *fl, const char *who) const;
+    // System::velocity_at_targets of the frame at the n_trg device targets d_trg into d_v, on the flow's stream
+    int eval(skb_flow *fl, const double *d_trg, long long n_trg, double *d_v);
+
+    bool set_ = false;
+    unsigned long long version_ = 0;
+    double eta_ = 0;
+    int n_interior_ = 0; // bodies with an interior test
+    DevBuf ff_, sd_, bd_, f_, t_, rigid_; // strengths; per body [kind, r0, r1, r2, cx, cy, cz, U, omega]
+    DevBuf trg_, vel_;                     // targets and velocities of one evaluation
+    // lines: state (SoA) and per-line output; slot -> line map and the active count of the last compaction
+    DevBuf st_x_, st_t_, st_dt_, st_k_, st_int_, out_x_, out_t_, out_val_, slots_, n_act_;
+    PinnedHost h_n_act_;
+};
 } // namespace skb
 
 struct skb_flow {
@@ -153,6 +188,7 @@ struct skb_flow {
     bool placed = false;             // ... valid until skb_flow_set_bodies changes the bodies otherwise
     skb::StepBuffers stepbuf;             // the buffers of skb_flow_step (skb_step.cu)
     skb::PeripheryShape shape;            // skb_flow_set_periphery_shape (skb_periphery.cu)
+    skb::Listener listener;               // skb_flow_set_listener_frame and its requests (skb_listener.cu)
     skb::Group grp; // multi-GPU group membership: one member per GPU, exchange through peer memory (skb_group.cu)
     // a member's whole-vector matvec in flight: matvec_core exchanges the bodies' partial link forces through the
     // window and the body flow reads their totals from ft_sum ([F | L], 6 per body)
@@ -215,6 +251,12 @@ int apply_matvec_core(skb_flow *fl, skb_dense *dn, const double *d_x, const doub
 // skb_flow_set_point_sources and the background flow of skb_flow_set_background at the n_trg targets d_trg, added to
 // the rows of d_v in this order: Oseen contraction, rotlet, background
 int add_sources(skb_flow *fl, const double *d_trg, long long n_trg, double eta, double *d_v, cudaStream_t st);
+// System::velocity_at_targets without its body-interior replacement (system.cpp:355-359) on fl->cur: the fibers'
+// flow (no self subtraction), the bodies', the periphery's and add_sources at the n_trg device targets d_trg, which
+// the arbitrary-target evaluators fib[0], shell[0] and body[0] hold as their targets.  Strengths as the evaluators take
+// them: d_ff 3 per fiber node, d_sd 3 per periphery node, d_bd 3 per body node, d_f and d_t 3 per body
+int velocity_dev(skb_flow *fl, const double *d_trg, long long n_trg, const double *d_ff, const double *d_sd,
+                 const double *d_bd, const double *d_f, const double *d_t, double eta, double *d_v);
 int load_source_kernels(); // the kernels of add_sources, loaded now
 int upload(skb_flow *fl, DevBuf &buf, const double *h, size_t n_doubles);
 int download(skb_flow *fl, double *h, const DevBuf &buf, size_t n_doubles);

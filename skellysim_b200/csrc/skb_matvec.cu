@@ -140,6 +140,16 @@ int skb::add_sources(skb_flow *fl, const double *d_trg, long long n_trg, double 
     return SKB_OK;
 }
 
+int skb::velocity_dev(skb_flow *fl, const double *d_trg, long long n_trg, const double *d_ff, const double *d_sd,
+                      const double *d_bd, const double *d_f, const double *d_t, double eta, double *d_v) {
+    // fc_->flow(r_trg, f_on_fibers, eta, /*subtract_self=*/false) + bc_.flow + shell_->flow   system.cpp:355-359
+    SKB_TRY(fibers_dev(fl, fl->fib[0].get(), kRaw, d_ff, eta, 0, d_v, 0, 0, 0));
+    SKB_TRY(bodies_dev(fl, fl->body[0].get(), d_bd, d_f, d_t, eta, d_v, 1));
+    SKB_TRY(periphery_dev(fl, fl->shell[0].get(), kNormalDensity, d_sd, eta, d_v, 1));
+    // + psc_.flow(r_trg, eta, time) + bs_.flow(r_trg, eta)                                  system.cpp:358-359
+    return add_sources(fl, d_trg, n_trg, eta, d_v, fl->cur);
+}
+
 int skb::load_source_kernels() {
     cudaFuncAttributes fa;
     CUDA_TRY(cudaFuncGetAttributes(&fa, oseen_contract_add_kernel));
@@ -603,13 +613,9 @@ int skb_flow_velocity_at_targets(skb_flow *fl, const double *r_trg, int64_t n_tr
         SKB_TRY(upload(fl, fl->in_body, s.bd, (size_t)fl->n_body * 3));
         SKB_TRY(upload(fl, fl->in_force, s.f, f.size()));
         SKB_TRY(upload(fl, fl->in_torque, s.t, t.size()));
-        // fc_->flow(r_trg, f_on_fibers, eta, /*subtract_self=*/false) + bc_.flow + shell_->flow   system.cpp:355-359
-        SKB_TRY(fibers_dev(fl, fl->fib[0].get(), kRaw, (const double *)fl->in_fib.ptr, eta, 0, d_v, 0, 0, 0));
-        SKB_TRY(bodies_dev(fl, fl->body[0].get(), (const double *)fl->in_body.ptr, (const double *)fl->in_force.ptr,
-                           (const double *)fl->in_torque.ptr, eta, d_v, 1));
-        SKB_TRY(periphery_dev(fl, fl->shell[0].get(), kNormalDensity, (const double *)fl->in_shell.ptr, eta, d_v, 1));
-        // + psc_.flow(r_trg, eta, time) + bs_.flow(r_trg, eta)                                  system.cpp:358-359
-        SKB_TRY(add_sources(fl, (const double *)fl->fib[0]->devs[0].r_trg.ptr, n_trg, eta, d_v, fl->stream));
+        SKB_TRY(velocity_dev(fl, (const double *)fl->fib[0]->devs[0].r_trg.ptr, n_trg, (const double *)fl->in_fib.ptr,
+                             (const double *)fl->in_shell.ptr, (const double *)fl->in_body.ptr,
+                             (const double *)fl->in_force.ptr, (const double *)fl->in_torque.ptr, eta, d_v));
         return download(fl, s.v, fl->vel, (size_t)n_trg * 3);
     };
     if (!s.pinned)
