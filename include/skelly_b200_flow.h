@@ -666,6 +666,57 @@ SKB_API int skb_flow_set_periphery_shape(skb_flow *fl, const skb_periphery_shape
 SKB_API int skb_flow_periphery_interaction(skb_flow *fl, double *f_periphery, int32_t *plus_hinged,
                                            int32_t *collided);
 
+/* ---- dynamic instability: catastrophe, growth and nucleation before each step --------------------------------------
+ * System::dynamic_instability (dynamic_instability.cpp:25-194), the first statement of System::prep_state_for_solver,
+ * on a single-device flow (DESIGN.md §3.11).  di.n_nodes == 0 changes nothing (the reference's early return).  Else,
+ * for each fiber f in container order, pinned = plus_pinned[f]:
+ *   v = v_growth, fc = f_catastrophe, each times its *_collision_scale when pinned;
+ *   the fiber is removed when u_f > exp(-dt fc) (u_f the draw (f, 0) of the stream below);
+ *   a survivor gets length_prev = length, length = length + dt v (v_growth_out = v); a bound survivor occupies its site.
+ * Then n_new = min(Poisson(dt nucleation_rate (n_sites - fibers bound before the catastrophe)), free sites), the sites
+ * picked uniformly without replacement (a partial Fisher-Yates over the free flat sites in ascending order), and one
+ * new fiber per pick appended after the survivors in pick order: di.n_nodes nodes, length = length_prev = min_length,
+ * radius, bending_rigidity, penalty_param 500, beta_tstep 1, minus_clamped 1, plus_hinged 0, v_growth 0, a straight
+ * line from the site (c + R(q) site_ref at the current placement) along (site - c) / |site - c|.
+ * The draws come from Philox4x32-10 with key = seed and counter = (i, purpose, call counter): the result depends on
+ * (seed, counter) and the inputs only.  It is not the reference's stream (DESIGN.md §5).
+ *   skb_flow_set_nucleation_sites: the bodies' nucleation_sites_ref_ (body frame), once per run: n_sites_per_body per
+ *     body of skb_flow_set_bodies, site_ref 3 per site, bodies concatenated.  Refused: a NULL count table with bodies,
+ *     a negative count, a non-finite site or one at the body's centre.
+ *   skb_flow_dynamic_instability: n_in == the flow's fiber count; params_in, binding_in ((body, site) per fiber, -1 for
+ *     a free fiber), plus_pinned (bc_plus_ of the last step: skb_flow_step_flags, or the caller's at the start) per
+ *     input fiber.  The outputs hold `capacity` fibers: *n_out, params_out, binding_out, v_growth_out and origin_out
+ *     (the input fiber output fiber f came from, -1 for a nucleated one: through it the caller carries its own
+ *     per-fiber arrays, such as force_scale).  On SKB_OK the flow holds the new fibers -- positions, node counts and
+ *     lengths through the skb_flow_set_fibers path, the periphery shape's per-fiber flags carried through origin (0
+ *     for new fibers) and its buffers sized, the GMRES workspace and the step's buffers sized at the num_blocks of the
+ *     last skb_flow_set_gmres -- and the next skb_flow_step needs no other set-up.  Refused (SKB_ERR_INVALID, before
+ *     any launch, the geometry untouched): a group member (its window is sized for a fixed fiber set), dt <= 0 or not
+ *     finite, a non-finite or negative rate or scale, a non-positive min_length or radius, a negative bending rigidity,
+ *     di.n_nodes outside [8, 128] or without skb_flow_set_fiber_class and _class_derivatives, a binding outside the
+ *     sites, a plus_pinned outside {0, 1}, bodies without sites or placement, n_in != the flow's fiber count,
+ *     capacity < n_in + the number of sites.  skb_mflow has no such call.
+ *   skb_flow_step_flags: plus_hinged of each fiber as the last installed skb_flow_step built it (the periphery
+ *     binding's value with a shape, the caller's otherwise): bc_plus_ at the next is_plus_pinned().  Carried through
+ *     skb_flow_dynamic_instability (0 for new fibers).  Refused when no step was installed for the current fiber count. */
+typedef struct skb_dynamic_instability { /* params.hpp:30-42 (min_separation is never used there) */
+    int32_t n_nodes;                     /* nodes of a nucleated fiber; 0: the model is off */
+    int32_t reserved;
+    double v_growth, f_catastrophe, v_grow_collision_scale, f_catastrophe_collision_scale, nucleation_rate;
+    double radius, min_length, bending_rigidity;
+} skb_dynamic_instability;
+typedef struct skb_dynamic_info {
+    int32_t removed, nucleated, grown, reserved;
+    double mu; /* the Poisson mean of the nucleation count */
+} skb_dynamic_info;
+SKB_API int skb_flow_set_nucleation_sites(skb_flow *fl, const int *n_sites_per_body, const double *site_ref);
+SKB_API int skb_flow_dynamic_instability(skb_flow *fl, const skb_dynamic_instability *di, double dt, uint64_t seed,
+                                         uint64_t counter, int n_in, const skb_fiber_params *params_in,
+                                         const int32_t *binding_in, const int32_t *plus_pinned, int capacity,
+                                         int *n_out, skb_fiber_params *params_out, int32_t *binding_out,
+                                         double *v_growth_out, int32_t *origin_out, skb_dynamic_info *info);
+SKB_API int skb_flow_step_flags(skb_flow *fl, int32_t *plus_hinged);
+
 /* ---- the whole-vector calls on one rank per GPU ---------------------------------------------------------------------
  * A group member (skb_flow_group_init ... skb_flow_group_warmup above) applies A, P^-1 and builds the RHS on its LOCAL
  * vector: its own rows of the whole vector [fibers | shell | bodies], in ascending global order --
@@ -860,6 +911,8 @@ SKB_API int skb_mflow_step(skb_mflow *mf, const skb_fiber_params *params, const 
                            const double *force_scale, const double *f_external, const double *body_forces_torques,
                            const int *fiber_body, const double *site_ref, double dt, double eta, double tol,
                            int num_blocks, int max_iters, double *x, double *tension, skb_step_info *info);
+/* skb_mflow has no dynamic instability (skb_flow_dynamic_instability): its members' windows are sized for a fixed fiber
+ * set at skb_flow_group_init. */
 /* skb_flow_set_periphery_shape on every member (the complete arrays); skb_mflow_step applies it on every member */
 SKB_API int skb_mflow_set_periphery_shape(skb_mflow *mf, const skb_periphery_shape *shape,
                                           const int32_t *fiber_minus_clamped, const double *body_radius);

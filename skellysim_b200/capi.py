@@ -76,6 +76,19 @@ class DenseStats(C.Structure):
     _fields_ = [("kernel_ms", C.c_double), ("total_ms", C.c_double), ("bytes", C.c_int64)]
 
 
+class DynamicInstability(C.Structure):
+    """skb_dynamic_instability (include/skelly_b200_flow.h): the [dynamic_instability] table (params.hpp:30-42)"""
+    _fields_ = [("n_nodes", C.c_int32), ("reserved", C.c_int32), ("v_growth", C.c_double),
+                ("f_catastrophe", C.c_double), ("v_grow_collision_scale", C.c_double),
+                ("f_catastrophe_collision_scale", C.c_double), ("nucleation_rate", C.c_double), ("radius", C.c_double),
+                ("min_length", C.c_double), ("bending_rigidity", C.c_double)]
+
+
+class DynamicInfo(C.Structure):
+    _fields_ = [("removed", C.c_int32), ("nucleated", C.c_int32), ("grown", C.c_int32), ("reserved", C.c_int32),
+                ("mu", C.c_double)]
+
+
 class FiberParams(C.Structure):
     """skb_fiber_params (include/skelly_b200_flow.h): the per-fiber scalars of skb_flow_build_fiber_operators."""
     _fields_ = [("length_prev", C.c_double), ("bending_rigidity", C.c_double), ("radius", C.c_double),
@@ -294,6 +307,13 @@ def library() -> C.CDLL:
         "skb_mflow_set_periphery_shape": ([ctxp, C.POINTER(PeripheryShape), C.POINTER(C.c_int32), _dp], C.c_int),
         "skb_mflow_periphery_interaction": ([ctxp, _dp, C.POINTER(C.c_int32), C.POINTER(C.c_int32)], C.c_int),
         "skb_mflow_get_placement": ([ctxp, _dp, _dp], C.c_int),
+        "skb_flow_set_nucleation_sites": ([ctxp, C.POINTER(C.c_int), _dp], C.c_int),
+        "skb_flow_dynamic_instability": ([ctxp, C.POINTER(DynamicInstability), C.c_double, C.c_uint64, C.c_uint64,
+                                          C.c_int, C.POINTER(FiberParams), C.POINTER(C.c_int32),
+                                          C.POINTER(C.c_int32), C.c_int, C.POINTER(C.c_int), C.POINTER(FiberParams),
+                                          C.POINTER(C.c_int32), _dp, C.POINTER(C.c_int32), C.POINTER(DynamicInfo)],
+                                         C.c_int),
+        "skb_flow_step_flags": ([ctxp, C.POINTER(C.c_int32)], C.c_int),
         "skb_mflow_solve_system": ([ctxp, _dp, C.c_double, C.c_double, C.c_int, C.c_int, _dp, C.POINTER(SolveInfo),
                                     _dp], C.c_int),
     }
@@ -1150,6 +1170,7 @@ class Flow:
     def set_gmres(self, num_blocks: int = 300):
         """Size the workspace of solve_system for the current solution size and up to num_blocks basis vectors."""
         _check(library().skb_flow_set_gmres(self._h, int(num_blocks)))
+        self._gmres_blocks = int(num_blocks)
 
     def solve_system(self, rhs, eta, dense=None, tol=1e-10, num_blocks=300, max_iters=1000):
         """Solver::solve (solver_hydro.cpp:64-95): x = A^-1 rhs by restarted right-preconditioned GMRES on the device.
@@ -1183,6 +1204,12 @@ class Flow:
         _shape_call(library().skb_flow_set_periphery_shape, self._h, self._n_fibers(), self.n_bodies, kind, a, b, c,
                     f_0, l_0, binding_active, polar_angle_start, polar_angle_end, binding_threshold,
                     fiber_minus_clamped, body_radius)
+        # kept so that the shape can be set again for another fiber set (timestep.Stepper.restore)
+        self._shape = dict(kind=kind, a=a, b=b, c=c, f_0=f_0, l_0=l_0, binding_active=binding_active,
+                           polar_angle_start=polar_angle_start, polar_angle_end=polar_angle_end,
+                           binding_threshold=binding_threshold, body_radius=body_radius,
+                           fiber_minus_clamped=np.zeros(self._n_fibers(), dtype=np.int32)
+                           if fiber_minus_clamped is None else np.array(fiber_minus_clamped, dtype=np.int32))
 
     set_periphery_shape.__doc__ = _SHAPE_DOC
 
@@ -1209,6 +1236,69 @@ class Flow:
 
     def _n_fibers(self):
         return len(getattr(self, "_fiber_off", [0])) - 1
+
+    def set_nucleation_sites(self, n_sites_per_body, site_ref):
+        """the bodies' nucleation_sites_ref_ (body frame), concatenated: n_sites_per_body per body, site_ref (total, 3)
+        (skb_flow_set_nucleation_sites)"""
+        n = np.ascontiguousarray(n_sites_per_body, dtype=np.int32).reshape(-1)
+        s = _arr(site_ref, 3)
+        if n.shape[0] != self.n_bodies or int(n.sum()) != s.shape[0]:
+            raise ValueError(f"expected {self.n_bodies} site counts summing to {s.shape[0]}, got {n}")
+        _check(library().skb_flow_set_nucleation_sites(self._h, n.ctypes.data_as(C.POINTER(C.c_int)), _p(s)))
+        self._sites = (n.copy(), s.copy())
+
+    def dynamic_instability(self, di, dt, seed, counter, params, binding, plus_pinned):
+        """System::dynamic_instability on the device (skb_flow_dynamic_instability).  di: a dict (or
+        DynamicInstability) of the [dynamic_instability] table; params: the seven per-fiber parameters of
+        build_fiber_operators (scalars or per fiber) or a FIBER_PARAMS_DTYPE array; binding (N_fibers, 2) ints (body,
+        site), -1 free; plus_pinned (N_fibers,) ints.  The flow then holds the new fiber set.  Returns a dict: params
+        (FIBER_PARAMS_DTYPE), binding, v_growth, origin (the input fiber of each output fiber, -1 nucleated), n_nodes,
+        lengths, and the info fields removed, nucleated, grown, mu."""
+        if not isinstance(di, DynamicInstability):
+            di = DynamicInstability(**{k: di.get(k, 0) for k, _ in DynamicInstability._fields_ if k != "reserved"})
+        nf = self._n_fibers()
+        p = params if isinstance(params, np.ndarray) and params.dtype == FIBER_PARAMS_DTYPE else fiber_params(nf, *params)
+        p = np.ascontiguousarray(p)
+        b = np.ascontiguousarray(binding, dtype=np.int32).reshape(nf, 2)
+        pp = np.ascontiguousarray(np.broadcast_to(np.asarray(plus_pinned, dtype=np.int32), (nf,)))
+        n_sites = int(self._sites[0].sum()) if getattr(self, "_sites", None) is not None and self.n_bodies else 0
+        cap = nf + n_sites
+        p_out = np.zeros(cap, dtype=FIBER_PARAMS_DTYPE)
+        b_out = np.zeros((cap, 2), dtype=np.int32)
+        v_out, origin = np.zeros(cap), np.zeros(cap, dtype=np.int32)
+        n_out, info = C.c_int(0), DynamicInfo()
+        i32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_int32))
+        _check(library().skb_flow_dynamic_instability(self._h, C.byref(di), float(dt), int(seed), int(counter), nf,
+                                                       _params_ptr(p), i32(b), i32(pp), cap, C.byref(n_out),
+                                                       _params_ptr(p_out), i32(b_out), _p(v_out), i32(origin),
+                                                       C.byref(info)))
+        m = n_out.value
+        origin = origin[:m].copy()
+        out = dict(params=p_out[:m].copy(), binding=b_out[:m].copy(), origin=origin, removed=info.removed,
+                   nucleated=info.nucleated, grown=info.grown, mu=info.mu)
+        old_n = np.diff(self._fiber_off).astype(np.int32) if nf else np.zeros(0, dtype=np.int32)
+        if di.n_nodes == 0:
+            out.update(v_growth=None, n_nodes=old_n, lengths=self._lengths.copy())
+            return out
+        out["v_growth"] = v_out[:m].copy()
+        out["n_nodes"] = np.where(origin >= 0, old_n[np.maximum(origin, 0)] if nf else 0, di.n_nodes).astype(np.int32)
+        # the lengths the device installed: length_prev + dt v (one rounded product and one rounded sum; min_length
+        # for a new fiber, whose v is 0)
+        out["lengths"] = out["params"]["length_prev"] + float(dt) * out["v_growth"]
+        self.n_fib = int(out["n_nodes"].sum())
+        self._fiber_off = np.concatenate([[0], np.cumsum(out["n_nodes"], dtype=np.int64)])
+        self._lengths = out["lengths"].copy()
+        if getattr(self, "_shape", None) is not None:
+            mc = self._shape["fiber_minus_clamped"]
+            self._shape["fiber_minus_clamped"] = np.where(origin >= 0, mc[np.maximum(origin, 0)] if nf else 0,
+                                                          0).astype(np.int32)
+        return out
+
+    def step_flags(self):
+        """plus_hinged (N_fibers,) int32 of each fiber as the last installed step built it (skb_flow_step_flags)"""
+        h = np.empty(self._n_fibers(), dtype=np.int32)
+        _check(library().skb_flow_step_flags(self._h, h.ctypes.data_as(C.POINTER(C.c_int32))))
+        return h
 
     def fiber_error(self):
         """fiber_error_local (fcfd.cpp:79-89) of the current geometry on the device: (max, per-fiber maxima)"""

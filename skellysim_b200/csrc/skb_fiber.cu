@@ -112,6 +112,14 @@ int FiberOps::upload_classes(cudaStream_t st) {
 }
 
 // derivatives: the device build's and the RHS's needs (class derivatives, n within the build's range)
+bool FiberOps::buildable(int n) const {
+    const auto it = classes.find(n);
+    return n >= kBuildMinNodes && n <= kBuildMaxNodes && it != classes.end() && !it->second.D.empty() &&
+           !it->second.D234.empty();
+}
+int FiberOps::build_min_nodes() { return kBuildMinNodes; }
+int FiberOps::build_max_nodes() { return kBuildMaxNodes; }
+
 int FiberOps::check_class(int f, int n, bool derivatives) const {
     auto it = classes.find(n);
     if (it == classes.end() || it->second.D.empty())

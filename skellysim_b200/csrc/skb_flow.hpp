@@ -72,6 +72,10 @@ class PeripheryShape {
     void note_clamped(int f0, int nf, const ::skb_fiber_params *params);
     // the same flags of ALL fibers as the group step all-gathered them (1.0 / 0.0 per fiber)
     void note_clamped_all(const std::vector<double> &flags);
+    // the per-fiber tables of n_old fibers carried to a new set of n_fibers fibers (skb_flow_dynamic_instability):
+    // fiber j takes the flags of fiber origin[j], 0 where origin[j] < 0; the pass's buffers sized for n_fib nodes.  A
+    // no-op without a shape, or when the tables were set for another fiber count (a step then refuses, as before)
+    int carry(const int *origin, int n_old, int n_fibers, long long n_fib, cudaStream_t st);
     // minus_clamped of params (fibers [f0, f0 + nf)) uploaded on st into the device table the group step's kernel
     // reads (clamp_table(), indexed by fiber among ALL fibers), without noting them
     int upload_clamped(int f0, int nf, const ::skb_fiber_params *params, cudaStream_t st);
@@ -93,6 +97,7 @@ class PeripheryShape {
     long long cap_nodes_ = -1;
     size_t flag_cap_ = 0; // ints of h_flags_
     std::vector<int> h_clamped_; // the collision test's node-0 skip per fiber
+    std::vector<int> h_force_skip_; // fiber_minus_clamped of the call (the repulsion's node-0 skip)
     DevBuf force_skip_, collide_skip_, radius_, force_, flags_;
     PinnedHost h_flags_;
 };
@@ -124,6 +129,17 @@ class Listener {
     // lines: state (SoA) and per-line output; slot -> line map and the active count of the last compaction
     DevBuf st_x_, st_t_, st_dt_, st_k_, st_int_, out_x_, out_t_, out_val_, slots_, n_act_;
     PinnedHost h_n_act_;
+};
+// The bodies' nucleation sites (skb_flow_set_nucleation_sites) and the buffers of skb_flow_dynamic_instability
+// (skb_dynamic.cu, dynamic_kernels.cuh)
+struct DynamicInstability {
+    std::vector<int> site_count;     // per body
+    std::vector<long long> site_off; // first flat site of every body (n_bodies + 1)
+    std::vector<double> site_ref;    // 3 per site, body frame, bodies concatenated
+    bool sites_set = false;
+    DevBuf d_site_ref, fib, len_new, counts, src, dst_off, picks, frames, r_new, len_out;
+    PinnedHost h_counts; // DiCounts, then the keep bytes, then the occupancy bytes
+    size_t h_cap = 0;    // bytes of h_counts
 };
 } // namespace skb
 
@@ -189,6 +205,8 @@ struct skb_flow {
     skb::StepBuffers stepbuf;             // the buffers of skb_flow_step (skb_step.cu)
     skb::PeripheryShape shape;            // skb_flow_set_periphery_shape (skb_periphery.cu)
     skb::Listener listener;               // skb_flow_set_listener_frame and its requests (skb_listener.cu)
+    skb::DynamicInstability dyn;          // skb_flow_set_nucleation_sites, skb_flow_dynamic_instability
+    std::vector<int> step_hinged;         // plus_hinged each fiber was built with by the last installed step
     skb::Group grp; // multi-GPU group membership: one member per GPU, exchange through peer memory (skb_group.cu)
     // a member's whole-vector matvec in flight: matvec_core exchanges the bodies' partial link forces through the
     // window and the body flow reads their totals from ft_sum ([F | L], 6 per body)

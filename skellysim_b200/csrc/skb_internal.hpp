@@ -221,6 +221,11 @@ class FiberOps {
     int size_build(const OwnFibers &own);
     bool build_sized_for(const OwnFibers &own) const { return build_key_ == build_key(own); }
     int ready(const char *who, bool with_inverse = false) const; // an error naming `who` unless they are resident
+    // a fiber of n nodes can be built: n within the build's range, skb_flow_set_fiber_class(n) and
+    // skb_flow_set_fiber_class_derivatives(n) called
+    bool buildable(int n) const;
+    static int build_min_nodes();
+    static int build_max_nodes();
     bool empty() const { return n_items_A == 0; }
     int n_fibers() const { return f1 - f0; }
     // drops the resident operators: no GEMV runs on them again (a flow left with no fibers has the empty set)

@@ -73,6 +73,7 @@ int PeripheryShape::set(const skb_periphery_shape *shape, const int *minus_clamp
         CUDA_TRY(cudaMemcpyAsync(radius_.ptr, radius.data(), radius.size() * 8, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaStreamSynchronize(st)); // (the host copies above go out of scope)
     h_clamped_ = skip;
+    h_force_skip_ = skip;
     n_fibers_ = n_fibers;
     n_bodies_ = n_bodies;
     s_ = *shape;
@@ -108,6 +109,26 @@ void PeripheryShape::note_clamped(int f0, int nf, const skb_fiber_params *params
 void PeripheryShape::note_clamped_all(const std::vector<double> &flags) {
     for (size_t f = 0; active_ && f < flags.size() && f < h_clamped_.size(); ++f)
         h_clamped_[f] = flags[f] != 0.0 ? 1 : 0;
+}
+
+int PeripheryShape::carry(const int *origin, int n_old, int n_fibers, long long n_fib, cudaStream_t st) {
+    if (!active_ || n_old != n_fibers_)
+        return SKB_OK;
+    std::vector<int> skip((size_t)n_fibers, 0), clamped((size_t)n_fibers, 0);
+    for (int f = 0; f < n_fibers; ++f)
+        if (origin[f] >= 0) {
+            skip[(size_t)f] = h_force_skip_[(size_t)origin[f]];
+            clamped[(size_t)f] = h_clamped_[(size_t)origin[f]];
+        }
+    SKB_TRY(force_skip_.ensure((size_t)n_fibers * sizeof(int) + 8));
+    SKB_TRY(collide_skip_.ensure((size_t)n_fibers * sizeof(int) + 8));
+    if (n_fibers > 0)
+        CUDA_TRY(cudaMemcpyAsync(force_skip_.ptr, skip.data(), skip.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaStreamSynchronize(st)); // (the host copy above goes out of scope)
+    h_force_skip_ = std::move(skip);
+    h_clamped_ = std::move(clamped);
+    n_fibers_ = n_fibers;
+    return size(n_fib);
 }
 
 int PeripheryShape::upload_clamped(int f0, int nf, const skb_fiber_params *params, cudaStream_t st) {

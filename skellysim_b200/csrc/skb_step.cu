@@ -385,6 +385,10 @@ static int step_run(skb_flow *fl, skb_dense *dn, const StepArgs &a, StepCall &c,
     SKB_TRY(skb_flow_set_fiber_links(fl, a.fiber_body, sites_new.data(), c.rigidity.data()));
     // System::check_collision of the installed geometry, node 0 skipped on this step's is_minus_clamped()
     fl->shape.note_clamped(0, nf, c.params(a));
+    // the bc_plus_ of the next dynamic instability's is_plus_pinned() (skb_flow_step_flags)
+    fl->step_hinged.resize((size_t)nf);
+    for (int f = 0; f < nf; ++f)
+        fl->step_hinged[(size_t)f] = c.params(a)[f].plus_hinged;
     return periphery_collided(fl, &info->collided, st, &fl->launches);
 }
 

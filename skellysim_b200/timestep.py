@@ -6,10 +6,18 @@ periphery shape (Flow.set_periphery_shape): the step reports the collision test 
 schedule stays the caller's host code (DESIGN.md §7): `run` takes it as the callable `forces(time, r_fib)`, and a
 caller's own `collided(r_fib, centers)` still replaces the step's test.
 
+With dynamic_instability (the [dynamic_instability] table as a dict), each step of `run` starts as
+System::prep_state_for_solver does: Stepper.dynamic_instability removes, grows and nucleates fibers on the device
+(Flow.dynamic_instability) before the forces are asked for, and the Stepper carries its per-fiber tables to the new fiber
+set.  Its random stream is (seed, call counter): the counter advances on every attempt and a rejected step does not
+rewind it, as the reference's restore() does not rewind its generator.
+
 One deviation from the reference's loop (DESIGN.md §5): the reference sets dt to the grown dt_new before it advances
 time on an accepted step (system.cpp:554-557), so time advances by a dt no step used.  Here time advances by the dt of
 the step that was accepted."""
 import numpy as np
+
+from . import capi
 
 class Stepper:
     """A capi.Flow or capi.MultiFlow and what its steps need: its Dense (None without periphery), the fibers' parameters (the seven of
@@ -18,12 +26,27 @@ class Stepper:
     copy of it: fiber positions, body centres and quaternions."""
 
     def __init__(self, flow, dense, params, eta, fiber_body=None, site_ref=None, v_growth=None, force_scale=None,
-                 tol=1e-10, num_blocks=300, max_iters=1000):
+                 tol=1e-10, num_blocks=300, max_iters=1000, dynamic_instability=None, seed=0, fiber_site=None):
+        """dynamic_instability: None (off) or a dict of the [dynamic_instability] table (capi.DynamicInstability's
+        fields); then the flow needs Flow.set_nucleation_sites, each bound fiber names its site by fiber_site (the
+        index among its body's sites) instead of site_ref, and seed starts the random stream."""
         self.flow, self.dense, self.params, self.eta = flow, dense, tuple(params), float(eta)
         self.fiber_body, self.site_ref = fiber_body, site_ref
         self.v_growth, self.force_scale = v_growth, force_scale
         self.tol, self.num_blocks, self.max_iters = tol, num_blocks, max_iters
         self._backup = None
+        self.di, self.seed, self.counter = dynamic_instability, int(seed), 0
+        if self.di is not None:
+            n = flow._n_fibers()
+            p = capi.fiber_params(n, *self.params)
+            self.params = tuple(p[name].copy() for name in capi.FIBER_PARAMS_DTYPE.names)
+            body = np.full(n, -1, dtype=np.int32) if fiber_body is None else np.asarray(fiber_body, dtype=np.int32)
+            site = np.full(n, -1, dtype=np.int32) if fiber_site is None else np.asarray(fiber_site, dtype=np.int32)
+            self.binding = np.stack([body, np.where(body >= 0, site, -1)], axis=1).astype(np.int32)
+            self.v_growth = np.zeros(n) if v_growth is None else capi._per_fiber(v_growth, n)
+            self.force_scale = None if force_scale is None else capi._per_fiber(force_scale, n)
+            self.plus_pinned = np.asarray(p["plus_hinged"], dtype=np.int32).copy()
+            self._bindings()
 
     def positions(self):
         return self.flow.fibers()
@@ -33,6 +56,38 @@ class Stepper:
             return np.zeros((0, 3)), np.zeros((0, 4))
         return self.flow.placement()
 
+    def _bindings(self):
+        """fiber_body and site_ref of the step from the (body, site) bindings and the flow's site table"""
+        body = self.binding[:, 0]
+        self.fiber_body = body.copy()
+        if not (body >= 0).any():
+            self.site_ref = None
+            return
+        counts, ref = self.flow._sites
+        off = np.concatenate([[0], np.cumsum(counts)])
+        flat = np.where(body >= 0, off[np.maximum(body, 0)] + self.binding[:, 1], 0)
+        self.site_ref = ref[flat]
+
+    def dynamic_instability(self, dt):
+        """System::dynamic_instability before a step (a no-op without the model); returns the call's dict or None"""
+        if self.di is None:
+            return None
+        call = self.counter
+        self.counter += 1
+        out = self.flow.dynamic_instability(self.di, dt, self.seed, call, self.params, self.binding, self.plus_pinned)
+        if out["v_growth"] is None:  # n_nodes == 0: nothing changed
+            return out
+        o = out["origin"]
+        carry = lambda a: np.where(o >= 0, a[np.maximum(o, 0)] if a.size else 0, 0).astype(a.dtype)
+        self.params = tuple(out["params"][name].copy() for name in capi.FIBER_PARAMS_DTYPE.names)
+        self.binding = out["binding"].astype(np.int32)
+        self.v_growth = out["v_growth"]
+        if self.force_scale is not None:
+            self.force_scale = carry(self.force_scale)
+        self.plus_pinned = carry(self.plus_pinned)
+        self._bindings()
+        return out
+
     def step(self, dt, f_external=None, body_forces_torques=None):
         """one System::step; returns the step's info (the solve's fields, fiber_error, worst_fiber; a NaN fiber_error:
         the solution was not finite and nothing was installed)"""
@@ -40,21 +95,38 @@ class Stepper:
                                     body_forces_torques=body_forces_torques, fiber_body=self.fiber_body,
                                     site_ref=self.site_ref, v_growth=self.v_growth, force_scale=self.force_scale,
                                     tol=self.tol, num_blocks=self.num_blocks, max_iters=self.max_iters)
+        if self.di is not None and np.isfinite(info["fiber_error"]):
+            self.plus_pinned = self.flow.step_flags()
         return info
 
     def backup(self):
         self._backup = (self.positions(), *self.placement())
+        if self.di is not None:  # the whole fiber set: counts, lengths, the per-fiber tables, the flags
+            shape = getattr(self.flow, "_shape", None)
+            self._fiber_set = (np.diff(self.flow._fiber_off), self.flow._lengths.copy(), self.params, self.binding,
+                               self.v_growth, self.force_scale, self.plus_pinned,
+                               None if shape is None else shape["fiber_minus_clamped"].copy())
 
     def restore(self):
         r, c, q = self._backup
-        self.flow.set_fibers(r, np.diff(self.flow._fiber_off), self.flow._lengths)
+        if self.di is None:
+            self.flow.set_fibers(r, np.diff(self.flow._fiber_off), self.flow._lengths)
+        else:
+            (n_nodes, lengths, self.params, self.binding, self.v_growth, self.force_scale, self.plus_pinned,
+             clamped) = self._fiber_set
+            self.flow.set_fibers(r, n_nodes, lengths)
+            self._bindings()
+            if clamped is not None:
+                self.flow.set_periphery_shape(**dict(self.flow._shape, fiber_minus_clamped=clamped))
+            self.flow.set_gmres(self.flow._gmres_blocks)
         if self.flow.n_bodies:
             self.flow.place_bodies(c, q)
 
 
 def run(stepper, t_final, dt, adaptive=True, dt_min=1e-5, dt_max=np.inf, beta_up=1.2, beta_down=0.5,
         fiber_error_tol=0.1, forces=None, collided=None, time=0.0):
-    """System::run's loop until time >= t_final.  Each step: backup, forces(time, r_fib) -> (f_external (N_f, 3),
+    """System::run's loop until time >= t_final.  Each step: backup, the dynamic instability (Stepper's model, if
+    any), forces(time, r_fib) -> (f_external (N_f, 3),
     F_T (n_bodies, 6)), either None (no callable: no external forces), the step, then the acceptance:
       adaptive: accept when converged and fiber_error <= fiber_error_tol, and then grow dt by beta_up (at most dt_max)
       when fiber_error <= 0.9 fiber_error_tol; otherwise shrink dt by beta_down.  A converged step that collided is
@@ -65,6 +137,8 @@ def run(stepper, t_final, dt, adaptive=True, dt_min=1e-5, dt_max=np.inf, beta_up
     log = []
     while time < t_final:
         stepper.backup()
+        if hasattr(stepper, "dynamic_instability"):  # (distributed.RankStepper and other steppers have no model)
+            stepper.dynamic_instability(dt)
         f_ext, ft = forces(time, stepper.positions()) if forces is not None else (None, None)
         info = stepper.step(dt, f_external=f_ext, body_forces_torques=ft)
         converged, err = bool(info["converged"]), info["fiber_error"]
