@@ -183,10 +183,8 @@ def library() -> C.CDLL:
         "skb_flow_set_target_window": ([ctxp, C.c_int64, C.c_int64], C.c_int),
         "skb_flow_set_self_exclusion": ([ctxp, C.c_int], C.c_int),
         "skb_flow_set_overlap": ([ctxp, C.c_int], C.c_int),
-        "skb_mflow_set_overlap": ([ctxp, C.c_int], C.c_int),
         "skb_dense_apply_background_device": ([ctxp, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p], C.c_int),
         "skb_flow_set_cross": ([ctxp, C.c_int], C.c_int),
-        "skb_mflow_set_cross": ([ctxp, C.c_int], C.c_int),
         "skb_flow_group_init": ([ctxp, C.c_int, C.c_int], C.c_int),
         "skb_flow_group_export": ([ctxp, C.c_void_p], C.c_int),
         "skb_flow_group_import": ([ctxp, C.c_int, C.c_void_p], C.c_int),
@@ -198,28 +196,12 @@ def library() -> C.CDLL:
         "skb_partition_query": ([C.POINTER(C.c_int), C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_int,
                                  C.POINTER(C.c_int64)], C.c_int),
         "skb_mflow_create": ([C.POINTER(C.c_int), C.c_int, C.POINTER(ctxp)], C.c_int),
-        "skb_mflow_destroy": ([ctxp], C.c_int),
         "skb_mflow_n_devices": ([ctxp, C.POINTER(C.c_int)], C.c_int),
-        "skb_mflow_set_fibers": ([ctxp, _dp, C.POINTER(C.c_int), _dp, C.c_int], C.c_int),
-        "skb_mflow_set_periphery": ([ctxp, _dp, _dp, C.c_int64], C.c_int),
-        "skb_mflow_set_bodies": ([ctxp, _dp, _dp, C.c_int64, _dp, C.c_int], C.c_int),
-        "skb_mflow_set_self_exclusion": ([ctxp, C.c_int], C.c_int),
         "skb_mflow_partition": ([ctxp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)] + [C.POINTER(C.c_int64)] * 4,
                                 C.c_int),
-        "skb_mflow_set_fiber_class": ([ctxp, C.c_int, _dp, _dp], C.c_int),
-        "skb_mflow_set_fiber_operators": ([ctxp, _dp, _dp, _dp, _dp, C.POINTER(C.c_int)], C.c_int),
-        "skb_mflow_set_fiber_preconditioner": ([ctxp, _dp], C.c_int),
-        "skb_mflow_set_fiber_class_derivatives": ([ctxp, C.c_int, _dp, _dp, _dp], C.c_int),
-        "skb_mflow_build_fiber_operators": ([ctxp, C.POINTER(FiberParams), C.c_double, C.c_double], C.c_int),
         "skb_mflow_set_dense": ([ctxp, C.c_int, _dp, C.c_int64, C.c_int64], C.c_int),
-        "skb_mflow_matvec": ([ctxp, _dp, _dp, _dp, _dp, C.c_double, _dp], C.c_int),
-        "skb_mflow_apply_matvec": ([ctxp, _dp, _dp, _dp, _dp, _dp, C.c_double, _dp, _dp, _dp], C.c_int),
-        "skb_mflow_set_body_operators": ([ctxp, C.POINTER(C.c_int), C.c_int, _dp, _dp, _dp, _dp, _dp], C.c_int),
-        "skb_mflow_set_fiber_links": ([ctxp, C.POINTER(C.c_int), _dp, _dp], C.c_int),
         "skb_mflow_apply_system_matvec": ([ctxp, _dp, C.c_double, _dp], C.c_int),
         "skb_mflow_apply_system_preconditioner": ([ctxp, _dp, _dp], C.c_int),
-        "skb_mflow_velocity_at_targets": ([ctxp, _dp, C.c_int64, _dp, _dp, _dp, _dp, C.c_double, _dp], C.c_int),
-        "skb_mflow_last_stats": ([ctxp, C.POINTER(FlowStats)], C.c_int),
         "skb_flow_set_target_ranges": ([ctxp, C.c_int, C.c_int] + [C.c_int64] * 4, C.c_int),
         "skb_flow_apply_fiber_force_device": ([ctxp, C.c_void_p, C.c_void_p, C.c_void_p], C.c_int),
         "skb_flow_fiber_matvec_device": ([ctxp] + [C.c_void_p] * 5, C.c_int),
@@ -237,8 +219,6 @@ def library() -> C.CDLL:
                                      C.c_int),
         "skb_flow_build_fiber_rhs_device": ([ctxp, C.POINTER(FiberParams), _dp, _dp, C.c_void_p, C.c_void_p,
                                              C.c_double, C.c_double, C.c_void_p, C.c_void_p], C.c_int),
-        "skb_mflow_build_fiber_rhs": ([ctxp, C.POINTER(FiberParams), _dp, _dp, _dp, _dp, C.c_double, C.c_double, _dp],
-                                      C.c_int),
         "skb_flow_apply_matvec": ([ctxp, _dp, _dp, _dp, _dp, _dp, C.c_double, _dp, _dp, _dp], C.c_int),
         "skb_flow_apply_matvec_dense": ([ctxp, ctxp, _dp, _dp, _dp, _dp, _dp, C.c_double, _dp, _dp, _dp], C.c_int),
         "skb_dense_apply_device": ([ctxp, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p], C.c_int),
@@ -262,27 +242,11 @@ def library() -> C.CDLL:
                                       C.c_int),
         "skb_flow_build_system_rhs_device": ([ctxp, C.POINTER(FiberParams), _dp, _dp] + [C.c_void_p] * 3
                                              + [C.c_double, C.c_double, C.c_void_p, C.c_void_p], C.c_int),
-        "skb_mflow_build_system_rhs": ([ctxp, C.POINTER(FiberParams), _dp, _dp, _dp, _dp, C.c_double, C.c_double, _dp],
-                                       C.c_int),
-        "skb_flow_group_set_body_operators": ([ctxp, C.POINTER(C.c_int), C.c_int, _dp, _dp, _dp, _dp, _dp], C.c_int),
-        "skb_flow_group_set_fiber_links": ([ctxp, C.POINTER(C.c_int), _dp, _dp], C.c_int),
-        "skb_flow_group_apply_system_matvec_device": ([ctxp, ctxp, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p],
-                                                      C.c_int),
-        "skb_flow_group_apply_system_preconditioner_device": ([ctxp, ctxp, C.c_void_p, C.c_void_p, C.c_void_p],
-                                                              C.c_int),
-        "skb_flow_group_build_system_rhs_device": ([ctxp, C.POINTER(FiberParams), _dp, _dp] + [C.c_void_p] * 3
-                                                   + [C.c_double, C.c_double, C.c_void_p, C.c_void_p], C.c_int),
         "skb_group_body_pieces": ([C.POINTER(C.c_int), C.c_int, C.c_int64, C.c_int64, C.POINTER(C.c_int64), C.c_int,
                                    C.POINTER(C.c_int)], C.c_int),
         "skb_flow_set_body_frames": ([ctxp, C.POINTER(C.c_int), C.c_int] + [_dp] * 7, C.c_int),
         "skb_flow_place_bodies": ([ctxp, _dp, _dp], C.c_int),
         "skb_flow_get_body_operators": ([ctxp, _dp, _dp, _dp, _dp], C.c_int),
-        "skb_flow_group_set_body_frames": ([ctxp, C.POINTER(C.c_int), C.c_int] + [_dp] * 7, C.c_int),
-        "skb_flow_group_place_bodies": ([ctxp, _dp, _dp], C.c_int),
-        "skb_mflow_set_body_frames": ([ctxp, C.POINTER(C.c_int), C.c_int] + [_dp] * 7, C.c_int),
-        "skb_mflow_place_bodies": ([ctxp, _dp, _dp], C.c_int),
-        "skb_mflow_set_point_sources": ([ctxp, _dp, _dp, _dp, C.c_int], C.c_int),
-        "skb_mflow_set_background": ([ctxp, C.POINTER(C.c_int), _dp, _dp], C.c_int),
         "skb_flow_set_gmres": ([ctxp, C.c_int], C.c_int),
         "skb_flow_solve_system": ([ctxp, ctxp, _dp, C.c_double, C.c_double, C.c_int, C.c_int, _dp,
                                    C.POINTER(SolveInfo), _dp], C.c_int),
@@ -290,7 +254,6 @@ def library() -> C.CDLL:
                                           C.c_void_p, C.POINTER(SolveInfo), _dp, C.c_void_p], C.c_int),
         "skb_flow_group_solve_system_device": ([ctxp, ctxp, ctxp, C.c_void_p, C.c_double, C.c_double, C.c_int, C.c_int,
                                                 C.c_void_p, C.POINTER(SolveInfo), _dp, C.c_void_p], C.c_int),
-        "skb_mflow_set_gmres": ([ctxp, C.c_int], C.c_int),
         "skb_flow_step": ([ctxp, ctxp, C.POINTER(FiberParams), _dp, _dp, _dp, _dp, C.POINTER(C.c_int), _dp, C.c_double,
                            C.c_double, C.c_double, C.c_int, C.c_int, _dp, _dp, C.POINTER(StepInfo)], C.c_int),
         "skb_flow_fiber_error": ([ctxp, _dp, _dp], C.c_int),
@@ -301,12 +264,8 @@ def library() -> C.CDLL:
         "skb_flow_group_step_device": ([ctxp, ctxp, ctxp, C.POINTER(FiberParams), _dp, _dp] + [C.c_void_p] * 3
                                        + [C.POINTER(C.c_int), _dp, C.c_double, C.c_double, C.c_double, C.c_int,
                                           C.c_int, C.c_void_p, C.c_void_p, C.POINTER(StepInfo), C.c_void_p], C.c_int),
-        "skb_mflow_get_fibers": ([ctxp, _dp], C.c_int),
         "skb_flow_set_periphery_shape": ([ctxp, C.POINTER(PeripheryShape), C.POINTER(C.c_int32), _dp], C.c_int),
         "skb_flow_periphery_interaction": ([ctxp, _dp, C.POINTER(C.c_int32), C.POINTER(C.c_int32)], C.c_int),
-        "skb_mflow_set_periphery_shape": ([ctxp, C.POINTER(PeripheryShape), C.POINTER(C.c_int32), _dp], C.c_int),
-        "skb_mflow_periphery_interaction": ([ctxp, _dp, C.POINTER(C.c_int32), C.POINTER(C.c_int32)], C.c_int),
-        "skb_mflow_get_placement": ([ctxp, _dp, _dp], C.c_int),
         "skb_flow_set_nucleation_sites": ([ctxp, C.POINTER(C.c_int), _dp], C.c_int),
         "skb_flow_dynamic_instability": ([ctxp, C.POINTER(DynamicInstability), C.c_double, C.c_uint64, C.c_uint64,
                                           C.c_int, C.POINTER(FiberParams), C.POINTER(C.c_int32),
@@ -317,6 +276,17 @@ def library() -> C.CDLL:
         "skb_mflow_solve_system": ([ctxp, _dp, C.c_double, C.c_double, C.c_int, C.c_int, _dp, C.POINTER(SolveInfo),
                                     _dp], C.c_int),
     }
+    # the skb_mflow_ and skb_flow_group_ calls whose arguments are those of their skb_flow_ twin
+    for name in ("destroy", "set_fibers", "set_periphery", "set_bodies", "set_self_exclusion", "set_cross",
+                 "set_overlap", "set_fiber_class", "set_fiber_class_derivatives", "set_fiber_operators",
+                 "set_fiber_preconditioner", "build_fiber_operators", "build_fiber_rhs", "matvec", "apply_matvec",
+                 "velocity_at_targets", "set_point_sources", "set_background", "set_body_operators", "set_body_frames",
+                 "place_bodies", "set_fiber_links", "set_periphery_shape", "periphery_interaction", "build_system_rhs",
+                 "set_gmres", "get_fibers", "get_placement", "last_stats"):
+        sig["skb_mflow_" + name] = sig["skb_flow_" + name]
+    for name in ("set_body_operators", "set_body_frames", "place_bodies", "set_fiber_links",
+                 "apply_system_matvec_device", "apply_system_preconditioner_device", "build_system_rhs_device"):
+        sig["skb_flow_group_" + name] = sig["skb_flow_" + name]
     global BOUND_FUNCTIONS
     BOUND_FUNCTIONS = tuple(sorted(sig))
     for name, (args, res) in sig.items():
@@ -384,23 +354,51 @@ def _opt_p(x):
     return None if x is None else _p(x)
 
 
-def _frame_arrays(n_nodes, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0, A_inv0_list):
-    """the arrays of skb_flow_set_body_frames (A_inv0 column-major and concatenated, or None)"""
+def _vp(a):
+    """a device address (an int, e.g. torch.Tensor.data_ptr()) as a void pointer; 0 is NULL"""
+    return C.c_void_p(a) if a else None
+
+
+def _dense_h(dense):
+    """the handle of a Dense, or NULL for None"""
+    return dense._h if dense is not None else None
+
+
+# The body and fiber-link set-up of a flow through its C call `name`: the plain call, or on a Flow its group_ twin,
+# which takes the same arguments.
+def _body_operators_call(fl, name, n_nodes, node_weights, ex, ey, ez, A_inv_list):
     n = np.ascontiguousarray(n_nodes, dtype=np.int32)
     w = np.ascontiguousarray(node_weights, dtype=np.float64).reshape(-1)
-    Ai = None if A_inv0_list is None else Flow._colmajor_concat(A_inv0_list)
-    return (n, _arr(node_pos_ref, 3), _arr(node_normal_ref, 3), w, _arr(ex0, 3), _arr(ey0, 3), _arr(ez0, 3), Ai)
+    ex, ey, ez = _arr(ex, 3), _arr(ey, 3), _arr(ez, 3)
+    Ai = None if A_inv_list is None else fl._colmajor_concat(A_inv_list)
+    fl._call(name, n.ctypes.data_as(C.POINTER(C.c_int)), int(n.shape[0]), _p(w), _p(ex), _p(ey), _p(ez), _opt_p(Ai))
+    fl._body_sol, fl._body_n = int(np.sum(3 * n + 6)), n
 
 
-def _frame_call(fn, h, arrays):
-    n, *rest, Ai = arrays
-    _check(fn(h, n.ctypes.data_as(C.POINTER(C.c_int)), int(n.shape[0]), *(_p(a) for a in rest), _opt_p(Ai)))
+def _frame_call(fl, name, n_nodes, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0, A_inv0_list):
+    n = np.ascontiguousarray(n_nodes, dtype=np.int32)
+    w = np.ascontiguousarray(node_weights, dtype=np.float64).reshape(-1)
+    Ai = None if A_inv0_list is None else fl._colmajor_concat(A_inv0_list)
+    rest = (_arr(node_pos_ref, 3), _arr(node_normal_ref, 3), w, _arr(ex0, 3), _arr(ey0, 3), _arr(ez0, 3))
+    fl._call(name, n.ctypes.data_as(C.POINTER(C.c_int)), int(n.shape[0]), *(_p(a) for a in rest), _opt_p(Ai))
+    fl._body_sol, fl._body_n = int(np.sum(3 * n + 6)), n
 
 
-def _place_call(fn, h, centers, orientations):
+def _place_call(fl, name, centers, orientations):
     c, q = _arr(centers, 3), _arr(orientations, 4)
     assert c.shape[0] == q.shape[0]
-    _check(fn(h, _p(c), _p(q)))
+    fl._call(name, _p(c), _p(q))
+
+
+def _links_call(fl, name, body, site, bending_rigidity):
+    if body is None:
+        fl._call(name, None, None, None)
+        return
+    b = np.ascontiguousarray(body, dtype=np.int32)
+    st = _arr(site, 3)
+    E = np.ascontiguousarray(np.broadcast_to(np.asarray(bending_rigidity, dtype=np.float64), b.shape))
+    assert st.shape[0] == b.shape[0]
+    fl._call(name, b.ctypes.data_as(C.POINTER(C.c_int)), _p(st), _p(E))
 
 
 def _fiber_rhs_args(n_fibers, n_nodes, params, v_growth, force_scale, v_on_fibers, f_external):
@@ -423,53 +421,12 @@ def _system_rhs_args(n_fibers, n_nodes, n_bodies, params, v_growth, force_scale,
     return p, vg, fs, f, ft
 
 
-def _step_call(fl, call, n_fibers, params, dt, eta, f_external, body_forces_torques, fiber_body, site_ref, v_growth,
-               force_scale, tol, num_blocks, max_iters):
-    """the arguments of skb_flow_step / skb_mflow_step after the handles; returns (x, tension, info dict).  SKB_ERR_STATE
-    with a NaN fiber_error is the step that was not installed; anything else non-zero raises"""
-    p, vg, fs, f, ft = _system_rhs_args(n_fibers, fl.n_fib, fl.n_bodies, params, v_growth, force_scale, f_external,
-                                        body_forces_torques)
-    fb = None if fiber_body is None else np.ascontiguousarray(fiber_body, dtype=np.int32).reshape(-1)
-    if fb is not None and fb.shape[0] != n_fibers:
-        raise ValueError(f"expected {n_fibers} fiber_body entries, got {fb.shape[0]}")
-    sr = None if site_ref is None else _arr(site_ref, 3)
-    x = np.empty(fl.solution_size())
-    tension = np.empty(fl.n_fib)
-    info = StepInfo()
-    rc = call(_params_ptr(p), _opt_p(vg), _opt_p(fs), _opt_p(f), _opt_p(ft),
-              None if fb is None else fb.ctypes.data_as(C.POINTER(C.c_int)), _opt_p(sr), float(dt), float(eta),
-              float(tol), int(num_blocks), int(max_iters), _p(x), _p(tension), C.byref(info))
-    if not (rc == ERR_STATE and np.isnan(info.fiber_error)):
-        _check(rc)
-    return x, tension, info.as_dict()
-
-
-def _shape_call(fn, h, n_fibers, n_bodies, kind, a, b, c, f_0, l_0, binding_active, polar_angle_start,
-                polar_angle_end, binding_threshold, fiber_minus_clamped, body_radius):
-    s = PeripheryShape(int(kind), int(binding_active), float(a), float(b), float(c), float(f_0), float(l_0),
-                       float(polar_angle_start), float(polar_angle_end), float(binding_threshold))
-    mc = None if fiber_minus_clamped is None else np.ascontiguousarray(fiber_minus_clamped, dtype=np.int32)
-    if mc is not None and mc.shape != (n_fibers,):
-        raise ValueError(f"expected {n_fibers} fiber_minus_clamped flags, got {mc.shape}")
-    br = None if body_radius is None else np.ascontiguousarray(body_radius, dtype=np.float64)
-    if br is not None and br.shape != (n_bodies,):
-        raise ValueError(f"expected {n_bodies} body radii, got {br.shape}")
-    _check(fn(h, C.byref(s), None if mc is None else mc.ctypes.data_as(C.POINTER(C.c_int32)), _opt_p(br)))
-
-
-def _interaction_call(fn, h, n_nodes, n_fibers):
+def _interaction_call(fl, n_nodes, n_fibers):
     f = np.empty((n_nodes, 3))
     hinged = np.empty(n_fibers, dtype=np.int32)
     collided = C.c_int32(0)
-    _check(fn(h, _p(f), hinged.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(collided)))
+    fl._call("periphery_interaction", _p(f), hinged.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(collided))
     return f, hinged, bool(collided.value)
-
-
-_SHAPE_DOC = """The periphery's shape for the step (skb_flow_set_periphery_shape): kind PERIPHERY_SPHERE (radius a),
-        PERIPHERY_ELLIPSOID (semi-axes a, b, c) or PERIPHERY_NONE (clears it); fiber_periphery_interaction f_0, l_0;
-        periphery_binding active, polar angles and threshold; per fiber the TOML flag minus_clamped_ (None: all 0);
-        per body the radius of a spherical body (0: not spherical; None: no body takes part).  The step then adds the
-        repulsion to f_external, takes plus_hinged from the binding and reports the collision test in info["collided"]."""
 
 
 def device_count() -> int:
@@ -507,23 +464,14 @@ def stresslet_direct(r_src, f_src, r_trg):
     return u
 
 
-class Context:
-    """Evaluator context: positions cached on the device(s), strengths shipped per evaluation."""
-
-    def __init__(self, n_gpus: int = 1, device_ids=None):
-        self._h = C.c_void_p()
-        L = library()
-        if device_ids is None:
-            _check(L.skb_ctx_create(int(n_gpus), C.byref(self._h)))
-        else:
-            ids = (C.c_int * len(device_ids))(*device_ids)
-            _check(L.skb_ctx_create_on(ids, len(device_ids), C.byref(self._h)))
-        self.n_trg = 0
-        self.n_src = {KERNEL_STOKESLET: 0, KERNEL_STRESSLET: 0}
+class _Handle:
+    """The lifetime of a library handle self._h: close() (or the end of a with block, or garbage collection) releases
+    it once through the C function named _destroy; closing again does nothing."""
+    _destroy = None
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
-            library().skb_ctx_destroy(self._h)
+            getattr(library(), self._destroy)(self._h)
             self._h = C.c_void_p()
 
     def __del__(self):
@@ -537,6 +485,22 @@ class Context:
 
     def __exit__(self, *a):
         self.close()
+
+
+class Context(_Handle):
+    """Evaluator context: positions cached on the device(s), strengths shipped per evaluation."""
+    _destroy = "skb_ctx_destroy"
+
+    def __init__(self, n_gpus: int = 1, device_ids=None):
+        self._h = C.c_void_p()
+        L = library()
+        if device_ids is None:
+            _check(L.skb_ctx_create(int(n_gpus), C.byref(self._h)))
+        else:
+            ids = (C.c_int * len(device_ids))(*device_ids)
+            _check(L.skb_ctx_create_on(ids, len(device_ids), C.byref(self._h)))
+        self.n_trg = 0
+        self.n_src = {KERNEL_STOKESLET: 0, KERNEL_STRESSLET: 0}
 
     @property
     def n_gpus(self) -> int:
@@ -645,53 +609,282 @@ class Context:
         return v.value
 
 
-class Flow:
-    """Device-resident flow() layer (include/skelly_b200_flow.h): FiberContainer / Periphery / BodyContainer flows
-    and the fused hydrodynamic part of System::apply_matvec."""
+class _FlowBase(_Handle):
+    """What Flow and MultiFlow share: every call whose C twins (skb_flow_* and skb_mflow_*) take the same arguments
+    after the handle.  A subclass names its C prefix, and its _own_fibers() / _pieces() give the fibers and rows the
+    calls cover: a Flow's own window or ranges, all of them on a MultiFlow."""
+    _prefix = None
+    _step_takes_dense = False  # skb_flow_step takes the Dense handle after the flow's; skb_mflow_step does not
 
-    def __init__(self, device: int = 0):
-        self._h = C.c_void_p()
-        _check(library().skb_flow_create(int(device), C.byref(self._h)))
-        self.n_fib = self.n_shell = self.n_body = self.n_bodies = 0
+    def _fn(self, name):
+        return getattr(library(), self._prefix + name)
 
-    def close(self):
-        if getattr(self, "_h", None) and self._h.value:
-            library().skb_flow_destroy(self._h)
-            self._h = C.c_void_p()
+    def _call(self, name, *args):
+        _check(self._fn(name)(self._h, *args))
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *a):
-        self.close()
+    def _n_fibers(self):
+        return len(getattr(self, "_fiber_off", [0])) - 1
 
     def set_fibers(self, r_fib, n_nodes, lengths):
         r_fib = _arr(r_fib, 3)
         n_nodes = np.ascontiguousarray(n_nodes, dtype=np.int32)
         lengths = np.ascontiguousarray(lengths, dtype=np.float64)
         assert n_nodes.shape == lengths.shape and int(n_nodes.sum()) == r_fib.shape[0]
-        _check(library().skb_flow_set_fibers(self._h, _p(r_fib), n_nodes.ctypes.data_as(C.POINTER(C.c_int)),
-                                             _p(lengths), int(n_nodes.shape[0])))
+        self._call("set_fibers", _p(r_fib), n_nodes.ctypes.data_as(C.POINTER(C.c_int)), _p(lengths),
+                   int(n_nodes.shape[0]))
         self.n_fib = r_fib.shape[0]
         self._fiber_off = np.concatenate([[0], np.cumsum(n_nodes, dtype=np.int64)])
         self._lengths = lengths.copy()
 
     def set_periphery(self, node_pos, node_normal):
         node_pos, node_normal = _arr(node_pos, 3), _arr(node_normal, 3)
-        _check(library().skb_flow_set_periphery(self._h, _p(node_pos), _p(node_normal), node_pos.shape[0]))
+        self._call("set_periphery", _p(node_pos), _p(node_normal), node_pos.shape[0])
         self.n_shell = node_pos.shape[0]
 
     def set_bodies(self, node_pos, node_normal, centers):
         node_pos, node_normal, centers = _arr(node_pos, 3), _arr(node_normal, 3), _arr(centers, 3)
-        _check(library().skb_flow_set_bodies(self._h, _p(node_pos), _p(node_normal), node_pos.shape[0], _p(centers),
-                                             centers.shape[0]))
+        self._call("set_bodies", _p(node_pos), _p(node_normal), node_pos.shape[0], _p(centers), centers.shape[0])
         self.n_body, self.n_bodies = node_pos.shape[0], centers.shape[0]
+
+    def set_point_sources(self, positions, forces, torques):
+        """The point sources (velocity_at_targets and build_system_rhs include them)."""
+        positions, forces, torques = _arr(positions, 3), _arr(forces, 3), _arr(torques, 3)
+        self._call("set_point_sources", _p(positions), _p(forces), _p(torques), positions.shape[0])
+
+    def set_background(self, components, scale_factor, uniform):
+        comp = (C.c_int * 3)(*[int(c) for c in components])
+        sc = np.ascontiguousarray(scale_factor, dtype=np.float64)
+        un = np.ascontiguousarray(uniform, dtype=np.float64)
+        self._call("set_background", comp, _p(sc), _p(un))
+
+    def velocity_at_targets(self, r_trg, fib_forces, shell_density, body_densities, body_forces_torques, eta):
+        """System::velocity_at_targets (system.cpp:355-359): fiber (no self subtraction) + body + periphery flows."""
+        r_trg = _arr(r_trg, 3)
+        a, b, c = _arr(fib_forces, 3), _arr(shell_density, 3), _arr(body_densities, 3)
+        ft = _arr(body_forces_torques, 6)
+        vel = np.empty((r_trg.shape[0], 3))
+        self._call("velocity_at_targets", _p(r_trg), r_trg.shape[0], _p(a), _p(b), _p(c), _p(ft), float(eta), _p(vel))
+        return vel
+
+    def set_cross(self, mode: int):
+        """Fiber <-> periphery pairs of the matvec in one geometry pass: -1 auto (default), 0 never, 1 whenever applicable."""
+        self._call("set_cross", int(mode))
+
+    def set_self_exclusion(self, fused: bool):
+        """Matvec self term: False = the reference's compute-then-subtract (default); True = the pair kernels skip
+        intra-fiber pairs (SURVEY.md 8f N3)."""
+        self._call("set_self_exclusion", int(bool(fused)))
+
+    def set_overlap(self, on: bool):
+        """Periphery dense operator beside the pair kernels on a side stream (default) or as one kernel at the end."""
+        self._call("set_overlap", int(bool(on)))
+
+    def matvec(self, fib_forces, shell_density, body_densities, body_forces_torques, eta):
+        a, b, c = _arr(fib_forces, 3), _arr(shell_density, 3), _arr(body_densities, 3)
+        ft = _arr(body_forces_torques, 6)
+        v = np.empty((sum(self._pieces()), 3))
+        self._call("matvec", _p(a), _p(b), _p(c), _p(ft), float(eta), _p(v))
+        return v
+
+    # ---- per-fiber dense operators (SURVEY.md §8f N2); matrices go in column-major like Eigen's .data() ----
+    def set_fiber_class(self, n_nodes: int, D_1_0, P_downsample_bc):
+        """FiberFiniteDifference::matrices_.at(n): D_1_0 (n,n), P_downsample_bc (4n-14,4n)."""
+        n = int(n_nodes)
+        D = np.asfortranarray(D_1_0, dtype=np.float64)
+        P = np.asfortranarray(P_downsample_bc, dtype=np.float64)
+        if D.shape != (n, n) or P.shape != (4 * n - 14, 4 * n):
+            raise ValueError(f"class matrices for n={n}: got {D.shape}, {P.shape}")
+        self._call("set_fiber_class", n, _p(D), _p(P))
+
+    @staticmethod
+    def _colmajor_concat(mats):
+        """Per-fiber matrices -> one buffer, every matrix column-major (Eigen's .data()).  A 3-D C-ordered stack of
+        equal shapes is transposed in one pass; a list may be ragged."""
+        if isinstance(mats, np.ndarray) and mats.ndim == 3:
+            return np.ascontiguousarray(np.asarray(mats, dtype=np.float64).transpose(0, 2, 1)).reshape(-1)
+        if len(mats) == 0:
+            return np.zeros(0)
+        return np.concatenate([np.asarray(m, dtype=np.float64).ravel(order="F") for m in mats])
+
+    def set_fiber_preconditioner(self, A_inv_list):
+        """Explicit inverses of A_ (fib.A_LU_.inverse()), same fibers and order as set_fiber_operators."""
+        Ai = self._colmajor_concat(A_inv_list)
+        self._call("set_fiber_preconditioner", _p(Ai))
+
+    def set_fiber_class_derivatives(self, n_nodes: int, D_2_0, D_3_0, D_4_0):
+        """The higher derivative matrices of FiberFiniteDifference::matrices_.at(n) (pre-transposed like D_1_0), needed
+        by build_fiber_operators for every node count in use."""
+        n, (D2, D3, D4) = _class_derivatives(n_nodes, D_2_0, D_3_0, D_4_0)
+        self._call("set_fiber_class_derivatives", n, _p(D2), _p(D3), _p(D4))
+
+    def build_fiber_operators(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
+                              plus_hinged, dt, eta):
+        """A_, force_operator_, xs_ and A_^-1 of the (own) fibers built on the device from the positions and lengths of
+        set_fibers (update_derivatives, update_linear_operator, update_force_operator, the operator half of
+        apply_bc_rectangular, update_preconditioner).  Per-fiber arrays or scalars; the flags are 0 / 1.  A MultiFlow
+        takes them for all fibers, and every device builds its own slice."""
+        f0, f1 = self._own_fibers()
+        p = fiber_params(f1 - f0, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
+                         plus_hinged)
+        self._call("build_fiber_operators", _params_ptr(p), float(dt), float(eta))
+
+    def build_fiber_rhs(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
+                        plus_hinged, dt, eta, v_on_fibers=None, f_external=None, v_growth=None, force_scale=None):
+        """The fiber block of the RHS (4 N_own,) as System::prep_state_for_solver leaves it: update_RHS with f_external
+        + force_scale xs_, then the RHS half of apply_bc_rectangular with f_external.  Parameters as for
+        build_fiber_operators; v_on_fibers / f_external (N_own, 3) and v_growth / force_scale (per-fiber arrays or
+        scalars) may be None: no flow / force, zero growth, no motors."""
+        f0, f1 = self._own_fibers()
+        n_own = self._pieces()[0]
+        p, vg, fs, v, f = _fiber_rhs_args(f1 - f0, n_own, (length_prev, bending_rigidity, radius, penalty_param,
+                                                           beta_tstep, minus_clamped, plus_hinged),
+                                          v_growth, force_scale, v_on_fibers, f_external)
+        rhs = np.empty(4 * n_own)
+        self._call("build_fiber_rhs", _params_ptr(p), _opt_p(vg), _opt_p(fs), _opt_p(v), _opt_p(f), float(dt),
+                   float(eta), _p(rhs))
+        return rhs
+
+    # ---- the whole solution vector [fibers | shell | bodies] with the bodies on the device ----
+    def set_body_operators(self, n_nodes, node_weights, ex, ey, ez, A_inv_list=None):
+        """Per body (order of set_bodies = order in the solution vector): node count, node_weights_ (N_b,), ex_ / ey_ /
+        ez_ (N_b, 3) each, and A_^-1 ((3n+6, 3n+6) per body, a list) or None (no system preconditioner for bodies).
+        On a MultiFlow every device keeps the bodies it owns rows of."""
+        _body_operators_call(self, "set_body_operators", n_nodes, node_weights, ex, ey, ez, A_inv_list)
+
+    def set_body_frames(self, n_nodes, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0, A_inv0_list=None):
+        """The bodies' operators in their body frame, once per run after set_bodies: per body its node count, per node
+        node_positions_ref_ / node_normals_ref_ (N_b, 3) and node_weights_ (N_b,), ex_ / ey_ / ez_ (N_b, 3) and
+        A_^-1 ((3n+6, 3n+6) per body, a list, or None) of the body at identity orientation.  place_bodies then forms
+        the placed operators on the device.  On a MultiFlow every device keeps the body-frame inverses it owns rows
+        of."""
+        _frame_call(self, "set_body_frames", n_nodes, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0,
+                    A_inv0_list)
+
+    def place_bodies(self, centers, orientations):
+        """Once per timestep: the bodies at centres (n_bodies, 3) and unit quaternions (w, x, y, z) (n_bodies, 4) --
+        their nodes, normals and operators, as set_bodies + set_body_operators with the placed ones would leave them.
+        The fiber links are dropped."""
+        _place_call(self, "place_bodies", centers, orientations)
+
+    def set_fiber_links(self, body=None, site=None, bending_rigidity=None):
+        """Per fiber: body index (-1 free), lab-frame nucleation site (n_fibers, 3), bending_rigidity_; body=None: no
+        fiber is bound."""
+        _links_call(self, "set_fiber_links", body, site, bending_rigidity)
+
+    def solution_size(self) -> int:
+        """4 N_f + 3 N_s + sum(3 n_b + 6) (the bodies' part as set_body_operators was last given)"""
+        return 4 * self.n_fib + 3 * self.n_shell + (getattr(self, "_body_sol", 0) if self.n_bodies else 0)
+
+    def build_system_rhs(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
+                         plus_hinged, dt, eta, f_external=None, body_forces_torques=None, v_growth=None,
+                         force_scale=None):
+        """System::prep_state_for_solver's RHS (system.cpp:398-458) as a whole solution vector (solution_size(),):
+        the flow of f_external (N_f, 3) and of the bodies' external forces / torques (n_bodies, 6), plus the point
+        sources and the background flow, into the fiber block (build_fiber_rhs's parameters), -v_shell and
+        [-v_body ; 0] per body.  f_external / body_forces_torques None: zero."""
+        f0, f1 = self._own_fibers()
+        p, vg, fs, f, ft = _system_rhs_args(f1 - f0, self.n_fib, self.n_bodies,
+                                            (length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
+                                             minus_clamped, plus_hinged), v_growth, force_scale, f_external,
+                                            body_forces_torques)
+        rhs = np.empty(self.solution_size())
+        self._call("build_system_rhs", _params_ptr(p), _opt_p(vg), _opt_p(fs), _opt_p(f), _opt_p(ft), float(dt),
+                   float(eta), _p(rhs))
+        return rhs
+
+    def set_gmres(self, num_blocks: int = 300):
+        """Size the workspace of solve_system for the current solution size and up to num_blocks basis vectors (after
+        set_body_operators; a MultiFlow also lays out every member's local rows)."""
+        self._call("set_gmres", int(num_blocks))
+        self._gmres_blocks = int(num_blocks)
+
+    def set_periphery_shape(self, kind, a, b=0.0, c=0.0, f_0=20.0, l_0=0.05, binding_active=False,
+                            polar_angle_start=0.0, polar_angle_end=np.pi, binding_threshold=0.75,
+                            fiber_minus_clamped=None, body_radius=None):
+        """The periphery's shape for the step (skb_flow_set_periphery_shape): kind PERIPHERY_SPHERE (radius a),
+        PERIPHERY_ELLIPSOID (semi-axes a, b, c) or PERIPHERY_NONE (clears it); fiber_periphery_interaction f_0, l_0;
+        periphery_binding active, polar angles and threshold; per fiber the TOML flag minus_clamped_ (None: all 0);
+        per body the radius of a spherical body (0: not spherical; None: no body takes part).  The step then adds the
+        repulsion to f_external, takes plus_hinged from the binding and reports the collision test in info["collided"]."""
+        n_fibers = self._n_fibers()
+        s = PeripheryShape(int(kind), int(binding_active), float(a), float(b), float(c), float(f_0), float(l_0),
+                           float(polar_angle_start), float(polar_angle_end), float(binding_threshold))
+        mc = None if fiber_minus_clamped is None else np.ascontiguousarray(fiber_minus_clamped, dtype=np.int32)
+        if mc is not None and mc.shape != (n_fibers,):
+            raise ValueError(f"expected {n_fibers} fiber_minus_clamped flags, got {mc.shape}")
+        br = None if body_radius is None else np.ascontiguousarray(body_radius, dtype=np.float64)
+        if br is not None and br.shape != (self.n_bodies,):
+            raise ValueError(f"expected {self.n_bodies} body radii, got {br.shape}")
+        self._call("set_periphery_shape", C.byref(s), None if mc is None else mc.ctypes.data_as(C.POINTER(C.c_int32)),
+                   _opt_p(br))
+        # kept so that the shape can be set again for another fiber set (timestep.Stepper.restore)
+        self._shape = dict(kind=kind, a=a, b=b, c=c, f_0=f_0, l_0=l_0, binding_active=binding_active,
+                           polar_angle_start=polar_angle_start, polar_angle_end=polar_angle_end,
+                           binding_threshold=binding_threshold, body_radius=body_radius,
+                           fiber_minus_clamped=np.zeros(n_fibers, dtype=np.int32)
+                           if fiber_minus_clamped is None else np.array(fiber_minus_clamped, dtype=np.int32))
+
+    def step(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped, plus_hinged, dt,
+             eta, dense=None, f_external=None, body_forces_torques=None, fiber_body=None, site_ref=None,
+             v_growth=None, force_scale=None, tol=1e-10, num_blocks=300, max_iters=1000):
+        """System::step (system.cpp:482-492) on the device: links, fiber operators, RHS and solve at the current
+        geometry, then the fibers' and bodies' step and the new geometry installed.  fiber_body (N_fibers,) ints, -1
+        free, or None; site_ref (N_fibers, 3) body-frame nucleation sites, or None.  Returns (x, tension, info): info
+        a dict of skb_step_info (the solve's fields, fiber_error, worst_fiber, collided).  A solution with non-finite
+        new positions installs nothing and returns fiber_error NaN.  With set_periphery_shape, plus_hinged is ignored
+        (the binding sets it) and the repulsion is added to f_external.  A MultiFlow does not use dense: the
+        periphery's operators come from set_dense."""
+        n_fibers = self._n_fibers()
+        p, vg, fs, f, ft = _system_rhs_args(n_fibers, self.n_fib, self.n_bodies,
+                                            (length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
+                                             minus_clamped, plus_hinged), v_growth, force_scale, f_external,
+                                            body_forces_torques)
+        fb = None if fiber_body is None else np.ascontiguousarray(fiber_body, dtype=np.int32).reshape(-1)
+        if fb is not None and fb.shape[0] != n_fibers:
+            raise ValueError(f"expected {n_fibers} fiber_body entries, got {fb.shape[0]}")
+        sr = None if site_ref is None else _arr(site_ref, 3)
+        x = np.empty(self.solution_size())
+        tension = np.empty(self.n_fib)
+        info = StepInfo()
+        handles = (self._h, _dense_h(dense)) if self._step_takes_dense else (self._h,)
+        rc = self._fn("step")(*handles, _params_ptr(p), _opt_p(vg), _opt_p(fs), _opt_p(f), _opt_p(ft),
+                              None if fb is None else fb.ctypes.data_as(C.POINTER(C.c_int)), _opt_p(sr), float(dt),
+                              float(eta), float(tol), int(num_blocks), int(max_iters), _p(x), _p(tension),
+                              C.byref(info))
+        # SKB_ERR_STATE with a NaN fiber_error is the step that was not installed: reported, not raised
+        if not (rc == ERR_STATE and np.isnan(info.fiber_error)):
+            _check(rc)
+        return x, tension, info.as_dict()
+
+    def fibers(self):
+        """the fiber positions (N_f, 3) of the last set_fibers or step"""
+        r = np.empty((self.n_fib, 3))
+        self._call("get_fibers", _p(r))
+        return r
+
+    def placement(self):
+        """(centres (n_bodies, 3), quaternions (n_bodies, 4)) of the last place_bodies or step"""
+        c, q = np.empty((self.n_bodies, 3)), np.empty((self.n_bodies, 4))
+        self._call("get_placement", _p(c), _p(q))
+        return c, q
+
+    def stats(self) -> dict:
+        s = FlowStats()
+        self._call("last_stats", C.byref(s))
+        return {k: getattr(s, k) for k, _ in FlowStats._fields_}
+
+
+class Flow(_FlowBase):
+    """Device-resident flow() layer (include/skelly_b200_flow.h): FiberContainer / Periphery / BodyContainer flows
+    and the fused hydrodynamic part of System::apply_matvec."""
+    _destroy = "skb_flow_destroy"
+    _prefix = "skb_flow_"
+    _step_takes_dense = True
+
+    def __init__(self, device: int = 0):
+        self._h = C.c_void_p()
+        _check(library().skb_flow_create(int(device), C.byref(self._h)))
+        self.n_fib = self.n_shell = self.n_body = self.n_bodies = 0
 
     def fiber_flow(self, r_trg, fib_forces, eta, subtract_self=True):
         r_trg, fib_forces = _arr(r_trg, 3), _arr(fib_forces, 3)
@@ -712,27 +905,6 @@ class Flow:
         vel = np.empty((r_trg.shape[0], 3))
         _check(library().skb_flow_bodies(self._h, _p(r_trg), r_trg.shape[0], _p(densities), _p(ft), float(eta),
                                          _p(vel)))
-        return vel
-
-    def set_point_sources(self, positions, forces, torques):
-        positions, forces, torques = _arr(positions, 3), _arr(forces, 3), _arr(torques, 3)
-        _check(library().skb_flow_set_point_sources(self._h, _p(positions), _p(forces), _p(torques),
-                                                    positions.shape[0]))
-
-    def set_background(self, components, scale_factor, uniform):
-        comp = (C.c_int * 3)(*[int(c) for c in components])
-        sc = np.ascontiguousarray(scale_factor, dtype=np.float64)
-        un = np.ascontiguousarray(uniform, dtype=np.float64)
-        _check(library().skb_flow_set_background(self._h, comp, _p(sc), _p(un)))
-
-    def velocity_at_targets(self, r_trg, fib_forces, shell_density, body_densities, body_forces_torques, eta):
-        """System::velocity_at_targets (system.cpp:355-359): fiber (no self subtraction) + body + periphery flows."""
-        r_trg = _arr(r_trg, 3)
-        a, b, c = _arr(fib_forces, 3), _arr(shell_density, 3), _arr(body_densities, 3)
-        ft = _arr(body_forces_torques, 6)
-        vel = np.empty((r_trg.shape[0], 3))
-        _check(library().skb_flow_velocity_at_targets(self._h, _p(r_trg), r_trg.shape[0], _p(a), _p(b), _p(c), _p(ft),
-                                                      float(eta), _p(vel)))
         return vel
 
     def set_listener_frame(self, fib_forces, shell_density, body_densities, body_forces_torques, body_velocities,
@@ -782,19 +954,6 @@ class Flow:
         +-1e-7); "val" is the vorticity, the exits still test the velocity."""
         return self._lines(1, x0, dt_init, t_final, abs_err, rel_err, back_integrate, max_points)
 
-    def set_cross(self, mode: int):
-        """Fiber <-> periphery pairs of the matvec in one geometry pass: -1 auto (default), 0 never, 1 whenever applicable."""
-        _check(library().skb_flow_set_cross(self._h, int(mode)))
-
-    def set_self_exclusion(self, fused: bool):
-        """Matvec self term: False = the reference's compute-then-subtract (default); True = the pair kernels skip
-        intra-fiber pairs (SURVEY.md 8f N3)."""
-        _check(library().skb_flow_set_self_exclusion(self._h, int(bool(fused))))
-
-    def set_overlap(self, on: bool):
-        """Periphery dense operator beside the pair kernels on a side stream (default) or as one kernel at the end."""
-        _check(library().skb_flow_set_overlap(self._h, int(bool(on))))
-
     def set_target_window(self, begin: int, end: int = -1):
         """Evaluate only rows [begin, end) of [fibers | periphery | bodies] in matvec() (one rank's block)."""
         _check(library().skb_flow_set_target_window(self._h, int(begin), int(end)))
@@ -835,33 +994,7 @@ class Flow:
                                                 C.c_void_p(d_body_torques), float(eta), C.c_void_p(d_v_window),
                                                 C.c_void_p(stream)))
 
-    def matvec(self, fib_forces, shell_density, body_densities, body_forces_torques, eta):
-        a, b, c = _arr(fib_forces, 3), _arr(shell_density, 3), _arr(body_densities, 3)
-        ft = _arr(body_forces_torques, 6)
-        v = np.empty((sum(self._pieces()), 3))
-        _check(library().skb_flow_matvec(self._h, _p(a), _p(b), _p(c), _p(ft), float(eta), _p(v)))
-        return v
-
     # ---- per-fiber dense operators (SURVEY.md §8f N2); matrices go in column-major like Eigen's .data() ----
-    def set_fiber_class(self, n_nodes: int, D_1_0, P_downsample_bc):
-        """FiberFiniteDifference::matrices_.at(n): D_1_0 (n,n), P_downsample_bc (4n-14,4n)."""
-        n = int(n_nodes)
-        D = np.asfortranarray(D_1_0, dtype=np.float64)
-        P = np.asfortranarray(P_downsample_bc, dtype=np.float64)
-        if D.shape != (n, n) or P.shape != (4 * n - 14, 4 * n):
-            raise ValueError(f"class matrices for n={n}: got {D.shape}, {P.shape}")
-        _check(library().skb_flow_set_fiber_class(self._h, n, _p(D), _p(P)))
-
-    @staticmethod
-    def _colmajor_concat(mats):
-        """Per-fiber matrices -> one buffer, every matrix column-major (Eigen's .data()).  A 3-D C-ordered stack of
-        equal shapes is transposed in one pass; a list may be ragged."""
-        if isinstance(mats, np.ndarray) and mats.ndim == 3:
-            return np.ascontiguousarray(np.asarray(mats, dtype=np.float64).transpose(0, 2, 1)).reshape(-1)
-        if len(mats) == 0:
-            return np.zeros(0)
-        return np.concatenate([np.asarray(m, dtype=np.float64).ravel(order="F") for m in mats])
-
     def set_fiber_operators(self, A_list, force_list, xs, length_prev, plus_bc_velocity, colmajor=False):
         """A_ (4n,4n) and force_operator_ (3n,4n) per fiber (lists, or (n_fibers, rows, cols) stacks), tangents xs
         (N_f,3), length_prev_, plus-end velocity BC -- of the OWN fibers when target ranges are set.  colmajor=True:
@@ -878,17 +1011,6 @@ class Flow:
         _check(library().skb_flow_set_fiber_operators(self._h, _p(A), _p(F), _p(xs), _p(lp),
                                                       pl.ctypes.data_as(C.POINTER(C.c_int))))
 
-    def set_fiber_preconditioner(self, A_inv_list):
-        """Explicit inverses of A_ (fib.A_LU_.inverse()), same fibers and order as set_fiber_operators."""
-        Ai = self._colmajor_concat(A_inv_list)
-        _check(library().skb_flow_set_fiber_preconditioner(self._h, _p(Ai)))
-
-    def set_fiber_class_derivatives(self, n_nodes: int, D_2_0, D_3_0, D_4_0):
-        """The higher derivative matrices of FiberFiniteDifference::matrices_.at(n) (pre-transposed like D_1_0), needed
-        by build_fiber_operators for every node count in use."""
-        n, (D2, D3, D4) = _class_derivatives(n_nodes, D_2_0, D_3_0, D_4_0)
-        _check(library().skb_flow_set_fiber_class_derivatives(self._h, n, _p(D2), _p(D3), _p(D4)))
-
     def _own_fibers(self):
         """(first, end) fiber of the current window / ranges (all fibers without either)."""
         off = getattr(self, "_fiber_off", np.zeros(1, dtype=np.int64))
@@ -902,32 +1024,6 @@ class Flow:
         w1 = nf if w1 < 0 else min(max(w1, w0), nf)
         return int(np.searchsorted(off, w0)), int(np.searchsorted(off, w1))
 
-    def build_fiber_operators(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
-                              plus_hinged, dt, eta):
-        """A_, force_operator_, xs_ and A_^-1 of the (own) fibers built on the device from the positions and lengths of
-        set_fibers (update_derivatives, update_linear_operator, update_force_operator, the operator half of
-        apply_bc_rectangular, update_preconditioner).  Per-fiber arrays or scalars; the flags are 0 / 1."""
-        f0, f1 = self._own_fibers()
-        p = fiber_params(f1 - f0, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
-                         plus_hinged)
-        _check(library().skb_flow_build_fiber_operators(self._h, _params_ptr(p), float(dt), float(eta)))
-
-    def build_fiber_rhs(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
-                        plus_hinged, dt, eta, v_on_fibers=None, f_external=None, v_growth=None, force_scale=None):
-        """The fiber block of the RHS (4 N_own,) as System::prep_state_for_solver leaves it: update_RHS with f_external
-        + force_scale xs_, then the RHS half of apply_bc_rectangular with f_external.  Parameters as for
-        build_fiber_operators; v_on_fibers / f_external (N_own, 3) and v_growth / force_scale (per-fiber arrays or
-        scalars) may be None: no flow / force, zero growth, no motors."""
-        f0, f1 = self._own_fibers()
-        n_own = self._pieces()[0]
-        p, vg, fs, v, f = _fiber_rhs_args(f1 - f0, n_own, (length_prev, bending_rigidity, radius, penalty_param,
-                                                           beta_tstep, minus_clamped, plus_hinged),
-                                          v_growth, force_scale, v_on_fibers, f_external)
-        rhs = np.empty(4 * n_own)
-        _check(library().skb_flow_build_fiber_rhs(self._h, _params_ptr(p), _opt_p(vg), _opt_p(fs), _opt_p(v), _opt_p(f),
-                                                  float(dt), float(eta), _p(rhs)))
-        return rhs
-
     def build_fiber_rhs_device(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
                                plus_hinged, dt, eta, d_v_on_fibers: int, d_f_external: int, d_rhs: int, v_growth=None,
                                force_scale=None, stream: int = 0):
@@ -937,10 +1033,9 @@ class Flow:
         p, vg, fs, _, _ = _fiber_rhs_args(f1 - f0, 0, (length_prev, bending_rigidity, radius, penalty_param,
                                                        beta_tstep, minus_clamped, plus_hinged),
                                           v_growth, force_scale, None, None)
-        _check(library().skb_flow_build_fiber_rhs_device(
-            self._h, _params_ptr(p), _opt_p(vg), _opt_p(fs), C.c_void_p(d_v_on_fibers) if d_v_on_fibers else None,
-            C.c_void_p(d_f_external) if d_f_external else None, float(dt), float(eta), C.c_void_p(d_rhs),
-            C.c_void_p(stream)))
+        _check(library().skb_flow_build_fiber_rhs_device(self._h, _params_ptr(p), _opt_p(vg), _opt_p(fs),
+                                                         _vp(d_v_on_fibers), _vp(d_f_external), float(dt), float(eta),
+                                                         C.c_void_p(d_rhs), C.c_void_p(stream)))
 
     def get_fiber_operators(self, inverse=True):
         """The resident operators of the (own) fibers: dict(A=[(4n,4n)], force=[(3n,4n)], xs=(N_own,3),
@@ -1000,8 +1095,7 @@ class Flow:
     def fiber_matvec_device(self, d_x_fibers: int, d_v_fibers: int, d_v_fib_boundary: int, d_res: int,
                             stream: int = 0):
         _check(library().skb_flow_fiber_matvec_device(self._h, C.c_void_p(d_x_fibers), C.c_void_p(d_v_fibers),
-                                                      C.c_void_p(d_v_fib_boundary) if d_v_fib_boundary else None,
-                                                      C.c_void_p(d_res), C.c_void_p(stream)))
+                                                      _vp(d_v_fib_boundary), C.c_void_p(d_res), C.c_void_p(stream)))
 
     def apply_matvec(self, x_fibers, shell_density, body_densities, body_forces_torques, eta,
                      fiber_link_conditions=None, dense=None, out=None):
@@ -1035,40 +1129,12 @@ class Flow:
                             d_out_shell: int, d_v_bodies: int, stream: int = 0):
         """System::apply_matvec with every operand already on the device (addresses as ints, 0 = NULL); OWN slices
         for a group member.  Asynchronous on `stream`."""
-        vp = lambda a: C.c_void_p(a) if a else None
-        _check(library().skb_flow_apply_matvec_device(self._h, dense._h if dense is not None else None, vp(d_x_fibers),
-                                                      vp(d_x_shell), vp(d_body_densities), vp(d_body_forces),
-                                                      vp(d_body_torques), vp(d_fiber_link_conditions), float(eta),
-                                                      vp(d_res_fibers), vp(d_out_shell), vp(d_v_bodies), vp(stream)))
+        _check(library().skb_flow_apply_matvec_device(self._h, _dense_h(dense), _vp(d_x_fibers), _vp(d_x_shell),
+                                                      _vp(d_body_densities), _vp(d_body_forces), _vp(d_body_torques),
+                                                      _vp(d_fiber_link_conditions), float(eta), _vp(d_res_fibers),
+                                                      _vp(d_out_shell), _vp(d_v_bodies), _vp(stream)))
 
     # ---- the whole solution vector [fibers | shell | bodies] with the bodies on the device ----
-    def set_body_operators(self, n_nodes, node_weights, ex, ey, ez, A_inv_list=None):
-        """Per body (order of set_bodies = order in the solution vector): node count, node_weights_ (N_b,), ex_ / ey_ /
-        ez_ (N_b, 3) each, and A_^-1 ((3n+6, 3n+6) per body, a list) or None (no system preconditioner for bodies)."""
-        n = np.ascontiguousarray(n_nodes, dtype=np.int32)
-        w = np.ascontiguousarray(node_weights, dtype=np.float64).reshape(-1)
-        ex, ey, ez = _arr(ex, 3), _arr(ey, 3), _arr(ez, 3)
-        Ai = None if A_inv_list is None else self._colmajor_concat(A_inv_list)
-        _check(library().skb_flow_set_body_operators(self._h, n.ctypes.data_as(C.POINTER(C.c_int)), int(n.shape[0]),
-                                                     _p(w), _p(ex), _p(ey), _p(ez), None if Ai is None else _p(Ai)))
-        self._body_sol = int(np.sum(3 * n + 6))
-        self._body_n = n
-
-    def set_body_frames(self, n_nodes, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0, A_inv0_list=None):
-        """The bodies' operators in their body frame, once per run after set_bodies: per body its node count, per node
-        node_positions_ref_ / node_normals_ref_ (N_b, 3) and node_weights_ (N_b,), ex_ / ey_ / ez_ (N_b, 3) and
-        A_^-1 ((3n+6, 3n+6) per body, a list, or None) of the body at identity orientation.  place_bodies then forms
-        the placed operators on the device."""
-        a = _frame_arrays(n_nodes, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0, A_inv0_list)
-        _frame_call(library().skb_flow_set_body_frames, self._h, a)
-        self._body_sol, self._body_n = int(np.sum(3 * a[0] + 6)), a[0]
-
-    def place_bodies(self, centers, orientations):
-        """Once per timestep: the bodies at centres (n_bodies, 3) and unit quaternions (w, x, y, z) (n_bodies, 4) --
-        their nodes, normals and operators, as set_bodies + set_body_operators with the placed ones would leave them.
-        The fiber links are dropped."""
-        _place_call(library().skb_flow_place_bodies, self._h, centers, orientations)
-
     def get_body_operators(self, inverse=True):
         """The resident body operators: dict(ex, ey, ez (N_b, 3) each, A_inv = per body its (3n+6, 3n+6) inverse, None
         for a body whose inverse a group member does not keep; A_inv None with inverse=False)."""
@@ -1092,66 +1158,29 @@ class Flow:
                 out.append(None)
         return dict(ex=ex, ey=ey, ez=ez, A_inv=out if inverse else None)
 
-    def set_fiber_links(self, body=None, site=None, bending_rigidity=None):
-        """Per fiber: body index (-1 free), lab-frame nucleation site (n_fibers, 3), bending_rigidity_; body=None: no
-        fiber is bound."""
-        if body is None:
-            _check(library().skb_flow_set_fiber_links(self._h, None, None, None))
-            return
-        b = np.ascontiguousarray(body, dtype=np.int32)
-        st = _arr(site, 3)
-        E = np.ascontiguousarray(np.broadcast_to(np.asarray(bending_rigidity, dtype=np.float64), b.shape))
-        assert st.shape[0] == b.shape[0]
-        _check(library().skb_flow_set_fiber_links(self._h, b.ctypes.data_as(C.POINTER(C.c_int)), _p(st), _p(E)))
-
-    def solution_size(self) -> int:
-        """4 N_f + 3 N_s + sum(3 n_b + 6) (the bodies' part as set_body_operators was last given)"""
-        return 4 * self.n_fib + 3 * self.n_shell + (getattr(self, "_body_sol", 0) if self.n_bodies else 0)
-
     def apply_system_matvec(self, x, eta, dense=None):
         """System::apply_matvec (system.cpp:269-324) on the whole solution vector x: returns res = A x."""
         x = np.ascontiguousarray(x, dtype=np.float64).reshape(-1)
         assert x.shape[0] == self.solution_size()
         res = np.empty_like(x)
-        _check(library().skb_flow_apply_system_matvec(self._h, dense._h if dense is not None else None, _p(x),
-                                                      float(eta), _p(res)))
+        _check(library().skb_flow_apply_system_matvec(self._h, _dense_h(dense), _p(x), float(eta), _p(res)))
         return res
 
     def apply_system_matvec_device(self, dense, d_x: int, eta: float, d_res: int, stream: int = 0):
-        _check(library().skb_flow_apply_system_matvec_device(self._h, dense._h if dense is not None else None,
-                                                             C.c_void_p(d_x), float(eta), C.c_void_p(d_res),
-                                                             C.c_void_p(stream)))
+        _check(library().skb_flow_apply_system_matvec_device(self._h, _dense_h(dense), C.c_void_p(d_x), float(eta),
+                                                             C.c_void_p(d_res), C.c_void_p(stream)))
 
     def apply_system_preconditioner(self, x, dense=None):
         """System::apply_preconditioner (system.cpp:248-262) on the whole solution vector x: returns y = P^-1 x."""
         x = np.ascontiguousarray(x, dtype=np.float64).reshape(-1)
         assert x.shape[0] == self.solution_size()
         y = np.empty_like(x)
-        _check(library().skb_flow_apply_system_preconditioner(self._h, dense._h if dense is not None else None, _p(x),
-                                                              _p(y)))
+        _check(library().skb_flow_apply_system_preconditioner(self._h, _dense_h(dense), _p(x), _p(y)))
         return y
 
     def apply_system_preconditioner_device(self, dense, d_x: int, d_y: int, stream: int = 0):
-        _check(library().skb_flow_apply_system_preconditioner_device(self._h, dense._h if dense is not None else None,
-                                                                     C.c_void_p(d_x), C.c_void_p(d_y),
-                                                                     C.c_void_p(stream)))
-
-    def build_system_rhs(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
-                         plus_hinged, dt, eta, f_external=None, body_forces_torques=None, v_growth=None,
-                         force_scale=None):
-        """System::prep_state_for_solver's RHS (system.cpp:398-458) as a whole solution vector (solution_size(),):
-        the flow of f_external (N_f, 3) and of the bodies' external forces / torques (n_bodies, 6), plus the point
-        sources and the background flow, into the fiber block (build_fiber_rhs's parameters), -v_shell and
-        [-v_body ; 0] per body.  f_external / body_forces_torques None: zero."""
-        f0, f1 = self._own_fibers()
-        p, vg, fs, f, ft = _system_rhs_args(f1 - f0, self.n_fib, self.n_bodies,
-                                            (length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
-                                             minus_clamped, plus_hinged), v_growth, force_scale, f_external,
-                                            body_forces_torques)
-        rhs = np.empty(self.solution_size())
-        _check(library().skb_flow_build_system_rhs(self._h, _params_ptr(p), _opt_p(vg), _opt_p(fs), _opt_p(f),
-                                                   _opt_p(ft), float(dt), float(eta), _p(rhs)))
-        return rhs
+        _check(library().skb_flow_apply_system_preconditioner_device(self._h, _dense_h(dense), C.c_void_p(d_x),
+                                                                     C.c_void_p(d_y), C.c_void_p(stream)))
 
     def build_system_rhs_device(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
                                 minus_clamped, plus_hinged, dt, eta, d_f_external: int, d_body_forces: int,
@@ -1162,15 +1191,9 @@ class Flow:
         p, vg, fs, _, _ = _system_rhs_args(f1 - f0, 0, self.n_bodies,
                                            (length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
                                             minus_clamped, plus_hinged), v_growth, force_scale, None, None)
-        vp = lambda a: C.c_void_p(a) if a else None
         _check(library().skb_flow_build_system_rhs_device(self._h, _params_ptr(p), _opt_p(vg), _opt_p(fs),
-                                                          vp(d_f_external), vp(d_body_forces), vp(d_body_torques),
-                                                          float(dt), float(eta), vp(d_rhs), vp(stream)))
-
-    def set_gmres(self, num_blocks: int = 300):
-        """Size the workspace of solve_system for the current solution size and up to num_blocks basis vectors."""
-        _check(library().skb_flow_set_gmres(self._h, int(num_blocks)))
-        self._gmres_blocks = int(num_blocks)
+                                                          _vp(d_f_external), _vp(d_body_forces), _vp(d_body_torques),
+                                                          float(dt), float(eta), _vp(d_rhs), _vp(stream)))
 
     def solve_system(self, rhs, eta, dense=None, tol=1e-10, num_blocks=300, max_iters=1000):
         """Solver::solve (solver_hydro.cpp:64-95): x = A^-1 rhs by restarted right-preconditioned GMRES on the device.
@@ -1181,9 +1204,8 @@ class Flow:
         x = np.empty_like(b)
         info = SolveInfo()
         hist = np.full(max(int(max_iters), 0) + 1, np.nan)
-        _check(library().skb_flow_solve_system(self._h, dense._h if dense is not None else None, _p(b), float(eta),
-                                               float(tol), int(num_blocks), int(max_iters), _p(x), C.byref(info),
-                                               _p(hist)))
+        _check(library().skb_flow_solve_system(self._h, _dense_h(dense), _p(b), float(eta), float(tol), int(num_blocks),
+                                               int(max_iters), _p(x), C.byref(info), _p(hist)))
         return x, info.as_dict(), hist[:info.iterations + 1]
 
     def solve_system_device(self, dense, d_rhs: int, eta: float, d_x: int, tol=1e-10, num_blocks=300,
@@ -1192,50 +1214,16 @@ class Flow:
         Returns (info, history) as solve_system."""
         info = SolveInfo()
         hist = np.full(max(int(max_iters), 0) + 1, np.nan)
-        _check(library().skb_flow_solve_system_device(self._h, dense._h if dense is not None else None,
-                                                      C.c_void_p(d_rhs), float(eta), float(tol), int(num_blocks),
-                                                      int(max_iters), C.c_void_p(d_x), C.byref(info), _p(hist),
-                                                      C.c_void_p(stream)))
+        _check(library().skb_flow_solve_system_device(self._h, _dense_h(dense), C.c_void_p(d_rhs), float(eta),
+                                                      float(tol), int(num_blocks), int(max_iters), C.c_void_p(d_x),
+                                                      C.byref(info), _p(hist), C.c_void_p(stream)))
         return info.as_dict(), hist[:info.iterations + 1]
-
-    def set_periphery_shape(self, kind, a, b=0.0, c=0.0, f_0=20.0, l_0=0.05, binding_active=False,
-                            polar_angle_start=0.0, polar_angle_end=np.pi, binding_threshold=0.75,
-                            fiber_minus_clamped=None, body_radius=None):
-        _shape_call(library().skb_flow_set_periphery_shape, self._h, self._n_fibers(), self.n_bodies, kind, a, b, c,
-                    f_0, l_0, binding_active, polar_angle_start, polar_angle_end, binding_threshold,
-                    fiber_minus_clamped, body_radius)
-        # kept so that the shape can be set again for another fiber set (timestep.Stepper.restore)
-        self._shape = dict(kind=kind, a=a, b=b, c=c, f_0=f_0, l_0=l_0, binding_active=binding_active,
-                           polar_angle_start=polar_angle_start, polar_angle_end=polar_angle_end,
-                           binding_threshold=binding_threshold, body_radius=body_radius,
-                           fiber_minus_clamped=np.zeros(self._n_fibers(), dtype=np.int32)
-                           if fiber_minus_clamped is None else np.array(fiber_minus_clamped, dtype=np.int32))
-
-    set_periphery_shape.__doc__ = _SHAPE_DOC
 
     def periphery_interaction(self, n_own_nodes=None, n_own_fibers=None):
         """(repulsion (N, 3) of the own nodes, plus_hinged (own fibers,) int32, collided bool over all fibers and
         bodies) at the current geometry (skb_flow_periphery_interaction); by default all nodes and fibers"""
-        return _interaction_call(library().skb_flow_periphery_interaction, self._h,
-                                 self.n_fib if n_own_nodes is None else int(n_own_nodes),
+        return _interaction_call(self, self.n_fib if n_own_nodes is None else int(n_own_nodes),
                                  self._n_fibers() if n_own_fibers is None else int(n_own_fibers))
-
-    def step(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped, plus_hinged, dt,
-             eta, dense=None, f_external=None, body_forces_torques=None, fiber_body=None, site_ref=None,
-             v_growth=None, force_scale=None, tol=1e-10, num_blocks=300, max_iters=1000):
-        """System::step (system.cpp:482-492) on the device: links, fiber operators, RHS and solve at the current
-        geometry, then the fibers' and bodies' step and the new geometry installed.  fiber_body (N_fibers,) ints, -1
-        free, or None; site_ref (N_fibers, 3) body-frame nucleation sites, or None.  Returns (x, tension, info): info
-        a dict of skb_step_info (the solve's fields, fiber_error, worst_fiber, collided).  A solution with non-finite
-        new positions installs nothing and returns fiber_error NaN.  With set_periphery_shape, plus_hinged is ignored
-        (the binding sets it) and the repulsion is added to f_external."""
-        return _step_call(self, lambda *a: library().skb_flow_step(self._h, dense._h if dense is not None else None, *a),
-                          self._n_fibers(), (length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
-                                             minus_clamped, plus_hinged), dt, eta, f_external, body_forces_torques,
-                          fiber_body, site_ref, v_growth, force_scale, tol, num_blocks, max_iters)
-
-    def _n_fibers(self):
-        return len(getattr(self, "_fiber_off", [0])) - 1
 
     def set_nucleation_sites(self, n_sites_per_body, site_ref):
         """the bodies' nucleation_sites_ref_ (body frame), concatenated: n_sites_per_body per body, site_ref (total, 3)
@@ -1307,18 +1295,6 @@ class Flow:
         _check(library().skb_flow_fiber_error(self._h, C.byref(m), _p(per)))
         return m.value, per
 
-    def fibers(self):
-        """the fiber positions (N_f, 3) of the last set_fibers or step"""
-        r = np.empty((self.n_fib, 3))
-        _check(library().skb_flow_get_fibers(self._h, _p(r)))
-        return r
-
-    def placement(self):
-        """(centres (n_bodies, 3), quaternions (n_bodies, 4)) of the last place_bodies or step"""
-        c, q = np.empty((self.n_bodies, 3)), np.empty((self.n_bodies, 4))
-        _check(library().skb_flow_get_placement(self._h, _p(c), _p(q)))
-        return c, q
-
     # ---- multi-GPU groups (peer memory) ----
     def last_sym_kernel(self):
         """(ms, ordered pairs) of the last launch of the symmetric fiber-fiber kernel inside matvec()."""
@@ -1358,52 +1334,33 @@ class Flow:
     def group_set_body_operators(self, n_nodes, node_weights, ex, ey, ez, A_inv_list=None):
         """set_body_operators on a group member (arrays of ALL bodies): it keeps what its body rows need, lays out its
         local vector's body rows and sizes the buffers of the group_* system calls.  Not a member: set_body_operators."""
-        n = np.ascontiguousarray(n_nodes, dtype=np.int32)
-        w = np.ascontiguousarray(node_weights, dtype=np.float64).reshape(-1)
-        ex, ey, ez = _arr(ex, 3), _arr(ey, 3), _arr(ez, 3)
-        Ai = None if A_inv_list is None else self._colmajor_concat(A_inv_list)
-        _check(library().skb_flow_group_set_body_operators(self._h, n.ctypes.data_as(C.POINTER(C.c_int)),
-                                                           int(n.shape[0]), _p(w), _p(ex), _p(ey), _p(ez),
-                                                           None if Ai is None else _p(Ai)))
-        self._body_sol = int(np.sum(3 * n + 6))
-        self._body_n = n
+        _body_operators_call(self, "group_set_body_operators", n_nodes, node_weights, ex, ey, ez, A_inv_list)
 
     def group_set_body_frames(self, n_nodes, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0,
                               A_inv0_list=None):
         """set_body_frames on a group member (arrays of ALL bodies): it keeps the body-frame inverses of the bodies it
         owns rows of, lays out its body rows and sizes every buffer, as group_set_body_operators does."""
-        a = _frame_arrays(n_nodes, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0, A_inv0_list)
-        _frame_call(library().skb_flow_group_set_body_frames, self._h, a)
-        self._body_sol, self._body_n = int(np.sum(3 * a[0] + 6)), a[0]
+        _frame_call(self, "group_set_body_frames", n_nodes, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0,
+                    A_inv0_list)
 
     def group_place_bodies(self, centers, orientations):
         """place_bodies on a group member; allocates no device memory"""
-        _place_call(library().skb_flow_group_place_bodies, self._h, centers, orientations)
+        _place_call(self, "group_place_bodies", centers, orientations)
 
     def group_set_fiber_links(self, body=None, site=None, bending_rigidity=None):
         """set_fiber_links on a group member: body index, nucleation site (n, 3) and bending_rigidity_ of the OWN
         fibers; body=None: none of them is bound."""
-        if body is None:
-            _check(library().skb_flow_group_set_fiber_links(self._h, None, None, None))
-            return
-        b = np.ascontiguousarray(body, dtype=np.int32)
-        st = _arr(site, 3)
-        E = np.ascontiguousarray(np.broadcast_to(np.asarray(bending_rigidity, dtype=np.float64), b.shape))
-        assert st.shape[0] == b.shape[0]
-        _check(library().skb_flow_group_set_fiber_links(self._h, b.ctypes.data_as(C.POINTER(C.c_int)), _p(st), _p(E)))
+        _links_call(self, "group_set_fiber_links", body, site, bending_rigidity)
 
     def group_apply_system_matvec_device(self, dense, d_x_local: int, eta: float, d_res_local: int, stream: int = 0):
         """the member's rows of A x from its rows of x (distributed.system_rows), asynchronous on `stream`"""
-        vp = lambda a: C.c_void_p(a) if a else None
-        _check(library().skb_flow_group_apply_system_matvec_device(self._h, dense._h if dense is not None else None,
-                                                                   vp(d_x_local), float(eta), vp(d_res_local),
-                                                                   vp(stream)))
+        _check(library().skb_flow_group_apply_system_matvec_device(self._h, _dense_h(dense), _vp(d_x_local), float(eta),
+                                                                   _vp(d_res_local), _vp(stream)))
 
     def group_apply_system_preconditioner_device(self, dense, d_x_local: int, d_y_local: int, stream: int = 0):
         """the member's rows of P^-1 x from its rows of x, asynchronous on `stream`"""
-        vp = lambda a: C.c_void_p(a) if a else None
         _check(library().skb_flow_group_apply_system_preconditioner_device(
-            self._h, dense._h if dense is not None else None, vp(d_x_local), vp(d_y_local), vp(stream)))
+            self._h, _dense_h(dense), _vp(d_x_local), _vp(d_y_local), _vp(stream)))
 
     def group_solve_system_device(self, dense_matvec, dense_minv, d_rhs_local: int, eta: float, d_x_local: int,
                                   tol=1e-10, num_blocks=300, max_iters=1000, stream: int = 0):
@@ -1411,11 +1368,10 @@ class Flow:
         calls it alike.  Returns (info, history), bitwise the same on every member."""
         info = SolveInfo()
         hist = np.full(max(int(max_iters), 0) + 1, np.nan)
-        vp = lambda a: C.c_void_p(a) if a else None
-        h = lambda d: d._h if d is not None else None
-        _check(library().skb_flow_group_solve_system_device(self._h, h(dense_matvec), h(dense_minv), vp(d_rhs_local),
-                                                            float(eta), float(tol), int(num_blocks), int(max_iters),
-                                                            vp(d_x_local), C.byref(info), _p(hist), vp(stream)))
+        _check(library().skb_flow_group_solve_system_device(self._h, _dense_h(dense_matvec), _dense_h(dense_minv),
+                                                            _vp(d_rhs_local), float(eta), float(tol), int(num_blocks),
+                                                            int(max_iters), _vp(d_x_local), C.byref(info), _p(hist),
+                                                            _vp(stream)))
         return info.as_dict(), hist[:info.iterations + 1]
 
     def group_build_system_rhs_device(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
@@ -1428,11 +1384,10 @@ class Flow:
         p, vg, fs, _, _ = _system_rhs_args(f1 - f0, 0, self.n_bodies,
                                            (length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
                                             minus_clamped, plus_hinged), v_growth, force_scale, None, None)
-        vp = lambda a: C.c_void_p(a) if a else None
         _check(library().skb_flow_group_build_system_rhs_device(self._h, _params_ptr(p), _opt_p(vg), _opt_p(fs),
-                                                                vp(d_f_external), vp(d_body_forces),
-                                                                vp(d_body_torques), float(dt), float(eta),
-                                                                vp(d_rhs_local), vp(stream)))
+                                                                _vp(d_f_external), _vp(d_body_forces),
+                                                                _vp(d_body_torques), float(dt), float(eta),
+                                                                _vp(d_rhs_local), _vp(stream)))
 
     def group_step_device(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
                           plus_hinged, dt, eta, dense_matvec=None, dense_minv=None, d_f_external: int = 0,
@@ -1452,28 +1407,23 @@ class Flow:
         if fb is not None and fb.shape[0] != f1 - f0:
             raise ValueError(f"expected {f1 - f0} fiber_body entries (the own fibers), got {fb.shape[0]}")
         sr = None if site_ref is None else _arr(site_ref, 3)
-        vp = lambda a: C.c_void_p(a) if a else None
-        h = lambda d: d._h if d is not None else None
         info = StepInfo()
         rc = library().skb_flow_group_step_device(
-            self._h, h(dense_matvec), h(dense_minv), _params_ptr(p), _opt_p(vg), _opt_p(fs), vp(d_f_external),
-            vp(d_body_forces), vp(d_body_torques), None if fb is None else fb.ctypes.data_as(C.POINTER(C.c_int)),
-            _opt_p(sr), float(dt), float(eta), float(tol), int(num_blocks), int(max_iters), vp(d_x_local),
-            vp(d_tension), C.byref(info), vp(stream))
+            self._h, _dense_h(dense_matvec), _dense_h(dense_minv), _params_ptr(p), _opt_p(vg), _opt_p(fs),
+            _vp(d_f_external), _vp(d_body_forces), _vp(d_body_torques),
+            None if fb is None else fb.ctypes.data_as(C.POINTER(C.c_int)), _opt_p(sr), float(dt), float(eta),
+            float(tol), int(num_blocks), int(max_iters), _vp(d_x_local), _vp(d_tension), C.byref(info), _vp(stream))
         if not (rc == ERR_STATE and np.isnan(info.fiber_error)):
             _check(rc)
         return info.as_dict()
 
-    def stats(self) -> dict:
-        s = FlowStats()
-        _check(library().skb_flow_last_stats(self._h, C.byref(s)))
-        return {k: getattr(s, k) for k, _ in FlowStats._fields_}
 
-
-class MultiFlow:
+class MultiFlow(_FlowBase):
     """skb_mflow: ONE process driving n GPUs (include/skelly_b200_flow.h) -- same conventions as Flow, complete host
     arrays in and out; fibers / periphery rows / body rows are partitioned over the devices, which exchange strengths
     and partial velocities through peer memory."""
+    _destroy = "skb_mflow_destroy"
+    _prefix = "skb_mflow_"
 
     def __init__(self, devices):
         devs = list(range(devices)) if isinstance(devices, int) else [int(d) for d in devices]
@@ -1481,55 +1431,20 @@ class MultiFlow:
         self._h = C.c_void_p()
         _check(library().skb_mflow_create(arr, len(devs), C.byref(self._h)))
         self.devices = devs
-        self.n_fib = self.n_shell = self.n_body = self.n_bodies = self.n_fibers = 0
+        self.n_fib = self.n_shell = self.n_body = self.n_bodies = 0
 
-    def close(self):
-        if getattr(self, "_h", None) and self._h.value:
-            library().skb_mflow_destroy(self._h)
-            self._h = C.c_void_p()
+    @property
+    def n_fibers(self) -> int:
+        """the number of fibers of the last set_fibers"""
+        return self._n_fibers()
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+    def _own_fibers(self):
+        """every call covers all fibers"""
+        return 0, self._n_fibers()
 
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *a):
-        self.close()
-
-    def set_fibers(self, r_fib, n_nodes, lengths):
-        r_fib = _arr(r_fib, 3)
-        n_nodes = np.ascontiguousarray(n_nodes, dtype=np.int32)
-        lengths = np.ascontiguousarray(lengths, dtype=np.float64)
-        assert n_nodes.shape == lengths.shape and int(n_nodes.sum()) == r_fib.shape[0]
-        _check(library().skb_mflow_set_fibers(self._h, _p(r_fib), n_nodes.ctypes.data_as(C.POINTER(C.c_int)),
-                                              _p(lengths), int(n_nodes.shape[0])))
-        self.n_fib, self.n_fibers = r_fib.shape[0], int(n_nodes.shape[0])
-        self._fiber_off = np.concatenate([[0], np.cumsum(n_nodes, dtype=np.int64)])
-        self._lengths = lengths.copy()
-
-    def set_periphery(self, node_pos, node_normal):
-        node_pos, node_normal = _arr(node_pos, 3), _arr(node_normal, 3)
-        _check(library().skb_mflow_set_periphery(self._h, _p(node_pos), _p(node_normal), node_pos.shape[0]))
-        self.n_shell = node_pos.shape[0]
-
-    def set_bodies(self, node_pos, node_normal, centers):
-        node_pos, node_normal, centers = _arr(node_pos, 3), _arr(node_normal, 3), _arr(centers, 3)
-        _check(library().skb_mflow_set_bodies(self._h, _p(node_pos), _p(node_normal), node_pos.shape[0], _p(centers),
-                                              centers.shape[0]))
-        self.n_body, self.n_bodies = node_pos.shape[0], centers.shape[0]
-
-    def set_self_exclusion(self, fused: bool):
-        _check(library().skb_mflow_set_self_exclusion(self._h, int(bool(fused))))
-
-    def set_cross(self, mode: int):
-        _check(library().skb_mflow_set_cross(self._h, int(mode)))
-
-    def set_overlap(self, on: bool):
-        _check(library().skb_mflow_set_overlap(self._h, int(bool(on))))
+    def _pieces(self):
+        """(fiber nodes, shell rows, body rows): every call covers all of them"""
+        return self.n_fib, self.n_shell, self.n_body
 
     def partition(self, member: int):
         f0, f1 = C.c_int(), C.c_int()
@@ -1537,20 +1452,12 @@ class MultiFlow:
         _check(library().skb_mflow_partition(self._h, int(member), C.byref(f0), C.byref(f1), *[C.byref(x) for x in r]))
         return (f0.value, f1.value) + tuple(x.value for x in r)
 
-    def set_fiber_class(self, n_nodes: int, D_1_0, P_downsample_bc):
-        n = int(n_nodes)
-        D = np.asfortranarray(D_1_0, dtype=np.float64)
-        P = np.asfortranarray(P_downsample_bc, dtype=np.float64)
-        if D.shape != (n, n) or P.shape != (4 * n - 14, 4 * n):
-            raise ValueError(f"class matrices for n={n}: got {D.shape}, {P.shape}")
-        _check(library().skb_mflow_set_fiber_class(self._h, n, _p(D), _p(P)))
-
     def set_fiber_operators(self, A_list, force_list, xs, length_prev, plus_bc_velocity, colmajor=False):
         if colmajor:
             A = np.ascontiguousarray(A_list, dtype=np.float64).reshape(-1)
             F = np.ascontiguousarray(force_list, dtype=np.float64).reshape(-1)
         else:
-            A, F = Flow._colmajor_concat(A_list), Flow._colmajor_concat(force_list)
+            A, F = self._colmajor_concat(A_list), self._colmajor_concat(force_list)
         xs = _arr(xs, 3)
         lp = np.ascontiguousarray(length_prev, dtype=np.float64)
         pl = np.ascontiguousarray(plus_bc_velocity, dtype=np.int32)
@@ -1558,44 +1465,10 @@ class MultiFlow:
         _check(library().skb_mflow_set_fiber_operators(self._h, _p(A), _p(F), _p(xs), _p(lp),
                                                        pl.ctypes.data_as(C.POINTER(C.c_int))))
 
-    def set_fiber_preconditioner(self, A_inv_list):
-        Ai = Flow._colmajor_concat(A_inv_list)
-        _check(library().skb_mflow_set_fiber_preconditioner(self._h, _p(Ai)))
-
-    def set_fiber_class_derivatives(self, n_nodes: int, D_2_0, D_3_0, D_4_0):
-        n, (D2, D3, D4) = _class_derivatives(n_nodes, D_2_0, D_3_0, D_4_0)
-        _check(library().skb_mflow_set_fiber_class_derivatives(self._h, n, _p(D2), _p(D3), _p(D4)))
-
-    def build_fiber_operators(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
-                              plus_hinged, dt, eta):
-        """Flow.build_fiber_operators for ALL fibers; every device builds its own slice."""
-        p = fiber_params(self.n_fibers, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
-                         plus_hinged)
-        _check(library().skb_mflow_build_fiber_operators(self._h, _params_ptr(p), float(dt), float(eta)))
-
-    def build_fiber_rhs(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
-                        plus_hinged, dt, eta, v_on_fibers=None, f_external=None, v_growth=None, force_scale=None):
-        """Flow.build_fiber_rhs for ALL fibers; every device forms its own slice."""
-        p, vg, fs, v, f = _fiber_rhs_args(self.n_fibers, self.n_fib, (length_prev, bending_rigidity, radius,
-                                                                      penalty_param, beta_tstep, minus_clamped,
-                                                                      plus_hinged),
-                                          v_growth, force_scale, v_on_fibers, f_external)
-        rhs = np.empty(4 * self.n_fib)
-        _check(library().skb_mflow_build_fiber_rhs(self._h, _params_ptr(p), _opt_p(vg), _opt_p(fs), _opt_p(v),
-                                                   _opt_p(f), float(dt), float(eta), _p(rhs)))
-        return rhs
-
     def set_dense(self, op: int, A):
         A = np.ascontiguousarray(A, dtype=np.float64)
         _check(library().skb_mflow_set_dense(self._h, int(op), _p(A), A.shape[0], A.shape[1]))
         self._has_dense = True
-
-    def matvec(self, fib_forces, shell_density, body_densities, body_forces_torques, eta):
-        a, b, c = _arr(fib_forces, 3), _arr(shell_density, 3), _arr(body_densities, 3)
-        ft = _arr(body_forces_torques, 6)
-        v = np.empty((self.n_fib + self.n_shell + self.n_body, 3))
-        _check(library().skb_mflow_matvec(self._h, _p(a), _p(b), _p(c), _p(ft), float(eta), _p(v)))
-        return v
 
     def apply_matvec(self, x_fibers, x_shell, body_densities, body_forces_torques, eta, fiber_link_conditions=None):
         """Returns (res_fibers (4 N_f,), out_shell (N_s,3), v_bodies (N_b,3)); out_shell is res_shell once
@@ -1611,75 +1484,9 @@ class MultiFlow:
                                                 float(eta), _p(res), _p(o_s), _p(v_b)))
         return res, o_s, v_b
 
-    # ---- the whole solution vector [fibers | shell | bodies] over the devices (the Flow twins' conventions) ----
-    def set_body_operators(self, n_nodes, node_weights, ex, ey, ez, A_inv_list=None):
-        """As Flow.set_body_operators, for all bodies; every device keeps the bodies it owns rows of."""
-        n = np.ascontiguousarray(n_nodes, dtype=np.int32)
-        w = np.ascontiguousarray(node_weights, dtype=np.float64).reshape(-1)
-        ex, ey, ez = _arr(ex, 3), _arr(ey, 3), _arr(ez, 3)
-        Ai = None if A_inv_list is None else Flow._colmajor_concat(A_inv_list)
-        _check(library().skb_mflow_set_body_operators(self._h, n.ctypes.data_as(C.POINTER(C.c_int)), int(n.shape[0]),
-                                                      _p(w), _p(ex), _p(ey), _p(ez), None if Ai is None else _p(Ai)))
-        self._body_sol = int(np.sum(3 * n + 6))
-
-    def set_body_frames(self, n_nodes, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0, A_inv0_list=None):
-        """As Flow.set_body_frames, for all bodies; every device keeps the body-frame inverses it owns rows of."""
-        a = _frame_arrays(n_nodes, node_pos_ref, node_normal_ref, node_weights, ex0, ey0, ez0, A_inv0_list)
-        _frame_call(library().skb_mflow_set_body_frames, self._h, a)
-        self._body_sol = int(np.sum(3 * a[0] + 6))
-
-    def place_bodies(self, centers, orientations):
-        """As Flow.place_bodies, on every device."""
-        _place_call(library().skb_mflow_place_bodies, self._h, centers, orientations)
-
-    def set_fiber_links(self, body=None, site=None, bending_rigidity=None):
-        """As Flow.set_fiber_links, for all fibers; body=None: no fiber is bound."""
-        if body is None:
-            _check(library().skb_mflow_set_fiber_links(self._h, None, None, None))
-            return
-        b = np.ascontiguousarray(body, dtype=np.int32)
-        st = _arr(site, 3)
-        E = np.ascontiguousarray(np.broadcast_to(np.asarray(bending_rigidity, dtype=np.float64), b.shape))
-        assert st.shape[0] == b.shape[0]
-        _check(library().skb_mflow_set_fiber_links(self._h, b.ctypes.data_as(C.POINTER(C.c_int)), _p(st), _p(E)))
-
-    def set_periphery_shape(self, kind, a, b=0.0, c=0.0, f_0=20.0, l_0=0.05, binding_active=False,
-                            polar_angle_start=0.0, polar_angle_end=np.pi, binding_threshold=0.75,
-                            fiber_minus_clamped=None, body_radius=None):
-        _shape_call(library().skb_mflow_set_periphery_shape, self._h, self.n_fibers, self.n_bodies, kind, a, b, c,
-                    f_0, l_0, binding_active, polar_angle_start, polar_angle_end, binding_threshold,
-                    fiber_minus_clamped, body_radius)
-
-    set_periphery_shape.__doc__ = _SHAPE_DOC
-
     def periphery_interaction(self):
         """Flow.periphery_interaction over the devices: the complete arrays of all fibers"""
-        return _interaction_call(library().skb_mflow_periphery_interaction, self._h, self.n_fib, self.n_fibers)
-
-    def step(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped, plus_hinged, dt,
-             eta, dense=None, f_external=None, body_forces_torques=None, fiber_body=None, site_ref=None,
-             v_growth=None, force_scale=None, tol=1e-10, num_blocks=300, max_iters=1000):
-        """Flow.step over the devices (dense: unused, the periphery's operators come from set_dense)"""
-        return _step_call(self, lambda *a: library().skb_mflow_step(self._h, *a), self.n_fibers,
-                          (length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
-                           plus_hinged), dt, eta, f_external, body_forces_torques, fiber_body, site_ref, v_growth,
-                          force_scale, tol, num_blocks, max_iters)
-
-    def fibers(self):
-        """the fiber positions (N_f, 3) every device holds"""
-        r = np.empty((self.n_fib, 3))
-        _check(library().skb_mflow_get_fibers(self._h, _p(r)))
-        return r
-
-    def placement(self):
-        """(centres (n_bodies, 3), quaternions (n_bodies, 4)) of the last place_bodies or step"""
-        c, q = np.empty((self.n_bodies, 3)), np.empty((self.n_bodies, 4))
-        _check(library().skb_mflow_get_placement(self._h, _p(c), _p(q)))
-        return c, q
-
-    def solution_size(self) -> int:
-        """4 N_f + 3 N_s + sum(3 n_b + 6) (the bodies' part as set_body_operators was last given)"""
-        return 4 * self.n_fib + 3 * self.n_shell + (getattr(self, "_body_sol", 0) if self.n_bodies else 0)
+        return _interaction_call(self, self.n_fib, self.n_fibers)
 
     def apply_system_matvec(self, x, eta):
         """System::apply_matvec on the whole solution vector x over the devices: returns res = A x.  The periphery's
@@ -1699,10 +1506,6 @@ class MultiFlow:
         _check(library().skb_mflow_apply_system_preconditioner(self._h, _p(x), _p(y)))
         return y
 
-    def set_gmres(self, num_blocks: int = 300):
-        """Lay out every member's local rows and size its solve workspace (after set_body_operators)."""
-        _check(library().skb_mflow_set_gmres(self._h, int(num_blocks)))
-
     def solve_system(self, rhs, eta, tol=1e-10, num_blocks=300, max_iters=1000):
         """Flow.solve_system over the devices, every member solving its own rows: returns (x, info, history)."""
         b = np.ascontiguousarray(rhs, dtype=np.float64).reshape(-1)
@@ -1714,55 +1517,15 @@ class MultiFlow:
                                                 int(max_iters), _p(x), C.byref(info), _p(hist)))
         return x, info.as_dict(), hist[:info.iterations + 1]
 
-    def build_system_rhs(self, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
-                         plus_hinged, dt, eta, f_external=None, body_forces_torques=None, v_growth=None,
-                         force_scale=None):
-        """Flow.build_system_rhs over the devices, every device forming its own rows: the whole vector
-        (solution_size(),)."""
-        p, vg, fs, f, ft = _system_rhs_args(self.n_fibers, self.n_fib, self.n_bodies,
-                                            (length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
-                                             minus_clamped, plus_hinged), v_growth, force_scale, f_external,
-                                            body_forces_torques)
-        rhs = np.empty(self.solution_size())
-        _check(library().skb_mflow_build_system_rhs(self._h, _params_ptr(p), _opt_p(vg), _opt_p(fs), _opt_p(f),
-                                                    _opt_p(ft), float(dt), float(eta), _p(rhs)))
-        return rhs
-
-    def set_point_sources(self, positions, forces, torques):
-        """Flow.set_point_sources on every device (velocity_at_targets and build_system_rhs include them)."""
-        positions, forces, torques = _arr(positions, 3), _arr(forces, 3), _arr(torques, 3)
-        _check(library().skb_mflow_set_point_sources(self._h, _p(positions), _p(forces), _p(torques),
-                                                     positions.shape[0]))
-
-    def set_background(self, components, scale_factor, uniform):
-        """Flow.set_background on every device."""
-        comp = (C.c_int * 3)(*[int(c) for c in components])
-        sc = np.ascontiguousarray(scale_factor, dtype=np.float64)
-        un = np.ascontiguousarray(uniform, dtype=np.float64)
-        _check(library().skb_mflow_set_background(self._h, comp, _p(sc), _p(un)))
-
-    def velocity_at_targets(self, r_trg, fib_forces, shell_density, body_densities, body_forces_torques, eta):
-        r_trg = _arr(r_trg, 3)
-        a, b, c = _arr(fib_forces, 3), _arr(shell_density, 3), _arr(body_densities, 3)
-        ft = _arr(body_forces_torques, 6)
-        vel = np.empty((r_trg.shape[0], 3))
-        _check(library().skb_mflow_velocity_at_targets(self._h, _p(r_trg), r_trg.shape[0], _p(a), _p(b), _p(c), _p(ft),
-                                                       float(eta), _p(vel)))
-        return vel
-
-    def stats(self) -> dict:
-        s = FlowStats()
-        _check(library().skb_mflow_last_stats(self._h, C.byref(s)))
-        return {k: getattr(s, k) for k, _ in FlowStats._fields_}
-
 
 DENSE_STRESSLET_PLUS_COMPLEMENTARY = 0
 DENSE_M_INV = 1
 
 
-class Dense:
+class Dense(_Handle):
     """The periphery's dense operators on the GPU (include/skelly_b200_dense.h): Periphery::matvec and
     Periphery::apply_preconditioner (periphery.cpp:21-47) as row-partitioned GEMVs."""
+    _destroy = "skb_dense_destroy"
 
     def __init__(self, n_gpus: int = 1, device_ids=None):
         self._h = C.c_void_p()
@@ -1772,23 +1535,6 @@ class Dense:
         else:
             _check(library().skb_dense_create(int(n_gpus), C.byref(self._h)))
         self.shape = {}
-
-    def close(self):
-        if getattr(self, "_h", None) and self._h.value:
-            library().skb_dense_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *a):
-        self.close()
 
     def set_matrix(self, op: int, A):
         A = np.ascontiguousarray(A, dtype=np.float64)
@@ -1810,14 +1556,14 @@ class Dense:
 
     def apply_device(self, op: int, d_x: int, d_v_add: int, d_y: int, stream: int = 0):
         """Single-device handle, operands already on its device (addresses as ints, 0 = NULL v_add); asynchronous."""
-        _check(library().skb_dense_apply_device(self._h, int(op), C.c_void_p(d_x), C.c_void_p(d_v_add) if d_v_add else None,
-                                                C.c_void_p(d_y), C.c_void_p(stream) if stream else None))
+        _check(library().skb_dense_apply_device(self._h, int(op), C.c_void_p(d_x), _vp(d_v_add), C.c_void_p(d_y),
+                                                _vp(stream)))
 
     def apply_background_device(self, op: int, d_x: int, d_y: int, stream: int = 0):
         """y = A x with the background row streamer (one small CTA per SM, TMA-fed): the form that can share the SMs
         with the pair kernels.  Single-device handle, device addresses as ints; asynchronous."""
         _check(library().skb_dense_apply_background_device(self._h, int(op), C.c_void_p(d_x), C.c_void_p(d_y),
-                                                           C.c_void_p(stream) if stream else None))
+                                                           _vp(stream)))
 
     def stats(self) -> dict:
         s = DenseStats()
