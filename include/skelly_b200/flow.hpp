@@ -101,6 +101,23 @@ template <class M> class FlowEngineT {
                                           body_radii.data(), eta),
               "skb_flow_set_listener_frame");
     }
+    /// the frame of the installed geometry and a step's solution x (tension: N_f values), as the reference's listener
+    /// unpacks a trajectory frame; leaves the fiber operators of the installed geometry resident, without their inverse
+    void set_listener_state(const std::vector<skb_fiber_params> &params, double dt, double eta,
+                            const std::vector<double> &tension, const std::vector<double> &x,
+                            const std::vector<int32_t> &body_kind, const M &body_radii, bool periphery_interaction) {
+        check(skb_flow_set_listener_state(st_->fl, params.data(), dt, eta, tension.data(), x.data(), body_kind.data(),
+                                          body_radii.data(), periphery_interaction ? 1 : 0),
+              "skb_flow_set_listener_state");
+    }
+    /// the same from d_tension and d_x on the flow's device, after the caller's work on `stream`
+    void set_listener_state_device(const std::vector<skb_fiber_params> &params, double dt, double eta,
+                                   const double *d_tension, const double *d_x, const std::vector<int32_t> &body_kind,
+                                   const M &body_radii, bool periphery_interaction, void *stream = nullptr) {
+        check(skb_flow_set_listener_state_device(st_->fl, params.data(), dt, eta, d_tension, d_x, body_kind.data(),
+                                                 body_radii.data(), periphery_interaction ? 1 : 0, stream),
+              "skb_flow_set_listener_state_device");
+    }
     /// System::velocity_at_targets on the frame, the body-interior replacement included
     M listener_velocity(const M &r_trg) const {
         M vel = M::Zero(3, r_trg.cols());

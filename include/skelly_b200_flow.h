@@ -84,6 +84,39 @@ SKB_API int skb_flow_set_listener_frame(skb_flow *fl, const double *fib_forces, 
                                         const double *body_densities, const double *body_forces_torques,
                                         const double *body_velocities, const int32_t *body_kind,
                                         const double *body_radii, double eta);
+/* The frame of the installed geometry and a step's solution, built on the device as the reference's listener unpacks a
+ * trajectory frame (trajectory_reader.cpp:150-249) and System::velocity_at_targets forms its strengths (system.cpp:
+ * 339-356):
+ *   fib_forces    = fc.apply_fiber_force([x; y; z; T]) per fiber, with x, y, z the flow's installed positions and T
+ *                   `tension` (N_f values, as skb_flow_step returns it) -- not the fiber block of the solution -- and
+ *                   force_operator_ built at those positions by skb_flow_build_fiber_operators(params, dt, eta);
+ *                   plus the fiber-periphery repulsion at the installed positions when periphery_interaction != 0
+ *                   (needs skb_flow_set_periphery_shape); no motor force;
+ *   body_forces_torques = the link forces and torques of calculate_link_conditions([x; y; z; T], x_bodies) at the
+ *                   links of skb_flow_set_fiber_links -- and no external forces or torques, as the reference computes
+ *                   calculate_external_forces_torques there and does not pass it to the body flow;
+ *   shell_density = the shell block of x; body_densities = the first 3 n_b entries of each body's block of x;
+ *   body_velocities = the last six entries of each body's block of x (SphericalBody::step's velocity_ and
+ *                   angular_velocity_).
+ * x is the whole solution vector as skb_flow_step returns it; only its shell and body blocks are read.  body_kind and
+ * body_radii are those of skb_flow_set_listener_frame.  The frame is the one skb_flow_set_listener_frame would hold for
+ * these strengths, with the same staleness and the same requests.  The call leaves A_, force_operator_ and xs_ of the
+ * installed geometry resident, built without their inverse: skb_flow_apply_fiber_preconditioner and the system calls
+ * that precondition refuse until the next skb_flow_build_fiber_operators (skb_flow_step builds its own).  It returns once the frame is complete; the _device form
+ * takes d_tension and d_x on the flow's device, waits for `stream` first and never moves them through the host.
+ * Refused (SKB_ERR_INVALID, before any launch): dt or eta not finite and > 0, a non-finite tension (host form), a bad
+ * body_kind or body_radii, NULL inputs of a non-empty block, a group member or a target window or ranges, fibers without
+ * their class derivatives or with bad params, bodies without operators, fibers and bodies without
+ * skb_flow_set_fiber_links for the current geometry, periphery_interaction with fiber nodes but no periphery shape.
+ * Any refusal or failure leaves no frame.  An empty block needs none of its set-up. */
+struct skb_fiber_params; /* below, with skb_flow_build_fiber_operators */
+SKB_API int skb_flow_set_listener_state(skb_flow *fl, const struct skb_fiber_params *params, double dt, double eta,
+                                        const double *tension, const double *x, const int32_t *body_kind,
+                                        const double *body_radii, int32_t periphery_interaction);
+SKB_API int skb_flow_set_listener_state_device(skb_flow *fl, const struct skb_fiber_params *params, double dt,
+                                               double eta,
+                                               const double *d_tension, const double *d_x, const int32_t *body_kind,
+                                               const double *body_radii, int32_t periphery_interaction, void *stream);
 /* System::velocity_at_targets (system.cpp:330-384) on the frame: skb_flow_velocity_at_targets's velocity, and at a
  * target inside a body (bodies in the library's order, the last match wins) the body's rigid motion U + omega x dx. */
 SKB_API int skb_flow_listener_velocity(skb_flow *fl, const double *r_trg, int64_t n_trg, double *vel);

@@ -177,6 +177,10 @@ def library() -> C.CDLL:
         "skb_flow_velocity_at_targets": ([ctxp, _dp, C.c_int64, _dp, _dp, _dp, _dp, C.c_double, _dp], C.c_int),
         "skb_flow_set_listener_frame": ([ctxp, _dp, _dp, _dp, _dp, _dp, C.POINTER(C.c_int32), _dp, C.c_double],
                                         C.c_int),
+        "skb_flow_set_listener_state": ([ctxp, C.POINTER(FiberParams), C.c_double, C.c_double, _dp, _dp,
+                                         C.POINTER(C.c_int32), _dp, C.c_int32], C.c_int),
+        "skb_flow_set_listener_state_device": ([ctxp, C.POINTER(FiberParams), C.c_double, C.c_double, C.c_void_p,
+                                                C.c_void_p, C.POINTER(C.c_int32), _dp, C.c_int32, C.c_void_p], C.c_int),
         "skb_flow_listener_velocity": ([ctxp, _dp, C.c_int64, _dp], C.c_int),
         "skb_flow_listener_lines": ([ctxp, C.c_int, _dp, C.c_int32, C.POINTER(LineRequest), _dp, _dp, _dp,
                                      C.POINTER(C.c_int32), C.POINTER(C.c_int32)], C.c_int),
@@ -1617,3 +1621,58 @@ def sym_plan_query(n_blocks, part=0, n_parts=1, num_sms=132):
     _check(library().skb_sym_plan_query(int(n_blocks), int(part), int(n_parts), int(num_sms), n.value, items,
                                         C.byref(n), rb))
     return [tuple(items[4 * i:4 * i + 4]) for i in range(n.value)], list(rb)
+
+
+def _state_args(flow, params, body_kind, body_radii):
+    p = fiber_params(flow._n_fibers(), *params)
+    kind = np.ascontiguousarray(np.zeros(0) if body_kind is None else body_kind, dtype=np.int32).reshape(-1)
+    radii = _arr(np.zeros((0, 3)) if body_radii is None else body_radii, 3)
+    if kind.shape != (flow.n_bodies,) or radii.shape[0] != flow.n_bodies:
+        raise ValueError(f"expected {flow.n_bodies} body kinds and radii, got {kind.shape} and {radii.shape}")
+    return p, kind, radii
+
+
+# The listener's frame of a step (skb_flow_set_listener_state), on a Flow only: the listener is single-device, and an
+# skb_mflow handle must never reach an skb_flow_ call.  Module functions taking the Flow rather than Flow methods:
+# Flow's public methods are pinned one by one by tests/test_capi_binding_cpu.py; these two are marshalled and checked
+# the same way in tests/test_listener_state_binding_cpu.py.
+def _listener_flow(flow):
+    if not isinstance(flow, Flow):
+        raise TypeError(f"the listener's frame needs a capi.Flow (one device), got {type(flow).__name__}")
+
+
+def set_listener_state(flow, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
+                       plus_hinged, dt, eta, tension, x, body_kind=None, body_radii=None, periphery_interaction=False):
+    """The listener's frame of `flow` (a Flow) from its installed geometry and a step's solution, as the reference's
+    listener unpacks a trajectory frame: the fiber forces of [positions; tension] with the operators built at the
+    installed positions (the fiber parameters of Flow.build_fiber_operators; the call leaves them resident without their
+    inverse, so the fiber preconditioner refuses until the next build), plus the
+    periphery repulsion when periphery_interaction; the bodies' link forces and torques (no external ones); the shell
+    and body densities and each body's [U, omega] from x (the step's whole solution vector).  tension (N_f,);
+    body_kind / body_radii as Flow.set_listener_frame.  Afterwards flow.velocity_field, .streamlines and .vortexlines
+    answer on that frame."""
+    _listener_flow(flow)
+    p, kind, radii = _state_args(flow, (length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
+                                        minus_clamped, plus_hinged), body_kind, body_radii)
+    t = np.ascontiguousarray(tension, dtype=np.float64).reshape(-1)
+    xs = np.ascontiguousarray(x, dtype=np.float64).reshape(-1)
+    if t.shape != (flow.n_fib,) or xs.shape != (flow.solution_size(),):
+        raise ValueError(f"expected {flow.n_fib} tensions and a solution of {flow.solution_size()}, got {t.shape} "
+                         f"and {xs.shape}")
+    _check(library().skb_flow_set_listener_state(flow._h, _params_ptr(p), float(dt), float(eta), _p(t), _p(xs),
+                                                 kind.ctypes.data_as(C.POINTER(C.c_int32)), _p(radii),
+                                                 int(bool(periphery_interaction))))
+
+
+def set_listener_state_device(flow, length_prev, bending_rigidity, radius, penalty_param, beta_tstep, minus_clamped,
+                              plus_hinged, dt, eta, d_tension: int, d_x: int, body_kind=None, body_radii=None,
+                              periphery_interaction=False, stream: int = 0):
+    """set_listener_state from device addresses (ints, e.g. torch.Tensor.data_ptr()) on the flow's device, after the
+    caller's work on `stream`; the solution never passes through the host."""
+    _listener_flow(flow)
+    p, kind, radii = _state_args(flow, (length_prev, bending_rigidity, radius, penalty_param, beta_tstep,
+                                        minus_clamped, plus_hinged), body_kind, body_radii)
+    _check(library().skb_flow_set_listener_state_device(flow._h, _params_ptr(p), float(dt), float(eta), _vp(d_tension),
+                                                        _vp(d_x), kind.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                        _p(radii), int(bool(periphery_interaction)),
+                                                        C.c_void_p(stream)))

@@ -17,15 +17,10 @@
 // K_ is never stored: K U = u + w x (x_i - c) and K^T lambda = [sum lambda_i ; sum (x_i - c) x lambda_i]
 // (update_K_matrix, body_spherical.cpp:74-86).
 #pragma once
+#include "skb_internal.hpp" // BodyItem
 #include <cuda_runtime.h>
 
 namespace skb {
-
-struct BodyItem {          // one body of the solution vector, in the order of skb_flow_set_bodies
-    long long node_off;    // first node among all body nodes
-    long long sol_off;     // first entry in x_bodies: [densities (3n) | U (3) | w (3)]
-    int n_nodes, pad;
-};
 
 struct LinkFiber {         // one fiber of the flow, in container order
     double s[3];           // nucleation site - body centre (body_container.cpp:209); unused for a free fiber

@@ -1,4 +1,5 @@
-// listener_kernels.cuh -- the listener's kernels (skb_listener.cu): the body-interior replacement of
+// listener_kernels.cuh -- the listener's kernels (skb_listener.cu): the frame of a step (the packing of
+// trajectory_reader.cpp:238-246 and the bodies' [U; omega]), the body-interior replacement of
 // System::velocity_at_targets (system.cpp:362-381) and the lockstep Cash-Karp 5(4) integration of many streamlines or
 // vortex lines (streamline.cpp with boost.odeint's integrate_adaptive / controlled_runge_kutta).
 //
@@ -6,11 +7,13 @@
 // the stage points of the active lines into one compacted target array (slot j of the last compaction is line
 // slots[j]), the flow evaluates them in one pass, and the next stage's kernel reads the velocities back by slot.
 #pragma once
+#include "skb_internal.hpp" // BodyItem
 #include <cuda_runtime.h>
 
 namespace skb {
 
 constexpr int kLineThreads = 128;
+constexpr int kStateThreads = 128;
 constexpr int kCompactThreads = 1024;
 constexpr int kLineMaxFails = 500;   // odeint's failed_step_checker
 constexpr double kVortexEps = 1e-7;  // get_vorticity_at_point (streamline.cpp:16-35)
@@ -49,6 +52,37 @@ __global__ void interior_replace_kernel(const double *__restrict__ trg, long lon
             vel[3 * i + 1] = __dadd_rn(p[8], __dsub_rn(__dmul_rn(w2, d0), __dmul_rn(w0, d2)));
             vel[3 * i + 2] = __dadd_rn(p[9], __dsub_rn(__dmul_rn(w0, d1), __dmul_rn(w1, d0)));
         }
+    }
+}
+
+// The frame of skb_flow_set_listener_state, one launch of n_fibers + n_bodies CTAs.  CTA f < n_fibers packs fiber f's
+// solution block [x; y; z; T] (4n, the layout fiber_gemv_kernel<1> and fiber_link_kernel read) from the installed
+// positions (3 per node) and the tension (1 per node), as trajectory_reader.cpp:238-246 fills sol_fibers from x_ and
+// tension_.  CTA n_fibers + b writes body b's [U; omega], the last six entries of its block of x_bodies
+// (SphericalBody::step, body_spherical.cpp:16-17), into its row of the rigid table.  Copies only: no rounding
+__global__ void __launch_bounds__(kStateThreads)
+    listener_state_kernel(const long long *__restrict__ fib_off, int n_fibers, const double *__restrict__ r_fib,
+                          const double *__restrict__ tension, double *__restrict__ x_fib,
+                          const BodyItem *__restrict__ bodies, const double *__restrict__ x_bodies,
+                          double *__restrict__ rigid) {
+    const int blk = blockIdx.x;
+    if (blk < n_fibers) {
+        const long long o = fib_off[blk];
+        const int n = (int)(fib_off[blk + 1] - o);
+        double *x = x_fib + 4 * o;
+        for (int i = threadIdx.x; i < n; i += kStateThreads) {
+            const double *r = r_fib + 3 * (o + i);
+            x[i] = r[0];
+            x[n + i] = r[1];
+            x[2 * n + i] = r[2];
+            x[3 * n + i] = tension[o + i];
+        }
+        return;
+    }
+    const int b = blk - n_fibers;
+    if (threadIdx.x < 6) {
+        const BodyItem it = bodies[b];
+        rigid[(size_t)b * kRigidStride + 7 + threadIdx.x] = x_bodies[it.sol_off + 3LL * it.n_nodes + threadIdx.x];
     }
 }
 

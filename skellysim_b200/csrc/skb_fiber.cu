@@ -273,7 +273,7 @@ static int check_params(const OwnFibers &own, const skb_fiber_params *params) {
 }
 
 int FiberOps::build(const OwnFibers &own, const skb_fiber_params *params, double dt, double eta, int *launches,
-                    const std::function<int(const Step &stage, const Step &launch)> &frame) {
+                    const std::function<int(const Step &stage, const Step &launch)> &frame, bool with_inverse) {
     ready_ = false;
     const int nfib = own.count();
     SKB_TRY(check_params(own, params));
@@ -283,7 +283,8 @@ int FiberOps::build(const OwnFibers &own, const skb_fiber_params *params, double
     const cudaStream_t st = own.stream;
     auto stage = [&]() -> int {
         SKB_TRY(upload_plan(own, b));
-        SKB_TRY(op_Ainv.ensure((size_t)b.offA * 8));
+        if (with_inverse)
+            SKB_TRY(op_Ainv.ensure((size_t)b.offA * 8));
         SKB_TRY(put_async(op_len, b.lp.data(), b.lp.size() * 8, st));
         SKB_TRY(put_async(op_plus, b.plus.data(), b.plus.size() * sizeof(int), st));
         SKB_TRY(put_async(bld_params, params, (size_t)nfib * sizeof(skb_fiber_params), st));
@@ -298,6 +299,8 @@ int FiberOps::build(const OwnFibers &own, const skb_fiber_params *params, double
                            (double *)op_F.ptr, (double *)op_xs.ptr};
         fiber_assemble_kernel<<<(unsigned)b.tiles.size(), kBuildThreads, b.smem, st>>>(ba);
         SKB_TRY(launched(launches));
+        if (!with_inverse)
+            return SKB_OK;
         size_t first = 0;
         for (const auto &kv : b.inv_by_n) {
             const int m = 4 * kv.first, cs = inverse_cluster_size(m);
@@ -334,7 +337,8 @@ int FiberOps::build(const OwnFibers &own, const skb_fiber_params *params, double
     if (nfib > 0)
         SKB_TRY(frame(stage, launch)); // (returns once the stream has drained: the plan's tables may go)
     commit(own, b);
-    precond_gen = ops_gen; // the inverse belongs to these operators
+    if (with_inverse)
+        precond_gen = ops_gen; // the inverse belongs to these operators
     return SKB_OK;
 }
 

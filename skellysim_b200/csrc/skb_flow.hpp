@@ -110,11 +110,18 @@ class Listener {
     int set_frame(skb_flow *fl, const double *fib_forces, const double *shell_density, const double *body_densities,
                   const double *body_forces_torques, const double *body_velocities, const int32_t *body_kind,
                   const double *body_radii, double eta);
+    // skb_flow_set_listener_state(_device): the frame of the installed geometry and a step's solution.  device: x and
+    // tension are device pointers whose writes the caller ordered on st
+    int set_state(skb_flow *fl, const ::skb_fiber_params *params, double dt, double eta, const double *tension,
+                  const double *x, const int32_t *body_kind, const double *body_radii, int periphery_interaction,
+                  bool device, cudaStream_t st);
     int velocity(skb_flow *fl, const double *r_trg, long long n_trg, double *vel);
     int lines(skb_flow *fl, int kind, const double *x0, int n_lines, const ::skb_line_request *req, double *x,
               double *t, double *val, int32_t *n_points, int32_t *status);
 
   private:
+    // the frame's buffers are written on the flow's stream: wait for them, then the frame is current
+    int commit(skb_flow *fl, int n_interior, double eta);
     // the refusal of a request without a current frame
     int current(const skb_flow *fl, const char *who) const;
     // System::velocity_at_targets of the frame at the n_trg device targets d_trg into d_v, on the flow's stream
@@ -125,6 +132,7 @@ class Listener {
     double eta_ = 0;
     int n_interior_ = 0; // bodies with an interior test
     DevBuf ff_, sd_, bd_, f_, t_, rigid_; // strengths; per body [kind, r0, r1, r2, cx, cy, cz, U, omega]
+    DevBuf xf_, sb_, ten_; // set_state: the packed [x; y; z; T] per fiber; the host form's shell and body blocks, tension
     DevBuf trg_, vel_;                     // targets and velocities of one evaluation
     // lines: state (SoA) and per-line output; slot -> line map and the active count of the last compaction
     DevBuf st_x_, st_t_, st_dt_, st_k_, st_int_, out_x_, out_t_, out_val_, slots_, n_act_;
@@ -373,6 +381,11 @@ struct StepCall {
 };
 
 // ---- the periphery's shape in the step (skb_periphery.cu) ----
+// an error naming `who` unless a periphery shape is set and fits the flow as it is
+int periphery_ready(const skb_flow *fl, const char *who);
+// d_ff += the repulsion of every fiber node at the current geometry (fc.periphery_force, system.cpp:340-341) on st;
+// refuses a non-finite repulsion.  After periphery_ready
+int periphery_add_repulsion(skb_flow *fl, const char *who, double *d_ff, cudaStream_t st, int *launches);
 // with a shape: the pass over the own fibers at the current geometry (the repulsion kept for
 // periphery_add_force, c.hinged filled); refuses a non-finite repulsion and a shape not set or sized for the flow.
 // Changes nothing the step's refusal would have to undo.  Without a shape: nothing

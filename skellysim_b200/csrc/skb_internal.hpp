@@ -181,6 +181,13 @@ struct StepItem {
     int bound;       // 1: repin to site
 };
 
+// one body of the solution vector, in the order of skb_flow_set_bodies (body_ops.cuh, listener_kernels.cuh)
+struct BodyItem {
+    long long node_off; // first node among all body nodes
+    long long sol_off;  // first entry in x_bodies: [densities (3n) | U (3) | w (3)]
+    int n_nodes, pad;
+};
+
 // A_, force_operator_, xs_ and A_^-1 of one set of own fibers, resident for the timestep, and the GEMVs over them.
 // The caller has checked its pointers for NULL and made the flow's device current.
 class FiberOps {
@@ -195,10 +202,11 @@ class FiberOps {
     int upload_inverse(const double *A_inv, cudaStream_t st);
     // the device build, checked and planned on the host first; `frame` runs stage (the table uploads), then launch
     // (assembly and inverse kernels, adding to *launches) and returns once own.stream has drained.  No own fibers:
-    // the empty set, without a frame
+    // the empty set, without a frame.  with_inverse false: A_, force_operator_ and xs_ only, and the preconditioner
+    // refuses (ready(who, true)) until a build with the inverse
     using Step = std::function<int()>;
     int build(const OwnFibers &own, const ::skb_fiber_params *params, double dt, double eta, int *launches,
-              const std::function<int(const Step &stage, const Step &launch)> &frame);
+              const std::function<int(const Step &stage, const Step &launch)> &frame, bool with_inverse = true);
     // the fiber block of the RHS into d_rhs (4 per own node) from d_v / d_f (3 per own node, either may be NULL),
     // checked on the host first; `frame` runs stage (the table uploads on own.stream), then launch.  Needs the class
     // matrices and derivatives, not the operators: its per-fiber tables are its own, and the resident operators, their
@@ -355,6 +363,7 @@ class BodyOps {
     // Over a member's own fibers the forces and torques are its partial sums
     int links(const FiberOps &ops, const double *d_length, const double *d_x_fib, const double *d_x_bodies,
               const double **d_link, cudaStream_t st, int *launches);
+    const BodyItem *items() const { return (const BodyItem *)items_.ptr; } // per body, on the device
     const double *densities() const { return (const double *)dens_.ptr; }
     const double *forces() const { return (const double *)force_.ptr; }
     const double *torques() const { return (const double *)torque_.ptr; }

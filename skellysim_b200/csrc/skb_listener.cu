@@ -1,4 +1,6 @@
-// skb_listener.cu -- the listener's requests on one frame (include/skelly_b200_flow.h, listener.cpp:86-136): the
+// skb_listener.cu -- the listener's frame and its requests (include/skelly_b200_flow.h, listener.cpp:86-136): the frame
+// from the caller's strengths (set_frame) or from the installed geometry and a step's solution (set_state, the unpacking
+// of trajectory_reader.cpp:150-249 and the strengths of System::velocity_at_targets, system.cpp:339-352); the
 // velocity field (System::velocity_at_targets with its body-interior replacement, system.cpp:330-384) and streamlines
 // and vortex lines (streamline.cpp), every line advanced at once (listener_kernels.cuh).  The velocity of every
 // evaluation is skb::velocity_dev, the sequence of skb_flow_velocity_at_targets, at device targets.
@@ -25,6 +27,7 @@ static int load_listener_kernels() {
         return SKB_OK;
     cudaFuncAttributes fa;
     CUDA_TRY(cudaFuncGetAttributes(&fa, interior_replace_kernel));
+    CUDA_TRY(cudaFuncGetAttributes(&fa, listener_state_kernel));
     CUDA_TRY(cudaFuncGetAttributes(&fa, line_init_kernel));
     CUDA_TRY(cudaFuncGetAttributes(&fa, line_compact_kernel));
     CUDA_TRY(cudaFuncGetAttributes(&fa, line_stage_kernel));
@@ -36,18 +39,14 @@ static int load_listener_kernels() {
 
 static unsigned blocks(long long n, int threads) { return (unsigned)((n + threads - 1) / threads); }
 
-int Listener::set_frame(skb_flow *fl, const double *fib_forces, const double *shell_density,
-                        const double *body_densities, const double *body_forces_torques, const double *body_velocities,
-                        const int32_t *body_kind, const double *body_radii, double eta) {
-    const char *who = "skb_flow_set_listener_frame";
-    if (!(eta > 0) || !std::isfinite(eta))
-        return set_error(SKB_ERR_INVALID, "%s: eta = %g (must be finite and > 0)", who, eta);
-    if ((fl->n_fib > 0 && !fib_forces) || (fl->n_shell > 0 && !shell_density) || (fl->n_body > 0 && !body_densities) ||
-        (fl->n_bodies > 0 && (!body_forces_torques || !body_velocities || !body_kind || !body_radii)))
-        return set_error(SKB_ERR_INVALID, "%s: NULL input for a non-empty class", who);
+// the rigid table (per body [kind, r0, r1, r2, cx, cy, cz, U, omega]) from the caller's interior tests and the body
+// centres, U and omega from body_velocities (6 per body) or zero (NULL: a later launch writes them); *n_interior: the
+// bodies with an interior test.  Refuses a bad kind or radius
+static int rigid_table(const skb_flow *fl, const char *who, const int32_t *body_kind, const double *body_radii,
+                       const double *body_velocities, std::vector<double> &rigid, int *n_interior) {
     const int nb = fl->n_bodies;
-    std::vector<double> rigid((size_t)nb * kRigidStride);
-    int n_interior = 0;
+    rigid.assign((size_t)nb * kRigidStride, 0.0);
+    *n_interior = 0;
     for (int b = 0; b < nb; ++b) {
         const int kind = body_kind[b];
         if (kind < 0 || kind > 2)
@@ -61,11 +60,40 @@ int Listener::set_frame(skb_flow *fl, const double *fib_forces, const double *sh
         for (int c = 0; c < 3; ++c) {
             p[1 + c] = body_radii[3 * b + c];
             p[4 + c] = fl->h_centers[3 * (size_t)b + c];
-            p[7 + c] = body_velocities[6 * (size_t)b + c];
-            p[10 + c] = body_velocities[6 * (size_t)b + 3 + c];
+            if (body_velocities) {
+                p[7 + c] = body_velocities[6 * (size_t)b + c];
+                p[10 + c] = body_velocities[6 * (size_t)b + 3 + c];
+            }
         }
-        n_interior += kind != 0;
+        *n_interior += kind != 0;
     }
+    return SKB_OK;
+}
+
+// the frame is complete on the flow's stream: it takes the flow's geometry version
+int Listener::commit(skb_flow *fl, int n_interior, double eta) {
+    CUDA_TRY(cudaStreamSynchronize(fl->stream));
+    SKB_TRY(load_listener_kernels());
+    n_interior_ = n_interior;
+    eta_ = eta;
+    version_ = fl->geom_version;
+    set_ = true;
+    return SKB_OK;
+}
+
+int Listener::set_frame(skb_flow *fl, const double *fib_forces, const double *shell_density,
+                        const double *body_densities, const double *body_forces_torques, const double *body_velocities,
+                        const int32_t *body_kind, const double *body_radii, double eta) {
+    const char *who = "skb_flow_set_listener_frame";
+    if (!(eta > 0) || !std::isfinite(eta))
+        return set_error(SKB_ERR_INVALID, "%s: eta = %g (must be finite and > 0)", who, eta);
+    if ((fl->n_fib > 0 && !fib_forces) || (fl->n_shell > 0 && !shell_density) || (fl->n_body > 0 && !body_densities) ||
+        (fl->n_bodies > 0 && (!body_forces_torques || !body_velocities || !body_kind || !body_radii)))
+        return set_error(SKB_ERR_INVALID, "%s: NULL input for a non-empty class", who);
+    const int nb = fl->n_bodies;
+    std::vector<double> rigid;
+    int n_interior = 0;
+    SKB_TRY(rigid_table(fl, who, body_kind, body_radii, body_velocities, rigid, &n_interior));
     CUDA_TRY(cudaSetDevice(fl->dev));
     set_ = false; // a failed upload leaves no frame
     std::vector<double> f, t;
@@ -77,13 +105,107 @@ int Listener::set_frame(skb_flow *fl, const double *fib_forces, const double *sh
     SKB_TRY(upload(fl, f_, f.data(), f.size()));
     SKB_TRY(upload(fl, t_, t.data(), t.size()));
     SKB_TRY(upload(fl, rigid_, rigid.data(), rigid.size()));
-    CUDA_TRY(cudaStreamSynchronize(fl->stream));
-    SKB_TRY(load_listener_kernels());
-    n_interior_ = n_interior;
-    eta_ = eta;
-    version_ = fl->geom_version;
-    set_ = true;
+    return commit(fl, n_interior, eta);
+}
+
+static int copy_async(DevBuf &dst, const double *src, size_t n_doubles, cudaStream_t st) {
+    if (n_doubles == 0)
+        return SKB_OK;
+    SKB_TRY(dst.ensure(n_doubles * 8));
+    CUDA_TRY(cudaMemcpyAsync(dst.ptr, src, n_doubles * 8, cudaMemcpyDeviceToDevice, st));
     return SKB_OK;
+}
+
+int Listener::set_state(skb_flow *fl, const skb_fiber_params *params, double dt, double eta, const double *tension,
+                        const double *x, const int32_t *body_kind, const double *body_radii, int periphery_interaction,
+                        bool device, cudaStream_t st) {
+    const char *who = device ? "skb_flow_set_listener_state_device" : "skb_flow_set_listener_state";
+    set_ = false; // a refused or failed call leaves no frame
+    if (fl->grp.member())
+        return set_error(SKB_ERR_INVALID, "%s: a group member's flow (the listener is single-device)", who);
+    if (!(dt > 0) || !std::isfinite(dt) || !(eta > 0) || !std::isfinite(eta))
+        return set_error(SKB_ERR_INVALID, "%s: dt = %g, eta = %g (both must be finite and > 0)", who, dt, eta);
+    const long long nf = fl->n_fib, ns = fl->n_shell;
+    const int nb = fl->n_bodies;
+    if ((fl->n_fibers > 0 && (!params || !tension)) || ((ns > 0 || nb > 0) && !x) ||
+        (nb > 0 && (!body_kind || !body_radii)))
+        return set_error(SKB_ERR_INVALID, "%s: NULL input for a non-empty class", who);
+    std::vector<double> rigid;
+    int n_interior = 0;
+    SKB_TRY(rigid_table(fl, who, body_kind, body_radii, nullptr, rigid, &n_interior));
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    SKB_TRY(whole_targets(fl, who, ""));
+    OwnFibers own;
+    SKB_TRY(own_fibers(fl, who, own));
+    SKB_TRY(fl->ops.check_step(own, params, nullptr, nullptr)); // the build's refusals: params, class derivatives
+    if (nb > 0 && !fl->bodies.has_operators())
+        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_body_operators (or skb_flow_set_body_frames and "
+                                          "skb_flow_place_bodies) after skb_flow_set_bodies", who);
+    if (nb > 0 && fl->n_fibers > 0 && !fl->bodies.has_links())
+        return set_error(SKB_ERR_INVALID, "%s: call skb_flow_set_fiber_links for the current geometry (NULL body: no "
+                                          "fiber is bound)", who);
+    if (periphery_interaction && nf > 0) // (the repulsion acts on fiber nodes only)
+        SKB_TRY(periphery_ready(fl, who));
+    for (long long i = 0; !device && i < nf; ++i)
+        if (!std::isfinite(tension[i]))
+            return set_error(SKB_ERR_INVALID, "%s: tension[%lld] = %g is not finite", who, i, tension[i]);
+    if (device)
+        CUDA_TRY(cudaStreamSynchronize(st)); // the caller's x and tension are complete
+    begin_stats(fl);
+    fl->cur = fl->stream;
+    const cudaStream_t fs = fl->stream;
+    // device_ms and total_ms both span the whole call on the flow's stream: elapsed stream time, the host waits after
+    // the build's stages and the periphery pass's flag read-back included -- not the kernels' time alone
+    CUDA_TRY(cudaEventRecord(fl->evt0, fs));
+    CUDA_TRY(cudaEventRecord(fl->ev0, fs));
+    // fc.update_cache_variables at the installed positions (trajectory_reader.cpp:248): force_operator_ and xs_ are
+    // all the frame reads, so the build leaves out the inverse (most of a full build's time)
+    SKB_TRY(fl->ops.build(
+        own, params, dt, eta, &fl->launches,
+        [&](const FiberOps::Step &stage, const FiberOps::Step &launch) -> int {
+            SKB_TRY(stage());
+            SKB_TRY(launch());
+            CUDA_TRY(cudaStreamSynchronize(fs));
+            return SKB_OK;
+        },
+        false));
+    // the solution's shell and body blocks and the tension on the device
+    const size_t n_sb = (size_t)(3 * ns + (nb > 0 ? fl->bodies.solution_size() : 0));
+    const double *d_tension = tension, *d_sb = x ? x + 4 * nf : nullptr;
+    if (!device) {
+        SKB_TRY(upload(fl, ten_, tension, (size_t)nf));
+        SKB_TRY(upload(fl, sb_, d_sb, n_sb));
+        d_tension = (const double *)ten_.ptr;
+        d_sb = (const double *)sb_.ptr;
+    }
+    const double *d_x_bodies = d_sb ? d_sb + 3 * ns : nullptr;
+    SKB_TRY(xf_.ensure((size_t)nf * 32 + 8));
+    SKB_TRY(ff_.ensure((size_t)nf * 24 + 8));
+    SKB_TRY(upload(fl, rigid_, rigid.data(), rigid.size()));
+    if (fl->n_fibers + nb > 0) {
+        listener_state_kernel<<<(unsigned)(fl->n_fibers + nb), kStateThreads, 0, fs>>>(
+            (const long long *)fl->fiber_offset.ptr, fl->n_fibers, (const double *)fl->r_fib.ptr, d_tension,
+            (double *)xf_.ptr, fl->bodies.items(), d_x_bodies, (double *)rigid_.ptr);
+        SKB_TRY(launched(fl, 1));
+    }
+    // f_on_fibers = fc.apply_fiber_force(sol_fibers) (+ fc.periphery_force(shell, fp))      system.cpp:339-341
+    SKB_TRY(fl->ops.force((const double *)xf_.ptr, (double *)ff_.ptr, fs, &fl->launches));
+    if (periphery_interaction && nf > 0)
+        SKB_TRY(periphery_add_repulsion(fl, who, (double *)ff_.ptr, fs, &fl->launches));
+    // calculate_link_conditions(sol_fibers, sol_bodies): the link forces and torques, and the densities   :349-350
+    if (nb > 0) {
+        const double *link = nullptr;
+        SKB_TRY(fl->bodies.links(fl->ops, (const double *)fl->fiber_length.ptr, (const double *)xf_.ptr, d_x_bodies,
+                                 &link, fs, &fl->launches));
+        SKB_TRY(copy_async(bd_, fl->bodies.densities(), (size_t)fl->n_body * 3, fs));
+        SKB_TRY(copy_async(f_, fl->bodies.forces(), (size_t)nb * 3, fs));
+        SKB_TRY(copy_async(t_, fl->bodies.torques(), (size_t)nb * 3, fs));
+    }
+    SKB_TRY(copy_async(sd_, d_sb, (size_t)ns * 3, fs));
+    CUDA_TRY(cudaEventRecord(fl->ev1, fs));
+    CUDA_TRY(cudaEventRecord(fl->evt1, fs));
+    SKB_TRY(commit(fl, n_interior, eta));
+    return finish_stats(fl);
 }
 
 int Listener::current(const skb_flow *fl, const char *who) const {
@@ -272,6 +394,24 @@ int skb_flow_set_listener_frame(skb_flow *fl, const double *fib_forces, const do
         return set_error(SKB_ERR_INVALID, "skb_flow_set_listener_frame: NULL flow");
     return fl->listener.set_frame(fl, fib_forces, shell_density, body_densities, body_forces_torques, body_velocities,
                                   body_kind, body_radii, eta);
+}
+
+int skb_flow_set_listener_state(skb_flow *fl, const skb_fiber_params *params, double dt, double eta,
+                                const double *tension, const double *x, const int32_t *body_kind,
+                                const double *body_radii, int32_t periphery_interaction) {
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "skb_flow_set_listener_state: NULL flow");
+    return fl->listener.set_state(fl, params, dt, eta, tension, x, body_kind, body_radii, periphery_interaction, false,
+                                  nullptr);
+}
+
+int skb_flow_set_listener_state_device(skb_flow *fl, const skb_fiber_params *params, double dt, double eta,
+                                       const double *d_tension, const double *d_x, const int32_t *body_kind,
+                                       const double *body_radii, int32_t periphery_interaction, void *stream) {
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "skb_flow_set_listener_state_device: NULL flow");
+    return fl->listener.set_state(fl, params, dt, eta, d_tension, d_x, body_kind, body_radii, periphery_interaction,
+                                  true, (cudaStream_t)stream);
 }
 
 int skb_flow_listener_velocity(skb_flow *fl, const double *r_trg, int64_t n_trg, double *vel) {

@@ -210,6 +210,23 @@ int skb::periphery_before_step(skb_flow *fl, const char *who, const StepArgs &a,
     return SKB_OK;
 }
 
+int skb::periphery_ready(const skb_flow *fl, const char *who) {
+    if (!fl->shape.active())
+        return set_error(SKB_ERR_INVALID, "%s: periphery_interaction needs skb_flow_set_periphery_shape", who);
+    return shape_fits(fl, who);
+}
+
+int skb::periphery_add_repulsion(skb_flow *fl, const char *who, double *d_ff, cudaStream_t st, int *launches) {
+    PeripheryShape &P = fl->shape;
+    SKB_TRY(P.run((const double *)fl->r_fib.ptr, (const long long *)fl->fiber_offset.ptr, 0, fl->n_fibers, true,
+                  nullptr, 0, st, launches));
+    for (int f = 0; f < fl->n_fibers; ++f)
+        if (P.flags()[f] & kPeriNonFinite)
+            return set_error(SKB_ERR_INVALID, "%s: a non-finite fiber-periphery force on fiber %d (a node at the "
+                                              "centre of the sphere)", who, f);
+    return P.add_force(d_ff, d_ff, 3 * fl->n_fib, st, launches);
+}
+
 int skb::periphery_add_force(skb_flow *fl, const double *d_f_external, long long m, double *d_out, cudaStream_t st,
                              int *launches) {
     return fl->shape.add_force(d_f_external, d_out, 3 * m, st, launches);

@@ -12,6 +12,11 @@ System::prep_state_for_solver does: Stepper.dynamic_instability removes, grows a
 set.  Its random stream is (seed, call counter): the counter advances on every attempt and a rejected step does not
 rewind it, as the reference's restore() does not rewind its generator.
 
+A run on the device can be observed on the device: `run` calls `observe(time, stepper, info)` after every accepted step,
+and Stepper.set_listener_state sets the flow's listener frame from the step it kept (the installed geometry, the step's
+solution and tension), so that the flow's velocity_field, streamlines and vortexlines answer on the state the step
+just installed, as the reference's listener does on a trajectory frame.
+
 One deviation from the reference's loop (DESIGN.md §5): the reference sets dt to the grown dt_new before it advances
 time on an accepted step (system.cpp:554-557), so time advances by a dt no step used.  Here time advances by the dt of
 the step that was accepted."""
@@ -35,6 +40,7 @@ class Stepper:
         self.v_growth, self.force_scale = v_growth, force_scale
         self.tol, self.num_blocks, self.max_iters = tol, num_blocks, max_iters
         self._backup = None
+        self.last = None  # (x, tension, dt) of the installed step: its solution vector, fiber tensions and timestep
         self.di, self.seed, self.counter = dynamic_instability, int(seed), 0
         if self.di is not None:
             n = flow._n_fibers()
@@ -91,13 +97,30 @@ class Stepper:
     def step(self, dt, f_external=None, body_forces_torques=None):
         """one System::step; returns the step's info (the solve's fields, fiber_error, worst_fiber; a NaN fiber_error:
         the solution was not finite and nothing was installed)"""
-        _, _, info = self.flow.step(*self.params, dt, self.eta, dense=self.dense, f_external=f_external,
+        x, tension, info = self.flow.step(*self.params, dt, self.eta, dense=self.dense, f_external=f_external,
                                     body_forces_torques=body_forces_torques, fiber_body=self.fiber_body,
                                     site_ref=self.site_ref, v_growth=self.v_growth, force_scale=self.force_scale,
                                     tol=self.tol, num_blocks=self.num_blocks, max_iters=self.max_iters)
+        # kept only for a step whose geometry is installed: the frame pairs that geometry with this solution
+        self.last = (x, tension, float(dt)) if np.isfinite(info["fiber_error"]) else None
         if self.di is not None and np.isfinite(info["fiber_error"]):
             self.plus_pinned = self.flow.step_flags()
         return info
+
+    def set_listener_state(self, body_kind=None, body_radii=None, periphery_interaction=False):
+        """The flow's listener frame from the last step (capi.set_listener_state): the installed geometry, the
+        step's solution and tension, the fiber parameters and dt it was taken with.  body_kind / body_radii as
+        Flow.set_listener_frame (None without bodies).  A capi.Flow only (the listener is single-device).  Refused
+        without an installed step: before the first step, after a step that was not installed, after restore()."""
+        if not isinstance(self.flow, capi.Flow):
+            raise TypeError(f"set_listener_state: the listener's frame needs a capi.Flow (one device), not a "
+                            f"{type(self.flow).__name__}")
+        if self.last is None:
+            raise RuntimeError("set_listener_state: no installed step (none was taken, the last one was not "
+                               "installed, or it was restored)")
+        x, tension, dt = self.last
+        capi.set_listener_state(self.flow, *self.params, dt, self.eta, tension, x, body_kind, body_radii,
+                                periphery_interaction)
 
     def backup(self):
         self._backup = (self.positions(), *self.placement())
@@ -109,6 +132,7 @@ class Stepper:
 
     def restore(self):
         r, c, q = self._backup
+        self.last = None  # the restored geometry is not the last step's
         if self.di is None:
             self.flow.set_fibers(r, np.diff(self.flow._fiber_off), self.flow._lengths)
         else:
@@ -124,7 +148,7 @@ class Stepper:
 
 
 def run(stepper, t_final, dt, adaptive=True, dt_min=1e-5, dt_max=np.inf, beta_up=1.2, beta_down=0.5,
-        fiber_error_tol=0.1, forces=None, collided=None, time=0.0):
+        fiber_error_tol=0.1, forces=None, collided=None, time=0.0, observe=None):
     """System::run's loop until time >= t_final.  Each step: backup, the dynamic instability (Stepper's model, if
     any), forces(time, r_fib) -> (f_external (N_f, 3),
     F_T (n_bodies, 6)), either None (no callable: no external forces), the step, then the acceptance:
@@ -133,7 +157,9 @@ def run(stepper, t_final, dt, adaptive=True, dt_min=1e-5, dt_max=np.inf, beta_up
       rejected with dt halved (system.cpp:542-546): collided(r_fib, centers) decides when given, else the step's
       info["collided"].  A dt below dt_min raises RuntimeError.
       not adaptive: every step is accepted, dt stays; a step that was not installed (NaN fiber_error) raises.
-    A rejected step is restored.  Returns (time, dt, log): log one (time, dt used, accepted, fiber_error) per step."""
+    A rejected step is restored.  observe(time, stepper, info), when given, is called after every accepted step with the
+    advanced time, while that step's geometry is installed (Stepper.set_listener_state then sets the listener's frame of
+    it); it changes nothing of the loop.  Returns (time, dt, log): log one (time, dt used, accepted, fiber_error) per step."""
     log = []
     while time < t_final:
         stepper.backup()
@@ -160,6 +186,8 @@ def run(stepper, t_final, dt, adaptive=True, dt_min=1e-5, dt_max=np.inf, beta_up
             raise RuntimeError(f"the step at time {time:g} was not finite and was not installed (dt = {dt:g})")
         if accept:
             time += dt
+            if observe is not None:
+                observe(time, stepper, info)
         else:
             stepper.restore()
         log.append((time, dt, accept, err))
