@@ -1,6 +1,6 @@
 // skb_body.cu -- the bodies' per-timestep operators and the fiber-body links of a flow (BodyOps, skb_internal.hpp): their
 // checks and uploads, and the launches of body_ops.cuh and of the body preconditioner's GEMV.  Knows nothing of skb_flow:
-// skb_matvec.cu hands it the geometry, the fibers and their operators.
+// skb_system.cu hands it the geometry, the fibers and their operators.
 #include "body_ops.cuh"
 #include "fiber_ops.cuh"
 #include "skb_internal.hpp"
@@ -11,21 +11,6 @@
 #include <vector>
 
 using namespace skb;
-
-static int launched(int *launches) {
-    CUDA_TRY(cudaGetLastError());
-    count_launch(1);
-    *launches += 1;
-    return SKB_OK;
-}
-
-static int put(DevBuf &b, const void *h, size_t bytes, cudaStream_t st) {
-    if (bytes == 0)
-        return SKB_OK;
-    SKB_TRY(b.ensure(bytes));
-    CUDA_TRY(cudaMemcpyAsync(b.ptr, h, bytes, cudaMemcpyHostToDevice, st));
-    return SKB_OK;
-}
 
 struct BodyOps::Plan {
     std::vector<BodyItem> items;
@@ -104,11 +89,11 @@ int BodyOps::plan(const char *who, const int *n_nodes, int n_bodies, long long n
 // the geometry and the tables of a plan, and the per-matvec buffers; on st, not synchronised
 int BodyOps::upload_layout(const Plan &pl, const double *r_body, const double *centers, const double *node_weights,
                            cudaStream_t st) {
-    SKB_TRY(put(items_, pl.items.data(), pl.items.size() * sizeof(BodyItem), st));
-    SKB_TRY(put(r_, r_body, (size_t)pl.nodes * 24, st));
-    SKB_TRY(put(centers_, centers, (size_t)pl.n_bodies * 24, st));
-    SKB_TRY(put(weights_, node_weights, (size_t)pl.nodes * 8, st));
-    SKB_TRY(put(gemv_items_, pl.gemv.data(), pl.gemv.size() * sizeof(FiberGemvItem), st));
+    SKB_TRY(items_.upload(pl.items.data(), pl.items.size() * sizeof(BodyItem), st));
+    SKB_TRY(r_.upload(r_body, (size_t)pl.nodes * 24, st));
+    SKB_TRY(centers_.upload(centers, (size_t)pl.n_bodies * 24, st));
+    SKB_TRY(weights_.upload(node_weights, (size_t)pl.nodes * 8, st));
+    SKB_TRY(gemv_items_.upload(pl.gemv.data(), pl.gemv.size() * sizeof(FiberGemvItem), st));
     SKB_TRY(dens_.ensure((size_t)pl.nodes * 24 + 8));
     SKB_TRY(force_.ensure((size_t)pl.n_bodies * 24 + 8));
     return torque_.ensure((size_t)pl.n_bodies * 24 + 8);
@@ -147,9 +132,9 @@ int BodyOps::set_operators(const int *n_nodes, int n_bodies, long long n_body_no
                  hi, pl));
     ops_set_ = inv_set_ = false;
     SKB_TRY(upload_layout(pl, r_body, centers, node_weights, st));
-    SKB_TRY(put(ex_, ex, (size_t)pl.nodes * 24, st));
-    SKB_TRY(put(ey_, ey, (size_t)pl.nodes * 24, st));
-    SKB_TRY(put(ez_, ez, (size_t)pl.nodes * 24, st));
+    SKB_TRY(ex_.upload(ex, (size_t)pl.nodes * 24, st));
+    SKB_TRY(ey_.upload(ey, (size_t)pl.nodes * 24, st));
+    SKB_TRY(ez_.upload(ez, (size_t)pl.nodes * 24, st));
     if (A_inv && pl.inv_own > 0) {
         SKB_TRY(a_inv_.ensure((size_t)pl.inv_own * 8));
         SKB_TRY(upload_pageable(a_inv_.ptr, A_inv + pl.inv_first, (size_t)pl.inv_own * 8, st));
@@ -170,15 +155,15 @@ int BodyOps::set_frames(const int *n_nodes, int n_bodies, long long n_body_nodes
     const size_t nodes = (size_t)pl.nodes;
     ops_set_ = inv_set_ = frames_set_ = false;
     // every buffer place writes, at its final size (place allocates nothing)
-    SKB_TRY(put(ex0_, ex0, nodes * 24, st));
-    SKB_TRY(put(ey0_, ey0, nodes * 24, st));
-    SKB_TRY(put(ez0_, ez0, nodes * 24, st));
-    SKB_TRY(put(place_items_, pl.place.data(), pl.place.size() * sizeof(PlaceBody), st));
+    SKB_TRY(ex0_.upload(ex0, nodes * 24, st));
+    SKB_TRY(ey0_.upload(ey0, nodes * 24, st));
+    SKB_TRY(ez0_.upload(ez0, nodes * 24, st));
+    SKB_TRY(place_items_.upload(pl.place.data(), pl.place.size() * sizeof(PlaceBody), st));
     SKB_TRY(rot_.ensure((size_t)n_bodies * 72 + 8));
     SKB_TRY(items_.ensure(pl.items.size() * sizeof(BodyItem) + 8));
     SKB_TRY(r_.ensure(nodes * 24 + 8));
     SKB_TRY(centers_.ensure((size_t)n_bodies * 24 + 8));
-    SKB_TRY(put(weights_, node_weights, nodes * 8, st));
+    SKB_TRY(weights_.upload(node_weights, nodes * 8, st));
     SKB_TRY(gemv_items_.ensure(pl.gemv.size() * sizeof(FiberGemvItem) + 8));
     SKB_TRY(ex_.ensure(nodes * 24 + 8));
     SKB_TRY(ey_.ensure(nodes * 24 + 8));
@@ -232,7 +217,7 @@ int BodyOps::place(const double *R, const double *r_body, const double *centers,
     ops_set_ = inv_set_ = false;
     // within the capacities set_frames gave (buffers only grow): nothing is allocated
     SKB_TRY(upload_layout(pl, r_body, centers, frame_w_.data(), st));
-    SKB_TRY(put(rot_, R, (size_t)pl.n_bodies * 72, st));
+    SKB_TRY(rot_.upload(R, (size_t)pl.n_bodies * 72, st));
     const int n_inv_ctas = frame_inv_ ? place_ctas_ : 0;
     if (n_inv_ctas + pl.n_bodies > 0) {
         body_place_kernel<<<(unsigned)(n_inv_ctas + pl.n_bodies), kPlaceThreads, 0, st>>>(
@@ -300,9 +285,9 @@ int BodyOps::set_links(const OwnFibers &own, const FiberOps &ops, int n_bodies, 
             csr_fib[(size_t)fill[(size_t)lf[(size_t)f].body]++] = f;
     links_set_ = false;
     if (any) {
-        SKB_TRY(put(link_fibers_, lf.data(), lf.size() * sizeof(LinkFiber), st));
-        SKB_TRY(put(csr_begin_, count.data(), count.size() * sizeof(int), st));
-        SKB_TRY(put(csr_fib_, csr_fib.data(), csr_fib.size() * sizeof(int), st));
+        SKB_TRY(link_fibers_.upload(lf.data(), lf.size() * sizeof(LinkFiber), st));
+        SKB_TRY(csr_begin_.upload(count.data(), count.size() * sizeof(int), st));
+        SKB_TRY(csr_fib_.upload(csr_fib.data(), csr_fib.size() * sizeof(int), st));
         SKB_TRY(link_.ensure((size_t)nfib * 56));
         SKB_TRY(contrib_.ensure((size_t)nfib * 48));
         CUDA_TRY(cudaStreamSynchronize(st)); // the host tables above go out of scope

@@ -1,7 +1,8 @@
 // skb_fiber.cu -- the per-fiber dense operators of a flow (FiberOps, skb_internal.hpp): the class matrices and their one
 // device table, the plan of the own fibers, the caller's operators and inverse or their device build (fiber_build.cuh),
 // the launches of fiber_gemv_kernel (fiber_ops.cuh), and the fiber block of the RHS (fiber_rhs.cuh) with per-fiber
-// tables of its own.  Knows nothing of skb_flow: skb_matvec.cu hands it the own fibers.
+// tables of its own.  Knows nothing of skb_flow: the fiber operators' entry points in skb_system.cu hand it the own
+// fibers.
 #include "fiber_build.cuh"
 #include "fiber_ops.cuh"
 #include "fiber_rhs.cuh"
@@ -32,13 +33,6 @@ struct FiberOps::Plan {
     size_t smem = 0;
 };
 
-static int launched(int *launches) {
-    CUDA_TRY(cudaGetLastError());
-    count_launch(1);
-    *launches += 1;
-    return SKB_OK;
-}
-
 // per line k < lines: first / one-past-last t < len with m[k * ks + t * ts] != 0, (0, 0) for a zero line
 static void nonzero_ranges(const double *m, int lines, size_t ks, int len, size_t ts, std::vector<int2> &out) {
     for (int k = 0; k < lines; ++k) {
@@ -50,12 +44,6 @@ static void nonzero_ranges(const double *m, int lines, size_t ks, int len, size_
             }
         out.push_back(t1 > t0 ? make_int2(t0, t1) : make_int2(0, 0));
     }
-}
-
-static int put_async(DevBuf &b, const void *h, size_t bytes, cudaStream_t st) {
-    SKB_TRY(b.ensure(bytes));
-    CUDA_TRY(cudaMemcpyAsync(b.ptr, h, bytes, cudaMemcpyHostToDevice, st));
-    return SKB_OK;
 }
 
 int FiberOps::set_class(int n_nodes, const double *D_1_0, const double *P_downsample_bc, cudaStream_t st) {
@@ -105,8 +93,8 @@ int FiberOps::upload_classes(cudaStream_t st) {
         nonzero_ranges(kv.second.D.data(), nn, nn, nn, 1, ranges);
     }
     CUDA_TRY(cudaDeviceSynchronize()); // the GEMVs, the build and the RHS may still read the table, on any stream
-    SKB_TRY(put_async(class_mats, mats.data(), mats.size() * 8, st));
-    SKB_TRY(put_async(class_ranges, ranges.data(), ranges.size() * sizeof(int2), st));
+    SKB_TRY(class_mats.upload(mats.data(), mats.size() * 8, st));
+    SKB_TRY(class_ranges.upload(ranges.data(), ranges.size() * sizeof(int2), st));
     CUDA_TRY(cudaStreamSynchronize(st)); // complete before any later launch, on any stream
     return SKB_OK;
 }
@@ -200,11 +188,11 @@ int FiberOps::upload_plan(const OwnFibers &own, const Plan &pl) {
     SKB_TRY(op_A.ensure((size_t)pl.offA * 8));
     SKB_TRY(op_F.ensure((size_t)pl.offF * 8));
     SKB_TRY(op_xs.ensure((size_t)own.nodes() * 24));
-    SKB_TRY(put_async(op_classD, pl.cD.data(), pl.cD.size() * 8, st));
-    SKB_TRY(put_async(op_classP, pl.cP.data(), pl.cP.size() * 8, st));
-    SKB_TRY(put_async(op_classR, pl.cR.data(), pl.cR.size() * 8, st));
-    SKB_TRY(put_async(items_A, pl.itA.data(), pl.itA.size() * sizeof(FiberGemvItem), st));
-    SKB_TRY(put_async(items_F, pl.itF.data(), pl.itF.size() * sizeof(FiberGemvItem), st));
+    SKB_TRY(op_classD.upload(pl.cD.data(), pl.cD.size() * 8, st));
+    SKB_TRY(op_classP.upload(pl.cP.data(), pl.cP.size() * 8, st));
+    SKB_TRY(op_classR.upload(pl.cR.data(), pl.cR.size() * 8, st));
+    SKB_TRY(items_A.upload(pl.itA.data(), pl.itA.size() * sizeof(FiberGemvItem), st));
+    SKB_TRY(items_F.upload(pl.itF.data(), pl.itF.size() * sizeof(FiberGemvItem), st));
     return SKB_OK;
 }
 
@@ -237,8 +225,8 @@ int FiberOps::upload(const OwnFibers &own, const double *A, const double *force_
     SKB_TRY(upload_pageable(op_A.ptr, A, (size_t)pl.offA * 8, own.stream));
     SKB_TRY(upload_pageable(op_F.ptr, force_operator, (size_t)pl.offF * 8, own.stream));
     CUDA_TRY(cudaMemcpyAsync(op_xs.ptr, xs, (size_t)own.nodes() * 24, cudaMemcpyHostToDevice, own.stream));
-    SKB_TRY(put_async(op_len, length_prev, (size_t)nfib * 8, own.stream));
-    SKB_TRY(put_async(op_plus, plus_bc_velocity, (size_t)nfib * sizeof(int), own.stream));
+    SKB_TRY(op_len.upload(length_prev, (size_t)nfib * 8, own.stream));
+    SKB_TRY(op_plus.upload(plus_bc_velocity, (size_t)nfib * sizeof(int), own.stream));
     CUDA_TRY(cudaStreamSynchronize(own.stream)); // the host vectors above go out of scope
     commit(own, pl);
     return SKB_OK;
@@ -285,12 +273,12 @@ int FiberOps::build(const OwnFibers &own, const skb_fiber_params *params, double
         SKB_TRY(upload_plan(own, b));
         if (with_inverse)
             SKB_TRY(op_Ainv.ensure((size_t)b.offA * 8));
-        SKB_TRY(put_async(op_len, b.lp.data(), b.lp.size() * 8, st));
-        SKB_TRY(put_async(op_plus, b.plus.data(), b.plus.size() * sizeof(int), st));
-        SKB_TRY(put_async(bld_params, params, (size_t)nfib * sizeof(skb_fiber_params), st));
-        SKB_TRY(put_async(bld_items, b.items.data(), b.items.size() * sizeof(FiberItem), st));
-        SKB_TRY(put_async(bld_tiles, b.tiles.data(), b.tiles.size() * sizeof(FiberTileItem), st));
-        return put_async(bld_inv, b.inv_off.data(), b.inv_off.size() * sizeof(long long), st);
+        SKB_TRY(op_len.upload(b.lp.data(), b.lp.size() * 8, st));
+        SKB_TRY(op_plus.upload(b.plus.data(), b.plus.size() * sizeof(int), st));
+        SKB_TRY(bld_params.upload(params, (size_t)nfib * sizeof(skb_fiber_params), st));
+        SKB_TRY(bld_items.upload(b.items.data(), b.items.size() * sizeof(FiberItem), st));
+        SKB_TRY(bld_tiles.upload(b.tiles.data(), b.tiles.size() * sizeof(FiberTileItem), st));
+        return bld_inv.upload(b.inv_off.data(), b.inv_off.size() * sizeof(long long), st);
     };
     auto launch = [&]() -> int {
         const BuildArgs ba{(const FiberItem *)bld_items.ptr, (const FiberTileItem *)bld_tiles.ptr,
@@ -367,9 +355,9 @@ int FiberOps::rhs(const OwnFibers &own, const skb_fiber_params *params, const do
     auto stage = [&]() -> int {
         if (rhs_pending) // the previous call's kernel, on whichever stream, still reads these tables
             CUDA_TRY(cudaStreamWaitEvent(st, rhs_done, 0));
-        SKB_TRY(put_async(rhs_items, items.data(), items.size() * sizeof(FiberItem), st));
-        SKB_TRY(put_async(rhs_params, params, (size_t)nfib * sizeof(skb_fiber_params), st));
-        return put_async(rhs_growth, growth.data(), growth.size() * sizeof(double2), st);
+        SKB_TRY(rhs_items.upload(items.data(), items.size() * sizeof(FiberItem), st));
+        SKB_TRY(rhs_params.upload(params, (size_t)nfib * sizeof(skb_fiber_params), st));
+        return rhs_growth.upload(growth.data(), growth.size() * sizeof(double2), st);
     };
     auto launch = [&]() -> int {
         const RhsArgs ra{(const FiberItem *)rhs_items.ptr, (const FiberParamsDev *)rhs_params.ptr,

@@ -1,7 +1,8 @@
 // skb_flow.hpp -- the flow (include/skelly_b200_flow.h) and what the translation units built on it share:
-// skb_matvec.cu (its lifetime, geometry, flows and matvec orchestration), skb_system.cu (the whole-system calls),
-// skb_listener.cu (the listener's requests),
-// skb_solve.cu, skb_step.cu, skb_periphery.cu and skb_mflow.cu.  Free functions in namespace skb that take the flow.
+// skb_flow.cu (its lifetime, geometry, knobs and statistics), skb_matvec.cu (its flows and matvec orchestration),
+// skb_system.cu (the whole-system calls and the fiber operators' entry points), skb_listener.cu (the listener's
+// requests), skb_solve.cu, skb_step.cu, skb_periphery.cu and skb_mflow.cu.  Free functions in namespace skb that take
+// the flow.
 #pragma once
 #include "skb_internal.hpp"
 #include "../../include/skelly_b200_flow.h"
@@ -253,12 +254,45 @@ inline OwnFibers all_fibers(const skb_flow *fl) {
                      (const double *)fl->fiber_length.ptr, fl->stream};
 }
 
-// ---- skb_matvec.cu ----
-// resolve the target window / ranges into fiber, shell and body pieces and (re)build the matvec target lists
-int prepare_matvec_targets(skb_flow *fl);
+// ---- skb_flow.cu ----
 // The fibers whose operators are resident: those whose rows are in this flow's target list -- all of them, or the
 // rank's own fibers under skb_flow_set_target_ranges / an aligned skb_flow_set_target_window.
 int own_fibers(skb_flow *fl, const char *who, OwnFibers &own);
+int upload(skb_flow *fl, DevBuf &buf, const double *h, size_t n_doubles);
+int download(skb_flow *fl, double *h, const DevBuf &buf, size_t n_doubles);
+void begin_stats(skb_flow *fl);
+int finish_stats(skb_flow *fl);
+// the device-pointer entry points run asynchronously on the caller's stream: no timings
+int device_stats(skb_flow *fl);
+
+// frame of the host-pointer entry points on fl->stream: device_ms spans the device work, total_ms also the uploads
+// before it and the downloads after it; returns once the downloads have landed
+template <class Up, class Work, class Down> int host_frame(skb_flow *fl, Up up, Work work, Down down) {
+    fl->cur = fl->stream;
+    CUDA_TRY(cudaEventRecord(fl->evt0, fl->stream));
+    SKB_TRY(up());
+    CUDA_TRY(cudaEventRecord(fl->ev0, fl->stream));
+    SKB_TRY(work());
+    CUDA_TRY(cudaEventRecord(fl->ev1, fl->stream));
+    SKB_TRY(down());
+    CUDA_TRY(cudaEventRecord(fl->evt1, fl->stream));
+    return finish_stats(fl);
+}
+// the step of host_frame that has nothing to do
+inline int nothing() { return SKB_OK; }
+// frame of the device-pointer entry points: work on the caller's stream, then the statistics of no timing
+template <class Work> int device_frame(skb_flow *fl, void *stream, Work work) {
+    fl->cur = (cudaStream_t)stream;
+    SKB_TRY(work());
+    return device_stats(fl);
+}
+
+// ---- skb_matvec.cu ----
+// resolve the target window / ranges into fiber, shell and body pieces and (re)build the matvec target lists
+int prepare_matvec_targets(skb_flow *fl);
+// skb_flow_set_fibers' device part, once the fibers' offsets, lengths and positions are on the device: the self term's
+// shared-memory limit for fibers of fl->max_fiber_nodes nodes, and the trapezoid weights of both fiber source sets
+int install_fiber_sources(skb_flow *fl);
 // the background streamer's buffers for n_rows own periphery rows
 int overlap_buffers(skb_flow *fl, long long n_rows);
 // device-side matvec flow on fl->cur, as fl->plan says: d_ff / d_sd are the strengths of the own fibers / periphery
@@ -284,26 +318,6 @@ int add_sources(skb_flow *fl, const double *d_trg, long long n_trg, double eta, 
 int velocity_dev(skb_flow *fl, const double *d_trg, long long n_trg, const double *d_ff, const double *d_sd,
                  const double *d_bd, const double *d_f, const double *d_t, double eta, double *d_v);
 int load_source_kernels(); // the kernels of add_sources, loaded now
-int upload(skb_flow *fl, DevBuf &buf, const double *h, size_t n_doubles);
-int download(skb_flow *fl, double *h, const DevBuf &buf, size_t n_doubles);
-void begin_stats(skb_flow *fl);
-int finish_stats(skb_flow *fl);
-// the device-pointer entry points run asynchronously on the caller's stream: no timings
-int device_stats(skb_flow *fl);
-
-// frame of the host-pointer entry points on fl->stream: device_ms spans the device work, total_ms also the uploads
-// before it and the downloads after it; returns once the downloads have landed
-template <class Up, class Work, class Down> int host_frame(skb_flow *fl, Up up, Work work, Down down) {
-    fl->cur = fl->stream;
-    CUDA_TRY(cudaEventRecord(fl->evt0, fl->stream));
-    SKB_TRY(up());
-    CUDA_TRY(cudaEventRecord(fl->ev0, fl->stream));
-    SKB_TRY(work());
-    CUDA_TRY(cudaEventRecord(fl->ev1, fl->stream));
-    SKB_TRY(down());
-    CUDA_TRY(cudaEventRecord(fl->evt1, fl->stream));
-    return finish_stats(fl);
-}
 
 // ---- skb_system.cu: the whole-system calls ----
 // the whole solution vector's size (of every member alike)

@@ -1,6 +1,7 @@
 // skb_group.cu -- one member of a multi-GPU group of flows (Group, skb_internal.hpp): its window, the window's set-up
 // and exchange with the other members (CUDA IPC or peer access), and the steps of one matvec's protocol -- push, flag
-// barriers, pull -- over the kernels of group_kernels.cuh.  Knows nothing of skb_flow: skb_matvec.cu runs the steps.
+// barriers, pull -- over the kernels of group_kernels.cuh.  Knows nothing of skb_flow: skb_flow.cu sets it up,
+// skb_matvec.cu runs the steps.
 #include "group_kernels.cuh"
 #include "skb_internal.hpp"
 #include "../../include/skelly_b200_flow.h"
@@ -12,13 +13,6 @@ using namespace skb;
 
 // a flag wait that outlasts this gives up and records the missing rank in the error word (~10 s at 2 GHz)
 static constexpr unsigned long long kFlagTimeoutCycles = 20ULL * 1000 * 1000 * 1000;
-
-static int launched(int *launches) {
-    CUDA_TRY(cudaGetLastError());
-    count_launch(1);
-    *launches += 1;
-    return SKB_OK;
-}
 
 int Group::init(int rank, int size, long long n_fib, long long n_pad_fib, long long n_shell, long long n_pad_shell,
                 long long n_body, int n_bodies, int n_fibers) {

@@ -45,6 +45,8 @@ struct DevBuf {
             cudaFree(ptr);
     }
     int ensure(size_t bytes); // grow-only; contents are NOT preserved
+    // ensure(bytes), then the host bytes h copied in on st (asynchronously); nothing at all for 0 bytes
+    int upload(const void *h, size_t bytes, cudaStream_t st);
 };
 static_assert(!std::is_copy_constructible<DevBuf>::value && !std::is_copy_assignable<DevBuf>::value,
               "a copy would free the buffer twice");
@@ -104,6 +106,14 @@ int set_error(int code, const char *fmt, ...) __attribute__((format(printf, 2, 3
 const char *last_error();
 void count_launch(int n);
 long long launch_count();
+// after n kernel launches: their launch error, else count them globally and in the statistics `launches` of the
+// call in flight
+inline int launched(int *launches, int n = 1) {
+    CUDA_TRY(cudaGetLastError());
+    count_launch(n);
+    *launches += n;
+    return SKB_OK;
+}
 
 // Large host -> device copy from PAGEABLE caller memory (per-timestep operator uploads, hundreds of MB): the bytes are
 // moved into pinned staging buffers by several host threads while the previous chunk is on the PCIe bus, instead of

@@ -14,13 +14,6 @@
 
 using namespace skb;
 
-static int launched(skb_flow *fl, int n) {
-    CUDA_TRY(cudaGetLastError());
-    count_launch(n);
-    fl->launches += n;
-    return SKB_OK;
-}
-
 static int load_listener_kernels() {
     static bool loaded = false;
     if (loaded)
@@ -186,7 +179,7 @@ int Listener::set_state(skb_flow *fl, const skb_fiber_params *params, double dt,
         listener_state_kernel<<<(unsigned)(fl->n_fibers + nb), kStateThreads, 0, fs>>>(
             (const long long *)fl->fiber_offset.ptr, fl->n_fibers, (const double *)fl->r_fib.ptr, d_tension,
             (double *)xf_.ptr, fl->bodies.items(), d_x_bodies, (double *)rigid_.ptr);
-        SKB_TRY(launched(fl, 1));
+        SKB_TRY(launched(&fl->launches));
     }
     // f_on_fibers = fc.apply_fiber_force(sol_fibers) (+ fc.periphery_force(shell, fp))      system.cpp:339-341
     SKB_TRY(fl->ops.force((const double *)xf_.ptr, (double *)ff_.ptr, fs, &fl->launches));
@@ -234,7 +227,7 @@ int Listener::eval(skb_flow *fl, const double *d_trg, long long n_trg, double *d
         return SKB_OK;
     interior_replace_kernel<<<blocks(n_trg, kLineThreads), kLineThreads, 0, fl->cur>>>(
         d_trg, n_trg, (const double *)rigid_.ptr, fl->n_bodies, d_v);
-    return launched(fl, 1);
+    return launched(&fl->launches);
 }
 
 int Listener::velocity(skb_flow *fl, const double *r_trg, long long n_trg, double *vel) {
@@ -322,11 +315,11 @@ int Listener::lines(skb_flow *fl, int kind, const double *x0, int n_lines, const
     auto work = [&]() -> int {
         line_init_kernel<<<blocks(L, kLineThreads), kLineThreads, 0, fl->stream>>>(s, d_trg, n_lines, req->dt_init,
                                                                                     req->back_integrate != 0);
-        SKB_TRY(launched(fl, 1));
+        SKB_TRY(launched(&fl->launches));
         for (;;) {
             line_compact_kernel<<<1, kCompactThreads, 0, fl->stream>>>(s.status, L, (int *)slots_.ptr,
                                                                        (int *)n_act_.ptr);
-            SKB_TRY(launched(fl, 1));
+            SKB_TRY(launched(&fl->launches));
             CUDA_TRY(cudaMemcpyAsync(h_n, n_act_.ptr, sizeof(int), cudaMemcpyDeviceToHost, fl->stream));
             CUDA_TRY(cudaStreamSynchronize(fl->stream));
             const int n_act = *h_n;
@@ -335,11 +328,11 @@ int Listener::lines(skb_flow *fl, int kind, const double *x0, int n_lines, const
             for (int stage = 1; stage <= 6; ++stage) {
                 line_stage_kernel<<<blocks(n_act, kLineThreads), kLineThreads, 0, fl->stream>>>(s, p, stage, n_act,
                                                                                                  d_vel, (double *)d_trg);
-                SKB_TRY(launched(fl, 1));
+                SKB_TRY(launched(&fl->launches));
                 SKB_TRY(eval(fl, d_trg, (long long)n_act * line_points(vortex), d_vel));
             }
             line_control_kernel<<<blocks(n_act, kLineThreads), kLineThreads, 0, fl->stream>>>(s, p, n_act, d_vel);
-            SKB_TRY(launched(fl, 1));
+            SKB_TRY(launched(&fl->launches));
         }
     };
     // the counts and exits, then the used part of every line's output in one strided copy per array

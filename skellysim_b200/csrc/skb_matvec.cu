@@ -1,7 +1,9 @@
-// skb_matvec.cu -- device-resident flow() layer (include/skelly_b200_flow.h): FiberContainer / Periphery /
-// BodyContainer flows of SkellySim and their fused sum, the hydrodynamic part of System::apply_matvec
-// (src/core/system.cpp:284-316).  Built on the pair-kernel contexts of skb_runtime.cu; everything between the
-// upload of the strengths and the download of the velocities stays on the device.
+// skb_matvec.cu -- the evaluations and the matvec of a flow (include/skelly_b200_flow.h): the FiberContainer /
+// Periphery / BodyContainer flows of SkellySim at arbitrary targets, the point sources and the background flow, their
+// sum at arbitrary targets (System::velocity_at_targets) with the CUDA-graph replay of small calls, the matvec target
+// lists and matvec_core -- the hydrodynamic part of System::apply_matvec (src/core/system.cpp:284-316) -- and
+// apply_matvec_core around it.  Built on the pair-kernel contexts of skb_runtime.cu; everything between the upload of
+// the strengths and the download of the velocities stays on the device.  The flow object itself is skb_flow.cu.
 #include "aux_kernels.cuh"
 #include "skb_flow.hpp"
 
@@ -9,7 +11,6 @@
 #include <cstdint>
 #include <cstdlib>
 #include <cstring>
-#include <memory>
 #include <vector>
 
 using namespace skb;
@@ -19,21 +20,6 @@ namespace {
 constexpr double kReg = 5e-3;
 constexpr double kEps = 1e-5;
 } // namespace
-
-static int create_ctx(int dev, CtxPtr &slot) {
-    skb_ctx *ctx = nullptr;
-    const int rc = skb_ctx_create_on(&dev, 1, &ctx);
-    slot.reset(ctx);
-    return rc;
-}
-
-// every kernel launch of this file: check it, count it globally and in the statistics of the call in flight
-static int launched(skb_flow *fl, int n) {
-    CUDA_TRY(cudaGetLastError());
-    count_launch(n);
-    fl->launches += n;
-    return SKB_OK;
-}
 
 // self term of the fibers (fcfd.cpp:203-210): d_vel rows [0, node_end - node_begin) are the fiber nodes
 // [node_begin, node_end), the packed strengths are those of ctx's last Stokeslet evaluation
@@ -46,7 +32,25 @@ static int fiber_self_term(skb_flow *fl, skb_ctx *ctx, double eta, double *d_vel
     fiber_self_subtract_kernel<<<fl->n_fibers, 128, smem, fl->cur>>>(
         (const double *)fl->r_fib.ptr, s.f_cur, (const long long *)fl->fiber_offset.ptr, 1.0 / (8.0 * M_PI * eta),
         kReg * kReg, kEps, d_vel, node_begin, node_end);
-    return launched(fl, 1);
+    return launched(&fl->launches);
+}
+
+int skb::install_fiber_sources(skb_flow *fl) {
+    const int max_n = fl->max_fiber_nodes, n_fibers = fl->n_fibers;
+    if (max_n * 48 > 48 * 1024)
+        CUDA_TRY(cudaFuncSetAttribute(fiber_self_subtract_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      max_n * 48));
+    // trapezoid weights straight into both Stokeslet source sets
+    for (int k = 0; k < 2; ++k) {
+        SourceSet &s = fl->fib[k]->devs[0].src[SKB_STOKESLET];
+        SKB_TRY(s.weights.ensure((size_t)fl->n_fib * 8));
+        fiber_weights_kernel<<<n_fibers, 64, 0, fl->stream>>>((const long long *)fl->fiber_offset.ptr,
+                                                              (const double *)fl->fiber_length.ptr, n_fibers,
+                                                              (double *)s.weights.ptr);
+        SKB_TRY(launched(&fl->launches));
+        s.has_weights = true;
+    }
+    return SKB_OK;
 }
 
 // ---- device-side flows: ctx already has its targets and sources ------------------------------------------------
@@ -114,7 +118,7 @@ static int bodies_dev(skb_flow *fl, skb_ctx *ctx, const double *d_density, const
         (const double *)fl->centers.ptr, d_torque, fl->n_bodies, (const double *)d.r_trg.ptr, d.n_trg,
         1.0 / (8.0 * M_PI * eta), kReg * kReg, kEps * kEps, d_vel);
     fl->pairs += (fl->n_body + 2 * (long long)fl->n_bodies) * d.n_trg;
-    return launched(fl, 1);
+    return launched(&fl->launches);
 }
 
 int skb::add_sources(skb_flow *fl, const double *d_trg, long long n_trg, double eta, double *d_v, cudaStream_t st) {
@@ -129,13 +133,13 @@ int skb::add_sources(skb_flow *fl, const double *d_trg, long long n_trg, double 
         rotlet_add_kernel<<<nblk, bs, 0, st>>>((const double *)fl->pt_pos.ptr, (const double *)fl->pt_torque.ptr,
                                                fl->n_points, d_trg, n_trg, 1.0 / (8.0 * M_PI * eta), kReg * kReg,
                                                kEps * kEps, d_v);
-        SKB_TRY(launched(fl, 2));
+        SKB_TRY(launched(&fl->launches, 2));
     }
     if (fl->has_background) {
         background_add_kernel<<<nblk, bs, 0, st>>>(d_trg, n_trg, fl->bg_comp[0], fl->bg_comp[1], fl->bg_comp[2],
                                                    fl->bg_scale[0], fl->bg_scale[1], fl->bg_scale[2],
                                                    fl->bg_uniform[0], fl->bg_uniform[1], fl->bg_uniform[2], d_v);
-        SKB_TRY(launched(fl, 1));
+        SKB_TRY(launched(&fl->launches));
     }
     return SKB_OK;
 }
@@ -158,18 +162,6 @@ int skb::load_source_kernels() {
     return SKB_OK;
 }
 
-int skb::upload(skb_flow *fl, DevBuf &buf, const double *h, size_t n_doubles) {
-    if (n_doubles == 0)
-        return SKB_OK;
-    SKB_TRY(buf.ensure(n_doubles * 8));
-    CUDA_TRY(cudaMemcpyAsync(buf.ptr, h, n_doubles * 8, cudaMemcpyHostToDevice, fl->stream));
-    return SKB_OK;
-}
-int skb::download(skb_flow *fl, double *h, const DevBuf &buf, size_t n_doubles) {
-    if (n_doubles > 0)
-        CUDA_TRY(cudaMemcpyAsync(h, buf.ptr, n_doubles * 8, cudaMemcpyDeviceToHost, fl->stream));
-    return SKB_OK;
-}
 
 static int set_targets_cached(skb_ctx *ctx, TargetCache &tc, const double *r_trg, long long n_trg) {
     if (tc.same(r_trg, n_trg) && ctx->n_trg == n_trg)
@@ -292,187 +284,7 @@ template <class Body> static int run_graphed(skb_flow *fl, skb_flow::GraphSlot &
     return body();
 }
 
-void skb::begin_stats(skb_flow *fl) {
-    fl->launches = 0;
-    fl->pairs = 0;
-}
-int skb::finish_stats(skb_flow *fl) {
-    CUDA_TRY(cudaStreamSynchronize(fl->stream));
-    float a = 0, b = 0;
-    cudaEventElapsedTime(&a, fl->ev0, fl->ev1);
-    cudaEventElapsedTime(&b, fl->evt0, fl->evt1);
-    fl->stats.device_ms = a;
-    fl->stats.total_ms = b;
-    fl->stats.n_pairs = fl->pairs;
-    fl->stats.launches = fl->launches;
-    return SKB_OK;
-}
-
-static int nothing() { return SKB_OK; }
-
-int skb::device_stats(skb_flow *fl) {
-    fl->stats.device_ms = fl->stats.total_ms = 0;
-    fl->stats.n_pairs = fl->pairs;
-    fl->stats.launches = fl->launches;
-    return SKB_OK;
-}
-
-// frame of the fiber operators' GEMV entry points: the operators' check (`inverse`: with their inverse), nothing to do
-// without own fibers, the arguments, then call(nodes of the own fibers) on the flow's device
-template <class Call> static int fiber_ops_call(skb_flow *fl, const char *who, bool inverse, bool args, Call call) {
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    SKB_TRY(fl->ops.ready(who, inverse));
-    begin_stats(fl);
-    if (fl->ops.empty())
-        return SKB_OK;
-    if (!args)
-        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    return call((size_t)(fl->fb - fl->fa));
-}
-
 extern "C" {
-
-int skb_flow_create(int device, skb_flow **out) {
-    if (!out)
-        return set_error(SKB_ERR_INVALID, "skb_flow_create: out == NULL");
-    *out = nullptr;
-    int n_dev = 0;
-    if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev == 0)
-        return set_error(SKB_ERR_NO_DEVICE, "no CUDA device available; this library has no CPU fallback");
-    if (device < 0 || device >= n_dev)
-        return set_error(SKB_ERR_INVALID, "skb_flow_create: device %d out of range (%d visible)", device, n_dev);
-    std::unique_ptr<skb_flow> fl(new skb_flow);
-    fl->dev = device;
-    CUDA_TRY(cudaSetDevice(device));
-    CUDA_TRY(cudaStreamCreateWithFlags(fl->stream.out(), cudaStreamNonBlocking));
-    CUDA_TRY(cudaEventCreate(fl->ev0.out()));
-    CUDA_TRY(cudaEventCreate(fl->ev1.out()));
-    CUDA_TRY(cudaEventCreate(fl->evt0.out()));
-    CUDA_TRY(cudaEventCreate(fl->evt1.out()));
-    if (const char *e = getenv("SKB_GRAPHS"))
-        fl->graphs_enabled = atoi(e) != 0;
-    if (const char *e = getenv("SKB_OVERLAP")) // A/B switch of skb_flow_set_overlap's default
-        fl->bg.enabled = atoi(e) != 0;
-    for (int k = 0; k < 2; ++k) {
-        SKB_TRY(create_ctx(device, fl->fib[k]));
-        SKB_TRY(create_ctx(device, fl->shell[k]));
-        SKB_TRY(create_ctx(device, fl->body[k]));
-    }
-    // empty classes until set_* is called
-    for (int k = 0; k < 2; ++k) {
-        SKB_TRY(skb_set_sources(fl->fib[k].get(), SKB_STOKESLET, nullptr, 0));
-        SKB_TRY(skb_set_sources(fl->shell[k].get(), SKB_STRESSLET, nullptr, 0));
-        SKB_TRY(skb_set_sources(fl->body[k].get(), SKB_STRESSLET, nullptr, 0));
-        SKB_TRY(skb_set_sources(fl->body[k].get(), SKB_STOKESLET, nullptr, 0));
-    }
-    *out = fl.release();
-    return SKB_OK;
-}
-
-int skb_flow_destroy(skb_flow *fl) {
-    if (!fl)
-        return SKB_OK;
-    cudaSetDevice(fl->dev);
-    cudaStreamSynchronize(fl->stream);
-    delete fl;
-    return SKB_OK;
-}
-
-int skb_flow_set_fibers(skb_flow *fl, const double *r_fib, const int *n_nodes, const double *length, int n_fibers) {
-    if (!fl || n_fibers < 0 || (n_fibers > 0 && (!r_fib || !n_nodes || !length)))
-        return set_error(SKB_ERR_INVALID, "skb_flow_set_fibers: bad arguments");
-    std::vector<long long> off((size_t)n_fibers + 1, 0);
-    int max_n = 0;
-    for (int f = 0; f < n_fibers; ++f) {
-        if (n_nodes[f] < 2)
-            return set_error(SKB_ERR_INVALID, "fiber %d has %d nodes (need >= 2)", f, n_nodes[f]);
-        off[f + 1] = off[f] + n_nodes[f];
-        max_n = std::max(max_n, n_nodes[f]);
-    }
-    if ((size_t)max_n * 48 > 200 * 1024)
-        return set_error(SKB_ERR_INVALID, "fiber with %d nodes exceeds the shared-memory self-term kernel", max_n);
-    fl->n_fibers = n_fibers;
-    fl->n_fib = off[n_fibers];
-    fl->max_fiber_nodes = max_n;
-    fl->h_r_fib.assign(r_fib, r_fib + 3 * fl->n_fib);
-    fl->h_fiber_n.assign(n_nodes, n_nodes + n_fibers);
-    fl->h_fiber_len.assign(length, length + n_fibers);
-    fl->h_fiber_off = off;
-    fl->ops.invalidate(); // operators belong to one set of fibers
-    fl->bodies.drop_links(); // ... and so do the links
-    fl->mv_dirty = true;
-    fl->geom_version++;
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    for (int k = 0; k < 2; ++k)
-        SKB_TRY(skb_set_sources(fl->fib[k].get(), SKB_STOKESLET, r_fib, fl->n_fib));
-    if (n_fibers == 0)
-        return SKB_OK;
-    SKB_TRY(fl->fiber_offset.ensure(off.size() * 8));
-    SKB_TRY(fl->fiber_length.ensure((size_t)n_fibers * 8));
-    SKB_TRY(fl->r_fib.ensure((size_t)fl->n_fib * 24));
-    CUDA_TRY(cudaMemcpyAsync(fl->fiber_offset.ptr, off.data(), off.size() * 8, cudaMemcpyHostToDevice, fl->stream));
-    CUDA_TRY(cudaMemcpyAsync(fl->fiber_length.ptr, length, (size_t)n_fibers * 8, cudaMemcpyHostToDevice, fl->stream));
-    CUDA_TRY(cudaMemcpyAsync(fl->r_fib.ptr, r_fib, (size_t)fl->n_fib * 24, cudaMemcpyHostToDevice, fl->stream));
-    if (max_n * 48 > 48 * 1024)
-        CUDA_TRY(cudaFuncSetAttribute(fiber_self_subtract_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      max_n * 48));
-    // trapezoid weights straight into both Stokeslet source sets
-    for (int k = 0; k < 2; ++k) {
-        SourceSet &s = fl->fib[k]->devs[0].src[SKB_STOKESLET];
-        SKB_TRY(s.weights.ensure((size_t)fl->n_fib * 8));
-        fiber_weights_kernel<<<n_fibers, 64, 0, fl->stream>>>((const long long *)fl->fiber_offset.ptr,
-                                                              (const double *)fl->fiber_length.ptr, n_fibers,
-                                                              (double *)s.weights.ptr);
-        SKB_TRY(launched(fl, 1));
-        s.has_weights = true;
-    }
-    CUDA_TRY(cudaStreamSynchronize(fl->stream));
-    return SKB_OK;
-}
-
-int skb_flow_set_periphery(skb_flow *fl, const double *node_pos, const double *node_normal, int64_t n_nodes) {
-    if (!fl || n_nodes < 0 || (n_nodes > 0 && (!node_pos || !node_normal)))
-        return set_error(SKB_ERR_INVALID, "skb_flow_set_periphery: bad arguments");
-    fl->n_shell = n_nodes;
-    fl->h_r_shell.assign(node_pos, node_pos + 3 * n_nodes);
-    fl->mv_dirty = true;
-    fl->geom_version++;
-    for (int k = 0; k < 2; ++k) {
-        SKB_TRY(skb_set_sources(fl->shell[k].get(), SKB_STRESSLET, node_pos, n_nodes));
-        SKB_TRY(skb_set_source_normals(fl->shell[k].get(), node_normal, n_nodes));
-    }
-    return SKB_OK;
-}
-
-int skb_flow_set_bodies(skb_flow *fl, const double *node_pos, const double *node_normal, int64_t n_nodes,
-                        const double *centers, int n_bodies) {
-    if (!fl || n_nodes < 0 || n_bodies < 0 || (n_nodes > 0 && (!node_pos || !node_normal)) ||
-        (n_bodies > 0 && !centers) || (n_bodies == 0 && n_nodes > 0))
-        return set_error(SKB_ERR_INVALID, "skb_flow_set_bodies: bad arguments");
-    fl->n_body = n_nodes;
-    fl->n_bodies = n_bodies;
-    fl->h_r_body.assign(node_pos, node_pos + 3 * n_nodes);
-    fl->h_centers.assign(centers, centers + 3 * (size_t)n_bodies);
-    fl->placed = false; // skb_flow_place_bodies sets it again after this call
-    fl->bodies.drop_operators(); // the bodies' operators and the nucleation sites belong to one placement
-    fl->bodies.drop_links();
-    fl->mv_dirty = true;
-    fl->geom_version++;
-    for (int k = 0; k < 2; ++k) {
-        SKB_TRY(skb_set_sources(fl->body[k].get(), SKB_STRESSLET, node_pos, n_nodes));
-        SKB_TRY(skb_set_source_normals(fl->body[k].get(), node_normal, n_nodes));
-        SKB_TRY(skb_set_sources(fl->body[k].get(), SKB_STOKESLET, centers, n_bodies));
-    }
-    if (n_bodies > 0) {
-        CUDA_TRY(cudaSetDevice(fl->dev));
-        SKB_TRY(fl->centers.ensure((size_t)n_bodies * 24));
-        CUDA_TRY(cudaMemcpyAsync(fl->centers.ptr, centers, (size_t)n_bodies * 24, cudaMemcpyHostToDevice, fl->stream));
-        CUDA_TRY(cudaStreamSynchronize(fl->stream));
-    }
-    return SKB_OK;
-}
 
 int skb_flow_fibers(skb_flow *fl, const double *r_trg, int64_t n_trg, const double *fib_forces, double eta,
                     int subtract_self, double *vel) {
@@ -545,43 +357,6 @@ int skb_flow_bodies(skb_flow *fl, const double *r_trg, int64_t n_trg, const doub
         [&] { return download(fl, vel, fl->vel, (size_t)n_trg * 3); });
 }
 
-int skb_flow_set_point_sources(skb_flow *fl, const double *positions, const double *forces, const double *torques,
-                               int n_points) {
-    if (!fl || n_points < 0 || (n_points > 0 && (!positions || !forces || !torques)))
-        return set_error(SKB_ERR_INVALID, "skb_flow_set_point_sources: bad arguments");
-    fl->n_points = n_points;
-    fl->geom_version++;
-    if (n_points == 0)
-        return SKB_OK;
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    SKB_TRY(fl->pt_pos.ensure((size_t)n_points * 24));
-    SKB_TRY(fl->pt_force.ensure((size_t)n_points * 24));
-    SKB_TRY(fl->pt_torque.ensure((size_t)n_points * 24));
-    CUDA_TRY(cudaMemcpyAsync(fl->pt_pos.ptr, positions, (size_t)n_points * 24, cudaMemcpyHostToDevice, fl->stream));
-    CUDA_TRY(cudaMemcpyAsync(fl->pt_force.ptr, forces, (size_t)n_points * 24, cudaMemcpyHostToDevice, fl->stream));
-    CUDA_TRY(cudaMemcpyAsync(fl->pt_torque.ptr, torques, (size_t)n_points * 24, cudaMemcpyHostToDevice, fl->stream));
-    CUDA_TRY(cudaStreamSynchronize(fl->stream));
-    return SKB_OK;
-}
-
-int skb_flow_set_background(skb_flow *fl, const int *components, const double *scale_factor, const double *uniform) {
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "skb_flow_set_background: NULL");
-    fl->geom_version++;
-    if (!components || !scale_factor || !uniform) {
-        fl->has_background = false;
-        return SKB_OK;
-    }
-    for (int j = 0; j < 3; ++j) {
-        if (components[j] < 0 || components[j] > 2)
-            return set_error(SKB_ERR_INVALID, "skb_flow_set_background: components must be 0, 1 or 2");
-        fl->bg_comp[j] = components[j];
-        fl->bg_scale[j] = scale_factor[j];
-        fl->bg_uniform[j] = uniform[j];
-    }
-    fl->has_background = true;
-    return SKB_OK;
-}
 
 int skb_flow_velocity_at_targets(skb_flow *fl, const double *r_trg, int64_t n_trg, const double *fib_forces,
                                  const double *shell_density, const double *body_densities,
@@ -850,12 +625,12 @@ static int periphery_rows(skb_flow *fl, StrengthMode mode, const double *sd, dou
         CUDA_TRY(cudaMemcpyAsync(d_v, d_tmp, (size_t)n_fr * 24, cudaMemcpyDeviceToDevice, fl->cur));
     } else if (n_fr > 0) {
         add_inplace_kernel<<<(unsigned)((3 * n_fr + bs - 1) / bs), bs, 0, fl->cur>>>(d_v, d_tmp, 3 * n_fr);
-        SKB_TRY(launched(fl, 1));
+        SKB_TRY(launched(&fl->launches));
     }
     if (n_bw > 0) {
         add_inplace_kernel<<<(unsigned)((3 * n_bw + bs - 1) / bs), bs, 0, fl->cur>>>(d_v + 3 * (n_fw + n_sw),
                                                                                   d_tmp + 3 * n_fr, 3 * n_bw);
-        SKB_TRY(launched(fl, 1));
+        SKB_TRY(launched(&fl->launches));
     }
     return SKB_OK;
 }
@@ -925,151 +700,6 @@ int skb::matvec_core(skb_flow *fl, const double *d_ff, const double *d_sd, const
 }
 
 extern "C" {
-
-// ---- group membership (multi-GPU through peer memory, skb_group.cu) ----------------------------------------------
-int skb_flow_group_init(skb_flow *fl, int rank, int size) {
-    if (!fl || size < 1 || size > kMaxGroup || rank < 0 || rank >= size)
-        return set_error(SKB_ERR_INVALID, "skb_flow_group_init: need 0 <= rank < size <= %d", kMaxGroup);
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    CUDA_TRY(cudaStreamSynchronize(fl->stream));
-    fl->mv_dirty = true;
-    fl->ops.invalidate();
-    fl->geom_version++;
-    // the same padded sizes the evaluator contexts use (set_sources_impl): the window replaces their f_packed
-    const long long n_pad_fib = fl->n_fib > 0 ? fl->fib[1]->devs[0].src[SKB_STOKESLET].n_pad : 0;
-    const long long n_pad_shell = fl->n_shell > 0 ? fl->shell[1]->devs[0].src[SKB_STRESSLET].n_pad : 0;
-    return fl->grp.init(rank, size, fl->n_fib, n_pad_fib, fl->n_shell, n_pad_shell, fl->n_body, fl->n_bodies,
-                        fl->n_fibers);
-}
-
-int skb_flow_group_export(skb_flow *fl, void *handle) {
-    if (!fl || !handle || !fl->grp.has_window())
-        return set_error(SKB_ERR_INVALID, "skb_flow_group_export: no group window (skb_flow_group_init with size > 1 first)");
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    return fl->grp.export_handle(handle);
-}
-
-int skb_flow_group_import(skb_flow *fl, int peer_rank, const void *handle) {
-    if (!fl || !handle || !fl->grp.has_window() || peer_rank < 0 || peer_rank >= fl->grp.size() ||
-        peer_rank == fl->grp.rank())
-        return set_error(SKB_ERR_INVALID, "skb_flow_group_import: bad arguments");
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    return fl->grp.import_handle(peer_rank, handle);
-}
-
-int skb_flow_group_connect(skb_flow *fl, int peer_rank, skb_flow *peer) {
-    if (!fl || !peer || !fl->grp.has_window() || !peer->grp.has_window() || peer_rank < 0 ||
-        peer_rank >= fl->grp.size() || peer_rank == fl->grp.rank() || peer->grp.rank() != peer_rank ||
-        peer->grp.size() != fl->grp.size())
-        return set_error(SKB_ERR_INVALID, "skb_flow_group_connect: bad arguments");
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    return fl->grp.connect(peer_rank, peer->grp, fl->dev, peer->dev);
-}
-
-// One matvec of this member alone (no flags, own window only, zero strengths): every buffer of the path reaches its
-// steady-state size, so that no cudaMalloc / cudaFree -- which synchronise the whole DEVICE -- happens later while a
-// peer on the same device sits in a flag wait.  Needed when members share a GPU; harmless otherwise.
-int skb_flow_group_warmup(skb_flow *fl) {
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "skb_flow_group_warmup: NULL flow");
-    if (!fl->grp.member())
-        return SKB_OK;
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    SKB_TRY(prepare_matvec_targets(fl));
-    const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
-    DevBuf z;
-    const size_t n_z = (size_t)std::max<long long>({4 * n_fw, 3 * n_sw, 3 * fl->n_body, 3LL * fl->n_bodies, 1LL});
-    SKB_TRY(z.ensure(n_z * 8));
-    CUDA_TRY(cudaMemsetAsync(z.ptr, 0, n_z * 8, fl->stream));
-    SKB_TRY(fl->vel.ensure((size_t)fl->n_win * 24 + 8));
-    SKB_TRY(fl->in_fib.ensure((size_t)n_fw * 24 + 8));
-    if (n_sw > 0 && fl->bg.enabled)
-        SKB_TRY(overlap_buffers(fl, 3 * n_sw));
-    fl->cur = fl->stream;
-    fl->grp.set_solo(true);
-    const double *zp = (const double *)z.ptr;
-    int rc = matvec_core(fl, zp, zp, zp, zp, zp, 1.0, (double *)fl->vel.ptr);
-    fl->grp.set_solo(false);
-    cudaError_t e = cudaStreamSynchronize(fl->stream);
-    fl->grp.restart();
-    if (rc != SKB_OK)
-        return rc;
-    if (e != cudaSuccess)
-        return set_error(SKB_ERR_CUDA, "skb_flow_group_warmup: %s", cudaGetErrorString(e));
-    return SKB_OK;
-}
-
-// Profiling aid: evaluate this member's share ALONE from now on (no flags, own window only) -- the per-rank device time
-// of an n-way group on one GPU.  Results are the member's partial view, not the group's.
-int skb_flow_group_set_solo(skb_flow *fl, int solo) {
-    if (!fl || !fl->grp.member())
-        return set_error(SKB_ERR_INVALID, "skb_flow_group_set_solo: not a group member");
-    fl->grp.set_solo(solo != 0);
-    return SKB_OK;
-}
-
-int skb_flow_group_error(skb_flow *fl, int *missing_peer) {
-    if (!fl || !missing_peer)
-        return set_error(SKB_ERR_INVALID, "skb_flow_group_error: NULL");
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    return fl->grp.missing_peer(missing_peer);
-}
-
-int skb_flow_set_cross(skb_flow *fl, int mode) {
-    if (!fl || mode < -1 || mode > 1)
-        return set_error(SKB_ERR_INVALID, "skb_flow_set_cross: mode must be -1 (auto), 0 (off) or 1 (on)");
-    fl->cross_mode = mode;
-    fl->mv_dirty = true;
-    fl->geom_version++;
-    return SKB_OK;
-}
-
-int skb_flow_set_overlap(skb_flow *fl, int on) {
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "skb_flow_set_overlap: NULL flow");
-    fl->bg.enabled = on != 0;
-    return SKB_OK;
-}
-
-int skb_flow_set_self_exclusion(skb_flow *fl, int fused) {
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "skb_flow_set_self_exclusion: NULL flow");
-    fl->self_excl = fused != 0;
-    fl->mv_dirty = true;
-    fl->geom_version++;
-    return SKB_OK;
-}
-
-int skb_flow_set_target_window(skb_flow *fl, int64_t begin, int64_t end) {
-    if (!fl || begin < 0 || (end >= 0 && end < begin))
-        return set_error(SKB_ERR_INVALID, "skb_flow_set_target_window: bad window [%lld, %lld)", (long long)begin,
-                         (long long)end);
-    fl->win_begin = begin;
-    fl->win_end = end;
-    fl->use_ranges = false;
-    fl->mv_dirty = true;
-    fl->ops.invalidate(); // resident fiber operators belong to one set of fiber rows
-    fl->geom_version++;
-    return SKB_OK;
-}
-
-int skb_flow_set_target_ranges(skb_flow *fl, int fiber_begin, int fiber_end, int64_t shell_begin, int64_t shell_end,
-                               int64_t body_begin, int64_t body_end) {
-    if (!fl || fiber_begin < 0 || fiber_end < fiber_begin || shell_begin < 0 || shell_end < shell_begin ||
-        body_begin < 0 || body_end < body_begin)
-        return set_error(SKB_ERR_INVALID, "skb_flow_set_target_ranges: bad ranges");
-    fl->rq_f0 = fiber_begin;
-    fl->rq_f1 = fiber_end;
-    fl->rq_s0 = shell_begin;
-    fl->rq_s1 = shell_end;
-    fl->rq_b0 = body_begin;
-    fl->rq_b1 = body_end;
-    fl->use_ranges = true;
-    fl->mv_dirty = true;
-    fl->ops.invalidate();
-    fl->geom_version++;
-    return SKB_OK;
-}
 
 int skb_flow_matvec(skb_flow *fl, const double *fib_forces, const double *shell_density, const double *body_densities,
                     const double *body_forces_torques, double eta, double *v_all) {
@@ -1141,224 +771,9 @@ int skb_flow_matvec_device(skb_flow *fl, const double *d_fib_forces, const doubl
     SKB_TRY(prepare_matvec_targets(fl));
     if (fl->n_win > 0 && !d_v_window)
         return set_error(SKB_ERR_INVALID, "skb_flow_matvec_device: NULL output");
-    fl->cur = (cudaStream_t)stream;
-    SKB_TRY(matvec_core(fl, d_fib_forces, d_shell_density, d_body_densities, d_body_forces, d_body_torques, eta,
-                        d_v_window));
-    return device_stats(fl);
-}
-
-// ---- per-fiber dense operators (SURVEY.md §8f N2, skb_fiber.cu) ------------------------------------------------
-
-int skb_flow_set_fiber_class(skb_flow *fl, int n_nodes, const double *D_1_0, const double *P_downsample_bc) {
-    if (!fl || !D_1_0 || !P_downsample_bc)
-        return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_class: NULL argument");
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    fl->bodies.drop_links(); // a new node count moves the class table's offsets the links hold
-    return fl->ops.set_class(n_nodes, D_1_0, P_downsample_bc, fl->stream);
-}
-
-int skb_flow_set_fiber_class_derivatives(skb_flow *fl, int n_nodes, const double *D_2_0, const double *D_3_0,
-                                         const double *D_4_0) {
-    if (!fl || !D_2_0 || !D_3_0 || !D_4_0)
-        return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_class_derivatives: NULL argument");
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    return fl->ops.set_class_derivatives(n_nodes, D_2_0, D_3_0, D_4_0, fl->stream);
-}
-
-} // extern "C"
-
-int skb::own_fibers(skb_flow *fl, const char *who, OwnFibers &own) {
-    SKB_TRY(prepare_matvec_targets(fl));
-    int f0 = 0, f1 = 0;
-    if (fl->n_fibers > 0) {
-        const auto &off = fl->h_fiber_off;
-        f0 = (int)(std::lower_bound(off.begin(), off.end(), fl->fa) - off.begin());
-        f1 = (int)(std::lower_bound(off.begin(), off.end(), fl->fb) - off.begin());
-        if (off[(size_t)f0] != fl->fa || off[(size_t)f1] != fl->fb)
-            return set_error(SKB_ERR_INVALID, "%s: the target window [%lld, %lld) cuts a fiber; use "
-                                              "skb_flow_set_target_ranges (whole fibers)", who, fl->fa, fl->fb);
-    }
-    own = OwnFibers{f0, f1, fl->h_fiber_n.data(), fl->h_fiber_off.data(), (const double *)fl->r_fib.ptr,
-                    (const double *)fl->fiber_length.ptr, fl->stream};
-    return SKB_OK;
-}
-
-extern "C" {
-
-int skb_flow_set_fiber_operators(skb_flow *fl, const double *A, const double *force_operator, const double *xs,
-                                 const double *length_prev, const int *plus_bc_velocity) {
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_operators: NULL flow");
-    fl->ops.invalidate();
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    OwnFibers own;
-    SKB_TRY(own_fibers(fl, "skb_flow_set_fiber_operators", own));
-    if (own.count() > 0 && (!A || !force_operator || !xs || !length_prev || !plus_bc_velocity))
-        return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_operators: NULL argument");
-    return fl->ops.upload(own, A, force_operator, xs, length_prev, plus_bc_velocity);
-}
-
-int skb_flow_set_fiber_preconditioner(skb_flow *fl, const double *A_inv) {
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_preconditioner: NULL flow");
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    return fl->ops.upload_inverse(A_inv, fl->stream);
-}
-
-int skb_flow_build_fiber_operators(skb_flow *fl, const skb_fiber_params *params, double dt, double eta) {
-    const char *who = "skb_flow_build_fiber_operators";
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    fl->ops.invalidate();
-    if (!(dt > 0) || !(eta > 0))
-        return set_error(SKB_ERR_INVALID, "%s: dt = %g, eta = %g (both must be > 0)", who, dt, eta);
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    OwnFibers own;
-    SKB_TRY(own_fibers(fl, who, own));
-    if (own.count() > 0 && !params)
-        return set_error(SKB_ERR_INVALID, "%s: NULL params", who);
-    // device_ms spans the assembly and inverse kernels, total_ms also the table uploads before them
-    return fl->ops.build(own, params, dt, eta, &fl->launches,
-                         [&](const FiberOps::Step &stage, const FiberOps::Step &launch) {
-                             begin_stats(fl);
-                             return host_frame(fl, stage, launch, nothing);
-                         });
-}
-
-// checks shared by the two forms of the fiber RHS, then the own fibers on the flow's device; stats of no launch
-static int fiber_rhs_args(skb_flow *fl, const char *who, const skb_fiber_params *params, const double *rhs, double dt,
-                          double eta, OwnFibers &own) {
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    if (!(dt > 0) || !(eta > 0))
-        return set_error(SKB_ERR_INVALID, "%s: dt = %g, eta = %g (both must be > 0)", who, dt, eta);
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    SKB_TRY(own_fibers(fl, who, own));
-    if (own.count() > 0 && (!params || !rhs))
-        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
-    begin_stats(fl);
-    return device_stats(fl);
-}
-
-int skb_flow_build_fiber_rhs(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
-                             const double *force_scale, const double *v_on_fibers, const double *f_external, double dt,
-                             double eta, double *rhs) {
-    OwnFibers own;
-    SKB_TRY(fiber_rhs_args(fl, "skb_flow_build_fiber_rhs", params, rhs, dt, eta, own));
-    const size_t nf = (size_t)own.nodes();
-    SKB_TRY(fl->vel.ensure(nf * 24));
-    SKB_TRY(fl->in_fib.ensure(nf * 24));
-    SKB_TRY(fl->res_fib.ensure(nf * 32));
-    // device_ms spans the kernel, total_ms also the uploads before it and the download after it
-    return fl->ops.rhs(own, params, v_growth, force_scale, v_on_fibers ? (const double *)fl->vel.ptr : nullptr,
-                       f_external ? (const double *)fl->in_fib.ptr : nullptr, dt, eta, (double *)fl->res_fib.ptr,
-                       &fl->launches, [&](const FiberOps::Step &stage, const FiberOps::Step &launch) {
-                           auto up = [&]() -> int {
-                               if (v_on_fibers)
-                                   SKB_TRY(upload(fl, fl->vel, v_on_fibers, nf * 3));
-                               if (f_external)
-                                   SKB_TRY(upload(fl, fl->in_fib, f_external, nf * 3));
-                               return stage();
-                           };
-                           return host_frame(fl, up, launch, [&] { return download(fl, rhs, fl->res_fib, nf * 4); });
-                       });
-}
-
-int skb_flow_build_fiber_rhs_device(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
-                                    const double *force_scale, const double *d_v_on_fibers, const double *d_f_external,
-                                    double dt, double eta, double *d_rhs, void *stream) {
-    OwnFibers own;
-    SKB_TRY(fiber_rhs_args(fl, "skb_flow_build_fiber_rhs_device", params, d_rhs, dt, eta, own));
-    own.stream = (cudaStream_t)stream;
-    return fl->ops.rhs(own, params, v_growth, force_scale, d_v_on_fibers, d_f_external, dt, eta, d_rhs, &fl->launches,
-                       [&](const FiberOps::Step &stage, const FiberOps::Step &launch) {
-                           fl->cur = own.stream;
-                           SKB_TRY(stage());
-                           SKB_TRY(launch());
-                           return device_stats(fl);
-                       });
-}
-
-int skb_flow_get_fiber_operators(skb_flow *fl, double *A, double *force_operator, double *xs, double *A_inv) {
-    const char *who = "skb_flow_get_fiber_operators";
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
-    SKB_TRY(fl->ops.ready(who, A_inv != nullptr));
-    CUDA_TRY(cudaSetDevice(fl->dev));
-    return fl->ops.read(A, force_operator, xs, A_inv, fl->stream);
-}
-
-// host pointers: through host_frame on the flow's stream; device pointers: asynchronously on the caller's stream
-int skb_flow_apply_fiber_preconditioner(skb_flow *fl, const double *x_fibers, double *y) {
-    return fiber_ops_call(fl, "skb_flow_apply_fiber_preconditioner", true, x_fibers && y, [&](size_t nf) {
-        SKB_TRY(fl->res_fib.ensure(nf * 32));
-        return host_frame(
-            fl, [&] { return upload(fl, fl->x_fib, x_fibers, nf * 4); },
-            [&] {
-                return fl->ops.precondition((const double *)fl->x_fib.ptr, (double *)fl->res_fib.ptr, fl->cur,
-                                            &fl->launches);
-            },
-            [&] { return download(fl, y, fl->res_fib, nf * 4); });
-    });
-}
-
-int skb_flow_apply_fiber_preconditioner_device(skb_flow *fl, const double *d_x_fibers, double *d_y, void *stream) {
-    return fiber_ops_call(fl, "skb_flow_apply_fiber_preconditioner_device", true, d_x_fibers && d_y, [&](size_t) {
-        fl->cur = (cudaStream_t)stream;
-        SKB_TRY(fl->ops.precondition(d_x_fibers, d_y, fl->cur, &fl->launches));
-        return device_stats(fl);
-    });
-}
-
-int skb_flow_apply_fiber_force(skb_flow *fl, const double *x_fibers, double *fw) {
-    return fiber_ops_call(fl, "skb_flow_apply_fiber_force", false, x_fibers && fw, [&](size_t nf) {
-        return host_frame(
-            fl,
-            [&]() -> int {
-                SKB_TRY(upload(fl, fl->x_fib, x_fibers, nf * 4));
-                return fl->in_fib.ensure(nf * 24);
-            },
-            [&] {
-                return fl->ops.force((const double *)fl->x_fib.ptr, (double *)fl->in_fib.ptr, fl->cur, &fl->launches);
-            },
-            [&] { return download(fl, fw, fl->in_fib, nf * 3); });
-    });
-}
-
-int skb_flow_fiber_matvec(skb_flow *fl, const double *x_fibers, const double *v_fibers, const double *v_fib_boundary,
-                          double *res) {
-    return fiber_ops_call(fl, "skb_flow_fiber_matvec", false, x_fibers && v_fibers && res, [&](size_t nf) {
-        SKB_TRY(fl->res_fib.ensure(nf * 32));
-        return host_frame(
-            fl,
-            [&]() -> int {
-                SKB_TRY(upload(fl, fl->x_fib, x_fibers, nf * 4));
-                SKB_TRY(upload(fl, fl->vel, v_fibers, nf * 3));
-                return v_fib_boundary ? upload(fl, fl->vb, v_fib_boundary, (size_t)fl->ops.n_fibers() * 7) : SKB_OK;
-            },
-            [&] {
-                return fl->ops.matvec((const double *)fl->x_fib.ptr, (const double *)fl->vel.ptr,
-                                      v_fib_boundary ? (const double *)fl->vb.ptr : nullptr,
-                                      (double *)fl->res_fib.ptr, fl->cur, &fl->launches);
-            },
-            [&] { return download(fl, res, fl->res_fib, nf * 4); });
-    });
-}
-
-int skb_flow_apply_fiber_force_device(skb_flow *fl, const double *d_x_fibers, double *d_fw, void *stream) {
-    return fiber_ops_call(fl, "skb_flow_apply_fiber_force_device", false, d_x_fibers && d_fw, [&](size_t) {
-        fl->cur = (cudaStream_t)stream;
-        SKB_TRY(fl->ops.force(d_x_fibers, d_fw, fl->cur, &fl->launches));
-        return device_stats(fl);
-    });
-}
-
-int skb_flow_fiber_matvec_device(skb_flow *fl, const double *d_x_fibers, const double *d_v_fibers,
-                                 const double *d_v_fib_boundary, double *d_res, void *stream) {
-    return fiber_ops_call(fl, "skb_flow_fiber_matvec_device", false, d_x_fibers && d_v_fibers && d_res, [&](size_t) {
-        fl->cur = (cudaStream_t)stream;
-        SKB_TRY(fl->ops.matvec(d_x_fibers, d_v_fibers, d_v_fib_boundary, d_res, fl->cur, &fl->launches));
-        return device_stats(fl);
+    return device_frame(fl, stream, [&] {
+        return matvec_core(fl, d_fib_forces, d_shell_density, d_body_densities, d_body_forces, d_body_torques, eta,
+                           d_v_window);
     });
 }
 
@@ -1394,7 +809,7 @@ int skb::apply_matvec_core(skb_flow *fl, skb_dense *dn, const double *d_x, const
             CUDA_TRY(cudaStreamWaitEvent(fl->cur, B.join, 0));
             add_out_kernel<<<(unsigned)((3 * n_sw + 255) / 256), 256, 0, fl->cur>>>(d_out_shell, (const double *)B.y.ptr,
                                                                                    d_v_shell, 3 * n_sw);
-            SKB_TRY(launched(fl, 1));
+            SKB_TRY(launched(&fl->launches));
         } else if (dn) {
             // res_shell = shell.matvec(x_shell, v_shell) = stresslet_plus_complementary_ * x_shell + v_shell in one
             // kernel at the end of the stream (skb_flow_set_overlap(fl, 0))
@@ -1511,23 +926,10 @@ int skb_flow_apply_matvec_device(skb_flow *fl, skb_dense *dn, const double *d_x_
         return set_error(SKB_ERR_INVALID, "skb_flow_apply_matvec_device: a flow that owns only part of the rows must be a "
                                           "group member (skb_flow_group_init): the fiber forces of the other rows' "
                                           "fibers have to come from somewhere");
-    fl->cur = (cudaStream_t)stream;
-    SKB_TRY(apply_matvec_core(fl, dn, d_x_fibers, d_x_shell, d_body_densities, d_body_forces, d_body_torques,
-                              d_fiber_link_conditions, eta, d_res_fibers, d_out_shell, d_v_bodies));
-    return device_stats(fl);
-}
-
-int skb_flow_last_sym_kernel(const skb_flow *fl, double *ms, int64_t *pairs) {
-    if (!fl)
-        return set_error(SKB_ERR_INVALID, "skb_flow_last_sym_kernel: NULL");
-    return skb_ctx_last_sym_kernel(fl->fib[1].get(), ms, pairs);
-}
-
-int skb_flow_last_stats(const skb_flow *fl, skb_flow_stats *out) {
-    if (!fl || !out)
-        return set_error(SKB_ERR_INVALID, "skb_flow_last_stats: NULL");
-    *out = fl->stats;
-    return SKB_OK;
+    return device_frame(fl, stream, [&] {
+        return apply_matvec_core(fl, dn, d_x_fibers, d_x_shell, d_body_densities, d_body_forces, d_body_torques,
+                                 d_fiber_link_conditions, eta, d_res_fibers, d_out_shell, d_v_bodies);
+    });
 }
 
 } // extern "C"

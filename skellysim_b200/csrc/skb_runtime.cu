@@ -225,6 +225,14 @@ int DevBuf::ensure(size_t bytes) {
     return SKB_OK;
 }
 
+int DevBuf::upload(const void *h, size_t bytes, cudaStream_t st) {
+    if (bytes == 0)
+        return SKB_OK;
+    SKB_TRY(ensure(bytes));
+    CUDA_TRY(cudaMemcpyAsync(ptr, h, bytes, cudaMemcpyHostToDevice, st));
+    return SKB_OK;
+}
+
 // ------------------------------------------------------------------------------------------------
 // pageable -> device upload through a pinned, multi-threaded staging ring
 // ------------------------------------------------------------------------------------------------

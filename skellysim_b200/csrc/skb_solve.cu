@@ -15,13 +15,6 @@ constexpr int kCtasPerSm = 4;                  // of the row-block passes: fixed
 constexpr double kBreakdown = 16.0 * 0x1p-53;  // a new vector at most this fraction of its norm before ICGS: breakdown
 constexpr int kWords = 4;                      // nrm[0] = |w|^2 after pass C, nrm[1] = |r|^2 of the last residual
 
-int launched(int n, int *launches) {
-    CUDA_TRY(cudaGetLastError());
-    count_launch(n);
-    *launches += n;
-    return SKB_OK;
-}
-
 unsigned elementwise_grid(long long n) { return (unsigned)std::clamp<long long>((n + 255) / 256, 1, 4096); }
 } // namespace
 
@@ -91,7 +84,7 @@ int Krylov::pass(int which, int k, double *d_w, const double *d_coef, double *d_
                                                                              part, ldp_);
     }
     krylov_combine_kernel<<<m, kCombineThreads, 0, st>>>(part, ctas_, ldp_, d_out);
-    SKB_TRY(launched(2, launches));
+    SKB_TRY(launched(launches, 2));
     return reduce ? reduce(d_out, m) : SKB_OK;
 }
 
@@ -100,7 +93,7 @@ int Krylov::residual(const double *d_b, const double *d_ax, const Reduce &reduce
     krylov_residual_kernel<<<ctas_, kKrylovThreads, 0, st>>>(d_b, d_ax, (double *)V_.ptr, n_, rows_per_,
                                                              (double *)part_.ptr, ldp_);
     krylov_combine_kernel<<<1, kCombineThreads, 0, st>>>((const double *)part_.ptr, ctas_, ldp_, nrm + 1);
-    SKB_TRY(launched(2, launches));
+    SKB_TRY(launched(launches, 2));
     return reduce ? reduce(nrm + 1, 1) : SKB_OK;
 }
 
@@ -135,7 +128,7 @@ int Krylov::solve(const Apply &A, const Apply &P_inv, const Reduce &reduce, cons
     while (!converged && total < max_iters) {
         // v_0 = r / ||r||
         krylov_scale_kernel<<<elementwise_grid(n), 256, 0, st>>>(V, n, d_nrm + 1);
-        SKB_TRY(launched(1, launches));
+        SKB_TRY(launched(launches));
         std::fill(g_.begin(), g_.end(), 0.0);
         g_[0] = beta;
         int k = 0;
@@ -176,7 +169,7 @@ int Krylov::solve(const Apply &A, const Apply &P_inv, const Reduce &reduce, cons
             if (breakdown || est <= target)
                 break;
             krylov_scale_kernel<<<elementwise_grid(n), 256, 0, st>>>(w, n, d_nrm);
-            SKB_TRY(launched(1, launches));
+            SKB_TRY(launched(launches));
         }
         // y = R^-1 g over the leading columns with a non-zero diagonal; x += P^-1 V y
         int kk = 0;
@@ -192,10 +185,10 @@ int Krylov::solve(const Apply &A, const Apply &P_inv, const Reduce &reduce, cons
             std::memcpy(h_y, y_.data(), (size_t)kk * 8);
             CUDA_TRY(cudaMemcpyAsync(d_y, h_y, (size_t)kk * 8, cudaMemcpyHostToDevice, st));
             krylov_gemv_kernel<<<elementwise_grid(n), kKrylovThreads, (size_t)kk * 8, st>>>(V, ld, kk, d_y, u, n);
-            SKB_TRY(launched(1, launches));
+            SKB_TRY(launched(launches));
             SKB_TRY(P_inv(u, z));
             krylov_axpy_kernel<<<elementwise_grid(n), 256, 0, st>>>(d_x, z, n);
-            SKB_TRY(launched(1, launches));
+            SKB_TRY(launched(launches));
         }
         // the explicit residual r = b - A x, into V col 0 for a restart
         SKB_TRY(A(d_x, u));

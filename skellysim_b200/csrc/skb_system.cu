@@ -1,7 +1,8 @@
-// skb_system.cu -- the whole-system calls of a flow (include/skelly_b200_flow.h): the bodies' operators, frames,
-// placement and the fiber-body links, System::apply_matvec / ::apply_preconditioner and the RHS of the mobility system
-// on whole solution vectors -- on one device (skb_flow_*) and on a group member (skb_flow_group_*, which skb_mflow
-// drives on its members) -- and the refusals they share.  Built on the matvec orchestration of skb_matvec.cu.
+// skb_system.cu -- the whole-system calls of a flow (include/skelly_b200_flow.h): the fibers' per-fiber operators (class
+// tables, upload or device build, RHS and GEMVs), the bodies' operators, frames, placement and the fiber-body links,
+// System::apply_matvec / ::apply_preconditioner and the RHS of the mobility system on whole solution vectors -- on one
+// device (skb_flow_*) and on a group member (skb_flow_group_*, which skb_mflow drives on its members) -- and the
+// refusals they share.  Built on the matvec orchestration of skb_matvec.cu.
 #include "skb_flow.hpp"
 
 #include <algorithm>
@@ -182,6 +183,218 @@ int skb_flow_get_body_operators(skb_flow *fl, double *ex, double *ey, double *ez
 
 } // extern "C"
 
+// ---- the per-fiber dense operators (FiberOps, skb_fiber.cu): their class tables, their upload or device build, the
+// fibers' RHS and the three GEMVs on the own fibers --------------------------------------------------------------
+
+// frame of the fiber operators' GEMV entry points: the operators' check (`inverse`: with their inverse), nothing to do
+// without own fibers, the arguments, then call(nodes of the own fibers) on the flow's device
+template <class Call> static int fiber_ops_call(skb_flow *fl, const char *who, bool inverse, bool args, Call call) {
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    SKB_TRY(fl->ops.ready(who, inverse));
+    begin_stats(fl);
+    if (fl->ops.empty())
+        return SKB_OK;
+    if (!args)
+        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    return call((size_t)(fl->fb - fl->fa));
+}
+
+extern "C" {
+
+int skb_flow_set_fiber_class(skb_flow *fl, int n_nodes, const double *D_1_0, const double *P_downsample_bc) {
+    if (!fl || !D_1_0 || !P_downsample_bc)
+        return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_class: NULL argument");
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    fl->bodies.drop_links(); // a new node count moves the class table's offsets the links hold
+    return fl->ops.set_class(n_nodes, D_1_0, P_downsample_bc, fl->stream);
+}
+
+int skb_flow_set_fiber_class_derivatives(skb_flow *fl, int n_nodes, const double *D_2_0, const double *D_3_0,
+                                         const double *D_4_0) {
+    if (!fl || !D_2_0 || !D_3_0 || !D_4_0)
+        return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_class_derivatives: NULL argument");
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    return fl->ops.set_class_derivatives(n_nodes, D_2_0, D_3_0, D_4_0, fl->stream);
+}
+
+int skb_flow_set_fiber_operators(skb_flow *fl, const double *A, const double *force_operator, const double *xs,
+                                 const double *length_prev, const int *plus_bc_velocity) {
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_operators: NULL flow");
+    fl->ops.invalidate();
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    OwnFibers own;
+    SKB_TRY(own_fibers(fl, "skb_flow_set_fiber_operators", own));
+    if (own.count() > 0 && (!A || !force_operator || !xs || !length_prev || !plus_bc_velocity))
+        return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_operators: NULL argument");
+    return fl->ops.upload(own, A, force_operator, xs, length_prev, plus_bc_velocity);
+}
+
+int skb_flow_set_fiber_preconditioner(skb_flow *fl, const double *A_inv) {
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "skb_flow_set_fiber_preconditioner: NULL flow");
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    return fl->ops.upload_inverse(A_inv, fl->stream);
+}
+
+int skb_flow_build_fiber_operators(skb_flow *fl, const skb_fiber_params *params, double dt, double eta) {
+    const char *who = "skb_flow_build_fiber_operators";
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    fl->ops.invalidate();
+    if (!(dt > 0) || !(eta > 0))
+        return set_error(SKB_ERR_INVALID, "%s: dt = %g, eta = %g (both must be > 0)", who, dt, eta);
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    OwnFibers own;
+    SKB_TRY(own_fibers(fl, who, own));
+    if (own.count() > 0 && !params)
+        return set_error(SKB_ERR_INVALID, "%s: NULL params", who);
+    // device_ms spans the assembly and inverse kernels, total_ms also the table uploads before them
+    return fl->ops.build(own, params, dt, eta, &fl->launches,
+                         [&](const FiberOps::Step &stage, const FiberOps::Step &launch) {
+                             begin_stats(fl);
+                             return host_frame(fl, stage, launch, nothing);
+                         });
+}
+
+// checks shared by the two forms of the fiber RHS, then the own fibers on the flow's device; stats of no launch
+static int fiber_rhs_args(skb_flow *fl, const char *who, const skb_fiber_params *params, const double *rhs, double dt,
+                          double eta, OwnFibers &own) {
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    if (!(dt > 0) || !(eta > 0))
+        return set_error(SKB_ERR_INVALID, "%s: dt = %g, eta = %g (both must be > 0)", who, dt, eta);
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    SKB_TRY(own_fibers(fl, who, own));
+    if (own.count() > 0 && (!params || !rhs))
+        return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
+    begin_stats(fl);
+    return device_stats(fl);
+}
+
+int skb_flow_build_fiber_rhs(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
+                             const double *force_scale, const double *v_on_fibers, const double *f_external, double dt,
+                             double eta, double *rhs) {
+    OwnFibers own;
+    SKB_TRY(fiber_rhs_args(fl, "skb_flow_build_fiber_rhs", params, rhs, dt, eta, own));
+    const size_t nf = (size_t)own.nodes();
+    SKB_TRY(fl->vel.ensure(nf * 24));
+    SKB_TRY(fl->in_fib.ensure(nf * 24));
+    SKB_TRY(fl->res_fib.ensure(nf * 32));
+    // device_ms spans the kernel, total_ms also the uploads before it and the download after it
+    return fl->ops.rhs(own, params, v_growth, force_scale, v_on_fibers ? (const double *)fl->vel.ptr : nullptr,
+                       f_external ? (const double *)fl->in_fib.ptr : nullptr, dt, eta, (double *)fl->res_fib.ptr,
+                       &fl->launches, [&](const FiberOps::Step &stage, const FiberOps::Step &launch) {
+                           auto up = [&]() -> int {
+                               if (v_on_fibers)
+                                   SKB_TRY(upload(fl, fl->vel, v_on_fibers, nf * 3));
+                               if (f_external)
+                                   SKB_TRY(upload(fl, fl->in_fib, f_external, nf * 3));
+                               return stage();
+                           };
+                           return host_frame(fl, up, launch, [&] { return download(fl, rhs, fl->res_fib, nf * 4); });
+                       });
+}
+
+int skb_flow_build_fiber_rhs_device(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
+                                    const double *force_scale, const double *d_v_on_fibers, const double *d_f_external,
+                                    double dt, double eta, double *d_rhs, void *stream) {
+    OwnFibers own;
+    SKB_TRY(fiber_rhs_args(fl, "skb_flow_build_fiber_rhs_device", params, d_rhs, dt, eta, own));
+    own.stream = (cudaStream_t)stream;
+    return fl->ops.rhs(own, params, v_growth, force_scale, d_v_on_fibers, d_f_external, dt, eta, d_rhs, &fl->launches,
+                       [&](const FiberOps::Step &stage, const FiberOps::Step &launch) {
+                           return device_frame(fl, stream, [&]() -> int {
+                               SKB_TRY(stage());
+                               return launch();
+                           });
+                       });
+}
+
+int skb_flow_get_fiber_operators(skb_flow *fl, double *A, double *force_operator, double *xs, double *A_inv) {
+    const char *who = "skb_flow_get_fiber_operators";
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "%s: NULL flow", who);
+    SKB_TRY(fl->ops.ready(who, A_inv != nullptr));
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    return fl->ops.read(A, force_operator, xs, A_inv, fl->stream);
+}
+
+// host pointers: through host_frame on the flow's stream; device pointers: asynchronously on the caller's stream
+int skb_flow_apply_fiber_preconditioner(skb_flow *fl, const double *x_fibers, double *y) {
+    return fiber_ops_call(fl, "skb_flow_apply_fiber_preconditioner", true, x_fibers && y, [&](size_t nf) {
+        SKB_TRY(fl->res_fib.ensure(nf * 32));
+        return host_frame(
+            fl, [&] { return upload(fl, fl->x_fib, x_fibers, nf * 4); },
+            [&] {
+                return fl->ops.precondition((const double *)fl->x_fib.ptr, (double *)fl->res_fib.ptr, fl->cur,
+                                            &fl->launches);
+            },
+            [&] { return download(fl, y, fl->res_fib, nf * 4); });
+    });
+}
+
+int skb_flow_apply_fiber_preconditioner_device(skb_flow *fl, const double *d_x_fibers, double *d_y, void *stream) {
+    return fiber_ops_call(fl, "skb_flow_apply_fiber_preconditioner_device", true, d_x_fibers && d_y, [&](size_t) {
+        return device_frame(fl, stream,
+                            [&] { return fl->ops.precondition(d_x_fibers, d_y, fl->cur, &fl->launches); });
+    });
+}
+
+int skb_flow_apply_fiber_force(skb_flow *fl, const double *x_fibers, double *fw) {
+    return fiber_ops_call(fl, "skb_flow_apply_fiber_force", false, x_fibers && fw, [&](size_t nf) {
+        return host_frame(
+            fl,
+            [&]() -> int {
+                SKB_TRY(upload(fl, fl->x_fib, x_fibers, nf * 4));
+                return fl->in_fib.ensure(nf * 24);
+            },
+            [&] {
+                return fl->ops.force((const double *)fl->x_fib.ptr, (double *)fl->in_fib.ptr, fl->cur, &fl->launches);
+            },
+            [&] { return download(fl, fw, fl->in_fib, nf * 3); });
+    });
+}
+
+int skb_flow_fiber_matvec(skb_flow *fl, const double *x_fibers, const double *v_fibers, const double *v_fib_boundary,
+                          double *res) {
+    return fiber_ops_call(fl, "skb_flow_fiber_matvec", false, x_fibers && v_fibers && res, [&](size_t nf) {
+        SKB_TRY(fl->res_fib.ensure(nf * 32));
+        return host_frame(
+            fl,
+            [&]() -> int {
+                SKB_TRY(upload(fl, fl->x_fib, x_fibers, nf * 4));
+                SKB_TRY(upload(fl, fl->vel, v_fibers, nf * 3));
+                return v_fib_boundary ? upload(fl, fl->vb, v_fib_boundary, (size_t)fl->ops.n_fibers() * 7) : SKB_OK;
+            },
+            [&] {
+                return fl->ops.matvec((const double *)fl->x_fib.ptr, (const double *)fl->vel.ptr,
+                                      v_fib_boundary ? (const double *)fl->vb.ptr : nullptr,
+                                      (double *)fl->res_fib.ptr, fl->cur, &fl->launches);
+            },
+            [&] { return download(fl, res, fl->res_fib, nf * 4); });
+    });
+}
+
+int skb_flow_apply_fiber_force_device(skb_flow *fl, const double *d_x_fibers, double *d_fw, void *stream) {
+    return fiber_ops_call(fl, "skb_flow_apply_fiber_force_device", false, d_x_fibers && d_fw, [&](size_t) {
+        return device_frame(fl, stream, [&] { return fl->ops.force(d_x_fibers, d_fw, fl->cur, &fl->launches); });
+    });
+}
+
+int skb_flow_fiber_matvec_device(skb_flow *fl, const double *d_x_fibers, const double *d_v_fibers,
+                                 const double *d_v_fib_boundary, double *d_res, void *stream) {
+    return fiber_ops_call(fl, "skb_flow_fiber_matvec_device", false, d_x_fibers && d_v_fibers && d_res, [&](size_t) {
+        return device_frame(fl, stream, [&] {
+            return fl->ops.matvec(d_x_fibers, d_v_fibers, d_v_fib_boundary, d_res, fl->cur, &fl->launches);
+        });
+    });
+}
+
+} // extern "C"
+
 // ---- the refusals of the system calls, of every family ----
 
 int skb::system_ready(skb_flow *fl, const char *who, const Calls &calls, bool precondition, bool step) {
@@ -312,9 +525,7 @@ int skb_flow_apply_system_matvec_device(skb_flow *fl, skb_dense *dn, const doubl
         return set_error(SKB_ERR_INVALID, "%s: eta = %g", who, eta);
     if (solution_size(fl) == 0)
         return SKB_OK;
-    fl->cur = (cudaStream_t)stream;
-    SKB_TRY(system_matvec_core(fl, dn, d_x, eta, d_res));
-    return device_stats(fl);
+    return device_frame(fl, stream, [&] { return system_matvec_core(fl, dn, d_x, eta, d_res); });
 }
 
 int skb_flow_apply_system_preconditioner(skb_flow *fl, skb_dense *dn, const double *x, double *y) {
@@ -337,9 +548,7 @@ int skb_flow_apply_system_preconditioner_device(skb_flow *fl, skb_dense *dn, con
     SKB_TRY(system_args(fl, dn, who, true, (d_x && d_y) || solution_size(fl) == 0));
     if (solution_size(fl) == 0)
         return SKB_OK;
-    fl->cur = (cudaStream_t)stream;
-    SKB_TRY(system_precondition_core(fl, dn, d_x, d_y));
-    return device_stats(fl);
+    return device_frame(fl, stream, [&] { return system_precondition_core(fl, dn, d_x, d_y); });
 }
 
 } // extern "C"
@@ -478,11 +687,11 @@ int skb_flow_build_system_rhs_device(skb_flow *fl, const skb_fiber_params *param
     if (solution_size(fl) == 0)
         return SKB_OK;
     const long long nf = fl->n_fib, ns = fl->n_shell;
-    fl->cur = (cudaStream_t)stream;
-    SKB_TRY(system_rhs_core(fl, own, params, v_growth, force_scale, nf ? d_f_external : nullptr,
-                            fl->n_bodies ? d_body_forces : nullptr, fl->n_bodies ? d_body_torques : nullptr, dt, eta,
-                            d_rhs, d_rhs + 4 * nf, d_rhs + 4 * nf + 3 * ns));
-    return device_stats(fl);
+    return device_frame(fl, stream, [&] {
+        return system_rhs_core(fl, own, params, v_growth, force_scale, nf ? d_f_external : nullptr,
+                               fl->n_bodies ? d_body_forces : nullptr, fl->n_bodies ? d_body_torques : nullptr, dt, eta,
+                               d_rhs, d_rhs + 4 * nf, d_rhs + 4 * nf + 3 * ns);
+    });
 }
 
 } // extern "C"
@@ -682,26 +891,25 @@ int skb_flow_group_apply_system_matvec_device(skb_flow *fl, skb_dense *dn, const
     if (group_local_size(fl) > 0 && (!d_x_local || !d_res_local))
         return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
     begin_stats(fl);
-    fl->cur = (cudaStream_t)stream;
-    Group &G = fl->grp;
-    const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
-    const double *x_fib = d_x_local, *x_shell = x_fib + 4 * n_fw, *x_body = x_shell + 3 * n_sw;
-    double *res_fib = d_res_local, *res_shell = res_fib + 4 * n_fw, *res_body = res_shell + 3 * n_sw;
-    double *full = (double *)fl->sys_rb.ptr;
-    const bool bodies = fl->n_bodies > 0;
-    SKB_TRY(G.begin());
-    if (bodies) { // the complete x_bodies in every window first: the links read the bodies' U, w before barrier A
-        SKB_TRY(G.store_rows(x_body, nullptr, 0, 0, fl->fib[1]->devs[0].info.num_sms, fl->cur, &fl->launches));
-        SKB_TRY(G.rows_barrier(true, true, fl->cur, &fl->launches));
-    }
-    fl->grp_open = true; // matvec_core's push, barriers and pull run in this epoch
-    const int rc = member_system_matvec_core(fl, dn, x_fib, x_shell, bodies ? G.x_body() : nullptr, eta, res_fib,
-                                             res_shell, full);
-    fl->grp_open = false;
-    SKB_TRY(rc);
-    if (bodies)
-        SKB_TRY(G.compact_rows(full, res_body, fl->cur, &fl->launches));
-    return device_stats(fl);
+    return device_frame(fl, stream, [&]() -> int {
+        Group &G = fl->grp;
+        const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
+        const double *x_fib = d_x_local, *x_shell = x_fib + 4 * n_fw, *x_body = x_shell + 3 * n_sw;
+        double *res_fib = d_res_local, *res_shell = res_fib + 4 * n_fw, *res_body = res_shell + 3 * n_sw;
+        double *full = (double *)fl->sys_rb.ptr;
+        const bool bodies = fl->n_bodies > 0;
+        SKB_TRY(G.begin());
+        if (bodies) { // the complete x_bodies in every window first: the links read the bodies' U, w before barrier A
+            SKB_TRY(G.store_rows(x_body, nullptr, 0, 0, fl->fib[1]->devs[0].info.num_sms, fl->cur, &fl->launches));
+            SKB_TRY(G.rows_barrier(true, true, fl->cur, &fl->launches));
+        }
+        fl->grp_open = true; // matvec_core's push, barriers and pull run in this epoch
+        const int rc = member_system_matvec_core(fl, dn, x_fib, x_shell, bodies ? G.x_body() : nullptr, eta, res_fib,
+                                                 res_shell, full);
+        fl->grp_open = false;
+        SKB_TRY(rc);
+        return bodies ? G.compact_rows(full, res_body, fl->cur, &fl->launches) : SKB_OK;
+    });
 }
 
 int skb_flow_group_apply_system_preconditioner_device(skb_flow *fl, skb_dense *dn, const double *d_x_local,
@@ -715,28 +923,29 @@ int skb_flow_group_apply_system_preconditioner_device(skb_flow *fl, skb_dense *d
     if (group_local_size(fl) > 0 && (!d_x_local || !d_y_local))
         return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
     begin_stats(fl);
-    fl->cur = (cudaStream_t)stream;
-    Group &G = fl->grp;
-    const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
-    const double *x_fib = d_x_local, *x_shell = x_fib + 4 * n_fw, *x_body = x_shell + 3 * n_sw;
-    double *y_fib = d_y_local, *y_shell = y_fib + 4 * n_fw, *y_body = y_shell + 3 * n_sw;
-    double *full = (double *)fl->sys_rb.ptr;
-    // the complete x_shell and x_bodies in every window; the fibers' A_^-1 runs while the peers' rows arrive
-    SKB_TRY(G.begin());
-    SKB_TRY(G.store_rows(x_body, n_sw > 0 ? x_shell : nullptr, fl->sa, n_sw, fl->fib[1]->devs[0].info.num_sms, fl->cur,
-                         &fl->launches));
-    SKB_TRY(G.rows_barrier(true, false, fl->cur, &fl->launches));
-    SKB_TRY(fl->ops.precondition(x_fib, y_fib, fl->cur, &fl->launches));
-    SKB_TRY(G.rows_barrier(false, true, fl->cur, &fl->launches));
-    if (n_sw > 0) { // the member's rows of M_inv times the complete x_shell
-        SKB_TRY(skb_dense_apply_device(dn, SKB_DENSE_M_INV, G.x_shell(), nullptr, y_shell, fl->cur));
-        fl->launches += 1;
-    }
-    if (fl->n_bodies > 0) {
-        SKB_TRY(fl->bodies.precondition(G.x_body(), full, fl->cur, &fl->launches));
-        SKB_TRY(G.compact_rows(full, y_body, fl->cur, &fl->launches));
-    }
-    return device_stats(fl);
+    return device_frame(fl, stream, [&]() -> int {
+        Group &G = fl->grp;
+        const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
+        const double *x_fib = d_x_local, *x_shell = x_fib + 4 * n_fw, *x_body = x_shell + 3 * n_sw;
+        double *y_fib = d_y_local, *y_shell = y_fib + 4 * n_fw, *y_body = y_shell + 3 * n_sw;
+        double *full = (double *)fl->sys_rb.ptr;
+        // the complete x_shell and x_bodies in every window; the fibers' A_^-1 runs while the peers' rows arrive
+        SKB_TRY(G.begin());
+        SKB_TRY(G.store_rows(x_body, n_sw > 0 ? x_shell : nullptr, fl->sa, n_sw, fl->fib[1]->devs[0].info.num_sms,
+                             fl->cur, &fl->launches));
+        SKB_TRY(G.rows_barrier(true, false, fl->cur, &fl->launches));
+        SKB_TRY(fl->ops.precondition(x_fib, y_fib, fl->cur, &fl->launches));
+        SKB_TRY(G.rows_barrier(false, true, fl->cur, &fl->launches));
+        if (n_sw > 0) { // the member's rows of M_inv times the complete x_shell
+            SKB_TRY(skb_dense_apply_device(dn, SKB_DENSE_M_INV, G.x_shell(), nullptr, y_shell, fl->cur));
+            fl->launches += 1;
+        }
+        if (fl->n_bodies > 0) {
+            SKB_TRY(fl->bodies.precondition(G.x_body(), full, fl->cur, &fl->launches));
+            SKB_TRY(G.compact_rows(full, y_body, fl->cur, &fl->launches));
+        }
+        return SKB_OK;
+    });
 }
 
 int skb_flow_group_build_system_rhs_device(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
@@ -764,17 +973,17 @@ int skb_flow_group_build_system_rhs_device(skb_flow *fl, const skb_fiber_params 
     if ((own.count() > 0 && !params) || (group_local_size(fl) > 0 && !d_rhs_local))
         return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
     begin_stats(fl);
-    fl->cur = (cudaStream_t)stream;
-    const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
-    double *rhs_fib = d_rhs_local, *rhs_shell = rhs_fib + 4 * n_fw, *rhs_body = rhs_shell + 3 * n_sw;
-    double *full = (double *)fl->sys_rb.ptr;
-    // the fiber block's checks come first inside system_rhs_core, before its first launch; F_T complete, as they are
-    SKB_TRY(system_rhs_core(fl, own, params, v_growth, force_scale, own.count() > 0 ? d_f_external : nullptr,
-                            fl->n_bodies ? d_body_forces : nullptr, fl->n_bodies ? d_body_torques : nullptr, dt, eta,
-                            rhs_fib, rhs_shell, full));
-    if (fl->n_bodies > 0)
-        SKB_TRY(fl->grp.compact_rows(full, rhs_body, fl->cur, &fl->launches));
-    return device_stats(fl);
+    return device_frame(fl, stream, [&]() -> int {
+        const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
+        double *rhs_fib = d_rhs_local, *rhs_shell = rhs_fib + 4 * n_fw, *rhs_body = rhs_shell + 3 * n_sw;
+        double *full = (double *)fl->sys_rb.ptr;
+        // the fiber block's checks come first inside system_rhs_core, before its first launch; F_T complete, as they
+        // are
+        SKB_TRY(system_rhs_core(fl, own, params, v_growth, force_scale, own.count() > 0 ? d_f_external : nullptr,
+                                fl->n_bodies ? d_body_forces : nullptr, fl->n_bodies ? d_body_torques : nullptr, dt,
+                                eta, rhs_fib, rhs_shell, full));
+        return fl->n_bodies > 0 ? fl->grp.compact_rows(full, rhs_body, fl->cur, &fl->launches) : SKB_OK;
+    });
 }
 
 } // extern "C"
