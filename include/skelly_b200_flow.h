@@ -120,6 +120,16 @@ SKB_API int skb_flow_set_listener_state_device(skb_flow *fl, const struct skb_fi
 /* System::velocity_at_targets (system.cpp:330-384) on the frame: skb_flow_velocity_at_targets's velocity, and at a
  * target inside a body (bodies in the library's order, the last match wins) the body's rigid motion U + omega x dx. */
 SKB_API int skb_flow_listener_velocity(skb_flow *fl, const double *r_trg, int64_t n_trg, double *vel);
+/* The velocity gradient and the pressure of the listener's frame at n_trg targets (3 each):
+ * grad[9 t + 3 i + j] = d u_i / d x_j, pressure[t].  Same frame, staleness and refusals as
+ * skb_flow_listener_velocity; n_trg == 0 is a no-op.  The gradient is the analytic one of every source of that
+ * velocity (fibers' Stokeslets, the bodies' and the periphery's stresslets, the bodies' net forces and torques, the
+ * point sources' regularised Oseen and rotlet kernels, the background flow); the pressure is that of the Stokeslets,
+ * stresslets and point forces, p -> 0 far from every source.  A coincident source adds exactly 0 to every output.  At a
+ * target inside a body (the velocity's test and order) the gradient is the rigid motion's, eps_ikj omega_k, and the
+ * pressure is NaN.  Both outputs are written for every target. */
+SKB_API int skb_flow_listener_gradient(skb_flow *fl, const double *r_trg, int64_t n_trg, double *grad,
+                                       double *pressure);
 
 /* StreamLine::compute / VortexLine::compute (streamline.cpp) for n_lines seeds x0 (3 each) at once: odeint's
  * integrate_adaptive with the controlled Cash-Karp 5(4) stepper (default error checker and step adjuster, 500 failed

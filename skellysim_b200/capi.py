@@ -182,6 +182,7 @@ def library() -> C.CDLL:
         "skb_flow_set_listener_state_device": ([ctxp, C.POINTER(FiberParams), C.c_double, C.c_double, C.c_void_p,
                                                 C.c_void_p, C.POINTER(C.c_int32), _dp, C.c_int32, C.c_void_p], C.c_int),
         "skb_flow_listener_velocity": ([ctxp, _dp, C.c_int64, _dp], C.c_int),
+        "skb_flow_listener_gradient": ([ctxp, _dp, C.c_int64, _dp, _dp], C.c_int),
         "skb_flow_listener_lines": ([ctxp, C.c_int, _dp, C.c_int32, C.POINTER(LineRequest), _dp, _dp, _dp,
                                      C.POINTER(C.c_int32), C.POINTER(C.c_int32)], C.c_int),
         "skb_flow_set_target_window": ([ctxp, C.c_int64, C.c_int64], C.c_int),
@@ -1634,8 +1635,8 @@ def _state_args(flow, params, body_kind, body_radii):
 
 # The listener's frame of a step (skb_flow_set_listener_state), on a Flow only: the listener is single-device, and an
 # skb_mflow handle must never reach an skb_flow_ call.  Module functions taking the Flow rather than Flow methods:
-# Flow's public methods are pinned one by one by tests/test_capi_binding_cpu.py; these two are marshalled and checked
-# the same way in tests/test_listener_state_binding_cpu.py.
+# Flow's public methods are pinned one by one by tests/test_capi_binding_cpu.py; these are marshalled and checked
+# the same way in tests/test_listener_state_binding_cpu.py and tests/test_listener_gradient_cpu.py.
 def _listener_flow(flow):
     if not isinstance(flow, Flow):
         raise TypeError(f"the listener's frame needs a capi.Flow (one device), got {type(flow).__name__}")
@@ -1676,3 +1677,16 @@ def set_listener_state_device(flow, length_prev, bending_rigidity, radius, penal
                                                         _vp(d_x), kind.ctypes.data_as(C.POINTER(C.c_int32)),
                                                         _p(radii), int(bool(periphery_interaction)),
                                                         C.c_void_p(stream)))
+
+
+def listener_gradient(flow, r):
+    """The velocity gradient and the pressure of `flow`'s listener frame (a Flow) at the points r (n, 3), on the
+    device: grad (n, 3, 3) with grad[t, i, j] = d u_i / d x_j, and pressure (n,).  The frame, staleness and refusals
+    are those of Flow.velocity_field; inside a body the gradient is the rigid motion's and the pressure NaN.  The
+    vorticity is omega_i = eps_ijk d_j u_k (omega = (G[2,1] - G[1,2], G[0,2] - G[2,0], G[1,0] - G[0,1])), the strain
+    rate E = (G + G^T) / 2."""
+    _listener_flow(flow)
+    r = _arr(r, 3)
+    grad, pressure = np.empty((r.shape[0], 3, 3)), np.empty(r.shape[0])
+    _check(library().skb_flow_listener_gradient(flow._h, _p(r), r.shape[0], _p(grad), _p(pressure)))
+    return grad, pressure

@@ -122,6 +122,76 @@ __global__ void oseen_contract_add_kernel(const double *__restrict__ r_src, cons
     u[3 * t + 2] += a2;
 }
 
+// ---- the gradients of the velocities above (skb_flow_listener_gradient): 10 per target, d u_i / d x_j at 3 i + j and
+// the pressure over eta at 9.  r = trg - src; the regularised branch is the velocity kernel's at that distance, with
+// d|r|_reg / d r_j = r_j / |r|_reg in both branches; a coincident pair adds exactly 0 (the reference's r == 0 rule).
+// rotlet_add_kernel's u = c (L x r) / D^3:  G_ij = c (eps_iaj L_a / D^3 - 3 (L x r)_i r_j / D^5), no pressure
+__global__ void rotlet_grad_add_kernel(const double *__restrict__ r_src, const double *__restrict__ torque, int n_src,
+                                       const double *__restrict__ r_trg, long long n_trg, double inv_8pi_eta,
+                                       double reg2, double eps2, double *__restrict__ g) {
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n_trg)
+        return;
+    const double x = r_trg[3 * t], y = r_trg[3 * t + 1], z = r_trg[3 * t + 2];
+    double a[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+    for (int s = 0; s < n_src; ++s) {
+        const double d[3] = {x - r_src[3 * s], y - r_src[3 * s + 1], z - r_src[3 * s + 2]};
+        const double dr2 = d[0] * d[0] + d[1] * d[1] + d[2] * d[2];
+        if (dr2 == 0.0)
+            continue;
+        const double dr = dr2 < eps2 ? sqrt(reg2 + dr2) : sqrt(dr2);
+        const double fr = 1.0 / (dr * dr * dr), hr = 3.0 * fr / (dr * dr);
+        const double l0 = torque[3 * s], l1 = torque[3 * s + 1], l2 = torque[3 * s + 2];
+        const double m[3] = {d[2] * l1 - d[1] * l2, d[0] * l2 - d[2] * l0, d[1] * l0 - d[0] * l1}; // L x r
+        const double e[9] = {0, -l2, l1, l2, 0, -l0, -l1, l0, 0};                               // eps_iaj L_a
+        for (int i = 0; i < 3; ++i)
+            for (int j = 0; j < 3; ++j)
+                a[3 * i + j] += fr * e[3 * i + j] - hr * m[i] * d[j];
+    }
+    for (int k = 0; k < 9; ++k)
+        g[10 * t + k] += inv_8pi_eta * a[k];
+}
+
+// oseen_contract_add_kernel's u = c (f / D + r (r.f) / D^3):
+//   G_ij = c ((delta_ij (r.f) + r_i f_j - f_i r_j) / D^3 - 3 r_i r_j (r.f) / D^5),  p / eta = 2 c (r.f) / D^3
+// with r = trg - src (the velocity kernel's src - trg is even; the pressure is odd)
+__global__ void oseen_grad_add_kernel(const double *__restrict__ r_src, const double *__restrict__ density, int n_src,
+                                      const double *__restrict__ r_trg, long long n_trg, double inv_8pi_eta,
+                                      double reg2, double eps, double *__restrict__ g) {
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n_trg)
+        return;
+    const double x = r_trg[3 * t], y = r_trg[3 * t + 1], z = r_trg[3 * t + 2];
+    double a[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+    for (int s = 0; s < n_src; ++s) {
+        const double d[3] = {x - r_src[3 * s], y - r_src[3 * s + 1], z - r_src[3 * s + 2]};
+        const double dr = sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+        if (dr == 0.0)
+            continue;
+        const double D = dr > eps ? dr : sqrt(dr * dr + reg2);
+        const double gr = 1.0 / (D * D * D), hr = 3.0 * gr / (D * D);
+        const double f[3] = {density[3 * s], density[3 * s + 1], density[3 * s + 2]};
+        const double rf = d[0] * f[0] + d[1] * f[1] + d[2] * f[2];
+        for (int i = 0; i < 3; ++i)
+            for (int j = 0; j < 3; ++j)
+                a[3 * i + j] += gr * ((i == j ? rf : 0.0) + d[i] * f[j] - f[i] * d[j]) - hr * rf * d[i] * d[j];
+        a[9] += 2.0 * gr * rf;
+    }
+    for (int k = 0; k < 10; ++k)
+        g[10 * t + k] += inv_8pi_eta * a[k];
+}
+
+// background_add_kernel's u_j = uniform_j + scale_j r[c_j]:  d u_j / d x_{c_j} += scale_j
+__global__ void background_grad_add_kernel(long long n_trg, int c0, int c1, int c2, double s0, double s1, double s2,
+                                           double *__restrict__ g) {
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n_trg)
+        return;
+    g[10 * t + 0 + c0] += s0;
+    g[10 * t + 3 + c1] += s1;
+    g[10 * t + 6 + c2] += s2;
+}
+
 // BackgroundSource::flow (background_source.cpp:15-24): u_j += uniform_j + r[components_j] * scale_j
 __global__ void background_add_kernel(const double *__restrict__ r_trg, long long n_trg, int c0, int c1, int c2,
                                       double s0, double s1, double s2, double u0, double u1, double u2,

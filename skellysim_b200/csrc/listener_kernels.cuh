@@ -22,8 +22,25 @@ constexpr double kSingularSpeed = 1e3; // push_back_points_and_time: "Possible s
 // per body of the interior replacement: kind (0 none, 1 sphere, 2 ellipsoid), radii[3], centre[3], U[3], omega[3]
 constexpr int kRigidStride = 13;
 
-// points inside a body take the body's rigid motion U + omega x dx; bodies in order, the last match wins.  Every
+// the interior test of the body with rigid-table row p at x (kind 0: never inside); d = x - centre.  Every
 // operation rounds on its own (no contraction), as the reference's separate products and sums do
+__device__ __forceinline__ bool inside_body(const double *p, double x0, double x1, double x2, double &d0, double &d1,
+                                            double &d2) {
+    const int kind = (int)p[0];
+    if (kind == 0)
+        return false;
+    d0 = __dsub_rn(x0, p[4]), d1 = __dsub_rn(x1, p[5]), d2 = __dsub_rn(x2, p[6]);
+    if (kind == 1) {
+        const double n2 = __dadd_rn(__dadd_rn(__dmul_rn(d0, d0), __dmul_rn(d1, d1)), __dmul_rn(d2, d2));
+        return __dsqrt_rn(n2) < p[1];
+    }
+    const double q0 = __ddiv_rn(__ddiv_rn(__dmul_rn(d0, d0), p[1]), p[1]);
+    const double q1 = __ddiv_rn(__ddiv_rn(__dmul_rn(d1, d1), p[2]), p[2]);
+    const double q2 = __ddiv_rn(__ddiv_rn(__dmul_rn(d2, d2), p[3]), p[3]);
+    return __dadd_rn(__dadd_rn(q0, q1), q2) < 1.0;
+}
+
+// points inside a body take the body's rigid motion U + omega x dx; bodies in order, the last match wins
 __global__ void interior_replace_kernel(const double *__restrict__ trg, long long n_trg,
                                         const double *__restrict__ rigid, int n_bodies, double *__restrict__ vel) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -32,27 +49,43 @@ __global__ void interior_replace_kernel(const double *__restrict__ trg, long lon
     const double x0 = trg[3 * i], x1 = trg[3 * i + 1], x2 = trg[3 * i + 2];
     for (int b = 0; b < n_bodies; ++b) {
         const double *p = rigid + (size_t)b * kRigidStride;
-        const int kind = (int)p[0];
-        if (kind == 0)
-            continue;
-        const double d0 = __dsub_rn(x0, p[4]), d1 = __dsub_rn(x1, p[5]), d2 = __dsub_rn(x2, p[6]);
-        bool inside;
-        if (kind == 1) {
-            const double n2 = __dadd_rn(__dadd_rn(__dmul_rn(d0, d0), __dmul_rn(d1, d1)), __dmul_rn(d2, d2));
-            inside = __dsqrt_rn(n2) < p[1];
-        } else {
-            const double q0 = __ddiv_rn(__ddiv_rn(__dmul_rn(d0, d0), p[1]), p[1]);
-            const double q1 = __ddiv_rn(__ddiv_rn(__dmul_rn(d1, d1), p[2]), p[2]);
-            const double q2 = __ddiv_rn(__ddiv_rn(__dmul_rn(d2, d2), p[3]), p[3]);
-            inside = __dadd_rn(__dadd_rn(q0, q1), q2) < 1.0;
-        }
-        if (inside) {
+        double d0, d1, d2;
+        if (inside_body(p, x0, x1, x2, d0, d1, d2)) {
             const double w0 = p[10], w1 = p[11], w2 = p[12];
             vel[3 * i] = __dadd_rn(p[7], __dsub_rn(__dmul_rn(w1, d2), __dmul_rn(w2, d1)));
             vel[3 * i + 1] = __dadd_rn(p[8], __dsub_rn(__dmul_rn(w2, d0), __dmul_rn(w0, d2)));
             vel[3 * i + 2] = __dadd_rn(p[9], __dsub_rn(__dmul_rn(w0, d1), __dmul_rn(w1, d0)));
         }
     }
+}
+
+// The gradient's last pass: g (10 per target, gradient_dev) splits into grad (9 per target) and the pressure, which
+// gradient_dev leaves over eta.  Inside a body (the test and order of interior_replace_kernel) the gradient is the
+// rigid motion's, d u_i / d x_j = eps_ikj omega_k, and the pressure NaN: a rigid body has no fluid pressure
+__global__ void gradient_finish_kernel(const double *__restrict__ trg, long long n_trg, const double *__restrict__ rigid,
+                                       int n_bodies, double eta, const double *__restrict__ g, double *__restrict__ grad,
+                                       double *__restrict__ pressure) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_trg)
+        return;
+    double o[10];
+    for (int k = 0; k < 10; ++k)
+        o[k] = g[10 * i + k];
+    o[9] *= eta;
+    const double x0 = trg[3 * i], x1 = trg[3 * i + 1], x2 = trg[3 * i + 2];
+    for (int b = 0; b < n_bodies; ++b) {
+        const double *p = rigid + (size_t)b * kRigidStride;
+        double d0, d1, d2;
+        if (inside_body(p, x0, x1, x2, d0, d1, d2)) {
+            const double w0 = p[10], w1 = p[11], w2 = p[12];
+            const double r[10] = {0.0, -w2, w1, w2, 0.0, -w0, -w1, w0, 0.0, __longlong_as_double(0x7ff8000000000000LL)};
+            for (int k = 0; k < 10; ++k)
+                o[k] = r[k];
+        }
+    }
+    for (int k = 0; k < 9; ++k)
+        grad[9 * i + k] = o[k];
+    pressure[i] = o[9];
 }
 
 // The frame of skb_flow_set_listener_state, one launch of n_fibers + n_bodies CTAs.  CTA f < n_fibers packs fiber f's

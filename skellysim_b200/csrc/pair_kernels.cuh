@@ -38,10 +38,15 @@ constexpr int kPrefetch = 2;        // tiles in flight ahead of the one being co
 constexpr int kCtaThreads = 128;    // 4 warps, one per SM sub-partition; every warp computes
 constexpr int kMaxSplits = 256;
 
-enum Kind : int { kStokeslet = 0, kStresslet = 1 };
+// the gradient kinds read the velocity kinds' packed strengths and write 10 outputs per target: d u_i / d x_j at
+// 3 i + j, then the pressure (listener_gradient, skb_listener.cu)
+enum Kind : int { kStokeslet = 0, kStresslet = 1, kStokesletGrad = 2, kStressletGrad = 3 };
 template <int KIND> struct KindTraits;
-template <> struct KindTraits<kStokeslet> { static constexpr int fdim = 3; };  // packed strengths / source
-template <> struct KindTraits<kStresslet> { static constexpr int fdim = 6; };  // sym6 combinations
+// fdim: packed strengths per source; odim: outputs per target
+template <> struct KindTraits<kStokeslet> { static constexpr int fdim = 3, odim = 3; };
+template <> struct KindTraits<kStresslet> { static constexpr int fdim = 6, odim = 3; };  // sym6 combinations
+template <> struct KindTraits<kStokesletGrad> { static constexpr int fdim = 3, odim = 10; };
+template <> struct KindTraits<kStressletGrad> { static constexpr int fdim = 6, odim = 10; };
 
 struct PairArgs {
     const double *r_src;   // [n_src_pad*3]   padded to a multiple of kSrcTile (pads replicate the last source)
@@ -353,6 +358,89 @@ __device__ __forceinline__ void stresslet_two_sources(const double (&tx)[T], con
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Velocity gradient and pressure of one source against the thread's T targets (the gradient kinds).  r = x_trg - x_src,
+// y = 1/|r| with the velocity kernels' seed, Newton step and r == 0 rule (a coincident pair adds exactly 0 everywhere).
+// The pressure output carries 2 (pressure numerator): with the velocity kind's post-scale s / eta it holds p / eta.
+//   Stokeslet:  G_ij = d_i (f_j y^3 - 3 (f.r) y^5 r_j) - f_i r_j y^3 + delta_ij (f.r) y^3,  P = 2 (f.r) y^3
+//   stresslet:  G_ij = d_i (h_j y^5 - 5 A y^7 r_j) + delta_ij A y^5,  h = grad_r A = 2 S_sym r,  A = r.S.r,
+//               P = 2 A y^5 - (2/3) tr(S) y^3       (the -3 of the post-scale is kappa's)
+// 10 accumulators per target; every output of a pair is an FMA chain into its accumulator.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ double rsqrt_or_zero(double r2) {
+    double y;
+    asm("rsqrt.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(r2));
+    if (__double2hiint(r2) < 0x00100000)
+        y = 0.0;
+    const double e = fma(-r2 * y, y, 1.0);
+    return fma(y, e * fma(0.375, e, 0.5), y);
+}
+
+template <int T>
+__device__ __forceinline__ void stokeslet_grad_source(const double (&tx)[T], const double (&ty)[T],
+                                                      const double (&tz)[T], const double (&s)[3],
+                                                      const double (&f)[3], double (&g)[10][T]) {
+#pragma unroll
+    for (int t = 0; t < T; ++t) {
+        const double d[3] = {tx[t] - s[0], ty[t] - s[1], tz[t] - s[2]};
+        const double y = rsqrt_or_zero(fma(d[2], d[2], fma(d[1], d[1], d[0] * d[0])));
+        const double y2 = y * y;
+        const double y3 = y2 * y;
+        const double a = fma(f[2], d[2], fma(f[1], d[1], f[0] * d[0])) * y3; // (f.r) / r^3
+        const double b = 3.0 * a * y2;                                        // 3 (f.r) / r^5
+        double p[3], q[3];
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            q[j] = d[j] * y3;
+            p[j] = fma(-d[j], b, f[j] * y3);
+        }
+#pragma unroll
+        for (int i = 0; i < 3; ++i)
+#pragma unroll
+            for (int j = 0; j < 3; ++j)
+                g[3 * i + j][t] = fma(-f[i], q[j], fma(d[i], p[j], g[3 * i + j][t]));
+#pragma unroll
+        for (int i = 0; i < 3; ++i)
+            g[4 * i][t] += a;
+        g[9][t] = fma(2.0, a, g[9][t]);
+    }
+}
+
+template <int T>
+__device__ __forceinline__ void stresslet_grad_source(const double (&tx)[T], const double (&ty)[T],
+                                                      const double (&tz)[T], const double (&s)[3],
+                                                      const double (&w)[6], double (&g)[10][T]) {
+    // w = (sxx, syy, szz, sxy+syx, sxz+szx, syz+szy); tr(S) = w0 + w1 + w2
+    const double tr23 = (2.0 / 3.0) * (w[0] + w[1] + w[2]);
+#pragma unroll
+    for (int t = 0; t < T; ++t) {
+        const double d[3] = {tx[t] - s[0], ty[t] - s[1], tz[t] - s[2]};
+        const double y = rsqrt_or_zero(fma(d[2], d[2], fma(d[1], d[1], d[0] * d[0])));
+        const double y2 = y * y;
+        const double y3 = y2 * y;
+        const double y5 = y3 * y2;
+        double h[3]; // grad_r (r.S.r)
+        h[0] = fma(2.0 * w[0], d[0], fma(w[3], d[1], w[4] * d[2]));
+        h[1] = fma(w[3], d[0], fma(2.0 * w[1], d[1], w[5] * d[2]));
+        h[2] = fma(w[4], d[0], fma(w[5], d[1], 2.0 * w[2] * d[2]));
+        const double A5 = 0.5 * fma(h[2], d[2], fma(h[1], d[1], h[0] * d[0])) * y5; // A / r^5
+        const double c = 5.0 * A5 * y2;
+        double v[3];
+#pragma unroll
+        for (int j = 0; j < 3; ++j)
+            v[j] = fma(-c, d[j], h[j] * y5);
+#pragma unroll
+        for (int i = 0; i < 3; ++i)
+#pragma unroll
+            for (int j = 0; j < 3; ++j)
+                g[3 * i + j][t] = fma(d[i], v[j], g[3 * i + j][t]);
+#pragma unroll
+        for (int i = 0; i < 3; ++i)
+            g[4 * i][t] += A5;
+        g[9][t] = fma(2.0, A5, fma(-tr23, y3, g[9][t]));
+    }
+}
+
 // shared-memory footprint of the main kernel
 template <int KIND, int T, bool EXCL = false> struct SmemLayout {
     static constexpr int fdim = KindTraits<KIND>::fdim;
@@ -437,7 +525,9 @@ __global__ void __launch_bounds__(kCtaThreads, MINB) pair_sum_kernel(const PairA
     }
     __syncthreads(); // barrier init + target block visible to everyone
 
+    constexpr int kOut = KindTraits<KIND>::odim;
     double tx[T], ty[T], tz[T], ux[T], uy[T], uz[T];
+    double g[kOut][T]; // the gradient kinds' outputs (the velocity kinds use ux, uy, uz)
     int tfid[T];
 #pragma unroll
     for (int t = 0; t < T; ++t) {
@@ -447,6 +537,10 @@ __global__ void __launch_bounds__(kCtaThreads, MINB) pair_sum_kernel(const PairA
         ty[t] = trg_s[3 * i + 1];
         tz[t] = trg_s[3 * i + 2];
         ux[t] = uy[t] = uz[t] = 0.0;
+        if constexpr (kOut > 3)
+#pragma unroll
+            for (int o = 0; o < kOut; ++o)
+                g[o][t] = 0.0;
     }
 
     for (int k = 0; k < n_tiles; ++k) {
@@ -480,12 +574,24 @@ __global__ void __launch_bounds__(kCtaThreads, MINB) pair_sum_kernel(const PairA
                     ida = id2.x, idb = id2.y;
                 }
                 stokeslet_two_sources<T, EXCL>(tx, ty, tz, sa, fa, sb, fb, ux, uy, uz, tfid, ida, idb);
-            } else {
+            } else if constexpr (KIND == kStresslet) {
                 const double2 f0 = fs[6 * j + 0], f1 = fs[6 * j + 1], f2 = fs[6 * j + 2];
                 const double2 f3 = fs[6 * j + 3], f4 = fs[6 * j + 4], f5 = fs[6 * j + 5];
                 const double fa[6] = {f0.x, f0.y, f1.x, f1.y, f2.x, f2.y};
                 const double fb[6] = {f3.x, f3.y, f4.x, f4.y, f5.x, f5.y};
                 stresslet_two_sources<T>(tx, ty, tz, sa, fa, sb, fb, ux, uy, uz);
+            } else if constexpr (KIND == kStokesletGrad) {
+                const double2 f0 = fs[3 * j + 0], f1 = fs[3 * j + 1], f2 = fs[3 * j + 2];
+                const double fa[3] = {f0.x, f0.y, f1.x}, fb[3] = {f1.y, f2.x, f2.y};
+                stokeslet_grad_source<T>(tx, ty, tz, sa, fa, g);
+                stokeslet_grad_source<T>(tx, ty, tz, sb, fb, g);
+            } else {
+                const double2 f0 = fs[6 * j + 0], f1 = fs[6 * j + 1], f2 = fs[6 * j + 2];
+                const double2 f3 = fs[6 * j + 3], f4 = fs[6 * j + 4], f5 = fs[6 * j + 5];
+                const double fa[6] = {f0.x, f0.y, f1.x, f1.y, f2.x, f2.y};
+                const double fb[6] = {f3.x, f3.y, f4.x, f4.y, f5.x, f5.y};
+                stresslet_grad_source<T>(tx, ty, tz, sa, fa, g);
+                stresslet_grad_source<T>(tx, ty, tz, sb, fb, g);
             }
         }
         __syncwarp();
@@ -493,14 +599,20 @@ __global__ void __launch_bounds__(kCtaThreads, MINB) pair_sum_kernel(const PairA
             mbar_arrive(&empty_bar[s]);
     }
 
-    double *out = a.partial + (size_t)blockIdx.y * (size_t)a.n_trg * 3;
+    double *out = a.partial + (size_t)blockIdx.y * (size_t)a.n_trg * kOut;
 #pragma unroll
     for (int t = 0; t < T; ++t) {
         const long long i = t_base + t * kCtaThreads + tid;
         if (i < a.n_trg) {
-            out[3 * i + 0] = ux[t];
-            out[3 * i + 1] = uy[t];
-            out[3 * i + 2] = uz[t];
+            if constexpr (kOut == 3) {
+                out[3 * i + 0] = ux[t];
+                out[3 * i + 1] = uy[t];
+                out[3 * i + 2] = uz[t];
+            } else {
+#pragma unroll
+                for (int o = 0; o < kOut; ++o)
+                    out[kOut * i + o] = g[o][t];
+            }
         }
     }
 }

@@ -117,6 +117,8 @@ class Listener {
                   const double *x, const int32_t *body_kind, const double *body_radii, int periphery_interaction,
                   bool device, cudaStream_t st);
     int velocity(skb_flow *fl, const double *r_trg, long long n_trg, double *vel);
+    // skb_flow_listener_gradient: d u_i / d x_j (9 per target) and the pressure (1 per target)
+    int gradient(skb_flow *fl, const double *r_trg, long long n_trg, double *grad, double *pressure);
     int lines(skb_flow *fl, int kind, const double *x0, int n_lines, const ::skb_line_request *req, double *x,
               double *t, double *val, int32_t *n_points, int32_t *status);
 
@@ -127,6 +129,9 @@ class Listener {
     int current(const skb_flow *fl, const char *who) const;
     // System::velocity_at_targets of the frame at the n_trg device targets d_trg into d_v, on the flow's stream
     int eval(skb_flow *fl, const double *d_trg, long long n_trg, double *d_v);
+    // the arbitrary-target evaluators take the n_trg device targets d_trg (the plain kernel only), and the host-target
+    // calls are told to upload their own again
+    int take_targets(skb_flow *fl, const double *d_trg, long long n_trg);
 
     bool set_ = false;
     unsigned long long version_ = 0;
@@ -135,6 +140,7 @@ class Listener {
     DevBuf ff_, sd_, bd_, f_, t_, rigid_; // strengths; per body [kind, r0, r1, r2, cx, cy, cz, U, omega]
     DevBuf xf_, sb_, ten_; // set_state: the packed [x; y; z; T] per fiber; the host form's shell and body blocks, tension
     DevBuf trg_, vel_;                     // targets and velocities of one evaluation
+    DevBuf g10_, grad_, p_;                // gradient: the sums (10 per target), then the gradient and the pressure
     // lines: state (SoA) and per-line output; slot -> line map and the active count of the last compaction
     DevBuf st_x_, st_t_, st_dt_, st_k_, st_int_, out_x_, out_t_, out_val_, slots_, n_act_;
     PinnedHost h_n_act_;
@@ -317,7 +323,12 @@ int add_sources(skb_flow *fl, const double *d_trg, long long n_trg, double eta, 
 // them: d_ff 3 per fiber node, d_sd 3 per periphery node, d_bd 3 per body node, d_f and d_t 3 per body
 int velocity_dev(skb_flow *fl, const double *d_trg, long long n_trg, const double *d_ff, const double *d_sd,
                  const double *d_bd, const double *d_f, const double *d_t, double eta, double *d_v);
-int load_source_kernels(); // the kernels of add_sources, loaded now
+// The velocity gradient and the pressure of the same sum (and the same evaluators' targets) into d_g, 10 per target:
+// d u_i / d x_j at 10 t + 3 i + j, and the pressure over eta at 10 t + 9 (the pair kernels' post-scale carries 1 / eta
+// for all ten outputs).  Overwrites d_g
+int gradient_dev(skb_flow *fl, const double *d_trg, long long n_trg, const double *d_ff, const double *d_sd,
+                 const double *d_bd, const double *d_f, const double *d_t, double eta, double *d_g);
+int load_source_kernels(); // the kernels of add_sources and gradient_dev, loaded now
 
 // ---- skb_system.cu: the whole-system calls ----
 // the whole solution vector's size (of every member alike)

@@ -19,7 +19,8 @@ namespace skb {
 struct DeviceInfo {
     int dev = 0;
     int num_sms = 0;
-    int occupancy[2][4] = {{1, 1, 1, 1}, {1, 1, 1, 1}}; // [kind][T index: 1,2,4,8] resident CTAs / SM
+    // [kind][T index: 1,2,4,8] resident CTAs / SM; the gradient kinds (2, 3) run at kGradT only
+    int occupancy[4][4] = {{1, 1, 1, 1}, {1, 1, 1, 1}, {1, 1, 1, 1}, {1, 1, 1, 1}};
 };
 
 struct LaunchPlan {
@@ -134,8 +135,9 @@ int launch_pair_sum(const DeviceInfo &di, int kind, const double *d_r_src, const
                     long long n_src_pad, const double *d_r_trg, long long n_trg, double *d_partial,
                     const LaunchPlan &plan, cudaStream_t st, const int *d_src_fid = nullptr,
                     const int *d_trg_fid = nullptr);
+// width: outputs per target (3, or 10 for the gradient kinds)
 int launch_reduce(const double *d_partial, double *d_u, long long n_trg, int n_splits, double scale, int accumulate,
-                  cudaStream_t st);
+                  cudaStream_t st, int width = 3);
 
 // kRaw: strengths as the caller ships them (3 or 9 per source); kNormalDensity: density, stresslet formed on the device;
 // kPacked: already in the kernels' packed, padded layout ([n_pad*3] weighted Stokeslet strengths / [n_pad*6] sym6
@@ -679,6 +681,13 @@ namespace skb {
 int eval_on_device(skb_ctx *ctx, DeviceState &d, int kind, StrengthMode mode, const double *d_f_raw, double two_eta,
                    double *d_u_out, int accumulate, cudaStream_t st, bool record_events, int *launches,
                    LaunchPlan *plan_out, double scale_mul, const EvalOpts &opts = EvalOpts());
+
+// The velocity gradient and pressure of d's sources of `kind` (strengths as eval_on_device takes them) at d's targets,
+// through the gradient kinds of the plain kernel: d_g[10 t + 3 i + j] += scale_mul * [1 | -3]/(8 pi) * sum of
+// d u_i / d x_j, and d_g[10 t + 9] += the same scale times 2 x the pressure numerator (p / eta when scale_mul is
+// 1 / eta).  Always accumulates; nothing to do without targets or sources.
+int eval_gradient_on_device(DeviceState &d, int kind, StrengthMode mode, const double *d_f_raw, double two_eta,
+                            double *d_g, cudaStream_t st, int *launches, double scale_mul);
 
 // strengths -> the kernels' packed, padded layout in s.f_packed (what eval_on_device does first); sets s.f_cur
 int pack_on_device(DeviceState &d, int kind, StrengthMode mode, const double *d_f_raw, double two_eta, cudaStream_t st,

@@ -20,6 +20,7 @@ static int load_listener_kernels() {
         return SKB_OK;
     cudaFuncAttributes fa;
     CUDA_TRY(cudaFuncGetAttributes(&fa, interior_replace_kernel));
+    CUDA_TRY(cudaFuncGetAttributes(&fa, gradient_finish_kernel));
     CUDA_TRY(cudaFuncGetAttributes(&fa, listener_state_kernel));
     CUDA_TRY(cudaFuncGetAttributes(&fa, line_init_kernel));
     CUDA_TRY(cudaFuncGetAttributes(&fa, line_compact_kernel));
@@ -210,7 +211,7 @@ int Listener::current(const skb_flow *fl, const char *who) const {
     return SKB_OK;
 }
 
-int Listener::eval(skb_flow *fl, const double *d_trg, long long n_trg, double *d_v) {
+int Listener::take_targets(skb_flow *fl, const double *d_trg, long long n_trg) {
     skb_ctx *ctxs[3] = {fl->fib[0].get(), fl->shell[0].get(), fl->body[0].get()};
     for (skb_ctx *c : ctxs)
         SKB_TRY(skb_set_targets_device(c, d_trg, n_trg, fl->stream));
@@ -221,6 +222,11 @@ int Listener::eval(skb_flow *fl, const double *d_trg, long long n_trg, double *d
     fl->tc_fib.invalidate();
     fl->tc_shell.invalidate();
     fl->tc_body.invalidate();
+    return SKB_OK;
+}
+
+int Listener::eval(skb_flow *fl, const double *d_trg, long long n_trg, double *d_v) {
+    SKB_TRY(take_targets(fl, d_trg, n_trg));
     SKB_TRY(velocity_dev(fl, d_trg, n_trg, (const double *)ff_.ptr, (const double *)sd_.ptr, (const double *)bd_.ptr,
                          (const double *)f_.ptr, (const double *)t_.ptr, eta_, d_v));
     if (n_interior_ == 0)
@@ -247,6 +253,42 @@ int Listener::velocity(skb_flow *fl, const double *r_trg, long long n_trg, doubl
         },
         [&] { return eval(fl, (const double *)trg_.ptr, n_trg, (double *)vel_.ptr); },
         [&] { return download(fl, vel, vel_, (size_t)n_trg * 3); });
+}
+
+int Listener::gradient(skb_flow *fl, const double *r_trg, long long n_trg, double *grad, double *pressure) {
+    const char *who = "skb_flow_listener_gradient";
+    if (n_trg < 0 || (n_trg > 0 && (!r_trg || !grad || !pressure)))
+        return set_error(SKB_ERR_INVALID, "%s: bad arguments", who);
+    SKB_TRY(current(fl, who));
+    begin_stats(fl);
+    if (n_trg == 0)
+        return SKB_OK;
+    CUDA_TRY(cudaSetDevice(fl->dev));
+    const double *d_trg = nullptr;
+    auto work = [&]() -> int {
+        SKB_TRY(take_targets(fl, d_trg, n_trg));
+        SKB_TRY(gradient_dev(fl, d_trg, n_trg, (const double *)ff_.ptr, (const double *)sd_.ptr,
+                             (const double *)bd_.ptr, (const double *)f_.ptr, (const double *)t_.ptr, eta_,
+                             (double *)g10_.ptr));
+        gradient_finish_kernel<<<blocks(n_trg, kLineThreads), kLineThreads, 0, fl->cur>>>(
+            d_trg, n_trg, (const double *)rigid_.ptr, fl->n_bodies, eta_, (const double *)g10_.ptr,
+            (double *)grad_.ptr, (double *)p_.ptr);
+        return launched(&fl->launches);
+    };
+    return host_frame(
+        fl,
+        [&]() -> int {
+            SKB_TRY(upload(fl, trg_, r_trg, (size_t)n_trg * 3));
+            d_trg = (const double *)trg_.ptr;
+            SKB_TRY(g10_.ensure((size_t)n_trg * 80));
+            SKB_TRY(grad_.ensure((size_t)n_trg * 72));
+            return p_.ensure((size_t)n_trg * 8);
+        },
+        work,
+        [&]() -> int {
+            SKB_TRY(download(fl, grad, grad_, (size_t)n_trg * 9));
+            return download(fl, pressure, p_, (size_t)n_trg);
+        });
 }
 
 static int line_args(const char *who, int kind, const double *x0, int n_lines, const skb_line_request *req,
@@ -411,6 +453,12 @@ int skb_flow_listener_velocity(skb_flow *fl, const double *r_trg, int64_t n_trg,
     if (!fl)
         return set_error(SKB_ERR_INVALID, "skb_flow_listener_velocity: NULL flow");
     return fl->listener.velocity(fl, r_trg, n_trg, vel);
+}
+
+int skb_flow_listener_gradient(skb_flow *fl, const double *r_trg, int64_t n_trg, double *grad, double *pressure) {
+    if (!fl)
+        return set_error(SKB_ERR_INVALID, "skb_flow_listener_gradient: NULL flow");
+    return fl->listener.gradient(fl, r_trg, n_trg, grad, pressure);
 }
 
 int skb_flow_listener_lines(skb_flow *fl, int kind, const double *x0, int32_t n_lines, const skb_line_request *req,

@@ -154,11 +154,54 @@ int skb::velocity_dev(skb_flow *fl, const double *d_trg, long long n_trg, const 
     return add_sources(fl, d_trg, n_trg, eta, d_v, fl->cur);
 }
 
+int skb::gradient_dev(skb_flow *fl, const double *d_trg, long long n_trg, const double *d_ff, const double *d_sd,
+                      const double *d_bd, const double *d_f, const double *d_t, double eta, double *d_g) {
+    if (n_trg == 0)
+        return SKB_OK;
+    cudaStream_t st = fl->cur;
+    const double c = 1.0 / (8.0 * M_PI * eta);
+    const int bs = 128;
+    const unsigned nblk = (unsigned)((n_trg + bs - 1) / bs);
+    CUDA_TRY(cudaMemsetAsync(d_g, 0, (size_t)n_trg * 80, st));
+    // the sources of velocity_dev in its order: fibers, bodies (surface, centres' forces and torques), periphery
+    DeviceState &df = fl->fib[0]->devs[0], &db = fl->body[0]->devs[0], &ds = fl->shell[0]->devs[0];
+    SKB_TRY(eval_gradient_on_device(df, SKB_STOKESLET, kRaw, d_ff, 0.0, d_g, st, &fl->launches, 1.0 / eta));
+    fl->pairs += fl->n_fib * n_trg;
+    if (fl->n_bodies > 0) {
+        SKB_TRY(eval_gradient_on_device(db, SKB_STRESSLET, kNormalDensity, d_bd, 2.0 * eta, d_g, st, &fl->launches,
+                                        1.0 / eta));
+        SKB_TRY(eval_gradient_on_device(db, SKB_STOKESLET, kRaw, d_f, 0.0, d_g, st, &fl->launches, 1.0 / eta));
+        rotlet_grad_add_kernel<<<nblk, bs, 0, st>>>((const double *)fl->centers.ptr, d_t, fl->n_bodies, d_trg, n_trg,
+                                                    c, kReg * kReg, kEps * kEps, d_g);
+        SKB_TRY(launched(&fl->launches));
+        fl->pairs += (fl->n_body + 2 * (long long)fl->n_bodies) * n_trg;
+    }
+    SKB_TRY(eval_gradient_on_device(ds, SKB_STRESSLET, kNormalDensity, d_sd, 2.0 * eta, d_g, st, &fl->launches,
+                                    1.0 / eta));
+    fl->pairs += fl->n_shell * n_trg;
+    if (fl->n_points > 0) {
+        oseen_grad_add_kernel<<<nblk, bs, 0, st>>>((const double *)fl->pt_pos.ptr, (const double *)fl->pt_force.ptr,
+                                                   fl->n_points, d_trg, n_trg, c, kReg * kReg, kEps, d_g);
+        rotlet_grad_add_kernel<<<nblk, bs, 0, st>>>((const double *)fl->pt_pos.ptr, (const double *)fl->pt_torque.ptr,
+                                                    fl->n_points, d_trg, n_trg, c, kReg * kReg, kEps * kEps, d_g);
+        SKB_TRY(launched(&fl->launches, 2));
+    }
+    if (fl->has_background) {
+        background_grad_add_kernel<<<nblk, bs, 0, st>>>(n_trg, fl->bg_comp[0], fl->bg_comp[1], fl->bg_comp[2],
+                                                        fl->bg_scale[0], fl->bg_scale[1], fl->bg_scale[2], d_g);
+        SKB_TRY(launched(&fl->launches));
+    }
+    return SKB_OK;
+}
+
 int skb::load_source_kernels() {
     cudaFuncAttributes fa;
     CUDA_TRY(cudaFuncGetAttributes(&fa, oseen_contract_add_kernel));
     CUDA_TRY(cudaFuncGetAttributes(&fa, rotlet_add_kernel));
     CUDA_TRY(cudaFuncGetAttributes(&fa, background_add_kernel));
+    CUDA_TRY(cudaFuncGetAttributes(&fa, oseen_grad_add_kernel));
+    CUDA_TRY(cudaFuncGetAttributes(&fa, rotlet_grad_add_kernel));
+    CUDA_TRY(cudaFuncGetAttributes(&fa, background_grad_add_kernel));
     return SKB_OK;
 }
 

@@ -75,6 +75,10 @@ template <int KIND, int T, int MINB> static int occupancy_variant() {
     default: CALL(KIND, 8, 2); break;                                                                                 \
     }
 
+// the gradient kinds' one configuration: 10 accumulators and 3 coordinates per target leave room for two targets per
+// thread at four CTAs per SM (-Xptxas -v: 122 registers, no spills, no stack frame)
+constexpr int kGradT = 2, kGradTIndex = 1, kGradMinB = 4;
+
 DeviceInfo query_device(int dev) {
     DeviceInfo di;
     di.dev = dev;
@@ -95,6 +99,8 @@ DeviceInfo query_device(int dev) {
 #undef OCC_CALL
             di.occupancy[k][ti] = occ;
         }
+    di.occupancy[kStokesletGrad][kGradTIndex] = occupancy_variant<kStokesletGrad, kGradT, kGradMinB>();
+    di.occupancy[kStressletGrad][kGradTIndex] = occupancy_variant<kStressletGrad, kGradT, kGradMinB>();
     return di;
 }
 
@@ -179,6 +185,12 @@ int launch_pair_sum(const DeviceInfo &di, int kind, const double *d_r_src, const
         SKB_DISPATCH_T(kStokeslet, plan.T, LAUNCH_CALL_EXCL)
     } else if (kind == kStokeslet) {
         SKB_DISPATCH_T(kStokeslet, plan.T, LAUNCH_CALL)
+    } else if (kind == kStokesletGrad || kind == kStressletGrad) {
+        if (plan.T != kGradT)
+            return set_error(SKB_ERR_INVALID, "launch_pair_sum: the gradient kinds run at T = %d (plan: %d)", kGradT,
+                             plan.T);
+        e = kind == kStokesletGrad ? launch_variant<kStokesletGrad, kGradT, kGradMinB>(a, grid, st)
+                                   : launch_variant<kStressletGrad, kGradT, kGradMinB>(a, grid, st);
     } else {
         SKB_DISPATCH_T(kStresslet, plan.T, LAUNCH_CALL)
     }
@@ -191,8 +203,8 @@ int launch_pair_sum(const DeviceInfo &di, int kind, const double *d_r_src, const
 }
 
 int launch_reduce(const double *d_partial, double *d_u, long long n_trg, int n_splits, double scale, int accumulate,
-                  cudaStream_t st) {
-    const long long n3 = 3 * n_trg;
+                  cudaStream_t st, int width) {
+    const long long n3 = width * n_trg;
     const int bs = 256;
     if (n_splits >= 4 * kReduceWideWarps && n3 <= 32LL * 4096) // few targets, many splits
         reduce_partials_wide_kernel<<<(unsigned)((n3 + 31) / 32), 32 * kReduceWideWarps, 0, st>>>(
@@ -354,6 +366,8 @@ int skb::prepare_device(int dev) {
 #undef SMEM_CALL
 #undef SMEM_CALL_EXCL
     }
+    CUDA_TRY((set_smem_variant<kStokesletGrad, kGradT, kGradMinB>()));
+    CUDA_TRY((set_smem_variant<kStressletGrad, kGradT, kGradMinB>()));
     SKB_TRY(prepare_sym_kernels());
     CUDA_TRY(cudaFuncSetAttribute(dense_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kStreamSmemBytes));
     CUDA_TRY(cudaFuncSetAttribute(dense_stream_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
@@ -843,6 +857,25 @@ int eval_on_device(skb_ctx *ctx, DeviceState &d, int kind, StrengthMode mode, co
         CUDA_TRY(cudaEventRecord(d.ev_k1, st));
     if (plan_out)
         *plan_out = plan;
+    return SKB_OK;
+}
+
+int eval_gradient_on_device(DeviceState &d, int kind, StrengthMode mode, const double *d_f_raw, double two_eta,
+                            double *d_g, cudaStream_t st, int *launches, double scale_mul) {
+    SourceSet &s = d.src[kind];
+    if (d.n_trg == 0 || s.n <= 0)
+        return SKB_OK;
+    SKB_TRY(pack_on_device(d, kind, mode, d_f_raw, two_eta, st, launches));
+    const int gkind = kind == SKB_STOKESLET ? kStokesletGrad : kStressletGrad;
+    constexpr int kOut = KindTraits<kStokesletGrad>::odim;
+    const LaunchPlan plan = plan_launch(d.info, gkind, d.n_trg, (int)((s.n + kSrcTile - 1) / kSrcTile), kGradT, 0);
+    SKB_TRY(d.partial.ensure((size_t)plan.n_splits * (size_t)d.n_trg * kOut * 8));
+    SKB_TRY(launch_pair_sum(d.info, gkind, (const double *)s.r.ptr, s.f_cur, s.n, s.n_pad, (const double *)d.r_trg.ptr,
+                            d.n_trg, (double *)d.partial.ptr, plan, st));
+    const double scale = scale_mul * (kind == SKB_STOKESLET ? 1.0 : -3.0) / (8.0 * M_PI);
+    SKB_TRY(launch_reduce((const double *)d.partial.ptr, d_g, d.n_trg, plan.n_splits, scale, 1, st, kOut));
+    if (launches)
+        *launches += 2;
     return SKB_OK;
 }
 } // namespace skb
