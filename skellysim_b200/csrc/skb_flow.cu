@@ -11,13 +11,6 @@
 
 using namespace skb;
 
-static int create_ctx(int dev, CtxPtr &slot) {
-    skb_ctx *ctx = nullptr;
-    const int rc = skb_ctx_create_on(&dev, 1, &ctx);
-    slot.reset(ctx);
-    return rc;
-}
-
 int skb::upload(skb_flow *fl, DevBuf &buf, const double *h, size_t n_doubles) {
     return buf.upload(h, n_doubles * 8, fl->stream);
 }
@@ -89,17 +82,16 @@ int skb_flow_create(int device, skb_flow **out) {
         fl->graphs_enabled = atoi(e) != 0;
     if (const char *e = getenv("SKB_OVERLAP")) // A/B switch of skb_flow_set_overlap's default
         fl->bg.enabled = atoi(e) != 0;
-    for (int k = 0; k < 2; ++k) {
-        SKB_TRY(create_ctx(device, fl->fib[k]));
-        SKB_TRY(create_ctx(device, fl->shell[k]));
-        SKB_TRY(create_ctx(device, fl->body[k]));
-    }
+    SKB_TRY(prepare_device(device));
+    const DeviceInfo di = query_device(device);
     // empty classes until set_* is called
     for (int k = 0; k < 2; ++k) {
-        SKB_TRY(skb_set_sources(fl->fib[k].get(), SKB_STOKESLET, nullptr, 0));
-        SKB_TRY(skb_set_sources(fl->shell[k].get(), SKB_STRESSLET, nullptr, 0));
-        SKB_TRY(skb_set_sources(fl->body[k].get(), SKB_STRESSLET, nullptr, 0));
-        SKB_TRY(skb_set_sources(fl->body[k].get(), SKB_STOKESLET, nullptr, 0));
+        for (Evaluator *e : {&fl->fib[k], &fl->shell[k], &fl->body[k]})
+            SKB_TRY(e->init(di));
+        SKB_TRY(fl->fib[k].set_sources(SKB_STOKESLET, nullptr, 0, false, fl->stream));
+        SKB_TRY(fl->shell[k].set_sources(SKB_STRESSLET, nullptr, 0, false, fl->stream));
+        SKB_TRY(fl->body[k].set_sources(SKB_STRESSLET, nullptr, 0, false, fl->stream));
+        SKB_TRY(fl->body[k].set_sources(SKB_STOKESLET, nullptr, 0, false, fl->stream));
     }
     *out = fl.release();
     return SKB_OK;
@@ -140,7 +132,7 @@ int skb_flow_set_fibers(skb_flow *fl, const double *r_fib, const int *n_nodes, c
     fl->geom_version++;
     CUDA_TRY(cudaSetDevice(fl->dev));
     for (int k = 0; k < 2; ++k)
-        SKB_TRY(skb_set_sources(fl->fib[k].get(), SKB_STOKESLET, r_fib, fl->n_fib));
+        SKB_TRY(fl->fib[k].set_sources(SKB_STOKESLET, r_fib, fl->n_fib, false, fl->stream));
     if (n_fibers == 0)
         return SKB_OK;
     SKB_TRY(fl->fiber_offset.upload(off.data(), off.size() * 8, fl->stream));
@@ -158,10 +150,12 @@ int skb_flow_set_periphery(skb_flow *fl, const double *node_pos, const double *n
     fl->h_r_shell.assign(node_pos, node_pos + 3 * n_nodes);
     fl->mv_dirty = true;
     fl->geom_version++;
+    CUDA_TRY(cudaSetDevice(fl->dev));
     for (int k = 0; k < 2; ++k) {
-        SKB_TRY(skb_set_sources(fl->shell[k].get(), SKB_STRESSLET, node_pos, n_nodes));
-        SKB_TRY(skb_set_source_normals(fl->shell[k].get(), node_normal, n_nodes));
+        SKB_TRY(fl->shell[k].set_sources(SKB_STRESSLET, node_pos, n_nodes, false, fl->stream));
+        SKB_TRY(fl->shell[k].set_normals(node_normal, n_nodes, fl->stream));
     }
+    CUDA_TRY(cudaStreamSynchronize(fl->stream));
     return SKB_OK;
 }
 
@@ -179,16 +173,15 @@ int skb_flow_set_bodies(skb_flow *fl, const double *node_pos, const double *node
     fl->bodies.drop_links();
     fl->mv_dirty = true;
     fl->geom_version++;
+    CUDA_TRY(cudaSetDevice(fl->dev));
     for (int k = 0; k < 2; ++k) {
-        SKB_TRY(skb_set_sources(fl->body[k].get(), SKB_STRESSLET, node_pos, n_nodes));
-        SKB_TRY(skb_set_source_normals(fl->body[k].get(), node_normal, n_nodes));
-        SKB_TRY(skb_set_sources(fl->body[k].get(), SKB_STOKESLET, centers, n_bodies));
+        SKB_TRY(fl->body[k].set_sources(SKB_STRESSLET, node_pos, n_nodes, false, fl->stream));
+        SKB_TRY(fl->body[k].set_normals(node_normal, n_nodes, fl->stream));
+        SKB_TRY(fl->body[k].set_sources(SKB_STOKESLET, centers, n_bodies, false, fl->stream));
     }
-    if (n_bodies > 0) {
-        CUDA_TRY(cudaSetDevice(fl->dev));
+    if (n_bodies > 0)
         SKB_TRY(fl->centers.upload(centers, (size_t)n_bodies * 24, fl->stream));
-        CUDA_TRY(cudaStreamSynchronize(fl->stream));
-    }
+    CUDA_TRY(cudaStreamSynchronize(fl->stream));
     return SKB_OK;
 }
 
@@ -236,9 +229,9 @@ int skb_flow_group_init(skb_flow *fl, int rank, int size) {
     fl->mv_dirty = true;
     fl->ops.invalidate();
     fl->geom_version++;
-    // the same padded sizes the evaluator contexts use (set_sources_impl): the window replaces their f_packed
-    const long long n_pad_fib = fl->n_fib > 0 ? fl->fib[1]->devs[0].src[SKB_STOKESLET].n_pad : 0;
-    const long long n_pad_shell = fl->n_shell > 0 ? fl->shell[1]->devs[0].src[SKB_STRESSLET].n_pad : 0;
+    // the same padded sizes the evaluators use (Evaluator::set_sources): the window replaces their f_packed
+    const long long n_pad_fib = fl->n_fib > 0 ? fl->fib[1].src[SKB_STOKESLET].n_pad : 0;
+    const long long n_pad_shell = fl->n_shell > 0 ? fl->shell[1].src[SKB_STRESSLET].n_pad : 0;
     return fl->grp.init(rank, size, fl->n_fib, n_pad_fib, fl->n_shell, n_pad_shell, fl->n_body, fl->n_bodies,
                         fl->n_fibers);
 }
@@ -376,7 +369,7 @@ int skb_flow_set_target_ranges(skb_flow *fl, int fiber_begin, int fiber_end, int
 int skb_flow_last_sym_kernel(const skb_flow *fl, double *ms, int64_t *pairs) {
     if (!fl)
         return set_error(SKB_ERR_INVALID, "skb_flow_last_sym_kernel: NULL");
-    return skb_ctx_last_sym_kernel(fl->fib[1].get(), ms, pairs);
+    return fl->fib[1].last_sym_kernel(ms, pairs);
 }
 
 int skb_flow_last_stats(const skb_flow *fl, skb_flow_stats *out) {

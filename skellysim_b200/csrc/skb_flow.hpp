@@ -33,7 +33,6 @@ struct TargetCache {
         ++version;
     }
 };
-using CtxPtr = std::unique_ptr<skb_ctx, Destroyer<skb_ctx_destroy>>;
 
 // the step's device buffers: per fiber its item and error, per fiber node its new position and tension, the external
 // forces and torques of the RHS; and a pinned host copy of skb_flow_group_step_device's device inputs (3 per fiber
@@ -168,7 +167,7 @@ struct skb_flow {
     skb::DevBuf fiber_offset, fiber_length, r_fib, r_shell, r_body, centers;
     std::vector<double> h_r_fib, h_r_shell, h_r_body; // host copies to assemble the matvec target lists
     // evaluators: [0] arbitrary targets, [1] matvec target lists
-    skb::CtxPtr fib[2], shell[2], body[2];
+    skb::Evaluator fib[2], shell[2], body[2];
     skb::TargetCache tc_fib, tc_shell, tc_body;
     bool mv_dirty = true;
     int cross_mode = -1;    // fiber <-> periphery cross kernel in the matvec: -1 auto, 0 off, 1 on whenever applicable
@@ -241,7 +240,7 @@ struct skb_flow {
         skb_dense *dn = nullptr;   // pending background product of the call in flight (nullptr: none)
         bool launched = false;
     } bg;
-    skb::DevBuf scratch_u; // group mode: landing zone of eval_on_device's default output (never read)
+    skb::DevBuf scratch_u; // group mode: landing zone of Evaluator::eval's default output (never read)
     // staging
     skb::DevBuf in_fib, in_shell, in_body, in_force, in_torque, vel, tmp, x_fib, res_fib, vb, res_shell, tmp_b;
     skb::DevBuf sys_x, sys_y; // the whole solution vector in and out of the host forms of the system operator

@@ -617,91 +617,89 @@ struct CrossState {
     std::array<long long, 5> key = {-1, -1, -1, -1, -1};
 };
 
-} // namespace skb
-
-// ---- context internals (shared by skb_runtime.cu, skb_sym.cu and skb_matvec.cu) ----
+// One set of sources of an Evaluator: Stokeslet (kind 0) or stresslet (kind 1)
 struct SourceSet {
     long long n = -1; // -1 = never set
     long long n_pad = 0;
     bool has_normals = false;
-    skb::DevBuf r;       // padded positions
+    DevBuf r;       // padded positions
     bool has_weights = false;
-    skb::DevBuf normals; // optional (double layer formed on device)
-    skb::DevBuf weights; // optional per-source quadrature weight folded into the Stokeslet strengths
-    skb::DevBuf f_raw;   // strengths as shipped by the caller (3 or 9 per source; all-gather landing zone)
-    skb::DevBuf f_packed;
+    DevBuf normals; // optional (double layer formed on device)
+    DevBuf weights; // optional per-source quadrature weight folded into the Stokeslet strengths
+    DevBuf f_raw;   // strengths as shipped by the caller (3 or 9 per source; all-gather landing zone)
+    DevBuf f_packed;
     const double *f_cur = nullptr; // packed strengths of the evaluation in flight (f_packed, or the caller's kPacked buffer)
     // opt-in fused self-exclusion (SURVEY.md 8f N3): Stokeslet sources and the leading targets carry an id (the fiber
     // index); pairs with equal ids contribute 0.  excl_ids: [n_pad] source ids; excl_trg: [n_trg] target ids (-1 beyond
     // the leading n targets), built on demand for the plain kernel
     bool excl = false;
-    skb::DevBuf excl_ids, excl_trg;
+    DevBuf excl_ids, excl_trg;
     long long excl_trg_n = -1;
-    skb::SymState sym; // symmetric (Newton's third law) path of the Stokeslet self-interaction
+    SymState sym; // symmetric (Newton's third law) path of the Stokeslet self-interaction
 };
 
-struct DeviceState {
-    skb::DeviceInfo info;
-    skb::Stream stream;
-    skb::Stream aux_stream;              // remainder targets run beside the symmetric kernel
-    skb::Event ev_fork, ev_join;
-    skb::Event ev_t0, ev_t1, ev_k0, ev_k1;
-    skb::Event ev_s0, ev_s1; // around the symmetric kernel's launch (its live duration inside a step)
-    bool sym_timed = false;
-    long long trg_begin = 0, n_trg = 0; // this device's block of the global target list
-    // symmetric multi-device layout: targets = [all n_self leading targets | remainder rows [rem_begin, +rem_count)]
-    long long rem_begin = 0, rem_count = 0;
-    int sym_part = 0, sym_parts = 1;    // block rows of the self-interaction this device evaluates
-    skb::DevBuf u_rs;                   // reduce-scatter output (this device's chunk of the leading rows)
-    skb::DevBuf r_trg, u, partial, scratch;
+// The pair sums of one device (skb_runtime.cu; the symmetric path: skb_sym.cu): its targets, both sets of sources and
+// the buffers and streams of the plain and symmetric kernels.  A flow holds six, a context (skb_ctx.cu) one per device.
+// The setters enqueue their copies on the stream the caller passes and do not wait for them; the caller synchronises
+// before a host buffer it passed goes out of scope.
+struct Evaluator {
+    DeviceInfo info;
+    long long trg_begin = 0, n_trg = 0; // this device's block of the caller's target list
+    DevBuf r_trg, partial, scratch;
     SourceSet src[2];
-};
-
-struct skb_ctx {
-    ~skb_ctx(); // releases each device's state with that device current
-    std::vector<DeviceState> devs;
-    long long n_trg = -1;
+    Stream aux_stream; // remainder targets run beside the symmetric kernel (created on its first use)
+    Event ev_fork, ev_join;
+    Event ev_s0, ev_s1; // around the symmetric kernel's launch (its live duration inside a step)
+    bool sym_timed = false;
+    int sym_part = 0, sym_parts = 1; // block rows of the self-interaction this device evaluates
+    // how it evaluates
     int force_T = 0, force_S = 0;
     int sym_mode = -1; // -1 auto, 0 never, 1 whenever the sources are the leading targets
-    bool last_was_sym = false;
-    // single-process multi-device symmetric layout (host-pointer API): host copies of the positions decide it
-    std::vector<double> h_trg, h_src[2];
-    bool sym_layout = false;    // devices currently hold the targets in the symmetric layout
-    bool layout_dirty = false;  // positions changed since the devices' target layout was decided
-    long long n_self = 0;       // leading targets that are the Stokeslet sources
-    skb_eval_stats stats{};
-    bool kernel_events_pending = false; // device-pointer path: kernel_ms is read back lazily
-    void *nccl = nullptr; // NcclGroup*, multi-device contexts only
+    // kOwn: the targets are this evaluator's alone; a multi-device context's plain block layout (kBlocks) takes neither
+    // the symmetric path nor the device's exclusion check, and its symmetric layout (kShared) reduce-scatters the
+    // leading rows' partial sums, so the symmetric path may not decline there
+    enum Layout { kOwn, kBlocks, kShared } layout = kOwn;
+    bool last_was_sym = false; // the last Stokeslet evaluation took the symmetric path
+
+    // on device di.dev, prepared and current: the symmetric path's events; sym_mode from SKB_SYMMETRIC
+    int init(const DeviceInfo &di);
+    // n targets [3 n] from host or device memory, all of them this evaluator's (trg_begin 0)
+    int set_targets(const double *r, long long n, bool on_device, cudaStream_t st);
+    // n sources of `kind`; f_raw holds n_parts slots of ceil(n / n_parts) sources (a context's all-gather)
+    int set_sources(int kind, const double *r, long long n, bool on_device, cudaStream_t st, long long n_parts = 1);
+    int set_normals(const double *normals, long long n, cudaStream_t st); // of the stresslet sources (host)
+    int set_exclusion_ids(const int32_t *ids, long long n, cudaStream_t st); // of the Stokeslet sources (host); NULL: off
+    // strengths -> the kernels' packed, padded layout in s.f_packed (what eval does first); sets s.f_cur
+    int pack(int kind, StrengthMode mode, const double *d_f_raw, double two_eta, cudaStream_t st, int *launches);
+    // pack -> pair sums -> split reduction; strengths already resident at d_f_raw.
+    // result (=|+=) scale_mul * [1 | -3]/(8 pi) * sum.  ev_k0 / ev_k1, when given, are recorded around the pair sums
+    int eval(int kind, StrengthMode mode, const double *d_f_raw, double two_eta, double *d_u_out, int accumulate,
+             cudaStream_t st, int *launches, LaunchPlan *plan_out, double scale_mul, const EvalOpts &opts = EvalOpts(),
+             cudaEvent_t ev_k0 = nullptr, cudaEvent_t ev_k1 = nullptr);
+    // The velocity gradient and pressure of the sources of `kind` (strengths as eval takes them) at the targets,
+    // through the gradient kinds of the plain kernel: d_g[10 t + 3 i + j] += scale_mul * [1 | -3]/(8 pi) * sum of
+    // d u_i / d x_j, and d_g[10 t + 9] += the same scale times 2 x the pressure numerator (p / eta when scale_mul is
+    // 1 / eta).  Always accumulates; nothing to do without targets or sources.
+    int gradient(int kind, StrengthMode mode, const double *d_f_raw, double two_eta, double *d_g, cudaStream_t st,
+                 int *launches, double scale_mul);
+    // the duration and pairs of the last symmetric kernel, once it has run (0 before)
+    int last_sym_kernel(double *ms, int64_t *pairs) const;
 };
-
-
-namespace skb {
-// pack -> pair sums -> split reduction for one device; strengths already resident at d_f_raw.
-// result (=|+=) scale_mul * [1 | -3]/(8 pi) * sum.
-int eval_on_device(skb_ctx *ctx, DeviceState &d, int kind, StrengthMode mode, const double *d_f_raw, double two_eta,
-                   double *d_u_out, int accumulate, cudaStream_t st, bool record_events, int *launches,
-                   LaunchPlan *plan_out, double scale_mul, const EvalOpts &opts = EvalOpts());
-
-// The velocity gradient and pressure of d's sources of `kind` (strengths as eval_on_device takes them) at d's targets,
-// through the gradient kinds of the plain kernel: d_g[10 t + 3 i + j] += scale_mul * [1 | -3]/(8 pi) * sum of
-// d u_i / d x_j, and d_g[10 t + 9] += the same scale times 2 x the pressure numerator (p / eta when scale_mul is
-// 1 / eta).  Always accumulates; nothing to do without targets or sources.
-int eval_gradient_on_device(DeviceState &d, int kind, StrengthMode mode, const double *d_f_raw, double two_eta,
-                            double *d_g, cudaStream_t st, int *launches, double scale_mul);
-
-// strengths -> the kernels' packed, padded layout in s.f_packed (what eval_on_device does first); sets s.f_cur
-int pack_on_device(DeviceState &d, int kind, StrengthMode mode, const double *d_f_raw, double two_eta, cudaStream_t st,
-                   int *launches);
+int check_kind(int kind); // SKB_STOKESLET or SKB_STRESSLET
+// the refusals of set_sources' arguments
+int check_sources(int kind, const double *r, long long n);
+// dfma_probe_kernel on st: blocks x threads, iters FMA chains of 8 into d_out (pair_kernels.cuh)
+int launch_fp64_probe(double *d_out, int blocks, int threads, int iters, cudaStream_t st);
 
 // the symmetric and cross kernels (skb_sym.cu)
 long long sym_block_nodes(); // nodes per block of the symmetric kernel (its I side)
 long long sym_mem_budget();  // bytes its reverse partials may occupy on one device
 // are the first n_src targets bit-identical to the Stokeslet sources (s.sym.self_state, decided once per positions)?
-int ensure_self_state(DeviceState &d, SourceSet &s, cudaStream_t st);
-// Decide whether the symmetric path serves d's Stokeslet sources (*use) and make sure its plan and buffers exist
-int sym_prepare(skb_ctx *ctx, DeviceState &d, cudaStream_t st, int *use);
+int ensure_self_state(Evaluator &e, SourceSet &s, cudaStream_t st);
+// Decide whether the symmetric path serves e's Stokeslet sources (*use) and make sure its plan and buffers exist
+int sym_prepare(Evaluator &e, cudaStream_t st, int *use);
 // u[0 : 3 n_src] (=|+=) scale_mul / (8 pi) * sum over the square block, using the plan above.  Strengths are packed
-int sym_eval(DeviceState &d, double *d_u_out, int accumulate, cudaStream_t st, double scale_mul, int *launches);
+int sym_eval(Evaluator &ev, double *d_u_out, int accumulate, cudaStream_t st, double scale_mul, int *launches);
 LaunchPlan sym_launch_plan(const SourceSet &s); // the last symmetric launch, as the stats report it
 // fiber <-> periphery in one geometry pass (cross_kernels.cuh), on the plan of cs (made again for a new shape):
 // u_fib[n_rows x 3] (=|+=) scale_dl * (stresslet sums of ALL periphery nodes at fiber nodes [node0, node0 + n_rows));

@@ -212,12 +212,11 @@ int Listener::current(const skb_flow *fl, const char *who) const {
 }
 
 int Listener::take_targets(skb_flow *fl, const double *d_trg, long long n_trg) {
-    skb_ctx *ctxs[3] = {fl->fib[0].get(), fl->shell[0].get(), fl->body[0].get()};
-    for (skb_ctx *c : ctxs)
-        SKB_TRY(skb_set_targets_device(c, d_trg, n_trg, fl->stream));
+    for (Evaluator *e : {&fl->fib[0], &fl->shell[0], &fl->body[0]})
+        SKB_TRY(e->set_targets(d_trg, n_trg, true, fl->stream));
     // evaluation points are never taken for the fiber nodes: the plain kernel, without a device check (and its host
     // wait) for the symmetric one; the plain kernel's sum is right whatever the targets are
-    fl->fib[0]->devs[0].src[SKB_STOKESLET].sym.self_state = 0;
+    fl->fib[0].src[SKB_STOKESLET].sym.self_state = 0;
     // the host-target calls must upload their targets again (and not replay a graph captured with theirs)
     fl->tc_fib.invalidate();
     fl->tc_shell.invalidate();

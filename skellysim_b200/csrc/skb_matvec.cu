@@ -2,8 +2,9 @@
 // Periphery / BodyContainer flows of SkellySim at arbitrary targets, the point sources and the background flow, their
 // sum at arbitrary targets (System::velocity_at_targets) with the CUDA-graph replay of small calls, the matvec target
 // lists and matvec_core -- the hydrodynamic part of System::apply_matvec (src/core/system.cpp:284-316) -- and
-// apply_matvec_core around it.  Built on the pair-kernel contexts of skb_runtime.cu; everything between the upload of
-// the strengths and the download of the velocities stays on the device.  The flow object itself is skb_flow.cu.
+// apply_matvec_core around it.  Built on the flow's evaluators (Evaluator, skb_runtime.cu); everything between the
+// upload of the strengths and the download of the velocities stays on the device.  The flow object itself is
+// skb_flow.cu.
 #include "aux_kernels.cuh"
 #include "skb_flow.hpp"
 
@@ -22,10 +23,10 @@ constexpr double kEps = 1e-5;
 } // namespace
 
 // self term of the fibers (fcfd.cpp:203-210): d_vel rows [0, node_end - node_begin) are the fiber nodes
-// [node_begin, node_end), the packed strengths are those of ctx's last Stokeslet evaluation
-static int fiber_self_term(skb_flow *fl, skb_ctx *ctx, double eta, double *d_vel, long long node_begin,
+// [node_begin, node_end), the packed strengths are those of e's last Stokeslet evaluation
+static int fiber_self_term(skb_flow *fl, const Evaluator &e, double eta, double *d_vel, long long node_begin,
                            long long node_end) {
-    const SourceSet &s = ctx->devs[0].src[SKB_STOKESLET];
+    const SourceSet &s = e.src[SKB_STOKESLET];
     if (node_end <= node_begin || s.excl) // fused form: the pair kernels skipped every intra-fiber pair
         return SKB_OK;
     const size_t smem = (size_t)fl->max_fiber_nodes * 6 * sizeof(double);
@@ -42,7 +43,7 @@ int skb::install_fiber_sources(skb_flow *fl) {
                                       max_n * 48));
     // trapezoid weights straight into both Stokeslet source sets
     for (int k = 0; k < 2; ++k) {
-        SourceSet &s = fl->fib[k]->devs[0].src[SKB_STOKESLET];
+        SourceSet &s = fl->fib[k].src[SKB_STOKESLET];
         SKB_TRY(s.weights.ensure((size_t)fl->n_fib * 8));
         fiber_weights_kernel<<<n_fibers, 64, 0, fl->stream>>>((const long long *)fl->fiber_offset.ptr,
                                                               (const double *)fl->fiber_length.ptr, n_fibers,
@@ -53,71 +54,54 @@ int skb::install_fiber_sources(skb_flow *fl) {
     return SKB_OK;
 }
 
-// ---- device-side flows: ctx already has its targets and sources ------------------------------------------------
+// ---- device-side flows: the evaluator already has its targets and sources ---------------------------------------
 // mode / d_forces: the caller's forces (kRaw) or already packed strengths (kPacked).
 // subtract_self: the first (node_end - node_begin) targets are the fiber nodes [node_begin, node_end)
-static int fibers_dev(skb_flow *fl, skb_ctx *ctx, StrengthMode mode, const double *d_forces, double eta,
+static int fibers_dev(skb_flow *fl, Evaluator &e, StrengthMode mode, const double *d_forces, double eta,
                       int subtract_self, double *d_vel, int accumulate, long long node_begin, long long node_end) {
-    DeviceState &d = ctx->devs[0];
-    if (d.n_trg == 0)
-        return SKB_OK;
-    if (fl->n_fibers == 0) { // fiber_container_finite_difference.cpp:178-179
-        if (!accumulate)
-            CUDA_TRY(cudaMemsetAsync(d_vel, 0, (size_t)d.n_trg * 24, fl->cur));
-        return SKB_OK;
-    }
+    // (no fibers: zeros, or nothing to add, fiber_container_finite_difference.cpp:178-179)
     // weighted forces -> Stokeslet all-to-all, / eta  (fcfd.cpp:185-199, kernels.cpp:365)
-    SKB_TRY(eval_on_device(ctx, d, SKB_STOKESLET, mode, d_forces, 0.0, d_vel, accumulate, fl->cur, false,
-                           &fl->launches, nullptr, 1.0 / eta));
-    fl->pairs += fl->n_fib * d.n_trg;
+    SKB_TRY(e.eval(SKB_STOKESLET, mode, d_forces, 0.0, d_vel, accumulate, fl->cur, &fl->launches, nullptr, 1.0 / eta));
+    fl->pairs += fl->n_fib * e.n_trg;
     if (!subtract_self)
         return SKB_OK;
-    if (!d.src[SKB_STOKESLET].excl && d.n_trg < node_end - node_begin)
+    if (!e.src[SKB_STOKESLET].excl && e.n_trg < node_end - node_begin)
         return set_error(SKB_ERR_INVALID, "fiber flow with subtract_self needs the fiber nodes as the first "
-                                          "%lld targets (n_trg = %lld)", node_end - node_begin, d.n_trg);
-    return fiber_self_term(fl, ctx, eta, d_vel, node_begin, node_end);
+                                          "%lld targets (n_trg = %lld)", node_end - node_begin, e.n_trg);
+    return fiber_self_term(fl, e, eta, d_vel, node_begin, node_end);
 }
 
 // mode / d_density: the caller's densities (kNormalDensity) or already packed sym6 strengths (kPacked)
-static int periphery_dev(skb_flow *fl, skb_ctx *ctx, StrengthMode mode, const double *d_density, double eta,
+static int periphery_dev(skb_flow *fl, Evaluator &e, StrengthMode mode, const double *d_density, double eta,
                          double *d_vel, int accumulate) {
-    DeviceState &d = ctx->devs[0];
-    if (d.n_trg == 0)
-        return SKB_OK;
-    if (fl->n_shell == 0) { // periphery.cpp:57-58
-        if (!accumulate)
-            CUDA_TRY(cudaMemsetAsync(d_vel, 0, (size_t)d.n_trg * 24, fl->cur));
-        return SKB_OK;
-    }
+    // (no periphery: zeros, or nothing to add, periphery.cpp:57-58)
     // f_dl = 2 eta n (x) rho formed on the device, stresslet, / eta  (periphery.cpp:68-74, kernels.cpp:358)
-    SKB_TRY(eval_on_device(ctx, d, SKB_STRESSLET, mode, d_density, 2.0 * eta, d_vel, accumulate, fl->cur, false,
-                           &fl->launches, nullptr, 1.0 / eta));
-    fl->pairs += fl->n_shell * d.n_trg;
+    SKB_TRY(e.eval(SKB_STRESSLET, mode, d_density, 2.0 * eta, d_vel, accumulate, fl->cur, &fl->launches, nullptr,
+                   1.0 / eta));
+    fl->pairs += fl->n_shell * e.n_trg;
     return SKB_OK;
 }
 
-static int bodies_dev(skb_flow *fl, skb_ctx *ctx, const double *d_density, const double *d_force,
+static int bodies_dev(skb_flow *fl, Evaluator &e, const double *d_density, const double *d_force,
                       const double *d_torque, double eta, double *d_vel, int accumulate) {
-    DeviceState &d = ctx->devs[0];
-    if (d.n_trg == 0)
+    if (e.n_trg == 0)
         return SKB_OK;
     if (fl->n_bodies == 0) { // body_container.cpp:273-276
         if (!accumulate)
-            CUDA_TRY(cudaMemsetAsync(d_vel, 0, (size_t)d.n_trg * 24, fl->cur));
+            CUDA_TRY(cudaMemsetAsync(d_vel, 0, (size_t)e.n_trg * 24, fl->cur));
         return SKB_OK;
     }
     // stresslet of the surface nodes (body_container.cpp:296-305)
-    SKB_TRY(eval_on_device(ctx, d, SKB_STRESSLET, kNormalDensity, d_density, 2.0 * eta, d_vel, accumulate, fl->cur,
-                           false, &fl->launches, nullptr, 1.0 / eta));
+    SKB_TRY(e.eval(SKB_STRESSLET, kNormalDensity, d_density, 2.0 * eta, d_vel, accumulate, fl->cur, &fl->launches,
+                   nullptr, 1.0 / eta));
     // Stokeslet of the net forces at the centres (:327)
-    SKB_TRY(eval_on_device(ctx, d, SKB_STOKESLET, kRaw, d_force, 0.0, d_vel, 1, fl->cur, false, &fl->launches,
-                           nullptr, 1.0 / eta));
+    SKB_TRY(e.eval(SKB_STOKESLET, kRaw, d_force, 0.0, d_vel, 1, fl->cur, &fl->launches, nullptr, 1.0 / eta));
     // rotlet of the net torques at the centres (:335, kernels.cpp:206-242)
     const int bs = 128;
-    rotlet_add_kernel<<<(unsigned)((d.n_trg + bs - 1) / bs), bs, 0, fl->cur>>>(
-        (const double *)fl->centers.ptr, d_torque, fl->n_bodies, (const double *)d.r_trg.ptr, d.n_trg,
+    rotlet_add_kernel<<<(unsigned)((e.n_trg + bs - 1) / bs), bs, 0, fl->cur>>>(
+        (const double *)fl->centers.ptr, d_torque, fl->n_bodies, (const double *)e.r_trg.ptr, e.n_trg,
         1.0 / (8.0 * M_PI * eta), kReg * kReg, kEps * kEps, d_vel);
-    fl->pairs += (fl->n_body + 2 * (long long)fl->n_bodies) * d.n_trg;
+    fl->pairs += (fl->n_body + 2 * (long long)fl->n_bodies) * e.n_trg;
     return launched(&fl->launches);
 }
 
@@ -147,9 +131,9 @@ int skb::add_sources(skb_flow *fl, const double *d_trg, long long n_trg, double 
 int skb::velocity_dev(skb_flow *fl, const double *d_trg, long long n_trg, const double *d_ff, const double *d_sd,
                       const double *d_bd, const double *d_f, const double *d_t, double eta, double *d_v) {
     // fc_->flow(r_trg, f_on_fibers, eta, /*subtract_self=*/false) + bc_.flow + shell_->flow   system.cpp:355-359
-    SKB_TRY(fibers_dev(fl, fl->fib[0].get(), kRaw, d_ff, eta, 0, d_v, 0, 0, 0));
-    SKB_TRY(bodies_dev(fl, fl->body[0].get(), d_bd, d_f, d_t, eta, d_v, 1));
-    SKB_TRY(periphery_dev(fl, fl->shell[0].get(), kNormalDensity, d_sd, eta, d_v, 1));
+    SKB_TRY(fibers_dev(fl, fl->fib[0], kRaw, d_ff, eta, 0, d_v, 0, 0, 0));
+    SKB_TRY(bodies_dev(fl, fl->body[0], d_bd, d_f, d_t, eta, d_v, 1));
+    SKB_TRY(periphery_dev(fl, fl->shell[0], kNormalDensity, d_sd, eta, d_v, 1));
     // + psc_.flow(r_trg, eta, time) + bs_.flow(r_trg, eta)                                  system.cpp:358-359
     return add_sources(fl, d_trg, n_trg, eta, d_v, fl->cur);
 }
@@ -164,20 +148,18 @@ int skb::gradient_dev(skb_flow *fl, const double *d_trg, long long n_trg, const 
     const unsigned nblk = (unsigned)((n_trg + bs - 1) / bs);
     CUDA_TRY(cudaMemsetAsync(d_g, 0, (size_t)n_trg * 80, st));
     // the sources of velocity_dev in its order: fibers, bodies (surface, centres' forces and torques), periphery
-    DeviceState &df = fl->fib[0]->devs[0], &db = fl->body[0]->devs[0], &ds = fl->shell[0]->devs[0];
-    SKB_TRY(eval_gradient_on_device(df, SKB_STOKESLET, kRaw, d_ff, 0.0, d_g, st, &fl->launches, 1.0 / eta));
+    Evaluator &ef = fl->fib[0], &eb = fl->body[0], &es = fl->shell[0];
+    SKB_TRY(ef.gradient(SKB_STOKESLET, kRaw, d_ff, 0.0, d_g, st, &fl->launches, 1.0 / eta));
     fl->pairs += fl->n_fib * n_trg;
     if (fl->n_bodies > 0) {
-        SKB_TRY(eval_gradient_on_device(db, SKB_STRESSLET, kNormalDensity, d_bd, 2.0 * eta, d_g, st, &fl->launches,
-                                        1.0 / eta));
-        SKB_TRY(eval_gradient_on_device(db, SKB_STOKESLET, kRaw, d_f, 0.0, d_g, st, &fl->launches, 1.0 / eta));
+        SKB_TRY(eb.gradient(SKB_STRESSLET, kNormalDensity, d_bd, 2.0 * eta, d_g, st, &fl->launches, 1.0 / eta));
+        SKB_TRY(eb.gradient(SKB_STOKESLET, kRaw, d_f, 0.0, d_g, st, &fl->launches, 1.0 / eta));
         rotlet_grad_add_kernel<<<nblk, bs, 0, st>>>((const double *)fl->centers.ptr, d_t, fl->n_bodies, d_trg, n_trg,
                                                     c, kReg * kReg, kEps * kEps, d_g);
         SKB_TRY(launched(&fl->launches));
         fl->pairs += (fl->n_body + 2 * (long long)fl->n_bodies) * n_trg;
     }
-    SKB_TRY(eval_gradient_on_device(ds, SKB_STRESSLET, kNormalDensity, d_sd, 2.0 * eta, d_g, st, &fl->launches,
-                                    1.0 / eta));
+    SKB_TRY(es.gradient(SKB_STRESSLET, kNormalDensity, d_sd, 2.0 * eta, d_g, st, &fl->launches, 1.0 / eta));
     fl->pairs += fl->n_shell * n_trg;
     if (fl->n_points > 0) {
         oseen_grad_add_kernel<<<nblk, bs, 0, st>>>((const double *)fl->pt_pos.ptr, (const double *)fl->pt_force.ptr,
@@ -206,10 +188,11 @@ int skb::load_source_kernels() {
 }
 
 
-static int set_targets_cached(skb_ctx *ctx, TargetCache &tc, const double *r_trg, long long n_trg) {
-    if (tc.same(r_trg, n_trg) && ctx->n_trg == n_trg)
+static int set_targets_cached(skb_flow *fl, Evaluator &e, TargetCache &tc, const double *r_trg, long long n_trg) {
+    if (tc.same(r_trg, n_trg) && e.n_trg == n_trg)
         return SKB_OK;
-    SKB_TRY(skb_set_targets(ctx, r_trg, n_trg));
+    SKB_TRY(e.set_targets(r_trg, n_trg, false, fl->stream));
+    CUDA_TRY(cudaStreamSynchronize(fl->stream));
     tc.store(r_trg, n_trg);
     return SKB_OK;
 }
@@ -245,14 +228,12 @@ static unsigned long long buffer_key(const skb_flow *fl, int which) {
                             &fl->tmp,    &fl->pt_pos,   &fl->pt_force, &fl->pt_torque, &fl->centers, &fl->r_fib};
     for (const DevBuf *b : bufs)
         h = mix_key(h, (unsigned long long)(uintptr_t)b->ptr);
-    const skb_ctx *ctxs[] = {fl->fib[which].get(), fl->shell[which].get(), fl->body[which].get()};
-    for (const skb_ctx *c : ctxs) {
-        const DeviceState &d = c->devs[0];
-        h = mix_key(h, (unsigned long long)(uintptr_t)d.r_trg.ptr);
-        h = mix_key(h, (unsigned long long)(uintptr_t)d.partial.ptr);
+    for (const Evaluator *e : {&fl->fib[which], &fl->shell[which], &fl->body[which]}) {
+        h = mix_key(h, (unsigned long long)(uintptr_t)e->r_trg.ptr);
+        h = mix_key(h, (unsigned long long)(uintptr_t)e->partial.ptr);
         for (int k = 0; k < 2; ++k) {
-            h = mix_key(h, (unsigned long long)(uintptr_t)d.src[k].f_packed.ptr);
-            h = mix_key(h, (unsigned long long)(uintptr_t)d.src[k].r.ptr);
+            h = mix_key(h, (unsigned long long)(uintptr_t)e->src[k].f_packed.ptr);
+            h = mix_key(h, (unsigned long long)(uintptr_t)e->src[k].r.ptr);
         }
     }
     return h;
@@ -335,7 +316,7 @@ int skb_flow_fibers(skb_flow *fl, const double *r_trg, int64_t n_trg, const doub
         return set_error(SKB_ERR_INVALID, "skb_flow_fibers: bad arguments");
     CUDA_TRY(cudaSetDevice(fl->dev));
     begin_stats(fl);
-    SKB_TRY(set_targets_cached(fl->fib[0].get(), fl->tc_fib, r_trg, n_trg));
+    SKB_TRY(set_targets_cached(fl, fl->fib[0], fl->tc_fib, r_trg, n_trg));
     if (n_trg == 0)
         return SKB_OK;
     return host_frame(
@@ -345,7 +326,7 @@ int skb_flow_fibers(skb_flow *fl, const double *r_trg, int64_t n_trg, const doub
             return fl->vel.ensure((size_t)n_trg * 24);
         },
         [&] {
-            return fibers_dev(fl, fl->fib[0].get(), kRaw, (const double *)fl->in_fib.ptr, eta, subtract_self,
+            return fibers_dev(fl, fl->fib[0], kRaw, (const double *)fl->in_fib.ptr, eta, subtract_self,
                               (double *)fl->vel.ptr, 0, 0, fl->n_fib);
         },
         [&] { return download(fl, vel, fl->vel, (size_t)n_trg * 3); });
@@ -357,7 +338,7 @@ int skb_flow_periphery(skb_flow *fl, const double *r_trg, int64_t n_trg, const d
         return set_error(SKB_ERR_INVALID, "skb_flow_periphery: bad arguments");
     CUDA_TRY(cudaSetDevice(fl->dev));
     begin_stats(fl);
-    SKB_TRY(set_targets_cached(fl->shell[0].get(), fl->tc_shell, r_trg, n_trg));
+    SKB_TRY(set_targets_cached(fl, fl->shell[0], fl->tc_shell, r_trg, n_trg));
     if (n_trg == 0)
         return SKB_OK;
     return host_frame(
@@ -367,7 +348,7 @@ int skb_flow_periphery(skb_flow *fl, const double *r_trg, int64_t n_trg, const d
             return fl->vel.ensure((size_t)n_trg * 24);
         },
         [&] {
-            return periphery_dev(fl, fl->shell[0].get(), kNormalDensity, (const double *)fl->in_shell.ptr, eta,
+            return periphery_dev(fl, fl->shell[0], kNormalDensity, (const double *)fl->in_shell.ptr, eta,
                                  (double *)fl->vel.ptr, 0);
         },
         [&] { return download(fl, vel, fl->vel, (size_t)n_trg * 3); });
@@ -380,7 +361,7 @@ int skb_flow_bodies(skb_flow *fl, const double *r_trg, int64_t n_trg, const doub
         return set_error(SKB_ERR_INVALID, "skb_flow_bodies: bad arguments");
     CUDA_TRY(cudaSetDevice(fl->dev));
     begin_stats(fl);
-    SKB_TRY(set_targets_cached(fl->body[0].get(), fl->tc_body, r_trg, n_trg));
+    SKB_TRY(set_targets_cached(fl, fl->body[0], fl->tc_body, r_trg, n_trg));
     if (n_trg == 0)
         return SKB_OK;
     std::vector<double> f, t;
@@ -394,7 +375,7 @@ int skb_flow_bodies(skb_flow *fl, const double *r_trg, int64_t n_trg, const doub
             return fl->vel.ensure((size_t)n_trg * 24);
         },
         [&] {
-            return bodies_dev(fl, fl->body[0].get(), (const double *)fl->in_body.ptr, (const double *)fl->in_force.ptr,
+            return bodies_dev(fl, fl->body[0], (const double *)fl->in_body.ptr, (const double *)fl->in_force.ptr,
                               (const double *)fl->in_torque.ptr, eta, (double *)fl->vel.ptr, 0);
         },
         [&] { return download(fl, vel, fl->vel, (size_t)n_trg * 3); });
@@ -412,9 +393,9 @@ int skb_flow_velocity_at_targets(skb_flow *fl, const double *r_trg, int64_t n_tr
     CUDA_TRY(cudaSetDevice(fl->dev));
     begin_stats(fl);
     // the three "arbitrary target" evaluators share one cached target list
-    SKB_TRY(set_targets_cached(fl->fib[0].get(), fl->tc_fib, r_trg, n_trg));
-    SKB_TRY(set_targets_cached(fl->shell[0].get(), fl->tc_shell, r_trg, n_trg));
-    SKB_TRY(set_targets_cached(fl->body[0].get(), fl->tc_body, r_trg, n_trg));
+    SKB_TRY(set_targets_cached(fl, fl->fib[0], fl->tc_fib, r_trg, n_trg));
+    SKB_TRY(set_targets_cached(fl, fl->shell[0], fl->tc_shell, r_trg, n_trg));
+    SKB_TRY(set_targets_cached(fl, fl->body[0], fl->tc_body, r_trg, n_trg));
     if (n_trg == 0)
         return SKB_OK;
     std::vector<double> f, t;
@@ -431,7 +412,7 @@ int skb_flow_velocity_at_targets(skb_flow *fl, const double *r_trg, int64_t n_tr
         SKB_TRY(upload(fl, fl->in_body, s.bd, (size_t)fl->n_body * 3));
         SKB_TRY(upload(fl, fl->in_force, s.f, f.size()));
         SKB_TRY(upload(fl, fl->in_torque, s.t, t.size()));
-        SKB_TRY(velocity_dev(fl, (const double *)fl->fib[0]->devs[0].r_trg.ptr, n_trg, (const double *)fl->in_fib.ptr,
+        SKB_TRY(velocity_dev(fl, (const double *)fl->fib[0].r_trg.ptr, n_trg, (const double *)fl->in_fib.ptr,
                              (const double *)fl->in_shell.ptr, (const double *)fl->in_body.ptr,
                              (const double *)fl->in_force.ptr, (const double *)fl->in_torque.ptr, eta, d_v));
         return download(fl, s.v, fl->vel, (size_t)n_trg * 3);
@@ -515,29 +496,32 @@ int skb::prepare_matvec_targets(skb_flow *fl) {
     if (!use_cross)
         r_fb.insert(r_fb.end(), fl->h_r_fib.begin() + 3 * fl->fa, fl->h_r_fib.begin() + 3 * fl->fb);
     r_fb.insert(r_fb.end(), fl->h_r_body.begin() + 3 * fl->ba, fl->h_r_body.begin() + 3 * fl->bb);
+    Evaluator &ef = fl->fib[1];
+    std::vector<double> r_own; // the fiber evaluator's targets when they are not r_win
     if (sym_partial) {
         // fiber sources meet [ALL fiber nodes | own shell rows | own body rows]; with the cross kernel the periphery
         // rows are not targets of this evaluator
-        std::vector<double> r_sym;
-        r_sym.reserve((size_t)(nf + n_sw + n_bw) * 3);
-        r_sym.insert(r_sym.end(), fl->h_r_fib.begin(), fl->h_r_fib.end());
+        r_own.reserve((size_t)(nf + n_sw + n_bw) * 3);
+        r_own.insert(r_own.end(), fl->h_r_fib.begin(), fl->h_r_fib.end());
         if (!use_cross)
-            r_sym.insert(r_sym.end(), fl->h_r_shell.begin() + 3 * fl->sa, fl->h_r_shell.begin() + 3 * fl->sb);
-        r_sym.insert(r_sym.end(), fl->h_r_body.begin() + 3 * fl->ba, fl->h_r_body.begin() + 3 * fl->bb);
-        SKB_TRY(skb_ctx_set_symmetric(fl->fib[1].get(), 1));
-        SKB_TRY(skb_ctx_set_sym_partition(fl->fib[1].get(), fl->grp.rank(), fl->grp.size()));
-        SKB_TRY(skb_set_targets(fl->fib[1].get(), r_sym.data(), (long long)r_sym.size() / 3));
-    } else if (use_cross) {
-        std::vector<double> r_fibbody(fl->h_r_fib.begin() + 3 * fl->fa, fl->h_r_fib.begin() + 3 * fl->fb);
-        r_fibbody.insert(r_fibbody.end(), fl->h_r_body.begin() + 3 * fl->ba, fl->h_r_body.begin() + 3 * fl->bb);
-        SKB_TRY(skb_ctx_set_sym_partition(fl->fib[1].get(), 0, 1));
-        SKB_TRY(skb_set_targets(fl->fib[1].get(), r_fibbody.data(), (long long)r_fibbody.size() / 3));
+            r_own.insert(r_own.end(), fl->h_r_shell.begin() + 3 * fl->sa, fl->h_r_shell.begin() + 3 * fl->sb);
+        r_own.insert(r_own.end(), fl->h_r_body.begin() + 3 * fl->ba, fl->h_r_body.begin() + 3 * fl->bb);
+        ef.sym_mode = 1;
+        ef.sym_part = fl->grp.rank();
+        ef.sym_parts = fl->grp.size();
     } else {
-        SKB_TRY(skb_ctx_set_sym_partition(fl->fib[1].get(), 0, 1));
-        SKB_TRY(skb_set_targets(fl->fib[1].get(), r_win.data(), fl->n_win));
+        if (use_cross) { // [own fiber rows | own body rows]
+            r_own.assign(fl->h_r_fib.begin() + 3 * fl->fa, fl->h_r_fib.begin() + 3 * fl->fb);
+            r_own.insert(r_own.end(), fl->h_r_body.begin() + 3 * fl->ba, fl->h_r_body.begin() + 3 * fl->bb);
+        }
+        ef.sym_part = 0;
+        ef.sym_parts = 1;
     }
-    SKB_TRY(skb_set_targets(fl->body[1].get(), r_win.data(), fl->n_win));
-    SKB_TRY(skb_set_targets(fl->shell[1].get(), r_fb.data(), (long long)r_fb.size() / 3));
+    const std::vector<double> &r_ef = sym_partial || use_cross ? r_own : r_win;
+    SKB_TRY(ef.set_targets(r_ef.data(), (long long)r_ef.size() / 3, false, fl->stream));
+    SKB_TRY(fl->body[1].set_targets(r_win.data(), fl->n_win, false, fl->stream));
+    SKB_TRY(fl->shell[1].set_targets(r_fb.data(), (long long)r_fb.size() / 3, false, fl->stream));
+    CUDA_TRY(cudaStreamSynchronize(fl->stream));
     const bool all_fibers_lead = (fl->fa == 0 && fl->fb == nf) || sym_partial;
     if (fl->self_excl && fl->n_fib > 0) {
         if (!all_fibers_lead)
@@ -547,9 +531,10 @@ int skb::prepare_matvec_targets(skb_flow *fl) {
         for (int f = 0; f < fl->n_fibers; ++f)
             for (long long i = fl->h_fiber_off[(size_t)f]; i < fl->h_fiber_off[(size_t)f + 1]; ++i)
                 ids[(size_t)i] = f;
-        SKB_TRY(skb_set_source_exclusion_ids(fl->fib[1].get(), ids.data(), nf));
+        SKB_TRY(ef.set_exclusion_ids(ids.data(), nf, fl->stream));
+        CUDA_TRY(cudaStreamSynchronize(fl->stream));
     } else {
-        SKB_TRY(skb_set_source_exclusion_ids(fl->fib[1].get(), nullptr, 0));
+        SKB_TRY(ef.set_exclusion_ids(nullptr, 0, fl->stream));
     }
     fl->mv_dirty = false;
     return SKB_OK;
@@ -602,18 +587,18 @@ static int overlap_launch(skb_flow *fl, const double *d_xs) {
 static int fiber_rows(skb_flow *fl, StrengthMode mode, const double *ff, double eta, double *d_v) {
     const skb_flow::MatvecPlan &P = fl->plan;
     if (P.fib_rows == skb_flow::MatvecPlan::kPlain)
-        return fibers_dev(fl, fl->fib[1].get(), mode, ff, eta, 0, d_v, 0, fl->fa, fl->fb);
+        return fibers_dev(fl, fl->fib[1], mode, ff, eta, 0, d_v, 0, fl->fa, fl->fb);
     const Group &G = fl->grp;
     const long long nf = fl->n_fib, n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa, n_bw = fl->bb - fl->ba;
-    DeviceState &df = fl->fib[1]->devs[0];
-    SKB_TRY(fl->scratch_u.ensure((size_t)df.n_trg * 24 + 8));
+    Evaluator &ef = fl->fib[1];
+    SKB_TRY(fl->scratch_u.ensure((size_t)ef.n_trg * 24 + 8));
     EvalOpts o;
     o.d_u_sym = P.grouped ? G.u_part() : d_v;
     o.d_u_rem = d_v + 3 * (n_fw + (P.cross ? n_sw : 0));
-    SKB_TRY(eval_on_device(fl->fib[1].get(), df, SKB_STOKESLET, mode, ff, 0.0, (double *)fl->scratch_u.ptr, 0, fl->cur,
-                           false, &fl->launches, nullptr, 1.0 / eta, o));
+    SKB_TRY(ef.eval(SKB_STOKESLET, mode, ff, 0.0, (double *)fl->scratch_u.ptr, 0, fl->cur, &fl->launches, nullptr,
+                    1.0 / eta, o));
     fl->pairs += nf * nf / (P.grouped ? G.size() : 1) + nf * ((P.cross ? 0 : n_sw) + n_bw);
-    if (fl->fib[1]->last_was_sym)
+    if (ef.last_was_sym)
         return SKB_OK;
     if (P.grouped)
         return set_error(SKB_ERR_STATE, "group member %d: the symmetric kernel declined (memory for the reverse "
@@ -635,10 +620,10 @@ static int fiber_rows(skb_flow *fl, StrengthMode mode, const double *ff, double 
 static int cross_rows(skb_flow *fl, const double *s6, double eta, double *d_v) {
     const bool grouped = fl->plan.grouped;
     const long long ns = fl->n_shell, n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa;
-    DeviceState &df = fl->fib[1]->devs[0];
-    const SourceSet &sf = df.src[SKB_STOKESLET], &ss = fl->shell[1]->devs[0].src[SKB_STRESSLET];
+    const Evaluator &ef = fl->fib[1];
+    const SourceSet &sf = ef.src[SKB_STOKESLET], &ss = fl->shell[1].src[SKB_STRESSLET];
     double *u_shell = grouped ? fl->grp.u_part_shell() : d_v + 3 * n_fw;
-    SKB_TRY(cross_eval(fl->cross, df.info, (const double *)sf.r.ptr, sf.f_cur, fl->fa, n_fw, (const double *)ss.r.ptr,
+    SKB_TRY(cross_eval(fl->cross, ef.info, (const double *)sf.r.ptr, sf.f_cur, fl->fa, n_fw, (const double *)ss.r.ptr,
                        s6, ns, ss.n_pad, -3.0 / (8.0 * M_PI * eta), 1.0 / (8.0 * M_PI * eta), d_v, grouped ? 0 : 1,
                        u_shell, 0, fl->cur, &fl->launches));
     fl->pairs += 2 * n_fw * ns;
@@ -662,7 +647,7 @@ static int periphery_rows(skb_flow *fl, StrengthMode mode, const double *sd, dou
     }
     SKB_TRY(fl->tmp.ensure((size_t)(n_fr + n_bw) * 24 + 8));
     double *d_tmp = (double *)fl->tmp.ptr;
-    SKB_TRY(periphery_dev(fl, fl->shell[1].get(), mode, sd, eta, d_tmp, 0));
+    SKB_TRY(periphery_dev(fl, fl->shell[1], mode, sd, eta, d_tmp, 0));
     const int bs = 256;
     if (n_fr > 0 && set_fib) {
         CUDA_TRY(cudaMemcpyAsync(d_v, d_tmp, (size_t)n_fr * 24, cudaMemcpyDeviceToDevice, fl->cur));
@@ -689,11 +674,11 @@ int skb::matvec_core(skb_flow *fl, const double *d_ff, const double *d_sd, const
     if (P.grouped) {
         if (!fl->grp_open)
             SKB_TRY(G.begin());
-        const DeviceState &df = fl->fib[1]->devs[0];
-        const SourceSet &sf = df.src[SKB_STOKESLET];
+        const Evaluator &ef = fl->fib[1];
+        const SourceSet &sf = ef.src[SKB_STOKESLET];
         SKB_TRY(G.push(d_ff, sf.has_weights ? (const double *)sf.weights.ptr : nullptr, fl->fa, n_fw, d_sd,
-                       fl->n_shell ? (const double *)fl->shell[1]->devs[0].src[SKB_STRESSLET].normals.ptr : nullptr,
-                       fl->sa, n_sw, 2.0 * eta, df.info.num_sms, fl->cur, &fl->launches));
+                       fl->n_shell ? (const double *)fl->shell[1].src[SKB_STRESSLET].normals.ptr : nullptr,
+                       fl->sa, n_sw, 2.0 * eta, ef.info.num_sms, fl->cur, &fl->launches));
         const bool ft = fl->ft_exchange && fl->n_bodies > 0; // d_f / d_t: this member's partial link forces
         if (ft)
             SKB_TRY(G.push_forces(d_f, d_t, fl->cur, &fl->launches));
@@ -715,13 +700,13 @@ int skb::matvec_core(skb_flow *fl, const double *d_ff, const double *d_sd, const
     // The self term subtracts from the fiber rows: without a group right after the fiber flow; a group member
     // subtracts it last, once the pull has completed its fiber rows (the plain-kernel member keeps that order too).
     if (!P.grouped)
-        SKB_TRY(fiber_self_term(fl, fl->fib[1].get(), eta, d_v, fl->fa, fl->fb));
+        SKB_TRY(fiber_self_term(fl, fl->fib[1], eta, d_v, fl->fa, fl->fb));
     if (P.cross) {
         if (!P.grouped) { // periphery strengths 2 eta n (x) rho -> sym6 (periphery.cpp:68-71), once for both uses
-            DeviceState &dsh = fl->shell[1]->devs[0];
-            SKB_TRY(pack_on_device(dsh, SKB_STRESSLET, kNormalDensity, d_sd, 2.0 * eta, fl->cur, &fl->launches));
+            Evaluator &es = fl->shell[1];
+            SKB_TRY(es.pack(SKB_STRESSLET, kNormalDensity, d_sd, 2.0 * eta, fl->cur, &fl->launches));
             smode = kPacked;
-            sd = dsh.src[SKB_STRESSLET].f_cur;
+            sd = es.src[SKB_STRESSLET].f_cur;
         }
         SKB_TRY(cross_rows(fl, sd, eta, d_v));
     }
@@ -730,7 +715,7 @@ int skb::matvec_core(skb_flow *fl, const double *d_ff, const double *d_sd, const
         SKB_TRY(G.barrier(1, true, false, fl->cur, &fl->launches)); // my partial sums are complete
     SKB_TRY(periphery_rows(fl, smode, sd, eta, d_v));
     // v_all += bc.flow(r_all, x_bodies, body_link_conditions, eta)     (system.cpp:316)
-    SKB_TRY(bodies_dev(fl, fl->body[1].get(), d_bd, d_f, d_t, eta, d_v, 1));
+    SKB_TRY(bodies_dev(fl, fl->body[1], d_bd, d_f, d_t, eta, d_v, 1));
     if (partial) {
         SKB_TRY(G.barrier(1, false, true, fl->cur, &fl->launches));
         SKB_TRY(G.pull(Group::kFiberRows, fl->fa, n_fw, d_v, fl->cur, &fl->launches));
@@ -738,7 +723,7 @@ int skb::matvec_core(skb_flow *fl, const double *d_ff, const double *d_sd, const
             SKB_TRY(G.pull(Group::kShellRows, fl->sa, n_sw, d_v + 3 * n_fw, fl->cur, &fl->launches));
     }
     if (P.grouped)
-        SKB_TRY(fiber_self_term(fl, fl->fib[1].get(), eta, d_v, fl->fa, fl->fb));
+        SKB_TRY(fiber_self_term(fl, fl->fib[1], eta, d_v, fl->fa, fl->fb));
     return SKB_OK;
 }
 

@@ -319,7 +319,7 @@ int skb_flow_set_gmres(skb_flow *fl, int num_blocks) {
     long long n = 0;
     std::array<long long, 6> key;
     SKB_TRY(flow_gmres_size(fl, who, &n, &key));
-    SKB_TRY(fl->kry.setup(n, num_blocks, fl->fib[1]->devs[0].info.num_sms, key));
+    SKB_TRY(fl->kry.setup(n, num_blocks, fl->fib[1].info.num_sms, key));
     // the buffers of skb_flow_step / skb_mflow_step / skb_flow_group_step_device beside the solve's
     SKB_TRY(fl->stepbuf.size(fl->n_fibers, fl->n_fib, fl->n_bodies));
     SKB_TRY(fl->shape.size(fl->n_fib));

@@ -434,7 +434,7 @@ int skb::group_step_run(skb_flow *fl, skb_dense *dn_spc, skb_dense *dn_minv, con
     std::vector<double> uw, c_new, q_new, sites_new;
     if (nb > 0) {
         SKB_TRY(G.begin());
-        SKB_TRY(G.store_rows(d_x + c.n - G.body_rows(), nullptr, 0, 0, fl->fib[1]->devs[0].info.num_sms, st,
+        SKB_TRY(G.store_rows(d_x + c.n - G.body_rows(), nullptr, 0, 0, fl->fib[1].info.num_sms, st,
                              launches));
         SKB_TRY(G.rows_barrier(true, true, st, launches));
         SKB_TRY(body_rows(fl, G.x_body(), uw, st));

@@ -1,6 +1,6 @@
 // skb_sym.cu -- host side of the symmetric Stokeslet kernel (sym_kernels.cuh) and the fiber <-> periphery cross kernel
 // (cross_kernels.cuh), the one unit that compiles them: launch attributes, the planner and ItemPlan they share, the
-// symmetric path of an evaluation (SymState), the cross pass of a flow (CrossState), and the C ABI calls about them.
+// symmetric path of an Evaluator (SymState), the cross pass of a flow (CrossState), and the C ABI calls about them.
 #include "sym_kernels.cuh"
 #include "cross_kernels.cuh"
 #include "skb_internal.hpp"
@@ -163,18 +163,18 @@ static int build_plan(ItemPlan &pl, const std::vector<ItemRow> &rows, int n_bloc
     return SKB_OK;
 }
 
-int ensure_self_state(DeviceState &d, SourceSet &s, cudaStream_t st) {
+int ensure_self_state(Evaluator &e, SourceSet &s, cudaStream_t st) {
     SymState &y = s.sym;
     if (y.self_state >= 0)
         return SKB_OK;
-    if (d.n_trg < s.n || s.n <= 0) {
+    if (e.n_trg < s.n || s.n <= 0) {
         y.self_state = 0;
         return SKB_OK;
     }
     SKB_TRY(y.flag.ensure(sizeof(int)));
     CUDA_TRY(cudaMemsetAsync(y.flag.ptr, 0, sizeof(int), st));
     const long long n3 = 3 * s.n;
-    self_check_kernel<<<(unsigned)((n3 + 255) / 256), 256, 0, st>>>((const double *)d.r_trg.ptr, (const double *)s.r.ptr,
+    self_check_kernel<<<(unsigned)((n3 + 255) / 256), 256, 0, st>>>((const double *)e.r_trg.ptr, (const double *)s.r.ptr,
                                                                     n3, (int *)y.flag.ptr);
     CUDA_TRY(cudaGetLastError());
     count_launch(1);
@@ -185,29 +185,29 @@ int ensure_self_state(DeviceState &d, SourceSet &s, cudaStream_t st) {
     return SKB_OK;
 }
 
-int sym_prepare(skb_ctx *ctx, DeviceState &d, cudaStream_t st, int *use) {
+int sym_prepare(Evaluator &e, cudaStream_t st, int *use) {
     *use = 0;
-    SourceSet &s = d.src[SKB_STOKESLET];
+    SourceSet &s = e.src[SKB_STOKESLET];
     SymState &y = s.sym;
     const long long block = sym_block_nodes();
-    if (s.n < 4096 && ctx->sym_mode != 1)
+    if (s.n < 4096 && e.sym_mode != 1)
         return SKB_OK; // too small to matter
-    if (s.n < 2 * block || d.n_trg < s.n)
+    if (s.n < 2 * block || e.n_trg < s.n)
         return SKB_OK;
     const long long nb = s.n_pad / block; // n_pad is a multiple of 1024
-    if ((long long)sym_owned_rows((int)nb, d.sym_part, d.sym_parts) * s.n_pad * 24 > sym_mem_budget())
+    if ((long long)sym_owned_rows((int)nb, e.sym_part, e.sym_parts) * s.n_pad * 24 > sym_mem_budget())
         return SKB_OK;
-    SKB_TRY(ensure_self_state(d, s, st));
+    SKB_TRY(ensure_self_state(e, s, st));
     if (y.self_state != 1)
         return SKB_OK;
-    const std::array<int, 3> key = {(int)nb, d.sym_part, d.sym_parts};
+    const std::array<int, 3> key = {(int)nb, e.sym_part, e.sym_parts};
     if (y.key != key) {
-        const std::vector<ItemRow> rows = sym_item_rows((int)nb, d.sym_part, d.sym_parts);
+        const std::vector<ItemRow> rows = sym_item_rows((int)nb, e.sym_part, e.sym_parts);
         const size_t p_bytes = rows.size() * (size_t)s.n_pad * 24;
         if (y.plan.P.ensure(p_bytes) != SKB_OK) { // not enough free memory for the reverse partials: the plain kernel
                                                   // serves this geometry
             (void)cudaGetLastError();
-            if (ctx->sym_layout) // every device holds ALL leading targets there and the caller reduce-scatters the
+            if (e.layout == Evaluator::kShared) // every device holds ALL leading targets there and the caller reduce-scatters the
                                  // partial sums: a silent switch to the plain kernel would count them P times
                 return set_error(SKB_ERR_ALLOC, "symmetric multi-device layout: no memory for the reverse partials "
                                                 "(%zu bytes); free memory or skb_ctx_set_symmetric(ctx, 0)",
@@ -226,7 +226,7 @@ int sym_prepare(skb_ctx *ctx, DeviceState &d, cudaStream_t st, int *use) {
         }
         SKB_TRY(y.row_ids.ensure(owned.size() * sizeof(int) + 16));
         CUDA_TRY(cudaMemcpyAsync(y.row_ids.ptr, owned.data(), owned.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-        SKB_TRY(build_plan(y.plan, rows, (int)nb, block, (long long)d.info.num_sms * kSymMinB, st)); // waits for owned
+        SKB_TRY(build_plan(y.plan, rows, (int)nb, block, (long long)e.info.num_sms * kSymMinB, st)); // waits for owned
         y.n_owned = (int)owned.size();
         y.pairs = pairs;
         y.key = key;
@@ -235,15 +235,15 @@ int sym_prepare(skb_ctx *ctx, DeviceState &d, cudaStream_t st, int *use) {
     return SKB_OK;
 }
 
-int sym_eval(DeviceState &d, double *d_u_out, int accumulate, cudaStream_t st, double scale_mul, int *launches) {
-    SourceSet &s = d.src[SKB_STOKESLET];
+int sym_eval(Evaluator &ev, double *d_u_out, int accumulate, cudaStream_t st, double scale_mul, int *launches) {
+    SourceSet &s = ev.src[SKB_STOKESLET];
     const SymState &y = s.sym;
     const SymArgs a{(const double *)s.r.ptr, s.f_cur, s.excl ? (const int *)s.excl_ids.ptr : nullptr,
                     (const SymItem *)y.plan.items.ptr, (double *)y.plan.P.ptr, (double *)y.plan.F.ptr, s.n_pad,
                     y.plan.n_blocks};
     cudaError_t e = cudaSuccess;
     if (y.plan.n_items > 0) {
-        CUDA_TRY(cudaEventRecord(d.ev_s0, st));
+        CUDA_TRY(cudaEventRecord(ev.ev_s0, st));
         constexpr int smem = SymSmem<kSymT>::total_bytes;
         if (s.excl)
             pair_sym_kernel<kSymT, kSymMinB, true><<<y.plan.n_items, kSymThreads, smem, st>>>(a);
@@ -251,8 +251,8 @@ int sym_eval(DeviceState &d, double *d_u_out, int accumulate, cudaStream_t st, d
             pair_sym_kernel<kSymT, kSymMinB, false><<<y.plan.n_items, kSymThreads, smem, st>>>(a);
         e = cudaGetLastError();
         if (e == cudaSuccess)
-            CUDA_TRY(cudaEventRecord(d.ev_s1, st));
-        d.sym_timed = true;
+            CUDA_TRY(cudaEventRecord(ev.ev_s1, st));
+        ev.sym_timed = true;
         if (e != cudaSuccess)
             return set_error(SKB_ERR_CUDA, "pair_sym_kernel launch failed: %s", cudaGetErrorString(e));
         count_launch(1);
@@ -272,6 +272,24 @@ int sym_eval(DeviceState &d, double *d_u_out, int accumulate, cudaStream_t st, d
 }
 
 LaunchPlan sym_launch_plan(const SourceSet &s) { return LaunchPlan{kSymT, 1, 0, (unsigned)s.sym.plan.n_items}; }
+
+int Evaluator::last_sym_kernel(double *ms, int64_t *pairs) const {
+    if (!ms || !pairs)
+        return set_error(SKB_ERR_INVALID, "skb_ctx_last_sym_kernel: NULL");
+    *ms = 0;
+    *pairs = 0;
+    if (!sym_timed)
+        return SKB_OK;
+    float t = 0;
+    cudaSetDevice(info.dev);
+    if (cudaEventElapsedTime(&t, ev_s0, ev_s1) == cudaSuccess) {
+        *ms = t;
+        *pairs = src[SKB_STOKESLET].sym.pairs;
+    } else {
+        (void)cudaGetLastError(); // not finished yet
+    }
+    return SKB_OK;
+}
 
 int cross_eval(CrossState &cs, const DeviceInfo &di, const double *d_r_fib, const double *d_h, long long node0,
                long long n_rows, const double *d_r_sh, const double *d_s6, long long n_sh, long long n_sh_pad,
@@ -338,24 +356,5 @@ int skb_sym_plan_query(int n_blocks, int part, int n_parts, int num_sms, int max
 }
 
 int skb_sym_groups_per_block(void) { return kSymGroupsPerBlock; }
-
-int skb_ctx_last_sym_kernel(const skb_ctx *ctx, double *ms, int64_t *pairs) {
-    if (!ctx || !ms || !pairs)
-        return set_error(SKB_ERR_INVALID, "skb_ctx_last_sym_kernel: NULL");
-    *ms = 0;
-    *pairs = 0;
-    const DeviceState &d = ctx->devs[0];
-    if (!d.sym_timed)
-        return SKB_OK;
-    float t = 0;
-    cudaSetDevice(d.info.dev);
-    if (cudaEventElapsedTime(&t, d.ev_s0, d.ev_s1) == cudaSuccess) {
-        *ms = t;
-        *pairs = d.src[SKB_STOKESLET].sym.pairs;
-    } else {
-        (void)cudaGetLastError(); // not finished yet
-    }
-    return SKB_OK;
-}
 
 } // extern "C"

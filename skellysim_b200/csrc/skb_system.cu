@@ -593,7 +593,7 @@ static int system_rhs_core(skb_flow *fl, OwnFibers own, const skb_fiber_params *
         // (:442).  F_T are complete on every member and go straight to the body flow (no ft_exchange): each counts once
         SKB_TRY(matvec_core(fl, d_fext ? d_fext : zero, zero, zero, d_f ? d_f : zero, d_t ? d_t : zero, eta, d_v));
         // v_all += psc.flow + bs.flow (:445-446).  The body evaluator's matvec targets are the rows of d_v, in its order
-        SKB_TRY(add_sources(fl, (const double *)fl->body[1]->devs[0].r_trg.ptr, fl->n_win, eta, d_v, fl->cur));
+        SKB_TRY(add_sources(fl, (const double *)fl->body[1].r_trg.ptr, fl->n_win, eta, d_v, fl->cur));
         // fc.update_rhs(dt, v_fibers, motor + f_ext) + fc.apply_bcs(dt, v_fibers, f_ext) (:451-453)
         if (launch)
             SKB_TRY((*launch)());
@@ -900,7 +900,7 @@ int skb_flow_group_apply_system_matvec_device(skb_flow *fl, skb_dense *dn, const
         const bool bodies = fl->n_bodies > 0;
         SKB_TRY(G.begin());
         if (bodies) { // the complete x_bodies in every window first: the links read the bodies' U, w before barrier A
-            SKB_TRY(G.store_rows(x_body, nullptr, 0, 0, fl->fib[1]->devs[0].info.num_sms, fl->cur, &fl->launches));
+            SKB_TRY(G.store_rows(x_body, nullptr, 0, 0, fl->fib[1].info.num_sms, fl->cur, &fl->launches));
             SKB_TRY(G.rows_barrier(true, true, fl->cur, &fl->launches));
         }
         fl->grp_open = true; // matvec_core's push, barriers and pull run in this epoch
@@ -931,7 +931,7 @@ int skb_flow_group_apply_system_preconditioner_device(skb_flow *fl, skb_dense *d
         double *full = (double *)fl->sys_rb.ptr;
         // the complete x_shell and x_bodies in every window; the fibers' A_^-1 runs while the peers' rows arrive
         SKB_TRY(G.begin());
-        SKB_TRY(G.store_rows(x_body, n_sw > 0 ? x_shell : nullptr, fl->sa, n_sw, fl->fib[1]->devs[0].info.num_sms,
+        SKB_TRY(G.store_rows(x_body, n_sw > 0 ? x_shell : nullptr, fl->sa, n_sw, fl->fib[1].info.num_sms,
                              fl->cur, &fl->launches));
         SKB_TRY(G.rows_barrier(true, false, fl->cur, &fl->launches));
         SKB_TRY(fl->ops.precondition(x_fib, y_fib, fl->cur, &fl->launches));
