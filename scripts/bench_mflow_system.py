@@ -1,12 +1,13 @@
 """Cost of the whole-vector operator over several devices (skb_mflow_apply_system_matvec, include/skelly_b200_flow.h)
-against the partial operator skb_mflow_apply_matvec on the same shape.
+against the partial operator skb_mflow_apply_matvec and the flow matvec skb_mflow_matvec on the same shape.
 
 C3 (3000 fibers x 32 nodes, 6000 periphery nodes) with 1 body x 400 nodes and 200 fibers bound to it, the shape of
-scripts/bench_system_matvec.py.  Per device list the two calls alternate, one of each per round: the system call forms
+scripts/bench_system_matvec.py.  Per device list the three calls alternate, one of each per round: the system call forms
 the links, the bodies' link forces (exchanged through the group window) and the body rows on the devices; the partial
 call is given the link conditions and the bodies' forces and torques of the same x, computed beforehand on the host by
-tests/system_reference.py (BodyContainer::calculate_link_conditions restated in numpy).  As a check that the two calls
-do the same work, the largest relative difference of their fiber and periphery rows is reported (rounding only).
+tests/system_reference.py (BodyContainer::calculate_link_conditions restated in numpy); the flow matvec takes the
+strengths of the same x.  As a check that the system call and the partial call do the same work, the largest
+relative difference of their fiber and periphery rows is reported (rounding only).
 Reported per call: device_ms (skb_mflow_last_stats: CUDA events around each member's work, the slowest member, copies
 excluded) and wall_ms (the host call, copies included), as medians with [min, max]; and the launches per call.  The
 card's name and power limit are printed by the same run.  Needs a GPU; there is no CPU path.
@@ -88,6 +89,9 @@ def run(devs, s, reps, warmup, rng):
         def existing():
             out["existing"] = mf.apply_matvec(x_f, x_s, dens, ft, 1.0, link)
 
+        def flow():
+            out["matvec"] = mf.matvec(x_f[:3 * nf].reshape(nf, 3), x_s, dens, ft, 1.0)
+
         def timed(fn):
             t0 = time.perf_counter()
             fn()
@@ -98,10 +102,12 @@ def run(devs, s, reps, warmup, rng):
         for _ in range(warmup):
             system()
             existing()
-        t = {"system": [], "existing": []}
+            flow()
+        t = {"system": [], "existing": [], "matvec": []}
         for _ in range(reps):  # alternating, one call of each per round
             t["system"].append(timed(system))
             t["existing"].append(timed(existing))
+            t["matvec"].append(timed(flow))
     r_f, r_s, _ = out["existing"]  # the last call of each
     got = out["system"]
     rel = lambda a, b: float(np.abs(a - b).max() / np.abs(b).max())

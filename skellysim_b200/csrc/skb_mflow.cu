@@ -87,6 +87,24 @@ class Workers {
     std::condition_variable cv_, done_;
     bool stop_ = false;
 };
+
+// A member's copies of one host-array call: each Run moves len doubles between the caller's array at `whole` and the
+// device array at `at`
+struct Run {
+    long long whole, at, len;
+};
+struct Transfer {
+    double *host;          // the caller's array (only read by an upload); NULL: nothing to copy
+    double *dev;           // a device array the callee owns, or the staging slot mflow_stage gives it
+    std::vector<Run> runs;
+};
+struct Transfers {
+    std::vector<Transfer> up, down; // before the call, after it
+};
+Transfer up(const double *h, std::vector<Run> runs, double *dev = nullptr) {
+    return Transfer{const_cast<double *>(h), dev, std::move(runs)};
+}
+Transfer down(double *h, std::vector<Run> runs, double *dev = nullptr) { return Transfer{h, dev, std::move(runs)}; }
 } // namespace
 
 struct skb_mflow {
@@ -109,8 +127,9 @@ struct skb_mflow {
     bool ops_ready = false;
     std::vector<int> body_n; // node counts of skb_mflow_set_body_operators (the body part of the solution vector)
     long long body_sol = 0;  // ... its size, sum(3 n + 6)
-    struct IO { // per-member device buffers of the host-pointer calls
-        DevBuf x, xs, bd, f, t, link, res, outs, vb, ff, v; // (x / res: also the local vector of the system calls)
+    struct IO {               // per member: the transfers of the host-array call in flight
+        Transfers xfer;
+        std::vector<DevBuf> stage; // the staging slots of xfer.up, then of xfer.down
         Event e0, e1;
     };
     std::vector<IO> io;
@@ -181,6 +200,15 @@ skb_mflow::~skb_mflow() {
         cudaSetDevice(devs[io.size() - 1]);
         io.pop_back();
     }
+}
+
+// set(member, a...) on every member in turn, on the calling thread, up to the first that fails
+template <class Set, class... A> static int each_member(skb_mflow *mf, const char *who, Set set, A... a) {
+    if (!mf)
+        return set_error(SKB_ERR_INVALID, "%s: NULL", who);
+    for (int g = 0; g < mf->n; ++g)
+        SKB_TRY(set(mf->m[g].get(), a...));
+    return SKB_OK;
 }
 
 extern "C" {
@@ -269,29 +297,19 @@ int skb_mflow_set_bodies(skb_mflow *mf, const double *node_pos, const double *no
 }
 
 int skb_mflow_set_cross(skb_mflow *mf, int mode) {
-    if (!mf)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_set_cross: NULL");
-    for (int g = 0; g < mf->n; ++g)
-        SKB_TRY(skb_flow_set_cross(mf->m[g].get(), mode));
+    SKB_TRY(each_member(mf, "skb_mflow_set_cross", skb_flow_set_cross, mode));
     mf->part_dirty = true; // the members' target lists change: re-run the warm-up
     return SKB_OK;
 }
 
 int skb_mflow_set_overlap(skb_mflow *mf, int on) {
-    if (!mf)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_set_overlap: NULL");
-    for (int g = 0; g < mf->n; ++g)
-        SKB_TRY(skb_flow_set_overlap(mf->m[g].get(), on));
-    return SKB_OK;
+    return each_member(mf, "skb_mflow_set_overlap", skb_flow_set_overlap, on);
 }
 
 int skb_mflow_set_periphery_shape(skb_mflow *mf, const skb_periphery_shape *shape, const int32_t *fiber_minus_clamped,
                                   const double *body_radius) {
-    if (!mf)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_set_periphery_shape: NULL");
-    for (int g = 0; g < mf->n; ++g)
-        SKB_TRY(skb_flow_set_periphery_shape(mf->m[g].get(), shape, fiber_minus_clamped, body_radius));
-    return SKB_OK;
+    return each_member(mf, "skb_mflow_set_periphery_shape", skb_flow_set_periphery_shape, shape, fiber_minus_clamped,
+                       body_radius);
 }
 
 // skb_flow_periphery_interaction of every member into the complete arrays: each member's own fibers, member 0's
@@ -310,11 +328,7 @@ int skb_mflow_periphery_interaction(skb_mflow *mf, double *f_periphery, int32_t 
 }
 
 int skb_mflow_set_self_exclusion(skb_mflow *mf, int fused) {
-    if (!mf)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_set_self_exclusion: NULL");
-    for (int g = 0; g < mf->n; ++g)
-        SKB_TRY(skb_flow_set_self_exclusion(mf->m[g].get(), fused));
-    return SKB_OK;
+    return each_member(mf, "skb_mflow_set_self_exclusion", skb_flow_set_self_exclusion, fused);
 }
 
 int skb_mflow_partition(skb_mflow *mf, int member, int *fiber_begin, int *fiber_end, int64_t *shell_begin,
@@ -349,10 +363,7 @@ int skb_partition_query(const int *n_nodes, int n_fibers, int64_t n_shell, int64
 }
 
 int skb_mflow_set_fiber_class(skb_mflow *mf, int n_nodes, const double *D_1_0, const double *P_downsample_bc) {
-    if (!mf)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_set_fiber_class: NULL");
-    for (int g = 0; g < mf->n; ++g)
-        SKB_TRY(skb_flow_set_fiber_class(mf->m[g].get(), n_nodes, D_1_0, P_downsample_bc));
+    SKB_TRY(each_member(mf, "skb_mflow_set_fiber_class", skb_flow_set_fiber_class, n_nodes, D_1_0, P_downsample_bc));
     mf->ops_ready = false;
     return SKB_OK;
 }
@@ -394,11 +405,8 @@ int skb_mflow_set_fiber_preconditioner(skb_mflow *mf, const double *A_inv) {
 
 int skb_mflow_set_fiber_class_derivatives(skb_mflow *mf, int n_nodes, const double *D_2_0, const double *D_3_0,
                                           const double *D_4_0) {
-    if (!mf)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_set_fiber_class_derivatives: NULL");
-    for (int g = 0; g < mf->n; ++g)
-        SKB_TRY(skb_flow_set_fiber_class_derivatives(mf->m[g].get(), n_nodes, D_2_0, D_3_0, D_4_0));
-    return SKB_OK;
+    return each_member(mf, "skb_mflow_set_fiber_class_derivatives", skb_flow_set_fiber_class_derivatives, n_nodes,
+                       D_2_0, D_3_0, D_4_0);
 }
 
 int skb_mflow_build_fiber_operators(skb_mflow *mf, const skb_fiber_params *params, double dt, double eta) {
@@ -485,6 +493,8 @@ static int mflow_collect_stats(skb_mflow *mf) {
     return SKB_OK;
 }
 
+} // extern "C"
+
 // rows of member g: fiber nodes [a, a + n_fw), n_fibers whole fibers, n_sw periphery rows, n_bw body rows
 struct MemberRows {
     long long a, n_fw, n_sw, n_bw;
@@ -496,38 +506,58 @@ static MemberRows member_rows(const skb_mflow *mf, int g) {
     return MemberRows{a, b - a, mf->s1[g] - mf->s0[g], mf->b1[g] - mf->b0[g], mf->f1[g] - mf->f0[g]};
 }
 
-// buf (n_dbl doubles, at least 8 bytes) <- h on st; h == NULL leaves it unset
-static int put(DevBuf &buf, const double *h, size_t n_dbl, cudaStream_t st) {
-    SKB_TRY(buf.ensure(n_dbl * 8 + 8));
-    if (n_dbl && h)
-        CUDA_TRY(cudaMemcpyAsync(buf.ptr, h, n_dbl * 8, cudaMemcpyHostToDevice, st));
-    return SKB_OK;
-}
-
-// Size every member's transfer buffers on the CALLING thread, before any member starts launching: cudaMalloc /
-// cudaFree may synchronise the whole device and must not run while a peer on the same device sits in a flag wait.
-static int mflow_size_io(skb_mflow *mf, size_t n_ft) {
+// On the calling thread, before any worker starts: member g's transfers of the call, describe(g), and the staging slots
+// they need, sized there -- cudaMalloc / cudaFree may synchronise the whole device and must not run while a peer on the
+// same device sits in a flag wait.  A slot holds at least 8 bytes, so a member call gets a device pointer for an empty
+// array too.  The background streamer's buffers take their size here as well.
+template <class Describe> static int mflow_stage(skb_mflow *mf, Describe describe) {
     for (int g = 0; g < mf->n; ++g) {
         CUDA_TRY(cudaSetDevice(mf->devs[g]));
         skb_mflow::IO &io = mf->io[g];
-        const MemberRows r = member_rows(mf, g);
-        const size_t n_fw = (size_t)r.n_fw, n_sw = (size_t)r.n_sw, n_bw = (size_t)r.n_bw, n_fibers = (size_t)r.n_fibers;
-        SKB_TRY(io.x.ensure(n_fw * 32 + 8));
-        SKB_TRY(io.ff.ensure(n_fw * 24 + 8));
-        SKB_TRY(io.xs.ensure(n_sw * 24 + 8));
-        SKB_TRY(io.bd.ensure((size_t)mf->n_body * 24 + 8));
-        SKB_TRY(io.f.ensure(n_ft * 8 + 8));
-        SKB_TRY(io.t.ensure(n_ft * 8 + 8));
-        SKB_TRY(io.link.ensure(n_fibers * 56 + 8));
-        SKB_TRY(io.res.ensure(n_fw * 32 + 8));
-        SKB_TRY(io.outs.ensure(n_sw * 24 + 8));
-        SKB_TRY(io.vb.ensure(n_bw * 24 + 8));
-        SKB_TRY(io.v.ensure((n_fw + n_sw + n_bw) * 24 + 8));
+        io.xfer = describe(g);
+        io.stage.resize(std::max(io.stage.size(), io.xfer.up.size() + io.xfer.down.size()));
+        size_t k = 0;
+        for (std::vector<Transfer> *list : {&io.xfer.up, &io.xfer.down})
+            for (Transfer &t : *list) {
+                DevBuf &slot = io.stage[k++];
+                if (t.dev)
+                    continue;
+                long long n = 0;
+                for (const Run &r : t.runs)
+                    n = std::max(n, r.at + r.len);
+                SKB_TRY(slot.ensure((size_t)n * 8 + 8));
+                t.dev = (double *)slot.ptr;
+            }
+        const long long n_sw = mf->s1[g] - mf->s0[g];
         if (mf->has_dense && n_sw > 0 && mf->m[g]->bg.enabled) // the background streamer's, if it is on
-            SKB_TRY(overlap_buffers(mf->m[g].get(), 3 * (long long)n_sw));
+            SKB_TRY(overlap_buffers(mf->m[g].get(), 3 * n_sw));
     }
     return SKB_OK;
 }
+
+// On member g's worker: the uploads mflow_stage described, call(stream, transfers) between the member's timing events,
+// then the downloads and, if the call has any, the wait for them.  Allocates nothing.
+template <class Call> static int member_call(skb_mflow *mf, int g, Call call) {
+    const skb_mflow::IO &io = mf->io[(size_t)g];
+    CUDA_TRY(cudaSetDevice(mf->devs[(size_t)g]));
+    const cudaStream_t st = mf->m[(size_t)g]->stream;
+    for (const Transfer &t : io.xfer.up)
+        for (const Run &r : t.runs)
+            if (t.host && r.len)
+                CUDA_TRY(cudaMemcpyAsync(t.dev + r.at, t.host + r.whole, (size_t)r.len * 8, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaEventRecord(io.e0, st));
+    SKB_TRY(call(st, io.xfer));
+    CUDA_TRY(cudaEventRecord(io.e1, st));
+    for (const Transfer &t : io.xfer.down)
+        for (const Run &r : t.runs)
+            if (t.host && r.len)
+                CUDA_TRY(cudaMemcpyAsync(t.host + r.whole, t.dev + r.at, (size_t)r.len * 8, cudaMemcpyDeviceToHost, st));
+    if (!io.xfer.down.empty())
+        CUDA_TRY(cudaStreamSynchronize(st));
+    return SKB_OK;
+}
+
+extern "C" {
 
 // v_all over [fibers | periphery | bodies] like skb_flow_matvec; complete host arrays in and out
 int skb_mflow_matvec(skb_mflow *mf, const double *fib_forces, const double *shell_density, const double *body_densities,
@@ -542,36 +572,20 @@ int skb_mflow_matvec(skb_mflow *mf, const double *fib_forces, const double *shel
     std::vector<double> f, t;
     if (mf->n_bodies > 0)
         split_forces_torques(body_forces_torques, mf->n_bodies, f, t);
-    SKB_TRY(mflow_size_io(mf, f.size()));
-    SKB_TRY(mf->workers->run([&](int g) -> int {
-        skb_flow *fl = mf->m[g].get();
-        skb_mflow::IO &io = mf->io[g];
-        CUDA_TRY(cudaSetDevice(mf->devs[g]));
+    const long long n_ft = (long long)f.size();
+    SKB_TRY(mflow_stage(mf, [&](int g) -> Transfers {
         const MemberRows r = member_rows(mf, g);
-        const long long a = r.a, n_fw = r.n_fw, n_sw = r.n_sw, n_bw = r.n_bw;
-        cudaStream_t st = fl->stream;
-        SKB_TRY(put(io.ff, fib_forces ? fib_forces + 3 * a : nullptr, (size_t)n_fw * 3, st));
-        SKB_TRY(put(io.xs, shell_density ? shell_density + 3 * mf->s0[g] : nullptr, (size_t)n_sw * 3, st));
-        SKB_TRY(put(io.bd, body_densities, (size_t)nb * 3, st));
-        SKB_TRY(put(io.f, f.data(), f.size(), st));
-        SKB_TRY(put(io.t, t.data(), t.size(), st));
-        SKB_TRY(io.v.ensure((size_t)(n_fw + n_sw + n_bw) * 24 + 8));
-        CUDA_TRY(cudaEventRecord(io.e0, st));
-        SKB_TRY(skb_flow_matvec_device(fl, (const double *)io.ff.ptr, (const double *)io.xs.ptr,
-                                       (const double *)io.bd.ptr, (const double *)io.f.ptr, (const double *)io.t.ptr, eta,
-                                       (double *)io.v.ptr, st));
-        CUDA_TRY(cudaEventRecord(io.e1, st));
-        double *d_v = (double *)io.v.ptr;
-        if (n_fw)
-            CUDA_TRY(cudaMemcpyAsync(v_all + 3 * a, d_v, (size_t)n_fw * 24, cudaMemcpyDeviceToHost, st));
-        if (n_sw)
-            CUDA_TRY(cudaMemcpyAsync(v_all + 3 * (nf + mf->s0[g]), d_v + 3 * n_fw, (size_t)n_sw * 24,
-                                     cudaMemcpyDeviceToHost, st));
-        if (n_bw)
-            CUDA_TRY(cudaMemcpyAsync(v_all + 3 * (nf + ns + mf->b0[g]), d_v + 3 * (n_fw + n_sw), (size_t)n_bw * 24,
-                                     cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-        return SKB_OK;
+        return {{up(fib_forces, {{3 * r.a, 0, 3 * r.n_fw}}), up(shell_density, {{3 * mf->s0[g], 0, 3 * r.n_sw}}),
+                 up(body_densities, {{0, 0, 3 * nb}}), up(f.data(), {{0, 0, n_ft}}), up(t.data(), {{0, 0, n_ft}})},
+                {down(v_all, {{3 * r.a, 0, 3 * r.n_fw},
+                              {3 * (nf + mf->s0[g]), 3 * r.n_fw, 3 * r.n_sw},
+                              {3 * (nf + ns + mf->b0[g]), 3 * (r.n_fw + r.n_sw), 3 * r.n_bw}})}};
+    }));
+    SKB_TRY(mf->workers->run([&](int g) -> int {
+        return member_call(mf, g, [&](cudaStream_t st, const Transfers &io) {
+            return skb_flow_matvec_device(mf->m[g].get(), io.up[0].dev, io.up[1].dev, io.up[2].dev, io.up[3].dev,
+                                          io.up[4].dev, eta, io.down[0].dev, st);
+        });
     }));
     return mflow_collect_stats(mf);
 }
@@ -593,41 +607,24 @@ int skb_mflow_apply_matvec(skb_mflow *mf, const double *x_fibers, const double *
     std::vector<double> f, t;
     if (mf->n_bodies > 0)
         split_forces_torques(body_forces_torques, mf->n_bodies, f, t);
-    SKB_TRY(mflow_size_io(mf, f.size()));
-    SKB_TRY(mf->workers->run([&](int g) -> int {
-        skb_flow *fl = mf->m[g].get();
-        skb_mflow::IO &io = mf->io[g];
-        CUDA_TRY(cudaSetDevice(mf->devs[g]));
-        const int f0 = mf->f0[g], f1 = mf->f1[g];
+    const long long n_ft = (long long)f.size();
+    SKB_TRY(mflow_stage(mf, [&](int g) -> Transfers {
         const MemberRows r = member_rows(mf, g);
-        const long long a = r.a, n_fw = r.n_fw, n_sw = r.n_sw, n_bw = r.n_bw;
-        cudaStream_t st = fl->stream;
-        SKB_TRY(put(io.x, x_fibers ? x_fibers + 4 * a : nullptr, (size_t)n_fw * 4, st));
-        SKB_TRY(put(io.xs, x_shell ? x_shell + 3 * mf->s0[g] : nullptr, (size_t)n_sw * 3, st));
-        SKB_TRY(put(io.bd, body_densities, (size_t)nb * 3, st));
-        SKB_TRY(put(io.f, f.data(), f.size(), st));
-        SKB_TRY(put(io.t, t.data(), t.size(), st));
-        SKB_TRY(put(io.link, fiber_link_conditions ? fiber_link_conditions + 7 * (long long)f0 : nullptr,
-                    (size_t)(f1 - f0) * 7, st));
-        SKB_TRY(io.res.ensure((size_t)n_fw * 32 + 8));
-        SKB_TRY(io.outs.ensure((size_t)n_sw * 24 + 8));
-        SKB_TRY(io.vb.ensure((size_t)n_bw * 24 + 8));
-        CUDA_TRY(cudaEventRecord(io.e0, st));
-        SKB_TRY(skb_flow_apply_matvec_device(
-            fl, mf->has_dense ? mf->dn[g].get() : nullptr, (const double *)io.x.ptr, (const double *)io.xs.ptr,
-            (const double *)io.bd.ptr, (const double *)io.f.ptr, (const double *)io.t.ptr,
-            (fiber_link_conditions && f1 > f0) ? (const double *)io.link.ptr : nullptr, eta, (double *)io.res.ptr,
-            (double *)io.outs.ptr, (double *)io.vb.ptr, st));
-        CUDA_TRY(cudaEventRecord(io.e1, st));
-        if (n_fw)
-            CUDA_TRY(cudaMemcpyAsync(res_fibers + 4 * a, io.res.ptr, (size_t)n_fw * 32, cudaMemcpyDeviceToHost, st));
-        if (n_sw)
-            CUDA_TRY(cudaMemcpyAsync(out_shell + 3 * mf->s0[g], io.outs.ptr, (size_t)n_sw * 24, cudaMemcpyDeviceToHost,
-                                     st));
-        if (n_bw)
-            CUDA_TRY(cudaMemcpyAsync(v_bodies + 3 * mf->b0[g], io.vb.ptr, (size_t)n_bw * 24, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-        return SKB_OK;
+        const long long s0 = mf->s0[g], b0 = mf->b0[g];
+        return {{up(x_fibers, {{4 * r.a, 0, 4 * r.n_fw}}), up(x_shell, {{3 * s0, 0, 3 * r.n_sw}}),
+                 up(body_densities, {{0, 0, 3 * nb}}), up(f.data(), {{0, 0, n_ft}}), up(t.data(), {{0, 0, n_ft}}),
+                 up(fiber_link_conditions, {{7LL * mf->f0[g], 0, 7LL * r.n_fibers}})},
+                {down(res_fibers, {{4 * r.a, 0, 4 * r.n_fw}}), down(out_shell, {{3 * s0, 0, 3 * r.n_sw}}),
+                 down(v_bodies, {{3 * b0, 0, 3 * r.n_bw}})}};
+    }));
+    SKB_TRY(mf->workers->run([&](int g) -> int {
+        const bool links = fiber_link_conditions && mf->f1[g] > mf->f0[g];
+        return member_call(mf, g, [&](cudaStream_t st, const Transfers &io) {
+            return skb_flow_apply_matvec_device(mf->m[g].get(), mf->has_dense ? mf->dn[g].get() : nullptr,
+                                                io.up[0].dev, io.up[1].dev, io.up[2].dev, io.up[3].dev, io.up[4].dev,
+                                                links ? io.up[5].dev : nullptr, eta, io.down[0].dev, io.down[1].dev,
+                                                io.down[2].dev, st);
+        });
     }));
     return mflow_collect_stats(mf);
 }
@@ -649,59 +646,26 @@ template <class T> static T *own_slice(const skb_mflow *mf, int g, T *all, int k
     return all && mf->f1[(size_t)g] > mf->f0[(size_t)g] ? all + (size_t)k * mf->f0[(size_t)g] : nullptr;
 }
 
-// member g's rows of a whole vector in its local order [fiber rows | shell rows | body pieces]: copy(whole offset,
-// local offset, length) per non-empty run, up to the first that fails
-template <class Copy> static int member_local(const skb_mflow *mf, int g, Copy copy) {
+// member g's rows of a whole vector in its local order [fiber rows | shell rows | body pieces], one run per non-empty
+// piece
+static std::vector<Run> member_local(const skb_mflow *mf, int g) {
     const MemberRows r = member_rows(mf, g);
     const long long body = 4 * mf->n_fib + 3 * mf->n_shell, at = 4 * r.n_fw + 3 * r.n_sw;
     std::vector<RowPiece> pieces;
     if (mf->n_bodies > 0)
         body_row_pieces(mf->body_n.data(), (int)mf->body_n.size(), mf->b0[(size_t)g], mf->b1[(size_t)g], pieces);
+    std::vector<Run> runs;
     if (r.n_fw)
-        SKB_TRY(copy(4 * r.a, 0, 4 * r.n_fw));
+        runs.push_back({4 * r.a, 0, 4 * r.n_fw});
     if (r.n_sw)
-        SKB_TRY(copy(4 * mf->n_fib + 3 * mf->s0[(size_t)g], 4 * r.n_fw, 3 * r.n_sw));
+        runs.push_back({4 * mf->n_fib + 3 * mf->s0[(size_t)g], 4 * r.n_fw, 3 * r.n_sw});
     for (const RowPiece &p : pieces)
-        SKB_TRY(copy(body + p.body, at + p.local, p.len));
-    return SKB_OK;
-}
-
-static long long member_local_size(const skb_mflow *mf, int g) {
-    long long n = 0;
-    member_local(mf, g, [&](long long, long long, long long len) {
-        n += len;
-        return SKB_OK;
-    });
-    return n;
-}
-
-// On member g's worker: its rows of the whole host vector `in` (NULL: the call has no input vector) into its local
-// vector d_in, call(stream) between the member's timing events, the local rows of d_out into the whole host vector `out`
-template <class Call>
-static int member_through(skb_mflow *mf, int g, const double *in, double *d_in, const double *d_out, double *out,
-                          Call call) {
-    skb_mflow::IO &io = mf->io[(size_t)g];
-    CUDA_TRY(cudaSetDevice(mf->devs[(size_t)g]));
-    const cudaStream_t st = mf->m[(size_t)g]->stream;
-    if (in)
-        SKB_TRY(member_local(mf, g, [&](long long whole, long long at, long long len) -> int {
-            CUDA_TRY(cudaMemcpyAsync(d_in + at, in + whole, (size_t)len * 8, cudaMemcpyHostToDevice, st));
-            return SKB_OK;
-        }));
-    CUDA_TRY(cudaEventRecord(io.e0, st));
-    SKB_TRY(call(st));
-    CUDA_TRY(cudaEventRecord(io.e1, st));
-    SKB_TRY(member_local(mf, g, [&](long long whole, long long at, long long len) -> int {
-        CUDA_TRY(cudaMemcpyAsync(out + whole, d_out + at, (size_t)len * 8, cudaMemcpyDeviceToHost, st));
-        return SKB_OK;
-    }));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    return SKB_OK;
+        runs.push_back({body + p.body, at + p.local, p.len});
+    return runs;
 }
 
 // On the calling thread, before any worker starts: every member whose rows are not laid out for its current ranges (a
-// new partition re-runs skb_flow_group_init) lays them out for the recorded bodies, and its local-vector buffers take
-// their size -- nothing allocates while a peer on the same device waits on a flag
+// new partition re-runs skb_flow_group_init) lays them out for the recorded bodies
 static int mflow_local_rows(skb_mflow *mf, const char *who) {
     if (mf->n_bodies > 0 && (int)mf->body_n.size() != mf->n_bodies)
         return set_error(SKB_ERR_INVALID, "%s: call skb_mflow_set_body_operators first", who);
@@ -711,9 +675,6 @@ static int mflow_local_rows(skb_mflow *mf, const char *who) {
         SKB_TRY(prepare_matvec_targets(fl));
         if (fl->grp.member() && !fl->grp.rows_for(group_ranges(fl)))
             SKB_TRY(flow_member_lay_out_rows(fl, who, mf->body_n.data(), mf->n_bodies));
-        const long long n = member_local_size(mf, g);
-        SKB_TRY(mf->io[(size_t)g].x.ensure((size_t)n * 8 + 8));
-        SKB_TRY(mf->io[(size_t)g].res.ensure((size_t)n * 8 + 8));
     }
     return SKB_OK;
 }
@@ -797,8 +758,7 @@ int skb_mflow_set_fiber_links(skb_mflow *mf, const int *body, const double *site
     });
 }
 
-// the refusals of both system calls, before any launch; then every member's rows are laid out and every buffer the
-// calls use is sized
+// the refusals of both system calls, before any launch; then every member's rows are laid out
 static int mflow_system_args(skb_mflow *mf, const char *who, bool precondition, bool args) {
     if (!mf)
         return set_error(SKB_ERR_INVALID, "%s: NULL", who);
@@ -826,8 +786,22 @@ static int mflow_system_args(skb_mflow *mf, const char *who, bool precondition, 
     }
     if (!args)
         return set_error(SKB_ERR_INVALID, "%s: NULL argument", who);
-    SKB_TRY(mflow_local_rows(mf, who));
-    return mflow_size_io(mf, 0);
+    return mflow_local_rows(mf, who);
+}
+
+// member g's rows of the whole host vector `in` up into its local vector, its local result down into the whole `out`
+static Transfers member_vector(const skb_mflow *mf, int g, const double *in, double *out, double *d_in = nullptr,
+                               double *d_out = nullptr) {
+    const std::vector<Run> rows = member_local(mf, g);
+    return {{up(in, rows, d_in)}, {down(out, rows, d_out)}};
+}
+
+// member g's uploads of the external forces: its fibers' rows of f_external, the bodies' complete forces and torques
+static std::vector<Transfer> external_forces(const skb_mflow *mf, int g, const double *f_external,
+                                             const std::vector<double> &f, const std::vector<double> &t) {
+    const MemberRows r = member_rows(mf, g);
+    const long long n_ft = (long long)f.size();
+    return {up(f_external, {{3 * r.a, 0, 3 * r.n_fw}}), up(f.data(), {{0, 0, n_ft}}), up(t.data(), {{0, 0, n_ft}})};
 }
 
 // System::apply_matvec (system.cpp:269-324) over n devices on the whole solution vector
@@ -838,12 +812,11 @@ int skb_mflow_apply_system_matvec(skb_mflow *mf, const double *x, double eta, do
         return set_error(SKB_ERR_INVALID, "%s: eta = %g", who, eta);
     if (mflow_solution_size(mf) == 0)
         return SKB_OK;
+    SKB_TRY(mflow_stage(mf, [&](int g) { return member_vector(mf, g, x, res); }));
     SKB_TRY(mf->workers->run([&](int g) -> int {
-        skb_mflow::IO &io = mf->io[g];
         skb_dense *dn = mf->has_dense ? mf->dn[g].get() : nullptr;
-        return member_through(mf, g, x, (double *)io.x.ptr, (const double *)io.res.ptr, res, [&](cudaStream_t st) {
-            return skb_flow_group_apply_system_matvec_device(mf->m[g].get(), dn, (const double *)io.x.ptr, eta,
-                                                             (double *)io.res.ptr, st);
+        return member_call(mf, g, [&](cudaStream_t st, const Transfers &io) {
+            return skb_flow_group_apply_system_matvec_device(mf->m[g].get(), dn, io.up[0].dev, eta, io.down[0].dev, st);
         });
     }));
     return mflow_collect_stats(mf);
@@ -855,11 +828,11 @@ int skb_mflow_apply_system_preconditioner(skb_mflow *mf, const double *x, double
     SKB_TRY(mflow_system_args(mf, who, true, (x && y) || (mf && mflow_solution_size(mf) == 0)));
     if (mflow_solution_size(mf) == 0)
         return SKB_OK;
+    SKB_TRY(mflow_stage(mf, [&](int g) { return member_vector(mf, g, x, y); }));
     SKB_TRY(mf->workers->run([&](int g) -> int {
-        skb_mflow::IO &io = mf->io[g];
-        return member_through(mf, g, x, (double *)io.x.ptr, (const double *)io.res.ptr, y, [&](cudaStream_t st) {
-            return skb_flow_group_apply_system_preconditioner_device(mf->m[g].get(), mf->dn[g].get(),
-                                                                     (const double *)io.x.ptr, (double *)io.res.ptr, st);
+        return member_call(mf, g, [&](cudaStream_t st, const Transfers &io) {
+            return skb_flow_group_apply_system_preconditioner_device(mf->m[g].get(), mf->dn[g].get(), io.up[0].dev,
+                                                                     io.down[0].dev, st);
         });
     }));
     return mflow_collect_stats(mf);
@@ -901,20 +874,15 @@ int skb_mflow_build_system_rhs(skb_mflow *mf, const skb_fiber_params *params, co
     if (body_forces_torques && mf->n_bodies > 0)
         split_forces_torques(body_forces_torques, mf->n_bodies, f, t);
     SKB_TRY(mflow_local_rows(mf, who));
-    SKB_TRY(mflow_size_io(mf, f.size()));
+    SKB_TRY(mflow_stage(mf, [&](int g) -> Transfers {
+        return {external_forces(mf, g, f_external, f, t), {down(rhs, member_local(mf, g))}};
+    }));
     SKB_TRY(mf->workers->run([&](int g) -> int {
-        skb_mflow::IO &io = mf->io[g];
-        const cudaStream_t st = mf->m[g]->stream;
-        CUDA_TRY(cudaSetDevice(mf->devs[g]));
-        const MemberRows r = member_rows(mf, g);
-        SKB_TRY(put(io.ff, f_external ? f_external + 3 * r.a : nullptr, (size_t)r.n_fw * 3, st));
-        SKB_TRY(put(io.f, f.data(), f.size(), st));
-        SKB_TRY(put(io.t, t.data(), t.size(), st));
-        return member_through(mf, g, nullptr, nullptr, (const double *)io.res.ptr, rhs, [&](cudaStream_t s) {
+        return member_call(mf, g, [&](cudaStream_t st, const Transfers &io) {
             return skb_flow_group_build_system_rhs_device(
                 mf->m[g].get(), own_slice(mf, g, params), own_slice(mf, g, v_growth), own_slice(mf, g, force_scale),
-                f_external ? (const double *)io.ff.ptr : nullptr, f.empty() ? nullptr : (const double *)io.f.ptr,
-                t.empty() ? nullptr : (const double *)io.t.ptr, dt, eta, (double *)io.res.ptr, s);
+                f_external ? io.up[0].dev : nullptr, f.empty() ? nullptr : io.up[1].dev,
+                t.empty() ? nullptr : io.up[2].dev, dt, eta, io.down[0].dev, st);
         });
     }));
     return mflow_collect_stats(mf);
@@ -923,20 +891,13 @@ int skb_mflow_build_system_rhs(skb_mflow *mf, const skb_fiber_params *params, co
 // the analytic sources of velocity_at_targets and of the system RHS, on every member
 int skb_mflow_set_point_sources(skb_mflow *mf, const double *positions, const double *forces, const double *torques,
                                 int n_points) {
-    if (!mf)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_set_point_sources: NULL");
-    for (int g = 0; g < mf->n; ++g)
-        SKB_TRY(skb_flow_set_point_sources(mf->m[g].get(), positions, forces, torques, n_points));
-    return SKB_OK;
+    return each_member(mf, "skb_mflow_set_point_sources", skb_flow_set_point_sources, positions, forces, torques,
+                       n_points);
 }
 
 int skb_mflow_set_background(skb_mflow *mf, const int *components, const double *scale_factor,
                              const double *uniform) {
-    if (!mf)
-        return set_error(SKB_ERR_INVALID, "skb_mflow_set_background: NULL");
-    for (int g = 0; g < mf->n; ++g)
-        SKB_TRY(skb_flow_set_background(mf->m[g].get(), components, scale_factor, uniform));
-    return SKB_OK;
+    return each_member(mf, "skb_mflow_set_background", skb_flow_set_background, components, scale_factor, uniform);
 }
 
 // System::velocity_at_targets (system.cpp:330-384) over n devices: the targets are block-partitioned, every device
@@ -988,6 +949,14 @@ static std::vector<long long> gmres_layout(const skb_mflow *mf) {
     return v;
 }
 
+// the members' rows must still be those skb_mflow_set_gmres laid out
+static int mflow_gmres_current(const skb_mflow *mf, const char *who) {
+    if (mf->gmres_set && mf->gmres_layout == gmres_layout(mf))
+        return SKB_OK;
+    return set_error(SKB_ERR_INVALID, "%s: call skb_mflow_set_gmres after the partition or the bodies' node counts "
+                                      "changed", who);
+}
+
 extern "C" {
 
 int skb_mflow_set_gmres(skb_mflow *mf, int num_blocks) {
@@ -1022,9 +991,7 @@ int skb_mflow_solve_system(skb_mflow *mf, const double *rhs, double eta, double 
         info->converged = 1;
         return SKB_OK;
     }
-    if (!mf->gmres_set || mf->gmres_layout != gmres_layout(mf))
-        return set_error(SKB_ERR_INVALID, "%s: call skb_mflow_set_gmres after the partition or the bodies' node counts "
-                                          "changed", who);
+    SKB_TRY(mflow_gmres_current(mf, who));
     for (int g = 0; g < mf->n; ++g) {
         skb_flow *fl = mf->m[(size_t)g].get();
         long long n = 0;
@@ -1036,13 +1003,15 @@ int skb_mflow_solve_system(skb_mflow *mf, const double *rhs, double eta, double 
     }
     std::vector<skb_solve_info> infos((size_t)mf->n);
     std::vector<std::vector<double>> hist((size_t)mf->n, std::vector<double>(history ? (size_t)max_iters + 1 : 0));
+    SKB_TRY(mflow_stage(mf, [&](int g) {
+        const Krylov &kry = mf->m[(size_t)g]->kry;
+        return member_vector(mf, g, rhs, x, kry.stage_b(), kry.stage_x());
+    }));
     SKB_TRY(mf->workers->run([&](int g) -> int {
-        skb_flow *fl = mf->m[(size_t)g].get();
-        const Krylov &kry = fl->kry;
         skb_dense *dn = mf->dn[(size_t)g].get();
-        return member_through(mf, g, rhs, kry.stage_b(), kry.stage_x(), x, [&](cudaStream_t st) {
-            return skb_flow_group_solve_system_device(fl, dn, dn, kry.stage_b(), eta, tol, num_blocks, max_iters,
-                                                      kry.stage_x(), &infos[(size_t)g],
+        return member_call(mf, g, [&](cudaStream_t st, const Transfers &io) {
+            return skb_flow_group_solve_system_device(mf->m[(size_t)g].get(), dn, dn, io.up[0].dev, eta, tol,
+                                                      num_blocks, max_iters, io.down[0].dev, &infos[(size_t)g],
                                                       history ? hist[(size_t)g].data() : nullptr, st);
         });
     }));
@@ -1080,9 +1049,7 @@ int skb_mflow_step(skb_mflow *mf, const skb_fiber_params *params, const double *
         info->solve.converged = 1;
         return SKB_OK;
     }
-    if (!mf->gmres_set || mf->gmres_layout != gmres_layout(mf))
-        return set_error(SKB_ERR_INVALID, "%s: call skb_mflow_set_gmres after the partition or the bodies' node counts "
-                                          "changed", who);
+    SKB_TRY(mflow_gmres_current(mf, who));
     std::vector<StepArgs> args((size_t)mf->n);
     std::vector<StepCall> calls((size_t)mf->n);
     for (int g = 0; g < mf->n; ++g) {
@@ -1098,35 +1065,24 @@ int skb_mflow_step(skb_mflow *mf, const skb_fiber_params *params, const double *
     std::vector<double> f, t;
     if (body_forces_torques && nb > 0)
         split_forces_torques(body_forces_torques, nb, f, t);
-    SKB_TRY(mflow_size_io(mf, f.size()));
+    SKB_TRY(mflow_stage(mf, [&](int g) { return Transfers{external_forces(mf, g, f_external, f, t), {}}; }));
 
     // ---- every member's step; its local rows of the solution and its own tensions into the complete host arrays ----
     std::vector<skb_step_info> infos((size_t)mf->n);
     const int rc = mf->workers->run([&](int g) -> int {
-        skb_flow *fl = mf->m[(size_t)g].get();
-        skb_mflow::IO &io = mf->io[(size_t)g];
-        CUDA_TRY(cudaSetDevice(mf->devs[(size_t)g]));
-        const MemberRows r = member_rows(mf, g);
-        const cudaStream_t st = fl->stream;
-        SKB_TRY(put(io.ff, f_external ? f_external + 3 * r.a : nullptr, (size_t)r.n_fw * 3, st));
-        SKB_TRY(put(io.f, f.data(), f.size(), st));
-        SKB_TRY(put(io.t, t.data(), t.size(), st));
         std::vector<double> loc(x ? (size_t)calls[(size_t)g].n : 0);
-        skb_dense *dn = mf->dn[(size_t)g].get();
-        CUDA_TRY(cudaEventRecord(io.e0, st));
-        const int rc_g = group_step_run(fl, dn, dn, args[(size_t)g], calls[(size_t)g],
-                                        f_external ? (const double *)io.ff.ptr : nullptr,
-                                        f.empty() ? nullptr : (const double *)io.f.ptr,
-                                        t.empty() ? nullptr : (const double *)io.t.ptr, x ? loc.data() : nullptr,
-                                        tension ? tension + r.a : nullptr, &infos[(size_t)g], who, st);
-        if (rc_g != SKB_OK && rc_g != SKB_ERR_STATE) // (SKB_ERR_STATE: not installed, the outputs are there)
-            return rc_g;
-        CUDA_TRY(cudaEventRecord(io.e1, st));
+        int rc_g = SKB_OK;
+        SKB_TRY(member_call(mf, g, [&](cudaStream_t st, const Transfers &io) {
+            skb_dense *dn = mf->dn[(size_t)g].get();
+            rc_g = group_step_run(mf->m[(size_t)g].get(), dn, dn, args[(size_t)g], calls[(size_t)g],
+                                  f_external ? io.up[0].dev : nullptr, f.empty() ? nullptr : io.up[1].dev,
+                                  t.empty() ? nullptr : io.up[2].dev, x ? loc.data() : nullptr,
+                                  tension ? tension + member_rows(mf, g).a : nullptr, &infos[(size_t)g], who, st);
+            return rc_g == SKB_ERR_STATE ? SKB_OK : rc_g; // (SKB_ERR_STATE: not installed, the outputs are there)
+        }));
         if (x)
-            member_local(mf, g, [&](long long whole, long long at, long long len) {
-                std::memcpy(x + whole, loc.data() + at, (size_t)len * 8);
-                return SKB_OK;
-            });
+            for (const Run &p : member_local(mf, g))
+                std::memcpy(x + p.whole, loc.data() + p.at, (size_t)p.len * 8);
         return rc_g;
     });
     mf->ops_ready = rc == SKB_ERR_STATE; // built by the step; an installed step set new fibers, which drops them

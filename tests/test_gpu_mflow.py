@@ -123,6 +123,58 @@ def test_mflow_apply_matvec_matches_oracle(with_dense):
         assert st["launches"] > 0 and st["n_pairs"] > 0
 
 
+def test_resized_geometry_matches_a_fresh_multiflow():
+    """Grow the fibers, then the periphery, then the bodies of one MultiFlow, and shrink them again in reverse order.
+    After every change each host-array call (matvec, apply_matvec with and without the periphery's dense operator, the
+    whole-system matvec, preconditioner and RHS) gives bitwise what a MultiFlow set up directly on that geometry gives:
+    every call stages its members' transfers for the sizes it meets, also for members that share a device."""
+    from test_gpu_system_edges import DT, ETA, edge_case, partial_inputs, setup_mflow_edges
+
+    small = dict(n_fibers=24, nodes=(8, 16), n_shell=200, n_body_nodes=400, n_bodies=2)
+    grown = [dict(small, n_fibers=40)]
+    grown.append(dict(grown[-1], n_shell=300))
+    grown.append(dict(grown[-1], n_body_nodes=600, n_bodies=3))
+    shapes = [small] + grown + grown[-2::-1] + [small]
+    cases = [edge_case(kw, 60 + i) for i, kw in enumerate(shapes)]
+
+    def set_up(mf, case, dense):
+        fib, shell, bodies, ops, links = case[:5]
+        if dense:
+            setup_mflow_edges(mf, fib, shell, bodies, ops, links)
+            return
+        load_m(mf, fib, shell, bodies)
+        for n in ops["D_1_0"]:
+            mf.set_fiber_class(n, ops["D_1_0"][n], ops["P"][n])
+        mf.set_fiber_operators(ops["A"], ops["force"], ops["xs"], ops["length_prev"], ops["plus"])
+
+    def calls(mf, case, dense):
+        fib, shell, bodies, ops, links, x, params, _, src = case
+        strengths, partial, _ = partial_inputs(fib, shell, bodies, x, 70)
+        link = np.random.default_rng(71).normal(size=(len(fib["n_nodes"]), 7))
+        if dense:
+            mf.set_point_sources(*src["points"])
+            mf.set_background(*src["background"])
+        out = [mf.matvec(*strengths, ETA), *mf.apply_matvec(*partial, ETA, link)]
+        if dense:
+            out += [mf.apply_system_matvec(x, ETA), mf.apply_system_preconditioner(x),
+                    mf.build_system_rhs(*params, DT, ETA, f_external=src["f_ext"], body_forces_torques=src["ft"],
+                                        v_growth=src["v_growth"], force_scale=src["force_scale"])]
+        return out
+
+    for devs in device_lists()[1:]:
+        for dense in (False, True):
+            with skb.MultiFlow(devs) as mf:
+                for kw, case in zip(shapes, cases):
+                    set_up(mf, case, dense)
+                    got = calls(mf, case, dense)
+                    with skb.MultiFlow(devs) as fresh:
+                        set_up(fresh, case, dense)
+                        want = calls(fresh, case, dense)
+                    assert len(got) == (7 if dense else 4)
+                    for k, (g, w) in enumerate(zip(got, want)):
+                        assert np.array_equal(g, w), (devs, dense, kw, k)
+
+
 def test_mflow_velocity_at_targets():
     fib, shell, body = make_system(77, 30, 300, 120, 1)
     rng = np.random.default_rng(3)
