@@ -1,5 +1,5 @@
 """GPU tests of skb_flow_listener_gradient (capi.listener_gradient): the velocity gradient and the pressure of the
-listener's frame against the long-double restatement of tests/listener_gradient_reference.py, source class by class and
+listener's frame against the long-double restatement of tests/gradient_reference.py, source class by class and
 for a whole frame; the frame of a step against the same frame from its parts; the rigid gradient inside bodies; the
 vorticity of the existing vortex-line request; reproducibility; the following velocity calls; staleness and refusals.
 
@@ -11,7 +11,8 @@ is below (n_src + 64) u M, M = sum over sources of m.  The pressure's parts are 
 import numpy as np
 import pytest
 
-import listener_gradient_reference as lg
+import gradient_reference as gr
+import pair_sum_reference as ps
 import skellysim_b200 as skb
 from skellysim_b200 import capi
 from test_gpu_flow import ft_of, load
@@ -23,9 +24,12 @@ U = 2.0 ** -53
 
 
 def reference(fr, r):
-    # the bodies with an interior test (Frame.inside tests every body)
-    inside = [m if fr.kind[b] else np.zeros(len(r), dtype=bool) for b, m in enumerate(fr.inside(r))]
-    return lg.frame_gradient(fr.fib, fr.shell, fr.body, fr.pts, fr.pf, fr.ptq, fr.bg, ETA, r, inside, fr.uw)
+    """(G, p) of the restatement, the interior rows replaced as gradient_finish_kernel replaces them"""
+    (ext, _, _), inside, rigid = gr.listener_gradient(fr.fib, fr.shell, fr.body, r, ETA, fr.kind, fr.radii, fr.uw,
+                                                      (fr.pts, fr.pf, fr.ptq), fr.bg)
+    ext = np.asarray(ext, dtype=np.float64)
+    ext[inside] = rigid[inside]
+    return gr.as_grad_pressure(ext)
 
 
 def _inv_r(src, r, p):
@@ -44,8 +48,7 @@ def magnitude(fr, r):
     M = np.zeros(len(r))
     n = 0
     if len(fib["n_nodes"]):
-        w = np.concatenate([np.asarray(lg.trapezoid_weights(k, L), dtype=np.float64)
-                            for k, L in zip(fib["n_nodes"], fib["lengths"])])
+        w = ps.trapezoid_weights(fib["n_nodes"], fib["lengths"])
         M += 6 * c * _inv_r(fib["pos"], r, 2) @ (np.linalg.norm(fib["forces"], axis=1) * w)
         n += len(w)
     for pos, nrm, rho in ((shell["pos"], shell["normals"], shell.get("density")),

@@ -1,11 +1,11 @@
-"""CPU tests of tests/listener_gradient_reference.py, the restatement the GPU tests of skb_flow_listener_gradient hold
-the device to: its gradients against long-double central differences of the oracle's velocities, class by class; the
-pressure against the Stokes equations (grad p = eta lap u); the trace of the gradient; the interior rule and the r == 0
-rule; and the marshalling of capi.listener_gradient."""
+"""CPU tests of the physics of tests/gradient_reference.py, the restatement the GPU tests of skb_flow_listener_gradient
+hold the device to: its gradients against long-double central differences of the oracle's velocities, class by class;
+the pressure against the Stokes equations (grad p = eta lap u); the trace of the gradient; the interior rule and the
+r == 0 rule; and the marshalling of capi.listener_gradient."""
 import numpy as np
 import pytest
 
-import listener_gradient_reference as lg
+import gradient_reference as gr
 import oracle as orc
 from skellysim_b200 import capi
 from test_capi_binding_cpu import _drive, _inputs, _twin_calls, calls  # noqa: F401 (the fixture)
@@ -31,15 +31,37 @@ def _fd_gradient(vel, r, h=1e-4):
     return G
 
 
+def _G(part):
+    return np.asarray(part[0][:, :9], dtype=LD).reshape(-1, 3, 3)
+
+
+def _Gp(part, eta=ETA):
+    """(G, p) of a part, its pressure multiplied by eta as gradient_finish_kernel does"""
+    return _G(part), part[0][:, 9] * LD(eta)
+
+
+def _sym6(S9):
+    S9 = np.asarray(S9, dtype=np.float64).reshape(-1, 9)
+    return np.stack([S9[:, 0], S9[:, 4], S9[:, 8], S9[:, 1] + S9[:, 3], S9[:, 2] + S9[:, 6], S9[:, 5] + S9[:, 7]], 1)
+
+
+def stokeslet(src, f, r):
+    return _Gp(gr.pair_grad_rows("sl", src, f, r, ETA))
+
+
+def stresslet(src, S9, r):
+    return _Gp(gr.pair_grad_rows("dl6", src, _sym6(S9), r, ETA))
+
+
 def _flows(rng, src):
     f = rng.normal(size=src.shape)
     S = rng.normal(size=(len(src), 9))
     L = rng.normal(size=src.shape)
     return {
-        "stokeslet": (lambda r: orc.stokeslet_direct_ld(src, f, r) / ETA, lambda r: lg.stokeslet(src, f, r, ETA)[0]),
-        "stresslet": (lambda r: orc.stresslet_direct_ld(src, S, r) / ETA, lambda r: lg.stresslet(src, S, r, ETA)[0]),
-        "rotlet": (lambda r: orc.rotlet(src, r, L, ETA), lambda r: lg.rotlet(src, L, r, ETA)),
-        "oseen": (lambda r: orc.oseen_contract(src, r, f, ETA), lambda r: lg.oseen(src, f, r, ETA)[0]),
+        "stokeslet": (lambda r: orc.stokeslet_direct_ld(src, f, r) / ETA, lambda r: stokeslet(src, f, r)[0]),
+        "stresslet": (lambda r: orc.stresslet_direct_ld(src, S, r) / ETA, lambda r: stresslet(src, S, r)[0]),
+        "rotlet": (lambda r: orc.rotlet(src, r, L, ETA), lambda r: _G(gr.rotlet_grad(r, src, L, ETA))),
+        "oseen": (lambda r: orc.oseen_contract(src, r, f, ETA), lambda r: _G(gr.oseen_grad(r, src, f, ETA))),
     }
 
 
@@ -54,7 +76,7 @@ def test_the_gradient_is_the_derivative_of_the_oracle_velocity(kind):
 
 def test_the_background_gradient_is_its_scale():
     comp, scale = [1, 0, 2], np.array([0.2, -0.1, 0.05])
-    G = lg.background(2, comp, scale)
+    G = _G(gr.background_grad(2, comp, scale))
     expect = np.zeros((3, 3))
     expect[0, 1], expect[1, 0], expect[2, 2] = scale
     assert np.array_equal(G[0], expect) and np.array_equal(G[1], expect)
@@ -65,9 +87,9 @@ def test_the_pressure_satisfies_the_stokes_equations(kind):
     rng, src, trg = _system(2)
     f, S = rng.normal(size=src.shape), rng.normal(size=(len(src), 9))
     if kind == "stokeslet":
-        gp = lambda r: lg.stokeslet(src, f, r, ETA)
+        gp = lambda r: stokeslet(src, f, np.asarray(r, dtype=np.float64))
     else:
-        gp = lambda r: lg.stresslet(src, S, r, ETA)
+        gp = lambda r: stresslet(src, S, np.asarray(r, dtype=np.float64))
     # lap u_i = d_j (d_j u_i): the Laplacian of the velocity from the analytic gradient's own divergence
     def lap_u(r):
         h = LD(1e-4)
@@ -89,8 +111,8 @@ def test_the_trace_vanishes_where_the_flow_is_incompressible():
     f, L = rng.normal(size=src.shape), rng.normal(size=src.shape)
     S = rng.normal(size=(len(src), 3, 3))
     S -= np.trace(S, axis1=1, axis2=2)[:, None, None] * np.eye(3) / 3
-    for G in (lg.stokeslet(src, f, trg, ETA)[0], lg.rotlet(src, L, trg, ETA),
-              lg.stresslet(src, S.reshape(-1, 9), trg, ETA)[0]):
+    for G in (stokeslet(src, f, trg)[0], _G(gr.rotlet_grad(trg, src, L, ETA)),
+              stresslet(src, S.reshape(-1, 9), trg)[0]):
         tr = np.trace(np.asarray(G, dtype=np.float64), axis1=1, axis2=2)
         assert np.abs(tr).max() <= 1e-15 * np.abs(np.asarray(G, dtype=np.float64)).max()
 
@@ -99,8 +121,9 @@ def test_a_coincident_pair_adds_nothing():
     rng, src, trg = _system(4)
     f, S, L = rng.normal(size=src.shape), rng.normal(size=(len(src), 9)), rng.normal(size=src.shape)
     r = np.concatenate([trg, src[:2]])
-    for fn in (lambda k, r: lg.stokeslet(src[k], f[k], r, ETA), lambda k, r: lg.stresslet(src[k], S[k], r, ETA),
-               lambda k, r: lg.oseen(src[k], f[k], r, ETA), lambda k, r: (lg.rotlet(src[k], L[k], r, ETA), None)):
+    for fn in (lambda k, r: stokeslet(src[k], f[k], r), lambda k, r: stresslet(src[k], S[k], r),
+               lambda k, r: _Gp(gr.oseen_grad(r, src[k], f[k], ETA)),
+               lambda k, r: (_G(gr.rotlet_grad(r, src[k], L[k], ETA)), None)):
         all_src = fn(slice(None), r)
         # target src[0] against the other sources only equals the full sum there
         others = fn(slice(1, None), r[-2:-1])
@@ -116,15 +139,15 @@ def test_the_interior_rule():
                  density=np.zeros((0, 3)))
     uw = np.array([[0, 0, 0, 1.0, 2.0, 3.0], [0, 0, 0, -1.0, 0.5, 0.25]])
     r = np.array([[0.05, 0, 0], [2.0, 0, 0]])
-    ins = [np.array([True, False]), np.array([True, False])]
-    G, p = lg.frame_gradient(empty, empty, body, np.zeros((0, 3)), None, None, None, ETA, r, ins, uw)
+    (ext, _, _), inside, rigid = gr.listener_gradient(empty, empty, body, r, ETA, [1, 1], [[0.4, 0, 0]] * 2, uw)
+    assert inside.tolist() == [True, False]
     w = uw[1, 3:]
-    assert np.array_equal(np.asarray(G[0], dtype=np.float64),
+    assert np.array_equal(rigid[0, :9].reshape(3, 3),
                           np.array([[0, -w[2], w[1]], [w[2], 0, -w[0]], [-w[1], w[0], 0]]))  # the last body wins
-    assert np.isnan(p[0]) and p[1] == 0 and not np.isnan(np.asarray(G[1], dtype=np.float64)).any()
+    assert np.isnan(rigid[0, 9]) and ext[1, 9] == 0 and np.isfinite(np.asarray(ext[1], dtype=np.float64)).all()
     # the rigid gradient is that of U + omega x dx
     dx = np.array([0.3, -0.2, 0.1])
-    assert np.allclose(np.asarray(lg.rigid_gradient(w), dtype=np.float64) @ dx, np.cross(w, dx), rtol=0, atol=1e-15)
+    assert np.allclose(gr.rigid_gradient(w)[:9].reshape(3, 3) @ dx, np.cross(w, dx), rtol=0, atol=1e-15)
 
 
 def test_listener_gradient_is_marshalled_as_declared(calls):
