@@ -20,6 +20,36 @@ int skb::download(skb_flow *fl, double *h, const DevBuf &buf, size_t n_doubles) 
     return SKB_OK;
 }
 
+int skb::stage_slots(std::vector<DevBuf> &slots, Transfers &x) {
+    slots.resize(std::max(slots.size(), x.up.size() + x.down.size()));
+    size_t k = 0;
+    for (std::vector<Transfer> *list : {&x.up, &x.down})
+        for (Transfer &t : *list) {
+            DevBuf &slot = slots[k++];
+            if (t.dev)
+                continue;
+            long long n = 0;
+            for (const Run &r : t.runs)
+                n = std::max(n, r.at + r.len);
+            SKB_TRY(slot.ensure((size_t)n * 8 + 8));
+            t.dev = (double *)slot.ptr;
+        }
+    return SKB_OK;
+}
+
+int skb::issue(const std::vector<Transfer> &list, bool upload, cudaStream_t st) {
+    for (const Transfer &t : list)
+        for (const Run &r : t.runs) {
+            if (!t.host || !r.len)
+                continue;
+            double *d = t.dev + r.at, *h = t.host + r.whole;
+            const size_t bytes = (size_t)r.len * 8;
+            CUDA_TRY(upload ? cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, st)
+                            : cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, st));
+        }
+    return SKB_OK;
+}
+
 void skb::begin_stats(skb_flow *fl) {
     fl->launches = 0;
     fl->pairs = 0;
@@ -276,7 +306,7 @@ int skb_flow_group_warmup(skb_flow *fl) {
     SKB_TRY(z.ensure(n_z * 8));
     CUDA_TRY(cudaMemsetAsync(z.ptr, 0, n_z * 8, fl->stream));
     SKB_TRY(fl->vel.ensure((size_t)fl->n_win * 24 + 8));
-    SKB_TRY(fl->in_fib.ensure((size_t)n_fw * 24 + 8));
+    SKB_TRY(fl->fw.ensure((size_t)n_fw * 24 + 8));
     if (n_sw > 0 && fl->bg.enabled)
         SKB_TRY(overlap_buffers(fl, 3 * n_sw));
     fl->cur = fl->stream;

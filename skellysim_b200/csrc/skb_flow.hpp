@@ -14,6 +14,35 @@
 #include <vector>
 
 namespace skb {
+// The copies of one host-array call (the flow's and skb_mflow's): each Run moves len doubles between the caller's array
+// at `whole` and the device array at `at`
+struct Run {
+    long long whole, at, len;
+};
+struct Transfer {
+    double *host;          // the caller's array (only read by an upload); NULL: nothing to copy
+    double *dev;           // a device array the callee owns, or the staging slot stage_slots gives it
+    std::vector<Run> runs;
+};
+struct Transfers {
+    std::vector<Transfer> up, down; // before the call, after it
+};
+inline Transfer up(const double *h, std::vector<Run> runs, double *dev = nullptr) {
+    return Transfer{const_cast<double *>(h), dev, std::move(runs)};
+}
+inline Transfer down(double *h, std::vector<Run> runs, double *dev = nullptr) {
+    return Transfer{h, dev, std::move(runs)};
+}
+// the whole array of n doubles
+inline Transfer up(const double *h, long long n) { return up(h, {{0, 0, n}}); }
+inline Transfer down(double *h, long long n) { return down(h, {{0, 0, n}}); }
+// Every transfer of x without a device array gets one of `slots` (the slots of x.up, then those of x.down), grown to
+// 8 bytes beyond the end of its runs, so that a call gets a device pointer for an empty array too.  Slots only grow;
+// a transfer that has a device array keeps it.  May allocate: skb_mflow stages on the calling thread
+int stage_slots(std::vector<DevBuf> &slots, Transfers &x);
+// the runs of `list` issued on st: x.up host to device (upload true), x.down device to host
+int issue(const std::vector<Transfer> &list, bool upload, cudaStream_t st);
+
 struct TargetCache {
     std::vector<double> host;
     bool valid = false;
@@ -240,12 +269,15 @@ struct skb_flow {
         skb_dense *dn = nullptr;   // pending background product of the call in flight (nullptr: none)
         bool launched = false;
     } bg;
-    skb::DevBuf scratch_u; // group mode: landing zone of Evaluator::eval's default output (never read)
-    // staging
-    skb::DevBuf in_fib, in_shell, in_body, in_force, in_torque, vel, tmp, x_fib, res_fib, vb, res_shell, tmp_b;
-    skb::DevBuf sys_x, sys_y; // the whole solution vector in and out of the host forms of the system operator
-    skb::DevBuf zeros;        // the system RHS: the zero densities (and absent forces) its flow takes, n_zeros doubles
+    // The device cores' workspace, like sys_rb and ft_sum above: they read and write it, and no transfer of a
+    // host-array call ever targets it.  vel: v_all of apply_matvec_core and the system RHS; fw: the fibers' force of apply_matvec_core; tmp: the
+    // periphery rows of matvec_core; tmp_b: the system matvec's v_bodies; scratch_u: group mode's landing zone of
+    // Evaluator::eval's default output (never read)
+    skb::DevBuf vel, fw, tmp, tmp_b, scratch_u;
+    skb::DevBuf zeros; // the system RHS: the zero densities (and absent forces) its flow takes, n_zeros doubles
     long long n_zeros = 0;
+    // the staging slots of the host-array calls (host_call): their inputs and outputs on the device
+    std::vector<skb::DevBuf> slots;
     skb::Krylov kry; // the workspace of skb_flow_solve_system (skb_solve.cu)
     skb_flow_stats stats{};
     int launches = 0;
@@ -285,6 +317,20 @@ template <class Up, class Work, class Down> int host_frame(skb_flow *fl, Up up, 
 }
 // the step of host_frame that has nothing to do
 inline int nothing() { return SKB_OK; }
+// Frame of the flow's host-array calls: x staged into the flow's slots (stage_slots), then in host_frame x's uploads
+// and before() (a call's own uploads, such as FiberOps::rhs's tables), work(x), x's downloads; returns once the
+// downloads have landed
+template <class Work, class Before = int (*)()>
+int host_call(skb_flow *fl, Transfers &x, Work work, Before before = nothing) {
+    SKB_TRY(stage_slots(fl->slots, x));
+    return host_frame(
+        fl,
+        [&]() -> int {
+            SKB_TRY(issue(x.up, true, fl->stream));
+            return before();
+        },
+        [&] { return work((const Transfers &)x); }, [&] { return issue(x.down, false, fl->stream); });
+}
 // frame of the device-pointer entry points: work on the caller's stream, then the statistics of no timing
 template <class Work> int device_frame(skb_flow *fl, void *stream, Work work) {
     fl->cur = (cudaStream_t)stream;

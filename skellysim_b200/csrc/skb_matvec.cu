@@ -221,11 +221,14 @@ static int ensure_stage(skb_flow *fl, size_t n_doubles) {
     return SKB_OK;
 }
 
-// every device address a captured sequence may bake in: a reallocation anywhere invalidates the graph
-static unsigned long long buffer_key(const skb_flow *fl, int which) {
+// every device address a captured sequence may bake in: a reallocation anywhere invalidates the graph.  The staging
+// slots of x, the workspace, the geometry and the buffers of the evaluators `which`
+static unsigned long long buffer_key(const skb_flow *fl, int which, const Transfers &x) {
     unsigned long long h = 0x1234567ULL;
-    const DevBuf *bufs[] = {&fl->in_fib, &fl->in_shell, &fl->in_body, &fl->in_force, &fl->in_torque, &fl->vel,
-                            &fl->tmp,    &fl->pt_pos,   &fl->pt_force, &fl->pt_torque, &fl->centers, &fl->r_fib};
+    for (const std::vector<Transfer> *list : {&x.up, &x.down})
+        for (const Transfer &t : *list)
+            h = mix_key(h, (unsigned long long)(uintptr_t)t.dev);
+    const DevBuf *bufs[] = {&fl->tmp, &fl->pt_pos, &fl->pt_force, &fl->pt_torque, &fl->centers, &fl->r_fib};
     for (const DevBuf *b : bufs)
         h = mix_key(h, (unsigned long long)(uintptr_t)b->ptr);
     for (const Evaluator *e : {&fl->fib[which], &fl->shell[which], &fl->body[which]}) {
@@ -237,33 +240,6 @@ static unsigned long long buffer_key(const skb_flow *fl, int which) {
         }
     }
     return h;
-}
-
-// Inputs and output of a call: the caller's arrays, or (pinned == true) copies in the pinned staging
-// [fiber forces | periphery densities | body densities | body forces | body torques | output] when the call is small
-// enough to be replayed as one CUDA graph, whose memcpy nodes need fixed host addresses
-struct Staged {
-    const double *ff, *sd, *bd, *f, *t;
-    double *v;
-    bool pinned;
-};
-static int stage_inputs(skb_flow *fl, const double *ff, const double *sd, const double *bd,
-                        const std::vector<double> &f, const std::vector<double> &t, double *v, size_t n_out,
-                        Staged &s) {
-    const long long nf = fl->n_fib, ns = fl->n_shell, nb = fl->n_body;
-    const size_t n_in = (size_t)(nf + ns + nb) * 3 + f.size() + t.size();
-    s = Staged{ff, sd, bd, f.data(), t.data(), v, false};
-    if (!fl->graphs_enabled || (n_in + n_out) * 8 > kGraphMaxBytes)
-        return SKB_OK;
-    SKB_TRY(ensure_stage(fl, n_in + n_out));
-    double *h_ff = fl->h_stage, *h_sd = h_ff + 3 * nf, *h_bd = h_sd + 3 * ns, *h_f = h_bd + 3 * nb, *h_t = h_f + f.size();
-    if (nf) std::memcpy(h_ff, ff, (size_t)nf * 24);
-    if (ns) std::memcpy(h_sd, sd, (size_t)ns * 24);
-    if (nb) std::memcpy(h_bd, bd, (size_t)nb * 24);
-    if (!f.empty()) std::memcpy(h_f, f.data(), f.size() * 8);
-    if (!t.empty()) std::memcpy(h_t, t.data(), t.size() * 8);
-    s = Staged{h_ff, h_sd, h_bd, h_f, h_t, h_t + t.size(), true};
-    return SKB_OK;
 }
 
 // Run `body` (asynchronous work on fl->stream, fixed addresses only) either directly, as a capture followed by a
@@ -308,6 +284,51 @@ template <class Body> static int run_graphed(skb_flow *fl, skb_flow::GraphSlot &
     return body();
 }
 
+// host_call of a launch-bound call.  When its copies are small enough (and graphs are on), the pinned mode: the
+// caller's arrays are copied into the pinned staging, whose fixed host addresses a graph's memcpy nodes need, laid
+// out as x's runs in order; the whole sequence, copies included, runs through run_graphed under `key` and the
+// addresses it bakes in (the evaluators `which`), between the frame's events; then the outputs go to the caller
+template <class Work>
+static int replayable_call(skb_flow *fl, skb_flow::GraphSlot &slot, int which, unsigned long long key, Transfers &x,
+                           Work work) {
+    size_t n = 0;
+    for (const std::vector<Transfer> *list : {&x.up, &x.down})
+        for (const Transfer &t : *list)
+            for (const Run &r : t.runs)
+                n += (size_t)r.len;
+    if (!fl->graphs_enabled || n * 8 > kGraphMaxBytes)
+        return host_call(fl, x, work);
+    SKB_TRY(ensure_stage(fl, n));
+    const std::vector<Transfer> out = x.down; // the caller's arrays
+    long long at = 0;
+    for (std::vector<Transfer> *list : {&x.up, &x.down})
+        for (Transfer &t : *list) {
+            for (Run &r : t.runs) {
+                if (list == &x.up && t.host && r.len)
+                    std::memcpy(fl->h_stage + at, t.host + r.whole, (size_t)r.len * 8);
+                r.whole = at;
+                at += r.len;
+            }
+            if (t.host)
+                t.host = fl->h_stage;
+        }
+    SKB_TRY(stage_slots(fl->slots, x));
+    key = mix_key(key, buffer_key(fl, which, x));
+    SKB_TRY(host_frame(fl, nothing, [&] {
+        return run_graphed(fl, slot, key, [&]() -> int {
+            SKB_TRY(issue(x.up, true, fl->stream));
+            SKB_TRY(work((const Transfers &)x));
+            return issue(x.down, false, fl->stream);
+        });
+    }, nothing));
+    for (size_t i = 0; i < out.size(); ++i)
+        for (size_t j = 0; j < out[i].runs.size(); ++j)
+            if (out[i].host && out[i].runs[j].len)
+                std::memcpy(out[i].host + out[i].runs[j].whole, fl->h_stage + x.down[i].runs[j].whole,
+                            (size_t)out[i].runs[j].len * 8);
+    return SKB_OK;
+}
+
 extern "C" {
 
 int skb_flow_fibers(skb_flow *fl, const double *r_trg, int64_t n_trg, const double *fib_forces, double eta,
@@ -319,17 +340,10 @@ int skb_flow_fibers(skb_flow *fl, const double *r_trg, int64_t n_trg, const doub
     SKB_TRY(set_targets_cached(fl, fl->fib[0], fl->tc_fib, r_trg, n_trg));
     if (n_trg == 0)
         return SKB_OK;
-    return host_frame(
-        fl,
-        [&]() -> int {
-            SKB_TRY(upload(fl, fl->in_fib, fib_forces, (size_t)fl->n_fib * 3));
-            return fl->vel.ensure((size_t)n_trg * 24);
-        },
-        [&] {
-            return fibers_dev(fl, fl->fib[0], kRaw, (const double *)fl->in_fib.ptr, eta, subtract_self,
-                              (double *)fl->vel.ptr, 0, 0, fl->n_fib);
-        },
-        [&] { return download(fl, vel, fl->vel, (size_t)n_trg * 3); });
+    Transfers xfer{{up(fib_forces, 3 * fl->n_fib)}, {down(vel, 3 * n_trg)}};
+    return host_call(fl, xfer, [&](const Transfers &io) {
+        return fibers_dev(fl, fl->fib[0], kRaw, io.up[0].dev, eta, subtract_self, io.down[0].dev, 0, 0, fl->n_fib);
+    });
 }
 
 int skb_flow_periphery(skb_flow *fl, const double *r_trg, int64_t n_trg, const double *density, double eta,
@@ -341,17 +355,10 @@ int skb_flow_periphery(skb_flow *fl, const double *r_trg, int64_t n_trg, const d
     SKB_TRY(set_targets_cached(fl, fl->shell[0], fl->tc_shell, r_trg, n_trg));
     if (n_trg == 0)
         return SKB_OK;
-    return host_frame(
-        fl,
-        [&]() -> int {
-            SKB_TRY(upload(fl, fl->in_shell, density, (size_t)fl->n_shell * 3));
-            return fl->vel.ensure((size_t)n_trg * 24);
-        },
-        [&] {
-            return periphery_dev(fl, fl->shell[0], kNormalDensity, (const double *)fl->in_shell.ptr, eta,
-                                 (double *)fl->vel.ptr, 0);
-        },
-        [&] { return download(fl, vel, fl->vel, (size_t)n_trg * 3); });
+    Transfers xfer{{up(density, 3 * fl->n_shell)}, {down(vel, 3 * n_trg)}};
+    return host_call(fl, xfer, [&](const Transfers &io) {
+        return periphery_dev(fl, fl->shell[0], kNormalDensity, io.up[0].dev, eta, io.down[0].dev, 0);
+    });
 }
 
 int skb_flow_bodies(skb_flow *fl, const double *r_trg, int64_t n_trg, const double *densities,
@@ -366,19 +373,11 @@ int skb_flow_bodies(skb_flow *fl, const double *r_trg, int64_t n_trg, const doub
         return SKB_OK;
     std::vector<double> f, t;
     split_forces_torques(forces_torques, fl->n_bodies, f, t);
-    return host_frame(
-        fl,
-        [&]() -> int {
-            SKB_TRY(upload(fl, fl->in_body, densities, (size_t)fl->n_body * 3));
-            SKB_TRY(upload(fl, fl->in_force, f.data(), f.size()));
-            SKB_TRY(upload(fl, fl->in_torque, t.data(), t.size()));
-            return fl->vel.ensure((size_t)n_trg * 24);
-        },
-        [&] {
-            return bodies_dev(fl, fl->body[0], (const double *)fl->in_body.ptr, (const double *)fl->in_force.ptr,
-                              (const double *)fl->in_torque.ptr, eta, (double *)fl->vel.ptr, 0);
-        },
-        [&] { return download(fl, vel, fl->vel, (size_t)n_trg * 3); });
+    Transfers xfer{{up(densities, 3 * fl->n_body), up(f.data(), f.size()), up(t.data(), t.size())},
+                   {down(vel, 3 * n_trg)}};
+    return host_call(fl, xfer, [&](const Transfers &io) {
+        return bodies_dev(fl, fl->body[0], io.up[0].dev, io.up[1].dev, io.up[2].dev, eta, io.down[0].dev, 0);
+    });
 }
 
 
@@ -401,35 +400,20 @@ int skb_flow_velocity_at_targets(skb_flow *fl, const double *r_trg, int64_t n_tr
     std::vector<double> f, t;
     if (fl->n_bodies > 0)
         split_forces_torques(body_forces_torques, fl->n_bodies, f, t);
-    SKB_TRY(fl->vel.ensure((size_t)n_trg * 24));
-    double *d_v = (double *)fl->vel.ptr;
-    Staged s;
-    SKB_TRY(stage_inputs(fl, fib_forces, shell_density, body_densities, f, t, vel, (size_t)n_trg * 3, s));
-    // device-side sequence from the (staged) strengths to the (staged) velocities
-    auto body = [&]() -> int {
-        SKB_TRY(upload(fl, fl->in_fib, s.ff, (size_t)fl->n_fib * 3));
-        SKB_TRY(upload(fl, fl->in_shell, s.sd, (size_t)fl->n_shell * 3));
-        SKB_TRY(upload(fl, fl->in_body, s.bd, (size_t)fl->n_body * 3));
-        SKB_TRY(upload(fl, fl->in_force, s.f, f.size()));
-        SKB_TRY(upload(fl, fl->in_torque, s.t, t.size()));
-        SKB_TRY(velocity_dev(fl, (const double *)fl->fib[0].r_trg.ptr, n_trg, (const double *)fl->in_fib.ptr,
-                             (const double *)fl->in_shell.ptr, (const double *)fl->in_body.ptr,
-                             (const double *)fl->in_force.ptr, (const double *)fl->in_torque.ptr, eta, d_v));
-        return download(fl, s.v, fl->vel, (size_t)n_trg * 3);
-    };
-    if (!s.pinned)
-        return host_frame(fl, nothing, body, nothing);
+    Transfers xfer{{up(fib_forces, 3 * fl->n_fib), up(shell_density, 3 * fl->n_shell),
+                    up(body_densities, 3 * fl->n_body), up(f.data(), f.size()), up(t.data(), t.size())},
+                   {down(vel, 3 * n_trg)}};
     // the listener / streamline integrator asks for 1-6 targets per call (streamline.cpp:11-35): launch-bound
     unsigned long long key = mix_key(fl->geom_version, (unsigned long long)n_trg);
     key = mix_key(key, dbl_bits(eta));
-    key = mix_key(key, buffer_key(fl, 0));
     // same count but different targets: the captured sequence assumed the old targets' relation to the sources
     key = mix_key(key, fl->tc_fib.version);
     key = mix_key(key, fl->tc_shell.version);
     key = mix_key(key, fl->tc_body.version);
-    SKB_TRY(host_frame(fl, nothing, [&] { return run_graphed(fl, fl->g_vat, key, body); }, nothing));
-    std::memcpy(vel, s.v, (size_t)n_trg * 24);
-    return SKB_OK;
+    return replayable_call(fl, fl->g_vat, 0, key, xfer, [&](const Transfers &io) {
+        return velocity_dev(fl, (const double *)fl->fib[0].r_trg.ptr, n_trg, io.up[0].dev, io.up[1].dev, io.up[2].dev,
+                            io.up[3].dev, io.up[4].dev, eta, io.down[0].dev);
+    });
 }
 
 } // extern "C"
@@ -748,39 +732,16 @@ int skb_flow_matvec(skb_flow *fl, const double *fib_forces, const double *shell_
     std::vector<double> f, t;
     if (fl->n_bodies > 0)
         split_forces_torques(body_forces_torques, fl->n_bodies, f, t);
-    SKB_TRY(fl->vel.ensure((size_t)n_win * 24));
-    Staged s;
-    SKB_TRY(stage_inputs(fl, fib_forces, shell_density, body_densities, f, t, v_all, (size_t)n_win * 3, s));
-    auto up = [&]() -> int {
-        SKB_TRY(upload(fl, fl->in_fib, s.ff, (size_t)nf * 3));
-        SKB_TRY(upload(fl, fl->in_shell, s.sd, (size_t)ns * 3));
-        SKB_TRY(upload(fl, fl->in_body, s.bd, (size_t)nb * 3));
-        SKB_TRY(upload(fl, fl->in_force, s.f, f.size()));
-        return upload(fl, fl->in_torque, s.t, t.size());
-    };
-    auto work = [&] {
-        return matvec_core(fl, (const double *)fl->in_fib.ptr, (const double *)fl->in_shell.ptr,
-                           (const double *)fl->in_body.ptr, (const double *)fl->in_force.ptr,
-                           (const double *)fl->in_torque.ptr, eta, (double *)fl->vel.ptr);
-    };
-    auto down = [&] { return download(fl, s.v, fl->vel, (size_t)n_win * 3); };
-    if (!s.pinned)
-        return host_frame(fl, up, work, down);
-    // launch-bound size: replay the whole sequence, copies included, as one CUDA graph
+    Transfers xfer{{up(fib_forces, 3 * nf), up(shell_density, 3 * ns), up(body_densities, 3 * nb),
+                    up(f.data(), f.size()), up(t.data(), t.size())},
+                   {down(v_all, 3 * n_win)}};
     unsigned long long key = mix_key(fl->geom_version, (unsigned long long)fl->fa);
     key = mix_key(key, (unsigned long long)fl->n_win);
     key = mix_key(key, dbl_bits(eta));
-    key = mix_key(key, buffer_key(fl, 1));
-    auto graphed = [&] {
-        return run_graphed(fl, fl->g_matvec, key, [&]() -> int {
-            SKB_TRY(up());
-            SKB_TRY(work());
-            return down();
-        });
-    };
-    SKB_TRY(host_frame(fl, nothing, graphed, nothing));
-    std::memcpy(v_all, s.v, (size_t)n_win * 24);
-    return SKB_OK;
+    return replayable_call(fl, fl->g_matvec, 1, key, xfer, [&](const Transfers &io) {
+        return matvec_core(fl, io.up[0].dev, io.up[1].dev, io.up[2].dev, io.up[3].dev, io.up[4].dev, eta,
+                           io.down[0].dev);
+    });
 }
 
 int skb_flow_matvec_device(skb_flow *fl, const double *d_fib_forces, const double *d_shell_density,
@@ -811,7 +772,7 @@ int skb::apply_matvec_core(skb_flow *fl, skb_dense *dn, const double *d_x, const
                            const double *d_f, const double *d_t, const double *d_link, double eta, double *d_res_fib,
                            double *d_out_shell, double *d_v_bodies) {
     const long long n_fw = fl->fb - fl->fa, n_sw = fl->sb - fl->sa, n_bw = fl->bb - fl->ba;
-    SKB_TRY(fl->in_fib.ensure((size_t)n_fw * 24 + 8));
+    SKB_TRY(fl->fw.ensure((size_t)n_fw * 24 + 8));
     SKB_TRY(fl->vel.ensure((size_t)fl->n_win * 24 + 8));
     // res_shell's dense part, stresslet_plus_complementary_ * x_shell (system.cpp:319, periphery.cpp:38-47), depends on
     // x_shell only: it is handed to the background streamer, which matvec_core launches as soon as x_shell is complete
@@ -825,9 +786,9 @@ int skb::apply_matvec_core(skb_flow *fl, skb_dense *dn, const double *d_x, const
         B.dn = dn;
     }
     // MatrixXd fw = fc.apply_fiber_force(x_fibers)                       system.cpp:298
-    SKB_TRY(fl->ops.force(d_x, (double *)fl->in_fib.ptr, fl->cur, &fl->launches));
+    SKB_TRY(fl->ops.force(d_x, (double *)fl->fw.ptr, fl->cur, &fl->launches));
     // v_all of system.cpp:299-316 (own rows)
-    SKB_TRY(matvec_core(fl, (const double *)fl->in_fib.ptr, d_xs, d_bd, d_f, d_t, eta, (double *)fl->vel.ptr));
+    SKB_TRY(matvec_core(fl, (const double *)fl->fw.ptr, d_xs, d_bd, d_f, d_t, eta, (double *)fl->vel.ptr));
     // res_fibers = fc.matvec(x_fibers, v_fibers, fiber_link_conditions)   system.cpp:318
     SKB_TRY(fl->ops.matvec(d_x, (const double *)fl->vel.ptr, d_link, d_res_fib, fl->cur, &fl->launches));
     const double *d_v_shell = (const double *)fl->vel.ptr + 3 * n_fw;
@@ -881,32 +842,14 @@ static int apply_matvec_impl(skb_flow *fl, skb_dense *dn, const double *x_fibers
     if (fl->n_bodies > 0)
         split_forces_torques(body_forces_torques, fl->n_bodies, f, t);
     const bool link = nf && fiber_link_conditions;
-    return host_frame(
-        fl,
-        [&]() -> int {
-            SKB_TRY(upload(fl, fl->x_fib, x_fibers, (size_t)nf * 4));
-            if (link)
-                SKB_TRY(upload(fl, fl->vb, fiber_link_conditions, (size_t)fl->ops.n_fibers() * 7));
-            SKB_TRY(upload(fl, fl->in_shell, shell_density, (size_t)ns * 3));
-            SKB_TRY(upload(fl, fl->in_body, body_densities, (size_t)nb * 3));
-            SKB_TRY(upload(fl, fl->in_force, f.data(), f.size()));
-            SKB_TRY(upload(fl, fl->in_torque, t.data(), t.size()));
-            SKB_TRY(fl->res_fib.ensure((size_t)nf * 32));
-            SKB_TRY(fl->res_shell.ensure((size_t)ns * 24 + 8));
-            return fl->tmp_b.ensure((size_t)nb * 24 + 8);
-        },
-        [&] {
-            return apply_matvec_core(fl, dn, (const double *)fl->x_fib.ptr, (const double *)fl->in_shell.ptr,
-                                     (const double *)fl->in_body.ptr, (const double *)fl->in_force.ptr,
-                                     (const double *)fl->in_torque.ptr, link ? (const double *)fl->vb.ptr : nullptr,
-                                     eta, (double *)fl->res_fib.ptr, (double *)fl->res_shell.ptr,
-                                     (double *)fl->tmp_b.ptr);
-        },
-        [&]() -> int {
-            SKB_TRY(download(fl, res_fibers, fl->res_fib, (size_t)nf * 4));
-            SKB_TRY(download(fl, v_shell, fl->res_shell, (size_t)ns * 3));
-            return download(fl, v_bodies, fl->tmp_b, (size_t)nb * 3);
-        });
+    Transfers xfer{{up(x_fibers, 4 * nf), up(link ? fiber_link_conditions : nullptr, 7LL * fl->ops.n_fibers()),
+                    up(shell_density, 3 * ns), up(body_densities, 3 * nb), up(f.data(), f.size()),
+                    up(t.data(), t.size())},
+                   {down(res_fibers, 4 * nf), down(v_shell, 3 * ns), down(v_bodies, 3 * nb)}};
+    return host_call(fl, xfer, [&](const Transfers &io) {
+        return apply_matvec_core(fl, dn, io.up[0].dev, io.up[2].dev, io.up[3].dev, io.up[4].dev, io.up[5].dev,
+                                 link ? io.up[1].dev : nullptr, eta, io.down[0].dev, io.down[1].dev, io.down[2].dev);
+    });
 }
 
 extern "C" {

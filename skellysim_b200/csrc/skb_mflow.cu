@@ -88,23 +88,6 @@ class Workers {
     bool stop_ = false;
 };
 
-// A member's copies of one host-array call: each Run moves len doubles between the caller's array at `whole` and the
-// device array at `at`
-struct Run {
-    long long whole, at, len;
-};
-struct Transfer {
-    double *host;          // the caller's array (only read by an upload); NULL: nothing to copy
-    double *dev;           // a device array the callee owns, or the staging slot mflow_stage gives it
-    std::vector<Run> runs;
-};
-struct Transfers {
-    std::vector<Transfer> up, down; // before the call, after it
-};
-Transfer up(const double *h, std::vector<Run> runs, double *dev = nullptr) {
-    return Transfer{const_cast<double *>(h), dev, std::move(runs)};
-}
-Transfer down(double *h, std::vector<Run> runs, double *dev = nullptr) { return Transfer{h, dev, std::move(runs)}; }
 } // namespace
 
 struct skb_mflow {
@@ -515,19 +498,7 @@ template <class Describe> static int mflow_stage(skb_mflow *mf, Describe describ
         CUDA_TRY(cudaSetDevice(mf->devs[g]));
         skb_mflow::IO &io = mf->io[g];
         io.xfer = describe(g);
-        io.stage.resize(std::max(io.stage.size(), io.xfer.up.size() + io.xfer.down.size()));
-        size_t k = 0;
-        for (std::vector<Transfer> *list : {&io.xfer.up, &io.xfer.down})
-            for (Transfer &t : *list) {
-                DevBuf &slot = io.stage[k++];
-                if (t.dev)
-                    continue;
-                long long n = 0;
-                for (const Run &r : t.runs)
-                    n = std::max(n, r.at + r.len);
-                SKB_TRY(slot.ensure((size_t)n * 8 + 8));
-                t.dev = (double *)slot.ptr;
-            }
+        SKB_TRY(stage_slots(io.stage, io.xfer));
         const long long n_sw = mf->s1[g] - mf->s0[g];
         if (mf->has_dense && n_sw > 0 && mf->m[g]->bg.enabled) // the background streamer's, if it is on
             SKB_TRY(overlap_buffers(mf->m[g].get(), 3 * n_sw));
@@ -541,17 +512,11 @@ template <class Call> static int member_call(skb_mflow *mf, int g, Call call) {
     const skb_mflow::IO &io = mf->io[(size_t)g];
     CUDA_TRY(cudaSetDevice(mf->devs[(size_t)g]));
     const cudaStream_t st = mf->m[(size_t)g]->stream;
-    for (const Transfer &t : io.xfer.up)
-        for (const Run &r : t.runs)
-            if (t.host && r.len)
-                CUDA_TRY(cudaMemcpyAsync(t.dev + r.at, t.host + r.whole, (size_t)r.len * 8, cudaMemcpyHostToDevice, st));
+    SKB_TRY(issue(io.xfer.up, true, st));
     CUDA_TRY(cudaEventRecord(io.e0, st));
     SKB_TRY(call(st, io.xfer));
     CUDA_TRY(cudaEventRecord(io.e1, st));
-    for (const Transfer &t : io.xfer.down)
-        for (const Run &r : t.runs)
-            if (t.host && r.len)
-                CUDA_TRY(cudaMemcpyAsync(t.host + r.whole, t.dev + r.at, (size_t)r.len * 8, cudaMemcpyDeviceToHost, st));
+    SKB_TRY(issue(io.xfer.down, false, st));
     if (!io.xfer.down.empty())
         CUDA_TRY(cudaStreamSynchronize(st));
     return SKB_OK;

@@ -279,22 +279,15 @@ int skb_flow_build_fiber_rhs(skb_flow *fl, const skb_fiber_params *params, const
                              double eta, double *rhs) {
     OwnFibers own;
     SKB_TRY(fiber_rhs_args(fl, "skb_flow_build_fiber_rhs", params, rhs, dt, eta, own));
-    const size_t nf = (size_t)own.nodes();
-    SKB_TRY(fl->vel.ensure(nf * 24));
-    SKB_TRY(fl->in_fib.ensure(nf * 24));
-    SKB_TRY(fl->res_fib.ensure(nf * 32));
-    // device_ms spans the kernel, total_ms also the uploads before it and the download after it
-    return fl->ops.rhs(own, params, v_growth, force_scale, v_on_fibers ? (const double *)fl->vel.ptr : nullptr,
-                       f_external ? (const double *)fl->in_fib.ptr : nullptr, dt, eta, (double *)fl->res_fib.ptr,
-                       &fl->launches, [&](const FiberOps::Step &stage, const FiberOps::Step &launch) {
-                           auto up = [&]() -> int {
-                               if (v_on_fibers)
-                                   SKB_TRY(upload(fl, fl->vel, v_on_fibers, nf * 3));
-                               if (f_external)
-                                   SKB_TRY(upload(fl, fl->in_fib, f_external, nf * 3));
-                               return stage();
-                           };
-                           return host_frame(fl, up, launch, [&] { return download(fl, rhs, fl->res_fib, nf * 4); });
+    const long long nf = own.nodes();
+    // staged here, so that the kernel's arguments are known before its frame (host_call keeps them); device_ms spans
+    // the kernel, total_ms also the uploads and the tables' stage before it and the download after it
+    Transfers xfer{{up(v_on_fibers, 3 * nf), up(f_external, 3 * nf)}, {down(rhs, 4 * nf)}};
+    SKB_TRY(stage_slots(fl->slots, xfer));
+    return fl->ops.rhs(own, params, v_growth, force_scale, v_on_fibers ? xfer.up[0].dev : nullptr,
+                       f_external ? xfer.up[1].dev : nullptr, dt, eta, xfer.down[0].dev, &fl->launches,
+                       [&](const FiberOps::Step &stage, const FiberOps::Step &launch) {
+                           return host_call(fl, xfer, [&](const Transfers &) { return launch(); }, stage);
                        });
 }
 
@@ -325,14 +318,10 @@ int skb_flow_get_fiber_operators(skb_flow *fl, double *A, double *force_operator
 // host pointers: through host_frame on the flow's stream; device pointers: asynchronously on the caller's stream
 int skb_flow_apply_fiber_preconditioner(skb_flow *fl, const double *x_fibers, double *y) {
     return fiber_ops_call(fl, "skb_flow_apply_fiber_preconditioner", true, x_fibers && y, [&](size_t nf) {
-        SKB_TRY(fl->res_fib.ensure(nf * 32));
-        return host_frame(
-            fl, [&] { return upload(fl, fl->x_fib, x_fibers, nf * 4); },
-            [&] {
-                return fl->ops.precondition((const double *)fl->x_fib.ptr, (double *)fl->res_fib.ptr, fl->cur,
-                                            &fl->launches);
-            },
-            [&] { return download(fl, y, fl->res_fib, nf * 4); });
+        Transfers xfer{{up(x_fibers, 4 * nf)}, {down(y, 4 * nf)}};
+        return host_call(fl, xfer, [&](const Transfers &io) {
+            return fl->ops.precondition(io.up[0].dev, io.down[0].dev, fl->cur, &fl->launches);
+        });
     });
 }
 
@@ -345,36 +334,22 @@ int skb_flow_apply_fiber_preconditioner_device(skb_flow *fl, const double *d_x_f
 
 int skb_flow_apply_fiber_force(skb_flow *fl, const double *x_fibers, double *fw) {
     return fiber_ops_call(fl, "skb_flow_apply_fiber_force", false, x_fibers && fw, [&](size_t nf) {
-        return host_frame(
-            fl,
-            [&]() -> int {
-                SKB_TRY(upload(fl, fl->x_fib, x_fibers, nf * 4));
-                return fl->in_fib.ensure(nf * 24);
-            },
-            [&] {
-                return fl->ops.force((const double *)fl->x_fib.ptr, (double *)fl->in_fib.ptr, fl->cur, &fl->launches);
-            },
-            [&] { return download(fl, fw, fl->in_fib, nf * 3); });
+        Transfers xfer{{up(x_fibers, 4 * nf)}, {down(fw, 3 * nf)}};
+        return host_call(fl, xfer, [&](const Transfers &io) {
+            return fl->ops.force(io.up[0].dev, io.down[0].dev, fl->cur, &fl->launches);
+        });
     });
 }
 
 int skb_flow_fiber_matvec(skb_flow *fl, const double *x_fibers, const double *v_fibers, const double *v_fib_boundary,
                           double *res) {
     return fiber_ops_call(fl, "skb_flow_fiber_matvec", false, x_fibers && v_fibers && res, [&](size_t nf) {
-        SKB_TRY(fl->res_fib.ensure(nf * 32));
-        return host_frame(
-            fl,
-            [&]() -> int {
-                SKB_TRY(upload(fl, fl->x_fib, x_fibers, nf * 4));
-                SKB_TRY(upload(fl, fl->vel, v_fibers, nf * 3));
-                return v_fib_boundary ? upload(fl, fl->vb, v_fib_boundary, (size_t)fl->ops.n_fibers() * 7) : SKB_OK;
-            },
-            [&] {
-                return fl->ops.matvec((const double *)fl->x_fib.ptr, (const double *)fl->vel.ptr,
-                                      v_fib_boundary ? (const double *)fl->vb.ptr : nullptr,
-                                      (double *)fl->res_fib.ptr, fl->cur, &fl->launches);
-            },
-            [&] { return download(fl, res, fl->res_fib, nf * 4); });
+        Transfers xfer{{up(x_fibers, 4 * nf), up(v_fibers, 3 * nf), up(v_fib_boundary, 7LL * fl->ops.n_fibers())},
+                       {down(res, 4 * nf)}};
+        return host_call(fl, xfer, [&](const Transfers &io) {
+            return fl->ops.matvec(io.up[0].dev, io.up[1].dev, v_fib_boundary ? io.up[2].dev : nullptr, io.down[0].dev,
+                                  fl->cur, &fl->launches);
+        });
     });
 }
 
@@ -509,12 +484,10 @@ int skb_flow_apply_system_matvec(skb_flow *fl, skb_dense *dn, const double *x, d
     const size_t n = (size_t)solution_size(fl);
     if (n == 0)
         return SKB_OK;
-    SKB_TRY(fl->sys_x.ensure(n * 8));
-    SKB_TRY(fl->sys_y.ensure(n * 8));
-    return host_frame(
-        fl, [&] { return upload(fl, fl->sys_x, x, n); },
-        [&] { return system_matvec_core(fl, dn, (const double *)fl->sys_x.ptr, eta, (double *)fl->sys_y.ptr); },
-        [&] { return download(fl, res, fl->sys_y, n); });
+    Transfers xfer{{up(x, n)}, {down(res, n)}};
+    return host_call(fl, xfer, [&](const Transfers &io) {
+        return system_matvec_core(fl, dn, io.up[0].dev, eta, io.down[0].dev);
+    });
 }
 
 int skb_flow_apply_system_matvec_device(skb_flow *fl, skb_dense *dn, const double *d_x, double eta, double *d_res,
@@ -534,12 +507,9 @@ int skb_flow_apply_system_preconditioner(skb_flow *fl, skb_dense *dn, const doub
     const size_t n = (size_t)solution_size(fl);
     if (n == 0)
         return SKB_OK;
-    SKB_TRY(fl->sys_x.ensure(n * 8));
-    SKB_TRY(fl->sys_y.ensure(n * 8));
-    return host_frame(
-        fl, [&] { return upload(fl, fl->sys_x, x, n); },
-        [&] { return system_precondition_core(fl, dn, (const double *)fl->sys_x.ptr, (double *)fl->sys_y.ptr); },
-        [&] { return download(fl, y, fl->sys_y, n); });
+    Transfers xfer{{up(x, n)}, {down(y, n)}};
+    return host_call(fl, xfer,
+                     [&](const Transfers &io) { return system_precondition_core(fl, dn, io.up[0].dev, io.down[0].dev); });
 }
 
 int skb_flow_apply_system_preconditioner_device(skb_flow *fl, skb_dense *dn, const double *d_x, double *d_y,
@@ -658,24 +628,13 @@ int skb_flow_build_system_rhs(skb_flow *fl, const skb_fiber_params *params, cons
     std::vector<double> f, t;
     if (body_forces_torques && fl->n_bodies > 0)
         split_forces_torques(body_forces_torques, fl->n_bodies, f, t);
-    SKB_TRY(fl->sys_y.ensure(n * 8));
-    double *d_rhs = (double *)fl->sys_y.ptr;
-    return host_frame(
-        fl,
-        [&]() -> int {
-            if (f_external)
-                SKB_TRY(upload(fl, fl->in_fib, f_external, (size_t)nf * 3));
-            SKB_TRY(upload(fl, fl->in_force, f.data(), f.size()));
-            return upload(fl, fl->in_torque, t.data(), t.size());
-        },
-        [&] {
-            return system_rhs_core(fl, own, params, v_growth, force_scale,
-                                   f_external && nf ? (const double *)fl->in_fib.ptr : nullptr,
-                                   f.empty() ? nullptr : (const double *)fl->in_force.ptr,
-                                   t.empty() ? nullptr : (const double *)fl->in_torque.ptr, dt, eta, d_rhs,
-                                   d_rhs + 4 * nf, d_rhs + 4 * nf + 3 * ns);
-        },
-        [&] { return download(fl, rhs, fl->sys_y, n); });
+    Transfers xfer{{up(f_external, 3 * nf), up(f.data(), f.size()), up(t.data(), t.size())}, {down(rhs, n)}};
+    return host_call(fl, xfer, [&](const Transfers &io) {
+        double *d_rhs = io.down[0].dev;
+        return system_rhs_core(fl, own, params, v_growth, force_scale, f_external && nf ? io.up[0].dev : nullptr,
+                               f.empty() ? nullptr : io.up[1].dev, t.empty() ? nullptr : io.up[2].dev, dt, eta, d_rhs,
+                               d_rhs + 4 * nf, d_rhs + 4 * nf + 3 * ns);
+    });
 }
 
 int skb_flow_build_system_rhs_device(skb_flow *fl, const skb_fiber_params *params, const double *v_growth,
